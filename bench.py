@@ -1,21 +1,22 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native SHAPY hot path (BASELINE.json metric).
+"""bench.py -- headline benchmark of the H100-native SHAPY hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 64]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 64] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
            bench.py --gpus N --steps K --warmup W
 
 metric : bodies/sec, image -> SMPL-X vertices (+ betas, measurements), B = 64 per GPU (BASELINE configs[2],
-         "Full SHAPY_A regressor (HRNet + iterative head + fused SMPL-X), batch=64, 1xB200, fp32 tol 1e-4";
+         "Full SHAPY_A regressor (HRNet + iterative head + fused SMPL-X), batch=64, 1 GPU, fp32 tol 1e-4";
          configs[4] shards 64 images per GPU, i.e. weak scaling).
 value  : whole-job bodies/s with the images already resident in HBM (CUDA events, max over ranks).
 e2e    : the same metric through the public serving loop with HOST buffers (shapy_b200.pipeline.HostPipeline around
          SMPLXRegressor.forward): every rank copies its own pinned host images H2D, runs the forward and copies
          vertices / betas / measurements D2H, the three stages overlapped across consecutive batches on three
          streams; all copies sit inside the timed region (one interval over the K batches, max over ranks).
-roofline: the dominant kernel is the tcgen05 implicit-GEMM convolution (HRNet = ~99 % of the step);
+roofline: the dominant kernel is the wgmma implicit-GEMM convolution (HRNet = most of the step);
          achieved = algorithmic conv FLOPs (36.93 GFLOP / image @224^2, SURVEY.md 8d) / HRNet device time.
-         `roofline_lbs` / `roofline_shape` report the HBM rooflines of the fused SMPL-X kernels.
+         `roofline_lbs` / `roofline_shape` report the HBM rooflines of the SMPL-X kernels.  Peaks are the H100 SXM
+         data-sheet figures (989 TFLOP/s dense FP16, 3.35 TB/s HBM3, at 700 W), not measured rates.
 cpu_baseline / --impl reference: the CPU restatement of the reference path (oracle/, "port") timed on the
          box's host cores on a bounded sample of the same workload: one warm-up pass, then timed passes over the same
          sample (the in-line cpu_baseline and the --impl reference arm use the same procedure).  The in-line leg
@@ -24,6 +25,9 @@ cpu_baseline / --impl reference: the CPU restatement of the reference path (orac
 config2 : BASELINE configs[1] (HRNet-W48 only, plain fp16 operands, B = 32) timed in the same run.
 config5 : (N > 1) BASELINE configs[4]: rank 0 holds the whole batch (N x 64 uint8 images) in HBM, NCCL scatter ->
          on-device crop / normalise -> forward -> NCCL gather of vertices / betas / measurements to rank 0.
+--dump-outputs DIR: after the timed steps, the arrays the last timed forward returned (features, every tensor of the
+         last stage, measurements) as DIR/<name>.npy in float32; the inputs are seeded, so two builds given the same
+         arguments can be compared output for output.
 """
 import argparse
 import json
@@ -45,12 +49,7 @@ SHAPE_BODY_BYTES = 40 + 125700
 
 
 def peaks():
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm=d['hbm_gbs'], tf_burst=d['bf16_tflops'], tf_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']),
-                    source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm=3350.0, tf_sustained=989.0, source='H100 SXM data sheet: dense FP16, HBM3, 700 W')
 
 
 class ClockSampler:
@@ -90,25 +89,43 @@ class ClockSampler:
                 'samples': len(sm)}
 
 
-def conv_traffic(batch: int, mode: int):
-    """DRAM bytes (read + write) of all conv launches of one HRNet forward, from the committed ncu capture
-    profiles/r02_traffic.json (r01 if absent; taken at B=64, split mode); None for any other configuration."""
-    path = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    if not os.path.exists(path):
-        path = os.path.join(ROOT, 'profiles', 'r01_traffic.json')
-    if batch != 64 or mode != 1 or not os.path.exists(path):
-        return None
-    with open(path) as f:
-        return json.load(f).get('conv_dram_bytes_per_step')
+DUMP_BYTES = 64 * 1024 * 1024
 
 
-def lbs_traffic(batch: int):
-    """DRAM bytes of one SMPL-X forward (fused LBS + joints kernels) from the committed ncu capture; B=64 only."""
-    path = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    if batch != 64 or not os.path.exists(path):
-        return None
-    with open(path) as f:
-        return json.load(f).get('lbs_B64', {}).get('dram_bytes_per_call')
+def dump_outputs(out, path):
+    """Writes every floating-point tensor of the forward's output dict (the last stage, features, measurements, joints
+    and projected joints out of their KeypointTensor wrappers, the camera parameters) as path/<name>.npy in float32.  Tensors that would push the total past DUMP_BYTES are replaced by a fixed, seeded sample
+    of their flattened elements (<name>.sample_idx.npy holds the indices)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    last = out['stage_keys'][-1]
+    arrays = {}
+
+    def walk(prefix, v):
+        if torch.is_tensor(v):
+            if v.is_floating_point():
+                arrays[prefix] = v
+        elif type(v).__name__ == 'KeypointTensor':
+            walk(prefix, v._t)
+        elif type(v).__name__ == 'CameraParams':
+            walk(prefix, {k: getattr(v, k) for k in ('translation', 'rotation', 'scale', 'focal_length')})
+        elif isinstance(v, dict):
+            for k in sorted(v):
+                walk(f'{prefix}.{k}' if prefix else str(k), v[k])
+    walk('', {k: v for k, v in out.items() if k == last or not k.startswith('stage_')})
+    used = 0
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if used + a.nbytes > DUMP_BYTES:
+            n = max(0, min(a.size, (DUMP_BYTES - used) // 12))     # 4 B of value + 8 B of int64 index each
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False)).astype(np.int64)
+            np.save(os.path.join(path, f'{name}.sample_idx.npy'), idx)
+            used += idx.nbytes
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, f'{name}.npy'), a)
+        used += a.nbytes
+    return sorted(arrays)
 
 
 def usable_cores() -> int:
@@ -149,9 +166,8 @@ def run_reference(args):
     sd = {k: v.clone() for k, v in model.state_dict().items()}
     smplx, lm = synth.make_smplx(), synth.load_landmarks()
     # One warm-up pass over the sample, then K timed passes.  The sample is `--ref-sample` bodies (8, the same as the
-    # in-line cpu_baseline leg of the GPU arm): the oneDNN / ATen convolutions of this port run at their best per-body
-    # rate there (21-25 bodies/s on the 16 host cores; 64 bodies per pass: 9.7 bodies/s, profiles/
-    # r02_bench_reference_arm_sample64.json), shrunk only if K passes would not fit in two minutes.
+    # in-line cpu_baseline leg of the GPU arm): the oneDNN / ATen convolutions of this port run at a better per-body
+    # rate there than at 64 bodies per pass; shrunk only if K passes would not fit in two minutes.
     x1 = torch.randn(1, 3, 224, 224, generator=torch.Generator().manual_seed(0))
     t0 = time.perf_counter()
     cpu_reference_step(sd, smplx, lm, x1)
@@ -188,6 +204,7 @@ def main():
     ap.add_argument('--mode', type=int, default=1, help='1 = split-fp16 parity mode (1e-4), 0 = plain fp16 (config 2)')
     ap.add_argument('--ref-sample', type=int, default=8)
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s outputs as DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         return run_reference(args)
@@ -215,7 +232,7 @@ def main():
     g = torch.Generator().manual_seed(1000 + rank)
     x_host = torch.randn(B, 3, 224, 224, generator=g).pin_memory()
     x_dev = x_host.to(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -223,9 +240,12 @@ def main():
             dist.barrier()
             torch.cuda.synchronize()
 
+    last_out = {}
+
     def step_resident():
         with torch.no_grad():
-            return model(x_dev)
+            last_out['out'] = model(x_dev)
+        return last_out['out']
 
     def timed(fn, k, pre=None):
         """Sum of per-step device times (CUDA events on the launching stream), L2 flushed before each step."""
@@ -260,6 +280,9 @@ def main():
     clocks = clk.summary()
     ms_per_step = total_ms / K
     value = world * B / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        dump_outputs(last_out['out'], args.dump_outputs)
 
     # ---------------------------------------------------------------- end-to-end with host buffers
     # Every rank serves its own stream of batches from its own pinned host buffers through the public serving loop
@@ -423,14 +446,13 @@ def main():
             'gpu_launches': int(launches_per_step * K),
             'clocks': clocks,
             'roofline': {'bound': 'tensor', 'achieved': conv_tf, 'peak': pk['tf_sustained'], 'unit': 'TFLOP/s',
-                         'frac': conv_tf / pk['tf_sustained'], 'traffic': conv_traffic(B, args.mode),
-                         'kernel': 'conv_halo_kernel / conv_umma_kernel (HRNet forward: all 331 convs + fuse + pool, 4 lanes)',
+                         'frac': conv_tf / pk['tf_sustained'],
+                         'kernel': 'conv_wgmma_kernel (HRNet forward: all 331 convs + fuse + pool, 4 lanes)',
                          'ms': hr_ms, 'mma_flops_factor': 3 if args.mode else 1, 'peak_source': pk['source']},
             'roofline_lbs': {'bound': 'hbm', 'achieved': lbs_gbs, 'peak': pk['hbm'], 'unit': 'GB/s',
-                             'frac': lbs_gbs / pk['hbm'], 'ms': lbs_ms, 'traffic': lbs_traffic(B),
-                             'kernel': 'smplx_lbs_kernel (fused tcgen05) + smplx_joints_kernel, B=%d posed; achieved counts the '
-                                       'algorithmic bytes of SURVEY 8d (all 486 pose-basis rows), traffic is what ncu measured: the '
-                                       'rows of identity joints are never read' % B},
+                             'frac': lbs_gbs / pk['hbm'], 'ms': lbs_ms,
+                             'kernel': 'smplx_pose_kernel + smplx_vertex_kernel + smplx_joints_kernel, B=%d posed; achieved '
+                                       'counts the algorithmic bytes of SURVEY 8d (all 486 pose-basis rows)' % B},
             'roofline_shape': {'bound': 'hbm', 'achieved': shp_gbs, 'peak': pk['hbm'], 'unit': 'GB/s',
                                'frac': shp_gbs / pk['hbm'], 'ms': shp_ms, 'kernel': 'smplx_shape_kernel, 4096 bodies (config 4)'},
             'roofline_measure': {'bound': 'hbm', 'achieved': meas_gbs, 'peak': pk['hbm'], 'unit': 'GB/s',

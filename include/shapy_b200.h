@@ -1,4 +1,4 @@
-/* shapy_b200 -- C ABI of the B200-native SHAPY inference hot path.
+/* shapy_b200 -- C ABI of the H100-native (sm_90a) SHAPY inference hot path.
  *
  * Every entry point is `extern "C"`, takes plain pointers / sizes / a CUDA stream
  * (passed as void* so the header needs no CUDA include) and returns 0 on success or
@@ -189,7 +189,7 @@ typedef struct {
 
 /* mode: 0 = fp16 operands, single pass (BASELINE config 2);
  *       1 = split-fp16 (hi + lo planes, 3 MMAs per tile, ~fp32 accuracy; parity mode);
- * engine: 0 = tcgen05 implicit GEMM where the shape allows, 1 = SIMT fp32 everywhere (debug). */
+ * engine: 0 = wgmma implicit GEMM where the shape allows, 1 = SIMT fp32 everywhere (debug). */
 int shapy_hrnet_create(shapy_hrnet_t **out, const shapy_conv_desc_t *convs, int n_convs, const shapy_op_t *ops,
                        int n_ops, const shapy_slot_t *slots, int n_slots, int feat_slot, int mode, int engine);
 void shapy_hrnet_destroy(shapy_hrnet_t *p);

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY -- builds the REFERENCE's own BVH operator into oracle/_ref/ (git-ignored, travels to the
-GPU box with the snapshot) so the GPU tests can compare shapy_mmi_forward with the real kernel on the same B200.
+GPU box with the snapshot) so the GPU tests can compare shapy_mmi_forward with the real kernel on the same GPU.
 
 Sources are compiled where they lie under /root/reference/mesh-mesh-intersection (never copied into the repo):
     src/mesh_mesh_intersect_cuda_op.cu   (op.cu)       include/*.h(pp)
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False):
         nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
         o_cu, o_cpp = os.path.join(tmp, 'op.o'), os.path.join(tmp, 'bind.o')
         run = lambda cmd: subprocess.run(cmd, check=True, capture_output=not verbose)
-        run([nvcc, '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
+        run([nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
              '--expt-relaxed-constexpr', '--expt-extended-lambda', '-DPRINT_TIMINGS=0', '-DDEBUG_PRINT=0', '-DERROR_CHECKING=1',
              '-DCOLLISION_ORDERING=1', '-w'] + defs + inc +
             ['-c', patched, '-o', o_cu])

@@ -1,4 +1,4 @@
-"""shapy_b200 -- B200-native (sm_100a) SHAPY inference hot path behind the reference's own module API.
+"""shapy_b200 -- H100-native (sm_90a) SHAPY inference hot path behind the reference's own module API.
 
     from shapy_b200.human_shape.models import build_model      # mirrors human_shape.models
     from shapy_b200 import mesh_mesh_intersect_cuda             # mirrors the reference's CUDA extension
@@ -15,7 +15,7 @@ __version__ = '0.1.0'
 def install_as_reference():
     """Registers `human_shape.models` (and sub-packages), `mesh_mesh_intersect_cuda`,
     `mesh_mesh_intersection` and `body_measurements` in sys.modules so that the reference's
-    regressor/demo.py and regressor/evaluate.py import the B200 path unchanged."""
+    regressor/demo.py and regressor/evaluate.py import the H100 path unchanged."""
     import importlib
     from . import body_measurements, mesh_mesh_intersect_cuda, mesh_mesh_intersection
     models = importlib.import_module('shapy_b200.human_shape.models')

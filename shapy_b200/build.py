@@ -1,4 +1,4 @@
-"""Builds shapy_b200/libshapy_b200.so in-tree with nvcc for sm_100a (no torch dependency).
+"""Builds shapy_b200/libshapy_b200.so in-tree with nvcc for sm_90a (no torch dependency).
 
     python -m shapy_b200.build [--force]
 
@@ -19,7 +19,7 @@ DEFS = os.environ.get('SHAPY_BUILD_DEFS', '').split()
 OBJ = os.path.join(HERE, '_obj' + ('_' + TAG if TAG else ''))
 LIB = os.path.join(HERE, 'libshapy_b200' + ('_' + TAG if TAG else '') + '.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC',
           '--expt-relaxed-constexpr']
 # per-file extra flags: the triangle predicates must round like the plain-C oracle

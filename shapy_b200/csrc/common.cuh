@@ -1,4 +1,4 @@
-// Shared helpers for the shapy_b200 CUDA library (sm_100a only).
+// Shared helpers for the shapy_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -29,17 +29,16 @@ struct ConvW {
   int cin = 0, cout = 0, ksize = 0, stride = 0;
 };
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one request per 32-byte sector instead of two half-sector
-// ones -- the epilogue's row-per-thread stores are bound by the request rate, not by bytes.  32-byte aligned addresses.
-__device__ __forceinline__ void ldg256(const void *p, uint4 &a, uint4 &b) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-               : "l"(p));
+// 32 consecutive bytes as two 16-byte accesses (16-byte aligned addresses)
+__device__ __forceinline__ void ldg32b(const void *p, uint4 &a, uint4 &b) {
+  const uint4 *q = reinterpret_cast<const uint4 *>(p);
+  a = __ldg(q);
+  b = __ldg(q + 1);
 }
-__device__ __forceinline__ void stg256(void *p, const uint4 &a, const uint4 &b) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w),
-               "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
+__device__ __forceinline__ void stg32b(void *p, const uint4 &a, const uint4 &b) {
+  uint4 *q = reinterpret_cast<uint4 *>(p);
+  q[0] = a;
+  q[1] = b;
 }
 
 __device__ __forceinline__ void split_store(float v, __half &hi, __half &lo) {
@@ -59,11 +58,11 @@ int launch_set_io_cells(void **cells, const float *images, float *feats, cudaStr
 int launch_nhwc_split(const float *x, const ActView &out, cudaStream_t st);          // fp32 NHWC -> planes
 int launch_nhwc_merge(const ActView &in, float *y, bool to_nchw, cudaStream_t st);   // planes -> fp32
 
-// tcgen05 implicit-GEMM engine.  `UmmaPlan` holds the TMA descriptors + geometry of one launch.
-struct UmmaPlan;
-bool umma_supported(const ConvW &w, const ActView &in, const ActView &out);
-UmmaPlan *umma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu);
-void umma_plan_destroy(UmmaPlan *p);
-int umma_plan_launch(const UmmaPlan *p, cudaStream_t st, bool pdl);   // pdl: programmatic dependent launch
+// TMA + wgmma implicit-GEMM engine (conv_wgmma.cu).  `WgmmaPlan` holds the TMA descriptors + geometry of one launch.
+struct WgmmaPlan;
+bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out);
+WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu);
+void wgmma_plan_destroy(WgmmaPlan *p);
+int wgmma_plan_launch(const WgmmaPlan *p, cudaStream_t st, bool pdl);   // pdl: programmatic dependent launch
 
 }  // namespace shapy

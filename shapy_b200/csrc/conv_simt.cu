@@ -1,6 +1,6 @@
 // SIMT (CUDA-core, fp32 accumulate) engines of the HRNet path: the 3-channel stem convolution, the
 // multi-resolution fuse sum, the final spatial mean, layout converters, and a generic implicit-GEMM
-// convolution on the same split-fp16 planes the tcgen05 engine uses.  The SIMT convolution is the
+// convolution on the same split-fp16 planes the wgmma engine uses.  The SIMT convolution is the
 // debug / cross-check engine (`engine = 1`): identical operands and rounding points, no tensor cores.
 // Reference: regressor/human_shape/models/backbone/hrnet.py:426-498 (forward), 175-193 (fuse).
 #include "conv.cuh"
@@ -236,8 +236,8 @@ __global__ void __launch_bounds__(256, 2) stem4_kernel(const float *__restrict__
 #pragma unroll
     for (int j = 0; j < 16; ++j) split_store(fmaxf(acc[p][j], 0.f), hi[j], lo[j]);
     const size_t o = (pix0 + p) * ctot + coff + g * 16;   // 32-byte aligned (launch_stem checks ctot, coff, base)
-    stg256(out_hi + o, reinterpret_cast<const uint4 *>(hi)[0], reinterpret_cast<const uint4 *>(hi)[1]);
-    if (out_lo) stg256(out_lo + o, reinterpret_cast<const uint4 *>(lo)[0], reinterpret_cast<const uint4 *>(lo)[1]);
+    stg32b(out_hi + o, reinterpret_cast<const uint4 *>(hi)[0], reinterpret_cast<const uint4 *>(hi)[1]);
+    if (out_lo) stg32b(out_lo + o, reinterpret_cast<const uint4 *>(lo)[0], reinterpret_cast<const uint4 *>(lo)[1]);
   }
 }
 
@@ -276,7 +276,7 @@ struct FuseParams {
 // CH = 8: 128-bit accesses; CH = 16: 256-bit accesses (rows 32-byte aligned), half the memory requests.
 template <int CH>
 __global__ void __launch_bounds__(256) fuse_kernel(FuseParams p) {
-  // programmatic dependent launch (see conv_umma.cu): this grid may be scheduled while the producer of its inputs is
+  // programmatic dependent launch (see conv_wgmma.cu): this grid may be scheduled while the producer of its inputs is
   // draining, and lets the next launch do the same; the wait returns once every earlier grid has completed
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -294,10 +294,10 @@ __global__ void __launch_bounds__(256) fuse_kernel(FuseParams p) {
     const int Hi = p.H >> s, Wi = p.W >> s;
     size_t o = (((size_t)n * Hi + (h >> s)) * Wi + (w >> s)) * p.ctot[i] + p.coff[i] + g * CH;
     uint4 hv[CH / 8], lv[CH / 8];
-    if (CH == 16) ldg256(p.hi[i] + o, hv[0], hv[CH / 8 - 1]); else hv[0] = *reinterpret_cast<const uint4 *>(p.hi[i] + o);
+    if (CH == 16) ldg32b(p.hi[i] + o, hv[0], hv[CH / 8 - 1]); else hv[0] = *reinterpret_cast<const uint4 *>(p.hi[i] + o);
     const __half *hh = reinterpret_cast<const __half *>(hv);
     if (p.lo[i]) {
-      if (CH == 16) ldg256(p.lo[i] + o, lv[0], lv[CH / 8 - 1]); else lv[0] = *reinterpret_cast<const uint4 *>(p.lo[i] + o);
+      if (CH == 16) ldg32b(p.lo[i] + o, lv[0], lv[CH / 8 - 1]); else lv[0] = *reinterpret_cast<const uint4 *>(p.lo[i] + o);
       const __half *ll = reinterpret_cast<const __half *>(lv);
 #pragma unroll
       for (int j = 0; j < CH; ++j) acc[j] += __half2float(hh[j]) + __half2float(ll[j]) * kLoInv;
@@ -312,8 +312,8 @@ __global__ void __launch_bounds__(256) fuse_kernel(FuseParams p) {
   size_t o = (size_t)pix * p.out_ctot + p.out_coff + g * CH;
   const uint4 *h4 = reinterpret_cast<const uint4 *>(hi), *l4 = reinterpret_cast<const uint4 *>(lo);
   if (CH == 16) {
-    stg256(p.out_hi + o, h4[0], h4[CH / 8 - 1]);
-    if (p.out_lo) stg256(p.out_lo + o, l4[0], l4[CH / 8 - 1]);
+    stg32b(p.out_hi + o, h4[0], h4[CH / 8 - 1]);
+    if (p.out_lo) stg32b(p.out_lo + o, l4[0], l4[CH / 8 - 1]);
   } else {
     *reinterpret_cast<uint4 *>(p.out_hi + o) = h4[0];
     if (p.out_lo) *reinterpret_cast<uint4 *>(p.out_lo + o) = l4[0];

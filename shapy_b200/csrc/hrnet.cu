@@ -5,7 +5,7 @@
 //   create : folds BatchNorm into the conv weights (scale) and a per-channel bias (shift), packs the
 //            weights as [tap][cout][cin] fp16 hi/lo planes on the device.
 //   bind   : (first forward for a given workspace / batch / image size) lays the slots out in the
-//            caller's workspace and encodes the TMA descriptors of every tcgen05 convolution.
+//            caller's workspace and encodes the TMA descriptors of every wgmma convolution.
 //   forward: ~380 launches (331 convs + fuse sums + pool) instead of the reference's ~1100.
 #include <array>
 #include <cmath>
@@ -26,7 +26,7 @@ struct shapy_hrnet {
   void *ws = nullptr;
   int B = 0, H = 0, W = 0;
   std::vector<ActView> views;
-  std::vector<UmmaPlan *> plans;  // per op (null when the op does not use the tcgen05 engine)
+  std::vector<WgmmaPlan *> plans;  // per op (null when the op does not use the wgmma engine)
   // lane schedule (built by bind): lane 0 is the caller's stream, lanes 1.. are streams owned by this object
   int n_lanes = 1;
   int device = -1;
@@ -47,7 +47,7 @@ struct shapy_hrnet {
 static void free_plans(shapy_hrnet *p) {
   if (p->graph_exec) cudaGraphExecDestroy(p->graph_exec);
   p->graph_exec = nullptr; p->graph_kernels = 0; p->warm = false; p->graph_failed = false;
-  for (auto *u : p->plans) if (u) umma_plan_destroy(u);
+  for (auto *u : p->plans) if (u) wgmma_plan_destroy(u);
   p->plans.clear();
   for (auto e : p->op_ev) if (e) cudaEventDestroy(e);
   p->op_ev.clear();
@@ -75,7 +75,7 @@ static void free_lanes(shapy_hrnet *p) {
 // every ordering between lanes is derived from the slots (and channel ranges) the ops read and write in PROGRAM
 // order -- RAW, WAR and WAW, so liveness-based slot reuse stays correct -- and reduced with vector clocks to the
 // cross-stream event waits that are really needed.  Persistent kernels of different lanes then back-fill each
-// other's tails: 896 equal work items on 148 SMs are 7 rounds of 6.05, 196 tiles 2 rounds of 1.32.
+// other's tails: 896 equal work items on 132 SMs are 7 rounds of 6.8, 196 tiles 2 rounds of 1.48.
 struct Access { int slot, c0, c1; bool write; };
 
 static void op_accesses(const shapy_hrnet *p, const shapy_op_t &o, std::vector<Access> &acc) {
@@ -110,9 +110,8 @@ static int max_lanes() {
   if (v < 0) { const char *e = getenv("SHAPY_HRNET_LANES"); v = e ? std::max(1, std::min(atoi(e), (int)SHAPY_MAX_LANES)) : SHAPY_MAX_LANES; }
   return v;
 }
-// SHAPY_PDL: 0 never, 1 (default) every conv launch, 2 only where no other lane can be running.  Measured (B = 64,
-// profiles/r02_lanes_ab.txt): 4 lanes with PDL everywhere 9.70 ms, with policy 2 10.43 ms, 1 lane 10.80 ms -- the
-// early-launched dependent's prologue overlap is worth more than the SMs it holds while it waits.
+// SHAPY_PDL: 0 never, 1 (default) every conv launch, 2 only where no other lane can be running.  The default lets the
+// early-launched dependent's prologue overlap its predecessor's tail.
 static int pdl_policy() {
   static int v = -1;
   if (v < 0) { const char *e = getenv("SHAPY_PDL"); v = e ? atoi(e) : 1; }
@@ -317,8 +316,8 @@ static int bind(shapy_hrnet *p, void *ws, int B, int H, int W) {
     ActView in = view_of(p, o.in_slot, 0, w.cin), out = view_of(p, o.out_slot, o.out_coff, w.cout);
     ActView res;
     if (o.res_slot >= 0) res = view_of(p, o.res_slot, 0, w.cout);
-    if (!umma_supported(w, in, out)) continue;  // falls back to the SIMT engine for this layer
-    p->plans[i] = umma_plan_create(w, in, out, o.res_slot >= 0 ? &res : nullptr, o.relu != 0);
+    if (!wgmma_supported(w, in, out)) continue;  // falls back to the SIMT engine for this layer
+    p->plans[i] = wgmma_plan_create(w, in, out, o.res_slot >= 0 ? &res : nullptr, o.relu != 0);
     if (!p->plans[i]) return SHAPY_ERR_STATE;
   }
   int rc = build_schedule(p);
@@ -374,7 +373,7 @@ static int enqueue_forward(shapy_hrnet *p, const float *images, float *feats, vo
       case SHAPY_OP_CONV: {
         const ConvW &w = p->convs[o.conv];
         if (p->plans[i]) {
-          rc = umma_plan_launch(p->plans[i], ls, p->op_pdl[i] != 0);
+          rc = wgmma_plan_launch(p->plans[i], ls, p->op_pdl[i] != 0);
         } else {
           ActView in = view_of(p, o.in_slot, 0, w.cin), out = view_of(p, o.out_slot, o.out_coff, w.cout), res;
           if (o.res_slot >= 0) res = view_of(p, o.res_slot, 0, w.cout);
@@ -412,7 +411,7 @@ static bool graph_enabled() {
   static int v = -1;
   if (v < 0) {
     const char *e = getenv("SHAPY_HRNET_GRAPH");
-    v = (e && e[0] == '0') || getenv("SHAPY_CONV_PHASES") ? 0 : 1;
+    v = (e && e[0] == '0') ? 0 : 1;
   }
   return v == 1;
 }
@@ -517,10 +516,10 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   cudaError_t err = cudaSuccess;
   ConvW w;
   int rc = SHAPY_OK;
-  UmmaPlan *plan = nullptr;
+  WgmmaPlan *plan = nullptr;
   auto cleanup = [&]() {
     cudaStreamSynchronize(st);
-    if (plan) umma_plan_destroy(plan);
+    if (plan) wgmma_plan_destroy(plan);
     for (void *a : allocs) cudaFree(a);
   };
   if (!pack_conv(*conv, false, w, allocs, err)) { cleanup(); set_error("conv_test: %s", cudaGetErrorString(err)); return (int)err; }
@@ -540,16 +539,16 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
   if (engine == 0) {
-    plan = umma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0);
+    plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }
-    rc = umma_plan_launch(plan, st, true);
+    rc = wgmma_plan_launch(plan, st, true);
     if (const char *reps_s = getenv("SHAPY_CONV_TEST_REPS")) {
       // timing aid for kernel work: re-launch the same plan and report the average launch time
       const int reps = atoi(reps_s);
       cudaEvent_t e0, e1;
       cudaEventCreate(&e0); cudaEventCreate(&e1);
       cudaEventRecord(e0, st);
-      for (int i = 0; i < reps && !rc; ++i) rc = umma_plan_launch(plan, st, true);
+      for (int i = 0; i < reps && !rc; ++i) rc = wgmma_plan_launch(plan, st, true);
       cudaEventRecord(e1, st);
       cudaStreamSynchronize(st);
       float ms = 0;

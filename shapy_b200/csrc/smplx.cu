@@ -1,4 +1,4 @@
-// Fused SMPL-X body-model evaluation for sm_100a.
+// Fused SMPL-X body-model evaluation for sm_90a.
 //
 // Replaces the ~90-launch reference chain (blend_shapes -> vertices2joints -> pose blend ->
 // batch_rigid_transform (54 serial bmm) -> skinning -> landmarks -> J14), reference
@@ -19,8 +19,8 @@
 #include <cmath>
 #include <cstring>
 
+#include "conv.cuh"
 #include "smplx.cuh"
-#include "umma.cuh"
 
 namespace shapy {
 
@@ -144,11 +144,34 @@ struct VertexArgs {
   const float *A, *pfT;
   int B, Bpad, Kp;
   float *vertices, *v_shaped;  // either may be null
+  const __half *pb_hi, *pb_lo;  // pose blend [B][pb_ld] as hi + lo / 2048 (wgmma GEMM); null: pose rows run here
+  int pb_ld;
 };
 
 __device__ __forceinline__ void cp_async16_zfill(void *smem_dst, const void *src, int src_bytes) {
   unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(src_bytes) : "memory");
+}
+
+// posedirs [k][V3] fp32 -> split-fp16 GEMM weights [V3g][Kpad] (the [cout][cin] layout of a 1x1 convolution), x kPoseScale
+__global__ void pack_pose_weights_kernel(const float *__restrict__ posedirs, int V3, int Kp, int Kpad, int V3g,
+                                         __half *__restrict__ hi, __half *__restrict__ lo) {
+  const size_t n = (size_t)V3g * Kpad;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i / Kpad), k = (int)(i % Kpad);
+    const float x = (c < V3 && k < Kp) ? posedirs[(size_t)k * V3 + c] * kPoseScale : 0.f;
+    split_store(x, hi[i], lo[i]);
+  }
+}
+
+// pose feature rows of pfT ([NC + k][Bpad] fp32) -> split-fp16 GEMM activations [B][Kpad], / kPoseScale
+__global__ void pose_features_split_kernel(const float *__restrict__ pfT, int Bpad, int NC, int Kp, int Kpad, int B,
+                                           __half *__restrict__ hi, __half *__restrict__ lo) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * Kpad) return;
+  const int b = i / Kpad, k = i % Kpad;
+  const float x = k < Kp ? pfT[(size_t)(NC + k) * Bpad + b] * (1.0f / kPoseScale) : 0.f;
+  split_store(x, hi[i], lo[i]);
 }
 
 // One tile = 32 vertices (one per lane) x 32 bodies (8 per warp).  All blend-shape rows (shape, expression, pose)
@@ -174,7 +197,7 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
   // row schedule: [0, NB) shape | [NB, NC) expression (only when given) | [NC, NC + Kp) pose (only for vertices)
   const bool posed = a.vertices != nullptr;
   const int n_expr = (a.expr && posed) ? m.NC - m.NB : 0;
-  const int n_rows = m.NB + n_expr + (posed ? a.Kp : 0);
+  const int n_rows = m.NB + n_expr + (posed && !a.pb_hi ? a.Kp : 0);
   auto row_of = [&](int i) { return i < m.NB + n_expr ? i : m.NC + (i - m.NB - n_expr); };
   // chunk boundaries: the first chunk ends exactly after the NB shape rows (v_shaped snapshot)
   auto chunk_begin = [&](int ch) { return ch == 0 ? 0 : m.NB + (ch - 1) * KC; };
@@ -231,6 +254,16 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
     __syncthreads();
   }
   if (!posed || !vok) return;
+  if (a.pb_hi) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int b = b0 + warp * 8 + i;
+      if (b >= a.B) break;
+      const size_t o = (size_t)b * a.pb_ld + 3 * v;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) acc[i][c] += __half2float(a.pb_hi[o + c]) + __half2float(a.pb_lo[o + c]) * kLoInv;
+    }
+  }
   // ---- sparse linear blend skinning: out = sum_j w_vj (A_j . [v_posed; 1])
   float out[8][3];
 #pragma unroll
@@ -430,6 +463,7 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
     for (int k = 0; k < KP; ++k) memcpy(&basis[(size_t)(NC + k) * V3p], d->posedirs + (size_t)k * V3, (size_t)V3 * sizeof(float));
     s.V3p = V3p;
     s.basis = upload(m, basis, err);
+    m->zero_bias = upload(m, std::vector<float>((size_t)(V3 + kPoseV3Align - 1) / kPoseV3Align * kPoseV3Align, 0.f), err);
   }
   // joint regression contracted with the template and the shape basis (fp64 accumulate)
   std::vector<float> Jt((size_t)J * 3), Jd((size_t)J * 3 * NC);
@@ -530,42 +564,6 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
   for (int i = 0; i < s.n_over; ++i) { os[i] = (int)d->source_idxs[i]; ot[i] = (int)d->target_idxs[i]; }
   s.over_src = upload(m, os, err);
   s.over_tgt = upload(m, ot, err);
-  {
-    // ---- operands of the fused tcgen05 LBS kernel (smplx_lbs.cu)
-    const int Vpad = (V + 127) / 128 * 128, KP = (J - 1) * 9, KPpad = (KP + 63) / 64 * 64;
-    s.Vpad = Vpad; s.KPpad = KPpad;
-    const int nKB = KPpad / 32;
-    std::vector<__half> pb((size_t)nKB * 3 * Vpad * 64, __float2half_rn(0.f));
-    for (int k = 0; k < KP; ++k) {
-      const float *row = d->posedirs + (size_t)k * V * 3;
-      const int kb = k / 32, kk = k % 32;
-      for (int v = 0; v < V; ++v)
-        for (int c = 0; c < 3; ++c) {
-          const float x = row[(size_t)v * 3 + c] * kPoseScale;
-          const __half h = __float2half_rn(x);
-          const size_t o = (((size_t)kb * 3 + c) * Vpad + v) * 64 + kk;
-          pb[o] = h;
-          pb[o + 32] = __float2half_rn((x - __half2float(h)) * 2048.0f);
-        }
-    }
-    s.pbasis = upload(m, pb, err);
-    std::vector<float> sp((size_t)(NB + 1) * 3 * Vpad, 0.f);
-    for (int v = 0; v < V; ++v)
-      for (int c = 0; c < 3; ++c) {
-        for (int l = 0; l < NB; ++l) sp[(size_t)(l * 3 + c) * Vpad + v] = d->shapedirs[((size_t)v * 3 + c) * NB + l];
-        sp[(size_t)(NB * 3 + c) * Vpad + v] = d->v_template[(size_t)v * 3 + c];
-      }
-    s.shape_planes = upload(m, sp, err);
-    m->h_lbs_weights.assign(d->lbs_weights, d->lbs_weights + (size_t)V * J);
-    m->h_parents = par;
-    m->fused_ok = false;
-    if (err == cudaSuccess && get_encode()) {
-      cuuint64_t dims[4] = {64, (cuuint64_t)Vpad, 3, (cuuint64_t)nKB};
-      cuuint64_t strides[3] = {128, (cuuint64_t)Vpad * 128, (cuuint64_t)3 * Vpad * 128};
-      cuuint32_t box[4] = {64, 128, 3, 1};
-      m->fused_ok = encode(&m->basis_map, s.pbasis, 4, dims, strides, box, 64);
-    }
-  }
   if (err != cudaSuccess) {
     set_error("shapy_smplx_create: %s", cudaGetErrorString(err));
     shapy_smplx_destroy(m);
@@ -578,7 +576,7 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
 extern "C" void shapy_smplx_destroy(shapy_smplx_t *m) {
   if (!m) return;
   for (void *p : m->allocs) cudaFree(p);
-  for (auto &kv : m->wtiles) if (kv.second.dev) cudaFree(kv.second.dev);
+  for (auto &kv : m->pw) { cudaFree(kv.second.hi); cudaFree(kv.second.lo); }
   delete m;
 }
 
@@ -587,13 +585,65 @@ extern "C" const int32_t *shapy_smplx_faces_i32(const shapy_smplx_t *m) { return
 
 static inline int bpad(int B) { return (B + 31) / 32 * 32; }
 
+static inline int pose_kpad(int Kp) { return (Kp + kPoseKAlign - 1) / kPoseKAlign * kPoseKAlign; }
+static inline int pose_v3g(const SmplxDev &d) { return (d.V * 3 + kPoseV3Align - 1) / kPoseV3Align * kPoseV3Align; }
+
+// workspace of the pose-blend GEMM: activations [B][Kpad] and result [B][V3g], split fp16 (hi, lo) each
+static size_t pose_gemm_bytes(const SmplxDev &d, int B) {
+  return 2 * align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256) +
+         2 * align_up((size_t)B * pose_v3g(d) * sizeof(__half), 256);
+}
+
+// Pose blend (R[1:] - I) . P of all B bodies as one split-fp16 tensor-core GEMM on the wgmma engine, expressed as a
+// 1x1 convolution: "pixels" = bodies, cin = pose features, cout = the 3V vertex coordinates.  Fills va.pb_*.
+static int pose_blend_gemm(const shapy_smplx *m, const float *pfT, int B, int Kp, char *xw, cudaStream_t st,
+                           VertexArgs &va) {
+  const SmplxDev &d = m->d;
+  const int Kpad = pose_kpad(Kp), V3g = pose_v3g(d);
+  shapy_smplx::PoseW pw;
+  {
+    std::lock_guard<std::mutex> lk(m->pw_mu);
+    auto it = m->pw.find(Kpad);
+    if (it == m->pw.end()) {
+      const size_t n = (size_t)V3g * Kpad;
+      SHAPY_CUDA_TRY(cudaMalloc((void **)&pw.hi, n * sizeof(__half)));
+      SHAPY_CUDA_TRY(cudaMalloc((void **)&pw.lo, n * sizeof(__half)));
+      pack_pose_weights_kernel<<<1024, 256, 0, st>>>(d.posedirs, d.V * 3, Kp, Kpad, V3g, pw.hi, pw.lo);
+      SHAPY_LAUNCH_CHECK();
+      m->pw[Kpad] = pw;
+    } else {
+      pw = it->second;
+    }
+  }
+  __half *x_hi = (__half *)xw;
+  __half *x_lo = (__half *)(xw + align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256));
+  char *yw = xw + 2 * align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256);
+  __half *y_hi = (__half *)yw;
+  __half *y_lo = (__half *)(yw + align_up((size_t)B * V3g * sizeof(__half), 256));
+  pose_features_split_kernel<<<ceil_div(B * Kpad, 256), 256, 0, st>>>(pfT, bpad(B), d.NC, Kp, Kpad, B, x_hi, x_lo);
+  SHAPY_LAUNCH_CHECK();
+  ConvW w;
+  w.w_hi = pw.hi; w.w_lo = pw.lo; w.bias = m->zero_bias;
+  w.cin = Kpad; w.cout = V3g; w.ksize = 1; w.stride = 1;
+  ActView in, out;
+  in.hi = x_hi; in.lo = x_lo; in.N = B; in.H = 1; in.W = 1; in.C = Kpad; in.Ctot = Kpad; in.coff = 0;
+  out.hi = y_hi; out.lo = y_lo; out.N = B; out.H = 1; out.W = 1; out.C = V3g; out.Ctot = V3g; out.coff = 0;
+  WgmmaPlan *plan = wgmma_plan_create(w, in, out, nullptr, false);
+  if (!plan) return SHAPY_ERR_UNSUPPORTED;
+  const int rc = wgmma_plan_launch(plan, st, false);
+  wgmma_plan_destroy(plan);
+  if (rc != SHAPY_OK) return rc;
+  va.pb_hi = y_hi; va.pb_lo = y_lo; va.pb_ld = V3g;
+  return SHAPY_OK;
+}
+
 extern "C" size_t shapy_smplx_workspace_bytes(const shapy_smplx_t *m, int B) {
   if (!m || B <= 0) return 0;
   size_t a = align_up((size_t)B * m->d.J * 12 * sizeof(float), 256);
   size_t p = align_up((size_t)((m->d.J - 1) * 9 + m->d.NC) * bpad(B) * sizeof(float), 256);
   size_t l = align_up((size_t)B * sizeof(int), 256);
   size_t j = align_up((size_t)B * m->d.K * 3 * sizeof(float), 256);
-  return a + p + l + j;
+  return a + p + l + j + pose_gemm_bytes(m->d, B);
 }
 
 extern "C" int shapy_decode_rot6d(const float *raw, int n, float *rot, void *stream) {
@@ -620,22 +670,19 @@ extern "C" int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, c
   float *A = (float *)w; w += align_up((size_t)B * d.J * 12 * sizeof(float), 256);
   float *pfT = (float *)w; w += align_up((size_t)((d.J - 1) * 9 + d.NC) * bpad(B) * sizeof(float), 256);
   int *lut = (int *)w; w += align_up((size_t)B * sizeof(int), 256);
-  float *jscratch = (float *)w;
+  float *jscratch = (float *)w; w += align_up((size_t)B * d.K * 3 * sizeof(float), 256);
+  char *xw = w;
   const int Kp = (n_rot - 1) * 9;
-  // fused tcgen05 kernel (pose chain + shape + pose blend + skinning in one launch) when the configuration allows:
-  // no expression coefficients, posed vertices requested, 10 betas, n_rot <= 29
-  bool fused = false;
-  if (vertices && !(d.NE && expr)) {
-    const int rc = launch_lbs_fused(m, betas, rot, n_rot, B, vertices, v_shaped, joints ? joints : jscratch, lut, st);
-    if (rc == SHAPY_OK) fused = true;
-    else if (rc != SHAPY_ERR_UNSUPPORTED) return rc;
-  }
-  if (!fused) {
+  {
     PoseArgs pa{d, betas, d.NE ? expr : nullptr, rot, n_rot, B, bpad(B), Kp, A, pfT, joints ? joints : jscratch, lut};
     smplx_pose_kernel<<<B, 128, 0, st>>>(pa);
     SHAPY_LAUNCH_CHECK();
     if (vertices || v_shaped) {
-      VertexArgs va{d, betas, d.NE ? expr : nullptr, A, pfT, B, bpad(B), Kp, vertices, v_shaped};
+      VertexArgs va{d, betas, d.NE ? expr : nullptr, A, pfT, B, bpad(B), Kp, vertices, v_shaped, nullptr, nullptr, 0};
+      if (vertices && Kp > 0) {
+        const int rc = pose_blend_gemm(m, pfT, B, Kp, xw, st, va);
+        if (rc != SHAPY_OK) return rc;
+      }
       dim3 grid(ceil_div(d.V, TV), ceil_div(B, TB));
       smplx_vertex_kernel<<<grid, 128, 0, st>>>(va);
       SHAPY_LAUNCH_CHECK();

@@ -1,7 +1,5 @@
-// Shared declarations of the SMPL-X kernels (smplx.cu, smplx_lbs.cu).
+// Shared declarations of the SMPL-X kernels (smplx.cu).
 #pragma once
-#include <cuda.h>
-
 #include <map>
 #include <mutex>
 
@@ -30,11 +28,6 @@ struct SmplxDev {
   int *ex_ptr, *ex_col;
   float *ex_val;
   int *over_src, *over_tgt;
-  // ---- packed operands of the fused tcgen05 LBS kernel (smplx_lbs.cu)
-  int Vpad;               /* V rounded up to a multiple of 128 */
-  int KPpad;              /* (J-1)*9 rounded up to a multiple of 64 */
-  __half *pbasis;         /* [KPpad / 32 k-blocks][3 planes][Vpad][hi 32 | lo 32] fp16: posedirs * kPoseScale as hi + lo / 2048 */
-  float *shape_planes;    /* [(NB + 1) * 3][Vpad]: row l*3+c = shapedirs coefficient l, coordinate c; rows NB*3+c = template */
 };
 
 }  // namespace shapy
@@ -42,23 +35,17 @@ struct SmplxDev {
 struct shapy_smplx {
   shapy::SmplxDev d;
   std::vector<void *> allocs;
-  CUtensorMap basis_map;                    // (64, Vpad, 3, KPpad / 32) fp16, box (64, 128, 3, 1), SWIZZLE_128B
-  bool fused_ok = false;                    // the packed operands above exist and the maps encoded
-  // blend-GEMM operand of the fused kernel: skinning weights folded onto the rotated joints (joints >= n_rot carry
-  // their nearest rotated ancestor's transform), built lazily per n_rot from the host copies below
-  std::vector<float> h_lbs_weights;         // (V, J) dense, as given
-  std::vector<int> h_parents;
-  struct WTiles { __half *dev = nullptr; CUtensorMap map; bool ok = false; };
-  mutable std::mutex wmu;
-  mutable std::map<int, WTiles> wtiles;
+  // pose blend on the tensor cores (wgmma): posedirs^T x kPoseScale as split-fp16 [V3g][Kpad] weights, built on first use
+  // per pose-feature width Kp (joints >= n_rot contribute exact zeros, so their rows are left out), and a zero bias
+  struct PoseW { __half *hi = nullptr, *lo = nullptr; };
+  mutable std::mutex pw_mu;
+  mutable std::map<int, PoseW> pw;
+  float *zero_bias = nullptr;   // [V3g]
 };
 
 namespace shapy {
-constexpr float kPoseScale = 1024.0f;       // posedirs entries (~1e-3) are scaled into fp16's normal range
-
-// Fused tcgen05 LBS (smplx_lbs.cu).  Returns SHAPY_ERR_UNSUPPORTED when the configuration is outside what the fused
-// kernel handles (the caller then runs the three-kernel path).
-int launch_lbs_fused(const shapy_smplx *m, const float *betas, const float *rot, int n_rot, int B, float *vertices,
-                     float *v_shaped, float *joints, int *lut, cudaStream_t st);
-
+constexpr float kPoseScale = 1024.0f;   // posedirs entries (~1e-3) are scaled into fp16's normal range
+constexpr int kPoseKAlign = 16;         // pose-feature width padding (wgmma K granularity)
+constexpr int kPoseV3Align = 384;       // 3V padding: a multiple of every cout tile of the wgmma engine
 }  // namespace shapy
+

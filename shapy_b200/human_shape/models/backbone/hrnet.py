@@ -4,8 +4,8 @@ Same class name, constructor argument (the `hrnet` config node), parameter tree 
 same 1 967 state-dict keys as the reference module (hrnet.py:202-288), so a SHAPY_A checkpoint loads
 unmodified.  nn.Conv2d / nn.BatchNorm2d objects are used purely as PARAMETER CONTAINERS: `forward`
 never calls them.  Instead the module tree is compiled (lazily, and again whenever the parameters
-change) into a flat program of fused conv+BN(+residual)(+ReLU) ops that the sm_100a library executes
-(shapy_b200/csrc/hrnet.cu, conv_umma.cu).  There is no PyTorch fallback: CPU tensors raise.
+change) into a flat program of fused conv+BN(+residual)(+ReLU) ops that the sm_90a library executes
+(shapy_b200/csrc/hrnet.cu, conv_wgmma.cu).  There is no PyTorch fallback: CPU tensors raise.
 """
 import os.path as osp
 
@@ -261,7 +261,7 @@ class _Outputs(dict):
 class HighResolutionNet(nn.Module):
     # numeric mode of the compiled plan: 1 = split-fp16 parity mode (fp32-grade), 0 = plain fp16 operands
     precision_mode = 1
-    engine = 0      # 0 = tcgen05 implicit GEMM, 1 = SIMT fp32 (debug cross-check)
+    engine = 0      # 0 = wgmma implicit GEMM, 1 = SIMT fp32 (debug cross-check)
 
     def __init__(self, cfg=None, **kwargs):
         self.inplanes = 64

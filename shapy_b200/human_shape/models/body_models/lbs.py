@@ -1,5 +1,5 @@
 """`lbs()` with the reference signature (regressor/human_shape/models/body_models/lbs.py:99-108),
-evaluated by the fused sm_100a kernels (csrc/smplx.cu).  The reference's own TODO reads "Create merged
+evaluated by the fused sm_90a kernels (csrc/smplx.cu).  The reference's own TODO reads "Create merged
 c++ and CUDA kernel" (lbs.py:97-98)."""
 from collections import defaultdict
 

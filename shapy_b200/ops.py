@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/shapy_b200.h).
 
 PyTorch is used for device memory and streams only: every function takes CUDA fp32 tensors, allocates
-the outputs with torch, and launches the hand-written sm_100a kernels on the current stream.  Nothing
+the outputs with torch, and launches the hand-written sm_90a kernels on the current stream.  Nothing
 here computes with torch ops, and nothing falls back to the CPU: non-CUDA inputs raise.
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-"""Unit parity of the two convolution engines (tcgen05 implicit GEMM / SIMT) against a plain PyTorch fp32
+"""Unit parity of the two convolution engines (wgmma implicit GEMM / SIMT) against a plain PyTorch fp32
 convolution of the same op (cuDNN with TF32 disabled), for every (cin, cout, k, stride, H) family that
 occurs in HRNet-W48 (SURVEY.md 8a) plus ragged sizes."""
 import pytest
@@ -24,7 +24,7 @@ SHAPES = [
     (48, 48, 3, 1, 8, 24, 1),      # non-square small map
     (96, 192, 3, 2, 28, 28, 2),    # stride-2 halo variant, KCH=32, two cout tiles
     (48, 48, 3, 2, 16, 24, 3),     # stride-2 halo variant, non-square, whole-image items
-    (64, 64, 3, 1, 136, 136, 1),   # W > 128 is not tiled by the tcgen05 engine -> unsupported, see below
+    (64, 64, 3, 1, 136, 136, 1),   # W > 128 is not tiled by the wgmma engine -> unsupported, see below
 ]
 
 
@@ -127,7 +127,7 @@ BENCH_SHAPES = [(48, 48, 3, 1, 56), (96, 96, 3, 1, 28), (192, 192, 3, 1, 14), (3
 
 @pytest.mark.parametrize('shape', BENCH_SHAPES)
 def test_conv_split_benchmark_batch(shape):
-    """configs[2] launch configurations: B = 64, split-fp16 mode, tcgen05 engine, with residual."""
+    """configs[2] launch configurations: B = 64, split-fp16 mode, wgmma engine, with residual."""
     from shapy_b200 import ops
     cin, cout, k, stride, H = shape
     x, w, bn, res = _case(cin, cout, k, stride, H, H, 64, seed=2)

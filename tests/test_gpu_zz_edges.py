@@ -1,5 +1,5 @@
 """Edge cases of the public entry points on the GPU: empty batches (torch semantics: empty in, empty out, nothing
-launched), batches that straddle the 32-body groups of the fused LBS kernel, single-face / no-face collision queries,
+launched), batches that straddle the 32-body tiles of the SMPL-X vertex kernel, single-face / no-face collision queries,
 and the argument errors the C ABI reports.  The reference never sees an empty batch on its demo path (its DataLoader
 drops them); torch modules accept one, so the mirror does too."""
 import numpy as np
@@ -67,7 +67,7 @@ def test_empty_batch_backbone_attributes_metrics():
 
 @pytest.mark.parametrize('B', [31, 32, 64, 65, 97])
 def test_lbs_group_boundaries_vs_oracle(env, B):
-    """The fused kernel works on groups of 32 bodies; every row of a batch that ends just before / on / after a
+    """The vertex kernel works on tiles of 32 bodies; every row of a batch that ends just before / on / after a
     group boundary must match the oracle, and must not depend on what else is in the batch."""
     model, packed, ops = env
     g = torch.Generator().manual_seed(100 + B)

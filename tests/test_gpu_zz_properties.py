@@ -1,5 +1,5 @@
-"""Size-independent properties of the posed SMPL-X path at BASELINE's config-4 batch (4 096 bodies, 128 groups of the
-fused tcgen05 kernel), where the oracle is too slow to run:
+"""Size-independent properties of the posed SMPL-X path at BASELINE's config-4 batch (4 096 bodies, 128 body tiles of the
+SMPL-X vertex kernel), where the oracle is too slow to run:
   * with the rotations fixed, lbs() is affine in the shape coefficients (joints, transforms and posed vertices all are),
   * a rotation applied in front of the global orientation rotates every vertex and joint about the pelvis joint
     (the pelvis transform multiplies every chain from the left; lbs.py:242-295)."""

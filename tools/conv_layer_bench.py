@@ -1,6 +1,6 @@
 """Per-layer timing of the HRNet-W48 main convolutions at the bench batch (B=64, 224x224 input):
-SHAPY_CONV_TEST_REPS launches of each plan, average time to stderr.  Optional SHAPY_CONV_PHASES=1 /
-SHAPY_CONV_DEBUG=1 in the environment print the halo kernel's per-role wait counters / tile configuration."""
+SHAPY_CONV_TEST_REPS launches of each plan, average time to stderr.  SHAPY_CONV_DEBUG=1 in the environment prints
+each plan's tile configuration."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ.setdefault('SHAPY_CONV_TEST_REPS', '20')

@@ -1,13 +1,13 @@
 """Same-box GPU baselines SURVEY.md 8d asks for (a tool, not part of bench.py: it executes oracle/ code on the GPU).
 
-  1. The reference's HRNet graph on this B200 through stock PyTorch / cuDNN (oracle.net_oracle.hrnet_forward: the same
+  1. The reference's HRNet graph on this GPU through stock PyTorch / cuDNN (oracle.net_oracle.hrnet_forward: the same
      conv2d / batch_norm / relu / interpolate call sequence as regressor/human_shape/models/backbone/hrnet.py), B = 64,
      224 x 224, three settings: fp32 (TF32 off), TF32 convolutions, fp16 autocast.
   2. The reference's own BVH kernel (oracle/_ref, mesh_mesh_intersect_cuda_op.cu patched for torch 2.11) on the
      measurement query of BASELINE configs[3] (2 plane triangles against the 20 908 body triangles, 3 planes per body),
      next to shapy_mmi_forward on the same inputs and to the fused measurement kernel that replaces all of it.
 
-    python tools/gpu_baselines.py > profiles/rNN_gpu_baselines.json
+    python tools/gpu_baselines.py        # one JSON document on stdout
 """
 import json
 import os

@@ -21,6 +21,11 @@ Everything written here is a small fixture that travels to the GPU box, where
   b2a.npz               reference Polynomial (B2A head) outputs with seeded male / female weights, routed by gender
   p2p.npz               reference v2vhdError (P2P metric) outputs on seeded sparse point regressors and meshes
   v2v.npz               reference PointError(TranslationAlignment / NoAlignment) outputs (`v2v_t` / `v2v`) on two seeded meshes
+  ref_smplx_live.npz    reference SMPL-X forward (ref_shim) of tests/test_oracle_pins.py's seeded bodies
+  ref_weak_persp_to_blender.npz   reference demo.py weak_persp_to_blender on tests/test_writer_cpu.py's inputs
+  ref_keypoint_tensor.{npz,json}  reference KeypointTensor under the tensor methods of tests/test_keypoint_tensor_cpu.py
+  ref_mmi_{plane,soup}.npz        reference mesh_to_mesh_forward (oracle/_ref via oracle/run_ref_mmi.py) collisions on
+                        the inputs of tests/test_gpu_zz_reference_op.py; GPU only: `python tools/make_golden.py mmi`
   preprocess.npz        reference input stage (transf_utils.crop with cv2 + ToTensor + Normalize) on seeded uint8 images:
                         crop windows, crops with OpenCV's portable path (IPP off) and with this container's IPP build
 """
@@ -312,8 +317,80 @@ def p2p_fixture():
     print('p2p.npz', os.path.getsize(os.path.join(G, 'p2p.npz')), 'bytes; mean aligned error', out['mean_aligned'])
 
 
+def smplx_live_fixture():
+    from oracle import smplx_oracle
+    from shapy_b200 import synth
+    model = synth.make_smplx()
+    g = torch.Generator().manual_seed(5)
+    betas = torch.randn(2, 10, generator=g)
+    raw = torch.randn(2, 132, generator=g) * 0.3 + synth.mean_params()[:132]
+    grot, bpose = smplx_oracle.decode_6d(raw[:, :6]), smplx_oracle.decode_6d(raw[:, 6:])
+    ref = ref_shim.smplx_forward_ref(model, betas, grot, bpose)
+    np.savez_compressed(os.path.join(G, 'ref_smplx_live.npz'),
+                        **{k: ref[k].numpy().astype(np.float32) for k in ('vertices', 'joints', 'v_shaped')})
+
+
+def writer_camera_fixture():
+    import ast
+    from collections import defaultdict
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_writer_cpu as tw
+    path = os.path.join(REF, 'regressor', 'demo.py')
+    fn = [n for n in ast.parse(open(path).read()).body if isinstance(n, ast.FunctionDef) and n.name == 'weak_persp_to_blender'][0]
+    ns = {'torch': torch, 'np': np, 'defaultdict': defaultdict}
+    exec(compile(ast.Module(body=[fn], type_ignores=[]), path, 'exec'), ns)     # executed where it lies
+    targets = tw.make_targets(5, np.random.default_rng(2))
+    scale = torch.rand(5, 1, generator=torch.Generator().manual_seed(3)) + 0.5
+    transl = torch.randn(5, 2, generator=torch.Generator().manual_seed(4)) * 0.1
+    r = ns['weak_persp_to_blender'](targets, scale, transl, H=720, W=1280, sensor_width=36, focal_length=5000)
+    np.savez_compressed(os.path.join(G, 'ref_weak_persp_to_blender.npz'), **{k: np.asarray(v) for k, v in r.items()})
+
+
+def keypoint_tensor_fixture():
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_keypoint_tensor_cpu as tk
+    path = os.path.join(REF, 'regressor', 'human_shape', 'models', 'body_models', 'utils.py')
+    src = open(path).read()
+    start = src.index('class KeypointTensor(object):')
+    end = src.index('\nclass ', start + 10) if '\nclass ' in src[start + 10:] else len(src)
+    ns = {'torch': torch}
+    exec(compile(src[start:end], path, 'exec'), ns)                           # executed where it lies
+    b = tk.make(ns['KeypointTensor'])
+    ops = [lambda k: k.view(2, 9), lambda k: k.detach(), lambda k: k.to(torch.float64), lambda k: k.sum(dim=2),
+           lambda k: k.matmul(torch.full((3, 3), 0.5)), lambda k: k.clone().reshape(3, 6), lambda k: k.permute(2, 0, 1)]
+    arrs, meta = {}, []
+    for i, f in enumerate(ops):
+        y = f(b)
+        arrs[f'op{i}'] = y._t.numpy()
+        meta.append(dict(keypoint_names=list(y.keypoint_names), source=y.source, connections=[list(c) for c in y.connections],
+                         part_indices={k: (v.tolist() if torch.is_tensor(v) else v) for k, v in y.part_indices.items()}))
+    arrs['index1'] = b[1].numpy()
+    arrs['numpy'] = b.numpy()
+    np.savez(os.path.join(G, 'ref_keypoint_tensor.npz'), **arrs)
+    json.dump(dict(ops=meta, index1_type=type(b[1]).__name__), open(os.path.join(G, 'ref_keypoint_tensor.json'), 'w'))
+
+
+def mmi_fixtures():
+    """Needs a GPU and oracle/_ref (python oracle/build_ref.py).  Stores the filled slots of the reference's output."""
+    import subprocess
+    import tempfile
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_gpu_zz_reference_op as t
+    for name, (query, target, M) in (('ref_mmi_plane', t.plane_inputs(G)), ('ref_mmi_soup', t.soup_inputs())):
+        with tempfile.TemporaryDirectory() as tmp:
+            inp, outp = os.path.join(tmp, 'in.npz'), os.path.join(tmp, 'out.npz')
+            np.savez(inp, query=query, target=target, max_collisions=np.int64(M))
+            subprocess.run([sys.executable, os.path.join(ROOT, 'oracle', 'run_ref_mmi.py'), inp, outp], check=True)
+            d = np.load(outp)
+            f, bcs = d['faces'], d['bcs']
+        keep = np.nonzero(f >= 0)
+        np.savez_compressed(os.path.join(G, f'{name}.npz'), shape=np.int64(f.shape), idx=np.stack(keep, 1).astype(np.int32),
+                            faces=f[keep].astype(np.int32), bcs=bcs[keep].astype(np.float32), query=query)
+
+
 if __name__ == '__main__':
-    which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v']
+    which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'smplx_live', 'camera',
+                             'keypoint']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -331,3 +408,11 @@ if __name__ == '__main__':
         p2p_fixture()
     if 'v2v' in which:
         v2v_fixture()
+    if 'smplx_live' in which:
+        smplx_live_fixture()
+    if 'camera' in which:
+        writer_camera_fixture()
+    if 'keypoint' in which:
+        keypoint_tensor_fixture()
+    if 'mmi' in which:
+        mmi_fixtures()
