@@ -19,6 +19,10 @@
  *                                                   + src/mesh_mesh_intersect_cuda_op.cu:969-1079
  *   shapy_head_*         IterativeRegression.forward regressor/human_shape/models/common/networks.py:536-592
  *   shapy_hrnet_*        HighResolutionNet.forward  regressor/human_shape/models/backbone/hrnet.py:426-498
+ *   shapy_p2p_error      v2vhdError.__call__        regressor/human_shape/utils/metrics.py:368-456
+ *   shapy_v2v_error      PointError, translation / no alignment   metrics.py:85-98, 232-277, 335-366
+ *   shapy_point_error_aligned   PointError, scale / root alignment   metrics.py:173-229, 279-303, 335-366
+ *   shapy_regress_points        J14 joint regression of mpjpe14    regressor/human_shape/evaluation.py:161-190
  */
 #ifndef SHAPY_B200_H_
 #define SHAPY_B200_H_
@@ -271,6 +275,30 @@ int shapy_p2p_error(const int *in_row_ptr, const int *in_col, const float *in_va
  * input / target: device (B, V, 3) fp32; error (B, V), mean_error (B); workspace >= shapy_p2p_workspace_bytes(B, V). */
 int shapy_v2v_error(const float *input_vertices, const float *target_vertices, int batch, int num_verts, int align,
                     float *error, float *mean_error, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Point error between point sets of the same topology after a scale or root alignment: PointError with ScaleAlignment /
+ * RootAlignment, regressor/human_shape/utils/metrics.py:173-229, 279-303, 335-366 (evaluation.py:595-620: the
+ * scale-corrected `v2v_t` and the root-aligned `mpjpe` / `mpjpe14`).  Per body b:
+ *   SHAPY_ALIGN_SCALE  s = sqrt(var2 / var1) from the centred sums of squares of est / gt about their means mu1 / mu2;
+ *                      error[b][p] = |s est + (mu2 - s mu1) - gt|.  var1 == 0 is not guarded (inf / NaN, as in fp32).
+ *   SHAPY_ALIGN_ROOT   r_est, r_gt = means of the points listed in `roots` (numpy indexing: -P <= index < P);
+ *                      error[b][p] = |(est - r_est) - (gt - r_gt)|.  An empty list gives NaN, numpy's mean of an empty axis.
+ * input_points / target_points : device (B, P, 3) fp32, points first;  roots : HOST int array of num_roots <=
+ * SHAPY_MAX_ROOTS entries, checked in the call and passed to the kernel by value (ignored in scale mode);
+ * error (B, P), mean_error (B) : device fp32;  workspace >= shapy_point_error_workspace_bytes(B) (per-body statistics).
+ * Every reduction has a fixed order: the result of a body is bit-identical run to run and whatever else is in the batch. */
+enum { SHAPY_ALIGN_SCALE = 1, SHAPY_ALIGN_ROOT = 2 };
+#define SHAPY_MAX_ROOTS 16
+size_t shapy_point_error_workspace_bytes(int batch);
+int shapy_point_error_aligned(const float *input_points, const float *target_points, int batch, int num_points, int mode,
+                              const int *roots, int num_roots, float *error, float *mean_error, void *workspace,
+                              size_t workspace_bytes, void *stream);
+
+/* Sparse point regression: points (B, P, 3) = (P x V regressor) times vertices (B, V, 3), per body; the J14 joints of
+ * `mpjpe14` (evaluation.py:161-190, np.einsum('jv,bvn->bjn', J14_regressor, vertices)).  row_ptr int32 [P+1], col
+ * int32 [nnz] (< V), val fp32 [nnz]: device CSR;  vertices, points : device fp32. */
+int shapy_regress_points(const int *row_ptr, const int *col, const float *val, const float *vertices, int batch,
+                         int num_points, int num_verts, float *points, void *stream);
 
 #ifdef __cplusplus
 }

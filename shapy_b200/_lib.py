@@ -50,6 +50,7 @@ class ImageDesc(C.Structure):
 
 
 OP_STEM, OP_CONV, OP_FUSE, OP_POOL = 0, 1, 2, 3
+ALIGN_SCALE, ALIGN_ROOT, MAX_ROOTS = 1, 2, 16      # SHAPY_ALIGN_*, SHAPY_MAX_ROOTS
 
 _SIGS = {
     'shapy_last_error': (C.c_char_p, []),
@@ -92,6 +93,10 @@ _SIGS = {
     'shapy_p2p_workspace_bytes': (c_size_t, [c_int, c_int]),
     'shapy_p2p_error': (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'shapy_v2v_error': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'shapy_point_error_workspace_bytes': (c_size_t, [c_int]),
+    'shapy_point_error_aligned': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, C.POINTER(c_int), c_int, c_void_p, c_void_p,
+                                          c_void_p, c_size_t, c_void_p]),
+    'shapy_regress_points': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'shapy_conv_test': (c_int, [C.POINTER(ConvDesc), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                 c_void_p, c_void_p]),
 }

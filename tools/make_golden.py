@@ -21,6 +21,8 @@ Everything written here is a small fixture that travels to the GPU box, where
   b2a.npz               reference Polynomial (B2A head) outputs with seeded male / female weights, routed by gender
   p2p.npz               reference v2vhdError (P2P metric) outputs on seeded sparse point regressors and meshes
   v2v.npz               reference PointError(TranslationAlignment / NoAlignment) outputs (`v2v_t` / `v2v`) on two seeded meshes
+  align.npz             reference PointError(ScaleAlignment / RootAlignment) outputs on seeded meshes and joints, and mpjpe14
+                        end to end through a seeded dense J14 regressor
   ref_smplx_live.npz    reference SMPL-X forward (ref_shim) of tests/test_oracle_pins.py's seeded bodies
   ref_weak_persp_to_blender.npz   reference demo.py weak_persp_to_blender on tests/test_writer_cpu.py's inputs
   ref_keypoint_tensor.{npz,json}  reference KeypointTensor under the tensor methods of tests/test_keypoint_tensor_cpu.py
@@ -33,6 +35,7 @@ import hashlib
 import json
 import os
 import sys
+import warnings
 
 import numpy as np
 import torch
@@ -269,6 +272,51 @@ def v2v_fixture():
     print('v2v.npz', os.path.getsize(os.path.join(G, 'v2v.npz')), 'bytes; mean aligned error', out['error_aligned'].mean())
 
 
+def align_fixture():
+    """Runs the reference's own PointError with ScaleAlignment and RootAlignment (metrics.py:173-229, 279-303, 335-366):
+    the scale-corrected `v2v_t` on two seeded same-topology meshes far from the origin (float32, as the evaluator passes
+    them), the root-aligned joint error for several root lists, and mpjpe14 end to end (evaluation.py:161-190, 616-620) with
+    a seeded dense float64 J14 regressor."""
+    mod = _load_ref_metrics()
+    rng = np.random.default_rng(79)
+    B, V, J = 3, 1500, 14
+    offset = np.array([0.3, 0.4, 2.5])
+    est = rng.normal(0, 0.4, (B, V, 3)).astype(np.float32)
+    gt = (1.1 * est + rng.normal(0, 0.02, (B, V, 3)) + offset).astype(np.float32)
+    out = dict(est=est, gt=gt)
+    out['error_scale'] = np.asarray(mod.PointError(mod.build_alignment('scale'))(est.copy(), gt.copy()), np.float64)
+    j_est = (rng.normal(0, 0.3, (B, J, 3)) + offset).astype(np.float32)
+    j_gt = (j_est + rng.normal(0, 0.03, (B, J, 3)) + [0.05, -0.02, 0.1]).astype(np.float32)
+    out.update(j_est=j_est, j_gt=j_gt)
+    for tag, root in ROOT_CASES:
+        pe = mod.PointError(mod.build_alignment('root', root=[0]))
+        pe.set_root(list(root))                         # as _compute_mpjpe does (evaluation.py:146-153)
+        with warnings.catch_warnings(), np.errstate(invalid='ignore'):
+            warnings.simplefilter('ignore', RuntimeWarning)           # the empty list: "Mean of empty slice"
+            out[f'error_root_{tag}'] = np.asarray(pe(j_est.copy(), j_gt.copy()), np.float64)
+        out[f'root_{tag}'] = np.array(root, np.int64)
+    # mpjpe14: a J14-like regressor with 32 positive weights per row summing to 1, float32-representable values stored as
+    # float64 (the dtype of the regressor pickle); the einsum line of evaluation.py:183-184 on float32 vertices
+    J14 = np.zeros((J, V))
+    for j in range(J):
+        J14[j, rng.choice(V, 32, replace=False)] = rng.dirichlet(np.ones(32)).astype(np.float32)
+    verts = (est + offset).astype(np.float32)
+    est_joints_np = np.einsum('jv,bvn->bjn', J14, verts)
+    j14_gt = (est_joints_np * 1.05 + rng.normal(0, 0.02, (B, J, 3))).astype(np.float32)
+    out.update(j14=J14, j14_verts=verts, j14_gt=j14_gt, j14_joints=est_joints_np)
+    for tag, name in (('root', 'root'), ('scale', 'scale')):
+        pe = mod.PointError(mod.build_alignment(name, root=[2, 3]))     # evaluation.py:616-619
+        out[f'error_mpjpe14_{tag}'] = np.asarray(pe(est_joints_np, j14_gt), np.float64)
+    np.savez_compressed(os.path.join(G, 'align.npz'), **out)
+    print('align.npz', os.path.getsize(os.path.join(G, 'align.npz')), 'bytes; mean scale error', out['error_scale'].mean(),
+          'mean mpjpe14 root error', out['error_mpjpe14_root'].mean())
+
+
+# (tag, root list) of the root-aligned cases in align.npz: mpjpe14's [2, 3], the default [0], a negative index and the
+# empty list the evaluator's default `root_joints = ()` gives (NaN)
+ROOT_CASES = (('r23', [2, 3]), ('r0', [0]), ('rm1', [-1]), ('rempty', []))
+
+
 def p2p_fixture():
     """Runs the reference's own v2vhdError (regressor/human_shape/utils/metrics.py:368-456, loaded by path behind stubs of
     open3d / .np_utils / .typing) on seeded sparse point regressors (3 barycentric weights per point) and meshes, in
@@ -389,8 +437,8 @@ def mmi_fixtures():
 
 
 if __name__ == '__main__':
-    which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'smplx_live', 'camera',
-                             'keypoint']
+    which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
+                             'camera', 'keypoint']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -408,6 +456,8 @@ if __name__ == '__main__':
         p2p_fixture()
     if 'v2v' in which:
         v2v_fixture()
+    if 'align' in which:
+        align_fixture()
     if 'smplx_live' in which:
         smplx_live_fixture()
     if 'camera' in which:
