@@ -206,7 +206,8 @@ int shapy_hrnet_read_slot(shapy_hrnet_t *p, int slot, float *dst, void *stream);
 double shapy_hrnet_flops(const shapy_hrnet_t *p, int batch, int height, int width);
 
 /* Standalone conv for unit tests of the implicit-GEMM kernel: x (B,H,W,Cin) fp32 NHWC device,
- * y (B,Ho,Wo,Cout) fp32 NHWC device, res optional (same shape as y). */
+ * y (B,Ho,Wo,Cout) fp32 NHWC device, res optional (same shape as y).  engine: 0 = wgmma with the path the network
+ * would take, 1 = SIMT, 2 = wgmma per-tap path, 3 = wgmma halo-resident path (error where it does not apply). */
 int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, const float *res, int batch, int height,
                     int width, int relu, int mode, int engine, float *y, void *stream);
 

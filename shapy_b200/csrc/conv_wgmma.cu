@@ -7,7 +7,15 @@
 //     tap; out-of-image rows / columns are ZERO-FILLED by the TMA unit = the padding (no im2col, no halo storage).
 //     Stride-2 layers use four parity views of the same plane so every tap is again a dense box.  Channel counts that
 //     are not a multiple of 64 still use 64-channel boxes: TMA zero-fills the channels past cin of both operands.
+//   * Halo path (3x3 stride 1, one image per tile): a work item is TH output rows x the full width, computed on the
+//     padded "wide" grid of pitch Wp = W + 2 (tile row r = output (h0 + r / Wp, r % Wp); columns >= W are computed and
+//     dropped by the epilogue).  Each 64-channel block is loaded ONCE with its halo as one (64, Wp, TH + 2) box at
+//     origin (-1, h0 - 1) into a separate halo ring; tap (ky, kx) is the same buffer read from row ky * Wp + kx on (the
+//     descriptor start moves by whole 128-byte rows, the swizzle is a function of the absolute address).  Activations
+//     then cross L2 -> shared memory ~1.4x per channel block instead of 9x; only the weights stream per (tap, block).
 //   * B: 3-D TMA box of the pre-packed [tap][cout][cin] fp16 weights (BN scale folded in).
+//   * k16 steps that lie wholly past cin (the zero-filled tail of the last channel block, e.g. 1 of 4 at cin 48) are
+//     not issued.
 //   * Both operands land in the canonical K-major SWIZZLE_128B layout the wgmma shared-memory descriptor names, so no
 //     thread touches operand data.
 //   * warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = consumers: each issues wgmma m64nNk16 for
@@ -23,6 +31,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "conv.cuh"
 #include "tma.cuh"
@@ -41,10 +50,13 @@ struct alignas(64) WgmmaParams {
   int tiles_w, tiles_h, tiles_n;
   int cin, cout, ksize, stride;
   int kpt;                       // k-blocks per tap = ceil(cin / KCH)
-  int stages;
+  int ks_last;                   // k16 steps of the last k-block that hold channels < cin
+  int stages;                    // (A +) B ring slots
+  int hstages;                   // halo path: halo ring slots
   int relu;
   int pdl_late;                  // 1: release the programmatic dependents when this CTA starts its LAST tile, not at entry
   uint32_t a_bytes, b_bytes, b_stride;  // per k-block: TMA bytes of A / B, smem pitch of the B_hi(+B_lo) block
+  uint32_t h_plane;              // halo path: smem pitch of one halo plane (hi or lo)
   const float *bias;
   __half *out_hi, *out_lo;
   int out_ctot, out_coff;
@@ -55,24 +67,36 @@ struct alignas(64) WgmmaParams {
 constexpr int kThreads = 384;                // producer warpgroup + two consumer warpgroups
 constexpr int kProdRegs = 40, kConsRegs = 232;
 
-template <bool SPLIT, int NT>
+template <bool SPLIT, int NT, bool HALO>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_constant__ WgmmaParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int NACC = (SPLIT ? 2 * NT : NT) / 2;   // fp32 accumulators per thread: [D0 | D1] of a 64 x NT(x2) tile
   constexpr int NLO = SPLIT ? NT / 2 : 1;           // A_lo . B_hi, kept apart: wgmma pipelines only disjoint or equal D
+  constexpr int PARTS = SPLIT ? 2 : 1;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t A_BLK = 128 * KCH * 2;
-  const uint32_t kblk_bytes = A_BLK * (SPLIT ? 2 : 1) + p.b_stride;   // one stage = one k-block of one tap
-  const uint32_t bar_base = smem_base + kblk_bytes * p.stages;
+  // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B] [mbarriers]
+  const uint32_t h_stage = p.h_plane * PARTS;
+  const uint32_t ring_base = smem_base + (HALO ? h_stage * p.hstages : 0u);
+  const uint32_t kblk_bytes = (HALO ? 0u : A_BLK * PARTS) + p.b_stride;   // one stage = one k-block of one tap
+  const uint32_t bar_base = ring_base + kblk_bytes * p.stages;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
+  auto hfull_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
+  auto hempty_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + p.hstages + s); };
   const int wg = threadIdx.x >> 7;
   const int n_tiles = p.cout / NT;
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * n_tiles;
-  const int iters = p.ksize * p.ksize * p.kpt;
+  const int taps = p.ksize * p.ksize;
+  const int iters = taps * p.kpt;
+  // k-block `it` of a tile: tap-major on the per-tap path, channel-block-major on the halo path (one halo load per block)
+  auto decode = [&](int it, int &tap, int &cb) {
+    if (HALO) { cb = it / taps; tap = it - cb * taps; } else { tap = it / p.kpt; cb = it - tap * p.kpt; }
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
+    for (int s = 0; s < (HALO ? p.hstages : 0); ++s) { mbar_init(hfull_bar(s), 1); mbar_init(hempty_bar(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -93,31 +117,43 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
     // ===================================================================== TMA producer
     setmaxnreg_dec<kProdRegs>();
     if (threadIdx.x < 32 && elect_one()) {
-      int s = 0;
-      uint32_t ph = 0;
+      int s = 0, hs = 0;
+      uint32_t ph = 0, hph = 0;
       const int pad = p.ksize / 2;
-      const uint32_t tx = (p.a_bytes + p.b_bytes) * (SPLIT ? 2u : 1u);
+      const uint32_t tx = (HALO ? p.b_bytes : p.a_bytes + p.b_bytes) * PARTS;
       for (int id = blockIdx.x; id < total_tiles; id += gridDim.x) {
         int w0, h0, n0, c_out0;
         tile_coords(id, w0, h0, n0, c_out0);
         if (p.pdl_late && id + (int)gridDim.x >= total_tiles) pdl_launch_dependents();   // last tile of this CTA
 #pragma unroll 1
         for (int it = 0; it < iters; ++it) {
-          const int tap = it / p.kpt, c0 = (it % p.kpt) * KCH;
-          const int ky = tap / p.ksize, kx = tap % p.ksize;
-          int mi = 0, x, y;
-          if (p.stride == 1) {
-            x = w0 + kx - pad; y = h0 + ky - pad;
-          } else {  // input row 2*oh + ky - 1: ky=0 -> odd rows, index oh-1; ky=1 -> even rows, oh; ky=2 -> odd rows, oh
-            mi = (ky != 1) * 2 + (kx != 1);
-            x = w0 + (kx == 0 ? -1 : 0); y = h0 + (ky == 0 ? -1 : 0);
+          int tap, cb;
+          decode(it, tap, cb);
+          const int c0 = cb * KCH;
+          if (HALO && tap == 0) {   // the channel block with its halo, once for all nine taps
+            mbar_wait(hempty_bar(hs), hph ^ 1);
+            mbar_expect_tx(hfull_bar(hs), p.a_bytes * PARTS);
+            const uint32_t hb = smem_base + h_stage * hs;
+            tma_load_4d(hb, &p.a_hi[0], hfull_bar(hs), c0, w0 - 1, h0 - 1, n0);
+            if (SPLIT) tma_load_4d(hb + p.h_plane, &p.a_lo[0], hfull_bar(hs), c0, w0 - 1, h0 - 1, n0);
+            if (++hs == p.hstages) { hs = 0; hph ^= 1; }
           }
           mbar_wait(empty_bar(s), ph ^ 1);
           mbar_expect_tx(full_bar(s), tx);
-          const uint32_t kb = smem_base + kblk_bytes * s;
-          tma_load_4d(kb, &p.a_hi[mi], full_bar(s), c0, x, y, n0);
-          if (SPLIT) tma_load_4d(kb + A_BLK, &p.a_lo[mi], full_bar(s), c0, x, y, n0);
-          const uint32_t bb = kb + A_BLK * (SPLIT ? 2 : 1);
+          const uint32_t kb = ring_base + kblk_bytes * s;
+          if (!HALO) {
+            const int ky = tap / p.ksize, kx = tap % p.ksize;
+            int mi = 0, x, y;
+            if (p.stride == 1) {
+              x = w0 + kx - pad; y = h0 + ky - pad;
+            } else {  // input row 2*oh + ky - 1: ky=0 -> odd rows, index oh-1; ky=1 -> even rows, oh; ky=2 -> odd rows, oh
+              mi = (ky != 1) * 2 + (kx != 1);
+              x = w0 + (kx == 0 ? -1 : 0); y = h0 + (ky == 0 ? -1 : 0);
+            }
+            tma_load_4d(kb, &p.a_hi[mi], full_bar(s), c0, x, y, n0);
+            if (SPLIT) tma_load_4d(kb + A_BLK, &p.a_lo[mi], full_bar(s), c0, x, y, n0);
+          }
+          const uint32_t bb = kb + (HALO ? 0u : A_BLK * PARTS);
           tma_load_3d(bb, &p.b_hi, full_bar(s), c0, c_out0, tap);
           if (SPLIT) tma_load_3d(bb + p.b_bytes, &p.b_lo, full_bar(s), c0, c_out0, tap);   // directly after the hi rows
           if (++s == p.stages) { s = 0; ph ^= 1; }
@@ -129,8 +165,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
     setmaxnreg_inc<kConsRegs>();
     const int cw = wg - 1;                        // rows 64 cw .. 64 cw + 63 of the tile
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
-    int s = 0;
-    uint32_t ph = 0;
+    int s = 0, hs = 0;
+    uint32_t ph = 0, hph = 0;
     float acc[NACC], acl[NLO];
     for (int id = blockIdx.x; id < total_tiles; id += gridDim.x) {
       int w0, h0, n0, c_out0;
@@ -139,36 +175,66 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
 #pragma unroll
       for (int i = 0; i < NLO; ++i) acl[i] = 0.f;
-      int prev = -1;
+      int prev = -1, prev_h = -1;                 // stages the last committed wgmma group reads (prev_h: halo, if its last)
 #pragma unroll 1
       for (int it = 0; it < iters; ++it) {
+        int tap, cb;
+        decode(it, tap, cb);
+        const int nks = cb == p.kpt - 1 ? p.ks_last : KCH / 16;
+        uint32_t a_addr, a_lo_off;
+        if (HALO) {
+          if (tap == 0) mbar_wait(hfull_bar(hs), hph);
+          // tap (ky, kx): the halo rows from ky * Wp + kx on (p.TW is the pitch Wp of the padded grid)
+          a_addr = smem_base + h_stage * hs + (uint32_t)(cw * 64 + (tap / 3) * p.TW + tap % 3) * (KCH * 2);
+          a_lo_off = p.h_plane;
+        }
         mbar_wait(full_bar(s), ph);
-        const uint32_t kb = smem_base + kblk_bytes * s;
-        const uint64_t a = wgmma_desc<KCH>(kb + cw * 64 * KCH * 2);
-        const uint64_t al = wgmma_desc<KCH>(kb + A_BLK + cw * 64 * KCH * 2);
-        const uint64_t b = wgmma_desc<KCH>(kb + A_BLK * (SPLIT ? 2 : 1));
+        const uint32_t kb = ring_base + kblk_bytes * s;
+        if (!HALO) { a_addr = kb + cw * 64 * KCH * 2; a_lo_off = A_BLK; }
+        const uint64_t a = wgmma_desc<KCH>(a_addr);
+        const uint64_t al = wgmma_desc<KCH>(a_addr + a_lo_off);
+        const uint64_t b = wgmma_desc<KCH>(kb + (HALO ? 0u : A_BLK * PARTS));
 #pragma unroll
         for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
 #pragma unroll
         for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
         wgmma_fence();
+        // the first nks k16 steps (channels past cin are zero-filled, nothing to add): one straight-line wgmma run and
+        // its commit per count, so no branch joins inside a group (a join there makes ptxas add a dummy wgmma)
+        auto issue = [&](auto nks_c) {
 #pragma unroll
-        for (int ks = 0; ks < KCH / 16; ++ks) {   // +32 bytes along K = +2 descriptor units
-          if (SPLIT) {
-            wgmma_f16<2 * NT>(acc, a + 2 * ks, b + 2 * ks, 1);   // [D0 | D1] += A_hi . [B_hi | B_lo]^T
-            wgmma_f16<NT>(acl, al + 2 * ks, b + 2 * ks, 1);       // D1' += A_lo . B_hi^T
-          } else {
-            wgmma_f16<NT>(acc, a + 2 * ks, b + 2 * ks, 1);
+          for (int ks = 0; ks < decltype(nks_c)::value; ++ks) {   // +32 bytes along K = +2 descriptor units
+            if (SPLIT) {
+              wgmma_f16<2 * NT>(acc, a + 2 * ks, b + 2 * ks, 1);   // [D0 | D1] += A_hi . [B_hi | B_lo]^T
+              wgmma_f16<NT>(acl, al + 2 * ks, b + 2 * ks, 1);       // D1' += A_lo . B_hi^T
+            } else {
+              wgmma_f16<NT>(acc, a + 2 * ks, b + 2 * ks, 1);
+            }
           }
+          wgmma_commit();
+        };
+        static_assert(KCH / 16 == 4, "k16 steps per k-block");
+        switch (nks) {
+          case 1: issue(std::integral_constant<int, 1>()); break;
+          case 2: issue(std::integral_constant<int, 2>()); break;
+          case 3: issue(std::integral_constant<int, 3>()); break;
+          default: issue(std::integral_constant<int, 4>()); break;
         }
-        wgmma_commit();
 #pragma unroll
         for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
 #pragma unroll
         for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
         wgmma_wait<1>();                          // the previous stage's wgmmas have read their operands
-        if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+        if (prev >= 0 && t == 0) {
+          mbar_arrive(empty_bar(prev));
+          if (prev_h >= 0) mbar_arrive(hempty_bar(prev_h));
+        }
         prev = s;
+        prev_h = -1;
+        if (HALO && tap == taps - 1) {            // the last tap of this halo buffer
+          prev_h = hs;
+          if (++hs == p.hstages) { hs = 0; hph ^= 1; }
+        }
         if (++s == p.stages) { s = 0; ph ^= 1; }
       }
       wgmma_wait<0>();
@@ -176,7 +242,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
 #pragma unroll
       for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
-      if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+      if (prev >= 0 && t == 0) {
+        mbar_arrive(empty_bar(prev));
+        if (prev_h >= 0) mbar_arrive(hempty_bar(prev_h));
+      }
 
       // ---- epilogue: this thread holds rows r0 and r0 + 8, two adjacent columns of every 8-column group
       const int q4 = lane & 3;
@@ -240,10 +309,22 @@ static int sm_count() {
 struct WgmmaPlan {
   WgmmaParams p;
   int NT;
-  bool split;
+  bool split, halo;
   dim3 grid;
   size_t smem;
+  double tma_bytes, mma_flops;   // per launch, as planned: TMA loads of both operands, tensor-core FLOPs issued
 };
+
+// SHAPY_CONV_HALO=0: every plan of WGMMA_AUTO takes the per-tap path
+static bool halo_enabled() {
+  static const bool v = []() { const char *e = getenv("SHAPY_CONV_HALO"); return !(e && e[0] == '0'); }();
+  return v;
+}
+
+void wgmma_plan_stats(const WgmmaPlan *pl, double *tma_bytes, double *mma_flops) {
+  *tma_bytes = pl->tma_bytes;
+  *mma_flops = pl->mma_flops;
+}
 
 static const int kNts[] = {128, 96, 64, 48, 32, 16};   // cout tiles with a kernel instantiation
 
@@ -256,7 +337,8 @@ bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out) {
   return get_encode() != nullptr;
 }
 
-WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu) {
+WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
+                             WgmmaPath path) {
   if (!wgmma_supported(w, in, out)) {
     set_error("wgmma_plan_create: unsupported convolution (cin %d cout %d k %d s %d)", w.cin, w.cout, w.ksize, w.stride);
     return nullptr;
@@ -265,6 +347,7 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   memset(&pl->p, 0, sizeof(pl->p));
   WgmmaParams &p = pl->p;
   const bool split = in.lo != nullptr;
+  const int PARTS = split ? 2 : 1;
   pl->split = split;
   const int sms = sm_count();
   p.N = out.N; p.Ho = out.H; p.Wo = out.W;
@@ -274,6 +357,39 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   p.tiles_w = ceil_div(out.W, p.TW); p.tiles_h = ceil_div(out.H, p.TH); p.tiles_n = ceil_div(out.N, p.TN);
   p.cin = w.cin; p.cout = w.cout; p.ksize = w.ksize; p.stride = w.stride;
   p.kpt = ceil_div(w.cin, KCH);
+  p.ks_last = (w.cin - (p.kpt - 1) * KCH) / 16;
+  // Halo path: 3x3 stride 1, bands of TH rows of one image on the padded grid of pitch Wp.  TH is balanced over the
+  // image (56 -> 2, 28 -> 4, 14 -> 7 rather than 8).  Taken where it is not more M tiles than the per-tap tiling and
+  // loads fewer activation bytes; multi-image per-tap tiles (7 x 7 maps) stay per-tap.
+  // A halo slot holds the rows the furthest tap reads, 128 + 2 Wp + 2: rows past the (TH + 2) Wp the TMA writes are
+  // stale, but only discarded output rows read them (wgmma rows are independent).
+  const int Wp = out.W + 2;
+  const uint32_t h_plane = (uint32_t)align_up((size_t)(128 + 2 * Wp + 2) * KCH * 2, 1024);
+  {
+    // two halo slots and at least two weight slots of the widest cout tile must fit the shared-memory budget
+    const size_t b_max = align_up((size_t)std::min(w.cout, split ? 96 : 128) * KCH * 2 * PARTS, 1024);
+    const bool possible = w.ksize == 3 && w.stride == 1 && Wp <= 128 && 2 * (h_plane * PARTS + b_max) <= 216 * 1024;
+    bool better = false;
+    int th = 0;
+    if (possible) {
+      const int per = 128 / Wp;
+      th = ceil_div(out.H, ceil_div(out.H, per));
+      const double pt_tiles = (double)p.tiles_w * p.tiles_h * p.tiles_n, h_tiles = (double)ceil_div(out.H, th) * out.N;
+      const double pt_a = pt_tiles * 9 * p.TW * p.TH * p.TN, h_a = h_tiles * Wp * (th + 2);   // rows loaded per k-block
+      better = p.TN == 1 && h_tiles <= pt_tiles && h_a < pt_a;
+    }
+    if (path == WGMMA_HALO && !possible) {
+      set_error("wgmma_plan_create: no halo path for cin %d cout %d k %d s %d %dx%d", w.cin, w.cout, w.ksize, w.stride,
+                out.H, out.W);
+      delete pl;
+      return nullptr;
+    }
+    pl->halo = path == WGMMA_HALO || (path == WGMMA_AUTO && better && halo_enabled());
+    if (pl->halo) {
+      p.TW = Wp; p.TH = th; p.TN = 1;
+      p.tiles_w = 1; p.tiles_h = ceil_div(out.H, th); p.tiles_n = out.N;
+    }
+  }
   {
     // cout tile: balance SM utilisation (tiles per CTA round) against the per-wgmma operand cost.  A 128-row tile is two
     // m64nNk16 per k-step; each reads 2 KB of A and N x 32 B of B from shared memory (128 B/cycle) and needs N / 2
@@ -293,22 +409,42 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   }
   p.relu = relu;
   p.pdl_late = 1;
-  const int rows = p.TW * p.TH * p.TN;
-  p.a_bytes = (uint32_t)rows * KCH * 2;
+  // per k-block TMA bytes of one plane: the A box (halo path: the band with its halo rows) and the weight box
+  const int a_rows = pl->halo ? p.TW * (p.TH + 2) : p.TW * p.TH * p.TN;
+  p.a_bytes = (uint32_t)a_rows * KCH * 2;
   p.b_bytes = (uint32_t)pl->NT * KCH * 2;
-  p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * (split ? 2 : 1), 1024);
-  const size_t stage = 128u * KCH * 2 * (split ? 2 : 1) + p.b_stride;
+  p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * PARTS, 1024);
   // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory
-  p.stages = (int)std::max<size_t>(2, std::min<size_t>(8, (216 * 1024) / stage));
-  pl->smem = stage * p.stages + 16 * p.stages + 1024;
+  if (pl->halo) {
+    p.h_plane = h_plane;
+    p.hstages = 2;
+    const size_t halo = (size_t)h_plane * PARTS * p.hstages;
+    p.stages = (int)std::min<size_t>(8, (216 * 1024 - halo) / p.b_stride);
+    pl->smem = halo + (size_t)p.b_stride * p.stages + 16 * (p.stages + p.hstages) + 1024;
+  } else {
+    const size_t stage = 128u * KCH * 2 * PARTS + p.b_stride;
+    p.stages = (int)std::max<size_t>(2, std::min<size_t>(8, (216 * 1024) / stage));
+    pl->smem = stage * p.stages + 16 * p.stages + 1024;
+  }
   p.bias = w.bias;
   p.out_hi = out.hi; p.out_lo = out.lo; p.out_ctot = out.Ctot; p.out_coff = out.coff;
   p.res_hi = res ? res->hi : nullptr; p.res_lo = res ? res->lo : nullptr;
   p.res_ctot = res ? res->Ctot : 0; p.res_coff = res ? res->coff : 0;
-  pl->grid = dim3(even_grid(p.tiles_w * p.tiles_h * p.tiles_n * (w.cout / pl->NT), sms), 1);
+  const int items = p.tiles_w * p.tiles_h * p.tiles_n * (w.cout / pl->NT);
+  pl->grid = dim3(even_grid(items, sms), 1);
+  {
+    const int taps = w.ksize * w.ksize;
+    const double a_loads = pl->halo ? p.kpt : taps * p.kpt;   // A boxes per work item
+    pl->tma_bytes = (double)items * PARTS * (a_loads * p.a_bytes + (double)taps * p.kpt * p.b_bytes);
+    const double k = (double)taps * ((p.kpt - 1) * KCH + p.ks_last * 16);   // K actually issued per work item
+    pl->mma_flops = (double)items * 2.0 * 128 * pl->NT * k * (split ? 3 : 1);
+  }
   if (getenv("SHAPY_CONV_DEBUG"))
-    fprintf(stderr, "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: NT %d tile %dx%dx%d grid %d stages %d\n", w.cin, w.cout,
-            w.ksize, w.stride, out.H, out.W, out.N, pl->NT, p.TW, p.TH, p.TN, pl->grid.x, p.stages);
+    fprintf(stderr,
+            "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: %s NT %d tile %dx%dx%d grid %d stages %d+%d, TMA %.1f MB, "
+            "MMA %.2f GFLOP\n",
+            w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N, pl->halo ? "halo" : "per-tap", pl->NT, p.TW, p.TH,
+            p.TN, pl->grid.x, p.hstages, p.stages, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
   bool ok = true;
   // activation maps
   const int nmaps = w.stride == 2 ? 4 : 1;
@@ -327,7 +463,8 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       strides[2] = (cuuint64_t)in.H * in.W * in.Ctot * 2;
       off = (size_t)in.coff + ((size_t)phy * in.W + phx) * in.Ctot;
     }
-    cuuint32_t box[4] = {(cuuint32_t)KCH, (cuuint32_t)p.TW, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
+    // halo path: the band plus one row above and below; p.TW = Wp already spans the two padding columns
+    cuuint32_t box[4] = {(cuuint32_t)KCH, (cuuint32_t)p.TW, (cuuint32_t)(p.TH + (pl->halo ? 2 : 0)), (cuuint32_t)p.TN};
     ok = ok && encode(&p.a_hi[mi], in.hi + off, 4, dims, strides, box, KCH);
     if (split) ok = ok && encode(&p.a_lo[mi], in.lo + off, 4, dims, strides, box, KCH);
   }
@@ -344,10 +481,10 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
 
 void wgmma_plan_destroy(WgmmaPlan *p) { delete p; }
 
-template <bool SPLIT, int NT>
-static int launch_t(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
+template <bool SPLIT, int NT, bool HALO>
+static int launch_h(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
   static std::atomic<unsigned long long> attr_done{0};
-  auto kernel = conv_wgmma_kernel<SPLIT, NT>;
+  auto kernel = conv_wgmma_kernel<SPLIT, NT, HALO>;
   SHAPY_CUDA_TRY(set_max_dynamic_smem(kernel, 227 * 1024, attr_done));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -363,6 +500,11 @@ static int launch_t(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
   SHAPY_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, pl->p));
   shapy::count_launch();
   return SHAPY_OK;
+}
+
+template <bool SPLIT, int NT>
+static int launch_t(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
+  return pl->halo ? launch_h<SPLIT, NT, true>(pl, st, pdl) : launch_h<SPLIT, NT, false>(pl, st, pdl);
 }
 
 template <bool SPLIT>

@@ -538,8 +538,9 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   if (err != cudaSuccess) { cleanup(); set_error("conv_test: %s", cudaGetErrorString(err)); return (int)err; }
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
-  if (engine == 0) {
-    plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0);
+  if (engine != 1) {
+    const WgmmaPath path = engine == 2 ? WGMMA_PER_TAP : (engine == 3 ? WGMMA_HALO : WGMMA_AUTO);
+    plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }
     rc = wgmma_plan_launch(plan, st, true);
     if (const char *reps_s = getenv("SHAPY_CONV_TEST_REPS")) {
@@ -554,9 +555,14 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
       float ms = 0;
       cudaEventElapsedTime(&ms, e0, e1);
       const double fl = 2.0 * B * Ho * Wo * (double)conv->cout * conv->cin * conv->ksize * conv->ksize;
-      fprintf(stderr, "[conv_test] cin %d cout %d k %d s %d %dx%d B %d mode %d: %.2f us/launch, %.1f TFLOP/s (x%d MMA flops)\n",
-              conv->cin, conv->cout, conv->ksize, conv->stride, H, W, B, mode, ms * 1e3 / reps, fl / (ms * 1e-3 / reps) * 1e-12,
-              mode ? 3 : 1);
+      const double sec = ms * 1e-3 / reps;
+      double tma = 0, mma = 0;
+      wgmma_plan_stats(plan, &tma, &mma);
+      fprintf(stderr,
+              "[conv_test] cin %d cout %d k %d s %d %dx%d B %d mode %d: %.2f us/launch, %.1f TFLOP/s (x%d MMA flops); "
+              "TMA %.0f MB = %.2f TB/s, MMA issued %.1f GFLOP = %.0f TFLOP/s\n",
+              conv->cin, conv->cout, conv->ksize, conv->stride, H, W, B, mode, sec * 1e6, fl / sec * 1e-12, mode ? 3 : 1,
+              tma * 1e-6, tma / sec * 1e-12, mma * 1e-9, mma / sec * 1e-12);
       cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
   } else {

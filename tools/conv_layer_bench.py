@@ -1,6 +1,8 @@
 """Per-layer timing of the HRNet-W48 main convolutions at the bench batch (B=64, 224x224 input):
-SHAPY_CONV_TEST_REPS launches of each plan, average time to stderr.  SHAPY_CONV_DEBUG=1 in the environment prints
-each plan's tile configuration."""
+SHAPY_CONV_TEST_REPS launches of each plan; to stderr the average time per launch, the useful conv FLOP/s, and the
+plan's TMA bytes and issued MMA FLOPs per launch with the rates they give at that time.  SHAPY_CONV_DEBUG=1 in the
+environment prints each plan's path and tile configuration; SHAPY_CONV_HALO=0 times the per-tap path everywhere.
+usage: python tools/conv_layer_bench.py [batch] [mode] [name,name,...]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ.setdefault('SHAPY_CONV_TEST_REPS', '20')

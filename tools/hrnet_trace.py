@@ -34,3 +34,14 @@ for o in ops:
 print('bucket(100us): in-flight fraction per lane')
 for b in range(nb):
     print(f'{b * 100:6d} ' + ' '.join(f'{v / 100:.2f}' for v in occ[b]))
+# per-family share: sum of (end - start) of every op of the family over that of all ops (lanes overlap, so the sum
+# exceeds the span; the share is of the summed op time)
+fam = {}
+for o in ops:
+    key = f'conv {o["cin"]}->{o["cout"]} k{o["k"]} s{o["s"]} /{o["div"]}' if o['kind'] in (0, 1) else f'kind {o["kind"]} /{o["div"]}'
+    n, t = fam.get(key, (0, 0.0))
+    fam[key] = (n + 1, t + o['t1'] - o['t0'])
+tot = sum(t for _, t in fam.values())
+print(f'per family: count, sum(end-start) us, share of {tot:.0f} us')
+for key, (n, t) in sorted(fam.items(), key=lambda kv: -kv[1][1]):
+    print(f'{key:32s} {n:4d} {t:9.0f} {100 * t / tot:6.1f} %')
