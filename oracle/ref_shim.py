@@ -143,19 +143,24 @@ def load_img00():
     return out
 
 
-def smplx_forward_ref(model: dict, betas, global_rot, body_pose):
+def smplx_forward_ref(model: dict, betas, global_rot, body_pose, jaw_pose=None, leye_pose=None, reye_pose=None,
+                      left_hand_pose=None, right_hand_pose=None, expression=None, transl=None):
     """Re-assembly of SMPLX.forward (body_models.py:628-767) on top of the verbatim lbs.py.
 
-    ``model`` is the dict produced by shapy_b200.synth.make_smplx (torch tensors).
-    Hands / jaw / eyes identity, expression zero, use_face_contour=True, J14 on.
+    ``model`` is the dict produced by shapy_b200.synth.make_smplx (torch tensors), in the dtype of ``betas``.
+    Pose parts that are not given are identity and a missing expression is zero, as in the reference;
+    use_face_contour=True, J14 on.
     """
     ref = load()
     lbs = ref.lbs
     B = betas.shape[0]
-    eye = torch.eye(3).view(1, 1, 3, 3)
+    eye = torch.eye(3, dtype=betas.dtype).view(1, 1, 3, 3)
     ident = lambda n: eye.expand(B, n, -1, -1).contiguous()  # noqa: E731
-    full_pose = torch.cat([global_rot, body_pose, ident(1), ident(1), ident(1), ident(15), ident(15)], dim=1)
-    expression = torch.zeros(B, model['expr_dirs'].shape[-1])
+    part = lambda p, n: ident(n) if p is None else p.reshape(B, n, 3, 3)  # noqa: E731
+    full_pose = torch.cat([global_rot, body_pose, part(jaw_pose, 1), part(leye_pose, 1), part(reye_pose, 1),
+                           part(left_hand_pose, 15), part(right_hand_pose, 15)], dim=1)
+    if expression is None:
+        expression = torch.zeros(B, model['expr_dirs'].shape[-1], dtype=betas.dtype)
     shape_components = torch.cat([betas, expression], dim=-1)
     shapedirs = torch.cat([model['shapedirs'], model['expr_dirs']], dim=-1)
     out = lbs.lbs(shape_components, full_pose, model['v_template'], shapedirs, model['posedirs'],
@@ -173,5 +178,8 @@ def smplx_forward_ref(model: dict, betas, global_rot, body_pose):
     joints = torch.cat([joints, landmarks], dim=1)
     reg = torch.einsum('ji,bik->bjk', model['extra_joint_regressor'], vertices)
     joints[:, model['source_idxs']] = joints[:, model['source_idxs']] * 0.0 + reg[:, model['target_idxs']] * 1.0
+    if transl is not None:
+        joints += transl.unsqueeze(dim=1)
+        vertices += transl.unsqueeze(dim=1)
     v_shaped = model['v_template'] + lbs.blend_shapes(betas, model['shapedirs'])
-    return dict(vertices=vertices, joints=joints, v_shaped=v_shaped)
+    return dict(vertices=vertices, joints=joints, v_shaped=v_shaped, full_pose=full_pose)

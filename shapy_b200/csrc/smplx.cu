@@ -153,13 +153,15 @@ __device__ __forceinline__ void cp_async16_zfill(void *smem_dst, const void *src
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(src_bytes) : "memory");
 }
 
-// posedirs [k][V3] fp32 -> split-fp16 GEMM weights [V3g][Kpad] (the [cout][cin] layout of a 1x1 convolution), x kPoseScale
-__global__ void pack_pose_weights_kernel(const float *__restrict__ posedirs, int V3, int Kp, int Kpad, int V3g,
+// posedirs [KP][V3] fp32 -> split-fp16 GEMM weights [V3g][Kpad] (the [cout][cin] layout of a 1x1 convolution), x kPoseScale.
+// Every real posedirs row below Kpad is packed (KP = 9 (J - 1), all of them), not only the Kp rows of the call that
+// builds the entry: the weights are cached per Kpad, and every pose width that rounds to this Kpad reuses them.
+__global__ void pack_pose_weights_kernel(const float *__restrict__ posedirs, int V3, int KP, int Kpad, int V3g,
                                          __half *__restrict__ hi, __half *__restrict__ lo) {
   const size_t n = (size_t)V3g * Kpad;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(i / Kpad), k = (int)(i % Kpad);
-    const float x = (c < V3 && k < Kp) ? posedirs[(size_t)k * V3 + c] * kPoseScale : 0.f;
+    const float x = (c < V3 && k < KP) ? posedirs[(size_t)k * V3 + c] * kPoseScale : 0.f;
     split_store(x, hi[i], lo[i]);
   }
 }
@@ -608,7 +610,7 @@ static int pose_blend_gemm(const shapy_smplx *m, const float *pfT, int B, int Kp
       const size_t n = (size_t)V3g * Kpad;
       SHAPY_CUDA_TRY(cudaMalloc((void **)&pw.hi, n * sizeof(__half)));
       SHAPY_CUDA_TRY(cudaMalloc((void **)&pw.lo, n * sizeof(__half)));
-      pack_pose_weights_kernel<<<1024, 256, 0, st>>>(d.posedirs, d.V * 3, Kp, Kpad, V3g, pw.hi, pw.lo);
+      pack_pose_weights_kernel<<<1024, 256, 0, st>>>(d.posedirs, d.V * 3, (d.J - 1) * 9, Kpad, V3g, pw.hi, pw.lo);
       SHAPY_LAUNCH_CHECK();
       m->pw[Kpad] = pw;
     } else {

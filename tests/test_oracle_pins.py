@@ -62,6 +62,26 @@ def test_smplx_oracle_vs_reference_lbs(golden_dir):
     assert _rel(o2['vertices'][:, ::97].numpy(), g['vertices2_sub']) < 2e-6
 
 
+def test_smplx_full_oracle_vs_reference_float64(golden_dir):
+    """ref_smplx_full.npz: the reference's forward in float64 with jaw, eyes, hands, expression and transl all given.
+    The oracle can differ from it in summation order only (measured: exactly 0 with torch 2.11's CPU kernels; the bar
+    leaves room for another BLAS)."""
+    g = np.load(os.path.join(golden_dir, 'ref_smplx_full.npz'))
+    model = synth.make_smplx(dtype=torch.float64)
+    out = smplx_oracle.smplx_forward_full(model, torch.from_numpy(g['betas']), torch.from_numpy(g['rot']),
+                                          expression=torch.from_numpy(g['expression']),
+                                          transl=torch.from_numpy(g['transl']))
+    assert out['vertices'].dtype == torch.float64
+    assert _rel(out['vertices'][:, ::7].numpy(), g['vertices_sub']) < 1e-12
+    assert _rel(out['joints'].numpy(), g['joints']) < 1e-12
+    assert _rel(out['v_shaped'][:, ::7].numpy(), g['v_shaped_sub']) < 1e-12
+    # the two turned necks select the LUT's last row (angle below -39 degrees) and its clamp (row 39)
+    df, _ = smplx_oracle.dynamic_landmarks(out['full_pose'], model['dynamic_lmk_faces_idx'],
+                                           model['dynamic_lmk_bary_coords'], model['neck_kin_chain'])
+    rows = [int((model['dynamic_lmk_faces_idx'] == df[b]).all(1).nonzero()[0]) for b in range(2)]
+    assert rows == [78, 39]
+
+
 def test_head_oracle_vs_reference(golden_dir):
     g = np.load(os.path.join(golden_dir, 'ref_head.npz'))
     sd = synth.make_head_state_dict()

@@ -24,6 +24,7 @@ Everything written here is a small fixture that travels to the GPU box, where
   align.npz             reference PointError(ScaleAlignment / RootAlignment) outputs on seeded meshes and joints, and mpjpe14
                         end to end through a seeded dense J14 regressor
   ref_smplx_live.npz    reference SMPL-X forward (ref_shim) of tests/test_oracle_pins.py's seeded bodies
+  ref_smplx_full.npz    reference SMPL-X forward in float64 with every pose part, expression and transl (float64)
   ref_weak_persp_to_blender.npz   reference demo.py weak_persp_to_blender on tests/test_writer_cpu.py's inputs
   ref_keypoint_tensor.{npz,json}  reference KeypointTensor under the tensor methods of tests/test_keypoint_tensor_cpu.py
   ref_mmi_{plane,soup}.npz        reference mesh_to_mesh_forward (oracle/_ref via oracle/run_ref_mmi.py) collisions on
@@ -378,6 +379,38 @@ def smplx_live_fixture():
                         **{k: ref[k].numpy().astype(np.float32) for k in ('vertices', 'joints', 'v_shaped')})
 
 
+def smplx_full_fixture():
+    """The reference's SMPL-X forward (ref_shim.smplx_forward_ref on the verbatim lbs(), find_dynamic_lmk_idx_and_bcoords
+    and vertices2landmarks) in float64 on the float64 synthetic model: every pose part non-identity, a nonzero expression
+    and transl, and the neck of bodies 0 / 1 turned past each end of the dynamic-contour LUT.  Vertices and v_shaped are
+    subsampled (every 7th vertex) to keep the fixture small."""
+    from shapy_b200 import synth
+    ref = ref_shim.load()
+    dt = torch.float64
+    model = synth.make_smplx(dtype=dt)
+    g = torch.Generator().manual_seed(21)
+    B = 4
+    betas = torch.randn(B, 10, generator=g, dtype=dt)
+    expression = torch.randn(B, 10, generator=g, dtype=dt)
+    transl = torch.randn(B, 3, generator=g, dtype=dt) * 0.5
+    aa = torch.randn(B, 55, 3, generator=g, dtype=dt) * 0.3
+    aa[:2, [0, 3, 6, 9, 15]] *= 0.1                              # the rest of the neck chain nearly straight
+    aa[0, 12] = torch.tensor([0.0, 1.2, 0.0], dtype=dt)         # neck about y, both ways: LUT row 78 and the clamp at 39
+    aa[1, 12] = torch.tensor([0.0, -1.2, 0.0], dtype=dt)
+    rot = ref.rot.batch_rodrigues(aa.reshape(-1, 3)).reshape(B, 55, 3, 3)
+    assert rot.dtype == dt
+    with torch.no_grad():
+        out = ref_shim.smplx_forward_ref(model, betas, rot[:, :1], rot[:, 1:22], jaw_pose=rot[:, 22:23],
+                                         leye_pose=rot[:, 23:24], reye_pose=rot[:, 24:25],
+                                         left_hand_pose=rot[:, 25:40], right_hand_pose=rot[:, 40:55],
+                                         expression=expression, transl=transl)
+    np.savez_compressed(
+        os.path.join(G, 'ref_smplx_full.npz'), betas=betas.numpy(), expression=expression.numpy(),
+        transl=transl.numpy(), rot=rot.numpy(), vertices_sub=out['vertices'][:, ::7].numpy(),
+        joints=out['joints'].numpy(), v_shaped_sub=out['v_shaped'][:, ::7].numpy())
+    print('ref_smplx_full.npz', os.path.getsize(os.path.join(G, 'ref_smplx_full.npz')), 'bytes')
+
+
 def writer_camera_fixture():
     import ast
     from collections import defaultdict
@@ -438,7 +471,7 @@ def mmi_fixtures():
 
 if __name__ == '__main__':
     which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
-                             'camera', 'keypoint']
+                             'smplx_full', 'camera', 'keypoint']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -460,6 +493,8 @@ if __name__ == '__main__':
         align_fixture()
     if 'smplx_live' in which:
         smplx_live_fixture()
+    if 'smplx_full' in which:
+        smplx_full_fixture()
     if 'camera' in which:
         writer_camera_fixture()
     if 'keypoint' in which:
