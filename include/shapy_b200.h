@@ -16,7 +16,7 @@
  *                        WeakPerspectiveCamera      regressor/human_shape/models/camera/camera_projection.py:181-213
  *   shapy_measure_*      BodyMeasurements.forward   mesh-mesh-intersection/body_measurements/body_measurements.py:217-246
  *   shapy_mmi_forward    mesh_to_mesh_forward       mesh-mesh-intersection/src/mesh_mesh_intersect.cpp:36-64
- *                                                   + src/mesh_mesh_intersect_cuda_op.cu:969-1079
+ *   shapy_mmi_forward_f64  (float / float64)        + src/mesh_mesh_intersect_cuda_op.cu:969-1079
  *   shapy_head_*         IterativeRegression.forward regressor/human_shape/models/common/networks.py:536-592
  *   shapy_hrnet_*        HighResolutionNet.forward  regressor/human_shape/models/backbone/hrnet.py:426-498
  *   shapy_p2p_error      v2vhdError.__call__        regressor/human_shape/utils/metrics.py:368-456
@@ -127,11 +127,20 @@ int shapy_measure_forward_tris(const float *triangles, int batch, int num_faces,
                                int32_t *plane_counts, int max_points, int32_t *status, void *stream);
 
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
- * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0. */
+ * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
+ * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */
 size_t shapy_mmi_workspace_bytes(int batch, int num_query, int num_target);
 int shapy_mmi_forward(const float *query, const float *target, int batch, int num_query, int num_target,
                       int max_collisions, int64_t *collision_faces, float *collision_bcs, void *workspace,
                       size_t workspace_bytes, void *stream);
+
+/* The same on float64 triangles, with the reference operator's double instantiation semantics: the SAT's CMP
+ * tolerance and its projected intervals are rounded to float as op.cu does, everything else (AABBs, the inclusive
+ * leaf test, the ray test, barycentrics) is computed in double.  collision_bcs is float64. */
+size_t shapy_mmi_workspace_bytes_f64(int batch, int num_query, int num_target);
+int shapy_mmi_forward_f64(const double *query, const double *target, int batch, int num_query, int num_target,
+                          int max_collisions, int64_t *collision_faces, double *collision_bcs, void *workspace,
+                          size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------ regression head */
 /* params_out (num_stages, B, P).  W0 (H0, F+P), W1 (H1, H0), W2 (P, H1) row-major as nn.Linear stores

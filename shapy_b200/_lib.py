@@ -72,6 +72,9 @@ _SIGS = {
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),
+    'shapy_mmi_workspace_bytes_f64': (c_size_t, [c_int, c_int, c_int]),
+    'shapy_mmi_forward_f64': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                      c_size_t, c_void_p]),
     'shapy_head_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     'shapy_head_forward': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,

@@ -16,6 +16,10 @@
 //                        written to warp-aggregated slots.  The reference uses one THREAD per query
 //                        triangle (2 active threads on the SHAPY path).
 // Nodes are 32 bytes (AABB + 2 child links) instead of the reference's 72-byte pointer-based node.
+// The prepare and query kernels are templated on the scalar type of the triangles (float or double, the
+// reference's AT_DISPATCH_FLOATING_TYPES).  Node and leaf boxes stay float in both: for double triangles they are
+// rounded outward, so the tree only prunes pairs whose double AABBs are disjoint, and the narrow phase repeats the
+// reference's inclusive leaf test on the exact double AABBs before the SAT.
 // Slot order within a query is unspecified (the reference's is traversal order); a collision without a
 // ray hit keeps zero barycentrics (see DESIGN.md).  More than `max_collisions` hits per query are dropped
 // (the reference writes out of bounds).  Compiled with -fmad=false.
@@ -51,11 +55,12 @@ static size_t ws_layout(int B, int F, BvhWs *w, char *base) {
   return off;
 }
 
-__device__ __forceinline__ mmi::Tri ld_tri(const float *p) {
-  mmi::Tri t;
-  t.v0 = make_float3(p[0], p[1], p[2]);
-  t.v1 = make_float3(p[3], p[4], p[5]);
-  t.v2 = make_float3(p[6], p[7], p[8]);
+template <typename T>
+__device__ __forceinline__ mmi::TriT<T> ld_tri(const T *p) {
+  mmi::TriT<T> t;
+  t.v0 = mmi::vec3<T>{p[0], p[1], p[2]};
+  t.v1 = mmi::vec3<T>{p[3], p[4], p[5]};
+  t.v2 = mmi::vec3<T>{p[6], p[7], p[8]};
   return t;
 }
 
@@ -73,43 +78,46 @@ __device__ __forceinline__ unsigned morton3d(float x, float y, float z) {
   return expand_bits((unsigned)x) * 4 + expand_bits((unsigned)y) * 2 + expand_bits((unsigned)z);
 }
 
-// One CTA per body.  Dynamic smem: codes[npow2] (u32) + ids[npow2] (u16/u32 depending on F).
-template <typename IdT>
-__global__ void __launch_bounds__(1024) bvh_prepare_kernel(const float *__restrict__ target, int F, int npow2, BvhWs w) {
+// One CTA per body.  Dynamic smem: codes[npow2] (u32) + ids[npow2] (u16/u32 depending on F).  The scene box and
+// the centroids are computed in T; the normalised centroid is rounded to float for the Morton code, which only
+// shapes the tree.
+template <typename T, typename IdT>
+__global__ void __launch_bounds__(1024) bvh_prepare_kernel(const T *__restrict__ target, int F, int npow2, BvhWs w) {
   extern __shared__ __align__(16) unsigned char sm[];
   unsigned *codes = reinterpret_cast<unsigned *>(sm);
   IdT *ids = reinterpret_cast<IdT *>(sm + (size_t)npow2 * 4);
-  __shared__ float red[6][32];
-  __shared__ float scene[6];
+  __shared__ T red[6][32];
+  __shared__ T scene[6];
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const float *tb = target + (size_t)b * F * 9;
-  float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+  const T *tb = target + (size_t)b * F * 9;
+  const T big = sizeof(T) == 4 ? (T)FLT_MAX : (T)DBL_MAX;
+  T lo[3] = {big, big, big}, hi[3] = {-big, -big, -big};
   for (int f = t; f < F; f += blockDim.x) {
-    mmi::Box bx = mmi::tri_box(ld_tri(tb + (size_t)f * 9));
-    lo[0] = fminf(lo[0], bx.lo.x); lo[1] = fminf(lo[1], bx.lo.y); lo[2] = fminf(lo[2], bx.lo.z);
-    hi[0] = fmaxf(hi[0], bx.hi.x); hi[1] = fmaxf(hi[1], bx.hi.y); hi[2] = fmaxf(hi[2], bx.hi.z);
+    mmi::BoxT<T> bx = mmi::tri_box(ld_tri(tb + (size_t)f * 9));
+    lo[0] = mmi::min_(lo[0], bx.lo.x); lo[1] = mmi::min_(lo[1], bx.lo.y); lo[2] = mmi::min_(lo[2], bx.lo.z);
+    hi[0] = mmi::max_(hi[0], bx.hi.x); hi[1] = mmi::max_(hi[1], bx.hi.y); hi[2] = mmi::max_(hi[2], bx.hi.z);
   }
   for (int o = 16; o; o >>= 1)
     for (int c = 0; c < 3; ++c) {
-      lo[c] = fminf(lo[c], __shfl_xor_sync(0xffffffffu, lo[c], o));
-      hi[c] = fmaxf(hi[c], __shfl_xor_sync(0xffffffffu, hi[c], o));
+      lo[c] = mmi::min_(lo[c], __shfl_xor_sync(0xffffffffu, lo[c], o));
+      hi[c] = mmi::max_(hi[c], __shfl_xor_sync(0xffffffffu, hi[c], o));
     }
   if (lane == 0) for (int c = 0; c < 3; ++c) { red[c][warp] = lo[c]; red[3 + c][warp] = hi[c]; }
   __syncthreads();
   if (t < 6) {
-    float v = red[t][0];
-    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) v = t < 3 ? fminf(v, red[t][i]) : fmaxf(v, red[t][i]);
+    T v = red[t][0];
+    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) v = t < 3 ? mmi::min_(v, red[t][i]) : mmi::max_(v, red[t][i]);
     scene[t] = v;
   }
   __syncthreads();
   for (int f = t; f < npow2; f += blockDim.x) {
     unsigned code = 0xFFFFFFFFu;
     if (f < F) {
-      mmi::Tri tr = ld_tri(tb + (size_t)f * 9);
-      float cx = (tr.v0.x + tr.v1.x + tr.v2.x) / 3.0f, cy = (tr.v0.y + tr.v1.y + tr.v2.y) / 3.0f,
-            cz = (tr.v0.z + tr.v1.z + tr.v2.z) / 3.0f;
-      code = morton3d((cx - scene[0]) / (scene[3] - scene[0]), (cy - scene[1]) / (scene[4] - scene[1]),
-                      (cz - scene[2]) / (scene[5] - scene[2]));
+      mmi::TriT<T> tr = ld_tri(tb + (size_t)f * 9);
+      T cx = (tr.v0.x + tr.v1.x + tr.v2.x) / (T)3, cy = (tr.v0.y + tr.v1.y + tr.v2.y) / (T)3,
+        cz = (tr.v0.z + tr.v1.z + tr.v2.z) / (T)3;
+      code = morton3d((float)((cx - scene[0]) / (scene[3] - scene[0])), (float)((cy - scene[1]) / (scene[4] - scene[1])),
+                      (float)((cz - scene[2]) / (scene[5] - scene[2])));
     }
     codes[f] = code;
     ids[f] = (IdT)f;
@@ -135,7 +143,7 @@ __global__ void __launch_bounds__(1024) bvh_prepare_kernel(const float *__restri
     int id = (int)ids[f];
     w.codes[(size_t)b * F + f] = codes[f];
     w.ids[(size_t)b * F + f] = id;
-    mmi::Box bx = mmi::tri_box(ld_tri(tb + (size_t)id * 9));
+    mmi::Box bx = mmi::box_f32(mmi::tri_box(ld_tri(tb + (size_t)id * 9)));
     float *lb = w.leaf_box + ((size_t)b * F + f) * 6;
     lb[0] = bx.lo.x; lb[1] = bx.lo.y; lb[2] = bx.lo.z; lb[3] = bx.hi.x; lb[4] = bx.hi.y; lb[5] = bx.hi.z;
   }
@@ -224,9 +232,10 @@ __device__ __forceinline__ bool overlap6(const mmi::Box &q, const float *bx) {
 }
 
 // 4 warps per CTA, one query triangle per warp.
-__global__ void __launch_bounds__(128) bvh_query_kernel(const float *__restrict__ query, const float *__restrict__ target,
+template <typename T>
+__global__ void __launch_bounds__(128) bvh_query_kernel(const T *__restrict__ query, const T *__restrict__ target,
                                                         int Q, int F, int M, BvhWs w, long long *faces_out,
-                                                        float *bcs_out) {
+                                                        T *bcs_out) {
   __shared__ int stack[4][kStackCap];
   __shared__ int queue[4][kQueueCap];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -234,13 +243,14 @@ __global__ void __launch_bounds__(128) bvh_query_kernel(const float *__restrict_
   const int b = blockIdx.y;
   const int qi = blockIdx.x * 4 + warp;
   if (qi >= Q) return;
-  const mmi::Tri qt = ld_tri(query + ((size_t)b * Q + qi) * 9);
-  const mmi::Box qb = mmi::tri_box(qt);
-  const float *tb = target + (size_t)b * F * 9;
+  const mmi::TriT<T> qt = ld_tri(query + ((size_t)b * Q + qi) * 9);
+  const mmi::BoxT<T> qbox = mmi::tri_box(qt);
+  const mmi::Box qb = mmi::box_f32(qbox);
+  const T *tb = target + (size_t)b * F * 9;
   const int *ids = w.ids + (size_t)b * F;
   const BvhNode *nodes = w.nodes + (size_t)b * (F - 1);
   long long *fo = faces_out + ((size_t)b * Q + qi) * M;
-  float *bo = bcs_out + ((size_t)b * Q + qi) * M * 6;
+  T *bo = bcs_out + ((size_t)b * Q + qi) * M * 6;
   int *st = stack[warp], *qu = queue[warp];
   int sp = 0, qn = 0, nhit = 0;
   if (F == 1) {  // a single leaf, no internal node
@@ -259,20 +269,22 @@ __global__ void __launch_bounds__(128) bvh_query_kernel(const float *__restrict_
       __syncwarp();
       qn -= n;
       bool hit = false;
-      float3 b1 = make_float3(0, 0, 0), b2 = b1;
+      mmi::vec3<T> b1{0, 0, 0}, b2 = b1;
       int tid = -1;
       if (cand >= 0) {
         tid = ids[cand];
-        const mmi::Tri T = ld_tri(tb + (size_t)tid * 9);
-        hit = mmi::sat11(qt, T);
-        if (hit) mmi::isect_points(qt, T, b1, b2);
+        const mmi::TriT<T> tt = ld_tri(tb + (size_t)tid * 9);
+        // float leaf boxes are the exact AABBs; double ones were rounded outward, so repeat the exact test
+        if constexpr (sizeof(T) == 4) hit = mmi::sat11(qt, tt);
+        else hit = mmi::box_overlap(qbox, mmi::tri_box(tt)) && mmi::sat11(qt, tt);
+        if (hit) mmi::isect_points(qt, tt, b1, b2);
       }
       const unsigned mh = __ballot_sync(0xffffffffu, hit);
       if (hit) {
         const int slot = nhit + __popc(mh & lt_mask);
         if (slot < M) {
           fo[slot] = tid;
-          float *o = bo + (size_t)slot * 6;
+          T *o = bo + (size_t)slot * 6;
           o[0] = b1.x; o[1] = b1.y; o[2] = b1.z; o[3] = b2.x; o[4] = b2.y; o[5] = b2.z;
         }
       }
@@ -323,17 +335,21 @@ extern "C" size_t shapy_mmi_workspace_bytes(int B, int Q, int F) {
   return ws_layout(B, F, nullptr, nullptr) + 256;
 }
 
-extern "C" int shapy_mmi_forward(const float *query, const float *target, int B, int Q, int F, int M,
-                                 int64_t *collision_faces, float *collision_bcs, void *workspace,
-                                 size_t workspace_bytes, void *stream) {
-  SHAPY_REQUIRE(query && target && collision_faces && collision_bcs, "shapy_mmi_forward: null argument");
-  SHAPY_REQUIRE(B > 0 && Q > 0 && F > 0 && M > 0, "shapy_mmi_forward: bad sizes");
-  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_mmi_workspace_bytes(B, Q, F), "shapy_mmi_forward: workspace too small");
+// The workspace holds float boxes and int links whatever the triangles' scalar type.
+extern "C" size_t shapy_mmi_workspace_bytes_f64(int B, int Q, int F) { return shapy_mmi_workspace_bytes(B, Q, F); }
+
+template <typename T>
+static int mmi_forward(const char *name, const T *query, const T *target, int B, int Q, int F, int M,
+                       int64_t *collision_faces, T *collision_bcs, void *workspace, size_t workspace_bytes,
+                       void *stream) {
+  SHAPY_REQUIRE(query && target && collision_faces && collision_bcs, "%s: null argument", name);
+  SHAPY_REQUIRE(B > 0 && Q > 0 && F > 0 && M > 0, "%s: bad sizes", name);
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_mmi_workspace_bytes(B, Q, F), "%s: workspace too small", name);
   cudaStream_t st = (cudaStream_t)stream;
   int npow2 = 1;
   while (npow2 < F) npow2 <<= 1;
   if (npow2 > 32768) {
-    set_error("shapy_mmi_forward: %d target triangles exceed the 32768 supported by the shared-memory sort", F);
+    set_error("%s: %d target triangles exceed the 32768 supported by the shared-memory sort", name, F);
     return SHAPY_ERR_UNSUPPORTED;
   }
   BvhWs w;
@@ -342,11 +358,11 @@ extern "C" int shapy_mmi_forward(const float *query, const float *target, int B,
   const size_t n_slots = (size_t)B * Q * M;
   fill_i64_kernel<<<(unsigned)((n_slots + 255) / 256), 256, 0, st>>>((long long *)collision_faces, n_slots, -1);
   SHAPY_LAUNCH_CHECK();
-  SHAPY_CUDA_TRY(cudaMemsetAsync(collision_bcs, 0, n_slots * 6 * sizeof(float), st));
+  SHAPY_CUDA_TRY(cudaMemsetAsync(collision_bcs, 0, n_slots * 6 * sizeof(T), st));
   const size_t smem = (size_t)npow2 * 4 + (size_t)npow2 * 2;
   static std::atomic<unsigned long long> attr_done{0};
-  SHAPY_CUDA_TRY(set_max_dynamic_smem(bvh_prepare_kernel<unsigned short>, 200 * 1024, attr_done));
-  bvh_prepare_kernel<unsigned short><<<B, 1024, smem, st>>>(target, F, npow2, w);
+  SHAPY_CUDA_TRY(set_max_dynamic_smem(bvh_prepare_kernel<T, unsigned short>, 200 * 1024, attr_done));
+  bvh_prepare_kernel<T, unsigned short><<<B, 1024, smem, st>>>(target, F, npow2, w);
   SHAPY_LAUNCH_CHECK();
   if (F > 1) {
     dim3 g1(ceil_div(F - 1, 128), B);
@@ -357,7 +373,21 @@ extern "C" int shapy_mmi_forward(const float *query, const float *target, int B,
     SHAPY_LAUNCH_CHECK();
   }
   dim3 g3(ceil_div(Q, 4), B);
-  bvh_query_kernel<<<g3, 128, 0, st>>>(query, target, Q, F, M, w, (long long *)collision_faces, collision_bcs);
+  bvh_query_kernel<T><<<g3, 128, 0, st>>>(query, target, Q, F, M, w, (long long *)collision_faces, collision_bcs);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
+}
+
+extern "C" int shapy_mmi_forward(const float *query, const float *target, int B, int Q, int F, int M,
+                                 int64_t *collision_faces, float *collision_bcs, void *workspace,
+                                 size_t workspace_bytes, void *stream) {
+  return mmi_forward("shapy_mmi_forward", query, target, B, Q, F, M, collision_faces, collision_bcs, workspace,
+                     workspace_bytes, stream);
+}
+
+extern "C" int shapy_mmi_forward_f64(const double *query, const double *target, int B, int Q, int F, int M,
+                                     int64_t *collision_faces, double *collision_bcs, void *workspace,
+                                     size_t workspace_bytes, void *stream) {
+  return mmi_forward("shapy_mmi_forward_f64", query, target, B, Q, F, M, collision_faces, collision_bcs, workspace,
+                     workspace_bytes, stream);
 }

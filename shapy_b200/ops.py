@@ -216,29 +216,39 @@ def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, tri
 
 
 def mesh_to_mesh_forward(query_triangles, target_triangles, max_collisions=16, print_timings=False):
-    """Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward (bind.cpp:59-64)."""
+    """Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward (bind.cpp:59-64).
+
+    Query and target triangles are both float32 or both float64, as the reference dispatches them; `collision_bcs`
+    takes their dtype.  The float64 path keeps the reference's double-instantiation semantics, including the points
+    where it rounds to float (see shapy_mmi_forward_f64 in include/shapy_b200.h).  Mixed, half and bfloat16 inputs
+    raise RuntimeError before anything is launched."""
     for name, t in (('query_triangles', query_triangles), ('target_triangles', target_triangles)):
         if not (torch.is_tensor(t) and t.is_cuda):
             raise RuntimeError(f'{name} must be a CUDA tensor')
         if not t.is_contiguous():
             raise RuntimeError(f'{name} must be contiguous')
-    if query_triangles.dtype != torch.float32 or target_triangles.dtype != torch.float32:
-        raise RuntimeError('shapy_b200 mesh_to_mesh_forward supports float32 triangles only')
+    dtype = query_triangles.dtype
+    if target_triangles.dtype != dtype or dtype not in (torch.float32, torch.float64):
+        raise RuntimeError(f'shapy_b200 mesh_to_mesh_forward: query and target triangles must both be float32 or both '
+                           f'float64, got {dtype} and {target_triangles.dtype}')
+    f64 = dtype == torch.float64
     B, Q = query_triangles.shape[:2]
     F = target_triangles.shape[1]
     dev = query_triangles.device
     M = int(max_collisions)
     faces = torch.empty(B, Q * M, dtype=torch.int64, device=dev)
-    bcs = torch.empty(B, Q * M, 2, 3, dtype=torch.float32, device=dev)
+    bcs = torch.empty(B, Q * M, 2, 3, dtype=dtype, device=dev)
     if B == 0 or Q == 0:
         return [faces, bcs]
     if F == 0:            # nothing to collide with: every slot is "no collision"
         return [faces.fill_(-1), bcs.zero_()]
+    L = lib()
+    ws_bytes, forward = ((L.shapy_mmi_workspace_bytes_f64, L.shapy_mmi_forward_f64) if f64 else
+                         (L.shapy_mmi_workspace_bytes, L.shapy_mmi_forward))
     with torch.cuda.device(dev):
-        nbytes = lib().shapy_mmi_workspace_bytes(B, Q, F)
-        ws = _WS.get('mmi', nbytes, dev)
-        check(lib().shapy_mmi_forward(ptr(query_triangles), ptr(target_triangles), B, Q, F, M, ptr(faces), ptr(bcs),
-                                      ptr(ws), ws.numel(), stream_ptr()), 'mmi_forward')
+        ws = _WS.get('mmi', ws_bytes(B, Q, F), dev)
+        check(forward(ptr(query_triangles), ptr(target_triangles), B, Q, F, M, ptr(faces), ptr(bcs),
+                      ptr(ws), ws.numel(), stream_ptr()), 'mmi_forward_f64' if f64 else 'mmi_forward')
     return [faces, bcs]
 
 

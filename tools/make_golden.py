@@ -29,6 +29,7 @@ Everything written here is a small fixture that travels to the GPU box, where
   ref_keypoint_tensor.{npz,json}  reference KeypointTensor under the tensor methods of tests/test_keypoint_tensor_cpu.py
   ref_mmi_{plane,soup}.npz        reference mesh_to_mesh_forward (oracle/_ref via oracle/run_ref_mmi.py) collisions on
                         the inputs of tests/test_gpu_zz_reference_op.py; GPU only: `python tools/make_golden.py mmi`
+  ref_mmi_{plane,soup,quirk}_f64.npz   the same in float64 on the inputs of tests/test_mmi_f64_cpu.py (same recipe)
   preprocess.npz        reference input stage (transf_utils.crop with cv2 + ToTensor + Normalize) on seeded uint8 images:
                         crop windows, crops with OpenCV's portable path (IPP off) and with this container's IPP build
 """
@@ -452,21 +453,30 @@ def keypoint_tensor_fixture():
 
 
 def mmi_fixtures():
-    """Needs a GPU and oracle/_ref (python oracle/build_ref.py).  Stores the filled slots of the reference's output."""
+    """Needs a GPU and oracle/_ref (python oracle/build_ref.py).  Stores the filled slots of the reference's output, in
+    the inputs' dtype: float32 for ref_mmi_{plane,soup}, float64 for ref_mmi_{plane,soup,quirk}_f64."""
     import subprocess
     import tempfile
     sys.path.insert(0, os.path.join(ROOT, 'tests'))
     import test_gpu_zz_reference_op as t
-    for name, (query, target, M) in (('ref_mmi_plane', t.plane_inputs(G)), ('ref_mmi_soup', t.soup_inputs())):
+    import test_mmi_f64_cpu as t64
+    quirk_q, quirk_t, quirk_m, quirk_pairs = t64.quirk_inputs_f64()
+    for name, (query, target, M) in (('ref_mmi_plane', t.plane_inputs(G)), ('ref_mmi_soup', t.soup_inputs()),
+                                     ('ref_mmi_plane_f64', t64.plane_inputs_f64(G)),
+                                     ('ref_mmi_soup_f64', t64.soup_inputs_f64()),
+                                     ('ref_mmi_quirk_f64', (quirk_q, quirk_t, quirk_m))):
         with tempfile.TemporaryDirectory() as tmp:
             inp, outp = os.path.join(tmp, 'in.npz'), os.path.join(tmp, 'out.npz')
             np.savez(inp, query=query, target=target, max_collisions=np.int64(M))
             subprocess.run([sys.executable, os.path.join(ROOT, 'oracle', 'run_ref_mmi.py'), inp, outp], check=True)
             d = np.load(outp)
             f, bcs = d['faces'], d['bcs']
+        assert bcs.dtype == query.dtype
+        if name == 'ref_mmi_quirk_f64':      # the fixture exists to show these pairs reported by the reference
+            t64.check_quirk(f[0], M, quirk_pairs, 'reference')
         keep = np.nonzero(f >= 0)
         np.savez_compressed(os.path.join(G, f'{name}.npz'), shape=np.int64(f.shape), idx=np.stack(keep, 1).astype(np.int32),
-                            faces=f[keep].astype(np.int32), bcs=bcs[keep].astype(np.float32), query=query)
+                            faces=f[keep].astype(np.int32), bcs=bcs[keep], query=query)
 
 
 if __name__ == '__main__':
