@@ -10,6 +10,10 @@
 // fallback axes, "first ray hit" point selection -- see mmi_device.cuh), hits are appended to a
 // shared-memory point list, and a warp per plane gift-wraps the 2-D hull (exact fp64 orientation
 // predicate on the fp32 points, as qhull sees them) and sums the 3-D edge lengths in fp32.
+// Both kernels hold 1 024 points per plane and 8 192 candidates per body, whichever entry point runs them.
+// Points that share (x, z) are told apart by value (pt_before), never by their slot, whose order depends on
+// timing.  A hull of zero area (fewer than 3 points, or all of them collinear or coincident in xz) is NaN:
+// qhull raises on it.
 // Compiled with -fmad=false (bit parity of the predicates with oracle/mmi_oracle.c).
 #include <cstdlib>
 
@@ -18,8 +22,8 @@
 
 namespace shapy {
 
-constexpr int kMaxPts = 512;
-constexpr int kMaxCand = 4096;  // (face, plane, query triangle) candidates that pass the AABB filter, per body
+constexpr int kMaxPts = 1024;
+constexpr int kMaxCand = 8192;  // (face, plane, query triangle) candidates that pass the AABB filter, per body
 
 struct MeasureArgs {
   const float *verts;  // (B,V,3) or null
@@ -62,15 +66,34 @@ __device__ __forceinline__ bool better_next(double cx, double cz, float ax, floa
   return (wx * wx + wz * wz) > (ux * ux + uz * uz);
 }
 
+// Total order on the float bit patterns (-0 before +0).
+__device__ __forceinline__ int ord_bits(float f) {
+  const int i = __float_as_int(f);
+  return i >= 0 ? i : (i ^ 0x7fffffff);
+}
+
+// Order between two points (x, y, z) with the same (x, z) as floats: smaller y, then z, then x, as bits.  The hull
+// takes the first of such points in this order, so its 3-D edge lengths do not depend on which point got which slot.
+__device__ __forceinline__ bool pt_before(const float *a, const float *b) {
+  const int ay = ord_bits(a[1]), by = ord_bits(b[1]);
+  if (ay != by) return ay < by;
+  const int az = ord_bits(a[2]), bz = ord_bits(b[2]);
+  if (az != bz) return az < bz;
+  return ord_bits(a[0]) < ord_bits(b[0]);
+}
+
+constexpr size_t kMeasSmemBytes = 3 * kMaxPts * 12 + kMaxCand * 4;   // points + candidate queue, dynamic
+
 constexpr int kMeasThreads = 512;
 __global__ void __launch_bounds__(kMeasThreads) measure_kernel(MeasureArgs a) {
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  __shared__ float pts[3][kMaxPts][3];
+  extern __shared__ __align__(16) unsigned char m1_smem[];
+  float (*pts)[kMaxPts][3] = reinterpret_cast<float (*)[kMaxPts][3]>(m1_smem);         // [3][kMaxPts][3]
+  int *cand = reinterpret_cast<int *>(m1_smem + 3 * kMaxPts * 12);                    // [kMaxCand]
   __shared__ int cnt[3];
   __shared__ float hs[3];
   __shared__ float lmy[2];
   __shared__ float red[kMeasThreads / 32];
-  __shared__ int cand[kMaxCand];
   __shared__ int ncand;
   if (t < 3) cnt[t] = 0;
   if (t == 0) ncand = 0;
@@ -160,18 +183,26 @@ __global__ void __launch_bounds__(kMeasThreads) measure_kernel(MeasureArgs a) {
       float bx = 0.f, bz = 0.f;
       for (int i = lane; i < n; i += 32) {
         float x = pts[p][i][0], z = pts[p][i][2];
-        if (best < 0 || x < bx || (x == bx && z < bz)) { best = i; bx = x; bz = z; }
+        if (best < 0 || x < bx || (x == bx && z < bz) || (x == bx && z == bz && pt_before(pts[p][i], pts[p][best]))) {
+          best = i; bx = x; bz = z;
+        }
       }
       for (int o = 16; o; o >>= 1) {
         int ob = __shfl_xor_sync(0xffffffffu, best, o);
         float ox = __shfl_xor_sync(0xffffffffu, bx, o), oz = __shfl_xor_sync(0xffffffffu, bz, o);
-        if (ob >= 0 && (best < 0 || ox < bx || (ox == bx && oz < bz) || (ox == bx && oz == bz && ob < best))) {
+        if (ob >= 0 && (best < 0 || ox < bx || (ox == bx && oz < bz) ||
+                        (ox == bx && oz == bz && pt_before(pts[p][ob], pts[p][best])))) {
           best = ob; bx = ox; bz = oz;
         }
       }
+      // lane 0's result for the whole warp: every lane then walks from the same point and leaves the walk together,
+      // whatever the comparisons did in the butterfly (a NaN point compares false both ways)
+      best = __shfl_sync(0xffffffffu, best, 0);
+      bx = __shfl_sync(0xffffffffu, bx, 0);
+      bz = __shfl_sync(0xffffffffu, bz, 0);
       const int start = best;
       const float sx = bx, sz = bz;
-      int cur = start;
+      int cur = start, edges = 0;
       for (int it = 0; it < n + 1; ++it) {
         const float cx = pts[p][cur][0], cz = pts[p][cur][2];
         int nb = -1;
@@ -179,24 +210,33 @@ __global__ void __launch_bounds__(kMeasThreads) measure_kernel(MeasureArgs a) {
         for (int i = lane; i < n; i += 32) {
           float x = pts[p][i][0], z = pts[p][i][2];
           if (x == cx && z == cz) continue;  // the point itself and its duplicates
-          if (nb < 0 || better_next(cx, cz, nx, nz, x, z)) { nb = i; nx = x; nz = z; }
+          if (nb < 0 || better_next(cx, cz, nx, nz, x, z) || (x == nx && z == nz && pt_before(pts[p][i], pts[p][nb]))) {
+            nb = i; nx = x; nz = z;
+          }
         }
         for (int o = 16; o; o >>= 1) {
           int ob = __shfl_xor_sync(0xffffffffu, nb, o);
           float ox = __shfl_xor_sync(0xffffffffu, nx, o), oz = __shfl_xor_sync(0xffffffffu, nz, o);
           if (ob >= 0) {
             bool take = nb < 0 || better_next(cx, cz, nx, nz, ox, oz) ||
-                        (ox == nx && oz == nz && ob < nb);
+                        (ox == nx && oz == nz && pt_before(pts[p][ob], pts[p][nb]));
             if (take) { nb = ob; nx = ox; nz = oz; }
           }
         }
+        nb = __shfl_sync(0xffffffffu, nb, 0);   // warp-uniform exits below: the shuffles above need every lane
+        nx = __shfl_sync(0xffffffffu, nx, 0);
+        nz = __shfl_sync(0xffffffffu, nz, 0);
         if (nb < 0) break;  // all points coincide
         float dx = pts[p][nb][0] - pts[p][cur][0], dy = pts[p][nb][1] - pts[p][cur][1],
               dz = pts[p][nb][2] - pts[p][cur][2];
         perim += sqrtf(dx * dx + dy * dy + dz * dz);
+        ++edges;
         cur = nb;
         if (nx == sx && nz == sz) break;
       }
+      // the walk skips collinear points, so a hull of positive area has at least 3 edges; 2 (collinear points) or 0
+      // (coincident ones) is a zero-area hull, on which qhull raises
+      if (edges < 3) perim = __int_as_float(0x7fc00000);
     }
     if (lane == 0) a.out[(size_t)b * 5 + 2 + p] = truncated ? __int_as_float(0x7fc00000) : perim;
   }
@@ -246,6 +286,7 @@ __global__ void __launch_bounds__(kM2Threads, 1) measure_smem_kernel(MeasureArgs
   __shared__ float red[kM2Threads / 32];
   __shared__ M2Ext ext[3][8];
   __shared__ float chain_len[3][8];
+  __shared__ int chain_edges[3][8];
   __shared__ int overflow;
   if (t < 3) cnt[t] = 0;
   if (t == 0) { ncand = 0; overflow = 0; }
@@ -344,12 +385,16 @@ __global__ void __launch_bounds__(kM2Threads, 1) measure_smem_kernel(MeasureArgs
     for (int i = lane; i < n; i += 32) {
       double k1, k2;
       m2_key(P[3 * i], P[3 * i + 2], hk, k1, k2);
-      if (best < 0 || k1 > b1 || (k1 == b1 && k2 > b2)) { best = i; b1 = k1; b2 = k2; }
+      if (best < 0 || k1 > b1 || (k1 == b1 && (k2 > b2 || (k2 == b2 && pt_before(P + 3 * i, P + 3 * best))))) {
+        best = i; b1 = k1; b2 = k2;
+      }
     }
     for (int o = 16; o; o >>= 1) {
       const int ob = __shfl_xor_sync(0xffffffffu, best, o);
       const double o1 = __shfl_xor_sync(0xffffffffu, b1, o), o2 = __shfl_xor_sync(0xffffffffu, b2, o);
-      if (ob >= 0 && (best < 0 || o1 > b1 || (o1 == b1 && (o2 > b2 || (o2 == b2 && ob < best))))) { best = ob; b1 = o1; b2 = o2; }
+      if (ob >= 0 && (best < 0 || o1 > b1 || (o1 == b1 && (o2 > b2 || (o2 == b2 && pt_before(P + 3 * ob, P + 3 * best)))))) {
+        best = ob; b1 = o1; b2 = o2;
+      }
     }
     if (lane == 0) {
       M2Ext e;
@@ -372,6 +417,7 @@ __global__ void __launch_bounds__(kM2Threads, 1) measure_smem_kernel(MeasureArgs
       }
     }
     float len = 0.f;
+    int edges = 0;
     const M2Ext e0 = ext[hp][hk], e1 = ext[hp][(hk + 1) & 7];
     if (n >= 3 && e0.idx >= 0 && !(e0.x == e1.x && e0.z == e1.z)) {
       // candidates of this chain: points on the outer side of (or on) the chord e0 -> e1
@@ -405,32 +451,41 @@ __global__ void __launch_bounds__(kM2Threads, 1) measure_smem_kernel(MeasureArgs
           const int i = listed ? (int)L[q] : q;
           const float x = P[3 * i], z = P[3 * i + 2];
           if (x == cx && z == cz) continue;
-          if (nb < 0 || better_next(cx, cz, nx, nz, x, z)) { nb = i; nx = x; nz = z; }
+          if (nb < 0 || better_next(cx, cz, nx, nz, x, z) || (x == nx && z == nz && pt_before(P + 3 * i, P + 3 * nb))) {
+            nb = i; nx = x; nz = z;
+          }
         }
         for (int o = 16; o; o >>= 1) {
           const int ob = __shfl_xor_sync(0xffffffffu, nb, o);
           const float ox = __shfl_xor_sync(0xffffffffu, nx, o), oz = __shfl_xor_sync(0xffffffffu, nz, o);
           if (ob >= 0) {
-            const bool take = nb < 0 || better_next(cx, cz, nx, nz, ox, oz) || (ox == nx && oz == nz && ob < nb);
+            const bool take = nb < 0 || better_next(cx, cz, nx, nz, ox, oz) ||
+                              (ox == nx && oz == nz && pt_before(P + 3 * ob, P + 3 * nb));
             if (take) { nb = ob; nx = ox; nz = oz; }
           }
         }
+        nb = __shfl_sync(0xffffffffu, nb, 0);   // warp-uniform exits below: the shuffles above need every lane
+        nx = __shfl_sync(0xffffffffu, nx, 0);
+        nz = __shfl_sync(0xffffffffu, nz, 0);
         if (nb < 0) break;
         const float dx = P[3 * nb] - P[3 * cur], dy = P[3 * nb + 1] - P[3 * cur + 1], dz = P[3 * nb + 2] - P[3 * cur + 2];
         len += sqrtf(dx * dx + dy * dy + dz * dz);
+        ++edges;
         cur = nb; cx = nx; cz = nz;
         if (nx == e1.x && nz == e1.z) break;
       }
     }
-    if (lane == 0) chain_len[hp][hk] = len;
+    if (lane == 0) { chain_len[hp][hk] = len; chain_edges[hp][hk] = edges; }
   }
   __syncthreads();
   if (t < 3) {
     const int p = t;
     float perim = 0.f;
-    for (int k = 0; k < 8; ++k) perim += chain_len[p][k];
-    const int np = cnt[p];
-    if (np < 3) perim = __int_as_float(0x7fc00000);                       // qhull would raise on a degenerate input
+    int edges = 0;
+    for (int k = 0; k < 8; ++k) { perim += chain_len[p][k]; edges += chain_edges[p][k]; }
+    // fewer than 3 hull edges: fewer than 3 points, or all of them collinear or coincident in xz.  The 8 extremes alone
+    // cannot tell: a thin triangle's obtuse vertex is extreme in none of the 8 directions.  qhull raises on these.
+    if (cnt[p] < 3 || edges < 3) perim = __int_as_float(0x7fc00000);
     if ((overflow & (1 << p))) perim = __int_as_float(0x7fc00000);   // truncated point set
     a.out[(size_t)b * 5 + 2 + p] = perim;
   }
@@ -451,12 +506,14 @@ static int launch_measure(MeasureArgs a, void *stream) {
   static const bool v1_only = []() { const char *e = getenv("SHAPY_MEASURE_V1"); return e && e[0] == '1'; }();
   if (a.verts && !v1_only && a.V < 65536 && measure_smem_bytes(a.V) <= 220 * 1024) {
     static std::atomic<unsigned long long> attr_done{0};
-    SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel, 226 * 1024, attr_done));   // + 560 B static <= 227 KB
+    SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel, 226 * 1024, attr_done));   // + 656 B static <= 227 KB
     measure_smem_kernel<<<a.B, kM2Threads, measure_smem_bytes(a.V), (cudaStream_t)stream>>>(a);
     SHAPY_LAUNCH_CHECK();
     return SHAPY_OK;
   }
-  measure_kernel<<<a.B, kMeasThreads, 0, (cudaStream_t)stream>>>(a);
+  static std::atomic<unsigned long long> attr_done_v1{0};
+  SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_kernel, (int)kMeasSmemBytes, attr_done_v1));      // 68 KB > 48 KB default
+  measure_kernel<<<a.B, kMeasThreads, kMeasSmemBytes, (cudaStream_t)stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

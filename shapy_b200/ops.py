@@ -175,10 +175,14 @@ def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, tri
             max_points=1024, strict=False):
     """Returns (B, 5) = mass, height, chest, waist, hips.  Either (v_shaped, faces_i32) or triangles (B,F,3,3).
 
-    The kernel's point / candidate buffers have a fixed capacity (1024 points per plane; the reference's
-    `max_collisions` has no equivalent).  A body that overflows them gets NaN circumferences, never a truncated value,
-    and the device status word is set: it is returned as `out.status` (a 1-element int32 CUDA tensor, readable at the
-    caller's next synchronisation point) and `strict=True` checks it here (one host synchronisation) and raises."""
+    The kernels' point / candidate buffers have a fixed capacity, the same for both entries: 1024 points per plane and
+    8192 AABB candidates per body (the reference's `max_collisions` has no equivalent).  A plane past 1024 points gets
+    a NaN circumference, a body past 8192 candidates NaN on all three, never a truncated value, and the device status
+    word is set; `max_points` below a plane's count truncates the returned points only, and also sets it.  A slice
+    whose xz hull has zero area (fewer than 3 points, all collinear or all coincident) is NaN too, where the
+    reference's qhull raises, but does not set the status.  The status word is returned as `out.status` (a 1-element
+    int32 CUDA tensor, readable at the caller's next synchronisation point) and `strict=True` checks it here (one host
+    synchronisation) and raises."""
     if triangles is not None:
         x = _cuda_f32(triangles, 'triangles')
         B, F = x.shape[0], x.shape[1]
