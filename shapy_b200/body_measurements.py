@@ -38,7 +38,7 @@ class BodyMeasurements(nn.Module):
         self.register_buffer('chest_bcs', torch.tensor(lm['chest']['bc'], dtype=torch.float32))
         self.register_buffer('belly_bcs', torch.tensor(lm['waist']['bc'], dtype=torch.float32))
         self.register_buffer('hips_bcs', torch.tensor(lm['hips']['bc'], dtype=torch.float32))
-        # accepted for config compatibility; the fused kernels have their own fixed capacity, the same for forward()
+        # accepted for config compatibility; the fused kernel has its own fixed capacity, the same for forward()
         # and forward_vertices() (1024 points per plane, 4x the reference default, and 8192 candidates per body) and
         # report overflow through NaN + `last_status` instead of truncating
         self.max_collisions = cfg.get('max_collisions', 256)

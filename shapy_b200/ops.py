@@ -175,7 +175,7 @@ def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, tri
             max_points=1024, strict=False):
     """Returns (B, 5) = mass, height, chest, waist, hips.  Either (v_shaped, faces_i32) or triangles (B,F,3,3).
 
-    The kernels' point / candidate buffers have a fixed capacity, the same for both entries: 1024 points per plane and
+    The kernel's point / candidate buffers have a fixed capacity, the same for every entry: 1024 points per plane and
     8192 AABB candidates per body (the reference's `max_collisions` has no equivalent).  A plane past 1024 points gets
     a NaN circumference, a body past 8192 candidates NaN on all three, never a truncated value, and the device status
     word is set; `max_points` below a plane's count truncates the returned points only, and also sets it.  A slice

@@ -1,7 +1,7 @@
 """Constructed meshes whose slices reach the edge cases of the measurement kernels (csrc/measure.cu).
 
 Not a test module: tests/test_measure_slices_cpu.py proves on the float C oracle that each construction reaches the
-case it is named for, and tests/test_gpu_measure_hull.py runs them through both measurement entries.
+case it is named for, and tests/test_gpu_measure_hull.py runs them through every measurement entry.
 
 Every mesh has three slicing planes, chest / waist / hips at y = 0, 2 and 4, far enough apart that no face of one
 plane's slice reaches another plane.  Faces 0..5 are markers outside the query quad's ±1 in x, so the kernels'
@@ -21,10 +21,10 @@ from oracle import measure_oracle
 
 PLANES = ('chest', 'waist', 'hips')
 HEIGHTS = (0.0, 2.0, 4.0)
-CAP_POINTS = 1024          # points per plane, both kernels
-CAP_CAND = 8192            # (face, plane, query triangle) candidates per body, both kernels
+CAP_POINTS = 1024          # points per plane, every entry
+CAP_CAND = 8192            # (face, plane, query triangle) candidates per body, every entry
 CHAIN_CAP = 640            # u16 candidate list per hull chain of measure_smem_kernel
-V1_FALLBACK_V = 20000      # vertex count beyond measure_smem_kernel's shared memory: the vertices entry runs v1
+GLOBAL_VERTS_V = 20000     # vertex count beyond what the kernel stages in shared memory: gathered from global memory
 
 
 class Builder:
@@ -90,8 +90,9 @@ class Mesh:
             out.append(np.float32(np.float32(y[0] * bc[0] + y[1] * bc[1]) + y[2] * bc[2]))
         return out
 
-    def padded(self, nverts=V1_FALLBACK_V):
-        """Same mesh with unused vertices appended up to `nverts` (the vertices entry then runs the v1 kernel)."""
+    def padded(self, nverts=GLOBAL_VERTS_V):
+        """Same mesh with unused vertices appended up to `nverts` (the vertices entry then gathers them from global
+        memory instead of staging them in shared memory)."""
         extra = np.full((nverts - len(self.verts), 3), 9.0, np.float32)
         return Mesh(np.concatenate([self.verts, extra]), self.faces, self.lm, dict(self.meta, padded=nverts))
 
@@ -354,7 +355,7 @@ def overhang(n_faces, rings=True):
 
 
 def value_families():
-    """Every family whose slices are measured (values, point sets, v1 vs v2)."""
+    """Every family whose slices are measured (values, point sets, entries against each other)."""
     return [ngon(3), ngon(4), ngon(7), ngon(64), ngon(333), ngon(500), ngon(150, center=(0.3, -0.2), r=0.45),
             clipped(), subdivided_square(), arc_cluster(), obtuse(), small_counts(), degenerate(), through_vertices(),
             face0_crossing(), identical_xz(), exact_count(CAP_POINTS), overhang(700)]

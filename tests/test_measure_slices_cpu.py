@@ -130,8 +130,9 @@ def test_candidate_counts(fam, pts):
 
 
 def test_padded_mesh_leaves_shared_memory():
-    """V = 20 000: measure_smem_kernel would need more than the 220 KB it may take, so the vertices entry runs v1."""
-    V = ms.V1_FALLBACK_V
+    """V = 20 000: staging the vertices would take more than the 220 KB of shared memory the kernel may use, so the
+    vertices entry gathers them from global memory."""
+    V = ms.GLOBAL_VERTS_V
     assert ((V * 12 + 15) & ~15) + 3 * 1024 * 12 + 8192 * 4 > 220 * 1024
     m = ms.exact_count(ms.CAP_POINTS).padded()
     assert m.verts.shape == (V, 3) and m.faces.max() < V

@@ -5,7 +5,8 @@
      224 x 224, three settings: fp32 (TF32 off), TF32 convolutions, fp16 autocast.
   2. The reference's own BVH kernel (oracle/_ref, mesh_mesh_intersect_cuda_op.cu patched for torch 2.11) on the
      measurement query of BASELINE configs[3] (2 plane triangles against the 20 908 body triangles, 3 planes per body),
-     next to shapy_mmi_forward on the same inputs and to the fused measurement kernel that replaces all of it.
+     next to shapy_mmi_forward on the same inputs and to the fused measurement kernel that replaces all of it, through
+     each of its entries: vertices + faces, triangles, and vertices padded to V = 20 000 (too many to stage).
   3. The same operator in float64 and float32, reference and shapy_b200, on those planes and on the seeded triangle
      soup of tests/test_gpu_zz_reference_op.py (float32) / tests/test_mmi_f64_cpu.py (float64).
 
@@ -127,6 +128,11 @@ def main():
     f_d = torch.from_numpy(g['faces']).to(torch.int32).cuda()
     lmk = ops.make_landmarks(lm)
     meas['shapy_measure_kernel_ms_64_bodies_all_5_measurements'] = round(timed(lambda: ops.measure(lmk, v_shaped=v_d, faces_i32=f_d), n=20), 4)
+    # the entries bench.py does not time: the triangles entry, and vertices too many to stage in shared memory
+    tri_d = torch.from_numpy(tris).cuda()
+    meas['shapy_measure_kernel_ms_64_bodies_triangles_entry'] = round(timed(lambda: ops.measure(lmk, triangles=tri_d), n=20), 4)
+    vpad_d = torch.cat([v_d, torch.full((nb, 20000 - v_d.shape[1], 3), 9.0, device='cuda')], 1).contiguous()
+    meas['shapy_measure_kernel_ms_64_bodies_vertices_padded_to_20000'] = round(timed(lambda: ops.measure(lmk, v_shaped=vpad_d, faces_i32=f_d), n=20), 4)
     out['measurements_64_bodies'] = meas
     dtypes = {'3_planes_64_bodies_ms': {k: round(sum(v), 4) for k, v in f64.items()}}
     sys.path.insert(0, os.path.join(ROOT, 'tests'))
