@@ -4,6 +4,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <atomic>
 #include <string>
 #include <vector>
@@ -59,27 +60,17 @@ static inline cudaError_t set_max_dynamic_smem(Kernel kernel, int bytes, std::at
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// RAII-less device buffer owned by long-lived objects (model constants).
+// Device copy of a host vector for a long-lived object (model constants), recorded in `allocs` for its owner to free.
+// Does nothing once `err` is set, so a sequence of uploads checks `err` once at the end.
 template <typename T>
-struct DevBuf {
-  T *ptr = nullptr;
-  size_t n = 0;
-  cudaError_t upload(const std::vector<T> &h) {
-    n = h.size();
-    cudaError_t e = cudaMalloc((void **)&ptr, std::max<size_t>(n, 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    if (n) e = cudaMemcpy(ptr, h.data(), n * sizeof(T), cudaMemcpyHostToDevice);
-    return e;
-  }
-  cudaError_t alloc(size_t count) {
-    n = count;
-    return cudaMalloc((void **)&ptr, std::max<size_t>(n, 1) * sizeof(T));
-  }
-  void release() {
-    if (ptr) cudaFree(ptr);
-    ptr = nullptr;
-    n = 0;
-  }
-};
+static T *upload(std::vector<void *> &allocs, const std::vector<T> &h, cudaError_t &err) {
+  T *p = nullptr;
+  if (err != cudaSuccess) return nullptr;
+  err = cudaMalloc((void **)&p, std::max<size_t>(h.size(), 1) * sizeof(T));
+  if (err != cudaSuccess) return nullptr;
+  allocs.push_back(p);
+  if (!h.empty()) err = cudaMemcpy(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
+  return p;
+}
 
 }  // namespace shapy

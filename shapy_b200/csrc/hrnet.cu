@@ -185,17 +185,6 @@ static int build_schedule(shapy_hrnet *p) {
   return SHAPY_OK;
 }
 
-template <typename T>
-static T *dev_upload(std::vector<void *> &allocs, const std::vector<T> &h, cudaError_t &err) {
-  T *d = nullptr;
-  if (err != cudaSuccess) return nullptr;
-  err = cudaMalloc((void **)&d, std::max<size_t>(h.size(), 1) * sizeof(T));
-  if (err != cudaSuccess) return nullptr;
-  allocs.push_back(d);
-  if (!h.empty()) err = cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  return d;
-}
-
 // Folds BN and packs one conv.  Returns false on CUDA failure.
 static bool pack_conv(const shapy_conv_desc_t &c, bool stem, ConvW &out, std::vector<void *> &allocs, cudaError_t &err) {
   const int taps = c.ksize * c.ksize;
@@ -212,14 +201,14 @@ static bool pack_conv(const shapy_conv_desc_t &c, bool stem, ConvW &out, std::ve
     }
   }
   out.cin = c.cin; out.cout = c.cout; out.ksize = c.ksize; out.stride = c.stride;
-  out.bias = dev_upload(allocs, bias, err);
+  out.bias = upload(allocs, bias, err);
   if (stem) {
     std::vector<float> wf((size_t)taps * c.cin * c.cout);
     for (int o = 0; o < c.cout; ++o)
       for (int i = 0; i < c.cin; ++i)
         for (int t = 0; t < taps; ++t)
           wf[((size_t)t * c.cin + i) * c.cout + o] = c.weight[((size_t)o * c.cin + i) * taps + t] * scale[o];
-    out.w_f32 = dev_upload(allocs, wf, err);
+    out.w_f32 = upload(allocs, wf, err);
     return err == cudaSuccess;
   }
   std::vector<__half> hi((size_t)taps * c.cout * c.cin), lo(hi.size());
@@ -232,8 +221,8 @@ static bool pack_conv(const shapy_conv_desc_t &c, bool stem, ConvW &out, std::ve
         hi[d] = h;
         lo[d] = __float2half_rn((v - __half2float(h)) * kLoScale);
       }
-  out.w_hi = dev_upload(allocs, hi, err);
-  out.w_lo = dev_upload(allocs, lo, err);
+  out.w_hi = upload(allocs, hi, err);
+  out.w_lo = upload(allocs, lo, err);
   return err == cudaSuccess;
 }
 

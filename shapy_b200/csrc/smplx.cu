@@ -2,18 +2,21 @@
 //
 // Replaces the ~90-launch reference chain (blend_shapes -> vertices2joints -> pose blend ->
 // batch_rigid_transform (54 serial bmm) -> skinning -> landmarks -> J14), reference
-// regressor/human_shape/models/body_models/lbs.py:99-295 and body_models.py:628-767, by three
+// regressor/human_shape/models/body_models/lbs.py:99-295 and body_models.py:628-767, by four
 // launches:
 //   smplx_pose_kernel    per body: joints from the (pre-contracted, exact) J_template + J_dirs . beta,
-//                        level-parallel kinematic chain, A = G - [0 | G . J], pose feature, contour LUT row
-//   smplx_vertex_kernel  tile of 32 vertices x 32 bodies: shape blend + pose blend (constants staged
-//                        through shared memory once per tile, reused by all 32 bodies) + sparse skinning
+//                        level-parallel kinematic chain, A = G - [0 | G . J], the pose feature as the
+//                        split-fp16 input of the pose-blend GEMM, contour LUT row
+//   pose-blend GEMM      (R[1:] - I) . posedirs of all bodies on the wgmma engine (pose_blend_gemm)
+//   smplx_vertex_kernel  tile of 32 vertices x 32 bodies: shape (+ expression) blend (constants staged
+//                        through shared memory once per tile, reused by all 32 bodies), plus the GEMM's
+//                        pose offsets, sparse skinning
 //   smplx_joints_kernel  per body: landmarks, sparse J14 regressor + overwrite, weak-perspective camera
 // plus smplx_shape_kernel for the T-pose path (SMPL.forward_shape, body_models.py:292-302).
 //
 // Exact structure that is exploited (changes summation order only):
 //   * J = J_regressor . (T + S.beta) = J_regressor.T + (J_regressor.S).beta  (contracted once, in fp64)
-//   * joints >= n_rot are identity => their pose-feature rows are exactly 0 and are skipped
+//   * joints >= n_rot are identity => their pose-feature columns are exactly 0 and are left out of the GEMM
 //   * lbs_weights and the J14 regressor are stored sparse (ELL / CSR); zero entries contribute exactly 0
 #include <algorithm>
 #include <cmath>
@@ -26,7 +29,7 @@ namespace shapy {
 
 constexpr int TV = 32;  // vertices per tile (one per lane)
 constexpr int TB = 32;  // bodies per tile (8 per warp, 4 warps)
-constexpr int KC = 32;  // pose-feature rows staged per chunk
+constexpr int KC = 32;  // blend-shape rows staged per chunk
 
 // ----------------------------------------------------------------------------------------------
 __global__ void decode_rot6d_kernel(const float *__restrict__ raw, int n, float *__restrict__ rot) {
@@ -49,13 +52,13 @@ __global__ void decode_rot6d_kernel(const float *__restrict__ raw, int n, float 
 }
 
 // ----------------------------------------------------------------------------------------------
-// Workspace layout (floats): A [B][J][12] | pfT [NC + Kp][Bpad] (blend coefficients, transposed) | lut [B] (int)
 struct PoseArgs {
   SmplxDev m;
   const float *betas, *expr, *rot;
-  int n_rot, B, Bpad, Kp;
+  int n_rot, B, Bpad, Kp, Kpad;
   float *A, *pfT, *joints;  // joints may be null
   int *lut;
+  __half *x_hi, *x_lo;      // pose-blend GEMM input [B][Kpad]; null when no GEMM runs
 };
 
 __global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
@@ -111,12 +114,16 @@ __global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
   if (a.joints) {
     for (int i = t; i < J * 3; i += blockDim.x) a.joints[((size_t)b * m.K) * 3 + i] = G[i / 3][(i % 3) * 4 + 3];
   }
-  // pose feature (R[1:] - I), transposed so that a body tile is contiguous
-  // blend coefficients of this body, one row per basis row: [betas | expression | pose feature]
+  // blend coefficients of this body, one row per basis row [betas | expression], transposed: a body tile is contiguous
   if (t < m.NC) a.pfT[(size_t)t * a.Bpad + b] = coef[t];
-  for (int k = t; k < a.Kp; k += blockDim.x) {
-    int j = 1 + k / 9, e = k % 9;
-    a.pfT[(size_t)(m.NC + k) * a.Bpad + b] = R[j][e] - ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f);
+  // pose feature (R[1:] - I) / kPoseScale as the split-fp16 GEMM input row of this body, zero-padded to Kpad
+  if (a.x_hi) {
+    __half *xh = a.x_hi + (size_t)b * a.Kpad, *xl = a.x_lo + (size_t)b * a.Kpad;
+    for (int k = t; k < a.Kpad; k += blockDim.x) {
+      int j = 1 + k / 9, e = k % 9;
+      const float x = k < a.Kp ? (R[j][e] - ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f)) * (1.0f / kPoseScale) : 0.f;
+      split_store(x, xh[k], xl[k]);
+    }
   }
   // dynamic-contour LUT row (lbs.py:30-41, rotation_utils.py:86-92)
   if (t == 0 && m.D > 0) {
@@ -142,9 +149,9 @@ struct VertexArgs {
   SmplxDev m;
   const float *betas, *expr;
   const float *A, *pfT;
-  int B, Bpad, Kp;
+  int B, Bpad;
   float *vertices, *v_shaped;  // either may be null
-  const __half *pb_hi, *pb_lo;  // pose blend [B][pb_ld] as hi + lo / 2048 (wgmma GEMM); null: pose rows run here
+  const __half *pb_hi, *pb_lo;  // pose blend [B][pb_ld] as hi + lo / 2048 (wgmma GEMM); null: none (n_rot 1, or no vertices)
   int pb_ld;
 };
 
@@ -166,17 +173,7 @@ __global__ void pack_pose_weights_kernel(const float *__restrict__ posedirs, int
   }
 }
 
-// pose feature rows of pfT ([NC + k][Bpad] fp32) -> split-fp16 GEMM activations [B][Kpad], / kPoseScale
-__global__ void pose_features_split_kernel(const float *__restrict__ pfT, int Bpad, int NC, int Kp, int Kpad, int B,
-                                           __half *__restrict__ hi, __half *__restrict__ lo) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * Kpad) return;
-  const int b = i / Kpad, k = i % Kpad;
-  const float x = k < Kp ? pfT[(size_t)(NC + k) * Bpad + b] * (1.0f / kPoseScale) : 0.f;
-  split_store(x, hi[i], lo[i]);
-}
-
-// One tile = 32 vertices (one per lane) x 32 bodies (8 per warp).  All blend-shape rows (shape, expression, pose)
+// One tile = 32 vertices (one per lane) x 32 bodies (8 per warp).  The shape and expression blend-shape rows
 // are one [rows][V3p] basis; a chunk of 32 rows (96 floats each) and the matching [rows][32 bodies] coefficient
 // block are staged in shared memory with 16-byte cp.async, double buffered, so every constant crosses L2 once
 // per tile and the loads of chunk i+1 overlap the FMAs of chunk i.
@@ -196,11 +193,9 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) { acc[i][0] = tx; acc[i][1] = ty; acc[i][2] = tz; }
   }
-  // row schedule: [0, NB) shape | [NB, NC) expression (only when given) | [NC, NC + Kp) pose (only for vertices)
+  // row schedule: [0, NB) shape | [NB, NC) expression (only when given, and only for vertices)
   const bool posed = a.vertices != nullptr;
-  const int n_expr = (a.expr && posed) ? m.NC - m.NB : 0;
-  const int n_rows = m.NB + n_expr + (posed && !a.pb_hi ? a.Kp : 0);
-  auto row_of = [&](int i) { return i < m.NB + n_expr ? i : m.NC + (i - m.NB - n_expr); };
+  const int n_rows = (a.expr && posed) ? m.NC : m.NB;
   // chunk boundaries: the first chunk ends exactly after the NB shape rows (v_shaped snapshot)
   auto chunk_begin = [&](int ch) { return ch == 0 ? 0 : m.NB + (ch - 1) * KC; };
   const int n_chunks = 1 + (n_rows > m.NB ? (n_rows - m.NB + KC - 1) / KC : 0);
@@ -211,12 +206,12 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
       const int k = i / 24, q = i % 24;
       const int col = c0 + q * 4;
       const int nb = max(0, min(16, (m.V3p - col) * 4));
-      const float *src = m.basis + (size_t)row_of(r0 + k) * m.V3p + (nb ? col : 0);
+      const float *src = m.basis + (size_t)(r0 + k) * m.V3p + (nb ? col : 0);
       cp_async16_zfill(&Ps[buf][k][q * 4], src, nb);
     }
     for (int i = t; i < nr * 8; i += 128) {             // 32 bodies = 8 x 16 bytes per row
       const int k = i / 8, q = i % 8;
-      cp_async16_zfill(&pfs[buf][k][q * 4], a.pfT + (size_t)row_of(r0 + k) * a.Bpad + b0 + q * 4, 16);
+      cp_async16_zfill(&pfs[buf][k][q * 4], a.pfT + (size_t)(r0 + k) * a.Bpad + b0 + q * 4, 16);
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
@@ -361,14 +356,14 @@ __global__ void __launch_bounds__(512) smplx_joints_kernel(JointsArgs a) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// T-pose path: v_shaped[b][c] = T[c] + sum_l beta[b][l] S[l][c].  One thread per coordinate, the NB
-// shape coefficients of that coordinate live in registers and are reused for SB bodies, so the only
-// HBM traffic is the (B, 3V) output stream (S and T are 1.4 MB and stay in L2).
+// T-pose path: v_shaped[b][c] = T[c] + sum_l beta[b][l] S[l][c], S = the shape rows of the basis (row pitch ld).
+// One thread per coordinate, the NB shape coefficients of that coordinate live in registers and are reused for SB
+// bodies, so the only HBM traffic is the (B, 3V) output stream (S and T are 1.4 MB and stay in L2).
 constexpr int SB = 64;
 constexpr int SBP = 12;   // padded beta row (float4 x 3) so a body's coefficients are 3 broadcast LDS.128
 template <int NB>
 __global__ void __launch_bounds__(256) smplx_shape_kernel(const float *__restrict__ T, const float *__restrict__ S,
-                                                          const float *__restrict__ betas, int V3, int B,
+                                                          int ld, const float *__restrict__ betas, int V3, int B,
                                                           float *__restrict__ out) {
   static_assert(NB <= SBP, "beta row padding");
   __shared__ __align__(16) float bs[SB][SBP];
@@ -385,12 +380,12 @@ __global__ void __launch_bounds__(256) smplx_shape_kernel(const float *__restric
   if (c0 < V3) {
     t0 = T[c0];
 #pragma unroll
-    for (int l = 0; l < NB; ++l) s0[l] = S[(size_t)l * V3 + c0];
+    for (int l = 0; l < NB; ++l) s0[l] = S[(size_t)l * ld + c0];
   }
   if (c1 < V3) {
     t1 = T[c1];
 #pragma unroll
-    for (int l = 0; l < NB; ++l) s1[l] = S[(size_t)l * V3 + c1];
+    for (int l = 0; l < NB; ++l) s1[l] = S[(size_t)l * ld + c1];
   }
   __syncthreads();
   const int nb = min(SB, B - b0);
@@ -409,26 +404,15 @@ __global__ void __launch_bounds__(256) smplx_shape_kernel(const float *__restric
   }
 }
 
-__global__ void smplx_shape_kernel_generic(const float *__restrict__ T, const float *__restrict__ S,
+__global__ void smplx_shape_kernel_generic(const float *__restrict__ T, const float *__restrict__ S, int ld,
                                            const float *__restrict__ betas, int NB, int V3, int B,
                                            float *__restrict__ out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (c >= V3) return;
   float v = T[c];
-  for (int l = 0; l < NB; ++l) v += betas[(size_t)b * NB + l] * S[(size_t)l * V3 + c];
+  for (int l = 0; l < NB; ++l) v += betas[(size_t)b * NB + l] * S[(size_t)l * ld + c];
   out[(size_t)b * V3 + c] = v;
-}
-
-template <typename T>
-static T *upload(shapy_smplx *m, const std::vector<T> &h, cudaError_t &err) {
-  T *p = nullptr;
-  if (err != cudaSuccess) return nullptr;
-  err = cudaMalloc((void **)&p, std::max<size_t>(h.size(), 1) * sizeof(T));
-  if (err != cudaSuccess) return nullptr;
-  m->allocs.push_back(p);
-  if (!h.empty()) err = cudaMemcpy(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  return p;
 }
 
 }  // namespace shapy
@@ -448,24 +432,22 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
   memset(&s, 0, sizeof(s));
   s.V = V; s.J = J; s.NB = NB; s.NE = NE; s.NC = NC; s.F = F;
   cudaError_t err = cudaSuccess;
-  s.v_template = upload(m, std::vector<float>(d->v_template, d->v_template + (size_t)V * 3), err);
+  s.v_template = upload(m->allocs, std::vector<float>(d->v_template, d->v_template + (size_t)V * 3), err);
   // shapedirs -> [NC][3V]
   std::vector<float> S((size_t)NC * V * 3);
   for (int c = 0; c < V * 3; ++c) {
     for (int l = 0; l < NB; ++l) S[(size_t)l * V * 3 + c] = d->shapedirs[(size_t)c * NB + l];
     for (int l = 0; l < NE; ++l) S[(size_t)(NB + l) * V * 3 + c] = d->expr_dirs[(size_t)c * NE + l];
   }
-  s.shapedirs = upload(m, S, err);
-  s.posedirs = upload(m, std::vector<float>(d->posedirs, d->posedirs + (size_t)(J - 1) * 9 * V * 3), err);
+  s.posedirs = upload(m->allocs, std::vector<float>(d->posedirs, d->posedirs + (size_t)(J - 1) * 9 * V * 3), err);
   {
-    // unified blend-shape basis with rows padded to a multiple of 4 floats (16-byte cp.async)
-    const int V3 = V * 3, V3p = (V3 + 3) / 4 * 4, KP = (J - 1) * 9;
-    std::vector<float> basis((size_t)(NC + KP) * V3p, 0.f);
+    // shape and expression blend-shape basis with rows padded to a multiple of 4 floats (16-byte cp.async)
+    const int V3 = V * 3, V3p = (V3 + 3) / 4 * 4;
+    std::vector<float> basis((size_t)NC * V3p, 0.f);
     for (int l = 0; l < NC; ++l) memcpy(&basis[(size_t)l * V3p], &S[(size_t)l * V3], (size_t)V3 * sizeof(float));
-    for (int k = 0; k < KP; ++k) memcpy(&basis[(size_t)(NC + k) * V3p], d->posedirs + (size_t)k * V3, (size_t)V3 * sizeof(float));
     s.V3p = V3p;
-    s.basis = upload(m, basis, err);
-    m->zero_bias = upload(m, std::vector<float>((size_t)(V3 + kPoseV3Align - 1) / kPoseV3Align * kPoseV3Align, 0.f), err);
+    s.basis = upload(m->allocs, basis, err);
+    m->zero_bias = upload(m->allocs, std::vector<float>((size_t)(V3 + kPoseV3Align - 1) / kPoseV3Align * kPoseV3Align, 0.f), err);
   }
   // joint regression contracted with the template and the shape basis (fp64 accumulate)
   std::vector<float> Jt((size_t)J * 3), Jd((size_t)J * 3 * NC);
@@ -484,8 +466,8 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
       for (int l = 0; l < NC; ++l) Jd[((size_t)j * 3 + c) * NC + l] = (float)ad[(size_t)c * NC + l];
     }
   }
-  s.J_template = upload(m, Jt, err);
-  s.J_dirs = upload(m, Jd, err);
+  s.J_template = upload(m->allocs, Jt, err);
+  s.J_dirs = upload(m->allocs, Jd, err);
   // ELL skinning weights
   int W = 1;
   for (int v = 0; v < V; ++v) {
@@ -503,8 +485,8 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
     }
   }
   s.ell_w_n = W;
-  s.ell_idx = upload(m, eidx, err);
-  s.ell_w = upload(m, ew, err);
+  s.ell_idx = upload(m->allocs, eidx, err);
+  s.ell_w = upload(m->allocs, ew, err);
   // kinematic levels
   std::vector<int> par(J), depth(J, 0);
   for (int j = 0; j < J; ++j) par[j] = j == 0 ? -1 : (int)d->parents[j];
@@ -521,31 +503,31 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
   }
   lo.push_back((int)lj.size());
   s.n_levels = maxd + 1;
-  s.parents = upload(m, par, err);
-  s.level_joints = upload(m, lj, err);
-  s.level_off = upload(m, lo, err);
+  s.parents = upload(m->allocs, par, err);
+  s.level_joints = upload(m->allocs, lj, err);
+  s.level_off = upload(m->allocs, lo, err);
   std::vector<int> faces((size_t)F * 3);
   for (size_t i = 0; i < faces.size(); ++i) faces[i] = (int)d->faces[i];
-  s.faces = upload(m, faces, err);
+  s.faces = upload(m->allocs, faces, err);
   // landmarks resolved to vertex triples
   s.L = d->lmk_faces_idx ? d->num_static_lmk : 0;
   std::vector<int> lv((size_t)s.L * 3);
   for (int i = 0; i < s.L; ++i)
     for (int c = 0; c < 3; ++c) lv[i * 3 + c] = faces[(size_t)d->lmk_faces_idx[i] * 3 + c];
-  s.lmk_vidx = upload(m, lv, err);
-  s.lmk_bc = upload(m, std::vector<float>(d->lmk_bary_coords, d->lmk_bary_coords + (size_t)s.L * 3), err);
+  s.lmk_vidx = upload(m->allocs, lv, err);
+  s.lmk_bc = upload(m->allocs, std::vector<float>(d->lmk_bary_coords, d->lmk_bary_coords + (size_t)s.L * 3), err);
   s.D = d->dynamic_lmk_faces_idx ? d->num_dyn_lmk : 0;
   s.rows = s.D ? d->num_dyn_rows : 0;
   std::vector<int> dv((size_t)s.rows * s.D * 3);
   for (size_t i = 0; i < (size_t)s.rows * s.D; ++i)
     for (int c = 0; c < 3; ++c) dv[i * 3 + c] = faces[(size_t)d->dynamic_lmk_faces_idx[i] * 3 + c];
-  s.dyn_vidx = upload(m, dv, err);
-  s.dyn_bc = upload(m, std::vector<float>(d->dynamic_lmk_bary_coords,
+  s.dyn_vidx = upload(m->allocs, dv, err);
+  s.dyn_bc = upload(m->allocs, std::vector<float>(d->dynamic_lmk_bary_coords,
                                           d->dynamic_lmk_bary_coords + (s.D ? (size_t)s.rows * s.D * 3 : 0)), err);
   s.n_chain = s.D ? d->neck_chain_len : 0;
   std::vector<int> neck(s.n_chain);
   for (int i = 0; i < s.n_chain; ++i) neck[i] = (int)d->neck_kin_chain[i];
-  s.neck = upload(m, neck, err);
+  s.neck = upload(m->allocs, neck, err);
   s.K = J + s.L + s.D;
   // J14 regressor -> CSR
   s.n_extra = d->extra_joint_regressor ? d->num_extra : 0;
@@ -558,14 +540,14 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
     }
     ep.push_back((int)ec.size());
   }
-  s.ex_ptr = upload(m, ep, err);
-  s.ex_col = upload(m, ec, err);
-  s.ex_val = upload(m, ev, err);
+  s.ex_ptr = upload(m->allocs, ep, err);
+  s.ex_col = upload(m->allocs, ec, err);
+  s.ex_val = upload(m->allocs, ev, err);
   s.n_over = s.n_extra ? d->num_overwrite : 0;
   std::vector<int> os(s.n_over), ot(s.n_over);
   for (int i = 0; i < s.n_over; ++i) { os[i] = (int)d->source_idxs[i]; ot[i] = (int)d->target_idxs[i]; }
-  s.over_src = upload(m, os, err);
-  s.over_tgt = upload(m, ot, err);
+  s.over_src = upload(m->allocs, os, err);
+  s.over_tgt = upload(m->allocs, ot, err);
   if (err != cudaSuccess) {
     set_error("shapy_smplx_create: %s", cudaGetErrorString(err));
     shapy_smplx_destroy(m);
@@ -590,15 +572,37 @@ static inline int bpad(int B) { return (B + 31) / 32 * 32; }
 static inline int pose_kpad(int Kp) { return (Kp + kPoseKAlign - 1) / kPoseKAlign * kPoseKAlign; }
 static inline int pose_v3g(const SmplxDev &d) { return (d.V * 3 + kPoseV3Align - 1) / kPoseV3Align * kPoseV3Align; }
 
-// workspace of the pose-blend GEMM: activations [B][Kpad] and result [B][V3g], split fp16 (hi, lo) each
-static size_t pose_gemm_bytes(const SmplxDev &d, int B) {
-  return 2 * align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256) +
-         2 * align_up((size_t)B * pose_v3g(d) * sizeof(__half), 256);
+// Workspace of shapy_smplx_forward, 256-byte aligned pieces.  The GEMM activations are sized for the widest pose
+// feature ((J - 1) * 9); a call uses the first B * Kpad of them.
+struct SmplxWorkspace {
+  float *A;              // [B][J][12] relative transforms
+  float *pfT;            // [NC][Bpad] blend coefficients, transposed
+  int *lut;              // [B] dynamic-contour LUT rows
+  float *joints;         // [B][K][3] joints when the caller asks for none
+  __half *x_hi, *x_lo;   // pose-blend GEMM activations [B][Kpad], split fp16
+  __half *y_hi, *y_lo;   // pose-blend GEMM result [B][V3g], split fp16
+  size_t bytes;
+};
+
+// base == nullptr: only `bytes` is meaningful
+static SmplxWorkspace smplx_workspace(const SmplxDev &d, int B, void *base) {
+  SmplxWorkspace w;
+  w.bytes = 0;
+  auto take = [&](size_t n) { void *p = base ? (char *)base + w.bytes : nullptr; w.bytes += align_up(n, 256); return p; };
+  const size_t x = (size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), y = (size_t)B * pose_v3g(d) * sizeof(__half);
+  w.A = (float *)take((size_t)B * d.J * 12 * sizeof(float));
+  w.pfT = (float *)take((size_t)d.NC * bpad(B) * sizeof(float));
+  w.lut = (int *)take((size_t)B * sizeof(int));
+  w.joints = (float *)take((size_t)B * d.K * 3 * sizeof(float));
+  w.x_hi = (__half *)take(x); w.x_lo = (__half *)take(x);
+  w.y_hi = (__half *)take(y); w.y_lo = (__half *)take(y);
+  return w;
 }
 
 // Pose blend (R[1:] - I) . P of all B bodies as one split-fp16 tensor-core GEMM on the wgmma engine, expressed as a
-// 1x1 convolution: "pixels" = bodies, cin = pose features, cout = the 3V vertex coordinates.  Fills va.pb_*.
-static int pose_blend_gemm(const shapy_smplx *m, const float *pfT, int B, int Kp, char *xw, cudaStream_t st,
+// 1x1 convolution: "pixels" = bodies, cin = pose features, cout = the 3V vertex coordinates.  Its input is what
+// smplx_pose_kernel wrote to ws.x_*.  Fills va.pb_*.
+static int pose_blend_gemm(const shapy_smplx *m, int B, int Kp, const SmplxWorkspace &ws, cudaStream_t st,
                            VertexArgs &va) {
   const SmplxDev &d = m->d;
   const int Kpad = pose_kpad(Kp), V3g = pose_v3g(d);
@@ -617,35 +621,24 @@ static int pose_blend_gemm(const shapy_smplx *m, const float *pfT, int B, int Kp
       pw = it->second;
     }
   }
-  __half *x_hi = (__half *)xw;
-  __half *x_lo = (__half *)(xw + align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256));
-  char *yw = xw + 2 * align_up((size_t)B * pose_kpad((d.J - 1) * 9) * sizeof(__half), 256);
-  __half *y_hi = (__half *)yw;
-  __half *y_lo = (__half *)(yw + align_up((size_t)B * V3g * sizeof(__half), 256));
-  pose_features_split_kernel<<<ceil_div(B * Kpad, 256), 256, 0, st>>>(pfT, bpad(B), d.NC, Kp, Kpad, B, x_hi, x_lo);
-  SHAPY_LAUNCH_CHECK();
   ConvW w;
   w.w_hi = pw.hi; w.w_lo = pw.lo; w.bias = m->zero_bias;
   w.cin = Kpad; w.cout = V3g; w.ksize = 1; w.stride = 1;
   ActView in, out;
-  in.hi = x_hi; in.lo = x_lo; in.N = B; in.H = 1; in.W = 1; in.C = Kpad; in.Ctot = Kpad; in.coff = 0;
-  out.hi = y_hi; out.lo = y_lo; out.N = B; out.H = 1; out.W = 1; out.C = V3g; out.Ctot = V3g; out.coff = 0;
+  in.hi = ws.x_hi; in.lo = ws.x_lo; in.N = B; in.H = 1; in.W = 1; in.C = Kpad; in.Ctot = Kpad; in.coff = 0;
+  out.hi = ws.y_hi; out.lo = ws.y_lo; out.N = B; out.H = 1; out.W = 1; out.C = V3g; out.Ctot = V3g; out.coff = 0;
   WgmmaPlan *plan = wgmma_plan_create(w, in, out, nullptr, false);
   if (!plan) return SHAPY_ERR_UNSUPPORTED;
   const int rc = wgmma_plan_launch(plan, st, false);
   wgmma_plan_destroy(plan);
   if (rc != SHAPY_OK) return rc;
-  va.pb_hi = y_hi; va.pb_lo = y_lo; va.pb_ld = V3g;
+  va.pb_hi = ws.y_hi; va.pb_lo = ws.y_lo; va.pb_ld = V3g;
   return SHAPY_OK;
 }
 
 extern "C" size_t shapy_smplx_workspace_bytes(const shapy_smplx_t *m, int B) {
   if (!m || B <= 0) return 0;
-  size_t a = align_up((size_t)B * m->d.J * 12 * sizeof(float), 256);
-  size_t p = align_up((size_t)((m->d.J - 1) * 9 + m->d.NC) * bpad(B) * sizeof(float), 256);
-  size_t l = align_up((size_t)B * sizeof(int), 256);
-  size_t j = align_up((size_t)B * m->d.K * 3 * sizeof(float), 256);
-  return a + p + l + j + pose_gemm_bytes(m->d, B);
+  return smplx_workspace(m->d, B, nullptr).bytes;
 }
 
 extern "C" int shapy_decode_rot6d(const float *raw, int n, float *rot, void *stream) {
@@ -668,21 +661,18 @@ extern "C" int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, c
   SHAPY_REQUIRE(!(joints && !vertices && (m->d.L + m->d.D + m->d.n_extra) > 0), "joints require vertices");
   cudaStream_t st = (cudaStream_t)stream;
   const SmplxDev &d = m->d;
-  char *w = (char *)workspace;
-  float *A = (float *)w; w += align_up((size_t)B * d.J * 12 * sizeof(float), 256);
-  float *pfT = (float *)w; w += align_up((size_t)((d.J - 1) * 9 + d.NC) * bpad(B) * sizeof(float), 256);
-  int *lut = (int *)w; w += align_up((size_t)B * sizeof(int), 256);
-  float *jscratch = (float *)w; w += align_up((size_t)B * d.K * 3 * sizeof(float), 256);
-  char *xw = w;
+  const SmplxWorkspace ws = smplx_workspace(d, B, workspace);
   const int Kp = (n_rot - 1) * 9;
+  const bool gemm = vertices && Kp > 0;
   {
-    PoseArgs pa{d, betas, d.NE ? expr : nullptr, rot, n_rot, B, bpad(B), Kp, A, pfT, joints ? joints : jscratch, lut};
+    PoseArgs pa{d, betas, d.NE ? expr : nullptr, rot, n_rot, B, bpad(B), Kp, pose_kpad(Kp), ws.A, ws.pfT,
+                joints ? joints : ws.joints, ws.lut, gemm ? ws.x_hi : nullptr, gemm ? ws.x_lo : nullptr};
     smplx_pose_kernel<<<B, 128, 0, st>>>(pa);
     SHAPY_LAUNCH_CHECK();
     if (vertices || v_shaped) {
-      VertexArgs va{d, betas, d.NE ? expr : nullptr, A, pfT, B, bpad(B), Kp, vertices, v_shaped, nullptr, nullptr, 0};
-      if (vertices && Kp > 0) {
-        const int rc = pose_blend_gemm(m, pfT, B, Kp, xw, st, va);
+      VertexArgs va{d, betas, d.NE ? expr : nullptr, ws.A, ws.pfT, B, bpad(B), vertices, v_shaped, nullptr, nullptr, 0};
+      if (gemm) {
+        const int rc = pose_blend_gemm(m, B, Kp, ws, st, va);
         if (rc != SHAPY_OK) return rc;
       }
       dim3 grid(ceil_div(d.V, TV), ceil_div(B, TB));
@@ -691,7 +681,7 @@ extern "C" int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, c
     }
   }
   if (joints && (d.L + d.D + d.n_extra > 0 || proj_joints)) {
-    JointsArgs ja{d, vertices, camera, lut, B, joints, proj_joints};
+    JointsArgs ja{d, vertices, camera, ws.lut, B, joints, proj_joints};
     size_t smem = ((size_t)d.K * 3 + (size_t)std::max(d.n_extra, 1) * 3) * sizeof(float);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -718,10 +708,10 @@ extern "C" int shapy_smplx_forward_shape(const shapy_smplx_t *m, const float *be
   const int V3 = d.V * 3;
   if (d.NB == 10) {
     dim3 grid(ceil_div(V3, 512), ceil_div(B, SB));
-    smplx_shape_kernel<10><<<grid, 256, 0, st>>>(d.v_template, d.shapedirs, betas, V3, B, v_shaped);
+    smplx_shape_kernel<10><<<grid, 256, 0, st>>>(d.v_template, d.basis, d.V3p, betas, V3, B, v_shaped);
   } else {
     dim3 grid(ceil_div(V3, 256), B);
-    smplx_shape_kernel_generic<<<grid, 256, 0, st>>>(d.v_template, d.shapedirs, betas, d.NB, V3, B, v_shaped);
+    smplx_shape_kernel_generic<<<grid, 256, 0, st>>>(d.v_template, d.basis, d.V3p, betas, d.NB, V3, B, v_shaped);
   }
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;

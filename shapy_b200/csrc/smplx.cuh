@@ -12,8 +12,8 @@ constexpr int kMaxCoef = 32;
 
 struct SmplxDev {
   int V, J, NB, NE, NC, F, L, D, rows, K, n_chain, n_levels, ell_w_n, n_extra, n_over;
-  float *v_template, *shapedirs /* [NC][3V] */, *posedirs /* [(J-1)*9][3V] */;
-  float *basis;   /* [NC + (J-1)*9][V3p]: shape, expression and pose blend-shape rows, 16-byte aligned rows */
+  float *v_template, *posedirs /* [(J-1)*9][3V], the source of the pose-blend GEMM weights */;
+  float *basis;   /* [NC][V3p]: shape then expression blend-shape rows, 16-byte aligned rows */
   int V3p;
   float *J_template /* [3J] */, *J_dirs /* [3J][NC] */;
   int *ell_idx;   /* [W][V] */
@@ -35,8 +35,9 @@ struct SmplxDev {
 struct shapy_smplx {
   shapy::SmplxDev d;
   std::vector<void *> allocs;
-  // pose blend on the tensor cores (wgmma): posedirs^T x kPoseScale as split-fp16 [V3g][Kpad] weights, built on first use
-  // per pose-feature width Kp (joints >= n_rot contribute exact zeros, so their rows are left out), and a zero bias
+  // pose blend on the tensor cores (wgmma), the only place the pose blend runs: posedirs^T x kPoseScale as split-fp16
+  // [V3g][Kpad] weights, built on first use per padded pose-feature width Kpad (joints >= n_rot contribute exact
+  // zeros, so a call's GEMM stops at its Kpad), and a zero bias
   struct PoseW { __half *hi = nullptr, *lo = nullptr; };
   mutable std::mutex pw_mu;
   mutable std::map<int, PoseW> pw;
