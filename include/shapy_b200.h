@@ -107,6 +107,13 @@ int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, const float 
 int shapy_smplx_forward_shape(const shapy_smplx_t *m, const float *betas, int batch, float *v_shaped,
                               void *stream);
 
+/* Adjoint of shapy_smplx_forward_shape (the betas term of lbs.blend_shapes, lbs.py:207-225, under autograd):
+ * grad_betas (B,NB) = shapedirs^T . grad_v_shaped (B,V,3), device fp32.  Deterministic; a body's result does not
+ * depend on the rest of the batch.  workspace: device, >= shapy_smplx_backward_shape_workspace_bytes(m, batch). */
+size_t shapy_smplx_backward_shape_workspace_bytes(const shapy_smplx_t *m, int batch);
+int shapy_smplx_backward_shape(const shapy_smplx_t *m, const float *grad_v_shaped, int batch, float *grad_betas,
+                               void *workspace, size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------------------- virtual measurements */
 typedef struct {
   int face_idx[5];      /* head_top, left_heel, chest, waist, hips landmark faces */
@@ -125,6 +132,23 @@ int shapy_measure_forward(const float *v_shaped, const int32_t *faces, int batch
 int shapy_measure_forward_tris(const float *triangles, int batch, int num_faces,
                                const shapy_measure_landmarks_t *lm, float *out, float *plane_points,
                                int32_t *plane_counts, int max_points, int32_t *status, void *stream);
+
+/* Backward of shapy_measure_forward with the reference's autograd semantics (body_measurements.py:137-173 for the
+ * circumferences, 182-199 height, 201-215 mass): grad_out (B,5) device -> grad_v (B,V,3) device, overwritten.
+ * The intersection points' barycentrics are constants (the reference selects them under no_grad, 137-139) and the
+ * plane height gets no gradient, so for the circumferences this is not what a finite difference of the mesh gives.
+ * inc_ptr (V+1) / inc (3F) int32 device: the vertex -> (face, corner) incidence of `faces` in CSR form, entries
+ * 3 f + k in ascending order per vertex.  The hull is recomputed from v_shaped (no forward state); the result is
+ * bit-identical from run to run and independent of the rest of the batch.  Where a circumference is NaN and its
+ * upstream gradient is non-zero, the body's whole gradient is NaN. */
+int shapy_measure_backward(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr, const int32_t *inc,
+                           int batch, int num_verts, int num_faces, const shapy_measure_landmarks_t *lm,
+                           const float *grad_out, float *grad_v, void *stream);
+
+/* Same on explicit triangles (B,F,3,3) -> grad_triangles (B,F,3,3) (BodyMeasurements.forward's input). */
+int shapy_measure_backward_tris(const float *triangles, int batch, int num_faces,
+                                const shapy_measure_landmarks_t *lm, const float *grad_out,
+                                float *grad_triangles, void *stream);
 
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.

@@ -69,6 +69,12 @@ _SIGS = {
                                       c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'shapy_measure_forward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,
                                            c_void_p, c_int, c_void_p, c_void_p]),
+    'shapy_smplx_backward_shape_workspace_bytes': (c_size_t, [c_void_p, c_int]),
+    'shapy_smplx_backward_shape': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'shapy_measure_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                       C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
+    'shapy_measure_backward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,
+                                            c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

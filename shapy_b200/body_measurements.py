@@ -11,6 +11,7 @@ import os.path as osp
 import torch
 import torch.nn as nn
 
+from . import autograd as _ag
 from . import ops as _ops
 
 
@@ -80,13 +81,20 @@ class BodyMeasurements(nn.Module):
             raise RuntimeError('BodyMeasurements: intersection-point capacity exceeded; affected values are NaN')
 
     def forward_vertices(self, v_shaped, faces_i32):
-        """Fast path: (B, V, 3) vertices + (F, 3) int32 faces; no (B, F, 3, 3) tensor is materialised."""
+        """Fast path: (B, V, 3) vertices + (F, 3) int32 faces; no (B, F, 3, 3) tensor is materialised.
+        Differentiable in v_shaped (shapy_b200.autograd) when grad mode is on and it requires grad."""
+        if _ag.wants_grad(v_shaped):
+            return self._pack(_ag.measure(self.landmarks(), v_shaped=v_shaped, faces_i32=faces_i32))
         return self._pack(_ops.measure(self.landmarks(), v_shaped=v_shaped, faces_i32=faces_i32))
 
     def forward(self, triangles, compute_mass=True, compute_height=True, compute_chest=True, compute_waist=True,
                 compute_hips=True, **kwargs):
-        """triangles: (B, F, 3, 3), as in the reference."""
-        out = self._pack(_ops.measure(self.landmarks(), triangles=triangles))
+        """triangles: (B, F, 3, 3), as in the reference.  Differentiable in triangles, as the reference is, when grad
+        mode is on and they require grad (first order only: see shapy_b200.autograd)."""
+        if _ag.wants_grad(triangles):
+            out = self._pack(_ag.measure(self.landmarks(), triangles=triangles))
+        else:
+            out = self._pack(_ops.measure(self.landmarks(), triangles=triangles))
         drop = [n for n, f in (('mass', compute_mass), ('height', compute_height), ('chest', compute_chest),
                                ('waist', compute_waist), ('hips', compute_hips)) if not f]
         for n in drop:

@@ -32,6 +32,23 @@
 // Points that share (x, z) are told apart by value (pt_before), never by their slot, whose order depends on timing.
 // A hull of zero area (fewer than 3 points, or all of them collinear or coincident in xz) is NaN: qhull raises on it.
 // Compiled with -fmad=false (bit parity of the predicates with oracle/mmi_oracle.c).
+//
+// measure_smem_kernel<SRC, true> is the backward of the five outputs (shapy_measure_backward*).  It reruns phases 0-3 from
+// the same code, so it walks exactly the hull whose edge lengths the forward summed, with no state saved by the
+// forward, and then writes the gradient (phase 4).  The reference's semantics (body_measurements.py:137-173, 182-215):
+//   mass    985/6 sign(sum det) d det/d v per face: v1 x v2, v2 x v0, v0 x v1 for the rows v0, v1, v2
+//   height  sign(y_head - y_heel) bc on the y components of the two landmark faces
+//   chest / waist / hips  p = bc . T with bc held constant (the reference selects the points under no_grad); each hull
+//           edge p_i -> p_j adds -u g to p_i and +u g to p_j, u the unit 3-D edge vector; points without a ray hit
+//           have bc = 0 and get nothing.  There is no gradient through the plane height: the landmark only places the
+//           query quad.
+//   sign(0) = 0, as torch.abs gives.  A NaN circumference with a non-zero upstream gradient makes the body's whole
+//   gradient NaN; with a zero upstream gradient it adds nothing.
+// The gradient kernel also keeps, per point slot, the (face, query half) code that produced it (phase 2) and, per hull
+// vertex, the next vertex of the walk (phase 3b); points with equal bits are ordered by that code, so the hull and its
+// gradient do not depend on timing either.  No float atomics touch the output: the dense mass term of a vertex (a
+// face corner) is summed over its incident faces in a fixed order, then the hull and height terms are added in a
+// fixed order, so a body's gradient is bit-identical from run to run and independent of the rest of the batch.
 #include "common.cuh"
 #include "mmi_device.cuh"
 
@@ -43,8 +60,17 @@ constexpr int kMaxCand = 8192;     // (face, plane, query triangle) candidates t
                                    // the buffer is reused for the per-chain candidate lists (u16) in phase 3
 constexpr int kChainCap = 640;     // 24 chains x 640 x 2 B = 30 KB <= 32 KB
 constexpr size_t kListBytes = 3 * kMaxPts * 12 + kMaxCand * 4;   // points + candidate queue, dynamic
+// gradient kernel only: per point slot its (face, query half) code (int) and the next hull vertex (u16)
+constexpr size_t kGradBytes = 3 * kMaxPts * 4 + 3 * kMaxPts * 2;
 
 enum TriSource { kStagedVerts, kGlobalVerts, kTriangles };
+
+struct MeasureGrad {
+  const float *gout;   // (B,5) upstream gradient
+  const int *inc_ptr;  // (V+1) CSR: vertex -> incident (face, corner) entries 3 f + k, stably sorted (vertex sources)
+  const int *inc;      // (3F)
+  float *grad;         // (B,V,3) or (B,F,3,3)
+};
 
 struct MeasureArgs {
   const float *verts;  // (B,V,3) or null
@@ -57,6 +83,7 @@ struct MeasureArgs {
   int *cnt_out;        // (B,3) or null
   int maxp;
   int *status;
+  MeasureGrad g;       // gradient kernel only
 };
 
 __device__ __forceinline__ bool better_next(double cx, double cz, float ax, float az, float bx, float bz) {
@@ -85,6 +112,18 @@ __device__ __forceinline__ bool pt_before(const float *a, const float *b) {
   return ord_bits(a[0]) < ord_bits(b[0]);
 }
 
+// pt_before; the gradient kernel breaks full ties between two slots of plane p by their (face, query half) code
+template <bool GRAD>
+__device__ __forceinline__ bool pt_order(const float *a, const float *b, const int *codes, int p, int i, int j) {
+  if constexpr (GRAD) {
+    if (pt_before(a, b)) return true;
+    if (pt_before(b, a)) return false;
+    return codes[p * kMaxPts + i] < codes[p * kMaxPts + j];
+  } else {
+    return pt_before(a, b);
+  }
+}
+
 struct Extreme { float x, z; int idx; };
 
 __device__ __forceinline__ void dir_key(float x, float z, int k, double &k1, double &k2) {
@@ -95,7 +134,16 @@ __device__ __forceinline__ void dir_key(float x, float z, int k, double &k1, dou
   k2 = -dz * (double)x + dx * (double)z;
 }
 
-template <int SRC>
+__device__ __forceinline__ float3 corner_cross(const mmi::Tri &T, int k) {
+  // d det[v0; v1; v2] / d v_k
+  const float3 a = k == 0 ? T.v1 : (k == 1 ? T.v2 : T.v0), c = k == 0 ? T.v2 : (k == 1 ? T.v0 : T.v1);
+  return make_float3(a.y * c.z - a.z * c.y, a.z * c.x - a.x * c.z, a.x * c.y - a.y * c.x);
+}
+
+__device__ __forceinline__ float sign_of(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : (x == 0.f ? 0.f : x)); }
+
+// GRAD = false: the forward; GRAD = true: the backward, see the top.
+template <int SRC, bool GRAD = false>
 __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -105,6 +153,16 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
   float *pts = reinterpret_cast<float *>(smem + vs_bytes);                          // [3][kMaxPts][3]
   int *cand = reinterpret_cast<int *>(smem + vs_bytes + 3 * kMaxPts * 12);          // [kMaxCand]
   unsigned short *clist = reinterpret_cast<unsigned short *>(cand);                // phase 3: [24][kChainCap]
+  int *codes = reinterpret_cast<int *>(smem + vs_bytes + kListBytes);              // GRAD: [3][kMaxPts]
+  unsigned short *nxt = reinterpret_cast<unsigned short *>(smem + vs_bytes + kListBytes + 3 * kMaxPts * 4);
+  // order of two point slots of plane p with the same (x, z): by value; the gradient kernel breaks full ties by code
+  auto quad = [](float h, int q) {
+    mmi::Tri Q;
+    Q.v0 = make_float3(-1.f, h, -1.f);
+    Q.v1 = q == 0 ? make_float3(1.f, h, -1.f) : make_float3(1.f, h, 1.f);
+    Q.v2 = q == 0 ? make_float3(1.f, h, 1.f) : make_float3(-1.f, h, 1.f);
+    return Q;
+  };
   __shared__ int cnt[3];
   __shared__ int ncand;
   __shared__ float hs[3], lmy[2];
@@ -193,7 +251,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       const int c = cand[i], f = c >> 3, p = (c >> 1) & 3, q = c & 1;
       const float h = p == 0 ? h0 : (p == 1 ? h1 : h2);
       mmi::Tri T = tri_of(f);
-      mmi::Tri Q;
+      mmi::Tri Q;       // = quad(h, q), spelled out: the forward kernel's code is kept as it was
       Q.v0 = make_float3(-1.f, h, -1.f);
       Q.v1 = q == 0 ? make_float3(1.f, h, -1.f) : make_float3(1.f, h, 1.f);
       Q.v2 = q == 0 ? make_float3(1.f, h, 1.f) : make_float3(-1.f, h, 1.f);
@@ -206,11 +264,12 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
         o[0] = T.v0.x * b1.x + T.v1.x * b1.y + T.v2.x * b1.z;
         o[1] = T.v0.y * b1.x + T.v1.y * b1.y + T.v2.y * b1.z;
         o[2] = T.v0.z * b1.x + T.v1.z * b1.y + T.v2.z * b1.z;
+        if constexpr (GRAD) codes[p * kMaxPts + slot] = (f << 1) | q;
       }
     }
   }
   __syncthreads();     // the candidate queue is dead from here on: its storage becomes the chain lists
-  if (t == 0) {
+  if (!GRAD && t == 0) {
     float v = 0.f;
     for (int i = 0; i < kThreads / 32; ++i) v += red[i];
     a.out[(size_t)b * 5 + 0] = fabsf(v) / 6.0f * 985.0f;
@@ -228,14 +287,14 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     for (int i = lane; i < n; i += 32) {
       double k1, k2;
       dir_key(P[3 * i], P[3 * i + 2], hk, k1, k2);
-      if (best < 0 || k1 > b1 || (k1 == b1 && (k2 > b2 || (k2 == b2 && pt_before(P + 3 * i, P + 3 * best))))) {
+      if (best < 0 || k1 > b1 || (k1 == b1 && (k2 > b2 || (k2 == b2 && pt_order<GRAD>(P + 3 * i, P + 3 * best, codes, hp, i, best))))) {
         best = i; b1 = k1; b2 = k2;
       }
     }
     for (int o = 16; o; o >>= 1) {
       const int ob = __shfl_xor_sync(0xffffffffu, best, o);
       const double o1 = __shfl_xor_sync(0xffffffffu, b1, o), o2 = __shfl_xor_sync(0xffffffffu, b2, o);
-      if (ob >= 0 && (best < 0 || o1 > b1 || (o1 == b1 && (o2 > b2 || (o2 == b2 && pt_before(P + 3 * ob, P + 3 * best)))))) {
+      if (ob >= 0 && (best < 0 || o1 > b1 || (o1 == b1 && (o2 > b2 || (o2 == b2 && pt_order<GRAD>(P + 3 * ob, P + 3 * best, codes, hp, ob, best)))))) {
         best = ob; b1 = o1; b2 = o2;
       }
     }
@@ -294,7 +353,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
           const int i = listed ? (int)L[q] : q;
           const float x = P[3 * i], z = P[3 * i + 2];
           if (x == cx && z == cz) continue;  // the point itself and its duplicates
-          if (nb < 0 || better_next(cx, cz, nx, nz, x, z) || (x == nx && z == nz && pt_before(P + 3 * i, P + 3 * nb))) {
+          if (nb < 0 || better_next(cx, cz, nx, nz, x, z) || (x == nx && z == nz && pt_order<GRAD>(P + 3 * i, P + 3 * nb, codes, hp, i, nb))) {
             nb = i; nx = x; nz = z;
           }
         }
@@ -303,7 +362,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
           const float ox = __shfl_xor_sync(0xffffffffu, nx, o), oz = __shfl_xor_sync(0xffffffffu, nz, o);
           if (ob >= 0) {
             const bool take = nb < 0 || better_next(cx, cz, nx, nz, ox, oz) ||
-                              (ox == nx && oz == nz && pt_before(P + 3 * ob, P + 3 * nb));
+                              (ox == nx && oz == nz && pt_order<GRAD>(P + 3 * ob, P + 3 * nb, codes, hp, ob, nb));
             if (take) { nb = ob; nx = ox; nz = oz; }
           }
         }
@@ -314,6 +373,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
         const float dx = P[3 * nb] - P[3 * cur], dy = P[3 * nb + 1] - P[3 * cur + 1], dz = P[3 * nb + 2] - P[3 * cur + 2];
         len += sqrtf(dx * dx + dy * dy + dz * dz);
         ++edges;
+        if constexpr (GRAD) { if (lane == 0) nxt[hp * kMaxPts + cur] = (unsigned short)nb; }
         cur = nb; cx = nx; cz = nz;
         if (nx == e1.x && nz == e1.z) break;
       }
@@ -321,6 +381,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     if (lane == 0) { chain_len[hp][hk] = len; chain_edges[hp][hk] = edges; }
   }
   __syncthreads();
+  __shared__ float perim_s[3];
   if (t < 3) {
     const int p = t;
     float perim = 0.f;
@@ -330,9 +391,127 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     // cannot tell: a thin triangle's obtuse vertex is extreme in none of the 8 directions.  qhull raises on these.
     if (cnt[p] < 3 || edges < 3) perim = __int_as_float(0x7fc00000);
     if ((overflow & (1 << p))) perim = __int_as_float(0x7fc00000);   // truncated point set
-    a.out[(size_t)b * 5 + 2 + p] = perim;
+    if constexpr (GRAD) perim_s[p] = perim;
+    else a.out[(size_t)b * 5 + 2 + p] = perim;
   }
-  if (t == 0 && overflow && a.status) atomicExch(a.status, 1);
+  if constexpr (!GRAD) {
+    if (t == 0 && overflow && a.status) atomicExch(a.status, 1);
+  } else {
+    // ---- phase 4: gradient.  The chain lists are dead: their storage holds the hull vertex list of each plane
+    // (hull[p][j] = start slot of the j-th edge, chains in order) and then a bitmap of the faces that carry a hull point.
+    unsigned short *hull = clist;                                                   // [3][kMaxPts]
+    unsigned *fbits = reinterpret_cast<unsigned *>(clist + 3 * kMaxPts);
+    const int nbits_words = (int)((kMaxCand * 4 - 3 * kMaxPts * 2) / 4);
+    const bool all_flagged = a.F > nbits_words * 32;                                // bitmap too small: scan every face
+    __shared__ float gs[5];           // mass scale, height scale, the 3 circumference gradients
+    __shared__ int nedge[3], poison;
+    const MeasureGrad &g = a.g;
+    const float *go = g.gout + (size_t)b * 5;
+    if (t == 0) {
+      float v = 0.f;
+      for (int i = 0; i < kThreads / 32; ++i) v += red[i];                          // the forward's volume, same order
+      gs[0] = go[0] * sign_of(v) * (985.0f / 6.0f);
+      gs[1] = go[1] * sign_of(lmy[0] - lmy[1]);
+      int bad = 0;
+      for (int p = 0; p < 3; ++p) {
+        gs[2 + p] = go[2 + p];
+        int m = 0;
+        for (int k = 0; k < 8; ++k) m += chain_edges[p][k];
+        if (go[2 + p] != 0.f && (isnan(perim_s[p]) || m > kMaxPts)) bad = 1;
+        nedge[p] = (go[2 + p] != 0.f && !isnan(perim_s[p]) && m <= kMaxPts) ? m : 0;
+      }
+      poison = bad;
+    }
+    if (warp < 24 && lane == 0) {
+      int off = 0, m = 0;
+      for (int k = 0; k < 8; ++k) { off += k < hk ? chain_edges[hp][k] : 0; m += chain_edges[hp][k]; }
+      int cur = ext[hp][hk].idx;
+      if (m <= kMaxPts)
+        for (int s = 0; s < chain_edges[hp][hk]; ++s) { hull[hp * kMaxPts + off + s] = (unsigned short)cur; cur = nxt[hp * kMaxPts + cur]; }
+    }
+    for (int i = t; i < nbits_words; i += kThreads) fbits[i] = 0u;
+    __syncthreads();
+    // per hull vertex j of plane p: g (u_in - u_out), u the unit vectors of the edges into and out of it.  The walk is
+    // one closed cycle (the end of each chain is the start of the next); a vertex where it is not poisons the body.
+    float3 val[3];
+    for (int it = 0; it < 3; ++it) {
+      val[it] = make_float3(0.f, 0.f, 0.f);
+      const int r = t + it * kThreads, p = r / kMaxPts, j = r % kMaxPts, m = nedge[p];
+      if (j >= m) continue;
+      const float *P = pts + (size_t)p * kMaxPts * 3;
+      const unsigned short *H = hull + p * kMaxPts;
+      const int cur = H[j], prev = H[(j + m - 1) % m], next = nxt[p * kMaxPts + cur];
+      if (nxt[p * kMaxPts + prev] != cur || next != H[(j + 1) % m]) { poison = 1; continue; }
+      const float ix = P[3 * cur] - P[3 * prev], iy = P[3 * cur + 1] - P[3 * prev + 1], iz = P[3 * cur + 2] - P[3 * prev + 2];
+      const float ox = P[3 * next] - P[3 * cur], oy = P[3 * next + 1] - P[3 * cur + 1], oz = P[3 * next + 2] - P[3 * cur + 2];
+      const float li = sqrtf(ix * ix + iy * iy + iz * iz), lo = sqrtf(ox * ox + oy * oy + oz * oz);
+      const float gp = gs[2 + p];
+      val[it] = make_float3(gp * (ix / li - ox / lo), gp * (iy / li - oy / lo), gp * (iz / li - oz / lo));
+      if (!all_flagged) {
+        const int f = codes[p * kMaxPts + cur] >> 1;
+        atomicOr(&fbits[f >> 5], 1u << (f & 31));
+      }
+    }
+    __syncthreads();                  // the points are dead: their storage takes the hull vertex gradients
+    for (int it = 0; it < 3; ++it) {
+      const int r = t + it * kThreads;
+      if (r % kMaxPts < nedge[r / kMaxPts]) {
+        pts[3 * r] = val[it].x; pts[3 * r + 1] = val[it].y; pts[3 * r + 2] = val[it].z;
+      }
+    }
+    __syncthreads();
+    const float sm = gs[0], sh = gs[1];
+    const float nan = __int_as_float(0x7fc00000);
+    const bool bad = poison != 0;
+    // hull and height terms of corner k of face f (T = its triangle), in a fixed order: planes, hull order, height
+    auto sparse = [&](int f, const mmi::Tri &T, int k, float3 &acc) {
+      if (all_flagged || (fbits[f >> 5] >> (f & 31)) & 1u) {
+        for (int p = 0; p < 3; ++p) {
+          for (int j = 0; j < nedge[p]; ++j) {
+            const int c = codes[p * kMaxPts + hull[p * kMaxPts + j]];
+            if ((c >> 1) != f) continue;
+            float3 b1 = make_float3(0, 0, 0), b2 = b1;
+            mmi::isect_points(quad(hs[p], c & 1), T, b1, b2);          // the bc phase 2 used for this point
+            const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+            const float *gv = pts + 3 * (p * kMaxPts + j);
+            acc.x += w * gv[0]; acc.y += w * gv[1]; acc.z += w * gv[2];
+          }
+        }
+      }
+      if (f == a.lm.face_idx[0]) acc.y += sh * a.lm.bc[0][k];
+      if (f == a.lm.face_idx[1]) acc.y -= sh * a.lm.bc[1][k];
+    };
+    if constexpr (SRC == kTriangles) {
+      for (int f = t; f < a.F; f += blockDim.x) {
+        const mmi::Tri T = tri_of(f);
+        float *o = g.grad + ((size_t)b * a.F + f) * 9;
+        for (int k = 0; k < 3; ++k) {
+          const float3 c = corner_cross(T, k);
+          float3 acc = make_float3(sm * c.x, sm * c.y, sm * c.z);
+          sparse(f, T, k, acc);
+          o[3 * k] = bad ? nan : acc.x; o[3 * k + 1] = bad ? nan : acc.y; o[3 * k + 2] = bad ? nan : acc.z;
+        }
+      }
+    } else {
+      for (int v = t; v < a.V; v += blockDim.x) {
+        const int e0 = __ldg(g.inc_ptr + v), e1 = __ldg(g.inc_ptr + v + 1);
+        float3 acc = make_float3(0.f, 0.f, 0.f);
+        for (int e = e0; e < e1; ++e) {
+          const int fk = __ldg(g.inc + e);
+          const float3 c = corner_cross(tri_of(fk / 3), fk % 3);
+          acc.x += c.x; acc.y += c.y; acc.z += c.z;
+        }
+        acc = make_float3(sm * acc.x, sm * acc.y, sm * acc.z);
+        for (int e = e0; e < e1; ++e) {
+          const int fk = __ldg(g.inc + e), f = fk / 3;
+          if (all_flagged || f == a.lm.face_idx[0] || f == a.lm.face_idx[1] || ((fbits[f >> 5] >> (f & 31)) & 1u))
+            sparse(f, tri_of(f), fk % 3, acc);
+        }
+        float *o = g.grad + ((size_t)b * a.V + v) * 3;
+        o[0] = bad ? nan : acc.x; o[1] = bad ? nan : acc.y; o[2] = bad ? nan : acc.z;
+      }
+    }
+  }
 }
 
 size_t measure_smem_bytes(int V) { return (((size_t)V * 12 + 15) & ~(size_t)15) + kListBytes; }
@@ -342,6 +521,15 @@ static int launch_source(const MeasureArgs &a, size_t smem, int max_smem, cudaSt
   static std::atomic<unsigned long long> attr_done{0};   // one per instantiation
   SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC>, max_smem, attr_done));
   measure_smem_kernel<SRC><<<a.B, kThreads, smem, stream>>>(a);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+template <int SRC>
+static int launch_grad_source(const MeasureArgs &a, size_t smem, int max_smem, cudaStream_t stream) {
+  static std::atomic<unsigned long long> attr_done{0};
+  SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC, true>, max_smem, attr_done));
+  measure_smem_kernel<SRC, true><<<a.B, kThreads, smem, stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
@@ -368,7 +556,7 @@ extern "C" int shapy_measure_forward(const float *v_shaped, const int32_t *faces
                                      void *stream) {
   SHAPY_REQUIRE(v_shaped && faces && lm, "shapy_measure_forward: null argument");
   MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, out, plane_points, plane_counts,
-                max_points, status};
+                max_points, status, MeasureGrad{}};
   return launch_measure(a, stream);
 }
 
@@ -377,6 +565,39 @@ extern "C" int shapy_measure_forward_tris(const float *triangles, int batch, int
                                           int32_t *plane_counts, int max_points, int32_t *status, void *stream) {
   SHAPY_REQUIRE(triangles && lm, "shapy_measure_forward_tris: null argument");
   MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, out, plane_points, plane_counts, max_points,
-                status};
+                status, MeasureGrad{}};
   return launch_measure(a, stream);
+}
+
+static int launch_measure_grad(const MeasureArgs &a, void *stream) {
+  const MeasureGrad &g = a.g;
+  SHAPY_REQUIRE(g.gout && g.grad && a.B > 0 && a.F > 0, "shapy_measure_backward: bad argument");
+  for (int i = 0; i < 5; ++i)
+    SHAPY_REQUIRE(a.lm.face_idx[i] >= 0 && a.lm.face_idx[i] < a.F, "landmark face %d out of range", a.lm.face_idx[i]);
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t list = kListBytes + kGradBytes;
+  if (a.tris) return launch_grad_source<kTriangles>(a, list, (int)list, s);
+  SHAPY_REQUIRE(g.inc_ptr && g.inc && a.V > 0, "shapy_measure_backward: null incidence table");
+  const size_t staged = measure_smem_bytes(a.V) + kGradBytes;
+  if (a.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts>(a, staged, 226 * 1024, s);
+  return launch_grad_source<kGlobalVerts>(a, list, (int)list, s);
+}
+
+extern "C" int shapy_measure_backward(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
+                                      const int32_t *inc, int batch, int num_verts, int num_faces,
+                                      const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_v,
+                                      void *stream) {
+  SHAPY_REQUIRE(v_shaped && faces && lm, "shapy_measure_backward: null argument");
+  MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
+                MeasureGrad{grad_out, inc_ptr, inc, grad_v}};
+  return launch_measure_grad(a, stream);
+}
+
+extern "C" int shapy_measure_backward_tris(const float *triangles, int batch, int num_faces,
+                                           const shapy_measure_landmarks_t *lm, const float *grad_out,
+                                           float *grad_triangles, void *stream) {
+  SHAPY_REQUIRE(triangles && lm, "shapy_measure_backward_tris: null argument");
+  MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
+                MeasureGrad{grad_out, nullptr, nullptr, grad_triangles}};
+  return launch_measure_grad(a, stream);
 }

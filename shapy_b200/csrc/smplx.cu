@@ -415,6 +415,84 @@ __global__ void smplx_shape_kernel_generic(const float *__restrict__ T, const fl
   out[(size_t)b * V3 + c] = v;
 }
 
+// Adjoint of the T-pose path: grad_betas[b][l] = sum_c S[l][c] grad_v[b][c].  The 3V coordinates are cut into
+// kShapeSplit fixed chunks; CTA (tile, chunk) writes the partial sums of its bodies over its chunk (per thread over a
+// fixed stride, then a fixed xor tree and a fixed order over warps) and smplx_shape_bwd_sum_kernel adds the chunks in
+// order.  Neither the chunking nor the order depends on B or on a body's place in the batch, so a body's gradient is
+// bit-identical alone and in any batch.  HBM traffic is the (B, 3V) gradient read once (S stays in L2, read once per
+// kShapeTile bodies).
+constexpr int kShapeSplit = 16;
+constexpr int kShapeTile = 8;
+template <int NB>
+__global__ void __launch_bounds__(256) smplx_shape_bwd_kernel(const float *__restrict__ S, int ld,
+                                                              const float *__restrict__ gv, int V3, int B,
+                                                              float *__restrict__ part) {
+  const int b0 = blockIdx.x * kShapeTile, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int nb = min(kShapeTile, B - b0);
+  const int chunk = (V3 + kShapeSplit - 1) / kShapeSplit, c_lo = blockIdx.y * chunk, c_hi = min(V3, c_lo + chunk);
+  float acc[kShapeTile][NB];
+#pragma unroll
+  for (int i = 0; i < kShapeTile; ++i)
+#pragma unroll
+    for (int l = 0; l < NB; ++l) acc[i][l] = 0.f;
+  for (int c = c_lo + t; c < c_hi; c += 256) {
+    float s[NB];
+#pragma unroll
+    for (int l = 0; l < NB; ++l) s[l] = __ldg(S + (size_t)l * ld + c);
+#pragma unroll
+    for (int i = 0; i < kShapeTile; ++i) {
+      if (i < nb) {
+        const float g = __ldcs(gv + (size_t)(b0 + i) * V3 + c);
+#pragma unroll
+        for (int l = 0; l < NB; ++l) acc[i][l] += g * s[l];
+      }
+    }
+  }
+  __shared__ float red[8][kShapeTile * NB];
+#pragma unroll
+  for (int i = 0; i < kShapeTile; ++i)
+#pragma unroll
+    for (int l = 0; l < NB; ++l) {
+      float v = acc[i][l];
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) red[warp][i * NB + l] = v;
+    }
+  __syncthreads();
+  for (int r = t; r < nb * NB; r += 256) {
+    float v = 0.f;
+    for (int w = 0; w < 8; ++w) v += red[w][r];
+    part[((size_t)(b0 + r / NB) * kShapeSplit + blockIdx.y) * NB + r % NB] = v;
+  }
+}
+
+// any NB: CTA (body, chunk, l)
+__global__ void __launch_bounds__(256) smplx_shape_bwd_kernel_generic(const float *__restrict__ S, int ld,
+                                                                      const float *__restrict__ gv, int NB, int V3,
+                                                                      float *__restrict__ part) {
+  const int b = blockIdx.x, l = blockIdx.z, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int chunk = (V3 + kShapeSplit - 1) / kShapeSplit, c_lo = blockIdx.y * chunk, c_hi = min(V3, c_lo + chunk);
+  float v = 0.f;
+  for (int c = c_lo + t; c < c_hi; c += 256) v += __ldg(gv + (size_t)b * V3 + c) * __ldg(S + (size_t)l * ld + c);
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __shared__ float red[8];
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  if (t == 0) {
+    float s = 0.f;
+    for (int w = 0; w < 8; ++w) s += red[w];
+    part[((size_t)b * kShapeSplit + blockIdx.y) * NB + l] = s;
+  }
+}
+
+__global__ void smplx_shape_bwd_sum_kernel(const float *__restrict__ part, int NB, int B, float *__restrict__ gb) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= B * NB) return;
+  const int b = r / NB, l = r % NB;
+  float v = 0.f;
+  for (int s = 0; s < kShapeSplit; ++s) v += part[((size_t)b * kShapeSplit + s) * NB + l];
+  gb[r] = v;
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -713,6 +791,32 @@ extern "C" int shapy_smplx_forward_shape(const shapy_smplx_t *m, const float *be
     dim3 grid(ceil_div(V3, 256), B);
     smplx_shape_kernel_generic<<<grid, 256, 0, st>>>(d.v_template, d.basis, d.V3p, betas, d.NB, V3, B, v_shaped);
   }
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" size_t shapy_smplx_backward_shape_workspace_bytes(const shapy_smplx_t *m, int batch) {
+  return m && batch > 0 ? (size_t)batch * kShapeSplit * m->d.NB * sizeof(float) : 0;
+}
+
+extern "C" int shapy_smplx_backward_shape(const shapy_smplx_t *m, const float *grad_v_shaped, int B, float *grad_betas,
+                                          void *workspace, size_t workspace_bytes, void *stream) {
+  SHAPY_REQUIRE(m && grad_v_shaped && grad_betas && B > 0, "shapy_smplx_backward_shape: bad argument");
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_smplx_backward_shape_workspace_bytes(m, B),
+                "shapy_smplx_backward_shape: workspace too small");
+  const SmplxDev &d = m->d;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int V3 = d.V * 3;
+  float *part = static_cast<float *>(workspace);
+  if (d.NB == 10) {
+    smplx_shape_bwd_kernel<10><<<dim3(ceil_div(B, kShapeTile), kShapeSplit), 256, 0, st>>>(d.basis, d.V3p,
+                                                                                         grad_v_shaped, V3, B, part);
+  } else {
+    smplx_shape_bwd_kernel_generic<<<dim3(B, kShapeSplit, d.NB), 256, 0, st>>>(d.basis, d.V3p, grad_v_shaped, d.NB,
+                                                                               V3, part);
+  }
+  SHAPY_LAUNCH_CHECK();
+  smplx_shape_bwd_sum_kernel<<<ceil_div(B * d.NB, 256), 256, 0, st>>>(part, d.NB, B, grad_betas);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

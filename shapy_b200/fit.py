@@ -1,0 +1,134 @@
+"""Batched fitting of SMPL-X betas to virtual measurements on the device.
+
+    from shapy_b200.fit import fit_betas_to_measurements
+    res = fit_betas_to_measurements(body_model, body_measurements, {'height': h, 'mass': m, ...})   # (B,) targets
+
+    python -m shapy_b200.fit --synthetic --height 1.80 --mass 80 --output fit.npz
+    python -m shapy_b200.fit --model-folder models/smplx --targets targets.npz --output fit.npz
+
+The loss is the one of the reference's mesh-mesh-intersection/examples/fit_measurements.py:111-133, per body:
+sum_k w_k (target_k - measured_k)^2 + betas_weight |betas|^2, default weights height 100, mass 1, chest 2000,
+waist 1000, hips 1000; a target <= 0 or a weight <= 1e-3 drops that term (per body for the targets).  The bodies go
+through SMPLX.forward_shape -> BodyMeasurements.forward_vertices, both differentiable (shapy_b200.autograd), and the
+whole batch is optimised at once with Adam: Adam is elementwise, so every body's trajectory is independent of the
+rest of the batch (the reference's L-BFGS / TrustRegion would couple them through the line search and needs a double
+backward, which is not supported).
+"""
+import argparse
+import json
+
+import numpy as np
+import torch
+
+NAMES = ('mass', 'height', 'chest', 'waist', 'hips')
+DEFAULT_WEIGHTS = {'height': 100.0, 'mass': 1.0, 'chest': 2000.0, 'waist': 1000.0, 'hips': 1000.0}
+
+
+def _targets(targets, B, device):
+    out = {}
+    for k in NAMES:
+        v = targets.get(k, -1.0)
+        t = torch.as_tensor(v, dtype=torch.float32, device=device).reshape(-1)
+        out[k] = t.expand(B).contiguous() if t.numel() == 1 else t
+        if out[k].numel() != B:
+            raise ValueError(f'target `{k}` has {out[k].numel()} values for {B} bodies')
+    return out
+
+
+def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=500,
+                              lr=0.05, betas_init=None, batch_size=None):
+    """Fits betas (B, NB) so that the model's T-pose measurements match `targets`.
+
+    body_model: shapy_b200 SMPLX (its forward_shape and faces are used); body_measurements: shapy_b200
+    BodyMeasurements on the same device.  targets: {name: float or (B,) values} for mass [kg], height, chest, waist,
+    hips [m]; a missing name or a value <= 0 drops that term.  batch_size: B when every target is a scalar (default 1).
+    Returns {'betas': (B, NB), 'measurements': (B, 5) of the final betas (mass, height, chest, waist, hips),
+    'loss': (B,) final per-body loss}."""
+    device = body_model.shapedirs.device
+    B = batch_size or max([torch.as_tensor(v).numel() for v in targets.values()] + [1])
+    if betas_init is not None:
+        B = betas_init.shape[0]
+    tg = _targets(targets, B, device)
+    w = dict(DEFAULT_WEIGHTS, **(weights or {}))
+    # per-body weight: 0 where the target is <= 0 or the weight is <= 1e-3 (fit_measurements.py:111-133)
+    wt = torch.stack([torch.where(tg[k] > 0, torch.full_like(tg[k], w[k]), torch.zeros_like(tg[k]))
+                      if w[k] > 1e-3 else torch.zeros_like(tg[k]) for k in NAMES], 1)
+    tgt = torch.stack([tg[k].clamp(min=0) for k in NAMES], 1)
+    faces = body_model.faces_i32
+    nb = body_model.shapedirs.shape[-1]
+    betas = (torch.zeros(B, nb, device=device) if betas_init is None else betas_init.detach().clone().float())
+    betas.requires_grad_(True)
+    opt = torch.optim.Adam([betas], lr=lr)
+    # the step size decays geometrically to lr / 100 over the run, so the last iterations refine instead of orbiting
+    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
+
+    def loss_fn(b):
+        v = body_model.forward_shape(betas=b)['v_shaped']
+        m = body_measurements.forward_vertices(v, faces)['measurements']
+        meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+        diff = torch.where(wt > 0, tgt - meas, torch.zeros_like(meas))    # a dropped term passes no (NaN) gradient
+        per_body = (wt * diff.pow(2)).sum(1) + betas_weight * b.pow(2).sum(1)
+        return per_body, meas
+
+    for _ in range(int(iterations)):
+        opt.zero_grad(set_to_none=True)
+        per_body, _ = loss_fn(betas)
+        per_body.sum().backward()
+        opt.step()
+        sched.step()
+    with torch.no_grad():
+        per_body, meas = loss_fn(betas)
+    return {'betas': betas.detach(), 'measurements': meas, 'loss': per_body}
+
+
+def main(argv=None):
+    p = argparse.ArgumentParser(description='Fit SMPL-X betas to virtual measurements (batched, on the GPU)')
+    src = p.add_mutually_exclusive_group(required=True)
+    src.add_argument('--model-folder', type=str, help='folder with SMPLX_{GENDER}.{ext}')
+    src.add_argument('--synthetic', action='store_true', help='the seeded synthetic SMPL-X model of shapy_b200.synth')
+    p.add_argument('--gender', type=str, default='neutral')
+    p.add_argument('--num-betas', dest='num_betas', type=int, default=10)
+    p.add_argument('--ext', type=str, default='npz')
+    p.add_argument('--height', type=float, default=1.80, help='height in metres')
+    p.add_argument('--mass', type=float, default=-1, help='mass in kilograms')
+    p.add_argument('--chest', type=float, default=-1, help='chest circumference in metres')
+    p.add_argument('--waist', type=float, default=-1, help='waist circumference in metres')
+    p.add_argument('--hips', type=float, default=-1, help='hips circumference in metres')
+    p.add_argument('--targets', type=str, default=None,
+                   help='npz with per-body arrays mass / height / chest / waist / hips (overrides the single targets)')
+    p.add_argument('--meas-definition-path', dest='meas_definition_path', type=str, default=None)
+    p.add_argument('--meas-vertices-path', dest='meas_vertices_path', type=str, default=None)
+    p.add_argument('--betas-weight', dest='betas_weight', type=float, default=0.0)
+    p.add_argument('--iterations', type=int, default=500)
+    p.add_argument('--lr', type=float, default=0.05)
+    p.add_argument('--output', type=str, default='fit_betas.npz')
+    a = p.parse_args(argv)
+
+    from . import synth
+    from .body_measurements import BodyMeasurements
+    from .human_shape.models.body_models.body_models import SMPLX
+    if a.synthetic:
+        model = SMPLX(data_struct=synth.make_smplx())
+    else:
+        model = SMPLX(model_folder=a.model_folder, gender=a.gender, ext=a.ext, betas={'num': a.num_betas})
+    model = model.cuda()
+    if a.meas_definition_path and a.meas_vertices_path:
+        cfg = {'meas_definition_path': a.meas_definition_path, 'meas_vertices_path': a.meas_vertices_path}
+    else:
+        cfg = {'landmarks': synth.load_landmarks()}
+    bm = BodyMeasurements(cfg).cuda()
+    if a.targets:
+        d = np.load(a.targets)
+        targets = {k: d[k].astype(np.float32) for k in NAMES if k in d.files}
+    else:
+        targets = {k: getattr(a, k) for k in NAMES}
+    res = fit_betas_to_measurements(model, bm, targets, betas_weight=a.betas_weight, iterations=a.iterations, lr=a.lr)
+    meas = res['measurements'].cpu().numpy()
+    np.savez(a.output, betas=res['betas'].cpu().numpy(), measurements=meas, names=np.array(NAMES),
+             loss=res['loss'].cpu().numpy())
+    print(json.dumps({'bodies': int(meas.shape[0]), 'output': a.output,
+                      'first_body': {k: float(meas[0, i]) for i, k in enumerate(NAMES)}}))
+
+
+if __name__ == '__main__':
+    main()

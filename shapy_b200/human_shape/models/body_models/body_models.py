@@ -15,6 +15,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from .... import autograd as _ag
 from .... import ops as _ops
 from .utils import KeypointTensor, find_joint_kin_chain, to_tensor
 
@@ -211,7 +212,11 @@ class SMPLX(nn.Module):
 
     # ------------------------------------------------------------------ forward
     def forward_shape(self, betas=None):
-        v_shaped = _ops.smplx_forward_shape(self.packed(betas.device), betas)
+        """T-pose vertices; differentiable in betas (shapy_b200.autograd) when grad mode is on and they require grad."""
+        if _ag.wants_grad(betas):
+            v_shaped = _ag.ShapeFunction.apply(self.packed(betas.device), betas)
+        else:
+            v_shaped = _ops.smplx_forward_shape(self.packed(betas.device), betas)
         return {'vertices': v_shaped, 'betas': betas, 'v_shaped': v_shaped}
 
     def forward(self, global_rot=None, body_pose=None, left_hand_pose=None, right_hand_pose=None, jaw_pose=None,

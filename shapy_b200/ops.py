@@ -219,6 +219,81 @@ def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, tri
     return out
 
 
+_INCIDENCE = {}      # id(faces tensor) -> (weak reference, version, incidence); entries leave with their tensor
+
+
+def face_incidence(faces_i32):
+    """Vertex -> (face, corner) incidence of a CUDA int32 (F, 3) faces tensor in CSR form: (inc_ptr (V+1), inc (3F)),
+    int32 on the same device, entries 3 f + k in ascending order per vertex (stable sort).  Built on the host once per
+    faces tensor (one copy to the host) and cached for as long as that tensor lives."""
+    key = id(faces_i32)
+    hit = _INCIDENCE.get(key)
+    if hit is not None and hit[0]() is faces_i32 and hit[1] == faces_i32._version:
+        return hit[2]
+    flat = faces_i32.detach().reshape(-1).cpu().numpy().astype(np.int64)
+    V = int(flat.max()) + 1 if flat.size else 0
+    order = np.argsort(flat, kind='stable').astype(np.int32)
+    ptr_ = np.zeros(V + 1, np.int32)
+    np.cumsum(np.bincount(flat, minlength=V), out=ptr_[1:])
+    inc = (torch.from_numpy(ptr_).to(faces_i32.device), torch.from_numpy(order).to(faces_i32.device))
+    if hit is None or hit[0]() is not faces_i32:
+        weakref.finalize(faces_i32, _INCIDENCE.pop, key, None)
+    _INCIDENCE[key] = (weakref.ref(faces_i32), faces_i32._version, inc)
+    return inc
+
+
+def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, faces_i32=None, triangles=None):
+    """Gradient of `measure` (B, 5) with respect to v_shaped (B, V, 3) or triangles (B, F, 3, 3), with the reference's
+    autograd semantics (include/shapy_b200.h, shapy_measure_backward): the intersection barycentrics are constants and
+    the plane heights get no gradient.  Deterministic, one launch."""
+    g = _cuda_f32(grad_out, 'grad_out')
+    if triangles is not None:
+        x = _cuda_f32(triangles, 'triangles')
+        B, F = x.shape[0], x.shape[1]
+    else:
+        x = _cuda_f32(v_shaped, 'v_shaped')
+        B, V = x.shape[0], x.shape[1]
+        if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
+            raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
+        faces_i32 = faces_i32.contiguous()
+        F = faces_i32.shape[0]
+    if g.shape != (B, 5):
+        raise RuntimeError(f'grad_out must be ({B}, 5), got {tuple(g.shape)}')
+    grad = torch.empty_like(x)
+    if B == 0:
+        return grad
+    with torch.cuda.device(x.device):
+        if triangles is not None:
+            check(lib().shapy_measure_backward_tris(ptr(x), B, F, C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()),
+                  'measure_backward')
+        else:
+            inc_ptr, inc = face_incidence(faces_i32)
+            if inc_ptr.numel() - 1 > V:
+                raise RuntimeError(f'faces index vertex {inc_ptr.numel() - 2} of a mesh with {V} vertices')
+            if inc_ptr.numel() - 1 < V:     # trailing vertices no face uses: empty rows
+                inc_ptr = torch.cat([inc_ptr, inc_ptr[-1:].expand(V + 1 - inc_ptr.numel())])
+            check(lib().shapy_measure_backward(ptr(x), ptr(faces_i32), ptr(inc_ptr), ptr(inc), B, V, F,
+                                               C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()), 'measure_backward')
+    return grad
+
+
+def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
+    """grad_betas (B, NB) = shapedirs^T . grad_v_shaped (B, V, 3): the adjoint of smplx_forward_shape."""
+    g = _cuda_f32(grad_v_shaped, 'grad_v_shaped')
+    B = g.shape[0]
+    if g.shape != (B, model.V, 3):
+        raise RuntimeError(f'grad_v_shaped must be ({B}, {model.V}, 3), got {tuple(g.shape)}')
+    out = torch.empty(B, model.NB, dtype=torch.float32, device=g.device)
+    if B == 0:
+        return out
+    with torch.cuda.device(g.device):
+        nbytes = lib().shapy_smplx_backward_shape_workspace_bytes(model.handle, B)
+        ws = _WS.get('shape_bwd', nbytes, g.device)
+        check(lib().shapy_smplx_backward_shape(model.handle, ptr(g), B, ptr(out), ptr(ws), ws.numel(), stream_ptr()),
+              'smplx_backward_shape')
+    return out
+
+
 def mesh_to_mesh_forward(query_triangles, target_triangles, max_collisions=16, print_timings=False):
     """Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward (bind.cpp:59-64).
 

@@ -30,6 +30,9 @@ Everything written here is a small fixture that travels to the GPU box, where
   ref_mmi_{plane,soup}.npz        reference mesh_to_mesh_forward (oracle/_ref via oracle/run_ref_mmi.py) collisions on
                         the inputs of tests/test_gpu_zz_reference_op.py; GPU only: `python tools/make_golden.py mmi`
   ref_mmi_{plane,soup,quirk}_f64.npz   the same in float64 on the inputs of tests/test_mmi_f64_cpu.py (same recipe)
+  ref_measure_grad.npz  reference BodyMeasurements autograd gradients (its own body_measurements.py, loaded by oracle/ref_body_measurements.py with
+                        the C operator oracle) of each measurement with respect to v_shaped, on img_00 and the 3 extra
+                        bodies: dense rows for mass, (rows, values) for height and the circumferences
   preprocess.npz        reference input stage (transf_utils.crop with cv2 + ToTensor + Normalize) on seeded uint8 images:
                         crop windows, crops with OpenCV's portable path (IPP off) and with this container's IPP build
 """
@@ -479,9 +482,31 @@ def mmi_fixtures():
                             faces=f[keep].astype(np.int32), bcs=bcs[keep], query=query)
 
 
+def measure_grad_fixture():
+    from oracle import ref_body_measurements
+    BM, cfg = ref_body_measurements.load()
+    bm = BM(cfg)
+    g = np.load(os.path.join(G, 'img00_body.npz'))
+    bodies = np.concatenate([g['v_shaped'][None], g['extra_v_shaped']], 0).astype(np.float32)
+    f = torch.from_numpy(g['faces'].astype(np.int64))
+    out = {'mass': np.zeros(bodies.shape, np.float32)}
+    for b in range(bodies.shape[0]):
+        for i, name in enumerate(('mass', 'height', 'chest', 'waist', 'hips')):
+            v = torch.from_numpy(bodies[b])[None].clone().requires_grad_(True)
+            bm(v[:, f])['measurements'][name]['tensor'].sum().backward()
+            gr = v.grad[0].numpy()
+            if name == 'mass':
+                out['mass'][b] = gr
+            else:
+                rows = np.nonzero(np.abs(gr).sum(1))[0].astype(np.int32)
+                out[f'{name}_{b}_rows'], out[f'{name}_{b}_values'] = rows, gr[rows]
+    np.savez_compressed(os.path.join(G, 'ref_measure_grad.npz'), **out)
+    print('ref_measure_grad.npz', {k: v.shape for k, v in out.items() if k.endswith('rows')})
+
+
 if __name__ == '__main__':
     which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
-                             'smplx_full', 'camera', 'keypoint']
+                             'smplx_full', 'camera', 'keypoint', 'measure_grad']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -511,3 +536,5 @@ if __name__ == '__main__':
         keypoint_tensor_fixture()
     if 'mmi' in which:
         mmi_fixtures()
+    if 'measure_grad' in which:
+        measure_grad_fixture()
