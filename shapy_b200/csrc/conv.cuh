@@ -61,11 +61,17 @@ int launch_nhwc_merge(const ActView &in, float *y, bool to_nchw, cudaStream_t st
 // TMA + wgmma implicit-GEMM engine (conv_wgmma.cu).  `WgmmaPlan` holds the TMA descriptors + geometry of one launch.
 struct WgmmaPlan;
 // AUTO: the halo-resident path for the 3x3 stride-1 layers where it loads fewer bytes (unless SHAPY_CONV_HALO=0),
-// otherwise per-tap; PER_TAP / HALO force one (HALO fails on a layer it cannot run).
-enum WgmmaPath { WGMMA_AUTO = 0, WGMMA_PER_TAP = 1, WGMMA_HALO = 2 };
+// otherwise per-tap; PER_TAP / HALO force one (HALO fails on a layer it cannot run).  The consumer schedule is chosen
+// by the planner's cost model (cooperative everywhere with SHAPY_CONV_PINGPONG=0) unless COOP or PINGPONG is or-ed in
+// (PINGPONG then limits the cout tile to what its accumulators fit).
+enum WgmmaPath { WGMMA_AUTO = 0, WGMMA_PER_TAP = 1, WGMMA_HALO = 2, WGMMA_COOP = 4, WGMMA_PINGPONG = 8 };
 bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out);
 WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
-                             WgmmaPath path = WGMMA_AUTO);
+                             int path = WGMMA_AUTO);
+#ifdef SHAPY_CONV_STAMPS
+void wgmma_stamps_reset();
+void wgmma_stamps_print(const WgmmaPlan *p);
+#endif
 void wgmma_plan_destroy(WgmmaPlan *p);
 void wgmma_plan_stats(const WgmmaPlan *p, double *tma_bytes, double *mma_flops);   // per launch, as planned
 int wgmma_plan_launch(const WgmmaPlan *p, cudaStream_t st, bool pdl);   // pdl: programmatic dependent launch

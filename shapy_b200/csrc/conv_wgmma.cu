@@ -18,13 +18,21 @@
 //     not issued.
 //   * Both operands land in the canonical K-major SWIZZLE_128B layout the wgmma shared-memory descriptor names, so no
 //     thread touches operand data.
-//   * warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = consumers: each issues wgmma m64nNk16 for
-//     64 of the 128 tile rows into fp32 register accumulators, then runs the epilogue of its rows.  The shared-memory
-//     ring of `stages` slots (full / empty mbarriers) runs ahead across tile boundaries, so the loads of the next tile
-//     overlap the epilogue of this one; persistent, one CTA per SM.
+//   * warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = consumers.  The shared-memory ring of
+//     `stages` slots (full / empty mbarriers) runs ahead across tile boundaries; persistent, one CTA per SM.  Two
+//     consumer schedules:
+//       - cooperative: both consumers work on the same tile, each issuing wgmma m64nNk16 for 64 of its 128 rows, and
+//         both run the epilogue of their rows at the same time (the tensor cores idle meanwhile);
+//       - ping-pong: each consumer owns whole tiles (two m64 accumulator sets, all 128 rows) and the two alternate
+//         through the CTA's tile sequence.  A pair of hand-off mbarriers orders the mainloops: a consumer starts its
+//         tile's k-blocks only after the other has issued all of the previous tile's, so one consumer's epilogue runs
+//         under the other's MMAs, and the ring positions each consumer waits on are at most one phase ahead.
+//     Both give every output row the same wgmma sequence and the same epilogue arithmetic.
 // Split-fp16 parity mode keeps activations and weights as fp16 hi + fp16 lo (x = hi + lo/2048) and issues
 // A_hi.[B_hi|B_lo] as ONE N = 2 NT wgmma into [D0|D1] plus A_lo.B_hi into D1' (out = D0 + (D1 + D1')/2048).
-// Epilogue: registers -> +bias (+residual) -> ReLU -> split to fp16 hi/lo -> global stores.
+// Epilogue: registers -> +bias (+residual) -> ReLU -> split to fp16 hi/lo -> global stores (cooperative), or -> the
+// consumer's shared-memory staging box, into which TMA loaded the residual during the mainloop, -> one TMA tensor store
+// per plane (ping-pong).
 // Replaces cuDNN conv + BatchNorm + ReLU + residual add (4 launches, 4 HBM round trips) of
 // regressor/human_shape/models/backbone/hrnet.py and torchvision BasicBlock / Bottleneck.
 #include <cmath>
@@ -62,29 +70,58 @@ struct alignas(64) WgmmaParams {
   int out_ctot, out_coff;
   const __half *res_hi, *res_lo;
   int res_ctot, res_coff;
+  // ping-pong epilogue: output / residual maps over the [N][Ho][Wo] x cout view (box NT x o_bw x TH x TN, the padded
+  // grid's junk columns excluded), and the shared-memory staging box of each consumer
+  CUtensorMap o_hi, o_lo, r_hi, r_lo;
+  int o_bw;                      // box width: Wo on the halo path, TW on the per-tap path
+  uint32_t o_plane;              // smem pitch of one staged plane (hi or lo)
+  uint32_t o_bytes;              // TMA bytes of one plane's box
 };
 
 constexpr int kThreads = 384;                // producer warpgroup + two consumer warpgroups
 constexpr int kProdRegs = 40, kConsRegs = 232;
 
-template <bool SPLIT, int NT, bool HALO>
+#ifdef SHAPY_CONV_STAMPS
+// Cycle-stamp build (tools/conv_phase_stamps.py): per consumer warpgroup and tile, clock64 at the first full-barrier
+// pass, the last commit, the return of wait<0> and the end of the epilogue, summed over all tiles of a launch as
+// [wait before the first k-block, mainloop, drain, epilogue, tiles].
+__device__ unsigned long long g_conv_stamps[5];
+#endif
+
+// fp32 accumulators per thread of one m64 set: [D0 | D1] of a 64 x NT(x2) tile, and A_lo . B_hi kept apart (wgmma
+// pipelines only disjoint or equal D)
+template <bool SPLIT, int NT>
+constexpr int cons_accs() { return (SPLIT ? 2 * NT : NT) / 2 + (SPLIT ? NT / 2 : 0); }
+
+template <bool SPLIT, int NT, bool HALO, bool PP>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_constant__ WgmmaParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int NACC = (SPLIT ? 2 * NT : NT) / 2;   // fp32 accumulators per thread: [D0 | D1] of a 64 x NT(x2) tile
   constexpr int NLO = SPLIT ? NT / 2 : 1;           // A_lo . B_hi, kept apart: wgmma pipelines only disjoint or equal D
   constexpr int PARTS = SPLIT ? 2 : 1;
+  constexpr int MT = PP ? 2 : 1;                    // m64 accumulator sets per consumer: ping-pong owns all 128 rows
+  constexpr int CONS = PP ? 1 : 2;                  // consumers that release each ring slot
+  static_assert(!PP || MT * cons_accs<SPLIT, NT>() <= 192, "ping-pong accumulators must fit the consumer registers");
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t A_BLK = 128 * KCH * 2;
-  // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B] [mbarriers]
+  // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B]
+  //                [ping-pong: output staging box of consumer 0, of consumer 1] [mbarriers]
   const uint32_t h_stage = p.h_plane * PARTS;
   const uint32_t ring_base = smem_base + (HALO ? h_stage * p.hstages : 0u);
   const uint32_t kblk_bytes = (HALO ? 0u : A_BLK * PARTS) + p.b_stride;   // one stage = one k-block of one tap
-  const uint32_t bar_base = ring_base + kblk_bytes * p.stages;
+  const uint32_t o_base = ring_base + kblk_bytes * p.stages;
+  const uint32_t bar_base = o_base + (PP ? 2u * p.o_plane * PARTS : 0u);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
   auto hfull_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
   auto hempty_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + p.hstages + s); };
-  const int wg = threadIdx.x >> 7;
+  // ping-pong: consumer c arrives on handoff_bar(c) once it has issued every k-block of its tile
+  auto handoff_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + c); };
+  // ping-pong: the residual box of consumer c's tile has landed in its staging box
+  auto res_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + 2 + c); };
+  // broadcast so ptxas sees a warp-uniform value: the ping-pong hand-off wait depends on it, and a wait it takes for
+  // divergent makes it serialise every wgmma of the kernel
+  const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);
   const int n_tiles = p.cout / NT;
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * n_tiles;
   const int taps = p.ksize * p.ksize;
@@ -95,8 +132,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
-    for (int s = 0; s < (HALO ? p.hstages : 0); ++s) { mbar_init(hfull_bar(s), 1); mbar_init(hempty_bar(s), 2); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS); }
+    for (int s = 0; s < (HALO ? p.hstages : 0); ++s) { mbar_init(hfull_bar(s), 1); mbar_init(hempty_bar(s), CONS); }
+    if (PP) for (int c = 0; c < 2; ++c) { mbar_init(handoff_bar(c), 1); mbar_init(res_bar(c), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -163,18 +201,46 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   } else {
     // ===================================================================== consumers: MMA + epilogue
     setmaxnreg_inc<kConsRegs>();
-    const int cw = wg - 1;                        // rows 64 cw .. 64 cw + 63 of the tile
+    const int cw = wg - 1;                        // cooperative: rows 64 cw .. 64 cw + 63 of every tile; ping-pong: the
+                                                  // CTA's tiles cw, cw + 2, ...
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     int s = 0, hs = 0;
-    uint32_t ph = 0, hph = 0;
-    float acc[NACC], acl[NLO];
-    for (int id = blockIdx.x; id < total_tiles; id += gridDim.x) {
+    uint32_t ph = 0, hph = 0, hoph = 0, rph = 0;
+    // ping-pong: this consumer's output staging box (hi plane, then lo), and the same bytes as a generic pointer
+    const uint32_t ob = o_base + (uint32_t)cw * p.o_plane * PARTS;
+    uint8_t *const ob_ptr = smem_raw + (ob - smem_u32(smem_raw));
+    // ping-pong: step the ring positions over the k-blocks (and halo loads) of the other consumer's tile
+    auto skip_tile = [&]() {
+      const int q = s + iters, hq = hs + p.kpt;
+      ph ^= (uint32_t)(q / p.stages) & 1u; s = q % p.stages;
+      if (HALO) { hph ^= (uint32_t)(hq / p.hstages) & 1u; hs = hq % p.hstages; }
+    };
+    if (PP && cw == 1) skip_tile();
+    float acc[MT][NACC], acl[MT][NLO];
+#ifdef SHAPY_CONV_STAMPS
+    long long st_end = clock64(), st0 = 0, st1 = 0, st2 = 0;
+#endif
+    for (int id = blockIdx.x + (PP ? cw : 0) * gridDim.x, k = 0; id < total_tiles; id += (PP ? 2 : 1) * gridDim.x, ++k) {
       int w0, h0, n0, c_out0;
       tile_coords(id, w0, h0, n0, c_out0);
+      if (PP && (k > 0 || cw == 1)) {             // the other consumer has issued the CTA's previous tile
+        mbar_wait(handoff_bar(cw ^ 1), hoph);
+        hoph ^= 1;
+      }
+      if (PP && p.res_hi && t == 0) {             // the residual box loads under the mainloop
+        bulk_wait_read();                         // once the previous tile's output has left the staging box
+        mbar_expect_tx(res_bar(cw), p.o_bytes * ((SPLIT && p.res_lo) ? 2u : 1u));
+        tma_load_4d(ob, &p.r_hi, res_bar(cw), c_out0, w0, h0, n0);
+        if (SPLIT && p.res_lo) tma_load_4d(ob + p.o_plane, &p.r_lo, res_bar(cw), c_out0, w0, h0, n0);
+      }
 #pragma unroll
-      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+      for (int m = 0; m < MT; ++m) {
 #pragma unroll
-      for (int i = 0; i < NLO; ++i) acl[i] = 0.f;
+        for (int i = 0; i < NACC; ++i) acc[m][i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < NLO; ++i) acl[m][i] = 0.f;
+      }
+      const uint32_t row0 = PP ? 0u : (uint32_t)cw * 64;   // first tile row of accumulator set 0
       int prev = -1, prev_h = -1;                 // stages the last committed wgmma group reads (prev_h: halo, if its last)
 #pragma unroll 1
       for (int it = 0; it < iters; ++it) {
@@ -185,30 +251,43 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
         if (HALO) {
           if (tap == 0) mbar_wait(hfull_bar(hs), hph);
           // tap (ky, kx): the halo rows from ky * Wp + kx on (p.TW is the pitch Wp of the padded grid)
-          a_addr = smem_base + h_stage * hs + (uint32_t)(cw * 64 + (tap / 3) * p.TW + tap % 3) * (KCH * 2);
+          a_addr = smem_base + h_stage * hs + (row0 + (uint32_t)((tap / 3) * p.TW + tap % 3)) * (KCH * 2);
           a_lo_off = p.h_plane;
         }
         mbar_wait(full_bar(s), ph);
+#ifdef SHAPY_CONV_STAMPS
+        if (it == 0) st0 = clock64();
+#endif
         const uint32_t kb = ring_base + kblk_bytes * s;
-        if (!HALO) { a_addr = kb + cw * 64 * KCH * 2; a_lo_off = A_BLK; }
-        const uint64_t a = wgmma_desc<KCH>(a_addr);
-        const uint64_t al = wgmma_desc<KCH>(a_addr + a_lo_off);
+        if (!HALO) { a_addr = kb + row0 * KCH * 2; a_lo_off = A_BLK; }
+        uint64_t a[MT], al[MT];
+#pragma unroll
+        for (int m = 0; m < MT; ++m) {            // set m: tile rows row0 + 64 m on
+          a[m] = wgmma_desc<KCH>(a_addr + m * 64 * KCH * 2);
+          al[m] = wgmma_desc<KCH>(a_addr + m * 64 * KCH * 2 + a_lo_off);
+        }
         const uint64_t b = wgmma_desc<KCH>(kb + (HALO ? 0u : A_BLK * PARTS));
 #pragma unroll
-        for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+        for (int m = 0; m < MT; ++m) {
 #pragma unroll
-        for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
+          for (int i = 0; i < NACC; ++i) reg_fence(acc[m][i]);
+#pragma unroll
+          for (int i = 0; i < NLO; ++i) reg_fence(acl[m][i]);
+        }
         wgmma_fence();
         // the first nks k16 steps (channels past cin are zero-filled, nothing to add): one straight-line wgmma run and
         // its commit per count, so no branch joins inside a group (a join there makes ptxas add a dummy wgmma)
         auto issue = [&](auto nks_c) {
 #pragma unroll
           for (int ks = 0; ks < decltype(nks_c)::value; ++ks) {   // +32 bytes along K = +2 descriptor units
-            if (SPLIT) {
-              wgmma_f16<2 * NT>(acc, a + 2 * ks, b + 2 * ks, 1);   // [D0 | D1] += A_hi . [B_hi | B_lo]^T
-              wgmma_f16<NT>(acl, al + 2 * ks, b + 2 * ks, 1);       // D1' += A_lo . B_hi^T
-            } else {
-              wgmma_f16<NT>(acc, a + 2 * ks, b + 2 * ks, 1);
+#pragma unroll
+            for (int m = 0; m < MT; ++m) {
+              if (SPLIT) {
+                wgmma_f16<2 * NT>(acc[m], a[m] + 2 * ks, b + 2 * ks, 1);   // [D0 | D1] += A_hi . [B_hi | B_lo]^T
+                wgmma_f16<NT>(acl[m], al[m] + 2 * ks, b + 2 * ks, 1);       // D1' += A_lo . B_hi^T
+              } else {
+                wgmma_f16<NT>(acc[m], a[m] + 2 * ks, b + 2 * ks, 1);
+              }
             }
           }
           wgmma_commit();
@@ -221,9 +300,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
           default: issue(std::integral_constant<int, 4>()); break;
         }
 #pragma unroll
-        for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+        for (int m = 0; m < MT; ++m) {
 #pragma unroll
-        for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
+          for (int i = 0; i < NACC; ++i) reg_fence(acc[m][i]);
+#pragma unroll
+          for (int i = 0; i < NLO; ++i) reg_fence(acl[m][i]);
+        }
         wgmma_wait<1>();                          // the previous stage's wgmmas have read their operands
         if (prev >= 0 && t == 0) {
           mbar_arrive(empty_bar(prev));
@@ -237,55 +319,109 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
         }
         if (++s == p.stages) { s = 0; ph ^= 1; }
       }
+      if (PP && t == 0) mbar_arrive(handoff_bar(cw));
+#ifdef SHAPY_CONV_STAMPS
+      st1 = clock64();
+#endif
       wgmma_wait<0>();
 #pragma unroll
-      for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+      for (int m = 0; m < MT; ++m) {
 #pragma unroll
-      for (int i = 0; i < NLO; ++i) reg_fence(acl[i]);
+        for (int i = 0; i < NACC; ++i) reg_fence(acc[m][i]);
+#pragma unroll
+        for (int i = 0; i < NLO; ++i) reg_fence(acl[m][i]);
+      }
       if (prev >= 0 && t == 0) {
         mbar_arrive(empty_bar(prev));
         if (prev_h >= 0) mbar_arrive(hempty_bar(prev_h));
       }
+      if (PP) skip_tile();
+#ifdef SHAPY_CONV_STAMPS
+      st2 = clock64();
+#endif
 
-      // ---- epilogue: this thread holds rows r0 and r0 + 8, two adjacent columns of every 8-column group
-      const int q4 = lane & 3;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * half;
-        const int dw = row % p.TW, dh = (row / p.TW) % p.TH, dn = row / (p.TW * p.TH);
-        const int ow = w0 + dw, oh = h0 + dh, on = n0 + dn;
-        if (!(dn < p.TN && ow < p.Wo && oh < p.Ho && on < p.N)) continue;
-        const size_t pix = ((size_t)on * p.Ho + oh) * p.Wo + ow;
-        const size_t oo = pix * p.out_ctot + p.out_coff + c_out0;
-        const size_t ro = pix * p.res_ctot + p.res_coff + c_out0;
-#pragma unroll
-        for (int j = 0; j < NT / 8; ++j) {
-          const int c = 8 * j + 2 * q4;
-          const int i = 4 * j + 2 * half;
-          const float2 bq = __ldg(reinterpret_cast<const float2 *>(p.bias + c_out0 + c));
-          float r0 = acc[i], r1 = acc[i + 1];
-          if (SPLIT) {
-            r0 += (acc[NT / 2 + i] + acl[SPLIT ? i : 0]) * kLoInv;
-            r1 += (acc[NT / 2 + i + 1] + acl[SPLIT ? i + 1 : 0]) * kLoInv;
-          }
-          r0 += bq.x; r1 += bq.y;
-          if (p.res_hi) {
-            const __half2 rh = *reinterpret_cast<const __half2 *>(p.res_hi + ro + c);
-            r0 += __low2float(rh); r1 += __high2float(rh);
-            if (SPLIT && p.res_lo) {
-              const __half2 rl = *reinterpret_cast<const __half2 *>(p.res_lo + ro + c);
-              r0 += __low2float(rl) * kLoInv; r1 += __high2float(rl) * kLoInv;
-            }
-          }
-          if (p.relu) { r0 = fmaxf(r0, 0.f); r1 = fmaxf(r1, 0.f); }
-          __half h0_, h1_, l0_, l1_;
-          split_store(r0, h0_, l0_);
-          split_store(r1, h1_, l1_);
-          *reinterpret_cast<__half2 *>(p.out_hi + oo + c) = __halves2half2(h0_, h1_);
-          if (SPLIT && p.out_lo) *reinterpret_cast<__half2 *>(p.out_lo + oo + c) = __halves2half2(l0_, l1_);
+      // ---- epilogue: this thread holds rows r0 and r0 + 8 of each m64 set, two adjacent columns of every 8-column group.
+      // Ping-pong stages the outputs in shared memory (over the residual, each element read and written by the same
+      // thread) and stores the box with one TMA store per plane; cooperative stores straight to global memory.
+      if (PP) {
+        if (p.res_hi) {
+          mbar_wait(res_bar(cw), rph);
+          rph ^= 1;
+        } else {
+          if (t == 0) bulk_wait_read();
+          named_bar_sync(1 + cw, 128);
         }
       }
+      const int q4 = lane & 3;
+#pragma unroll
+      for (int m = 0; m < MT; ++m) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int row = (int)row0 + m * 64 + warp * 16 + (lane >> 2) + 8 * half;
+          const int dw = row % p.TW, dh = (row / p.TW) % p.TH, dn = row / (p.TW * p.TH);
+          const int ow = w0 + dw, oh = h0 + dh, on = n0 + dn;
+          if (!(dn < p.TN && ow < p.Wo && oh < p.Ho && on < p.N)) continue;
+          const size_t pix = ((size_t)on * p.Ho + oh) * p.Wo + ow;
+          const size_t oo = pix * p.out_ctot + p.out_coff + c_out0;
+          const size_t ro = pix * p.res_ctot + p.res_coff + c_out0;
+          const uint32_t so = (uint32_t)((dn * p.TH + dh) * p.o_bw + dw) * NT;   // element of the staging box
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j) {
+            const int c = 8 * j + 2 * q4;
+            const int i = 4 * j + 2 * half;
+            const float2 bq = __ldg(reinterpret_cast<const float2 *>(p.bias + c_out0 + c));
+            float r0 = acc[m][i], r1 = acc[m][i + 1];
+            if (SPLIT) {
+              r0 += (acc[m][NT / 2 + i] + acl[m][SPLIT ? i : 0]) * kLoInv;
+              r1 += (acc[m][NT / 2 + i + 1] + acl[m][SPLIT ? i + 1 : 0]) * kLoInv;
+            }
+            r0 += bq.x; r1 += bq.y;
+            __half2 *const sh = reinterpret_cast<__half2 *>(ob_ptr + 2u * (so + c));
+            __half2 *const sl = reinterpret_cast<__half2 *>(ob_ptr + p.o_plane + 2u * (so + c));
+            if (p.res_hi) {
+              const __half2 rh = PP ? *sh : *reinterpret_cast<const __half2 *>(p.res_hi + ro + c);
+              r0 += __low2float(rh); r1 += __high2float(rh);
+              if (SPLIT && p.res_lo) {
+                const __half2 rl = PP ? *sl : *reinterpret_cast<const __half2 *>(p.res_lo + ro + c);
+                r0 += __low2float(rl) * kLoInv; r1 += __high2float(rl) * kLoInv;
+              }
+            }
+            if (p.relu) { r0 = fmaxf(r0, 0.f); r1 = fmaxf(r1, 0.f); }
+            __half h0_, h1_, l0_, l1_;
+            split_store(r0, h0_, l0_);
+            split_store(r1, h1_, l1_);
+            if (PP) {
+              *sh = __halves2half2(h0_, h1_);
+              if (SPLIT && p.out_lo) *sl = __halves2half2(l0_, l1_);
+            } else {
+              *reinterpret_cast<__half2 *>(p.out_hi + oo + c) = __halves2half2(h0_, h1_);
+              if (SPLIT && p.out_lo) *reinterpret_cast<__half2 *>(p.out_lo + oo + c) = __halves2half2(l0_, l1_);
+            }
+          }
+        }
+      }
+      if (PP) {                                   // the staged box -> global memory; TMA drops rows past the map
+        fence_proxy_async_smem();
+        named_bar_sync(1 + cw, 128);
+        if (t == 0) {
+          tma_store_4d(&p.o_hi, ob, c_out0, w0, h0, n0);
+          if (SPLIT && p.out_lo) tma_store_4d(&p.o_lo, ob + p.o_plane, c_out0, w0, h0, n0);
+          bulk_commit();
+        }
+      }
+#ifdef SHAPY_CONV_STAMPS
+      if (t == 0) {                               // warp 0's end of the epilogue
+        const long long st3 = clock64();
+        atomicAdd(&g_conv_stamps[0], (unsigned long long)(st0 - st_end));
+        atomicAdd(&g_conv_stamps[1], (unsigned long long)(st1 - st0));
+        atomicAdd(&g_conv_stamps[2], (unsigned long long)(st2 - st1));
+        atomicAdd(&g_conv_stamps[3], (unsigned long long)(st3 - st2));
+        atomicAdd(&g_conv_stamps[4], 1ull);
+        st_end = st3;
+      }
+#endif
     }
+    if (PP && t == 0) bulk_wait();                // the last stores have completed before shared memory is released
   }
 }
 
@@ -309,7 +445,7 @@ static int sm_count() {
 struct WgmmaPlan {
   WgmmaParams p;
   int NT;
-  bool split, halo;
+  bool split, halo, pingpong;
   dim3 grid;
   size_t smem;
   double tma_bytes, mma_flops;   // per launch, as planned: TMA loads of both operands, tensor-core FLOPs issued
@@ -320,6 +456,30 @@ static bool halo_enabled() {
   static const bool v = []() { const char *e = getenv("SHAPY_CONV_HALO"); return !(e && e[0] == '0'); }();
   return v;
 }
+
+// SHAPY_CONV_PINGPONG=0: every plan without a forced schedule takes the cooperative one
+static bool pingpong_enabled() {
+  static const bool v = []() { const char *e = getenv("SHAPY_CONV_PINGPONG"); return !(e && e[0] == '0'); }();
+  return v;
+}
+
+// the ping-pong schedule holds two m64 accumulator sets per consumer thread
+static bool pingpong_fits(bool split, int nt) { return split ? nt <= 64 : nt <= 128; }
+
+#ifdef SHAPY_CONV_STAMPS
+void wgmma_stamps_reset() {
+  const unsigned long long z[5] = {0, 0, 0, 0, 0};
+  cudaMemcpyToSymbol(g_conv_stamps, z, sizeof(z));
+}
+void wgmma_stamps_print(const WgmmaPlan *pl) {
+  unsigned long long v[5];
+  cudaDeviceSynchronize();
+  cudaMemcpyFromSymbol(v, g_conv_stamps, sizeof(v));
+  const double n = v[4] ? (double)v[4] : 1.0;
+  fprintf(stderr, "[stamps] %s NT %d: %llu warpgroup-tiles, cycles per tile: wait %.0f mainloop %.0f drain %.0f epilogue %.0f\n",
+          pl->pingpong ? "ping-pong" : "cooperative", pl->NT, v[4], v[0] / n, v[1] / n, v[2] / n, v[3] / n);
+}
+#endif
 
 void wgmma_plan_stats(const WgmmaPlan *pl, double *tma_bytes, double *mma_flops) {
   *tma_bytes = pl->tma_bytes;
@@ -338,11 +498,13 @@ bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out) {
 }
 
 WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
-                             WgmmaPath path) {
+                             int path) {
   if (!wgmma_supported(w, in, out)) {
     set_error("wgmma_plan_create: unsupported convolution (cin %d cout %d k %d s %d)", w.cin, w.cout, w.ksize, w.stride);
     return nullptr;
   }
+  const int data_path = path & (WGMMA_PER_TAP | WGMMA_HALO);
+  const int sched = path & (WGMMA_COOP | WGMMA_PINGPONG);
   auto *pl = new WgmmaPlan();
   memset(&pl->p, 0, sizeof(pl->p));
   WgmmaParams &p = pl->p;
@@ -378,13 +540,13 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       const double pt_a = pt_tiles * 9 * p.TW * p.TH * p.TN, h_a = h_tiles * Wp * (th + 2);   // rows loaded per k-block
       better = p.TN == 1 && h_tiles <= pt_tiles && h_a < pt_a;
     }
-    if (path == WGMMA_HALO && !possible) {
+    if (data_path == WGMMA_HALO && !possible) {
       set_error("wgmma_plan_create: no halo path for cin %d cout %d k %d s %d %dx%d", w.cin, w.cout, w.ksize, w.stride,
                 out.H, out.W);
       delete pl;
       return nullptr;
     }
-    pl->halo = path == WGMMA_HALO || (path == WGMMA_AUTO && better && halo_enabled());
+    pl->halo = data_path == WGMMA_HALO || (data_path == WGMMA_AUTO && better && halo_enabled());
     if (pl->halo) {
       p.TW = Wp; p.TH = th; p.TN = 1;
       p.tiles_w = 1; p.tiles_h = ceil_div(out.H, th); p.tiles_n = out.N;
@@ -396,16 +558,35 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     // tensor cycles, plus a fixed per-tile epilogue / barrier cost.
     const double m_tiles = (double)p.tiles_w * p.tiles_h * p.tiles_n;
     auto mma_cyc = [](double n) { return 2.0 * std::max((2048.0 + 32.0 * n) / 128.0, n * 0.5); };
+    auto main_cyc = [&](int nt) {
+      return (split ? mma_cyc(2.0 * nt) + mma_cyc(nt) : mma_cyc(nt)) * w.ksize * w.ksize * p.kpt * (KCH / 16);
+    };
+    auto rounds = [&](int nt) { return std::ceil(m_tiles * (w.cout / nt) / sms); };
     double best = 1e30;
     int best_nt = 0;
     for (int nt : kNts) {
       if (w.cout % nt || (split && nt > 96)) continue;   // split: 3 NT / 2 accumulators per thread must fit 232 registers
-      const double per_k = split ? mma_cyc(2.0 * nt) + mma_cyc(nt) : mma_cyc(nt);
-      const double cost = std::ceil(m_tiles * (w.cout / nt) / sms) *
-                          (per_k * w.ksize * w.ksize * p.kpt * (KCH / 16) + 400.0 * nt / 16);
+      const double cost = rounds(nt) * (main_cyc(nt) + 400.0 * nt / 16);
       if (cost < best) { best = cost; best_nt = nt; }
     }
-    pl->NT = best_nt;
+    // Schedule, from the cycle stamps of tools/conv_phase_stamps.py (H100 SXM, README): the per-tile cost outside the
+    // mainloop (epilogue, drain, refill) is ~100 cycles per cout in split mode and ~72 in fp16; one consumer issuing
+    // both m64 halves takes 1.25-1.6x (split) / 1.0-1.1x (fp16) the mainloop time of two consumers issuing one each.  The
+    // cooperative schedule pays mainloop + epilogue per tile, the ping-pong one the larger of the two (the epilogue
+    // runs under the other consumer's mainloop) and one exposed epilogue at the end.  The planner only weighs ping-pong
+    // at the cooperative cout tile: smaller tiles re-load the activations per cout tile and measured slower.
+    const double epi_c = split ? 100.0 : 72.0, pp_slow = split ? 1.3 : 1.1;
+    auto pp_cost = [&](int nt) { return rounds(nt) * std::max(pp_slow * main_cyc(nt), epi_c * nt) + epi_c * nt; };
+    if (sched == WGMMA_PINGPONG) {               // forced: the cheapest cout tile whose accumulators fit
+      double c = 1e30;
+      for (int nt : kNts)
+        if (w.cout % nt == 0 && pingpong_fits(split, nt) && pp_cost(nt) < c) { c = pp_cost(nt); pl->NT = nt; }
+      pl->pingpong = true;
+    } else {
+      pl->NT = best_nt;
+      pl->pingpong = sched == 0 && pingpong_enabled() && pingpong_fits(split, best_nt) &&
+                     pp_cost(best_nt) < rounds(best_nt) * (main_cyc(best_nt) + epi_c * best_nt);
+    }
   }
   p.relu = relu;
   p.pdl_late = 1;
@@ -414,17 +595,40 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   p.a_bytes = (uint32_t)a_rows * KCH * 2;
   p.b_bytes = (uint32_t)pl->NT * KCH * 2;
   p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * PARTS, 1024);
-  // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory
-  if (pl->halo) {
-    p.h_plane = h_plane;
-    p.hstages = 2;
-    const size_t halo = (size_t)h_plane * PARTS * p.hstages;
-    p.stages = (int)std::min<size_t>(8, (216 * 1024 - halo) / p.b_stride);
-    pl->smem = halo + (size_t)p.b_stride * p.stages + 16 * (p.stages + p.hstages) + 1024;
-  } else {
-    const size_t stage = 128u * KCH * 2 * PARTS + p.b_stride;
-    p.stages = (int)std::max<size_t>(2, std::min<size_t>(8, (216 * 1024) / stage));
-    pl->smem = stage * p.stages + 16 * p.stages + 1024;
+  // ping-pong output staging: one box per consumer and plane (the output tile without the padded grid's junk columns)
+  p.o_bw = pl->halo ? out.W : p.TW;
+  p.o_bytes = (uint32_t)pl->NT * p.o_bw * p.TH * p.TN * 2;
+  p.o_plane = (uint32_t)align_up((size_t)p.o_bytes, 1024);
+  // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory; ping-pong takes its two staging boxes
+  // out of the weight ring and may use up to 222 KB
+  auto plan_smem = [&]() {
+    const size_t staging = pl->pingpong ? 2 * (size_t)p.o_plane * PARTS : 0;
+    const size_t budget = (pl->pingpong ? 222 : 216) * 1024 - staging;
+    if (pl->halo) {
+      p.h_plane = h_plane;
+      p.hstages = 2;
+      const size_t halo = (size_t)h_plane * PARTS * p.hstages;
+      p.stages = halo + 2 * p.b_stride <= budget ? (int)std::min<size_t>(8, (budget - halo) / p.b_stride) : 0;
+      pl->smem = halo + staging + (size_t)p.b_stride * p.stages + 16 * (p.stages + p.hstages + 2) + 1024;
+    } else {
+      const size_t stage = 128u * KCH * 2 * PARTS + p.b_stride;
+      p.stages = (int)std::min<size_t>(8, budget / stage);
+      if (!pl->pingpong) p.stages = std::max(2, p.stages);
+      pl->smem = staging + stage * p.stages + 16 * (p.stages + 2) + 1024;
+    }
+    // a planned ping-pong needs three weight slots: with two, the ring stalls the mainloop (split b64, NT 64: 111.8
+    // against 103.9 us cooperative)
+    return p.stages >= (pl->pingpong && sched != WGMMA_PINGPONG ? 3 : 2);
+  };
+  if (!plan_smem()) {
+    if (sched == WGMMA_PINGPONG) {
+      set_error("wgmma_plan_create: no room for the ping-pong staging boxes (cin %d cout %d %dx%d)", w.cin, w.cout,
+                out.H, out.W);
+      delete pl;
+      return nullptr;
+    }
+    pl->pingpong = false;                         // the planner's choice is always at the cooperative cout tile
+    plan_smem();
   }
   p.bias = w.bias;
   p.out_hi = out.hi; p.out_lo = out.lo; p.out_ctot = out.Ctot; p.out_coff = out.coff;
@@ -441,10 +645,11 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   }
   if (getenv("SHAPY_CONV_DEBUG"))
     fprintf(stderr,
-            "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: %s NT %d tile %dx%dx%d grid %d stages %d+%d, TMA %.1f MB, "
-            "MMA %.2f GFLOP\n",
-            w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N, pl->halo ? "halo" : "per-tap", pl->NT, p.TW, p.TH,
-            p.TN, pl->grid.x, p.hstages, p.stages, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
+            "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: %s %s NT %d tile %dx%dx%d grid %d stages %d+%d, staging "
+            "2x%ux%u B, smem %zu B, TMA %.1f MB, MMA %.2f GFLOP\n",
+            w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N, pl->halo ? "halo" : "per-tap",
+            pl->pingpong ? "ping-pong" : "cooperative", pl->NT, p.TW, p.TH, p.TN, pl->grid.x, p.hstages, p.stages,
+            pl->pingpong ? (unsigned)PARTS : 0u, p.o_plane, pl->smem, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
   bool ok = true;
   // activation maps
   const int nmaps = w.stride == 2 ? 4 : 1;
@@ -475,16 +680,28 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     ok = ok && encode(&p.b_hi, w.w_hi, 3, dims, strides, box, KCH);
     if (split) ok = ok && encode(&p.b_lo, w.w_lo, 3, dims, strides, box, KCH);
   }
+  // ping-pong epilogue maps: the output view (out_coff / out_ctot as the activation maps carry coff / Ctot) and the
+  // residual view, in boxes of the staged tile; no swizzle (the epilogue addresses the box row-major)
+  auto view_map = [&](CUtensorMap *m, const __half *base, const ActView &v) {
+    cuuint64_t dims[4] = {(cuuint64_t)w.cout, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N};
+    cuuint64_t strides[3] = {(cuuint64_t)v.Ctot * 2, (cuuint64_t)v.W * v.Ctot * 2, (cuuint64_t)v.H * v.W * v.Ctot * 2};
+    cuuint32_t box[4] = {(cuuint32_t)pl->NT, (cuuint32_t)p.o_bw, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
+    return encode(m, base + v.coff, 4, dims, strides, box, 0);
+  };
+  if (ok && pl->pingpong) {
+    ok = view_map(&p.o_hi, out.hi, out) && (!out.lo || view_map(&p.o_lo, out.lo, out));
+    if (ok && res) ok = view_map(&p.r_hi, res->hi, *res) && (!split || !res->lo || view_map(&p.r_lo, res->lo, *res));
+  }
   if (!ok) { delete pl; return nullptr; }
   return pl;
 }
 
 void wgmma_plan_destroy(WgmmaPlan *p) { delete p; }
 
-template <bool SPLIT, int NT, bool HALO>
+template <bool SPLIT, int NT, bool HALO, bool PP>
 static int launch_h(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
   static std::atomic<unsigned long long> attr_done{0};
-  auto kernel = conv_wgmma_kernel<SPLIT, NT, HALO>;
+  auto kernel = conv_wgmma_kernel<SPLIT, NT, HALO, PP>;
   SHAPY_CUDA_TRY(set_max_dynamic_smem(kernel, 227 * 1024, attr_done));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -502,9 +719,17 @@ static int launch_h(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
   return SHAPY_OK;
 }
 
+template <bool SPLIT, int NT, bool PP>
+static int launch_s(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
+  return pl->halo ? launch_h<SPLIT, NT, true, PP>(pl, st, pdl) : launch_h<SPLIT, NT, false, PP>(pl, st, pdl);
+}
+
 template <bool SPLIT, int NT>
 static int launch_t(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
-  return pl->halo ? launch_h<SPLIT, NT, true>(pl, st, pdl) : launch_h<SPLIT, NT, false>(pl, st, pdl);
+  if (!pl->pingpong) return launch_s<SPLIT, NT, false>(pl, st, pdl);
+  if constexpr (SPLIT ? NT <= 64 : NT <= 128) return launch_s<SPLIT, NT, true>(pl, st, pdl);   // pingpong_fits
+  set_error("wgmma engine: no ping-pong kernel for NT %d in split mode", NT);
+  return SHAPY_ERR_STATE;
 }
 
 template <bool SPLIT>

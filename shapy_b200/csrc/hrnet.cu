@@ -528,11 +528,18 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
   if (engine != 1) {
-    const WgmmaPath path = engine == 2 ? WGMMA_PER_TAP : (engine == 3 ? WGMMA_HALO : WGMMA_AUTO);
+    // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo; engine / 10: 0 = the planner's
+    // schedule, 1 = cooperative, 2 = ping-pong
+    const int e_path = engine % 10, e_sched = engine / 10;
+    const int path = (e_path == 2 ? WGMMA_PER_TAP : (e_path == 3 ? WGMMA_HALO : WGMMA_AUTO)) |
+                     (e_sched == 1 ? WGMMA_COOP : (e_sched == 2 ? WGMMA_PINGPONG : 0));
     plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }
     rc = wgmma_plan_launch(plan, st, true);
     if (const char *reps_s = getenv("SHAPY_CONV_TEST_REPS")) {
+#ifdef SHAPY_CONV_STAMPS
+      wgmma_stamps_reset();
+#endif
       // timing aid for kernel work: re-launch the same plan and report the average launch time
       const int reps = atoi(reps_s);
       cudaEvent_t e0, e1;
@@ -552,6 +559,9 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
               "TMA %.0f MB = %.2f TB/s, MMA issued %.1f GFLOP = %.0f TFLOP/s\n",
               conv->cin, conv->cout, conv->ksize, conv->stride, H, W, B, mode, sec * 1e6, fl / sec * 1e-12, mode ? 3 : 1,
               tma * 1e-6, tma / sec * 1e-12, mma * 1e-9, mma / sec * 1e-12);
+#ifdef SHAPY_CONV_STAMPS
+      wgmma_stamps_print(plan);
+#endif
       cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
   } else {
