@@ -63,8 +63,11 @@ struct WgmmaPlan;
 // AUTO: the halo-resident path for the 3x3 stride-1 layers where it loads fewer bytes (unless SHAPY_CONV_HALO=0),
 // otherwise per-tap; PER_TAP / HALO force one (HALO fails on a layer it cannot run).  The consumer schedule is chosen
 // by the planner's cost model (cooperative everywhere with SHAPY_CONV_PINGPONG=0) unless COOP or PINGPONG is or-ed in
-// (PINGPONG then limits the cout tile to what its accumulators fit).
-enum WgmmaPath { WGMMA_AUTO = 0, WGMMA_PER_TAP = 1, WGMMA_HALO = 2, WGMMA_COOP = 4, WGMMA_PINGPONG = 8 };
+// (PINGPONG then limits the cout tile to what its accumulators fit).  AUTO takes the weight-resident halo path (weights
+// loaded once per CTA, 16-channel operand slices) where it fits, unless SHAPY_CONV_RESIDENT=0; RESIDENT forces it and
+// fails on a layer it cannot hold.
+enum WgmmaPath { WGMMA_AUTO = 0, WGMMA_PER_TAP = 1, WGMMA_HALO = 2, WGMMA_COOP = 4, WGMMA_PINGPONG = 8,
+                 WGMMA_RESIDENT = 16 };
 bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out);
 WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
                              int path = WGMMA_AUTO);

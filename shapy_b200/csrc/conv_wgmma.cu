@@ -5,14 +5,20 @@
 // GEMM view: M = 128 output pixels, N = cout tile (<= 128), K = taps * cin walked in 64-channel k-blocks.
 //   * A: one 4-D TMA box per (tap, k-block) straight out of the NHWC activation plane, the box origin shifted by the
 //     tap; out-of-image rows / columns are ZERO-FILLED by the TMA unit = the padding (no im2col, no halo storage).
-//     Stride-2 layers use four parity views of the same plane so every tap is again a dense box.  Channel counts that
-//     are not a multiple of 64 still use 64-channel boxes: TMA zero-fills the channels past cin of both operands.
+//     Stride-2 layers use four parity views of the same plane so every tap is again a dense box.  A layer with
+//     cin < 64 loads boxes of cin channels into the same 128-byte rows and leaves the rest of each row unwritten (no
+//     issued k16 step reads it); wider channel counts that are not a multiple of 64 use 64-channel boxes, and TMA
+//     zero-fills the channels past cin of both operands.
 //   * Halo path (3x3 stride 1, one image per tile): a work item is TH output rows x the full width, computed on the
 //     padded "wide" grid of pitch Wp = W + 2 (tile row r = output (h0 + r / Wp, r % Wp); columns >= W are computed and
 //     dropped by the epilogue).  Each 64-channel block is loaded ONCE with its halo as one (64, Wp, TH + 2) box at
 //     origin (-1, h0 - 1) into a separate halo ring; tap (ky, kx) is the same buffer read from row ky * Wp + kx on (the
 //     descriptor start moves by whole 128-byte rows, the swizzle is a function of the absolute address).  Activations
 //     then cross L2 -> shared memory ~1.4x per channel block instead of 9x; only the weights stream per (tap, block).
+//   * Weight-resident path (halo path with cin <= 64 and one cout tile, where the whole weight set fits): operands
+//     are stored as 16-channel k16 slices with 32-byte rows (SWIZZLE_32B) instead of zero-padded 128-byte rows, every
+//     CTA loads the layer's [tap][cout][cin] weights ONCE (before waiting on the previous kernel), and each tile loads
+//     only its halo band.  The k16 steps and their order are those of the halo path: taps 0..8, slices 0, 1, ...
 //   * B: 3-D TMA box of the pre-packed [tap][cout][cin] fp16 weights (BN scale folded in).
 //   * k16 steps that lie wholly past cin (the zero-filled tail of the last channel block, e.g. 1 of 4 at cin 48) are
 //     not issued.
@@ -63,8 +69,11 @@ struct alignas(64) WgmmaParams {
   int hstages;                   // halo path: halo ring slots
   int relu;
   int pdl_late;                  // 1: release the programmatic dependents when this CTA starts its LAST tile, not at entry
-  uint32_t a_bytes, b_bytes, b_stride;  // per k-block: TMA bytes of A / B, smem pitch of the B_hi(+B_lo) block
+  uint32_t a_bytes, b_bytes, b_stride;  // per k-block: TMA bytes of A, smem pitch of B_hi (B_lo follows) and of B_hi + B_lo
+  uint32_t b_tx;                 // per k-block: TMA bytes of B (one plane)
   uint32_t h_plane;              // halo path: smem pitch of one halo plane (hi or lo)
+  uint32_t h_slice;              // resident path: smem pitch of one 16-channel slice of a halo plane
+  uint32_t w_bytes;              // resident path: TMA bytes (= smem bytes) of the whole weight set, all planes
   const float *bias;
   __half *out_hi, *out_lo;
   int out_ctot, out_coff;
@@ -84,8 +93,8 @@ constexpr int kProdRegs = 40, kConsRegs = 232;
 #ifdef SHAPY_CONV_STAMPS
 // Cycle-stamp build (tools/conv_phase_stamps.py): per consumer warpgroup and tile, clock64 at the first full-barrier
 // pass, the last commit, the return of wait<0> and the end of the epilogue, summed over all tiles of a launch as
-// [wait before the first k-block, mainloop, drain, epilogue, tiles].
-__device__ unsigned long long g_conv_stamps[5];
+// [wait before the first k-block, mainloop, drain, epilogue, tiles, operand waits inside the mainloop].
+__device__ unsigned long long g_conv_stamps[6];
 #endif
 
 // fp32 accumulators per thread of one m64 set: [D0 | D1] of a 64 x NT(x2) tile, and A_lo . B_hi kept apart (wgmma
@@ -93,8 +102,9 @@ __device__ unsigned long long g_conv_stamps[5];
 template <bool SPLIT, int NT>
 constexpr int cons_accs() { return (SPLIT ? 2 * NT : NT) / 2 + (SPLIT ? NT / 2 : 0); }
 
-template <bool SPLIT, int NT, bool HALO, bool PP>
+template <bool SPLIT, int NT, bool HALO, bool PP, bool RES>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_constant__ WgmmaParams p) {
+  static_assert(!RES || HALO, "the weight-resident path is a halo path");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int NACC = (SPLIT ? 2 * NT : NT) / 2;   // fp32 accumulators per thread: [D0 | D1] of a 64 x NT(x2) tile
   constexpr int NLO = SPLIT ? NT / 2 : 1;           // A_lo . B_hi, kept apart: wgmma pipelines only disjoint or equal D
@@ -104,12 +114,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   static_assert(!PP || MT * cons_accs<SPLIT, NT>() <= 192, "ping-pong accumulators must fit the consumer registers");
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t A_BLK = 128 * KCH * 2;
-  // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B]
+  // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B | resident weights]
   //                [ping-pong: output staging box of consumer 0, of consumer 1] [mbarriers]
   const uint32_t h_stage = p.h_plane * PARTS;
   const uint32_t ring_base = smem_base + (HALO ? h_stage * p.hstages : 0u);
   const uint32_t kblk_bytes = (HALO ? 0u : A_BLK * PARTS) + p.b_stride;   // one stage = one k-block of one tap
-  const uint32_t o_base = ring_base + kblk_bytes * p.stages;
+  const uint32_t o_base = ring_base + (RES ? p.w_bytes : kblk_bytes * p.stages);
   const uint32_t bar_base = o_base + (PP ? 2u * p.o_plane * PARTS : 0u);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
@@ -119,6 +129,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   auto handoff_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + c); };
   // ping-pong: the residual box of consumer c's tile has landed in its staging box
   auto res_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + 2 + c); };
+  // resident path: the weight set has landed
+  const uint32_t w_bar = bar_base + 8u * (2 * p.stages + 2 * p.hstages + 4);
   // broadcast so ptxas sees a warp-uniform value: the ping-pong hand-off wait depends on it, and a wait it takes for
   // divergent makes it serialise every wgmma of the kernel
   const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);
@@ -135,9 +147,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
     for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS); }
     for (int s = 0; s < (HALO ? p.hstages : 0); ++s) { mbar_init(hfull_bar(s), 1); mbar_init(hempty_bar(s), CONS); }
     if (PP) for (int c = 0; c < 2; ++c) { mbar_init(handoff_bar(c), 1); mbar_init(res_bar(c), 1); }
+    if (RES) mbar_init(w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  // The weights are packed once, before any launch, so no earlier kernel of the stream writes them: their load
+  // overlaps the previous kernel's tail.  Slice (tap, j) holds cin 16 j .. 16 j + 15 of all cout, hi rows then lo rows.
+  if (RES && threadIdx.x == 0) {
+    const int S = p.cin / 16;
+    mbar_expect_tx(w_bar, p.w_bytes);
+    for (int i = 0; i < 9 * S; ++i) {
+      const uint32_t wb = ring_base + (uint32_t)i * PARTS * p.b_tx;
+      tma_load_3d(wb, &p.b_hi, w_bar, (i % S) * 16, 0, i / S);
+      if (SPLIT) tma_load_3d(wb + p.b_tx, &p.b_lo, w_bar, (i % S) * 16, 0, i / S);
+    }
+  }
   // Programmatic dependent launch: the next kernel of this stream may start its prologue once every CTA here has
   // released it.  Released at entry, its CTAs occupy SMs (which another lane's kernel could use) for this kernel's whole
   // duration; released when a CTA starts its last tile (pdl_late), they only cover this kernel's tail.
@@ -158,11 +182,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       int s = 0, hs = 0;
       uint32_t ph = 0, hph = 0;
       const int pad = p.ksize / 2;
-      const uint32_t tx = (HALO ? p.b_bytes : p.a_bytes + p.b_bytes) * PARTS;
+      const uint32_t tx = (HALO ? p.b_tx : p.a_bytes + p.b_tx) * PARTS;
       for (int id = blockIdx.x; id < total_tiles; id += gridDim.x) {
         int w0, h0, n0, c_out0;
         tile_coords(id, w0, h0, n0, c_out0);
         if (p.pdl_late && id + (int)gridDim.x >= total_tiles) pdl_launch_dependents();   // last tile of this CTA
+        if (RES) {                // the band with its halo, one box per 16-channel slice and plane
+          mbar_wait(hempty_bar(hs), hph ^ 1);
+          mbar_expect_tx(hfull_bar(hs), p.a_bytes * PARTS);
+          const uint32_t hb = smem_base + h_stage * hs;
+          for (int j = 0; j < p.cin / 16; ++j) {
+            tma_load_4d(hb + j * p.h_slice, &p.a_hi[0], hfull_bar(hs), 16 * j, w0 - 1, h0 - 1, n0);
+            if (SPLIT) tma_load_4d(hb + p.h_plane + j * p.h_slice, &p.a_lo[0], hfull_bar(hs), 16 * j, w0 - 1, h0 - 1, n0);
+          }
+          if (++hs == p.hstages) { hs = 0; hph ^= 1; }
+          continue;
+        }
 #pragma unroll 1
         for (int it = 0; it < iters; ++it) {
           int tap, cb;
@@ -212,13 +247,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
     // ping-pong: step the ring positions over the k-blocks (and halo loads) of the other consumer's tile
     auto skip_tile = [&]() {
       const int q = s + iters, hq = hs + p.kpt;
-      ph ^= (uint32_t)(q / p.stages) & 1u; s = q % p.stages;
+      if (!RES) { ph ^= (uint32_t)(q / p.stages) & 1u; s = q % p.stages; }
       if (HALO) { hph ^= (uint32_t)(hq / p.hstages) & 1u; hs = hq % p.hstages; }
     };
     if (PP && cw == 1) skip_tile();
     float acc[MT][NACC], acl[MT][NLO];
+    if (RES) mbar_wait(w_bar, 0);
 #ifdef SHAPY_CONV_STAMPS
-    long long st_end = clock64(), st0 = 0, st1 = 0, st2 = 0;
+    long long st_end = clock64(), st0 = 0, st1 = 0, st2 = 0, st_w = 0;
 #endif
     for (int id = blockIdx.x + (PP ? cw : 0) * gridDim.x, k = 0; id < total_tiles; id += (PP ? 2 : 1) * gridDim.x, ++k) {
       int w0, h0, n0, c_out0;
@@ -242,12 +278,64 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       }
       const uint32_t row0 = PP ? 0u : (uint32_t)cw * 64;   // first tile row of accumulator set 0
       int prev = -1, prev_h = -1;                 // stages the last committed wgmma group reads (prev_h: halo, if its last)
+      if (RES) {                                  // every operand is in shared memory once the halo band has landed
+        mbar_wait(hfull_bar(hs), hph);
+#ifdef SHAPY_CONV_STAMPS
+        st0 = clock64();
+#endif
+        const uint32_t hb = smem_base + h_stage * hs + row0 * 32;
+        auto fence_accs = [&]() {
+#pragma unroll
+          for (int m = 0; m < MT; ++m) {
+#pragma unroll
+            for (int i = 0; i < NACC; ++i) reg_fence(acc[m][i]);
+#pragma unroll
+            for (int i = 0; i < NLO; ++i) reg_fence(acl[m][i]);
+          }
+        };
+        fence_accs();
+        wgmma_fence();
+        // all k16 steps of the tile in the halo path's order (tap-major, then slice) as one group
+        auto issue_res = [&](auto slices) {
+#pragma unroll
+          for (int tap = 0; tap < 9; ++tap) {
+            const uint32_t a_tap = hb + (uint32_t)((tap / 3) * p.TW + tap % 3) * 32;   // 32-byte rows from ky Wp + kx
+#pragma unroll
+            for (int j = 0; j < decltype(slices)::value; ++j) {
+              const uint64_t b = wgmma_desc<16>(ring_base + (uint32_t)(tap * decltype(slices)::value + j) * PARTS * p.b_tx);
+#pragma unroll
+              for (int m = 0; m < MT; ++m) {
+                const uint32_t a_addr = a_tap + j * p.h_slice + m * 64 * 32;
+                if (SPLIT) {
+                  wgmma_f16<2 * NT>(acc[m], wgmma_desc<16>(a_addr), b, 1);
+                  wgmma_f16<NT>(acl[m], wgmma_desc<16>(a_addr + p.h_plane), b, 1);
+                } else {
+                  wgmma_f16<NT>(acc[m], wgmma_desc<16>(a_addr), b, 1);
+                }
+              }
+            }
+          }
+          wgmma_commit();
+        };
+        switch (p.cin / 16) {
+          case 1: issue_res(std::integral_constant<int, 1>()); break;
+          case 2: issue_res(std::integral_constant<int, 2>()); break;
+          case 3: issue_res(std::integral_constant<int, 3>()); break;
+          default: issue_res(std::integral_constant<int, 4>()); break;
+        }
+        fence_accs();
+        prev_h = hs;
+        if (++hs == p.hstages) { hs = 0; hph ^= 1; }
+      }
 #pragma unroll 1
-      for (int it = 0; it < iters; ++it) {
+      for (int it = 0; it < (RES ? 0 : iters); ++it) {
         int tap, cb;
         decode(it, tap, cb);
         const int nks = cb == p.kpt - 1 ? p.ks_last : KCH / 16;
         uint32_t a_addr, a_lo_off;
+#ifdef SHAPY_CONV_STAMPS
+        const long long st_w0 = clock64();
+#endif
         if (HALO) {
           if (tap == 0) mbar_wait(hfull_bar(hs), hph);
           // tap (ky, kx): the halo rows from ky * Wp + kx on (p.TW is the pitch Wp of the padded grid)
@@ -256,7 +344,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
         }
         mbar_wait(full_bar(s), ph);
 #ifdef SHAPY_CONV_STAMPS
-        if (it == 0) st0 = clock64();
+        if (it == 0) st0 = clock64(); else st_w += clock64() - st_w0;
 #endif
         const uint32_t kb = ring_base + kblk_bytes * s;
         if (!HALO) { a_addr = kb + row0 * KCH * 2; a_lo_off = A_BLK; }
@@ -331,8 +419,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
 #pragma unroll
         for (int i = 0; i < NLO; ++i) reg_fence(acl[m][i]);
       }
-      if (prev >= 0 && t == 0) {
-        mbar_arrive(empty_bar(prev));
+      if (t == 0) {
+        if (prev >= 0) mbar_arrive(empty_bar(prev));
         if (prev_h >= 0) mbar_arrive(hempty_bar(prev_h));
       }
       if (PP) skip_tile();
@@ -417,7 +505,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
         atomicAdd(&g_conv_stamps[2], (unsigned long long)(st2 - st1));
         atomicAdd(&g_conv_stamps[3], (unsigned long long)(st3 - st2));
         atomicAdd(&g_conv_stamps[4], 1ull);
+        atomicAdd(&g_conv_stamps[5], (unsigned long long)st_w);
         st_end = st3;
+        st_w = 0;
       }
 #endif
     }
@@ -445,7 +535,7 @@ static int sm_count() {
 struct WgmmaPlan {
   WgmmaParams p;
   int NT;
-  bool split, halo, pingpong;
+  bool split, halo, pingpong, resident;
   dim3 grid;
   size_t smem;
   double tma_bytes, mma_flops;   // per launch, as planned: TMA loads of both operands, tensor-core FLOPs issued
@@ -463,21 +553,29 @@ static bool pingpong_enabled() {
   return v;
 }
 
+// SHAPY_CONV_RESIDENT=0: no plan of WGMMA_AUTO takes the weight-resident path
+static bool resident_enabled() {
+  static const bool v = []() { const char *e = getenv("SHAPY_CONV_RESIDENT"); return !(e && e[0] == '0'); }();
+  return v;
+}
+
 // the ping-pong schedule holds two m64 accumulator sets per consumer thread
 static bool pingpong_fits(bool split, int nt) { return split ? nt <= 64 : nt <= 128; }
 
 #ifdef SHAPY_CONV_STAMPS
 void wgmma_stamps_reset() {
-  const unsigned long long z[5] = {0, 0, 0, 0, 0};
+  const unsigned long long z[6] = {0, 0, 0, 0, 0, 0};
   cudaMemcpyToSymbol(g_conv_stamps, z, sizeof(z));
 }
 void wgmma_stamps_print(const WgmmaPlan *pl) {
-  unsigned long long v[5];
+  unsigned long long v[6];
   cudaDeviceSynchronize();
   cudaMemcpyFromSymbol(v, g_conv_stamps, sizeof(v));
   const double n = v[4] ? (double)v[4] : 1.0;
-  fprintf(stderr, "[stamps] %s NT %d: %llu warpgroup-tiles, cycles per tile: wait %.0f mainloop %.0f drain %.0f epilogue %.0f\n",
-          pl->pingpong ? "ping-pong" : "cooperative", pl->NT, v[4], v[0] / n, v[1] / n, v[2] / n, v[3] / n);
+  fprintf(stderr,
+          "[stamps] %s NT %d: %llu warpgroup-tiles, cycles per tile: wait %.0f mainloop %.0f (operand waits %.0f) "
+          "drain %.0f epilogue %.0f\n",
+          pl->pingpong ? "ping-pong" : "cooperative", pl->NT, v[4], v[0] / n, v[1] / n, v[5] / n, v[2] / n, v[3] / n);
 }
 #endif
 
@@ -503,7 +601,7 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     set_error("wgmma_plan_create: unsupported convolution (cin %d cout %d k %d s %d)", w.cin, w.cout, w.ksize, w.stride);
     return nullptr;
   }
-  const int data_path = path & (WGMMA_PER_TAP | WGMMA_HALO);
+  const int data_path = path & (WGMMA_PER_TAP | WGMMA_HALO | WGMMA_RESIDENT);
   const int sched = path & (WGMMA_COOP | WGMMA_PINGPONG);
   auto *pl = new WgmmaPlan();
   memset(&pl->p, 0, sizeof(pl->p));
@@ -540,13 +638,13 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       const double pt_a = pt_tiles * 9 * p.TW * p.TH * p.TN, h_a = h_tiles * Wp * (th + 2);   // rows loaded per k-block
       better = p.TN == 1 && h_tiles <= pt_tiles && h_a < pt_a;
     }
-    if (data_path == WGMMA_HALO && !possible) {
+    if ((data_path == WGMMA_HALO || data_path == WGMMA_RESIDENT) && !possible) {
       set_error("wgmma_plan_create: no halo path for cin %d cout %d k %d s %d %dx%d", w.cin, w.cout, w.ksize, w.stride,
                 out.H, out.W);
       delete pl;
       return nullptr;
     }
-    pl->halo = data_path == WGMMA_HALO || (data_path == WGMMA_AUTO && better && halo_enabled());
+    pl->halo = data_path == WGMMA_HALO || data_path == WGMMA_RESIDENT || (data_path == WGMMA_AUTO && better && halo_enabled());
     if (pl->halo) {
       p.TW = Wp; p.TH = th; p.TN = 1;
       p.tiles_w = 1; p.tiles_h = ceil_div(out.H, th); p.tiles_n = out.N;
@@ -588,17 +686,61 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
                      pp_cost(best_nt) < rounds(best_nt) * (main_cyc(best_nt) + epi_c * best_nt);
     }
   }
+  // Weight-resident path: a halo layer with one cout tile (kernels exist for cout 48 and 64) and cin <= 64, in 16-channel
+  // slices.  Forced, it takes that cout tile and the requested (or the planner's) schedule.
+  const bool res_shape = pl->halo && w.cin % 16 == 0 && w.cin <= KCH && (w.cout == 48 || w.cout == 64);
+  if (data_path == WGMMA_RESIDENT) {
+    if (!res_shape) {
+      set_error("wgmma_plan_create: no weight-resident path for cin %d cout %d", w.cin, w.cout);
+      delete pl;
+      return nullptr;
+    }
+    pl->NT = w.cout;
+    pl->pingpong = sched == WGMMA_PINGPONG || (sched == 0 && pingpong_enabled() && pingpong_fits(split, pl->NT));
+  }
+  pl->resident = res_shape && pl->NT == w.cout && (data_path == WGMMA_RESIDENT || (data_path == WGMMA_AUTO && resident_enabled()));
   p.relu = relu;
   p.pdl_late = 1;
-  // per k-block TMA bytes of one plane: the A box (halo path: the band with its halo rows) and the weight box
-  const int a_rows = pl->halo ? p.TW * (p.TH + 2) : p.TW * p.TH * p.TN;
-  p.a_bytes = (uint32_t)a_rows * KCH * 2;
-  p.b_bytes = (uint32_t)pl->NT * KCH * 2;
-  p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * PARTS, 1024);
   // ping-pong output staging: one box per consumer and plane (the output tile without the padded grid's junk columns)
   p.o_bw = pl->halo ? out.W : p.TW;
   p.o_bytes = (uint32_t)pl->NT * p.o_bw * p.TH * p.TN * 2;
   p.o_plane = (uint32_t)align_up((size_t)p.o_bytes, 1024);
+  if (pl->resident) {
+    // two halo slots of cin / 16 slices per plane, each slice the rows the furthest tap reads in 32-byte rows, the
+    // whole weight set, the staging boxes: up to the 227 KB a CTA may own
+    const int S = w.cin / 16;
+    p.h_slice = (uint32_t)align_up((size_t)(128 + 2 * Wp + 2) * 32, 256);
+    p.h_plane = p.h_slice * S;
+    p.hstages = 2;
+    p.stages = 0;
+    p.b_tx = (uint32_t)pl->NT * 32;
+    p.w_bytes = 9u * S * PARTS * p.b_tx;
+    p.a_bytes = (uint32_t)p.TW * (p.TH + 2) * w.cin * 2;
+    const size_t staging = pl->pingpong ? 2 * (size_t)p.o_plane * PARTS : 0;
+    pl->smem = (size_t)p.h_plane * PARTS * p.hstages + p.w_bytes + staging + 8 * (2 * p.hstages + 5) + 1024;
+    if (pl->smem > 227 * 1024) {
+      if (data_path == WGMMA_RESIDENT) {
+        set_error("wgmma_plan_create: the weight-resident path does not fit shared memory (cin %d cout %d, %zu B)",
+                  w.cin, w.cout, pl->smem);
+        delete pl;
+        return nullptr;
+      }
+      pl->resident = false;
+    }
+  }
+  // Channels per TMA box.  With cin < 64 a box of cin channels fills the first cin * 2 bytes of each 128-byte row; a
+  // 64-channel box would also write the zero fill past cin, which no issued k16 step reads, and the c48 mainloop is
+  // short of shared-memory bandwidth rather than of loaded stages (README).
+  // The resident path loads 16-channel boxes into 32-byte rows.
+  const int kbox = pl->resident ? 16 : (p.kpt == 1 ? w.cin : KCH);
+  if (!pl->resident) {
+    // per k-block TMA bytes of one plane: the A box (halo path: the band with its halo rows) and the weight box
+    const int a_rows = pl->halo ? p.TW * (p.TH + 2) : p.TW * p.TH * p.TN;
+    p.a_bytes = (uint32_t)a_rows * kbox * 2;
+    p.b_bytes = (uint32_t)pl->NT * KCH * 2;
+    p.b_tx = (uint32_t)pl->NT * kbox * 2;
+    p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * PARTS, 1024);
+  }
   // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory; ping-pong takes its two staging boxes
   // out of the weight ring and may use up to 222 KB
   auto plan_smem = [&]() {
@@ -620,7 +762,7 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     // against 103.9 us cooperative)
     return p.stages >= (pl->pingpong && sched != WGMMA_PINGPONG ? 3 : 2);
   };
-  if (!plan_smem()) {
+  if (!pl->resident && !plan_smem()) {
     if (sched == WGMMA_PINGPONG) {
       set_error("wgmma_plan_create: no room for the ping-pong staging boxes (cin %d cout %d %dx%d)", w.cin, w.cout,
                 out.H, out.W);
@@ -639,7 +781,8 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   {
     const int taps = w.ksize * w.ksize;
     const double a_loads = pl->halo ? p.kpt : taps * p.kpt;   // A boxes per work item
-    pl->tma_bytes = (double)items * PARTS * (a_loads * p.a_bytes + (double)taps * p.kpt * p.b_bytes);
+    pl->tma_bytes = pl->resident ? (double)items * PARTS * p.a_bytes + (double)pl->grid.x * p.w_bytes   // weights once per CTA
+                                 : (double)items * PARTS * (a_loads * p.a_bytes + (double)taps * p.kpt * p.b_tx);
     const double k = (double)taps * ((p.kpt - 1) * KCH + p.ks_last * 16);   // K actually issued per work item
     pl->mma_flops = (double)items * 2.0 * 128 * pl->NT * k * (split ? 3 : 1);
   }
@@ -647,10 +790,12 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     fprintf(stderr,
             "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: %s %s NT %d tile %dx%dx%d grid %d stages %d+%d, staging "
             "2x%ux%u B, smem %zu B, TMA %.1f MB, MMA %.2f GFLOP\n",
-            w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N, pl->halo ? "halo" : "per-tap",
+            w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N,
+            pl->resident ? "resident" : (pl->halo ? "halo" : "per-tap"),
             pl->pingpong ? "ping-pong" : "cooperative", pl->NT, p.TW, p.TH, p.TN, pl->grid.x, p.hstages, p.stages,
             pl->pingpong ? (unsigned)PARTS : 0u, p.o_plane, pl->smem, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
   bool ok = true;
+  const int swz = pl->resident ? 16 : KCH;   // row width of the shared-memory operands in channels: picks the swizzle
   // activation maps
   const int nmaps = w.stride == 2 ? 4 : 1;
   for (int mi = 0; mi < nmaps && ok; ++mi) {
@@ -669,16 +814,16 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       off = (size_t)in.coff + ((size_t)phy * in.W + phx) * in.Ctot;
     }
     // halo path: the band plus one row above and below; p.TW = Wp already spans the two padding columns
-    cuuint32_t box[4] = {(cuuint32_t)KCH, (cuuint32_t)p.TW, (cuuint32_t)(p.TH + (pl->halo ? 2 : 0)), (cuuint32_t)p.TN};
-    ok = ok && encode(&p.a_hi[mi], in.hi + off, 4, dims, strides, box, KCH);
-    if (split) ok = ok && encode(&p.a_lo[mi], in.lo + off, 4, dims, strides, box, KCH);
+    cuuint32_t box[4] = {(cuuint32_t)kbox, (cuuint32_t)p.TW, (cuuint32_t)(p.TH + (pl->halo ? 2 : 0)), (cuuint32_t)p.TN};
+    ok = ok && encode(&p.a_hi[mi], in.hi + off, 4, dims, strides, box, swz);
+    if (split) ok = ok && encode(&p.a_lo[mi], in.lo + off, 4, dims, strides, box, swz);
   }
   if (ok) {
     cuuint64_t dims[3] = {(cuuint64_t)w.cin, (cuuint64_t)w.cout, (cuuint64_t)(w.ksize * w.ksize)};
     cuuint64_t strides[2] = {(cuuint64_t)w.cin * 2, (cuuint64_t)w.cin * w.cout * 2};
-    cuuint32_t box[3] = {(cuuint32_t)KCH, (cuuint32_t)pl->NT, 1};
-    ok = ok && encode(&p.b_hi, w.w_hi, 3, dims, strides, box, KCH);
-    if (split) ok = ok && encode(&p.b_lo, w.w_lo, 3, dims, strides, box, KCH);
+    cuuint32_t box[3] = {(cuuint32_t)kbox, (cuuint32_t)pl->NT, 1};
+    ok = ok && encode(&p.b_hi, w.w_hi, 3, dims, strides, box, swz);
+    if (split) ok = ok && encode(&p.b_lo, w.w_lo, 3, dims, strides, box, swz);
   }
   // ping-pong epilogue maps: the output view (out_coff / out_ctot as the activation maps carry coff / Ctot) and the
   // residual view, in boxes of the staged tile; no swizzle (the epilogue addresses the box row-major)
@@ -698,10 +843,10 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
 
 void wgmma_plan_destroy(WgmmaPlan *p) { delete p; }
 
-template <bool SPLIT, int NT, bool HALO, bool PP>
+template <bool SPLIT, int NT, bool HALO, bool PP, bool RES = false>
 static int launch_h(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
   static std::atomic<unsigned long long> attr_done{0};
-  auto kernel = conv_wgmma_kernel<SPLIT, NT, HALO, PP>;
+  auto kernel = conv_wgmma_kernel<SPLIT, NT, HALO, PP, RES>;
   SHAPY_CUDA_TRY(set_max_dynamic_smem(kernel, 227 * 1024, attr_done));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -721,6 +866,11 @@ static int launch_h(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
 
 template <bool SPLIT, int NT, bool PP>
 static int launch_s(const WgmmaPlan *pl, cudaStream_t st, bool pdl) {
+  if (pl->resident) {
+    if constexpr (NT == 48 || NT == 64) return launch_h<SPLIT, NT, true, PP, true>(pl, st, pdl);
+    set_error("wgmma engine: no weight-resident kernel for NT %d", NT);
+    return SHAPY_ERR_STATE;
+  }
   return pl->halo ? launch_h<SPLIT, NT, true, PP>(pl, st, pdl) : launch_h<SPLIT, NT, false, PP>(pl, st, pdl);
 }
 

@@ -528,10 +528,11 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
   if (engine != 1) {
-    // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo; engine / 10: 0 = the planner's
-    // schedule, 1 = cooperative, 2 = ping-pong
+    // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo, 4 = weight-resident halo; engine / 10:
+    // 0 = the planner's schedule, 1 = cooperative, 2 = ping-pong
     const int e_path = engine % 10, e_sched = engine / 10;
-    const int path = (e_path == 2 ? WGMMA_PER_TAP : (e_path == 3 ? WGMMA_HALO : WGMMA_AUTO)) |
+    const int path = (e_path == 2 ? WGMMA_PER_TAP
+                                  : (e_path == 3 ? WGMMA_HALO : (e_path == 4 ? WGMMA_RESIDENT : WGMMA_AUTO))) |
                      (e_sched == 1 ? WGMMA_COOP : (e_sched == 2 ? WGMMA_PINGPONG : 0));
     plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }

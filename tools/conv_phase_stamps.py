@@ -1,7 +1,8 @@
 """Where the time of a wgmma convolution tile goes: builds the cycle-stamp variant of the library (-DSHAPY_CONV_STAMPS,
 which the default build leaves out) into OUT, then for each layer, precision mode and consumer schedule prints the
 mean clock64 cycles per warpgroup-tile spent waiting for the first k-block, in the mainloop (first full-barrier pass
-to the last commit), in the drain (last commit to the return of wait<0>) and in the epilogue.  Cooperative tiles are
+to the last commit; of that, the operand waits on the later k-blocks' full barriers), in the drain (last commit to the
+return of wait<0>) and in the epilogue.  Cooperative tiles are
 64-row halves issued by both consumers at once; ping-pong tiles are whole 128-row tiles of one consumer.
 usage: python tools/conv_phase_stamps.py [--out DIR] [--layers c48,c96,...] [--reps N]"""
 import argparse
