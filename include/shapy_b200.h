@@ -114,6 +114,29 @@ size_t shapy_smplx_backward_shape_workspace_bytes(const shapy_smplx_t *m, int ba
 int shapy_smplx_backward_shape(const shapy_smplx_t *m, const float *grad_v_shaped, int batch, float *grad_betas,
                                void *workspace, size_t workspace_bytes, void *stream);
 
+/* Adjoint of shapy_smplx_forward (the reference's lbs() and SMPLX.forward under autograd, pose2rot=False), first
+ * order.  Inputs as in shapy_smplx_forward; it recomputes the forward from them, nothing is kept between the calls.
+ *   cotangents (any may be NULL = zero): grad_vertices (B,V,3), grad_v_shaped (B,V,3), grad_joints (B,K,3),
+ *                                        grad_proj_joints (B,K,2)
+ *   gradients  (any may be NULL = not wanted): grad_betas (B,NB), grad_rot (B,n_rot,3,3), grad_expr (B,NE),
+ *                                        grad_camera (B,3)
+ * Semantics: a rotation's gradient is the raw dL/dR (9 entries, no tangent projection); v_shaped carries no
+ * expression, so its cotangent reaches betas only; the dynamic-contour LUT row is a constant (the barycentric mix of
+ * its vertices is differentiated); an overwritten J14 keypoint's cotangent goes to the J14 regression of the
+ * vertices, not to the joint or landmark it replaced; proj = softplus(c0) (xy + c[1:3]) with softplus' threshold 20.
+ * grad_expr is the gradient at expr (zeros when expr is NULL).  grad_proj_joints and grad_camera require camera.
+ * Deterministic, no atomics; a body's gradient does not depend on the rest of the batch.  batch 0: no launch.
+ * workspace: device, >= shapy_smplx_backward_workspace_bytes(m, batch, n_rot) (about 3 x 12 V bytes per body). */
+size_t shapy_smplx_backward_workspace_bytes(const shapy_smplx_t *m, int batch, int n_rot);
+int shapy_smplx_backward(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot, const float *expr,
+                         const float *camera, int batch, const float *grad_vertices, const float *grad_v_shaped,
+                         const float *grad_joints, const float *grad_proj_joints, float *grad_betas, float *grad_rot,
+                         float *grad_expr, float *grad_camera, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Adjoint of shapy_decode_rot6d: grad_raw (n, 6) from raw (n, 6) and grad_rot (n, 3, 3), elementwise.  The 1e-12
+ * clamp of each norm passes gradient to the norm only where the norm is >= 1e-12 (torch's clamp_min). */
+int shapy_decode_rot6d_backward(const float *raw, int n, const float *grad_rot, float *grad_raw, void *stream);
+
 /* ------------------------------------------------------- virtual measurements */
 typedef struct {
   int face_idx[5];      /* head_top, left_heel, chest, waist, hips landmark faces */

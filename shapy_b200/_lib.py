@@ -71,6 +71,10 @@ _SIGS = {
                                            c_void_p, c_int, c_void_p, c_void_p]),
     'shapy_smplx_backward_shape_workspace_bytes': (c_size_t, [c_void_p, c_int]),
     'shapy_smplx_backward_shape': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'shapy_smplx_backward_workspace_bytes': (c_size_t, [c_void_p, c_int, c_int]),
+    'shapy_smplx_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 8
+                             + [c_void_p, c_size_t, c_void_p]),
+    'shapy_decode_rot6d_backward': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                        C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,

@@ -1,15 +1,21 @@
-"""Autograd for the T-pose shape blend and the virtual measurements (first order only).
+"""Autograd for the SMPL-X forward, the 6D decoder, the T-pose shape blend and the virtual measurements (first order
+only).
 
     measure(landmarks, v_shaped=, faces_i32=)   (B,V,3) vertices + (F,3) int32 faces -> (B,5)
     measure(landmarks, triangles=)              (B,F,3,3) triangles -> (B,5)
     ShapeFunction.apply(packed_model, betas)    betas (B,NB) -> v_shaped (B,V,3)
+    SmplxFunction.apply(packed_model, betas, rot, expression, camera, want_v_shaped)
+                                                -> vertices, v_shaped, joints, proj_joints (None where not computed)
+    Rot6dFunction.apply(raw)                    raw (B,6n) -> (B,n,3,3)
 
-The forward of each is the same launch as the no-grad path; the backward is one CUDA launch (measure_smem_kernel in
-gradient mode, or the shape-blend adjoint).  The semantics are the reference's autograd ones
-(mesh-mesh-intersection/body_measurements/body_measurements.py:137-215): the intersection points' barycentrics are
+The forward of each is the same launches as the no-grad path; the backward is the matching CUDA adjoint
+(measure_smem_kernel in gradient mode, the shape-blend adjoint, shapy_smplx_backward which recomputes the posed
+forward, or the decoder's elementwise adjoint).  SmplxFunction's semantics are those of the reference's lbs() and
+SMPLX.forward under autograd: see include/shapy_b200.h and DESIGN.md §6b.  For the measurements they are the
+reference's autograd ones (mesh-mesh-intersection/body_measurements/body_measurements.py:137-215): the intersection points' barycentrics are
 constants and the slicing planes' heights get no gradient, so a circumference's gradient is the derivative of the
 perimeter with the hull's points sliding on fixed faces at fixed barycentrics, not the finite difference of the mesh.
-Both functions are `once_differentiable`: a double backward (`create_graph=True`, e.g. the TrustRegion optimiser of
+Every function is `once_differentiable`: a double backward (`create_graph=True`, e.g. the TrustRegion optimiser of
 the reference's examples/fit_measurements.py) raises.
 """
 import torch
@@ -52,6 +58,42 @@ class ShapeFunction(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, grad_v):
         return None, _ops.smplx_backward_shape(ctx.packed, grad_v.contiguous())
+
+
+class SmplxFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, packed, betas, rot, expression, camera, want_v_shaped):
+        out = _ops.smplx_forward(packed, betas, rot, expr=expression, camera=camera, want_vertices=True,
+                                 want_v_shaped=want_v_shaped, want_joints=True)
+        ctx.packed = packed
+        ctx.save_for_backward(betas, rot, expression, camera)
+        ctx.set_materialize_grads(False)      # an unused output passes None, read as a zero cotangent
+        return out['vertices'], out['v_shaped'], out['joints'], out['proj_joints']
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_vertices, g_v_shaped, g_joints, g_proj):
+        betas, rot, expression, camera = ctx.saved_tensors
+        names = ('betas', 'rot', 'expr', 'camera')
+        want = tuple(n for n, need in zip(names, ctx.needs_input_grad[1:5]) if need)
+        c = lambda g: None if g is None else g.contiguous()  # noqa: E731
+        r = _ops.smplx_backward(ctx.packed, betas, rot, expression, camera, grad_vertices=c(g_vertices),
+                                grad_v_shaped=c(g_v_shaped), grad_joints=c(g_joints), grad_proj_joints=c(g_proj),
+                                want=want)
+        return (None,) + tuple(r[n] for n in names) + (None,)
+
+
+class Rot6dFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, raw):
+        ctx.save_for_backward(raw)
+        return _ops.decode_rot6d(raw)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_rot):
+        raw, = ctx.saved_tensors
+        return _ops.decode_rot6d_backward(raw, grad_rot.contiguous()).view_as(raw)
 
 
 def wants_grad(t) -> bool:

@@ -12,7 +12,8 @@
 //                        through shared memory once per tile, reused by all 32 bodies), plus the GEMM's
 //                        pose offsets, sparse skinning
 //   smplx_joints_kernel  per body: landmarks, sparse J14 regressor + overwrite, weak-perspective camera
-// plus smplx_shape_kernel for the T-pose path (SMPL.forward_shape, body_models.py:292-302).
+// plus smplx_shape_kernel for the T-pose path (SMPL.forward_shape, body_models.py:292-302), and the adjoints of both
+// (shapy_smplx_backward, shapy_smplx_backward_shape, shapy_decode_rot6d_backward; see "posed backward" below).
 //
 // Exact structure that is exploited (changes summation order only):
 //   * J = J_regressor . (T + S.beta) = J_regressor.T + (J_regressor.S).beta  (contracted once, in fp64)
@@ -61,18 +62,18 @@ struct PoseArgs {
   __half *x_hi, *x_lo;      // pose-blend GEMM input [B][Kpad]; null when no GEMM runs
 };
 
-__global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
-  const SmplxDev &m = a.m;
-  const int b = blockIdx.x, t = threadIdx.x;
-  __shared__ float R[kMaxJoints][9];
-  __shared__ float Jr[kMaxJoints][3];
-  __shared__ float G[kMaxJoints][12];
-  __shared__ float coef[kMaxCoef];
+// Per body: blend coefficients [betas | expression], rotations (identity past n_rot), rest joints
+// J = J_template + J_dirs . coef and the world transforms G = [G.R | G.t] of the kinematic chain, level by level.
+// Shared by smplx_pose_kernel and smplx_chain_bwd_kernel, so the backward walks the same G bit for bit.
+__device__ __forceinline__ void body_chain(const SmplxDev &m, const float *betas, const float *expr, const float *rot,
+                                           int n_rot, int b, float (*R)[9], float (*Jr)[3], float (*G)[12],
+                                           float *coef) {
+  const int t = threadIdx.x;
   const int J = m.J;
-  if (t < m.NC) coef[t] = t < m.NB ? a.betas[(size_t)b * m.NB + t] : (a.expr ? a.expr[(size_t)b * m.NE + (t - m.NB)] : 0.f);
+  if (t < m.NC) coef[t] = t < m.NB ? betas[(size_t)b * m.NB + t] : (expr ? expr[(size_t)b * m.NE + (t - m.NB)] : 0.f);
   for (int i = t; i < J * 9; i += blockDim.x) {
     int j = i / 9, e = i % 9;
-    R[j][e] = j < a.n_rot ? a.rot[((size_t)b * a.n_rot + j) * 9 + e] : ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f);
+    R[j][e] = j < n_rot ? rot[((size_t)b * n_rot + j) * 9 + e] : ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f);
   }
   __syncthreads();
   for (int i = t; i < J * 3; i += blockDim.x) {
@@ -104,6 +105,17 @@ __global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
     }
     __syncthreads();
   }
+}
+
+__global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
+  const SmplxDev &m = a.m;
+  const int b = blockIdx.x, t = threadIdx.x;
+  __shared__ float R[kMaxJoints][9];
+  __shared__ float Jr[kMaxJoints][3];
+  __shared__ float G[kMaxJoints][12];
+  __shared__ float coef[kMaxCoef];
+  const int J = m.J;
+  body_chain(m, a.betas, a.expr, a.rot, a.n_rot, b, R, Jr, G, coef);
   // relative transforms A = G - [0 | G.R . J_rest]   (lbs.py:289-293)
   for (int i = t; i < J * 12; i += blockDim.x) {
     int j = i / 12, e = i % 12, r = e / 4, c = e % 4;
@@ -177,16 +189,18 @@ __global__ void pack_pose_weights_kernel(const float *__restrict__ posedirs, int
 // are one [rows][V3p] basis; a chunk of 32 rows (96 floats each) and the matching [rows][32 bodies] coefficient
 // block are staged in shared memory with 16-byte cp.async, double buffered, so every constant crosses L2 once
 // per tile and the loads of chunk i+1 overlap the FMAs of chunk i.
-__global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
+//
+// v_posed of one tile, in acc[body][xyz]: the shape (+ expression) blend and, when posed, the pose-blend GEMM's
+// offsets; v_shaped is written after the shape rows when asked.  The forward vertex kernel and the backward
+// (smplx_vertex_bwd_kernel) both compute v_posed here, so they see the same bits.  Every thread of the CTA calls it.
+__device__ __forceinline__ void tile_v_posed(const VertexArgs &a, bool posed, float (&acc)[8][3],
+                                             float (&Ps)[2][KC][TV * 3], float (&pfs)[2][KC][TB]) {
   const SmplxDev &m = a.m;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, t = threadIdx.x;
   const int v0 = blockIdx.x * TV, b0 = blockIdx.y * TB;
   const int c0 = v0 * 3;
-  __shared__ __align__(16) float Ps[2][KC][TV * 3];
-  __shared__ __align__(16) float pfs[2][KC][TB];
   const int v = v0 + lane;
   const bool vok = v < m.V;
-  float acc[8][3];
   {
     float tx = 0.f, ty = 0.f, tz = 0.f;
     if (vok) { tx = m.v_template[3 * v]; ty = m.v_template[3 * v + 1]; tz = m.v_template[3 * v + 2]; }
@@ -194,7 +208,6 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
     for (int i = 0; i < 8; ++i) { acc[i][0] = tx; acc[i][1] = ty; acc[i][2] = tz; }
   }
   // row schedule: [0, NB) shape | [NB, NC) expression (only when given, and only for vertices)
-  const bool posed = a.vertices != nullptr;
   const int n_rows = (a.expr && posed) ? m.NC : m.NB;
   // chunk boundaries: the first chunk ends exactly after the NB shape rows (v_shaped snapshot)
   auto chunk_begin = [&](int ch) { return ch == 0 ? 0 : m.NB + (ch - 1) * KC; };
@@ -250,8 +263,7 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
     }
     __syncthreads();
   }
-  if (!posed || !vok) return;
-  if (a.pb_hi) {
+  if (posed && vok && a.pb_hi) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int b = b0 + warp * 8 + i;
@@ -261,6 +273,18 @@ __global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
       for (int c = 0; c < 3; ++c) acc[i][c] += __half2float(a.pb_hi[o + c]) + __half2float(a.pb_lo[o + c]) * kLoInv;
     }
   }
+}
+
+__global__ void __launch_bounds__(128) smplx_vertex_kernel(VertexArgs a) {
+  const SmplxDev &m = a.m;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int v = blockIdx.x * TV + lane, b0 = blockIdx.y * TB;
+  __shared__ __align__(16) float Ps[2][KC][TV * 3];
+  __shared__ __align__(16) float pfs[2][KC][TB];
+  float acc[8][3];
+  const bool posed = a.vertices != nullptr;
+  tile_v_posed(a, posed, acc, Ps, pfs);
+  if (!posed || v >= m.V) return;
   // ---- sparse linear blend skinning: out = sum_j w_vj (A_j . [v_posed; 1])
   float out[8][3];
 #pragma unroll
@@ -415,64 +439,75 @@ __global__ void smplx_shape_kernel_generic(const float *__restrict__ T, const fl
   out[(size_t)b * V3 + c] = v;
 }
 
-// Adjoint of the T-pose path: grad_betas[b][l] = sum_c S[l][c] grad_v[b][c].  The 3V coordinates are cut into
+// Adjoint of the blend shapes: part of grad_coef[b][l] = sum_c S[l][c] g[b][c] over the NB shape rows and the NE
+// expression rows that follow them in the basis.  g = gv for every row, plus gv2 (when given) for the shape rows only:
+// the posed backward passes the cotangent of v_posed as gv and that of v_shaped, which carries no expression
+// (body_models.py:763-765), as gv2; the T-pose path passes gv alone with NE = 0.  The 3V coordinates are cut into
 // kShapeSplit fixed chunks; CTA (tile, chunk) writes the partial sums of its bodies over its chunk (per thread over a
 // fixed stride, then a fixed xor tree and a fixed order over warps) and smplx_shape_bwd_sum_kernel adds the chunks in
 // order.  Neither the chunking nor the order depends on B or on a body's place in the batch, so a body's gradient is
 // bit-identical alone and in any batch.  HBM traffic is the (B, 3V) gradient read once (S stays in L2, read once per
-// kShapeTile bodies).
+// TILE bodies).
 constexpr int kShapeSplit = 16;
 constexpr int kShapeTile = 8;
-template <int NB>
+template <int NB, int NE, int TILE>
 __global__ void __launch_bounds__(256) smplx_shape_bwd_kernel(const float *__restrict__ S, int ld,
-                                                              const float *__restrict__ gv, int V3, int B,
+                                                              const float *__restrict__ gv,
+                                                              const float *__restrict__ gv2, int V3, int B,
                                                               float *__restrict__ part) {
-  const int b0 = blockIdx.x * kShapeTile, t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const int nb = min(kShapeTile, B - b0);
+  constexpr int NR = NB + NE;
+  const int b0 = blockIdx.x * TILE, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int nb = min(TILE, B - b0);
   const int chunk = (V3 + kShapeSplit - 1) / kShapeSplit, c_lo = blockIdx.y * chunk, c_hi = min(V3, c_lo + chunk);
-  float acc[kShapeTile][NB];
+  float acc[TILE][NR];
 #pragma unroll
-  for (int i = 0; i < kShapeTile; ++i)
+  for (int i = 0; i < TILE; ++i)
 #pragma unroll
-    for (int l = 0; l < NB; ++l) acc[i][l] = 0.f;
+    for (int l = 0; l < NR; ++l) acc[i][l] = 0.f;
   for (int c = c_lo + t; c < c_hi; c += 256) {
-    float s[NB];
+    float s[NR];
 #pragma unroll
-    for (int l = 0; l < NB; ++l) s[l] = __ldg(S + (size_t)l * ld + c);
+    for (int l = 0; l < NR; ++l) s[l] = __ldg(S + (size_t)l * ld + c);
 #pragma unroll
-    for (int i = 0; i < kShapeTile; ++i) {
+    for (int i = 0; i < TILE; ++i) {
       if (i < nb) {
         const float g = __ldcs(gv + (size_t)(b0 + i) * V3 + c);
+        const float gs = gv2 ? g + __ldcs(gv2 + (size_t)(b0 + i) * V3 + c) : g;
 #pragma unroll
-        for (int l = 0; l < NB; ++l) acc[i][l] += g * s[l];
+        for (int l = 0; l < NR; ++l) acc[i][l] += (l < NB ? gs : g) * s[l];
       }
     }
   }
-  __shared__ float red[8][kShapeTile * NB];
+  __shared__ float red[8][TILE * NR];
 #pragma unroll
-  for (int i = 0; i < kShapeTile; ++i)
+  for (int i = 0; i < TILE; ++i)
 #pragma unroll
-    for (int l = 0; l < NB; ++l) {
+    for (int l = 0; l < NR; ++l) {
       float v = acc[i][l];
       for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) red[warp][i * NB + l] = v;
+      if (lane == 0) red[warp][i * NR + l] = v;
     }
   __syncthreads();
-  for (int r = t; r < nb * NB; r += 256) {
+  for (int r = t; r < nb * NR; r += 256) {
     float v = 0.f;
     for (int w = 0; w < 8; ++w) v += red[w][r];
-    part[((size_t)(b0 + r / NB) * kShapeSplit + blockIdx.y) * NB + r % NB] = v;
+    part[((size_t)(b0 + r / NR) * kShapeSplit + blockIdx.y) * NR + r % NR] = v;
   }
 }
 
-// any NB: CTA (body, chunk, l)
+// any row count: CTA (body, chunk, l), l < NR; gv2 adds to the rows below NB
 __global__ void __launch_bounds__(256) smplx_shape_bwd_kernel_generic(const float *__restrict__ S, int ld,
-                                                                      const float *__restrict__ gv, int NB, int V3,
-                                                                      float *__restrict__ part) {
+                                                                      const float *__restrict__ gv,
+                                                                      const float *__restrict__ gv2, int NB, int NR,
+                                                                      int V3, float *__restrict__ part) {
   const int b = blockIdx.x, l = blockIdx.z, t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int chunk = (V3 + kShapeSplit - 1) / kShapeSplit, c_lo = blockIdx.y * chunk, c_hi = min(V3, c_lo + chunk);
+  const float *g2 = (gv2 && l < NB) ? gv2 : nullptr;
   float v = 0.f;
-  for (int c = c_lo + t; c < c_hi; c += 256) v += __ldg(gv + (size_t)b * V3 + c) * __ldg(S + (size_t)l * ld + c);
+  for (int c = c_lo + t; c < c_hi; c += 256) {
+    const float g = __ldg(gv + (size_t)b * V3 + c);
+    v += (g2 ? g + __ldg(g2 + (size_t)b * V3 + c) : g) * __ldg(S + (size_t)l * ld + c);
+  }
   for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   __shared__ float red[8];
   if (lane == 0) red[warp] = v;
@@ -480,7 +515,7 @@ __global__ void __launch_bounds__(256) smplx_shape_bwd_kernel_generic(const floa
   if (t == 0) {
     float s = 0.f;
     for (int w = 0; w < 8; ++w) s += red[w];
-    part[((size_t)b * kShapeSplit + blockIdx.y) * NB + l] = s;
+    part[((size_t)b * kShapeSplit + blockIdx.y) * NR + l] = s;
   }
 }
 
@@ -491,6 +526,344 @@ __global__ void smplx_shape_bwd_sum_kernel(const float *__restrict__ part, int N
   float v = 0.f;
   for (int s = 0; s < kShapeSplit; ++s) v += part[((size_t)b * kShapeSplit + s) * NB + l];
   gb[r] = v;
+}
+
+// ============================================================================================== posed backward
+// Adjoint of shapy_smplx_forward, first order, with the reference's autograd semantics (DESIGN.md §6b).  It recomputes
+// the forward from its inputs (smplx_pose_kernel and the pose-blend GEMM give A, the LUT rows and the pose offsets bit
+// for bit; tile_v_posed gives v_posed), then runs the adjoints below.  No float atomics: every sum has a fixed order
+// that does not depend on B or on a body's place in the batch.
+
+// 6D decoder: the adjoint of decode_rot6d_kernel's Gram-Schmidt.  clamp_min(norm, 1e-12) passes the gradient to the
+// norm only where norm >= 1e-12, as torch's clamp_min does under autograd.
+__global__ void decode_rot6d_bwd_kernel(const float *__restrict__ raw, int n, const float *__restrict__ grot,
+                                        float *__restrict__ graw) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float *x = raw + 6 * (size_t)i;
+  const float *G = grot + 9 * (size_t)i;
+  float a[3] = {x[0], x[2], x[4]}, c[3] = {x[1], x[3], x[5]};
+  const float n1r = sqrtf(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]), n1 = fmaxf(n1r, 1e-12f);
+  float b1[3], u[3], b2[3];
+  for (int k = 0; k < 3; ++k) b1[k] = a[k] / n1;
+  const float d = b1[0] * c[0] + b1[1] * c[1] + b1[2] * c[2];
+  for (int k = 0; k < 3; ++k) u[k] = c[k] - d * b1[k];
+  const float n2r = sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), n2 = fmaxf(n2r, 1e-12f);
+  for (int k = 0; k < 3; ++k) b2[k] = u[k] / n2;
+  // R = [b1 b2 b3] by columns
+  float g1[3] = {G[0], G[3], G[6]}, g2[3] = {G[1], G[4], G[7]}, g3[3] = {G[2], G[5], G[8]};
+  // b3 = b1 x b2
+  g1[0] += b2[1] * g3[2] - b2[2] * g3[1]; g1[1] += b2[2] * g3[0] - b2[0] * g3[2]; g1[2] += b2[0] * g3[1] - b2[1] * g3[0];
+  g2[0] += g3[1] * b1[2] - g3[2] * b1[1]; g2[1] += g3[2] * b1[0] - g3[0] * b1[2]; g2[2] += g3[0] * b1[1] - g3[1] * b1[0];
+  // b2 = u / n2
+  float gu[3];
+  const float gn2 = -(g2[0] * u[0] + g2[1] * u[1] + g2[2] * u[2]) / (n2 * n2);
+  for (int k = 0; k < 3; ++k) gu[k] = g2[k] / n2 + (n2r >= 1e-12f ? gn2 * u[k] / n2r : 0.f);
+  // u = c - d b1, d = b1 . c
+  const float gd = -(gu[0] * b1[0] + gu[1] * b1[1] + gu[2] * b1[2]);
+  float gc[3];
+  for (int k = 0; k < 3; ++k) {
+    gc[k] = gu[k] + gd * b1[k];
+    g1[k] += -d * gu[k] + gd * c[k];
+  }
+  // b1 = a / n1
+  float ga[3];
+  const float gn1 = -(g1[0] * a[0] + g1[1] * a[1] + g1[2] * a[2]) / (n1 * n1);
+  for (int k = 0; k < 3; ++k) ga[k] = g1[k] / n1 + (n1r >= 1e-12f ? gn1 * a[k] / n1r : 0.f);
+  float *o = graw + 6 * (size_t)i;
+  o[0] = ga[0]; o[1] = gc[0]; o[2] = ga[1]; o[3] = gc[1]; o[4] = ga[2]; o[5] = gc[2];
+}
+
+// Joints backward, per body: the cotangent of the keypoints (joints + the proj_joints term), the camera gradient, the
+// J14 routing (an overwritten keypoint's cotangent goes to its J14 row, the joint or landmark it replaced gets none),
+// and the split into posed-joint cotangents gP [B][J][3] and landmark / J14 cotangents gkp [B][nkp][3].
+struct JointsBwdArgs {
+  SmplxDev m;
+  const float *joints;            // forward joints [B][K][3]; read only for the camera gradient
+  const float *camera, *g_joints, *g_proj;
+  float *gP, *gkp, *g_camera;
+};
+
+__global__ void __launch_bounds__(128) smplx_joints_bwd_kernel(JointsBwdArgs a) {
+  const SmplxDev &m = a.m;
+  const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  extern __shared__ float sm[];
+  float *gj = sm;                 // [K][3]
+  float *greg = sm + m.K * 3;     // [n_extra][3]
+  const int nkp = m.L + m.D + m.n_extra;
+  const float *gproj = a.camera ? a.g_proj : nullptr;
+  float s = 0.f, c0 = 0.f;
+  if (a.camera) {
+    c0 = a.camera[3 * b];
+    s = c0 > 20.f ? c0 : log1pf(expf(c0));
+  }
+  for (int i = t; i < m.K * 3; i += blockDim.x) {
+    float g = a.g_joints ? a.g_joints[(size_t)b * m.K * 3 + i] : 0.f;
+    if (gproj && i % 3 < 2) g += s * gproj[((size_t)b * m.K + i / 3) * 2 + i % 3];
+    gj[i] = g;
+  }
+  for (int i = t; i < m.n_extra * 3; i += blockDim.x) greg[i] = 0.f;
+  if (a.g_camera && warp == 0) {
+    // proj = s (xy + t): d/ds = sum g (xy + t), d/dt = sum s g; ds/dc0 = sigmoid(c0), or 1 past softplus' threshold
+    float gs = 0.f, gx = 0.f, gy = 0.f;
+    if (gproj) {
+      const float tx = a.camera[3 * b + 1], ty = a.camera[3 * b + 2];
+      const float *jt = a.joints + (size_t)b * m.K * 3;
+      for (int i = lane; i < m.K; i += 32) {
+        const float px = gproj[((size_t)b * m.K + i) * 2], py = gproj[((size_t)b * m.K + i) * 2 + 1];
+        gs += px * (jt[3 * i] + tx) + py * (jt[3 * i + 1] + ty);
+        gx += s * px;
+        gy += s * py;
+      }
+    }
+    for (int o = 16; o; o >>= 1) {
+      gs += __shfl_xor_sync(0xffffffffu, gs, o);
+      gx += __shfl_xor_sync(0xffffffffu, gx, o);
+      gy += __shfl_xor_sync(0xffffffffu, gy, o);
+    }
+    if (lane == 0) {
+      a.g_camera[3 * b] = gs * (c0 > 20.f ? 1.f : 1.f / (1.f + expf(-c0)));
+      a.g_camera[3 * b + 1] = gx;
+      a.g_camera[3 * b + 2] = gy;
+    }
+  }
+  __syncthreads();
+  if (t == 0) {
+    for (int q = 0; q < m.n_over; ++q)
+      for (int c = 0; c < 3; ++c) greg[m.over_tgt[q] * 3 + c] += gj[m.over_src[q] * 3 + c];
+    for (int q = 0; q < m.n_over; ++q)
+      for (int c = 0; c < 3; ++c) gj[m.over_src[q] * 3 + c] = 0.f;
+  }
+  __syncthreads();
+  if (!a.gP) return;
+  for (int i = t; i < m.J * 3; i += blockDim.x) a.gP[(size_t)b * m.J * 3 + i] = gj[i];
+  float *gk = a.gkp + (size_t)b * nkp * 3;
+  for (int i = t; i < (m.L + m.D) * 3; i += blockDim.x) gk[i] = gj[m.J * 3 + i];
+  for (int i = t; i < m.n_extra * 3; i += blockDim.x) gk[(m.L + m.D) * 3 + i] = greg[i];
+}
+
+// Vertex backward on the forward's tile of 32 vertices x 32 bodies: v_posed (tile_v_posed), the total vertex
+// cotangent gv = grad_vertices + the landmark and J14 cotangents gathered through the per-vertex keypoint entries, and
+// its pull-back through the skinning, gvp = sum_s w_s R_{A_s}^T gv.  Writes v_posed, gv and gvp, each [B][V][3].
+struct VertexBwdArgs {
+  VertexArgs f;                   // recompute of v_posed; f.vertices and f.v_shaped are unused
+  const float *g_vertices, *gkp;  // either may be null (zero)
+  const int *lut;
+  float *vp, *gv, *gvp;
+};
+
+__global__ void __launch_bounds__(128) smplx_vertex_bwd_kernel(VertexBwdArgs a) {
+  const SmplxDev &m = a.f.m;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int v = blockIdx.x * TV + lane, b0 = blockIdx.y * TB;
+  __shared__ __align__(16) float Ps[2][KC][TV * 3];
+  __shared__ __align__(16) float pfs[2][KC][TB];
+  float acc[8][3];
+  tile_v_posed(a.f, true, acc, Ps, pfs);
+  if (v >= m.V) return;
+  const int nkp = m.L + m.D + m.n_extra;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int b = b0 + warp * 8 + i;
+    if (b >= a.f.B) break;
+    const size_t o = ((size_t)b * m.V + v) * 3;
+    a.vp[o] = acc[i][0]; a.vp[o + 1] = acc[i][1]; a.vp[o + 2] = acc[i][2];
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    if (a.g_vertices) { g0 = a.g_vertices[o]; g1 = a.g_vertices[o + 1]; g2 = a.g_vertices[o + 2]; }
+    if (a.gkp) {
+      const int row = m.D ? a.lut[b] : -1;
+      for (int e = m.vk_ptr[v]; e < m.vk_ptr[v + 1]; ++e) {
+        const int r = m.vk_row[e];
+        if (r >= 0 && r != row) continue;
+        const float w = m.vk_w[e];
+        const float *q = a.gkp + ((size_t)b * nkp + m.vk_slot[e]) * 3;
+        g0 += w * q[0]; g1 += w * q[1]; g2 += w * q[2];
+      }
+    }
+    a.gv[o] = g0; a.gv[o + 1] = g1; a.gv[o + 2] = g2;
+    float h0 = 0.f, h1 = 0.f, h2 = 0.f;
+    for (int s = 0; s < m.ell_w_n; ++s) {
+      const float w = m.ell_w[(size_t)s * m.V + v];
+      if (w == 0.f) continue;
+      const int j = m.ell_idx[(size_t)s * m.V + v];
+      const float4 *Ab = reinterpret_cast<const float4 *>(a.f.A + ((size_t)b * m.J + j) * 12);
+      const float4 r0 = __ldg(Ab), r1 = __ldg(Ab + 1), r2 = __ldg(Ab + 2);
+      h0 += w * (r0.x * g0 + r1.x * g1 + r2.x * g2);
+      h1 += w * (r0.y * g0 + r1.y * g1 + r2.y * g2);
+      h2 += w * (r0.z * g0 + r1.z * g1 + r2.z * g2);
+    }
+    a.gvp[o] = h0; a.gvp[o + 1] = h1; a.gvp[o + 2] = h2;
+  }
+}
+
+// Skinning-transform adjoint: gA[b][j] = sum_v w_vj gv[b][v] (x) [v_posed[b][v]; 1], over the per-joint vertex list
+// built in shapy_smplx_create.  One CTA per body, one warp per joint at a time: lanes stride the list, then a fixed
+// xor tree.
+__global__ void __launch_bounds__(256) smplx_skin_bwd_kernel(SmplxDev m, const float *__restrict__ gv,
+                                                             const float *__restrict__ vp, float *__restrict__ gA) {
+  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float *gvb = gv + (size_t)b * m.V * 3, *vpb = vp + (size_t)b * m.V * 3;
+  for (int j = warp; j < m.J; j += 8) {
+    float acc[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) acc[k] = 0.f;
+    for (int e = m.jv_ptr[j] + lane; e < m.jv_ptr[j + 1]; e += 32) {
+      const int v = m.jv_idx[e];
+      const float w = m.jv_w[e];
+      const float g[3] = {w * gvb[3 * v], w * gvb[3 * v + 1], w * gvb[3 * v + 2]};
+      const float p[3] = {vpb[3 * v], vpb[3 * v + 1], vpb[3 * v + 2]};
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[r * 4 + c] += g[r] * p[c];
+        acc[r * 4 + 3] += g[r];
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 12; ++k) {
+      float v = acc[k];
+      for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      acc[k] = v;
+    }
+    if (lane < 12) {
+      float v = acc[0];
+#pragma unroll
+      for (int k = 1; k < 12; ++k) v = lane == k ? acc[k] : v;
+      gA[((size_t)b * m.J + j) * 12 + lane] = v;
+    }
+  }
+}
+
+// Pose-feature adjoint: part[b][split][k] = sum over chunk `split` of the 3V coordinates of P[k][c] gvp[b][c], k < Kp,
+// from the fp32 posedirs rows (the rows past Kp multiply exact zeros).  A SIMT GEMM with a fixed split-K: the 3V
+// coordinates are cut into kPfSplit chunks whatever B is, a CTA computes a 64-body x 64-row tile over one chunk in
+// steps of 32 coordinates (4 x 4 outputs per thread), and smplx_chain_bwd_kernel adds the chunks in order.
+constexpr int kPfSplit = 16;
+constexpr int kPfTB = 64, kPfTK = 64, kPfTC = 32;
+__global__ void __launch_bounds__(256) smplx_posefeat_bwd_kernel(const float *__restrict__ P, const float *__restrict__ gvp,
+                                                                 int V3, int Kp, int B, float *__restrict__ part) {
+  __shared__ __align__(16) float Gs[kPfTC][kPfTB + 4];
+  __shared__ float Pk[kPfTC][kPfTK + 1];
+  const int t = threadIdx.x, tb = t / 16, tk = t % 16;
+  const int k0 = blockIdx.x * kPfTK, b0 = blockIdx.y * kPfTB;
+  const int chunk = (V3 + kPfSplit - 1) / kPfSplit, c_lo = blockIdx.z * chunk, c_hi = min(V3, c_lo + chunk);
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[i][q] = 0.f;
+  for (int cb = c_lo; cb < c_hi; cb += kPfTC) {
+    for (int i = t; i < kPfTB * kPfTC; i += 256) {
+      const int bb = i / kPfTC, cc = i % kPfTC, c = cb + cc;
+      Gs[cc][bb] = (b0 + bb < B && c < c_hi) ? __ldcs(gvp + (size_t)(b0 + bb) * V3 + c) : 0.f;
+    }
+    for (int i = t; i < kPfTK * kPfTC; i += 256) {
+      const int kk = i / kPfTC, cc = i % kPfTC, c = cb + cc;
+      Pk[cc][kk] = (k0 + kk < Kp && c < c_hi) ? __ldg(P + (size_t)(k0 + kk) * V3 + c) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int cc = 0; cc < kPfTC; ++cc) {
+      const float4 g = *reinterpret_cast<const float4 *>(&Gs[cc][tb * 4]);
+      const float gg[4] = {g.x, g.y, g.z, g.w};
+      float p[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) p[q] = Pk[cc][tk + 16 * q];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[i][q] += gg[i] * p[q];
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int b = b0 + tb * 4 + i;
+    if (b >= B) break;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int k = k0 + tk + 16 * q;
+      if (k < Kp) part[((size_t)b * kPfSplit + blockIdx.z) * Kp + k] = acc[i][q];
+    }
+  }
+}
+
+// Chain backward, per body: recompute G (body_chain), seed its cotangent from A = G - [0 | G.R . J_rest] and the
+// posed joints, walk the joints in reverse topological order (one joint per step, so a parent's cotangent is summed
+// over its children in a fixed order), add the pose-feature cotangent to R[1:], and finish the coefficient gradient
+// with J_dirs^T g_J_rest.
+struct ChainBwdArgs {
+  SmplxDev m;
+  const float *betas, *expr, *rot;
+  int n_rot, Kp;
+  const float *gA, *gP, *pf_part, *gcoef;   // gP, pf_part, gcoef may be null (zero)
+  int n_gcoef;                              // rows of gcoef per body
+  float *g_rot, *g_betas, *g_expr;          // any may be null
+};
+
+__global__ void __launch_bounds__(128) smplx_chain_bwd_kernel(ChainBwdArgs a) {
+  const SmplxDev &m = a.m;
+  const int b = blockIdx.x, t = threadIdx.x;
+  __shared__ float R[kMaxJoints][9];
+  __shared__ float Jr[kMaxJoints][3];
+  __shared__ float G[kMaxJoints][12];
+  __shared__ float coef[kMaxCoef];
+  __shared__ float gG[kMaxJoints][12];
+  __shared__ float gR[kMaxJoints][9];
+  __shared__ float gJ[kMaxJoints][3];
+  const int J = m.J;
+  body_chain(m, a.betas, a.expr, a.rot, a.n_rot, b, R, Jr, G, coef);
+  const float *gAb = a.gA + (size_t)b * J * 12;
+  for (int i = t; i < J * 12; i += blockDim.x) {
+    const int j = i / 12, e = i % 12, r = e / 4, c = e % 4;
+    float g = gAb[i];
+    if (c < 3) g -= gAb[j * 12 + r * 4 + 3] * Jr[j][c];
+    else if (a.gP) g += a.gP[((size_t)b * J + j) * 3 + r];
+    gG[j][e] = g;
+  }
+  for (int i = t; i < J * 3; i += blockDim.x) {
+    const int j = i / 3, c = i % 3;
+    gJ[j][c] = -(G[j][c] * gAb[j * 12 + 3] + G[j][4 + c] * gAb[j * 12 + 7] + G[j][8 + c] * gAb[j * 12 + 11]);
+  }
+  __syncthreads();
+  for (int j = J - 1; j >= 1; --j) {
+    const int p = m.parents[j];
+    if (t < 12) {
+      const int r = t / 4, c = t % 4;
+      if (c < 3)
+        gG[p][t] += gG[j][r * 4] * R[j][c * 3] + gG[j][r * 4 + 1] * R[j][c * 3 + 1] + gG[j][r * 4 + 2] * R[j][c * 3 + 2] +
+                    gG[j][r * 4 + 3] * (Jr[j][c] - Jr[p][c]);
+      else
+        gG[p][t] += gG[j][t];
+    } else if (t < 21) {
+      const int k = (t - 12) / 3, c = (t - 12) % 3;
+      gR[j][k * 3 + c] = G[p][k] * gG[j][c] + G[p][4 + k] * gG[j][4 + c] + G[p][8 + k] * gG[j][8 + c];
+    } else if (t < 24) {
+      const int c = t - 21;
+      const float rel = G[p][c] * gG[j][3] + G[p][4 + c] * gG[j][7] + G[p][8 + c] * gG[j][11];
+      gJ[j][c] += rel;
+      gJ[p][c] -= rel;
+    }
+    __syncthreads();
+  }
+  if (t < 9) gR[0][t] = gG[0][(t / 3) * 4 + t % 3];
+  if (t < 3) gJ[0][t] += gG[0][t * 4 + 3];
+  __syncthreads();
+  if (a.g_rot) {
+    for (int i = t; i < a.n_rot * 9; i += blockDim.x) {
+      float g = gR[i / 9][i % 9];
+      const int k = i - 9;                   // pose feature (R[1:] - I), k = 9 (j - 1) + e
+      if (a.pf_part && k >= 0 && k < a.Kp)
+        for (int s = 0; s < kPfSplit; ++s) g += a.pf_part[((size_t)b * kPfSplit + s) * a.Kp + k];
+      a.g_rot[(size_t)b * a.n_rot * 9 + i] = g;
+    }
+  }
+  if (t < m.NC && (t < m.NB ? a.g_betas != nullptr : a.g_expr != nullptr)) {
+    float g = (a.gcoef && t < a.n_gcoef) ? a.gcoef[(size_t)b * a.n_gcoef + t] : 0.f;
+    for (int i = 0; i < J * 3; ++i) g += m.J_dirs[(size_t)i * m.NC + t] * gJ[i / 3][i % 3];
+    if (t < m.NB) a.g_betas[(size_t)b * m.NB + t] = g;
+    else a.g_expr[(size_t)b * m.NE + (t - m.NB)] = g;
+  }
 }
 
 }  // namespace shapy
@@ -626,6 +999,47 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
   for (int i = 0; i < s.n_over; ++i) { os[i] = (int)d->source_idxs[i]; ot[i] = (int)d->target_idxs[i]; }
   s.over_src = upload(m->allocs, os, err);
   s.over_tgt = upload(m->allocs, ot, err);
+  {
+    // backward tables: the vertices of every joint's skinning weights, ascending
+    std::vector<int> jp(1, 0), jvi;
+    std::vector<float> jvw;
+    for (int j = 0; j < J; ++j) {
+      for (int v = 0; v < V; ++v) {
+        const float w = d->lbs_weights[(size_t)v * J + j];
+        if (w != 0.f) { jvi.push_back(v); jvw.push_back(w); }
+      }
+      jp.push_back((int)jvi.size());
+    }
+    s.jv_ptr = upload(m->allocs, jp, err);
+    s.jv_idx = upload(m->allocs, jvi, err);
+    s.jv_w = upload(m->allocs, jvw, err);
+    // ... and the keypoint entries of every vertex: static landmarks, dynamic landmarks (per LUT row), J14 rows
+    std::vector<std::vector<int>> slot(V), row(V);
+    std::vector<std::vector<float>> wt(V);
+    auto add = [&](int v, int sl, int r, float w) { slot[v].push_back(sl); row[v].push_back(r); wt[v].push_back(w); };
+    for (int i = 0; i < s.L; ++i)
+      for (int c = 0; c < 3; ++c) add(lv[i * 3 + c], i, -1, d->lmk_bary_coords[i * 3 + c]);
+    for (int r = 0; r < s.rows; ++r)
+      for (int i = 0; i < s.D; ++i)
+        for (int c = 0; c < 3; ++c) {
+          const size_t o = ((size_t)r * s.D + i) * 3 + c;
+          add(dv[o], s.L + i, r, d->dynamic_lmk_bary_coords[o]);
+        }
+    for (int r = 0; r < s.n_extra; ++r)
+      for (int e = ep[r]; e < ep[r + 1]; ++e) add(ec[e], s.L + s.D + r, -1, ev[e]);
+    std::vector<int> vp(1, 0), vs, vr;
+    std::vector<float> vw;
+    for (int v = 0; v < V; ++v) {
+      vs.insert(vs.end(), slot[v].begin(), slot[v].end());
+      vr.insert(vr.end(), row[v].begin(), row[v].end());
+      vw.insert(vw.end(), wt[v].begin(), wt[v].end());
+      vp.push_back((int)vs.size());
+    }
+    s.vk_ptr = upload(m->allocs, vp, err);
+    s.vk_slot = upload(m->allocs, vs, err);
+    s.vk_row = upload(m->allocs, vr, err);
+    s.vk_w = upload(m->allocs, vw, err);
+  }
   if (err != cudaSuccess) {
     set_error("shapy_smplx_create: %s", cudaGetErrorString(err));
     shapy_smplx_destroy(m);
@@ -727,6 +1141,27 @@ extern "C" int shapy_decode_rot6d(const float *raw, int n, float *rot, void *str
   return SHAPY_OK;
 }
 
+// smplx_joints_kernel as a programmatic dependent of the vertex kernel before it
+static int launch_joints(const SmplxDev &d, const float *vertices, const float *camera, const int *lut, int B,
+                         float *joints, float *proj_joints, cudaStream_t st) {
+  JointsArgs ja{d, vertices, camera, lut, B, joints, proj_joints};
+  size_t smem = ((size_t)d.K * 3 + (size_t)std::max(d.n_extra, 1) * 3) * sizeof(float);
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(B);
+  cfg.blockDim = dim3(512);     // 16 warps: the 14 sparse J14 rows and the 68 landmarks are each one pass of dependent loads
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  SHAPY_CUDA_TRY(cudaLaunchKernelEx(&cfg, smplx_joints_kernel, ja));
+  count_launch();
+  return SHAPY_OK;
+}
+
 extern "C" int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
                                    const float *expr, const float *camera, int B, float *vertices, float *v_shaped,
                                    float *joints, float *proj_joints, void *workspace, size_t workspace_bytes,
@@ -758,23 +1193,8 @@ extern "C" int shapy_smplx_forward(const shapy_smplx_t *m, const float *betas, c
       SHAPY_LAUNCH_CHECK();
     }
   }
-  if (joints && (d.L + d.D + d.n_extra > 0 || proj_joints)) {
-    JointsArgs ja{d, vertices, camera, ws.lut, B, joints, proj_joints};
-    size_t smem = ((size_t)d.K * 3 + (size_t)std::max(d.n_extra, 1) * 3) * sizeof(float);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(B);
-    cfg.blockDim = dim3(512);     // 16 warps: the 14 sparse J14 rows and the 68 landmarks are each one pass of dependent loads
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    SHAPY_CUDA_TRY(cudaLaunchKernelEx(&cfg, smplx_joints_kernel, ja));
-    count_launch();
-  }
+  if (joints && (d.L + d.D + d.n_extra > 0 || proj_joints))
+    return launch_joints(d, vertices, camera, ws.lut, B, joints, proj_joints, st);
   return SHAPY_OK;
 }
 
@@ -809,14 +1229,146 @@ extern "C" int shapy_smplx_backward_shape(const shapy_smplx_t *m, const float *g
   const int V3 = d.V * 3;
   float *part = static_cast<float *>(workspace);
   if (d.NB == 10) {
-    smplx_shape_bwd_kernel<10><<<dim3(ceil_div(B, kShapeTile), kShapeSplit), 256, 0, st>>>(d.basis, d.V3p,
-                                                                                         grad_v_shaped, V3, B, part);
+    smplx_shape_bwd_kernel<10, 0, kShapeTile><<<dim3(ceil_div(B, kShapeTile), kShapeSplit), 256, 0, st>>>(
+        d.basis, d.V3p, grad_v_shaped, nullptr, V3, B, part);
   } else {
-    smplx_shape_bwd_kernel_generic<<<dim3(B, kShapeSplit, d.NB), 256, 0, st>>>(d.basis, d.V3p, grad_v_shaped, d.NB,
-                                                                               V3, part);
+    smplx_shape_bwd_kernel_generic<<<dim3(B, kShapeSplit, d.NB), 256, 0, st>>>(d.basis, d.V3p, grad_v_shaped, nullptr,
+                                                                               d.NB, d.NB, V3, part);
   }
   SHAPY_LAUNCH_CHECK();
   smplx_shape_bwd_sum_kernel<<<ceil_div(B * d.NB, 256), 256, 0, st>>>(part, d.NB, B, grad_betas);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" int shapy_decode_rot6d_backward(const float *raw, int n, const float *grad_rot, float *grad_raw,
+                                           void *stream) {
+  SHAPY_REQUIRE(raw && grad_rot && grad_raw && n >= 0, "shapy_decode_rot6d_backward: bad argument");
+  if (n == 0) return SHAPY_OK;
+  decode_rot6d_bwd_kernel<<<ceil_div(n, 128), 128, 0, (cudaStream_t)stream>>>(raw, n, grad_rot, grad_raw);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+// Workspace of shapy_smplx_backward: the forward's, then the backward's buffers, 256-byte aligned pieces.
+struct SmplxBwdWorkspace {
+  SmplxWorkspace f;
+  float *vp, *gv, *gvp;      // [B][V][3] v_posed, vertex cotangent (first the recomputed vertices), its pull-back
+  float *gP, *gkp, *gA;      // [B][J][3] posed-joint, [B][nkp][3] landmark / J14, [B][J][12] transform cotangents
+  float *pf_part;            // [B][kPfSplit][Kp] pose-feature adjoint partial sums
+  float *shape_part, *gcoef; // [B][kShapeSplit][NC] shape adjoint partial sums, [B][NC] their sums
+  size_t bytes;
+};
+
+static SmplxBwdWorkspace smplx_bwd_workspace(const SmplxDev &d, int B, int n_rot, void *base) {
+  SmplxBwdWorkspace w;
+  w.f = smplx_workspace(d, B, base);
+  w.bytes = w.f.bytes;
+  auto take = [&](size_t n) {
+    float *p = base ? (float *)((char *)base + w.bytes) : nullptr;
+    w.bytes += align_up(std::max<size_t>(n, 1) * sizeof(float), 256);
+    return p;
+  };
+  const size_t Bs = (size_t)B, V3 = (size_t)d.V * 3;
+  const int nkp = d.L + d.D + d.n_extra, Kp = (n_rot - 1) * 9;
+  w.vp = take(Bs * V3); w.gv = take(Bs * V3); w.gvp = take(Bs * V3);
+  w.gP = take(Bs * d.J * 3); w.gkp = take(Bs * nkp * 3); w.gA = take(Bs * d.J * 12);
+  w.pf_part = take(Bs * kPfSplit * Kp);
+  w.shape_part = take(Bs * kShapeSplit * d.NC); w.gcoef = take(Bs * d.NC);
+  return w;
+}
+
+extern "C" size_t shapy_smplx_backward_workspace_bytes(const shapy_smplx_t *m, int B, int n_rot) {
+  if (!m || B <= 0 || n_rot < 1 || n_rot > m->d.J) return 0;
+  return smplx_bwd_workspace(m->d, B, n_rot, nullptr).bytes;
+}
+
+extern "C" int shapy_smplx_backward(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
+                                    const float *expr, const float *camera, int B, const float *grad_vertices,
+                                    const float *grad_v_shaped, const float *grad_joints,
+                                    const float *grad_proj_joints, float *grad_betas, float *grad_rot,
+                                    float *grad_expr, float *grad_camera, void *workspace, size_t workspace_bytes,
+                                    void *stream) {
+  SHAPY_REQUIRE(m && betas && rot, "shapy_smplx_backward: null argument");
+  SHAPY_REQUIRE(B >= 0, "shapy_smplx_backward: batch %d", B);
+  SHAPY_REQUIRE(n_rot >= 1 && n_rot <= m->d.J, "shapy_smplx_backward: n_rot %d out of range", n_rot);
+  SHAPY_REQUIRE(!((grad_proj_joints || grad_camera) && !camera),
+                "shapy_smplx_backward: grad_proj_joints and grad_camera require camera");
+  SHAPY_REQUIRE(!(grad_expr && m->d.NE == 0), "shapy_smplx_backward: grad_expr of a model without expression basis");
+  if (B == 0) return SHAPY_OK;
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_smplx_backward_workspace_bytes(m, B, n_rot),
+                "shapy_smplx_backward: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const SmplxDev &d = m->d;
+  const SmplxBwdWorkspace ws = smplx_bwd_workspace(d, B, n_rot, workspace);
+  const int Kp = (n_rot - 1) * 9, V3 = d.V * 3;
+  const float *ex = d.NE ? expr : nullptr;
+  const bool chain = grad_betas || grad_rot || grad_expr;   // anything behind the vertices and the chain
+  const bool kp = grad_joints || grad_proj_joints;          // keypoint cotangents
+  const bool cam = grad_camera && grad_proj_joints;         // the camera gradient reads the forward joints
+  if (!chain && !grad_camera) return SHAPY_OK;
+  // ---- recompute: A, LUT rows, posed joints, pose offsets (the forward's launches, bit for bit)
+  const bool gemm = (chain || cam) && Kp > 0;
+  PoseArgs pa{d, betas, ex, rot, n_rot, B, bpad(B), Kp, pose_kpad(Kp), ws.f.A, ws.f.pfT, ws.f.joints, ws.f.lut,
+              gemm ? ws.f.x_hi : nullptr, gemm ? ws.f.x_lo : nullptr};
+  smplx_pose_kernel<<<B, 128, 0, st>>>(pa);
+  SHAPY_LAUNCH_CHECK();
+  VertexArgs va{d, betas, ex, ws.f.A, ws.f.pfT, B, bpad(B), nullptr, nullptr, nullptr, nullptr, 0};
+  if (gemm) {
+    const int rc = pose_blend_gemm(m, B, Kp, ws.f, st, va);
+    if (rc != SHAPY_OK) return rc;
+  }
+  const dim3 vgrid(ceil_div(d.V, TV), ceil_div(B, TB));
+  if (cam) {   // the forward's vertices (into gv, free until the vertex backward) and joints
+    VertexArgs vf = va;
+    vf.vertices = ws.gv;
+    smplx_vertex_kernel<<<vgrid, 128, 0, st>>>(vf);
+    SHAPY_LAUNCH_CHECK();
+    if (d.L + d.D + d.n_extra > 0) {
+      const int rc = launch_joints(d, ws.gv, nullptr, ws.f.lut, B, ws.f.joints, nullptr, st);
+      if (rc != SHAPY_OK) return rc;
+    }
+  }
+  // ---- adjoints
+  if (kp || grad_camera) {
+    JointsBwdArgs ja{d, ws.f.joints, camera, grad_joints, grad_proj_joints, chain ? ws.gP : nullptr, ws.gkp,
+                     grad_camera};
+    const size_t smem = ((size_t)d.K * 3 + (size_t)std::max(d.n_extra, 1) * 3) * sizeof(float);
+    smplx_joints_bwd_kernel<<<B, 128, smem, st>>>(ja);
+    SHAPY_LAUNCH_CHECK();
+  }
+  if (!chain) return SHAPY_OK;
+  VertexBwdArgs vb{va, grad_vertices, kp ? ws.gkp : nullptr, ws.f.lut, ws.vp, ws.gv, ws.gvp};
+  smplx_vertex_bwd_kernel<<<vgrid, 128, 0, st>>>(vb);
+  SHAPY_LAUNCH_CHECK();
+  smplx_skin_bwd_kernel<<<B, 256, 0, st>>>(d, ws.gv, ws.vp, ws.gA);
+  SHAPY_LAUNCH_CHECK();
+  const bool pf = grad_rot && Kp > 0;
+  if (pf) {
+    smplx_posefeat_bwd_kernel<<<dim3(ceil_div(Kp, kPfTK), ceil_div(B, kPfTB), kPfSplit), 256, 0, st>>>(
+        d.posedirs, ws.gvp, V3, Kp, B, ws.pf_part);
+    SHAPY_LAUNCH_CHECK();
+  }
+  int NR = 0;   // basis rows of the shape adjoint: the shape rows, and the expression rows when their gradient is wanted
+  if (grad_betas || grad_expr) {
+    NR = grad_expr ? d.NC : d.NB;
+    if (d.NB == 10 && NR == 10) {
+      smplx_shape_bwd_kernel<10, 0, kShapeTile><<<dim3(ceil_div(B, kShapeTile), kShapeSplit), 256, 0, st>>>(
+          d.basis, d.V3p, ws.gvp, grad_v_shaped, V3, B, ws.shape_part);
+    } else if (d.NB == 10 && NR == 20) {
+      smplx_shape_bwd_kernel<10, 10, 4><<<dim3(ceil_div(B, 4), kShapeSplit), 256, 0, st>>>(
+          d.basis, d.V3p, ws.gvp, grad_v_shaped, V3, B, ws.shape_part);
+    } else {
+      smplx_shape_bwd_kernel_generic<<<dim3(B, kShapeSplit, NR), 256, 0, st>>>(d.basis, d.V3p, ws.gvp, grad_v_shaped,
+                                                                               d.NB, NR, V3, ws.shape_part);
+    }
+    SHAPY_LAUNCH_CHECK();
+    smplx_shape_bwd_sum_kernel<<<ceil_div(B * NR, 256), 256, 0, st>>>(ws.shape_part, NR, B, ws.gcoef);
+    SHAPY_LAUNCH_CHECK();
+  }
+  ChainBwdArgs ca{d, betas, ex, rot, n_rot, Kp, ws.gA, kp ? ws.gP : nullptr, pf ? ws.pf_part : nullptr,
+                  NR ? ws.gcoef : nullptr, NR, grad_rot, grad_betas, grad_expr};
+  smplx_chain_bwd_kernel<<<B, 128, 0, st>>>(ca);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

@@ -28,6 +28,14 @@ struct SmplxDev {
   int *ex_ptr, *ex_col;
   float *ex_val;
   int *over_src, *over_tgt;
+  // backward only: per-joint skinning lists (CSR over joints, vertices ascending) for the skinning-transform adjoint,
+  // and per-vertex keypoint entries (CSR over vertices) that gather the landmark and J14 cotangents onto a vertex;
+  // an entry's slot indexes [static landmarks | dynamic landmarks | J14 rows], row >= 0 only for a dynamic landmark
+  // of that LUT row
+  int *jv_ptr, *jv_idx;
+  float *jv_w;
+  int *vk_ptr, *vk_slot, *vk_row;
+  float *vk_w;
 };
 
 }  // namespace shapy

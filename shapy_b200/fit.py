@@ -1,7 +1,8 @@
-"""Batched fitting of SMPL-X betas to virtual measurements on the device.
+"""Batched fitting of SMPL-X bodies on the device: betas to virtual measurements, and pose and shape to 3D keypoints.
 
-    from shapy_b200.fit import fit_betas_to_measurements
+    from shapy_b200.fit import fit_betas_to_measurements, fit_body_to_keypoints
     res = fit_betas_to_measurements(body_model, body_measurements, {'height': h, 'mass': m, ...})   # (B,) targets
+    res = fit_body_to_keypoints(body_model, keypoints)                                             # (B, K, 3)
 
     python -m shapy_b200.fit --synthetic --height 1.80 --mass 80 --output fit.npz
     python -m shapy_b200.fit --model-folder models/smplx --targets targets.npz --output fit.npz
@@ -13,6 +14,11 @@ through SMPLX.forward_shape -> BodyMeasurements.forward_vertices, both different
 whole batch is optimised at once with Adam: Adam is elementwise, so every body's trajectory is independent of the
 rest of the batch (the reference's L-BFGS / TrustRegion would couple them through the line search and needs a double
 backward, which is not supported).
+
+fit_body_to_keypoints optimises the raw 6D global and body pose (through the 6D decoder), betas and transl of every
+body against its K 3D keypoints (the model's joints output: posed joints, landmarks, J14 overwrite), loss per body
+sum_k w_k |joint_k - keypoint_k|^2, with the same batched Adam: SMPLX.forward and the decoder are differentiable
+(shapy_b200.autograd), and a body's gradient does not depend on the rest of the batch.
 """
 import argparse
 import json
@@ -79,6 +85,58 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     with torch.no_grad():
         per_body, meas = loss_fn(betas)
     return {'betas': betas.detach(), 'measurements': meas, 'loss': per_body}
+
+
+IDENT6 = (1.0, 0.0, 0.0, 1.0, 0.0, 0.0)      # the 6D code of the identity rotation (row-major 3x2)
+
+
+def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=600, lr=0.05, init=None):
+    """Fits pose and shape so that the model's keypoints match `keypoints` (B, K, 3), K = body_model's keypoint count.
+
+    weights: None (all 1), (K,) or (B, K) per-keypoint weights.  init: optional {'global_rot': (B, 6),
+    'body_pose': (B, 126) raw 6D, 'betas': (B, NB), 'transl': (B, 3)}; a missing entry starts at the identity pose,
+    zero betas or zero transl.  Adam with the step size decaying geometrically from lr to lr / 100.
+    Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (B, 1, 3, 3),
+    'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss}."""
+    from .autograd import Rot6dFunction
+    device = body_model.shapedirs.device
+    kp = torch.as_tensor(keypoints, dtype=torch.float32, device=device)
+    B, K = kp.shape[0], kp.shape[1]
+    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
+                                                                             device=device)
+    w = w.expand(B, K).contiguous()
+    init = init or {}
+    ident = torch.tensor(IDENT6, device=device)
+    start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
+             'betas': torch.zeros(B, body_model.num_betas, device=device), 'transl': torch.zeros(B, 3, device=device)}
+    params = {}
+    for k, v in start.items():
+        t = init.get(k)
+        t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
+        params[k] = t.detach().clone().contiguous().requires_grad_(True)
+    opt = torch.optim.Adam(list(params.values()), lr=lr)
+    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
+                         return_shaped=False)
+        joints = out['joints'][:]                  # the KeypointTensor's tensor, still in the graph
+        per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
+        return per_body, joints, grot, bpose
+
+    for _ in range(int(iterations)):
+        opt.zero_grad(set_to_none=True)
+        per_body = loss_fn()[0]
+        per_body.sum().backward()
+        opt.step()
+        sched.step()
+    with torch.no_grad():
+        per_body, joints, grot, bpose = loss_fn()
+    res = {k: v.detach() for k, v in params.items()}
+    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, loss=per_body)
+    return res
 
 
 def main(argv=None):

@@ -5,7 +5,8 @@ Same buffer names (v_template, shapedirs, posedirs, J_regressor, lbs_weights, pa
 expr_dirs, lmk_*, dynamic_lmk_*, neck_kin_chain, extra_joint_regressor, source_idxs, target_idxs,
 head_vertices_ids) so `model.*` checkpoint entries load; the buffers are the source of truth and the
 packed device-side model (shapy_smplx_create) is rebuilt lazily after load_state_dict / .to() / deepcopy.
-The forward pass is three launches of csrc/smplx.cu; there is no PyTorch fallback.
+The forward pass is three launches of csrc/smplx.cu; there is no PyTorch fallback.  forward and forward_shape are
+differentiable (shapy_b200.autograd) when grad mode is on and an input requires grad.
 """
 import os.path as osp
 import pickle
@@ -242,8 +243,14 @@ class SMPLX(nn.Module):
         for i, (p, n) in enumerate(extra[:last + 1]):
             parts.append(p.reshape(bs, n, 3, 3) if p is not None else eye.expand(bs, n, -1, -1))
         rot = torch.cat([p.to(torch.float32) for p in parts], dim=1).contiguous()
-        out = _ops.smplx_forward(self.packed(device), betas, rot, expr=expression, camera=camera,
-                                 want_vertices=True, want_v_shaped=return_shaped, want_joints=True)
+        if any(_ag.wants_grad(t) for t in (betas, rot, expression, camera)):
+            # differentiable in betas, expression, the rotations and camera (shapy_b200.autograd); transl below is a
+            # torch add either way
+            v, vs, j, pj = _ag.SmplxFunction.apply(self.packed(device), betas, rot, expression, camera, return_shaped)
+            out = dict(vertices=v, v_shaped=vs, joints=j, proj_joints=pj)
+        else:
+            out = _ops.smplx_forward(self.packed(device), betas, rot, expr=expression, camera=camera,
+                                     want_vertices=True, want_v_shaped=return_shaped, want_joints=True)
         vertices, joints = out['vertices'], out['joints']
         if transl is not None:
             joints += transl.unsqueeze(dim=1)

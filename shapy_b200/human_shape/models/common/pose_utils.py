@@ -6,6 +6,7 @@ from dataclasses import dataclass
 import torch
 import torch.nn as nn
 
+from .... import autograd as _ag
 from .... import ops as _ops
 
 
@@ -53,6 +54,9 @@ class ContinuousRotReprDecoder(nn.Module):
         return self.mean.clone()
 
     def forward(self, module_input):
+        """Differentiable (shapy_b200.autograd.Rot6dFunction) when grad mode is on and the input requires grad."""
+        if _ag.wants_grad(module_input):
+            return _ag.Rot6dFunction.apply(module_input)
         return _ops.decode_rot6d(module_input)
 
 

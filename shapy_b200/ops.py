@@ -160,6 +160,64 @@ def smplx_forward_shape(model: SmplxModel, betas) -> torch.Tensor:
     return out
 
 
+def decode_rot6d_backward(raw: torch.Tensor, grad_rot: torch.Tensor) -> torch.Tensor:
+    """Gradient of decode_rot6d with respect to raw (B, 6n), from grad_rot (B, n, 3, 3)."""
+    raw = _cuda_f32(raw, 'raw')
+    g = _cuda_f32(grad_rot, 'grad_rot')
+    n = raw.numel() // 6
+    if g.numel() != 9 * n:
+        raise RuntimeError(f'grad_rot has {g.numel()} values for {n} rotations')
+    out = torch.empty_like(raw)
+    if n == 0:
+        return out
+    with torch.cuda.device(raw.device):
+        check(lib().shapy_decode_rot6d_backward(ptr(raw), n, ptr(g), ptr(out), stream_ptr()), 'decode_rot6d_backward')
+    return out
+
+
+def smplx_backward(model: SmplxModel, betas, rot, expr=None, camera=None, grad_vertices=None, grad_v_shaped=None,
+                   grad_joints=None, grad_proj_joints=None, want=('betas', 'rot', 'expr', 'camera')):
+    """Adjoint of smplx_forward (include/shapy_b200.h, shapy_smplx_backward).  A cotangent left None is zero; `want`
+    names the gradients to compute.  Returns {'betas', 'rot', 'expr', 'camera'}, None where not wanted (and for expr /
+    camera when the model has no expression basis / no camera was given)."""
+    betas = _cuda_f32(betas, 'betas')
+    rot = _cuda_f32(rot, 'rot')
+    B, n_rot = rot.shape[0], rot.shape[1]
+    if betas.shape != (B, model.NB):
+        raise RuntimeError(f'betas must be ({B}, {model.NB}), got {tuple(betas.shape)}')
+    dev = betas.device
+    expr = None if expr is None else _cuda_f32(expr, 'expression')
+    camera = None if camera is None else _cuda_f32(camera, 'camera')
+    shapes = dict(grad_vertices=(B, model.V, 3), grad_v_shaped=(B, model.V, 3), grad_joints=(B, model.K, 3),
+                  grad_proj_joints=(B, model.K, 2))
+    gs = {}
+    for name, g in (('grad_vertices', grad_vertices), ('grad_v_shaped', grad_v_shaped), ('grad_joints', grad_joints),
+                    ('grad_proj_joints', grad_proj_joints)):
+        if g is not None:
+            g = _cuda_f32(g, name)
+            if tuple(g.shape) != shapes[name]:
+                raise RuntimeError(f'{name} must be {shapes[name]}, got {tuple(g.shape)}')
+        gs[name] = g
+    if camera is None:
+        gs['grad_proj_joints'] = None
+    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+    out = dict(betas=mk(B, model.NB) if 'betas' in want else None,
+               rot=mk(B, n_rot, 3, 3) if 'rot' in want else None,
+               expr=mk(B, model.NE) if ('expr' in want and model.NE) else None,
+               camera=mk(B, 3) if ('camera' in want and camera is not None) else None)
+    if B == 0:
+        return out
+    with torch.cuda.device(dev):
+        nbytes = lib().shapy_smplx_backward_workspace_bytes(model.handle, B, n_rot)
+        ws = _WS.get('smplx_bwd', nbytes, dev)
+        check(lib().shapy_smplx_backward(model.handle, ptr(betas), ptr(rot), n_rot, ptr(expr), ptr(camera), B,
+                                         ptr(gs['grad_vertices']), ptr(gs['grad_v_shaped']), ptr(gs['grad_joints']),
+                                         ptr(gs['grad_proj_joints']), ptr(out['betas']), ptr(out['rot']),
+                                         ptr(out['expr']), ptr(out['camera']), ptr(ws), ws.numel(), stream_ptr()),
+              'smplx_backward')
+    return out
+
+
 # ------------------------------------------------------------------------------------ measurements
 def make_landmarks(lm: dict) -> _lib.MeasureLandmarks:
     """lm: {'head_top','left_heel','chest','waist','hips'} -> {'face_idx', 'bc'}."""

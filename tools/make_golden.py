@@ -25,6 +25,9 @@ Everything written here is a small fixture that travels to the GPU box, where
                         end to end through a seeded dense J14 regressor
   ref_smplx_live.npz    reference SMPL-X forward (ref_shim) of tests/test_oracle_pins.py's seeded bodies
   ref_smplx_full.npz    reference SMPL-X forward in float64 with every pose part, expression and transl (float64)
+  ref_smplx_grad.npz    gradients of the reference's SMPL-X forward (ref_shim.smplx_forward_ref, its own lbs() under autograd)
+                        in float64 with respect to betas, expression, every pose rotation, transl and camera, for
+                        closed-form cotangents on vertices, joints, v_shaped and proj_joints (grad_pattern)
   ref_weak_persp_to_blender.npz   reference demo.py weak_persp_to_blender on tests/test_writer_cpu.py's inputs
   ref_keypoint_tensor.{npz,json}  reference KeypointTensor under the tensor methods of tests/test_keypoint_tensor_cpu.py
   ref_mmi_{plane,soup}.npz        reference mesh_to_mesh_forward (oracle/_ref via oracle/run_ref_mmi.py) collisions on
@@ -415,6 +418,60 @@ def smplx_full_fixture():
     print('ref_smplx_full.npz', os.path.getsize(os.path.join(G, 'ref_smplx_full.npz')), 'bytes')
 
 
+# cotangent name -> (frequency, phase, amplitude): g.flat[i] = amplitude * sin(frequency * i + phase), float64
+GRAD_PATTERN = {'vertices': (0.731, 0.1, 1.0), 'joints': (1.913, 0.7, 1.0), 'v_shaped': (0.377, 1.9, 0.5),
+                'proj_joints': (2.71, 0.3, 1.0)}
+
+
+def grad_pattern(name, shape):
+    f, ph, amp = GRAD_PATTERN[name]
+    return amp * np.sin(f * np.arange(int(np.prod(shape)), dtype=np.float64) + ph).reshape(shape)
+
+
+def smplx_grad_fixture():
+    """Gradients of the reference's SMPL-X forward under its own autograd (ref_shim.smplx_forward_ref on the verbatim
+    lbs(), pose2rot=False) in float64 on the float64 synthetic model, for the loss
+    <g_v, vertices> + <g_j, joints> + <g_s, v_shaped> + <g_p, proj_joints> with the closed-form cotangents of
+    grad_pattern.  The bodies are smplx_full_fixture's (every pose part, expression, transl, the neck past both ends
+    of the LUT) plus a camera.  transl is added to vertices and joints after the forward and proj_joints projects the
+    joints before transl, as shapy_b200's SMPLX.forward does; proj = softplus(c0) (xy + c[1:3])
+    (camera_projection.py:181-213)."""
+    from shapy_b200 import synth
+    ref = ref_shim.load()
+    dt = torch.float64
+    model = synth.make_smplx(dtype=dt)
+    g = torch.Generator().manual_seed(21)
+    B = 4
+    betas = torch.randn(B, 10, generator=g, dtype=dt)
+    expression = torch.randn(B, 10, generator=g, dtype=dt)
+    transl = torch.randn(B, 3, generator=g, dtype=dt) * 0.5
+    aa = torch.randn(B, 55, 3, generator=g, dtype=dt) * 0.3
+    aa[:2, [0, 3, 6, 9, 15]] *= 0.1
+    aa[0, 12] = torch.tensor([0.0, 1.2, 0.0], dtype=dt)
+    aa[1, 12] = torch.tensor([0.0, -1.2, 0.0], dtype=dt)
+    rot = ref.rot.batch_rodrigues(aa.reshape(-1, 3)).reshape(B, 55, 3, 3)
+    camera = torch.tensor([[0.9, 0.05, -0.1], [-1.5, 0.2, 0.1], [21.0, -0.3, 0.2], [2.0, 0.0, 0.4]], dtype=dt)
+    leaves = dict(betas=betas, expression=expression, transl=transl, rot=rot, camera=camera)
+    leaves = {k: v.detach().clone().requires_grad_(True) for k, v in leaves.items()}
+    r = leaves['rot']
+    out = ref_shim.smplx_forward_ref(model, leaves['betas'], r[:, :1], r[:, 1:22], jaw_pose=r[:, 22:23],
+                                     leye_pose=r[:, 23:24], reye_pose=r[:, 24:25], left_hand_pose=r[:, 25:40],
+                                     right_hand_pose=r[:, 40:55], expression=leaves['expression'])
+    t = leaves['transl'].unsqueeze(1)
+    vertices, joints = out['vertices'] + t, out['joints'] + t
+    cam = leaves['camera']
+    proj = torch.nn.functional.softplus(cam[:, 0]).view(-1, 1, 1) * (out['joints'][:, :, :2] + cam[:, 1:3].view(-1, 1, 2))
+    loss = 0
+    for name, y in (('vertices', vertices), ('joints', joints), ('v_shaped', out['v_shaped']), ('proj_joints', proj)):
+        loss = loss + (torch.from_numpy(grad_pattern(name, tuple(y.shape))) * y).sum()
+    loss.backward()
+    np.savez_compressed(
+        os.path.join(G, 'ref_smplx_grad.npz'), **{k: v.detach().numpy() for k, v in leaves.items()},
+        **{f'grad_{k}': v.grad.numpy() for k, v in leaves.items()},
+        pattern_names=np.array(list(GRAD_PATTERN)), pattern=np.array(list(GRAD_PATTERN.values())))
+    print('ref_smplx_grad.npz', os.path.getsize(os.path.join(G, 'ref_smplx_grad.npz')), 'bytes')
+
+
 def writer_camera_fixture():
     import ast
     from collections import defaultdict
@@ -506,7 +563,7 @@ def measure_grad_fixture():
 
 if __name__ == '__main__':
     which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
-                             'smplx_full', 'camera', 'keypoint', 'measure_grad']
+                             'smplx_full', 'camera', 'keypoint', 'measure_grad', 'smplx_grad']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -530,6 +587,8 @@ if __name__ == '__main__':
         smplx_live_fixture()
     if 'smplx_full' in which:
         smplx_full_fixture()
+    if 'smplx_grad' in which:
+        smplx_grad_fixture()
     if 'camera' in which:
         writer_camera_fixture()
     if 'keypoint' in which:
