@@ -173,6 +173,34 @@ int shapy_measure_backward_tris(const float *triangles, int batch, int num_faces
                                 const shapy_measure_landmarks_t *lm, const float *grad_out,
                                 float *grad_triangles, void *stream);
 
+/* The measurements of shapy_measure_forward and their Jacobian with respect to betas, in one launch:
+ * out (B,5) bit-identical to shapy_measure_forward on the same v_shaped (NaNs included), jac (B,5,NB) device fp32,
+ * row k = shapedirs^T . (the gradient shapy_measure_backward gives for the cotangent e_k), with its semantics (constant
+ * barycentrics, no gradient through the plane heights, sign(0) = 0).  Faces, V and NB come from the model; v_shaped
+ * (B,V,3), 16-byte aligned, need not come from shapy_smplx_forward_shape.  inc_ptr / inc: the incidence table of the model's faces, as
+ * for shapy_measure_backward.  A NaN circumference makes its row NaN, the other rows stay finite; an inconsistent
+ * hull walk makes the body's five rows NaN.  status as in shapy_measure_forward.  No atomics touch out or jac: a
+ * body's result is bit-identical from run to run and independent of the rest of the batch.  1 <= NB <= 16, else
+ * SHAPY_ERR_UNSUPPORTED. */
+int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float *v_shaped, const int32_t *inc_ptr,
+                                 const int32_t *inc, int batch, const shapy_measure_landmarks_t *lm,
+                                 float *out, float *jac, int32_t *status, void *stream);
+
+/* One Levenberg-Marquardt step per body of the fit of betas to the five measurements, one warp per body.  Loss
+ * L = sum_{w_k > 0} w_k (t_k - m_k)^2 + betas_weight |beta|^2; a term with weight 0 is skipped (its measurement and
+ * Jacobian row may be NaN).  targets, weights (B,5); the state betas (B,NB), meas (B,5), jac (B,5,NB), loss (B),
+ * lambda (B), accepted (B, a count); trial (B,NB) is the point whose trial_meas (B,5) / trial_jac (B,5,NB) were
+ * evaluated, and receives the next trial.  With `first` the trial becomes the state and lambda = 1e-3 max(diag
+ * (J^T W J), 1e-6); otherwise a finite trial loss below the state's is accepted (state := trial, lambda /= lambda_down,
+ * accepted += 1) and any other rejected (lambda *= lambda_up).  lambda is clamped to [1e-9, 1e9].  The next trial is
+ * beta + delta, (J^T W J + (betas_weight + lambda) I) delta = -(J^T W (m - t) + betas_weight beta), by Cholesky in
+ * fp64; a body whose loss is not finite, or whose factorisation fails, gets its state as the trial.  A non-finite
+ * starting loss is reported as NaN.  Deterministic, no atomics, per-body independent.  1 <= NB <= 16. */
+int shapy_fit_lm_step(int batch, int nb, const float *targets, const float *weights, float betas_weight,
+                      float lambda_up, float lambda_down, int first, float *betas, float *meas, float *jac,
+                      float *loss, float *lambda, int32_t *accepted, float *trial, const float *trial_meas,
+                      const float *trial_jac, void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

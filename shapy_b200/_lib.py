@@ -79,6 +79,10 @@ _SIGS = {
                                        C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,
                                             c_void_p]),
+    'shapy_measure_jacobian_betas': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, C.POINTER(MeasureLandmarks),
+                                             c_void_p, c_void_p, c_void_p, c_void_p]),
+    'shapy_fit_lm_step': (c_int, [c_int, c_int, c_void_p, c_void_p, C.c_float, C.c_float, C.c_float, c_int]
+                          + [c_void_p] * 9 + [c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

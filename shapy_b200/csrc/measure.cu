@@ -49,8 +49,13 @@
 // gradient do not depend on timing either.  No float atomics touch the output: the dense mass term of a vertex (a
 // face corner) is summed over its incident faces in a fixed order, then the hull and height terms are added in a
 // fixed order, so a body's gradient is bit-identical from run to run and independent of the rest of the batch.
-#include "common.cuh"
+//
+// measure_smem_kernel<SRC, kJacobian> (shapy_measure_jacobian_betas, vertex sources only) reruns the same phases 0-3,
+// writes the forward's five outputs and then, in its own phase 4, jac (B,5,NB): row k is S^T times the gradient the
+// backward gives for the cotangent e_k, S the model's shape rows -- the mass row densely over the vertices, the height
+// row from the two landmark faces, each circumference row from its hull vertices only (see DESIGN.md section 4).
 #include "mmi_device.cuh"
+#include "smplx.cuh"
 
 namespace shapy {
 
@@ -64,12 +69,17 @@ constexpr size_t kListBytes = 3 * kMaxPts * 12 + kMaxCand * 4;   // points + can
 constexpr size_t kGradBytes = 3 * kMaxPts * 4 + 3 * kMaxPts * 2;
 
 enum TriSource { kStagedVerts, kGlobalVerts, kTriangles };
+enum MeasureMode { kForward, kGradient, kJacobian };
+constexpr int kMaxJacBetas = 16;   // shape rows of the Jacobian mode
 
 struct MeasureGrad {
   const float *gout;   // (B,5) upstream gradient
   const int *inc_ptr;  // (V+1) CSR: vertex -> incident (face, corner) entries 3 f + k, stably sorted (vertex sources)
   const int *inc;      // (3F)
   float *grad;         // (B,V,3) or (B,F,3,3)
+  const float *S;      // Jacobian mode: the shape rows of the model's basis, [nb][ld]
+  int ld, nb;
+  float *jac;          // Jacobian mode: (B,5,nb)
 };
 
 struct MeasureArgs {
@@ -142,9 +152,11 @@ __device__ __forceinline__ float3 corner_cross(const mmi::Tri &T, int k) {
 
 __device__ __forceinline__ float sign_of(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : (x == 0.f ? 0.f : x)); }
 
-// GRAD = false: the forward; GRAD = true: the backward, see the top.
-template <int SRC, bool GRAD = false>
+// MODE kForward: the forward; kGradient: the backward; kJacobian: the forward's outputs and their Jacobian with
+// respect to betas, see the top.
+template <int SRC, int MODE = kForward>
 __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a) {
+  constexpr bool GRAD = MODE != kForward;    // phases 0-3 keep the point codes and the hull walk
   extern __shared__ __align__(16) unsigned char smem[];
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int nvf = a.V * 3;
@@ -269,7 +281,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     }
   }
   __syncthreads();     // the candidate queue is dead from here on: its storage becomes the chain lists
-  if (!GRAD && t == 0) {
+  if (MODE != kGradient && t == 0) {
     float v = 0.f;
     for (int i = 0; i < kThreads / 32; ++i) v += red[i];
     a.out[(size_t)b * 5 + 0] = fabsf(v) / 6.0f * 985.0f;
@@ -392,11 +404,12 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     if (cnt[p] < 3 || edges < 3) perim = __int_as_float(0x7fc00000);
     if ((overflow & (1 << p))) perim = __int_as_float(0x7fc00000);   // truncated point set
     if constexpr (GRAD) perim_s[p] = perim;
-    else a.out[(size_t)b * 5 + 2 + p] = perim;
+    if constexpr (MODE != kGradient) a.out[(size_t)b * 5 + 2 + p] = perim;
   }
-  if constexpr (!GRAD) {
+  if constexpr (MODE != kGradient) {
     if (t == 0 && overflow && a.status) atomicExch(a.status, 1);
-  } else {
+  }
+  if constexpr (MODE == kGradient) {
     // ---- phase 4: gradient.  The chain lists are dead: their storage holds the hull vertex list of each plane
     // (hull[p][j] = start slot of the j-th edge, chains in order) and then a bitmap of the faces that carry a hull point.
     unsigned short *hull = clist;                                                   // [3][kMaxPts]
@@ -512,6 +525,130 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       }
     }
   }
+  if constexpr (MODE == kJacobian && SRC != kTriangles) {
+    // ---- phase 4 (Jacobian): row k of jac is S^T times the gradient the backward gives for the cotangent e_k, S the
+    // nb shape rows of the basis.  The points' storage takes the hull vertex vectors u_in - u_out (the backward's with
+    // g = 1), the chain lists the hull vertex list, as in the gradient mode.
+    unsigned short *hull = clist;                                                   // [3][kMaxPts]
+    __shared__ float sc[2];           // mass scale, height scale
+    __shared__ int nedge[3], rownan[3], poison;
+    __shared__ float jred[kThreads / 32][kMaxJacBetas];
+    const MeasureGrad &g = a.g;
+    const int nb = g.nb;
+    if (t == 0) {
+      float v = 0.f;
+      for (int i = 0; i < kThreads / 32; ++i) v += red[i];                          // the forward's volume, same order
+      sc[0] = sign_of(v) * (985.0f / 6.0f);
+      sc[1] = sign_of(lmy[0] - lmy[1]);
+      for (int p = 0; p < 3; ++p) {
+        int m = 0;
+        for (int k = 0; k < 8; ++k) m += chain_edges[p][k];
+        rownan[p] = isnan(perim_s[p]) || m > kMaxPts;
+        nedge[p] = rownan[p] ? 0 : m;
+      }
+      poison = 0;
+    }
+    if (warp < 24 && lane == 0) {
+      int off = 0, m = 0;
+      for (int k = 0; k < 8; ++k) { off += k < hk ? chain_edges[hp][k] : 0; m += chain_edges[hp][k]; }
+      int cur = ext[hp][hk].idx;
+      if (m <= kMaxPts)
+        for (int s = 0; s < chain_edges[hp][hk]; ++s) { hull[hp * kMaxPts + off + s] = (unsigned short)cur; cur = nxt[hp * kMaxPts + cur]; }
+    }
+    __syncthreads();
+    float3 val[3];
+    for (int it = 0; it < 3; ++it) {
+      val[it] = make_float3(0.f, 0.f, 0.f);
+      const int r = t + it * kThreads, p = r / kMaxPts, j = r % kMaxPts, m = nedge[p];
+      if (j >= m) continue;
+      const float *P = pts + (size_t)p * kMaxPts * 3;
+      const unsigned short *H = hull + p * kMaxPts;
+      const int cur = H[j], prev = H[(j + m - 1) % m], next = nxt[p * kMaxPts + cur];
+      if (nxt[p * kMaxPts + prev] != cur || next != H[(j + 1) % m]) { poison = 1; continue; }
+      const float ix = P[3 * cur] - P[3 * prev], iy = P[3 * cur + 1] - P[3 * prev + 1], iz = P[3 * cur + 2] - P[3 * prev + 2];
+      const float ox = P[3 * next] - P[3 * cur], oy = P[3 * next + 1] - P[3 * cur + 1], oz = P[3 * next + 2] - P[3 * cur + 2];
+      const float li = sqrtf(ix * ix + iy * iy + iz * iz), lo = sqrtf(ox * ox + oy * oy + oz * oz);
+      val[it] = make_float3(ix / li - ox / lo, iy / li - oy / lo, iz / li - oz / lo);
+    }
+    __syncthreads();                  // the points are dead: their storage takes the hull vertex vectors
+    for (int it = 0; it < 3; ++it) {
+      const int r = t + it * kThreads;
+      if (r % kMaxPts < nedge[r / kMaxPts]) {
+        pts[3 * r] = val[it].x; pts[3 * r + 1] = val[it].y; pts[3 * r + 2] = val[it].z;
+      }
+    }
+    // mass row: sum over the vertices of (sum of the incident corner_cross, in CSR order) . S[l][v], one thread per
+    // vertex at a time, then a fixed xor tree per warp and the warps in order
+    float part[kMaxJacBetas];
+#pragma unroll
+    for (int l = 0; l < kMaxJacBetas; ++l) part[l] = 0.f;
+    for (int v = t; v < a.V; v += kThreads) {
+      const int e0 = __ldg(g.inc_ptr + v), e1 = __ldg(g.inc_ptr + v + 1);
+      float3 c = make_float3(0.f, 0.f, 0.f);
+      for (int e = e0; e < e1; ++e) {
+        const int fk = __ldg(g.inc + e);
+        const float3 d = corner_cross(tri_of(fk / 3), fk % 3);
+        c.x += d.x; c.y += d.y; c.z += d.z;
+      }
+      const float *Sv = g.S + 3 * (size_t)v;
+#pragma unroll
+      for (int l = 0; l < kMaxJacBetas; ++l)
+        if (l < nb) {
+          const float *s = Sv + (size_t)l * g.ld;
+          part[l] += c.x * __ldg(s) + c.y * __ldg(s + 1) + c.z * __ldg(s + 2);
+        }
+    }
+#pragma unroll
+    for (int l = 0; l < kMaxJacBetas; ++l) {
+      if (l < nb) {
+        float x = part[l];
+        for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+        if (lane == 0) jred[warp][l] = x;
+      }
+    }
+    __syncthreads();
+    const float nan = __int_as_float(0x7fc00000);
+    const bool bad = poison != 0;
+    float *J = g.jac + (size_t)b * 5 * nb;
+    if (t < nb) {
+      const int l = t;
+      float s = 0.f;
+      for (int w = 0; w < kThreads / 32; ++w) s += jred[w][l];
+      J[l] = bad ? nan : sc[0] * s;
+      // height row: the y components of the two landmark faces' corners
+      const float *Sl = g.S + (size_t)l * g.ld + 1;
+      float h = 0.f;
+      for (int k = 0; k < 3; ++k) h += a.lm.bc[0][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[0] + k]);
+      for (int k = 0; k < 3; ++k) h -= a.lm.bc[1][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[1] + k]);
+      J[nb + l] = bad ? nan : sc[1] * h;
+    }
+    // circumference rows: warp (plane p, row l); lane i takes the hull vertices j = i mod 32, the bc-weighted sum over
+    // its face's corners of (u_in - u_out) . S[l][corner] (the bc phase 2 used, recomputed from the (face, query half)
+    // code), and the warp adds them in hull order
+    for (int r = warp; r < 3 * nb; r += kThreads / 32) {
+      const int p = r / nb, l = r % nb, m = nedge[p];
+      const float *Sl = g.S + (size_t)l * g.ld;
+      float acc = 0.f;
+      for (int base = 0; base < m; base += 32) {
+        const int j = base + lane;
+        float c = 0.f;
+        if (j < m) {
+          const int code = codes[p * kMaxPts + hull[p * kMaxPts + j]], f = code >> 1;
+          float3 b1 = make_float3(0, 0, 0), b2 = b1;
+          mmi::isect_points(quad(hs[p], code & 1), tri_of(f), b1, b2);
+          const float *gv = pts + 3 * (p * kMaxPts + j);
+          for (int k = 0; k < 3; ++k) {
+            const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+            const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
+            c += w * (gv[0] * __ldg(s) + gv[1] * __ldg(s + 1) + gv[2] * __ldg(s + 2));
+          }
+        }
+        const int nj = min(32, m - base);
+        for (int i = 0; i < nj; ++i) acc += __shfl_sync(0xffffffffu, c, i);
+      }
+      if (lane == 0) J[(size_t)(2 + p) * nb + l] = (bad || rownan[p]) ? nan : acc;
+    }
+  }
 }
 
 size_t measure_smem_bytes(int V) { return (((size_t)V * 12 + 15) & ~(size_t)15) + kListBytes; }
@@ -525,11 +662,11 @@ static int launch_source(const MeasureArgs &a, size_t smem, int max_smem, cudaSt
   return SHAPY_OK;
 }
 
-template <int SRC>
+template <int SRC, int MODE>
 static int launch_grad_source(const MeasureArgs &a, size_t smem, int max_smem, cudaStream_t stream) {
   static std::atomic<unsigned long long> attr_done{0};
-  SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC, true>, max_smem, attr_done));
-  measure_smem_kernel<SRC, true><<<a.B, kThreads, smem, stream>>>(a);
+  SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC, MODE>, max_smem, attr_done));
+  measure_smem_kernel<SRC, MODE><<<a.B, kThreads, smem, stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
@@ -576,11 +713,11 @@ static int launch_measure_grad(const MeasureArgs &a, void *stream) {
     SHAPY_REQUIRE(a.lm.face_idx[i] >= 0 && a.lm.face_idx[i] < a.F, "landmark face %d out of range", a.lm.face_idx[i]);
   cudaStream_t s = (cudaStream_t)stream;
   const size_t list = kListBytes + kGradBytes;
-  if (a.tris) return launch_grad_source<kTriangles>(a, list, (int)list, s);
+  if (a.tris) return launch_grad_source<kTriangles, kGradient>(a, list, (int)list, s);
   SHAPY_REQUIRE(g.inc_ptr && g.inc && a.V > 0, "shapy_measure_backward: null incidence table");
   const size_t staged = measure_smem_bytes(a.V) + kGradBytes;
-  if (a.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts>(a, staged, 226 * 1024, s);
-  return launch_grad_source<kGlobalVerts>(a, list, (int)list, s);
+  if (a.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts, kGradient>(a, staged, 226 * 1024, s);
+  return launch_grad_source<kGlobalVerts, kGradient>(a, list, (int)list, s);
 }
 
 extern "C" int shapy_measure_backward(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
@@ -600,4 +737,27 @@ extern "C" int shapy_measure_backward_tris(const float *triangles, int batch, in
   MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
                 MeasureGrad{grad_out, nullptr, nullptr, grad_triangles}};
   return launch_measure_grad(a, stream);
+}
+
+extern "C" int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float *v_shaped, const int32_t *inc_ptr,
+                                            const int32_t *inc, int batch, const shapy_measure_landmarks_t *lm,
+                                            float *out, float *jac, int32_t *status, void *stream) {
+  SHAPY_REQUIRE(m && v_shaped && inc_ptr && inc && lm && out && jac && batch > 0,
+                "shapy_measure_jacobian_betas: bad argument");
+  SHAPY_REQUIRE(((uintptr_t)v_shaped & 15) == 0, "shapy_measure_jacobian_betas: v_shaped must be 16-byte aligned");
+  const SmplxDev &d = m->d;
+  if (d.NB < 1 || d.NB > kMaxJacBetas) {
+    set_error("shapy_measure_jacobian_betas: %d betas, at most %d are supported", d.NB, kMaxJacBetas);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  for (int i = 0; i < 5; ++i)
+    SHAPY_REQUIRE(lm->face_idx[i] >= 0 && lm->face_idx[i] < d.F, "landmark face %d out of range", lm->face_idx[i]);
+  MeasureArgs a{v_shaped, d.faces, nullptr, batch, d.V, d.F, *lm, out, nullptr, nullptr, 0, status,
+                MeasureGrad{nullptr, inc_ptr, inc, nullptr, d.basis, d.V3p, d.NB, jac}};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (status) SHAPY_CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int), s));
+  // the same shared-memory layout as the gradient mode; its static part is 2 KB larger (the per-warp reduction rows)
+  const size_t staged = measure_smem_bytes(d.V) + kGradBytes, list = kListBytes + kGradBytes;
+  if (d.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts, kJacobian>(a, staged, 220 * 1024, s);
+  return launch_grad_source<kGlobalVerts, kJacobian>(a, list, (int)list, s);
 }

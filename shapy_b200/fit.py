@@ -15,6 +15,13 @@ whole batch is optimised at once with Adam: Adam is elementwise, so every body's
 rest of the batch (the reference's L-BFGS / TrustRegion would couple them through the line search and needs a double
 backward, which is not supported).
 
+method='lm' fits the same loss with a batched Levenberg-Marquardt loop instead: per iteration, forward_shape of the
+trial betas, then the measurements and their (5, NB) Jacobian with respect to betas in one launch
+(ops.measure_jacobian_betas), then one damped Gauss-Newton step per body (ops.fit_lm_step: accept the trial if its
+loss is lower, adapt the damping, solve the NB x NB normal equations in fp64).  Three launches per iteration, no host
+synchronisation, and every body's loss is non-increasing.  measurement_jacobian(body_model, body_measurements, betas)
+exposes the Jacobian itself.
+
 fit_body_to_keypoints optimises the raw 6D global and body pose (through the 6D decoder), betas and transl of every
 body against its K 3D keypoints (the model's joints output: posed joints, landmarks, J14 overwrite), loss per body
 sum_k w_k |joint_k - keypoint_k|^2, with the same batched Adam: SMPLX.forward and the decoder are differentiable
@@ -41,15 +48,21 @@ def _targets(targets, B, device):
     return out
 
 
-def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=500,
-                              lr=0.05, betas_init=None, batch_size=None):
+def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
+                              lr=0.05, betas_init=None, batch_size=None, method='adam'):
     """Fits betas (B, NB) so that the model's T-pose measurements match `targets`.
 
     body_model: shapy_b200 SMPLX (its forward_shape and faces are used); body_measurements: shapy_b200
     BodyMeasurements on the same device.  targets: {name: float or (B,) values} for mass [kg], height, chest, waist,
     hips [m]; a missing name or a value <= 0 drops that term.  batch_size: B when every target is a scalar (default 1).
+    method: 'adam' (the default) or 'lm' (Levenberg-Marquardt, see the top; `lr` is ignored).  iterations: None means
+    500 for Adam and 50 for LM.
     Returns {'betas': (B, NB), 'measurements': (B, 5) of the final betas (mass, height, chest, waist, hips),
     'loss': (B,) final per-body loss}."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if iterations is None:
+        iterations = 500 if method == 'adam' else 50
     device = body_model.shapedirs.device
     B = batch_size or max([torch.as_tensor(v).numel() for v in targets.values()] + [1])
     if betas_init is not None:
@@ -61,6 +74,9 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
                       if w[k] > 1e-3 else torch.zeros_like(tg[k]) for k in NAMES], 1)
     tgt = torch.stack([tg[k].clamp(min=0) for k in NAMES], 1)
     faces = body_model.faces_i32
+    if method == 'lm':
+        return _fit_lm(body_model, body_measurements, tgt.contiguous(), wt.contiguous(), betas_weight, iterations,
+                       betas_init, B, device)
     nb = body_model.shapedirs.shape[-1]
     betas = (torch.zeros(B, nb, device=device) if betas_init is None else betas_init.detach().clone().float())
     betas.requires_grad_(True)
@@ -85,6 +101,45 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     with torch.no_grad():
         per_body, meas = loss_fn(betas)
     return {'betas': betas.detach(), 'measurements': meas, 'loss': per_body}
+
+
+# Levenberg-Marquardt damping: divided by LM_DOWN after an accepted step, multiplied by LM_UP after a rejected one
+LM_UP, LM_DOWN = 10.0, 3.0
+
+
+def measurement_jacobian(body_model, body_measurements, betas):
+    """The measurements of forward_shape(betas) and their Jacobian with respect to betas, without autograd:
+    {'measurements': (B, 5) (mass, height, chest, waist, hips, bit-identical to BodyMeasurements.forward_vertices),
+    'jacobian': (B, 5, NB)}.  The Jacobian has the semantics of the measurements' backward (constant barycentrics, no
+    gradient through the plane heights); a NaN circumference gives a NaN row."""
+    from . import ops
+    betas = torch.as_tensor(betas, dtype=torch.float32, device=body_model.shapedirs.device).detach().contiguous()
+    packed = body_model.packed(betas.device)
+    v = ops.smplx_forward_shape(packed, betas)
+    out, jac, status = ops.measure_jacobian_betas(packed, body_measurements.landmarks(), v, body_model.faces_i32)
+    body_measurements.last_status = status
+    return {'measurements': out, 'jacobian': jac}
+
+
+def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, betas_init, B, device):
+    from . import ops
+    packed = body_model.packed(device)
+    faces = body_model.faces_i32
+    lm = body_measurements.landmarks()
+    nb = packed.NB
+    trial = (torch.zeros(B, nb, device=device) if betas_init is None
+             else betas_init.detach().to(device=device, dtype=torch.float32).clone().contiguous())
+    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+    state = {'betas': mk(B, nb), 'meas': mk(B, 5), 'jac': mk(B, 5, nb), 'loss': mk(B), 'lambda': mk(B),
+             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    if B == 0:
+        return {'betas': state['betas'], 'measurements': state['meas'], 'loss': state['loss']}
+    ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
+    for it in range(int(iterations) + 1):
+        v = ops.smplx_forward_shape(packed, trial)
+        meas, jac, _ = ops.measure_jacobian_betas(packed, lm, v, faces)
+        ops.fit_lm_step(state, tgt, wt, betas_weight, LM_UP, LM_DOWN, it == 0, trial, meas, jac)
+    return {'betas': state['betas'], 'measurements': state['meas'], 'loss': state['loss']}
 
 
 IDENT6 = (1.0, 0.0, 0.0, 1.0, 0.0, 0.0)      # the 6D code of the identity rotation (row-major 3x2)
@@ -157,8 +212,10 @@ def main(argv=None):
     p.add_argument('--meas-definition-path', dest='meas_definition_path', type=str, default=None)
     p.add_argument('--meas-vertices-path', dest='meas_vertices_path', type=str, default=None)
     p.add_argument('--betas-weight', dest='betas_weight', type=float, default=0.0)
-    p.add_argument('--iterations', type=int, default=500)
-    p.add_argument('--lr', type=float, default=0.05)
+    p.add_argument('--method', choices=('adam', 'lm'), default='adam',
+                   help='optimiser: Adam, or batched Levenberg-Marquardt on the measurement Jacobian')
+    p.add_argument('--iterations', type=int, default=None, help='default 500 for adam, 50 for lm')
+    p.add_argument('--lr', type=float, default=0.05, help='Adam step size (ignored by lm)')
     p.add_argument('--output', type=str, default='fit_betas.npz')
     a = p.parse_args(argv)
 
@@ -180,7 +237,8 @@ def main(argv=None):
         targets = {k: d[k].astype(np.float32) for k in NAMES if k in d.files}
     else:
         targets = {k: getattr(a, k) for k in NAMES}
-    res = fit_betas_to_measurements(model, bm, targets, betas_weight=a.betas_weight, iterations=a.iterations, lr=a.lr)
+    res = fit_betas_to_measurements(model, bm, targets, betas_weight=a.betas_weight, iterations=a.iterations, lr=a.lr,
+                                    method=a.method)
     meas = res['measurements'].cpu().numpy()
     np.savez(a.output, betas=res['betas'].cpu().numpy(), measurements=meas, names=np.array(NAMES),
              loss=res['loss'].cpu().numpy())

@@ -335,6 +335,75 @@ def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, 
     return grad
 
 
+def _incidence_rows(faces_i32, V):
+    inc_ptr, inc = face_incidence(faces_i32)
+    if inc_ptr.numel() - 1 > V:
+        raise RuntimeError(f'faces index vertex {inc_ptr.numel() - 2} of a mesh with {V} vertices')
+    if inc_ptr.numel() - 1 < V:     # trailing vertices no face uses: empty rows
+        inc_ptr = torch.cat([inc_ptr, inc_ptr[-1:].expand(V + 1 - inc_ptr.numel())])
+    return inc_ptr, inc
+
+
+MAX_JACOBIAN_BETAS = 16
+
+
+def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, v_shaped, faces_i32):
+    """The measurements (B, 5) of `measure` and their Jacobian (B, 5, NB) with respect to the model's betas at the
+    vertices v_shaped (B, V, 3), one launch (include/shapy_b200.h, shapy_measure_jacobian_betas).  faces_i32: the
+    model's faces as a CUDA int32 (F, 3) tensor (its incidence table is cached).  Returns (out, jac, status), status the
+    device status word of `measure`."""
+    x = _cuda_f32(v_shaped, 'v_shaped')
+    if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
+        raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
+    if x.dim() != 3 or x.shape[1:] != (model.V, 3):
+        raise RuntimeError(f'v_shaped must be (B, {model.V}, 3), got {tuple(x.shape)}')
+    if tuple(faces_i32.shape) != (model.F, 3):
+        raise RuntimeError(f'faces_i32 must be ({model.F}, 3), got {tuple(faces_i32.shape)}')
+    if model.NB > MAX_JACOBIAN_BETAS:
+        raise RuntimeError(f'measure_jacobian_betas supports at most {MAX_JACOBIAN_BETAS} betas, the model has '
+                           f'{model.NB}')
+    B, dev = x.shape[0], x.device
+    if x.data_ptr() % 16:           # the kernel stages the vertices with 16-byte loads from a 16-byte aligned base
+        x = x.clone()
+    out = torch.empty(B, 5, dtype=torch.float32, device=dev)
+    jac = torch.empty(B, 5, model.NB, dtype=torch.float32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    if B == 0:
+        return out, jac, status
+    faces_i32 = faces_i32.contiguous()
+    with torch.cuda.device(dev):
+        inc_ptr, inc = _incidence_rows(faces_i32, model.V)
+        check(lib().shapy_measure_jacobian_betas(model.handle, ptr(x), ptr(inc_ptr), ptr(inc), B, C.byref(landmarks),
+                                                 ptr(out), ptr(jac), ptr(status), stream_ptr()),
+              'measure_jacobian_betas')
+    return out, jac, status
+
+
+def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, first, trial, trial_meas, trial_jac):
+    """One Levenberg-Marquardt step per body (include/shapy_b200.h, shapy_fit_lm_step), in place.  state: {'betas'
+    (B, NB), 'meas' (B, 5), 'jac' (B, 5, NB), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32}, CUDA tensors;
+    trial (B, NB) is the evaluated trial on entry and the next trial on return."""
+    B, nb = trial.shape
+    ts = [state[k] for k in ('betas', 'meas', 'jac', 'loss', 'lambda')] + [targets, weights, trial, trial_meas,
+                                                                           trial_jac]
+    for t in ts + [state['accepted']]:
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
+            raise RuntimeError('fit_lm_step: every tensor must be a contiguous CUDA tensor')
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise RuntimeError('fit_lm_step: the state, targets, weights and trial must be float32')
+    if state['accepted'].dtype != torch.int32:
+        raise RuntimeError('fit_lm_step: accepted must be int32')
+    if B == 0:
+        return
+    with torch.cuda.device(trial.device):
+        check(lib().shapy_fit_lm_step(B, nb, ptr(targets), ptr(weights), float(betas_weight), float(lambda_up),
+                                      float(lambda_down), int(bool(first)), ptr(state['betas']), ptr(state['meas']),
+                                      ptr(state['jac']), ptr(state['loss']), ptr(state['lambda']),
+                                      ptr(state['accepted']), ptr(trial), ptr(trial_meas), ptr(trial_jac),
+                                      stream_ptr()), 'fit_lm_step')
+
+
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
     """grad_betas (B, NB) = shapedirs^T . grad_v_shaped (B, V, 3): the adjoint of smplx_forward_shape."""
     g = _cuda_f32(grad_v_shaped, 'grad_v_shaped')
