@@ -33,9 +33,10 @@
 // A hull of zero area (fewer than 3 points, or all of them collinear or coincident in xz) is NaN: qhull raises on it.
 // Compiled with -fmad=false (bit parity of the predicates with oracle/mmi_oracle.c).
 //
-// measure_smem_kernel<SRC, true> is the backward of the five outputs (shapy_measure_backward*).  It reruns phases 0-3 from
-// the same code, so it walks exactly the hull whose edge lengths the forward summed, with no state saved by the
-// forward, and then writes the gradient (phase 4).  The reference's semantics (body_measurements.py:137-173, 182-215):
+// measure_smem_kernel<SRC, kGradient> is the backward of the five outputs (shapy_measure_backward*).  It reruns phases
+// 0-3 from the same code, so it walks exactly the hull whose edge lengths the forward summed, with no state saved by
+// the forward, and then writes the gradient (phase 4).  The reference's semantics (body_measurements.py:137-173,
+// 182-215):
 //   mass    985/6 sign(sum det) d det/d v per face: v1 x v2, v2 x v0, v0 x v1 for the rows v0, v1, v2
 //   height  sign(y_head - y_heel) bc on the y components of the two landmark faces
 //   chest / waist / hips  p = bc . T with bc held constant (the reference selects the points under no_grad); each hull
@@ -44,16 +45,16 @@
 //           query quad.
 //   sign(0) = 0, as torch.abs gives.  A NaN circumference with a non-zero upstream gradient makes the body's whole
 //   gradient NaN; with a zero upstream gradient it adds nothing.
-// The gradient kernel also keeps, per point slot, the (face, query half) code that produced it (phase 2) and, per hull
+// The gradient mode also keeps, per point slot, the (face, query half) code that produced it (phase 2) and, per hull
 // vertex, the next vertex of the walk (phase 3b); points with equal bits are ordered by that code, so the hull and its
 // gradient do not depend on timing either.  No float atomics touch the output: the dense mass term of a vertex (a
 // face corner) is summed over its incident faces in a fixed order, then the hull and height terms are added in a
 // fixed order, so a body's gradient is bit-identical from run to run and independent of the rest of the batch.
 //
 // measure_smem_kernel<SRC, kJacobian> (shapy_measure_jacobian_betas, vertex sources only) reruns the same phases 0-3,
-// writes the forward's five outputs and then, in its own phase 4, jac (B,5,NB): row k is S^T times the gradient the
-// backward gives for the cotangent e_k, S the model's shape rows -- the mass row densely over the vertices, the height
-// row from the two landmark faces, each circumference row from its hull vertices only (see DESIGN.md section 4).
+// writes the forward's five outputs and then, in phase 4, jac (B,5,NB): row k is S^T times the gradient the backward
+// gives for the cotangent e_k, S the model's shape rows -- the mass row densely over the vertices, the height row from
+// the two landmark faces, each circumference row from its hull vertices only (see DESIGN.md section 4).
 #include "mmi_device.cuh"
 #include "smplx.cuh"
 
@@ -65,7 +66,7 @@ constexpr int kMaxCand = 8192;     // (face, plane, query triangle) candidates t
                                    // the buffer is reused for the per-chain candidate lists (u16) in phase 3
 constexpr int kChainCap = 640;     // 24 chains x 640 x 2 B = 30 KB <= 32 KB
 constexpr size_t kListBytes = 3 * kMaxPts * 12 + kMaxCand * 4;   // points + candidate queue, dynamic
-// gradient kernel only: per point slot its (face, query half) code (int) and the next hull vertex (u16)
+// gradient and Jacobian modes only: per point slot its (face, query half) code (int) and the next hull vertex (u16)
 constexpr size_t kGradBytes = 3 * kMaxPts * 4 + 3 * kMaxPts * 2;
 
 enum TriSource { kStagedVerts, kGlobalVerts, kTriangles };
@@ -93,7 +94,7 @@ struct MeasureArgs {
   int *cnt_out;        // (B,3) or null
   int maxp;
   int *status;
-  MeasureGrad g;       // gradient kernel only
+  MeasureGrad g;       // gradient and Jacobian modes only
 };
 
 __device__ __forceinline__ bool better_next(double cx, double cz, float ax, float az, float bx, float bz) {
@@ -122,7 +123,7 @@ __device__ __forceinline__ bool pt_before(const float *a, const float *b) {
   return ord_bits(a[0]) < ord_bits(b[0]);
 }
 
-// pt_before; the gradient kernel breaks full ties between two slots of plane p by their (face, query half) code
+// pt_before, with full ties between two slots of plane p broken by their (face, query half) code when GRAD
 template <bool GRAD>
 __device__ __forceinline__ bool pt_order(const float *a, const float *b, const int *codes, int p, int i, int j) {
   if constexpr (GRAD) {
@@ -167,7 +168,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
   unsigned short *clist = reinterpret_cast<unsigned short *>(cand);                // phase 3: [24][kChainCap]
   int *codes = reinterpret_cast<int *>(smem + vs_bytes + kListBytes);              // GRAD: [3][kMaxPts]
   unsigned short *nxt = reinterpret_cast<unsigned short *>(smem + vs_bytes + kListBytes + 3 * kMaxPts * 4);
-  // order of two point slots of plane p with the same (x, z): by value; the gradient kernel breaks full ties by code
+  // query triangle q (0 or 1) of the horizontal quad [-1, 1]^2 at height h
   auto quad = [](float h, int q) {
     mmi::Tri Q;
     Q.v0 = make_float3(-1.f, h, -1.f);
@@ -263,10 +264,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       const int c = cand[i], f = c >> 3, p = (c >> 1) & 3, q = c & 1;
       const float h = p == 0 ? h0 : (p == 1 ? h1 : h2);
       mmi::Tri T = tri_of(f);
-      mmi::Tri Q;       // = quad(h, q), spelled out: the forward kernel's code is kept as it was
-      Q.v0 = make_float3(-1.f, h, -1.f);
-      Q.v1 = q == 0 ? make_float3(1.f, h, -1.f) : make_float3(1.f, h, 1.f);
-      Q.v2 = q == 0 ? make_float3(1.f, h, 1.f) : make_float3(-1.f, h, 1.f);
+      const mmi::Tri Q = quad(h, q);
       if (!mmi::sat11(Q, T)) continue;
       float3 b1 = make_float3(0, 0, 0), b2 = b1;
       mmi::isect_points(Q, T, b1, b2);  // no hit -> barycentrics stay 0 (first-body semantics)
@@ -409,31 +407,38 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
   if constexpr (MODE != kGradient) {
     if (t == 0 && overflow && a.status) atomicExch(a.status, 1);
   }
-  if constexpr (MODE == kGradient) {
-    // ---- phase 4: gradient.  The chain lists are dead: their storage holds the hull vertex list of each plane
-    // (hull[p][j] = start slot of the j-th edge, chains in order) and then a bitmap of the faces that carry a hull point.
+  if constexpr (MODE != kForward) {
+    static_assert(MODE == kGradient || SRC != kTriangles, "the Jacobian mode reads the model's faces and shape rows");
+    // ---- phase 4: gradient or Jacobian.  The chain lists are dead: their storage holds the hull vertex list of each
+    // plane (hull[p][j] = start slot of the j-th edge, chains in order) and, in gradient mode, then a bitmap of the
+    // faces that carry a hull point.  The Jacobian mode builds what the gradient mode builds for an upstream gradient
+    // of 1 on every output.
     unsigned short *hull = clist;                                                   // [3][kMaxPts]
     unsigned *fbits = reinterpret_cast<unsigned *>(clist + 3 * kMaxPts);
     const int nbits_words = (int)((kMaxCand * 4 - 3 * kMaxPts * 2) / 4);
     const bool all_flagged = a.F > nbits_words * 32;                                // bitmap too small: scan every face
-    __shared__ float gs[5];           // mass scale, height scale, the 3 circumference gradients
+    // mass scale, height scale, the 3 circumference gradients (NaN where the hull is unusable: a NaN circumference or
+    // more than kMaxPts edges)
+    __shared__ float gs[5];
     __shared__ int nedge[3], poison;
     const MeasureGrad &g = a.g;
-    const float *go = g.gout + (size_t)b * 5;
+    const float *go = MODE == kGradient ? g.gout + (size_t)b * 5 : nullptr;
     if (t == 0) {
+      auto up = [&](int k) { return MODE == kGradient ? go[k] : 1.f; };            // the upstream gradient
       float v = 0.f;
       for (int i = 0; i < kThreads / 32; ++i) v += red[i];                          // the forward's volume, same order
-      gs[0] = go[0] * sign_of(v) * (985.0f / 6.0f);
-      gs[1] = go[1] * sign_of(lmy[0] - lmy[1]);
+      gs[0] = up(0) * sign_of(v) * (985.0f / 6.0f);
+      gs[1] = up(1) * sign_of(lmy[0] - lmy[1]);
       int bad = 0;
       for (int p = 0; p < 3; ++p) {
-        gs[2 + p] = go[2 + p];
         int m = 0;
         for (int k = 0; k < 8; ++k) m += chain_edges[p][k];
-        if (go[2 + p] != 0.f && (isnan(perim_s[p]) || m > kMaxPts)) bad = 1;
-        nedge[p] = (go[2 + p] != 0.f && !isnan(perim_s[p]) && m <= kMaxPts) ? m : 0;
+        const bool usable = !isnan(perim_s[p]) && m <= kMaxPts, active = up(2 + p) != 0.f;
+        gs[2 + p] = usable ? up(2 + p) : __int_as_float(0x7fc00000);
+        nedge[p] = active && usable ? m : 0;
+        bad |= active && !usable;
       }
-      poison = bad;
+      poison = MODE == kGradient && bad;   // the Jacobian makes only the rows of unusable hulls NaN
     }
     if (warp < 24 && lane == 0) {
       int off = 0, m = 0;
@@ -442,7 +447,8 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       if (m <= kMaxPts)
         for (int s = 0; s < chain_edges[hp][hk]; ++s) { hull[hp * kMaxPts + off + s] = (unsigned short)cur; cur = nxt[hp * kMaxPts + cur]; }
     }
-    for (int i = t; i < nbits_words; i += kThreads) fbits[i] = 0u;
+    if constexpr (MODE == kGradient)
+      for (int i = t; i < nbits_words; i += kThreads) fbits[i] = 0u;
     __syncthreads();
     // per hull vertex j of plane p: g (u_in - u_out), u the unit vectors of the edges into and out of it.  The walk is
     // one closed cycle (the end of each chain is the start of the next); a vertex where it is not poisons the body.
@@ -460,115 +466,12 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       const float li = sqrtf(ix * ix + iy * iy + iz * iz), lo = sqrtf(ox * ox + oy * oy + oz * oz);
       const float gp = gs[2 + p];
       val[it] = make_float3(gp * (ix / li - ox / lo), gp * (iy / li - oy / lo), gp * (iz / li - oz / lo));
-      if (!all_flagged) {
-        const int f = codes[p * kMaxPts + cur] >> 1;
-        atomicOr(&fbits[f >> 5], 1u << (f & 31));
-      }
-    }
-    __syncthreads();                  // the points are dead: their storage takes the hull vertex gradients
-    for (int it = 0; it < 3; ++it) {
-      const int r = t + it * kThreads;
-      if (r % kMaxPts < nedge[r / kMaxPts]) {
-        pts[3 * r] = val[it].x; pts[3 * r + 1] = val[it].y; pts[3 * r + 2] = val[it].z;
-      }
-    }
-    __syncthreads();
-    const float sm = gs[0], sh = gs[1];
-    const float nan = __int_as_float(0x7fc00000);
-    const bool bad = poison != 0;
-    // hull and height terms of corner k of face f (T = its triangle), in a fixed order: planes, hull order, height
-    auto sparse = [&](int f, const mmi::Tri &T, int k, float3 &acc) {
-      if (all_flagged || (fbits[f >> 5] >> (f & 31)) & 1u) {
-        for (int p = 0; p < 3; ++p) {
-          for (int j = 0; j < nedge[p]; ++j) {
-            const int c = codes[p * kMaxPts + hull[p * kMaxPts + j]];
-            if ((c >> 1) != f) continue;
-            float3 b1 = make_float3(0, 0, 0), b2 = b1;
-            mmi::isect_points(quad(hs[p], c & 1), T, b1, b2);          // the bc phase 2 used for this point
-            const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
-            const float *gv = pts + 3 * (p * kMaxPts + j);
-            acc.x += w * gv[0]; acc.y += w * gv[1]; acc.z += w * gv[2];
-          }
+      if constexpr (MODE == kGradient) {
+        if (!all_flagged) {
+          const int f = codes[p * kMaxPts + cur] >> 1;
+          atomicOr(&fbits[f >> 5], 1u << (f & 31));
         }
       }
-      if (f == a.lm.face_idx[0]) acc.y += sh * a.lm.bc[0][k];
-      if (f == a.lm.face_idx[1]) acc.y -= sh * a.lm.bc[1][k];
-    };
-    if constexpr (SRC == kTriangles) {
-      for (int f = t; f < a.F; f += blockDim.x) {
-        const mmi::Tri T = tri_of(f);
-        float *o = g.grad + ((size_t)b * a.F + f) * 9;
-        for (int k = 0; k < 3; ++k) {
-          const float3 c = corner_cross(T, k);
-          float3 acc = make_float3(sm * c.x, sm * c.y, sm * c.z);
-          sparse(f, T, k, acc);
-          o[3 * k] = bad ? nan : acc.x; o[3 * k + 1] = bad ? nan : acc.y; o[3 * k + 2] = bad ? nan : acc.z;
-        }
-      }
-    } else {
-      for (int v = t; v < a.V; v += blockDim.x) {
-        const int e0 = __ldg(g.inc_ptr + v), e1 = __ldg(g.inc_ptr + v + 1);
-        float3 acc = make_float3(0.f, 0.f, 0.f);
-        for (int e = e0; e < e1; ++e) {
-          const int fk = __ldg(g.inc + e);
-          const float3 c = corner_cross(tri_of(fk / 3), fk % 3);
-          acc.x += c.x; acc.y += c.y; acc.z += c.z;
-        }
-        acc = make_float3(sm * acc.x, sm * acc.y, sm * acc.z);
-        for (int e = e0; e < e1; ++e) {
-          const int fk = __ldg(g.inc + e), f = fk / 3;
-          if (all_flagged || f == a.lm.face_idx[0] || f == a.lm.face_idx[1] || ((fbits[f >> 5] >> (f & 31)) & 1u))
-            sparse(f, tri_of(f), fk % 3, acc);
-        }
-        float *o = g.grad + ((size_t)b * a.V + v) * 3;
-        o[0] = bad ? nan : acc.x; o[1] = bad ? nan : acc.y; o[2] = bad ? nan : acc.z;
-      }
-    }
-  }
-  if constexpr (MODE == kJacobian && SRC != kTriangles) {
-    // ---- phase 4 (Jacobian): row k of jac is S^T times the gradient the backward gives for the cotangent e_k, S the
-    // nb shape rows of the basis.  The points' storage takes the hull vertex vectors u_in - u_out (the backward's with
-    // g = 1), the chain lists the hull vertex list, as in the gradient mode.
-    unsigned short *hull = clist;                                                   // [3][kMaxPts]
-    __shared__ float sc[2];           // mass scale, height scale
-    __shared__ int nedge[3], rownan[3], poison;
-    __shared__ float jred[kThreads / 32][kMaxJacBetas];
-    const MeasureGrad &g = a.g;
-    const int nb = g.nb;
-    if (t == 0) {
-      float v = 0.f;
-      for (int i = 0; i < kThreads / 32; ++i) v += red[i];                          // the forward's volume, same order
-      sc[0] = sign_of(v) * (985.0f / 6.0f);
-      sc[1] = sign_of(lmy[0] - lmy[1]);
-      for (int p = 0; p < 3; ++p) {
-        int m = 0;
-        for (int k = 0; k < 8; ++k) m += chain_edges[p][k];
-        rownan[p] = isnan(perim_s[p]) || m > kMaxPts;
-        nedge[p] = rownan[p] ? 0 : m;
-      }
-      poison = 0;
-    }
-    if (warp < 24 && lane == 0) {
-      int off = 0, m = 0;
-      for (int k = 0; k < 8; ++k) { off += k < hk ? chain_edges[hp][k] : 0; m += chain_edges[hp][k]; }
-      int cur = ext[hp][hk].idx;
-      if (m <= kMaxPts)
-        for (int s = 0; s < chain_edges[hp][hk]; ++s) { hull[hp * kMaxPts + off + s] = (unsigned short)cur; cur = nxt[hp * kMaxPts + cur]; }
-    }
-    __syncthreads();
-    float3 val[3];
-    for (int it = 0; it < 3; ++it) {
-      val[it] = make_float3(0.f, 0.f, 0.f);
-      const int r = t + it * kThreads, p = r / kMaxPts, j = r % kMaxPts, m = nedge[p];
-      if (j >= m) continue;
-      const float *P = pts + (size_t)p * kMaxPts * 3;
-      const unsigned short *H = hull + p * kMaxPts;
-      const int cur = H[j], prev = H[(j + m - 1) % m], next = nxt[p * kMaxPts + cur];
-      if (nxt[p * kMaxPts + prev] != cur || next != H[(j + 1) % m]) { poison = 1; continue; }
-      const float ix = P[3 * cur] - P[3 * prev], iy = P[3 * cur + 1] - P[3 * prev + 1], iz = P[3 * cur + 2] - P[3 * prev + 2];
-      const float ox = P[3 * next] - P[3 * cur], oy = P[3 * next + 1] - P[3 * cur + 1], oz = P[3 * next + 2] - P[3 * cur + 2];
-      const float li = sqrtf(ix * ix + iy * iy + iz * iz), lo = sqrtf(ox * ox + oy * oy + oz * oz);
-      val[it] = make_float3(ix / li - ox / lo, iy / li - oy / lo, iz / li - oz / lo);
     }
     __syncthreads();                  // the points are dead: their storage takes the hull vertex vectors
     for (int it = 0; it < 3; ++it) {
@@ -577,166 +480,213 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
         pts[3 * r] = val[it].x; pts[3 * r + 1] = val[it].y; pts[3 * r + 2] = val[it].z;
       }
     }
-    // mass row: sum over the vertices of (sum of the incident corner_cross, in CSR order) . S[l][v], one thread per
-    // vertex at a time, then a fixed xor tree per warp and the warps in order
-    float part[kMaxJacBetas];
-#pragma unroll
-    for (int l = 0; l < kMaxJacBetas; ++l) part[l] = 0.f;
-    for (int v = t; v < a.V; v += kThreads) {
-      const int e0 = __ldg(g.inc_ptr + v), e1 = __ldg(g.inc_ptr + v + 1);
+    const float nan = __int_as_float(0x7fc00000);
+    // sum of d det / d v over the (face, corner) entries e0..e1 of a vertex's incidence row, in that order
+    auto incident_cross = [&](int e0, int e1) {
       float3 c = make_float3(0.f, 0.f, 0.f);
       for (int e = e0; e < e1; ++e) {
         const int fk = __ldg(g.inc + e);
         const float3 d = corner_cross(tri_of(fk / 3), fk % 3);
         c.x += d.x; c.y += d.y; c.z += d.z;
       }
-      const float *Sv = g.S + 3 * (size_t)v;
-#pragma unroll
-      for (int l = 0; l < kMaxJacBetas; ++l)
-        if (l < nb) {
-          const float *s = Sv + (size_t)l * g.ld;
-          part[l] += c.x * __ldg(s) + c.y * __ldg(s + 1) + c.z * __ldg(s + 2);
-        }
-    }
-#pragma unroll
-    for (int l = 0; l < kMaxJacBetas; ++l) {
-      if (l < nb) {
-        float x = part[l];
-        for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-        if (lane == 0) jred[warp][l] = x;
-      }
-    }
-    __syncthreads();
-    const float nan = __int_as_float(0x7fc00000);
-    const bool bad = poison != 0;
-    float *J = g.jac + (size_t)b * 5 * nb;
-    if (t < nb) {
-      const int l = t;
-      float s = 0.f;
-      for (int w = 0; w < kThreads / 32; ++w) s += jred[w][l];
-      J[l] = bad ? nan : sc[0] * s;
-      // height row: the y components of the two landmark faces' corners
-      const float *Sl = g.S + (size_t)l * g.ld + 1;
-      float h = 0.f;
-      for (int k = 0; k < 3; ++k) h += a.lm.bc[0][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[0] + k]);
-      for (int k = 0; k < 3; ++k) h -= a.lm.bc[1][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[1] + k]);
-      J[nb + l] = bad ? nan : sc[1] * h;
-    }
-    // circumference rows: warp (plane p, row l); lane i takes the hull vertices j = i mod 32, the bc-weighted sum over
-    // its face's corners of (u_in - u_out) . S[l][corner] (the bc phase 2 used, recomputed from the (face, query half)
-    // code), and the warp adds them in hull order
-    for (int r = warp; r < 3 * nb; r += kThreads / 32) {
-      const int p = r / nb, l = r % nb, m = nedge[p];
-      const float *Sl = g.S + (size_t)l * g.ld;
-      float acc = 0.f;
-      for (int base = 0; base < m; base += 32) {
-        const int j = base + lane;
-        float c = 0.f;
-        if (j < m) {
-          const int code = codes[p * kMaxPts + hull[p * kMaxPts + j]], f = code >> 1;
-          float3 b1 = make_float3(0, 0, 0), b2 = b1;
-          mmi::isect_points(quad(hs[p], code & 1), tri_of(f), b1, b2);
-          const float *gv = pts + 3 * (p * kMaxPts + j);
-          for (int k = 0; k < 3; ++k) {
-            const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
-            const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
-            c += w * (gv[0] * __ldg(s) + gv[1] * __ldg(s + 1) + gv[2] * __ldg(s + 2));
+      return c;
+    };
+    // the barycentrics phase 2 used for the point with (face, query half) code c of plane p, T the face's triangle
+    auto hull_bc = [&](int p, int c, const mmi::Tri &T) {
+      float3 b1 = make_float3(0, 0, 0), b2 = b1;
+      mmi::isect_points(quad(hs[p], c & 1), T, b1, b2);
+      return b1;
+    };
+    if constexpr (MODE == kGradient) {
+      __syncthreads();
+      const float sm = gs[0], sh = gs[1];
+      const bool bad = poison != 0;
+      // hull and height terms of corner k of face f (T = its triangle), in a fixed order: planes, hull order, height
+      auto sparse = [&](int f, const mmi::Tri &T, int k, float3 &acc) {
+        if (all_flagged || (fbits[f >> 5] >> (f & 31)) & 1u) {
+          for (int p = 0; p < 3; ++p) {
+            for (int j = 0; j < nedge[p]; ++j) {
+              const int c = codes[p * kMaxPts + hull[p * kMaxPts + j]];
+              if ((c >> 1) != f) continue;
+              const float3 b1 = hull_bc(p, c, T);
+              const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+              const float *gv = pts + 3 * (p * kMaxPts + j);
+              acc.x += w * gv[0]; acc.y += w * gv[1]; acc.z += w * gv[2];
+            }
           }
         }
-        const int nj = min(32, m - base);
-        for (int i = 0; i < nj; ++i) acc += __shfl_sync(0xffffffffu, c, i);
+        if (f == a.lm.face_idx[0]) acc.y += sh * a.lm.bc[0][k];
+        if (f == a.lm.face_idx[1]) acc.y -= sh * a.lm.bc[1][k];
+      };
+      if constexpr (SRC == kTriangles) {
+        for (int f = t; f < a.F; f += blockDim.x) {
+          const mmi::Tri T = tri_of(f);
+          float *o = g.grad + ((size_t)b * a.F + f) * 9;
+          for (int k = 0; k < 3; ++k) {
+            const float3 c = corner_cross(T, k);
+            float3 acc = make_float3(sm * c.x, sm * c.y, sm * c.z);
+            sparse(f, T, k, acc);
+            o[3 * k] = bad ? nan : acc.x; o[3 * k + 1] = bad ? nan : acc.y; o[3 * k + 2] = bad ? nan : acc.z;
+          }
+        }
+      } else {
+        for (int v = t; v < a.V; v += blockDim.x) {
+          const int e0 = __ldg(g.inc_ptr + v), e1 = __ldg(g.inc_ptr + v + 1);
+          const float3 c = incident_cross(e0, e1);
+          float3 acc = make_float3(sm * c.x, sm * c.y, sm * c.z);
+          for (int e = e0; e < e1; ++e) {
+            const int fk = __ldg(g.inc + e), f = fk / 3;
+            if (all_flagged || f == a.lm.face_idx[0] || f == a.lm.face_idx[1] || ((fbits[f >> 5] >> (f & 31)) & 1u))
+              sparse(f, tri_of(f), fk % 3, acc);
+          }
+          float *o = g.grad + ((size_t)b * a.V + v) * 3;
+          o[0] = bad ? nan : acc.x; o[1] = bad ? nan : acc.y; o[2] = bad ? nan : acc.z;
+        }
       }
-      if (lane == 0) J[(size_t)(2 + p) * nb + l] = (bad || rownan[p]) ? nan : acc;
+    } else {
+      // Jacobian: row k of jac is S^T times the gradient for the cotangent e_k, S the nb shape rows of the basis.
+      // Mass row: sum over the vertices of incident_cross . S[l][v], one thread per vertex at a time, then a fixed xor
+      // tree per warp and the warps in order.
+      __shared__ float jred[kThreads / 32][kMaxJacBetas];
+      const int nb = g.nb;
+      float part[kMaxJacBetas];
+#pragma unroll
+      for (int l = 0; l < kMaxJacBetas; ++l) part[l] = 0.f;
+      for (int v = t; v < a.V; v += kThreads) {
+        const float3 c = incident_cross(__ldg(g.inc_ptr + v), __ldg(g.inc_ptr + v + 1));
+        const float *Sv = g.S + 3 * (size_t)v;
+#pragma unroll
+        for (int l = 0; l < kMaxJacBetas; ++l)
+          if (l < nb) {
+            const float *s = Sv + (size_t)l * g.ld;
+            part[l] += c.x * __ldg(s) + c.y * __ldg(s + 1) + c.z * __ldg(s + 2);
+          }
+      }
+#pragma unroll
+      for (int l = 0; l < kMaxJacBetas; ++l) {
+        if (l < nb) {
+          float x = part[l];
+          for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+          if (lane == 0) jred[warp][l] = x;
+        }
+      }
+      __syncthreads();
+      const bool bad = poison != 0;
+      float *J = g.jac + (size_t)b * 5 * nb;
+      if (t < nb) {
+        const int l = t;
+        float s = 0.f;
+        for (int w = 0; w < kThreads / 32; ++w) s += jred[w][l];
+        J[l] = bad ? nan : gs[0] * s;
+        // height row: the y components of the two landmark faces' corners
+        const float *Sl = g.S + (size_t)l * g.ld + 1;
+        float h = 0.f;
+        for (int k = 0; k < 3; ++k) h += a.lm.bc[0][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[0] + k]);
+        for (int k = 0; k < 3; ++k) h -= a.lm.bc[1][k] * __ldg(Sl + 3 * a.faces[3 * a.lm.face_idx[1] + k]);
+        J[nb + l] = bad ? nan : gs[1] * h;
+      }
+      // circumference rows: warp (plane p, row l); lane i takes the hull vertices j = i mod 32, the bc-weighted sum
+      // over its face's corners of (u_in - u_out) . S[l][corner], and the warp adds them in hull order
+      for (int r = warp; r < 3 * nb; r += kThreads / 32) {
+        const int p = r / nb, l = r % nb, m = nedge[p];
+        const float *Sl = g.S + (size_t)l * g.ld;
+        float acc = 0.f;
+        for (int base = 0; base < m; base += 32) {
+          const int j = base + lane;
+          float c = 0.f;
+          if (j < m) {
+            const int code = codes[p * kMaxPts + hull[p * kMaxPts + j]], f = code >> 1;
+            const float3 b1 = hull_bc(p, code, tri_of(f));
+            const float *gv = pts + 3 * (p * kMaxPts + j);
+            for (int k = 0; k < 3; ++k) {
+              const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+              const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
+              c += w * (gv[0] * __ldg(s) + gv[1] * __ldg(s + 1) + gv[2] * __ldg(s + 2));
+            }
+          }
+          const int nj = min(32, m - base);
+          for (int i = 0; i < nj; ++i) acc += __shfl_sync(0xffffffffu, c, i);
+        }
+        if (lane == 0) J[(size_t)(2 + p) * nb + l] = (bad || isnan(gs[2 + p])) ? nan : acc;
+      }
     }
   }
 }
 
-size_t measure_smem_bytes(int V) { return (((size_t)V * 12 + 15) & ~(size_t)15) + kListBytes; }
-
-template <int SRC>
-static int launch_source(const MeasureArgs &a, size_t smem, int max_smem, cudaStream_t stream) {
-  static std::atomic<unsigned long long> attr_done{0};   // one per instantiation
-  SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC>, max_smem, attr_done));
-  measure_smem_kernel<SRC><<<a.B, kThreads, smem, stream>>>(a);
-  SHAPY_LAUNCH_CHECK();
-  return SHAPY_OK;
-}
+// Dynamic shared memory holds the staged vertices (when they fit under kMaxDynSmem), the point and candidate lists
+// and, for the gradient and the Jacobian, the point codes and the hull walk: always more than the 48 KB default.
+// kMaxDynSmem plus the largest static part (the Jacobian's 2 752 B) fits the SM's 227 KB.
+constexpr size_t kMaxDynSmem = 220 * 1024;
 
 template <int SRC, int MODE>
-static int launch_grad_source(const MeasureArgs &a, size_t smem, int max_smem, cudaStream_t stream) {
-  static std::atomic<unsigned long long> attr_done{0};
+static int launch_source(const MeasureArgs &a, size_t smem, cudaStream_t stream) {
+  static std::atomic<unsigned long long> attr_done{0};   // one per instantiation
+  // set once per instantiation: the staged size varies with V, the others do not
+  const int max_smem = (int)(SRC == kStagedVerts ? kMaxDynSmem : smem);
   SHAPY_CUDA_TRY(set_max_dynamic_smem(measure_smem_kernel<SRC, MODE>, max_smem, attr_done));
   measure_smem_kernel<SRC, MODE><<<a.B, kThreads, smem, stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
 
-}  // namespace shapy
-
-using namespace shapy;
-
-static int launch_measure(MeasureArgs a, void *stream) {
-  SHAPY_REQUIRE(a.out && a.B > 0 && a.F > 0, "shapy_measure: bad argument");
+// The work every entry shares: the landmark check, the status clear, and the source of the triangles with its
+// shared memory.
+template <int MODE>
+static int launch_measure(const MeasureArgs &a, void *stream) {
+  SHAPY_REQUIRE(a.B > 0 && a.F > 0, "shapy_measure: bad argument");
   for (int i = 0; i < 5; ++i)
     SHAPY_REQUIRE(a.lm.face_idx[i] >= 0 && a.lm.face_idx[i] < a.F, "landmark face %d out of range", a.lm.face_idx[i]);
   cudaStream_t s = (cudaStream_t)stream;
   if (a.status) SHAPY_CUDA_TRY(cudaMemsetAsync(a.status, 0, sizeof(int), s));
-  if (a.tris) return launch_source<kTriangles>(a, kListBytes, (int)kListBytes, s);          // 68 KB > 48 KB default
-  if (a.V < 65536 && measure_smem_bytes(a.V) <= 220 * 1024)
-    return launch_source<kStagedVerts>(a, measure_smem_bytes(a.V), 226 * 1024, s);        // + 656 B static <= 227 KB
-  return launch_source<kGlobalVerts>(a, kListBytes, (int)kListBytes, s);
+  const size_t list = kListBytes + (MODE == kForward ? 0 : kGradBytes);
+  if constexpr (MODE != kJacobian)
+    if (a.tris) return launch_source<kTriangles, MODE>(a, list, s);
+  const size_t staged = (((size_t)a.V * 12 + 15) & ~(size_t)15) + list;
+  if (a.V < 65536 && staged <= kMaxDynSmem) return launch_source<kStagedVerts, MODE>(a, staged, s);
+  return launch_source<kGlobalVerts, MODE>(a, list, s);
 }
+
+}  // namespace shapy
+
+using namespace shapy;
 
 extern "C" int shapy_measure_forward(const float *v_shaped, const int32_t *faces, int batch, int num_verts,
                                      int num_faces, const shapy_measure_landmarks_t *lm, float *out,
                                      float *plane_points, int32_t *plane_counts, int max_points, int32_t *status,
                                      void *stream) {
-  SHAPY_REQUIRE(v_shaped && faces && lm, "shapy_measure_forward: null argument");
+  SHAPY_REQUIRE(v_shaped && faces && lm && out, "shapy_measure_forward: null argument");
   MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, out, plane_points, plane_counts,
                 max_points, status, MeasureGrad{}};
-  return launch_measure(a, stream);
+  return launch_measure<kForward>(a, stream);
 }
 
 extern "C" int shapy_measure_forward_tris(const float *triangles, int batch, int num_faces,
                                           const shapy_measure_landmarks_t *lm, float *out, float *plane_points,
                                           int32_t *plane_counts, int max_points, int32_t *status, void *stream) {
-  SHAPY_REQUIRE(triangles && lm, "shapy_measure_forward_tris: null argument");
+  SHAPY_REQUIRE(triangles && lm && out, "shapy_measure_forward_tris: null argument");
   MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, out, plane_points, plane_counts, max_points,
                 status, MeasureGrad{}};
-  return launch_measure(a, stream);
-}
-
-static int launch_measure_grad(const MeasureArgs &a, void *stream) {
-  const MeasureGrad &g = a.g;
-  SHAPY_REQUIRE(g.gout && g.grad && a.B > 0 && a.F > 0, "shapy_measure_backward: bad argument");
-  for (int i = 0; i < 5; ++i)
-    SHAPY_REQUIRE(a.lm.face_idx[i] >= 0 && a.lm.face_idx[i] < a.F, "landmark face %d out of range", a.lm.face_idx[i]);
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t list = kListBytes + kGradBytes;
-  if (a.tris) return launch_grad_source<kTriangles, kGradient>(a, list, (int)list, s);
-  SHAPY_REQUIRE(g.inc_ptr && g.inc && a.V > 0, "shapy_measure_backward: null incidence table");
-  const size_t staged = measure_smem_bytes(a.V) + kGradBytes;
-  if (a.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts, kGradient>(a, staged, 226 * 1024, s);
-  return launch_grad_source<kGlobalVerts, kGradient>(a, list, (int)list, s);
+  return launch_measure<kForward>(a, stream);
 }
 
 extern "C" int shapy_measure_backward(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
                                       const int32_t *inc, int batch, int num_verts, int num_faces,
                                       const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_v,
                                       void *stream) {
-  SHAPY_REQUIRE(v_shaped && faces && lm, "shapy_measure_backward: null argument");
+  SHAPY_REQUIRE(v_shaped && faces && lm && grad_out && grad_v, "shapy_measure_backward: null argument");
+  SHAPY_REQUIRE(inc_ptr && inc && num_verts > 0, "shapy_measure_backward: null incidence table");
   MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
                 MeasureGrad{grad_out, inc_ptr, inc, grad_v}};
-  return launch_measure_grad(a, stream);
+  return launch_measure<kGradient>(a, stream);
 }
 
 extern "C" int shapy_measure_backward_tris(const float *triangles, int batch, int num_faces,
                                            const shapy_measure_landmarks_t *lm, const float *grad_out,
                                            float *grad_triangles, void *stream) {
-  SHAPY_REQUIRE(triangles && lm, "shapy_measure_backward_tris: null argument");
+  SHAPY_REQUIRE(triangles && lm && grad_out && grad_triangles, "shapy_measure_backward_tris: null argument");
   MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
                 MeasureGrad{grad_out, nullptr, nullptr, grad_triangles}};
-  return launch_measure_grad(a, stream);
+  return launch_measure<kGradient>(a, stream);
 }
 
 extern "C" int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float *v_shaped, const int32_t *inc_ptr,
@@ -750,14 +700,7 @@ extern "C" int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float 
     set_error("shapy_measure_jacobian_betas: %d betas, at most %d are supported", d.NB, kMaxJacBetas);
     return SHAPY_ERR_UNSUPPORTED;
   }
-  for (int i = 0; i < 5; ++i)
-    SHAPY_REQUIRE(lm->face_idx[i] >= 0 && lm->face_idx[i] < d.F, "landmark face %d out of range", lm->face_idx[i]);
   MeasureArgs a{v_shaped, d.faces, nullptr, batch, d.V, d.F, *lm, out, nullptr, nullptr, 0, status,
                 MeasureGrad{nullptr, inc_ptr, inc, nullptr, d.basis, d.V3p, d.NB, jac}};
-  cudaStream_t s = (cudaStream_t)stream;
-  if (status) SHAPY_CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int), s));
-  // the same shared-memory layout as the gradient mode; its static part is 2 KB larger (the per-warp reduction rows)
-  const size_t staged = measure_smem_bytes(d.V) + kGradBytes, list = kListBytes + kGradBytes;
-  if (d.V < 65536 && staged <= 220 * 1024) return launch_grad_source<kStagedVerts, kJacobian>(a, staged, 220 * 1024, s);
-  return launch_grad_source<kGlobalVerts, kJacobian>(a, list, (int)list, s);
+  return launch_measure<kJacobian>(a, stream);
 }

@@ -229,6 +229,22 @@ def make_landmarks(lm: dict) -> _lib.MeasureLandmarks:
     return s
 
 
+def _faces_i32(faces_i32):
+    if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
+        raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
+    return faces_i32.contiguous()
+
+
+def _measure_input(v_shaped, faces_i32, triangles):
+    """(x, faces_i32, B, V, F) of a measurement call on either (v_shaped (B,V,3), faces_i32) or triangles (B,F,3,3)."""
+    if triangles is not None:
+        x = _cuda_f32(triangles, 'triangles')
+        return x, None, x.shape[0], 0, x.shape[1]
+    x = _cuda_f32(v_shaped, 'v_shaped')
+    faces_i32 = _faces_i32(faces_i32)
+    return x, faces_i32, x.shape[0], x.shape[1], faces_i32.shape[0]
+
+
 def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, triangles=None, return_points=False,
             max_points=1024, strict=False):
     """Returns (B, 5) = mass, height, chest, waist, hips.  Either (v_shaped, faces_i32) or triangles (B,F,3,3).
@@ -241,16 +257,7 @@ def measure(landmarks: _lib.MeasureLandmarks, v_shaped=None, faces_i32=None, tri
     reference's qhull raises, but does not set the status.  The status word is returned as `out.status` (a 1-element
     int32 CUDA tensor, readable at the caller's next synchronisation point) and `strict=True` checks it here (one host
     synchronisation) and raises."""
-    if triangles is not None:
-        x = _cuda_f32(triangles, 'triangles')
-        B, F = x.shape[0], x.shape[1]
-    else:
-        x = _cuda_f32(v_shaped, 'v_shaped')
-        B, V = x.shape[0], x.shape[1]
-        if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
-            raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
-        faces_i32 = faces_i32.contiguous()
-        F = faces_i32.shape[0]
+    x, faces_i32, B, V, F = _measure_input(v_shaped, faces_i32, triangles)
     dev = x.device
     out = torch.empty(B, 5, dtype=torch.float32, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -305,16 +312,7 @@ def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, 
     autograd semantics (include/shapy_b200.h, shapy_measure_backward): the intersection barycentrics are constants and
     the plane heights get no gradient.  Deterministic, one launch."""
     g = _cuda_f32(grad_out, 'grad_out')
-    if triangles is not None:
-        x = _cuda_f32(triangles, 'triangles')
-        B, F = x.shape[0], x.shape[1]
-    else:
-        x = _cuda_f32(v_shaped, 'v_shaped')
-        B, V = x.shape[0], x.shape[1]
-        if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
-            raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
-        faces_i32 = faces_i32.contiguous()
-        F = faces_i32.shape[0]
+    x, faces_i32, B, V, F = _measure_input(v_shaped, faces_i32, triangles)
     if g.shape != (B, 5):
         raise RuntimeError(f'grad_out must be ({B}, 5), got {tuple(g.shape)}')
     grad = torch.empty_like(x)
@@ -325,11 +323,7 @@ def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, 
             check(lib().shapy_measure_backward_tris(ptr(x), B, F, C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()),
                   'measure_backward')
         else:
-            inc_ptr, inc = face_incidence(faces_i32)
-            if inc_ptr.numel() - 1 > V:
-                raise RuntimeError(f'faces index vertex {inc_ptr.numel() - 2} of a mesh with {V} vertices')
-            if inc_ptr.numel() - 1 < V:     # trailing vertices no face uses: empty rows
-                inc_ptr = torch.cat([inc_ptr, inc_ptr[-1:].expand(V + 1 - inc_ptr.numel())])
+            inc_ptr, inc = _incidence_rows(faces_i32, V)
             check(lib().shapy_measure_backward(ptr(x), ptr(faces_i32), ptr(inc_ptr), ptr(inc), B, V, F,
                                                C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()), 'measure_backward')
     return grad
@@ -353,8 +347,7 @@ def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, 
     model's faces as a CUDA int32 (F, 3) tensor (its incidence table is cached).  Returns (out, jac, status), status the
     device status word of `measure`."""
     x = _cuda_f32(v_shaped, 'v_shaped')
-    if not (torch.is_tensor(faces_i32) and faces_i32.is_cuda and faces_i32.dtype == torch.int32):
-        raise RuntimeError('faces_i32 must be a CUDA int32 tensor')
+    faces_i32 = _faces_i32(faces_i32)
     if x.dim() != 3 or x.shape[1:] != (model.V, 3):
         raise RuntimeError(f'v_shaped must be (B, {model.V}, 3), got {tuple(x.shape)}')
     if tuple(faces_i32.shape) != (model.F, 3):
@@ -370,7 +363,6 @@ def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, 
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     if B == 0:
         return out, jac, status
-    faces_i32 = faces_i32.contiguous()
     with torch.cuda.device(dev):
         inc_ptr, inc = _incidence_rows(faces_i32, model.V)
         check(lib().shapy_measure_jacobian_betas(model.handle, ptr(x), ptr(inc_ptr), ptr(inc), B, C.byref(landmarks),
