@@ -133,6 +133,19 @@ int shapy_smplx_backward(const shapy_smplx_t *m, const float *betas, const float
                          const float *grad_joints, const float *grad_proj_joints, float *grad_betas, float *grad_rot,
                          float *grad_expr, float *grad_camera, void *workspace, size_t workspace_bytes, void *stream);
 
+/* The keypoints of shapy_smplx_forward (its `joints`, expression zero) plus transl, and their Jacobian, in one launch.
+ *   betas (B,NB), rot (B,n_rot,3,3) as in shapy_smplx_forward (joints >= n_rot are the identity), transl (B,3) or
+ *   NULL (zero); outputs keypoints (B,K,3) and jac (B,3K,P) fp32, rows keypoint-major in xyz order, device.
+ * Columns, P = 3 n_rot + NB + 3: delta_j (3 per joint j < n_rot, the right-multiplied tangent R_j Exp(delta_j) at
+ * delta = 0), then betas, then transl.  Semantics of shapy_smplx_backward: the dynamic-contour LUT row is a constant,
+ * an overwritten J14 keypoint takes the J14 row's derivative, the model buffers are constants.  Only the vertices the
+ * landmarks and J14 rows reference are evaluated (v_posed from the fp32 posedirs rows below 9 (n_rot - 1)); the cost
+ * grows with the J14 regressor's non-zeros.  The keypoints agree with shapy_smplx_forward to fp32 rounding (its pose
+ * blend is the split-fp16 GEMM).  No atomics: a body's result is bit-identical from run to run and independent of the
+ * rest of the batch.  1 <= n_rot <= J; batch 0: no launch. */
+int shapy_smplx_keypoint_jacobian(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
+                                  const float *transl, int batch, float *keypoints, float *jac, void *stream);
+
 /* Adjoint of shapy_decode_rot6d: grad_raw (n, 6) from raw (n, 6) and grad_rot (n, 3, 3), elementwise.  The 1e-12
  * clamp of each norm passes gradient to the norm only where the norm is >= 1e-12 (torch's clamp_min). */
 int shapy_decode_rot6d_backward(const float *raw, int n, const float *grad_rot, float *grad_raw, void *stream);
@@ -200,6 +213,25 @@ int shapy_fit_lm_step(int batch, int nb, const float *targets, const float *weig
                       float lambda_up, float lambda_down, int first, float *betas, float *meas, float *jac,
                       float *loss, float *lambda, int32_t *accepted, float *trial, const float *trial_meas,
                       const float *trial_jac, void *stream);
+
+/* One Levenberg-Marquardt step per body of the fit of pose and shape to K 3D keypoints, one CTA per body, with
+ * shapy_fit_lm_step's policy and lambda constants.  Parameters as the columns of shapy_smplx_keypoint_jacobian,
+ * P = 3 n_rot + nb + 3.  Loss L = sum_{w_k > 0} w_k |kp_k - target_k|^2 in fp64, k order; a keypoint with weight
+ * <= 0 is dropped (its rows are never read).  targets (B,K,3), weights (B,K); the state rot (B,n_rot,3,3), betas
+ * (B,nb), transl (B,3), keypoints (B,K,3), jac (B,3K,P), loss (B), lambda (B), accepted (B, a count); trial_rot /
+ * trial_betas / trial_transl is the point whose trial_keypoints / trial_jac were evaluated, and receives the next
+ * trial.  With `first` the trial becomes the state and lambda = 1e-3 max(diag(J^T W J), 1e-6); otherwise a finite
+ * trial loss below the state's is accepted (state := trial, lambda /= lambda_down, accepted += 1) and any other
+ * rejected (lambda *= lambda_up); lambda is clamped to [1e-9, 1e9].  (J^T W J + lambda I) delta = -J^T W (kp - target)
+ * by Cholesky in fp64; the next trial is R_j Exp(delta_j) (Rodrigues in fp64, re-orthonormalised by the 6D decoder's
+ * Gram-Schmidt of the first two columns), beta + delta_beta, t + delta_t, rounded to fp32.  A body whose loss is not
+ * finite, or whose factorisation fails, gets its state as the trial; a non-finite starting loss is reported as NaN.
+ * Deterministic, no atomics, per-body independent.  P > 96: SHAPY_ERR_UNSUPPORTED.  batch 0: no launch. */
+int shapy_fit_lm_keypoints_step(int batch, int num_keypoints, int n_rot, int nb, const float *targets,
+                                const float *weights, float lambda_up, float lambda_down, int first, float *rot,
+                                float *betas, float *transl, float *keypoints, float *jac, float *loss, float *lambda,
+                                int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+                                const float *trial_keypoints, const float *trial_jac, void *stream);
 
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.

@@ -75,6 +75,8 @@ _SIGS = {
     'shapy_smplx_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 8
                              + [c_void_p, c_size_t, c_void_p]),
     'shapy_decode_rot6d_backward': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    'shapy_smplx_keypoint_jacobian': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                              c_void_p]),
     'shapy_measure_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                        C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,
@@ -83,6 +85,8 @@ _SIGS = {
                                              c_void_p, c_void_p, c_void_p, c_void_p]),
     'shapy_fit_lm_step': (c_int, [c_int, c_int, c_void_p, c_void_p, C.c_float, C.c_float, C.c_float, c_int]
                           + [c_void_p] * 9 + [c_void_p]),
+    'shapy_fit_lm_keypoints_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, C.c_float, C.c_float, c_int]
+                                    + [c_void_p] * 13 + [c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

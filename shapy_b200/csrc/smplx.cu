@@ -107,6 +107,25 @@ __device__ __forceinline__ void body_chain(const SmplxDev &m, const float *betas
   }
 }
 
+// Dynamic-contour LUT row of a body from its rotations (lbs.py:30-41, rotation_utils.py:86-92).  Shared by
+// smplx_pose_kernel and smplx_kp_jac_kernel, so both pick the same row.
+__device__ __forceinline__ int contour_lut_row(const SmplxDev &m, const float (*R)[9]) {
+  float rel[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  for (int q = 0; q < m.n_chain; ++q) {
+    const float *Rq = R[m.neck[q]];
+    float o[9];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) o[r * 3 + c] = Rq[r * 3] * rel[c] + Rq[r * 3 + 1] * rel[3 + c] + Rq[r * 3 + 2] * rel[6 + c];
+    for (int e = 0; e < 9; ++e) rel[e] = o[e];
+  }
+  float sy = sqrtf(rel[0] * rel[0] + rel[3] * rel[3]);
+  float ang = atan2f(-rel[6], sy);
+  float deg = fminf(-ang * 180.0f / 3.14159265358979323846f, 39.0f);
+  int y = (int)rintf(deg);  // torch.round == round-half-even
+  int row = y < 0 ? (y < -39 ? 78 : 39 - y) : y;
+  return min(max(row, 0), m.rows - 1);
+}
+
 __global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
   const SmplxDev &m = a.m;
   const int b = blockIdx.x, t = threadIdx.x;
@@ -137,23 +156,7 @@ __global__ void __launch_bounds__(128) smplx_pose_kernel(PoseArgs a) {
       split_store(x, xh[k], xl[k]);
     }
   }
-  // dynamic-contour LUT row (lbs.py:30-41, rotation_utils.py:86-92)
-  if (t == 0 && m.D > 0) {
-    float rel[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    for (int q = 0; q < m.n_chain; ++q) {
-      const float *Rq = R[m.neck[q]];
-      float o[9];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) o[r * 3 + c] = Rq[r * 3] * rel[c] + Rq[r * 3 + 1] * rel[3 + c] + Rq[r * 3 + 2] * rel[6 + c];
-      for (int e = 0; e < 9; ++e) rel[e] = o[e];
-    }
-    float sy = sqrtf(rel[0] * rel[0] + rel[3] * rel[3]);
-    float ang = atan2f(-rel[6], sy);
-    float deg = fminf(-ang * 180.0f / 3.14159265358979323846f, 39.0f);
-    int y = (int)rintf(deg);  // torch.round == round-half-even
-    int row = y < 0 ? (y < -39 ? 78 : 39 - y) : y;
-    a.lut[b] = min(max(row, 0), m.rows - 1);
-  }
+  if (t == 0 && m.D > 0) a.lut[b] = contour_lut_row(m, R);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -866,6 +869,276 @@ __global__ void __launch_bounds__(128) smplx_chain_bwd_kernel(ChainBwdArgs a) {
   }
 }
 
+// ============================================================================================== keypoint Jacobian
+// The keypoints (joints + transl, expression zero) and their Jacobian (3K, P) with respect to the parameters
+// [delta_j (3 n_rot) | beta (NB) | t (3)], R_j(delta) = R_j Exp(delta_j), at delta = 0, with the backward's semantics
+// (constant LUT row, J14 overwrite, constant model buffers; DESIGN.md §6b).  One CTA per body.  Only the vertices the
+// keypoints reference are evaluated: a keypoint entry is one (vertex, weight) pair of a landmark or a J14 row, indexed
+// [static landmarks (3 L) | dynamic landmarks of the body's LUT row (3 D) | J14 rows (CSR order)].  Each entry's
+// vertex state (v_posed, M = sum_s w_s G_s.R and the posed vertex) is computed once into shared memory when the entries
+// fit there, else recomputed where it is used (same function, same bits).  A thread owns one (keypoint, column block)
+// and sums that block's entries in entry order: no atomics, and nothing depends on the rest of the batch.
+constexpr int kKpJacThreads = 256;
+constexpr int kKpState = 15;              // v_posed (3), M (9), posed vertex (3)
+constexpr int kKpCacheEntries = 2048;     // entries cached in shared memory (120 KB)
+
+struct KpJacArgs {
+  SmplxDev m;
+  const float *betas, *rot, *transl;      // transl may be null (zero)
+  int n_rot, Kp, P, n_entries, cached;
+  float *kp, *jac;
+};
+
+__device__ __forceinline__ void kp_entry(const SmplxDev &m, int row, int e, int &v, float &w) {
+  if (e < 3 * m.L) { v = m.lmk_vidx[e]; w = m.lmk_bc[e]; return; }
+  e -= 3 * m.L;
+  if (e < 3 * m.D) {
+    const size_t o = (size_t)row * m.D * 3 + e;
+    v = m.dyn_vidx[o]; w = m.dyn_bc[o];
+    return;
+  }
+  e -= 3 * m.D;
+  v = m.ex_col[e]; w = m.ex_val[e];
+}
+
+// entries [e0, e1) of keypoint k; false for a skeleton joint (not overwritten by a J14 row)
+__device__ __forceinline__ bool kp_range(const SmplxDev &m, int k, int &e0, int &e1) {
+  int r = -1;
+  for (int q = 0; q < m.n_over; ++q)
+    if (m.over_src[q] == k) r = m.over_tgt[q];
+  if (r >= 0) {
+    e0 = 3 * (m.L + m.D) + m.ex_ptr[r]; e1 = 3 * (m.L + m.D) + m.ex_ptr[r + 1];
+    return true;
+  }
+  if (k < m.J) return false;
+  e0 = 3 * (k - m.J); e1 = e0 + 3;
+  return true;
+}
+
+__device__ __forceinline__ float kp_jdir(const SmplxDev &m, int j, int c, int l) {
+  return m.J_dirs[((size_t)j * 3 + c) * m.NC + l];
+}
+
+// v_posed of vertex v (template, the NB shape rows, the fp32 posedirs rows below Kp, in that order), M and the posed
+// vertex sum_s w_s (G_s.R (v_posed - J_s) + G_s.t), the skinning weights in ELL order
+__device__ __forceinline__ void kp_vertex_state(const SmplxDev &m, int v, int Kp, const float *coef, const float *pf,
+                                                const float (*G)[12], const float (*Jr)[3], float *st) {
+  const int V3 = m.V * 3;
+  float p0 = m.v_template[3 * v], p1 = m.v_template[3 * v + 1], p2 = m.v_template[3 * v + 2];
+  for (int l = 0; l < m.NB; ++l) {
+    const float *S = m.basis + (size_t)l * m.V3p + 3 * v;
+    p0 += S[0] * coef[l]; p1 += S[1] * coef[l]; p2 += S[2] * coef[l];
+  }
+#pragma unroll 8
+  for (int k = 0; k < Kp; ++k) {
+    const float *P = m.posedirs + (size_t)k * V3 + 3 * v;
+    p0 += P[0] * pf[k]; p1 += P[1] * pf[k]; p2 += P[2] * pf[k];
+  }
+  float M[9], x[3];
+  for (int i = 0; i < 9; ++i) M[i] = 0.f;
+  x[0] = x[1] = x[2] = 0.f;
+  for (int s = 0; s < m.ell_w_n; ++s) {
+    const float w = m.ell_w[(size_t)s * m.V + v];
+    if (w == 0.f) continue;
+    const int j = m.ell_idx[(size_t)s * m.V + v];
+    const float q0 = p0 - Jr[j][0], q1 = p1 - Jr[j][1], q2 = p2 - Jr[j][2];
+    for (int r = 0; r < 3; ++r) {
+      x[r] += w * (G[j][r * 4] * q0 + G[j][r * 4 + 1] * q1 + G[j][r * 4 + 2] * q2 + G[j][r * 4 + 3]);
+      for (int c = 0; c < 3; ++c) M[r * 3 + c] += w * G[j][r * 4 + c];
+    }
+  }
+  st[0] = p0; st[1] = p1; st[2] = p2;
+  for (int i = 0; i < 9; ++i) st[3 + i] = M[i];
+  st[12] = x[0]; st[13] = x[1]; st[14] = x[2];
+}
+
+// d x_v / d delta_{j,a} into d[a][c]: the skinning term omega_a x (sum_{s in sub(j)} w_s (G_s.R (v_p - J_s) + G_s.t)
+// - W o_j), W = sum_{s in sub(j)} w_s, plus the pose-feature term M . P_v^(j) . vec(R_j [e_a]x) for j >= 1
+__device__ __forceinline__ void kp_vertex_drot(const SmplxDev &m, int v, int j, const float *st, const float (*G)[12],
+                                               const float (*Jr)[3], const float (*R)[9],
+                                               const unsigned long long *sub, float (&d)[3][3]) {
+  float Y0 = 0.f, Y1 = 0.f, Y2 = 0.f, W = 0.f;
+  for (int s = 0; s < m.ell_w_n; ++s) {
+    const float w = m.ell_w[(size_t)s * m.V + v];
+    if (w == 0.f) continue;
+    const int i = m.ell_idx[(size_t)s * m.V + v];
+    if (!((sub[i] >> j) & 1ull)) continue;
+    const float q0 = st[0] - Jr[i][0], q1 = st[1] - Jr[i][1], q2 = st[2] - Jr[i][2];
+    Y0 += w * (G[i][0] * q0 + G[i][1] * q1 + G[i][2] * q2 + G[i][3]);
+    Y1 += w * (G[i][4] * q0 + G[i][5] * q1 + G[i][6] * q2 + G[i][7]);
+    Y2 += w * (G[i][8] * q0 + G[i][9] * q1 + G[i][10] * q2 + G[i][11]);
+    W += w;
+  }
+  const float q0 = Y0 - W * G[j][3], q1 = Y1 - W * G[j][7], q2 = Y2 - W * G[j][11];
+  for (int a = 0; a < 3; ++a) {
+    const float w0 = G[j][a], w1 = G[j][4 + a], w2 = G[j][8 + a];
+    d[a][0] = w1 * q2 - w2 * q1; d[a][1] = w2 * q0 - w0 * q2; d[a][2] = w0 * q1 - w1 * q0;
+  }
+  if (j == 0) return;
+  float P[9][3];
+  const float *Pj = m.posedirs + (size_t)9 * (j - 1) * m.V * 3 + 3 * v;
+  for (int e = 0; e < 9; ++e)
+    for (int c = 0; c < 3; ++c) P[e][c] = Pj[(size_t)e * m.V * 3 + c];
+  for (int a = 0; a < 3; ++a) {
+    // R_j [e_a]x: column c is R_j (e_a x e_c), the column of R_j at (a + 2) % 3 or (a + 1) % 3, signed
+    float D[9];
+    const int a1 = (a + 1) % 3, a2 = (a + 2) % 3;
+    for (int r = 0; r < 3; ++r) {
+      D[r * 3 + a] = 0.f;
+      D[r * 3 + a1] = R[j][r * 3 + a2];
+      D[r * 3 + a2] = -R[j][r * 3 + a1];
+    }
+    float dv[3];
+    for (int c = 0; c < 3; ++c) {
+      float s = 0.f;
+      for (int e = 0; e < 9; ++e) s += P[e][c] * D[e];
+      dv[c] = s;
+    }
+    for (int r = 0; r < 3; ++r) d[a][r] += st[3 + r * 3] * dv[0] + st[4 + r * 3] * dv[1] + st[5 + r * 3] * dv[2];
+  }
+}
+
+// d x_v / d beta_l = M S_l[v] + sum_s w_s (dG_s.t/dbeta_l - G_s.R dJ_s/dbeta_l)
+__device__ __forceinline__ void kp_vertex_dbeta(const SmplxDev &m, int v, int l, const float *st,
+                                                const float (*G)[12], const float (*dGt)[3][kMaxCoef],
+                                                float (&d)[3]) {
+  const float *S = m.basis + (size_t)l * m.V3p + 3 * v;
+  const float s0 = S[0], s1 = S[1], s2 = S[2];
+  for (int c = 0; c < 3; ++c) d[c] = st[3 + c * 3] * s0 + st[4 + c * 3] * s1 + st[5 + c * 3] * s2;
+  for (int s = 0; s < m.ell_w_n; ++s) {
+    const float w = m.ell_w[(size_t)s * m.V + v];
+    if (w == 0.f) continue;
+    const int i = m.ell_idx[(size_t)s * m.V + v];
+    const float j0 = kp_jdir(m, i, 0, l), j1 = kp_jdir(m, i, 1, l), j2 = kp_jdir(m, i, 2, l);
+    for (int c = 0; c < 3; ++c)
+      d[c] += w * (dGt[i][c][l] - (G[i][c * 4] * j0 + G[i][c * 4 + 1] * j1 + G[i][c * 4 + 2] * j2));
+  }
+}
+
+__global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a) {
+  const SmplxDev &m = a.m;
+  const int b = blockIdx.x, t = threadIdx.x;
+  __shared__ float R[kMaxJoints][9];
+  __shared__ float Jr[kMaxJoints][3];
+  __shared__ float G[kMaxJoints][12];
+  __shared__ float coef[kMaxCoef];
+  __shared__ float pf[(kMaxJoints - 1) * 9];
+  __shared__ float dGt[kMaxJoints][3][kMaxCoef];    // dG_j.t / dbeta
+  __shared__ unsigned long long sub[kMaxJoints];    // bit i of sub[s]: i is s or one of its ancestors
+  __shared__ int lut_row;
+  extern __shared__ float cache[];                  // [n_entries][kKpState] when cached
+  const int NB = m.NB;
+  body_chain(m, a.betas, nullptr, a.rot, a.n_rot, b, R, Jr, G, coef);
+  if (t == 0) {
+    for (int s = 0; s < m.J; ++s) sub[s] = (s ? sub[m.parents[s]] : 0ull) | (1ull << s);
+    lut_row = m.D > 0 ? contour_lut_row(m, R) : 0;
+  }
+  for (int k = t; k < a.Kp; k += blockDim.x) {
+    const int j = 1 + k / 9, e = k % 9;
+    pf[k] = R[j][e] - ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f);
+  }
+  // dG_j.t / dbeta level by level: dG_0.t = dJ_0, dG_j.t = G_p.R (dJ_j - dJ_p) + dG_p.t
+  for (int i = t; i < 3 * NB; i += blockDim.x) dGt[0][i / NB][i % NB] = kp_jdir(m, 0, i / NB, i % NB);
+  __syncthreads();
+  for (int lv = 1; lv < m.n_levels; ++lv) {
+    const int off = m.level_off[lv], cnt = m.level_off[lv + 1] - off;
+    for (int i = t; i < cnt * 3 * NB; i += blockDim.x) {
+      const int j = m.level_joints[off + i / (3 * NB)], c = (i / NB) % 3, l = i % NB, p = m.parents[j];
+      const float r0 = kp_jdir(m, j, 0, l) - kp_jdir(m, p, 0, l), r1 = kp_jdir(m, j, 1, l) - kp_jdir(m, p, 1, l),
+                  r2 = kp_jdir(m, j, 2, l) - kp_jdir(m, p, 2, l);
+      dGt[j][c][l] = G[p][c * 4] * r0 + G[p][c * 4 + 1] * r1 + G[p][c * 4 + 2] * r2 + dGt[p][c][l];
+    }
+    __syncthreads();
+  }
+  const int row = lut_row;
+  if (a.cached) {
+    for (int e = t; e < a.n_entries; e += blockDim.x) {
+      int v;
+      float w;
+      kp_entry(m, row, e, v, w);
+      kp_vertex_state(m, v, a.Kp, coef, pf, G, Jr, cache + (size_t)e * kKpState);
+    }
+    __syncthreads();
+  }
+  // work items (keypoint k, column block g): g < n_rot the 3 x 3 block of delta_g, g = n_rot the betas, g = n_rot + 1
+  // the translation and the keypoint itself
+  const int NG = a.n_rot + 2, P = a.P, K = m.K;
+  const float *tr = a.transl ? a.transl + (size_t)b * 3 : nullptr;
+  float *jb = a.jac + (size_t)b * 3 * K * P;
+  float local[kKpState];
+  for (int i = t; i < K * NG; i += blockDim.x) {
+    const int k = i / NG, g = i % NG;
+    int e0 = 0, e1 = 0;
+    const bool mix = kp_range(m, k, e0, e1);
+    float *o = jb + (size_t)3 * k * P;          // row 3 k + c at o + c P
+    auto state = [&](int e, int &v, float &w) -> const float * {
+      kp_entry(m, row, e, v, w);
+      if (a.cached) return cache + (size_t)e * kKpState;
+      kp_vertex_state(m, v, a.Kp, coef, pf, G, Jr, local);
+      return local;
+    };
+    if (g < a.n_rot) {
+      float acc[3][3];                           // [a][c]
+      for (int x = 0; x < 3; ++x) acc[x][0] = acc[x][1] = acc[x][2] = 0.f;
+      if (!mix) {
+        if (g != k && ((sub[k] >> g) & 1ull)) {  // omega_a x (J_k - o_g) for a proper ancestor g
+          const float q0 = G[k][3] - G[g][3], q1 = G[k][7] - G[g][7], q2 = G[k][11] - G[g][11];
+          for (int x = 0; x < 3; ++x) {
+            const float w0 = G[g][x], w1 = G[g][4 + x], w2 = G[g][8 + x];
+            acc[x][0] = w1 * q2 - w2 * q1; acc[x][1] = w2 * q0 - w0 * q2; acc[x][2] = w0 * q1 - w1 * q0;
+          }
+        }
+      } else {
+        for (int e = e0; e < e1; ++e) {
+          int v;
+          float w;
+          const float *st = state(e, v, w);
+          float d[3][3];
+          kp_vertex_drot(m, v, g, st, G, Jr, R, sub, d);
+          for (int x = 0; x < 3; ++x)
+            for (int c = 0; c < 3; ++c) acc[x][c] += w * d[x][c];
+        }
+      }
+      for (int c = 0; c < 3; ++c)
+        for (int x = 0; x < 3; ++x) o[(size_t)c * P + 3 * g + x] = acc[x][c];
+    } else if (g == a.n_rot) {
+      for (int l = 0; l < NB; ++l) {
+        float acc[3] = {0.f, 0.f, 0.f};
+        if (!mix) {
+          for (int c = 0; c < 3; ++c) acc[c] = dGt[k][c][l];
+        } else {
+          for (int e = e0; e < e1; ++e) {
+            int v;
+            float w;
+            const float *st = state(e, v, w);
+            float d[3];
+            kp_vertex_dbeta(m, v, l, st, G, dGt, d);
+            for (int c = 0; c < 3; ++c) acc[c] += w * d[c];
+          }
+        }
+        for (int c = 0; c < 3; ++c) o[(size_t)c * P + 3 * a.n_rot + l] = acc[c];
+      }
+    } else {
+      float x[3];
+      if (!mix) {
+        for (int c = 0; c < 3; ++c) x[c] = G[k][c * 4 + 3];
+      } else {
+        x[0] = x[1] = x[2] = 0.f;
+        for (int e = e0; e < e1; ++e) {
+          int v;
+          float w;
+          const float *st = state(e, v, w);
+          for (int c = 0; c < 3; ++c) x[c] += w * st[12 + c];
+        }
+      }
+      for (int c = 0; c < 3; ++c) {
+        a.kp[((size_t)b * K + k) * 3 + c] = tr ? x[c] + tr[c] : x[c];
+        for (int x2 = 0; x2 < 3; ++x2) o[(size_t)c * P + 3 * a.n_rot + NB + x2] = c == x2 ? 1.f : 0.f;
+      }
+    }
+  }
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -994,6 +1267,7 @@ extern "C" int shapy_smplx_create(shapy_smplx_t **out, const shapy_smplx_desc_t 
   s.ex_ptr = upload(m->allocs, ep, err);
   s.ex_col = upload(m->allocs, ec, err);
   s.ex_val = upload(m->allocs, ev, err);
+  m->extra_nnz = (int)ec.size();
   s.n_over = s.n_extra ? d->num_overwrite : 0;
   std::vector<int> os(s.n_over), ot(s.n_over);
   for (int i = 0; i < s.n_over; ++i) { os[i] = (int)d->source_idxs[i]; ot[i] = (int)d->target_idxs[i]; }
@@ -1369,6 +1643,25 @@ extern "C" int shapy_smplx_backward(const shapy_smplx_t *m, const float *betas, 
   ChainBwdArgs ca{d, betas, ex, rot, n_rot, Kp, ws.gA, kp ? ws.gP : nullptr, pf ? ws.pf_part : nullptr,
                   NR ? ws.gcoef : nullptr, NR, grad_rot, grad_betas, grad_expr};
   smplx_chain_bwd_kernel<<<B, 128, 0, st>>>(ca);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" int shapy_smplx_keypoint_jacobian(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
+                                             const float *transl, int B, float *keypoints, float *jac, void *stream) {
+  SHAPY_REQUIRE(m && betas && rot && keypoints && jac, "shapy_smplx_keypoint_jacobian: null argument");
+  SHAPY_REQUIRE(B >= 0, "shapy_smplx_keypoint_jacobian: batch %d", B);
+  SHAPY_REQUIRE(n_rot >= 1 && n_rot <= m->d.J, "shapy_smplx_keypoint_jacobian: n_rot %d out of range", n_rot);
+  if (B == 0) return SHAPY_OK;
+  const SmplxDev &d = m->d;
+  const int n_entries = 3 * (d.L + d.D) + m->extra_nnz;
+  const int cached = n_entries <= kKpCacheEntries;
+  const size_t smem = cached ? (size_t)n_entries * kKpState * sizeof(float) : 0;
+  // the static shared memory (33.6 KB) plus the entry cache passes the 48 KB a launch gets without opting in
+  if (smem > 0)
+    SHAPY_CUDA_TRY(cudaFuncSetAttribute(smplx_kp_jac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  KpJacArgs a{d, betas, rot, transl, n_rot, (n_rot - 1) * 9, 3 * n_rot + d.NB + 3, n_entries, cached, keypoints, jac};
+  smplx_kp_jac_kernel<<<B, kKpJacThreads, smem, (cudaStream_t)stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

@@ -50,6 +50,7 @@ struct shapy_smplx {
   mutable std::mutex pw_mu;
   mutable std::map<int, PoseW> pw;
   float *zero_bias = nullptr;   // [V3g]
+  int extra_nnz = 0;            // non-zeros of the J14 regressor (host copy of ex_ptr[n_extra])
 };
 
 namespace shapy {

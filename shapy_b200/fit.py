@@ -26,6 +26,14 @@ fit_body_to_keypoints optimises the raw 6D global and body pose (through the 6D 
 body against its K 3D keypoints (the model's joints output: posed joints, landmarks, J14 overwrite), loss per body
 sum_k w_k |joint_k - keypoint_k|^2, with the same batched Adam: SMPLX.forward and the decoder are differentiable
 (shapy_b200.autograd), and a body's gradient does not depend on the rest of the batch.
+
+fit_body_to_keypoints(..., method='lm') fits the same loss (a keypoint with weight <= 0 dropped) with a batched
+Levenberg-Marquardt loop: the raw 6D start is decoded once, and each iteration evaluates the trial's keypoints and
+their (3K, P) Jacobian with respect to right-multiplied rotation tangents, betas and transl in one launch
+(ops.smplx_keypoint_jacobian), then takes one damped Gauss-Newton step per body (ops.fit_lm_keypoints_step: the
+measurement LM's policy, the P x P normal equations in fp64, the next rotations R Exp(delta) re-orthonormalised).  Two
+launches per iteration, no host synchronisation, and one SMPLX.forward at the end gives the returned keypoints and
+loss.  keypoint_jacobian(body_model, rot, betas, transl) exposes the Jacobian itself.
 """
 import argparse
 import json
@@ -145,14 +153,32 @@ def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, be
 IDENT6 = (1.0, 0.0, 0.0, 1.0, 0.0, 0.0)      # the 6D code of the identity rotation (row-major 3x2)
 
 
-def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=600, lr=0.05, init=None):
+def keypoint_jacobian(body_model, rot, betas, transl=None):
+    """The model's keypoints (its joints output, expression zero, plus transl) and their Jacobian without autograd:
+    rot (B, n_rot, 3, 3) of the first n_rot joints, betas (B, NB), transl (B, 3) or None.  Returns {'keypoints'
+    (B, K, 3), 'jacobian' (B, 3K, 3 n_rot + NB + 3)}, columns [delta_j (R_j Exp(delta_j) at delta = 0) | betas |
+    transl], with the semantics of the SMPL-X backward (constant LUT row, J14 overwrite)."""
+    from . import ops
+    device = body_model.shapedirs.device
+    f = lambda t: None if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).detach().contiguous()  # noqa: E731
+    kp, jac = ops.smplx_keypoint_jacobian(body_model.packed(device), f(betas), f(rot), f(transl))
+    return {'keypoints': kp, 'jacobian': jac}
+
+
+def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam'):
     """Fits pose and shape so that the model's keypoints match `keypoints` (B, K, 3), K = body_model's keypoint count.
 
     weights: None (all 1), (K,) or (B, K) per-keypoint weights.  init: optional {'global_rot': (B, 6),
     'body_pose': (B, 126) raw 6D, 'betas': (B, NB), 'transl': (B, 3)}; a missing entry starts at the identity pose,
-    zero betas or zero transl.  Adam with the step size decaying geometrically from lr to lr / 100.
+    zero betas or zero transl.  method: 'adam' (the default: the step size decays geometrically from lr to lr / 100)
+    or 'lm' (batched Levenberg-Marquardt on the keypoint Jacobian, see the top; `lr` is ignored, a keypoint with
+    weight <= 0 is dropped).  iterations: None means 600 for Adam and 50 for LM.
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (B, 1, 3, 3),
     'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss}."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if iterations is None:
+        iterations = 600 if method == 'adam' else 50
     from .autograd import Rot6dFunction
     device = body_model.shapedirs.device
     kp = torch.as_tensor(keypoints, dtype=torch.float32, device=device)
@@ -161,14 +187,17 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=600, l
                                                                              device=device)
     w = w.expand(B, K).contiguous()
     init = init or {}
-    ident = torch.tensor(IDENT6, device=device)
+    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
+    ident[0::3].fill_(1.0)
     start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
              'betas': torch.zeros(B, body_model.num_betas, device=device), 'transl': torch.zeros(B, 3, device=device)}
     params = {}
     for k, v in start.items():
         t = init.get(k)
         t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
-        params[k] = t.detach().clone().contiguous().requires_grad_(True)
+        params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    if method == 'lm':
+        return _fit_keypoints_lm(body_model, kp, w, params, int(iterations))
     opt = torch.optim.Adam(list(params.values()), lr=lr)
     sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
 
@@ -192,6 +221,36 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=600, l
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, loss=per_body)
     return res
+
+
+def _fit_keypoints_lm(body_model, kp, w, params, iterations):
+    from . import ops
+    device = kp.device
+    packed = body_model.packed(device)
+    B, K = kp.shape[0], kp.shape[1]
+    n_rot, nb = 22, params['betas'].shape[1]
+    P = 3 * n_rot + nb + 3
+    trial = {'rot': ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1)).contiguous(),
+             'betas': params['betas'].contiguous(), 'transl': params['transl'].contiguous()}
+    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+    state = {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), 'transl': mk(B, 3), 'keypoints': mk(B, K, 3),
+             'jac': mk(B, 3 * K, P), 'loss': mk(B), 'lambda': mk(B),
+             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    tg = kp.contiguous()
+    if B > 0:
+        for it in range(iterations + 1):
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
+            ops.fit_lm_keypoints_step(state, trial, tg, w, LM_UP, LM_DOWN, it == 0, tkp, tjac)
+    rot = state['rot']
+    with torch.no_grad():
+        out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], transl=state['transl'],
+                         return_shaped=False)
+        joints = out['joints'][:]
+        per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
+    raw = rot[..., :2].reshape(B, n_rot * 6)       # the first two columns in the decoder's row-major 3x2 layout
+    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
+            'transl': state['transl'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], 'keypoints': joints,
+            'loss': per_body}
 
 
 def main(argv=None):

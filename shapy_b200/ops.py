@@ -396,6 +396,60 @@ def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, f
                                       stream_ptr()), 'fit_lm_step')
 
 
+def smplx_keypoint_jacobian(model: SmplxModel, betas, rot, transl=None):
+    """The keypoints (B, K, 3) of smplx_forward (its joints, expression zero) plus transl, and their Jacobian
+    (B, 3K, P), P = 3 n_rot + NB + 3, with respect to [delta_j (right-multiplied tangents R_j Exp(delta_j)) | betas |
+    transl], in one launch (include/shapy_b200.h, shapy_smplx_keypoint_jacobian).  Returns (keypoints, jac)."""
+    betas = _cuda_f32(betas, 'betas')
+    rot = _cuda_f32(rot, 'rot')
+    B, n_rot = rot.shape[0], rot.shape[1]
+    if rot.shape[2:] != (3, 3) or betas.shape != (B, model.NB):
+        raise RuntimeError(f'rot must be (B, n_rot, 3, 3) and betas ({B}, {model.NB}), got {tuple(rot.shape)} and '
+                           f'{tuple(betas.shape)}')
+    transl = None if transl is None else _cuda_f32(transl, 'transl')
+    if transl is not None and transl.shape != (B, 3):
+        raise RuntimeError(f'transl must be ({B}, 3), got {tuple(transl.shape)}')
+    dev = betas.device
+    kp = torch.empty(B, model.K, 3, dtype=torch.float32, device=dev)
+    jac = torch.empty(B, 3 * model.K, 3 * n_rot + model.NB + 3, dtype=torch.float32, device=dev)
+    if B == 0:
+        return kp, jac
+    with torch.cuda.device(dev):
+        check(lib().shapy_smplx_keypoint_jacobian(model.handle, ptr(betas), ptr(rot), n_rot, ptr(transl), B, ptr(kp),
+                                                  ptr(jac), stream_ptr()), 'smplx_keypoint_jacobian')
+    return kp, jac
+
+
+def fit_lm_keypoints_step(state, trial, targets, weights, lambda_up, lambda_down, first, trial_keypoints, trial_jac):
+    """One Levenberg-Marquardt step per body of the keypoint fit (include/shapy_b200.h, shapy_fit_lm_keypoints_step),
+    in place.  state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB), 'transl' (B, 3), 'keypoints' (B, K, 3), 'jac'
+    (B, 3K, P), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32}; trial: {'rot', 'betas', 'transl'}, the evaluated
+    trial on entry and the next trial on return; targets (B, K, 3), weights (B, K)."""
+    B, n_rot = trial['rot'].shape[:2]
+    nb, K = trial['betas'].shape[1], targets.shape[1]
+    ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + \
+        [trial[k] for k in ('rot', 'betas', 'transl')] + [targets, weights, trial_keypoints, trial_jac]
+    for t in ts + [state['accepted']]:
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
+            raise RuntimeError('fit_lm_keypoints_step: every tensor must be a contiguous CUDA tensor')
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise RuntimeError('fit_lm_keypoints_step: the state, trial, targets and weights must be float32')
+    if state['accepted'].dtype != torch.int32:
+        raise RuntimeError('fit_lm_keypoints_step: accepted must be int32')
+    P = 3 * n_rot + nb + 3
+    if trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K):
+        raise RuntimeError(f'fit_lm_keypoints_step: jac must be ({B}, {3 * K}, {P}) and weights ({B}, {K})')
+    if B == 0:
+        return
+    with torch.cuda.device(trial['rot'].device):
+        check(lib().shapy_fit_lm_keypoints_step(
+            B, K, n_rot, nb, ptr(targets), ptr(weights), float(lambda_up), float(lambda_down), int(bool(first)),
+            *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+            ptr(trial['rot']), ptr(trial['betas']), ptr(trial['transl']), ptr(trial_keypoints), ptr(trial_jac),
+            stream_ptr()), 'fit_lm_keypoints_step')
+
+
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
     """grad_betas (B, NB) = shapedirs^T . grad_v_shaped (B, V, 3): the adjoint of smplx_forward_shape."""
     g = _cuda_f32(grad_v_shaped, 'grad_v_shaped')
