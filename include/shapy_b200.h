@@ -233,6 +233,27 @@ int shapy_fit_lm_keypoints_step(int batch, int num_keypoints, int n_rot, int nb,
                                 int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
                                 const float *trial_keypoints, const float *trial_jac, void *stream);
 
+/* shapy_fit_lm_keypoints_step with the five virtual measurements and a betas regulariser stacked under the keypoint
+ * rows: one Gauss-Newton step on L = L_kp + sum_{w_k > 0} w_k (t_k - m_k)^2 + betas_weight |beta|^2, summed left to
+ * right, L_kp as in shapy_fit_lm_keypoints_step, the measurement terms in k order (mass, height, chest, waist, hips),
+ * |beta|^2 in l order.  meas_targets, meas_weights (B,5); the state adds meas (B,5) and meas_jac (B,5,nb), the trial
+ * trial_meas / trial_meas_jac (shapy_measure_jacobian_betas at the trial betas); on accept they are copied into the
+ * state too.  A measurement with weight <= 0 is dropped (its value and Jacobian row are never read and may be NaN); a
+ * weighted NaN trial measurement makes the trial loss NaN, so the trial is rejected.  Normal equations: A = J_kp^T W
+ * J_kp, then + J_m^T W_m J_m in the betas block (k order); g = J_kp^T W (kp - target), then + J_m^T W_m (m - t), then
+ * + betas_weight beta.  The first lambda is 1e-3 max(diag A, 1e-6), without betas_weight; the diagonal then gets
+ * betas_weight + lambda on the betas columns and lambda elsewhere.  The policy, the solve and the next trial are those
+ * of shapy_fit_lm_keypoints_step.  With every measurement weight <= 0 and betas_weight = 0 the outputs equal
+ * shapy_fit_lm_keypoints_step's bit for bit.  A null pointer, betas_weight < 0 or a lambda factor < 1:
+ * SHAPY_ERR_ARG; P > 96: SHAPY_ERR_UNSUPPORTED.  batch 0: no launch. */
+int shapy_fit_lm_keypoints_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *meas_targets, const float *meas_weights, float betas_weight, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+    const float *trial_keypoints, const float *trial_jac, const float *trial_meas, const float *trial_meas_jac,
+    void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

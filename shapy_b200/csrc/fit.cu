@@ -163,6 +163,13 @@ __global__ void __launch_bounds__(128) lm_step_kernel(LmArgs a) {
 // lambda / down or * up, clamped; then (J^T W J + lambda I) delta = -J^T W (kp - target) by a right-looking Cholesky of
 // the P x P normal matrix in fp64 shared memory, and the next trial R_j Exp(delta_j) (Rodrigues in fp64, re-orthonormalised
 // by the 6D decoder's Gram-Schmidt of the first two columns), beta + delta_beta, t + delta_t, rounded to fp32.
+//
+// MEAS (shapy_fit_lm_keypoints_measurements_step) stacks the five virtual measurements and the betas regulariser under
+// the keypoint rows: L = L_kp + sum_{w_k > 0} w_k (t_k - m_k)^2 (k order) + rho |beta|^2 (l order), left to right.  The
+// measurement Jacobian (5, NB) only has betas columns, so its rows are accumulated after the keypoint rows into the
+// betas block of A and g (k order), then rho beta into g; the first lambda comes from diag(A) without rho (as in
+// lm_step_kernel) and the betas diagonal gets (double)rho + (double)lambda.  With every measurement weight <= 0 and
+// rho = 0 each extra term is skipped or adds an exact 0, so the step equals the keypoint step bit for bit.
 constexpr int kLmKpMaxP = 96;
 constexpr int kLmKpThreads = 256;
 constexpr int kLmKpPairs = (kLmKpMaxP * (kLmKpMaxP + 1) / 2 + kLmKpThreads - 1) / kLmKpThreads;
@@ -179,7 +186,15 @@ struct LmKpArgs {
   const float *tkp, *tjac;
 };
 
-__global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
+struct LmMeasArgs {                     // the measurement block of the MEAS step (unused otherwise)
+  const float *targets, *weights;       // (B, 5): mass, height, chest, waist, hips
+  float rho;                            // betas_weight
+  float *meas, *jac;                    // state (B, 5), (B, 5, NB)
+  const float *tmeas, *tjac;            // the trial's
+};
+
+template <bool MEAS>
+__global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, LmMeasArgs mb) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of J^T W J + lambda I, then its Cholesky factor
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
   __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
@@ -199,6 +214,24 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
                    r2 = (double)m[3 * k + 2] - (double)tg[3 * k + 2];
       L += w * (r0 * r0 + r1 * r1 + r2 * r2);
     }
+    if constexpr (MEAS) {
+      const float *tm = mb.tmeas + (size_t)b * 5, *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+      double Lm = 0.0;
+      for (int k = 0; k < 5; ++k) {
+        const double w = mw[k];
+        if (w > 0.0) {                     // a dropped term is never read: its measurement may be NaN
+          const double r = (double)mt[k] - (double)tm[k];
+          Lm += w * r * r;
+        }
+      }
+      L += Lm;
+      if (mb.rho > 0.f) {
+        const float *tb = a.tbetas + (size_t)b * a.nb;
+        double reg = 0.0;
+        for (int l = 0; l < a.nb; ++l) reg += (double)tb[l] * (double)tb[l];
+        L += (double)mb.rho * reg;
+      }
+    }
     lt_s = L;
   }
   __syncthreads();
@@ -215,6 +248,10 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
     if (t < 3) a.transl[(size_t)b * 3 + t] = a.ttransl[(size_t)b * 3 + t];
     for (int i = t; i < R3; i += blockDim.x) a.kp[(size_t)b * R3 + i] = M[i];
     for (size_t i = t; i < (size_t)R3 * P; i += blockDim.x) a.jac[(size_t)b * R3 * P + i] = J[i];
+    if constexpr (MEAS) {
+      for (int i = t; i < 5; i += blockDim.x) mb.meas[(size_t)b * 5 + i] = mb.tmeas[(size_t)b * 5 + i];
+      for (int i = t; i < 5 * a.nb; i += blockDim.x) mb.jac[(size_t)b * 5 * a.nb + i] = mb.tjac[(size_t)b * 5 * a.nb + i];
+    }
     if (t == 0) a.loss[b] = lnew;
   }
   // 3. normal equations: A_ij = sum_rows (w J_ri) J_rj (i >= j), g_i = sum_rows (w J_ri) (kp_r - target_r), rows in
@@ -261,6 +298,38 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
       if (t < P) g += WJs[row][t] * rs[row];
     }
   }
+  if constexpr (MEAS) {
+    // the five measurement rows, staged like the keypoint rows, into the betas block [o, o + nb) of A and g
+    const int o = 3 * a.n_rot, nb = a.nb;
+    const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+    const float *Jm = (accept ? mb.tjac : mb.jac) + (size_t)b * 5 * nb;
+    const float *Mm = (accept ? mb.tmeas : mb.meas) + (size_t)b * 5;
+    __syncthreads();
+    for (int i = t; i < 5; i += blockDim.x) {
+      const double w = mw[i];
+      ws[i] = w;
+      rs[i] = w > 0.0 ? (double)Mm[i] - (double)mt[i] : 0.0;
+    }
+    for (int i = t; i < 5 * nb; i += blockDim.x) {
+      const int row = i / nb;
+      const double w = mw[row];
+      if (w > 0.0) {                       // a dropped term's row is never read: it may be NaN
+        const double x = Jm[i];
+        Js[row][i % nb] = x;
+        WJs[row][i % nb] = w * x;
+      }
+    }
+    __syncthreads();
+    for (int row = 0; row < 5; ++row) {
+      if (!(ws[row] > 0.0)) continue;
+#pragma unroll
+      for (int i = 0; i < kLmKpPairs; ++i)
+        if (pc[i] >= o && pr[i] >= 0 && pr[i] < o + nb) acc[i] += WJs[row][pr[i] - o] * Js[row][pc[i] - o];
+      if (t >= o && t < o + nb) g += WJs[row][t - o] * rs[row];
+    }
+    if (mb.rho > 0.f && t >= o && t < o + nb)
+      g += (double)mb.rho * (double)(accept ? a.tbetas : a.betas)[(size_t)b * nb + t - o];
+  }
 #pragma unroll
   for (int i = 0; i < kLmKpPairs; ++i)
     if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
@@ -280,7 +349,13 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
     lam = fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
     a.lambda[b] = lam;
     if (accept && !a.first) a.accepted[b] += 1;
-    for (int j = 0; j < P; ++j) A[j * P + j] += (double)lam;
+    if constexpr (MEAS) {
+      const int o = 3 * a.n_rot;
+      const double damp = (double)mb.rho + (double)lam;
+      for (int j = 0; j < P; ++j) A[j * P + j] += j >= o && j < o + a.nb ? damp : (double)lam;
+    } else {
+      for (int j = 0; j < P; ++j) A[j * P + j] += (double)lam;
+    }
     ok_s = isfinite(lnew);               // a body without a finite loss does not move
   }
   // 4. Cholesky A = L L^T, right-looking: column j scaled, then the trailing lower triangle updated
@@ -370,6 +445,18 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a) {
   }
 }
 
+template <bool MEAS>
+int launch_lm_kp(int batch, const LmKpArgs &a, const LmMeasArgs &m, void *stream) {
+  const size_t smem = (size_t)a.P * a.P * sizeof(double);
+  // with the 25 KB of static shared memory
+  if (smem + 25 * 1024 > 48 * 1024)
+    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp_step_kernel<MEAS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)smem));
+  lm_kp_step_kernel<MEAS><<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, m);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -414,13 +501,36 @@ extern "C" int shapy_fit_lm_keypoints_step(int batch, int num_keypoints, int n_r
     return SHAPY_ERR_UNSUPPORTED;
   }
   if (batch == 0) return SHAPY_OK;
-  const size_t smem = (size_t)P * P * sizeof(double);
-  // with the 25 KB of static shared memory
-  if (smem + 25 * 1024 > 48 * 1024)
-    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   LmKpArgs a{num_keypoints, n_rot, nb, P, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
-  lm_kp_step_kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a);
-  SHAPY_LAUNCH_CHECK();
-  return SHAPY_OK;
+  return launch_lm_kp<false>(batch, a, LmMeasArgs{}, stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *meas_targets, const float *meas_weights, float betas_weight, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+    const float *trial_keypoints, const float *trial_jac, const float *trial_meas, const float *trial_meas_jac,
+    void *stream) {
+  SHAPY_REQUIRE(targets && weights && meas_targets && meas_weights && rot && betas && transl && keypoints && jac &&
+                    meas && meas_jac && loss && lambda && accepted && trial_rot && trial_betas && trial_transl &&
+                    trial_keypoints && trial_jac && trial_meas && trial_meas_jac,
+                "shapy_fit_lm_keypoints_measurements_step: null argument");
+  SHAPY_REQUIRE(batch >= 0 && num_keypoints >= 1 && n_rot >= 1 && n_rot <= 64 && nb >= 1,
+                "shapy_fit_lm_keypoints_measurements_step: bad size (batch %d, %d keypoints, n_rot %d, %d betas)",
+                batch, num_keypoints, n_rot, nb);
+  SHAPY_REQUIRE(lambda_up >= 1.f && lambda_down >= 1.f && betas_weight >= 0.f,
+                "shapy_fit_lm_keypoints_measurements_step: lambda_up and lambda_down must be >= 1 and betas_weight "
+                ">= 0");
+  const int P = 3 * n_rot + nb + 3;
+  if (P > kLmKpMaxP) {
+    set_error("shapy_fit_lm_keypoints_measurements_step: %d parameters, at most %d are supported", P, kLmKpMaxP);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  if (batch == 0) return SHAPY_OK;
+  LmKpArgs a{num_keypoints, n_rot, nb, P, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmMeasArgs m{meas_targets, meas_weights, betas_weight, meas, meas_jac, trial_meas, trial_meas_jac};
+  return launch_lm_kp<true>(batch, a, m, stream);
 }

@@ -34,6 +34,18 @@ their (3K, P) Jacobian with respect to right-multiplied rotation tangents, betas
 measurement LM's policy, the P x P normal equations in fp64, the next rotations R Exp(delta) re-orthonormalised).  Two
 launches per iteration, no host synchronisation, and one SMPLX.forward at the end gives the returned keypoints and
 loss.  keypoint_jacobian(body_model, rot, betas, transl) exposes the Jacobian itself.
+
+fit_body_to_keypoints(..., body_measurements=bm, measurements={'height': h, 'mass': m, ...}) fits the keypoints and
+known measurements of the same bodies together, loss per body: the keypoint loss + the measurement loss of
+fit_betas_to_measurements on the T-pose of the fitted betas (same targets, weights and dropping rule) +
+betas_weight |betas|^2.  Keypoints pin down the bone lengths, the measurements the soft tissue behind the
+circumferences and the mass; fitting one after the other lets the second fit undo the first.  With Adam the
+measurement term goes through forward_shape and BodyMeasurements.forward_vertices; with method='lm' each iteration
+stacks the five measurement rows under the keypoint rows of one damped Gauss-Newton step (four launches: the keypoint
+Jacobian, forward_shape and the measurement Jacobian of the trial, then ops.fit_lm_keypoints_measurements_step), no
+host synchronisation, and every body's total loss is non-increasing.  The measurement rows have the measurement
+backward's semantics (constant barycentrics, no gradient through the plane heights), so they are not the exact
+derivative of a circumference: LM may reject more steps, but accept / reject uses the true loss.
 """
 import argparse
 import json
@@ -56,6 +68,23 @@ def _targets(targets, B, device):
     return out
 
 
+def _measurement_terms(targets, weights, B, device):
+    """(targets (B, 5), weights (B, 5)) in NAMES order: the weight is 0 where the target is <= 0 or the weight is
+    <= 1e-3 (fit_measurements.py:111-133), and such a target is clamped to 0."""
+    tg = _targets(targets, B, device)
+    w = dict(DEFAULT_WEIGHTS, **(weights or {}))
+    wt = torch.stack([torch.where(tg[k] > 0, torch.full_like(tg[k], w[k]), torch.zeros_like(tg[k]))
+                      if w[k] > 1e-3 else torch.zeros_like(tg[k]) for k in NAMES], 1)
+    tgt = torch.stack([tg[k].clamp(min=0) for k in NAMES], 1)
+    return tgt, wt
+
+
+def _measurement_loss(tgt, wt, meas, betas, betas_weight):
+    """sum_k w_k (t_k - m_k)^2 + betas_weight |betas|^2 per body; a dropped term passes no (NaN) value or gradient."""
+    diff = torch.where(wt > 0, tgt - meas, torch.zeros_like(meas))
+    return (wt * diff.pow(2)).sum(1) + betas_weight * betas.pow(2).sum(1)
+
+
 def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
                               lr=0.05, betas_init=None, batch_size=None, method='adam'):
     """Fits betas (B, NB) so that the model's T-pose measurements match `targets`.
@@ -75,12 +104,7 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     B = batch_size or max([torch.as_tensor(v).numel() for v in targets.values()] + [1])
     if betas_init is not None:
         B = betas_init.shape[0]
-    tg = _targets(targets, B, device)
-    w = dict(DEFAULT_WEIGHTS, **(weights or {}))
-    # per-body weight: 0 where the target is <= 0 or the weight is <= 1e-3 (fit_measurements.py:111-133)
-    wt = torch.stack([torch.where(tg[k] > 0, torch.full_like(tg[k], w[k]), torch.zeros_like(tg[k]))
-                      if w[k] > 1e-3 else torch.zeros_like(tg[k]) for k in NAMES], 1)
-    tgt = torch.stack([tg[k].clamp(min=0) for k in NAMES], 1)
+    tgt, wt = _measurement_terms(targets, weights, B, device)
     faces = body_model.faces_i32
     if method == 'lm':
         return _fit_lm(body_model, body_measurements, tgt.contiguous(), wt.contiguous(), betas_weight, iterations,
@@ -96,9 +120,7 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
         v = body_model.forward_shape(betas=b)['v_shaped']
         m = body_measurements.forward_vertices(v, faces)['measurements']
         meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-        diff = torch.where(wt > 0, tgt - meas, torch.zeros_like(meas))    # a dropped term passes no (NaN) gradient
-        per_body = (wt * diff.pow(2)).sum(1) + betas_weight * b.pow(2).sum(1)
-        return per_body, meas
+        return _measurement_loss(tgt, wt, meas, b, betas_weight), meas
 
     for _ in range(int(iterations)):
         opt.zero_grad(set_to_none=True)
@@ -165,7 +187,8 @@ def keypoint_jacobian(body_model, rot, betas, transl=None):
     return {'keypoints': kp, 'jacobian': jac}
 
 
-def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam'):
+def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam',
+                          body_measurements=None, measurements=None, measurement_weights=None, betas_weight=0.0):
     """Fits pose and shape so that the model's keypoints match `keypoints` (B, K, 3), K = body_model's keypoint count.
 
     weights: None (all 1), (K,) or (B, K) per-keypoint weights.  init: optional {'global_rot': (B, 6),
@@ -173,10 +196,23 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     zero betas or zero transl.  method: 'adam' (the default: the step size decays geometrically from lr to lr / 100)
     or 'lm' (batched Levenberg-Marquardt on the keypoint Jacobian, see the top; `lr` is ignored, a keypoint with
     weight <= 0 is dropped).  iterations: None means 600 for Adam and 50 for LM.
+    measurements: optional known measurements of the bodies, fitted together with the keypoints: the targets dict of
+    fit_betas_to_measurements ({name: float or (B,) values}, mass [kg], height, chest, waist, hips [m]), with
+    measurement_weights over DEFAULT_WEIGHTS and the same dropping rule (a target <= 0 or a weight <= 1e-3 drops
+    that term), measured by body_measurements (required with them) on the T-pose of the fitted betas; betas_weight
+    adds betas_weight |betas|^2 and needs measurements.
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (B, 1, 3, 3),
-    'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss}."""
+    'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss},
+    with measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss'
+    the total: keypoints + measurements + betas_weight |betas|^2."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if measurements is not None and body_measurements is None:
+        raise ValueError('fit_body_to_keypoints: measurements need body_measurements')
+    if measurements is None and betas_weight != 0:
+        raise ValueError('fit_body_to_keypoints: betas_weight needs measurements (the keypoint fit has no betas prior)')
+    if not betas_weight >= 0:
+        raise ValueError(f'fit_body_to_keypoints: betas_weight must be >= 0, got {betas_weight}')
     if iterations is None:
         iterations = 600 if method == 'adam' else 50
     from .autograd import Rot6dFunction
@@ -186,6 +222,10 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
                                                                              device=device)
     w = w.expand(B, K).contiguous()
+    mterms = None
+    if measurements is not None:
+        tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
+        mterms = (tgt.contiguous(), wt.contiguous(), float(betas_weight))
     init = init or {}
     ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
     ident[0::3].fill_(1.0)
@@ -197,7 +237,7 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
         params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
     if method == 'lm':
-        return _fit_keypoints_lm(body_model, kp, w, params, int(iterations))
+        return _fit_keypoints_lm(body_model, kp, w, params, int(iterations), body_measurements, mterms)
     opt = torch.optim.Adam(list(params.values()), lr=lr)
     sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
 
@@ -208,7 +248,13 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
                          return_shaped=False)
         joints = out['joints'][:]                  # the KeypointTensor's tensor, still in the graph
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
-        return per_body, joints, grot, bpose
+        meas = None
+        if mterms is not None:
+            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
+            m = body_measurements.forward_vertices(v, body_model.faces_i32)['measurements']
+            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], mterms[2])
+        return per_body, joints, grot, bpose, meas
 
     for _ in range(int(iterations)):
         opt.zero_grad(set_to_none=True)
@@ -217,13 +263,15 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         opt.step()
         sched.step()
     with torch.no_grad():
-        per_body, joints, grot, bpose = loss_fn()
+        per_body, joints, grot, bpose, meas = loss_fn()
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, loss=per_body)
+    if meas is not None:
+        res['measurements'] = meas
     return res
 
 
-def _fit_keypoints_lm(body_model, kp, w, params, iterations):
+def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=None, mterms=None):
     from . import ops
     device = kp.device
     packed = body_model.packed(device)
@@ -237,20 +285,37 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations):
              'jac': mk(B, 3 * K, P), 'loss': mk(B), 'lambda': mk(B),
              'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
     tg = kp.contiguous()
-    if B > 0:
+    if mterms is not None:
+        state.update(meas=mk(B, 5), meas_jac=mk(B, 5, nb))
+    if B > 0 and mterms is None:
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
             ops.fit_lm_keypoints_step(state, trial, tg, w, LM_UP, LM_DOWN, it == 0, tkp, tjac)
+    elif B > 0:
+        tgt, wt, rho = mterms
+        faces, lm = body_model.faces_i32, body_measurements.landmarks()
+        ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
+        for it in range(iterations + 1):
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
+            v = ops.smplx_forward_shape(packed, trial['betas'])
+            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces)
+            ops.fit_lm_keypoints_measurements_step(state, trial, tg, w, tgt, wt, rho, LM_UP, LM_DOWN, it == 0, tkp,
+                                                   tjac, tm, tmj)
     rot = state['rot']
     with torch.no_grad():
         out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], transl=state['transl'],
                          return_shaped=False)
         joints = out['joints'][:]
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
+        if mterms is not None:
+            per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], mterms[2])
     raw = rot[..., :2].reshape(B, n_rot * 6)       # the first two columns in the decoder's row-major 3x2 layout
-    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
-            'transl': state['transl'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], 'keypoints': joints,
-            'loss': per_body}
+    res = {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
+           'transl': state['transl'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], 'keypoints': joints,
+           'loss': per_body}
+    if mterms is not None:
+        res['measurements'] = state['meas']
+    return res
 
 
 def main(argv=None):

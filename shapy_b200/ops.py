@@ -450,6 +450,46 @@ def fit_lm_keypoints_step(state, trial, targets, weights, lambda_up, lambda_down
             stream_ptr()), 'fit_lm_keypoints_step')
 
 
+def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targets, meas_weights, betas_weight,
+                                       lambda_up, lambda_down, first, trial_keypoints, trial_jac, trial_meas,
+                                       trial_meas_jac):
+    """fit_lm_keypoints_step with the five measurements and a betas regulariser stacked under the keypoint rows
+    (include/shapy_b200.h, shapy_fit_lm_keypoints_measurements_step), in place.  state: fit_lm_keypoints_step's plus
+    'meas' (B, 5) and 'meas_jac' (B, 5, NB); meas_targets, meas_weights (B, 5) in the order mass, height, chest, waist,
+    hips; trial_meas (B, 5) / trial_meas_jac (B, 5, NB) from measure_jacobian_betas at the trial betas."""
+    B, n_rot = trial['rot'].shape[:2]
+    nb, K = trial['betas'].shape[1], targets.shape[1]
+    ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss', 'lambda')] + \
+        [trial[k] for k in ('rot', 'betas', 'transl')] + [targets, weights, meas_targets, meas_weights,
+                                                          trial_keypoints, trial_jac, trial_meas, trial_meas_jac]
+    what = 'fit_lm_keypoints_measurements_step'
+    for t in ts + [state['accepted']]:
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
+            raise RuntimeError(f'{what}: every tensor must be a contiguous CUDA tensor')
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise RuntimeError(f'{what}: the state, trial, targets and weights must be float32')
+    if state['accepted'].dtype != torch.int32:
+        raise RuntimeError(f'{what}: accepted must be int32')
+    P = 3 * n_rot + nb + 3
+    if trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K):
+        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}) and weights ({B}, {K})')
+    if (trial_meas_jac.shape != (B, 5, nb) or state['meas_jac'].shape != (B, 5, nb) or
+            any(t.shape != (B, 5) for t in (meas_targets, meas_weights, trial_meas, state['meas']))):
+        raise RuntimeError(f'{what}: meas_jac must be ({B}, 5, {nb}) and the measurements, their targets and weights '
+                           f'({B}, 5)')
+    if B == 0:
+        return
+    with torch.cuda.device(trial['rot'].device):
+        check(lib().shapy_fit_lm_keypoints_measurements_step(
+            B, K, n_rot, nb, ptr(targets), ptr(weights), ptr(meas_targets), ptr(meas_weights), float(betas_weight),
+            float(lambda_up), float(lambda_down), int(bool(first)),
+            *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
+                                      'lambda', 'accepted')],
+            ptr(trial['rot']), ptr(trial['betas']), ptr(trial['transl']), ptr(trial_keypoints), ptr(trial_jac),
+            ptr(trial_meas), ptr(trial_meas_jac), stream_ptr()), what)
+
+
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
     """grad_betas (B, NB) = shapedirs^T . grad_v_shaped (B, V, 3): the adjoint of smplx_forward_shape."""
     g = _cuda_f32(grad_v_shaped, 'grad_v_shaped')
