@@ -199,6 +199,26 @@ int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float *v_shaped, 
                                  const int32_t *inc, int batch, const shapy_measure_landmarks_t *lm,
                                  float *out, float *jac, int32_t *status, void *stream);
 
+/* The _exact entries: shapy_measure_backward, shapy_measure_backward_tris and shapy_measure_jacobian_betas with the
+ * exact derivative of the chest, waist and hip circumferences instead of the reference's autograd semantics.  With
+ * the hull's combinatorics held fixed (which points, in what order, from which face and ray), each hull point moves
+ * with its triangle's corners and with the plane height h = bc . y of its landmark face: a point on a triangle edge
+ * a -> b is a + s (b - a) with s = (h - a_y) / (b_y - a_y), a point where a query-quad edge pierces the triangle is
+ * the line-plane intersection, and a point without a ray hit is a constant.  The height's adjoint reaches the y
+ * components of the landmark face's corners, weighted by its barycentrics.  This is the derivative of the measured
+ * circumference wherever the hull's combinatorics do not change.  Mass and height terms and rows, the measurements,
+ * the NaN rules, determinism and batch independence are those of the non-exact entries, bit for bit. */
+int shapy_measure_backward_exact(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
+                                 const int32_t *inc, int batch, int num_verts, int num_faces,
+                                 const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_v,
+                                 void *stream);
+int shapy_measure_backward_tris_exact(const float *triangles, int batch, int num_faces,
+                                      const shapy_measure_landmarks_t *lm, const float *grad_out,
+                                      float *grad_triangles, void *stream);
+int shapy_measure_jacobian_betas_exact(const shapy_smplx_t *m, const float *v_shaped, const int32_t *inc_ptr,
+                                       const int32_t *inc, int batch, const shapy_measure_landmarks_t *lm,
+                                       float *out, float *jac, int32_t *status, void *stream);
+
 /* One Levenberg-Marquardt step per body of the fit of betas to the five measurements, one warp per body.  Loss
  * L = sum_{w_k > 0} w_k (t_k - m_k)^2 + betas_weight |beta|^2; a term with weight 0 is skipped (its measurement and
  * Jacobian row may be NaN).  targets, weights (B,5); the state betas (B,NB), meas (B,5), jac (B,5,NB), loss (B),

@@ -83,6 +83,13 @@ _SIGS = {
                                             c_void_p]),
     'shapy_measure_jacobian_betas': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, C.POINTER(MeasureLandmarks),
                                              c_void_p, c_void_p, c_void_p, c_void_p]),
+    'shapy_measure_backward_exact': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                             C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
+    'shapy_measure_backward_tris_exact': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p,
+                                                  c_void_p, c_void_p]),
+    'shapy_measure_jacobian_betas_exact': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                   C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p,
+                                                   c_void_p]),
     'shapy_fit_lm_step': (c_int, [c_int, c_int, c_void_p, c_void_p, C.c_float, C.c_float, C.c_float, c_int]
                           + [c_void_p] * 9 + [c_void_p]),
     'shapy_fit_lm_keypoints_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, C.c_float, C.c_float, c_int]

@@ -15,6 +15,8 @@ SMPLX.forward under autograd: see include/shapy_b200.h and DESIGN.md §6b.  For 
 reference's autograd ones (mesh-mesh-intersection/body_measurements/body_measurements.py:137-215): the intersection points' barycentrics are
 constants and the slicing planes' heights get no gradient, so a circumference's gradient is the derivative of the
 perimeter with the hull's points sliding on fixed faces at fixed barycentrics, not the finite difference of the mesh.
+measure(..., exact=True) backpropagates the exact derivative of the circumferences instead (ops.measure_backward
+with exact=True; the forward is the same launch).
 Every function is `once_differentiable`: a double backward (`create_graph=True`, e.g. the TrustRegion optimiser of
 the reference's examples/fit_measurements.py) raises.
 """
@@ -26,12 +28,13 @@ from . import ops as _ops
 
 class MeasureFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, landmarks, x, faces_i32, status):
+    def forward(ctx, landmarks, x, faces_i32, status, exact):
         if faces_i32 is None:
             out = _ops.measure(landmarks, triangles=x)
         else:
             out = _ops.measure(landmarks, v_shaped=x, faces_i32=faces_i32)
         ctx.landmarks = landmarks
+        ctx.exact = exact
         ctx.save_for_backward(x, faces_i32)
         status.append(out.status)
         return out
@@ -42,10 +45,10 @@ class MeasureFunction(torch.autograd.Function):
         x, faces_i32 = ctx.saved_tensors
         grad_out = grad_out.contiguous()
         if faces_i32 is None:
-            g = _ops.measure_backward(ctx.landmarks, grad_out, triangles=x)
+            g = _ops.measure_backward(ctx.landmarks, grad_out, triangles=x, exact=ctx.exact)
         else:
-            g = _ops.measure_backward(ctx.landmarks, grad_out, v_shaped=x, faces_i32=faces_i32)
-        return None, g, None, None
+            g = _ops.measure_backward(ctx.landmarks, grad_out, v_shaped=x, faces_i32=faces_i32, exact=ctx.exact)
+        return None, g, None, None, None
 
 
 class ShapeFunction(torch.autograd.Function):
@@ -101,12 +104,13 @@ def wants_grad(t) -> bool:
     return torch.is_grad_enabled() and torch.is_tensor(t) and t.requires_grad
 
 
-def measure(landmarks, v_shaped=None, faces_i32=None, triangles=None):
-    """ops.measure, differentiable in v_shaped / triangles; `out.status` is the forward's device status word."""
+def measure(landmarks, v_shaped=None, faces_i32=None, triangles=None, exact=False):
+    """ops.measure, differentiable in v_shaped / triangles; `out.status` is the forward's device status word.
+    exact: the backward gives the exact circumference derivative (ops.measure_backward)."""
     status = []
     if triangles is not None:
-        out = MeasureFunction.apply(landmarks, triangles, None, status)
+        out = MeasureFunction.apply(landmarks, triangles, None, status, bool(exact))
     else:
-        out = MeasureFunction.apply(landmarks, v_shaped, faces_i32, status)
+        out = MeasureFunction.apply(landmarks, v_shaped, faces_i32, status, bool(exact))
     out.status = status[0]
     return out

@@ -14,6 +14,20 @@ import torch.nn as nn
 from . import autograd as _ag
 from . import ops as _ops
 
+CIRCUMFERENCE_DERIVATIVES = ('reference', 'exact')
+
+
+def exact_circumferences(circumference_derivative) -> bool:
+    """True for 'exact', False for 'reference'; anything else raises ValueError.
+
+    'reference' (the default everywhere) differentiates the chest, waist and hip circumferences as the reference's
+    autograd does: the hull points' barycentrics are constants and the slicing planes' heights get no gradient.
+    'exact' gives the derivative of the measured circumference: the hull points move with their faces and with the
+    planes, which follow their landmarks (include/shapy_b200.h, shapy_measure_backward_exact)."""
+    if circumference_derivative not in CIRCUMFERENCE_DERIVATIVES:
+        raise ValueError(f"circumference_derivative must be 'reference' or 'exact', got {circumference_derivative!r}")
+    return circumference_derivative == 'exact'
+
 
 class BodyMeasurements(nn.Module):
     DENSITY = 985
@@ -80,19 +94,23 @@ class BodyMeasurements(nn.Module):
         if st is not None and int(st.item()) != 0:
             raise RuntimeError('BodyMeasurements: intersection-point capacity exceeded; affected values are NaN')
 
-    def forward_vertices(self, v_shaped, faces_i32):
+    def forward_vertices(self, v_shaped, faces_i32, circumference_derivative='reference'):
         """Fast path: (B, V, 3) vertices + (F, 3) int32 faces; no (B, F, 3, 3) tensor is materialised.
-        Differentiable in v_shaped (shapy_b200.autograd) when grad mode is on and it requires grad."""
+        Differentiable in v_shaped (shapy_b200.autograd) when grad mode is on and it requires grad;
+        circumference_derivative: 'reference' or 'exact', see exact_circumferences."""
+        exact = exact_circumferences(circumference_derivative)
         if _ag.wants_grad(v_shaped):
-            return self._pack(_ag.measure(self.landmarks(), v_shaped=v_shaped, faces_i32=faces_i32))
+            return self._pack(_ag.measure(self.landmarks(), v_shaped=v_shaped, faces_i32=faces_i32, exact=exact))
         return self._pack(_ops.measure(self.landmarks(), v_shaped=v_shaped, faces_i32=faces_i32))
 
     def forward(self, triangles, compute_mass=True, compute_height=True, compute_chest=True, compute_waist=True,
-                compute_hips=True, **kwargs):
+                compute_hips=True, circumference_derivative='reference', **kwargs):
         """triangles: (B, F, 3, 3), as in the reference.  Differentiable in triangles, as the reference is, when grad
-        mode is on and they require grad (first order only: see shapy_b200.autograd)."""
+        mode is on and they require grad (first order only: see shapy_b200.autograd); circumference_derivative:
+        'reference' (the reference's gradient) or 'exact', see exact_circumferences."""
+        exact = exact_circumferences(circumference_derivative)
         if _ag.wants_grad(triangles):
-            out = self._pack(_ag.measure(self.landmarks(), triangles=triangles))
+            out = self._pack(_ag.measure(self.landmarks(), triangles=triangles, exact=exact))
         else:
             out = self._pack(_ops.measure(self.landmarks(), triangles=triangles))
         drop = [n for n, f in (('mass', compute_mass), ('height', compute_height), ('chest', compute_chest),

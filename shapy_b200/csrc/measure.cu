@@ -55,6 +55,14 @@
 // writes the forward's five outputs and then, in phase 4, jac (B,5,NB): row k is S^T times the gradient the backward
 // gives for the cotangent e_k, S the model's shape rows -- the mass row densely over the vertices, the height row from
 // the two landmark faces, each circumference row from its hull vertices only (see DESIGN.md section 4).
+//
+// kGradientExact / kJacobianExact (the _exact entries) are those two modes with the exact derivative of the
+// circumferences.  Only the hull's combinatorics are held fixed: which points, in what order, from which face and which
+// ray.  Phase 4 recovers each hull point's ray with mmi::isect_first_ray (the same ray tests in the same order as phase
+// 2, nothing new stored), and hull_point_adjoint gives its corners' adjoints and the plane height's, the point moving
+// with its triangle and with the plane.  Warp p sums the height adjoints of plane p in hull order (gh[p]), which reach
+// the y components of the plane's landmark face with weights bc.  Everything else -- the measurements, the mass and
+// height terms, the NaN rules, the summation orders -- is the mode's twin's.
 #include "mmi_device.cuh"
 #include "smplx.cuh"
 
@@ -70,7 +78,8 @@ constexpr size_t kListBytes = 3 * kMaxPts * 12 + kMaxCand * 4;   // points + can
 constexpr size_t kGradBytes = 3 * kMaxPts * 4 + 3 * kMaxPts * 2;
 
 enum TriSource { kStagedVerts, kGlobalVerts, kTriangles };
-enum MeasureMode { kForward, kGradient, kJacobian };
+// kGradientExact / kJacobianExact: kGradient / kJacobian with the exact circumference derivative (see the top)
+enum MeasureMode { kForward, kGradient, kJacobian, kGradientExact, kJacobianExact };
 constexpr int kMaxJacBetas = 16;   // shape rows of the Jacobian mode
 
 struct MeasureGrad {
@@ -153,11 +162,48 @@ __device__ __forceinline__ float3 corner_cross(const mmi::Tri &T, int k) {
 
 __device__ __forceinline__ float sign_of(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : (x == 0.f ? 0.f : x)); }
 
+// Exact modes: the adjoint of one hull point of the plane at height h, produced on triangle T by ray `ray` of
+// mmi::isect_first_ray against the query triangle Q, for the upstream vector g.  Writes the adjoint of T's corner k to
+// dk and returns the plane height's.  The hull's combinatorics are held fixed (DESIGN.md section 4):
+//   ray 3-5, edge point p = a + s (b - a), s = (h - a_y) / D, D = b_y - a_y (a, b the edge's corners; |D| >= 2.5e-5
+//            by the ray test's |det| >= 1e-4):  d_a = (1 - s) g + e_y (g.(b - a)) (s - 1) / D,
+//            d_b = s g - e_y (g.(b - a)) s / D, the third corner 0, d_h = g.(b - a) / D
+//   ray 0-2, line point p = o + s w, o = (o_x, h, o_z) and w horizontal (the query edge), s = n.(v0 - o) / n.w,
+//            n = (v1 - v0) x (v2 - v0), r = v0 - p, c = g.w / n.w:  d_v1 = c (v2 - v0) x r, d_v2 = c r x (v1 - v0),
+//            d_v0 = c n - d_v1 - d_v2, d_h = g_y - c n_y
+//   no ray   the point is a constant: all 0
+__device__ __forceinline__ float hull_point_adjoint(const mmi::Tri &T, const mmi::Tri &Q, int ray, float h, float3 g,
+                                                    int k, float3 &dk) {
+  using mmi::cross3; using mmi::dot3; using mmi::sub3;
+  auto corner = [](const mmi::Tri &X, int c) { return c == 0 ? X.v0 : (c == 1 ? X.v1 : X.v2); };
+  dk = make_float3(0.f, 0.f, 0.f);
+  if (ray >= 3) {
+    const int i = ray - 3, j = i == 2 ? 0 : i + 1;
+    const float3 a = corner(T, i), e = sub3(corner(T, j), a);
+    const float D = e.y, s = (h - a.y) / D, q = dot3(g, e) / D;
+    if (k == i) dk = make_float3((1.f - s) * g.x, (1.f - s) * g.y + q * (s - 1.f), (1.f - s) * g.z);
+    if (k == j) dk = make_float3(s * g.x, s * g.y - q * s, s * g.z);
+    return q;
+  }
+  if (ray < 0) return 0.f;
+  const float3 o = corner(Q, ray), w = sub3(corner(Q, ray == 2 ? 0 : ray + 1), o);
+  const float3 e1 = sub3(T.v1, T.v0), e2 = sub3(T.v2, T.v0), n = cross3(e1, e2);
+  const float nw = dot3(n, w), s = dot3(n, sub3(T.v0, o)) / nw, c = dot3(g, w) / nw;
+  const float3 r = make_float3(T.v0.x - (o.x + s * w.x), T.v0.y - (o.y + s * w.y), T.v0.z - (o.z + s * w.z));
+  const float3 a = cross3(e2, r), b = cross3(r, e1);
+  if (k == 0) dk = make_float3(c * (n.x - a.x - b.x), c * (n.y - a.y - b.y), c * (n.z - a.z - b.z));
+  if (k == 1) dk = make_float3(c * a.x, c * a.y, c * a.z);
+  if (k == 2) dk = make_float3(c * b.x, c * b.y, c * b.z);
+  return g.y - c * n.y;
+}
+
 // MODE kForward: the forward; kGradient: the backward; kJacobian: the forward's outputs and their Jacobian with
-// respect to betas, see the top.
+// respect to betas; kGradientExact / kJacobianExact: the last two with the exact circumference derivative; see the top.
 template <int SRC, int MODE = kForward>
 __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a) {
   constexpr bool GRAD = MODE != kForward;    // phases 0-3 keep the point codes and the hull walk
+  constexpr bool BWD = MODE == kGradient || MODE == kGradientExact;      // writes a gradient
+  constexpr bool EXACT = MODE == kGradientExact || MODE == kJacobianExact;
   extern __shared__ __align__(16) unsigned char smem[];
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int nvf = a.V * 3;
@@ -279,7 +325,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     }
   }
   __syncthreads();     // the candidate queue is dead from here on: its storage becomes the chain lists
-  if (MODE != kGradient && t == 0) {
+  if (!BWD && t == 0) {
     float v = 0.f;
     for (int i = 0; i < kThreads / 32; ++i) v += red[i];
     a.out[(size_t)b * 5 + 0] = fabsf(v) / 6.0f * 985.0f;
@@ -402,13 +448,13 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     if (cnt[p] < 3 || edges < 3) perim = __int_as_float(0x7fc00000);
     if ((overflow & (1 << p))) perim = __int_as_float(0x7fc00000);   // truncated point set
     if constexpr (GRAD) perim_s[p] = perim;
-    if constexpr (MODE != kGradient) a.out[(size_t)b * 5 + 2 + p] = perim;
+    if constexpr (!BWD) a.out[(size_t)b * 5 + 2 + p] = perim;
   }
-  if constexpr (MODE != kGradient) {
+  if constexpr (!BWD) {
     if (t == 0 && overflow && a.status) atomicExch(a.status, 1);
   }
   if constexpr (MODE != kForward) {
-    static_assert(MODE == kGradient || SRC != kTriangles, "the Jacobian mode reads the model's faces and shape rows");
+    static_assert(BWD || SRC != kTriangles, "the Jacobian mode reads the model's faces and shape rows");
     // ---- phase 4: gradient or Jacobian.  The chain lists are dead: their storage holds the hull vertex list of each
     // plane (hull[p][j] = start slot of the j-th edge, chains in order) and, in gradient mode, then a bitmap of the
     // faces that carry a hull point.  The Jacobian mode builds what the gradient mode builds for an upstream gradient
@@ -422,9 +468,9 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
     __shared__ float gs[5];
     __shared__ int nedge[3], poison;
     const MeasureGrad &g = a.g;
-    const float *go = MODE == kGradient ? g.gout + (size_t)b * 5 : nullptr;
+    const float *go = BWD ? g.gout + (size_t)b * 5 : nullptr;
     if (t == 0) {
-      auto up = [&](int k) { return MODE == kGradient ? go[k] : 1.f; };            // the upstream gradient
+      auto up = [&](int k) { return BWD ? go[k] : 1.f; };                          // the upstream gradient
       float v = 0.f;
       for (int i = 0; i < kThreads / 32; ++i) v += red[i];                          // the forward's volume, same order
       gs[0] = up(0) * sign_of(v) * (985.0f / 6.0f);
@@ -438,7 +484,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
         nedge[p] = active && usable ? m : 0;
         bad |= active && !usable;
       }
-      poison = MODE == kGradient && bad;   // the Jacobian makes only the rows of unusable hulls NaN
+      poison = BWD && bad;   // the Jacobian makes only the rows of unusable hulls NaN
     }
     if (warp < 24 && lane == 0) {
       int off = 0, m = 0;
@@ -447,7 +493,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       if (m <= kMaxPts)
         for (int s = 0; s < chain_edges[hp][hk]; ++s) { hull[hp * kMaxPts + off + s] = (unsigned short)cur; cur = nxt[hp * kMaxPts + cur]; }
     }
-    if constexpr (MODE == kGradient)
+    if constexpr (BWD)
       for (int i = t; i < nbits_words; i += kThreads) fbits[i] = 0u;
     __syncthreads();
     // per hull vertex j of plane p: g (u_in - u_out), u the unit vectors of the edges into and out of it.  The walk is
@@ -466,7 +512,7 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       const float li = sqrtf(ix * ix + iy * iy + iz * iz), lo = sqrtf(ox * ox + oy * oy + oz * oz);
       const float gp = gs[2 + p];
       val[it] = make_float3(gp * (ix / li - ox / lo), gp * (iy / li - oy / lo), gp * (iz / li - oz / lo));
-      if constexpr (MODE == kGradient) {
+      if constexpr (BWD) {
         if (!all_flagged) {
           const int f = codes[p * kMaxPts + cur] >> 1;
           atomicOr(&fbits[f >> 5], 1u << (f & 31));
@@ -497,24 +543,64 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
       mmi::isect_points(quad(hs[p], c & 1), T, b1, b2);
       return b1;
     };
-    if constexpr (MODE == kGradient) {
+    // exact modes: the ray that gave phase 2 that point, and the adjoint of its triangle's corner k for the hull vertex
+    // vector at gv (returns the plane height's)
+    auto hull_ray = [&](int p, int c, const mmi::Tri &T) { return mmi::isect_first_ray(quad(hs[p], c & 1), T); };
+    auto hull_adj = [&](int p, int c, const mmi::Tri &T, int ray, const float *gv, int k, float3 &dk) {
+      return hull_point_adjoint(T, quad(hs[p], c & 1), ray, hs[p], make_float3(gv[0], gv[1], gv[2]), k, dk);
+    };
+    // exact modes: gh[p], the adjoint of plane p's height, summed over its hull vertices in hull order by warp p
+    float *gh = nullptr;
+    if constexpr (EXACT) {
+      __shared__ float gh_s[3];
+      gh = gh_s;
+      __syncthreads();
+      if (warp < 3) {
+        const int p = warp, m = nedge[p];
+        float acc = 0.f;
+        for (int base = 0; base < m; base += 32) {
+          const int j = base + lane;
+          float c = 0.f;
+          if (j < m) {
+            const int code = codes[p * kMaxPts + hull[p * kMaxPts + j]];
+            const mmi::Tri T = tri_of(code >> 1);
+            float3 dk;
+            c = hull_adj(p, code, T, hull_ray(p, code, T), pts + 3 * (p * kMaxPts + j), 0, dk);
+          }
+          const int nj = min(32, m - base);
+          for (int i = 0; i < nj; ++i) acc += __shfl_sync(0xffffffffu, c, i);
+        }
+        if (lane == 0) gh_s[p] = acc;
+      }
+    }
+    if constexpr (BWD) {
       __syncthreads();
       const float sm = gs[0], sh = gs[1];
       const bool bad = poison != 0;
-      // hull and height terms of corner k of face f (T = its triangle), in a fixed order: planes, hull order, height
+      // hull and height terms of corner k of face f (T = its triangle), in a fixed order: planes, hull order, (exact
+      // modes) plane heights, height
       auto sparse = [&](int f, const mmi::Tri &T, int k, float3 &acc) {
         if (all_flagged || (fbits[f >> 5] >> (f & 31)) & 1u) {
           for (int p = 0; p < 3; ++p) {
             for (int j = 0; j < nedge[p]; ++j) {
               const int c = codes[p * kMaxPts + hull[p * kMaxPts + j]];
               if ((c >> 1) != f) continue;
-              const float3 b1 = hull_bc(p, c, T);
-              const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
               const float *gv = pts + 3 * (p * kMaxPts + j);
-              acc.x += w * gv[0]; acc.y += w * gv[1]; acc.z += w * gv[2];
+              if constexpr (EXACT) {
+                float3 dk;
+                hull_adj(p, c, T, hull_ray(p, c, T), gv, k, dk);
+                acc.x += dk.x; acc.y += dk.y; acc.z += dk.z;
+              } else {
+                const float3 b1 = hull_bc(p, c, T);
+                const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+                acc.x += w * gv[0]; acc.y += w * gv[1]; acc.z += w * gv[2];
+              }
             }
           }
         }
+        if constexpr (EXACT)
+          for (int p = 0; p < 3; ++p)
+            if (f == a.lm.face_idx[2 + p] && nedge[p] > 0) acc.y += gh[p] * a.lm.bc[2 + p][k];
         if (f == a.lm.face_idx[0]) acc.y += sh * a.lm.bc[0][k];
         if (f == a.lm.face_idx[1]) acc.y -= sh * a.lm.bc[1][k];
       };
@@ -536,8 +622,9 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
           float3 acc = make_float3(sm * c.x, sm * c.y, sm * c.z);
           for (int e = e0; e < e1; ++e) {
             const int fk = __ldg(g.inc + e), f = fk / 3;
-            if (all_flagged || f == a.lm.face_idx[0] || f == a.lm.face_idx[1] || ((fbits[f >> 5] >> (f & 31)) & 1u))
-              sparse(f, tri_of(f), fk % 3, acc);
+            bool want = all_flagged || f == a.lm.face_idx[0] || f == a.lm.face_idx[1] || ((fbits[f >> 5] >> (f & 31)) & 1u);
+            if constexpr (EXACT) want = want || f == a.lm.face_idx[2] || f == a.lm.face_idx[3] || f == a.lm.face_idx[4];
+            if (want) sparse(f, tri_of(f), fk % 3, acc);
           }
           float *o = g.grad + ((size_t)b * a.V + v) * 3;
           o[0] = bad ? nan : acc.x; o[1] = bad ? nan : acc.y; o[2] = bad ? nan : acc.z;
@@ -596,16 +683,37 @@ __global__ void __launch_bounds__(kThreads, 1) measure_smem_kernel(MeasureArgs a
           float c = 0.f;
           if (j < m) {
             const int code = codes[p * kMaxPts + hull[p * kMaxPts + j]], f = code >> 1;
-            const float3 b1 = hull_bc(p, code, tri_of(f));
             const float *gv = pts + 3 * (p * kMaxPts + j);
-            for (int k = 0; k < 3; ++k) {
-              const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
-              const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
-              c += w * (gv[0] * __ldg(s) + gv[1] * __ldg(s + 1) + gv[2] * __ldg(s + 2));
+            if constexpr (EXACT) {
+              // exact modes: the corner adjoints . S[l][corner]
+              const mmi::Tri T = tri_of(f);
+              const int ray = hull_ray(p, code, T);
+              for (int k = 0; k < 3; ++k) {
+                float3 dk;
+                hull_adj(p, code, T, ray, gv, k, dk);
+                const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
+                c += dk.x * __ldg(s) + dk.y * __ldg(s + 1) + dk.z * __ldg(s + 2);
+              }
+            } else {
+              const float3 b1 = hull_bc(p, code, tri_of(f));
+              for (int k = 0; k < 3; ++k) {
+                const float w = k == 0 ? b1.x : (k == 1 ? b1.y : b1.z);
+                const float *s = Sl + 3 * __ldg(a.faces + 3 * f + k);
+                c += w * (gv[0] * __ldg(s) + gv[1] * __ldg(s + 1) + gv[2] * __ldg(s + 2));
+              }
             }
           }
           const int nj = min(32, m - base);
           for (int i = 0; i < nj; ++i) acc += __shfl_sync(0xffffffffu, c, i);
+        }
+        if constexpr (EXACT) {
+          // the plane height's adjoint gh[p] reaches the y components of the landmark face's corners
+          if (lane == 0) {
+            const int lf = a.lm.face_idx[2 + p];
+            float hy = 0.f;
+            for (int k = 0; k < 3; ++k) hy += a.lm.bc[2 + p][k] * __ldg(Sl + 3 * a.faces[3 * lf + k] + 1);
+            acc += gh[p] * hy;
+          }
         }
         if (lane == 0) J[(size_t)(2 + p) * nb + l] = (bad || isnan(gs[2 + p])) ? nan : acc;
       }
@@ -639,7 +747,7 @@ static int launch_measure(const MeasureArgs &a, void *stream) {
   cudaStream_t s = (cudaStream_t)stream;
   if (a.status) SHAPY_CUDA_TRY(cudaMemsetAsync(a.status, 0, sizeof(int), s));
   const size_t list = kListBytes + (MODE == kForward ? 0 : kGradBytes);
-  if constexpr (MODE != kJacobian)
+  if constexpr (MODE != kJacobian && MODE != kJacobianExact)
     if (a.tris) return launch_source<kTriangles, MODE>(a, list, s);
   const size_t staged = (((size_t)a.V * 12 + 15) & ~(size_t)15) + list;
   if (a.V < 65536 && staged <= kMaxDynSmem) return launch_source<kStagedVerts, MODE>(a, staged, s);
@@ -669,38 +777,85 @@ extern "C" int shapy_measure_forward_tris(const float *triangles, int batch, int
   return launch_measure<kForward>(a, stream);
 }
 
+template <int MODE>
+static int measure_backward(const char *name, const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
+                            const int32_t *inc, int batch, int num_verts, int num_faces,
+                            const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_v, void *stream) {
+  SHAPY_REQUIRE(v_shaped && faces && lm && grad_out && grad_v, "%s: null argument", name);
+  SHAPY_REQUIRE(inc_ptr && inc && num_verts > 0, "%s: null incidence table", name);
+  MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
+                MeasureGrad{grad_out, inc_ptr, inc, grad_v}};
+  return launch_measure<MODE>(a, stream);
+}
+
+template <int MODE>
+static int measure_backward_tris(const char *name, const float *triangles, int batch, int num_faces,
+                                 const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_triangles,
+                                 void *stream) {
+  SHAPY_REQUIRE(triangles && lm && grad_out && grad_triangles, "%s: null argument", name);
+  MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
+                MeasureGrad{grad_out, nullptr, nullptr, grad_triangles}};
+  return launch_measure<MODE>(a, stream);
+}
+
+template <int MODE>
+static int measure_jacobian_betas(const char *name, const shapy_smplx_t *m, const float *v_shaped,
+                                  const int32_t *inc_ptr, const int32_t *inc, int batch,
+                                  const shapy_measure_landmarks_t *lm, float *out, float *jac, int32_t *status,
+                                  void *stream) {
+  SHAPY_REQUIRE(m && v_shaped && inc_ptr && inc && lm && out && jac && batch > 0, "%s: bad argument", name);
+  SHAPY_REQUIRE(((uintptr_t)v_shaped & 15) == 0, "%s: v_shaped must be 16-byte aligned", name);
+  const SmplxDev &d = m->d;
+  if (d.NB < 1 || d.NB > kMaxJacBetas) {
+    set_error("%s: %d betas, at most %d are supported", name, d.NB, kMaxJacBetas);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  MeasureArgs a{v_shaped, d.faces, nullptr, batch, d.V, d.F, *lm, out, nullptr, nullptr, 0, status,
+                MeasureGrad{nullptr, inc_ptr, inc, nullptr, d.basis, d.V3p, d.NB, jac}};
+  return launch_measure<MODE>(a, stream);
+}
+
 extern "C" int shapy_measure_backward(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
                                       const int32_t *inc, int batch, int num_verts, int num_faces,
                                       const shapy_measure_landmarks_t *lm, const float *grad_out, float *grad_v,
                                       void *stream) {
-  SHAPY_REQUIRE(v_shaped && faces && lm && grad_out && grad_v, "shapy_measure_backward: null argument");
-  SHAPY_REQUIRE(inc_ptr && inc && num_verts > 0, "shapy_measure_backward: null incidence table");
-  MeasureArgs a{v_shaped, faces, nullptr, batch, num_verts, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
-                MeasureGrad{grad_out, inc_ptr, inc, grad_v}};
-  return launch_measure<kGradient>(a, stream);
+  return measure_backward<kGradient>("shapy_measure_backward", v_shaped, faces, inc_ptr, inc, batch, num_verts,
+                                     num_faces, lm, grad_out, grad_v, stream);
+}
+
+extern "C" int shapy_measure_backward_exact(const float *v_shaped, const int32_t *faces, const int32_t *inc_ptr,
+                                            const int32_t *inc, int batch, int num_verts, int num_faces,
+                                            const shapy_measure_landmarks_t *lm, const float *grad_out,
+                                            float *grad_v, void *stream) {
+  return measure_backward<kGradientExact>("shapy_measure_backward_exact", v_shaped, faces, inc_ptr, inc, batch,
+                                          num_verts, num_faces, lm, grad_out, grad_v, stream);
 }
 
 extern "C" int shapy_measure_backward_tris(const float *triangles, int batch, int num_faces,
                                            const shapy_measure_landmarks_t *lm, const float *grad_out,
                                            float *grad_triangles, void *stream) {
-  SHAPY_REQUIRE(triangles && lm && grad_out && grad_triangles, "shapy_measure_backward_tris: null argument");
-  MeasureArgs a{nullptr, nullptr, triangles, batch, 0, num_faces, *lm, nullptr, nullptr, nullptr, 0, nullptr,
-                MeasureGrad{grad_out, nullptr, nullptr, grad_triangles}};
-  return launch_measure<kGradient>(a, stream);
+  return measure_backward_tris<kGradient>("shapy_measure_backward_tris", triangles, batch, num_faces, lm, grad_out,
+                                          grad_triangles, stream);
+}
+
+extern "C" int shapy_measure_backward_tris_exact(const float *triangles, int batch, int num_faces,
+                                                 const shapy_measure_landmarks_t *lm, const float *grad_out,
+                                                 float *grad_triangles, void *stream) {
+  return measure_backward_tris<kGradientExact>("shapy_measure_backward_tris_exact", triangles, batch, num_faces, lm,
+                                               grad_out, grad_triangles, stream);
 }
 
 extern "C" int shapy_measure_jacobian_betas(const shapy_smplx_t *m, const float *v_shaped, const int32_t *inc_ptr,
                                             const int32_t *inc, int batch, const shapy_measure_landmarks_t *lm,
                                             float *out, float *jac, int32_t *status, void *stream) {
-  SHAPY_REQUIRE(m && v_shaped && inc_ptr && inc && lm && out && jac && batch > 0,
-                "shapy_measure_jacobian_betas: bad argument");
-  SHAPY_REQUIRE(((uintptr_t)v_shaped & 15) == 0, "shapy_measure_jacobian_betas: v_shaped must be 16-byte aligned");
-  const SmplxDev &d = m->d;
-  if (d.NB < 1 || d.NB > kMaxJacBetas) {
-    set_error("shapy_measure_jacobian_betas: %d betas, at most %d are supported", d.NB, kMaxJacBetas);
-    return SHAPY_ERR_UNSUPPORTED;
-  }
-  MeasureArgs a{v_shaped, d.faces, nullptr, batch, d.V, d.F, *lm, out, nullptr, nullptr, 0, status,
-                MeasureGrad{nullptr, inc_ptr, inc, nullptr, d.basis, d.V3p, d.NB, jac}};
-  return launch_measure<kJacobian>(a, stream);
+  return measure_jacobian_betas<kJacobian>("shapy_measure_jacobian_betas", m, v_shaped, inc_ptr, inc, batch, lm, out,
+                                           jac, status, stream);
+}
+
+extern "C" int shapy_measure_jacobian_betas_exact(const shapy_smplx_t *m, const float *v_shaped,
+                                                  const int32_t *inc_ptr, const int32_t *inc, int batch,
+                                                  const shapy_measure_landmarks_t *lm, float *out, float *jac,
+                                                  int32_t *status, void *stream) {
+  return measure_jacobian_betas<kJacobianExact>("shapy_measure_jacobian_betas_exact", m, v_shaped, inc_ptr, inc,
+                                                batch, lm, out, jac, status, stream);
 }

@@ -157,6 +157,24 @@ __device__ inline bool isect_points(const TriT<T> &Q, const TriT<T> &T_, vec3<T>
   return found_first;
 }
 
+// Which ray gives isect_points its first point: 0-2 the query's edge i (origin Q.v_i, direction Q.v_i+1 - Q.v_i)
+// against T_, 3-5 T_'s edge i (origin T_.v_i, direction T_.v_i+1 - T_.v_i) against the query, -1 none.  The same
+// ray tests in the same order as isect_points, so the same choice: a ray is taken when it hits with 0 <= t <= 1.
+template <typename T>
+__device__ inline int isect_first_ray(const TriT<T> &Q, const TriT<T> &T_) {
+  using V = vec3<T>;
+  const V qo[3] = {Q.v0, Q.v1, Q.v2}, to[3] = {T_.v0, T_.v1, T_.v2};
+  T t = 0;
+  V ip;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    if (ray_tri(qo[i], sub3(qo[(i + 1) % 3], qo[i]), T_.v0, T_.v1, T_.v2, t, ip) && !(t > 1 || t < 0)) return i;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    if (ray_tri(to[i], sub3(to[(i + 1) % 3], to[i]), Q.v0, Q.v1, Q.v2, t, ip) && !(t > 1 || t < 0)) return 3 + i;
+  return -1;
+}
+
 template <typename T>
 struct BoxT {
   vec3<T> lo, hi;

@@ -43,15 +43,23 @@ circumferences and the mass; fitting one after the other lets the second fit und
 measurement term goes through forward_shape and BodyMeasurements.forward_vertices; with method='lm' each iteration
 stacks the five measurement rows under the keypoint rows of one damped Gauss-Newton step (four launches: the keypoint
 Jacobian, forward_shape and the measurement Jacobian of the trial, then ops.fit_lm_keypoints_measurements_step), no
-host synchronisation, and every body's total loss is non-increasing.  The measurement rows have the measurement
-backward's semantics (constant barycentrics, no gradient through the plane heights), so they are not the exact
-derivative of a circumference: LM may reject more steps, but accept / reject uses the true loss.
+host synchronisation, and every body's total loss is non-increasing.
+
+circumference_derivative (every measurement fit, Adam and LM, and measurement_jacobian; python -m shapy_b200.fit
+--circumference-derivative): how the chest, waist and hip circumferences are differentiated.  'reference' (the
+default) keeps the reference's autograd semantics: the hull points' barycentrics are constants and the slicing planes'
+heights get no gradient, so those rows are not the derivative of the measured circumference, and with the
+circumferences at their default weights LM stalls.  'exact' uses the exact derivative (the hull points move with their
+faces and with the planes, which follow their landmarks; include/shapy_b200.h, shapy_measure_backward_exact).  The
+launches are the same in number, and LM still never synchronises with the host.
 """
 import argparse
 import json
 
 import numpy as np
 import torch
+
+from .body_measurements import CIRCUMFERENCE_DERIVATIVES, exact_circumferences
 
 NAMES = ('mass', 'height', 'chest', 'waist', 'hips')
 DEFAULT_WEIGHTS = {'height': 100.0, 'mass': 1.0, 'chest': 2000.0, 'waist': 1000.0, 'hips': 1000.0}
@@ -86,18 +94,20 @@ def _measurement_loss(tgt, wt, meas, betas, betas_weight):
 
 
 def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
-                              lr=0.05, betas_init=None, batch_size=None, method='adam'):
+                              lr=0.05, betas_init=None, batch_size=None, method='adam',
+                              circumference_derivative='reference'):
     """Fits betas (B, NB) so that the model's T-pose measurements match `targets`.
 
     body_model: shapy_b200 SMPLX (its forward_shape and faces are used); body_measurements: shapy_b200
     BodyMeasurements on the same device.  targets: {name: float or (B,) values} for mass [kg], height, chest, waist,
     hips [m]; a missing name or a value <= 0 drops that term.  batch_size: B when every target is a scalar (default 1).
     method: 'adam' (the default) or 'lm' (Levenberg-Marquardt, see the top; `lr` is ignored).  iterations: None means
-    500 for Adam and 50 for LM.
+    500 for Adam and 50 for LM.  circumference_derivative: 'reference' or 'exact' (see the top).
     Returns {'betas': (B, NB), 'measurements': (B, 5) of the final betas (mass, height, chest, waist, hips),
     'loss': (B,) final per-body loss}."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    exact = exact_circumferences(circumference_derivative)
     if iterations is None:
         iterations = 500 if method == 'adam' else 50
     device = body_model.shapedirs.device
@@ -108,7 +118,7 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     faces = body_model.faces_i32
     if method == 'lm':
         return _fit_lm(body_model, body_measurements, tgt.contiguous(), wt.contiguous(), betas_weight, iterations,
-                       betas_init, B, device)
+                       betas_init, B, device, exact)
     nb = body_model.shapedirs.shape[-1]
     betas = (torch.zeros(B, nb, device=device) if betas_init is None else betas_init.detach().clone().float())
     betas.requires_grad_(True)
@@ -118,7 +128,7 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
 
     def loss_fn(b):
         v = body_model.forward_shape(betas=b)['v_shaped']
-        m = body_measurements.forward_vertices(v, faces)['measurements']
+        m = body_measurements.forward_vertices(v, faces, circumference_derivative)['measurements']
         meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
         return _measurement_loss(tgt, wt, meas, b, betas_weight), meas
 
@@ -137,21 +147,24 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
 LM_UP, LM_DOWN = 10.0, 3.0
 
 
-def measurement_jacobian(body_model, body_measurements, betas):
+def measurement_jacobian(body_model, body_measurements, betas, circumference_derivative='reference'):
     """The measurements of forward_shape(betas) and their Jacobian with respect to betas, without autograd:
     {'measurements': (B, 5) (mass, height, chest, waist, hips, bit-identical to BodyMeasurements.forward_vertices),
-    'jacobian': (B, 5, NB)}.  The Jacobian has the semantics of the measurements' backward (constant barycentrics, no
-    gradient through the plane heights); a NaN circumference gives a NaN row."""
+    'jacobian': (B, 5, NB)}.  The Jacobian has the semantics of the measurements' backward for the same
+    circumference_derivative ('reference': constant barycentrics, no gradient through the plane heights; 'exact': the
+    circumferences' exact derivative); a NaN circumference gives a NaN row."""
     from . import ops
+    exact = exact_circumferences(circumference_derivative)
     betas = torch.as_tensor(betas, dtype=torch.float32, device=body_model.shapedirs.device).detach().contiguous()
     packed = body_model.packed(betas.device)
     v = ops.smplx_forward_shape(packed, betas)
-    out, jac, status = ops.measure_jacobian_betas(packed, body_measurements.landmarks(), v, body_model.faces_i32)
+    out, jac, status = ops.measure_jacobian_betas(packed, body_measurements.landmarks(), v, body_model.faces_i32,
+                                                  exact=exact)
     body_measurements.last_status = status
     return {'measurements': out, 'jacobian': jac}
 
 
-def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, betas_init, B, device):
+def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, betas_init, B, device, exact):
     from . import ops
     packed = body_model.packed(device)
     faces = body_model.faces_i32
@@ -167,7 +180,7 @@ def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, be
     ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
     for it in range(int(iterations) + 1):
         v = ops.smplx_forward_shape(packed, trial)
-        meas, jac, _ = ops.measure_jacobian_betas(packed, lm, v, faces)
+        meas, jac, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
         ops.fit_lm_step(state, tgt, wt, betas_weight, LM_UP, LM_DOWN, it == 0, trial, meas, jac)
     return {'betas': state['betas'], 'measurements': state['meas'], 'loss': state['loss']}
 
@@ -188,7 +201,8 @@ def keypoint_jacobian(body_model, rot, betas, transl=None):
 
 
 def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam',
-                          body_measurements=None, measurements=None, measurement_weights=None, betas_weight=0.0):
+                          body_measurements=None, measurements=None, measurement_weights=None, betas_weight=0.0,
+                          circumference_derivative='reference'):
     """Fits pose and shape so that the model's keypoints match `keypoints` (B, K, 3), K = body_model's keypoint count.
 
     weights: None (all 1), (K,) or (B, K) per-keypoint weights.  init: optional {'global_rot': (B, 6),
@@ -200,13 +214,15 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     fit_betas_to_measurements ({name: float or (B,) values}, mass [kg], height, chest, waist, hips [m]), with
     measurement_weights over DEFAULT_WEIGHTS and the same dropping rule (a target <= 0 or a weight <= 1e-3 drops
     that term), measured by body_measurements (required with them) on the T-pose of the fitted betas; betas_weight
-    adds betas_weight |betas|^2 and needs measurements.
+    adds betas_weight |betas|^2 and needs measurements.  circumference_derivative: 'reference' or 'exact', how the
+    circumferences of the measurement term are differentiated (see the top).
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (B, 1, 3, 3),
     'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss},
     with measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss'
     the total: keypoints + measurements + betas_weight |betas|^2."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    exact_circumferences(circumference_derivative)
     if measurements is not None and body_measurements is None:
         raise ValueError('fit_body_to_keypoints: measurements need body_measurements')
     if measurements is None and betas_weight != 0:
@@ -225,7 +241,7 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     mterms = None
     if measurements is not None:
         tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
-        mterms = (tgt.contiguous(), wt.contiguous(), float(betas_weight))
+        mterms = (tgt.contiguous(), wt.contiguous(), float(betas_weight), circumference_derivative)
     init = init or {}
     ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
     ident[0::3].fill_(1.0)
@@ -251,7 +267,7 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         meas = None
         if mterms is not None:
             v = body_model.forward_shape(betas=params['betas'])['v_shaped']
-            m = body_measurements.forward_vertices(v, body_model.faces_i32)['measurements']
+            m = body_measurements.forward_vertices(v, body_model.faces_i32, mterms[3])['measurements']
             meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
             per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], mterms[2])
         return per_body, joints, grot, bpose, meas
@@ -292,13 +308,14 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=N
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
             ops.fit_lm_keypoints_step(state, trial, tg, w, LM_UP, LM_DOWN, it == 0, tkp, tjac)
     elif B > 0:
-        tgt, wt, rho = mterms
+        tgt, wt, rho, cd = mterms
+        exact = exact_circumferences(cd)
         faces, lm = body_model.faces_i32, body_measurements.landmarks()
         ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
             v = ops.smplx_forward_shape(packed, trial['betas'])
-            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces)
+            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
             ops.fit_lm_keypoints_measurements_step(state, trial, tg, w, tgt, wt, rho, LM_UP, LM_DOWN, it == 0, tkp,
                                                    tjac, tm, tmj)
     rot = state['rot']
@@ -338,6 +355,9 @@ def main(argv=None):
     p.add_argument('--betas-weight', dest='betas_weight', type=float, default=0.0)
     p.add_argument('--method', choices=('adam', 'lm'), default='adam',
                    help='optimiser: Adam, or batched Levenberg-Marquardt on the measurement Jacobian')
+    p.add_argument('--circumference-derivative', dest='circumference_derivative', choices=CIRCUMFERENCE_DERIVATIVES,
+                   default='reference', help="how the circumferences are differentiated: the reference's autograd "
+                                             "semantics, or their exact derivative")
     p.add_argument('--iterations', type=int, default=None, help='default 500 for adam, 50 for lm')
     p.add_argument('--lr', type=float, default=0.05, help='Adam step size (ignored by lm)')
     p.add_argument('--output', type=str, default='fit_betas.npz')
@@ -362,7 +382,7 @@ def main(argv=None):
     else:
         targets = {k: getattr(a, k) for k in NAMES}
     res = fit_betas_to_measurements(model, bm, targets, betas_weight=a.betas_weight, iterations=a.iterations, lr=a.lr,
-                                    method=a.method)
+                                    method=a.method, circumference_derivative=a.circumference_derivative)
     meas = res['measurements'].cpu().numpy()
     np.savez(a.output, betas=res['betas'].cpu().numpy(), measurements=meas, names=np.array(NAMES),
              loss=res['loss'].cpu().numpy())

@@ -307,10 +307,13 @@ def face_incidence(faces_i32):
     return inc
 
 
-def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, faces_i32=None, triangles=None):
+def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, faces_i32=None, triangles=None,
+                     exact=False):
     """Gradient of `measure` (B, 5) with respect to v_shaped (B, V, 3) or triangles (B, F, 3, 3), with the reference's
     autograd semantics (include/shapy_b200.h, shapy_measure_backward): the intersection barycentrics are constants and
-    the plane heights get no gradient.  Deterministic, one launch."""
+    the plane heights get no gradient.  exact=True gives the exact derivative of the circumferences instead
+    (shapy_measure_backward_exact: the hull points move with their faces and with the plane heights); the mass and
+    height terms are the same bits.  Deterministic, one launch."""
     g = _cuda_f32(grad_out, 'grad_out')
     x, faces_i32, B, V, F = _measure_input(v_shaped, faces_i32, triangles)
     if g.shape != (B, 5):
@@ -320,12 +323,13 @@ def measure_backward(landmarks: _lib.MeasureLandmarks, grad_out, v_shaped=None, 
         return grad
     with torch.cuda.device(x.device):
         if triangles is not None:
-            check(lib().shapy_measure_backward_tris(ptr(x), B, F, C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()),
-                  'measure_backward')
+            fn = lib().shapy_measure_backward_tris_exact if exact else lib().shapy_measure_backward_tris
+            check(fn(ptr(x), B, F, C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()), 'measure_backward')
         else:
             inc_ptr, inc = _incidence_rows(faces_i32, V)
-            check(lib().shapy_measure_backward(ptr(x), ptr(faces_i32), ptr(inc_ptr), ptr(inc), B, V, F,
-                                               C.byref(landmarks), ptr(g), ptr(grad), stream_ptr()), 'measure_backward')
+            fn = lib().shapy_measure_backward_exact if exact else lib().shapy_measure_backward
+            check(fn(ptr(x), ptr(faces_i32), ptr(inc_ptr), ptr(inc), B, V, F, C.byref(landmarks), ptr(g), ptr(grad),
+                     stream_ptr()), 'measure_backward')
     return grad
 
 
@@ -341,11 +345,12 @@ def _incidence_rows(faces_i32, V):
 MAX_JACOBIAN_BETAS = 16
 
 
-def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, v_shaped, faces_i32):
+def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, v_shaped, faces_i32, exact=False):
     """The measurements (B, 5) of `measure` and their Jacobian (B, 5, NB) with respect to the model's betas at the
     vertices v_shaped (B, V, 3), one launch (include/shapy_b200.h, shapy_measure_jacobian_betas).  faces_i32: the
-    model's faces as a CUDA int32 (F, 3) tensor (its incidence table is cached).  Returns (out, jac, status), status the
-    device status word of `measure`."""
+    model's faces as a CUDA int32 (F, 3) tensor (its incidence table is cached).  exact=True gives the exact
+    circumference rows (shapy_measure_jacobian_betas_exact, see measure_backward); the measurements and the mass and
+    height rows are the same bits.  Returns (out, jac, status), status the device status word of `measure`."""
     x = _cuda_f32(v_shaped, 'v_shaped')
     faces_i32 = _faces_i32(faces_i32)
     if x.dim() != 3 or x.shape[1:] != (model.V, 3):
@@ -365,9 +370,9 @@ def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, 
         return out, jac, status
     with torch.cuda.device(dev):
         inc_ptr, inc = _incidence_rows(faces_i32, model.V)
-        check(lib().shapy_measure_jacobian_betas(model.handle, ptr(x), ptr(inc_ptr), ptr(inc), B, C.byref(landmarks),
-                                                 ptr(out), ptr(jac), ptr(status), stream_ptr()),
-              'measure_jacobian_betas')
+        fn = lib().shapy_measure_jacobian_betas_exact if exact else lib().shapy_measure_jacobian_betas
+        check(fn(model.handle, ptr(x), ptr(inc_ptr), ptr(inc), B, C.byref(landmarks), ptr(out), ptr(jac), ptr(status),
+                 stream_ptr()), 'measure_jacobian_betas')
     return out, jac, status
 
 
