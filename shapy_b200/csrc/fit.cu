@@ -448,8 +448,10 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
 template <bool MEAS>
 int launch_lm_kp(int batch, const LmKpArgs &a, const LmMeasArgs &m, void *stream) {
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
-  // with the 25 KB of static shared memory
-  if (smem + 25 * 1024 > 48 * 1024)
+  // past 48 KB of static plus dynamic shared memory the launch has to opt in
+  cudaFuncAttributes attr;
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp_step_kernel<MEAS>));
+  if (smem + attr.sharedSizeBytes > 48 * 1024)
     SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp_step_kernel<MEAS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)smem));
   lm_kp_step_kernel<MEAS><<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, m);

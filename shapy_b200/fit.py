@@ -33,7 +33,8 @@ their (3K, P) Jacobian with respect to right-multiplied rotation tangents, betas
 (ops.smplx_keypoint_jacobian), then takes one damped Gauss-Newton step per body (ops.fit_lm_keypoints_step: the
 measurement LM's policy, the P x P normal equations in fp64, the next rotations R Exp(delta) re-orthonormalised).  Two
 launches per iteration, no host synchronisation, and one SMPLX.forward at the end gives the returned keypoints and
-loss.  keypoint_jacobian(body_model, rot, betas, transl) exposes the Jacobian itself.
+loss.  keypoint_jacobian(body_model, rot, betas, transl) exposes the Jacobian itself.  The step takes at most 96
+parameters, so a model with more than 27 betas raises ValueError before any launch.
 
 fit_body_to_keypoints(..., body_measurements=bm, measurements={'height': h, 'mass': m, ...}) fits the keypoints and
 known measurements of the same bodies together, loss per body: the keypoint loss + the measurement loss of
@@ -69,7 +70,10 @@ def _targets(targets, B, device):
     out = {}
     for k in NAMES:
         v = targets.get(k, -1.0)
-        t = torch.as_tensor(v, dtype=torch.float32, device=device).reshape(-1)
+        if isinstance(v, (int, float)):            # filled on the device: no host-to-device copy
+            t = torch.full((B,), float(v), dtype=torch.float32, device=device)
+        else:
+            t = torch.as_tensor(v, dtype=torch.float32, device=device).reshape(-1)
         out[k] = t.expand(B).contiguous() if t.numel() == 1 else t
         if out[k].numel() != B:
             raise ValueError(f'target `{k}` has {out[k].numel()} values for {B} bodies')
@@ -145,6 +149,8 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
 
 # Levenberg-Marquardt damping: divided by LM_DOWN after an accepted step, multiplied by LM_UP after a rejected one
 LM_UP, LM_DOWN = 10.0, 3.0
+# parameters of one body the keypoint LM step takes (kLmKpMaxP of fit.cu): 22 rotations, the betas and the translation
+LM_KP_MAX_PARAMS = 96
 
 
 def measurement_jacobian(body_model, body_measurements, betas, circumference_derivative='reference'):
@@ -229,6 +235,10 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         raise ValueError('fit_body_to_keypoints: betas_weight needs measurements (the keypoint fit has no betas prior)')
     if not betas_weight >= 0:
         raise ValueError(f'fit_body_to_keypoints: betas_weight must be >= 0, got {betas_weight}')
+    if method == 'lm' and 3 * 22 + body_model.num_betas + 3 > LM_KP_MAX_PARAMS:
+        raise ValueError(f"fit_body_to_keypoints(method='lm'): 22 rotations, {body_model.num_betas} betas and the "
+                         f'translation are {3 * 22 + body_model.num_betas + 3} parameters, at most {LM_KP_MAX_PARAMS} '
+                         f'are supported (at most {LM_KP_MAX_PARAMS - 3 * 22 - 3} betas)')
     if iterations is None:
         iterations = 600 if method == 'adam' else 50
     from .autograd import Rot6dFunction

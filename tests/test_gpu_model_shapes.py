@@ -1,0 +1,465 @@
+"""GPU: the posed SMPL-X backward, the keypoint Jacobian, the keypoint LM steps and the keypoint LM fit on every model
+shape they accept: the variants of tests/test_model_shapes_cpu.py (NB 1 to 27, NE 0 to 16, NC up to 32, J14 from 448
+to 2 100 non-zeros, the keypoint Jacobian's cached and uncached entry paths), against the float64 restatements that
+test_model_shapes_cpu.py pins at those shapes.
+
+  * posed backward (shapy_smplx_backward) against float64 autograd: the generic shape adjoint at NB != 10 and with the
+    expression gradient at NE != 10; bar of test_gpu_smplx_grad.check, max |g - g64| <= 1e-4 max |g64| per body and
+    tensor
+  * keypoint Jacobian against kp_lm_oracle: bar of test_gpu_fit_lm_keypoints, 1e-4 per body and column block
+  * cached against uncached Jacobian entries (edge_2048 / edge_2049): the same bits
+  * J^T c against the posed backward on the uncached NB = 27 model
+  * both LM step kernels against their restatements at P = 7, 54, 55 (the 48 KB opt-in boundary) and 96, K = 1 to 127
+  * fit_body_to_keypoints(method='lm') at NB = 27 (P = 96) and NB = 16 with height and mass"""
+import numpy as np
+import pytest
+import torch
+
+import kp_lm_oracle
+import kpm_lm_oracle
+from shapy_b200 import synth
+from smplx_grad_ref import oracle_grads
+from test_model_shapes_cpu import KP_CACHE_ENTRIES, VARIANTS, keypoint_entries, variant_model
+
+pytestmark = pytest.mark.gpu
+TOL = 1e-4
+NAMES = list(VARIANTS)
+CHANGED_KP = 15                   # the keypoint J14 row 13 overwrites (source_idxs[13]): edge_2049's added entry
+
+
+def _bits(t):
+    return t.contiguous().view(torch.int32)
+
+
+def _rodrigues(aa):
+    aa = aa.double()
+    th = aa.norm(dim=-1, keepdim=True)
+    k = aa / th.clamp_min(1e-300)
+    kx, ky, kz = k.unbind(-1)
+    z = torch.zeros_like(kx)
+    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
+    s, c = th.sin()[..., None], th.cos()[..., None]
+    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
+
+
+def _inputs(seed, B, n_rot, NB, NE=0):
+    """Rotations, betas (B, NB), expression (B, NE) or None, transl, camera; necks turned past both ends of the contour
+    LUT in bodies 0 and 1."""
+    gen = torch.Generator().manual_seed(seed)
+    rot = _rodrigues(torch.randn(B, n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
+    if n_rot > 15 and B > 1:
+        rot[0, 12] = _rodrigues(torch.tensor([0.0, 1.2, 0.0])).float()
+        rot[1, 12] = _rodrigues(torch.tensor([0.0, -1.2, 0.0])).float()
+    return dict(rot=rot, betas=torch.randn(B, NB, generator=gen),
+                expression=torch.randn(B, NE, generator=gen) if NE else None,
+                transl=torch.randn(B, 3, generator=gen) * 0.1,
+                camera=torch.randn(B, 3, generator=gen) * torch.tensor([3.0, 0.2, 0.2]) + torch.tensor([1.0, 0, 0]))
+
+
+def _check(name, got, ref, tol=TOL):
+    """test_gpu_smplx_grad.check; returns the largest error over its bar."""
+    got, ref = got.detach().double().cpu(), torch.as_tensor(ref).double().cpu()
+    assert got.shape == ref.shape, (name, got.shape, ref.shape)
+    worst = 0.0
+    for b in range(ref.shape[0]):
+        scale = float(ref[b].abs().max())
+        err = float((got[b] - ref[b]).abs().max())
+        assert err <= tol * scale + 1e-30, (name, b, err, scale)
+        worst = max(worst, err / (tol * scale + 1e-30))
+    return worst
+
+
+@pytest.fixture(scope='module')
+def packed():
+    from shapy_b200 import ops
+    cache = {}
+
+    def get(name):
+        if name not in cache:
+            cache[name] = ops.SmplxModel(dict(variant_model(name), use_face_contour=True), 'cuda')
+        return cache[name]
+    return get
+
+
+def _module(name):
+    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
+    NB, NE, _ = VARIANTS[name]
+    return SMPLX(data_struct=variant_model(name), betas={'num': NB}, expression={'num': NE},
+                 use_face_contour=True).cuda()
+
+
+# ------------------------------------------------------------------------------------------------ posed backward
+@pytest.mark.parametrize('kind', ['mixed', 'j14'])
+@pytest.mark.parametrize('B', [1, 33])
+@pytest.mark.parametrize('n_rot', [1, 22, 55])
+@pytest.mark.parametrize('name', NAMES)
+def test_backward_vs_float64(packed, name, n_rot, B, kind):
+    """B = 33 is a multiple of neither the 8- or 4-body shape-adjoint tile nor the 32-body vertex tile: rows in the
+    first, a middle and the partial last tile are checked.  The expression gradient is wanted wherever NE > 0."""
+    from shapy_b200 import ops
+    m, pk = variant_model(name), packed(name)
+    NB, NE, _ = VARIANTS[name]
+    x = _inputs(10000 * NB + 100 * n_rot + B, B, n_rot, NB, NE)
+    gen = torch.Generator().manual_seed(NB + n_rot + B)
+    if kind == 'mixed':
+        cot = dict(vertices=torch.randn(B, pk.V, 3, generator=gen), joints=torch.randn(B, pk.K, 3, generator=gen),
+                   v_shaped=torch.randn(B, pk.V, 3, generator=gen) * 0.5,
+                   proj_joints=torch.randn(B, pk.K, 2, generator=gen))
+    else:                         # a one-hot on the keypoint J14 row 0 overwrites
+        cot = dict(joints=torch.zeros(B, pk.K, 3))
+        cot['joints'][:, int(m['source_idxs'][0]), 1] = 1.0
+    c = lambda t: None if t is None else t.cuda()  # noqa: E731
+    got = ops.smplx_backward(pk, c(x['betas']), c(x['rot']), expr=c(x['expression']), camera=c(x['camera']),
+                             grad_vertices=c(cot.get('vertices')), grad_v_shaped=c(cot.get('v_shaped')),
+                             grad_joints=c(cot.get('joints')), grad_proj_joints=c(cot.get('proj_joints')))
+    assert (got['expr'] is None) == (NE == 0)
+    rows = [0] if B == 1 else [0, 7, 8, 31, 32]
+    sub = lambda t: None if t is None else t[rows]  # noqa: E731
+    ref, _ = oracle_grads(m, {k: sub(v) for k, v in cot.items()}, sub(x['betas']), sub(x['rot']),
+                          expression=sub(x['expression']), camera=sub(x['camera']))
+    worst = max(_check('betas', got['betas'][rows], ref['betas']), _check('rot', got['rot'][rows], ref['rot']),
+                _check('camera', got['camera'][rows], ref['camera']))
+    if NE:
+        worst = max(worst, _check('expression', got['expr'][rows], ref['expression']))
+    print(f'[model-shapes] backward {name} n_rot={n_rot} B={B} {kind}: worst error / bar {worst:.3f}')
+
+
+def test_module_autograd_with_expression():
+    """SMPLX.forward through autograd on nb16_ne16 (NC = 32): betas, expression, the rotations, transl."""
+    name = 'nb16_ne16'
+    module = _module(name)
+    NB, NE, _ = VARIANTS[name]
+    B = 9
+    x = _inputs(16, B, 22, NB, NE)
+    leaf = {k: x[k].cuda().requires_grad_(True) for k in ('betas', 'expression', 'transl')}
+    leaf['rot'] = x['rot'].cuda().requires_grad_(True)
+    out = module(global_rot=leaf['rot'][:, :1], body_pose=leaf['rot'][:, 1:], betas=leaf['betas'],
+                 expression=leaf['expression'], transl=leaf['transl'])
+    gen = torch.Generator().manual_seed(17)
+    V = module.get_num_verts()
+    cot = dict(vertices=torch.randn(B, V, 3, generator=gen), joints=torch.randn(B, 123, 3, generator=gen),
+               v_shaped=torch.randn(B, V, 3, generator=gen) * 0.5)
+    loss = sum((out[k][:] * cot[k].cuda()).sum() for k in cot)
+    loss.backward()
+    ref, _ = oracle_grads(variant_model(name), cot, x['betas'], x['rot'], expression=x['expression'],
+                          transl=x['transl'])
+    worst = max(_check(k, leaf[k].grad, ref[k]) for k in ('betas', 'expression', 'rot', 'transl'))
+    print(f'[model-shapes] module autograd {name}: worst error / bar {worst:.3f}')
+
+
+# ------------------------------------------------------------------------------------------------ keypoint Jacobian
+def _blocks(n_rot, NB):
+    return (('rot', slice(0, 3 * n_rot)), ('betas', slice(3 * n_rot, 3 * n_rot + NB)))
+
+
+@pytest.mark.parametrize('with_transl', [False, True])
+@pytest.mark.parametrize('n_rot', [1, 22, 55])
+@pytest.mark.parametrize('name', NAMES)
+def test_jacobian_vs_float64(packed, name, n_rot, with_transl):
+    from shapy_b200 import ops
+    m, pk = variant_model(name), packed(name)
+    NB = VARIANTS[name][0]
+    B = 2
+    x = _inputs(1000 * NB + 10 * n_rot + with_transl, B, n_rot, NB)
+    transl = x['transl'] if with_transl else None
+    kp, jac = ops.smplx_keypoint_jacobian(pk, x['betas'].cuda(), x['rot'].cuda(),
+                                          None if transl is None else transl.cuda())
+    P = 3 * n_rot + NB + 3
+    assert jac.shape == (B, 3 * pk.K, P) and kp.shape == (B, pk.K, 3)
+    kp, jac = kp.double().cpu().numpy(), jac.double().cpu().numpy()
+    worst = 0.0
+    for b in range(B):
+        k64, j64 = kp_lm_oracle.keypoint_jacobian(m, x['betas'][b], x['rot'][b], None if transl is None else transl[b])
+        assert np.abs(kp[b] - k64).max() <= 1e-5 * np.abs(k64).max(), b
+        for block, cols in _blocks(n_rot, NB):
+            err, scale = np.abs(jac[b][:, cols] - j64[:, cols]).max(), np.abs(j64[:, cols]).max()
+            assert err <= TOL * scale, (b, block, err, scale)
+            worst = max(worst, err / (TOL * scale))
+        assert np.array_equal(jac[b][:, 3 * n_rot + NB:], np.tile(np.eye(3), (pk.K, 1)))
+    print(f'[model-shapes] jacobian {name} n_rot={n_rot} transl={with_transl}: worst error / bar {worst:.3f}')
+
+
+@pytest.mark.parametrize('n_rot', [1, 22, 55])
+def test_cached_and_uncached_entries_give_the_same_bits(packed, n_rot):
+    """edge_2048 caches its 2 048 keypoint entries in shared memory, edge_2049 (one more J14 non-zero, in the row of
+    keypoint 15) recomputes each entry's vertex state where it is used.  Every other keypoint row, and every keypoint,
+    must be bit-identical."""
+    from shapy_b200 import ops
+    a, b = variant_model('edge_2048'), variant_model('edge_2049')
+    assert keypoint_entries(a) == KP_CACHE_ENTRIES < keypoint_entries(b)
+    B = 64
+    x = _inputs(2048 + n_rot, B, n_rot, 10)
+    args = (x['betas'].cuda(), x['rot'].cuda(), x['transl'].cuda())
+    kp_a, jac_a = ops.smplx_keypoint_jacobian(packed('edge_2048'), *args)
+    kp_b, jac_b = ops.smplx_keypoint_jacobian(packed('edge_2049'), *args)
+    K = kp_a.shape[1]
+    keep = torch.tensor([k for k in range(K) if k != CHANGED_KP], device='cuda')
+    rows = (3 * keep[:, None] + torch.arange(3, device='cuda')).reshape(-1)
+    assert torch.equal(_bits(kp_a[:, keep]), _bits(kp_b[:, keep]))
+    assert torch.equal(_bits(jac_a[:, rows]), _bits(jac_b[:, rows]))
+    # the added entry does reach keypoint 15 (the two models differ there)
+    assert not torch.equal(kp_a[:, CHANGED_KP], kp_b[:, CHANGED_KP])
+
+
+def test_jacobian_transpose_equals_backward(packed):
+    """nb27_ne5_dense at B = 256: J^T c for a random joints cotangent c against shapy_smplx_backward (whose betas
+    gradient comes from the generic shape adjoint over 27 rows): the betas block equals grad_betas, each rotation block
+    the tangent projection sum_e (dL/dR_j)_e (R_j [e_a]x)_e of grad_rot."""
+    from shapy_b200 import ops
+    name = 'nb27_ne5_dense'
+    pk, NB = packed(name), VARIANTS[name][0]
+    B, n_rot = 256, 22
+    x = _inputs(7, B, n_rot, NB)
+    rot, betas, transl = x['rot'].cuda(), x['betas'].cuda(), x['transl'].cuda()
+    c = torch.randn(B, pk.K, 3, generator=torch.Generator().manual_seed(8)).cuda()
+    _, jac = ops.smplx_keypoint_jacobian(pk, betas, rot, transl)
+    jtc = torch.einsum('brp,br->bp', jac.double(), c.double().reshape(B, -1))
+    del jac
+    g = ops.smplx_backward(pk, betas, rot, grad_joints=c, want=('betas', 'rot'))
+    E = torch.zeros(3, 3, 3, dtype=torch.float64, device='cuda')   # [e_a]x
+    for a in range(3):
+        E[a, (a + 2) % 3, (a + 1) % 3], E[a, (a + 1) % 3, (a + 2) % 3] = 1.0, -1.0
+    D = torch.einsum('bjrm,amc->bjarc', rot.double(), E)           # R_j [e_a]x
+    proj = torch.einsum('bjrc,bjarc->bja', g['rot'].double(), D).reshape(B, -1)
+    worst = 0.0
+    for block, got, ref in (('rot', jtc[:, :3 * n_rot], proj),
+                            ('betas', jtc[:, 3 * n_rot:3 * n_rot + NB], g['betas'].double())):
+        err = (got - ref).abs().amax(1)
+        scale = ref.abs().amax(1)
+        assert bool((err <= TOL * scale).all()), (block, float((err / scale).max()))
+        worst = max(worst, float((err / (TOL * scale)).max()))
+    print(f'[model-shapes] J^T c vs backward {name}: worst error / bar {worst:.3f}')
+
+
+# ------------------------------------------------------------------------------------------------ LM steps
+# (n_rot, nb): P = 3 n_rot + nb + 3 = 7, 54 (the largest P under 48 KB of shared memory without opting in), 55 (the
+# smallest that opts in, twice: nb 16 and 1), 96 (kLmKpMaxP)
+STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27)]
+STEP_K = [1, 5, 6, 127]           # 3K < 16 rows; K = 6 has a dropped keypoint 5 whose rows 15-17 straddle row 16
+
+
+def _step_case(n_rot, nb, K, meas):
+    """Six bodies with random well-conditioned Jacobians: body 0's trial hits its targets (accepted), body 1's state
+    does and its trial is far (rejected), body 2 has a weighted NaN trial keypoint (rejected), with measurements body
+    3 a weighted NaN trial measurement (rejected), 4 and 5 random.  With K >= 6 keypoint 5 has weight 0 and NaN
+    keypoints and rows in state and trial; with measurements the height has weight 0 and NaN values and rows."""
+    B, P = 6, 3 * n_rot + nb + 3
+    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + (7 if meas else 0))
+    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
+    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
+    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
+    betas, transl = rn(B, nb), rn(B, 3) * 0.1
+    tbetas, ttransl = betas + 0.05 * rn(B, nb), transl + 0.01 * rn(B, 3)
+    kp, jac = rn(B, K, 3), rn(B, 3 * K, P)
+    tkp, tjac = kp + 0.05 * rn(B, K, 3), jac + 0.1 * rn(B, 3 * K, P)
+    tg = kp + 0.05 * rn(B, K, 3)
+    w = torch.rand(B, K, generator=gen) + 0.5
+    kp[0] = tkp[0] + 0.5
+    tg[0] = tkp[0]
+    tg[1], tkp[1] = kp[1], kp[1] + 0.5
+    tkp[2, 0, 1] = float('nan')
+    if K >= 6:
+        w[:, 5] = 0.0
+        for t in (kp, tkp):
+            t[:, 5] = float('nan')
+        for t in (jac, tjac):
+            t[:, 15:18] = float('nan')
+    c = dict(rot=rot, betas=betas, transl=transl, kp=kp, jac=jac, trot=trot, tbetas=tbetas, ttransl=ttransl, tkp=tkp,
+             tjac=tjac, tg=tg, w=w, lam=torch.rand(B, generator=gen) + 0.01)
+    if meas:
+        m, mj = torch.rand(B, 5, generator=gen) + 0.5, rn(B, 5, nb)
+        tm, tmj = m + 0.01 * rn(B, 5), mj + 0.1 * rn(B, 5, nb)
+        mt = m + 0.02 * rn(B, 5)
+        mt[0], mt[1] = tm[0], m[1]
+        mw = torch.rand(B, 5, generator=gen) * 2 + 0.5
+        mw[:, 1] = 0.0
+        for t in (m, tm, mj, tmj):
+            t[:, 1] = float('nan')
+        tm[3, 3] = float('nan')
+        c.update(meas=m, mjac=mj, tmeas=tm, tmjac=tmj, mt=mt, mw=mw)
+    return c
+
+
+def _run_step(c, first, rho=None):
+    """The kernel on the case (rho None: the keypoint step), then the restatement body by body; returns the largest
+    trial error over its bar and the accepted flags."""
+    from shapy_b200 import ops
+    B = c['rot'].shape[0]
+    meas = rho is not None
+    n = lambda t: t.numpy()  # noqa: E731
+    s_np = []
+    for b in range(B):
+        s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'transl': n(c['transl'][b]), 'keypoints': n(c['kp'][b]),
+             'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
+        if meas:
+            s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
+            s['loss'] = np.float32(kpm_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], n(c['mt'][b]),
+                                                      n(c['mw'][b]), s['meas'], rho, s['betas']))
+        else:
+            s['loss'] = np.float32(kp_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints']))
+        s_np.append(s)
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'transl': cu(c['transl']), 'keypoints': cu(c['kp']),
+             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([s['loss'] for s in s_np]))),
+             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
+    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'transl': cu(c['ttransl'])}
+    if meas:
+        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
+        ops.fit_lm_keypoints_measurements_step(state, trial, cu(c['tg']), cu(c['w']), cu(c['mt']), cu(c['mw']), rho,
+                                               10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']), cu(c['tmeas']),
+                                               cu(c['tmjac']))
+    else:
+        ops.fit_lm_keypoints_step(state, trial, cu(c['tg']), cu(c['w']), 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']))
+    got = {k: v.cpu().numpy() for k, v in state.items()}
+    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
+    flags, worst = [], 0.0
+    for b in range(B):
+        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
+        if meas:
+            new, want, acc = kpm_lm_oracle.lm_keypoints_measurements_step(
+                s_np[b], n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), rho, 10.0, 3.0, first, tr,
+                n(c['tkp'][b]), n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]))
+        else:
+            new, want, acc = kp_lm_oracle.lm_keypoints_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
+                                                            n(c['tkp'][b]), n(c['tjac'][b]))
+        flags.append(acc)
+        assert got['accepted'][b] == new['accepted'], b
+        assert got['lambda'][b] == new['lambda'], (b, got['lambda'][b], new['lambda'])
+        assert np.array_equal(got['loss'][b], new['loss'], equal_nan=True), (b, got['loss'][b], new['loss'])
+        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac') + (('meas', 'meas_jac') if meas else ()):
+            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
+        for k in ('rot', 'betas', 'transl'):
+            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
+            err = np.abs(nxt[k][b] - want[k]).max()
+            assert err <= bar, (b, k, err)
+            worst = max(worst, err / bar)
+    if first:
+        assert all(flags)
+    else:
+        assert flags[:3] == [True, False, False] and (not meas or not flags[3]), flags
+    return worst
+
+
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('K', STEP_K)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_keypoint_step_vs_oracle(n_rot, nb, K, first):
+    worst = _run_step(_step_case(n_rot, nb, K, False), first)
+    print(f'[model-shapes] kp step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first}: trial error / bar {worst:.3f}')
+
+
+@pytest.mark.parametrize('rho', [0.0, 0.05])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('K', STEP_K)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_keypoint_measurement_step_vs_oracle(n_rot, nb, K, first, rho):
+    worst = _run_step(_step_case(n_rot, nb, K, True), first, rho)
+    print(f'[model-shapes] kpm step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first} rho={rho}: '
+          f'trial error / bar {worst:.3f}')
+
+
+def test_steps_refuse_97_parameters_without_a_launch():
+    from shapy_b200 import _lib
+    L = _lib.lib()
+    z = lambda *s: torch.zeros(*s, device='cuda')  # noqa: E731
+    B, K, n_rot, nb = 2, 6, 31, 1
+    P = 3 * n_rot + nb + 3
+    assert P == 97
+    st = [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]
+    tr = [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]
+    loss, lam, acc = z(B), z(B), torch.zeros(B, dtype=torch.int32, device='cuda')
+    p = lambda ts: [_lib.ptr(t) for t in ts]  # noqa: E731
+    torch.cuda.synchronize()
+    n0 = L.shapy_launch_count()
+    rc = L.shapy_fit_lm_keypoints_step(B, K, n_rot, nb, _lib.ptr(z(B, K, 3)), _lib.ptr(z(B, K)), 10.0, 3.0, 1,
+                                       *p(st), *p([loss, lam, acc]), *p(tr), None)
+    assert rc == -3                                  # SHAPY_ERR_UNSUPPORTED
+    rc = L.shapy_fit_lm_keypoints_measurements_step(
+        B, K, n_rot, nb, _lib.ptr(z(B, K, 3)), _lib.ptr(z(B, K)), _lib.ptr(z(B, 5)), _lib.ptr(z(B, 5)), 0.0, 10.0, 3.0,
+        1, *p(st), *p([z(B, 5), z(B, 5, nb), loss, lam, acc]), *p(tr), *p([z(B, 5), z(B, 5, nb)]), None)
+    assert rc == -3
+    torch.cuda.synchronize()
+    assert L.shapy_launch_count() == n0
+
+
+# ------------------------------------------------------------------------------------------------ fits
+FIT_CASES = {'nb27_ne5_dense': None, 'nb16_ne16': ('height', 'mass')}
+
+
+def _fit_targets(module, NB, B, bm=None, seed=31):
+    """The recipe of test_gpu_fit_lm_keypoints._targets at the model's NB, plus the measurements of the generating
+    betas."""
+    from shapy_b200 import ops
+    gen = torch.Generator().manual_seed(seed)
+    bstar = torch.randn(B, NB, generator=gen).clamp(-2, 2).cuda()
+    raw = synth.mean_params()[:132] + 0.3 * torch.randn(B, 132, generator=gen)
+    with torch.no_grad():
+        rot = ops.decode_rot6d(raw.cuda())
+        kp = module(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=bstar)['joints'][:].clone()
+        meas = None
+        if bm is not None:
+            m = bm.forward_vertices(module.forward_shape(betas=bstar)['v_shaped'], module.faces_i32)['measurements']
+            meas = {k: m[k]['tensor'].clone() for k in m}
+    return kp, meas
+
+
+@pytest.mark.parametrize('name', list(FIT_CASES))
+def test_lm_fit(packed, name):
+    """fit_body_to_keypoints(method='lm') on 32 bodies: nb27_ne5_dense (P = 96, the uncached Jacobian) and nb16_ne16
+    with height and mass (the four-launch stacked loop at NB = 16).  Every body's loss is at most its start, 8 bodies
+    fitted alone equal their batch rows, the loop never synchronises, and the Jacobian and the backward repeat their
+    bits."""
+    from shapy_b200 import ops
+    from shapy_b200.fit import fit_body_to_keypoints
+    NB, NE, _ = VARIANTS[name]
+    module = _module(name)
+    bm, kw = None, {}
+    if FIT_CASES[name]:
+        from shapy_b200.body_measurements import BodyMeasurements
+        bm = BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda()
+    B = 32
+    kp, meas = _fit_targets(module, NB, B, bm)
+    if bm is not None:
+        kw = dict(body_measurements=bm, measurements={k: meas[k] for k in FIT_CASES[name]})
+    mean = synth.mean_params().cuda()              # a CPU init would be copied to the device inside the fit
+
+    def fit(kp, kw, iterations=None):
+        n = kp.shape[0]
+        init = {'global_rot': mean[:6].expand(n, 6), 'body_pose': mean[6:132].expand(n, 126)}
+        return fit_body_to_keypoints(module, kp, init=init, method='lm', iterations=iterations, **kw)
+
+    res = fit(kp, kw)
+    start = fit(kp, kw, iterations=0)['loss']
+    assert res['betas'].shape == (B, NB)
+    fin = torch.isfinite(start)
+    assert int(fin.sum()) >= B - 2
+    assert bool((res['loss'][fin] <= start[fin]).all()), (res['loss'], start)
+    print(f'[model-shapes] lm fit {name}: median loss {float(res["loss"].median()):.4g} from '
+          f'{float(start[fin].median()):.4g}')
+    rows = [3, 4, 9, 15, 16, 22, 30, 31]
+    kw8 = dict(kw)
+    if bm is not None:
+        kw8['measurements'] = {k: v[rows].contiguous() for k, v in kw['measurements'].items()}
+    res8 = fit(kp[rows].contiguous(), kw8)
+    keys = ('global_rot', 'body_pose', 'betas', 'transl') + (('measurements',) if bm is not None else ())
+    for k in keys:
+        assert torch.equal(_bits(res8[k]), _bits(res[k][rows])), k
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode('error')
+    try:
+        fit(kp, kw, iterations=3)
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
+    # the Jacobian and the backward twice on the same inputs
+    pk = packed(name)
+    x = _inputs(99, B, 22, NB, NE)
+    c = lambda t: None if t is None else t.cuda()  # noqa: E731
+    j1, j2 = (ops.smplx_keypoint_jacobian(pk, c(x['betas']), c(x['rot']), c(x['transl'])) for _ in range(2))
+    assert all(torch.equal(_bits(a), _bits(b)) for a, b in zip(j1, j2))
+    gen = torch.Generator().manual_seed(100)
+    cot = dict(grad_vertices=torch.randn(B, pk.V, 3, generator=gen).cuda(),
+               grad_joints=torch.randn(B, pk.K, 3, generator=gen).cuda(),
+               grad_v_shaped=torch.randn(B, pk.V, 3, generator=gen).cuda())
+    g1, g2 = (ops.smplx_backward(pk, c(x['betas']), c(x['rot']), expr=c(x['expression']), **cot) for _ in range(2))
+    for k in ('betas', 'rot', 'expr'):
+        assert torch.equal(_bits(g1[k]), _bits(g2[k])), k

@@ -1,0 +1,254 @@
+"""CPU: the model variants of the shape tests (tests/test_gpu_model_shapes.py) and the float64 restatements at their
+shapes, before the GPU kernels are compared with them.
+
+Variants of synth.make_smplx() (shape and expression rows randn * 5e-3 seeded as in
+test_gpu_smplx_poses.test_shape_expression_counts, J14 rows seeded random supports with softmax weights as in
+synth.make_smplx's sparse_rows):
+
+  nb1_ne0          NB 1, NE 0, the synthetic J14 (448 non-zeros)      smallest coefficient count
+  nb10_ne0         NB 10, NE 0, the synthetic J14                    NC = NB, no expression rows
+  nb16_ne16        NB 16, NE 16, the synthetic J14                   NC = 32 = kMaxCoef, NB = 16 = kMaxJacBetas
+  nb27_ne5_dense   NB 27, NE 5, J14 14 x 150                         NC = 32, P = 96 at n_rot = 22, uncached Jacobian
+  edge_2048        NB 10, NE 10, J14 with 1 844 non-zeros            2 048 keypoint entries: the last cached count
+  edge_2049        edge_2048 plus one non-zero in the last J14 row    2 049 entries: the first uncached count
+
+  * kp_lm_oracle.keypoint_jacobian against central differences of the float64 forward on nb1_ne0 and nb27_ne5_dense
+  * kp_lm_oracle.lm_keypoints_step and kpm_lm_oracle against a dense solve of the damped normal equations at P = 7 and
+    P = 96
+  * fit_body_to_keypoints(method='lm') refuses more than 96 parameters before it touches the device"""
+import functools
+import math
+
+import numpy as np
+import pytest
+import torch
+
+import kp_lm_oracle
+import kpm_lm_oracle
+from shapy_b200 import synth
+from test_fit_lm_keypoints_cpu import _keypoints, _rodrigues
+
+KP_CACHE_ENTRIES = 2048           # kKpCacheEntries of smplx.cu: keypoint entries the Jacobian caches in shared memory
+LM_KP_MAX_P = 96                  # kLmKpMaxP of fit.cu
+# name -> (NB, NE, J14 non-zeros per row or None for synth.make_smplx's own 14 x 32)
+VARIANTS = {
+    'nb1_ne0': (1, 0, None),
+    'nb10_ne0': (10, 0, None),
+    'nb16_ne16': (16, 16, None),
+    'nb27_ne5_dense': (27, 5, [150] * 14),
+    'edge_2048': (10, 10, [132] * 13 + [128]),
+    'edge_2049': (10, 10, [132] * 13 + [128]),
+}
+EDGE_EXTRA = 0.02                 # the weight of edge_2049's added non-zero
+
+
+@functools.lru_cache(maxsize=None)
+def _base():
+    return synth.make_smplx()
+
+
+def _j14(seed, counts):
+    V = synth.NUM_VERTS
+    g = torch.Generator().manual_seed(seed)
+    R = torch.zeros(len(counts), V)
+    for r, n in enumerate(counts):
+        idx = torch.randperm(V, generator=g)[:n]
+        R[r, idx] = torch.softmax(torch.randn(n, generator=g), 0)
+    return R
+
+
+@functools.lru_cache(maxsize=None)
+def _variant(name):
+    NB, NE, counts = VARIANTS[name]
+    m = dict(_base())
+    V = m['v_template'].shape[0]
+    g = torch.Generator().manual_seed(NB * 100 + NE)
+    m['shapedirs'] = torch.randn(V, 3, NB, generator=g) * 5e-3
+    m['expr_dirs'] = torch.randn(V, 3, NE, generator=g) * 5e-3      # (V, 3, 0) when NE = 0: no expression basis
+    if counts is not None:
+        R = _j14(sum(counts), counts)
+        if name == 'edge_2049':
+            free = [int(v) for v in torch.randperm(V, generator=torch.Generator().manual_seed(5)) if R[-1, v] == 0]
+            R[-1, free[0]] = EDGE_EXTRA
+        m['extra_joint_regressor'] = R
+    return m
+
+
+def variant_model(name):
+    """A fresh dict of the variant's tensors (the tensors are shared: do not edit them in place)."""
+    return dict(_variant(name))
+
+
+def keypoint_entries(m, use_face_contour=True):
+    """3 (L + D) + nnz(J14): the entry count the keypoint Jacobian compares with KP_CACHE_ENTRIES."""
+    L = m['lmk_faces_idx'].shape[0]
+    D = m['dynamic_lmk_faces_idx'].shape[1] if use_face_contour else 0
+    return 3 * (L + D) + int((m['extra_joint_regressor'] != 0).sum())
+
+
+# ------------------------------------------------------------------------------------------------ variants
+def test_variants_have_their_shapes():
+    want_nnz = {'nb1_ne0': 448, 'nb10_ne0': 448, 'nb16_ne16': 448, 'nb27_ne5_dense': 2100, 'edge_2048': 1844,
+                'edge_2049': 1845}
+    for name, (NB, NE, _) in VARIANTS.items():
+        m = variant_model(name)
+        assert m['shapedirs'].shape[-1] == NB and m['expr_dirs'].shape[-1] == NE, name
+        assert int((m['extra_joint_regressor'] != 0).sum()) == want_nnz[name], name
+        assert NB + NE <= 32, name
+    entries = {name: keypoint_entries(variant_model(name)) for name in VARIANTS}
+    assert entries['edge_2048'] == KP_CACHE_ENTRIES and entries['edge_2049'] == KP_CACHE_ENTRIES + 1
+    assert entries['nb27_ne5_dense'] == 2304 > KP_CACHE_ENTRIES
+    assert 3 * 22 + VARIANTS['nb27_ne5_dense'][0] + 3 == LM_KP_MAX_P
+    # edge_2049 is edge_2048 with one added non-zero in the last J14 row, everything else shared
+    a, b = variant_model('edge_2048'), variant_model('edge_2049')
+    diff = (a['extra_joint_regressor'] != b['extra_joint_regressor']).nonzero()
+    assert diff.shape[0] == 1 and int(diff[0, 0]) == 13 and float(a['extra_joint_regressor'][tuple(diff[0])]) == 0.0
+    for k in a:
+        if k != 'extra_joint_regressor':
+            assert a[k] is b[k] or torch.equal(a[k], b[k]), k
+
+
+# ------------------------------------------------------------------------------------------------ oracle Jacobian
+@pytest.mark.parametrize('name', ['nb1_ne0', 'nb27_ne5_dense'])
+def test_oracle_jacobian_vs_central_differences(name):
+    """The recipe and bar of test_fit_lm_keypoints_cpu.test_oracle_jacobian_vs_central_differences at the variant's
+    NB (and its own J14)."""
+    model = variant_model(name)
+    NB = VARIANTS[name][0]
+    gen = torch.Generator().manual_seed(4)
+    n_rot = 22
+    P = 3 * n_rot + NB + 3
+    for b, neck in enumerate((1.2, -1.2)):                 # necks turned past both ends of the contour LUT
+        rot = _rodrigues(torch.randn(n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
+        rot[12] = _rodrigues(torch.tensor([0.0, neck, 0.0])).float()
+        betas = torch.randn(NB, generator=gen)
+        transl = torch.randn(3, generator=gen) * 0.1
+        kp, jac = kp_lm_oracle.keypoint_jacobian(model, betas, rot, transl)
+        assert jac.shape == (3 * 123, P) and kp.shape == (123, 3)
+        base = _keypoints(model, betas, rot, transl, torch.zeros(1, P, dtype=torch.float64))[0].numpy()
+        assert np.abs(kp - base).max() <= 1e-9 * np.abs(base).max()
+        h = 1e-5
+        fd = []
+        for half in (range(0, P // 2), range(P // 2, P)):
+            e = torch.zeros(2 * len(half), P, dtype=torch.float64)
+            for i, c in enumerate(half):
+                e[2 * i, c], e[2 * i + 1, c] = h, -h
+            y = _keypoints(model, betas, rot, transl, e).reshape(len(half), 2, -1).numpy()
+            fd.append(((y[:, 0] - y[:, 1]) / (2 * h)).T)
+        fd = np.concatenate(fd, 1)
+        for block, cols in (('rot', slice(0, 3 * n_rot)), ('betas', slice(3 * n_rot, 3 * n_rot + NB)),
+                            ('transl', slice(3 * n_rot + NB, P))):
+            err = np.abs(jac[:, cols] - fd[:, cols]).max()
+            assert err <= 1e-6 * np.abs(fd[:, cols]).max(), (b, block, err)
+
+
+# ------------------------------------------------------------------------------------------------ oracle steps
+# (n_rot, nb) -> P = 3 n_rot + nb + 3: the smallest and the largest parameter count the step kernel takes
+STEP_SHAPES = {7: (1, 1), 96: (22, 27)}
+
+
+def _random_step_problem(seed, n_rot, nb, K):
+    """A random state of one body: rotations, betas, transl, keypoints, a (3K, P) Jacobian, targets and weights with
+    a dropped keypoint whose keypoint and rows are NaN, five measurements with one dropped (NaN value and row)."""
+    rng = np.random.default_rng(seed)
+    P = 3 * n_rot + nb + 3
+    x = {'rot': np.stack([kp_lm_oracle.exp_gram_schmidt(np.eye(3), rng.normal(size=3)) for _ in range(n_rot)]),
+         'betas': rng.normal(size=nb), 'transl': rng.normal(size=3) * 0.1}
+    kp, jac = rng.normal(size=(K, 3)), rng.normal(size=(3 * K, P))
+    tg = kp + rng.normal(size=(K, 3)) * 0.1
+    w = rng.uniform(0.5, 1.5, K)
+    w[K // 2] = 0.0
+    kp[K // 2], jac[3 * (K // 2):3 * (K // 2) + 3] = np.nan, np.nan
+    meas, mjac = rng.uniform(0.5, 1.5, 5), rng.normal(size=(5, nb))
+    mt, mw = meas + rng.normal(size=5) * 0.02, np.array([3.0, 0.0, 20.0, 10.0, 5.0])
+    meas[1], mjac[1] = np.nan, np.nan
+    return x, kp, jac, tg, w, meas, mjac, mt, mw
+
+
+def _dense(jac, kp, tg, w, o, nb, mjac=None, meas=None, mt=None, mw=None, rho=0.0):
+    """A and g of the stacked weighted residual, built densely, the rows of a dropped term left out."""
+    rows, res = [], []
+    for k in range(len(w)):
+        if w[k] > 0:
+            for c in range(3):
+                rows.append(math.sqrt(w[k]) * jac[3 * k + c])
+                res.append(math.sqrt(w[k]) * (kp[k, c] - tg[k, c]))
+    P = jac.shape[1]
+    if mjac is not None:
+        for k in range(5):
+            if mw[k] > 0:
+                row = np.zeros(P)
+                row[o:o + nb] = math.sqrt(mw[k]) * mjac[k]
+                rows.append(row)
+                res.append(math.sqrt(mw[k]) * (meas[k] - mt[k]))
+    J, r = np.array(rows), np.array(res)
+    return J.T @ J, J.T @ r, r
+
+
+@pytest.mark.parametrize('P', sorted(STEP_SHAPES))
+def test_oracle_keypoint_step_vs_dense_solve(P):
+    n_rot, nb = STEP_SHAPES[P]
+    x, kp, jac, tg, w, _, _, _, _ = _random_step_problem(P, n_rot, nb, 40)
+    o = 3 * n_rot
+    new, nxt, acc = kp_lm_oracle.lm_keypoints_step({}, tg, w, 10.0, 3.0, True, x, kp, jac, dtype=np.float64)
+    assert acc
+    A, g, r = _dense(jac, kp, tg, w, o, nb)
+    lam = float(new['lambda'])
+    assert lam == pytest.approx(1e-3 * max(np.diag(A).max(), 1e-6), rel=1e-12)
+    assert float(new['loss']) == pytest.approx(float(r @ r), rel=1e-12)
+    want = np.linalg.solve(A + lam * np.eye(P), -g)
+    scale = max(1.0, np.abs(want).max())
+    assert np.abs(nxt['betas'] - (x['betas'] + want[o:o + nb])).max() <= 1e-8 * scale
+    assert np.abs(nxt['transl'] - (x['transl'] + want[o + nb:])).max() <= 1e-8 * scale
+    for j in range(n_rot):
+        R = kp_lm_oracle.exp_gram_schmidt(x['rot'][j], want[3 * j:3 * j + 3])
+        assert np.abs(nxt['rot'][j] - R).max() <= 1e-8 * scale, j
+
+
+@pytest.mark.parametrize('rho', [0.0, 0.05])
+@pytest.mark.parametrize('P', sorted(STEP_SHAPES))
+def test_oracle_keypoint_measurement_step_vs_dense_solve(P, rho):
+    """As test_fit_lm_kp_meas_cpu.test_delta_solves_stacked_normal_equations, at P = 7 and P = 96; without
+    measurement rows and rho the step is the keypoint step's, bit for bit."""
+    n_rot, nb = STEP_SHAPES[P]
+    x, kp, jac, tg, w, meas, mjac, mt, mw = _random_step_problem(P + 1, n_rot, nb, 40)
+    o = 3 * n_rot
+    new, _, acc, delta = kpm_lm_oracle.lm_keypoints_measurements_step(
+        {}, tg, w, mt, mw, rho, 10.0, 3.0, True, x, kp, jac, meas, mjac, dtype=np.float64, return_delta=True)
+    assert acc
+    A, g, r = _dense(jac, kp, tg, w, o, nb, mjac, meas, mt, mw)
+    rho32 = float(np.float32(rho))
+    lam = float(new['lambda'])
+    assert lam == pytest.approx(1e-3 * max(np.diag(A).max(), 1e-6), rel=1e-12)   # the first lambda leaves rho out
+    A[o:o + nb, o:o + nb] += rho32 * np.eye(nb)
+    g[o:o + nb] += rho32 * x['betas']
+    assert float(new['loss']) == pytest.approx(float(r @ r) + rho32 * float(x['betas'] @ x['betas']), rel=1e-12)
+    want = np.linalg.solve(A + lam * np.eye(P), -g)
+    assert np.abs(delta - want).max() <= 1e-8 * np.abs(want).max()
+    # no measurement rows, rho = 0: the keypoint step, bit for bit
+    f = lambda t: np.asarray(t, np.float32)  # noqa: E731
+    x32 = {k: f(v) for k, v in x.items()}
+    a = kp_lm_oracle.lm_keypoints_step({}, f(tg), f(w), 10.0, 3.0, True, x32, f(kp), f(jac))
+    b = kpm_lm_oracle.lm_keypoints_measurements_step({}, f(tg), f(w), f(mt), np.zeros(5, np.float32), 0.0, 10.0, 3.0,
+                                                     True, x32, f(kp), f(jac), f(meas), f(mjac))
+    for k in ('rot', 'betas', 'transl', 'loss', 'lambda', 'accepted'):
+        assert np.array_equal(a[0][k], b[0][k]), k
+    for k in ('rot', 'betas', 'transl'):
+        assert np.array_equal(a[1][k], b[1][k]), k
+
+
+# ------------------------------------------------------------------------------------------------ fit arguments
+def test_lm_fit_refuses_more_than_96_parameters():
+    """NB = 28 gives P = 3 * 22 + 28 + 3 = 97: a ValueError naming the limit, raised before the model is packed or any
+    kernel launched (the module here is on the CPU, where either would fail)."""
+    from shapy_b200.fit import fit_body_to_keypoints
+    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
+    m = dict(_base())
+    g = torch.Generator().manual_seed(2800)
+    m['shapedirs'] = torch.randn(m['v_template'].shape[0], 3, 28, generator=g) * 5e-3
+    m['expr_dirs'] = m['expr_dirs'][:, :, :4]
+    module = SMPLX(data_struct=m, betas={'num': 28}, expression={'num': 4}, use_face_contour=True)
+    kp = torch.zeros(2, 123, 3)
+    with pytest.raises(ValueError, match='96'):
+        fit_body_to_keypoints(module, kp, method='lm')
+    assert module._packed is None
