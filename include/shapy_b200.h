@@ -274,6 +274,34 @@ int shapy_fit_lm_keypoints_measurements_step(
     const float *trial_keypoints, const float *trial_jac, const float *trial_meas, const float *trial_meas_jac,
     void *stream);
 
+/* One Levenberg-Marquardt step per body of the fit of pose, shape and weak-perspective camera to K 2D keypoints, one
+ * CTA per body, with shapy_fit_lm_keypoints_step's policy, lambda constants, solve and rotation update.  Parameters
+ * [delta_j (3 n_rot) | beta (nb) | c0, c1, c2], P = 3 n_rot + nb + 3: the camera (B,3) of shapy_smplx_forward takes
+ * the place of transl, p_k = softplus(c0) (kp_k,xy + (c1, c2)) with the forward's softplus threshold of 20.  Loss, fp64,
+ * left to right: sum_{w_k > 0} w_k rho(|p_k - x_k|^2) (k order) + pose_prior_weight / 2 sum_{j = 1}^{n_rot - 1}
+ * |R_j - R0_j|_F^2 + betas_weight |beta|^2; rho(e) = e when robust_sigma = +inf, else sigma^2 e / (sigma^2 + e)
+ * (Geman-McClure).  A keypoint with weight <= 0 is dropped (its target, keypoint and rows are never read).
+ * targets (B,K,2) in the frame of proj_joints, weights (B,K), pose_anchor (B,n_rot,3,3) the rotations R0 (read only
+ * when pose_prior_weight > 0, may be null otherwise).  The state rot (B,n_rot,3,3), betas (B,nb), camera (B,3),
+ * keypoints (B,K,3) and jac (B,3K,P) are those of shapy_smplx_keypoint_jacobian without transl (its transl columns
+ * are not read), loss (B), lambda (B), accepted (B, a count); trial_rot / trial_betas / trial_camera is the point
+ * whose trial_keypoints / trial_jac were evaluated, and receives the next trial.  Gauss-Newton rows: the x and y rows
+ * of the keypoints, projected (s J on the rotation and betas columns, ds/dc0 (kp_xy + c_xy) on c0, s on c1 / c2),
+ * weighted by w_k rho'(e_k) = w_k sigma^4 / (sigma^2 + e_k)^2 at the state (IRLS); then per prior joint the nine
+ * rows (R_j - R0_j) / sqrt(2) with Jacobian R_j [e_a]x / sqrt(2) in its three columns; then betas_weight beta in the
+ * gradient.  The first lambda is 1e-3 max(diag, 1e-6) of the keypoint rows alone; the diagonal gets betas_weight +
+ * lambda on the betas columns and lambda elsewhere.  Accept / reject compares the true robust losses, so a body's loss
+ * never increases.  The next trial is R_j Exp(delta_j), beta + delta_beta, c + delta_c.  A null pointer,
+ * robust_sigma <= 0 or NaN, a negative prior weight or a lambda factor < 1: SHAPY_ERR_ARG; P > 96:
+ * SHAPY_ERR_UNSUPPORTED.  batch 0: no launch.  Deterministic, no atomics, per-body independent. */
+int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int n_rot, int nb, const float *targets,
+                                   const float *weights, const float *pose_anchor, float robust_sigma,
+                                   float pose_prior_weight, float betas_weight, float lambda_up, float lambda_down,
+                                   int first, float *rot, float *betas, float *camera, float *keypoints, float *jac,
+                                   float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+                                   float *trial_camera, const float *trial_keypoints, const float *trial_jac,
+                                   void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

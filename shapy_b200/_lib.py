@@ -97,6 +97,9 @@ _SIGS = {
     'shapy_fit_lm_keypoints_measurements_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                                          c_void_p, C.c_float, C.c_float, C.c_float, c_int]
                                                  + [c_void_p] * 17 + [c_void_p]),
+    'shapy_fit_lm_keypoints_2d_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, C.c_float,
+                                               C.c_float, C.c_float, C.c_float, C.c_float, c_int]
+                                       + [c_void_p] * 13 + [c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

@@ -53,6 +53,19 @@ heights get no gradient, so those rows are not the derivative of the measured ci
 circumferences at their default weights LM stalls.  'exact' uses the exact derivative (the hull points move with their
 faces and with the planes, which follow their landmarks; include/shapy_b200.h, shapy_measure_backward_exact).  The
 launches are the same in number, and LM still never synchronises with the host.
+
+fit_body_to_keypoints_2d refines a prediction against 2D keypoints (B, K, 2) in the crop frame of the regressor's
+proj_joints = softplus(c0) (joints_xy + c[1:3]): pose, betas and the weak-perspective camera, with an optional
+Geman-McClure robust loss (robust_sigma), a chordal prior keeping the body pose near its start (pose_prior_weight) and
+a betas prior.  With method='lm' each iteration is the keypoint Jacobian of the trial and one
+ops.fit_lm_keypoints_2d_step (the 3D step's policy, the projected rows with IRLS weights, the prior rows), two
+launches, no host synchronisation, every body's loss non-increasing; keypoint_jacobian_2d exposes the projected
+Jacobian.
+
+    python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
+
+shapy_b200.keypoints2d reads OpenPose detections and maps them into that frame; with raw detections and their crop
+descriptors in kp.npz, --keypoint-map openpose_smplx_map.json does the same on the command line.
 """
 import argparse
 import json
@@ -345,6 +358,169 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=N
     return res
 
 
+def keypoint_jacobian_2d(body_model, rot, betas, camera):
+    """The projected keypoints p_k = softplus(c0) (kp_k,xy + c[1:3]) and their Jacobian, composed from
+    keypoint_jacobian (no transl): rot (B, n_rot, 3, 3), betas (B, NB), camera (B, 3).  Returns {'proj_joints'
+    (B, K, 2), 'jacobian' (B, 2K, 3 n_rot + NB + 3)}, rows 2k + c (x, y), columns [delta_j | betas | c0, c1, c2]: the x
+    and y rows of the 3D Jacobian times s on the rotation and betas columns, sigmoid(c0) (kp_xy + c[1:3]) on c0 (1 past
+    softplus' threshold of 20), s on c1 and c2 (the step kernel stages the same rows in fp64)."""
+    device = body_model.shapedirs.device
+    camera = torch.as_tensor(camera, dtype=torch.float32, device=device)
+    res = keypoint_jacobian(body_model, rot, betas)
+    kp, jac = res['keypoints'], res['jacobian']
+    B, K = kp.shape[:2]
+    P = jac.shape[2]
+    c0 = camera[:, 0]
+    s = torch.nn.functional.softplus(c0)                                      # threshold 20, as the forward
+    ds = torch.where(c0 > 20, torch.ones_like(c0), torch.sigmoid(c0))
+    xy = kp[..., :2] + camera[:, None, 1:3]                                   # (B, K, 2)
+    j2 = torch.zeros(B, K, 2, P, dtype=torch.float32, device=device)
+    j2[..., :P - 3] = s[:, None, None, None] * jac.view(B, K, 3, P)[:, :, :2, :P - 3]
+    j2[..., P - 3] = ds[:, None, None] * xy
+    j2[:, :, 0, P - 2] = s[:, None]
+    j2[:, :, 1, P - 1] = s[:, None]
+    return {'proj_joints': s[:, None, None] * xy, 'jacobian': j2.view(B, 2 * K, P)}
+
+
+def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas):
+    """The 2D fit's per-body loss: sum_{w_k > 0} w_k rho(|proj_k - target_k|^2) + pose_w / 2 sum_{j >= 1}
+    |R_j - R0_j|_F^2 + betas_w |betas|^2, rho(e) = e (sigma None) or sigma^2 e / (sigma^2 + e)."""
+    keep = w > 0
+    diff = torch.where(keep[..., None], proj - torch.where(keep[..., None], target, torch.zeros_like(target)),
+                       torch.zeros_like(proj))
+    e = diff.pow(2).sum(-1)
+    if sigma is not None:
+        e = sigma * sigma * e / (sigma * sigma + e)
+    per_body = (torch.where(keep, w, torch.zeros_like(w)) * e).sum(1)
+    if pose_w > 0:
+        per_body = per_body + 0.5 * pose_w * (rot[:, 1:] - anchor[:, 1:]).pow(2).sum((1, 2, 3))
+    if betas_w > 0:
+        per_body = per_body + betas_w * betas.pow(2).sum(1)
+    return per_body
+
+
+def _init_2d(init, B, nb, device, method):
+    """The raw 6D global and body pose, betas and camera to start from: fit_body_to_keypoints' init with 'camera' in
+    place of 'transl'; the regressor's stage output (raw_global_rot, raw_body_pose, betas, camera) works as-is."""
+    init = dict(init or {})
+    for k in ('global_rot', 'body_pose'):
+        if init.get('raw_' + k) is not None:
+            init[k] = init['raw_' + k]
+    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
+    ident[0::3].fill_(1.0)
+    cam = torch.zeros(B, 3, device=device)     # scale softplus(0.9) ~ 1.24, the regressor's mean scale
+    cam[:, 0].fill_(0.9)
+    start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
+             'betas': torch.zeros(B, nb, device=device), 'camera': cam}
+    params = {}
+    for k, v in start.items():
+        t = init.get(k)
+        t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
+        params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    return params
+
+
+def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
+                             robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05):
+    """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
+    (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
+    the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
+
+    Loss per body: sum_{w_k > 0} w_k rho(|p_k - x_k|^2) + pose_prior_weight / 2 sum_{j=1}^{21} |R_j - R0_j|_F^2 +
+    betas_weight |betas|^2, rho(e) = e when robust_sigma is None, else the Geman-McClure sigma^2 e / (sigma^2 + e).
+    R0 = pose_anchor (B, 22, 3, 3), by default the starting rotations: the prior keeps the body pose near the
+    regressor's prediction (the global rotation has no prior).  weights: None (all 1), (K,) or (B, K); a keypoint with
+    weight <= 0 is dropped and its target may be NaN.  init: fit_body_to_keypoints' init with 'camera' (B, 3) in place
+    of 'transl' (the regressor's stage output, with raw_global_rot / raw_body_pose, works as-is); without a camera the
+    fit starts at c = (0.9, 0, 0).  method: 'adam' (the step size decays geometrically from lr to lr / 100, through
+    SMPLX.forward(camera=...) and the 6D decoder) or 'lm' (batched Levenberg-Marquardt: the raw 6D start is decoded
+    once, then per iteration the keypoint Jacobian of the trial and one ops.fit_lm_keypoints_2d_step, two launches,
+    no host synchronisation; every body's loss is non-increasing).  iterations: None means 600 for Adam and 50 for LM.
+    Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'camera', 'global_rot_mat' (B, 1, 3, 3), 'body_pose_mat'
+    (B, 21, 3, 3), 'keypoints' (B, K, 3) and 'proj_joints' (B, K, 2) of the final parameters, 'loss' (B,)}."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if robust_sigma is not None and not robust_sigma > 0:
+        raise ValueError(f'fit_body_to_keypoints_2d: robust_sigma must be > 0 or None, got {robust_sigma}')
+    if not (pose_prior_weight >= 0 and betas_weight >= 0):
+        raise ValueError('fit_body_to_keypoints_2d: pose_prior_weight and betas_weight must be >= 0')
+    nb = body_model.num_betas
+    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
+        raise ValueError(f"fit_body_to_keypoints_2d(method='lm'): 22 rotations, {nb} betas and the camera are "
+                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
+    if iterations is None:
+        iterations = 600 if method == 'adam' else 50
+    from . import ops
+    from .autograd import Rot6dFunction
+    device = body_model.shapedirs.device
+    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device).contiguous()
+    if x.dim() != 3 or x.shape[2] != 2:
+        raise ValueError(f'fit_body_to_keypoints_2d: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    B, K = x.shape[0], x.shape[1]
+    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
+                                                                             device=device)
+    w = w.expand(B, K).contiguous()
+    params = _init_2d(init, B, nb, device, method)
+    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
+                                                              device=device).reshape(B, 22, 3, 3).contiguous()
+    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
+    pw, bw = float(pose_prior_weight), float(betas_weight)
+    if method == 'lm':
+        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw)
+    opt = torch.optim.Adam(list(params.values()), lr=lr)
+    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], camera=params['camera'],
+                         return_shaped=False)
+        rot = torch.cat([grot, bpose], 1)
+        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
+        return per_body, out, grot, bpose
+
+    for _ in range(int(iterations)):
+        opt.zero_grad(set_to_none=True)
+        loss_fn()[0].sum().backward()
+        opt.step()
+        sched.step()
+    with torch.no_grad():
+        per_body, out, grot, bpose = loss_fn()
+    res = {k: v.detach() for k, v in params.items()}
+    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
+               loss=per_body)
+    return res
+
+
+def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw):
+    from . import ops
+    device = x.device
+    packed = body_model.packed(device)
+    B, K = x.shape[0], x.shape[1]
+    n_rot, nb = 22, params['betas'].shape[1]
+    P = 3 * n_rot + nb + 3
+    trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'camera': params['camera'].contiguous()}
+    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+    state = {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), 'camera': mk(B, 3), 'keypoints': mk(B, K, 3),
+             'jac': mk(B, 3 * K, P), 'loss': mk(B), 'lambda': mk(B),
+             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    if B > 0:
+        for it in range(iterations + 1):
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
+            ops.fit_lm_keypoints_2d_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac,
+                                         pose_anchor=anchor if pw > 0 else None)
+    rot = state['rot']
+    with torch.no_grad():
+        out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
+                         return_shaped=False)
+        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
+    raw = rot[..., :2].reshape(B, n_rot * 6)       # the first two columns in the decoder's row-major 3x2 layout
+    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
+            'camera': state['camera'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:],
+            'keypoints': out['joints'][:], 'proj_joints': out['proj_joints'], 'loss': per_body}
+
+
 def main(argv=None):
     p = argparse.ArgumentParser(description='Fit SMPL-X betas to virtual measurements (batched, on the GPU)')
     src = p.add_mutually_exclusive_group(required=True)
@@ -371,6 +547,19 @@ def main(argv=None):
     p.add_argument('--iterations', type=int, default=None, help='default 500 for adam, 50 for lm')
     p.add_argument('--lr', type=float, default=0.05, help='Adam step size (ignored by lm)')
     p.add_argument('--output', type=str, default='fit_betas.npz')
+    p.add_argument('--keypoints-2d', dest='keypoints_2d', type=str, default=None,
+                   help='npz with keypoints (B, K, 2) in the crop frame of proj_joints and optional weights (B, K), or '
+                        'raw OpenPose detections openpose (B, 135, 3) in pixels with the crop descriptors center '
+                        '(B, 2) and scale (B,) (and optionally crop_size, default 256; needs --keypoint-map): fit pose, '
+                        'shape and camera to them instead of betas to measurements')
+    p.add_argument('--keypoint-map', dest='keypoint_map', type=str, default=None,
+                   help='JSON OpenPose -> model keypoint map (shapy_b200.keypoints2d), e.g. '
+                        'tests/golden/openpose_smplx_map.json')
+    p.add_argument('--init', type=str, default=None,
+                   help='npz with raw_global_rot / raw_body_pose (or global_rot / body_pose raw 6D), betas and camera, '
+                        'e.g. a saved regressor prediction')
+    p.add_argument('--robust-sigma', dest='robust_sigma', type=float, default=None)
+    p.add_argument('--pose-prior-weight', dest='pose_prior_weight', type=float, default=0.0)
     a = p.parse_args(argv)
 
     from . import synth
@@ -381,6 +570,8 @@ def main(argv=None):
     else:
         model = SMPLX(model_folder=a.model_folder, gender=a.gender, ext=a.ext, betas={'num': a.num_betas})
     model = model.cuda()
+    if a.keypoints_2d:
+        return _main_keypoints_2d(a, model)
     if a.meas_definition_path and a.meas_vertices_path:
         cfg = {'meas_definition_path': a.meas_definition_path, 'meas_vertices_path': a.meas_vertices_path}
     else:
@@ -398,6 +589,34 @@ def main(argv=None):
              loss=res['loss'].cpu().numpy())
     print(json.dumps({'bodies': int(meas.shape[0]), 'output': a.output,
                       'first_body': {k: float(meas[0, i]) for i, k in enumerate(NAMES)}}))
+
+
+def _main_keypoints_2d(a, model):
+    d = np.load(a.keypoints_2d)
+    if 'openpose' in d.files:
+        from . import keypoints2d as k2d
+        if not a.keypoint_map:
+            raise SystemExit('--keypoints-2d with raw OpenPose detections needs --keypoint-map')
+        kmap = k2d.load_keypoint_map(a.keypoint_map)
+        op = k2d.threshold_confidence(d['openpose'].reshape(-1, k2d.NUM_OPENPOSE, 3), kmap)
+        size = int(d['crop_size']) if 'crop_size' in d.files else 256
+        x, w = k2d.map_keypoints(k2d.to_crop(op, d['center'], d['scale'], size), kmap, model.packed().K)
+    else:
+        x = d['keypoints'].astype(np.float32)
+        x = x[None] if x.ndim == 2 else x
+        w = d['weights'].astype(np.float32).reshape(x.shape[:2]) if 'weights' in d.files else None
+    init = None
+    if a.init:
+        p = np.load(a.init)
+        init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(x.shape[0], -1)
+                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera')
+                if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+    res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
+                                   robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
+                                   betas_weight=a.betas_weight, lr=a.lr)
+    out = {k: v.detach().cpu().numpy() for k, v in res.items()}
+    np.savez(a.output, **out)
+    print(json.dumps({'bodies': int(x.shape[0]), 'output': a.output, 'median_loss': float(np.median(out['loss']))}))
 
 
 if __name__ == '__main__':

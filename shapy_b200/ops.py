@@ -495,6 +495,50 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
             ptr(trial_meas), ptr(trial_meas_jac), stream_ptr()), what)
 
 
+def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
+                             lambda_down, first, trial_keypoints, trial_jac, pose_anchor=None):
+    """One Levenberg-Marquardt step per body of the fit of pose, shape and weak-perspective camera to 2D keypoints
+    (include/shapy_b200.h, shapy_fit_lm_keypoints_2d_step), in place.  state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB),
+    'camera' (B, 3), 'keypoints' (B, K, 3), 'jac' (B, 3K, P), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32};
+    trial: {'rot', 'betas', 'camera'}, the evaluated trial on entry and the next trial on return; trial_keypoints /
+    trial_jac from smplx_keypoint_jacobian without transl; targets (B, K, 2), weights (B, K); robust_sigma None or inf
+    for least squares; pose_anchor (B, n_rot, 3, 3), needed when pose_prior_weight > 0."""
+    what = 'fit_lm_keypoints_2d_step'
+    B, n_rot = trial['rot'].shape[:2]
+    nb, K = trial['betas'].shape[1], targets.shape[1]
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    anchor = [] if pose_anchor is None else [pose_anchor]
+    ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + \
+        [trial[k] for k in ('rot', 'betas', 'camera')] + [targets, weights, trial_keypoints, trial_jac] + anchor
+    for t in ts + [state['accepted']]:
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
+            raise RuntimeError(f'{what}: every tensor must be a contiguous CUDA tensor')
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise RuntimeError(f'{what}: the state, trial, targets, weights and anchor must be float32')
+    if state['accepted'].dtype != torch.int32:
+        raise RuntimeError(f'{what}: accepted must be int32')
+    P = 3 * n_rot + nb + 3
+    if (trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K)
+            or targets.shape != (B, K, 2)):
+        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
+    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if B == 0:
+        return
+    with torch.cuda.device(trial['rot'].device):
+        check(lib().shapy_fit_lm_keypoints_2d_step(
+            B, K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma, float(pose_prior_weight),
+            float(betas_weight), float(lambda_up), float(lambda_down), int(bool(first)),
+            *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+            ptr(trial['rot']), ptr(trial['betas']), ptr(trial['camera']), ptr(trial_keypoints), ptr(trial_jac),
+            stream_ptr()), what)
+
+
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
     """grad_betas (B, NB) = shapedirs^T . grad_v_shaped (B, V, 3): the adjoint of smplx_forward_shape."""
     g = _cuda_f32(grad_v_shaped, 'grad_v_shaped')

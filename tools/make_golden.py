@@ -36,6 +36,11 @@ Everything written here is a small fixture that travels to the GPU box, where
   ref_measure_grad.npz  reference BodyMeasurements autograd gradients (its own body_measurements.py, loaded by oracle/ref_body_measurements.py with
                         the C operator oracle) of each measurement with respect to v_shaped, on img_00 and the 3 extra
                         bodies: dense rows for mass, (rows, values) for height and the circumferences
+  ref_openpose.npz      the reference's OpenPose reading on its 22 sample JSONs (samples/openpose): read_keypoints per
+                        person, the confidences after the OpenPose dataset's per-part thresholds and binarisation,
+                        keyps_to_bbox -> bbox_to_center_scale (factor 1.2), and Keypoints2D.crop + normalize at 256
+  openpose_smplx_map.json   index data of the reference's name tables: the (SMPL-X keypoint, OpenPose keypoint) pairs of
+                        map_keypoints('openpose25_v1' -> 'smplx') and the OpenPose part index lists the thresholds use
   preprocess.npz        reference input stage (transf_utils.crop with cv2 + ToTensor + Normalize) on seeded uint8 images:
                         crop windows, crops with OpenCV's portable path (IPP off) and with this container's IPP build
 """
@@ -561,9 +566,113 @@ def measure_grad_fixture():
     print('ref_measure_grad.npz', {k: v.shape for k, v in out.items() if k.endswith('rows')})
 
 
+def _load_ref_keypoint_utils():
+    """The reference's data/utils/keypoints.py, keypoint_names.py, bbox.py, transf_utils.get_transform and the crop /
+    normalize methods of Keypoints2D, loaded where they lie behind stub parent packages (open3d and the structure
+    base classes are not needed by these functions)."""
+    import types
+    HS = ref_shim.HS
+
+    def stub(name):
+        m = sys.modules.get(name) or types.ModuleType(name)
+        m.__path__ = []
+        sys.modules[name] = m
+        return m
+    o3 = types.ModuleType('open3d')
+    o3.geometry = types.SimpleNamespace(PointCloud=object)
+    sys.modules.setdefault('open3d', o3)
+    for n in ('human_shape', 'human_shape.data', 'human_shape.data.utils'):
+        stub(n)
+    u = stub('human_shape.utils')
+    ty = types.ModuleType('human_shape.utils.typing')
+    ty.Array = ty.Tensor = object
+    sys.modules['human_shape.utils.typing'] = ty
+    npu = ref_shim._load('human_shape.utils.np_utils', HS + '/utils/np_utils.py', 'human_shape.utils')
+    bu = ref_shim._load('human_shape.utils.bool_utils', HS + '/utils/bool_utils.py', 'human_shape.utils')
+    for n in ('Array', 'StringList', 'IntList', 'Tensor'):
+        setattr(u, n, object)
+    u.binarize, u.nand = npu.binarize, bu.nand
+    kpm = ref_shim._load('human_shape.data.utils.keypoints', HS + '/data/utils/keypoints.py', 'human_shape.data.utils')
+    names = ref_shim._load('human_shape.data.utils.keypoint_names', HS + '/data/utils/keypoint_names.py',
+                           'human_shape.data.utils')
+    bbox = ref_shim._load('human_shape.data.utils.bbox', HS + '/data/utils/bbox.py', 'human_shape.data.utils')
+    tu = ref_shim._load('human_shape.utils.transf_utils', HS + '/utils/transf_utils.py', 'human_shape.utils')
+    path = HS + '/data/structures/keypoints.py'
+    src = open(path).read()
+    start = src.index('    def crop(self, center, scale, crop_size=224')
+    end = src.index('    def ', src.index('    def normalize(self', start) + 10)
+    ns = {'np': np, 'torch': torch, 'get_transform': tu.get_transform, 'AbstractStructure': type(None)}
+    body = 'class _Methods:\n' + src[start:end]
+    exec(compile(body, path, 'exec'), ns)                                    # executed where it lies
+
+    class Kp2D:                                                              # the fields the two methods read
+        def __init__(self, kp, size, flip_indices=None, source=None, apply_crop=True, flip_axis=0, dtype=None):
+            kp = np.asarray(kp)
+            self.keypoints, self.conf, self.size = kp[:, :-1], kp[:, -1], size
+            self.apply_crop, self.flip_indices, self.source, self.flip_axis = apply_crop, flip_indices, source, flip_axis
+            self.extra_fields = {}
+
+        def add_field(self, k, v):
+            self.extra_fields[k] = v
+    Kp2D.crop, Kp2D.normalize = ns['_Methods'].crop, ns['_Methods'].normalize
+    return kpm, names, bbox, Kp2D
+
+
+def openpose_fixture(crop_size=256):
+    """The OpenPose dataset's __getitem__ (datasets/openpose.py:148-215) with its defaults: body / hand / face thresholds
+    0.1 / 0.2 / 0.4, binarisation, no face contour, body_dset_factor 1.2."""
+    if not hasattr(np, 'int'):
+        np.int = int                      # Keypoints2D.crop casts with np.int (removed from NumPy 1.24)
+    kpm, names, bbox, Kp2D = _load_ref_keypoint_utils()
+    src_names = names.KEYPOINT_NAMES_DICT['openpose25_v1']
+    parts = kpm.get_part_idxs(src_names, names.KEYPOINT_PARTS)
+    face = parts['face'][:-17]
+    tgt, srcidx, n_target = kpm.map_keypoints('openpose25_v1', 'smplx', names.KEYPOINT_NAMES_DICT)
+    mapping = {'source': 'openpose25_v1', 'target': 'smplx', 'num_target': int(n_target),
+               'pairs': [[int(t), int(s)] for t, s in zip(tgt, srcidx)],
+               'parts': {'body': parts['body'].tolist(), 'left_hand': parts['left_hand'].tolist(),
+                         'right_hand': parts['right_hand'].tolist(), 'face': face.tolist()},
+               'thresholds': {'body': 0.1, 'hand': 0.2, 'face': 0.4}, 'bbox_scale_factor': 1.2}
+    json.dump(mapping, open(os.path.join(G, 'openpose_smplx_map.json'), 'w'), indent=1)
+    out = {k: [] for k in ('raw', 'thresholded', 'center', 'scale', 'bbox_size', 'cropped', 'file_index', 'valid')}
+    folder = os.path.join(REF, 'samples', 'openpose')
+    files = sorted(f for f in os.listdir(folder) if f.endswith('.json'))
+    for fi, f in enumerate(files):
+        people = kpm.read_keypoints(os.path.join(folder, f))
+        for raw in ([] if people is None else people):
+            kp = raw.copy()
+            kp[:, -1] = np.clip(kp[:, -1], 0, 1)
+            body_conf, face_conf = kp[parts['body'], -1], kp[face, -1]
+            lh, rh = kp[parts['left_hand'], -1], kp[parts['right_hand'], -1]
+            body_conf[body_conf < 0.1] = 0.0
+            face_conf[face_conf < 0.4] = 0.0
+            lh[lh < 0.2] = 0.0
+            rh[rh < 0.2] = 0.0
+            kp[parts['body'], -1] = kpm.binarize(body_conf, 0.1, kp.dtype)
+            kp[parts['left_hand'], -1] = kpm.binarize(lh, 0.2, kp.dtype)
+            kp[parts['right_hand'], -1] = kpm.binarize(rh, 0.2, kp.dtype)
+            kp[face, -1] = kpm.binarize(face_conf, 0.4, kp.dtype)
+            center, scale, size = bbox.bbox_to_center_scale(bbox.keyps_to_bbox(kp[:, :-1], kp[:, -1]),
+                                                            dset_scale_factor=1.2)
+            valid = center is not None
+            if valid:
+                c = Kp2D(kp, (1000, 1000, 3)).crop(center, scale, crop_size=crop_size).normalize()
+                cropped = np.concatenate([c.keypoints, c.conf[:, None]], 1)
+            else:
+                center, scale, size, cropped = np.full(2, np.nan), np.nan, np.nan, np.full_like(kp, np.nan)
+            for k, v in (('raw', raw), ('thresholded', kp), ('center', center), ('scale', scale), ('bbox_size', size),
+                         ('cropped', cropped), ('file_index', fi), ('valid', valid)):
+                out[k].append(v)
+    arrs = {k: np.asarray(v) for k, v in out.items()}
+    arrs['files'] = np.array(files)
+    arrs['crop_size'] = np.int32(crop_size)
+    np.savez_compressed(os.path.join(G, 'ref_openpose.npz'), **arrs)
+    print('ref_openpose.npz', {k: v.shape for k, v in arrs.items()}, len(mapping['pairs']), 'mapped keypoints')
+
+
 if __name__ == '__main__':
     which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
-                             'smplx_full', 'camera', 'keypoint', 'measure_grad', 'smplx_grad']
+                             'smplx_full', 'camera', 'keypoint', 'measure_grad', 'smplx_grad', 'openpose']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -597,3 +706,5 @@ if __name__ == '__main__':
         mmi_fixtures()
     if 'measure_grad' in which:
         measure_grad_fixture()
+    if 'openpose' in which:
+        openpose_fixture()
