@@ -20,6 +20,31 @@ constexpr float kLambdaMin = 1e-9f, kLambdaMax = 1e9f;   // lambda is clamped to
 constexpr double kLambdaInit = 1e-3;                     // first lambda = kLambdaInit * max diag(J^T W J) ...
 constexpr double kDiagFloor = 1e-6;                      // ... with that diagonal floored here
 
+// The policy of every step kernel of this file.  The trial is accepted on the first step, and afterwards when its loss
+// is finite and below the state's
+__device__ __forceinline__ bool lm_accept(int first, double lt, float lcur) {
+  const bool better = isfinite(lt) && lt < (double)lcur;   // evaluated either way: `first || (...)` in one expression
+  return first || better;                                  // costs lm_step_kernel eight registers
+}
+
+// The state's loss after that decision; a non-finite start reports NaN
+__device__ __forceinline__ float lm_loss(bool accept, double lt, float lcur) {
+  return accept ? (isfinite(lt) ? (float)lt : __int_as_float(0x7fc00000)) : lcur;
+}
+
+// The damping: on the first step from dmax, the largest diagonal entry of the undamped normal matrix floored at
+// kDiagFloor; afterwards the previous lambda over `down` after an accepted trial, times `up` after a rejected one
+__device__ __forceinline__ float lm_lambda(int first, bool accept, float lam, double dmax, float up, float down) {
+  if (first) {
+    lam = (float)(kLambdaInit * dmax);
+  } else if (accept) {
+    lam = lam / down;
+  } else {
+    lam = lam * up;
+  }
+  return fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
+}
+
 struct LmArgs {
   int B, nb;
   const float *targets, *weights;
@@ -57,14 +82,13 @@ __global__ void __launch_bounds__(128) lm_step_kernel(LmArgs a) {
   const double lt = data + (double)a.rho * reg;
   // 2. accept or reject
   const float lcur = a.loss[b];
-  const bool accept = a.first || (isfinite(lt) && lt < (double)lcur);
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
   float lam = a.first ? 0.f : a.lambda[b];
   const float *J = accept ? tjac : jac;
   const float *M = accept ? tmeas : meas;
   float bcur = lane < nb ? (accept ? tb : beta[lane]) : 0.f;
-  float lnew = lcur;
   if (accept) {
-    lnew = isfinite(lt) ? (float)lt : __int_as_float(0x7fc00000);   // a non-finite start reports NaN
     if (lane < nb) beta[lane] = tb;
     if (lane < 5) meas[lane] = tmeas[lane];
     for (int i = lane; i < 5 * nb; i += 32) jac[i] = tjac[i];
@@ -86,18 +110,13 @@ __global__ void __launch_bounds__(128) lm_step_kernel(LmArgs a) {
     g += wi * r;
   }
   g += (double)a.rho * (double)bcur;
+  double dmax = kDiagFloor;
   if (a.first) {
-    double dmax = kDiagFloor;
 #pragma unroll
     for (int j = 0; j < kLmMaxBetas; ++j)
       if (j < nb) dmax = fmax(dmax, __shfl_sync(0xffffffffu, A[j], j));     // lane j's diagonal
-    lam = (float)(kLambdaInit * dmax);
-  } else if (accept) {
-    lam = lam / a.down;
-  } else {
-    lam = lam * a.up;
   }
-  lam = fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
+  lam = lm_lambda(a.first, accept, lam, dmax, a.up, a.down);
   if (lane == 0) {
     a.lambda[b] = lam;
     if (accept && !a.first) a.accepted[b] += 1;
@@ -156,46 +175,108 @@ __global__ void __launch_bounds__(128) lm_step_kernel(LmArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// One Levenberg-Marquardt step of the fit of pose and shape to 3D keypoints (shapy_fit_lm_keypoints_step), one CTA per
-// body.  Parameters [delta_j (3 n_rot) | beta (NB) | t (3)], P = 3 n_rot + NB + 3, R_j(delta) = R_j Exp(delta_j); the
-// caller evaluates the trial with shapy_smplx_keypoint_jacobian.  The policy is lm_step_kernel's without the betas
-// regulariser: L = sum_{w_k > 0} w_k |kp_k - target_k|^2 (fp64, k order), accept a finite trial loss below the state's,
-// lambda / down or * up, clamped; then (J^T W J + lambda I) delta = -J^T W (kp - target) by a right-looking Cholesky of
-// the P x P normal matrix in fp64 shared memory, and the next trial R_j Exp(delta_j) (Rodrigues in fp64, re-orthonormalised
-// by the 6D decoder's Gram-Schmidt of the first two columns), beta + delta_beta, t + delta_t, rounded to fp32.
-//
-// MEAS (shapy_fit_lm_keypoints_measurements_step) stacks the five virtual measurements and the betas regulariser under
-// the keypoint rows: L = L_kp + sum_{w_k > 0} w_k (t_k - m_k)^2 (k order) + rho |beta|^2 (l order), left to right.  The
-// measurement Jacobian (5, NB) only has betas columns, so its rows are accumulated after the keypoint rows into the
-// betas block of A and g (k order), then rho beta into g; the first lambda comes from diag(A) without rho (as in
-// lm_step_kernel) and the betas diagonal gets (double)rho + (double)lambda.  With every measurement weight <= 0 and
-// rho = 0 each extra term is skipped or adds an exact 0, so the step equals the keypoint step bit for bit.
+// The Levenberg-Marquardt steps of the keypoint fits, one CTA per body: pose and shape with a translation against 3D
+// keypoints (lm_kp_step_kernel), or with a weak-perspective camera against 2D keypoints (lm_kp2d_step_kernel).
+// Parameters [delta_j (3 n_rot) | beta (NB) | the last 3: t or c], P =3 n_rot + NB + 3, R_j(delta) = R_j Exp(delta_j);
+// the caller evaluates the trial with shapy_smplx_keypoint_jacobian.  The kernels differ in their loss and in the rows
+// they stage; the phases below, each by the whole CTA on the shared-memory state, are the same code in both:
+//   2. lm_kp_take_trial: an accepted trial becomes the state;
+//   3. lm_kp_pairs, lm_kp_add_rows, lm_kp_damp: the P x P normal matrix J^T W J and g = J^T W r from staged rows, the
+//      lower triangle spread over the threads' registers, then lambda by lm_step_kernel's policy on the diagonal;
+//   4. lm_kp_solve: a right-looking Cholesky in fp64 shared memory and the two triangular solves;
+//   5. lm_kp_next_trial: R_j Exp(delta_j), beta + delta_beta and the last three + their delta, rounded to fp32.
 constexpr int kLmKpMaxP = 96;
 constexpr int kLmKpThreads = 256;
 constexpr int kLmKpPairs = (kLmKpMaxP * (kLmKpMaxP + 1) / 2 + kLmKpThreads - 1) / kLmKpThreads;
 constexpr int kLmKpRows = 16;           // Jacobian rows staged in shared memory at a time
 
-struct LmKpArgs {
+struct LmKpArgs {                       // what the keypoint steps share; `last` is transl (3D) or camera (2D)
   int K, n_rot, nb, P;
   const float *targets, *weights;
   float up, down;
   int first;
-  float *rot, *betas, *transl, *kp, *jac, *loss, *lambda;
+  float *rot, *betas, *last, *kp, *jac, *loss, *lambda;
   int *accepted;
-  float *trot, *tbetas, *ttransl;
+  float *trot, *tbetas, *tlast;
   const float *tkp, *tjac;
 };
 
-struct LmMeasArgs {                     // the measurement block of the MEAS step (unused otherwise)
-  const float *targets, *weights;       // (B, 5): mass, height, chest, waist, hips
-  float rho;                            // betas_weight
-  float *meas, *jac;                    // state (B, 5), (B, 5, NB)
-  const float *tmeas, *tjac;            // the trial's
-};
+// Phase 2 on accept: the trial's parameters, keypoints, Jacobian and loss become the state
+__device__ __forceinline__ void lm_kp_take_trial(const LmKpArgs &a, int b, float lnew) {
+  const int t = threadIdx.x, nb = a.nb, R3 = 3 * a.K;
+  const size_t nr9 = (size_t)a.n_rot * 9;
+  for (size_t i = t; i < nr9; i += blockDim.x) a.rot[b * nr9 + i] = a.trot[b * nr9 + i];
+  for (int i = t; i < nb; i += blockDim.x) a.betas[(size_t)b * nb + i] = a.tbetas[(size_t)b * nb + i];
+  if (t < 3) a.last[(size_t)b * 3 + t] = a.tlast[(size_t)b * 3 + t];
+  for (int i = t; i < R3; i += blockDim.x) a.kp[(size_t)b * R3 + i] = a.tkp[(size_t)b * R3 + i];
+  for (size_t i = t; i < (size_t)R3 * a.P; i += blockDim.x)
+    a.jac[(size_t)b * R3 * a.P + i] = a.tjac[(size_t)b * R3 * a.P + i];
+  if (t == 0) a.loss[b] = lnew;
+}
 
-// Phase 4 of the keypoint steps, by the whole CTA: Cholesky A = L L^T of the P x P lower triangle in shared memory,
-// right-looking (column j scaled, then the trailing lower triangle updated), then L y = -g and L^T delta = y in place
-// in y; thread 0 clears ok_s on a pivot that is not positive and finite
+// Phase 3, ownership: thread t accumulates the lower-triangle entries t + kLmKpThreads i (row-major) of the normal
+// matrix in acc[i], entry (pr[i], pc[i]), pr[i] = -1 past the last one (and g_t, by the caller)
+__device__ __forceinline__ void lm_kp_pairs(int P, int (&pr)[kLmKpPairs], int (&pc)[kLmKpPairs],
+                                            double (&acc)[kLmKpPairs]) {
+  const int npairs = P * (P + 1) / 2;
+#pragma unroll
+  for (int i = 0; i < kLmKpPairs; ++i) {
+    const int p = threadIdx.x + kLmKpThreads * i;
+    int r = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
+    while ((r + 1) * (r + 2) / 2 <= p) ++r;
+    while (r * (r + 1) / 2 > p) --r;
+    pr[i] = p < npairs ? r : -1;
+    pc[i] = p - r * (r + 1) / 2;
+    acc[i] = 0.0;
+  }
+}
+
+// Phase 3, accumulation: A_ij += (w J_ri) J_rj and g_t += (w J_rt) res_r over the nr staged rows in order (Js = J_r,
+// WJs = w J_r, ws = w, rs = res); a row with w <= 0 was not staged and is never read
+__device__ __forceinline__ void lm_kp_add_rows(int nr, int P, const double (*Js)[kLmKpMaxP],
+                                               const double (*WJs)[kLmKpMaxP], const double *ws, const double *rs,
+                                               const int (&pr)[kLmKpPairs], const int (&pc)[kLmKpPairs],
+                                               double (&acc)[kLmKpPairs], double &g) {
+  for (int row = 0; row < nr; ++row) {
+    const double w = ws[row];
+    if (!(w > 0.0)) continue;
+#pragma unroll
+    for (int i = 0; i < kLmKpPairs; ++i)
+      if (pr[i] >= 0) acc[i] += WJs[row][pr[i]] * Js[row][pc[i]];
+    if (threadIdx.x < P) g += WJs[row][threadIdx.x] * rs[row];
+  }
+}
+
+// Phase 3, the end: A and y = -g go to shared memory, then thread 0 sets lambda (lm_lambda; the first from the P
+// entries diag[0], diag[stride], ...: the caller says which rows' diagonal counts), counts an accepted trial and damps
+// the diagonal, by (double)rho + (double)lambda on the columns [lo, hi) and lambda elsewhere.  ok_s starts as "the
+// state's loss is finite": a body without a finite loss does not move
+__device__ __forceinline__ void lm_kp_damp(const LmKpArgs &a, int b, bool accept, float lnew, double *A, double *y,
+                                           const int (&pr)[kLmKpPairs], const int (&pc)[kLmKpPairs],
+                                           const double (&acc)[kLmKpPairs], double g, const double *diag, int stride,
+                                           int lo, int hi, float rho, int &ok_s) {
+  const int P = a.P;
+#pragma unroll
+  for (int i = 0; i < kLmKpPairs; ++i)
+    if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
+  if (threadIdx.x < P) y[threadIdx.x] = -g;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double dmax = kDiagFloor;
+    if (a.first)
+      for (int j = 0; j < P; ++j) dmax = fmax(dmax, diag[j * stride]);
+    const float lam = lm_lambda(a.first, accept, a.first ? 0.f : a.lambda[b], dmax, a.up, a.down);
+    a.lambda[b] = lam;
+    if (accept && !a.first) a.accepted[b] += 1;
+    const double damp = (double)rho + (double)lam;
+    for (int j = 0; j < P; ++j) A[j * P + j] += j >= lo && j < hi ? damp : (double)lam;
+    ok_s = isfinite(lnew);
+  }
+}
+
+// Phase 4: Cholesky A = L L^T of the P x P lower triangle in shared memory, right-looking (column j scaled, then the
+// trailing lower triangle updated), then L y = -g and L^T delta = y in place in y; thread 0 clears ok_s on a pivot that
+// is not positive and finite
 __device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int &ok_s) {
   const int t = threadIdx.x;
   for (int j = 0; j < P; ++j) {
@@ -233,220 +314,11 @@ __device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int &ok
   __syncthreads();
 }
 
-// The next trial rotations of the 2D keypoint step: R_j Exp(delta_j) by Rodrigues in fp64, re-orthonormalised by the 6D
-// decoder's Gram-Schmidt of the first two columns and rounded to fp32, or R_j itself when the step failed (!ok).  The
-// same operations as phase 5 of lm_kp_step_kernel, which keeps its own copy: inlining this helper there reorders
-// its machine code.
-__device__ __forceinline__ void lm_kp_next_rot(const float *sr, float *trr, int n_rot, const double *y, bool ok) {
-  for (int j = threadIdx.x; j < n_rot; j += blockDim.x) {
-    const float *Rs = sr + 9 * j;
-    float *Rt = trr + 9 * j;
-    if (!ok) {
-      for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
-      continue;
-    }
-    const double d0 = y[3 * j], d1 = y[3 * j + 1], d2 = y[3 * j + 2];
-    const double th2 = d0 * d0 + d1 * d1 + d2 * d2, th = sqrt(th2);
-    double s, c;                          // Exp(d) = I + s [d]x + c [d]x^2
-    if (th < 1e-8) {
-      s = 1.0 - th2 / 6.0;
-      c = 0.5 - th2 / 24.0;
-    } else {
-      s = sin(th) / th;
-      c = (1.0 - cos(th)) / th2;
-    }
-    const double dv[3] = {d0, d1, d2};
-    const double Kx[9] = {0.0, -d2, d1, d2, 0.0, -d0, -d1, d0, 0.0};
-    double E[9], Mr[9];
-    for (int r = 0; r < 3; ++r)
-      for (int q = 0; q < 3; ++q) E[r * 3 + q] = (r == q ? 1.0 : 0.0) + s * Kx[r * 3 + q] + c * (dv[r] * dv[q] - (r == q ? th2 : 0.0));
-    for (int r = 0; r < 3; ++r)
-      for (int q = 0; q < 3; ++q)
-        Mr[r * 3 + q] = (double)Rs[r * 3] * E[q] + (double)Rs[r * 3 + 1] * E[3 + q] + (double)Rs[r * 3 + 2] * E[6 + q];
-    // the 6D decoder's Gram-Schmidt of the first two columns
-    const double x0 = Mr[0], x1 = Mr[3], x2 = Mr[6], c0 = Mr[1], c1 = Mr[4], c2 = Mr[7];
-    const double n1 = fmax(sqrt(x0 * x0 + x1 * x1 + x2 * x2), 1e-12);
-    const double b10 = x0 / n1, b11 = x1 / n1, b12 = x2 / n1;
-    const double dd = b10 * c0 + b11 * c1 + b12 * c2;
-    const double u0 = c0 - dd * b10, u1 = c1 - dd * b11, u2 = c2 - dd * b12;
-    const double n2 = fmax(sqrt(u0 * u0 + u1 * u1 + u2 * u2), 1e-12);
-    const double b20 = u0 / n2, b21 = u1 / n2, b22 = u2 / n2;
-    const double b30 = b11 * b22 - b12 * b21, b31 = b12 * b20 - b10 * b22, b32 = b10 * b21 - b11 * b20;
-    Rt[0] = (float)b10; Rt[1] = (float)b20; Rt[2] = (float)b30;
-    Rt[3] = (float)b11; Rt[4] = (float)b21; Rt[5] = (float)b31;
-    Rt[6] = (float)b12; Rt[7] = (float)b22; Rt[8] = (float)b32;
-  }
-}
-
-
-template <bool MEAS>
-__global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, LmMeasArgs mb) {
-  extern __shared__ double A[];         // [P][P]: the lower triangle of J^T W J + lambda I, then its Cholesky factor
-  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
-  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
-  __shared__ double lt_s;
-  __shared__ int ok_s;
-  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K;
-  const float *tg = a.targets + (size_t)b * R3, *wt = a.weights + (size_t)b * K;
-  const float lcur = a.loss[b];
-  // 1. trial loss
-  if (t == 0) {
-    const float *m = a.tkp + (size_t)b * R3;
-    double L = 0.0;
-    for (int k = 0; k < K; ++k) {
-      const double w = wt[k];
-      if (!(w > 0.0)) continue;
-      const double r0 = (double)m[3 * k] - (double)tg[3 * k], r1 = (double)m[3 * k + 1] - (double)tg[3 * k + 1],
-                   r2 = (double)m[3 * k + 2] - (double)tg[3 * k + 2];
-      L += w * (r0 * r0 + r1 * r1 + r2 * r2);
-    }
-    if constexpr (MEAS) {
-      const float *tm = mb.tmeas + (size_t)b * 5, *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
-      double Lm = 0.0;
-      for (int k = 0; k < 5; ++k) {
-        const double w = mw[k];
-        if (w > 0.0) {                     // a dropped term is never read: its measurement may be NaN
-          const double r = (double)mt[k] - (double)tm[k];
-          Lm += w * r * r;
-        }
-      }
-      L += Lm;
-      if (mb.rho > 0.f) {
-        const float *tb = a.tbetas + (size_t)b * a.nb;
-        double reg = 0.0;
-        for (int l = 0; l < a.nb; ++l) reg += (double)tb[l] * (double)tb[l];
-        L += (double)mb.rho * reg;
-      }
-    }
-    lt_s = L;
-  }
-  __syncthreads();
-  // 2. accept or reject; on accept the trial's parameters, keypoints, Jacobian and loss become the state
-  const double lt = lt_s;
-  const bool accept = a.first || (isfinite(lt) && lt < (double)lcur);
-  const float lnew = accept ? (isfinite(lt) ? (float)lt : __int_as_float(0x7fc00000)) : lcur;
-  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
-  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
-  if (accept) {
-    const size_t nr = (size_t)a.n_rot * 9;
-    for (size_t i = t; i < nr; i += blockDim.x) a.rot[b * nr + i] = a.trot[b * nr + i];
-    for (int i = t; i < a.nb; i += blockDim.x) a.betas[(size_t)b * a.nb + i] = a.tbetas[(size_t)b * a.nb + i];
-    if (t < 3) a.transl[(size_t)b * 3 + t] = a.ttransl[(size_t)b * 3 + t];
-    for (int i = t; i < R3; i += blockDim.x) a.kp[(size_t)b * R3 + i] = M[i];
-    for (size_t i = t; i < (size_t)R3 * P; i += blockDim.x) a.jac[(size_t)b * R3 * P + i] = J[i];
-    if constexpr (MEAS) {
-      for (int i = t; i < 5; i += blockDim.x) mb.meas[(size_t)b * 5 + i] = mb.tmeas[(size_t)b * 5 + i];
-      for (int i = t; i < 5 * a.nb; i += blockDim.x) mb.jac[(size_t)b * 5 * a.nb + i] = mb.tjac[(size_t)b * 5 * a.nb + i];
-    }
-    if (t == 0) a.loss[b] = lnew;
-  }
-  // 3. normal equations: A_ij = sum_rows (w J_ri) J_rj (i >= j), g_i = sum_rows (w J_ri) (kp_r - target_r), rows in
-  // keypoint-major xyz order, the rows of a dropped keypoint never read; thread t owns the lower-triangle entries
-  // t + kLmKpThreads i (row-major) and g_t
-  const int npairs = P * (P + 1) / 2;
-  int pr[kLmKpPairs], pc[kLmKpPairs];
-  double acc[kLmKpPairs];
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i) {
-    const int p = t + kLmKpThreads * i;
-    int r = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
-    while ((r + 1) * (r + 2) / 2 <= p) ++r;
-    while (r * (r + 1) / 2 > p) --r;
-    pr[i] = p < npairs ? r : -1;
-    pc[i] = p - r * (r + 1) / 2;
-    acc[i] = 0.0;
-  }
-  double g = 0.0;
-  for (int r0 = 0; r0 < R3; r0 += kLmKpRows) {
-    const int nr = min(kLmKpRows, R3 - r0);
-    __syncthreads();
-    for (int i = t; i < nr; i += blockDim.x) {
-      const double w = wt[(r0 + i) / 3];
-      ws[i] = w;
-      rs[i] = w > 0.0 ? (double)M[r0 + i] - (double)tg[r0 + i] : 0.0;
-    }
-    for (int i = t; i < nr * P; i += blockDim.x) {
-      const int row = i / P;
-      const double w = wt[(r0 + row) / 3];
-      if (w > 0.0) {
-        const double x = J[(size_t)(r0 + row) * P + i % P];
-        Js[row][i % P] = x;
-        WJs[row][i % P] = w * x;
-      }
-    }
-    __syncthreads();
-    for (int row = 0; row < nr; ++row) {
-      const double w = ws[row];
-      if (!(w > 0.0)) continue;
-#pragma unroll
-      for (int i = 0; i < kLmKpPairs; ++i)
-        if (pr[i] >= 0) acc[i] += WJs[row][pr[i]] * Js[row][pc[i]];
-      if (t < P) g += WJs[row][t] * rs[row];
-    }
-  }
-  if constexpr (MEAS) {
-    // the five measurement rows, staged like the keypoint rows, into the betas block [o, o + nb) of A and g
-    const int o = 3 * a.n_rot, nb = a.nb;
-    const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
-    const float *Jm = (accept ? mb.tjac : mb.jac) + (size_t)b * 5 * nb;
-    const float *Mm = (accept ? mb.tmeas : mb.meas) + (size_t)b * 5;
-    __syncthreads();
-    for (int i = t; i < 5; i += blockDim.x) {
-      const double w = mw[i];
-      ws[i] = w;
-      rs[i] = w > 0.0 ? (double)Mm[i] - (double)mt[i] : 0.0;
-    }
-    for (int i = t; i < 5 * nb; i += blockDim.x) {
-      const int row = i / nb;
-      const double w = mw[row];
-      if (w > 0.0) {                       // a dropped term's row is never read: it may be NaN
-        const double x = Jm[i];
-        Js[row][i % nb] = x;
-        WJs[row][i % nb] = w * x;
-      }
-    }
-    __syncthreads();
-    for (int row = 0; row < 5; ++row) {
-      if (!(ws[row] > 0.0)) continue;
-#pragma unroll
-      for (int i = 0; i < kLmKpPairs; ++i)
-        if (pc[i] >= o && pr[i] >= 0 && pr[i] < o + nb) acc[i] += WJs[row][pr[i] - o] * Js[row][pc[i] - o];
-      if (t >= o && t < o + nb) g += WJs[row][t - o] * rs[row];
-    }
-    if (mb.rho > 0.f && t >= o && t < o + nb)
-      g += (double)mb.rho * (double)(accept ? a.tbetas : a.betas)[(size_t)b * nb + t - o];
-  }
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i)
-    if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
-  if (t < P) y[t] = -g;
-  __syncthreads();
-  if (t == 0) {
-    float lam = a.first ? 0.f : a.lambda[b];
-    if (a.first) {
-      double dmax = kDiagFloor;
-      for (int j = 0; j < P; ++j) dmax = fmax(dmax, A[j * P + j]);
-      lam = (float)(kLambdaInit * dmax);
-    } else if (accept) {
-      lam = lam / a.down;
-    } else {
-      lam = lam * a.up;
-    }
-    lam = fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
-    a.lambda[b] = lam;
-    if (accept && !a.first) a.accepted[b] += 1;
-    if constexpr (MEAS) {
-      const int o = 3 * a.n_rot;
-      const double damp = (double)mb.rho + (double)lam;
-      for (int j = 0; j < P; ++j) A[j * P + j] += j >= o && j < o + a.nb ? damp : (double)lam;
-    } else {
-      for (int j = 0; j < P; ++j) A[j * P + j] += (double)lam;
-    }
-    ok_s = isfinite(lnew);               // a body without a finite loss does not move
-  }
-  lm_kp_solve(A, y, P, ok_s);
-  // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
-  const bool ok = ok_s;
+// Phase 5, the next trial from the state and delta = y: the rotations R_j Exp(delta_j) by Rodrigues in fp64,
+// re-orthonormalised by the 6D decoder's Gram-Schmidt of the first two columns, beta + delta_beta and the last three
+// parameters + their delta, all rounded to fp32; the state itself when the step failed (!ok)
+__device__ __forceinline__ void lm_kp_next_trial(const LmKpArgs &a, int b, const double *y, bool ok) {
+  const int t = threadIdx.x, nb = a.nb, o = 3 * a.n_rot;
   const float *sr = a.rot + (size_t)b * a.n_rot * 9;
   float *trr = a.trot + (size_t)b * a.n_rot * 9;
   for (int j = t; j < a.n_rot; j += blockDim.x) {
@@ -487,23 +359,159 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
     Rt[3] = (float)b11; Rt[4] = (float)b21; Rt[5] = (float)b31;
     Rt[6] = (float)b12; Rt[7] = (float)b22; Rt[8] = (float)b32;
   }
-  const int o = 3 * a.n_rot;
-  for (int l = t; l < a.nb; l += blockDim.x) {
-    const float x = a.betas[(size_t)b * a.nb + l];
-    a.tbetas[(size_t)b * a.nb + l] = ok ? (float)((double)x + y[o + l]) : x;
+  for (int l = t; l < nb; l += blockDim.x) {
+    const float x = a.betas[(size_t)b * nb + l];
+    a.tbetas[(size_t)b * nb + l] = ok ? (float)((double)x + y[o + l]) : x;
   }
   if (t < 3) {
-    const float x = a.transl[(size_t)b * 3 + t];
-    a.ttransl[(size_t)b * 3 + t] = ok ? (float)((double)x + y[o + a.nb + t]) : x;
+    const float x = a.last[(size_t)b * 3 + t];
+    a.tlast[(size_t)b * 3 + t] = ok ? (float)((double)x + y[o + nb + t]) : x;
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// One Levenberg-Marquardt step of the fit of pose, shape and weak-perspective camera to 2D keypoints
-// (shapy_fit_lm_keypoints_2d_step), one CTA per body, with lm_kp_step_kernel's policy, solve and rotation update.
-// Parameters [delta_j (3 n_rot) | beta (NB) | c0, c1, c2], P = 3 n_rot + NB + 3: the camera takes the columns of transl
-// (which a weak-perspective camera cannot see along z, and which duplicates c1, c2 in x and y).  With s = softplus(c0)
-// (threshold 20, as the forward) the projection is p_k = s (kp_k,xy + (c1, c2)), and per body, in fp64, left to right:
+// The step of the fit to 3D keypoints (shapy_fit_lm_keypoints_step), the last three parameters the translation t.  The
+// policy is lm_step_kernel's without the betas regulariser: L = sum_{w_k > 0} w_k |kp_k - target_k|^2 (fp64, k order),
+// the rows the keypoint Jacobian's in keypoint-major xyz order, (J^T W J + lambda I) delta = -J^T W (kp - target).
+//
+// MEAS (shapy_fit_lm_keypoints_measurements_step) stacks the five virtual measurements and the betas regulariser under
+// the keypoint rows: L = L_kp + sum_{w_k > 0} w_k (t_k - m_k)^2 (k order) + rho |beta|^2 (l order), left to right.  The
+// measurement Jacobian (5, NB) only has betas columns, so its rows are accumulated after the keypoint rows into the
+// betas block of A and g (k order), then rho beta into g; the first lambda comes from diag(A) without rho (as in
+// lm_step_kernel) and the betas diagonal gets (double)rho + (double)lambda.  With every measurement weight <= 0 and
+// rho = 0 each extra term is skipped or adds an exact 0, so the step equals the keypoint step bit for bit.
+struct LmMeasArgs {                     // the measurement block of the MEAS step (unused otherwise)
+  const float *targets, *weights;       // (B, 5): mass, height, chest, waist, hips
+  float rho;                            // betas_weight
+  float *meas, *jac;                    // state (B, 5), (B, 5, NB)
+  const float *tmeas, *tjac;            // the trial's
+};
+
+template <bool MEAS>
+__global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, LmMeasArgs mb) {
+  extern __shared__ double A[];         // [P][P]: the lower triangle of J^T W J + lambda I, then its Cholesky factor
+  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
+  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
+  __shared__ double lt_s;
+  __shared__ int ok_s;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K;
+  const int o = 3 * a.n_rot;              // first betas column
+  const float *tg = a.targets + (size_t)b * R3, *wt = a.weights + (size_t)b * K;
+  const float lcur = a.loss[b];
+  // 1. trial loss
+  if (t == 0) {
+    const float *m = a.tkp + (size_t)b * R3;
+    double L = 0.0;
+    for (int k = 0; k < K; ++k) {
+      const double w = wt[k];
+      if (!(w > 0.0)) continue;
+      const double r0 = (double)m[3 * k] - (double)tg[3 * k], r1 = (double)m[3 * k + 1] - (double)tg[3 * k + 1],
+                   r2 = (double)m[3 * k + 2] - (double)tg[3 * k + 2];
+      L += w * (r0 * r0 + r1 * r1 + r2 * r2);
+    }
+    if constexpr (MEAS) {
+      const float *tm = mb.tmeas + (size_t)b * 5, *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+      double Lm = 0.0;
+      for (int k = 0; k < 5; ++k) {
+        const double w = mw[k];
+        if (w > 0.0) {                     // a dropped term is never read: its measurement may be NaN
+          const double r = (double)mt[k] - (double)tm[k];
+          Lm += w * r * r;
+        }
+      }
+      L += Lm;
+      if (mb.rho > 0.f) {
+        const float *tb = a.tbetas + (size_t)b * a.nb;
+        double reg = 0.0;
+        for (int l = 0; l < a.nb; ++l) reg += (double)tb[l] * (double)tb[l];
+        L += (double)mb.rho * reg;
+      }
+    }
+    lt_s = L;
+  }
+  __syncthreads();
+  // 2. accept or reject
+  const double lt = lt_s;
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
+  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
+  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
+  const float *Jm = MEAS ? (accept ? mb.tjac : mb.jac) + (size_t)b * 5 * a.nb : nullptr;   // the measurement block's
+  const float *Mm = MEAS ? (accept ? mb.tmeas : mb.meas) + (size_t)b * 5 : nullptr;
+  if (accept) {
+    lm_kp_take_trial(a, b, lnew);
+    if constexpr (MEAS) {
+      for (int i = t; i < 5; i += blockDim.x) mb.meas[(size_t)b * 5 + i] = mb.tmeas[(size_t)b * 5 + i];
+      for (int i = t; i < 5 * a.nb; i += blockDim.x) mb.jac[(size_t)b * 5 * a.nb + i] = mb.tjac[(size_t)b * 5 * a.nb + i];
+    }
+  }
+  // 3. normal equations: A_ij = sum_rows (w J_ri) J_rj (i >= j), g_i = sum_rows (w J_ri) (kp_r - target_r), rows in
+  // keypoint-major xyz order, the rows of a dropped keypoint never read
+  int pr[kLmKpPairs], pc[kLmKpPairs];
+  double acc[kLmKpPairs], g = 0.0;
+  lm_kp_pairs(P, pr, pc, acc);
+  for (int r0 = 0; r0 < R3; r0 += kLmKpRows) {
+    const int nr = min(kLmKpRows, R3 - r0);
+    __syncthreads();
+    for (int i = t; i < nr; i += blockDim.x) {
+      const double w = wt[(r0 + i) / 3];
+      ws[i] = w;
+      rs[i] = w > 0.0 ? (double)M[r0 + i] - (double)tg[r0 + i] : 0.0;
+    }
+    for (int i = t; i < nr * P; i += blockDim.x) {
+      const int row = i / P;
+      const double w = wt[(r0 + row) / 3];
+      if (w > 0.0) {
+        const double x = J[(size_t)(r0 + row) * P + i % P];
+        Js[row][i % P] = x;
+        WJs[row][i % P] = w * x;
+      }
+    }
+    __syncthreads();
+    lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
+  }
+  if constexpr (MEAS) {
+    // the five measurement rows, staged like the keypoint rows, into the betas block [o, o + nb) of A and g
+    const int nb = a.nb;
+    const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+    __syncthreads();
+    for (int i = t; i < 5; i += blockDim.x) {
+      const double w = mw[i];
+      ws[i] = w;
+      rs[i] = w > 0.0 ? (double)Mm[i] - (double)mt[i] : 0.0;
+    }
+    for (int i = t; i < 5 * nb; i += blockDim.x) {
+      const int row = i / nb;
+      const double w = mw[row];
+      if (w > 0.0) {                       // a dropped term's row is never read: it may be NaN
+        const double x = Jm[i];
+        Js[row][i % nb] = x;
+        WJs[row][i % nb] = w * x;
+      }
+    }
+    __syncthreads();
+    for (int row = 0; row < 5; ++row) {
+      if (!(ws[row] > 0.0)) continue;
+#pragma unroll
+      for (int i = 0; i < kLmKpPairs; ++i)
+        if (pc[i] >= o && pr[i] >= 0 && pr[i] < o + nb) acc[i] += WJs[row][pr[i] - o] * Js[row][pc[i] - o];
+      if (t >= o && t < o + nb) g += WJs[row][t - o] * rs[row];
+    }
+    if (mb.rho > 0.f && t >= o && t < o + nb)
+      g += (double)mb.rho * (double)(accept ? a.tbetas : a.betas)[(size_t)b * nb + t - o];
+  }
+  // the first lambda from all of diag(A); only the MEAS step has a betas regulariser to damp with
+  lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, A, P + 1, MEAS ? o : 0, MEAS ? o + a.nb : 0, mb.rho, ok_s);
+  lm_kp_solve(A, y, P, ok_s);
+  // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
+  lm_kp_next_trial(a, b, y, ok_s);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The step of the fit of pose, shape and weak-perspective camera to 2D keypoints (shapy_fit_lm_keypoints_2d_step).
+// The camera c = (c0, c1, c2) takes the columns of transl (which a weak-perspective camera cannot see along z, and
+// which duplicates c1, c2 in x and y).  With s = softplus(c0) (threshold 20, as the forward) the projection is
+// p_k = s (kp_k,xy + (c1, c2)), and per body, in fp64, left to right:
 //   L = sum_{w_k > 0} w_k rho(|p_k - x_k|^2)  (k order)
 //     + 1/2 pose_w sum_{j >= 1} |R_j - R0_j|_F^2  (j order, row-major entries; when pose_w > 0)
 //     + betas_w |beta|^2  (l order; when betas_w > 0)
@@ -516,16 +524,10 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
 //     j = 1 .. n_rot - 1, e in row-major order: they only reach the 3 x 3 diagonal block of joint j;
 //   then g += betas_w beta on the betas columns.
 // The first lambda is 1e-3 max(diag A, 1e-6) of the keypoint rows alone; the diagonal then gets betas_w + lambda on the
-// betas columns and lambda elsewhere.  The next trial is R_j Exp(delta_j), beta + delta_beta, c + delta_c.
-struct LmKp2dArgs {
-  int K, n_rot, nb, P;
-  const float *targets, *weights, *anchor;    // (B, K, 2), (B, K), (B, n_rot, 3, 3)
-  float sigma, pose_w, betas_w, up, down;
-  int first;
-  float *rot, *betas, *camera, *kp, *jac, *loss, *lambda;
-  int *accepted;
-  float *trot, *tbetas, *tcamera;
-  const float *tkp, *tjac;
+// betas columns and lambda elsewhere.
+struct LmKp2dArgs {                     // what the 2D step takes beside LmKpArgs (targets (B, K, 2), last = camera)
+  const float *anchor;                  // (B, n_rot, 3, 3), or null without a pose prior
+  float sigma, pose_w, betas_w;
 };
 
 // softplus(c0) and its derivative, with F.softplus' threshold of 20 (smplx.cu's projection)
@@ -549,7 +551,7 @@ __device__ __forceinline__ double rot_tangent(const float *R, int a, int e) {
   return ((q - a + 3) % 3 == 1) ? v : -v;      // -eps_{a m q} R_rm
 }
 
-__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKp2dArgs a) {
+__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, LmKp2dArgs x2) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
   __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP], dg[kLmKpMaxP];
@@ -558,13 +560,13 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKp2dArg
   const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nb = a.nb, nr9 = 9 * a.n_rot;
   const int o = 3 * a.n_rot, oc = o + nb;     // first betas and first camera column
   const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
-  const float *anc = a.anchor ? a.anchor + (size_t)b * nr9 : nullptr;
-  const bool robust = isfinite(a.sigma);
-  const double s2 = (double)a.sigma * (double)a.sigma;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
   const float lcur = a.loss[b];
   // 1. trial loss
   if (t == 0) {
-    const float *m = a.tkp + (size_t)b * R3, *cam = a.tcamera + (size_t)b * 3;
+    const float *m = a.tkp + (size_t)b * R3, *cam = a.tlast + (size_t)b * 3;
     double s, ds;
     softplus_d((double)cam[0], s, ds);
     const double cx = cam[1], cy = cam[2];
@@ -577,59 +579,41 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKp2dArg
       const double e = dx * dx + dy * dy;
       L += w * (robust ? e * (s2 / (s2 + e)) : e);
     }
-    if (a.pose_w > 0.f) {
+    if (x2.pose_w > 0.f) {
       const float *tr = a.trot + (size_t)b * nr9;
       double q = 0.0;
       for (int i = 9; i < nr9; ++i) {
         const double d = (double)tr[i] - (double)anc[i];
         q += d * d;
       }
-      L += 0.5 * (double)a.pose_w * q;
+      L += 0.5 * (double)x2.pose_w * q;
     }
-    if (a.betas_w > 0.f) {
+    if (x2.betas_w > 0.f) {
       const float *tb = a.tbetas + (size_t)b * nb;
       double reg = 0.0;
       for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
-      L += (double)a.betas_w * reg;
+      L += (double)x2.betas_w * reg;
     }
     lt_s = L;
   }
   __syncthreads();
-  // 2. accept or reject; on accept the trial's parameters, keypoints, Jacobian and loss become the state
+  // 2. accept or reject
   const double lt = lt_s;
-  const bool accept = a.first || (isfinite(lt) && lt < (double)lcur);
-  const float lnew = accept ? (isfinite(lt) ? (float)lt : __int_as_float(0x7fc00000)) : lcur;
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
   const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
   const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
   const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
   const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
-  const float *Cst = (accept ? a.tcamera : a.camera) + (size_t)b * 3;
-  if (accept) {
-    for (int i = t; i < nr9; i += blockDim.x) a.rot[(size_t)b * nr9 + i] = a.trot[(size_t)b * nr9 + i];
-    for (int i = t; i < nb; i += blockDim.x) a.betas[(size_t)b * nb + i] = a.tbetas[(size_t)b * nb + i];
-    if (t < 3) a.camera[(size_t)b * 3 + t] = a.tcamera[(size_t)b * 3 + t];
-    for (int i = t; i < R3; i += blockDim.x) a.kp[(size_t)b * R3 + i] = M[i];
-    for (size_t i = t; i < (size_t)R3 * P; i += blockDim.x) a.jac[(size_t)b * R3 * P + i] = J[i];
-    if (t == 0) a.loss[b] = lnew;
-  }
+  const float *Cst = (accept ? a.tlast : a.last) + (size_t)b * 3;
+  if (accept) lm_kp_take_trial(a, b, lnew);
   double s, ds;
   softplus_d((double)Cst[0], s, ds);
   const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
-  // 3. normal equations, thread t owning the lower-triangle entries t + kLmKpThreads i (row-major) and g_t
-  const int npairs = P * (P + 1) / 2;
+  // 3. normal equations
   int pr[kLmKpPairs], pc[kLmKpPairs];
-  double acc[kLmKpPairs];
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i) {
-    const int p = t + kLmKpThreads * i;
-    int r = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
-    while ((r + 1) * (r + 2) / 2 <= p) ++r;
-    while (r * (r + 1) / 2 > p) --r;
-    pr[i] = p < npairs ? r : -1;
-    pc[i] = p - r * (r + 1) / 2;
-    acc[i] = 0.0;
-  }
-  double g = 0.0;
+  double acc[kLmKpPairs], g = 0.0;
+  lm_kp_pairs(P, pr, pc, acc);
   const int R2 = 2 * K;
   for (int r0 = 0; r0 < R2; r0 += kLmKpRows) {
     const int nr = min(kLmKpRows, R2 - r0);
@@ -665,21 +649,14 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKp2dArg
       }
     }
     __syncthreads();
-    for (int row = 0; row < nr; ++row) {
-      const double w = ws[row];
-      if (!(w > 0.0)) continue;
-#pragma unroll
-      for (int i = 0; i < kLmKpPairs; ++i)
-        if (pr[i] >= 0) acc[i] += WJs[row][pr[i]] * Js[row][pc[i]];
-      if (t < P) g += WJs[row][t] * rs[row];
-    }
+    lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
   }
 #pragma unroll
   for (int i = 0; i < kLmKpPairs; ++i)
     if (pr[i] >= 0 && pr[i] == pc[i]) dg[pr[i]] = acc[i];     // the diagonal of the keypoint rows: the first lambda
-  if (a.pose_w > 0.f) {
+  if (x2.pose_w > 0.f) {
     // the pose-prior rows of joint j only reach its diagonal block: no staging
-    const double hw = 0.5 * (double)a.pose_w;
+    const double hw = 0.5 * (double)x2.pose_w;
 #pragma unroll
     for (int i = 0; i < kLmKpPairs; ++i) {
       const int j = pr[i] / 3;
@@ -693,55 +670,39 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKp2dArg
       for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
     }
   }
-  if (a.betas_w > 0.f && t >= o && t < oc) g += (double)a.betas_w * (double)Bst[t - o];
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i)
-    if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
-  if (t < P) y[t] = -g;
-  __syncthreads();
-  if (t == 0) {
-    float lam = a.first ? 0.f : a.lambda[b];
-    if (a.first) {
-      double dmax = kDiagFloor;
-      for (int j = 0; j < P; ++j) dmax = fmax(dmax, dg[j]);
-      lam = (float)(kLambdaInit * dmax);
-    } else if (accept) {
-      lam = lam / a.down;
-    } else {
-      lam = lam * a.up;
-    }
-    lam = fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
-    a.lambda[b] = lam;
-    if (accept && !a.first) a.accepted[b] += 1;
-    const double damp = (double)a.betas_w + (double)lam;
-    for (int j = 0; j < P; ++j) A[j * P + j] += j >= o && j < oc ? damp : (double)lam;
-    ok_s = isfinite(lnew);               // a body without a finite loss does not move
-  }
+  if (x2.betas_w > 0.f && t >= o && t < oc) g += (double)x2.betas_w * (double)Bst[t - o];
+  lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, dg, 1, o, oc, x2.betas_w, ok_s);
   // 4. Cholesky and the two triangular solves
   lm_kp_solve(A, y, P, ok_s);
   // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
-  const bool ok = ok_s;
-  lm_kp_next_rot(a.rot + (size_t)b * nr9, a.trot + (size_t)b * nr9, a.n_rot, y, ok);
-  for (int l = t; l < nb; l += blockDim.x) {
-    const float x = a.betas[(size_t)b * nb + l];
-    a.tbetas[(size_t)b * nb + l] = ok ? (float)((double)x + y[o + l]) : x;
-  }
-  if (t < 3) {
-    const float x = a.camera[(size_t)b * 3 + t];
-    a.tcamera[(size_t)b * 3 + t] = ok ? (float)((double)x + y[oc + t]) : x;
-  }
+  lm_kp_next_trial(a, b, y, ok_s);
 }
 
-// One CTA of kLmKpThreads per body with P x P doubles of dynamic shared memory; past 48 KB of static plus dynamic
-// shared memory the launch has to opt in
-template <typename... Args>
-int launch_lm_kp(void (*kernel)(Args...), int batch, int P, void *stream, Args... args) {
-  const size_t smem = (size_t)P * P * sizeof(double);
+// What the three keypoint entry points share, `fn` naming the one called: the checks of the arguments in `a` (its P is
+// set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors` its own scalars and the
+// sentence that states their and the lambda factors' ranges; then the launch, one CTA of kLmKpThreads per body with
+// P x P doubles of dynamic shared memory.  Past 48 KB of static plus dynamic shared memory the launch has to opt in
+template <typename Extra>
+int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
+              bool factors_ok, const char *factors, void *stream) {
+  SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
+                    a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && extra_ok,
+                "%s: null argument", fn);
+  SHAPY_REQUIRE(batch >= 0 && a.K >= 1 && a.n_rot >= 1 && a.n_rot <= 64 && a.nb >= 1,
+                "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas)", fn, batch, a.K, a.n_rot, a.nb);
+  SHAPY_REQUIRE(a.up >= 1.f && a.down >= 1.f && factors_ok, "%s: %s", fn, factors);
+  a.P = 3 * a.n_rot + a.nb + 3;
+  if (a.P > kLmKpMaxP) {
+    set_error("%s: %d parameters, at most %d are supported", fn, a.P, kLmKpMaxP);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  if (batch == 0) return SHAPY_OK;
+  const size_t smem = (size_t)a.P * a.P * sizeof(double);
   cudaFuncAttributes attr;
   SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, kernel));
   if (smem + attr.sharedSizeBytes > 48 * 1024)
     SHAPY_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(args...);
+  kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
@@ -776,23 +737,10 @@ extern "C" int shapy_fit_lm_keypoints_step(int batch, int num_keypoints, int n_r
                                            float *loss, float *lambda, int32_t *accepted, float *trial_rot,
                                            float *trial_betas, float *trial_transl, const float *trial_keypoints,
                                            const float *trial_jac, void *stream) {
-  SHAPY_REQUIRE(targets && weights && rot && betas && transl && keypoints && jac && loss && lambda && accepted &&
-                    trial_rot && trial_betas && trial_transl && trial_keypoints && trial_jac,
-                "shapy_fit_lm_keypoints_step: null argument");
-  SHAPY_REQUIRE(batch >= 0 && num_keypoints >= 1 && n_rot >= 1 && n_rot <= 64 && nb >= 1,
-                "shapy_fit_lm_keypoints_step: bad size (batch %d, %d keypoints, n_rot %d, %d betas)", batch,
-                num_keypoints, n_rot, nb);
-  SHAPY_REQUIRE(lambda_up >= 1.f && lambda_down >= 1.f,
-                "shapy_fit_lm_keypoints_step: lambda_up and lambda_down must be >= 1");
-  const int P = 3 * n_rot + nb + 3;
-  if (P > kLmKpMaxP) {
-    set_error("shapy_fit_lm_keypoints_step: %d parameters, at most %d are supported", P, kLmKpMaxP);
-    return SHAPY_ERR_UNSUPPORTED;
-  }
-  if (batch == 0) return SHAPY_OK;
-  LmKpArgs a{num_keypoints, n_rot, nb, P, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
-  return launch_lm_kp(lm_kp_step_kernel<false>, batch, P, stream, a, LmMeasArgs{});
+  return run_lm_kp("shapy_fit_lm_keypoints_step", lm_kp_step_kernel<false>, batch, a, LmMeasArgs{}, true, true,
+                   "lambda_up and lambda_down must be >= 1", stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_measurements_step(
@@ -802,26 +750,12 @@ extern "C" int shapy_fit_lm_keypoints_measurements_step(
     float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
     const float *trial_keypoints, const float *trial_jac, const float *trial_meas, const float *trial_meas_jac,
     void *stream) {
-  SHAPY_REQUIRE(targets && weights && meas_targets && meas_weights && rot && betas && transl && keypoints && jac &&
-                    meas && meas_jac && loss && lambda && accepted && trial_rot && trial_betas && trial_transl &&
-                    trial_keypoints && trial_jac && trial_meas && trial_meas_jac,
-                "shapy_fit_lm_keypoints_measurements_step: null argument");
-  SHAPY_REQUIRE(batch >= 0 && num_keypoints >= 1 && n_rot >= 1 && n_rot <= 64 && nb >= 1,
-                "shapy_fit_lm_keypoints_measurements_step: bad size (batch %d, %d keypoints, n_rot %d, %d betas)",
-                batch, num_keypoints, n_rot, nb);
-  SHAPY_REQUIRE(lambda_up >= 1.f && lambda_down >= 1.f && betas_weight >= 0.f,
-                "shapy_fit_lm_keypoints_measurements_step: lambda_up and lambda_down must be >= 1 and betas_weight "
-                ">= 0");
-  const int P = 3 * n_rot + nb + 3;
-  if (P > kLmKpMaxP) {
-    set_error("shapy_fit_lm_keypoints_measurements_step: %d parameters, at most %d are supported", P, kLmKpMaxP);
-    return SHAPY_ERR_UNSUPPORTED;
-  }
-  if (batch == 0) return SHAPY_OK;
-  LmKpArgs a{num_keypoints, n_rot, nb, P, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
   LmMeasArgs m{meas_targets, meas_weights, betas_weight, meas, meas_jac, trial_meas, trial_meas_jac};
-  return launch_lm_kp(lm_kp_step_kernel<true>, batch, P, stream, a, m);
+  return run_lm_kp("shapy_fit_lm_keypoints_measurements_step", lm_kp_step_kernel<true>, batch, a, m,
+                   meas_targets && meas_weights && meas && meas_jac && trial_meas && trial_meas_jac,
+                   betas_weight >= 0.f, "lambda_up and lambda_down must be >= 1 and betas_weight >= 0", stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int n_rot, int nb, const float *targets,
@@ -832,25 +766,13 @@ extern "C" int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int 
                                               int32_t *accepted, float *trial_rot, float *trial_betas,
                                               float *trial_camera, const float *trial_keypoints, const float *trial_jac,
                                               void *stream) {
-  SHAPY_REQUIRE(targets && weights && rot && betas && camera && keypoints && jac && loss && lambda && accepted &&
-                    trial_rot && trial_betas && trial_camera && trial_keypoints && trial_jac &&
-                    (pose_anchor || !(pose_prior_weight > 0.f)),
-                "shapy_fit_lm_keypoints_2d_step: null argument");
-  SHAPY_REQUIRE(batch >= 0 && num_keypoints >= 1 && n_rot >= 1 && n_rot <= 64 && nb >= 1,
-                "shapy_fit_lm_keypoints_2d_step: bad size (batch %d, %d keypoints, n_rot %d, %d betas)", batch,
-                num_keypoints, n_rot, nb);
-  SHAPY_REQUIRE(robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f && lambda_up >= 1.f &&
-                    lambda_down >= 1.f,
-                "shapy_fit_lm_keypoints_2d_step: robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 "
-                "and lambda_up and lambda_down >= 1");
-  const int P = 3 * n_rot + nb + 3;
-  if (P > kLmKpMaxP) {
-    set_error("shapy_fit_lm_keypoints_2d_step: %d parameters, at most %d are supported", P, kLmKpMaxP);
-    return SHAPY_ERR_UNSUPPORTED;
-  }
-  if (batch == 0) return SHAPY_OK;
-  LmKp2dArgs a{num_keypoints, n_rot, nb, P, targets, weights, pose_anchor, robust_sigma, pose_prior_weight,
-               betas_weight, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera, keypoints, jac, loss, lambda,
-               accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
-  return launch_lm_kp(lm_kp2d_step_kernel, batch, P, stream, a);
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight};
+  return run_lm_kp("shapy_fit_lm_keypoints_2d_step", lm_kp2d_step_kernel, batch, a, x,
+                   pose_anchor || !(pose_prior_weight > 0.f),
+                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
+                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                   "lambda_down >= 1",
+                   stream);
 }

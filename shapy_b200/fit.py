@@ -110,6 +110,21 @@ def _measurement_loss(tgt, wt, meas, betas, betas_weight):
     return (wt * diff.pow(2)).sum(1) + betas_weight * betas.pow(2).sum(1)
 
 
+def _adam(params, lr, iterations, loss_fn):
+    """Adam on the tensors `params` over the batch sum of loss_fn()[0], the per-body loss; returns loss_fn() at the
+    result, without a graph."""
+    opt = torch.optim.Adam(params, lr=lr)
+    # the step size decays geometrically to lr / 100 over the run, so the last iterations refine instead of orbiting
+    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
+    for _ in range(int(iterations)):
+        opt.zero_grad(set_to_none=True)
+        loss_fn()[0].sum().backward()
+        opt.step()
+        sched.step()
+    with torch.no_grad():
+        return loss_fn()
+
+
 def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
                               lr=0.05, betas_init=None, batch_size=None, method='adam',
                               circumference_derivative='reference'):
@@ -139,24 +154,14 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     nb = body_model.shapedirs.shape[-1]
     betas = (torch.zeros(B, nb, device=device) if betas_init is None else betas_init.detach().clone().float())
     betas.requires_grad_(True)
-    opt = torch.optim.Adam([betas], lr=lr)
-    # the step size decays geometrically to lr / 100 over the run, so the last iterations refine instead of orbiting
-    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
 
-    def loss_fn(b):
-        v = body_model.forward_shape(betas=b)['v_shaped']
+    def loss_fn():
+        v = body_model.forward_shape(betas=betas)['v_shaped']
         m = body_measurements.forward_vertices(v, faces, circumference_derivative)['measurements']
         meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-        return _measurement_loss(tgt, wt, meas, b, betas_weight), meas
+        return _measurement_loss(tgt, wt, meas, betas, betas_weight), meas
 
-    for _ in range(int(iterations)):
-        opt.zero_grad(set_to_none=True)
-        per_body, _ = loss_fn(betas)
-        per_body.sum().backward()
-        opt.step()
-        sched.step()
-    with torch.no_grad():
-        per_body, meas = loss_fn(betas)
+    per_body, meas = _adam([betas], lr, iterations, loss_fn)
     return {'betas': betas.detach(), 'measurements': meas, 'loss': per_body}
 
 
@@ -205,6 +210,24 @@ def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, be
 
 
 IDENT6 = (1.0, 0.0, 0.0, 1.0, 0.0, 0.0)      # the 6D code of the identity rotation (row-major 3x2)
+
+
+def _start_params(init, B, nb, device, method, last, last0=0.0):
+    """The raw 6D global and body pose, betas and last three parameters (named `last`: 'transl' or 'camera') a keypoint
+    fit starts from: init's entries, and for a missing one the identity pose, zero betas and (last0, 0, 0)."""
+    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
+    ident[0::3].fill_(1.0)
+    last3 = torch.zeros(B, 3, device=device)
+    if last0:
+        last3[:, 0].fill_(last0)
+    start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
+             'betas': torch.zeros(B, nb, device=device), last: last3}
+    params = {}
+    for k, v in start.items():
+        t = init.get(k)
+        t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
+        params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    return params
 
 
 def keypoint_jacobian(body_model, rot, betas, transl=None):
@@ -265,20 +288,9 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     if measurements is not None:
         tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
         mterms = (tgt.contiguous(), wt.contiguous(), float(betas_weight), circumference_derivative)
-    init = init or {}
-    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
-    ident[0::3].fill_(1.0)
-    start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
-             'betas': torch.zeros(B, body_model.num_betas, device=device), 'transl': torch.zeros(B, 3, device=device)}
-    params = {}
-    for k, v in start.items():
-        t = init.get(k)
-        t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
-        params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    params = _start_params(init or {}, B, body_model.num_betas, device, method, 'transl')
     if method == 'lm':
         return _fit_keypoints_lm(body_model, kp, w, params, int(iterations), body_measurements, mterms)
-    opt = torch.optim.Adam(list(params.values()), lr=lr)
-    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -295,19 +307,28 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
             per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], mterms[2])
         return per_body, joints, grot, bpose, meas
 
-    for _ in range(int(iterations)):
-        opt.zero_grad(set_to_none=True)
-        per_body = loss_fn()[0]
-        per_body.sum().backward()
-        opt.step()
-        sched.step()
-    with torch.no_grad():
-        per_body, joints, grot, bpose, meas = loss_fn()
+    per_body, joints, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, loss=per_body)
     if meas is not None:
         res['measurements'] = meas
     return res
+
+
+def _kp_lm_state(B, K, n_rot, nb, last, device):
+    """The state tensors of a keypoint LM step (ops.fit_lm_keypoints_step), `last` naming the last three parameters."""
+    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+    return {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), last: mk(B, 3), 'keypoints': mk(B, K, 3),
+            'jac': mk(B, 3 * K, 3 * n_rot + nb + 3), 'loss': mk(B), 'lambda': mk(B),
+            'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+
+
+def _kp_lm_result(state, last, **outputs):
+    """The fitted parameters of a keypoint LM state as the fits return them, the rotations also as raw 6D."""
+    rot = state['rot']
+    raw = rot[..., :2].reshape(rot.shape[0], 6 * rot.shape[1])   # the first two columns, the decoder's row-major 3x2
+    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
+            last: state[last], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], **outputs}
 
 
 def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=None, mterms=None):
@@ -316,16 +337,13 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=N
     packed = body_model.packed(device)
     B, K = kp.shape[0], kp.shape[1]
     n_rot, nb = 22, params['betas'].shape[1]
-    P = 3 * n_rot + nb + 3
     trial = {'rot': ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1)).contiguous(),
              'betas': params['betas'].contiguous(), 'transl': params['transl'].contiguous()}
-    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-    state = {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), 'transl': mk(B, 3), 'keypoints': mk(B, K, 3),
-             'jac': mk(B, 3 * K, P), 'loss': mk(B), 'lambda': mk(B),
-             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    state = _kp_lm_state(B, K, n_rot, nb, 'transl', device)
     tg = kp.contiguous()
     if mterms is not None:
-        state.update(meas=mk(B, 5), meas_jac=mk(B, 5, nb))
+        state.update(meas=torch.empty(B, 5, dtype=torch.float32, device=device),
+                     meas_jac=torch.empty(B, 5, nb, dtype=torch.float32, device=device))
     if B > 0 and mterms is None:
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
@@ -349,10 +367,7 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=N
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
         if mterms is not None:
             per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], mterms[2])
-    raw = rot[..., :2].reshape(B, n_rot * 6)       # the first two columns in the decoder's row-major 3x2 layout
-    res = {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
-           'transl': state['transl'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], 'keypoints': joints,
-           'loss': per_body}
+    res = _kp_lm_result(state, 'transl', keypoints=joints, loss=per_body)
     if mterms is not None:
         res['measurements'] = state['meas']
     return res
@@ -406,18 +421,7 @@ def _init_2d(init, B, nb, device, method):
     for k in ('global_rot', 'body_pose'):
         if init.get('raw_' + k) is not None:
             init[k] = init['raw_' + k]
-    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device: no host-to-device copy
-    ident[0::3].fill_(1.0)
-    cam = torch.zeros(B, 3, device=device)     # scale softplus(0.9) ~ 1.24, the regressor's mean scale
-    cam[:, 0].fill_(0.9)
-    start = {'global_rot': ident.repeat(B, 1), 'body_pose': ident.repeat(B, 21),
-             'betas': torch.zeros(B, nb, device=device), 'camera': cam}
-    params = {}
-    for k, v in start.items():
-        t = init.get(k)
-        t = v if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(v.shape)
-        params[k] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
-    return params
+    return _start_params(init, B, nb, device, method, 'camera', 0.9)   # softplus(0.9) ~ 1.24, the regressor's mean scale
 
 
 def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
@@ -468,8 +472,6 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     pw, bw = float(pose_prior_weight), float(betas_weight)
     if method == 'lm':
         return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw)
-    opt = torch.optim.Adam(list(params.values()), lr=lr)
-    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda i: 0.01 ** (i / max(1, int(iterations))))
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -480,13 +482,7 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
         return per_body, out, grot, bpose
 
-    for _ in range(int(iterations)):
-        opt.zero_grad(set_to_none=True)
-        loss_fn()[0].sum().backward()
-        opt.step()
-        sched.step()
-    with torch.no_grad():
-        per_body, out, grot, bpose = loss_fn()
+    per_body, out, grot, bpose = _adam(list(params.values()), lr, iterations, loss_fn)
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
                loss=per_body)
@@ -498,13 +494,8 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
     device = x.device
     packed = body_model.packed(device)
     B, K = x.shape[0], x.shape[1]
-    n_rot, nb = 22, params['betas'].shape[1]
-    P = 3 * n_rot + nb + 3
     trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'camera': params['camera'].contiguous()}
-    mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-    state = {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), 'camera': mk(B, 3), 'keypoints': mk(B, K, 3),
-             'jac': mk(B, 3 * K, P), 'loss': mk(B), 'lambda': mk(B),
-             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    state = _kp_lm_state(B, K, 22, params['betas'].shape[1], 'camera', device)
     if B > 0:
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
@@ -515,10 +506,7 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
         out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
                          return_shaped=False)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
-    raw = rot[..., :2].reshape(B, n_rot * 6)       # the first two columns in the decoder's row-major 3x2 layout
-    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
-            'camera': state['camera'], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:],
-            'keypoints': out['joints'][:], 'proj_joints': out['proj_joints'], 'loss': per_body}
+    return _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
 
 
 def main(argv=None):

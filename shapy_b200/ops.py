@@ -376,6 +376,24 @@ def measure_jacobian_betas(model: SmplxModel, landmarks: _lib.MeasureLandmarks, 
     return out, jac, status
 
 
+def _check_step_tensors(what, f32, f32_names, accepted):
+    """What every LM step wrapper requires of its tensors: `f32` (named by f32_names in the message) and the counter
+    `accepted` contiguous on the device, float32 and int32."""
+    for t in f32 + [accepted]:
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
+            raise RuntimeError(f'{what}: every tensor must be a contiguous CUDA tensor')
+    for t in f32:
+        if t.dtype != torch.float32:
+            raise RuntimeError(f'{what}: {f32_names} must be float32')
+    if accepted.dtype != torch.int32:
+        raise RuntimeError(f'{what}: accepted must be int32')
+
+
+def _kp_step_shapes_ok(state, trial_jac, weights, B, K, P):
+    """Whether both Jacobians and the weights of a keypoint step have the shapes its sizes give."""
+    return trial_jac.shape == (B, 3 * K, P) and state['jac'].shape == (B, 3 * K, P) and weights.shape == (B, K)
+
+
 def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, first, trial, trial_meas, trial_jac):
     """One Levenberg-Marquardt step per body (include/shapy_b200.h, shapy_fit_lm_step), in place.  state: {'betas'
     (B, NB), 'meas' (B, 5), 'jac' (B, 5, NB), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32}, CUDA tensors;
@@ -383,14 +401,7 @@ def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, f
     B, nb = trial.shape
     ts = [state[k] for k in ('betas', 'meas', 'jac', 'loss', 'lambda')] + [targets, weights, trial, trial_meas,
                                                                            trial_jac]
-    for t in ts + [state['accepted']]:
-        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
-            raise RuntimeError('fit_lm_step: every tensor must be a contiguous CUDA tensor')
-    for t in ts:
-        if t.dtype != torch.float32:
-            raise RuntimeError('fit_lm_step: the state, targets, weights and trial must be float32')
-    if state['accepted'].dtype != torch.int32:
-        raise RuntimeError('fit_lm_step: accepted must be int32')
+    _check_step_tensors('fit_lm_step', ts, 'the state, targets, weights and trial', state['accepted'])
     if B == 0:
         return
     with torch.cuda.device(trial.device):
@@ -434,16 +445,9 @@ def fit_lm_keypoints_step(state, trial, targets, weights, lambda_up, lambda_down
     nb, K = trial['betas'].shape[1], targets.shape[1]
     ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + \
         [trial[k] for k in ('rot', 'betas', 'transl')] + [targets, weights, trial_keypoints, trial_jac]
-    for t in ts + [state['accepted']]:
-        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
-            raise RuntimeError('fit_lm_keypoints_step: every tensor must be a contiguous CUDA tensor')
-    for t in ts:
-        if t.dtype != torch.float32:
-            raise RuntimeError('fit_lm_keypoints_step: the state, trial, targets and weights must be float32')
-    if state['accepted'].dtype != torch.int32:
-        raise RuntimeError('fit_lm_keypoints_step: accepted must be int32')
+    _check_step_tensors('fit_lm_keypoints_step', ts, 'the state, trial, targets and weights', state['accepted'])
     P = 3 * n_rot + nb + 3
-    if trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K):
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P):
         raise RuntimeError(f'fit_lm_keypoints_step: jac must be ({B}, {3 * K}, {P}) and weights ({B}, {K})')
     if B == 0:
         return
@@ -468,16 +472,9 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
         [trial[k] for k in ('rot', 'betas', 'transl')] + [targets, weights, meas_targets, meas_weights,
                                                           trial_keypoints, trial_jac, trial_meas, trial_meas_jac]
     what = 'fit_lm_keypoints_measurements_step'
-    for t in ts + [state['accepted']]:
-        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
-            raise RuntimeError(f'{what}: every tensor must be a contiguous CUDA tensor')
-    for t in ts:
-        if t.dtype != torch.float32:
-            raise RuntimeError(f'{what}: the state, trial, targets and weights must be float32')
-    if state['accepted'].dtype != torch.int32:
-        raise RuntimeError(f'{what}: accepted must be int32')
+    _check_step_tensors(what, ts, 'the state, trial, targets and weights', state['accepted'])
     P = 3 * n_rot + nb + 3
-    if trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K):
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}) and weights ({B}, {K})')
     if (trial_meas_jac.shape != (B, 5, nb) or state['meas_jac'].shape != (B, 5, nb) or
             any(t.shape != (B, 5) for t in (meas_targets, meas_weights, trial_meas, state['meas']))):
@@ -514,17 +511,9 @@ def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_
     anchor = [] if pose_anchor is None else [pose_anchor]
     ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + \
         [trial[k] for k in ('rot', 'betas', 'camera')] + [targets, weights, trial_keypoints, trial_jac] + anchor
-    for t in ts + [state['accepted']]:
-        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous()):
-            raise RuntimeError(f'{what}: every tensor must be a contiguous CUDA tensor')
-    for t in ts:
-        if t.dtype != torch.float32:
-            raise RuntimeError(f'{what}: the state, trial, targets, weights and anchor must be float32')
-    if state['accepted'].dtype != torch.int32:
-        raise RuntimeError(f'{what}: accepted must be int32')
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights and anchor', state['accepted'])
     P = 3 * n_rot + nb + 3
-    if (trial_jac.shape != (B, 3 * K, P) or state['jac'].shape != (B, 3 * K, P) or weights.shape != (B, K)
-            or targets.shape != (B, K, 2)):
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
     if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
