@@ -302,6 +302,31 @@ int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int n_rot, int 
                                    float *trial_camera, const float *trial_keypoints, const float *trial_jac,
                                    void *stream);
 
+/* shapy_fit_lm_keypoints_2d_step with the five virtual measurements stacked under its rows, as
+ * shapy_fit_lm_keypoints_measurements_step is to shapy_fit_lm_keypoints_step: one Gauss-Newton step on, in fp64, left
+ * to right, L = sum_{w_k > 0} w_k rho(|p_k - x_k|^2) + pose_prior_weight / 2 sum_j |R_j - R0_j|_F^2 +
+ * sum_{u_m > 0} u_m (t_m - meas_m)^2 (m order: mass, height, chest, waist, hips; summed on its own, then added) +
+ * betas_weight |beta|^2 (the 2D step's betas prior: one regulariser).  2D keypoints fix the proportions of a body and
+ * not its metric size (a larger body under a smaller softplus(c0) projects to the same points); a known height or mass
+ * removes that freedom.  meas_targets, meas_weights (B,5); the state adds meas (B,5) and meas_jac (B,5,nb), the trial
+ * trial_meas / trial_meas_jac (shapy_measure_jacobian_betas or _exact at the trial betas); on accept they are copied
+ * into the state too.  A measurement with weight <= 0 is dropped (its value and Jacobian row are never read and may be
+ * NaN); a weighted NaN trial measurement makes the trial loss NaN, so the trial is rejected.  Normal equations: the 2D
+ * step's keypoint rows (IRLS weights at the state), then its pose-prior rows, then J_m^T U J_m into the betas block and
+ * J_m^T U (meas - t) into g in m order (plain least squares: rho applies to keypoints only), then betas_weight beta.
+ * The first lambda is 1e-3 max(diag, 1e-6) of the keypoint rows alone, as in the 2D step; policy, damping, solve and
+ * next trial are the 2D step's.  With every measurement weight <= 0 every output equals
+ * shapy_fit_lm_keypoints_2d_step's bit for bit, for any robust_sigma, pose prior and betas_weight.  Errors as
+ * shapy_fit_lm_keypoints_2d_step, the measurement pointers included.  batch 0: no launch.  Deterministic, no atomics,
+ * per-body independent. */
+int shapy_fit_lm_keypoints_2d_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_camera, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

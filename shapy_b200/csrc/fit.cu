@@ -387,6 +387,62 @@ struct LmMeasArgs {                     // the measurement block of the MEAS ste
   const float *tmeas, *tjac;            // the trial's
 };
 
+// The measurement block's three pieces, shared by the 3D and the 2D MEAS kernels.  Phase 1, by thread 0: the trial's
+// sum_{w_k > 0} w_k (t_k - m_k)^2 in k order, summed on its own; a dropped term is never read: its measurement may be NaN
+__device__ __forceinline__ double lm_meas_loss(const LmMeasArgs &mb, int b) {
+  const float *tm = mb.tmeas + (size_t)b * 5, *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+  double Lm = 0.0;
+  for (int k = 0; k < 5; ++k) {
+    const double w = mw[k];
+    if (w > 0.0) {
+      const double r = (double)mt[k] - (double)tm[k];
+      Lm += w * r * r;
+    }
+  }
+  return Lm;
+}
+
+// Phase 2 on accept: the trial's measurements and their Jacobian become the state's
+__device__ __forceinline__ void lm_meas_take_trial(const LmMeasArgs &mb, int b, int nb) {
+  const int t = threadIdx.x;
+  for (int i = t; i < 5; i += blockDim.x) mb.meas[(size_t)b * 5 + i] = mb.tmeas[(size_t)b * 5 + i];
+  for (int i = t; i < 5 * nb; i += blockDim.x) mb.jac[(size_t)b * 5 * nb + i] = mb.tjac[(size_t)b * 5 * nb + i];
+}
+
+// Phase 3: the five measurement rows (values Mm (5), Jacobian Jm (5, nb), at the state), staged like the keypoint rows,
+// into the betas block [o, o + nb) of A and g in k order, residual m_k - t_k; a dropped term's row is never read: it
+// may be NaN
+__device__ __forceinline__ void lm_meas_add_rows(const LmMeasArgs &mb, int b, int nb, int o, const float *Mm,
+                                                 const float *Jm, double (*Js)[kLmKpMaxP], double (*WJs)[kLmKpMaxP],
+                                                 double *ws, double *rs, const int (&pr)[kLmKpPairs],
+                                                 const int (&pc)[kLmKpPairs], double (&acc)[kLmKpPairs], double &g) {
+  const int t = threadIdx.x;
+  const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+  __syncthreads();
+  for (int i = t; i < 5; i += blockDim.x) {
+    const double w = mw[i];
+    ws[i] = w;
+    rs[i] = w > 0.0 ? (double)Mm[i] - (double)mt[i] : 0.0;
+  }
+  for (int i = t; i < 5 * nb; i += blockDim.x) {
+    const int row = i / nb;
+    const double w = mw[row];
+    if (w > 0.0) {
+      const double x = Jm[i];
+      Js[row][i % nb] = x;
+      WJs[row][i % nb] = w * x;
+    }
+  }
+  __syncthreads();
+  for (int row = 0; row < 5; ++row) {
+    if (!(ws[row] > 0.0)) continue;
+#pragma unroll
+    for (int i = 0; i < kLmKpPairs; ++i)
+      if (pc[i] >= o && pr[i] >= 0 && pr[i] < o + nb) acc[i] += WJs[row][pr[i] - o] * Js[row][pc[i] - o];
+    if (t >= o && t < o + nb) g += WJs[row][t - o] * rs[row];
+  }
+}
+
 template <bool MEAS>
 __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, LmMeasArgs mb) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of J^T W J + lambda I, then its Cholesky factor
@@ -410,16 +466,7 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
       L += w * (r0 * r0 + r1 * r1 + r2 * r2);
     }
     if constexpr (MEAS) {
-      const float *tm = mb.tmeas + (size_t)b * 5, *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
-      double Lm = 0.0;
-      for (int k = 0; k < 5; ++k) {
-        const double w = mw[k];
-        if (w > 0.0) {                     // a dropped term is never read: its measurement may be NaN
-          const double r = (double)mt[k] - (double)tm[k];
-          Lm += w * r * r;
-        }
-      }
-      L += Lm;
+      L += lm_meas_loss(mb, b);
       if (mb.rho > 0.f) {
         const float *tb = a.tbetas + (size_t)b * a.nb;
         double reg = 0.0;
@@ -440,10 +487,7 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
   const float *Mm = MEAS ? (accept ? mb.tmeas : mb.meas) + (size_t)b * 5 : nullptr;
   if (accept) {
     lm_kp_take_trial(a, b, lnew);
-    if constexpr (MEAS) {
-      for (int i = t; i < 5; i += blockDim.x) mb.meas[(size_t)b * 5 + i] = mb.tmeas[(size_t)b * 5 + i];
-      for (int i = t; i < 5 * a.nb; i += blockDim.x) mb.jac[(size_t)b * 5 * a.nb + i] = mb.tjac[(size_t)b * 5 * a.nb + i];
-    }
+    if constexpr (MEAS) lm_meas_take_trial(mb, b, a.nb);
   }
   // 3. normal equations: A_ij = sum_rows (w J_ri) J_rj (i >= j), g_i = sum_rows (w J_ri) (kp_r - target_r), rows in
   // keypoint-major xyz order, the rows of a dropped keypoint never read
@@ -471,32 +515,9 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
     lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
   }
   if constexpr (MEAS) {
-    // the five measurement rows, staged like the keypoint rows, into the betas block [o, o + nb) of A and g
+    // the five measurement rows into the betas block [o, o + nb) of A and g
     const int nb = a.nb;
-    const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
-    __syncthreads();
-    for (int i = t; i < 5; i += blockDim.x) {
-      const double w = mw[i];
-      ws[i] = w;
-      rs[i] = w > 0.0 ? (double)Mm[i] - (double)mt[i] : 0.0;
-    }
-    for (int i = t; i < 5 * nb; i += blockDim.x) {
-      const int row = i / nb;
-      const double w = mw[row];
-      if (w > 0.0) {                       // a dropped term's row is never read: it may be NaN
-        const double x = Jm[i];
-        Js[row][i % nb] = x;
-        WJs[row][i % nb] = w * x;
-      }
-    }
-    __syncthreads();
-    for (int row = 0; row < 5; ++row) {
-      if (!(ws[row] > 0.0)) continue;
-#pragma unroll
-      for (int i = 0; i < kLmKpPairs; ++i)
-        if (pc[i] >= o && pr[i] >= 0 && pr[i] < o + nb) acc[i] += WJs[row][pr[i] - o] * Js[row][pc[i] - o];
-      if (t >= o && t < o + nb) g += WJs[row][t - o] * rs[row];
-    }
+    lm_meas_add_rows(mb, b, nb, o, Mm, Jm, Js, WJs, ws, rs, pr, pc, acc, g);
     if (mb.rho > 0.f && t >= o && t < o + nb)
       g += (double)mb.rho * (double)(accept ? a.tbetas : a.betas)[(size_t)b * nb + t - o];
   }
@@ -525,10 +546,18 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
 //   then g += betas_w beta on the betas columns.
 // The first lambda is 1e-3 max(diag A, 1e-6) of the keypoint rows alone; the diagonal then gets betas_w + lambda on the
 // betas columns and lambda elsewhere.
+//
+// MEAS (shapy_fit_lm_keypoints_2d_measurements_step) stacks the five virtual measurements under those rows, as the 3D
+// MEAS step does: L gains sum_{u_m > 0} u_m (t_m - meas_m)^2 (m order, summed on its own) between the pose prior and
+// the betas prior, and the measurement rows (plain least squares: rho applies to keypoints only) go into the betas
+// block of A and g after the pose-prior rows and before betas_w beta.  They do not count for the first lambda.  With
+// every measurement weight <= 0 the loss gains an exact 0 and no row is added, so the step equals the 2D step bit for
+// bit, for any sigma, pose prior and betas_w.
 struct LmKp2dArgs {                     // what the 2D step takes beside LmKpArgs (targets (B, K, 2), last = camera)
   const float *anchor;                  // (B, n_rot, 3, 3), or null without a pose prior
   float sigma, pose_w, betas_w;
-};
+  LmMeasArgs mb;                        // the MEAS step's block (unused otherwise); its rho is not read: betas_w is the
+};                                      // one betas regulariser
 
 // softplus(c0) and its derivative, with F.softplus' threshold of 20 (smplx.cu's projection)
 __device__ __forceinline__ void softplus_d(double c0, double &s, double &ds) {
@@ -551,6 +580,7 @@ __device__ __forceinline__ double rot_tangent(const float *R, int a, int e) {
   return ((q - a + 3) % 3 == 1) ? v : -v;      // -eps_{a m q} R_rm
 }
 
+template <bool MEAS>
 __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, LmKp2dArgs x2) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
@@ -588,6 +618,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
       }
       L += 0.5 * (double)x2.pose_w * q;
     }
+    if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
     if (x2.betas_w > 0.f) {
       const float *tb = a.tbetas + (size_t)b * nb;
       double reg = 0.0;
@@ -606,7 +637,10 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
   const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
   const float *Cst = (accept ? a.tlast : a.last) + (size_t)b * 3;
-  if (accept) lm_kp_take_trial(a, b, lnew);
+  if (accept) {
+    lm_kp_take_trial(a, b, lnew);
+    if constexpr (MEAS) lm_meas_take_trial(x2.mb, b, nb);
+  }
   double s, ds;
   softplus_d((double)Cst[0], s, ds);
   const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
@@ -670,6 +704,9 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
       for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
     }
   }
+  if constexpr (MEAS)
+    lm_meas_add_rows(x2.mb, b, nb, o, (accept ? x2.mb.tmeas : x2.mb.meas) + (size_t)b * 5,
+                     (accept ? x2.mb.tjac : x2.mb.jac) + (size_t)b * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, g);
   if (x2.betas_w > 0.f && t >= o && t < oc) g += (double)x2.betas_w * (double)Bst[t - o];
   lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, dg, 1, o, oc, x2.betas_w, ok_s);
   // 4. Cholesky and the two triangular solves
@@ -678,7 +715,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   lm_kp_next_trial(a, b, y, ok_s);
 }
 
-// What the three keypoint entry points share, `fn` naming the one called: the checks of the arguments in `a` (its P is
+// What the four keypoint entry points share, `fn` naming the one called: the checks of the arguments in `a` (its P is
 // set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors` its own scalars and the
 // sentence that states their and the lambda factors' ranges; then the launch, one CTA of kLmKpThreads per body with
 // P x P doubles of dynamic shared memory.  Past 48 KB of static plus dynamic shared memory the launch has to opt in
@@ -768,9 +805,29 @@ extern "C" int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int 
                                               void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
-  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight};
-  return run_lm_kp("shapy_fit_lm_keypoints_2d_step", lm_kp2d_step_kernel, batch, a, x,
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
+  return run_lm_kp("shapy_fit_lm_keypoints_2d_step", lm_kp2d_step_kernel<false>, batch, a, x,
                    pose_anchor || !(pose_prior_weight > 0.f),
+                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
+                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                   "lambda_down >= 1",
+                   stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_camera, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
+               LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
+  return run_lm_kp("shapy_fit_lm_keypoints_2d_measurements_step", lm_kp2d_step_kernel<true>, batch, a, x,
+                   (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas && meas_jac &&
+                       trial_meas && trial_meas_jac,
                    robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
                    "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                    "lambda_down >= 1",

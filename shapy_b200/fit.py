@@ -62,7 +62,18 @@ ops.fit_lm_keypoints_2d_step (the 3D step's policy, the projected rows with IRLS
 launches, no host synchronisation, every body's loss non-increasing; keypoint_jacobian_2d exposes the projected
 Jacobian.
 
+fit_body_to_keypoints_2d(..., body_measurements=bm, measurements={'height': h, 'mass': m, ...}) adds the measurement
+loss of fit_body_to_keypoints (same targets, weights and dropping rule, T-pose of the fitted betas) to the 2D loss.
+Under the weak-perspective camera a larger body seen by a smaller scale projects to the same points, so 2D keypoints
+fix a body's proportions and not its metric size: a known height removes that freedom, a known mass pins the soft
+tissue no joint sees.  With method='lm' each iteration is four launches (the keypoint Jacobian, forward_shape and the
+measurement Jacobian of the trial, then ops.fit_lm_keypoints_2d_measurements_step), none synchronising.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
+    python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
+
+With --keypoints-2d, known measurements are read from --targets only (per-body arrays height / mass / ...); --height
+and the other single-target flags are not used there, so a command line without --targets fits the keypoints alone.
 
 shapy_b200.keypoints2d reads OpenPose detections and maps them into that frame; with raw detections and their crop
 descriptors in kp.npz, --keypoint-map openpose_smplx_map.json does the same on the command line.
@@ -425,7 +436,9 @@ def _init_2d(init, B, nb, device, method):
 
 
 def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
-                             robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05):
+                             robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
+                             body_measurements=None, measurements=None, measurement_weights=None,
+                             circumference_derivative='reference'):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -440,10 +453,20 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     SMPLX.forward(camera=...) and the 6D decoder) or 'lm' (batched Levenberg-Marquardt: the raw 6D start is decoded
     once, then per iteration the keypoint Jacobian of the trial and one ops.fit_lm_keypoints_2d_step, two launches,
     no host synchronisation; every body's loss is non-increasing).  iterations: None means 600 for Adam and 50 for LM.
+    measurements: optional known measurements of the bodies, fitted together with the keypoints, with the vocabulary
+    of fit_body_to_keypoints: the targets dict of fit_betas_to_measurements, measurement_weights over DEFAULT_WEIGHTS,
+    the same dropping rule, measured by body_measurements (required with them) on the T-pose of the fitted betas, and
+    circumference_derivative 'reference' or 'exact'.  The loss gains sum_m u_m (t_m - meas_m)^2; betas_weight stays the
+    one betas regulariser.  With 'lm' an iteration then takes four launches (see the top).
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'camera', 'global_rot_mat' (B, 1, 3, 3), 'body_pose_mat'
-    (B, 21, 3, 3), 'keypoints' (B, K, 3) and 'proj_joints' (B, K, 2) of the final parameters, 'loss' (B,)}."""
+    (B, 21, 3, 3), 'keypoints' (B, K, 3) and 'proj_joints' (B, K, 2) of the final parameters, 'loss' (B,)}, with
+    measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss' the
+    total."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    exact_circumferences(circumference_derivative)
+    if measurements is not None and body_measurements is None:
+        raise ValueError('fit_body_to_keypoints_2d: measurements need body_measurements')
     if robust_sigma is not None and not robust_sigma > 0:
         raise ValueError(f'fit_body_to_keypoints_2d: robust_sigma must be > 0 or None, got {robust_sigma}')
     if not (pose_prior_weight >= 0 and betas_weight >= 0):
@@ -470,8 +493,13 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                                                               device=device).reshape(B, 22, 3, 3).contiguous()
     sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
     pw, bw = float(pose_prior_weight), float(betas_weight)
+    mterms = None
+    if measurements is not None:
+        tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
+        mterms = (tgt.contiguous(), wt.contiguous(), circumference_derivative)
     if method == 'lm':
-        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw)
+        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw,
+                                    body_measurements, mterms)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -480,33 +508,64 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                          return_shaped=False)
         rot = torch.cat([grot, bpose], 1)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
-        return per_body, out, grot, bpose
+        meas = None
+        if mterms is not None:
+            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
+            m = body_measurements.forward_vertices(v, body_model.faces_i32, mterms[2])['measurements']
+            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+            # _kp2d_loss already counted betas_weight |betas|^2
+            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], 0.0)
+        return per_body, out, grot, bpose, meas
 
-    per_body, out, grot, bpose = _adam(list(params.values()), lr, iterations, loss_fn)
+    per_body, out, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
                loss=per_body)
+    if meas is not None:
+        res['measurements'] = meas
     return res
 
 
-def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw):
+def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw, body_measurements=None,
+                         mterms=None):
     from . import ops
     device = x.device
     packed = body_model.packed(device)
     B, K = x.shape[0], x.shape[1]
+    nb = params['betas'].shape[1]
     trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'camera': params['camera'].contiguous()}
-    state = _kp_lm_state(B, K, 22, params['betas'].shape[1], 'camera', device)
-    if B > 0:
+    state = _kp_lm_state(B, K, 22, nb, 'camera', device)
+    pose_anchor = anchor if pw > 0 else None
+    if mterms is not None:
+        state.update(meas=torch.empty(B, 5, dtype=torch.float32, device=device),
+                     meas_jac=torch.empty(B, 5, nb, dtype=torch.float32, device=device))
+    if B > 0 and mterms is None:
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
             ops.fit_lm_keypoints_2d_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac,
-                                         pose_anchor=anchor if pw > 0 else None)
+                                         pose_anchor=pose_anchor)
+    elif B > 0:
+        tgt, wt, cd = mterms
+        exact = exact_circumferences(cd)
+        faces, lm = body_model.faces_i32, body_measurements.landmarks()
+        ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
+        for it in range(iterations + 1):
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
+            v = ops.smplx_forward_shape(packed, trial['betas'])
+            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
+            ops.fit_lm_keypoints_2d_measurements_step(state, trial, x, w, sigma, pw, bw, tgt, wt, LM_UP, LM_DOWN,
+                                                      it == 0, tkp, tjac, tm, tmj, pose_anchor=pose_anchor)
     rot = state['rot']
     with torch.no_grad():
         out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
                          return_shaped=False)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
-    return _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+        if mterms is not None:      # _kp2d_loss already counted betas_weight |betas|^2
+            per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], 0.0)
+    res = _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+    if mterms is not None:
+        res['measurements'] = state['meas']
+    return res
 
 
 def main(argv=None):
@@ -523,7 +582,9 @@ def main(argv=None):
     p.add_argument('--waist', type=float, default=-1, help='waist circumference in metres')
     p.add_argument('--hips', type=float, default=-1, help='hips circumference in metres')
     p.add_argument('--targets', type=str, default=None,
-                   help='npz with per-body arrays mass / height / chest / waist / hips (overrides the single targets)')
+                   help='npz with per-body arrays mass / height / chest / waist / hips (overrides the single targets); '
+                        'with --keypoints-2d, the known measurements fitted together with the keypoints (the single '
+                        'targets are not used there)')
     p.add_argument('--meas-definition-path', dest='meas_definition_path', type=str, default=None)
     p.add_argument('--meas-vertices-path', dest='meas_vertices_path', type=str, default=None)
     p.add_argument('--betas-weight', dest='betas_weight', type=float, default=0.0)
@@ -558,17 +619,18 @@ def main(argv=None):
     else:
         model = SMPLX(model_folder=a.model_folder, gender=a.gender, ext=a.ext, betas={'num': a.num_betas})
     model = model.cuda()
-    if a.keypoints_2d:
-        return _main_keypoints_2d(a, model)
     if a.meas_definition_path and a.meas_vertices_path:
         cfg = {'meas_definition_path': a.meas_definition_path, 'meas_vertices_path': a.meas_vertices_path}
     else:
         cfg = {'landmarks': synth.load_landmarks()}
-    bm = BodyMeasurements(cfg).cuda()
+    targets = None
     if a.targets:
         d = np.load(a.targets)
         targets = {k: d[k].astype(np.float32) for k in NAMES if k in d.files}
-    else:
+    if a.keypoints_2d:      # known measurements only from --targets: --height has a default and is not used here
+        return _main_keypoints_2d(a, model, BodyMeasurements(cfg).cuda() if targets else None, targets)
+    bm = BodyMeasurements(cfg).cuda()
+    if targets is None:
         targets = {k: getattr(a, k) for k in NAMES}
     res = fit_betas_to_measurements(model, bm, targets, betas_weight=a.betas_weight, iterations=a.iterations, lr=a.lr,
                                     method=a.method, circumference_derivative=a.circumference_derivative)
@@ -579,7 +641,7 @@ def main(argv=None):
                       'first_body': {k: float(meas[0, i]) for i, k in enumerate(NAMES)}}))
 
 
-def _main_keypoints_2d(a, model):
+def _main_keypoints_2d(a, model, bm, targets):
     d = np.load(a.keypoints_2d)
     if 'openpose' in d.files:
         from . import keypoints2d as k2d
@@ -601,7 +663,8 @@ def _main_keypoints_2d(a, model):
                 if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
-                                   betas_weight=a.betas_weight, lr=a.lr)
+                                   betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
+                                   circumference_derivative=a.circumference_derivative)
     out = {k: v.detach().cpu().numpy() for k, v in res.items()}
     np.savez(a.output, **out)
     print(json.dumps({'bodies': int(x.shape[0]), 'output': a.output, 'median_loss': float(np.median(out['loss']))}))

@@ -394,6 +394,12 @@ def _kp_step_shapes_ok(state, trial_jac, weights, B, K, P):
     return trial_jac.shape == (B, 3 * K, P) and state['jac'].shape == (B, 3 * K, P) and weights.shape == (B, K)
 
 
+def _meas_step_shapes_ok(state, trial_meas, trial_meas_jac, meas_targets, meas_weights, B, nb):
+    """Whether the measurement block of a stacked keypoint + measurement step has the shapes its sizes give."""
+    return (trial_meas_jac.shape == (B, 5, nb) and state['meas_jac'].shape == (B, 5, nb) and
+            all(t.shape == (B, 5) for t in (meas_targets, meas_weights, trial_meas, state['meas'])))
+
+
 def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, first, trial, trial_meas, trial_jac):
     """One Levenberg-Marquardt step per body (include/shapy_b200.h, shapy_fit_lm_step), in place.  state: {'betas'
     (B, NB), 'meas' (B, 5), 'jac' (B, 5, NB), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32}, CUDA tensors;
@@ -476,8 +482,7 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
     P = 3 * n_rot + nb + 3
     if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}) and weights ({B}, {K})')
-    if (trial_meas_jac.shape != (B, 5, nb) or state['meas_jac'].shape != (B, 5, nb) or
-            any(t.shape != (B, 5) for t in (meas_targets, meas_weights, trial_meas, state['meas']))):
+    if not _meas_step_shapes_ok(state, trial_meas, trial_meas_jac, meas_targets, meas_weights, B, nb):
         raise RuntimeError(f'{what}: meas_jac must be ({B}, 5, {nb}) and the measurements, their targets and weights '
                            f'({B}, 5)')
     if B == 0:
@@ -492,15 +497,10 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
             ptr(trial_meas), ptr(trial_meas_jac), stream_ptr()), what)
 
 
-def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
-                             lambda_down, first, trial_keypoints, trial_jac, pose_anchor=None):
-    """One Levenberg-Marquardt step per body of the fit of pose, shape and weak-perspective camera to 2D keypoints
-    (include/shapy_b200.h, shapy_fit_lm_keypoints_2d_step), in place.  state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB),
-    'camera' (B, 3), 'keypoints' (B, K, 3), 'jac' (B, 3K, P), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32};
-    trial: {'rot', 'betas', 'camera'}, the evaluated trial on entry and the next trial on return; trial_keypoints /
-    trial_jac from smplx_keypoint_jacobian without transl; targets (B, K, 2), weights (B, K); robust_sigma None or inf
-    for least squares; pose_anchor (B, n_rot, 3, 3), needed when pose_prior_weight > 0."""
-    what = 'fit_lm_keypoints_2d_step'
+def _fit_lm_kp2d(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
+                 lambda_down, first, trial_keypoints, trial_jac, pose_anchor, meas=None):
+    """What the two 2D keypoint steps share: the checks and the call, `meas` None or the measurement block
+    (meas_targets, meas_weights, trial_meas, trial_meas_jac) of the stacked step."""
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
     sigma = float('inf') if robust_sigma is None else float(robust_sigma)
@@ -509,23 +509,62 @@ def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_
     if pose_prior_weight > 0 and pose_anchor is None:
         raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
     anchor = [] if pose_anchor is None else [pose_anchor]
-    ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + \
-        [trial[k] for k in ('rot', 'betas', 'camera')] + [targets, weights, trial_keypoints, trial_jac] + anchor
+    mstate = [] if meas is None else [state['meas'], state['meas_jac']]
+    ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
+        [trial[k] for k in ('rot', 'betas', 'camera')] + [targets, weights, trial_keypoints, trial_jac] + anchor + \
+        list(meas or ())
     _check_step_tensors(what, ts, 'the state, trial, targets, weights and anchor', state['accepted'])
     P = 3 * n_rot + nb + 3
     if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
     if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], B, nb):
+        raise RuntimeError(f'{what}: meas_jac must be ({B}, 5, {nb}) and the measurements, their targets and weights '
+                           f'({B}, 5)')
     if B == 0:
         return
+    head = [B, K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma, float(pose_prior_weight),
+            float(betas_weight)]
+    lam = [float(lambda_up), float(lambda_down), int(bool(first))]
+    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['camera']), ptr(trial_keypoints), ptr(trial_jac)]
     with torch.cuda.device(trial['rot'].device):
-        check(lib().shapy_fit_lm_keypoints_2d_step(
-            B, K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma, float(pose_prior_weight),
-            float(betas_weight), float(lambda_up), float(lambda_down), int(bool(first)),
-            *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
-            ptr(trial['rot']), ptr(trial['betas']), ptr(trial['camera']), ptr(trial_keypoints), ptr(trial_jac),
-            stream_ptr()), what)
+        if meas is None:
+            check(lib().shapy_fit_lm_keypoints_2d_step(
+                *head, *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+                *tr, stream_ptr()), what)
+        else:
+            check(lib().shapy_fit_lm_keypoints_2d_measurements_step(
+                *head, ptr(meas[0]), ptr(meas[1]), *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
+                                          'lambda', 'accepted')],
+                *tr, ptr(meas[2]), ptr(meas[3]), stream_ptr()), what)
+
+
+def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
+                             lambda_down, first, trial_keypoints, trial_jac, pose_anchor=None):
+    """One Levenberg-Marquardt step per body of the fit of pose, shape and weak-perspective camera to 2D keypoints
+    (include/shapy_b200.h, shapy_fit_lm_keypoints_2d_step), in place.  state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB),
+    'camera' (B, 3), 'keypoints' (B, K, 3), 'jac' (B, 3K, P), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32};
+    trial: {'rot', 'betas', 'camera'}, the evaluated trial on entry and the next trial on return; trial_keypoints /
+    trial_jac from smplx_keypoint_jacobian without transl; targets (B, K, 2), weights (B, K); robust_sigma None or inf
+    for least squares; pose_anchor (B, n_rot, 3, 3), needed when pose_prior_weight > 0."""
+    _fit_lm_kp2d('fit_lm_keypoints_2d_step', state, trial, targets, weights, robust_sigma, pose_prior_weight,
+                 betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac, pose_anchor)
+
+
+def fit_lm_keypoints_2d_measurements_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight,
+                                          meas_targets, meas_weights, lambda_up, lambda_down, first, trial_keypoints,
+                                          trial_jac, trial_meas, trial_meas_jac, pose_anchor=None):
+    """fit_lm_keypoints_2d_step with the five measurements stacked under its rows (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_measurements_step), in place.  state: fit_lm_keypoints_2d_step's plus 'meas' (B, 5) and
+    'meas_jac' (B, 5, NB); meas_targets, meas_weights (B, 5) in the order mass, height, chest, waist, hips; trial_meas
+    (B, 5) / trial_meas_jac (B, 5, NB) from measure_jacobian_betas at the trial betas.  betas_weight is the one betas
+    regulariser, the 2D step's."""
+    _fit_lm_kp2d('fit_lm_keypoints_2d_measurements_step', state, trial, targets, weights, robust_sigma,
+                 pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                 pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac))
 
 
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
