@@ -327,6 +327,48 @@ int shapy_fit_lm_keypoints_2d_measurements_step(
     int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_camera, const float *trial_keypoints,
     const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream);
 
+/* shapy_fit_lm_keypoints_2d_step over groups of images of one person: the images [group_offsets[g],
+ * group_offsets[g+1]) of group g share one beta_g, each keeps its own rotations and camera.  Loss per group, fp64, left
+ * to right: the sum over its images (image order) of the 2D step's keypoint term and pose prior, + betas_weight
+ * |beta_g|^2.  group_offsets: num_groups + 1 int32 in host memory, non-decreasing from 0 to batch, every group
+ * non-empty; copied into the workspace on the stream at every call.  Per image (batch rows): targets, weights,
+ * pose_anchor, rot, camera, keypoints, jac, trial_rot, trial_camera, trial_keypoints, trial_jac and trial_betas_images
+ * (batch,nb), the trial betas of each image's group (what shapy_smplx_keypoint_jacobian evaluated).  Per group
+ * (num_groups rows): betas (G,nb), loss, lambda, accepted and trial_betas (G,nb).  Policy, lambda constants, damping
+ * and rotation update are the 2D step's, per group: one decision, lambda, loss and accept count; the first lambda is
+ * 1e-3 max(1e-6, the largest diagonal entry of the group's keypoint rows), per image on the pose and camera columns
+ * and summed over the images on the betas columns.  The step is the exact LM step of the group's block-arrow normal
+ * matrix by its Schur complement: each image's [pose | camera] block (damped by lambda) is eliminated, the nb x nb
+ * system (damped by betas_weight + lambda) solved for dbeta, each image's delta back-substituted.  Three launches, no
+ * synchronisation, no atomics: a group's results do not depend on the rest of the batch.  If the group's loss is not
+ * finite or one of its factorisations fails, the group keeps its state.  The next trial goes to trial_betas and to
+ * each image's row of trial_betas_images.  workspace: shapy_fit_lm_groups_workspace_bytes(batch, num_groups, n_rot, nb)
+ * bytes of device memory.  Errors as shapy_fit_lm_keypoints_2d_step, and SHAPY_ERR_ARG for bad offsets or an empty
+ * group.  batch 0 (with num_groups 0): no launch. */
+size_t shapy_fit_lm_groups_workspace_bytes(int batch, int num_groups, int n_rot, int nb);
+int shapy_fit_lm_keypoints_2d_groups_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *camera,
+    float *keypoints, float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_betas_images, float *trial_camera, const float *trial_keypoints, const float *trial_jac,
+    void *workspace, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_groups_step with the five virtual measurements of each group (on the T-pose of beta_g):
+ * the group loss gains sum_{u_m > 0} u_m (t_gm - meas_gm)^2 (m order, summed on its own) before the betas prior, and
+ * J_m^T U J_m, J_m^T U (meas - t) (m order) join the betas system before betas_weight beta.  meas_targets,
+ * meas_weights, meas, trial_meas (G,5), meas_jac, trial_meas_jac (G,5,nb): shapy_measure_jacobian_betas of the G
+ * trial betas.  With every measurement weight <= 0 every output equals shapy_fit_lm_keypoints_2d_groups_step's bit for
+ * bit.  Errors as that entry, the measurement pointers included. */
+int shapy_fit_lm_keypoints_2d_groups_measurements_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
+    const float *trial_meas_jac, void *workspace, void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

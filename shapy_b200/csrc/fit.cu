@@ -201,17 +201,19 @@ struct LmKpArgs {                       // what the keypoint steps share; `last`
   const float *tkp, *tjac;
 };
 
-// Phase 2 on accept: the trial's parameters, keypoints, Jacobian and loss become the state
-__device__ __forceinline__ void lm_kp_take_trial(const LmKpArgs &a, int b, float lnew) {
+// Phase 2 on accept: the trial's parameters, keypoints, Jacobian and loss become the state; without `body` only the
+// image's own part (rotations, the last three, keypoints, Jacobian): the grouped step keeps betas and loss per group
+__device__ __forceinline__ void lm_kp_take_trial(const LmKpArgs &a, int b, float lnew, bool body = true) {
   const int t = threadIdx.x, nb = a.nb, R3 = 3 * a.K;
   const size_t nr9 = (size_t)a.n_rot * 9;
   for (size_t i = t; i < nr9; i += blockDim.x) a.rot[b * nr9 + i] = a.trot[b * nr9 + i];
-  for (int i = t; i < nb; i += blockDim.x) a.betas[(size_t)b * nb + i] = a.tbetas[(size_t)b * nb + i];
+  if (body)
+    for (int i = t; i < nb; i += blockDim.x) a.betas[(size_t)b * nb + i] = a.tbetas[(size_t)b * nb + i];
   if (t < 3) a.last[(size_t)b * 3 + t] = a.tlast[(size_t)b * 3 + t];
   for (int i = t; i < R3; i += blockDim.x) a.kp[(size_t)b * R3 + i] = a.tkp[(size_t)b * R3 + i];
   for (size_t i = t; i < (size_t)R3 * a.P; i += blockDim.x)
     a.jac[(size_t)b * R3 * a.P + i] = a.tjac[(size_t)b * R3 * a.P + i];
-  if (t == 0) a.loss[b] = lnew;
+  if (body && t == 0) a.loss[b] = lnew;
 }
 
 // Phase 3, ownership: thread t accumulates the lower-triangle entries t + kLmKpThreads i (row-major) of the normal
@@ -247,7 +249,17 @@ __device__ __forceinline__ void lm_kp_add_rows(int nr, int P, const double (*Js)
   }
 }
 
-// Phase 3, the end: A and y = -g go to shared memory, then thread 0 sets lambda (lm_lambda; the first from the P
+// Phase 3, the end: A (the P x P lower triangle) and y = -g go to shared memory
+__device__ __forceinline__ void lm_kp_store(int P, double *A, double *y, const int (&pr)[kLmKpPairs],
+                                            const int (&pc)[kLmKpPairs], const double (&acc)[kLmKpPairs], double g) {
+#pragma unroll
+  for (int i = 0; i < kLmKpPairs; ++i)
+    if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
+  if (threadIdx.x < P) y[threadIdx.x] = -g;
+  __syncthreads();
+}
+
+// Phase 3, the end: lm_kp_store, then thread 0 sets lambda (lm_lambda; the first from the P
 // entries diag[0], diag[stride], ...: the caller says which rows' diagonal counts), counts an accepted trial and damps
 // the diagonal, by (double)rho + (double)lambda on the columns [lo, hi) and lambda elsewhere.  ok_s starts as "the
 // state's loss is finite": a body without a finite loss does not move
@@ -256,11 +268,7 @@ __device__ __forceinline__ void lm_kp_damp(const LmKpArgs &a, int b, bool accept
                                            const double (&acc)[kLmKpPairs], double g, const double *diag, int stride,
                                            int lo, int hi, float rho, int &ok_s) {
   const int P = a.P;
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i)
-    if (pr[i] >= 0) A[pr[i] * P + pc[i]] = acc[i];
-  if (threadIdx.x < P) y[threadIdx.x] = -g;
-  __syncthreads();
+  lm_kp_store(P, A, y, pr, pc, acc, g);
   if (threadIdx.x == 0) {
     double dmax = kDiagFloor;
     if (a.first)
@@ -276,10 +284,11 @@ __device__ __forceinline__ void lm_kp_damp(const LmKpArgs &a, int b, bool accept
 
 // Phase 4: Cholesky A = L L^T of the P x P lower triangle in shared memory, right-looking (column j scaled, then the
 // trailing lower triangle updated), then L y = -g and L^T delta = y in place in y; thread 0 clears ok_s on a pivot that
-// is not positive and finite
-__device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int &ok_s) {
+// is not positive and finite.  With n < P only the leading n columns are eliminated: the trailing block is then the
+// Schur complement C - B^T A11^-1 B, y's tail -(g2 - B^T A11^-1 g1), and y's head -A11^-1 g1
+__device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int n, int &ok_s) {
   const int t = threadIdx.x;
-  for (int j = 0; j < P; ++j) {
+  for (int j = 0; j < n; ++j) {
     __syncthreads();
     const double d = A[j * P + j];
     const double ljj = sqrt(d);
@@ -297,14 +306,14 @@ __device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int &ok
     }
   }
   // L y = -g, then L^T delta = y
-  for (int j = 0; j < P; ++j) {
+  for (int j = 0; j < n; ++j) {
     __syncthreads();
     const double yj = y[j] / A[j * P + j];
     __syncthreads();
     if (t == 0) y[j] = yj;
     for (int i = j + 1 + t; i < P; i += blockDim.x) y[i] -= A[i * P + j] * yj;
   }
-  for (int j = P - 1; j >= 0; --j) {
+  for (int j = n - 1; j >= 0; --j) {
     __syncthreads();
     const double dj = y[j] / A[j * P + j];
     __syncthreads();
@@ -312,6 +321,40 @@ __device__ __forceinline__ void lm_kp_solve(double *A, double *y, int P, int &ok
     for (int i = t; i < j; i += blockDim.x) y[i] -= A[j * P + i] * dj;
   }
   __syncthreads();
+}
+
+// R Exp(d) by Rodrigues in fp64, re-orthonormalised by the 6D decoder's Gram-Schmidt of the first two columns, rounded
+// to fp32: the rotation update of every keypoint step
+__device__ __forceinline__ void lm_exp_gs(const float *Rs, double d0, double d1, double d2, float *Rt) {
+  const double th2 = d0 * d0 + d1 * d1 + d2 * d2, th = sqrt(th2);
+  double s, c;                          // Exp(d) = I + s [d]x + c [d]x^2
+  if (th < 1e-8) {
+    s = 1.0 - th2 / 6.0;
+    c = 0.5 - th2 / 24.0;
+  } else {
+    s = sin(th) / th;
+    c = (1.0 - cos(th)) / th2;
+  }
+  const double dv[3] = {d0, d1, d2};
+  const double Kx[9] = {0.0, -d2, d1, d2, 0.0, -d0, -d1, d0, 0.0};
+  double E[9], Mr[9];
+  for (int r = 0; r < 3; ++r)
+    for (int q = 0; q < 3; ++q) E[r * 3 + q] = (r == q ? 1.0 : 0.0) + s * Kx[r * 3 + q] + c * (dv[r] * dv[q] - (r == q ? th2 : 0.0));
+  for (int r = 0; r < 3; ++r)
+    for (int q = 0; q < 3; ++q)
+      Mr[r * 3 + q] = (double)Rs[r * 3] * E[q] + (double)Rs[r * 3 + 1] * E[3 + q] + (double)Rs[r * 3 + 2] * E[6 + q];
+  // the 6D decoder's Gram-Schmidt of the first two columns
+  const double x0 = Mr[0], x1 = Mr[3], x2 = Mr[6], c0 = Mr[1], c1 = Mr[4], c2 = Mr[7];
+  const double n1 = fmax(sqrt(x0 * x0 + x1 * x1 + x2 * x2), 1e-12);
+  const double b10 = x0 / n1, b11 = x1 / n1, b12 = x2 / n1;
+  const double dd = b10 * c0 + b11 * c1 + b12 * c2;
+  const double u0 = c0 - dd * b10, u1 = c1 - dd * b11, u2 = c2 - dd * b12;
+  const double n2 = fmax(sqrt(u0 * u0 + u1 * u1 + u2 * u2), 1e-12);
+  const double b20 = u0 / n2, b21 = u1 / n2, b22 = u2 / n2;
+  const double b30 = b11 * b22 - b12 * b21, b31 = b12 * b20 - b10 * b22, b32 = b10 * b21 - b11 * b20;
+  Rt[0] = (float)b10; Rt[1] = (float)b20; Rt[2] = (float)b30;
+  Rt[3] = (float)b11; Rt[4] = (float)b21; Rt[5] = (float)b31;
+  Rt[6] = (float)b12; Rt[7] = (float)b22; Rt[8] = (float)b32;
 }
 
 // Phase 5, the next trial from the state and delta = y: the rotations R_j Exp(delta_j) by Rodrigues in fp64,
@@ -328,36 +371,7 @@ __device__ __forceinline__ void lm_kp_next_trial(const LmKpArgs &a, int b, const
       for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
       continue;
     }
-    const double d0 = y[3 * j], d1 = y[3 * j + 1], d2 = y[3 * j + 2];
-    const double th2 = d0 * d0 + d1 * d1 + d2 * d2, th = sqrt(th2);
-    double s, c;                          // Exp(d) = I + s [d]x + c [d]x^2
-    if (th < 1e-8) {
-      s = 1.0 - th2 / 6.0;
-      c = 0.5 - th2 / 24.0;
-    } else {
-      s = sin(th) / th;
-      c = (1.0 - cos(th)) / th2;
-    }
-    const double dv[3] = {d0, d1, d2};
-    const double Kx[9] = {0.0, -d2, d1, d2, 0.0, -d0, -d1, d0, 0.0};
-    double E[9], Mr[9];
-    for (int r = 0; r < 3; ++r)
-      for (int q = 0; q < 3; ++q) E[r * 3 + q] = (r == q ? 1.0 : 0.0) + s * Kx[r * 3 + q] + c * (dv[r] * dv[q] - (r == q ? th2 : 0.0));
-    for (int r = 0; r < 3; ++r)
-      for (int q = 0; q < 3; ++q)
-        Mr[r * 3 + q] = (double)Rs[r * 3] * E[q] + (double)Rs[r * 3 + 1] * E[3 + q] + (double)Rs[r * 3 + 2] * E[6 + q];
-    // the 6D decoder's Gram-Schmidt of the first two columns
-    const double x0 = Mr[0], x1 = Mr[3], x2 = Mr[6], c0 = Mr[1], c1 = Mr[4], c2 = Mr[7];
-    const double n1 = fmax(sqrt(x0 * x0 + x1 * x1 + x2 * x2), 1e-12);
-    const double b10 = x0 / n1, b11 = x1 / n1, b12 = x2 / n1;
-    const double dd = b10 * c0 + b11 * c1 + b12 * c2;
-    const double u0 = c0 - dd * b10, u1 = c1 - dd * b11, u2 = c2 - dd * b12;
-    const double n2 = fmax(sqrt(u0 * u0 + u1 * u1 + u2 * u2), 1e-12);
-    const double b20 = u0 / n2, b21 = u1 / n2, b22 = u2 / n2;
-    const double b30 = b11 * b22 - b12 * b21, b31 = b12 * b20 - b10 * b22, b32 = b10 * b21 - b11 * b20;
-    Rt[0] = (float)b10; Rt[1] = (float)b20; Rt[2] = (float)b30;
-    Rt[3] = (float)b11; Rt[4] = (float)b21; Rt[5] = (float)b31;
-    Rt[6] = (float)b12; Rt[7] = (float)b22; Rt[8] = (float)b32;
+    lm_exp_gs(Rs, y[3 * j], y[3 * j + 1], y[3 * j + 2], Rt);
   }
   for (int l = t; l < nb; l += blockDim.x) {
     const float x = a.betas[(size_t)b * nb + l];
@@ -523,7 +537,7 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
   }
   // the first lambda from all of diag(A); only the MEAS step has a betas regulariser to damp with
   lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, A, P + 1, MEAS ? o : 0, MEAS ? o + a.nb : 0, mb.rho, ok_s);
-  lm_kp_solve(A, y, P, ok_s);
+  lm_kp_solve(A, y, P, P, ok_s);
   // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
   lm_kp_next_trial(a, b, y, ok_s);
 }
@@ -580,6 +594,122 @@ __device__ __forceinline__ double rot_tangent(const float *R, int a, int e) {
   return ((q - a + 3) % 3 == 1) ? v : -v;      // -eps_{a m q} R_rm
 }
 
+// Phase 1 of the 2D steps, by one thread: the trial's robust keypoint term (k order) and pose prior, left to right
+__device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const LmKp2dArgs &x2, int b, const float *tg,
+                                                     const float *wt, const float *anc, bool robust, double s2) {
+  const int K = a.K, R3 = 3 * a.K, nr9 = 9 * a.n_rot;
+  const float *m = a.tkp + (size_t)b * R3, *cam = a.tlast + (size_t)b * 3;
+  double s, ds;
+  softplus_d((double)cam[0], s, ds);
+  const double cx = cam[1], cy = cam[2];
+  double L = 0.0;
+  for (int k = 0; k < K; ++k) {
+    const double w = wt[k];
+    if (!(w > 0.0)) continue;
+    const double dx = s * ((double)m[3 * k] + cx) - (double)tg[2 * k];
+    const double dy = s * ((double)m[3 * k + 1] + cy) - (double)tg[2 * k + 1];
+    const double e = dx * dx + dy * dy;
+    L += w * (robust ? e * (s2 / (s2 + e)) : e);
+  }
+  if (x2.pose_w > 0.f) {
+    const float *tr = a.trot + (size_t)b * nr9;
+    double q = 0.0;
+    for (int i = 9; i < nr9; ++i) {
+      const double d = (double)tr[i] - (double)anc[i];
+      q += d * d;
+    }
+    L += 0.5 * (double)x2.pose_w * q;
+  }
+  return L;
+}
+
+// Phase 3 of the 2D steps: row c of keypoint k at the state (keypoints M, scale s, offset cxy), its weight w_k q_k^2 (the
+// IRLS weight, w_k at sigma = inf) and residual; a dropped keypoint (w_k <= 0) keeps w_k and a zero residual
+__device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, const float *wt, double s,
+                                            const double (&cxy)[2], bool robust, double s2, int k, int c, double &wr,
+                                            double &res) {
+  const double w = wt[k];
+  wr = w;
+  res = 0.0;
+  if (w > 0.0) {
+    const double dx = s * ((double)M[3 * k] + cxy[0]) - (double)tg[2 * k];
+    const double dy = s * ((double)M[3 * k + 1] + cxy[1]) - (double)tg[2 * k + 1];
+    if (robust) {
+      const double q = s2 / (s2 + (dx * dx + dy * dy));
+      wr = w * (q * q);
+    }
+    res = c ? dy : dx;
+  }
+}
+
+// Column col of that row, the camera columns at oc: s J_{3k+c} on the rotation and betas columns, ds (kp_kc + c_{1+c})
+// on c0, s on c_{1+c}.  REORDER: columns [delta | c | beta] (the grouped step), else [delta | beta | c]
+template <bool REORDER>
+__device__ __forceinline__ double lm_kp2d_entry(const float *J, const float *M, int P, int oc, int k, int c, int col,
+                                                double s, double ds, const double (&cxy)[2]) {
+  const bool betas = REORDER && col > oc + 2;
+  if (col < oc || betas) return s * (double)J[(size_t)(3 * k + c) * P + (betas ? col - 3 : col)];
+  if (col == oc) return ds * ((double)M[3 * k + c] + cxy[c]);
+  return col - oc - 1 == c ? s : 0.0;
+}
+
+// Phase 3 of the 2D steps: the keypoint rows 2k + c, staged kLmKpRows at a time and accumulated in row order
+template <bool REORDER>
+__device__ __forceinline__ void lm_kp2d_keypoint_rows(int K, int P, const float *J, const float *M,
+                                                      const float *tg, const float *wt, double s, double ds,
+                                                      const double (&cxy)[2], bool robust, double s2, int oc,
+                                                      double (*Js)[kLmKpMaxP], double (*WJs)[kLmKpMaxP], double *ws,
+                                                      double *rs, const int (&pr)[kLmKpPairs],
+                                                      const int (&pc)[kLmKpPairs], double (&acc)[kLmKpPairs],
+                                                      double &g) {
+  const int t = threadIdx.x, R2 = 2 * K;
+  for (int r0 = 0; r0 < R2; r0 += kLmKpRows) {
+    const int nr = min(kLmKpRows, R2 - r0);
+    __syncthreads();
+    for (int i = t; i < nr; i += blockDim.x) {   // row weight (IRLS at the state) and residual
+      double wr, res;
+      lm_kp2d_row(M, tg, wt, s, cxy, robust, s2, (r0 + i) >> 1, (r0 + i) & 1, wr, res);
+      ws[i] = wr;
+      rs[i] = res;
+    }
+    __syncthreads();
+    for (int i = t; i < nr * P; i += blockDim.x) {
+      const int row = i / P, col = i % P;
+      const double wr = ws[row];
+      if (wr > 0.0) {                    // a dropped keypoint's rows are never read: they may be NaN
+        const double x = lm_kp2d_entry<REORDER>(J, M, P, oc, (r0 + row) >> 1, (r0 + row) & 1, col, s, ds, cxy);
+        Js[row][col] = x;
+        WJs[row][col] = wr * x;
+      }
+    }
+    __syncthreads();
+    lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
+  }
+}
+
+// Phase 3 of the 2D steps: the pose-prior rows of joint j only reach its diagonal block (columns 3 j .. 3 j + 2, the
+// same in both column orders): no staging
+__device__ __forceinline__ void lm_kp2d_prior_rows(const LmKp2dArgs &x2, int o, const float *Rst, const float *anc,
+                                                   const int (&pr)[kLmKpPairs], const int (&pc)[kLmKpPairs],
+                                                   double (&acc)[kLmKpPairs], double &g) {
+  const int t = threadIdx.x;
+  if (x2.pose_w > 0.f) {
+    const double hw = 0.5 * (double)x2.pose_w;
+#pragma unroll
+    for (int i = 0; i < kLmKpPairs; ++i) {
+      const int j = pr[i] / 3;
+      if (pr[i] >= 3 && pr[i] < o && pc[i] / 3 == j) {
+        const float *R = Rst + 9 * j;
+        for (int e = 0; e < 9; ++e) acc[i] += (hw * rot_tangent(R, pr[i] % 3, e)) * rot_tangent(R, pc[i] % 3, e);
+      }
+    }
+    if (t >= 3 && t < o) {
+      const float *R = Rst + 9 * (t / 3), *R0 = anc + 9 * (t / 3);
+      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
+    }
+  }
+}
+
 template <bool MEAS>
 __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, LmKp2dArgs x2) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
@@ -596,28 +726,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   const float lcur = a.loss[b];
   // 1. trial loss
   if (t == 0) {
-    const float *m = a.tkp + (size_t)b * R3, *cam = a.tlast + (size_t)b * 3;
-    double s, ds;
-    softplus_d((double)cam[0], s, ds);
-    const double cx = cam[1], cy = cam[2];
-    double L = 0.0;
-    for (int k = 0; k < K; ++k) {
-      const double w = wt[k];
-      if (!(w > 0.0)) continue;
-      const double dx = s * ((double)m[3 * k] + cx) - (double)tg[2 * k];
-      const double dy = s * ((double)m[3 * k + 1] + cy) - (double)tg[2 * k + 1];
-      const double e = dx * dx + dy * dy;
-      L += w * (robust ? e * (s2 / (s2 + e)) : e);
-    }
-    if (x2.pose_w > 0.f) {
-      const float *tr = a.trot + (size_t)b * nr9;
-      double q = 0.0;
-      for (int i = 9; i < nr9; ++i) {
-        const double d = (double)tr[i] - (double)anc[i];
-        q += d * d;
-      }
-      L += 0.5 * (double)x2.pose_w * q;
-    }
+    double L = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
     if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
     if (x2.betas_w > 0.f) {
       const float *tb = a.tbetas + (size_t)b * nb;
@@ -648,69 +757,18 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   int pr[kLmKpPairs], pc[kLmKpPairs];
   double acc[kLmKpPairs], g = 0.0;
   lm_kp_pairs(P, pr, pc, acc);
-  const int R2 = 2 * K;
-  for (int r0 = 0; r0 < R2; r0 += kLmKpRows) {
-    const int nr = min(kLmKpRows, R2 - r0);
-    __syncthreads();
-    for (int i = t; i < nr; i += blockDim.x) {   // row weight (IRLS at the state) and residual
-      const int k = (r0 + i) >> 1, c = (r0 + i) & 1;
-      const double w = wt[k];
-      double wr = w, res = 0.0;
-      if (w > 0.0) {
-        const double dx = s * ((double)M[3 * k] + cxy[0]) - (double)tg[2 * k];
-        const double dy = s * ((double)M[3 * k + 1] + cxy[1]) - (double)tg[2 * k + 1];
-        if (robust) {
-          const double q = s2 / (s2 + (dx * dx + dy * dy));
-          wr = w * (q * q);
-        }
-        res = c ? dy : dx;
-      }
-      ws[i] = wr;
-      rs[i] = res;
-    }
-    __syncthreads();
-    for (int i = t; i < nr * P; i += blockDim.x) {
-      const int row = i / P, col = i % P;
-      const double wr = ws[row];
-      if (wr > 0.0) {                    // a dropped keypoint's rows are never read: they may be NaN
-        const int k = (r0 + row) >> 1, c = (r0 + row) & 1;
-        double x;
-        if (col < oc) x = s * (double)J[(size_t)(3 * k + c) * P + col];
-        else if (col == oc) x = ds * ((double)M[3 * k + c] + cxy[c]);
-        else x = col - oc - 1 == c ? s : 0.0;
-        Js[row][col] = x;
-        WJs[row][col] = wr * x;
-      }
-    }
-    __syncthreads();
-    lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
-  }
+  lm_kp2d_keypoint_rows<false>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc, g);
 #pragma unroll
   for (int i = 0; i < kLmKpPairs; ++i)
     if (pr[i] >= 0 && pr[i] == pc[i]) dg[pr[i]] = acc[i];     // the diagonal of the keypoint rows: the first lambda
-  if (x2.pose_w > 0.f) {
-    // the pose-prior rows of joint j only reach its diagonal block: no staging
-    const double hw = 0.5 * (double)x2.pose_w;
-#pragma unroll
-    for (int i = 0; i < kLmKpPairs; ++i) {
-      const int j = pr[i] / 3;
-      if (pr[i] >= 3 && pr[i] < o && pc[i] / 3 == j) {
-        const float *R = Rst + 9 * j;
-        for (int e = 0; e < 9; ++e) acc[i] += (hw * rot_tangent(R, pr[i] % 3, e)) * rot_tangent(R, pc[i] % 3, e);
-      }
-    }
-    if (t >= 3 && t < o) {
-      const float *R = Rst + 9 * (t / 3), *R0 = anc + 9 * (t / 3);
-      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
-    }
-  }
+  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
   if constexpr (MEAS)
     lm_meas_add_rows(x2.mb, b, nb, o, (accept ? x2.mb.tmeas : x2.mb.meas) + (size_t)b * 5,
                      (accept ? x2.mb.tjac : x2.mb.jac) + (size_t)b * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, g);
   if (x2.betas_w > 0.f && t >= o && t < oc) g += (double)x2.betas_w * (double)Bst[t - o];
   lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, dg, 1, o, oc, x2.betas_w, ok_s);
   // 4. Cholesky and the two triangular solves
-  lm_kp_solve(A, y, P, ok_s);
+  lm_kp_solve(A, y, P, P, ok_s);
   // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
   lm_kp_next_trial(a, b, y, ok_s);
 }
@@ -719,9 +777,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
 // set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors` its own scalars and the
 // sentence that states their and the lambda factors' ranges; then the launch, one CTA of kLmKpThreads per body with
 // P x P doubles of dynamic shared memory.  Past 48 KB of static plus dynamic shared memory the launch has to opt in
-template <typename Extra>
-int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
-              bool factors_ok, const char *factors, void *stream) {
+inline int check_lm_kp(const char *fn, int batch, LmKpArgs &a, bool extra_ok, bool factors_ok, const char *factors) {
   SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
                     a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && extra_ok,
                 "%s: null argument", fn);
@@ -733,6 +789,14 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
     set_error("%s: %d parameters, at most %d are supported", fn, a.P, kLmKpMaxP);
     return SHAPY_ERR_UNSUPPORTED;
   }
+  return SHAPY_OK;
+}
+
+template <typename Extra>
+int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
+              bool factors_ok, const char *factors, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, extra_ok, factors_ok, factors);
+  if (rc != SHAPY_OK) return rc;
   if (batch == 0) return SHAPY_OK;
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
   cudaFuncAttributes attr;
@@ -740,6 +804,303 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
   if (smem + attr.sharedSizeBytes > 48 * 1024)
     SHAPY_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The grouped 2D step (shapy_fit_lm_keypoints_2d_groups_step): the images [off[g], off[g + 1]) of group g share one
+// beta_g, each keeps its rotations and camera.  Per group, in fp64, left to right:
+//   L_g = sum_{i in g} (image order) [the 2D step's keypoint term + pose prior of image i]
+//       + sum_{u_m > 0} u_m (t_gm - meas_gm)^2 (m order, summed on its own; the MEAS entry, on the T-pose of beta_g)
+//       + betas_w |beta_g|^2 (l order; when betas_w > 0).
+// The normal matrix of a group is block-arrow shaped: image i's block [delta_i | c_i] (n1 = 3 n_rot + 3 columns) only
+// meets beta.  The exact LM step eliminates each image's block (a Schur complement), in three launches:
+//   1. lm_kp2dg_loss_kernel, per image: the bracket of the trial's loss into its scratch; on the first step also the
+//      diagonal of the trial's keypoint rows (the max of its n1 leading entries and its nb betas entries);
+//   2. lm_kp2dg_image_kernel, per image: the group's decision (lm_group_decide from the siblings' scratch), on accept
+//      the image's trial becomes its state; the 2D step's keypoint and pose-prior rows staged in the column order
+//      [delta | c | beta], the leading n1 x n1 block damped by lambda and factored alone (lm_kp_solve with n = n1), then
+//      X_i = A_i^-1 B_i by the solve's backward substitution on the rows of L21; into scratch S_i = C_i - B_i^T X_i
+//      (the factor's trailing block), s_i = g_beta,i - B_i^T A_i^-1 g_i, X_i, x_i = A_i^-1 g_i and the pivots' flag;
+//   3. lm_kp2dg_group_kernel, per group: the same decision, the group's state (loss, lambda, accepted; on accept beta
+//      and the measurements), S = sum_i S_i and s = sum_i s_i (image order), then the measurement rows (m order) and
+//      betas_w beta_g, (S + (betas_w + lambda) I) dbeta = -s by the same Cholesky, and per image delta_i = -x_i -
+//      X_i dbeta (l order) and the next trial R Exp(delta), c + delta_c, beta_g + dbeta (both trial betas arrays).
+// The first lambda is 1e-3 max(1e-6, the largest diagonal entry of the group's keypoint rows): per image on its pose
+// and camera columns, summed over the images (image order) on the betas columns.  A group whose loss is not finite, or
+// one of whose factorisations fails, keeps its state.  Every CTA of a group decides from the same scratch in the same
+// order; no atomics, so a group's bits do not depend on the rest of the batch.  A group of one has the 2D step's loss,
+// lambda and decision bit for bit; its trial differs by the order of elimination.
+struct LmGroupArgs {
+  int G;
+  const int *off;                       // (G + 1) offsets, the device copy in the workspace
+  double *scr;                          // per image scratch, `stride` doubles each (lm_group_scratch)
+  int stride;
+  float *tbetas_img;                    // (B, nb): the trial betas per image, for the keypoint Jacobian
+};
+
+// The slots of an image's scratch: the bracket of its trial loss, the factorisation flag, the max of its first-step
+// keypoint diagonal over [delta | c], then its nb betas diagonal entries, S_i (nb x nb, lower), s_i (nb), X_i (n1 x nb)
+// and x_i (n1)
+constexpr int kScrLoss = 0, kScrOk = 1, kScrDmax = 2, kScrDiag = 3;
+__host__ __device__ inline int lm_group_stride(int n1, int nb) { return kScrDiag + 2 * nb + nb * nb + n1 * nb + n1; }
+inline size_t lm_group_offsets_bytes(int G) { return ((size_t)(G + 1) * sizeof(int) + 15) / 16 * 16; }
+
+struct LmGroupDecision {
+  bool accept;
+  float lnew, lam;
+};
+
+// The group's decision, by one thread, from the images' scratch of launch 1 and the group state: its trial loss L_g,
+// accept (lm_accept), the state's loss after it (lm_loss) and lambda (lm_lambda, the first from the group diagonal)
+__device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &x2, const LmGroupArgs &gr, int g) {
+  const int i0 = gr.off[g], i1 = gr.off[g + 1], nb = a.nb;
+  const double *s0 = gr.scr + (size_t)i0 * gr.stride;
+  double L = s0[kScrLoss];
+  for (int i = i0 + 1; i < i1; ++i) L += gr.scr[(size_t)i * gr.stride + kScrLoss];
+  if (x2.mb.weights) L += lm_meas_loss(x2.mb, g);
+  if (x2.betas_w > 0.f) {
+    const float *tb = a.tbetas + (size_t)g * nb;
+    double reg = 0.0;
+    for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
+    L += (double)x2.betas_w * reg;
+  }
+  const float lcur = a.loss[g];
+  LmGroupDecision d;
+  d.accept = lm_accept(a.first, L, lcur);
+  d.lnew = lm_loss(d.accept, L, lcur);
+  double dmax = kDiagFloor;
+  if (a.first) {
+    for (int i = i0; i < i1; ++i) dmax = fmax(dmax, gr.scr[(size_t)i * gr.stride + kScrDmax]);
+    for (int l = 0; l < nb; ++l) {
+      double d2 = s0[kScrDiag + l];
+      for (int i = i0 + 1; i < i1; ++i) d2 += gr.scr[(size_t)i * gr.stride + kScrDiag + l];
+      dmax = fmax(dmax, d2);
+    }
+  }
+  d.lam = lm_lambda(a.first, d.accept, a.first ? 0.f : a.lambda[g], dmax, a.up, a.down);
+  return d;
+}
+
+__global__ void __launch_bounds__(128) lm_kp2dg_loss_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
+  __shared__ double dg[kLmKpMaxP];
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, nb = a.nb, o = 3 * a.n_rot;
+  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * 9 * a.n_rot : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  double *scr = gr.scr + (size_t)b * gr.stride;
+  if (t == 0) scr[kScrLoss] = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
+  if (!a.first) return;
+  // the first step accepts: the diagonal of the trial's keypoint rows, column t of [delta | c | beta], in row order
+  if (t < P) {
+    const float *J = a.tjac + (size_t)b * 3 * K * P, *M = a.tkp + (size_t)b * 3 * K, *cam = a.tlast + (size_t)b * 3;
+    double s, ds;
+    softplus_d((double)cam[0], s, ds);
+    const double cxy[2] = {(double)cam[1], (double)cam[2]};
+    double d = 0.0;
+    for (int r = 0; r < 2 * K; ++r) {
+      double wr, res;
+      lm_kp2d_row(M, tg, wt, s, cxy, robust, s2, r >> 1, r & 1, wr, res);
+      if (!(wr > 0.0)) continue;
+      const double x = lm_kp2d_entry<true>(J, M, P, o, r >> 1, r & 1, t, s, ds, cxy);
+      d += (wr * x) * x;
+    }
+    dg[t] = d;
+  }
+  __syncthreads();
+  if (t == 0) {
+    double m = kDiagFloor;
+    for (int j = 0; j < o + 3; ++j) m = fmax(m, dg[j]);
+    scr[kScrDmax] = m;
+  }
+  if (t < nb) scr[kScrDiag + t] = dg[o + 3 + t];
+}
+
+__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
+  extern __shared__ double A[];         // [P][P]: the lower triangle of the image's normal matrix, then its factor
+  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
+  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
+  __shared__ float lam_s;
+  __shared__ int accept_s, ok_s;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nb = a.nb, nr9 = 9 * a.n_rot;
+  const int o = 3 * a.n_rot, n1 = o + 3;      // first camera and first betas column
+  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  // 2. the group's decision
+  if (t == 0) {
+    int lo = 0, hi = gr.G - 1;            // the group g with off[g] <= b < off[g + 1]
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (gr.off[mid] <= b) lo = mid;
+      else hi = mid - 1;
+    }
+    const LmGroupDecision d = lm_group_decide(a, x2, gr, lo);
+    accept_s = d.accept;
+    lam_s = d.lam;
+    ok_s = 1;
+  }
+  __syncthreads();
+  const bool accept = accept_s;
+  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
+  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
+  const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
+  const float *Cst = (accept ? a.tlast : a.last) + (size_t)b * 3;
+  if (accept) lm_kp_take_trial(a, b, 0.f, false);
+  double s, ds;
+  softplus_d((double)Cst[0], s, ds);
+  const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
+  // 3. the image's normal equations, columns [delta | c | beta]
+  int pr[kLmKpPairs], pc[kLmKpPairs];
+  double acc[kLmKpPairs], g = 0.0;
+  lm_kp_pairs(P, pr, pc, acc);
+  lm_kp2d_keypoint_rows<true>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, o, Js, WJs, ws, rs, pr, pc, acc, g);
+  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
+  lm_kp_store(P, A, y, pr, pc, acc, g);
+  if (t == 0)
+    for (int j = 0; j < n1; ++j) A[j * P + j] += (double)lam_s;
+  // 4. the leading block factored alone: S_i in the trailing block, -s_i in y's tail, -x_i in y's head
+  lm_kp_solve(A, y, P, n1, ok_s);
+  // X_i = A_i^-1 B_i: L11^T X = L21^T in place in the rows n1.. of A, as the solve's L^T delta = y, column by column
+  for (int j = n1 - 1; j >= 0; --j) {
+    for (int l = t; l < nb; l += blockDim.x) A[(n1 + l) * P + j] /= A[j * P + j];
+    __syncthreads();
+    for (int q = t; q < nb * j; q += blockDim.x) {
+      const int l = q / j, i = q % j;
+      A[(n1 + l) * P + i] -= A[j * P + i] * A[(n1 + l) * P + j];
+    }
+    __syncthreads();
+  }
+  double *scr = gr.scr + (size_t)b * gr.stride;
+  double *S = scr + kScrDiag + nb, *sv = S + nb * nb, *X = sv + nb, *xv = X + n1 * nb;
+  for (int q = t; q < nb * nb; q += blockDim.x) {
+    const int r = q / nb, c = q % nb;
+    S[q] = c <= r ? A[(n1 + r) * P + n1 + c] : 0.0;
+  }
+  for (int l = t; l < nb; l += blockDim.x) sv[l] = -y[n1 + l];
+  for (int q = t; q < n1 * nb; q += blockDim.x) X[q] = A[(n1 + q % nb) * P + q / nb];
+  for (int j = t; j < n1; j += blockDim.x) xv[j] = -y[j];
+  if (t == 0) scr[kScrOk] = ok_s ? 1.0 : 0.0;
+}
+
+__global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
+  extern __shared__ double A[];         // [nb][nb]: S + the measurement rows, then its factor; then delta_i (n1)
+  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // the staged measurement rows
+  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
+  __shared__ float lam_s;
+  __shared__ int accept_s, ok_s;
+  const int g = blockIdx.x, t = threadIdx.x, nb = a.nb, o = 3 * a.n_rot, n1 = o + 3, nr9 = 9 * a.n_rot;
+  const int i0 = gr.off[g], i1 = gr.off[g + 1];
+  const LmMeasArgs &mb = x2.mb;
+  if (t == 0) {
+    const LmGroupDecision d = lm_group_decide(a, x2, gr, g);
+    accept_s = d.accept;
+    lam_s = d.lam;
+    if (d.accept) a.loss[g] = d.lnew;
+    a.lambda[g] = d.lam;
+    if (d.accept && !a.first) a.accepted[g] += 1;
+    bool ok = isfinite(d.lnew);         // a group without a finite loss does not move, nor one with a failed block
+    for (int i = i0; i < i1; ++i) ok = ok && gr.scr[(size_t)i * gr.stride + kScrOk] != 0.0;
+    ok_s = ok;
+  }
+  __syncthreads();
+  const bool accept = accept_s;
+  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)g * nb;
+  if (accept) {
+    for (int l = t; l < nb; l += blockDim.x) a.betas[(size_t)g * nb + l] = a.tbetas[(size_t)g * nb + l];
+    if (mb.weights) lm_meas_take_trial(mb, g, nb);
+  }
+  // S = sum_i S_i, s = sum_i s_i in image order, then the measurement rows and betas_w beta
+  int pr[kLmKpPairs], pc[kLmKpPairs];
+  double acc[kLmKpPairs], gs = 0.0;
+  lm_kp_pairs(nb, pr, pc, acc);
+  for (int i = i0; i < i1; ++i) {
+    const double *S = gr.scr + (size_t)i * gr.stride + kScrDiag + nb;
+#pragma unroll
+    for (int q = 0; q < kLmKpPairs; ++q)
+      if (pr[q] >= 0) acc[q] += S[pr[q] * nb + pc[q]];
+    if (t < nb) gs += S[nb * nb + t];
+  }
+  if (mb.weights)
+    lm_meas_add_rows(mb, g, nb, 0, (accept ? mb.tmeas : mb.meas) + (size_t)g * 5,
+                     (accept ? mb.tjac : mb.jac) + (size_t)g * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, gs);
+  if (x2.betas_w > 0.f && t < nb) gs += (double)x2.betas_w * (double)Bst[t];
+  lm_kp_store(nb, A, y, pr, pc, acc, gs);
+  if (t == 0) {
+    const double damp = (double)x2.betas_w + (double)lam_s;
+    for (int j = 0; j < nb; ++j) A[j * nb + j] += damp;
+  }
+  lm_kp_solve(A, y, nb, nb, ok_s);
+  const bool ok = ok_s;
+  // the next trial of every image: delta_i = -x_i - X_i dbeta, then R Exp(delta), c + delta_c, beta + dbeta
+  double *dv = A + nb * nb;
+  for (int i = i0; i < i1; ++i) {
+    const double *X = gr.scr + (size_t)i * gr.stride + kScrDiag + 2 * nb + nb * nb, *xv = X + n1 * nb;
+    for (int j = t; j < n1; j += blockDim.x) {
+      double v = -xv[j];
+      for (int l = 0; l < nb; ++l) v -= X[j * nb + l] * y[l];
+      dv[j] = v;
+    }
+    __syncthreads();
+    for (int j = t; j < a.n_rot; j += blockDim.x) {
+      const float *Rs = a.rot + (size_t)i * nr9 + 9 * j;
+      float *Rt = a.trot + (size_t)i * nr9 + 9 * j;
+      if (ok) lm_exp_gs(Rs, dv[3 * j], dv[3 * j + 1], dv[3 * j + 2], Rt);
+      else
+        for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
+    }
+    if (t < 3) {
+      const float x = a.last[(size_t)i * 3 + t];
+      a.tlast[(size_t)i * 3 + t] = ok ? (float)((double)x + dv[o + t]) : x;
+    }
+    for (int l = t; l < nb; l += blockDim.x)
+      gr.tbetas_img[(size_t)i * nb + l] = ok ? (float)((double)Bst[l] + y[l]) : Bst[l];
+    __syncthreads();
+  }
+  for (int l = t; l < nb; l += blockDim.x) {
+    const float x = Bst[l];
+    a.tbetas[(size_t)g * nb + l] = ok ? (float)((double)x + y[l]) : x;
+  }
+}
+
+// The grouped entries' checks (check_lm_kp's, then the offsets, read on the host) and the three launches; the offsets
+// are copied into the workspace on the stream
+int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpArgs a, LmKp2dArgs x,
+                 float *tbetas_img, void *workspace, bool extra_ok, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, extra_ok && offsets && tbetas_img && workspace,
+                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f,
+                             "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                             "lambda_down >= 1");
+  if (rc != SHAPY_OK) return rc;
+  SHAPY_REQUIRE(G >= 0 && offsets[0] == 0 && offsets[G] == batch,
+                "%s: group_offsets must run from 0 to the batch (%d) over %d groups", fn, batch, G);
+  for (int g = 0; g < G; ++g)
+    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: group %d is empty (offsets %d, %d)", fn, g, offsets[g],
+                  offsets[g + 1]);
+  if (batch == 0) return SHAPY_OK;
+  const int n1 = 3 * a.n_rot + 3, nb = a.nb;
+  int *off = (int *)workspace;
+  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_group_stride(n1, nb),
+                 tbetas_img};
+  cudaStream_t st = (cudaStream_t)stream;
+  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  lm_kp2dg_loss_kernel<<<batch, 128, 0, st>>>(a, x, gr);
+  SHAPY_LAUNCH_CHECK();
+  const size_t smem = (size_t)a.P * a.P * sizeof(double);
+  cudaFuncAttributes attr;
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_image_kernel));
+  if (smem + attr.sharedSizeBytes > 48 * 1024)
+    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2dg_image_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  lm_kp2dg_image_kernel<<<batch, kLmKpThreads, smem, st>>>(a, x, gr);
+  SHAPY_LAUNCH_CHECK();
+  const size_t smem3 = (size_t)(nb * nb + n1) * sizeof(double);
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_group_kernel));
+  if (smem3 + attr.sharedSizeBytes > 48 * 1024)
+    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2dg_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+  lm_kp2dg_group_kernel<<<G, kLmKpThreads, smem3, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
@@ -832,4 +1193,42 @@ extern "C" int shapy_fit_lm_keypoints_2d_measurements_step(
                    "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                    "lambda_down >= 1",
                    stream);
+}
+
+extern "C" size_t shapy_fit_lm_groups_workspace_bytes(int batch, int num_groups, int n_rot, int nb) {
+  if (batch < 0 || num_groups < 0 || n_rot < 1 || nb < 1) return 0;
+  return lm_group_offsets_bytes(num_groups) + (size_t)batch * lm_group_stride(3 * n_rot + 3, nb) * sizeof(double);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_groups_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *camera,
+    float *keypoints, float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_betas_images, float *trial_camera, const float *trial_keypoints, const float *trial_jac,
+    void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
+  return run_lm_kp2dg("shapy_fit_lm_keypoints_2d_groups_step", batch, num_groups, group_offsets, a, x,
+                      trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_groups_measurements_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
+    const float *trial_meas_jac, void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
+               LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
+  return run_lm_kp2dg("shapy_fit_lm_keypoints_2d_groups_measurements_step", batch, num_groups, group_offsets, a, x,
+                      trial_betas_images, workspace,
+                      (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
+                          meas_jac && trial_meas && trial_meas_jac,
+                      stream);
 }

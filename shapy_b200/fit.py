@@ -69,11 +69,21 @@ fix a body's proportions and not its metric size: a known height removes that fr
 tissue no joint sees.  With method='lm' each iteration is four launches (the keypoint Jacobian, forward_shape and the
 measurement Jacobian of the trial, then ops.fit_lm_keypoints_2d_measurements_step), none synchronising.
 
+fit_body_to_keypoints_2d(..., groups=labels) fits several images of one person with one shape: images with the same
+label 0 .. G-1 share their betas, each keeps its pose and camera, and the loss of a group is the sum of its images'
+2D losses + its measurement terms + betas_weight |betas|^2.  A bone foreshortened in one view is seen at full length in
+another, and every view must agree on the same proportions.  With method='lm' each iteration is the keypoint Jacobian
+of every image and ops.fit_lm_keypoints_2d_groups_step, whose three launches eliminate each image's pose and camera
+block (a Schur complement) and solve for the group's betas (six launches with measurements), no host synchronisation,
+every group's loss non-increasing.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
 With --keypoints-2d, known measurements are read from --targets only (per-body arrays height / mass / ...); --height
 and the other single-target flags are not used there, so a command line without --targets fits the keypoints alone.
+An optional `groups` array (B,) in kp.npz fits the images of one label with one shape; the --targets arrays are then
+per group, and the output carries `groups`.
 
 shapy_b200.keypoints2d reads OpenPose detections and maps them into that frame; with raw detections and their crop
 descriptors in kp.npz, --keypoint-map openpose_smplx_map.json does the same on the command line.
@@ -435,10 +445,49 @@ def _init_2d(init, B, nb, device, method):
     return _start_params(init, B, nb, device, method, 'camera', 0.9)   # softplus(0.9) ~ 1.24, the regressor's mean scale
 
 
+def group_plan(groups, B):
+    """The images of each group, from labels (B,) of integers 0 .. G-1, each used at least once: (order (B,) int64, the
+    stable sort of the labels, so that the caller's order within a group is kept; offsets (G + 1,) int32, group g the
+    sorted images [offsets[g], offsets[g + 1])), both on the CPU.  Labels on the device are read once on the host
+    (one synchronisation, before any fit loop); labels on the CPU cost none."""
+    g = torch.as_tensor(groups).detach().cpu()
+    if g.dtype.is_floating_point or g.dtype == torch.bool or g.dtype.is_complex or g.shape != (B,):
+        raise ValueError(f'groups must be a ({B},) integer tensor, got {g.dtype} {tuple(g.shape)}')
+    g = g.long()
+    if B and int(g.min()) < 0:
+        raise ValueError('groups: labels must be >= 0')
+    counts = torch.bincount(g) if B else torch.zeros(0, dtype=torch.long)
+    if bool((counts == 0).any()):
+        raise ValueError(f'groups: labels must be 0 .. G-1, each used at least once; label {int((counts == 0).nonzero()[0])} '
+                         f'is not used')
+    order = torch.sort(g, stable=True).indices
+    offsets = torch.cat([torch.zeros(1, dtype=torch.long), counts.cumsum(0)]).to(torch.int32)
+    return order, offsets
+
+
+def _to_device(t, device):
+    """A host tensor on `device` without synchronising (a non-blocking copy from pinned memory)."""
+    if torch.device(device).type != 'cuda':
+        return t.to(device)
+    return t.pin_memory().to(device, non_blocking=True)
+
+
+def _group_sum(x, offsets):
+    """Per group, the sum of the rows of x (sorted by group) in image order, left to right: (G, ...)."""
+    off = offsets.long()
+    cnt = off[1:] - off[:-1]
+    start, cnt_d = _to_device(off[:-1], x.device), _to_device(cnt, x.device)
+    acc = x[start]
+    for j in range(1, int(cnt.max()) if cnt.numel() else 0):
+        more = (cnt_d > j).view(-1, *([1] * (x.dim() - 1)))
+        acc = torch.where(more, acc + x[(start + j).clamp(max=x.shape[0] - 1)], acc)
+    return acc
+
+
 def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
                              robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
                              body_measurements=None, measurements=None, measurement_weights=None,
-                             circumference_derivative='reference'):
+                             circumference_derivative='reference', groups=None):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -461,7 +510,13 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'camera', 'global_rot_mat' (B, 1, 3, 3), 'body_pose_mat'
     (B, 21, 3, 3), 'keypoints' (B, K, 3) and 'proj_joints' (B, K, 2) of the final parameters, 'loss' (B,)}, with
     measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss' the
-    total."""
+    total.
+    groups: None, or (B,) integer labels 0 .. G-1, each used at least once: images with the same label are one person
+    and share their betas.  init, weights and pose_anchor stay per image; a group starts from the mean of its images'
+    init betas (image order).  measurements and measurement_weights are then per group ((G,) values or scalars).
+    'betas' (G, NB), 'measurements' (G, 5) and 'loss' (G,) are per group, the rest per image in the caller's order.
+    With 'lm' the returned loss is the step's fp64 loss of the final state; the images of a group are summed in the
+    caller's order."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
     exact_circumferences(circumference_derivative)
@@ -493,6 +548,10 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                                                               device=device).reshape(B, 22, 3, 3).contiguous()
     sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
     pw, bw = float(pose_prior_weight), float(betas_weight)
+    if groups is not None:
+        return _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, int(iterations), sigma, pw, bw,
+                                        lr, groups, body_measurements, measurements, measurement_weights,
+                                        circumference_derivative)
     mterms = None
     if measurements is not None:
         tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
@@ -565,6 +624,97 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
     res = _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
     if mterms is not None:
         res['measurements'] = state['meas']
+    return res
+
+
+def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, iterations, sigma, pw, bw, lr, groups,
+                             body_measurements, measurements, measurement_weights, cd):
+    """fit_body_to_keypoints_2d with groups: the images sorted by group once, fitted, and returned in the caller's
+    order."""
+    from . import ops
+    from .autograd import Rot6dFunction
+    device = x.device
+    B, K = x.shape[0], x.shape[1]
+    order, offsets = group_plan(groups, B)
+    G, nb = offsets.numel() - 1, params['betas'].shape[1]
+    counts = (offsets[1:] - offsets[:-1]).long()
+    od = _to_device(order, device)
+    inv = torch.argsort(od)
+    gidx = _to_device(torch.repeat_interleave(torch.arange(G), counts), device)     # each sorted image's group
+    x, w, rot0, anchor = x[od].contiguous(), w[od].contiguous(), rot0[od].contiguous(), anchor[od].contiguous()
+    sp = {k: v.detach()[od].contiguous() for k, v in params.items()}
+    cnt = _to_device(counts.float(), device)
+    betas0 = (_group_sum(sp['betas'], offsets) / cnt[:, None]).contiguous() if G else torch.zeros(0, nb, device=device)
+    mterms = None
+    if measurements is not None:
+        tgt, wt = _measurement_terms(measurements, measurement_weights, G, device)
+        mterms = (tgt.contiguous(), wt.contiguous())
+    packed = body_model.packed(device)
+    faces = body_model.faces_i32
+    if method == 'lm':
+        trial = {'rot': rot0.clone(), 'betas': betas0, 'image_betas': betas0[gidx].contiguous(),
+                 'camera': sp['camera']}
+        state = _kp_lm_state(B, K, 22, nb, 'camera', device)
+        mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+        state.update({'betas': mk(G, nb), 'loss': mk(G), 'lambda': mk(G),     # per group
+                      'accepted': torch.zeros(G, dtype=torch.int32, device=device)})
+        if mterms is not None:
+            state.update(meas=mk(G, 5), meas_jac=mk(G, 5, nb))
+        pose_anchor = anchor if pw > 0 else None
+        if B > 0:
+            ws = ops.fit_lm_groups_workspace(B, G, 22, nb, device)
+            exact = exact_circumferences(cd)
+            lm = body_measurements.landmarks() if mterms is not None else None
+            if mterms is not None:
+                ops.face_incidence(faces)      # built (one copy to the host) before the loop, which never synchronises
+            for it in range(iterations + 1):
+                tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['image_betas'], trial['rot'])
+                if mterms is None:
+                    ops.fit_lm_keypoints_2d_groups_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0,
+                                                        tkp, tjac, offsets, ws, pose_anchor=pose_anchor)
+                else:
+                    v = ops.smplx_forward_shape(packed, trial['betas'])
+                    tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
+                    ops.fit_lm_keypoints_2d_groups_measurements_step(
+                        state, trial, x, w, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0, tkp, tjac,
+                        tm, tmj, offsets, ws, pose_anchor=pose_anchor)
+        rot = state['rot']
+        with torch.no_grad():
+            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'][gidx],
+                             camera=state['camera'], return_shaped=False)
+        res = _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'],
+                            loss=state['loss'])
+        if mterms is not None:
+            res['measurements'] = state['meas']
+    else:
+        p = {k: sp[k].clone().requires_grad_(True) for k in ('global_rot', 'body_pose', 'camera')}
+        p['betas'] = betas0.clone().requires_grad_(True)
+
+        def loss_fn():
+            grot = Rot6dFunction.apply(p['global_rot'])
+            bpose = Rot6dFunction.apply(p['body_pose'])
+            out = body_model(global_rot=grot, body_pose=bpose, betas=p['betas'][gidx], camera=p['camera'],
+                             return_shaped=False)
+            rot = torch.cat([grot, bpose], 1)
+            per_group = _group_sum(_kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, 0.0, None), offsets)
+            meas = None
+            if mterms is not None:
+                v = body_model.forward_shape(betas=p['betas'])['v_shaped']
+                m = body_measurements.forward_vertices(v, faces, cd)['measurements']
+                meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+                per_group = per_group + _measurement_loss(mterms[0], mterms[1], meas, p['betas'], 0.0)
+            if bw > 0:
+                per_group = per_group + bw * p['betas'].pow(2).sum(1)
+            return per_group, out, grot, bpose, meas
+
+        per_group, out, grot, bpose, meas = _adam(list(p.values()), lr, iterations, loss_fn)
+        res = {k: v.detach() for k, v in p.items()}
+        res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:],
+                   proj_joints=out['proj_joints'], loss=per_group)
+        if meas is not None:
+            res['measurements'] = meas
+    for k in ('global_rot', 'body_pose', 'camera', 'global_rot_mat', 'body_pose_mat', 'keypoints', 'proj_joints'):
+        res[k] = res[k][inv]
     return res
 
 
@@ -661,11 +811,14 @@ def _main_keypoints_2d(a, model, bm, targets):
         init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(x.shape[0], -1)
                 for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera')
                 if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+    groups = d['groups'].astype(np.int64).reshape(-1) if 'groups' in d.files else None
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
-                                   circumference_derivative=a.circumference_derivative)
+                                   circumference_derivative=a.circumference_derivative, groups=groups)
     out = {k: v.detach().cpu().numpy() for k, v in res.items()}
+    if groups is not None:
+        out['groups'] = groups
     np.savez(a.output, **out)
     print(json.dumps({'bodies': int(x.shape[0]), 'output': a.output, 'median_loss': float(np.median(out['loss']))}))
 

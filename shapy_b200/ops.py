@@ -773,3 +773,98 @@ def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=
         check(lib().shapy_conv_test(C.byref(d), ptr(x), ptr(res), B, H, W, int(relu), mode, engine, ptr(y),
                                     stream_ptr()), 'conv_test')
     return y
+
+
+def fit_lm_groups_workspace(B, G, n_rot, nb, device):
+    """The scratch of the grouped 2D step (include/shapy_b200.h, shapy_fit_lm_groups_workspace_bytes): a uint8 CUDA
+    tensor, allocated once before an LM loop."""
+    n = lib().shapy_fit_lm_groups_workspace_bytes(int(B), int(G), int(n_rot), int(nb))
+    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+
+
+def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
+                        lambda_down, first, trial_keypoints, trial_jac, group_offsets, workspace, pose_anchor,
+                        meas=None):
+    """What the two grouped 2D steps share: the checks and the call, `meas` None or (meas_targets, meas_weights,
+    trial_meas, trial_meas_jac), all (G, ...)."""
+    B, n_rot = trial['rot'].shape[:2]
+    nb, K = trial['betas'].shape[1], targets.shape[1]
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    off = group_offsets
+    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
+            off.is_contiguous()):
+        raise RuntimeError(f'{what}: group_offsets must be a contiguous (G + 1,) int32 CPU tensor')
+    G = off.numel() - 1
+    if G < 0 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
+        raise ValueError(f'{what}: group_offsets must rise strictly from 0 to the batch ({B})')
+    anchor = [] if pose_anchor is None else [pose_anchor]
+    mstate = [] if meas is None else [state['meas'], state['meas_jac']]
+    ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
+        [trial[k] for k in ('rot', 'betas', 'image_betas', 'camera')] + [targets, weights, trial_keypoints,
+                                                                         trial_jac] + anchor + list(meas or ())
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights and anchor', state['accepted'])
+    P = 3 * n_rot + nb + 3
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
+        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
+    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if (state['betas'].shape != (G, nb) or trial['betas'].shape != (G, nb) or trial['image_betas'].shape != (B, nb) or
+            any(state[k].shape != (G,) for k in ('loss', 'lambda', 'accepted'))):
+        raise RuntimeError(f'{what}: betas and trial betas must be ({G}, {nb}), image_betas ({B}, {nb}) and loss, '
+                           f'lambda and accepted ({G},)')
+    if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], G, nb):
+        raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
+                           f'({G}, 5)')
+    need = lib().shapy_fit_lm_groups_workspace_bytes(B, G, n_rot, nb)
+    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
+        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    if B == 0:
+        return
+    head = [B, G, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma,
+            float(pose_prior_weight), float(betas_weight)]
+    lam = [float(lambda_up), float(lambda_down), int(bool(first))]
+    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['image_betas']), ptr(trial['camera']),
+          ptr(trial_keypoints), ptr(trial_jac)]
+    with torch.cuda.device(trial['rot'].device):
+        if meas is None:
+            check(lib().shapy_fit_lm_keypoints_2d_groups_step(
+                *head, *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+                *tr, ptr(workspace), stream_ptr()), what)
+        else:
+            check(lib().shapy_fit_lm_keypoints_2d_groups_measurements_step(
+                *head, ptr(meas[0]), ptr(meas[1]), *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
+                                          'lambda', 'accepted')],
+                *tr, ptr(meas[2]), ptr(meas[3]), ptr(workspace), stream_ptr()), what)
+
+
+def fit_lm_keypoints_2d_groups_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight,
+                                    lambda_up, lambda_down, first, trial_keypoints, trial_jac, group_offsets,
+                                    workspace, pose_anchor=None):
+    """One Levenberg-Marquardt step of the 2D fit over groups of images sharing their betas (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_groups_step), in place.  group_offsets: (G + 1,) int32 CPU tensor, group g the images
+    [off[g], off[g + 1]).  state: fit_lm_keypoints_2d_step's, with 'betas' (G, NB), 'loss', 'lambda', 'accepted' (G,);
+    trial: {'rot' (B, n_rot, 3, 3), 'betas' (G, NB), 'image_betas' (B, NB) (each image's group betas, what
+    smplx_keypoint_jacobian evaluated), 'camera' (B, 3)}, the evaluated trial on entry and the next on return;
+    workspace from fit_lm_groups_workspace.  Three launches, no host synchronisation."""
+    _fit_lm_kp2d_groups('fit_lm_keypoints_2d_groups_step', state, trial, targets, weights, robust_sigma,
+                        pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                        group_offsets, workspace, pose_anchor)
+
+
+def fit_lm_keypoints_2d_groups_measurements_step(state, trial, targets, weights, robust_sigma, pose_prior_weight,
+                                                 betas_weight, meas_targets, meas_weights, lambda_up, lambda_down,
+                                                 first, trial_keypoints, trial_jac, trial_meas, trial_meas_jac,
+                                                 group_offsets, workspace, pose_anchor=None):
+    """fit_lm_keypoints_2d_groups_step with the five measurements of each group (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_groups_measurements_step), in place.  state adds 'meas' (G, 5) and 'meas_jac'
+    (G, 5, NB); meas_targets, meas_weights (G, 5); trial_meas (G, 5) / trial_meas_jac (G, 5, NB) from
+    measure_jacobian_betas at the G trial betas."""
+    _fit_lm_kp2d_groups('fit_lm_keypoints_2d_groups_measurements_step', state, trial, targets, weights, robust_sigma,
+                        pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                        group_offsets, workspace, pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac))

@@ -1,0 +1,473 @@
+"""GPU: the grouped 2D keypoint Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_groups_step and its measurements
+entry) against its NumPy restatement (tests/kp2dg_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_groups_cpu.py), groups
+of one against shapy_fit_lm_keypoints_2d_step, dropped measurements against the plain entry; and
+fit_body_to_keypoints_2d(groups=) end to end on the synthetic SMPL-X: deterministic, group independent, monotone, never
+synchronising, four (six) launches per iteration, and the quality of one shape fitted from four views."""
+import math
+
+import numpy as np
+import pytest
+import torch
+
+import kp2d_lm_oracle as o2
+import kp2dg_lm_oracle as og
+from kpm_lm_oracle import meas_loss
+from test_gpu_fit_lm_kp2d_meas import NAMES, N_ROT, _bits, _measure, _rodrigues, model  # noqa: F401
+from test_gpu_fit_lm_kp2d_meas import quality as quality_2d
+
+pytestmark = pytest.mark.gpu
+TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
+SIZES = (1, 2, 3, 5)
+
+
+# ------------------------------------------------------------------------------------------------ step
+def _eval(packed, rot, betas):
+    from shapy_b200 import ops
+    kp, jac = ops.smplx_keypoint_jacobian(packed, betas.cuda().contiguous(), rot.cuda().contiguous())
+    return kp.cpu(), jac.cpu()
+
+
+def _group_case(model, terms, exact=False, sizes=SIZES, seed=43):
+    """Groups of `sizes` images: group 0 targets the trial (accepted), 1 the state with the priors on its side and a
+    worse trial camera (rejected), 2 the trial (accepted), 3 noisy targets.  Keypoint 7 has weight 0 and NaN targets,
+    keypoints and rows in state and trial; measurement 2 of group 2 is dropped with NaN values and rows."""
+    from shapy_b200 import ops
+    smplx, bm = model
+    sigma, pw, bw = terms
+    packed, faces, lm = smplx.packed(), smplx.faces_i32, bm.landmarks()
+    G, B = len(sizes), sum(sizes)
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
+    gidx = torch.repeat_interleave(torch.arange(G), torch.tensor(sizes))
+    gen = torch.Generator().manual_seed(seed)
+    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
+    rot = _rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
+    betas = rn(G, 10).clamp(-2, 2)
+    cam = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
+    trot = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.02)).float()
+    anchor = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.05)).float()
+    tbetas, tcam = betas + 0.05 * rn(G, 10), cam + 0.01 * rn(B, 3)
+    for g in (0, 2):
+        tbetas[g] = 0.9 * betas[g]
+    tbetas[1] = 1.1 * betas[1]
+    r1 = slice(off[1], off[2])
+    tcam[r1, 1] += 0.05
+    kp, jac = _eval(packed, rot, betas[gidx])
+    tkp, tjac = _eval(packed, trot, tbetas[gidx])
+    ops.face_incidence(faces)
+    m = [t.cpu() for t in ops.measure_jacobian_betas(packed, lm, ops.smplx_forward_shape(packed, betas.cuda()), faces,
+                                                     exact=exact)[:2]]
+    tm = [t.cpu() for t in ops.measure_jacobian_betas(packed, lm, ops.smplx_forward_shape(packed, tbetas.cuda()),
+                                                      faces, exact=exact)[:2]]
+    K = packed.K
+    proj = lambda k, c: torch.stack([torch.from_numpy(o2.project(k[b].numpy(), c[b].numpy())).float()  # noqa: E731
+                                     for b in range(B)])
+    ps, pt = proj(kp, cam), proj(tkp, tcam)
+    tg = ps + 0.02 * rn(B, K, 2)
+    mt = tm[0] * (1 + 0.02 * rn(G, 5))
+    for g in (0, 2):
+        r = slice(off[g], off[g + 1])
+        tg[r], anchor[r], mt[g] = pt[r], trot[r], tm[0][g]
+    tg[r1], anchor[r1], mt[1] = ps[r1], rot[r1], m[0][1]
+    w = torch.rand(B, K, generator=gen) + 0.5
+    w[:, 7] = 0.0
+    tg[:, 7] = float('nan')
+    for t in (kp, tkp):
+        t[:, 7] = float('nan')
+    for t in (jac, tjac):
+        t[:, 21:24] = float('nan')
+    mw = torch.tensor([1.0, 100.0, 2000.0, 1000.0, 1000.0]).repeat(G, 1)
+    mw[2, 2] = 0.0
+    for t in (m[0], tm[0], m[1], tm[1]):
+        t[2, 2] = float('nan')
+    return dict(off=off, gidx=gidx, rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, meas=m[0], mjac=m[1], trot=trot,
+                tbetas=tbetas, tcam=tcam, tkp=tkp, tjac=tjac, tmeas=tm[0], tmjac=tm[1], tg=tg, w=w, mt=mt, mw=mw,
+                anchor=anchor, lam=torch.rand(G, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
+
+
+def _state_loss(c, g, with_meas):
+    n = lambda t: t.numpy()  # noqa: E731
+    L = 0.0
+    for i in range(c['off'][g], c['off'][g + 1]):
+        L += o2.loss(n(c['tg'][i]), n(c['w'][i]), n(c['kp'][i]), n(c['cam'][i]), c['sigma'], n(c['rot'][i]),
+                     n(c['anchor'][i]), c['pw'])
+    if with_meas:
+        L += meas_loss(n(c['mt'][g]), n(c['mw'][g]), n(c['meas'][g]))
+    if c['bw'] > 0:
+        L += float(np.float32(c['bw'])) * float(np.sum(n(c['betas'][g]).astype(np.float64) ** 2))
+    return L
+
+
+def _device(c, with_meas):
+    G = len(c['off']) - 1
+    B = c['rot'].shape[0]
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    loss = torch.tensor([_state_loss(c, g, with_meas) for g in range(G)]).float()
+    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
+             'jac': cu(c['jac']), 'loss': cu(loss), 'lambda': cu(c['lam']),
+             'accepted': torch.zeros(G, dtype=torch.int32, device='cuda')}
+    if with_meas:
+        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
+    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'image_betas': cu(c['tbetas'][c['gidx']]),
+             'camera': cu(c['tcam'])}
+    return state, trial, B, G
+
+
+def _groups_step(c, state, trial, first, with_meas):
+    from shapy_b200 import ops
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    B, G = c['rot'].shape[0], len(c['off']) - 1
+    ws = ops.fit_lm_groups_workspace(B, G, N_ROT, 10, 'cuda')
+    off = torch.from_numpy(c['off'])
+    if with_meas:
+        ops.fit_lm_keypoints_2d_groups_measurements_step(
+            state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], cu(c['mt']), cu(c['mw']), 10.0, 3.0,
+            first, cu(c['tkp']), cu(c['tjac']), cu(c['tmeas']), cu(c['tmjac']), off, ws, pose_anchor=cu(c['anchor']))
+    else:
+        ops.fit_lm_keypoints_2d_groups_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0,
+                                            3.0, first, cu(c['tkp']), cu(c['tjac']), off, ws,
+                                            pose_anchor=cu(c['anchor']))
+
+
+@pytest.mark.parametrize('meas', [None, 'reference', 'exact'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+def test_step_kernels_vs_oracle(model, first, terms, meas):
+    c = _group_case(model, terms, exact=meas == 'exact')
+    with_meas = meas is not None
+    state, trial, B, G = _device(c, with_meas)
+    s0 = {k: v.cpu().numpy() for k, v in state.items()}
+    _groups_step(c, state, trial, first, with_meas)
+    got = {k: v.cpu().numpy() for k, v in state.items()}
+    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
+    n = lambda t: t.numpy()  # noqa: E731
+    flags, worst = [], 0.0
+    for g in range(G):
+        r = range(c['off'][g], c['off'][g + 1])
+        st = {k: [s0[k2][i] for i in r] for k, k2 in (('rot', 'rot'), ('camera', 'camera'), ('keypoints', 'keypoints'),
+                                                        ('jac', 'jac'))}
+        st.update(betas=s0['betas'][g], loss=s0['loss'][g], accepted=0, **{'lambda': s0['lambda'][g]})
+        if with_meas:
+            st.update(meas=s0['meas'][g], meas_jac=s0['meas_jac'][g])
+        images = [{'targets': n(c['tg'][i]), 'weights': n(c['w'][i]), 'anchor': n(c['anchor'][i]),
+                   'trial_kp': n(c['tkp'][i]), 'trial_jac': n(c['tjac'][i])} for i in r]
+        tr = {'rot': [n(c['trot'][i]) for i in r], 'camera': [n(c['tcam'][i]) for i in r],
+              'betas': n(c['tbetas'][g])}
+        mb = None if not with_meas else {'targets': n(c['mt'][g]), 'weights': n(c['mw'][g]),
+                                         'trial_meas': n(c['tmeas'][g]), 'trial_meas_jac': n(c['tmjac'][g])}
+        new, want, acc, _, _ = og.lm_groups_step(st, images, 10.0, 3.0, first, tr, c['sigma'], c['pw'], c['bw'], mb)
+        flags.append(acc)
+        assert got['accepted'][g] == new['accepted'], g
+        assert np.isclose(got['lambda'][g], new['lambda'], rtol=3e-7, atol=0), (g, got['lambda'][g], new['lambda'])
+        assert np.isclose(got['loss'][g], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (g, got['loss'][g],
+                                                                                          new['loss'])
+        assert np.array_equal(got['betas'][g], new['betas'], equal_nan=True), g
+        if with_meas:
+            for k in ('meas', 'meas_jac'):
+                assert np.array_equal(got[k][g], new[k], equal_nan=True), (g, k)
+        for j, i in enumerate(r):
+            for k in ('rot', 'camera', 'keypoints', 'jac'):
+                assert np.array_equal(got[k][i], new[k][j], equal_nan=True), (g, i, k)
+            for k in ('rot', 'camera'):
+                bar = 2e-6 * max(1.0, np.abs(want[k][j]).max())
+                err = np.abs(nxt[k][i] - want[k][j]).max()
+                assert err <= bar, (g, i, k, err)
+                worst = max(worst, err / bar)
+            assert np.array_equal(nxt['image_betas'][i], nxt['betas'][g])
+        bar = 2e-6 * max(1.0, np.abs(want['betas']).max())
+        err = np.abs(nxt['betas'][g] - want['betas']).max()
+        assert err <= bar, (g, 'betas', err)
+        worst = max(worst, err / bar)
+    if first:
+        assert all(flags)
+    else:
+        assert flags[:3] == [True, False, True], flags
+    print(f'[kp2dg] step first={first} terms={terms} meas={meas}: accepted {flags}, trial error / bar {worst:.3f}')
+
+
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+def test_groups_of_one_equal_the_2d_step(model, first, terms):
+    """Eight groups of one: loss, lambda, accepted and the state bit for bit as shapy_fit_lm_keypoints_2d_step; the
+    next trial within 4e-6 max(1, |x|) (the CPU oracle test bounds the two eliminations' fp64 difference by 1e-10; what
+    is left is the fp32 rounding of the result)."""
+    from shapy_b200 import ops
+    c = _group_case(model, terms, sizes=(1,) * 8)
+    state, trial, B, G = _device(c, False)
+    b_state = {k: v.clone() for k, v in state.items()}
+    b_trial = {k: v.clone() for k, v in trial.items() if k != 'image_betas'}
+    _groups_step(c, state, trial, first, False)
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    ops.fit_lm_keypoints_2d_step(b_state, b_trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
+                                 first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
+    for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
+        assert torch.equal(_bits(state[k]), _bits(b_state[k])), k
+    for k in ('rot', 'betas', 'camera'):
+        err = (trial[k] - b_trial[k]).abs().max()
+        assert float(err) <= 4e-6 * max(1.0, float(b_trial[k].abs().max())), (k, float(err))
+
+
+@pytest.mark.parametrize('first', [False, True])
+def test_dropped_measurements_equal_the_plain_groups_step_bit_for_bit(model, first):
+    c = _group_case(model, TERMS[1])
+    for k in ('meas', 'tmeas', 'mjac', 'tmjac'):
+        c[k][:] = float('nan')
+    c['mw'][:] = 0.0
+    c['mw'][:, 1] = -1.0
+    a_state, a_trial, _, _ = _device(c, True)
+    b_state = {k: v.clone() for k, v in a_state.items() if k not in ('meas', 'meas_jac')}
+    b_trial = {k: v.clone() for k, v in a_trial.items()}
+    _groups_step(c, a_state, a_trial, first, True)
+    _groups_step(c, b_state, b_trial, first, False)
+    for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
+        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
+    for k in ('rot', 'betas', 'image_betas', 'camera'):
+        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+
+
+def test_argument_errors_and_empty_batch(model):
+    from shapy_b200 import _lib, ops
+    module, bm = model
+    L = _lib.lib()
+    K = module.packed().K
+    z = lambda *s: torch.zeros(*s, device='cuda')  # noqa: E731
+    torch.cuda.synchronize()
+    n0 = L.shapy_launch_count()
+
+    def step(B=3, off=(0, 1, 3), n_rot=22, nb=10, null=None, meas=False):
+        G = len(off) - 1
+        P = 3 * n_rot + nb + 3
+        ws = z(max(1, L.shapy_fit_lm_groups_workspace_bytes(B, max(G, 0), n_rot, nb) // 4 + 1))
+        o = torch.tensor(off, dtype=torch.int32)
+        p = [_lib.ptr(t) for t in (z(B, n_rot, 3, 3), z(G, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P))]
+        mp = [_lib.ptr(z(G, 5)), _lib.ptr(z(G, 5, nb))]
+        p2 = [_lib.ptr(t) for t in (z(G), z(G), torch.zeros(G, dtype=torch.int32, device='cuda'))]
+        q = [_lib.ptr(t) for t in (z(B, n_rot, 3, 3), z(G, nb), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P))]
+        head = [B, G, None if null == 'offsets' else o.data_ptr(), K, n_rot, nb, _lib.ptr(z(B, K, 2)),
+                _lib.ptr(z(B, K)), None, 1.0, 0.0, 0.0]
+        if null == 'jac':
+            p[4] = None
+        if null == 'image_betas':
+            q[2] = None
+        wsp = None if null == 'workspace' else _lib.ptr(ws)
+        if meas:
+            mq = [_lib.ptr(z(G, 5)), None if null == 'trial_meas_jac' else _lib.ptr(z(G, 5, nb))]
+            return L.shapy_fit_lm_keypoints_2d_groups_measurements_step(
+                *head, _lib.ptr(z(G, 5)), _lib.ptr(z(G, 5)), 10.0, 3.0, 1, *p, *mp, *p2, *q, *mq, wsp, None)
+        return L.shapy_fit_lm_keypoints_2d_groups_step(*head, 10.0, 3.0, 1, *p, *p2, *q, wsp, None)
+    assert step(n_rot=30) == -3                     # P = 103 > 96
+    for kw in (dict(null='jac'), dict(null='offsets'), dict(null='workspace'), dict(null='image_betas'),
+               dict(null='trial_meas_jac', meas=True), dict(off=(0, 1, 2)), dict(off=(1, 3)), dict(off=(0, 3, 3)),
+               dict(off=(0, 2, 1, 3)), dict(n_rot=0)):
+        assert step(**kw) == -1, kw
+    st = {'rot': z(0, 22, 3, 3), 'betas': z(0, 10), 'camera': z(0, 3), 'keypoints': z(0, K, 3),
+          'jac': z(0, 3 * K, 79), 'loss': z(0), 'lambda': z(0), 'accepted': torch.zeros(0, dtype=torch.int32,
+                                                                                         device='cuda')}
+    tr = {'rot': z(0, 22, 3, 3), 'betas': z(0, 10), 'image_betas': z(0, 10), 'camera': z(0, 3)}
+    ws = ops.fit_lm_groups_workspace(0, 0, 22, 10, 'cuda')
+    off0 = torch.zeros(1, dtype=torch.int32)
+    ops.fit_lm_keypoints_2d_groups_step(st, tr, z(0, K, 2), z(0, K), None, 0.0, 0.0, 10.0, 3.0, True, z(0, K, 3),
+                                        z(0, 3 * K, 79), off0, ws)
+    assert L.shapy_launch_count() == n0            # batch 0: nothing launched
+    with pytest.raises(ValueError):                # offsets that do not end at the batch
+        ops.fit_lm_keypoints_2d_groups_step(st, tr, z(0, K, 2), z(0, K), None, 0.0, 0.0, 10.0, 3.0, True, z(0, K, 3),
+                                            z(0, 3 * K, 79), torch.tensor([0, 1], dtype=torch.int32), ws)
+    with pytest.raises(RuntimeError):              # offsets on the device
+        ops.fit_lm_keypoints_2d_groups_step(st, tr, z(0, K, 2), z(0, K), None, 0.0, 0.0, 10.0, 3.0, True, z(0, K, 3),
+                                            z(0, 3 * K, 79), off0.cuda(), ws)
+    with pytest.raises(ValueError):                # prior without anchor
+        ops.fit_lm_keypoints_2d_groups_step(st, tr, z(0, K, 2), z(0, K), None, 1.0, 0.0, 10.0, 3.0, True, z(0, K, 3),
+                                            z(0, 3 * K, 79), off0, ws)
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    with pytest.raises(ValueError):                # label 1 unused
+        fit_body_to_keypoints_2d(module, z(3, K, 2), method='lm', groups=torch.tensor([0, 2, 2]))
+    with pytest.raises(ValueError):                # per-group measurements with B values
+        fit_body_to_keypoints_2d(module, z(3, K, 2), method='lm', groups=torch.tensor([0, 1, 1]),
+                                 body_measurements=bm, measurements={'height': z(3) + 1.7})
+
+
+# ------------------------------------------------------------------------------------------------ fit
+def _problem(module, bm, n_id, views=4, seed=41):
+    """n_id identities seen in `views` images each, image b of identity b % n_id (the labels are not sorted):
+    betas* ~ N(0, 1) clipped to +-2 per identity, a raw pose (mean + 0.3 N) and camera per image; the start perturbs
+    every image as the 2D recipe does (tests/test_gpu_fit_lm_keypoints_2d.py)."""
+    from shapy_b200 import ops, synth
+    gen = torch.Generator().manual_seed(seed)
+    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
+    B = n_id * views
+    groups = torch.arange(B) % n_id
+    bstar = rn(n_id, module.num_betas).clamp(-2, 2)
+    raw = synth.mean_params()[:132] + 0.3 * rn(B, 132)
+    cam = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
+    with torch.no_grad():
+        rot = ops.decode_rot6d(raw.cuda())
+        out = module(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=bstar[groups].cuda(), camera=cam.cuda())
+        tgt = _measure(module, bm, bstar.cuda())
+    init = {'global_rot': (raw[:, :6] + 0.1 * rn(B, 6)).cuda(), 'body_pose': (raw[:, 6:] + 0.1 * rn(B, 126)).cuda(),
+            'betas': (bstar[groups] + 0.5 * rn(B, module.num_betas)).cuda(), 'camera': (cam + 0.05 * rn(B, 3)).cuda()}
+    return dict(x=out['proj_joints'].clone(), joints=out['joints'][:].clone(), init=init, bstar=bstar.cuda(), tgt=tgt,
+                tg={k: tgt[:, i].contiguous() for i, k in enumerate(NAMES)}, groups=groups.cuda())
+
+
+def _lm_loop(module, bm, p, iterations, sigma=0.1, pw=0.5, bw=0.01, meas=None):
+    """The LM loop of fit_body_to_keypoints_2d(groups=) written out over the ops, keeping every iteration's state loss
+    and the launches per iteration; p's labels must already be sorted."""
+    from shapy_b200 import _lib, ops
+    from shapy_b200.fit import LM_DOWN, LM_UP, _group_sum, _measurement_terms, group_plan
+    x, init = p['x'], p['init']
+    packed = module.packed(x.device)
+    B, K = x.shape[:2]
+    order, off = group_plan(p['groups'], B)
+    assert torch.equal(order, torch.arange(B))
+    G, nb = off.numel() - 1, 10
+    gidx = p['groups']
+    rot0 = ops.decode_rot6d(torch.cat([init['global_rot'], init['body_pose']], 1)).contiguous()
+    b0 = (_group_sum(init['betas'], off) / (off[1:] - off[:-1]).float().cuda()[:, None]).contiguous()
+    trial = {'rot': rot0.clone(), 'betas': b0, 'image_betas': b0[gidx].contiguous(), 'camera': init['camera'].clone()}
+    mk = lambda *s: torch.empty(*s, device='cuda')  # noqa: E731
+    state = {'rot': mk(B, N_ROT, 3, 3), 'betas': mk(G, nb), 'camera': mk(B, 3), 'keypoints': mk(B, K, 3),
+             'jac': mk(B, 3 * K, 3 * N_ROT + nb + 3), 'loss': mk(G), 'lambda': mk(G),
+             'accepted': torch.zeros(G, dtype=torch.int32, device='cuda')}
+    ws = ops.fit_lm_groups_workspace(B, G, N_ROT, nb, 'cuda')
+    w = torch.ones(B, K, device='cuda')
+    if meas is not None:
+        state.update(meas=mk(G, 5), meas_jac=mk(G, 5, nb))
+        mt, mw = _measurement_terms(meas, None, G, 'cuda')
+        faces, lm = module.faces_i32, bm.landmarks()
+        ops.face_incidence(faces)
+    losses, launches = [], []
+    for it in range(iterations + 1):
+        n0 = _lib.lib().shapy_launch_count()
+        tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['image_betas'], trial['rot'])
+        if meas is None:
+            ops.fit_lm_keypoints_2d_groups_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac,
+                                                off, ws, pose_anchor=rot0)
+        else:
+            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, ops.smplx_forward_shape(packed, trial['betas']), faces)
+            ops.fit_lm_keypoints_2d_groups_measurements_step(state, trial, x, w, sigma, pw, bw, mt.contiguous(),
+                                                             mw.contiguous(), LM_UP, LM_DOWN, it == 0, tkp, tjac, tm,
+                                                             tmj, off, ws, pose_anchor=rot0)
+        launches.append(_lib.lib().shapy_launch_count() - n0)
+        losses.append(state['loss'].clone())
+    return state, torch.stack(losses), launches
+
+
+@pytest.mark.parametrize('with_meas', [False, True])
+def test_lm_losses_monotone_launch_count_and_returned_by_the_fit(model, with_meas):
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    module, bm = model
+    p = _problem(module, bm, 16, seed=5)
+    o = torch.argsort(p['groups'].cpu(), stable=True).cuda()           # sorted labels for the written-out loop
+    ps = dict(p, x=p['x'][o].contiguous(), groups=p['groups'][o], init={k: v[o].contiguous()
+                                                                          for k, v in p['init'].items()})
+    meas = {k: p['tg'][k] for k in ('height', 'mass')} if with_meas else None
+    state, losses, launches = _lm_loop(module, bm, ps, 15, meas=meas)
+    assert launches == [6 if with_meas else 4] * 16, launches
+    assert bool(torch.isfinite(losses).all())
+    assert bool((losses[1:] <= losses[:-1]).all())
+    kw = dict(body_measurements=bm, measurements=meas) if with_meas else {}
+    res = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], method='lm', iterations=15, robust_sigma=0.1,
+                                   pose_prior_weight=0.5, betas_weight=0.01, groups=p['groups'], **kw)
+    assert res['betas'].shape == (16, 10) and res['loss'].shape == (16,) and res['camera'].shape == (64, 3)
+    for k in ('betas', 'loss'):
+        assert torch.equal(_bits(res[k]), _bits(state[k])), k
+    inv = torch.argsort(o)
+    assert torch.equal(_bits(res['camera']), _bits(state['camera'][inv]))
+    assert torch.equal(_bits(res['global_rot_mat']), _bits(state['rot'][inv][:, :1]))
+    if with_meas:
+        assert torch.equal(_bits(res['measurements']), _bits(state['meas']))
+
+
+def test_lm_deterministic_and_group_independent(model):
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    module, bm = model
+    p = _problem(module, bm, 16, seed=8)
+    kw = dict(method='lm', iterations=12, robust_sigma=0.1, pose_prior_weight=0.5, body_measurements=bm)
+    meas = {k: p['tg'][k] for k in ('height', 'mass')}
+    r1 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
+    r2 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
+    for k in r1:
+        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+    rows = (p['groups'] == 5).nonzero()[:, 0]                          # identity 5 alone, as label 0
+    one = fit_body_to_keypoints_2d(module, p['x'][rows].contiguous(),
+                                   init={k: v[rows].contiguous() for k, v in p['init'].items()},
+                                   measurements={k: v[5:6].contiguous() for k, v in meas.items()},
+                                   groups=torch.zeros(len(rows), dtype=torch.int64), **kw)
+    for k in ('betas', 'measurements', 'loss'):
+        assert torch.equal(_bits(one[k]), _bits(r1[k][5:6])), k
+    for k in ('camera', 'global_rot', 'body_pose'):
+        assert torch.equal(_bits(one[k]), _bits(r1[k][rows])), k
+
+
+def test_lm_loop_never_synchronises(model):
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    module, bm = model
+    p = _problem(module, bm, 8, seed=7)
+    kw = dict(init=p['init'], method='lm', robust_sigma=0.1, pose_prior_weight=1.0, betas_weight=0.01,
+              body_measurements=bm, measurements=p['tg'], groups=p['groups'].cpu())   # labels on the host: no read
+    fit_body_to_keypoints_2d(module, p['x'], iterations=1, **kw)       # packs the model, builds the incidence table
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode('error')
+    try:
+        res = fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw)
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
+    assert res['measurements'].shape == (8, 5)
+
+
+def test_adam_fits_one_betas_per_group(model):
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    module, bm = model
+    p = _problem(module, bm, 4, seed=9)
+    res = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], iterations=5, betas_weight=0.3,
+                                   body_measurements=bm, measurements={'height': p['tg']['height']},
+                                   groups=p['groups'])
+    assert res['betas'].shape == (4, 10) and res['measurements'].shape == (4, 5) and res['loss'].shape == (4,)
+    assert res['proj_joints'].shape == p['x'].shape and bool(torch.isfinite(res['loss']).all())
+
+
+# Quality, 64 identities x 4 views (256 images), 50 LM iterations: the per-image fit (groups=None, one betas per image)
+# against the grouped fit (one betas per identity), with and without known height and mass, with all keypoints and with
+# the 22 posed body joints only.  First run on an H100 80GB HBM3 (700 W), all keypoints, per image / grouped: median
+# |beta - beta*| 1.24 / 0.84 (1.18 / 0.80 with height and mass), 2D RMS < 2e-3 0.25 / 0.0, root-aligned joint error
+# 0.203 / 0.219 m.  Seven views in ten stay in local minima of the 2D loss from this start; a shared betas is pulled by
+# them, so with all keypoints no view of a group fits its image exactly, while the betas error drops by a third.  With
+# the 22 body joints (every view converges in the image): |beta - beta*| 1.04 / 0.33 (0.90 / 0.26), height < 1 mm
+# 0.17 / 0.61 (0.97 / 1.0), 2D RMS < 2e-3 1.0 / 1.0, joint error 0.128 / 0.108 m (0.125 / 0.101 m).
+BETA_BARS = {'all': {'grouped': 0.86, 'grouped_height_mass': 0.82},
+             'body': {'grouped': 0.35, 'grouped_height_mass': 0.28}}
+def quality(module, bm, p, res, grouped):
+    q = quality_2d(module, bm, dict(p, tgt=p['tgt'][p['groups']], bstar=p['bstar'][p['groups']]),
+                   dict(res, betas=res['betas'][p['groups']],
+                        **({'measurements': res['measurements'][p['groups']]} if 'measurements' in res else {})),
+                   p.get('w'))
+    if grouped:                       # per identity, not per image
+        meas = res['measurements'] if 'measurements' in res else _measure(module, bm, res['betas'])
+        q['median_beta_err'] = float((res['betas'] - p['bstar']).norm(dim=1).median())
+        q['height_1mm'] = float(((meas[:, 1] - p['tgt'][:, 1]).abs() < 1e-3).float().mean())
+    return q
+
+
+@pytest.mark.parametrize('which', ['all', 'body'])
+def test_fit_quality_64_identities_4_views(model, which):
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    module, bm = model
+    p = _problem(module, bm, 64)
+    w = torch.ones(p['x'].shape[1], device='cuda')
+    if which == 'body':                       # only the posed skeleton joints of the 22 fitted rotations
+        w[N_ROT:] = 0.0
+    p['w'] = w
+    kw = dict(init=p['init'], method='lm', weights=w)
+    gm = {k: p['tg'][k] for k in ('height', 'mass')}
+    hm = dict(body_measurements=bm, measurements={k: v[p['groups']] for k, v in gm.items()})
+    q = {'per_image': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], **kw), False),
+         'grouped': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], groups=p['groups'], **kw), True),
+         'per_image_height_mass': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], **hm, **kw), False),
+         'grouped_height_mass': quality(module, bm, p, fit_body_to_keypoints_2d(
+             module, p['x'], groups=p['groups'], body_measurements=bm, measurements=gm, **kw), True)}
+    print(f'fit_kp2d_groups_lm_64x4[{which}]', q)
+    for a, b in (('per_image', 'grouped'), ('per_image_height_mass', 'grouped_height_mass')):
+        assert q[b]['median_beta_err'] < q[a]['median_beta_err'], (a, b)
+        assert q[b]['median_beta_err'] <= BETA_BARS[which][b], (b, q[b])
+        if which == 'body':                   # where the views are fitted, sharing betas keeps them fitted
+            assert q[b]['frac_rms2d'] >= 0.98 and q[b]['frac_rms2d'] >= 0.9 * q[a]['frac_rms2d'], (a, b)
+            assert q[b]['median_root_mpjpe_m'] < q[a]['median_root_mpjpe_m'], (a, b)
