@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
+import kp2dm_lm_oracle as o2m
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -37,10 +38,13 @@ STEP_K = [1, 8, 9, 127]
 TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
 
 
-def _step_case(n_rot, nb, K, terms):
+def _step_case(n_rot, nb, K, terms, meas=False):
     """Six bodies with random Jacobians: body 0's trial hits its targets (accepted), body 1's state does and its trial
     is far (rejected), body 2 has a weighted NaN trial keypoint (rejected), 3 to 5 random.  With K >= 8 keypoint 7 has
-    weight 0 and NaN targets, keypoints and rows in state and trial."""
+    weight 0 and NaN targets, keypoints and rows in state and trial.  With `meas`, five random measurements and rows
+    stacked under them (drawn after everything else): body 0's trial and body 1's state hit their targets, body 3 has a
+    weighted NaN trial measurement (rejected), and the height has weight 0 and NaN values and rows in state and
+    trial."""
     sigma, pw, bw = terms
     B, P = 6, 3 * n_rot + nb + 3
     gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + (3 if pw else 0))
@@ -70,44 +74,94 @@ def _step_case(n_rot, nb, K, terms):
             t[:, 7] = float('nan')
         for t in (jac, tjac):
             t[:, 21:24] = float('nan')
-    return dict(rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, trot=trot, tbetas=tbetas, tcam=tcam, tkp=tkp,
-                tjac=tjac, tg=tg, w=w, anchor=anchor, lam=torch.rand(B, generator=gen) + 0.01,
-                sigma=sigma, pw=pw, bw=bw)
+    c = dict(rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, trot=trot, tbetas=tbetas, tcam=tcam, tkp=tkp, tjac=tjac,
+             tg=tg, w=w, anchor=anchor, lam=torch.rand(B, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
+    if meas:
+        m, mj = torch.rand(B, 5, generator=gen) + 0.5, rn(B, 5, nb)
+        tm, tmj = m + 0.01 * rn(B, 5), mj + 0.1 * rn(B, 5, nb)
+        mt = m + 0.02 * rn(B, 5)
+        mt[0], mt[1] = tm[0], m[1]
+        mw = torch.rand(B, 5, generator=gen) * 2 + 0.5
+        mw[:, 1] = 0.0
+        for t in (m, tm, mj, tmj):
+            t[:, 1] = float('nan')
+        tm[3, 3] = float('nan')
+        c.update(meas=m, mjac=mj, tmeas=tm, tmjac=tmj, mt=mt, mw=mw)
+    return c
+
+
+def _state_np(c, b):
+    """Body b's state for the restatement, its loss the restatement's (float32)."""
+    n = lambda t: t.numpy()  # noqa: E731
+    s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'camera': n(c['cam'][b]), 'keypoints': n(c['kp'][b]),
+         'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
+    if 'meas' in c:
+        s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
+        s['loss'] = np.float32(o2m.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], n(c['mt'][b]),
+                                        n(c['mw'][b]), s['meas'], c['sigma'], s['rot'], n(c['anchor'][b]), c['pw'],
+                                        s['betas'], c['bw']))
+    else:
+        s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
+                                       n(c['anchor'][b]), c['pw'], s['betas'], c['bw']))
+    return s
+
+
+def _device(c):
+    """The case's state and trial on the device, the state's loss from the restatement."""
+    B = c['rot'].shape[0]
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
+             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([_state_np(c, b)['loss'] for b in range(B)]))),
+             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
+    if 'meas' in c:
+        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
+    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'camera': cu(c['tcam'])}
+    return state, trial
+
+
+def _step(c, state, trial, first):
+    """One 2D step (with the case's measurement block, the stacked step) on the case's inputs."""
+    from shapy_b200 import ops
+    cu = lambda t: t.cuda().contiguous()  # noqa: E731
+    if 'meas' in c:
+        ops.fit_lm_keypoints_2d_measurements_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'],
+                                                  cu(c['mt']), cu(c['mw']), 10.0, 3.0, first, cu(c['tkp']),
+                                                  cu(c['tjac']), cu(c['tmeas']), cu(c['tmjac']),
+                                                  pose_anchor=cu(c['anchor']))
+    else:
+        ops.fit_lm_keypoints_2d_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
+                                     first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
 
 
 def _run_step(c, first):
-    from shapy_b200 import ops
+    """The kernel on the case (with its measurement block, the stacked step), then the restatement body by body;
+    returns the largest trial error over its bar."""
     B = c['rot'].shape[0]
+    meas = 'meas' in c
     n = lambda t: t.numpy()  # noqa: E731
     kw = dict(sigma=c['sigma'], pose_w=c['pw'], betas_w=c['bw'])
-    s_np = []
-    for b in range(B):
-        s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'camera': n(c['cam'][b]), 'keypoints': n(c['kp'][b]),
-             'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-        s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
-                                       n(c['anchor'][b]), c['pw'], s['betas'], c['bw']))
-        s_np.append(s)
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([s['loss'] for s in s_np]))),
-             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'camera': cu(c['tcam'])}
-    ops.fit_lm_keypoints_2d_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0, first,
-                                 cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
+    s_np = [_state_np(c, b) for b in range(B)]
+    state, trial = _device(c)
+    _step(c, state, trial, first)
     got = {k: v.cpu().numpy() for k, v in state.items()}
     nxt = {k: v.cpu().numpy() for k, v in trial.items()}
     flags, worst = [], 0.0
     for b in range(B):
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'camera': n(c['tcam'][b])}
-        new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                 n(c['tkp'][b]), n(c['tjac'][b]), anchor=n(c['anchor'][b]), **kw)
+        if meas:
+            new, want, acc = o2m.lm_keypoints_2d_measurements_step(
+                s_np[b], n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), 10.0, 3.0, first, tr,
+                n(c['tkp'][b]), n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]), anchor=n(c['anchor'][b]), **kw)
+        else:
+            new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
+                                                     n(c['tkp'][b]), n(c['tjac'][b]), anchor=n(c['anchor'][b]), **kw)
         flags.append(acc)
         assert got['accepted'][b] == new['accepted'], b
         # softplus' exp / log1p may round differently on the device: loss and lambda to fp32 rounding
         assert np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), (b, got['lambda'][b], new['lambda'])
         assert np.isclose(got['loss'][b], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (b, got['loss'][b],
                                                                                           new['loss'])
-        for k in ('rot', 'betas', 'camera', 'keypoints', 'jac'):
+        for k in ('rot', 'betas', 'camera', 'keypoints', 'jac') + (('meas', 'meas_jac') if meas else ()):
             assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
         for k in ('rot', 'betas', 'camera'):
             bar = 2e-6 * max(1.0, np.abs(want[k]).max())
@@ -117,7 +171,7 @@ def _run_step(c, first):
     if first:
         assert all(flags)
     else:
-        assert flags[:3] == [True, False, False], flags
+        assert flags[:3] == [True, False, False] and (not meas or not flags[3]), flags
     return worst
 
 

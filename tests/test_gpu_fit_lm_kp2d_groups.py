@@ -112,11 +112,13 @@ def _device(c, with_meas):
     return state, trial, B, G
 
 
-def _groups_step(c, state, trial, first, with_meas):
+def _groups_step(c, state, trial, first, with_meas, ws=None):
+    """One grouped step on the case at its n_rot and nb; ws: the workspace (by default a fresh one)."""
     from shapy_b200 import ops
     cu = lambda t: t.cuda().contiguous()  # noqa: E731
     B, G = c['rot'].shape[0], len(c['off']) - 1
-    ws = ops.fit_lm_groups_workspace(B, G, N_ROT, 10, 'cuda')
+    if ws is None:
+        ws = ops.fit_lm_groups_workspace(B, G, c['rot'].shape[1], c['betas'].shape[1], 'cuda')
     off = torch.from_numpy(c['off'])
     if with_meas:
         ops.fit_lm_keypoints_2d_groups_measurements_step(
@@ -128,15 +130,11 @@ def _groups_step(c, state, trial, first, with_meas):
                                             pose_anchor=cu(c['anchor']))
 
 
-@pytest.mark.parametrize('meas', [None, 'reference', 'exact'])
-@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
-@pytest.mark.parametrize('first', [False, True])
-def test_step_kernels_vs_oracle(model, first, terms, meas):
-    c = _group_case(model, terms, exact=meas == 'exact')
-    with_meas = meas is not None
-    state, trial, B, G = _device(c, with_meas)
-    s0 = {k: v.cpu().numpy() for k, v in state.items()}
-    _groups_step(c, state, trial, first, with_meas)
+def _check_vs_oracle(c, s0, state, trial, first, with_meas):
+    """The stepped device state and next trial against kp2dg_lm_oracle group by group, from the state s0 (NumPy) before
+    the step: loss and lambda to fp32 rounding, the state bit for bit, the next trial within 2e-6 max(1, |x|) and each
+    image's trial betas its group's.  Returns (the groups' accepted flags, the largest trial error over its bar)."""
+    G = len(c['off']) - 1
     got = {k: v.cpu().numpy() for k, v in state.items()}
     nxt = {k: v.cpu().numpy() for k, v in trial.items()}
     n = lambda t: t.numpy()  # noqa: E731
@@ -177,6 +175,19 @@ def test_step_kernels_vs_oracle(model, first, terms, meas):
         err = np.abs(nxt['betas'][g] - want['betas']).max()
         assert err <= bar, (g, 'betas', err)
         worst = max(worst, err / bar)
+    return flags, worst
+
+
+@pytest.mark.parametrize('meas', [None, 'reference', 'exact'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+def test_step_kernels_vs_oracle(model, first, terms, meas):
+    c = _group_case(model, terms, exact=meas == 'exact')
+    with_meas = meas is not None
+    state, trial, B, G = _device(c, with_meas)
+    s0 = {k: v.cpu().numpy() for k, v in state.items()}
+    _groups_step(c, state, trial, first, with_meas)
+    flags, worst = _check_vs_oracle(c, s0, state, trial, first, with_meas)
     if first:
         assert all(flags)
     else:
@@ -190,8 +201,12 @@ def test_groups_of_one_equal_the_2d_step(model, first, terms):
     """Eight groups of one: loss, lambda, accepted and the state bit for bit as shapy_fit_lm_keypoints_2d_step; the
     next trial within 4e-6 max(1, |x|) (the CPU oracle test bounds the two eliminations' fp64 difference by 1e-10; what
     is left is the fp32 rounding of the result)."""
+    _check_groups_of_one(_group_case(model, terms, sizes=(1,) * 8), first)
+
+
+def _check_groups_of_one(c, first):
+    """The grouped step on a case of groups of one against shapy_fit_lm_keypoints_2d_step on the same images."""
     from shapy_b200 import ops
-    c = _group_case(model, terms, sizes=(1,) * 8)
     state, trial, B, G = _device(c, False)
     b_state = {k: v.clone() for k, v in state.items()}
     b_trial = {k: v.clone() for k, v in trial.items() if k != 'image_betas'}
@@ -208,7 +223,12 @@ def test_groups_of_one_equal_the_2d_step(model, first, terms):
 
 @pytest.mark.parametrize('first', [False, True])
 def test_dropped_measurements_equal_the_plain_groups_step_bit_for_bit(model, first):
-    c = _group_case(model, TERMS[1])
+    _check_dropped_measurements(_group_case(model, TERMS[1]), first)
+
+
+def _check_dropped_measurements(c, first):
+    """Every measurement of the case dropped (weight 0 or -1, NaN values and rows): the measurements entry equals the
+    plain grouped entry bit for bit."""
     for k in ('meas', 'tmeas', 'mjac', 'tmjac'):
         c[k][:] = float('nan')
     c['mw'][:] = 0.0

@@ -10,13 +10,22 @@ test_model_shapes_cpu.py pins at those shapes.
   * cached against uncached Jacobian entries (edge_2048 / edge_2049): the same bits
   * J^T c against the posed backward on the uncached NB = 27 model
   * both LM step kernels against their restatements at P = 7, 54, 55 (the 48 KB opt-in boundary) and 96, K = 1 to 127
-  * fit_body_to_keypoints(method='lm') at NB = 27 (P = 96) and NB = 16 with height and mass"""
+  * every keypoint step entry launches at P = 96 and refuses P = 97 without a launch
+  * the 2D measurement step and both grouped 2D steps on random Jacobians against kp2dm_lm_oracle and kp2dg_lm_oracle at
+    the same shapes, groups of 1 to 64 images in regular and irregular layouts; groups of one against the 2D step and
+    dropped measurements against the plain grouped step at every shape; no write outside any output or past the
+    workspace
+  * fit_body_to_keypoints(method='lm') at NB = 27 (P = 96) and NB = 16 with height and mass, and
+    fit_body_to_keypoints_2d(method='lm') on the same two, per image and with groups"""
 import numpy as np
 import pytest
 import torch
 
+import kp2d_lm_oracle as o2
 import kp_lm_oracle
 import kpm_lm_oracle
+import test_gpu_fit_lm_keypoints_2d as kp2d
+import test_gpu_fit_lm_kp2d_groups as grp
 from shapy_b200 import synth
 from smplx_grad_ref import oracle_grads
 from test_model_shapes_cpu import KP_CACHE_ENTRIES, VARIANTS, keypoint_entries, variant_model
@@ -358,28 +367,219 @@ def test_keypoint_measurement_step_vs_oracle(n_rot, nb, K, first, rho):
           f'trial error / bar {worst:.3f}')
 
 
-def test_steps_refuse_97_parameters_without_a_launch():
+def _call_every_step(n_rot, nb):
+    """Each keypoint LM step entry once on zero inputs at (n_rot, nb), two bodies (two groups of one), first step: 3D,
+    3D + measurements, 2D, 2D + measurements, grouped 2D, grouped 2D + measurements.  Returns their return codes."""
     from shapy_b200 import _lib
     L = _lib.lib()
-    z = lambda *s: torch.zeros(*s, device='cuda')  # noqa: E731
-    B, K, n_rot, nb = 2, 6, 31, 1
+    keep = []                                        # every tensor lives until the launches are done
+
+    def z(*s, dtype=torch.float32):
+        keep.append(torch.zeros(*s, dtype=dtype, device='cuda'))
+        return _lib.ptr(keep[-1])
+    B, G, K = 2, 2, 6
     P = 3 * n_rot + nb + 3
-    assert P == 97
-    st = [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]
-    tr = [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]
-    loss, lam, acc = z(B), z(B), torch.zeros(B, dtype=torch.int32, device='cuda')
-    p = lambda ts: [_lib.ptr(t) for t in ts]  # noqa: E731
+    off = torch.tensor([0, 1, 2], dtype=torch.int32)
+    ws = z(L.shapy_fit_lm_groups_workspace_bytes(B, G, n_rot, nb) // 4 + 1)
+    st = lambda: [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]  # noqa: E731
+    tr = lambda: [z(B, n_rot, 3, 3), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]  # noqa: E731
+    head2d = lambda: [z(B, K, 2), z(B, K), z(B, n_rot, 3, 3), 1.0, 0.5, 0.1]  # noqa: E731
+    counters = lambda: [z(B), z(B), z(B, dtype=torch.int32)]  # noqa: E731
+    ms = lambda: [z(B, 5), z(B, 5, nb)]  # noqa: E731
+    gst = lambda: [z(B, n_rot, 3, 3), z(G, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]  # noqa: E731
+    gtr = lambda: [z(B, n_rot, 3, 3), z(G, nb), z(B, nb), z(B, 3), z(B, K, 3), z(B, 3 * K, P)]  # noqa: E731
+    rc = [L.shapy_fit_lm_keypoints_step(B, K, n_rot, nb, z(B, K, 3), z(B, K), 10.0, 3.0, 1, *st(), *counters(), *tr(),
+                                        None),
+          L.shapy_fit_lm_keypoints_measurements_step(B, K, n_rot, nb, z(B, K, 3), z(B, K), z(B, 5), z(B, 5), 0.0, 10.0,
+                                                     3.0, 1, *st(), *ms(), *counters(), *tr(), *ms(), None),
+          L.shapy_fit_lm_keypoints_2d_step(B, K, n_rot, nb, *head2d(), 10.0, 3.0, 1, *st(), *counters(), *tr(), None),
+          L.shapy_fit_lm_keypoints_2d_measurements_step(B, K, n_rot, nb, *head2d(), z(B, 5), z(B, 5), 10.0, 3.0, 1,
+                                                        *st(), *ms(), *counters(), *tr(), *ms(), None),
+          L.shapy_fit_lm_keypoints_2d_groups_step(B, G, off.data_ptr(), K, n_rot, nb, *head2d(), 10.0, 3.0, 1, *gst(),
+                                                  *counters(), *gtr(), ws, None),
+          L.shapy_fit_lm_keypoints_2d_groups_measurements_step(B, G, off.data_ptr(), K, n_rot, nb, *head2d(), z(G, 5),
+                                                               z(G, 5), 10.0, 3.0, 1, *gst(), *ms(), *counters(),
+                                                               *gtr(), *ms(), ws, None)]
+    torch.cuda.synchronize()
+    return rc
+
+
+def test_steps_refuse_97_parameters_without_a_launch():
+    """P = 96 (n_rot 22, nb 27) launches every keypoint step (one launch each, three for the grouped ones); P = 97, as
+    (22, 28) and as (31, 1), is SHAPY_ERR_UNSUPPORTED from each, with nothing launched."""
+    from shapy_b200 import _lib
+    L = _lib.lib()
     torch.cuda.synchronize()
     n0 = L.shapy_launch_count()
-    rc = L.shapy_fit_lm_keypoints_step(B, K, n_rot, nb, _lib.ptr(z(B, K, 3)), _lib.ptr(z(B, K)), 10.0, 3.0, 1,
-                                       *p(st), *p([loss, lam, acc]), *p(tr), None)
-    assert rc == -3                                  # SHAPY_ERR_UNSUPPORTED
-    rc = L.shapy_fit_lm_keypoints_measurements_step(
-        B, K, n_rot, nb, _lib.ptr(z(B, K, 3)), _lib.ptr(z(B, K)), _lib.ptr(z(B, 5)), _lib.ptr(z(B, 5)), 0.0, 10.0, 3.0,
-        1, *p(st), *p([z(B, 5), z(B, 5, nb), loss, lam, acc]), *p(tr), *p([z(B, 5), z(B, 5, nb)]), None)
-    assert rc == -3
+    assert _call_every_step(22, 27) == [0] * 6
+    assert L.shapy_launch_count() == n0 + 10
+    for n_rot, nb in ((22, 28), (31, 1)):
+        assert 3 * n_rot + nb + 3 == 97
+        n0 = L.shapy_launch_count()
+        assert _call_every_step(n_rot, nb) == [-3] * 6, (n_rot, nb)        # SHAPY_ERR_UNSUPPORTED
+        assert L.shapy_launch_count() == n0, (n_rot, nb)
+
+
+# ------------------------------------------------------------------------------------------------ 2D LM steps
+# the 2D steps on random Jacobians at STEP_SHAPES, against kp2dm_lm_oracle and kp2dg_lm_oracle (which
+# test_model_shapes_cpu.py pins at these shapes); K: 2K = 2, 16 (one full staging tile), 18 and 254 rows
+STEP_K_2D = [1, 8, 9, 127]
+GROUP_K = [1, 9, 127]
+LAYOUTS = {'1-2-3-5': (1, 2, 3, 5), '1-7-1-33-2': (1, 7, 1, 33, 2), '64': (64,)}
+
+
+@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('K', STEP_K_2D)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_keypoint_2d_measurement_step_vs_oracle(n_rot, nb, K, first, terms):
+    worst = kp2d._run_step(kp2d._step_case(n_rot, nb, K, terms, meas=True), first)
+    print(f'[model-shapes] kp2dm step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first} terms={terms}: '
+          f'trial error / bar {worst:.3f}')
+
+
+def _group_case(n_rot, nb, K, terms, sizes):
+    """test_gpu_fit_lm_kp2d_groups._group_case's cases on random Jacobians at (n_rot, nb): groups of `sizes` images,
+    group 0 targets the trial (accepted), 1 the state with the priors on its side and a trial 0.5 away (rejected), 2 the
+    trial (accepted), the rest noisy targets.  With K >= 8 keypoint 7 has weight 0 and NaN targets, keypoints and rows
+    in state and trial; measurement 2 of group 2 (of the last group when there are fewer) is dropped with NaN values
+    and rows."""
+    sigma, pw, bw = terms
+    G, B, P = len(sizes), sum(sizes), 3 * n_rot + nb + 3
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
+    gidx = torch.repeat_interleave(torch.arange(G), torch.tensor(sizes))
+    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + B + (3 if pw else 0))
+    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
+    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
+    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
+    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
+    betas, cam = rn(G, nb), rn(B, 3) * torch.tensor([0.5, 0.1, 0.1])
+    tbetas, tcam = betas + 0.05 * rn(G, nb), cam + 0.01 * rn(B, 3)
+    kp, jac = rn(B, K, 3), rn(B, 3 * K, P)
+    tkp, tjac = kp + 0.05 * rn(B, K, 3), jac + 0.1 * rn(B, 3 * K, P)
+    m, mj = torch.rand(G, 5, generator=gen) + 0.5, rn(G, 5, nb)
+    tm, tmj = m + 0.01 * rn(G, 5), mj + 0.1 * rn(G, 5, nb)
+    proj = lambda k, c: torch.stack([torch.from_numpy(o2.project(k[b].numpy(), c[b].numpy())).float()  # noqa: E731
+                                     for b in range(k.shape[0])])
+    tg = proj(kp, cam) + 0.05 * rn(B, K, 2)
+    mt = m + 0.02 * rn(G, 5)
+    for g, to_trial in zip(range(G), (True, False, True)):
+        r = slice(off[g], off[g + 1])
+        if to_trial:
+            kp[r] = tkp[r] + 0.5
+            tg[r], anchor[r], tbetas[g], mt[g] = proj(tkp[r], tcam[r]), trot[r], 0.9 * betas[g], tm[g]
+        else:
+            tkp[r] = kp[r] + 0.5
+            tg[r], anchor[r], tbetas[g], mt[g] = proj(kp[r], cam[r]), rot[r], 1.1 * betas[g], m[g]
+    w = torch.rand(B, K, generator=gen) + 0.5
+    if K >= 8:
+        w[:, 7] = 0.0
+        tg[:, 7] = float('nan')
+        for t in (kp, tkp):
+            t[:, 7] = float('nan')
+        for t in (jac, tjac):
+            t[:, 21:24] = float('nan')
+    mw = torch.rand(G, 5, generator=gen) * 2 + 0.5
+    gd = min(2, G - 1)
+    mw[gd, 2] = 0.0
+    for t in (m, tm, mj, tmj):
+        t[gd, 2] = float('nan')
+    return dict(off=off, gidx=gidx, rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, meas=m, mjac=mj, trot=trot,
+                tbetas=tbetas, tcam=tcam, tkp=tkp, tjac=tjac, tmeas=tm, tmjac=tmj, tg=tg, w=w, mt=mt, mw=mw,
+                anchor=anchor, lam=torch.rand(G, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
+
+
+@pytest.mark.parametrize('with_meas', [False, True], ids=['kp2dg', 'kp2dgm'])
+@pytest.mark.parametrize('layout', list(LAYOUTS))
+@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('K', GROUP_K)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_groups_step_vs_oracle(n_rot, nb, K, first, terms, layout, with_meas):
+    """Both grouped entries against kp2dg_lm_oracle: groups (1, 2, 3, 5), an irregular layout whose image kernel finds
+    the groups of 1, 7, 1, 33 and 2 images by its binary search, and one group of 64 images."""
+    c = _group_case(n_rot, nb, K, terms, LAYOUTS[layout])
+    state, trial, _, G = grp._device(c, with_meas)
+    s0 = {k: v.cpu().numpy() for k, v in state.items()}
+    grp._groups_step(c, state, trial, first, with_meas)
+    flags, worst = grp._check_vs_oracle(c, s0, state, trial, first, with_meas)
+    if first:
+        assert all(flags)
+    else:
+        assert flags[:3] == [True, False, True][:G], flags
+    print(f'[model-shapes] {"kp2dgm" if with_meas else "kp2dg"} step P={3 * n_rot + nb + 3} nb={nb} K={K} '
+          f'layout={layout} first={first} terms={terms}: trial error / bar {worst:.3f}')
+
+
+@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_groups_of_one_equal_the_2d_step(n_rot, nb, first, terms):
+    grp._check_groups_of_one(_group_case(n_rot, nb, 9, terms, (1,) * 6), first)
+
+
+@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_dropped_measurements_equal_the_plain_groups_step(n_rot, nb, first, terms):
+    grp._check_dropped_measurements(_group_case(n_rot, nb, 9, terms, (1, 2, 3, 5)), first)
+
+
+GUARD = 64                        # sentinel elements on each side of a guarded output: 256 bytes, the alignment kept
+SENTINEL = 0x7FA5A5A5
+
+
+def _guarded(t):
+    """A copy of t inside a larger int32 buffer with GUARD sentinel elements on each side; returns (copy, buffer)."""
+    n = t.numel()
+    buf = torch.full((n + 2 * GUARD,), SENTINEL, dtype=torch.int32, device='cuda')
+    v = buf[GUARD:GUARD + n].view(t.dtype).view(t.shape)
+    v.copy_(t)
+    return v, buf
+
+
+@pytest.mark.parametrize('entry', ['kp2dm', 'kp2dg', 'kp2dgm'])
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_steps_write_nothing_outside_their_outputs(n_rot, nb, entry):
+    """A first and a second step with every output (state, trial, image_betas, meas, meas_jac) a slice between
+    sentinel guards and the workspace followed by sentinel bytes: the guards, the bytes past
+    shapy_fit_lm_groups_workspace_bytes and every input keep their bits, and the outputs equal those of unguarded
+    tensors bit for bit."""
+    from shapy_b200 import _lib
+    terms, K = kp2d.TERMS[1], 9
+    keys = ['tg', 'w', 'anchor', 'tkp', 'tjac'] + ([] if entry == 'kp2dg' else ['mt', 'mw', 'tmeas', 'tmjac'])
+    if entry == 'kp2dm':
+        c = kp2d._step_case(n_rot, nb, K, terms, meas=True)
+        state, trial = kp2d._device(c)
+    else:
+        c = _group_case(n_rot, nb, K, terms, (1, 2, 3, 5))
+        state, trial, B, G = grp._device(c, entry == 'kp2dgm')
+        need = _lib.lib().shapy_fit_lm_groups_workspace_bytes(B, G, n_rot, nb)
+        wbuf = torch.full((need // 4 + 1 + GUARD,), SENTINEL, dtype=torch.int32, device='cuda')
+        ws = wbuf.view(torch.uint8)[:need]
+        tail = wbuf.view(torch.uint8)[need:].clone()
+    cd = dict(c, **{k: c[k].cuda().contiguous() for k in keys})       # the inputs on the device, read in place
+    inputs = {k: cd[k].clone() for k in keys}
+    g_state = {k: _guarded(v) for k, v in state.items()}
+    g_trial = {k: _guarded(v) for k, v in trial.items()}
+    for first in (True, False):
+        a_st, a_tr = {k: v[0] for k, v in g_state.items()}, {k: v[0] for k, v in g_trial.items()}
+        if entry == 'kp2dm':
+            kp2d._step(cd, a_st, a_tr, first)
+            kp2d._step(cd, state, trial, first)
+        else:
+            grp._groups_step(cd, a_st, a_tr, first, entry == 'kp2dgm', ws)
+            grp._groups_step(cd, state, trial, first, entry == 'kp2dgm')
     torch.cuda.synchronize()
-    assert L.shapy_launch_count() == n0
+    for what, gd, ref in (('state', g_state, state), ('trial', g_trial, trial)):
+        for k, (v, buf) in gd.items():
+            n = v.numel()
+            assert bool((buf[:GUARD] == SENTINEL).all()) and bool((buf[GUARD + n:] == SENTINEL).all()), (what, k)
+            assert torch.equal(_bits(v), _bits(ref[k])), (what, k)
+    for k in keys:
+        assert torch.equal(_bits(cd[k]), _bits(inputs[k])), k
+    if entry != 'kp2dm':
+        assert torch.equal(wbuf.view(torch.uint8)[need:], tail)
 
 
 # ------------------------------------------------------------------------------------------------ fits
@@ -463,3 +663,86 @@ def test_lm_fit(packed, name):
     g1, g2 = (ops.smplx_backward(pk, c(x['betas']), c(x['rot']), expr=c(x['expression']), **cot) for _ in range(2))
     for k in ('betas', 'rot', 'expr'):
         assert torch.equal(_bits(g1[k]), _bits(g2[k])), k
+
+
+def _fit_problem_2d(module, NB, G, views, bm=None, seed=33):
+    """G identities seen in `views` images each, image b of identity b % G (the labels are not sorted): betas* per
+    identity, a raw pose (mean + 0.3 N) and camera per image; the targets their projected keypoints, with bm the
+    identities' measurements; a start camera near the true one."""
+    from shapy_b200 import ops
+    gen = torch.Generator().manual_seed(seed)
+    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
+    B = G * views
+    labels = torch.arange(B) % G
+    bstar = rn(G, NB).clamp(-2, 2).cuda()
+    raw = synth.mean_params()[:132] + 0.3 * rn(B, 132)
+    cam = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
+    meas = None
+    with torch.no_grad():
+        rot = ops.decode_rot6d(raw.cuda())
+        x = module(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=bstar[labels.cuda()],
+                   camera=cam.cuda())['proj_joints'].clone()
+        if bm is not None:
+            m = bm.forward_vertices(module.forward_shape(betas=bstar)['v_shaped'], module.faces_i32)['measurements']
+            meas = {k: m[k]['tensor'].clone() for k in m}
+    return x, labels, (cam + 0.05 * rn(B, 3)).cuda(), meas
+
+
+@pytest.mark.parametrize('grouped', [False, True], ids=['per_image', 'groups_8x4'])
+@pytest.mark.parametrize('name', list(FIT_CASES))
+def test_lm_fit_2d(name, grouped):
+    """fit_body_to_keypoints_2d(method='lm') on 32 images of nb27_ne5_dense (P = 96) and of nb16_ne16 with height and
+    mass, per image and as 8 identities x 4 views: every body's (group's) loss is at most its start, betas is (G, NB),
+    a sub-batch of whole groups gives the batch's rows bit for bit, and the loop never synchronises."""
+    from shapy_b200.fit import fit_body_to_keypoints_2d
+    NB = VARIANTS[name][0]
+    module = _module(name)
+    bm = None
+    if FIT_CASES[name]:
+        from shapy_b200.body_measurements import BodyMeasurements
+        bm = BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda()
+    G = 8 if grouped else 32
+    x, labels, cam0, meas = _fit_problem_2d(module, NB, G, 32 // G, bm)
+    mean = synth.mean_params().cuda()
+
+    def args(ids):
+        """The arguments of the fit of the identities `ids` (sorted), relabelled 0 .. len(ids) - 1 in their order, on
+        the device (a copy from the host would synchronise), and their images' rows."""
+        ids = torch.tensor(ids)
+        rows = torch.isin(labels, ids).nonzero()[:, 0].cuda()
+        n = len(rows)
+        kw = dict(init={'global_rot': mean[:6].expand(n, 6), 'body_pose': mean[6:132].expand(n, 126),
+                        'camera': cam0[rows].contiguous()},
+                  method='lm', robust_sigma=0.1, pose_prior_weight=0.5, betas_weight=0.01)
+        if grouped:
+            kw['groups'] = torch.searchsorted(ids, labels[rows.cpu()])  # on the host: group_plan reads no device
+        if bm is not None:
+            kw.update(body_measurements=bm,
+                      measurements={k: meas[k][ids.cuda()].contiguous() for k in FIT_CASES[name]})
+        return x[rows].contiguous(), kw, rows
+
+    def fit(a, iterations=None):
+        return fit_body_to_keypoints_2d(module, a[0], iterations=iterations, **a[1])
+
+    every = args(range(G))
+    res = fit(every)
+    start = fit(every, iterations=0)['loss']
+    assert res['betas'].shape == (G, NB) and res['loss'].shape == (G,)
+    fin = torch.isfinite(start)
+    assert int(fin.sum()) >= G - 2
+    assert bool((res['loss'][fin] <= start[fin]).all()), (res['loss'], start)
+    print(f'[model-shapes] lm fit 2d {name} grouped={grouped}: median loss {float(res["loss"].median()):.4g} from '
+          f'{float(start[fin].median()):.4g}')
+    ids = [1, 4, 6] if grouped else [3, 4, 9, 15, 16, 22, 30, 31]
+    a = args(ids)
+    sub, rows = fit(a), a[2]
+    for k in ('global_rot', 'body_pose', 'camera'):
+        assert torch.equal(_bits(sub[k]), _bits(res[k][rows])), k
+    for k in ('betas',) + (('measurements',) if bm is not None else ()) + (('loss',) if grouped else ()):
+        assert torch.equal(_bits(sub[k]), _bits(res[k][ids])), k
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode('error')
+    try:
+        fit(every, iterations=3)
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
