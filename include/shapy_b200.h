@@ -369,6 +369,42 @@ int shapy_fit_lm_keypoints_2d_groups_measurements_step(
     float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
     const float *trial_meas_jac, void *workspace, void *stream);
 
+/* shapy_fit_lm_keypoints_2d_groups_step for views of one posed body at one moment: the images of group g share beta_g
+ * and the body rotations R_g,j, j = 1 .. n_rot-1; each keeps its global rotation R_0,i and camera.  Loss per group,
+ * fp64, left to right: the sum over its images (image order) of the 2D step's keypoint term, + pose_prior_weight / 2
+ * sum_{j >= 1} |R_g,j - R0_g,j|_F^2 once per group, + betas_weight |beta_g|^2.  Arguments as
+ * shapy_fit_lm_keypoints_2d_groups_step, except pose_anchor, which is per group, (G,n_rot,3,3), joint 0 unread.  rot
+ * and trial_rot stay per image (batch,n_rot,3,3): the kernels read each group's body rotations from its first image's
+ * rows and write the same values to all of its images' rows, so on the first step the caller fills every image's
+ * rows of joints 1.. with the group's rotations.  The step is the exact LM step of the group's normal matrix by its
+ * Schur complement: each image's [delta_0 | camera] block (damped by lambda) is eliminated, the (3 (n_rot-1) + nb)
+ * square shared system (lambda on the rotation diagonal, betas_weight + lambda on the betas diagonal) solved, each
+ * image's delta back-substituted.  The first lambda is 1e-3 max(1e-6, the largest diagonal entry of the group's
+ * keypoint rows), per image on the [delta_0 | camera] columns and summed over the images on the shared columns.
+ * A group of one has shapy_fit_lm_keypoints_2d_step's loss, lambda and decision bit for bit; with n_rot 1 every
+ * output is shapy_fit_lm_keypoints_2d_groups_step's.  workspace: shapy_fit_lm_shared_pose_workspace_bytes(batch,
+ * num_groups, n_rot, nb) bytes of device memory.  Three launches; errors as shapy_fit_lm_keypoints_2d_groups_step. */
+size_t shapy_fit_lm_shared_pose_workspace_bytes(int batch, int num_groups, int n_rot, int nb);
+int shapy_fit_lm_keypoints_2d_shared_pose_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *camera,
+    float *keypoints, float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_betas_images, float *trial_camera, const float *trial_keypoints, const float *trial_jac,
+    void *workspace, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_shared_pose_step with the five virtual measurements of each group, as
+ * shapy_fit_lm_keypoints_2d_groups_measurements_step adds them; their rows join the betas block of the shared system.
+ * With every measurement weight <= 0 every output equals shapy_fit_lm_keypoints_2d_shared_pose_step's bit for bit. */
+int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
+    const float *trial_meas_jac, void *workspace, void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

@@ -113,6 +113,16 @@ _SIGS = {
                                                                    C.c_float, c_void_p, c_void_p, C.c_float,
                                                                    C.c_float, c_int] + [c_void_p] * 18
                                                            + [c_void_p, c_void_p]),
+    'shapy_fit_lm_shared_pose_workspace_bytes': (C.c_size_t, [c_int, c_int, c_int, c_int]),
+    'shapy_fit_lm_keypoints_2d_shared_pose_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                                                           c_void_p, c_void_p, C.c_float, C.c_float, C.c_float,
+                                                           C.c_float, C.c_float, c_int] + [c_void_p] * 14
+                                                   + [c_void_p, c_void_p]),
+    'shapy_fit_lm_keypoints_2d_shared_pose_measurements_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int,
+                                                                        c_void_p, c_void_p, c_void_p, C.c_float,
+                                                                        C.c_float, C.c_float, c_void_p, c_void_p,
+                                                                        C.c_float, C.c_float, c_int] + [c_void_p] * 18
+                                                                + [c_void_p, c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

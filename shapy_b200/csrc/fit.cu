@@ -594,6 +594,17 @@ __device__ __forceinline__ double rot_tangent(const float *R, int a, int e) {
   return ((q - a + 3) % 3 == 1) ? v : -v;      // -eps_{a m q} R_rm
 }
 
+// Phase 1 of the 2D steps, by one thread: the pose prior 1/2 pose_w sum_{j >= 1} |R_j - R0_j|_F^2 of the rotations tr
+// (row-major entries in j order) against the anchor anc
+__device__ __forceinline__ double lm_kp2d_prior_loss(const LmKp2dArgs &x2, const float *tr, const float *anc, int nr9) {
+  double q = 0.0;
+  for (int i = 9; i < nr9; ++i) {
+    const double d = (double)tr[i] - (double)anc[i];
+    q += d * d;
+  }
+  return 0.5 * (double)x2.pose_w * q;
+}
+
 // Phase 1 of the 2D steps, by one thread: the trial's robust keypoint term (k order) and pose prior, left to right
 __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const LmKp2dArgs &x2, int b, const float *tg,
                                                      const float *wt, const float *anc, bool robust, double s2) {
@@ -611,15 +622,7 @@ __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const Lm
     const double e = dx * dx + dy * dy;
     L += w * (robust ? e * (s2 / (s2 + e)) : e);
   }
-  if (x2.pose_w > 0.f) {
-    const float *tr = a.trot + (size_t)b * nr9;
-    double q = 0.0;
-    for (int i = 9; i < nr9; ++i) {
-      const double d = (double)tr[i] - (double)anc[i];
-      q += d * d;
-    }
-    L += 0.5 * (double)x2.pose_w * q;
-  }
+  if (x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x2, a.trot + (size_t)b * nr9, anc, nr9);
   return L;
 }
 
@@ -687,8 +690,10 @@ __device__ __forceinline__ void lm_kp2d_keypoint_rows(int K, int P, const float 
   }
 }
 
-// Phase 3 of the 2D steps: the pose-prior rows of joint j only reach its diagonal block (columns 3 j .. 3 j + 2, the
-// same in both column orders): no staging
+// Phase 3 of the 2D steps: the pose-prior rows of joint j only reach its diagonal block (parameters 3 j .. 3 j + 2, the
+// same in both column orders): no staging.  Column c of A holds parameter c + SHIFT: 0 in the image steps, 3 in the
+// shared block [delta_1 .. | beta] of the shared-pose group step
+template <int SHIFT = 0>
 __device__ __forceinline__ void lm_kp2d_prior_rows(const LmKp2dArgs &x2, int o, const float *Rst, const float *anc,
                                                    const int (&pr)[kLmKpPairs], const int (&pc)[kLmKpPairs],
                                                    double (&acc)[kLmKpPairs], double &g) {
@@ -697,15 +702,16 @@ __device__ __forceinline__ void lm_kp2d_prior_rows(const LmKp2dArgs &x2, int o, 
     const double hw = 0.5 * (double)x2.pose_w;
 #pragma unroll
     for (int i = 0; i < kLmKpPairs; ++i) {
-      const int j = pr[i] / 3;
-      if (pr[i] >= 3 && pr[i] < o && pc[i] / 3 == j) {
+      const int j = (pr[i] + SHIFT) / 3;
+      if (pr[i] + SHIFT >= 3 && pr[i] + SHIFT < o && (pc[i] + SHIFT) / 3 == j) {
         const float *R = Rst + 9 * j;
-        for (int e = 0; e < 9; ++e) acc[i] += (hw * rot_tangent(R, pr[i] % 3, e)) * rot_tangent(R, pc[i] % 3, e);
+        for (int e = 0; e < 9; ++e)
+          acc[i] += (hw * rot_tangent(R, (pr[i] + SHIFT) % 3, e)) * rot_tangent(R, (pc[i] + SHIFT) % 3, e);
       }
     }
-    if (t >= 3 && t < o) {
-      const float *R = Rst + 9 * (t / 3), *R0 = anc + 9 * (t / 3);
-      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
+    if (t + SHIFT >= 3 && t + SHIFT < o) {
+      const float *R = Rst + 9 * ((t + SHIFT) / 3), *R0 = anc + 9 * ((t + SHIFT) / 3);
+      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, (t + SHIFT) % 3, e)) * ((double)R[e] - (double)R0[e]);
     }
   }
 }
@@ -832,6 +838,22 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
 // one of whose factorisations fails, keeps its state.  Every CTA of a group decides from the same scratch in the same
 // order; no atomics, so a group's bits do not depend on the rest of the batch.  A group of one has the 2D step's loss,
 // lambda and decision bit for bit; its trial differs by the order of elimination.
+//
+// SHARE, the shared-pose group step (shapy_fit_lm_keypoints_2d_shared_pose_step): the images of a group are views of
+// one posed body at one moment, so they also share the body rotations R_g,j, j = 1 .. n_rot - 1 (each relative to its
+// parent); only the global rotation R_0,i (which absorbs the camera's rotation) and the camera c_i are per image.  The
+// group's pose prior is counted once, against a per-group anchor:
+//   L_g = sum_{i in g} (image order) [the 2D step's keypoint term of image i]
+//       + 1/2 pose_w sum_{j >= 1} |R_g,j - R0_g,j|_F^2 (j order, row-major entries; when pose_w > 0)
+//       + the measurement and betas terms as above.
+// The phases are the same with the image block [delta_0 | c] (n1 = 6) and the shared block [delta_1 .. delta_{n_rot-1}
+// | beta] (ns = 3 (n_rot - 1) + nb): the keypoint rows staged in the order [delta_0 | c | delta_1 .. | beta] and no
+// prior rows in launch 2; lm_group_decide adds the prior after the summed brackets, from the group's trial rotations
+// (its first image's rows); launch 3 adds the pose-prior rows of joints 1 .. n_rot - 1 on the group's state rotations
+// (again the first image's rows) before the measurement rows, which go to the betas block at 3 (n_rot - 1), damps the
+// rotation diagonal by lambda and the betas diagonal by betas_w + lambda, and writes R_g,j Exp(dshared_j) identically
+// into every image's trial rows.  The rows of joints 1 .. of every image of a group must hold the same rotations on the
+// first step; the step keeps them so.  With n_rot = 1 nothing is shared but beta, and the step is the grouped step's.
 struct LmGroupArgs {
   int G;
   const int *off;                       // (G + 1) offsets, the device copy in the workspace
@@ -841,8 +863,8 @@ struct LmGroupArgs {
 };
 
 // The slots of an image's scratch: the bracket of its trial loss, the factorisation flag, the max of its first-step
-// keypoint diagonal over [delta | c], then its nb betas diagonal entries, S_i (nb x nb, lower), s_i (nb), X_i (n1 x nb)
-// and x_i (n1)
+// keypoint diagonal over the image block, then its ns shared-column diagonal entries, S_i (ns x ns, lower), s_i (ns),
+// X_i (n1 x ns) and x_i (n1); ns = nb in the grouped step
 constexpr int kScrLoss = 0, kScrOk = 1, kScrDmax = 2, kScrDiag = 3;
 __host__ __device__ inline int lm_group_stride(int n1, int nb) { return kScrDiag + 2 * nb + nb * nb + n1 * nb + n1; }
 inline size_t lm_group_offsets_bytes(int G) { return ((size_t)(G + 1) * sizeof(int) + 15) / 16 * 16; }
@@ -853,12 +875,19 @@ struct LmGroupDecision {
 };
 
 // The group's decision, by one thread, from the images' scratch of launch 1 and the group state: its trial loss L_g,
-// accept (lm_accept), the state's loss after it (lm_loss) and lambda (lm_lambda, the first from the group diagonal)
+// accept (lm_accept), the state's loss after it (lm_loss) and lambda (lm_lambda, the first from the group diagonal).
+// SHARE adds the group's pose prior after the keypoint brackets
+template <bool SHARE>
 __device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &x2, const LmGroupArgs &gr, int g) {
   const int i0 = gr.off[g], i1 = gr.off[g + 1], nb = a.nb;
+  const int ns = SHARE ? a.P - 6 : nb;  // the shared columns
   const double *s0 = gr.scr + (size_t)i0 * gr.stride;
   double L = s0[kScrLoss];
   for (int i = i0 + 1; i < i1; ++i) L += gr.scr[(size_t)i * gr.stride + kScrLoss];
+  if constexpr (SHARE) {
+    const int nr9 = 9 * a.n_rot;
+    if (x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x2, a.trot + (size_t)i0 * nr9, x2.anchor + (size_t)g * nr9, nr9);
+  }
   if (x2.mb.weights) L += lm_meas_loss(x2.mb, g);
   if (x2.betas_w > 0.f) {
     const float *tb = a.tbetas + (size_t)g * nb;
@@ -873,7 +902,7 @@ __device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &
   double dmax = kDiagFloor;
   if (a.first) {
     for (int i = i0; i < i1; ++i) dmax = fmax(dmax, gr.scr[(size_t)i * gr.stride + kScrDmax]);
-    for (int l = 0; l < nb; ++l) {
+    for (int l = 0; l < ns; ++l) {
       double d2 = s0[kScrDiag + l];
       for (int i = i0 + 1; i < i1; ++i) d2 += gr.scr[(size_t)i * gr.stride + kScrDiag + l];
       dmax = fmax(dmax, d2);
@@ -883,17 +912,28 @@ __device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &
   return d;
 }
 
+template <bool SHARE>
 __global__ void __launch_bounds__(128) lm_kp2dg_loss_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
   __shared__ double dg[kLmKpMaxP];
-  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, nb = a.nb, o = 3 * a.n_rot;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, o = 3 * a.n_rot;
+  const int oc = SHARE ? 3 : o, ns = SHARE ? P - 6 : a.nb;   // the first camera column, the shared columns
   const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
   const float *anc = x2.anchor ? x2.anchor + (size_t)b * 9 * a.n_rot : nullptr;
   const bool robust = isfinite(x2.sigma);
   const double s2 = (double)x2.sigma * (double)x2.sigma;
   double *scr = gr.scr + (size_t)b * gr.stride;
-  if (t == 0) scr[kScrLoss] = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
+  if (t == 0) {
+    if constexpr (SHARE) {
+      LmKp2dArgs xk = x2;                 // the keypoint term alone: the group counts its prior once
+      xk.pose_w = 0.f;
+      scr[kScrLoss] = lm_kp2d_trial_loss(a, xk, b, tg, wt, nullptr, robust, s2);
+    } else {
+      scr[kScrLoss] = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
+    }
+  }
   if (!a.first) return;
-  // the first step accepts: the diagonal of the trial's keypoint rows, column t of [delta | c | beta], in row order
+  // the first step accepts: the diagonal of the trial's keypoint rows, column t of [delta | c | beta] (SHARE: [delta_0 |
+  // c | delta_1 .. | beta]), in row order
   if (t < P) {
     const float *J = a.tjac + (size_t)b * 3 * K * P, *M = a.tkp + (size_t)b * 3 * K, *cam = a.tlast + (size_t)b * 3;
     double s, ds;
@@ -904,7 +944,7 @@ __global__ void __launch_bounds__(128) lm_kp2dg_loss_kernel(LmKpArgs a, LmKp2dAr
       double wr, res;
       lm_kp2d_row(M, tg, wt, s, cxy, robust, s2, r >> 1, r & 1, wr, res);
       if (!(wr > 0.0)) continue;
-      const double x = lm_kp2d_entry<true>(J, M, P, o, r >> 1, r & 1, t, s, ds, cxy);
+      const double x = lm_kp2d_entry<true>(J, M, P, oc, r >> 1, r & 1, t, s, ds, cxy);
       d += (wr * x) * x;
     }
     dg[t] = d;
@@ -912,20 +952,22 @@ __global__ void __launch_bounds__(128) lm_kp2dg_loss_kernel(LmKpArgs a, LmKp2dAr
   __syncthreads();
   if (t == 0) {
     double m = kDiagFloor;
-    for (int j = 0; j < o + 3; ++j) m = fmax(m, dg[j]);
+    for (int j = 0; j < oc + 3; ++j) m = fmax(m, dg[j]);
     scr[kScrDmax] = m;
   }
-  if (t < nb) scr[kScrDiag + t] = dg[o + 3 + t];
+  if (t < ns) scr[kScrDiag + t] = dg[oc + 3 + t];
 }
 
+template <bool SHARE>
 __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of the image's normal matrix, then its factor
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
   __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
   __shared__ float lam_s;
   __shared__ int accept_s, ok_s;
-  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nb = a.nb, nr9 = 9 * a.n_rot;
-  const int o = 3 * a.n_rot, n1 = o + 3;      // first camera and first betas column
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nr9 = 9 * a.n_rot;
+  const int o = 3 * a.n_rot, oc = SHARE ? 3 : o, n1 = oc + 3;  // first camera and first shared column
+  const int ns = SHARE ? P - n1 : a.nb;                         // the shared columns
   const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
   const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
   const bool robust = isfinite(x2.sigma);
@@ -938,7 +980,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArg
       if (gr.off[mid] <= b) lo = mid;
       else hi = mid - 1;
     }
-    const LmGroupDecision d = lm_group_decide(a, x2, gr, lo);
+    const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, lo);
     accept_s = d.accept;
     lam_s = d.lam;
     ok_s = 1;
@@ -953,12 +995,12 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArg
   double s, ds;
   softplus_d((double)Cst[0], s, ds);
   const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
-  // 3. the image's normal equations, columns [delta | c | beta]
+  // 3. the image's normal equations, columns [delta | c | beta] (SHARE: [delta_0 | c | delta_1 .. | beta], no prior)
   int pr[kLmKpPairs], pc[kLmKpPairs];
   double acc[kLmKpPairs], g = 0.0;
   lm_kp_pairs(P, pr, pc, acc);
-  lm_kp2d_keypoint_rows<true>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, o, Js, WJs, ws, rs, pr, pc, acc, g);
-  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
+  lm_kp2d_keypoint_rows<true>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc, g);
+  if constexpr (!SHARE) lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
   lm_kp_store(P, A, y, pr, pc, acc, g);
   if (t == 0)
     for (int j = 0; j < n1; ++j) A[j * P + j] += (double)lam_s;
@@ -966,37 +1008,40 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArg
   lm_kp_solve(A, y, P, n1, ok_s);
   // X_i = A_i^-1 B_i: L11^T X = L21^T in place in the rows n1.. of A, as the solve's L^T delta = y, column by column
   for (int j = n1 - 1; j >= 0; --j) {
-    for (int l = t; l < nb; l += blockDim.x) A[(n1 + l) * P + j] /= A[j * P + j];
+    for (int l = t; l < ns; l += blockDim.x) A[(n1 + l) * P + j] /= A[j * P + j];
     __syncthreads();
-    for (int q = t; q < nb * j; q += blockDim.x) {
+    for (int q = t; q < ns * j; q += blockDim.x) {
       const int l = q / j, i = q % j;
       A[(n1 + l) * P + i] -= A[j * P + i] * A[(n1 + l) * P + j];
     }
     __syncthreads();
   }
   double *scr = gr.scr + (size_t)b * gr.stride;
-  double *S = scr + kScrDiag + nb, *sv = S + nb * nb, *X = sv + nb, *xv = X + n1 * nb;
-  for (int q = t; q < nb * nb; q += blockDim.x) {
-    const int r = q / nb, c = q % nb;
+  double *S = scr + kScrDiag + ns, *sv = S + ns * ns, *X = sv + ns, *xv = X + n1 * ns;
+  for (int q = t; q < ns * ns; q += blockDim.x) {
+    const int r = q / ns, c = q % ns;
     S[q] = c <= r ? A[(n1 + r) * P + n1 + c] : 0.0;
   }
-  for (int l = t; l < nb; l += blockDim.x) sv[l] = -y[n1 + l];
-  for (int q = t; q < n1 * nb; q += blockDim.x) X[q] = A[(n1 + q % nb) * P + q / nb];
+  for (int l = t; l < ns; l += blockDim.x) sv[l] = -y[n1 + l];
+  for (int q = t; q < n1 * ns; q += blockDim.x) X[q] = A[(n1 + q % ns) * P + q / ns];
   for (int j = t; j < n1; j += blockDim.x) xv[j] = -y[j];
   if (t == 0) scr[kScrOk] = ok_s ? 1.0 : 0.0;
 }
 
+template <bool SHARE>
 __global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a, LmKp2dArgs x2, LmGroupArgs gr) {
-  extern __shared__ double A[];         // [nb][nb]: S + the measurement rows, then its factor; then delta_i (n1)
+  extern __shared__ double A[];         // [ns][ns]: S + the prior and measurement rows, then its factor; then delta_i (n1)
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // the staged measurement rows
   __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP];
   __shared__ float lam_s;
   __shared__ int accept_s, ok_s;
-  const int g = blockIdx.x, t = threadIdx.x, nb = a.nb, o = 3 * a.n_rot, n1 = o + 3, nr9 = 9 * a.n_rot;
+  const int g = blockIdx.x, t = threadIdx.x, nb = a.nb, o = 3 * a.n_rot, nr9 = 9 * a.n_rot;
+  const int oc = SHARE ? 3 : o, n1 = oc + 3;           // the image block: [delta | c] (SHARE: [delta_0 | c])
+  const int ob = SHARE ? o - 3 : 0, ns = ob + nb;      // the shared block's first betas column and its size
   const int i0 = gr.off[g], i1 = gr.off[g + 1];
   const LmMeasArgs &mb = x2.mb;
   if (t == 0) {
-    const LmGroupDecision d = lm_group_decide(a, x2, gr, g);
+    const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, g);
     accept_s = d.accept;
     lam_s = d.lam;
     if (d.accept) a.loss[g] = d.lnew;
@@ -1013,61 +1058,74 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a
     for (int l = t; l < nb; l += blockDim.x) a.betas[(size_t)g * nb + l] = a.tbetas[(size_t)g * nb + l];
     if (mb.weights) lm_meas_take_trial(mb, g, nb);
   }
-  // S = sum_i S_i, s = sum_i s_i in image order, then the measurement rows and betas_w beta
+  // S = sum_i S_i, s = sum_i s_i in image order, then (SHARE) the pose-prior rows, the measurement rows and betas_w beta
   int pr[kLmKpPairs], pc[kLmKpPairs];
   double acc[kLmKpPairs], gs = 0.0;
-  lm_kp_pairs(nb, pr, pc, acc);
+  lm_kp_pairs(ns, pr, pc, acc);
   for (int i = i0; i < i1; ++i) {
-    const double *S = gr.scr + (size_t)i * gr.stride + kScrDiag + nb;
+    const double *S = gr.scr + (size_t)i * gr.stride + kScrDiag + ns;
 #pragma unroll
     for (int q = 0; q < kLmKpPairs; ++q)
-      if (pr[q] >= 0) acc[q] += S[pr[q] * nb + pc[q]];
-    if (t < nb) gs += S[nb * nb + t];
+      if (pr[q] >= 0) acc[q] += S[pr[q] * ns + pc[q]];
+    if (t < ns) gs += S[ns * ns + t];
   }
+  // the group's state rotations are its first image's rows, which launch 2 updated on accept
+  if constexpr (SHARE)
+    lm_kp2d_prior_rows<3>(x2, o, a.rot + (size_t)i0 * nr9, x2.anchor ? x2.anchor + (size_t)g * nr9 : nullptr, pr, pc,
+                          acc, gs);
   if (mb.weights)
-    lm_meas_add_rows(mb, g, nb, 0, (accept ? mb.tmeas : mb.meas) + (size_t)g * 5,
+    lm_meas_add_rows(mb, g, nb, ob, (accept ? mb.tmeas : mb.meas) + (size_t)g * 5,
                      (accept ? mb.tjac : mb.jac) + (size_t)g * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, gs);
-  if (x2.betas_w > 0.f && t < nb) gs += (double)x2.betas_w * (double)Bst[t];
-  lm_kp_store(nb, A, y, pr, pc, acc, gs);
+  if (x2.betas_w > 0.f && (SHARE ? t >= ob && t < ns : t < nb)) gs += (double)x2.betas_w * (double)Bst[t - ob];
+  lm_kp_store(ns, A, y, pr, pc, acc, gs);
   if (t == 0) {
     const double damp = (double)x2.betas_w + (double)lam_s;
-    for (int j = 0; j < nb; ++j) A[j * nb + j] += damp;
+    for (int j = 0; j < ns; ++j) A[j * ns + j] += SHARE && j < ob ? (double)lam_s : damp;
   }
-  lm_kp_solve(A, y, nb, nb, ok_s);
+  lm_kp_solve(A, y, ns, ns, ok_s);
   const bool ok = ok_s;
-  // the next trial of every image: delta_i = -x_i - X_i dbeta, then R Exp(delta), c + delta_c, beta + dbeta
-  double *dv = A + nb * nb;
+  // the next trial of every image: delta_i = -x_i - X_i dshared, then R Exp(delta), c + delta_c, beta + dbeta; SHARE:
+  // R_j Exp(dshared_j) of the group's rotations (its first image's) into every image's rows, j >= 1
+  double *dv = A + ns * ns;
   for (int i = i0; i < i1; ++i) {
-    const double *X = gr.scr + (size_t)i * gr.stride + kScrDiag + 2 * nb + nb * nb, *xv = X + n1 * nb;
+    const double *X = gr.scr + (size_t)i * gr.stride + kScrDiag + 2 * ns + ns * ns, *xv = X + n1 * ns;
     for (int j = t; j < n1; j += blockDim.x) {
       double v = -xv[j];
-      for (int l = 0; l < nb; ++l) v -= X[j * nb + l] * y[l];
+      for (int l = 0; l < ns; ++l) v -= X[j * ns + l] * y[l];
       dv[j] = v;
     }
     __syncthreads();
     for (int j = t; j < a.n_rot; j += blockDim.x) {
       const float *Rs = a.rot + (size_t)i * nr9 + 9 * j;
       float *Rt = a.trot + (size_t)i * nr9 + 9 * j;
+      if (SHARE && j > 0) {               // a shared rotation: the group's, from its first image's rows
+        Rs = a.rot + (size_t)i0 * nr9 + 9 * j;
+        if (ok) lm_exp_gs(Rs, y[3 * j - 3], y[3 * j - 2], y[3 * j - 1], Rt);
+        else
+          for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
+        continue;
+      }
       if (ok) lm_exp_gs(Rs, dv[3 * j], dv[3 * j + 1], dv[3 * j + 2], Rt);
       else
         for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
     }
     if (t < 3) {
       const float x = a.last[(size_t)i * 3 + t];
-      a.tlast[(size_t)i * 3 + t] = ok ? (float)((double)x + dv[o + t]) : x;
+      a.tlast[(size_t)i * 3 + t] = ok ? (float)((double)x + dv[oc + t]) : x;
     }
     for (int l = t; l < nb; l += blockDim.x)
-      gr.tbetas_img[(size_t)i * nb + l] = ok ? (float)((double)Bst[l] + y[l]) : Bst[l];
+      gr.tbetas_img[(size_t)i * nb + l] = ok ? (float)((double)Bst[l] + y[ob + l]) : Bst[l];
     __syncthreads();
   }
   for (int l = t; l < nb; l += blockDim.x) {
     const float x = Bst[l];
-    a.tbetas[(size_t)g * nb + l] = ok ? (float)((double)x + y[l]) : x;
+    a.tbetas[(size_t)g * nb + l] = ok ? (float)((double)x + y[ob + l]) : x;
   }
 }
 
 // The grouped entries' checks (check_lm_kp's, then the offsets, read on the host) and the three launches; the offsets
-// are copied into the workspace on the stream
+// are copied into the workspace on the stream.  SHARE: the shared-pose entries, with the group anchor
+template <bool SHARE>
 int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpArgs a, LmKp2dArgs x,
                  float *tbetas_img, void *workspace, bool extra_ok, void *stream) {
   const int rc = check_lm_kp(fn, batch, a, extra_ok && offsets && tbetas_img && workspace,
@@ -1081,26 +1139,28 @@ int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
     SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: group %d is empty (offsets %d, %d)", fn, g, offsets[g],
                   offsets[g + 1]);
   if (batch == 0) return SHAPY_OK;
-  const int n1 = 3 * a.n_rot + 3, nb = a.nb;
+  const int n1 = SHARE ? 6 : 3 * a.n_rot + 3, ns = a.P - n1;
   int *off = (int *)workspace;
-  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_group_stride(n1, nb),
+  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_group_stride(n1, ns),
                  tbetas_img};
   cudaStream_t st = (cudaStream_t)stream;
   SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  lm_kp2dg_loss_kernel<<<batch, 128, 0, st>>>(a, x, gr);
+  lm_kp2dg_loss_kernel<SHARE><<<batch, 128, 0, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
   cudaFuncAttributes attr;
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_image_kernel));
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_image_kernel<SHARE>));
   if (smem + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2dg_image_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  lm_kp2dg_image_kernel<<<batch, kLmKpThreads, smem, st>>>(a, x, gr);
+    SHAPY_CUDA_TRY(
+        cudaFuncSetAttribute(lm_kp2dg_image_kernel<SHARE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  lm_kp2dg_image_kernel<SHARE><<<batch, kLmKpThreads, smem, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
-  const size_t smem3 = (size_t)(nb * nb + n1) * sizeof(double);
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_group_kernel));
+  const size_t smem3 = (size_t)(ns * ns + n1) * sizeof(double);
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_group_kernel<SHARE>));
   if (smem3 + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2dg_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-  lm_kp2dg_group_kernel<<<G, kLmKpThreads, smem3, st>>>(a, x, gr);
+    SHAPY_CUDA_TRY(
+        cudaFuncSetAttribute(lm_kp2dg_group_kernel<SHARE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+  lm_kp2dg_group_kernel<SHARE><<<G, kLmKpThreads, smem3, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
@@ -1210,8 +1270,8 @@ extern "C" int shapy_fit_lm_keypoints_2d_groups_step(
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
-  return run_lm_kp2dg("shapy_fit_lm_keypoints_2d_groups_step", batch, num_groups, group_offsets, a, x,
-                      trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+  return run_lm_kp2dg<false>("shapy_fit_lm_keypoints_2d_groups_step", batch, num_groups, group_offsets, a, x,
+                             trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_groups_measurements_step(
@@ -1226,9 +1286,47 @@ extern "C" int shapy_fit_lm_keypoints_2d_groups_measurements_step(
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
                LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
-  return run_lm_kp2dg("shapy_fit_lm_keypoints_2d_groups_measurements_step", batch, num_groups, group_offsets, a, x,
-                      trial_betas_images, workspace,
+  return run_lm_kp2dg<false>("shapy_fit_lm_keypoints_2d_groups_measurements_step", batch, num_groups, group_offsets,
+                             a, x, trial_betas_images, workspace,
                       (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
                           meas_jac && trial_meas && trial_meas_jac,
                       stream);
+}
+
+extern "C" size_t shapy_fit_lm_shared_pose_workspace_bytes(int batch, int num_groups, int n_rot, int nb) {
+  if (batch < 0 || num_groups < 0 || n_rot < 1 || nb < 1) return 0;
+  return lm_group_offsets_bytes(num_groups) + (size_t)batch * lm_group_stride(6, 3 * (n_rot - 1) + nb) * sizeof(double);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *camera,
+    float *keypoints, float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_betas_images, float *trial_camera, const float *trial_keypoints, const float *trial_jac,
+    void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
+  return run_lm_kp2dg<true>("shapy_fit_lm_keypoints_2d_shared_pose_step", batch, num_groups, group_offsets, a, x,
+                            trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
+    int batch, int num_groups, const int32_t *group_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *pose_anchor, float robust_sigma, float pose_prior_weight,
+    float betas_weight, const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down,
+    int first, float *rot, float *betas, float *camera, float *keypoints, float *jac, float *meas, float *meas_jac,
+    float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
+    const float *trial_meas_jac, void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
+               LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
+  return run_lm_kp2dg<true>("shapy_fit_lm_keypoints_2d_shared_pose_measurements_step", batch, num_groups,
+                            group_offsets, a, x, trial_betas_images, workspace,
+                            (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
+                                meas_jac && trial_meas && trial_meas_jac,
+                            stream);
 }

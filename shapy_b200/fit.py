@@ -77,13 +77,21 @@ of every image and ops.fit_lm_keypoints_2d_groups_step, whose three launches eli
 block (a Schur complement) and solve for the group's betas (six launches with measurements), no host synchronisation,
 every group's loss non-increasing.
 
+fit_body_to_keypoints_2d(..., groups=labels, share_pose=True) fits simultaneous views of one posed body: the images of a
+group share the betas and the body pose (joints 1 .., each relative to its parent, so the same in every view), each
+keeps its global rotation and camera.  A weak-perspective view cannot see depth; a limb that one view sees
+foreshortened another sees side-on.  With method='lm' each iteration is the keypoint Jacobian of every image and
+ops.fit_lm_keypoints_2d_shared_pose_step, the grouped step with [global rotation | camera] eliminated per image and
+[body pose | betas] solved per group.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
 With --keypoints-2d, known measurements are read from --targets only (per-body arrays height / mass / ...); --height
 and the other single-target flags are not used there, so a command line without --targets fits the keypoints alone.
 An optional `groups` array (B,) in kp.npz fits the images of one label with one shape; the --targets arrays are then
-per group, and the output carries `groups`.
+per group, and the output carries `groups`.  With --share-pose the images of one label are simultaneous views of one
+posed body: they share the body pose too, and body_pose is then per group in the output.
 
 shapy_b200.keypoints2d reads OpenPose detections and maps them into that frame; with raw detections and their crop
 descriptors in kp.npz, --keypoint-map openpose_smplx_map.json does the same on the command line.
@@ -487,7 +495,7 @@ def _group_sum(x, offsets):
 def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
                              robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
                              body_measurements=None, measurements=None, measurement_weights=None,
-                             circumference_derivative='reference', groups=None):
+                             circumference_derivative='reference', groups=None, share_pose=False):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -516,9 +524,19 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     init betas (image order).  measurements and measurement_weights are then per group ((G,) values or scalars).
     'betas' (G, NB), 'measurements' (G, 5) and 'loss' (G,) are per group, the rest per image in the caller's order.
     With 'lm' the returned loss is the step's fp64 loss of the final state; the images of a group are summed in the
-    caller's order."""
+    caller's order.
+    share_pose: with groups, the images of a group are simultaneous views of one posed body (a synchronised rig, or
+    front and side photos of one held pose) and also share the body pose: each keeps its global rotation (which absorbs
+    the camera's rotation) and camera.  A limb one view sees foreshortened another sees side-on, which a single
+    weak-perspective view cannot.  A group starts from the image-order mean of its images' decoded starting body
+    rotations, made rotations again by the 6D decoder's Gram-Schmidt; pose_anchor is then per group, (G, 22, 3, 3)
+    with the global rows unread, by default that start, and the pose prior counts once per group.  'body_pose' and
+    'body_pose_mat' are then per group as well.  With 'lm' an iteration is the keypoint Jacobian of every image and
+    ops.fit_lm_keypoints_2d_shared_pose_step (six launches with measurements)."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if share_pose and groups is None:
+        raise ValueError('fit_body_to_keypoints_2d: share_pose needs groups')
     exact_circumferences(circumference_derivative)
     if measurements is not None and body_measurements is None:
         raise ValueError('fit_body_to_keypoints_2d: measurements need body_measurements')
@@ -544,14 +562,17 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     w = w.expand(B, K).contiguous()
     params = _init_2d(init, B, nb, device, method)
     rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
-    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
-                                                              device=device).reshape(B, 22, 3, 3).contiguous()
+    if share_pose:          # per group: its shape is checked once the groups are known
+        anchor = None if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32, device=device)
+    else:
+        anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
+                                                                  device=device).reshape(B, 22, 3, 3).contiguous()
     sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
     pw, bw = float(pose_prior_weight), float(betas_weight)
     if groups is not None:
         return _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, int(iterations), sigma, pw, bw,
                                         lr, groups, body_measurements, measurements, measurement_weights,
-                                        circumference_derivative)
+                                        circumference_derivative, bool(share_pose))
     mterms = None
     if measurements is not None:
         tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
@@ -628,9 +649,9 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
 
 
 def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, iterations, sigma, pw, bw, lr, groups,
-                             body_measurements, measurements, measurement_weights, cd):
+                             body_measurements, measurements, measurement_weights, cd, share_pose=False):
     """fit_body_to_keypoints_2d with groups: the images sorted by group once, fitted, and returned in the caller's
-    order."""
+    order; share_pose: the body pose per group too, anchor None or the caller's per-group anchor."""
     from . import ops
     from .autograd import Rot6dFunction
     device = x.device
@@ -641,10 +662,23 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
     od = _to_device(order, device)
     inv = torch.argsort(od)
     gidx = _to_device(torch.repeat_interleave(torch.arange(G), counts), device)     # each sorted image's group
-    x, w, rot0, anchor = x[od].contiguous(), w[od].contiguous(), rot0[od].contiguous(), anchor[od].contiguous()
+    x, w, rot0 = x[od].contiguous(), w[od].contiguous(), rot0[od].contiguous()
     sp = {k: v.detach()[od].contiguous() for k, v in params.items()}
     cnt = _to_device(counts.float(), device)
     betas0 = (_group_sum(sp['betas'], offsets) / cnt[:, None]).contiguous() if G else torch.zeros(0, nb, device=device)
+    if share_pose:
+        first = _to_device(offsets[:-1].long(), device)                              # each group's first image
+        raw0 = _shared_body_raw(rot0, offsets, cnt)
+        body0 = ops.decode_rot6d(raw0) if G else rot0.new_zeros(0, 21, 3, 3)
+        rot0 = torch.cat([rot0[:, :1], body0[gidx]], 1).contiguous()
+        if anchor is None:
+            anchor = torch.cat([rot0[first, :1], body0], 1).contiguous()
+        elif anchor.numel() != G * 22 * 9:
+            raise ValueError(f'fit_body_to_keypoints_2d: with share_pose, pose_anchor must be ({G}, 22, 3, 3)')
+        else:
+            anchor = anchor.reshape(G, 22, 3, 3).contiguous()
+    else:
+        anchor = anchor[od].contiguous()
     mterms = None
     if measurements is not None:
         tgt, wt = _measurement_terms(measurements, measurement_weights, G, device)
@@ -662,7 +696,10 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
             state.update(meas=mk(G, 5), meas_jac=mk(G, 5, nb))
         pose_anchor = anchor if pw > 0 else None
         if B > 0:
-            ws = ops.fit_lm_groups_workspace(B, G, 22, nb, device)
+            ws = (ops.fit_lm_shared_pose_workspace if share_pose else ops.fit_lm_groups_workspace)(B, G, 22, nb, device)
+            step = ops.fit_lm_keypoints_2d_shared_pose_step if share_pose else ops.fit_lm_keypoints_2d_groups_step
+            mstep = (ops.fit_lm_keypoints_2d_shared_pose_measurements_step if share_pose else
+                     ops.fit_lm_keypoints_2d_groups_measurements_step)
             exact = exact_circumferences(cd)
             lm = body_measurements.landmarks() if mterms is not None else None
             if mterms is not None:
@@ -670,14 +707,13 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
             for it in range(iterations + 1):
                 tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['image_betas'], trial['rot'])
                 if mterms is None:
-                    ops.fit_lm_keypoints_2d_groups_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0,
-                                                        tkp, tjac, offsets, ws, pose_anchor=pose_anchor)
+                    step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, offsets, ws,
+                         pose_anchor=pose_anchor)
                 else:
                     v = ops.smplx_forward_shape(packed, trial['betas'])
                     tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-                    ops.fit_lm_keypoints_2d_groups_measurements_step(
-                        state, trial, x, w, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0, tkp, tjac,
-                        tm, tmj, offsets, ws, pose_anchor=pose_anchor)
+                    mstep(state, trial, x, w, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0, tkp, tjac,
+                          tm, tmj, offsets, ws, pose_anchor=pose_anchor)
         rot = state['rot']
         with torch.no_grad():
             out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'][gidx],
@@ -686,17 +722,30 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
                             loss=state['loss'])
         if mterms is not None:
             res['measurements'] = state['meas']
+        if share_pose:
+            for k in ('body_pose', 'body_pose_mat'):
+                res[k] = res[k][first]
     else:
         p = {k: sp[k].clone().requires_grad_(True) for k in ('global_rot', 'body_pose', 'camera')}
+        if share_pose:
+            p['body_pose'] = raw0.clone().requires_grad_(True)
         p['betas'] = betas0.clone().requires_grad_(True)
 
         def loss_fn():
             grot = Rot6dFunction.apply(p['global_rot'])
             bpose = Rot6dFunction.apply(p['body_pose'])
-            out = body_model(global_rot=grot, body_pose=bpose, betas=p['betas'][gidx], camera=p['camera'],
+            body = bpose[gidx] if share_pose else bpose
+            out = body_model(global_rot=grot, body_pose=body, betas=p['betas'][gidx], camera=p['camera'],
                              return_shaped=False)
-            rot = torch.cat([grot, bpose], 1)
-            per_group = _group_sum(_kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, 0.0, None), offsets)
+            if share_pose:      # the keypoint terms per image, the pose prior once per group
+                per_group = _group_sum(_kp2d_loss(out['proj_joints'], x, w, sigma, 0.0, None, None, 0.0, None),
+                                       offsets)
+                if pw > 0:
+                    per_group = per_group + 0.5 * pw * (bpose - anchor[:, 1:]).pow(2).sum((1, 2, 3))
+            else:
+                rot = torch.cat([grot, bpose], 1)
+                per_group = _group_sum(_kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, 0.0, None),
+                                       offsets)
             meas = None
             if mterms is not None:
                 v = body_model.forward_shape(betas=p['betas'])['v_shaped']
@@ -713,9 +762,20 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
                    proj_joints=out['proj_joints'], loss=per_group)
         if meas is not None:
             res['measurements'] = meas
-    for k in ('global_rot', 'body_pose', 'camera', 'global_rot_mat', 'body_pose_mat', 'keypoints', 'proj_joints'):
+    per_image = ('global_rot', 'camera', 'global_rot_mat', 'keypoints', 'proj_joints')
+    for k in per_image if share_pose else per_image + ('body_pose', 'body_pose_mat'):
         res[k] = res[k][inv]
     return res
+
+
+def _shared_body_raw(rot0, offsets, cnt):
+    """A group's starting body pose as raw 6D (G, 126): the image-order mean of its images' (sorted by group) rotations
+    of joints 1 .., as the 6D decoder's input, its first two columns; the decoder's Gram-Schmidt makes it rotations."""
+    G = offsets.numel() - 1
+    if G == 0:
+        return rot0.new_zeros(0, 6 * 21)
+    mean = _group_sum(rot0[:, 1:], offsets) / cnt[:, None, None, None]
+    return mean[..., :2].reshape(G, 6 * 21).contiguous()
 
 
 def main(argv=None):
@@ -759,6 +819,9 @@ def main(argv=None):
                         'e.g. a saved regressor prediction')
     p.add_argument('--robust-sigma', dest='robust_sigma', type=float, default=None)
     p.add_argument('--pose-prior-weight', dest='pose_prior_weight', type=float, default=0.0)
+    p.add_argument('--share-pose', dest='share_pose', action='store_true',
+                   help="with --keypoints-2d and a `groups` array: the images of a group are simultaneous views of "
+                        "one posed body and share its body pose as well as its shape")
     a = p.parse_args(argv)
 
     from . import synth
@@ -815,7 +878,8 @@ def _main_keypoints_2d(a, model, bm, targets):
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
-                                   circumference_derivative=a.circumference_derivative, groups=groups)
+                                   circumference_derivative=a.circumference_derivative, groups=groups,
+                                   share_pose=a.share_pose)
     out = {k: v.detach().cpu().numpy() for k, v in res.items()}
     if groups is not None:
         out['groups'] = groups

@@ -784,9 +784,9 @@ def fit_lm_groups_workspace(B, G, n_rot, nb, device):
 
 def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
                         lambda_down, first, trial_keypoints, trial_jac, group_offsets, workspace, pose_anchor,
-                        meas=None):
-    """What the two grouped 2D steps share: the checks and the call, `meas` None or (meas_targets, meas_weights,
-    trial_meas, trial_meas_jac), all (G, ...)."""
+                        meas=None, share_pose=False):
+    """What the four grouped 2D steps share: the checks and the call, `meas` None or (meas_targets, meas_weights,
+    trial_meas, trial_meas_jac), all (G, ...); share_pose: the shared-pose steps, with a per-group pose_anchor."""
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
     sigma = float('inf') if robust_sigma is None else float(robust_sigma)
@@ -810,8 +810,9 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
     P = 3 * n_rot + nb + 3
     if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
-    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
-        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    na = G if share_pose else B
+    if pose_anchor is not None and pose_anchor.shape != (na, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({na}, {n_rot}, 3, 3)')
     if (state['betas'].shape != (G, nb) or trial['betas'].shape != (G, nb) or trial['image_betas'].shape != (B, nb) or
             any(state[k].shape != (G,) for k in ('loss', 'lambda', 'accepted'))):
         raise RuntimeError(f'{what}: betas and trial betas must be ({G}, {nb}), image_betas ({B}, {nb}) and loss, '
@@ -819,7 +820,9 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
     if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], G, nb):
         raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
                            f'({G}, 5)')
-    need = lib().shapy_fit_lm_groups_workspace_bytes(B, G, n_rot, nb)
+    L = lib()
+    need = (L.shapy_fit_lm_shared_pose_workspace_bytes if share_pose else L.shapy_fit_lm_groups_workspace_bytes)(
+        B, G, n_rot, nb)
     if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
         raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
     if B == 0:
@@ -831,12 +834,16 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
           ptr(trial_keypoints), ptr(trial_jac)]
     with torch.cuda.device(trial['rot'].device):
         if meas is None:
-            check(lib().shapy_fit_lm_keypoints_2d_groups_step(
+            step = L.shapy_fit_lm_keypoints_2d_shared_pose_step if share_pose else \
+                L.shapy_fit_lm_keypoints_2d_groups_step
+            check(step(
                 *head, *lam,
                 *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
                 *tr, ptr(workspace), stream_ptr()), what)
         else:
-            check(lib().shapy_fit_lm_keypoints_2d_groups_measurements_step(
+            step = L.shapy_fit_lm_keypoints_2d_shared_pose_measurements_step if share_pose else \
+                L.shapy_fit_lm_keypoints_2d_groups_measurements_step
+            check(step(
                 *head, ptr(meas[0]), ptr(meas[1]), *lam,
                 *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
                                           'lambda', 'accepted')],
@@ -868,3 +875,37 @@ def fit_lm_keypoints_2d_groups_measurements_step(state, trial, targets, weights,
     _fit_lm_kp2d_groups('fit_lm_keypoints_2d_groups_measurements_step', state, trial, targets, weights, robust_sigma,
                         pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
                         group_offsets, workspace, pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac))
+
+
+def fit_lm_shared_pose_workspace(B, G, n_rot, nb, device):
+    """The scratch of the shared-pose 2D step (include/shapy_b200.h, shapy_fit_lm_shared_pose_workspace_bytes): a uint8
+    CUDA tensor, allocated once before an LM loop."""
+    n = lib().shapy_fit_lm_shared_pose_workspace_bytes(int(B), int(G), int(n_rot), int(nb))
+    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+
+
+def fit_lm_keypoints_2d_shared_pose_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight,
+                                         lambda_up, lambda_down, first, trial_keypoints, trial_jac, group_offsets,
+                                         workspace, pose_anchor=None):
+    """fit_lm_keypoints_2d_groups_step for simultaneous views of one posed body (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_shared_pose_step), in place: the images of a group also share the body rotations of
+    joints 1 .., each keeps its global rotation and camera.  state and trial as fit_lm_keypoints_2d_groups_step's;
+    'rot' stays per image, and every image of a group holds the group's body rotations in rows 1 .. (the step reads
+    the first image's and writes all).  pose_anchor (G, n_rot, 3, 3), joint 0 unread; the pose prior counts once per
+    group.  workspace from fit_lm_shared_pose_workspace.  Three launches, no host synchronisation."""
+    _fit_lm_kp2d_groups('fit_lm_keypoints_2d_shared_pose_step', state, trial, targets, weights, robust_sigma,
+                        pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                        group_offsets, workspace, pose_anchor, share_pose=True)
+
+
+def fit_lm_keypoints_2d_shared_pose_measurements_step(state, trial, targets, weights, robust_sigma, pose_prior_weight,
+                                                      betas_weight, meas_targets, meas_weights, lambda_up,
+                                                      lambda_down, first, trial_keypoints, trial_jac, trial_meas,
+                                                      trial_meas_jac, group_offsets, workspace, pose_anchor=None):
+    """fit_lm_keypoints_2d_shared_pose_step with the five measurements of each group (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_shared_pose_measurements_step), in place; the measurement arguments as
+    fit_lm_keypoints_2d_groups_measurements_step's."""
+    _fit_lm_kp2d_groups('fit_lm_keypoints_2d_shared_pose_measurements_step', state, trial, targets, weights,
+                        robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints,
+                        trial_jac, group_offsets, workspace, pose_anchor,
+                        (meas_targets, meas_weights, trial_meas, trial_meas_jac), share_pose=True)
