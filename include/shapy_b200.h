@@ -327,6 +327,41 @@ int shapy_fit_lm_keypoints_2d_measurements_step(
     int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_camera, const float *trial_keypoints,
     const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream);
 
+/* shapy_fit_lm_keypoints_2d_step under a perspective camera with known intrinsics: one Levenberg-Marquardt step per
+ * body of the fit of pose, shape and translation to K 2D keypoints.  Camera frame x right, y down, z forward;
+ * intrinsics (B,3) = (f, px, py) per body, f > 0, in the units of the targets (pixels, or any other: the kernel does
+ * not care).  Parameters [delta_j (3 n_rot) | beta (nb) | t], P = 3 n_rot + nb + 3, the translation t (B,3) in the
+ * place of the camera.  With Y_k = kp_k + t (fp64, kp_k the keypoint of shapy_smplx_keypoint_jacobian without transl):
+ *   p_k = f (Y_k,x / Y_k,z, Y_k,y / Y_k,z) + (px, py);
+ * the loss is the 2D step's term for term with this p_k: sum_{w_k > 0} w_k rho(|p_k - x_k|^2) (k order) +
+ * pose_prior_weight / 2 sum_{j >= 1} |R_j - R0_j|_F^2 + betas_weight |beta|^2.  Keypoint rows 2k + c (IRLS weights at
+ * the state): (f / Y_z) (J_{3k+c} - (Y_c / Y_z) J_{3k+2}) on the rotation and betas columns, and on the t columns with
+ * J_t = I (the transl columns of jac are not read).  Depth rule: a trial with a weighted keypoint at Y_z <= 0 or
+ * non-finite has loss +inf and is rejected (a point behind the camera would project mirrored); a start that breaks the
+ * rule, or a body whose f is not finite and > 0, has a non-finite loss, reports NaN and does not move.  Pose-prior
+ * rows, first lambda, damping, solve and next trial (t + delta_t rounded to fp32) are the 2D step's.  A null
+ * intrinsics, like any null pointer, is SHAPY_ERR_ARG; other errors as shapy_fit_lm_keypoints_2d_step.  batch 0: no
+ * launch.  Deterministic, no atomics, per-body independent. */
+int shapy_fit_lm_keypoints_2d_perspective_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints,
+    float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_perspective_step with the five virtual measurements stacked under its rows, as
+ * shapy_fit_lm_keypoints_2d_measurements_step is to shapy_fit_lm_keypoints_2d_step (same loss order, rows, first
+ * lambda and arguments).  A known height fixes the body's metric size; with a known focal length the projected size
+ * then fixes its distance.  With every measurement weight <= 0 every output equals
+ * shapy_fit_lm_keypoints_2d_perspective_step's bit for bit. */
+int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream);
+
 /* shapy_fit_lm_keypoints_2d_step over groups of images of one person: the images [group_offsets[g],
  * group_offsets[g+1]) of group g share one beta_g, each keeps its own rotations and camera.  Loss per group, fp64, left
  * to right: the sum over its images (image order) of the 2D step's keypoint term and pose prior, + betas_weight

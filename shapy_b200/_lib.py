@@ -104,6 +104,14 @@ _SIGS = {
                                                             C.c_float, C.c_float, C.c_float, c_void_p, c_void_p,
                                                             C.c_float, C.c_float, c_int]
                                                     + [c_void_p] * 17 + [c_void_p]),
+    'shapy_fit_lm_keypoints_2d_perspective_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                                           c_void_p, C.c_float, C.c_float, C.c_float, C.c_float,
+                                                           C.c_float, c_int] + [c_void_p] * 13 + [c_void_p]),
+    'shapy_fit_lm_keypoints_2d_perspective_measurements_step': (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                                        c_void_p, c_void_p, C.c_float, C.c_float,
+                                                                        C.c_float, c_void_p, c_void_p, C.c_float,
+                                                                        C.c_float, c_int]
+                                                                + [c_void_p] * 17 + [c_void_p]),
     'shapy_fit_lm_groups_workspace_bytes': (C.c_size_t, [c_int, c_int, c_int, c_int]),
     'shapy_fit_lm_keypoints_2d_groups_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                                       c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,

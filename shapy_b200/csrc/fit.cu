@@ -11,6 +11,8 @@
 // Everything but the final roundings is fp64, the file is compiled with -fmad=false and every sum has a fixed order, so
 // oracle/lm_oracle.py restates the decisions exactly.  No host synchronisation, no atomics: a body's trajectory is
 // bit-identical from run to run and independent of the rest of the batch.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace shapy {
@@ -567,11 +569,53 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
 // block of A and g after the pose-prior rows and before betas_w beta.  They do not count for the first lambda.  With
 // every measurement weight <= 0 the loss gains an exact 0 and no row is added, so the step equals the 2D step bit for
 // bit, for any sigma, pose prior and betas_w.
+//
+// The perspective 2D step (shapy_fit_lm_keypoints_2d_perspective_step, and _measurements_ with MEAS) is the same kernel
+// with the projection of a pinhole camera of known intrinsics (f, px, py) per body: camera frame x right, y down, z
+// forward, the last three parameters the translation t.  With Y_k = kp_k + t (fp64),
+//   p_k = f (Y_k,x / Y_k,z, Y_k,y / Y_k,z) + (px, py);
+// the loss is the 2D step's term for term with this p_k, and keypoint row 2k + c is (f / Y_z) (J_{3k+c} - (Y_c / Y_z)
+// J_{3k+2}) on every column, J_t = I on the t columns.  Depth rule: a trial with a weighted keypoint at Y_z <= 0 or
+// non-finite, or a body whose f is not finite and > 0, has loss +inf: it is rejected, and a start that breaks the rule
+// reports NaN and does not move.  The pose-prior and measurement rows, lambda, damping, solve and next trial (t +
+// delta_t) are the 2D step's.
 struct LmKp2dArgs {                     // what the 2D step takes beside LmKpArgs (targets (B, K, 2), last = camera)
   const float *anchor;                  // (B, n_rot, 3, 3), or null without a pose prior
   float sigma, pose_w, betas_w;
   LmMeasArgs mb;                        // the MEAS step's block (unused otherwise); its rho is not read: betas_w is the
 };                                      // one betas regulariser
+
+// The perspective step's arguments: the intrinsics ride after LmKp2dArgs, so that the grouped kernels, which take
+// LmKp2dArgs before their own block, keep their parameter layout
+struct LmKp2dPerspArgs : LmKp2dArgs {
+  const float *intr;                    // (B, 3): f, px, py
+};
+
+template <bool PERSP>
+using Kp2dX = std::conditional_t<PERSP, LmKp2dPerspArgs, LmKp2dArgs>;
+
+// One body's pinhole camera at a point of the fit: focal length, principal point and translation t, in fp64
+struct PerspCam {
+  double f, pp[2], t[3];
+};
+
+__device__ __forceinline__ PerspCam persp_cam(const float *in, const float *t) {
+  return PerspCam{(double)in[0], {(double)in[1], (double)in[2]}, {(double)t[0], (double)t[1], (double)t[2]}};
+}
+
+// Y_k = kp_k + t and the residual p_k - x_k of the perspective projection, in fp64
+__device__ __forceinline__ void persp_residual(const float *m, const float *tg, const PerspCam &pc, int k, double (&Y)[3],
+                                               double &dx, double &dy) {
+  for (int c = 0; c < 3; ++c) Y[c] = (double)m[3 * k + c] + pc.t[c];
+  dx = pc.f * (Y[0] / Y[2]) + pc.pp[0] - (double)tg[2 * k];
+  dy = pc.f * (Y[1] / Y[2]) + pc.pp[1] - (double)tg[2 * k + 1];
+}
+
+// The perspective rows' factors f / Y_z and Y_c / Y_z per staged row: shared memory only the perspective kernels have
+__device__ __forceinline__ double *lm_persp_factors() {
+  __shared__ double fz[2 * kLmKpRows];
+  return fz;
+}
 
 // softplus(c0) and its derivative, with F.softplus' threshold of 20 (smplx.cu's projection)
 __device__ __forceinline__ void softplus_d(double c0, double &s, double &ds) {
@@ -605,20 +649,32 @@ __device__ __forceinline__ double lm_kp2d_prior_loss(const LmKp2dArgs &x2, const
   return 0.5 * (double)x2.pose_w * q;
 }
 
-// Phase 1 of the 2D steps, by one thread: the trial's robust keypoint term (k order) and pose prior, left to right
+// Phase 1 of the 2D steps, by one thread: the trial's robust keypoint term (k order) and pose prior, left to right.
+// PERSP: the projection of the trial's camera pc, +inf under the depth rule
+template <bool PERSP = false>
 __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const LmKp2dArgs &x2, int b, const float *tg,
-                                                     const float *wt, const float *anc, bool robust, double s2) {
+                                                     const float *wt, const float *anc, bool robust, double s2,
+                                                     const PerspCam *pc = nullptr) {
   const int K = a.K, R3 = 3 * a.K, nr9 = 9 * a.n_rot;
   const float *m = a.tkp + (size_t)b * R3, *cam = a.tlast + (size_t)b * 3;
   double s, ds;
   softplus_d((double)cam[0], s, ds);
   const double cx = cam[1], cy = cam[2];
+  if constexpr (PERSP)
+    if (!(pc->f > 0.0) || !isfinite(pc->f)) return INFINITY;
   double L = 0.0;
   for (int k = 0; k < K; ++k) {
     const double w = wt[k];
     if (!(w > 0.0)) continue;
-    const double dx = s * ((double)m[3 * k] + cx) - (double)tg[2 * k];
-    const double dy = s * ((double)m[3 * k + 1] + cy) - (double)tg[2 * k + 1];
+    double dx, dy;
+    if constexpr (PERSP) {
+      double Y[3];
+      persp_residual(m, tg, *pc, k, Y, dx, dy);
+      if (!(Y[2] > 0.0) || !isfinite(Y[2])) return INFINITY;
+    } else {
+      dx = s * ((double)m[3 * k] + cx) - (double)tg[2 * k];
+      dy = s * ((double)m[3 * k + 1] + cy) - (double)tg[2 * k + 1];
+    }
     const double e = dx * dx + dy * dy;
     L += w * (robust ? e * (s2 / (s2 + e)) : e);
   }
@@ -627,16 +683,26 @@ __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const Lm
 }
 
 // Phase 3 of the 2D steps: row c of keypoint k at the state (keypoints M, scale s, offset cxy), its weight w_k q_k^2 (the
-// IRLS weight, w_k at sigma = inf) and residual; a dropped keypoint (w_k <= 0) keeps w_k and a zero residual
+// IRLS weight, w_k at sigma = inf) and residual; a dropped keypoint (w_k <= 0) keeps w_k and a zero residual.  PERSP:
+// the state's camera pc, and the row's factors f / Y_z, Y_c / Y_z into fz[0], fz[1]
+template <bool PERSP = false>
 __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, const float *wt, double s,
                                             const double (&cxy)[2], bool robust, double s2, int k, int c, double &wr,
-                                            double &res) {
+                                            double &res, const PerspCam *pc = nullptr, double *fz = nullptr) {
   const double w = wt[k];
   wr = w;
   res = 0.0;
   if (w > 0.0) {
-    const double dx = s * ((double)M[3 * k] + cxy[0]) - (double)tg[2 * k];
-    const double dy = s * ((double)M[3 * k + 1] + cxy[1]) - (double)tg[2 * k + 1];
+    double dx, dy;
+    if constexpr (PERSP) {
+      double Y[3];
+      persp_residual(M, tg, *pc, k, Y, dx, dy);
+      fz[0] = pc->f / Y[2];
+      fz[1] = Y[c] / Y[2];
+    } else {
+      dx = s * ((double)M[3 * k] + cxy[0]) - (double)tg[2 * k];
+      dy = s * ((double)M[3 * k + 1] + cxy[1]) - (double)tg[2 * k + 1];
+    }
     if (robust) {
       const double q = s2 / (s2 + (dx * dx + dy * dy));
       wr = w * (q * q);
@@ -646,32 +712,43 @@ __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, con
 }
 
 // Column col of that row, the camera columns at oc: s J_{3k+c} on the rotation and betas columns, ds (kp_kc + c_{1+c})
-// on c0, s on c_{1+c}.  REORDER: columns [delta | c | beta] (the grouped step), else [delta | beta | c]
-template <bool REORDER>
+// on c0, s on c_{1+c}.  REORDER: columns [delta | c | beta] (the grouped step), else [delta | beta | c].  PERSP (columns
+// [delta | beta | t]): fz[0] (J_{3k+c} - fz[1] J_{3k+2}) with the row's factors fz, J_t = I
+template <bool REORDER, bool PERSP = false>
 __device__ __forceinline__ double lm_kp2d_entry(const float *J, const float *M, int P, int oc, int k, int c, int col,
-                                                double s, double ds, const double (&cxy)[2]) {
+                                                double s, double ds, const double (&cxy)[2],
+                                                const double *fz = nullptr) {
+  if constexpr (PERSP) {
+    const double jc = col < oc ? (double)J[(size_t)(3 * k + c) * P + col] : (col - oc == c ? 1.0 : 0.0);
+    const double jz = col < oc ? (double)J[(size_t)(3 * k + 2) * P + col] : (col - oc == 2 ? 1.0 : 0.0);
+    return fz[0] * (jc - fz[1] * jz);
+  }
   const bool betas = REORDER && col > oc + 2;
   if (col < oc || betas) return s * (double)J[(size_t)(3 * k + c) * P + (betas ? col - 3 : col)];
   if (col == oc) return ds * ((double)M[3 * k + c] + cxy[c]);
   return col - oc - 1 == c ? s : 0.0;
 }
 
-// Phase 3 of the 2D steps: the keypoint rows 2k + c, staged kLmKpRows at a time and accumulated in row order
-template <bool REORDER>
+// Phase 3 of the 2D steps: the keypoint rows 2k + c, staged kLmKpRows at a time and accumulated in row order.  PERSP:
+// the perspective rows of the state's camera cam
+template <bool REORDER, bool PERSP = false>
 __device__ __forceinline__ void lm_kp2d_keypoint_rows(int K, int P, const float *J, const float *M,
                                                       const float *tg, const float *wt, double s, double ds,
                                                       const double (&cxy)[2], bool robust, double s2, int oc,
                                                       double (*Js)[kLmKpMaxP], double (*WJs)[kLmKpMaxP], double *ws,
                                                       double *rs, const int (&pr)[kLmKpPairs],
                                                       const int (&pc)[kLmKpPairs], double (&acc)[kLmKpPairs],
-                                                      double &g) {
+                                                      double &g, const PerspCam *cam = nullptr) {
   const int t = threadIdx.x, R2 = 2 * K;
+  double *fz = nullptr;
+  if constexpr (PERSP) fz = lm_persp_factors();
   for (int r0 = 0; r0 < R2; r0 += kLmKpRows) {
     const int nr = min(kLmKpRows, R2 - r0);
     __syncthreads();
     for (int i = t; i < nr; i += blockDim.x) {   // row weight (IRLS at the state) and residual
       double wr, res;
-      lm_kp2d_row(M, tg, wt, s, cxy, robust, s2, (r0 + i) >> 1, (r0 + i) & 1, wr, res);
+      lm_kp2d_row<PERSP>(M, tg, wt, s, cxy, robust, s2, (r0 + i) >> 1, (r0 + i) & 1, wr, res, cam,
+                         PERSP ? fz + 2 * i : nullptr);
       ws[i] = wr;
       rs[i] = res;
     }
@@ -680,7 +757,8 @@ __device__ __forceinline__ void lm_kp2d_keypoint_rows(int K, int P, const float 
       const int row = i / P, col = i % P;
       const double wr = ws[row];
       if (wr > 0.0) {                    // a dropped keypoint's rows are never read: they may be NaN
-        const double x = lm_kp2d_entry<REORDER>(J, M, P, oc, (r0 + row) >> 1, (r0 + row) & 1, col, s, ds, cxy);
+        const double x = lm_kp2d_entry<REORDER, PERSP>(J, M, P, oc, (r0 + row) >> 1, (r0 + row) & 1, col, s, ds, cxy,
+                                                       PERSP ? fz + 2 * row : nullptr);
         Js[row][col] = x;
         WJs[row][col] = wr * x;
       }
@@ -716,8 +794,8 @@ __device__ __forceinline__ void lm_kp2d_prior_rows(const LmKp2dArgs &x2, int o, 
   }
 }
 
-template <bool MEAS>
-__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, LmKp2dArgs x2) {
+template <bool MEAS, bool PERSP = false>
+__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, Kp2dX<PERSP> x2) {
   extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
   __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
   __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP], dg[kLmKpMaxP];
@@ -732,7 +810,13 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   const float lcur = a.loss[b];
   // 1. trial loss
   if (t == 0) {
-    double L = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
+    double L;
+    if constexpr (PERSP) {
+      const PerspCam tc = persp_cam(x2.intr + (size_t)b * 3, a.tlast + (size_t)b * 3);
+      L = lm_kp2d_trial_loss<true>(a, x2, b, tg, wt, anc, robust, s2, &tc);
+    } else {
+      L = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
+    }
     if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
     if (x2.betas_w > 0.f) {
       const float *tb = a.tbetas + (size_t)b * nb;
@@ -763,7 +847,13 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
   int pr[kLmKpPairs], pc[kLmKpPairs];
   double acc[kLmKpPairs], g = 0.0;
   lm_kp_pairs(P, pr, pc, acc);
-  lm_kp2d_keypoint_rows<false>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc, g);
+  if constexpr (PERSP) {
+    const PerspCam sc = persp_cam(x2.intr + (size_t)b * 3, Cst);
+    lm_kp2d_keypoint_rows<false, true>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc,
+                                       g, &sc);
+  } else {
+    lm_kp2d_keypoint_rows<false>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc, g);
+  }
 #pragma unroll
   for (int i = 0; i < kLmKpPairs; ++i)
     if (pr[i] >= 0 && pr[i] == pc[i]) dg[pr[i]] = acc[i];     // the diagonal of the keypoint rows: the first lambda
@@ -1249,6 +1339,45 @@ extern "C" int shapy_fit_lm_keypoints_2d_measurements_step(
   return run_lm_kp("shapy_fit_lm_keypoints_2d_measurements_step", lm_kp2d_step_kernel<true>, batch, a, x,
                    (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas && meas_jac &&
                        trial_meas && trial_meas_jac,
+                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
+                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                   "lambda_down >= 1",
+                   stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_perspective_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints,
+    float *jac, float *loss, float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dPerspArgs x{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics};
+  return run_lm_kp("shapy_fit_lm_keypoints_2d_perspective_step", lm_kp2d_step_kernel<false, true>, batch, a, x,
+                   intrinsics && (pose_anchor || !(pose_prior_weight > 0.f)),
+                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
+                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                   "lambda_down >= 1",
+                   stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
+    int batch, int num_keypoints, int n_rot, int nb, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dPerspArgs x{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
+                     LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}},
+                    intrinsics};
+  return run_lm_kp("shapy_fit_lm_keypoints_2d_perspective_measurements_step", lm_kp2d_step_kernel<true, true>, batch,
+                   a, x,
+                   intrinsics && (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
+                       meas_jac && trial_meas && trial_meas_jac,
                    robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
                    "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                    "lambda_down >= 1",

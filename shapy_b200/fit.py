@@ -84,12 +84,24 @@ foreshortened another sees side-on.  With method='lm' each iteration is the keyp
 ops.fit_lm_keypoints_2d_shared_pose_step, the grouped step with [global rotation | camera] eliminated per image and
 [body pose | betas] solved per group.
 
+fit_body_to_keypoints_2d(..., focal_length=f, principal_point=pp) fits under a perspective camera with known
+intrinsics instead: the keypoints in the intrinsics' units (usually pixels), the last three parameters the body's
+translation t in the camera frame (x right, y down, z forward), p_k = f (Y_x / Y_z, Y_y / Y_z) + pp with Y_k =
+joint_k + t (PerspectiveCamera).  A weak-perspective camera cannot see depth; a pinhole camera sees a limb nearer the
+camera larger, and with a known height a known focal length fixes the body's distance.  With method='lm' each
+iteration is the keypoint Jacobian and ops.fit_lm_keypoints_2d_perspective_step (four launches with measurements), no
+host synchronisation.  A trial with a weighted keypoint at Y_z <= 0 is rejected, and a body whose start has one
+reports an infinite loss.  perspective_start converts the regressor's crop camera into a starting translation.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
 With --keypoints-2d, known measurements are read from --targets only (per-body arrays height / mass / ...); --height
 and the other single-target flags are not used there, so a command line without --targets fits the keypoints alone.
-An optional `groups` array (B,) in kp.npz fits the images of one label with one shape; the --targets arrays are then
+With a `focal_length` (scalar or (B,)) in kp.npz, and `principal_point` ((2,) or (B, 2), by default the centre of
+`image_size` (W, H)), the fit is perspective: raw `openpose` detections are mapped onto the model's keypoints in
+pixels (no crop frame), an --init `camera` is converted by perspective_start with kp.npz's `center` / `scale`, and the
+output holds `transl`.  An optional `groups` array (B,) in kp.npz fits the images of one label with one shape; the --targets arrays are then
 per group, and the output carries `groups`.  With --share-pose the images of one label are simultaneous views of one
 posed body: they share the body pose too, and body_pose is then per group in the output.
 
@@ -443,14 +455,80 @@ def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas):
     return per_body
 
 
-def _init_2d(init, B, nb, device, method):
+def _init_2d(init, B, nb, device, method, x=None, w=None, intr=None):
     """The raw 6D global and body pose, betas and camera to start from: fit_body_to_keypoints' init with 'camera' in
-    place of 'transl'; the regressor's stage output (raw_global_rot, raw_body_pose, betas, camera) works as-is."""
+    place of 'transl'; the regressor's stage output (raw_global_rot, raw_body_pose, betas, camera) works as-is.  With
+    intrinsics intr (B, 3) the last three are 'transl', by default START_DEPTH in front of the camera on the ray
+    through the centroid of the keypoints x with weight w > 0 (the principal point without one)."""
     init = dict(init or {})
     for k in ('global_rot', 'body_pose'):
         if init.get('raw_' + k) is not None:
             init[k] = init['raw_' + k]
-    return _start_params(init, B, nb, device, method, 'camera', 0.9)   # softplus(0.9) ~ 1.24, the regressor's mean scale
+    if intr is None:
+        return _start_params(init, B, nb, device, method, 'camera', 0.9)   # softplus(0.9) ~ 1.24, the mean scale
+    if init.get('transl') is None:
+        keep = (w > 0)[..., None]
+        n = keep.sum(1).clamp(min=1)
+        c = torch.where(keep, x, torch.zeros_like(x)).sum(1) / n
+        c = torch.where(keep.any(1), c, intr[:, 1:])
+        init['transl'] = torch.cat([(c - intr[:, 1:]) * START_DEPTH / intr[:, :1],
+                                    torch.full((B, 1), START_DEPTH, device=device)], 1)
+    return _start_params(init, B, nb, device, method, 'transl')
+
+
+# the distance [m] a perspective fit starts at without a translation: a person photographed whole with a phone
+START_DEPTH = 3.0
+
+
+def _intrinsics(focal_length, principal_point, B, device):
+    """(B, 3) float32 (f, px, py) from a scalar or (B,) focal length and a (2,) or (B, 2) principal point; numbers are
+    filled on the device (no host-to-device copy)."""
+    num = lambda v: isinstance(v, (int, float, np.floating))  # noqa: E731
+    if num(focal_length):
+        f = torch.full((B,), float(focal_length), device=device)
+    else:
+        f = torch.as_tensor(focal_length, dtype=torch.float32, device=device).reshape(-1)
+    if isinstance(principal_point, (tuple, list)) and len(principal_point) == 2 and all(map(num, principal_point)):
+        pp = torch.stack([torch.full((B,), float(v), device=device) for v in principal_point], 1)
+    else:
+        pp = torch.as_tensor(principal_point, dtype=torch.float32, device=device).reshape(-1, 2)
+    if f.numel() not in (1, B) or pp.shape[0] not in (1, B):
+        raise ValueError(f'fit_body_to_keypoints_2d: focal_length must be a scalar or ({B},) and principal_point (2,) '
+                         f'or ({B}, 2), got {tuple(f.shape)} and {tuple(pp.shape)}')
+    return torch.cat([f.expand(B)[:, None], pp.expand(B, 2)], 1).contiguous()
+
+
+def _project(joints, intr):
+    """The perspective projection of the fit, through the camera module's PerspectiveCamera: joints (B, K, 3) in the
+    camera frame (transl included), intr (B, 3)."""
+    from .human_shape.models.camera.camera_projection import PerspectiveCamera
+    return PerspectiveCamera()(joints, focal_length=intr[:, 0], camera_center=intr[:, 1:])
+
+
+def _depth_rule(per_body, joints, w):
+    """+inf for a body with a weighted keypoint at Y_z <= 0 or not finite (the perspective step's rule)."""
+    z = joints[..., 2]
+    bad = ((w > 0) & ~(z > 0)).any(1) | ((w > 0) & ~torch.isfinite(z)).any(1)
+    return torch.where(bad, torch.full_like(per_body, float('inf')), per_body)
+
+
+def perspective_start(camera, center, scale, focal_length, principal_point):
+    """The starting translation (B, 3) of a perspective fit from the regressor's weak-perspective crop camera (B, 3)
+    and the crop descriptors: center (B, 2) in pixels and scale (B,) = box / 200 (as keypoints2d.to_crop), focal_length
+    a scalar or (B,) and principal_point (2,) or (B, 2) in pixels.  With s = softplus(c0) and h = 200 scale:
+    t_z = 2 f / (s h), t_xy = c[1:3] + (center - pp) t_z / f.  Points at Y_z = t_z then project exactly where the crop
+    projection puts them, mapped back to pixels (up to to_crop's +1 and pixel rounding); nearer or farther points
+    differ by O(depth / t_z).  Unlike the reference demo's conversion, the real principal point is kept."""
+    camera = torch.as_tensor(camera, dtype=torch.float32)
+    dev = camera.device
+    center = torch.as_tensor(center, dtype=torch.float32, device=dev).reshape(-1, 2)
+    h = 200.0 * torch.as_tensor(scale, dtype=torch.float32, device=dev).reshape(-1)
+    f = torch.as_tensor(focal_length, dtype=torch.float32, device=dev).reshape(-1)
+    pp = torch.as_tensor(principal_point, dtype=torch.float32, device=dev).reshape(-1, 2)
+    s = torch.nn.functional.softplus(camera[:, 0])
+    tz = 2.0 * f / (s * h)
+    txy = camera[:, 1:3] + (center - pp) * (tz / f)[:, None]
+    return torch.cat([txy, tz[:, None]], 1)
 
 
 def group_plan(groups, B):
@@ -495,7 +573,8 @@ def _group_sum(x, offsets):
 def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, method='adam', iterations=None,
                              robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
                              body_measurements=None, measurements=None, measurement_weights=None,
-                             circumference_derivative='reference', groups=None, share_pose=False):
+                             circumference_derivative='reference', groups=None, share_pose=False, focal_length=None,
+                             principal_point=None):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -532,11 +611,27 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     rotations, made rotations again by the 6D decoder's Gram-Schmidt; pose_anchor is then per group, (G, 22, 3, 3)
     with the global rows unread, by default that start, and the pose prior counts once per group.  'body_pose' and
     'body_pose_mat' are then per group as well.  With 'lm' an iteration is the keypoint Jacobian of every image and
-    ops.fit_lm_keypoints_2d_shared_pose_step (six launches with measurements)."""
+    ops.fit_lm_keypoints_2d_shared_pose_step (six launches with measurements).
+    focal_length: None (the weak-perspective fit above), or a scalar or (B,) focal length f > 0 with principal_point
+    (2,) or (B, 2) (required with it): the fit is then perspective, p_k = f (Y_x / Y_z, Y_y / Y_z) + principal_point,
+    Y_k = joint_k + transl, camera frame x right, y down, z forward.  keypoints2d are then in the intrinsics' units,
+    init may carry 'transl' (B, 3) in the place of 'camera' (without one the fit starts 3 m in front of the camera, on
+    the ray through the centroid of the weighted keypoints; perspective_start converts a regressor's crop camera), and
+    the result has 'transl' instead of 'camera' and perspective 'proj_joints'.  'lm' loops over the keypoint Jacobian
+    and ops.fit_lm_keypoints_2d_perspective_step (with measurements, forward_shape and the measurement Jacobian as
+    well); 'adam' fits raw 6D pose, betas and transl through SMPLX.forward(transl=...) and PerspectiveCamera.  A trial
+    with a weighted keypoint at Y_z <= 0 is rejected by 'lm'; the returned loss is +inf for a body that has one.
+    The measurement weights are the crop frame's; with targets in pixels a known height needs a larger weight to
+    count (measurement_weights={'height': 1e6}: 1 mm of height costs what 1 px of one keypoint does).  groups and
+    share_pose are not supported with a focal length."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
     if share_pose and groups is None:
         raise ValueError('fit_body_to_keypoints_2d: share_pose needs groups')
+    if focal_length is not None and (groups is not None or share_pose):
+        raise ValueError('fit_body_to_keypoints_2d: groups and share_pose are not supported with a focal_length')
+    if focal_length is not None and principal_point is None:
+        raise ValueError('fit_body_to_keypoints_2d: focal_length needs principal_point')
     exact_circumferences(circumference_derivative)
     if measurements is not None and body_measurements is None:
         raise ValueError('fit_body_to_keypoints_2d: measurements need body_measurements')
@@ -560,7 +655,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
                                                                              device=device)
     w = w.expand(B, K).contiguous()
-    params = _init_2d(init, B, nb, device, method)
+    intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
+    params = _init_2d(init, B, nb, device, method, x, w, intr)
     rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
     if share_pose:          # per group: its shape is checked once the groups are known
         anchor = None if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32, device=device)
@@ -579,13 +675,18 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         mterms = (tgt.contiguous(), wt.contiguous(), circumference_derivative)
     if method == 'lm':
         return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw,
-                                    body_measurements, mterms)
+                                    body_measurements, mterms, intr)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
         bpose = Rot6dFunction.apply(params['body_pose'])
-        out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], camera=params['camera'],
-                         return_shaped=False)
+        if intr is None:
+            out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], camera=params['camera'],
+                             return_shaped=False)
+        else:
+            out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
+                             return_shaped=False)
+            out['proj_joints'] = _project(out['joints'][:], intr)
         rot = torch.cat([grot, bpose], 1)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
         meas = None
@@ -598,6 +699,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         return per_body, out, grot, bpose, meas
 
     per_body, out, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
+    if intr is not None:
+        per_body = _depth_rule(per_body, out['joints'][:], w)
     res = {k: v.detach() for k, v in params.items()}
     res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
                loss=per_body)
@@ -607,14 +710,21 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
 
 
 def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw, body_measurements=None,
-                         mterms=None):
+                         mterms=None, intr=None):
     from . import ops
     device = x.device
     packed = body_model.packed(device)
     B, K = x.shape[0], x.shape[1]
     nb = params['betas'].shape[1]
-    trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'camera': params['camera'].contiguous()}
-    state = _kp_lm_state(B, K, 22, nb, 'camera', device)
+    last = 'camera' if intr is None else 'transl'
+    trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), last: params[last].contiguous()}
+    state = _kp_lm_state(B, K, 22, nb, last, device)
+    if intr is None:
+        step, mstep = ops.fit_lm_keypoints_2d_step, ops.fit_lm_keypoints_2d_measurements_step
+    else:       # the perspective steps, the intrinsics bound after the weights
+        step = lambda st, tr, x, w, *r, **kw: ops.fit_lm_keypoints_2d_perspective_step(st, tr, x, w, intr, *r, **kw)  # noqa: E731
+        mstep = lambda st, tr, x, w, *r, **kw: ops.fit_lm_keypoints_2d_perspective_measurements_step(  # noqa: E731
+            st, tr, x, w, intr, *r, **kw)
     pose_anchor = anchor if pw > 0 else None
     if mterms is not None:
         state.update(meas=torch.empty(B, 5, dtype=torch.float32, device=device),
@@ -622,8 +732,7 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
     if B > 0 and mterms is None:
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
-            ops.fit_lm_keypoints_2d_step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac,
-                                         pose_anchor=pose_anchor)
+            step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, pose_anchor=pose_anchor)
     elif B > 0:
         tgt, wt, cd = mterms
         exact = exact_circumferences(cd)
@@ -633,16 +742,23 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
             v = ops.smplx_forward_shape(packed, trial['betas'])
             tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-            ops.fit_lm_keypoints_2d_measurements_step(state, trial, x, w, sigma, pw, bw, tgt, wt, LM_UP, LM_DOWN,
-                                                      it == 0, tkp, tjac, tm, tmj, pose_anchor=pose_anchor)
+            mstep(state, trial, x, w, sigma, pw, bw, tgt, wt, LM_UP, LM_DOWN, it == 0, tkp, tjac, tm, tmj,
+                  pose_anchor=pose_anchor)
     rot = state['rot']
     with torch.no_grad():
-        out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
-                         return_shaped=False)
+        if intr is None:
+            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
+                             return_shaped=False)
+        else:
+            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'],
+                             transl=state['transl'], return_shaped=False)
+            out['proj_joints'] = _project(out['joints'][:], intr)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
         if mterms is not None:      # _kp2d_loss already counted betas_weight |betas|^2
             per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], 0.0)
-    res = _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+        if intr is not None:
+            per_body = _depth_rule(per_body, out['joints'][:], w)
+    res = _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
     if mterms is not None:
         res['measurements'] = state['meas']
     return res
@@ -810,13 +926,16 @@ def main(argv=None):
                    help='npz with keypoints (B, K, 2) in the crop frame of proj_joints and optional weights (B, K), or '
                         'raw OpenPose detections openpose (B, 135, 3) in pixels with the crop descriptors center '
                         '(B, 2) and scale (B,) (and optionally crop_size, default 256; needs --keypoint-map): fit pose, '
-                        'shape and camera to them instead of betas to measurements')
+                        'shape and camera to them instead of betas to measurements; with focal_length (and '
+                        'principal_point, or image_size (W, H) for its centre) in the npz the keypoints and detections '
+                        'are in pixels and the fit is perspective')
     p.add_argument('--keypoint-map', dest='keypoint_map', type=str, default=None,
                    help='JSON OpenPose -> model keypoint map (shapy_b200.keypoints2d), e.g. '
                         'tests/golden/openpose_smplx_map.json')
     p.add_argument('--init', type=str, default=None,
                    help='npz with raw_global_rot / raw_body_pose (or global_rot / body_pose raw 6D), betas and camera, '
-                        'e.g. a saved regressor prediction')
+                        'e.g. a saved regressor prediction; a perspective fit converts the camera with '
+                        'perspective_start and the npz center / scale, or takes transl')
     p.add_argument('--robust-sigma', dest='robust_sigma', type=float, default=None)
     p.add_argument('--pose-prior-weight', dest='pose_prior_weight', type=float, default=0.0)
     p.add_argument('--share-pose', dest='share_pose', action='store_true',
@@ -856,14 +975,26 @@ def main(argv=None):
 
 def _main_keypoints_2d(a, model, bm, targets):
     d = np.load(a.keypoints_2d)
+    persp = 'focal_length' in d.files
+    focal = pp = None
+    if persp:
+        focal = d['focal_length'].astype(np.float32)
+        if 'principal_point' in d.files:
+            pp = d['principal_point'].astype(np.float32)
+        elif 'image_size' in d.files:
+            pp = d['image_size'].astype(np.float32).reshape(-1, 2) / 2.0
+        else:
+            raise SystemExit('--keypoints-2d with a focal_length needs principal_point or image_size (W, H)')
     if 'openpose' in d.files:
         from . import keypoints2d as k2d
         if not a.keypoint_map:
             raise SystemExit('--keypoints-2d with raw OpenPose detections needs --keypoint-map')
         kmap = k2d.load_keypoint_map(a.keypoint_map)
         op = k2d.threshold_confidence(d['openpose'].reshape(-1, k2d.NUM_OPENPOSE, 3), kmap)
-        size = int(d['crop_size']) if 'crop_size' in d.files else 256
-        x, w = k2d.map_keypoints(k2d.to_crop(op, d['center'], d['scale'], size), kmap, model.packed().K)
+        if not persp:       # the perspective fit takes the detections in pixels
+            size = int(d['crop_size']) if 'crop_size' in d.files else 256
+            op = k2d.to_crop(op, d['center'], d['scale'], size)
+        x, w = k2d.map_keypoints(op, kmap, model.packed().K)
     else:
         x = d['keypoints'].astype(np.float32)
         x = x[None] if x.ndim == 2 else x
@@ -872,14 +1003,18 @@ def _main_keypoints_2d(a, model, bm, targets):
     if a.init:
         p = np.load(a.init)
         init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(x.shape[0], -1)
-                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera')
+                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera', 'transl')
                 if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+        if persp and 'transl' not in init and 'camera' in init:
+            if not ('center' in d.files and 'scale' in d.files):
+                raise SystemExit('--init with a camera and a focal_length needs center and scale in --keypoints-2d')
+            init['transl'] = perspective_start(init['camera'], d['center'], d['scale'], focal, pp)
     groups = d['groups'].astype(np.int64).reshape(-1) if 'groups' in d.files else None
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
                                    circumference_derivative=a.circumference_derivative, groups=groups,
-                                   share_pose=a.share_pose)
+                                   share_pose=a.share_pose, focal_length=focal, principal_point=pp)
     out = {k: v.detach().cpu().numpy() for k, v in res.items()}
     if groups is not None:
         out['groups'] = groups

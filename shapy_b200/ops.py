@@ -498,46 +498,52 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
 
 
 def _fit_lm_kp2d(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
-                 lambda_down, first, trial_keypoints, trial_jac, pose_anchor, meas=None):
-    """What the two 2D keypoint steps share: the checks and the call, `meas` None or the measurement block
-    (meas_targets, meas_weights, trial_meas, trial_meas_jac) of the stacked step."""
+                 lambda_down, first, trial_keypoints, trial_jac, pose_anchor, meas=None, intrinsics=None):
+    """What the 2D keypoint steps share: the checks and the call, `meas` None or the measurement block
+    (meas_targets, meas_weights, trial_meas, trial_meas_jac) of the stacked step, `intrinsics` None (the
+    weak-perspective camera 'camera') or (B, 3) (the perspective steps, translation 'transl')."""
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
+    last = 'camera' if intrinsics is None else 'transl'
     sigma = float('inf') if robust_sigma is None else float(robust_sigma)
     if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
         raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
     if pose_prior_weight > 0 and pose_anchor is None:
         raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
     anchor = [] if pose_anchor is None else [pose_anchor]
+    intr = [] if intrinsics is None else [intrinsics]
     mstate = [] if meas is None else [state['meas'], state['meas_jac']]
-    ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
-        [trial[k] for k in ('rot', 'betas', 'camera')] + [targets, weights, trial_keypoints, trial_jac] + anchor + \
+    ts = [state[k] for k in ('rot', 'betas', last, 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
+        [trial[k] for k in ('rot', 'betas', last)] + [targets, weights, trial_keypoints, trial_jac] + anchor + intr + \
         list(meas or ())
-    _check_step_tensors(what, ts, 'the state, trial, targets, weights and anchor', state['accepted'])
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights, anchor and intrinsics', state['accepted'])
     P = 3 * n_rot + nb + 3
     if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
         raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
     if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if intrinsics is not None and intrinsics.shape != (B, 3):
+        raise RuntimeError(f'{what}: intrinsics must be ({B}, 3)')
     if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], B, nb):
         raise RuntimeError(f'{what}: meas_jac must be ({B}, 5, {nb}) and the measurements, their targets and weights '
                            f'({B}, 5)')
     if B == 0:
         return
-    head = [B, K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma, float(pose_prior_weight),
-            float(betas_weight)]
+    head = [B, K, n_rot, nb, ptr(targets), ptr(weights)] + [ptr(t) for t in intr] + \
+        [ptr(pose_anchor), sigma, float(pose_prior_weight), float(betas_weight)]
     lam = [float(lambda_up), float(lambda_down), int(bool(first))]
-    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['camera']), ptr(trial_keypoints), ptr(trial_jac)]
+    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial[last]), ptr(trial_keypoints), ptr(trial_jac)]
+    persp = '' if intrinsics is None else '_perspective'
     with torch.cuda.device(trial['rot'].device):
         if meas is None:
-            check(lib().shapy_fit_lm_keypoints_2d_step(
+            check(getattr(lib(), f'shapy_fit_lm_keypoints_2d{persp}_step')(
                 *head, *lam,
-                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+                *[ptr(state[k]) for k in ('rot', 'betas', last, 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
                 *tr, stream_ptr()), what)
         else:
-            check(lib().shapy_fit_lm_keypoints_2d_measurements_step(
+            check(getattr(lib(), f'shapy_fit_lm_keypoints_2d{persp}_measurements_step')(
                 *head, ptr(meas[0]), ptr(meas[1]), *lam,
-                *[ptr(state[k]) for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
+                *[ptr(state[k]) for k in ('rot', 'betas', last, 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
                                           'lambda', 'accepted')],
                 *tr, ptr(meas[2]), ptr(meas[3]), stream_ptr()), what)
 
@@ -565,6 +571,31 @@ def fit_lm_keypoints_2d_measurements_step(state, trial, targets, weights, robust
     _fit_lm_kp2d('fit_lm_keypoints_2d_measurements_step', state, trial, targets, weights, robust_sigma,
                  pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
                  pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac))
+
+
+def fit_lm_keypoints_2d_perspective_step(state, trial, targets, weights, intrinsics, robust_sigma, pose_prior_weight,
+                                         betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                                         pose_anchor=None):
+    """fit_lm_keypoints_2d_step under a perspective camera with known intrinsics (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_perspective_step), in place: p_k = f (Y_x / Y_z, Y_y / Y_z) + (px, py), Y_k = kp_k + t,
+    camera frame x right, y down, z forward.  state and trial hold 'transl' (B, 3) in the place of 'camera';
+    intrinsics (B, 3) = (f, px, py) in the units of targets (B, K, 2).  A trial with a weighted keypoint at Y_z <= 0 is
+    rejected; a start with one reports NaN and does not move."""
+    _fit_lm_kp2d('fit_lm_keypoints_2d_perspective_step', state, trial, targets, weights, robust_sigma,
+                 pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                 pose_anchor, intrinsics=intrinsics)
+
+
+def fit_lm_keypoints_2d_perspective_measurements_step(state, trial, targets, weights, intrinsics, robust_sigma,
+                                                      pose_prior_weight, betas_weight, meas_targets, meas_weights,
+                                                      lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                                                      trial_meas, trial_meas_jac, pose_anchor=None):
+    """fit_lm_keypoints_2d_perspective_step with the five measurements stacked under its rows (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_perspective_measurements_step), with fit_lm_keypoints_2d_measurements_step's
+    measurement block."""
+    _fit_lm_kp2d('fit_lm_keypoints_2d_perspective_measurements_step', state, trial, targets, weights, robust_sigma,
+                 pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                 pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac), intrinsics)
 
 
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
