@@ -440,6 +440,47 @@ int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
     float *trial_camera, const float *trial_keypoints, const float *trial_jac, const float *trial_meas,
     const float *trial_meas_jac, void *workspace, void *stream);
 
+/* One Levenberg-Marquardt step per body of the fit of bodies seen by a calibrated rig: num_bodies (G) bodies in one
+ * world frame, body g seen by the views [view_offsets[g], view_offsets[g+1]) (num_bodies + 1 int32 in host memory,
+ * rising strictly from 0 to num_views, copied into the workspace on the stream at every call).  Per view (num_views
+ * rows): targets (B,K,2), weights (B,K), intrinsics (B,3) = (f, px, py) and extrinsics (B,12) = world-to-camera R
+ * (row-major) then T, camera frame x right, y down, z forward.  Per body (G rows): pose_anchor, rot, betas, transl (the
+ * world translation t), keypoints, jac (of shapy_smplx_keypoint_jacobian without transl), loss, lambda, accepted and
+ * the trial.  Parameters [delta_j (3 n_rot) | beta (nb) | t], P = 3 n_rot + nb + 3.  With X_k = kp_k + t and Y_vk =
+ * R_v X_k + T_v (fp64), p_vk = f_v (Y_x / Y_z, Y_y / Y_z) + (px_v, py_v); loss per body, fp64, left to right: the sum
+ * over its views (view order) of sum_{w_vk > 0} w_vk rho(|p_vk - x_vk|^2) (k order), + pose_prior_weight / 2
+ * sum_{j >= 1} |R_j - R0_j|_F^2 + betas_weight |beta|^2.  Keypoint rows 2k + c of each view in view order (IRLS
+ * weights at the state): (f_v / Y_z) (R_v[c,:] - (Y_c / Y_z) R_v[2,:]) J3_k, J3_k the 3 x P block of keypoint k with
+ * J_t = I.  Depth rule per view: a trial with a weighted keypoint at Y_z <= 0 or non-finite in any view, or a view
+ * whose f is not finite and > 0, has loss +inf and is rejected; a start that breaks it reports NaN and does not move.
+ * Pose-prior rows, first lambda (from the keypoint rows alone), damping and solve are the 2D step's, the next trial
+ * R Exp(delta), beta + delta_beta, t + delta_t.  One launch, one CTA per body; no synchronisation, no atomics: a
+ * body's results do not depend on the rest of the batch.  workspace: shapy_fit_lm_calibrated_workspace_bytes(
+ * num_views, num_bodies) bytes of device memory.  Errors as shapy_fit_lm_keypoints_2d_perspective_step (over the G
+ * bodies), and SHAPY_ERR_ARG for a null extrinsics or workspace, bad offsets or a body without a view.  num_bodies 0
+ * (with num_views 0): no launch. */
+size_t shapy_fit_lm_calibrated_workspace_bytes(int num_views, int num_bodies);
+int shapy_fit_lm_keypoints_2d_calibrated_step(
+    int num_views, int num_bodies, const int32_t *view_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *extrinsics,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight, float lambda_up,
+    float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+    const float *trial_keypoints, const float *trial_jac, void *workspace, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_calibrated_step with the five virtual measurements of each body stacked under its rows, as
+ * shapy_fit_lm_keypoints_2d_measurements_step adds them (meas_targets, meas_weights, meas, trial_meas (G,5), meas_jac,
+ * trial_meas_jac (G,5,nb)).  With every measurement weight <= 0 every output equals
+ * shapy_fit_lm_keypoints_2d_calibrated_step's bit for bit. */
+int shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
+    int num_views, int num_bodies, const int32_t *view_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *extrinsics,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *workspace, void *stream);
+
 /* Drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward: query (B,Q,3,3), target (B,F,3,3) fp32;
  * collision_faces (B,Q*M) int64 pre-filled by the callee with -1; collision_bcs (B,Q*M,2,3) with 0.
  * num_target > 32768 returns SHAPY_ERR_UNSUPPORTED. */

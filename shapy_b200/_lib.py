@@ -131,6 +131,16 @@ _SIGS = {
                                                                         C.c_float, C.c_float, c_void_p, c_void_p,
                                                                         C.c_float, C.c_float, c_int] + [c_void_p] * 18
                                                                 + [c_void_p, c_void_p]),
+    'shapy_fit_lm_calibrated_workspace_bytes': (C.c_size_t, [c_int, c_int]),
+    'shapy_fit_lm_keypoints_2d_calibrated_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                                                          c_void_p, c_void_p, c_void_p, c_void_p, C.c_float, C.c_float,
+                                                          C.c_float, C.c_float, C.c_float, c_int] + [c_void_p] * 13
+                                                  + [c_void_p, c_void_p]),
+    'shapy_fit_lm_keypoints_2d_calibrated_measurements_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int,
+                                                                       c_void_p, c_void_p, c_void_p, c_void_p,
+                                                                       c_void_p, C.c_float, C.c_float, C.c_float,
+                                                                       c_void_p, c_void_p, C.c_float, C.c_float, c_int]
+                                                               + [c_void_p] * 17 + [c_void_p, c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

@@ -611,6 +611,43 @@ __device__ __forceinline__ void persp_residual(const float *m, const float *tg, 
   dy = pc.f * (Y[1] / Y[2]) + pc.pp[1] - (double)tg[2 * k + 1];
 }
 
+// The factors of perspective row c at Y: f / Y_z and Y_c / Y_z into fz[0], fz[1]
+__device__ __forceinline__ void persp_factors(const PerspCam &pc, const double (&Y)[3], int c, double *fz) {
+  fz[0] = pc.f / Y[2];
+  fz[1] = Y[c] / Y[2];
+}
+
+// One calibrated view of a body at a point of the fit: the view's intrinsics, the body's world translation t (in
+// PerspCam) and the view's world-to-camera extrinsics R (row-major), T, in fp64
+struct CalibCam : PerspCam {
+  double R[9], T[3];
+};
+
+__device__ __forceinline__ CalibCam calib_cam(const float *in, const float *ex, const float *t) {
+  CalibCam c;
+  static_cast<PerspCam &>(c) = persp_cam(in, t);
+  for (int i = 0; i < 9; ++i) c.R[i] = (double)ex[i];
+  for (int i = 0; i < 3; ++i) c.T[i] = (double)ex[9 + i];
+  return c;
+}
+
+// Y_k = R (kp_k + t) + T (each row left to right, then + T_c) and the residual p_k - x_k of its projection, in fp64
+__device__ __forceinline__ void persp_residual(const float *m, const float *tg, const CalibCam &pc, int k, double (&Y)[3],
+                                               double &dx, double &dy) {
+  double X[3];
+  for (int c = 0; c < 3; ++c) X[c] = (double)m[3 * k + c] + pc.t[c];
+  for (int c = 0; c < 3; ++c) Y[c] = pc.R[3 * c] * X[0] + pc.R[3 * c + 1] * X[1] + pc.R[3 * c + 2] * X[2] + pc.T[c];
+  dx = pc.f * (Y[0] / Y[2]) + pc.pp[0] - (double)tg[2 * k];
+  dy = pc.f * (Y[1] / Y[2]) + pc.pp[1] - (double)tg[2 * k + 1];
+}
+
+// The factors of calibrated row c at Y: the projected rotation row u_d = (f / Y_z) (R_cd - (Y_c / Y_z) R_2d) into
+// fz[0 .. 2], so that the row is u . J3_k (u_d itself on the t column d)
+__device__ __forceinline__ void persp_factors(const CalibCam &pc, const double (&Y)[3], int c, double *fz) {
+  const double a = pc.f / Y[2], b = Y[c] / Y[2];
+  for (int d = 0; d < 3; ++d) fz[d] = a * (pc.R[3 * c + d] - b * pc.R[6 + d]);
+}
+
 // The perspective rows' factors f / Y_z and Y_c / Y_z per staged row: shared memory only the perspective kernels have
 __device__ __forceinline__ double *lm_persp_factors() {
   __shared__ double fz[2 * kLmKpRows];
@@ -650,11 +687,12 @@ __device__ __forceinline__ double lm_kp2d_prior_loss(const LmKp2dArgs &x2, const
 }
 
 // Phase 1 of the 2D steps, by one thread: the trial's robust keypoint term (k order) and pose prior, left to right.
-// PERSP: the projection of the trial's camera pc, +inf under the depth rule
-template <bool PERSP = false>
+// PERSP: the projection of the trial's camera pc (Cam: PerspCam, or CalibCam for one calibrated view), +inf under the
+// depth rule
+template <bool PERSP = false, typename Cam = PerspCam>
 __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const LmKp2dArgs &x2, int b, const float *tg,
                                                      const float *wt, const float *anc, bool robust, double s2,
-                                                     const PerspCam *pc = nullptr) {
+                                                     const Cam *pc = nullptr) {
   const int K = a.K, R3 = 3 * a.K, nr9 = 9 * a.n_rot;
   const float *m = a.tkp + (size_t)b * R3, *cam = a.tlast + (size_t)b * 3;
   double s, ds;
@@ -684,11 +722,11 @@ __device__ __forceinline__ double lm_kp2d_trial_loss(const LmKpArgs &a, const Lm
 
 // Phase 3 of the 2D steps: row c of keypoint k at the state (keypoints M, scale s, offset cxy), its weight w_k q_k^2 (the
 // IRLS weight, w_k at sigma = inf) and residual; a dropped keypoint (w_k <= 0) keeps w_k and a zero residual.  PERSP:
-// the state's camera pc, and the row's factors f / Y_z, Y_c / Y_z into fz[0], fz[1]
-template <bool PERSP = false>
+// the state's camera pc, and the row's factors into fz (persp_factors of its Cam)
+template <bool PERSP = false, typename Cam = PerspCam>
 __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, const float *wt, double s,
                                             const double (&cxy)[2], bool robust, double s2, int k, int c, double &wr,
-                                            double &res, const PerspCam *pc = nullptr, double *fz = nullptr) {
+                                            double &res, const Cam *pc = nullptr, double *fz = nullptr) {
   const double w = wt[k];
   wr = w;
   res = 0.0;
@@ -697,8 +735,7 @@ __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, con
     if constexpr (PERSP) {
       double Y[3];
       persp_residual(M, tg, *pc, k, Y, dx, dy);
-      fz[0] = pc->f / Y[2];
-      fz[1] = Y[c] / Y[2];
+      persp_factors(*pc, Y, c, fz);
     } else {
       dx = s * ((double)M[3 * k] + cxy[0]) - (double)tg[2 * k];
       dy = s * ((double)M[3 * k + 1] + cxy[1]) - (double)tg[2 * k + 1];
@@ -713,12 +750,17 @@ __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, con
 
 // Column col of that row, the camera columns at oc: s J_{3k+c} on the rotation and betas columns, ds (kp_kc + c_{1+c})
 // on c0, s on c_{1+c}.  REORDER: columns [delta | c | beta] (the grouped step), else [delta | beta | c].  PERSP (columns
-// [delta | beta | t]): fz[0] (J_{3k+c} - fz[1] J_{3k+2}) with the row's factors fz, J_t = I
-template <bool REORDER, bool PERSP = false>
+// [delta | beta | t]): fz[0] (J_{3k+c} - fz[1] J_{3k+2}) with the row's factors fz, J_t = I; with a CalibCam, fz[0]
+// J_{3k} + fz[1] J_{3k+1} + fz[2] J_{3k+2} (fz[d] on t column d)
+template <bool REORDER, bool PERSP = false, typename Cam = PerspCam>
 __device__ __forceinline__ double lm_kp2d_entry(const float *J, const float *M, int P, int oc, int k, int c, int col,
                                                 double s, double ds, const double (&cxy)[2],
                                                 const double *fz = nullptr) {
-  if constexpr (PERSP) {
+  if constexpr (PERSP && std::is_same_v<Cam, CalibCam>) {
+    if (col >= oc) return fz[col - oc];
+    const float *Jk = J + (size_t)(3 * k) * P + col;
+    return fz[0] * (double)Jk[0] + fz[1] * (double)Jk[P] + fz[2] * (double)Jk[2 * P];
+  } else if constexpr (PERSP) {
     const double jc = col < oc ? (double)J[(size_t)(3 * k + c) * P + col] : (col - oc == c ? 1.0 : 0.0);
     const double jz = col < oc ? (double)J[(size_t)(3 * k + 2) * P + col] : (col - oc == 2 ? 1.0 : 0.0);
     return fz[0] * (jc - fz[1] * jz);
@@ -889,11 +931,7 @@ inline int check_lm_kp(const char *fn, int batch, LmKpArgs &a, bool extra_ok, bo
 }
 
 template <typename Extra>
-int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
-              bool factors_ok, const char *factors, void *stream) {
-  const int rc = check_lm_kp(fn, batch, a, extra_ok, factors_ok, factors);
-  if (rc != SHAPY_OK) return rc;
-  if (batch == 0) return SHAPY_OK;
+int launch_lm_kp(void (*kernel)(LmKpArgs, Extra), int batch, const LmKpArgs &a, const Extra &x, void *stream) {
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
   cudaFuncAttributes attr;
   SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, kernel));
@@ -902,6 +940,15 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
   kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
+}
+
+template <typename Extra>
+int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
+              bool factors_ok, const char *factors, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, extra_ok, factors_ok, factors);
+  if (rc != SHAPY_OK) return rc;
+  if (batch == 0) return SHAPY_OK;
+  return launch_lm_kp(kernel, batch, a, x, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1255,6 +1302,145 @@ int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
   return SHAPY_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The calibrated step (shapy_fit_lm_keypoints_2d_calibrated_step, and _measurements_ with MEAS): G bodies in one world
+// frame, body g seen by the views [off[g], off[g + 1]) of a synchronised rig with known intrinsics (f_v, px_v, py_v) and
+// world-to-camera extrinsics R_v, T_v (camera frame x right, y down, z forward).  One CTA per body, whose parameters are
+// its world rotations, betas and world translation t, [delta | beta | t], P = 3 n_rot + NB + 3: the keypoint Jacobian
+// is evaluated once per body whatever the number of views.  With X_k = kp_k + t and Y_vk = R_v X_k + T_v (fp64),
+// p_vk = f_v (Y_x / Y_z, Y_y / Y_z) + pp_v, and per body, left to right:
+//   L = sum_v (view order) [sum_{w_vk > 0} w_vk rho(|p_vk - x_vk|^2) (k order)]
+//     + the 2D step's pose prior (against the body's anchor), measurement term (MEAS) and betas prior.
+// Keypoint rows: view by view, rows 2k + c of each, weight w_vk q_vk^2 at the state, residual p_vkc - x_vkc, row
+// u . J3_k with u = (f_v / Y_z) (R_v[c, :] - (Y_c / Y_z) R_v[2, :]) and J3_k the (3 x P) block of keypoint k (J_t = I:
+// u itself on the t columns), staged kLmKpRows at a time (a block may straddle two views).  The prior, measurement and
+// betas rows, the first lambda (the keypoint rows' diagonal), damping and solve are the 2D step's, the next trial the
+// 3D step's.  Depth rule, per view: a trial with a weighted keypoint at Y_z <= 0 or non-finite in any view, or a view
+// whose f is not finite and > 0, has loss +inf; a start that breaks it reports NaN and does not move.
+struct LmKp2dCalibArgs : LmKp2dPerspArgs {    // targets (B, K, 2), weights (B, K) and intr (B, 3) per view
+  const float *extr;                          // (B, 12) per view: R row-major, then T
+  const int *off;                             // (G + 1) view offsets, the device copy in the workspace
+};
+
+template <bool MEAS>
+__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dc_step_kernel(LmKpArgs a, LmKp2dCalibArgs x2) {
+  extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
+  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
+  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP], dg[kLmKpMaxP], fz[3 * kLmKpRows];
+  __shared__ double lt_s;
+  __shared__ int kr[kLmKpRows], ok_s;   // kr: the keypoint of each staged row
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R2 = 2 * a.K, R3 = 3 * a.K, nb = a.nb;
+  const int nr9 = 9 * a.n_rot, o = 3 * a.n_rot, oc = o + nb;     // first betas and first t column
+  const int v0 = x2.off[b], v1 = x2.off[b + 1];
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  const float lcur = a.loss[b];
+  // 1. trial loss: the keypoint term of each view, then the pose prior once
+  if (t == 0) {
+    LmKp2dArgs xk = x2;
+    xk.pose_w = 0.f;
+    double L = 0.0;
+    for (int v = v0; v < v1; ++v) {
+      const CalibCam tc = calib_cam(x2.intr + (size_t)v * 3, x2.extr + (size_t)v * 12, a.tlast + (size_t)b * 3);
+      L += lm_kp2d_trial_loss<true>(a, xk, b, a.targets + (size_t)v * R2, a.weights + (size_t)v * K, nullptr, robust,
+                                    s2, &tc);
+    }
+    if (x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x2, a.trot + (size_t)b * nr9, anc, nr9);
+    if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
+    if (x2.betas_w > 0.f) {
+      const float *tb = a.tbetas + (size_t)b * nb;
+      double reg = 0.0;
+      for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
+      L += (double)x2.betas_w * reg;
+    }
+    lt_s = L;
+  }
+  __syncthreads();
+  // 2. accept or reject
+  const double lt = lt_s;
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
+  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
+  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
+  const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
+  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
+  const float *Tst = (accept ? a.tlast : a.last) + (size_t)b * 3;
+  if (accept) {
+    lm_kp_take_trial(a, b, lnew);
+    if constexpr (MEAS) lm_meas_take_trial(x2.mb, b, nb);
+  }
+  // 3. normal equations: the keypoint rows of the views in order, rows 2k + c of each
+  int pr[kLmKpPairs], pc[kLmKpPairs];
+  double acc[kLmKpPairs], g = 0.0;
+  lm_kp_pairs(P, pr, pc, acc);
+  const double cxy[2] = {0.0, 0.0};     // the weak-perspective camera of lm_kp2d_row / lm_kp2d_entry: not read
+  const int nrows = (v1 - v0) * R2;
+  for (int r0 = 0; r0 < nrows; r0 += kLmKpRows) {
+    const int nr = min(kLmKpRows, nrows - r0);
+    __syncthreads();
+    for (int i = t; i < nr; i += blockDim.x) {   // row weight (IRLS at the state), residual and factors
+      const int v = v0 + (r0 + i) / R2, q = (r0 + i) % R2;
+      const CalibCam sc = calib_cam(x2.intr + (size_t)v * 3, x2.extr + (size_t)v * 12, Tst);
+      double wr, res;
+      lm_kp2d_row<true>(M, a.targets + (size_t)v * R2, a.weights + (size_t)v * K, 0.0, cxy, robust, s2, q >> 1, q & 1,
+                        wr, res, &sc, fz + 3 * i);
+      ws[i] = wr;
+      rs[i] = res;
+      kr[i] = q >> 1;
+    }
+    __syncthreads();
+    for (int i = t; i < nr * P; i += blockDim.x) {
+      const int row = i / P, col = i % P;
+      const double wr = ws[row];
+      if (wr > 0.0) {                    // a dropped keypoint's rows are never read: they may be NaN
+        const double x = lm_kp2d_entry<false, true, CalibCam>(J, M, P, oc, kr[row], 0, col, 0.0, 0.0, cxy,
+                                                              fz + 3 * row);
+        Js[row][col] = x;
+        WJs[row][col] = wr * x;
+      }
+    }
+    __syncthreads();
+    lm_kp_add_rows(nr, P, Js, WJs, ws, rs, pr, pc, acc, g);
+  }
+#pragma unroll
+  for (int i = 0; i < kLmKpPairs; ++i)
+    if (pr[i] >= 0 && pr[i] == pc[i]) dg[pr[i]] = acc[i];     // the diagonal of the keypoint rows: the first lambda
+  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
+  if constexpr (MEAS)
+    lm_meas_add_rows(x2.mb, b, nb, o, (accept ? x2.mb.tmeas : x2.mb.meas) + (size_t)b * 5,
+                     (accept ? x2.mb.tjac : x2.mb.jac) + (size_t)b * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, g);
+  if (x2.betas_w > 0.f && t >= o && t < oc) g += (double)x2.betas_w * (double)Bst[t - o];
+  lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, dg, 1, o, oc, x2.betas_w, ok_s);
+  // 4. Cholesky and the two triangular solves
+  lm_kp_solve(A, y, P, P, ok_s);
+  // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
+  lm_kp_next_trial(a, b, y, ok_s);
+}
+
+// The calibrated entries' checks (check_lm_kp's over the G bodies, then the view offsets, read on the host) and the
+// launch; the offsets are copied into the workspace on the stream
+template <bool MEAS>
+int run_lm_kp2dc(const char *fn, int views, int G, const int32_t *offsets, LmKpArgs a, LmKp2dCalibArgs x,
+                 void *workspace, bool extra_ok, void *stream) {
+  const int rc = check_lm_kp(fn, G, a, extra_ok && offsets && x.intr && x.extr && workspace,
+                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f,
+                             "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                             "lambda_down >= 1");
+  if (rc != SHAPY_OK) return rc;
+  SHAPY_REQUIRE(offsets[0] == 0 && offsets[G] == views,
+                "%s: view_offsets must run from 0 to the number of views (%d) over %d bodies", fn, views, G);
+  for (int g = 0; g < G; ++g)
+    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: body %d has no view (offsets %d, %d)", fn, g, offsets[g],
+                  offsets[g + 1]);
+  if (G == 0) return SHAPY_OK;
+  int *off = (int *)workspace;
+  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice,
+                                 (cudaStream_t)stream));
+  x.off = off;
+  return launch_lm_kp(lm_kp2dc_step_kernel<MEAS>, G, a, x, stream);
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -1455,6 +1641,47 @@ extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
                LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
   return run_lm_kp2dg<true>("shapy_fit_lm_keypoints_2d_shared_pose_measurements_step", batch, num_groups,
                             group_offsets, a, x, trial_betas_images, workspace,
+                            (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
+                                meas_jac && trial_meas && trial_meas_jac,
+                            stream);
+}
+
+extern "C" size_t shapy_fit_lm_calibrated_workspace_bytes(int num_views, int num_bodies) {
+  if (num_views < 0 || num_bodies < 0) return 0;
+  return lm_group_offsets_bytes(num_bodies);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_calibrated_step(
+    int num_views, int num_bodies, const int32_t *view_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *extrinsics,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight, float lambda_up,
+    float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+    const float *trial_keypoints, const float *trial_jac, void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dCalibArgs x{{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics},
+                    extrinsics, nullptr};
+  return run_lm_kp2dc<false>("shapy_fit_lm_keypoints_2d_calibrated_step", num_views, num_bodies, view_offsets, a, x,
+                             workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
+    int num_views, int num_bodies, const int32_t *view_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *extrinsics,
+    const float *pose_anchor, float robust_sigma, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_keypoints,
+    const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dCalibArgs x{{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
+                      LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}},
+                     intrinsics},
+                    extrinsics, nullptr};
+  return run_lm_kp2dc<true>("shapy_fit_lm_keypoints_2d_calibrated_measurements_step", num_views, num_bodies,
+                            view_offsets, a, x, workspace,
                             (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
                                 meas_jac && trial_meas && trial_meas_jac,
                             stream);

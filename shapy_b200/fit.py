@@ -93,6 +93,14 @@ iteration is the keypoint Jacobian and ops.fit_lm_keypoints_2d_perspective_step 
 host synchronisation.  A trial with a weighted keypoint at Y_z <= 0 is rejected, and a body whose start has one
 reports an infinite loss.  perspective_start converts the regressor's crop camera into a starting translation.
 
+fit_body_to_calibrated_views fits bodies seen by a synchronised rig of calibrated cameras: each view has known
+intrinsics and world-to-camera extrinsics (R_v, T_v), each body one pose, shape and world translation t, and every view
+is a fixed projection of the same 3D keypoints, p_vk = f_v (Y_x / Y_z, Y_y / Y_z) + pp_v with Y_vk = R_v (joint_k + t) +
+T_v.  The metric baseline between the cameras fixes the body's size and position, which no single view does.  With
+method='lm' each iteration is the keypoint Jacobian of the bodies (one per body, whatever the number of views) and
+ops.fit_lm_keypoints_2d_calibrated_step, two launches (four with measurements), no host synchronisation.
+calibrated_start maps a camera-frame start of one view (a perspective fit, or perspective_start) into the world frame.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
@@ -894,6 +902,237 @@ def _shared_body_raw(rot0, offsets, cnt):
     return mean[..., :2].reshape(G, 6 * 21).contiguous()
 
 
+# the global rotation of the regressor's mean pose (6D (1, 0, 0, -1, 0, 0)): upright and facing a y-down camera
+MEAN_GLOBAL_ROT = ((1.0, 0.0, 0.0), (0.0, -1.0, 0.0), (0.0, 0.0, -1.0))
+# the weight, relative to one ray, that keeps the default start of a calibrated fit near START_DEPTH along its first
+# view's ray: it fixes the point along a single ray or parallel rays and moves a crossing by about 1e-6 of its distance
+RAY_START_WEIGHT = 1e-6
+
+
+def _root_joint(body_model, betas):
+    """J_0(betas) (B, 3): the root joint of the shaped body, about which SMPL-X applies the global rotation (a few
+    small products on any device: the start of a fit, not its hot path)."""
+    with torch.no_grad():
+        v = body_model.v_template + torch.einsum('bl,mkl->bmk', betas, body_model.shapedirs[..., :betas.shape[1]])
+        return torch.einsum('m,bmk->bk', body_model.J_regressor[0].to(v.dtype), v)
+
+
+def calibrated_start(body_model, global_rot_mat, transl, betas, cam_rot, cam_transl):
+    """Maps a camera-frame start of one view into the world frame of a calibrated fit: global_rot_mat (B, 3, 3) and
+    transl (B, 3) of a body in the frame of a camera with world-to-camera extrinsics cam_rot (B, 3, 3), cam_transl
+    (B, 3), for example a perspective fit of that view or perspective_start of the regressor's crop camera; betas
+    (B, NB).  SMPL-X rotates about the root joint J_0(betas), so the world start is R_0' = R_v^T R_0 and
+    t' = R_v^T (J_0 + t - T_v) - J_0.  Returns (global_rot_mat', transl')."""
+    f = lambda t: torch.as_tensor(t, dtype=torch.float32, device=body_model.shapedirs.device)  # noqa: E731
+    R0, t, Rv, Tv = f(global_rot_mat).reshape(-1, 3, 3), f(transl).reshape(-1, 3), f(cam_rot), f(cam_transl)
+    j0 = _root_joint(body_model, f(betas).reshape(R0.shape[0], -1).contiguous())
+    Rt = Rv.reshape(-1, 3, 3).transpose(1, 2)
+    return Rt @ R0, (Rt @ (j0 + t - Tv.reshape(-1, 3))[..., None])[..., 0] - j0
+
+
+def _ray_start(x, w, intr, cam_rot, cam_transl, offsets):
+    """The default world translation of each body of a calibrated fit (G, 3), without synchronising: the least-squares
+    point nearest the rays of its views (sorted by body) through the centroids of their weighted keypoints (the
+    principal point without one), plus RAY_START_WEIGHT times the squared distance to the point START_DEPTH in front of
+    its first view on that view's ray.  Solved in float64."""
+    keep = (w > 0)[..., None]
+    c = torch.where(keep, x, torch.zeros_like(x)).sum(1) / keep.sum(1).clamp(min=1)
+    c = torch.where(keep.any(1), c, intr[:, 1:])
+    u = torch.cat([(c - intr[:, 1:]) / intr[:, :1], torch.ones_like(c[:, :1])], 1).double()   # the ray, camera frame
+    Rt = cam_rot.double().transpose(1, 2)
+    centre = -(Rt @ cam_transl.double()[..., None])[..., 0]
+    d = (Rt @ u[..., None])[..., 0]
+    d = d / d.norm(dim=1, keepdim=True)
+    M = torch.eye(3, dtype=torch.float64, device=x.device) - d[:, :, None] * d[:, None, :]
+    first = _to_device(offsets[:-1].long(), x.device)
+    p0 = centre[first] + START_DEPTH * (Rt[first] @ u[first][..., None])[..., 0]
+    eps = RAY_START_WEIGHT
+    A = _group_sum(M, offsets) + eps * torch.eye(3, dtype=torch.float64, device=x.device)
+    rhs = _group_sum((M @ centre[..., None])[..., 0], offsets) + eps * p0
+    return torch.linalg.solve_ex(A, rhs)[0].float()
+
+
+def _view_offsets(groups, B):
+    """(order, offsets) of the views of a calibrated fit: group_plan's, or one body seeing every view."""
+    if groups is not None:
+        return group_plan(groups, B)
+    return torch.arange(B), torch.tensor([0, B] if B else [0], dtype=torch.int32)
+
+
+def _calibrated_loss(joints, x, w, intr, cam_rot, cam_transl, gidx, offsets, sigma, pw, bpose, anchor, bw, betas):
+    """The calibrated fit's loss per body, through PerspectiveCamera(rotation=, translation=): joints (G, K, 3) in the
+    world frame, the views (B, ...) sorted by body, gidx (B,) each view's body.  The keypoint terms per view summed in
+    view order, + the pose prior once per body + betas_w |betas|^2.  Returns (per_body (G,), proj_joints (B, K, 2),
+    behind (G,) bool: the step's depth rule, a weighted keypoint at Y_z <= 0 or not finite in one of the body's views,
+    or a view whose focal length is not finite and > 0)."""
+    from .human_shape.models.camera.camera_projection import PerspectiveCamera
+    jv = joints[gidx]
+    proj = PerspectiveCamera()(jv, focal_length=intr[:, 0], rotation=cam_rot, translation=cam_transl,
+                               camera_center=intr[:, 1:])
+    per_body = _group_sum(_kp2d_loss(proj, x, w, sigma, 0.0, None, None, 0.0, None), offsets)
+    if pw > 0:
+        per_body = per_body + 0.5 * pw * (bpose - anchor[:, 1:]).pow(2).sum((1, 2, 3))
+    if bw > 0:
+        per_body = per_body + bw * betas.pow(2).sum(1)
+    y = torch.einsum('bji,bmi->bmj', cam_rot, jv.detach()) + cam_transl[:, None]
+    f = intr[:, 0]
+    behind = _depth_rule(torch.zeros_like(proj[:, 0, 0]), y, w).isinf() | ~(f > 0) | ~torch.isfinite(f)
+    return per_body, proj, _group_sum(behind.float(), offsets) > 0
+
+
+def fit_body_to_calibrated_views(body_model, keypoints2d, focal_length, principal_point, cam_rot, cam_transl,
+                                 groups=None, weights=None, init=None, method='lm', iterations=None, robust_sigma=None,
+                                 pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
+                                 body_measurements=None, measurements=None, measurement_weights=None,
+                                 circumference_derivative='reference'):
+    """Fits bodies seen by a synchronised rig of calibrated cameras: pose, shape and world translation of each body so
+    that its keypoints, projected into every view that sees it, match `keypoints2d` (B, K, 2), one row per view.
+
+    Each view v has intrinsics (focal_length a scalar or (B,), principal_point (2,) or (B, 2), as
+    fit_body_to_keypoints_2d's) and world-to-camera extrinsics cam_rot (B, 3, 3), cam_transl (B, 3): Y = R_v X + T_v,
+    camera frame x right, y down, z forward, p = f (Y_x / Y_z, Y_y / Y_z) + pp, X = joint + transl in the world frame.
+    groups: None (every view sees one body) or (B,) labels 0 .. G-1 (group_plan's rules), the body each view sees.
+    Loss per body: the sum over its views (in the caller's order) of sum_{w_k > 0} w_k rho(|p_k - x_k|^2), +
+    pose_prior_weight / 2 sum_{j >= 1} |R_j - R0_j|_F^2, + the measurement terms of fit_body_to_keypoints_2d, +
+    betas_weight |betas|^2; +inf for a body with a weighted keypoint behind one of its cameras, or with a view whose
+    focal length is not finite and > 0 (the step's depth rule).  The baseline between
+    the cameras fixes the body's metric size and position, which no single view does.  weights: None, (K,) or (B, K)
+    per view.  init: per body, fit_body_to_keypoints' init with 'transl' in the world frame (calibrated_start maps a
+    camera-frame start of one view); without a global rotation a body starts at the mean pose seen from its first view
+    (R_0 = R_v^T MEAN_GLOBAL_ROT), without a translation at the least-squares point nearest the rays through its views'
+    weighted-keypoint centroids.  pose_anchor (G, 22, 3, 3), by default the start.  method: 'lm' (per iteration the
+    keypoint Jacobian of the G trial bodies and one ops.fit_lm_keypoints_2d_calibrated_step, two launches, four with
+    measurements, no host synchronisation) or 'adam' (SMPLX.forward(transl=) and PerspectiveCamera(rotation=,
+    translation=)).  iterations: None means 50 for LM and 600 for Adam.
+    Returns per body {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (G, 1, 3, 3),
+    'body_pose_mat' (G, 21, 3, 3), 'keypoints' (G, K, 3) in the world frame, 'loss' (G,) recomputed through
+    PerspectiveCamera}, with measurements 'measurements' (G, 5), and per view in the caller's order 'proj_joints'
+    (B, K, 2)."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    exact_circumferences(circumference_derivative)
+    if measurements is not None and body_measurements is None:
+        raise ValueError('fit_body_to_calibrated_views: measurements need body_measurements')
+    if robust_sigma is not None and not robust_sigma > 0:
+        raise ValueError(f'fit_body_to_calibrated_views: robust_sigma must be > 0 or None, got {robust_sigma}')
+    if not (pose_prior_weight >= 0 and betas_weight >= 0):
+        raise ValueError('fit_body_to_calibrated_views: pose_prior_weight and betas_weight must be >= 0')
+    nb = body_model.num_betas
+    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
+        raise ValueError(f"fit_body_to_calibrated_views(method='lm'): 22 rotations, {nb} betas and the translation are "
+                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
+    if iterations is None:
+        iterations = 600 if method == 'adam' else 50
+    from . import ops
+    from .autograd import Rot6dFunction
+    device = body_model.shapedirs.device
+    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device)
+    if x.dim() != 3 or x.shape[2] != 2:
+        raise ValueError(f'fit_body_to_calibrated_views: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    B, K = x.shape[0], x.shape[1]
+    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
+                                                                             device=device)
+    w = w.expand(B, K)
+    intr = _intrinsics(focal_length, principal_point, B, device)
+    R = torch.as_tensor(cam_rot, dtype=torch.float32, device=device)
+    T = torch.as_tensor(cam_transl, dtype=torch.float32, device=device)
+    if R.shape != (B, 3, 3) or T.shape != (B, 3):
+        raise ValueError(f'fit_body_to_calibrated_views: cam_rot must be ({B}, 3, 3) and cam_transl ({B}, 3), got '
+                         f'{tuple(R.shape)} and {tuple(T.shape)}')
+    order, offsets = _view_offsets(groups, B)
+    G = offsets.numel() - 1
+    od = _to_device(order, device)
+    inv = torch.argsort(od)
+    gidx = _to_device(torch.repeat_interleave(torch.arange(G), (offsets[1:] - offsets[:-1]).long()), device)
+    x, w, intr, R, T = (t[od].contiguous() for t in (x, w, intr, R, T))
+    first = _to_device(offsets[:-1].long(), device)
+    init = dict(init or {})
+    for k in ('global_rot', 'body_pose'):
+        if init.get('raw_' + k) is not None:
+            init[k] = init['raw_' + k]
+    if init.get('global_rot') is None:
+        mean = torch.ones(3, device=device)          # MEAN_GLOBAL_ROT, filled on the device: no host-to-device copy
+        mean[1:].fill_(-1.0)
+        init['global_rot'] = (R[first].transpose(1, 2) * mean)[..., :2].reshape(G, 6)
+    if init.get('transl') is None:
+        init['transl'] = _ray_start(x, w, intr, R, T, offsets) if G else torch.zeros(0, 3, device=device)
+    params = _start_params(init, G, nb, device, method, 'transl')
+    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
+                                                              device=device).reshape(G, 22, 3, 3).contiguous()
+    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
+    pw, bw = float(pose_prior_weight), float(betas_weight)
+    mterms = None
+    if measurements is not None:
+        tgt, wt = _measurement_terms(measurements, measurement_weights, G, device)
+        mterms = (tgt.contiguous(), wt.contiguous())
+    def loss(joints, bpose, betas):
+        return _calibrated_loss(joints, x, w, intr, R, T, gidx, offsets, sigma, pw, bpose, anchor, bw, betas)
+    if method == 'lm':
+        state = _kp_lm_state(G, K, 22, nb, 'transl', device)
+        if mterms is not None:
+            state.update(meas=torch.empty(G, 5, device=device), meas_jac=torch.empty(G, 5, nb, device=device))
+        if G > 0:
+            trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(),
+                     'transl': params['transl'].contiguous()}
+            ext = torch.cat([R.reshape(B, 9), T], 1).contiguous()
+            ws = ops.fit_lm_calibrated_workspace(B, G, device)
+            packed = body_model.packed(device)
+            pose_anchor = anchor if pw > 0 else None
+            if mterms is not None:
+                exact = exact_circumferences(circumference_derivative)
+                faces, lmk = body_model.faces_i32, body_measurements.landmarks()
+                ops.face_incidence(faces)      # built (one copy to the host) before the loop, which never synchronises
+            for it in range(int(iterations) + 1):
+                tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
+                if mterms is None:
+                    ops.fit_lm_keypoints_2d_calibrated_step(state, trial, x, w, intr, ext, sigma, pw, bw, LM_UP,
+                                                            LM_DOWN, it == 0, tkp, tjac, offsets, ws,
+                                                            pose_anchor=pose_anchor)
+                else:
+                    v = ops.smplx_forward_shape(packed, trial['betas'])
+                    tm, tmj, _ = ops.measure_jacobian_betas(packed, lmk, v, faces, exact=exact)
+                    ops.fit_lm_keypoints_2d_calibrated_measurements_step(
+                        state, trial, x, w, intr, ext, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0,
+                        tkp, tjac, tm, tmj, offsets, ws, pose_anchor=pose_anchor)
+        rot = state['rot']
+        with torch.no_grad():
+            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], transl=state['transl'],
+                             return_shaped=False)
+            joints = out['joints'][:]
+            per_body, proj, behind = loss(joints, rot[:, 1:], state['betas'])
+            if mterms is not None:
+                per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], 0.0)
+            per_body = torch.where(behind, torch.full_like(per_body, float('inf')), per_body)
+        res = _kp_lm_result(state, 'transl', keypoints=joints, proj_joints=proj[inv], loss=per_body)
+        if mterms is not None:
+            res['measurements'] = state['meas']
+        return res
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
+                         return_shaped=False)
+        joints = out['joints'][:]
+        per_body, proj, behind = loss(joints, bpose, params['betas'])
+        meas = None
+        if mterms is not None:
+            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
+            m = body_measurements.forward_vertices(v, body_model.faces_i32, circumference_derivative)['measurements']
+            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], 0.0)
+        return per_body, joints, proj, grot, bpose, meas, behind
+
+    per_body, joints, proj, grot, bpose, meas, behind = _adam(list(params.values()), lr, iterations, loss_fn)
+    per_body = torch.where(behind, torch.full_like(per_body, float('inf')), per_body)
+    res = {k: v.detach() for k, v in params.items()}
+    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, proj_joints=proj[inv], loss=per_body)
+    if meas is not None:
+        res['measurements'] = meas
+    return res
+
+
 def main(argv=None):
     p = argparse.ArgumentParser(description='Fit SMPL-X betas to virtual measurements (batched, on the GPU)')
     src = p.add_mutually_exclusive_group(required=True)
@@ -941,6 +1180,10 @@ def main(argv=None):
     p.add_argument('--share-pose', dest='share_pose', action='store_true',
                    help="with --keypoints-2d and a `groups` array: the images of a group are simultaneous views of "
                         "one posed body and share its body pose as well as its shape")
+    p.add_argument('--calibrated', action='store_true',
+                   help='with --keypoints-2d, a focal_length and cam_rot (B, 3, 3) / cam_transl (B, 3) in the npz: the '
+                        'rows are views of a calibrated rig, fitted in its world frame (fit_body_to_calibrated_views); '
+                        'an optional `groups` array labels the body each view sees')
     a = p.parse_args(argv)
 
     from . import synth
@@ -1000,7 +1243,9 @@ def _main_keypoints_2d(a, model, bm, targets):
         x = x[None] if x.ndim == 2 else x
         w = d['weights'].astype(np.float32).reshape(x.shape[:2]) if 'weights' in d.files else None
     init = None
-    if a.init:
+    if a.calibrated and not (persp and 'cam_rot' in d.files and 'cam_transl' in d.files):
+        raise SystemExit('--calibrated needs focal_length, cam_rot and cam_transl in --keypoints-2d')
+    if a.init and not a.calibrated:
         p = np.load(a.init)
         init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(x.shape[0], -1)
                 for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera', 'transl')
@@ -1010,6 +1255,8 @@ def _main_keypoints_2d(a, model, bm, targets):
                 raise SystemExit('--init with a camera and a focal_length needs center and scale in --keypoints-2d')
             init['transl'] = perspective_start(init['camera'], d['center'], d['scale'], focal, pp)
     groups = d['groups'].astype(np.int64).reshape(-1) if 'groups' in d.files else None
+    if a.calibrated:
+        return _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups)
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
@@ -1020,6 +1267,30 @@ def _main_keypoints_2d(a, model, bm, targets):
         out['groups'] = groups
     np.savez(a.output, **out)
     print(json.dumps({'bodies': int(x.shape[0]), 'output': a.output, 'median_loss': float(np.median(out['loss']))}))
+
+
+def _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups):
+    """--keypoints-2d --calibrated: the per-body result (G rows) and each view's proj_joints (B rows, the npz's order).
+    An --init npz is per body, with transl in the world frame."""
+    G = int(groups.max()) + 1 if groups is not None and groups.size else 1
+    init = None
+    if a.init:
+        p = np.load(a.init)
+        init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(G, -1)
+                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'transl')
+                if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+    res = fit_body_to_calibrated_views(model, x, focal, pp, d['cam_rot'].astype(np.float32),
+                                       d['cam_transl'].astype(np.float32), groups=groups, weights=w, init=init,
+                                       method=a.method, iterations=a.iterations, robust_sigma=a.robust_sigma,
+                                       pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight, lr=a.lr,
+                                       body_measurements=bm, measurements=targets,
+                                       circumference_derivative=a.circumference_derivative)
+    out = {k: v.detach().cpu().numpy() for k, v in res.items()}
+    if groups is not None:
+        out['groups'] = groups
+    np.savez(a.output, **out)
+    print(json.dumps({'bodies': int(out['loss'].shape[0]), 'views': int(x.shape[0]), 'output': a.output,
+                      'median_loss': float(np.median(out['loss']))}))
 
 
 if __name__ == '__main__':

@@ -940,3 +940,102 @@ def fit_lm_keypoints_2d_shared_pose_measurements_step(state, trial, targets, wei
                         robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints,
                         trial_jac, group_offsets, workspace, pose_anchor,
                         (meas_targets, meas_weights, trial_meas, trial_meas_jac), share_pose=True)
+
+
+def fit_lm_calibrated_workspace(B, G, device):
+    """The scratch of the calibrated 2D step (include/shapy_b200.h, shapy_fit_lm_calibrated_workspace_bytes): a uint8
+    CUDA tensor, allocated once before an LM loop."""
+    n = lib().shapy_fit_lm_calibrated_workspace_bytes(int(B), int(G))
+    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+
+
+def _fit_lm_kp2d_calibrated(what, state, trial, targets, weights, intrinsics, extrinsics, robust_sigma,
+                            pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                            view_offsets, workspace, pose_anchor, meas=None):
+    """What the two calibrated 2D steps share: the checks and the call, `meas` None or (meas_targets, meas_weights,
+    trial_meas, trial_meas_jac), all (G, ...)."""
+    G, n_rot = trial['rot'].shape[:2]
+    nb, B, K = trial['betas'].shape[1], targets.shape[0], targets.shape[1]
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    off = view_offsets
+    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
+            off.is_contiguous()):
+        raise RuntimeError(f'{what}: view_offsets must be a contiguous (G + 1,) int32 CPU tensor')
+    if off.numel() != G + 1 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
+        raise ValueError(f'{what}: view_offsets must rise strictly from 0 to the number of views ({B}) over {G} bodies')
+    anchor = [] if pose_anchor is None else [pose_anchor]
+    mstate = [] if meas is None else [state['meas'], state['meas_jac']]
+    ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
+        [trial[k] for k in ('rot', 'betas', 'transl')] + [targets, weights, intrinsics, extrinsics, trial_keypoints,
+                                                          trial_jac] + anchor + list(meas or ())
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights, cameras and anchor', state['accepted'])
+    P = 3 * n_rot + nb + 3
+    if trial_jac.shape != (G, 3 * K, P) or state['jac'].shape != (G, 3 * K, P) or \
+            any(state[k].shape != (G,) for k in ('loss', 'lambda', 'accepted')):
+        raise RuntimeError(f'{what}: per body, jac must be ({G}, {3 * K}, {P}) and loss, lambda and accepted ({G},)')
+    if targets.shape != (B, K, 2) or weights.shape != (B, K) or intrinsics.shape != (B, 3) or \
+            extrinsics.shape != (B, 12):
+        raise RuntimeError(f'{what}: per view, targets must be ({B}, {K}, 2), weights ({B}, {K}), intrinsics ({B}, 3) '
+                           f'and extrinsics ({B}, 12)')
+    if pose_anchor is not None and pose_anchor.shape != (G, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({G}, {n_rot}, 3, 3)')
+    if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], G, nb):
+        raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
+                           f'({G}, 5)')
+    L = lib()
+    need = L.shapy_fit_lm_calibrated_workspace_bytes(B, G)
+    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
+        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    if G == 0:
+        return
+    head = [B, G, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(extrinsics),
+            ptr(pose_anchor), sigma, float(pose_prior_weight), float(betas_weight)]
+    lam = [float(lambda_up), float(lambda_down), int(bool(first))]
+    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['transl']), ptr(trial_keypoints), ptr(trial_jac)]
+    with torch.cuda.device(trial['rot'].device):
+        if meas is None:
+            check(L.shapy_fit_lm_keypoints_2d_calibrated_step(
+                *head, *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+                *tr, ptr(workspace), stream_ptr()), what)
+        else:
+            check(L.shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
+                *head, ptr(meas[0]), ptr(meas[1]), *lam,
+                *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
+                                          'lambda', 'accepted')],
+                *tr, ptr(meas[2]), ptr(meas[3]), ptr(workspace), stream_ptr()), what)
+
+
+def fit_lm_keypoints_2d_calibrated_step(state, trial, targets, weights, intrinsics, extrinsics, robust_sigma,
+                                        pose_prior_weight, betas_weight, lambda_up, lambda_down, first,
+                                        trial_keypoints, trial_jac, view_offsets, workspace, pose_anchor=None):
+    """One Levenberg-Marquardt step per body of the fit to the 2D keypoints of a calibrated rig (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_calibrated_step), in place.  view_offsets: (G + 1,) int32 CPU tensor, body g seen by the
+    views [off[g], off[g + 1]).  Per view (B rows): targets (B, K, 2), weights (B, K), intrinsics (B, 3) = (f, px, py)
+    and extrinsics (B, 12) = world-to-camera R (row-major) then T.  Per body (G rows): state {'rot' (G, n_rot, 3, 3),
+    'betas', 'transl' (the world translation), 'keypoints', 'jac', 'loss', 'lambda', 'accepted'}, trial {'rot',
+    'betas', 'transl'} (the evaluated trial on entry and the next on return), trial_keypoints / trial_jac from
+    smplx_keypoint_jacobian without transl and pose_anchor (G, n_rot, 3, 3).  workspace from
+    fit_lm_calibrated_workspace.  One launch, no host synchronisation."""
+    _fit_lm_kp2d_calibrated('fit_lm_keypoints_2d_calibrated_step', state, trial, targets, weights, intrinsics,
+                            extrinsics, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down, first,
+                            trial_keypoints, trial_jac, view_offsets, workspace, pose_anchor)
+
+
+def fit_lm_keypoints_2d_calibrated_measurements_step(state, trial, targets, weights, intrinsics, extrinsics,
+                                                     robust_sigma, pose_prior_weight, betas_weight, meas_targets,
+                                                     meas_weights, lambda_up, lambda_down, first, trial_keypoints,
+                                                     trial_jac, trial_meas, trial_meas_jac, view_offsets, workspace,
+                                                     pose_anchor=None):
+    """fit_lm_keypoints_2d_calibrated_step with the five measurements of each body (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_calibrated_measurements_step), in place: state adds 'meas' (G, 5) and 'meas_jac'
+    (G, 5, NB); meas_targets, meas_weights, trial_meas (G, 5) and trial_meas_jac (G, 5, NB) as
+    fit_lm_keypoints_2d_measurements_step's."""
+    _fit_lm_kp2d_calibrated('fit_lm_keypoints_2d_calibrated_measurements_step', state, trial, targets, weights,
+                            intrinsics, extrinsics, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
+                            lambda_down, first, trial_keypoints, trial_jac, view_offsets, workspace, pose_anchor,
+                            (meas_targets, meas_weights, trial_meas, trial_meas_jac))
