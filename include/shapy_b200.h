@@ -468,6 +468,36 @@ int shapy_fit_lm_keypoints_2d_calibrated_step(
     float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
     const float *trial_keypoints, const float *trial_jac, void *workspace, void *stream);
 
+/* One Levenberg-Marquardt step of the perspective 2D fit over video sequences of one person filmed by one camera: the
+ * frames [sequence_offsets[s], sequence_offsets[s+1]) of sequence s (num_sequences + 1 int32 in host memory, rising
+ * strictly from 0 to batch, copied into the workspace on the stream at every call), in time order, share one beta_s;
+ * each frame keeps its rotations and camera-frame translation tau_t and projects as
+ * shapy_fit_lm_keypoints_2d_perspective_step does with its own intrinsics (batch,3).  Loss per sequence, fp64, left to
+ * right: the sum over its frames (frame order) of [the perspective step's keypoint term and pose prior, +
+ * smooth_rot_weight / 2 sum_{j >= 0} |R_{t+1},j - R_t,j|_F^2 + smooth_transl_weight |tau_{t+1} - tau_t|^2 when frame
+ * t + 1 is in the sequence], + betas_weight |beta_s|^2.  Per frame (batch rows): targets, weights, intrinsics,
+ * pose_anchor, rot, transl, keypoints, jac, trial_rot, trial_transl, trial_keypoints, trial_jac and trial_betas_images
+ * (batch,nb), the trial betas of each frame's sequence.  Per sequence (num_sequences rows): betas, loss, lambda,
+ * accepted and trial_betas.  Policy, lambda constants and rotation update are the grouped step's, per sequence; the
+ * first lambda is 1e-3 max(1e-6, the largest diagonal entry of the sequence's keypoint rows), per frame on the
+ * [rotation | translation] columns and summed over the frames on the betas columns.  The normal matrix of a sequence is
+ * block tridiagonal in its frames with an arrow of betas columns; the step solves it exactly by a block LDL^T sweep along
+ * the frames (each frame's block damped by lambda, the betas block by betas_weight + lambda).  Depth rule per frame, as
+ * the perspective step's: a weighted keypoint at Y_z <= 0 or a bad focal length in any frame gives the trial a loss of
+ * +inf.  If a sequence's loss is not finite or one of its pivots fails, it keeps its state.  Three launches, no
+ * synchronisation, no atomics: a sequence's results do not depend on the rest of the batch.  A sequence of one frame has
+ * the perspective step's loss, lambda and decision bit for bit.  workspace: shapy_fit_lm_sequence_workspace_bytes(batch,
+ * num_sequences, n_rot, nb) bytes of device memory.  Errors as shapy_fit_lm_keypoints_2d_groups_step, with a null
+ * intrinsics and smoothness weights < 0 or not finite refused.  batch 0 (with num_sequences 0): no launch. */
+size_t shapy_fit_lm_sequence_workspace_bytes(int batch, int num_sequences, int n_rot, int nb);
+int shapy_fit_lm_keypoints_2d_sequence_step(
+    int batch, int num_sequences, const int32_t *sequence_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *pose_anchor, float robust_sigma,
+    float pose_prior_weight, float betas_weight, float smooth_rot_weight, float smooth_transl_weight, float lambda_up,
+    float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *workspace, void *stream);
+
 /* shapy_fit_lm_keypoints_2d_calibrated_step with the five virtual measurements of each body stacked under its rows, as
  * shapy_fit_lm_keypoints_2d_measurements_step adds them (meas_targets, meas_weights, meas, trial_meas (G,5), meas_jac,
  * trial_meas_jac (G,5,nb)).  With every measurement weight <= 0 every output equals

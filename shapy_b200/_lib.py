@@ -141,6 +141,10 @@ _SIGS = {
                                                                        c_void_p, C.c_float, C.c_float, C.c_float,
                                                                        c_void_p, c_void_p, C.c_float, C.c_float, c_int]
                                                                + [c_void_p] * 17 + [c_void_p, c_void_p]),
+    'shapy_fit_lm_sequence_workspace_bytes': (C.c_size_t, [c_int, c_int, c_int, c_int]),
+    'shapy_fit_lm_keypoints_2d_sequence_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                        c_void_p, c_void_p] + [C.c_float] * 7 + [c_int]
+                                                + [c_void_p] * 14 + [c_void_p, c_void_p]),
     'shapy_mmi_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_size_t, c_void_p]),

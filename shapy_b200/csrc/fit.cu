@@ -751,7 +751,8 @@ __device__ __forceinline__ void lm_kp2d_row(const float *M, const float *tg, con
 // Column col of that row, the camera columns at oc: s J_{3k+c} on the rotation and betas columns, ds (kp_kc + c_{1+c})
 // on c0, s on c_{1+c}.  REORDER: columns [delta | c | beta] (the grouped step), else [delta | beta | c].  PERSP (columns
 // [delta | beta | t]): fz[0] (J_{3k+c} - fz[1] J_{3k+2}) with the row's factors fz, J_t = I; with a CalibCam, fz[0]
-// J_{3k} + fz[1] J_{3k+1} + fz[2] J_{3k+2} (fz[d] on t column d)
+// J_{3k} + fz[1] J_{3k+1} + fz[2] J_{3k+2} (fz[d] on t column d).  REORDER and PERSP: the perspective row in the
+// columns [delta | t | beta] (the sequence step), t at oc .. oc + 2
 template <bool REORDER, bool PERSP = false, typename Cam = PerspCam>
 __device__ __forceinline__ double lm_kp2d_entry(const float *J, const float *M, int P, int oc, int k, int c, int col,
                                                 double s, double ds, const double (&cxy)[2],
@@ -760,6 +761,12 @@ __device__ __forceinline__ double lm_kp2d_entry(const float *J, const float *M, 
     if (col >= oc) return fz[col - oc];
     const float *Jk = J + (size_t)(3 * k) * P + col;
     return fz[0] * (double)Jk[0] + fz[1] * (double)Jk[P] + fz[2] * (double)Jk[2 * P];
+  } else if constexpr (PERSP && REORDER) {
+    const bool tcol = col >= oc && col < oc + 3;
+    const int jcol = col < oc ? col : col - 3;      // a betas column of the Jacobian sits 3 to the left
+    const double jc = tcol ? (col - oc == c ? 1.0 : 0.0) : (double)J[(size_t)(3 * k + c) * P + jcol];
+    const double jz = tcol ? (col - oc == 2 ? 1.0 : 0.0) : (double)J[(size_t)(3 * k + 2) * P + jcol];
+    return fz[0] * (jc - fz[1] * jz);
   } else if constexpr (PERSP) {
     const double jc = col < oc ? (double)J[(size_t)(3 * k + c) * P + col] : (col - oc == c ? 1.0 : 0.0);
     const double jz = col < oc ? (double)J[(size_t)(3 * k + 2) * P + col] : (col - oc == 2 ? 1.0 : 0.0);
@@ -1441,6 +1448,403 @@ int run_lm_kp2dc(const char *fn, int views, int G, const int32_t *offsets, LmKpA
   return launch_lm_kp(lm_kp2dc_step_kernel<MEAS>, G, a, x, stream);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The sequence step (shapy_fit_lm_keypoints_2d_sequence_step): the frames [off[s], off[s + 1]) of sequence s are one
+// person filmed by one camera, in time order.  Frame t keeps its rotations R_t,j and camera-frame translation tau_t
+// (n1 = 3 n_rot + 3 columns [delta | tau]) and projects as the perspective step does with its own intrinsics; the
+// sequence shares one beta.  Per sequence, in fp64, left to right:
+//   L_s = sum_t (frame order) [the perspective step's keypoint term + pose prior of frame t
+//                              + 1/2 srot_w sum_{j >= 0} |R_{t+1},j - R_t,j|_F^2 (j order, row-major entries)
+//                              + stransl_w |tau_{t+1} - tau_t|^2]  (the last two when t + 1 is in s and the weight > 0)
+//       + betas_w |beta|^2.
+// The smoothness rows of the pair (t, t + 1) are the pose prior's rows with the anchor replaced by the neighbour: weight
+// srot_w / 2, residual R_{t+1},j - R_t,j, Jacobian -R_t,j [e_a]x on frame t's column 3 j + a and +R_{t+1},j [e_a]x on
+// frame t + 1's; then weight stransl_w, residual tau_{t+1} - tau_t, Jacobian -I and +I.  The normal matrix of a sequence
+// is block tridiagonal in its frames with an arrow of betas columns: the diagonal block D_t, the coupling B_t of frame
+// t with beta, and C_t, the block of frame t + 1's rows and frame t's columns, block diagonal: per joint -srot_w / 2
+// D_{t+1},j^T D_t,j (D = the 9 x 3 tangent rows), and -stransl_w I on tau.  Three launches after the keypoint Jacobian:
+//   1. lm_kp2ds_loss_kernel, per frame: the bracket of the trial's loss into its scratch and, on the first step, the
+//      diagonal of its keypoint rows (lm_kp2dg_loss_kernel's slots), so that lm_group_decide<false> decides unchanged;
+//   2. lm_kp2ds_frame_kernel, per frame: the sequence's decision, on accept the frame's trial becomes its state; the
+//      perspective keypoint rows in the column order [delta | tau | beta], the pose-prior rows, then the diagonal blocks
+//      and gradient of the smoothness rows of the previous and the next frame (a neighbour read as accept ? trial :
+//      state, neither written during the launch); A_t (P x P lower) and -g_t into the frame's scratch;
+//   3. lm_kp2ds_sequence_kernel, per sequence: the decision, the sequence's state, then a block LDL^T sweep over its
+//      frames (block Thomas, the arrow carried along): with Dt_0 = D_0 + lambda I,
+//        Dt_t = D_t + lambda I - C_{t-1} Dt_{t-1}^-1 C_{t-1}^T,  Bt_t = B_t - C_{t-1} Dt_{t-1}^-1 Bt_{t-1},
+//        rt_t = -g_t - C_{t-1} Dt_{t-1}^-1 rt_{t-1},  Et = E - sum_t Bt_t^T Dt_t^-1 Bt_t,  et = -g_beta - sum_t ...,
+//      each frame's [Dt_t | Bt_t] factored by lm_kp_solve with n = n1 in shared memory (the trailing block carries Et),
+//      then X_t = Dt_t^-1 Bt_t, Y_t = Dt_t^-1 C_t^T and y_t = Dt_t^-1 rt_t into the frame's scratch; Et (+ betas_w +
+//      lambda on its diagonal) dbeta = et - betas_w beta; from the last frame back, x_t = y_t - X_t dbeta - Y_t x_{t+1}
+//      and the next trial R Exp(delta), tau + dtau, beta + dbeta (trial betas per sequence and per frame).
+// The policy is the grouped step's per sequence: one decision, lambda, loss and accept count, the first lambda from the
+// diagonal of the keypoint rows (per frame on [delta | tau], summed over the frames on beta); a sequence whose loss is
+// not finite or one of whose pivots fails keeps its state.  Depth rule per frame, as the perspective step's: a trial
+// with a weighted keypoint at Y_z <= 0 or a bad f in any frame gives the sequence a loss of +inf.  No atomics; a
+// sequence's bits do not depend on the rest of the batch.  A sequence of one frame has the perspective step's loss,
+// lambda and decision bit for bit.
+struct LmKp2dSeqArgs : LmKp2dPerspArgs {     // intr (B, 3) per frame
+  float srot_w, stransl_w;                   // the smoothness weights
+};
+
+// A frame's scratch: lm_group_decide's slots (kScrLoss, kScrDmax, then the nb betas diagonal entries), then A_t (P x P,
+// lower), -g_t (P), and from launch 3 y_t (n1), X_t (nb x n1, beta-major) and Y_t^T (n1 x n1, row k = column k of Y_t)
+constexpr int kSeqA = kScrDiag;               // + nb
+__host__ __device__ inline int lm_seq_stride(int n1, int nb) {
+  const int P = n1 + nb;
+  return kSeqA + nb + P * P + P + n1 + nb * n1 + n1 * n1;
+}
+
+// The sequence of frame b (off[s] <= b < off[s + 1]), by one thread
+__device__ __forceinline__ int lm_seq_of(const LmGroupArgs &gr, int b) {
+  int lo = 0, hi = gr.G - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (gr.off[mid] <= b) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Phase 1: the smoothness term of the pair (b, b + 1) of the trial, rotations then translation
+__device__ __forceinline__ double lm_seq_smooth_loss(const LmKpArgs &a, const LmKp2dSeqArgs &x2, int b) {
+  const int nr9 = 9 * a.n_rot;
+  double L = 0.0;
+  if (x2.srot_w > 0.f) {
+    const float *r0 = a.trot + (size_t)b * nr9, *r1 = r0 + nr9;
+    double q = 0.0;
+    for (int i = 0; i < nr9; ++i) {
+      const double d = (double)r1[i] - (double)r0[i];
+      q += d * d;
+    }
+    L += 0.5 * (double)x2.srot_w * q;
+  }
+  if (x2.stransl_w > 0.f) {
+    const float *t0 = a.tlast + (size_t)b * 3;
+    double q = 0.0;
+    for (int c = 0; c < 3; ++c) {
+      const double d = (double)t0[3 + c] - (double)t0[c];
+      q += d * d;
+    }
+    L += (double)x2.stransl_w * q;
+  }
+  return L;
+}
+
+// Phase 3: the smoothness rows of the pair of frame b (rotations R, translation T) and one neighbour (Rn, Tn), on b's
+// columns [delta | tau]: the diagonal blocks srot_w / 2 D_j^T D_j and stransl_w I, the gradient srot_w / 2 D_j^T (R_j -
+// Rn_j) and stransl_w (T - Tn)
+__device__ __forceinline__ void lm_seq_smooth_rows(const LmKp2dSeqArgs &x2, int o, const float *R, const float *Rn,
+                                                   const float *T, const float *Tn, const int (&pr)[kLmKpPairs],
+                                                   const int (&pc)[kLmKpPairs], double (&acc)[kLmKpPairs], double &g) {
+  const int t = threadIdx.x;
+  if (x2.srot_w > 0.f) {
+    const double hw = 0.5 * (double)x2.srot_w;
+#pragma unroll
+    for (int i = 0; i < kLmKpPairs; ++i) {
+      if (pr[i] >= 0 && pr[i] < o && pc[i] / 3 == pr[i] / 3) {
+        const float *Rj = R + 9 * (pr[i] / 3);
+        for (int e = 0; e < 9; ++e) acc[i] += (hw * rot_tangent(Rj, pr[i] % 3, e)) * rot_tangent(Rj, pc[i] % 3, e);
+      }
+    }
+    if (t < o) {
+      const float *Rj = R + 9 * (t / 3), *Nj = Rn + 9 * (t / 3);
+      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(Rj, t % 3, e)) * ((double)Rj[e] - (double)Nj[e]);
+    }
+  }
+  if (x2.stransl_w > 0.f) {
+    const double w = x2.stransl_w;
+#pragma unroll
+    for (int i = 0; i < kLmKpPairs; ++i)
+      if (pr[i] >= o && pr[i] < o + 3 && pc[i] == pr[i]) acc[i] += w;
+    if (t >= o && t < o + 3) g += w * ((double)T[t - o] - (double)Tn[t - o]);
+  }
+}
+
+__global__ void __launch_bounds__(128) lm_kp2ds_loss_kernel(LmKpArgs a, LmKp2dSeqArgs x2, LmGroupArgs gr) {
+  __shared__ double dg[kLmKpMaxP];
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, nb = a.nb, n1 = 3 * a.n_rot + 3;
+  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * 9 * a.n_rot : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  double *scr = gr.scr + (size_t)b * gr.stride;
+  const PerspCam tc = persp_cam(x2.intr + (size_t)b * 3, a.tlast + (size_t)b * 3);
+  if (t == 0) {
+    double L = lm_kp2d_trial_loss<true>(a, x2, b, tg, wt, anc, robust, s2, &tc);
+    if (b + 1 < gr.off[lm_seq_of(gr, b) + 1]) L += lm_seq_smooth_loss(a, x2, b);
+    scr[kScrLoss] = L;
+  }
+  if (!a.first) return;
+  // the first step accepts: the diagonal of the trial's keypoint rows, column t of [delta | tau | beta], in row order
+  if (t < P) {
+    const float *J = a.tjac + (size_t)b * 3 * K * P, *M = a.tkp + (size_t)b * 3 * K;
+    const double cxy[2] = {0.0, 0.0};   // the weak-perspective camera of lm_kp2d_row / lm_kp2d_entry: not read
+    double d = 0.0;
+    for (int r = 0; r < 2 * K; ++r) {
+      double wr, res, fz[2];
+      lm_kp2d_row<true>(M, tg, wt, 0.0, cxy, robust, s2, r >> 1, r & 1, wr, res, &tc, fz);
+      if (!(wr > 0.0)) continue;
+      const double x = lm_kp2d_entry<true, true>(J, M, P, n1 - 3, r >> 1, r & 1, t, 0.0, 0.0, cxy, fz);
+      d += (wr * x) * x;
+    }
+    dg[t] = d;
+  }
+  __syncthreads();
+  if (t == 0) {
+    double m = kDiagFloor;
+    for (int j = 0; j < n1; ++j) m = fmax(m, dg[j]);
+    scr[kScrDmax] = m;
+  }
+  if (t < nb) scr[kScrDiag + t] = dg[n1 + t];
+}
+
+__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2ds_frame_kernel(LmKpArgs a, LmKp2dSeqArgs x2, LmGroupArgs gr) {
+  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
+  __shared__ double rs[kLmKpRows], ws[kLmKpRows];
+  __shared__ int accept_s, prev_s, next_s;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nr9 = 9 * a.n_rot, o = 3 * a.n_rot;
+  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
+  const bool robust = isfinite(x2.sigma);
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  // 2. the sequence's decision
+  if (t == 0) {
+    const int s = lm_seq_of(gr, b);
+    accept_s = lm_group_decide<false>(a, x2, gr, s).accept;
+    prev_s = b > gr.off[s];
+    next_s = b + 1 < gr.off[s + 1];
+  }
+  __syncthreads();
+  const bool accept = accept_s;
+  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
+  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
+  const float *Rs = accept ? a.trot : a.rot, *Ts = accept ? a.tlast : a.last;   // every frame of the sequence's state
+  const float *Rst = Rs + (size_t)b * nr9, *Tst = Ts + (size_t)b * 3;
+  if (accept) lm_kp_take_trial(a, b, 0.f, false);
+  // 3. the frame's rows, columns [delta | tau | beta]
+  int pr[kLmKpPairs], pc[kLmKpPairs];
+  double acc[kLmKpPairs], g = 0.0;
+  lm_kp_pairs(P, pr, pc, acc);
+  const double cxy[2] = {0.0, 0.0};     // the weak-perspective camera of lm_kp2d_row / lm_kp2d_entry: not read
+  const PerspCam sc = persp_cam(x2.intr + (size_t)b * 3, Tst);
+  lm_kp2d_keypoint_rows<true, true>(K, P, J, M, tg, wt, 0.0, 0.0, cxy, robust, s2, o, Js, WJs, ws, rs, pr, pc, acc, g,
+                                    &sc);
+  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
+  if (prev_s) lm_seq_smooth_rows(x2, o, Rst, Rst - nr9, Tst, Tst - 3, pr, pc, acc, g);
+  if (next_s) lm_seq_smooth_rows(x2, o, Rst, Rst + nr9, Tst, Tst + 3, pr, pc, acc, g);
+  double *At = gr.scr + (size_t)b * gr.stride + kSeqA + a.nb;
+  lm_kp_store(P, At, At + P * P, pr, pc, acc, g);
+}
+
+__global__ void __launch_bounds__(kLmKpThreads) lm_kp2ds_sequence_kernel(LmKpArgs a, LmKp2dSeqArgs x2,
+                                                                          LmGroupArgs gr) {
+  extern __shared__ double S[];         // [P][P]: [Dt_t | Bt_t^T ; Et] lower, then its partial factor; then [n1][n1]: Y_t
+  __shared__ double y[kLmKpMaxP], xs[2][kLmKpMaxP], db[kLmKpMaxP], Cs[kLmKpMaxP][3];   // Cs: row k of C_t, its block
+  __shared__ float lam_s;
+  __shared__ int accept_s, ok_s;
+  const int s = blockIdx.x, t = threadIdx.x, P = a.P, nb = a.nb, o = 3 * a.n_rot, n1 = o + 3, nr9 = 9 * a.n_rot;
+  const int i0 = gr.off[s], i1 = gr.off[s + 1];
+  double *Ys = S + P * P;
+  if (t == 0) {
+    const LmGroupDecision d = lm_group_decide<false>(a, x2, gr, s);
+    accept_s = d.accept;
+    lam_s = d.lam;
+    if (d.accept) a.loss[s] = d.lnew;
+    a.lambda[s] = d.lam;
+    if (d.accept && !a.first) a.accepted[s] += 1;
+    ok_s = isfinite(d.lnew);            // a sequence without a finite loss does not move, nor one with a failed pivot
+  }
+  __syncthreads();
+  const bool accept = accept_s;
+  const double lam = (double)lam_s;
+  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)s * nb;
+  if (accept)
+    for (int l = t; l < nb; l += blockDim.x) a.betas[(size_t)s * nb + l] = a.tbetas[(size_t)s * nb + l];
+  // the forward sweep
+  for (int i = i0; i < i1; ++i) {
+    double *scr = gr.scr + (size_t)i * gr.stride;
+    const double *Ai = scr + kSeqA + nb, *gi = Ai + P * P;
+    const double *pv = scr - gr.stride + kSeqA + nb + P * P + P;   // the previous frame's y, X, (Y in shared memory)
+    const double *yp = pv, *Xp = pv + n1;
+    const bool more = i > i0;
+    for (int q = t; q < P * P; q += blockDim.x) {
+      const int r = q / P, c = q % P;
+      if (c > r) continue;
+      double v = Ai[q];
+      if (r < n1) {                     // Dt_t: D_t + lambda I - C_{t-1} Y_{t-1}
+        if (r == c) v += lam;
+        if (more) {
+          const int m0 = 3 * (r / 3);
+          for (int m = 0; m < 3; ++m) v -= Cs[r][m] * Ys[(m0 + m) * n1 + c];
+        }
+        S[q] = v;
+      } else if (c < n1) {              // Bt_t^T: B_t^T - (C_{t-1} X_{t-1})^T
+        if (more) {
+          const int m0 = 3 * (c / 3);
+          for (int m = 0; m < 3; ++m) v -= Cs[c][m] * Xp[(r - n1) * n1 + m0 + m];
+        }
+        S[q] = v;
+      } else {                          // E, summed in frame order under the Schur updates so far
+        S[q] = more ? S[q] + v : v;
+      }
+    }
+    for (int j = t; j < P; j += blockDim.x) {
+      double v = gi[j];
+      if (j < n1) {
+        if (more) {
+          const int m0 = 3 * (j / 3);
+          for (int m = 0; m < 3; ++m) v -= Cs[j][m] * yp[m0 + m];
+        }
+        y[j] = v;
+      } else {
+        y[j] = more ? y[j] + v : v;
+      }
+    }
+    // Dt_t factored: the trailing block becomes Et - Bt_t^T Dt_t^-1 Bt_t, y's tail et - Bt_t^T Dt_t^-1 rt_t, y's head
+    // Dt_t^-1 rt_t (lm_kp_solve starts with a barrier)
+    lm_kp_solve(S, y, P, n1, ok_s);
+    // X_t = Dt_t^-1 Bt_t in place in the rows n1.. of S, as the grouped image kernel does
+    for (int j = n1 - 1; j >= 0; --j) {
+      for (int l = t; l < nb; l += blockDim.x) S[(n1 + l) * P + j] /= S[j * P + j];
+      __syncthreads();
+      for (int q = t; q < nb * j; q += blockDim.x) {
+        const int l = q / j, k = q % j;
+        S[(n1 + l) * P + k] -= S[j * P + k] * S[(n1 + l) * P + j];
+      }
+      __syncthreads();
+    }
+    double *yo = scr + kSeqA + nb + P * P + P, *Xo = yo + n1, *Yo = Xo + nb * n1;
+    for (int j = t; j < n1; j += blockDim.x) yo[j] = y[j];
+    for (int q = t; q < nb * n1; q += blockDim.x) Xo[q] = S[(n1 + q / n1) * P + q % n1];
+    if (i + 1 < i1) {
+      // C_t from the state rotations of frames t and t + 1 (launch 2 made an accepted trial the state)
+      for (int k = t; k < n1; k += blockDim.x) {
+        for (int m = 0; m < 3; ++m) {
+          double v = 0.0;
+          if (k < o) {
+            if (x2.srot_w > 0.f) {
+              const double hw = 0.5 * (double)x2.srot_w;
+              const float *Rn = a.rot + (size_t)(i + 1) * nr9 + 9 * (k / 3), *Rc = a.rot + (size_t)i * nr9 + 9 * (k / 3);
+              for (int e = 0; e < 9; ++e) v += (hw * rot_tangent(Rn, k % 3, e)) * rot_tangent(Rc, m, e);
+            }
+          } else if (m == k - o) {
+            v = (double)x2.stransl_w;
+          }
+          Cs[k][m] = -v;
+        }
+      }
+      __syncthreads();
+      // Y_t = Dt_t^-1 C_t^T: C_t^T into Ys (row m, column k), then L z = C^T and L^T Y = z, each row scaled by its
+      // pivot after the elimination.  Column k of C_t^T is zero above its block, and stays so under L^-1
+      for (int q = t; q < n1 * n1; q += blockDim.x) {
+        const int m = q / n1, k = q % n1;
+        Ys[q] = m / 3 == k / 3 ? Cs[k][m % 3] : 0.0;
+      }
+      __syncthreads();
+      for (int j = 0; j < n1; ++j) {
+        const int kmax = 3 * (j / 3) + 3, rows = n1 - j - 1;
+        for (int q = t; q < rows * kmax; q += blockDim.x) {
+          const int r = j + 1 + q / kmax, k = q % kmax;
+          Ys[r * n1 + k] -= (S[r * P + j] / S[j * P + j]) * Ys[j * n1 + k];
+        }
+        __syncthreads();
+      }
+      for (int q = t; q < n1 * n1; q += blockDim.x) Ys[q] /= S[(q / n1) * P + q / n1];
+      __syncthreads();
+      for (int j = n1 - 1; j > 0; --j) {
+        for (int q = t; q < j * n1; q += blockDim.x) {
+          const int r = q / n1, k = q % n1;
+          Ys[r * n1 + k] -= (S[j * P + r] / S[j * P + j]) * Ys[j * n1 + k];
+        }
+        __syncthreads();
+      }
+      for (int q = t; q < n1 * n1; q += blockDim.x) Ys[q] /= S[(q / n1) * P + q / n1];
+      __syncthreads();
+      for (int q = t; q < n1 * n1; q += blockDim.x) Yo[q] = Ys[(q % n1) * n1 + q / n1];
+    }
+    __syncthreads();
+  }
+  // Et dbeta = et: the trailing block, betas_w beta and the damping betas_w + lambda
+  double *E = Ys;
+  for (int q = t; q < nb * nb; q += blockDim.x) {
+    const int r = q / nb, c = q % nb;
+    E[q] = c <= r ? S[(n1 + r) * P + n1 + c] + (r == c ? (double)x2.betas_w + lam : 0.0) : 0.0;
+  }
+  for (int l = t; l < nb; l += blockDim.x)
+    db[l] = x2.betas_w > 0.f ? y[n1 + l] - (double)x2.betas_w * (double)Bst[l] : y[n1 + l];
+  lm_kp_solve(E, db, nb, nb, ok_s);
+  const bool ok = ok_s;
+  // the back-substitution from the last frame, and each frame's next trial
+  for (int i = i1 - 1; i >= i0; --i) {
+    const double *yo = gr.scr + (size_t)i * gr.stride + kSeqA + nb + P * P + P, *Xo = yo + n1, *Yo = Xo + nb * n1;
+    double *xc = xs[i & 1];
+    const double *xn = xs[(i + 1) & 1];
+    for (int j = t; j < n1; j += blockDim.x) {
+      double v = yo[j];
+      for (int l = 0; l < nb; ++l) v -= Xo[l * n1 + j] * db[l];
+      if (i + 1 < i1)
+        for (int k = 0; k < n1; ++k) v -= Yo[k * n1 + j] * xn[k];
+      xc[j] = v;
+    }
+    __syncthreads();
+    for (int j = t; j < a.n_rot; j += blockDim.x) {
+      const float *Rs = a.rot + (size_t)i * nr9 + 9 * j;
+      float *Rt = a.trot + (size_t)i * nr9 + 9 * j;
+      if (ok) lm_exp_gs(Rs, xc[3 * j], xc[3 * j + 1], xc[3 * j + 2], Rt);
+      else
+        for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
+    }
+    if (t < 3) {
+      const float x = a.last[(size_t)i * 3 + t];
+      a.tlast[(size_t)i * 3 + t] = ok ? (float)((double)x + xc[o + t]) : x;
+    }
+    for (int l = t; l < nb; l += blockDim.x)
+      gr.tbetas_img[(size_t)i * nb + l] = ok ? (float)((double)Bst[l] + db[l]) : Bst[l];
+  }
+  for (int l = t; l < nb; l += blockDim.x) {
+    const float x = Bst[l];
+    a.tbetas[(size_t)s * nb + l] = ok ? (float)((double)x + db[l]) : x;
+  }
+}
+
+// The sequence entry's checks (check_lm_kp's, the smoothness weights, then the offsets, read on the host) and the three
+// launches; the offsets are copied into the workspace on the stream
+int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpArgs a, LmKp2dSeqArgs x,
+                 float *tbetas_img, void *workspace, bool extra_ok, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, extra_ok && offsets && x.intr && tbetas_img && workspace,
+                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f && x.srot_w >= 0.f &&
+                                 isfinite(x.srot_w) && x.stransl_w >= 0.f && isfinite(x.stransl_w),
+                             "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0, the smoothness "
+                             "weights finite and >= 0 and lambda_up and lambda_down >= 1");
+  if (rc != SHAPY_OK) return rc;
+  SHAPY_REQUIRE(G >= 0 && offsets[0] == 0 && offsets[G] == batch,
+                "%s: sequence_offsets must run from 0 to the batch (%d) over %d sequences", fn, batch, G);
+  for (int g = 0; g < G; ++g)
+    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: sequence %d is empty (offsets %d, %d)", fn, g, offsets[g],
+                  offsets[g + 1]);
+  if (batch == 0) return SHAPY_OK;
+  const int n1 = 3 * a.n_rot + 3;
+  int *off = (int *)workspace;
+  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_seq_stride(n1, a.nb),
+                 tbetas_img};
+  cudaStream_t st = (cudaStream_t)stream;
+  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  lm_kp2ds_loss_kernel<<<batch, 128, 0, st>>>(a, x, gr);
+  SHAPY_LAUNCH_CHECK();
+  lm_kp2ds_frame_kernel<<<batch, kLmKpThreads, 0, st>>>(a, x, gr);
+  SHAPY_LAUNCH_CHECK();
+  const int ny = n1 > a.nb ? n1 : a.nb;
+  const size_t smem = (size_t)(a.P * a.P + ny * ny) * sizeof(double);
+  cudaFuncAttributes attr;
+  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2ds_sequence_kernel));
+  if (smem + attr.sharedSizeBytes > 48 * 1024)
+    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2ds_sequence_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  lm_kp2ds_sequence_kernel<<<G, kLmKpThreads, smem, st>>>(a, x, gr);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -1685,4 +2089,24 @@ extern "C" int shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
                             (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
                                 meas_jac && trial_meas && trial_meas_jac,
                             stream);
+}
+
+extern "C" size_t shapy_fit_lm_sequence_workspace_bytes(int batch, int num_sequences, int n_rot, int nb) {
+  if (batch < 0 || num_sequences < 0 || n_rot < 1 || nb < 1) return 0;
+  return lm_group_offsets_bytes(num_sequences) + (size_t)batch * lm_seq_stride(3 * n_rot + 3, nb) * sizeof(double);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_sequence_step(
+    int batch, int num_sequences, const int32_t *sequence_offsets, int num_keypoints, int n_rot, int nb,
+    const float *targets, const float *weights, const float *intrinsics, const float *pose_anchor, float robust_sigma,
+    float pose_prior_weight, float betas_weight, float smooth_rot_weight, float smooth_transl_weight, float lambda_up,
+    float lambda_down, int first, float *rot, float *betas, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_betas_images,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *workspace, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dSeqArgs x{{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics},
+                  smooth_rot_weight, smooth_transl_weight};
+  return run_lm_kp2ds("shapy_fit_lm_keypoints_2d_sequence_step", batch, num_sequences, sequence_offsets, a, x,
+                      trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
 }

@@ -101,6 +101,12 @@ method='lm' each iteration is the keypoint Jacobian of the bodies (one per body,
 ops.fit_lm_keypoints_2d_calibrated_step, two launches (four with measurements), no host synchronisation.
 calibrated_start maps a camera-frame start of one view (a perspective fit, or perspective_start) into the world frame.
 
+fit_body_to_sequence fits videos of one person filmed by one camera with known intrinsics: per frame the pose and the
+camera-frame translation, per sequence one betas, and smoothness terms tying each frame to the next, so the pose and
+translation do not jitter from frame to frame.  With method='lm' each iteration is the keypoint Jacobian of every frame
+and ops.fit_lm_keypoints_2d_sequence_step, whose three launches solve each sequence's block-tridiagonal normal matrix
+exactly by a block LDL^T sweep along its frames, no host synchronisation.
+
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
@@ -1133,6 +1139,140 @@ def fit_body_to_calibrated_views(body_model, keypoints2d, focal_length, principa
     return res
 
 
+def _smoothness(rot, transl, gidx, srw, stw):
+    """Per frame (sorted by sequence) the smoothness term of the pair (t, t + 1), 0 for a sequence's last frame:
+    srw / 2 sum_j |R_{t+1},j - R_t,j|_F^2 + stw |tau_{t+1} - tau_t|^2."""
+    out = torch.zeros(rot.shape[0], dtype=rot.dtype, device=rot.device)
+    if rot.shape[0] < 2 or not (srw > 0 or stw > 0):
+        return out
+    d = torch.zeros_like(out[1:])
+    if srw > 0:
+        d = d + 0.5 * srw * (rot[1:] - rot[:-1]).pow(2).sum((1, 2, 3))
+    if stw > 0:
+        d = d + stw * (transl[1:] - transl[:-1]).pow(2).sum(1)
+    return torch.cat([torch.where(gidx[1:] == gidx[:-1], d, torch.zeros_like(d)), out[:1]])
+
+
+def fit_body_to_sequence(body_model, keypoints2d, focal_length, principal_point, sequences=None, weights=None,
+                         init=None, method='lm', iterations=None, robust_sigma=None, pose_prior_weight=0.0,
+                         betas_weight=0.0, pose_anchor=None, smooth_rot_weight=0.0, smooth_transl_weight=0.0, lr=0.05):
+    """Fits videos of one person filmed by one camera: per frame the pose and the camera-frame translation, per
+    sequence one betas, with smoothness between consecutive frames, to the full-image 2D keypoints (B, K, 2) of every
+    frame under a perspective camera with known intrinsics (focal_length a scalar or (B,), principal_point (2,) or
+    (B, 2), as fit_body_to_keypoints_2d's; camera frame x right, y down, z forward).
+    sequences: None (the whole batch is one sequence) or (B,) integer labels 0 .. S-1 (group_plan's rules); the frames
+    of a label, in the caller's order, are that sequence in time order.  Loss per sequence: the sum over its frames of
+    fit_body_to_keypoints_2d's perspective loss (keypoint term and pose prior), + smooth_rot_weight / 2 sum_{j >= 0}
+    |R_{t+1},j - R_t,j|_F^2 (the global rotation included) + smooth_transl_weight |transl_{t+1} - transl_t|^2 over
+    consecutive frames, + betas_weight |betas|^2; +inf when a frame has a weighted keypoint at Y_z <= 0.  The smoothness
+    weights are in the targets' units: with pixel targets a 1 cm jump of the translation between two frames costs
+    smooth_transl_weight * 1e-4 px^2, and a small rotation change of theta rad costs about smooth_rot_weight * theta^2
+    px^2.  With both weights 0 this is the grouped perspective fit: one betas per sequence, independent frames.
+    weights, init and pose_anchor (B, 22, 3, 3) are per frame; init as fit_body_to_keypoints_2d's perspective init
+    ('transl', by default 3 m in front of the camera on the ray through the weighted keypoints' centroid), a sequence
+    starts from the frame-order mean of its frames' init betas.  method: 'lm' (per iteration the keypoint Jacobian of
+    every frame and ops.fit_lm_keypoints_2d_sequence_step, whose three launches solve the sequence's block-tridiagonal
+    normal matrix exactly; no host synchronisation, every sequence's loss non-increasing) or 'adam' (SMPLX.forward
+    (transl=), PerspectiveCamera and the smoothness terms in torch).  iterations: None means 50 for LM, 600 for Adam.
+    Returns per sequence 'betas' (S, NB) and 'loss' (S,) (with 'lm' the step's fp64 loss of the final state), and per
+    frame in the caller's order 'global_rot', 'body_pose' (raw 6D), 'transl', 'global_rot_mat', 'body_pose_mat',
+    'keypoints' (B, K, 3) in the camera frame and 'proj_joints' (B, K, 2)."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    if robust_sigma is not None and not robust_sigma > 0:
+        raise ValueError(f'fit_body_to_sequence: robust_sigma must be > 0 or None, got {robust_sigma}')
+    if not (pose_prior_weight >= 0 and betas_weight >= 0):
+        raise ValueError('fit_body_to_sequence: pose_prior_weight and betas_weight must be >= 0')
+    srw, stw = float(smooth_rot_weight), float(smooth_transl_weight)
+    if not (0 <= srw < float('inf') and 0 <= stw < float('inf')):
+        raise ValueError('fit_body_to_sequence: the smoothness weights must be finite and >= 0')
+    nb = body_model.num_betas
+    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
+        raise ValueError(f"fit_body_to_sequence(method='lm'): 22 rotations, {nb} betas and the translation are "
+                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
+    if iterations is None:
+        iterations = 600 if method == 'adam' else 50
+    from . import ops
+    from .autograd import Rot6dFunction
+    device = body_model.shapedirs.device
+    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device).contiguous()
+    if x.dim() != 3 or x.shape[2] != 2:
+        raise ValueError(f'fit_body_to_sequence: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    B, K = x.shape[0], x.shape[1]
+    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
+                                                                             device=device)
+    w = w.expand(B, K).contiguous()
+    intr = _intrinsics(focal_length, principal_point, B, device)
+    params = _init_2d(init, B, nb, device, method, x, w, intr)
+    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
+                                                              device=device).reshape(B, 22, 3, 3).contiguous()
+    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
+    pw, bw = float(pose_prior_weight), float(betas_weight)
+    order, offsets = _view_offsets(sequences, B)
+    S = offsets.numel() - 1
+    counts = (offsets[1:] - offsets[:-1]).long()
+    od = _to_device(order, device)
+    inv = torch.argsort(od)
+    gidx = _to_device(torch.repeat_interleave(torch.arange(S), counts), device)     # each sorted frame's sequence
+    x, w, intr, rot0, anchor = (t[od].contiguous() for t in (x, w, intr, rot0, anchor))
+    sp = {k: v.detach()[od].contiguous() for k, v in params.items()}
+    cnt = _to_device(counts.float(), device)
+    betas0 = (_group_sum(sp['betas'], offsets) / cnt[:, None]).contiguous() if S else torch.zeros(0, nb, device=device)
+    if method == 'lm':
+        state = _kp_lm_state(B, K, 22, nb, 'transl', device)
+        mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
+        state.update({'betas': mk(S, nb), 'loss': mk(S), 'lambda': mk(S),     # per sequence
+                      'accepted': torch.zeros(S, dtype=torch.int32, device=device)})
+        if B > 0:
+            trial = {'rot': rot0.clone(), 'betas': betas0, 'image_betas': betas0[gidx].contiguous(),
+                     'transl': sp['transl']}
+            ws = ops.fit_lm_sequence_workspace(B, S, 22, nb, device)
+            packed = body_model.packed(device)
+            pose_anchor = anchor if pw > 0 else None
+            for it in range(int(iterations) + 1):
+                tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['image_betas'], trial['rot'])
+                ops.fit_lm_keypoints_2d_sequence_step(state, trial, x, w, intr, sigma, pw, bw, srw, stw, LM_UP,
+                                                      LM_DOWN, it == 0, tkp, tjac, offsets, ws,
+                                                      pose_anchor=pose_anchor)
+        rot = state['rot']
+        with torch.no_grad():
+            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'][gidx],
+                             transl=state['transl'], return_shaped=False)
+            joints = out['joints'][:]
+            proj = _project(joints, intr)
+        # a start that breaks the depth rule leaves the kernel's loss NaN: its loss is +inf
+        loss = torch.where(torch.isnan(state['loss']), torch.full_like(state['loss'], float('inf')), state['loss'])
+        res = _kp_lm_result(state, 'transl', keypoints=joints, proj_joints=proj, loss=loss)
+    else:
+        p = {k: sp[k].clone().requires_grad_(True) for k in ('global_rot', 'body_pose', 'transl')}
+        p['betas'] = betas0.clone().requires_grad_(True)
+
+        def loss_fn():
+            grot = Rot6dFunction.apply(p['global_rot'])
+            bpose = Rot6dFunction.apply(p['body_pose'])
+            out = body_model(global_rot=grot, body_pose=bpose, betas=p['betas'][gidx], transl=p['transl'],
+                             return_shaped=False)
+            joints = out['joints'][:]
+            proj = _project(joints, intr)
+            rot = torch.cat([grot, bpose], 1)
+            per_frame = _kp2d_loss(proj, x, w, sigma, pw, rot, anchor, 0.0, None) + \
+                _smoothness(rot, p['transl'], gidx, srw, stw)
+            per_seq = _group_sum(per_frame, offsets)
+            if bw > 0:
+                per_seq = per_seq + bw * p['betas'].pow(2).sum(1)
+            return per_seq, joints, proj, grot, bpose
+
+        per_seq, joints, proj, grot, bpose = _adam(list(p.values()), lr, iterations, loss_fn)
+        behind = _group_sum(_depth_rule(torch.zeros_like(x[:, 0, 0]), joints, w).isinf().float(), offsets) > 0
+        res = {k: v.detach() for k, v in p.items()}
+        res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, proj_joints=proj,
+                   loss=torch.where(behind, torch.full_like(per_seq, float('inf')), per_seq))
+    for k in ('global_rot', 'body_pose', 'transl', 'global_rot_mat', 'body_pose_mat', 'keypoints', 'proj_joints'):
+        res[k] = res[k][inv]
+    return res
+
+
 def main(argv=None):
     p = argparse.ArgumentParser(description='Fit SMPL-X betas to virtual measurements (batched, on the GPU)')
     src = p.add_mutually_exclusive_group(required=True)
@@ -1184,6 +1324,14 @@ def main(argv=None):
                    help='with --keypoints-2d, a focal_length and cam_rot (B, 3, 3) / cam_transl (B, 3) in the npz: the '
                         'rows are views of a calibrated rig, fitted in its world frame (fit_body_to_calibrated_views); '
                         'an optional `groups` array labels the body each view sees')
+    p.add_argument('--sequence', action='store_true',
+                   help='with --keypoints-2d and a focal_length in the npz: the rows are the frames of videos of one '
+                        'person filmed by one camera, in time order (fit_body_to_sequence); an optional `sequences` '
+                        'array labels the video of each frame')
+    p.add_argument('--smooth-rot', dest='smooth_rot', type=float, default=0.0,
+                   help='with --sequence: the weight of |R_{t+1} - R_t|_F^2 / 2 between consecutive frames')
+    p.add_argument('--smooth-transl', dest='smooth_transl', type=float, default=0.0,
+                   help='with --sequence: the weight of |transl_{t+1} - transl_t|^2 between consecutive frames')
     a = p.parse_args(argv)
 
     from . import synth
@@ -1257,6 +1405,8 @@ def _main_keypoints_2d(a, model, bm, targets):
     groups = d['groups'].astype(np.int64).reshape(-1) if 'groups' in d.files else None
     if a.calibrated:
         return _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups)
+    if a.sequence:
+        return _main_sequence(a, model, d, x, w, focal, pp, init)
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
@@ -1290,6 +1440,23 @@ def _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups):
         out['groups'] = groups
     np.savez(a.output, **out)
     print(json.dumps({'bodies': int(out['loss'].shape[0]), 'views': int(x.shape[0]), 'output': a.output,
+                      'median_loss': float(np.median(out['loss']))}))
+
+
+def _main_sequence(a, model, d, x, w, focal, pp, init):
+    """--keypoints-2d --sequence: per frame (B rows, the npz's order) and per sequence ('betas', 'loss') results."""
+    if focal is None:
+        raise SystemExit('--sequence needs focal_length in --keypoints-2d')
+    seq = d['sequences'].astype(np.int64).reshape(-1) if 'sequences' in d.files else None
+    res = fit_body_to_sequence(model, x, focal, pp, sequences=seq, weights=w, init=init, method=a.method,
+                               iterations=a.iterations, robust_sigma=a.robust_sigma,
+                               pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight,
+                               smooth_rot_weight=a.smooth_rot, smooth_transl_weight=a.smooth_transl, lr=a.lr)
+    out = {k: v.detach().cpu().numpy() for k, v in res.items()}
+    if seq is not None:
+        out['sequences'] = seq
+    np.savez(a.output, **out)
+    print(json.dumps({'frames': int(x.shape[0]), 'sequences': int(out['loss'].shape[0]), 'output': a.output,
                       'median_loss': float(np.median(out['loss']))}))
 
 

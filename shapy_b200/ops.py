@@ -942,6 +942,74 @@ def fit_lm_keypoints_2d_shared_pose_measurements_step(state, trial, targets, wei
                         (meas_targets, meas_weights, trial_meas, trial_meas_jac), share_pose=True)
 
 
+def fit_lm_sequence_workspace(B, S, n_rot, nb, device):
+    """The scratch of the sequence 2D step (include/shapy_b200.h, shapy_fit_lm_sequence_workspace_bytes): a uint8 CUDA
+    tensor, allocated once before an LM loop."""
+    n = lib().shapy_fit_lm_sequence_workspace_bytes(int(B), int(S), int(n_rot), int(nb))
+    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+
+
+def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics, robust_sigma, pose_prior_weight,
+                                      betas_weight, smooth_rot_weight, smooth_transl_weight, lambda_up, lambda_down,
+                                      first, trial_keypoints, trial_jac, sequence_offsets, workspace, pose_anchor=None):
+    """One Levenberg-Marquardt step of the perspective 2D fit over video sequences (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_sequence_step), in place.  sequence_offsets: (S + 1,) int32 CPU tensor, sequence s the
+    frames [off[s], off[s + 1]) in time order.  Per frame (B rows): targets (B, K, 2), weights (B, K), intrinsics (B, 3)
+    = (f, px, py), pose_anchor (B, n_rot, 3, 3), state 'rot', 'transl', 'keypoints', 'jac' and trial 'rot', 'transl',
+    'image_betas' (each frame's sequence betas, what smplx_keypoint_jacobian evaluated).  Per sequence (S rows): state
+    'betas', 'loss', 'lambda', 'accepted' and trial 'betas'.  smooth_rot_weight / 2 |R_{t+1} - R_t|_F^2 over every
+    rotation and smooth_transl_weight |t_{t+1} - t_t|^2 tie consecutive frames.  workspace from
+    fit_lm_sequence_workspace.  Three launches, no host synchronisation."""
+    what = 'fit_lm_keypoints_2d_sequence_step'
+    B, n_rot = trial['rot'].shape[:2]
+    nb, K = trial['betas'].shape[1], targets.shape[1]
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    srw, stw = float(smooth_rot_weight), float(smooth_transl_weight)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
+    if not (0 <= srw < float('inf') and 0 <= stw < float('inf')):
+        raise ValueError(f'{what}: the smoothness weights must be finite and >= 0')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    off = sequence_offsets
+    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
+            off.is_contiguous()):
+        raise RuntimeError(f'{what}: sequence_offsets must be a contiguous (S + 1,) int32 CPU tensor')
+    S = off.numel() - 1
+    if S < 0 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
+        raise ValueError(f'{what}: sequence_offsets must rise strictly from 0 to the batch ({B})')
+    anchor = [] if pose_anchor is None else [pose_anchor]
+    ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + \
+        [trial[k] for k in ('rot', 'betas', 'image_betas', 'transl')] + [targets, weights, intrinsics, trial_keypoints,
+                                                                         trial_jac] + anchor
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights, intrinsics and anchor', state['accepted'])
+    P = 3 * n_rot + nb + 3
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
+        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
+    if intrinsics.shape != (B, 3) or state['transl'].shape != (B, 3) or trial['transl'].shape != (B, 3):
+        raise RuntimeError(f'{what}: intrinsics and transl must be ({B}, 3)')
+    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if (state['betas'].shape != (S, nb) or trial['betas'].shape != (S, nb) or trial['image_betas'].shape != (B, nb) or
+            any(state[k].shape != (S,) for k in ('loss', 'lambda', 'accepted'))):
+        raise RuntimeError(f'{what}: betas and trial betas must be ({S}, {nb}), image_betas ({B}, {nb}) and loss, '
+                           f'lambda and accepted ({S},)')
+    L = lib()
+    need = L.shapy_fit_lm_sequence_workspace_bytes(B, S, n_rot, nb)
+    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
+        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    if B == 0:
+        return
+    with torch.cuda.device(trial['rot'].device):
+        check(L.shapy_fit_lm_keypoints_2d_sequence_step(
+            B, S, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(pose_anchor), sigma,
+            float(pose_prior_weight), float(betas_weight), srw, stw, float(lambda_up), float(lambda_down),
+            int(bool(first)),
+            *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+            ptr(trial['rot']), ptr(trial['betas']), ptr(trial['image_betas']), ptr(trial['transl']),
+            ptr(trial_keypoints), ptr(trial_jac), ptr(workspace), stream_ptr()), what)
+
+
 def fit_lm_calibrated_workspace(B, G, device):
     """The scratch of the calibrated 2D step (include/shapy_b200.h, shapy_fit_lm_calibrated_workspace_bytes): a uint8
     CUDA tensor, allocated once before an LM loop."""
