@@ -921,7 +921,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs 
 // What the four keypoint entry points share, `fn` naming the one called: the checks of the arguments in `a` (its P is
 // set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors` its own scalars and the
 // sentence that states their and the lambda factors' ranges; then the launch, one CTA of kLmKpThreads per body with
-// P x P doubles of dynamic shared memory.  Past 48 KB of static plus dynamic shared memory the launch has to opt in
+// P x P doubles of dynamic shared memory
 inline int check_lm_kp(const char *fn, int batch, LmKpArgs &a, bool extra_ok, bool factors_ok, const char *factors) {
   SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
                     a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && extra_ok,
@@ -937,13 +937,21 @@ inline int check_lm_kp(const char *fn, int batch, LmKpArgs &a, bool extra_ok, bo
   return SHAPY_OK;
 }
 
+// Lets `kernel` launch with `smem` bytes of dynamic shared memory: past 48 KB of static plus dynamic shared memory a
+// launch has to opt in
+template <typename... Args>
+cudaError_t allow_dynamic_smem(void (*kernel)(Args...), size_t smem) {
+  cudaFuncAttributes attr;
+  cudaError_t e = cudaFuncGetAttributes(&attr, kernel);
+  if (e == cudaSuccess && smem + attr.sharedSizeBytes > 48 * 1024)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  return e;
+}
+
 template <typename Extra>
 int launch_lm_kp(void (*kernel)(LmKpArgs, Extra), int batch, const LmKpArgs &a, const Extra &x, void *stream) {
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
-  cudaFuncAttributes attr;
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, kernel));
-  if (smem + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
   kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
@@ -1012,6 +1020,22 @@ struct LmGroupArgs {
 constexpr int kScrLoss = 0, kScrOk = 1, kScrDmax = 2, kScrDiag = 3;
 __host__ __device__ inline int lm_group_stride(int n1, int nb) { return kScrDiag + 2 * nb + nb * nb + n1 * nb + n1; }
 inline size_t lm_group_offsets_bytes(int G) { return ((size_t)(G + 1) * sizeof(int) + 15) / 16 * 16; }
+
+// The offsets `name` of a grouped entry, checked on the host: (G + 1) entries rising strictly from 0 to `rows` (the
+// images, views or frames), so that no group, body or sequence is empty.  Then copied on the stream into the head of
+// the workspace, where the kernels read them; nothing is copied for G = 0
+inline int put_group_offsets(const char *fn, const char *name, int rows, int G, const int32_t *offsets,
+                             void *workspace, void *stream) {
+  SHAPY_REQUIRE(G >= 0 && offsets[0] == 0 && offsets[G] == rows, "%s: %s must run from 0 to %d over %d entries + 1",
+                fn, name, rows, G);
+  for (int g = 0; g < G; ++g)
+    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: %s must rise strictly (entries %d, %d: %d, %d)", fn, name, g,
+                  g + 1, offsets[g], offsets[g + 1]);
+  if (G > 0)
+    SHAPY_CUDA_TRY(cudaMemcpyAsync(workspace, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice,
+                                   (cudaStream_t)stream));
+  return SHAPY_OK;
+}
 
 struct LmGroupDecision {
   bool accept;
@@ -1277,33 +1301,20 @@ int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
                              "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                              "lambda_down >= 1");
   if (rc != SHAPY_OK) return rc;
-  SHAPY_REQUIRE(G >= 0 && offsets[0] == 0 && offsets[G] == batch,
-                "%s: group_offsets must run from 0 to the batch (%d) over %d groups", fn, batch, G);
-  for (int g = 0; g < G; ++g)
-    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: group %d is empty (offsets %d, %d)", fn, g, offsets[g],
-                  offsets[g + 1]);
-  if (batch == 0) return SHAPY_OK;
+  const int orc = put_group_offsets(fn, "group_offsets", batch, G, offsets, workspace, stream);
+  if (orc != SHAPY_OK || batch == 0) return orc;
   const int n1 = SHARE ? 6 : 3 * a.n_rot + 3, ns = a.P - n1;
-  int *off = (int *)workspace;
-  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_group_stride(n1, ns),
-                 tbetas_img};
+  LmGroupArgs gr{G, (int *)workspace, (double *)((char *)workspace + lm_group_offsets_bytes(G)),
+                 lm_group_stride(n1, ns), tbetas_img};
   cudaStream_t st = (cudaStream_t)stream;
-  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   lm_kp2dg_loss_kernel<SHARE><<<batch, 128, 0, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   const size_t smem = (size_t)a.P * a.P * sizeof(double);
-  cudaFuncAttributes attr;
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_image_kernel<SHARE>));
-  if (smem + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(
-        cudaFuncSetAttribute(lm_kp2dg_image_kernel<SHARE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2dg_image_kernel<SHARE>, smem));
   lm_kp2dg_image_kernel<SHARE><<<batch, kLmKpThreads, smem, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   const size_t smem3 = (size_t)(ns * ns + n1) * sizeof(double);
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2dg_group_kernel<SHARE>));
-  if (smem3 + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(
-        cudaFuncSetAttribute(lm_kp2dg_group_kernel<SHARE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2dg_group_kernel<SHARE>, smem3));
   lm_kp2dg_group_kernel<SHARE><<<G, kLmKpThreads, smem3, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
@@ -1435,16 +1446,9 @@ int run_lm_kp2dc(const char *fn, int views, int G, const int32_t *offsets, LmKpA
                              "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                              "lambda_down >= 1");
   if (rc != SHAPY_OK) return rc;
-  SHAPY_REQUIRE(offsets[0] == 0 && offsets[G] == views,
-                "%s: view_offsets must run from 0 to the number of views (%d) over %d bodies", fn, views, G);
-  for (int g = 0; g < G; ++g)
-    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: body %d has no view (offsets %d, %d)", fn, g, offsets[g],
-                  offsets[g + 1]);
-  if (G == 0) return SHAPY_OK;
-  int *off = (int *)workspace;
-  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice,
-                                 (cudaStream_t)stream));
-  x.off = off;
+  const int orc = put_group_offsets(fn, "view_offsets", views, G, offsets, workspace, stream);
+  if (orc != SHAPY_OK || G == 0) return orc;
+  x.off = (const int *)workspace;
   return launch_lm_kp(lm_kp2dc_step_kernel<MEAS>, G, a, x, stream);
 }
 
@@ -1818,28 +1822,19 @@ int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
                              "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0, the smoothness "
                              "weights finite and >= 0 and lambda_up and lambda_down >= 1");
   if (rc != SHAPY_OK) return rc;
-  SHAPY_REQUIRE(G >= 0 && offsets[0] == 0 && offsets[G] == batch,
-                "%s: sequence_offsets must run from 0 to the batch (%d) over %d sequences", fn, batch, G);
-  for (int g = 0; g < G; ++g)
-    SHAPY_REQUIRE(offsets[g + 1] > offsets[g], "%s: sequence %d is empty (offsets %d, %d)", fn, g, offsets[g],
-                  offsets[g + 1]);
-  if (batch == 0) return SHAPY_OK;
+  const int orc = put_group_offsets(fn, "sequence_offsets", batch, G, offsets, workspace, stream);
+  if (orc != SHAPY_OK || batch == 0) return orc;
   const int n1 = 3 * a.n_rot + 3;
-  int *off = (int *)workspace;
-  LmGroupArgs gr{G, off, (double *)((char *)workspace + lm_group_offsets_bytes(G)), lm_seq_stride(n1, a.nb),
-                 tbetas_img};
+  LmGroupArgs gr{G, (int *)workspace, (double *)((char *)workspace + lm_group_offsets_bytes(G)),
+                 lm_seq_stride(n1, a.nb), tbetas_img};
   cudaStream_t st = (cudaStream_t)stream;
-  SHAPY_CUDA_TRY(cudaMemcpyAsync(off, offsets, (size_t)(G + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   lm_kp2ds_loss_kernel<<<batch, 128, 0, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   lm_kp2ds_frame_kernel<<<batch, kLmKpThreads, 0, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   const int ny = n1 > a.nb ? n1 : a.nb;
   const size_t smem = (size_t)(a.P * a.P + ny * ny) * sizeof(double);
-  cudaFuncAttributes attr;
-  SHAPY_CUDA_TRY(cudaFuncGetAttributes(&attr, lm_kp2ds_sequence_kernel));
-  if (smem + attr.sharedSizeBytes > 48 * 1024)
-    SHAPY_CUDA_TRY(cudaFuncSetAttribute(lm_kp2ds_sequence_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2ds_sequence_kernel, smem));
   lm_kp2ds_sequence_kernel<<<G, kLmKpThreads, smem, st>>>(a, x, gr);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;

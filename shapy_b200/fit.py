@@ -165,6 +165,56 @@ def _measurement_loss(tgt, wt, meas, betas, betas_weight):
     return (wt * diff.pow(2)).sum(1) + betas_weight * betas.pow(2).sum(1)
 
 
+class _MeasurementTerm:
+    """The measurement term of a fit over n bodies or groups: targets and weights (n, 5) (_measurement_terms), measured
+    by body_measurements on the T-pose of the fitted betas, the circumferences differentiated as
+    circumference_derivative says."""
+
+    def __init__(self, tgt, wt, body_measurements, circumference_derivative):
+        self.tgt, self.wt = tgt.contiguous(), wt.contiguous()
+        self.bm, self.cd = body_measurements, circumference_derivative
+        self.exact = exact_circumferences(circumference_derivative)
+
+    def measure(self, body_model, betas):
+        """The measurements (n, 5) of betas through forward_shape and BodyMeasurements.forward_vertices (Adam)."""
+        v = body_model.forward_shape(betas=betas)['v_shaped']
+        m = self.bm.forward_vertices(v, body_model.faces_i32, self.cd)['measurements']
+        return torch.stack([m[k]['tensor'] for k in NAMES], 1)
+
+    def loss(self, meas, betas, rho):
+        return _measurement_loss(self.tgt, self.wt, meas, betas, rho)
+
+    def prime(self, body_model):
+        """Builds the faces' incidence table (one copy to the host) and the landmarks before an LM loop, which never
+        synchronises."""
+        from . import ops
+        ops.face_incidence(body_model.faces_i32)
+        self.bm.landmarks()
+
+    def trial(self, packed, body_model, betas):
+        """(trial_meas (n, 5), trial_meas_jac (n, 5, NB)) of the trial betas of an LM step: forward_shape and the
+        measurement Jacobian, two launches."""
+        from . import ops
+        v = ops.smplx_forward_shape(packed, betas)
+        meas, jac, _ = ops.measure_jacobian_betas(packed, self.bm.landmarks(), v, body_model.faces_i32,
+                                                  exact=self.exact)
+        return meas, jac
+
+    def state(self, nb, device):
+        """The entries an LM step's state gains with measurements: 'meas' (n, 5) and 'meas_jac' (n, 5, NB)."""
+        n = self.tgt.shape[0]
+        return {'meas': torch.empty(n, 5, dtype=torch.float32, device=device),
+                'meas_jac': torch.empty(n, 5, nb, dtype=torch.float32, device=device)}
+
+
+def _measurement_term(measurements, measurement_weights, n, device, body_measurements, circumference_derivative):
+    """The _MeasurementTerm of n bodies or groups, or None without measurements."""
+    if measurements is None:
+        return None
+    tgt, wt = _measurement_terms(measurements, measurement_weights, n, device)
+    return _MeasurementTerm(tgt, wt, body_measurements, circumference_derivative)
+
+
 def _adam(params, lr, iterations, loss_fn):
     """Adam on the tensors `params` over the batch sum of loss_fn()[0], the per-body loss; returns loss_fn() at the
     result, without a graph."""
@@ -194,27 +244,23 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
     'loss': (B,) final per-body loss}."""
     if method not in ('adam', 'lm'):
         raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
-    exact = exact_circumferences(circumference_derivative)
+    exact_circumferences(circumference_derivative)
     if iterations is None:
         iterations = 500 if method == 'adam' else 50
     device = body_model.shapedirs.device
     B = batch_size or max([torch.as_tensor(v).numel() for v in targets.values()] + [1])
     if betas_init is not None:
         B = betas_init.shape[0]
-    tgt, wt = _measurement_terms(targets, weights, B, device)
-    faces = body_model.faces_i32
+    mt = _measurement_term(targets, weights, B, device, body_measurements, circumference_derivative)
     if method == 'lm':
-        return _fit_lm(body_model, body_measurements, tgt.contiguous(), wt.contiguous(), betas_weight, iterations,
-                       betas_init, B, device, exact)
+        return _fit_lm(body_model, mt, betas_weight, iterations, betas_init, B, device)
     nb = body_model.shapedirs.shape[-1]
     betas = (torch.zeros(B, nb, device=device) if betas_init is None else betas_init.detach().clone().float())
     betas.requires_grad_(True)
 
     def loss_fn():
-        v = body_model.forward_shape(betas=betas)['v_shaped']
-        m = body_measurements.forward_vertices(v, faces, circumference_derivative)['measurements']
-        meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-        return _measurement_loss(tgt, wt, meas, betas, betas_weight), meas
+        meas = mt.measure(body_model, betas)
+        return mt.loss(meas, betas, betas_weight), meas
 
     per_body, meas = _adam([betas], lr, iterations, loss_fn)
     return {'betas': betas.detach(), 'measurements': meas, 'loss': per_body}
@@ -224,6 +270,28 @@ def fit_betas_to_measurements(body_model, body_measurements, targets, weights=No
 LM_UP, LM_DOWN = 10.0, 3.0
 # parameters of one body the keypoint LM step takes (kLmKpMaxP of fit.cu): 22 rotations, the betas and the translation
 LM_KP_MAX_PARAMS = 96
+
+
+def _check_kp_fit(fn, body_model, method, iterations, circumference_derivative='reference', body_measurements=None,
+                  measurements=None, robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0):
+    """The argument checks every keypoint fit makes, `fn` naming it in the messages.  Returns the iterations (None
+    means 600 for Adam and 50 for LM) and robust_sigma as the fits take it (None for least squares)."""
+    if method not in ('adam', 'lm'):
+        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    exact_circumferences(circumference_derivative)
+    if measurements is not None and body_measurements is None:
+        raise ValueError(f'{fn}: measurements need body_measurements')
+    if robust_sigma is not None and not robust_sigma > 0:
+        raise ValueError(f'{fn}: robust_sigma must be > 0 or None, got {robust_sigma}')
+    if not (pose_prior_weight >= 0 and betas_weight >= 0):
+        raise ValueError(f'{fn}: pose_prior_weight and betas_weight must be >= 0')
+    if method == 'lm' and 3 * 22 + body_model.num_betas + 3 > LM_KP_MAX_PARAMS:
+        raise ValueError(f"{fn}(method='lm'): 22 rotations, {body_model.num_betas} betas and the translation or camera "
+                         f'are {3 * 22 + body_model.num_betas + 3} parameters, at most {LM_KP_MAX_PARAMS} are '
+                         f'supported (at most {LM_KP_MAX_PARAMS - 3 * 22 - 3} betas)')
+    if iterations is None:
+        iterations = 600 if method == 'adam' else 50
+    return iterations, None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
 
 
 def measurement_jacobian(body_model, body_measurements, betas, circumference_derivative='reference'):
@@ -243,11 +311,9 @@ def measurement_jacobian(body_model, body_measurements, betas, circumference_der
     return {'measurements': out, 'jacobian': jac}
 
 
-def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, betas_init, B, device, exact):
+def _fit_lm(body_model, mt, betas_weight, iterations, betas_init, B, device):
     from . import ops
     packed = body_model.packed(device)
-    faces = body_model.faces_i32
-    lm = body_measurements.landmarks()
     nb = packed.NB
     trial = (torch.zeros(B, nb, device=device) if betas_init is None
              else betas_init.detach().to(device=device, dtype=torch.float32).clone().contiguous())
@@ -256,11 +322,10 @@ def _fit_lm(body_model, body_measurements, tgt, wt, betas_weight, iterations, be
              'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
     if B == 0:
         return {'betas': state['betas'], 'measurements': state['meas'], 'loss': state['loss']}
-    ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
+    mt.prime(body_model)
     for it in range(int(iterations) + 1):
-        v = ops.smplx_forward_shape(packed, trial)
-        meas, jac, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-        ops.fit_lm_step(state, tgt, wt, betas_weight, LM_UP, LM_DOWN, it == 0, trial, meas, jac)
+        meas, jac = mt.trial(packed, body_model, trial)
+        ops.fit_lm_step(state, mt.tgt, mt.wt, betas_weight, LM_UP, LM_DOWN, it == 0, trial, meas, jac)
     return {'betas': state['betas'], 'measurements': state['meas'], 'loss': state['loss']}
 
 
@@ -317,21 +382,12 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss},
     with measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss'
     the total: keypoints + measurements + betas_weight |betas|^2."""
-    if method not in ('adam', 'lm'):
-        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
-    exact_circumferences(circumference_derivative)
-    if measurements is not None and body_measurements is None:
-        raise ValueError('fit_body_to_keypoints: measurements need body_measurements')
+    iterations, _ = _check_kp_fit('fit_body_to_keypoints', body_model, method, iterations, circumference_derivative,
+                                  body_measurements, measurements)
     if measurements is None and betas_weight != 0:
         raise ValueError('fit_body_to_keypoints: betas_weight needs measurements (the keypoint fit has no betas prior)')
     if not betas_weight >= 0:
         raise ValueError(f'fit_body_to_keypoints: betas_weight must be >= 0, got {betas_weight}')
-    if method == 'lm' and 3 * 22 + body_model.num_betas + 3 > LM_KP_MAX_PARAMS:
-        raise ValueError(f"fit_body_to_keypoints(method='lm'): 22 rotations, {body_model.num_betas} betas and the "
-                         f'translation are {3 * 22 + body_model.num_betas + 3} parameters, at most {LM_KP_MAX_PARAMS} '
-                         f'are supported (at most {LM_KP_MAX_PARAMS - 3 * 22 - 3} betas)')
-    if iterations is None:
-        iterations = 600 if method == 'adam' else 50
     from .autograd import Rot6dFunction
     device = body_model.shapedirs.device
     kp = torch.as_tensor(keypoints, dtype=torch.float32, device=device)
@@ -339,13 +395,11 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
                                                                              device=device)
     w = w.expand(B, K).contiguous()
-    mterms = None
-    if measurements is not None:
-        tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
-        mterms = (tgt.contiguous(), wt.contiguous(), float(betas_weight), circumference_derivative)
+    mt = _measurement_term(measurements, measurement_weights, B, device, body_measurements, circumference_derivative)
+    rho = float(betas_weight)
     params = _start_params(init or {}, B, body_model.num_betas, device, method, 'transl')
     if method == 'lm':
-        return _fit_keypoints_lm(body_model, kp, w, params, int(iterations), body_measurements, mterms)
+        return _fit_keypoints_lm(body_model, kp, w, params, int(iterations), mt, rho)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -355,38 +409,48 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         joints = out['joints'][:]                  # the KeypointTensor's tensor, still in the graph
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
         meas = None
-        if mterms is not None:
-            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
-            m = body_measurements.forward_vertices(v, body_model.faces_i32, mterms[3])['measurements']
-            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], mterms[2])
+        if mt is not None:
+            meas = mt.measure(body_model, params['betas'])
+            per_body = per_body + mt.loss(meas, params['betas'], rho)
         return per_body, joints, grot, bpose, meas
 
     per_body, joints, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
+    return _adam_result(params, grot, bpose, meas, keypoints=joints, loss=per_body)
+
+
+def _adam_result(params, grot, bpose, meas, **outputs):
+    """What an Adam keypoint fit returns: the fitted raw parameters, the rotations, `outputs` and, with measurements
+    (meas not None), 'measurements'."""
     res = {k: v.detach() for k, v in params.items()}
-    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, loss=per_body)
+    res.update(global_rot_mat=grot, body_pose_mat=bpose, **outputs)
     if meas is not None:
         res['measurements'] = meas
     return res
 
 
-def _kp_lm_state(B, K, n_rot, nb, last, device):
-    """The state tensors of a keypoint LM step (ops.fit_lm_keypoints_step), `last` naming the last three parameters."""
+def _kp_lm_state(B, K, n_rot, nb, last, device, G=None):
+    """The state tensors of a keypoint LM step (ops.fit_lm_keypoints_step), `last` naming the last three parameters;
+    with G, the grouped steps' state: 'betas', 'loss', 'lambda' and 'accepted' per group."""
+    G = B if G is None else G
     mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-    return {'rot': mk(B, n_rot, 3, 3), 'betas': mk(B, nb), last: mk(B, 3), 'keypoints': mk(B, K, 3),
-            'jac': mk(B, 3 * K, 3 * n_rot + nb + 3), 'loss': mk(B), 'lambda': mk(B),
-            'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    return {'rot': mk(B, n_rot, 3, 3), 'betas': mk(G, nb), last: mk(B, 3), 'keypoints': mk(B, K, 3),
+            'jac': mk(B, 3 * K, 3 * n_rot + nb + 3), 'loss': mk(G), 'lambda': mk(G),
+            'accepted': torch.zeros(G, dtype=torch.int32, device=device)}
 
 
 def _kp_lm_result(state, last, **outputs):
-    """The fitted parameters of a keypoint LM state as the fits return them, the rotations also as raw 6D."""
+    """The fitted parameters of a keypoint LM state as the fits return them, the rotations also as raw 6D, then
+    `outputs` and, with measurements, 'measurements'."""
     rot = state['rot']
     raw = rot[..., :2].reshape(rot.shape[0], 6 * rot.shape[1])   # the first two columns, the decoder's row-major 3x2
-    return {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
-            last: state[last], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], **outputs}
+    res = {'global_rot': raw[:, :6].contiguous(), 'body_pose': raw[:, 6:].contiguous(), 'betas': state['betas'],
+           last: state[last], 'global_rot_mat': rot[:, :1], 'body_pose_mat': rot[:, 1:], **outputs}
+    if 'meas' in state:
+        res['measurements'] = state['meas']
+    return res
 
 
-def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=None, mterms=None):
+def _fit_keypoints_lm(body_model, kp, w, params, iterations, mt, rho):
     from . import ops
     device = kp.device
     packed = body_model.packed(device)
@@ -396,36 +460,28 @@ def _fit_keypoints_lm(body_model, kp, w, params, iterations, body_measurements=N
              'betas': params['betas'].contiguous(), 'transl': params['transl'].contiguous()}
     state = _kp_lm_state(B, K, n_rot, nb, 'transl', device)
     tg = kp.contiguous()
-    if mterms is not None:
-        state.update(meas=torch.empty(B, 5, dtype=torch.float32, device=device),
-                     meas_jac=torch.empty(B, 5, nb, dtype=torch.float32, device=device))
-    if B > 0 and mterms is None:
+    if mt is not None:
+        state.update(mt.state(nb, device))
+    if B > 0:
+        if mt is not None:
+            mt.prime(body_model)
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
-            ops.fit_lm_keypoints_step(state, trial, tg, w, LM_UP, LM_DOWN, it == 0, tkp, tjac)
-    elif B > 0:
-        tgt, wt, rho, cd = mterms
-        exact = exact_circumferences(cd)
-        faces, lm = body_model.faces_i32, body_measurements.landmarks()
-        ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
-        for it in range(iterations + 1):
-            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
-            v = ops.smplx_forward_shape(packed, trial['betas'])
-            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-            ops.fit_lm_keypoints_measurements_step(state, trial, tg, w, tgt, wt, rho, LM_UP, LM_DOWN, it == 0, tkp,
-                                                   tjac, tm, tmj)
+            if mt is None:
+                ops.fit_lm_keypoints_step(state, trial, tg, w, LM_UP, LM_DOWN, it == 0, tkp, tjac)
+            else:
+                tm, tmj = mt.trial(packed, body_model, trial['betas'])
+                ops.fit_lm_keypoints_measurements_step(state, trial, tg, w, mt.tgt, mt.wt, rho, LM_UP, LM_DOWN,
+                                                       it == 0, tkp, tjac, tm, tmj)
     rot = state['rot']
     with torch.no_grad():
         out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], transl=state['transl'],
                          return_shaped=False)
         joints = out['joints'][:]
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
-        if mterms is not None:
-            per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], mterms[2])
-    res = _kp_lm_result(state, 'transl', keypoints=joints, loss=per_body)
-    if mterms is not None:
-        res['measurements'] = state['meas']
-    return res
+        if mt is not None:
+            per_body = per_body + mt.loss(state['meas'], state['betas'], rho)
+    return _kp_lm_result(state, 'transl', keypoints=joints, loss=per_body)
 
 
 def keypoint_jacobian_2d(body_model, rot, betas, camera):
@@ -469,15 +525,53 @@ def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas):
     return per_body
 
 
+def _raw_init(init):
+    """A copy of init with the regressor's raw_global_rot / raw_body_pose, when given, as global_rot / body_pose."""
+    init = dict(init or {})
+    for k in ('global_rot', 'body_pose'):
+        if init.get('raw_' + k) is not None:
+            init[k] = init['raw_' + k]
+    return init
+
+
+def _keypoints_2d(fn, keypoints2d, weights, device):
+    """The 2D targets as a contiguous float32 (B, K, 2) tensor and their weights (None: all 1, (K,) or (B, K)) as
+    (B, K)."""
+    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device).contiguous()
+    if x.dim() != 3 or x.shape[2] != 2:
+        raise ValueError(f'{fn}: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    B, K = x.shape[0], x.shape[1]
+    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
+                                                                             device=device)
+    return x, w.expand(B, K).contiguous()
+
+
+def _start_rotations(params, pose_anchor, n):
+    """The decoded starting rotations (n, 22, 3, 3) of a fit's raw 6D params, and the pose prior's anchor:
+    pose_anchor as (n, 22, 3, 3), by default the start."""
+    from . import ops
+    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    if pose_anchor is None:
+        return rot0, rot0
+    return rot0, torch.as_tensor(pose_anchor, dtype=torch.float32, device=rot0.device).reshape(n, 22, 3, 3).contiguous()
+
+
+def _forward_2d(body_model, grot, bpose, betas, last, intr):
+    """SMPLX.forward of a 2D fit with its proj_joints: `last` the weak-perspective camera (intr None) or the
+    translation seen by the perspective camera with intrinsics intr (B, 3)."""
+    if intr is None:
+        return body_model(global_rot=grot, body_pose=bpose, betas=betas, camera=last, return_shaped=False)
+    out = body_model(global_rot=grot, body_pose=bpose, betas=betas, transl=last, return_shaped=False)
+    out['proj_joints'] = _project(out['joints'][:], intr)
+    return out
+
+
 def _init_2d(init, B, nb, device, method, x=None, w=None, intr=None):
     """The raw 6D global and body pose, betas and camera to start from: fit_body_to_keypoints' init with 'camera' in
     place of 'transl'; the regressor's stage output (raw_global_rot, raw_body_pose, betas, camera) works as-is.  With
     intrinsics intr (B, 3) the last three are 'transl', by default START_DEPTH in front of the camera on the ray
     through the centroid of the keypoints x with weight w > 0 (the principal point without one)."""
-    init = dict(init or {})
-    for k in ('global_rot', 'body_pose'):
-        if init.get('raw_' + k) is not None:
-            init[k] = init['raw_' + k]
+    init = _raw_init(init)
     if intr is None:
         return _start_params(init, B, nb, device, method, 'camera', 0.9)   # softplus(0.9) ~ 1.24, the mean scale
     if init.get('transl') is None:
@@ -638,93 +732,54 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     The measurement weights are the crop frame's; with targets in pixels a known height needs a larger weight to
     count (measurement_weights={'height': 1e6}: 1 mm of height costs what 1 px of one keypoint does).  groups and
     share_pose are not supported with a focal length."""
-    if method not in ('adam', 'lm'):
-        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
+    iterations, sigma = _check_kp_fit('fit_body_to_keypoints_2d', body_model, method, iterations,
+                                      circumference_derivative, body_measurements, measurements, robust_sigma,
+                                      pose_prior_weight, betas_weight)
     if share_pose and groups is None:
         raise ValueError('fit_body_to_keypoints_2d: share_pose needs groups')
     if focal_length is not None and (groups is not None or share_pose):
         raise ValueError('fit_body_to_keypoints_2d: groups and share_pose are not supported with a focal_length')
     if focal_length is not None and principal_point is None:
         raise ValueError('fit_body_to_keypoints_2d: focal_length needs principal_point')
-    exact_circumferences(circumference_derivative)
-    if measurements is not None and body_measurements is None:
-        raise ValueError('fit_body_to_keypoints_2d: measurements need body_measurements')
-    if robust_sigma is not None and not robust_sigma > 0:
-        raise ValueError(f'fit_body_to_keypoints_2d: robust_sigma must be > 0 or None, got {robust_sigma}')
-    if not (pose_prior_weight >= 0 and betas_weight >= 0):
-        raise ValueError('fit_body_to_keypoints_2d: pose_prior_weight and betas_weight must be >= 0')
-    nb = body_model.num_betas
-    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
-        raise ValueError(f"fit_body_to_keypoints_2d(method='lm'): 22 rotations, {nb} betas and the camera are "
-                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
-    if iterations is None:
-        iterations = 600 if method == 'adam' else 50
-    from . import ops
     from .autograd import Rot6dFunction
     device = body_model.shapedirs.device
-    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device).contiguous()
-    if x.dim() != 3 or x.shape[2] != 2:
-        raise ValueError(f'fit_body_to_keypoints_2d: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
-    B, K = x.shape[0], x.shape[1]
-    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
-                                                                             device=device)
-    w = w.expand(B, K).contiguous()
+    x, w = _keypoints_2d('fit_body_to_keypoints_2d', keypoints2d, weights, device)
+    B = x.shape[0]
     intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
-    params = _init_2d(init, B, nb, device, method, x, w, intr)
-    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    params = _init_2d(init, B, body_model.num_betas, device, method, x, w, intr)
+    rot0, anchor = _start_rotations(params, None if share_pose else pose_anchor, B)
     if share_pose:          # per group: its shape is checked once the groups are known
         anchor = None if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32, device=device)
-    else:
-        anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
-                                                                  device=device).reshape(B, 22, 3, 3).contiguous()
-    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
     pw, bw = float(pose_prior_weight), float(betas_weight)
     if groups is not None:
         return _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, int(iterations), sigma, pw, bw,
                                         lr, groups, body_measurements, measurements, measurement_weights,
                                         circumference_derivative, bool(share_pose))
-    mterms = None
-    if measurements is not None:
-        tgt, wt = _measurement_terms(measurements, measurement_weights, B, device)
-        mterms = (tgt.contiguous(), wt.contiguous(), circumference_derivative)
+    mt = _measurement_term(measurements, measurement_weights, B, device, body_measurements, circumference_derivative)
+    last = 'camera' if intr is None else 'transl'
     if method == 'lm':
-        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw,
-                                    body_measurements, mterms, intr)
+        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw, mt, intr)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
         bpose = Rot6dFunction.apply(params['body_pose'])
-        if intr is None:
-            out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], camera=params['camera'],
-                             return_shaped=False)
-        else:
-            out = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
-                             return_shaped=False)
-            out['proj_joints'] = _project(out['joints'][:], intr)
+        out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr)
         rot = torch.cat([grot, bpose], 1)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
         meas = None
-        if mterms is not None:
-            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
-            m = body_measurements.forward_vertices(v, body_model.faces_i32, mterms[2])['measurements']
-            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-            # _kp2d_loss already counted betas_weight |betas|^2
-            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], 0.0)
+        if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
+            meas = mt.measure(body_model, params['betas'])
+            per_body = per_body + mt.loss(meas, params['betas'], 0.0)
         return per_body, out, grot, bpose, meas
 
     per_body, out, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
     if intr is not None:
         per_body = _depth_rule(per_body, out['joints'][:], w)
-    res = {k: v.detach() for k, v in params.items()}
-    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
-               loss=per_body)
-    if meas is not None:
-        res['measurements'] = meas
-    return res
+    return _adam_result(params, grot, bpose, meas, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
+                        loss=per_body)
 
 
-def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw, body_measurements=None,
-                         mterms=None, intr=None):
+def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw, mt, intr):
     from . import ops
     device = x.device
     packed = body_model.packed(device)
@@ -740,42 +795,54 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
         mstep = lambda st, tr, x, w, *r, **kw: ops.fit_lm_keypoints_2d_perspective_measurements_step(  # noqa: E731
             st, tr, x, w, intr, *r, **kw)
     pose_anchor = anchor if pw > 0 else None
-    if mterms is not None:
-        state.update(meas=torch.empty(B, 5, dtype=torch.float32, device=device),
-                     meas_jac=torch.empty(B, 5, nb, dtype=torch.float32, device=device))
-    if B > 0 and mterms is None:
+    if mt is not None:
+        state.update(mt.state(nb, device))
+    if B > 0:
+        if mt is not None:
+            mt.prime(body_model)
         for it in range(iterations + 1):
             tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
-            step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, pose_anchor=pose_anchor)
-    elif B > 0:
-        tgt, wt, cd = mterms
-        exact = exact_circumferences(cd)
-        faces, lm = body_model.faces_i32, body_measurements.landmarks()
-        ops.face_incidence(faces)          # built (one copy to the host) before the loop, which never synchronises
-        for it in range(iterations + 1):
-            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
-            v = ops.smplx_forward_shape(packed, trial['betas'])
-            tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-            mstep(state, trial, x, w, sigma, pw, bw, tgt, wt, LM_UP, LM_DOWN, it == 0, tkp, tjac, tm, tmj,
-                  pose_anchor=pose_anchor)
+            if mt is None:
+                step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, pose_anchor=pose_anchor)
+            else:
+                tm, tmj = mt.trial(packed, body_model, trial['betas'])
+                mstep(state, trial, x, w, sigma, pw, bw, mt.tgt, mt.wt, LM_UP, LM_DOWN, it == 0, tkp, tjac, tm, tmj,
+                      pose_anchor=pose_anchor)
     rot = state['rot']
     with torch.no_grad():
-        if intr is None:
-            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], camera=state['camera'],
-                             return_shaped=False)
-        else:
-            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'],
-                             transl=state['transl'], return_shaped=False)
-            out['proj_joints'] = _project(out['joints'][:], intr)
+        out = _forward_2d(body_model, rot[:, :1], rot[:, 1:], state['betas'], state[last], intr)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
-        if mterms is not None:      # _kp2d_loss already counted betas_weight |betas|^2
-            per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], 0.0)
+        if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
+            per_body = per_body + mt.loss(state['meas'], state['betas'], 0.0)
         if intr is not None:
             per_body = _depth_rule(per_body, out['joints'][:], w)
-    res = _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
-    if mterms is not None:
-        res['measurements'] = state['meas']
-    return res
+    return _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+
+
+class _SortedBatch:
+    """A batch sorted by group once: labels (B,) with group_plan's rules, or None for one group of every row.  order
+    (B,), group_plan's stable sort, and inv its inverse; offsets (G + 1,) int32 on the CPU, group g the sorted rows
+    [offsets[g], offsets[g + 1]); gidx (B,) each sorted row's group, first (G,) each group's first sorted row and
+    counts (G,) its number of rows (float).  All but offsets on `device`."""
+
+    def __init__(self, labels, B, device):
+        if labels is None:
+            order, offsets = torch.arange(B), torch.tensor([0, B] if B else [0], dtype=torch.int32)
+        else:
+            order, offsets = group_plan(labels, B)
+        counts = (offsets[1:] - offsets[:-1]).long()
+        self.G, self.offsets = offsets.numel() - 1, offsets
+        self.order = _to_device(order, device)
+        self.inv = torch.argsort(self.order)
+        self.gidx = _to_device(torch.repeat_interleave(torch.arange(self.G), counts), device)
+        self.first = _to_device(offsets[:-1].long(), device)
+        self.counts = _to_device(counts.float(), device)
+
+    def mean(self, betas):
+        """Per group, the mean (G, NB) of the sorted rows' betas (B, NB), summed in row order: a group's start."""
+        if self.G == 0:
+            return betas.new_zeros(0, betas.shape[1])
+        return (_group_sum(betas, self.offsets) / self.counts[:, None]).contiguous()
 
 
 def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, iterations, sigma, pw, bw, lr, groups,
@@ -786,75 +853,57 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
     from .autograd import Rot6dFunction
     device = x.device
     B, K = x.shape[0], x.shape[1]
-    order, offsets = group_plan(groups, B)
-    G, nb = offsets.numel() - 1, params['betas'].shape[1]
-    counts = (offsets[1:] - offsets[:-1]).long()
-    od = _to_device(order, device)
-    inv = torch.argsort(od)
-    gidx = _to_device(torch.repeat_interleave(torch.arange(G), counts), device)     # each sorted image's group
-    x, w, rot0 = x[od].contiguous(), w[od].contiguous(), rot0[od].contiguous()
-    sp = {k: v.detach()[od].contiguous() for k, v in params.items()}
-    cnt = _to_device(counts.float(), device)
-    betas0 = (_group_sum(sp['betas'], offsets) / cnt[:, None]).contiguous() if G else torch.zeros(0, nb, device=device)
+    plan = _SortedBatch(groups, B, device)
+    G, offsets, gidx, nb = plan.G, plan.offsets, plan.gidx, params['betas'].shape[1]
+    x, w, rot0 = (t[plan.order].contiguous() for t in (x, w, rot0))
+    sp = {k: v.detach()[plan.order].contiguous() for k, v in params.items()}
+    betas0 = plan.mean(sp['betas'])
     if share_pose:
-        first = _to_device(offsets[:-1].long(), device)                              # each group's first image
-        raw0 = _shared_body_raw(rot0, offsets, cnt)
+        raw0 = _shared_body_raw(rot0, offsets, plan.counts)
         body0 = ops.decode_rot6d(raw0) if G else rot0.new_zeros(0, 21, 3, 3)
         rot0 = torch.cat([rot0[:, :1], body0[gidx]], 1).contiguous()
         if anchor is None:
-            anchor = torch.cat([rot0[first, :1], body0], 1).contiguous()
+            anchor = torch.cat([rot0[plan.first, :1], body0], 1).contiguous()
         elif anchor.numel() != G * 22 * 9:
             raise ValueError(f'fit_body_to_keypoints_2d: with share_pose, pose_anchor must be ({G}, 22, 3, 3)')
         else:
             anchor = anchor.reshape(G, 22, 3, 3).contiguous()
     else:
-        anchor = anchor[od].contiguous()
-    mterms = None
-    if measurements is not None:
-        tgt, wt = _measurement_terms(measurements, measurement_weights, G, device)
-        mterms = (tgt.contiguous(), wt.contiguous())
-    packed = body_model.packed(device)
-    faces = body_model.faces_i32
+        anchor = anchor[plan.order].contiguous()
+    mt = _measurement_term(measurements, measurement_weights, G, device, body_measurements, cd)
     if method == 'lm':
+        packed = body_model.packed(device)
         trial = {'rot': rot0.clone(), 'betas': betas0, 'image_betas': betas0[gidx].contiguous(),
                  'camera': sp['camera']}
-        state = _kp_lm_state(B, K, 22, nb, 'camera', device)
-        mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-        state.update({'betas': mk(G, nb), 'loss': mk(G), 'lambda': mk(G),     # per group
-                      'accepted': torch.zeros(G, dtype=torch.int32, device=device)})
-        if mterms is not None:
-            state.update(meas=mk(G, 5), meas_jac=mk(G, 5, nb))
+        state = _kp_lm_state(B, K, 22, nb, 'camera', device, G)
+        if mt is not None:
+            state.update(mt.state(nb, device))
         pose_anchor = anchor if pw > 0 else None
         if B > 0:
             ws = (ops.fit_lm_shared_pose_workspace if share_pose else ops.fit_lm_groups_workspace)(B, G, 22, nb, device)
             step = ops.fit_lm_keypoints_2d_shared_pose_step if share_pose else ops.fit_lm_keypoints_2d_groups_step
             mstep = (ops.fit_lm_keypoints_2d_shared_pose_measurements_step if share_pose else
                      ops.fit_lm_keypoints_2d_groups_measurements_step)
-            exact = exact_circumferences(cd)
-            lm = body_measurements.landmarks() if mterms is not None else None
-            if mterms is not None:
-                ops.face_incidence(faces)      # built (one copy to the host) before the loop, which never synchronises
+            if mt is not None:
+                mt.prime(body_model)
             for it in range(iterations + 1):
                 tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['image_betas'], trial['rot'])
-                if mterms is None:
+                if mt is None:
                     step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, offsets, ws,
                          pose_anchor=pose_anchor)
                 else:
-                    v = ops.smplx_forward_shape(packed, trial['betas'])
-                    tm, tmj, _ = ops.measure_jacobian_betas(packed, lm, v, faces, exact=exact)
-                    mstep(state, trial, x, w, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0, tkp, tjac,
-                          tm, tmj, offsets, ws, pose_anchor=pose_anchor)
+                    tm, tmj = mt.trial(packed, body_model, trial['betas'])
+                    mstep(state, trial, x, w, sigma, pw, bw, mt.tgt, mt.wt, LM_UP, LM_DOWN, it == 0, tkp, tjac, tm,
+                          tmj, offsets, ws, pose_anchor=pose_anchor)
         rot = state['rot']
         with torch.no_grad():
             out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'][gidx],
                              camera=state['camera'], return_shaped=False)
         res = _kp_lm_result(state, 'camera', keypoints=out['joints'][:], proj_joints=out['proj_joints'],
                             loss=state['loss'])
-        if mterms is not None:
-            res['measurements'] = state['meas']
         if share_pose:
             for k in ('body_pose', 'body_pose_mat'):
-                res[k] = res[k][first]
+                res[k] = res[k][plan.first]
     else:
         p = {k: sp[k].clone().requires_grad_(True) for k in ('global_rot', 'body_pose', 'camera')}
         if share_pose:
@@ -877,24 +926,19 @@ def _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, ite
                 per_group = _group_sum(_kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, 0.0, None),
                                        offsets)
             meas = None
-            if mterms is not None:
-                v = body_model.forward_shape(betas=p['betas'])['v_shaped']
-                m = body_measurements.forward_vertices(v, faces, cd)['measurements']
-                meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-                per_group = per_group + _measurement_loss(mterms[0], mterms[1], meas, p['betas'], 0.0)
+            if mt is not None:
+                meas = mt.measure(body_model, p['betas'])
+                per_group = per_group + mt.loss(meas, p['betas'], 0.0)
             if bw > 0:
                 per_group = per_group + bw * p['betas'].pow(2).sum(1)
             return per_group, out, grot, bpose, meas
 
         per_group, out, grot, bpose, meas = _adam(list(p.values()), lr, iterations, loss_fn)
-        res = {k: v.detach() for k, v in p.items()}
-        res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=out['joints'][:],
-                   proj_joints=out['proj_joints'], loss=per_group)
-        if meas is not None:
-            res['measurements'] = meas
+        res = _adam_result(p, grot, bpose, meas, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
+                           loss=per_group)
     per_image = ('global_rot', 'camera', 'global_rot_mat', 'keypoints', 'proj_joints')
     for k in per_image if share_pose else per_image + ('body_pose', 'body_pose_mat'):
-        res[k] = res[k][inv]
+        res[k] = res[k][plan.inv]
     return res
 
 
@@ -958,13 +1002,6 @@ def _ray_start(x, w, intr, cam_rot, cam_transl, offsets):
     return torch.linalg.solve_ex(A, rhs)[0].float()
 
 
-def _view_offsets(groups, B):
-    """(order, offsets) of the views of a calibrated fit: group_plan's, or one body seeing every view."""
-    if groups is not None:
-        return group_plan(groups, B)
-    return torch.arange(B), torch.tensor([0, B] if B else [0], dtype=torch.int32)
-
-
 def _calibrated_loss(joints, x, w, intr, cam_rot, cam_transl, gidx, offsets, sigma, pw, bpose, anchor, bw, betas):
     """The calibrated fit's loss per body, through PerspectiveCamera(rotation=, translation=): joints (G, K, 3) in the
     world frame, the views (B, ...) sorted by body, gidx (B,) each view's body.  The keypoint terms per view summed in
@@ -1014,70 +1051,41 @@ def fit_body_to_calibrated_views(body_model, keypoints2d, focal_length, principa
     'body_pose_mat' (G, 21, 3, 3), 'keypoints' (G, K, 3) in the world frame, 'loss' (G,) recomputed through
     PerspectiveCamera}, with measurements 'measurements' (G, 5), and per view in the caller's order 'proj_joints'
     (B, K, 2)."""
-    if method not in ('adam', 'lm'):
-        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
-    exact_circumferences(circumference_derivative)
-    if measurements is not None and body_measurements is None:
-        raise ValueError('fit_body_to_calibrated_views: measurements need body_measurements')
-    if robust_sigma is not None and not robust_sigma > 0:
-        raise ValueError(f'fit_body_to_calibrated_views: robust_sigma must be > 0 or None, got {robust_sigma}')
-    if not (pose_prior_weight >= 0 and betas_weight >= 0):
-        raise ValueError('fit_body_to_calibrated_views: pose_prior_weight and betas_weight must be >= 0')
-    nb = body_model.num_betas
-    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
-        raise ValueError(f"fit_body_to_calibrated_views(method='lm'): 22 rotations, {nb} betas and the translation are "
-                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
-    if iterations is None:
-        iterations = 600 if method == 'adam' else 50
+    iterations, sigma = _check_kp_fit('fit_body_to_calibrated_views', body_model, method, iterations,
+                                      circumference_derivative, body_measurements, measurements, robust_sigma,
+                                      pose_prior_weight, betas_weight)
     from . import ops
     from .autograd import Rot6dFunction
     device = body_model.shapedirs.device
-    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device)
-    if x.dim() != 3 or x.shape[2] != 2:
-        raise ValueError(f'fit_body_to_calibrated_views: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    x, w = _keypoints_2d('fit_body_to_calibrated_views', keypoints2d, weights, device)
     B, K = x.shape[0], x.shape[1]
-    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
-                                                                             device=device)
-    w = w.expand(B, K)
+    nb = body_model.num_betas
     intr = _intrinsics(focal_length, principal_point, B, device)
     R = torch.as_tensor(cam_rot, dtype=torch.float32, device=device)
     T = torch.as_tensor(cam_transl, dtype=torch.float32, device=device)
     if R.shape != (B, 3, 3) or T.shape != (B, 3):
         raise ValueError(f'fit_body_to_calibrated_views: cam_rot must be ({B}, 3, 3) and cam_transl ({B}, 3), got '
                          f'{tuple(R.shape)} and {tuple(T.shape)}')
-    order, offsets = _view_offsets(groups, B)
-    G = offsets.numel() - 1
-    od = _to_device(order, device)
-    inv = torch.argsort(od)
-    gidx = _to_device(torch.repeat_interleave(torch.arange(G), (offsets[1:] - offsets[:-1]).long()), device)
-    x, w, intr, R, T = (t[od].contiguous() for t in (x, w, intr, R, T))
-    first = _to_device(offsets[:-1].long(), device)
-    init = dict(init or {})
-    for k in ('global_rot', 'body_pose'):
-        if init.get('raw_' + k) is not None:
-            init[k] = init['raw_' + k]
+    plan = _SortedBatch(groups, B, device)
+    G, offsets, gidx = plan.G, plan.offsets, plan.gidx
+    x, w, intr, R, T = (t[plan.order].contiguous() for t in (x, w, intr, R, T))
+    init = _raw_init(init)
     if init.get('global_rot') is None:
         mean = torch.ones(3, device=device)          # MEAN_GLOBAL_ROT, filled on the device: no host-to-device copy
         mean[1:].fill_(-1.0)
-        init['global_rot'] = (R[first].transpose(1, 2) * mean)[..., :2].reshape(G, 6)
+        init['global_rot'] = (R[plan.first].transpose(1, 2) * mean)[..., :2].reshape(G, 6)
     if init.get('transl') is None:
         init['transl'] = _ray_start(x, w, intr, R, T, offsets) if G else torch.zeros(0, 3, device=device)
     params = _start_params(init, G, nb, device, method, 'transl')
-    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
-    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
-                                                              device=device).reshape(G, 22, 3, 3).contiguous()
-    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
+    rot0, anchor = _start_rotations(params, pose_anchor, G)
     pw, bw = float(pose_prior_weight), float(betas_weight)
-    mterms = None
-    if measurements is not None:
-        tgt, wt = _measurement_terms(measurements, measurement_weights, G, device)
-        mterms = (tgt.contiguous(), wt.contiguous())
+    mt = _measurement_term(measurements, measurement_weights, G, device, body_measurements, circumference_derivative)
     def loss(joints, bpose, betas):
         return _calibrated_loss(joints, x, w, intr, R, T, gidx, offsets, sigma, pw, bpose, anchor, bw, betas)
     if method == 'lm':
         state = _kp_lm_state(G, K, 22, nb, 'transl', device)
-        if mterms is not None:
-            state.update(meas=torch.empty(G, 5, device=device), meas_jac=torch.empty(G, 5, nb, device=device))
+        if mt is not None:
+            state.update(mt.state(nb, device))
         if G > 0:
             trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(),
                      'transl': params['transl'].contiguous()}
@@ -1085,35 +1093,29 @@ def fit_body_to_calibrated_views(body_model, keypoints2d, focal_length, principa
             ws = ops.fit_lm_calibrated_workspace(B, G, device)
             packed = body_model.packed(device)
             pose_anchor = anchor if pw > 0 else None
-            if mterms is not None:
-                exact = exact_circumferences(circumference_derivative)
-                faces, lmk = body_model.faces_i32, body_measurements.landmarks()
-                ops.face_incidence(faces)      # built (one copy to the host) before the loop, which never synchronises
+            if mt is not None:
+                mt.prime(body_model)
             for it in range(int(iterations) + 1):
                 tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
-                if mterms is None:
+                if mt is None:
                     ops.fit_lm_keypoints_2d_calibrated_step(state, trial, x, w, intr, ext, sigma, pw, bw, LM_UP,
                                                             LM_DOWN, it == 0, tkp, tjac, offsets, ws,
                                                             pose_anchor=pose_anchor)
                 else:
-                    v = ops.smplx_forward_shape(packed, trial['betas'])
-                    tm, tmj, _ = ops.measure_jacobian_betas(packed, lmk, v, faces, exact=exact)
+                    tm, tmj = mt.trial(packed, body_model, trial['betas'])
                     ops.fit_lm_keypoints_2d_calibrated_measurements_step(
-                        state, trial, x, w, intr, ext, sigma, pw, bw, mterms[0], mterms[1], LM_UP, LM_DOWN, it == 0,
-                        tkp, tjac, tm, tmj, offsets, ws, pose_anchor=pose_anchor)
+                        state, trial, x, w, intr, ext, sigma, pw, bw, mt.tgt, mt.wt, LM_UP, LM_DOWN, it == 0, tkp,
+                        tjac, tm, tmj, offsets, ws, pose_anchor=pose_anchor)
         rot = state['rot']
         with torch.no_grad():
             out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'], transl=state['transl'],
                              return_shaped=False)
             joints = out['joints'][:]
             per_body, proj, behind = loss(joints, rot[:, 1:], state['betas'])
-            if mterms is not None:
-                per_body = per_body + _measurement_loss(mterms[0], mterms[1], state['meas'], state['betas'], 0.0)
+            if mt is not None:
+                per_body = per_body + mt.loss(state['meas'], state['betas'], 0.0)
             per_body = torch.where(behind, torch.full_like(per_body, float('inf')), per_body)
-        res = _kp_lm_result(state, 'transl', keypoints=joints, proj_joints=proj[inv], loss=per_body)
-        if mterms is not None:
-            res['measurements'] = state['meas']
-        return res
+        return _kp_lm_result(state, 'transl', keypoints=joints, proj_joints=proj[plan.inv], loss=per_body)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -1123,20 +1125,14 @@ def fit_body_to_calibrated_views(body_model, keypoints2d, focal_length, principa
         joints = out['joints'][:]
         per_body, proj, behind = loss(joints, bpose, params['betas'])
         meas = None
-        if mterms is not None:
-            v = body_model.forward_shape(betas=params['betas'])['v_shaped']
-            m = body_measurements.forward_vertices(v, body_model.faces_i32, circumference_derivative)['measurements']
-            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
-            per_body = per_body + _measurement_loss(mterms[0], mterms[1], meas, params['betas'], 0.0)
+        if mt is not None:
+            meas = mt.measure(body_model, params['betas'])
+            per_body = per_body + mt.loss(meas, params['betas'], 0.0)
         return per_body, joints, proj, grot, bpose, meas, behind
 
     per_body, joints, proj, grot, bpose, meas, behind = _adam(list(params.values()), lr, iterations, loss_fn)
     per_body = torch.where(behind, torch.full_like(per_body, float('inf')), per_body)
-    res = {k: v.detach() for k, v in params.items()}
-    res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, proj_joints=proj[inv], loss=per_body)
-    if meas is not None:
-        res['measurements'] = meas
-    return res
+    return _adam_result(params, grot, bpose, meas, keypoints=joints, proj_joints=proj[plan.inv], loss=per_body)
 
 
 def _smoothness(rot, transl, gidx, srw, stw):
@@ -1177,53 +1173,29 @@ def fit_body_to_sequence(body_model, keypoints2d, focal_length, principal_point,
     Returns per sequence 'betas' (S, NB) and 'loss' (S,) (with 'lm' the step's fp64 loss of the final state), and per
     frame in the caller's order 'global_rot', 'body_pose' (raw 6D), 'transl', 'global_rot_mat', 'body_pose_mat',
     'keypoints' (B, K, 3) in the camera frame and 'proj_joints' (B, K, 2)."""
-    if method not in ('adam', 'lm'):
-        raise ValueError(f"method must be 'adam' or 'lm', got {method!r}")
-    if robust_sigma is not None and not robust_sigma > 0:
-        raise ValueError(f'fit_body_to_sequence: robust_sigma must be > 0 or None, got {robust_sigma}')
-    if not (pose_prior_weight >= 0 and betas_weight >= 0):
-        raise ValueError('fit_body_to_sequence: pose_prior_weight and betas_weight must be >= 0')
+    iterations, sigma = _check_kp_fit('fit_body_to_sequence', body_model, method, iterations,
+                                      robust_sigma=robust_sigma, pose_prior_weight=pose_prior_weight,
+                                      betas_weight=betas_weight)
     srw, stw = float(smooth_rot_weight), float(smooth_transl_weight)
     if not (0 <= srw < float('inf') and 0 <= stw < float('inf')):
         raise ValueError('fit_body_to_sequence: the smoothness weights must be finite and >= 0')
-    nb = body_model.num_betas
-    if method == 'lm' and 3 * 22 + nb + 3 > LM_KP_MAX_PARAMS:
-        raise ValueError(f"fit_body_to_sequence(method='lm'): 22 rotations, {nb} betas and the translation are "
-                         f'{3 * 22 + nb + 3} parameters, at most {LM_KP_MAX_PARAMS} are supported')
-    if iterations is None:
-        iterations = 600 if method == 'adam' else 50
     from . import ops
     from .autograd import Rot6dFunction
     device = body_model.shapedirs.device
-    x = torch.as_tensor(keypoints2d, dtype=torch.float32, device=device).contiguous()
-    if x.dim() != 3 or x.shape[2] != 2:
-        raise ValueError(f'fit_body_to_sequence: keypoints2d must be (B, K, 2), got {tuple(x.shape)}')
+    x, w = _keypoints_2d('fit_body_to_sequence', keypoints2d, weights, device)
     B, K = x.shape[0], x.shape[1]
-    w = torch.ones(K, device=device) if weights is None else torch.as_tensor(weights, dtype=torch.float32,
-                                                                             device=device)
-    w = w.expand(B, K).contiguous()
+    nb = body_model.num_betas
     intr = _intrinsics(focal_length, principal_point, B, device)
     params = _init_2d(init, B, nb, device, method, x, w, intr)
-    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
-    anchor = rot0 if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32,
-                                                              device=device).reshape(B, 22, 3, 3).contiguous()
-    sigma = None if robust_sigma is None or robust_sigma == float('inf') else float(robust_sigma)
+    rot0, anchor = _start_rotations(params, pose_anchor, B)
     pw, bw = float(pose_prior_weight), float(betas_weight)
-    order, offsets = _view_offsets(sequences, B)
-    S = offsets.numel() - 1
-    counts = (offsets[1:] - offsets[:-1]).long()
-    od = _to_device(order, device)
-    inv = torch.argsort(od)
-    gidx = _to_device(torch.repeat_interleave(torch.arange(S), counts), device)     # each sorted frame's sequence
-    x, w, intr, rot0, anchor = (t[od].contiguous() for t in (x, w, intr, rot0, anchor))
-    sp = {k: v.detach()[od].contiguous() for k, v in params.items()}
-    cnt = _to_device(counts.float(), device)
-    betas0 = (_group_sum(sp['betas'], offsets) / cnt[:, None]).contiguous() if S else torch.zeros(0, nb, device=device)
+    plan = _SortedBatch(sequences, B, device)
+    S, offsets, gidx = plan.G, plan.offsets, plan.gidx
+    x, w, intr, rot0, anchor = (t[plan.order].contiguous() for t in (x, w, intr, rot0, anchor))
+    sp = {k: v.detach()[plan.order].contiguous() for k, v in params.items()}
+    betas0 = plan.mean(sp['betas'])
     if method == 'lm':
-        state = _kp_lm_state(B, K, 22, nb, 'transl', device)
-        mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-        state.update({'betas': mk(S, nb), 'loss': mk(S), 'lambda': mk(S),     # per sequence
-                      'accepted': torch.zeros(S, dtype=torch.int32, device=device)})
+        state = _kp_lm_state(B, K, 22, nb, 'transl', device, S)
         if B > 0:
             trial = {'rot': rot0.clone(), 'betas': betas0, 'image_betas': betas0[gidx].contiguous(),
                      'transl': sp['transl']}
@@ -1237,13 +1209,10 @@ def fit_body_to_sequence(body_model, keypoints2d, focal_length, principal_point,
                                                       pose_anchor=pose_anchor)
         rot = state['rot']
         with torch.no_grad():
-            out = body_model(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=state['betas'][gidx],
-                             transl=state['transl'], return_shaped=False)
-            joints = out['joints'][:]
-            proj = _project(joints, intr)
+            out = _forward_2d(body_model, rot[:, :1], rot[:, 1:], state['betas'][gidx], state['transl'], intr)
         # a start that breaks the depth rule leaves the kernel's loss NaN: its loss is +inf
         loss = torch.where(torch.isnan(state['loss']), torch.full_like(state['loss'], float('inf')), state['loss'])
-        res = _kp_lm_result(state, 'transl', keypoints=joints, proj_joints=proj, loss=loss)
+        res = _kp_lm_result(state, 'transl', keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=loss)
     else:
         p = {k: sp[k].clone().requires_grad_(True) for k in ('global_rot', 'body_pose', 'transl')}
         p['betas'] = betas0.clone().requires_grad_(True)
@@ -1251,25 +1220,22 @@ def fit_body_to_sequence(body_model, keypoints2d, focal_length, principal_point,
         def loss_fn():
             grot = Rot6dFunction.apply(p['global_rot'])
             bpose = Rot6dFunction.apply(p['body_pose'])
-            out = body_model(global_rot=grot, body_pose=bpose, betas=p['betas'][gidx], transl=p['transl'],
-                             return_shaped=False)
-            joints = out['joints'][:]
-            proj = _project(joints, intr)
+            out = _forward_2d(body_model, grot, bpose, p['betas'][gidx], p['transl'], intr)
             rot = torch.cat([grot, bpose], 1)
-            per_frame = _kp2d_loss(proj, x, w, sigma, pw, rot, anchor, 0.0, None) + \
+            per_frame = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, 0.0, None) + \
                 _smoothness(rot, p['transl'], gidx, srw, stw)
             per_seq = _group_sum(per_frame, offsets)
             if bw > 0:
                 per_seq = per_seq + bw * p['betas'].pow(2).sum(1)
-            return per_seq, joints, proj, grot, bpose
+            return per_seq, out, grot, bpose
 
-        per_seq, joints, proj, grot, bpose = _adam(list(p.values()), lr, iterations, loss_fn)
+        per_seq, out, grot, bpose = _adam(list(p.values()), lr, iterations, loss_fn)
+        joints = out['joints'][:]
         behind = _group_sum(_depth_rule(torch.zeros_like(x[:, 0, 0]), joints, w).isinf().float(), offsets) > 0
-        res = {k: v.detach() for k, v in p.items()}
-        res.update(global_rot_mat=grot, body_pose_mat=bpose, keypoints=joints, proj_joints=proj,
-                   loss=torch.where(behind, torch.full_like(per_seq, float('inf')), per_seq))
+        res = _adam_result(p, grot, bpose, None, keypoints=joints, proj_joints=out['proj_joints'],
+                           loss=torch.where(behind, torch.full_like(per_seq, float('inf')), per_seq))
     for k in ('global_rot', 'body_pose', 'transl', 'global_rot_mat', 'body_pose_mat', 'keypoints', 'proj_joints'):
-        res[k] = res[k][inv]
+        res[k] = res[k][plan.inv]
     return res
 
 
@@ -1394,10 +1360,7 @@ def _main_keypoints_2d(a, model, bm, targets):
     if a.calibrated and not (persp and 'cam_rot' in d.files and 'cam_transl' in d.files):
         raise SystemExit('--calibrated needs focal_length, cam_rot and cam_transl in --keypoints-2d')
     if a.init and not a.calibrated:
-        p = np.load(a.init)
-        init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(x.shape[0], -1)
-                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'camera', 'transl')
-                if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+        init = _load_init(a.init, x.shape[0], ('camera', 'transl'))
         if persp and 'transl' not in init and 'camera' in init:
             if not ('center' in d.files and 'scale' in d.files):
                 raise SystemExit('--init with a camera and a focal_length needs center and scale in --keypoints-2d')
@@ -1412,35 +1375,38 @@ def _main_keypoints_2d(a, model, bm, targets):
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
                                    circumference_derivative=a.circumference_derivative, groups=groups,
                                    share_pose=a.share_pose, focal_length=focal, principal_point=pp)
+    _save_result(a.output, res, {'bodies': int(x.shape[0])}, groups=groups)
+
+
+def _load_init(path, n, last):
+    """An --init npz as a fit's init of n rows: its raw 6D pose (raw_ entries first), betas and the `last` entries."""
+    p = np.load(path)
+    return {k: torch.as_tensor(p[k].astype(np.float32)).reshape(n, -1)
+            for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas') + last
+            if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+
+
+def _save_result(path, res, counts, **labels):
+    """Saves a keypoint fit's result and the labels that are not None to the npz `path`, and prints its summary:
+    `counts`, the path and the median loss, as one JSON line."""
     out = {k: v.detach().cpu().numpy() for k, v in res.items()}
-    if groups is not None:
-        out['groups'] = groups
-    np.savez(a.output, **out)
-    print(json.dumps({'bodies': int(x.shape[0]), 'output': a.output, 'median_loss': float(np.median(out['loss']))}))
+    out.update({k: v for k, v in labels.items() if v is not None})
+    np.savez(path, **out)
+    print(json.dumps({**counts, 'output': path, 'median_loss': float(np.median(out['loss']))}))
 
 
 def _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups):
     """--keypoints-2d --calibrated: the per-body result (G rows) and each view's proj_joints (B rows, the npz's order).
     An --init npz is per body, with transl in the world frame."""
     G = int(groups.max()) + 1 if groups is not None and groups.size else 1
-    init = None
-    if a.init:
-        p = np.load(a.init)
-        init = {k: torch.as_tensor(p[k].astype(np.float32)).reshape(G, -1)
-                for k in ('raw_global_rot', 'raw_body_pose', 'global_rot', 'body_pose', 'betas', 'transl')
-                if k in p.files and not (k in ('global_rot', 'body_pose') and 'raw_' + k in p.files)}
+    init = _load_init(a.init, G, ('transl',)) if a.init else None
     res = fit_body_to_calibrated_views(model, x, focal, pp, d['cam_rot'].astype(np.float32),
                                        d['cam_transl'].astype(np.float32), groups=groups, weights=w, init=init,
                                        method=a.method, iterations=a.iterations, robust_sigma=a.robust_sigma,
                                        pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight, lr=a.lr,
                                        body_measurements=bm, measurements=targets,
                                        circumference_derivative=a.circumference_derivative)
-    out = {k: v.detach().cpu().numpy() for k, v in res.items()}
-    if groups is not None:
-        out['groups'] = groups
-    np.savez(a.output, **out)
-    print(json.dumps({'bodies': int(out['loss'].shape[0]), 'views': int(x.shape[0]), 'output': a.output,
-                      'median_loss': float(np.median(out['loss']))}))
+    _save_result(a.output, res, {'bodies': int(res['loss'].shape[0]), 'views': int(x.shape[0])}, groups=groups)
 
 
 def _main_sequence(a, model, d, x, w, focal, pp, init):
@@ -1452,12 +1418,7 @@ def _main_sequence(a, model, d, x, w, focal, pp, init):
                                iterations=a.iterations, robust_sigma=a.robust_sigma,
                                pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight,
                                smooth_rot_weight=a.smooth_rot, smooth_transl_weight=a.smooth_transl, lr=a.lr)
-    out = {k: v.detach().cpu().numpy() for k, v in res.items()}
-    if seq is not None:
-        out['sequences'] = seq
-    np.savez(a.output, **out)
-    print(json.dumps({'frames': int(x.shape[0]), 'sequences': int(out['loss'].shape[0]), 'output': a.output,
-                      'median_loss': float(np.median(out['loss']))}))
+    _save_result(a.output, res, {'frames': int(x.shape[0]), 'sequences': int(res['loss'].shape[0])}, sequences=seq)
 
 
 if __name__ == '__main__':

@@ -400,6 +400,40 @@ def _meas_step_shapes_ok(state, trial_meas, trial_meas_jac, meas_targets, meas_w
             all(t.shape == (B, 5) for t in (meas_targets, meas_weights, trial_meas, state['meas'])))
 
 
+def _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down, pose_anchor):
+    """The scalar checks of every 2D keypoint step; returns robust_sigma as the step takes it (inf for None)."""
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    return sigma
+
+
+def _check_offsets(what, name, off, B, G=None):
+    """The offsets `name` of a grouped step: a contiguous int32 CPU tensor rising strictly from 0 to B (no empty group),
+    with G + 1 entries when G is given.  Returns the number of groups."""
+    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
+            off.is_contiguous()):
+        raise RuntimeError(f'{what}: {name} must be a contiguous (G + 1,) int32 CPU tensor')
+    n = off.numel() - 1
+    if n < 0 or G not in (None, n) or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
+        entries = '' if G is None else f' in {G + 1} entries'
+        raise ValueError(f'{what}: {name} must rise strictly from 0 to {B}{entries}')
+    return n
+
+
+def _workspace(n, device):
+    """The scratch of a grouped step, n bytes from its *_workspace_bytes entry: a uint8 CUDA tensor, allocated once
+    before an LM loop."""
+    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+
+
+def _check_workspace(what, workspace, need):
+    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
+        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+
+
 def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, first, trial, trial_meas, trial_jac):
     """One Levenberg-Marquardt step per body (include/shapy_b200.h, shapy_fit_lm_step), in place.  state: {'betas'
     (B, NB), 'meas' (B, 5), 'jac' (B, 5, NB), 'loss' (B,), 'lambda' (B,), 'accepted' (B,) int32}, CUDA tensors;
@@ -505,11 +539,8 @@ def _fit_lm_kp2d(what, state, trial, targets, weights, robust_sigma, pose_prior_
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
     last = 'camera' if intrinsics is None else 'transl'
-    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
-    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
-        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
-    if pose_prior_weight > 0 and pose_anchor is None:
-        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
+    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
+                                pose_anchor)
     anchor = [] if pose_anchor is None else [pose_anchor]
     intr = [] if intrinsics is None else [intrinsics]
     mstate = [] if meas is None else [state['meas'], state['meas_jac']]
@@ -809,8 +840,7 @@ def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=
 def fit_lm_groups_workspace(B, G, n_rot, nb, device):
     """The scratch of the grouped 2D step (include/shapy_b200.h, shapy_fit_lm_groups_workspace_bytes): a uint8 CUDA
     tensor, allocated once before an LM loop."""
-    n = lib().shapy_fit_lm_groups_workspace_bytes(int(B), int(G), int(n_rot), int(nb))
-    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+    return _workspace(lib().shapy_fit_lm_groups_workspace_bytes(int(B), int(G), int(n_rot), int(nb)), device)
 
 
 def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
@@ -820,18 +850,9 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
     trial_meas, trial_meas_jac), all (G, ...); share_pose: the shared-pose steps, with a per-group pose_anchor."""
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
-    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
-    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
-        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
-    if pose_prior_weight > 0 and pose_anchor is None:
-        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
-    off = group_offsets
-    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
-            off.is_contiguous()):
-        raise RuntimeError(f'{what}: group_offsets must be a contiguous (G + 1,) int32 CPU tensor')
-    G = off.numel() - 1
-    if G < 0 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
-        raise ValueError(f'{what}: group_offsets must rise strictly from 0 to the batch ({B})')
+    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
+                                pose_anchor)
+    G = _check_offsets(what, 'group_offsets', group_offsets, B)
     anchor = [] if pose_anchor is None else [pose_anchor]
     mstate = [] if meas is None else [state['meas'], state['meas_jac']]
     ts = [state[k] for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
@@ -852,13 +873,11 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
         raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
                            f'({G}, 5)')
     L = lib()
-    need = (L.shapy_fit_lm_shared_pose_workspace_bytes if share_pose else L.shapy_fit_lm_groups_workspace_bytes)(
-        B, G, n_rot, nb)
-    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
-        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    _check_workspace(what, workspace, (L.shapy_fit_lm_shared_pose_workspace_bytes if share_pose else
+                                       L.shapy_fit_lm_groups_workspace_bytes)(B, G, n_rot, nb))
     if B == 0:
         return
-    head = [B, G, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma,
+    head = [B, G, group_offsets.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(pose_anchor), sigma,
             float(pose_prior_weight), float(betas_weight)]
     lam = [float(lambda_up), float(lambda_down), int(bool(first))]
     tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['image_betas']), ptr(trial['camera']),
@@ -911,8 +930,7 @@ def fit_lm_keypoints_2d_groups_measurements_step(state, trial, targets, weights,
 def fit_lm_shared_pose_workspace(B, G, n_rot, nb, device):
     """The scratch of the shared-pose 2D step (include/shapy_b200.h, shapy_fit_lm_shared_pose_workspace_bytes): a uint8
     CUDA tensor, allocated once before an LM loop."""
-    n = lib().shapy_fit_lm_shared_pose_workspace_bytes(int(B), int(G), int(n_rot), int(nb))
-    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+    return _workspace(lib().shapy_fit_lm_shared_pose_workspace_bytes(int(B), int(G), int(n_rot), int(nb)), device)
 
 
 def fit_lm_keypoints_2d_shared_pose_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight,
@@ -945,8 +963,7 @@ def fit_lm_keypoints_2d_shared_pose_measurements_step(state, trial, targets, wei
 def fit_lm_sequence_workspace(B, S, n_rot, nb, device):
     """The scratch of the sequence 2D step (include/shapy_b200.h, shapy_fit_lm_sequence_workspace_bytes): a uint8 CUDA
     tensor, allocated once before an LM loop."""
-    n = lib().shapy_fit_lm_sequence_workspace_bytes(int(B), int(S), int(n_rot), int(nb))
-    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+    return _workspace(lib().shapy_fit_lm_sequence_workspace_bytes(int(B), int(S), int(n_rot), int(nb)), device)
 
 
 def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics, robust_sigma, pose_prior_weight,
@@ -963,21 +980,12 @@ def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics
     what = 'fit_lm_keypoints_2d_sequence_step'
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
-    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
+                                pose_anchor)
     srw, stw = float(smooth_rot_weight), float(smooth_transl_weight)
-    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
-        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
     if not (0 <= srw < float('inf') and 0 <= stw < float('inf')):
         raise ValueError(f'{what}: the smoothness weights must be finite and >= 0')
-    if pose_prior_weight > 0 and pose_anchor is None:
-        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
-    off = sequence_offsets
-    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
-            off.is_contiguous()):
-        raise RuntimeError(f'{what}: sequence_offsets must be a contiguous (S + 1,) int32 CPU tensor')
-    S = off.numel() - 1
-    if S < 0 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
-        raise ValueError(f'{what}: sequence_offsets must rise strictly from 0 to the batch ({B})')
+    S = _check_offsets(what, 'sequence_offsets', sequence_offsets, B)
     anchor = [] if pose_anchor is None else [pose_anchor]
     ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + \
         [trial[k] for k in ('rot', 'betas', 'image_betas', 'transl')] + [targets, weights, intrinsics, trial_keypoints,
@@ -995,14 +1003,12 @@ def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics
         raise RuntimeError(f'{what}: betas and trial betas must be ({S}, {nb}), image_betas ({B}, {nb}) and loss, '
                            f'lambda and accepted ({S},)')
     L = lib()
-    need = L.shapy_fit_lm_sequence_workspace_bytes(B, S, n_rot, nb)
-    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
-        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    _check_workspace(what, workspace, L.shapy_fit_lm_sequence_workspace_bytes(B, S, n_rot, nb))
     if B == 0:
         return
     with torch.cuda.device(trial['rot'].device):
         check(L.shapy_fit_lm_keypoints_2d_sequence_step(
-            B, S, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(pose_anchor), sigma,
+            B, S, sequence_offsets.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(pose_anchor), sigma,
             float(pose_prior_weight), float(betas_weight), srw, stw, float(lambda_up), float(lambda_down),
             int(bool(first)),
             *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
@@ -1013,8 +1019,7 @@ def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics
 def fit_lm_calibrated_workspace(B, G, device):
     """The scratch of the calibrated 2D step (include/shapy_b200.h, shapy_fit_lm_calibrated_workspace_bytes): a uint8
     CUDA tensor, allocated once before an LM loop."""
-    n = lib().shapy_fit_lm_calibrated_workspace_bytes(int(B), int(G))
-    return torch.empty(max(int(n), 1), dtype=torch.uint8, device=device)
+    return _workspace(lib().shapy_fit_lm_calibrated_workspace_bytes(int(B), int(G)), device)
 
 
 def _fit_lm_kp2d_calibrated(what, state, trial, targets, weights, intrinsics, extrinsics, robust_sigma,
@@ -1024,17 +1029,9 @@ def _fit_lm_kp2d_calibrated(what, state, trial, targets, weights, intrinsics, ex
     trial_meas, trial_meas_jac), all (G, ...)."""
     G, n_rot = trial['rot'].shape[:2]
     nb, B, K = trial['betas'].shape[1], targets.shape[0], targets.shape[1]
-    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
-    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and lambda_up >= 1 and lambda_down >= 1):
-        raise ValueError(f'{what}: robust_sigma must be > 0, the prior weights >= 0 and the lambda factors >= 1')
-    if pose_prior_weight > 0 and pose_anchor is None:
-        raise ValueError(f'{what}: pose_prior_weight > 0 needs pose_anchor')
-    off = view_offsets
-    if not (torch.is_tensor(off) and off.device.type == 'cpu' and off.dtype == torch.int32 and off.dim() == 1 and
-            off.is_contiguous()):
-        raise RuntimeError(f'{what}: view_offsets must be a contiguous (G + 1,) int32 CPU tensor')
-    if off.numel() != G + 1 or int(off[0]) != 0 or int(off[-1]) != B or not bool((off[1:] > off[:-1]).all()):
-        raise ValueError(f'{what}: view_offsets must rise strictly from 0 to the number of views ({B}) over {G} bodies')
+    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
+                                pose_anchor)
+    _check_offsets(what, 'view_offsets', view_offsets, B, G)
     anchor = [] if pose_anchor is None else [pose_anchor]
     mstate = [] if meas is None else [state['meas'], state['meas_jac']]
     ts = [state[k] for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
@@ -1055,12 +1052,10 @@ def _fit_lm_kp2d_calibrated(what, state, trial, targets, weights, intrinsics, ex
         raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
                            f'({G}, 5)')
     L = lib()
-    need = L.shapy_fit_lm_calibrated_workspace_bytes(B, G)
-    if not (workspace.is_cuda and workspace.is_contiguous() and workspace.numel() * workspace.element_size() >= need):
-        raise RuntimeError(f'{what}: the workspace must be a contiguous CUDA tensor of at least {need} bytes')
+    _check_workspace(what, workspace, L.shapy_fit_lm_calibrated_workspace_bytes(B, G))
     if G == 0:
         return
-    head = [B, G, off.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(extrinsics),
+    head = [B, G, view_offsets.data_ptr(), K, n_rot, nb, ptr(targets), ptr(weights), ptr(intrinsics), ptr(extrinsics),
             ptr(pose_anchor), sigma, float(pose_prior_weight), float(betas_weight)]
     lam = [float(lambda_up), float(lambda_down), int(bool(first))]
     tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial['transl']), ptr(trial_keypoints), ptr(trial_jac)]
