@@ -146,6 +146,15 @@ int shapy_smplx_backward(const shapy_smplx_t *m, const float *betas, const float
 int shapy_smplx_keypoint_jacobian(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
                                   const float *transl, int batch, float *keypoints, float *jac, void *stream);
 
+/* shapy_smplx_keypoint_jacobian at a non-zero facial expression, with its columns: expr (B,NE) as in
+ * shapy_smplx_forward, P = 3 n_rot + NB + NE + 3, the columns [delta_j | betas | expression | transl].  The expression
+ * rows are rows NB .. NC-1 of the shape basis, so their columns have the betas columns' form.  At expr = 0 the keypoints
+ * and every column but the expression's are shapy_smplx_keypoint_jacobian's bit for bit.  SHAPY_ERR_ARG for a model
+ * without an expression basis; otherwise the same rules. */
+int shapy_smplx_keypoint_jacobian_expr(const shapy_smplx_t *m, const float *betas, const float *expr, const float *rot,
+                                       int n_rot, const float *transl, int batch, float *keypoints, float *jac,
+                                       void *stream);
+
 /* Adjoint of shapy_decode_rot6d: grad_raw (n, 6) from raw (n, 6) and grad_rot (n, 3, 3), elementwise.  The 1e-12
  * clamp of each norm passes gradient to the norm only where the norm is >= 1e-12 (torch's clamp_min). */
 int shapy_decode_rot6d_backward(const float *raw, int n, const float *grad_rot, float *grad_raw, void *stream);
@@ -361,6 +370,37 @@ int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
     float *betas, float *transl, float *keypoints, float *jac, float *meas, float *meas_jac, float *loss, float *lambda,
     int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_keypoints,
     const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_step for the whole SMPL-X body: any n_rot (the hands, jaw and eyes past joint 21) and ne
+ * expression coefficients, P = 3 n_rot + nb + ne + 3 <= 200 (SHAPY_ERR_UNSUPPORTED past that).  Parameters [delta_j
+ * (3 n_rot) | beta (nb) | psi (ne) | c], the columns of shapy_smplx_keypoint_jacobian_expr (of
+ * shapy_smplx_keypoint_jacobian when ne = 0) without transl.  Loss per body, fp64, left to right: the 2D step's
+ * keypoint term and pose prior, + betas_weight |beta|^2, + expression_weight |psi|^2.  joint_weights: null (every
+ * joint j >= 1 weighted pose_prior_weight, the 2D step's prior) or (n_rot) device floats w_j, the prior then
+ * sum_{j >= 1, w_j > 0} (w_j / 2) |R_j - R0_j|_F^2 (j order; joint 0 is not read and has no prior), which lets the
+ * hands, jaw and eyes be held apart from the body.  The expression columns are damped by expression_weight + lambda,
+ * the betas columns by betas_weight + lambda, the rest by lambda; g gains expression_weight psi.  expression /
+ * trial_expression (B,ne) may be null when ne = 0.  With ne = 0 and joint_weights null every output equals
+ * shapy_fit_lm_keypoints_2d_step's bit for bit (at n_rot, nb where that step runs).  One CTA per body, the packed
+ * normal matrix in shared memory (one CTA per SM).  Other rules and errors as shapy_fit_lm_keypoints_2d_step. */
+int shapy_fit_lm_keypoints_2d_expressive_step(
+    int batch, int num_keypoints, int n_rot, int nb, int ne, const float *targets, const float *weights,
+    const float *pose_anchor, const float *joint_weights, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float expression_weight, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *expression, float *camera, float *keypoints, float *jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_expression, float *trial_camera,
+    const float *trial_keypoints, const float *trial_jac, void *stream);
+
+/* shapy_fit_lm_keypoints_2d_expressive_step under the perspective camera of
+ * shapy_fit_lm_keypoints_2d_perspective_step (intrinsics (B,3), translation t in the place of the camera, its depth
+ * rule).  With ne = 0 and joint_weights null every output equals that step's bit for bit. */
+int shapy_fit_lm_keypoints_2d_expressive_perspective_step(
+    int batch, int num_keypoints, int n_rot, int nb, int ne, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, const float *joint_weights, float robust_sigma,
+    float pose_prior_weight, float betas_weight, float expression_weight, float lambda_up, float lambda_down, int first,
+    float *rot, float *betas, float *expression, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_expression,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream);
 
 /* shapy_fit_lm_keypoints_2d_step over groups of images of one person: the images [group_offsets[g],
  * group_offsets[g+1]) of group g share one beta_g, each keeps its own rotations and camera.  Loss per group, fp64, left

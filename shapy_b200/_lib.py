@@ -77,6 +77,8 @@ _SIGS = {
     'shapy_decode_rot6d_backward': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'shapy_smplx_keypoint_jacobian': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                               c_void_p]),
+    'shapy_smplx_keypoint_jacobian_expr': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                                   c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                        C.POINTER(MeasureLandmarks), c_void_p, c_void_p, c_void_p]),
     'shapy_measure_backward_tris': (c_int, [c_void_p, c_int, c_int, C.POINTER(MeasureLandmarks), c_void_p, c_void_p,
@@ -112,6 +114,10 @@ _SIGS = {
                                                                         C.c_float, c_void_p, c_void_p, C.c_float,
                                                                         C.c_float, c_int]
                                                                 + [c_void_p] * 17 + [c_void_p]),
+    'shapy_fit_lm_keypoints_2d_expressive_step': (c_int, [c_int] * 5 + [c_void_p] * 4 + [C.c_float] * 6 + [c_int]
+                                                  + [c_void_p] * 15 + [c_void_p]),
+    'shapy_fit_lm_keypoints_2d_expressive_perspective_step': (c_int, [c_int] * 5 + [c_void_p] * 5 + [C.c_float] * 6
+                                                              + [c_int] + [c_void_p] * 15 + [c_void_p]),
     'shapy_fit_lm_groups_workspace_bytes': (C.c_size_t, [c_int, c_int, c_int, c_int]),
     'shapy_fit_lm_keypoints_2d_groups_step': (c_int, [c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                                       c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,

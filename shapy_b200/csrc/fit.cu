@@ -1840,6 +1840,304 @@ int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
   return SHAPY_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The wide 2D step (shapy_fit_lm_keypoints_2d_expressive_step, and _perspective_ with PERSP): the single-image 2D step
+// for the hands, jaw, eyes and facial expression of SMPL-X.  Parameters [delta_j (3 n_rot) | beta (nb) | psi (ne) | c
+// or t], P = 3 n_rot + nb + ne + 3 <= kLmWideMaxP, the columns of shapy_smplx_keypoint_jacobian_expr (of
+// shapy_smplx_keypoint_jacobian with ne = 0).  Per body, in fp64, left to right:
+//   L = the 2D step's keypoint term and pose prior (robust, the PERSP depth rule)
+//     + betas_w |beta|^2 (l order; when betas_w > 0) + expr_w |psi|^2 (l order; when expr_w > 0).
+// The pose prior is the 2D step's with the scalar pose_w; with per-joint weights w_j (joint_w, n_rot entries, joint 0
+// not read) it is sum_{j >= 1, w_j > 0} (1/2 w_j) |R_j - R0_j|_F^2 in j order, and joint j's rows have weight w_j / 2.
+// Rows, first lambda and policy are the 2D step's; the diagonal gets betas_w + lambda on the betas columns, expr_w +
+// lambda on the expression columns and lambda elsewhere, and g gains expr_w psi after betas_w beta.
+//
+// One CTA of kLmKpThreads per body, one CTA per SM: the packed fp64 lower triangle of A (P (P + 1) / 2 entries, 160.8
+// KB at P = 200) and kLmKpRows staged rows of width P live in dynamic shared memory.  Each staged chunk is added into
+// the shared triangle (thread t owns the packed entries t + 256 i, each entry summing its rows in row order, as the
+// registers of the 2D step do), then the pose-prior rows into the joints' diagonal blocks.  The Cholesky is the 2D
+// step's right-looking one on the packed triangle, one warp per trailing row; the triangular solves keep its order.
+// With ne = 0, n_rot = 22 and scalar weights every operation is the 2D step's in the same order: the results are its
+// bits.
+constexpr int kLmWideMaxP = 200;
+
+struct LmKp2dWideArgs : LmKp2dPerspArgs {   // intr is null in the weak-perspective step
+  const float *joint_w;                     // (n_rot) per-joint pose-prior weights, or null: pose_w for every joint
+  float expr_w;
+  int ne;
+  float *expr, *texpr;                      // state and trial expression (B, ne); null when ne = 0
+};
+
+// dynamic shared memory of the wide step, in doubles: the packed triangle, Js and WJs (kLmKpRows x P each), y, z, dg,
+// the scaled column and the Cholesky diagonal (P each), ws and rs (kLmKpRows each)
+__host__ __device__ inline size_t lm_wide_smem_doubles(int P) {
+  return (size_t)P * (P + 1) / 2 + (size_t)2 * kLmKpRows * P + (size_t)5 * P + 2 * kLmKpRows;
+}
+
+// the packed position of the lower-triangle entry (i, k), k <= i
+__device__ __forceinline__ int tri(int i, int k) { return i * (i + 1) / 2 + k; }
+
+// the packed entry p of thread t's first entry: row r, column c (c <= r)
+__device__ __forceinline__ void tri_rc(int p, int &r, int &c) {
+  r = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
+  while ((r + 1) * (r + 2) / 2 <= p) ++r;
+  while (r * (r + 1) / 2 > p) --r;
+  c = p - r * (r + 1) / 2;
+}
+
+template <bool PERSP>
+__global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs a, LmKp2dWideArgs x2) {
+  extern __shared__ double smem[];
+  __shared__ double lt_s, lam_s;
+  __shared__ int ok_s;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nb = a.nb, ne = x2.ne, nr9 = 9 * a.n_rot;
+  const int o = 3 * a.n_rot, oe = o + nb, oc = oe + ne;   // first betas, expression and camera column
+  const int npk = P * (P + 1) / 2;
+  double *A = smem, *Js = A + npk, *WJs = Js + kLmKpRows * P, *y = WJs + kLmKpRows * P, *z = y + P, *dg = z + P,
+         *col = dg + P, *ld = col + P, *ws = ld + P, *rs = ws + kLmKpRows;
+  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
+  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
+  const bool robust = isfinite(x2.sigma), prior = x2.joint_w || x2.pose_w > 0.f;
+  const double s2 = (double)x2.sigma * (double)x2.sigma;
+  const float lcur = a.loss[b];
+  // 1. trial loss
+  if (t == 0) {
+    LmKp2dArgs xs = x2;
+    if (x2.joint_w) xs.pose_w = 0.f;       // the per-joint prior follows the keypoint term
+    double L;
+    if constexpr (PERSP) {
+      const PerspCam tc = persp_cam(x2.intr + (size_t)b * 3, a.tlast + (size_t)b * 3);
+      L = lm_kp2d_trial_loss<true>(a, xs, b, tg, wt, anc, robust, s2, &tc);
+    } else {
+      L = lm_kp2d_trial_loss(a, xs, b, tg, wt, anc, robust, s2);
+    }
+    if (x2.joint_w) {
+      const float *tr = a.trot + (size_t)b * nr9;
+      for (int j = 1; j < a.n_rot; ++j) {
+        if (!(x2.joint_w[j] > 0.f)) continue;
+        double q = 0.0;
+        for (int e = 9 * j; e < 9 * j + 9; ++e) {
+          const double d = (double)tr[e] - (double)anc[e];
+          q += d * d;
+        }
+        L += (0.5 * (double)x2.joint_w[j]) * q;
+      }
+    }
+    if (x2.betas_w > 0.f) {
+      const float *tb = a.tbetas + (size_t)b * nb;
+      double reg = 0.0;
+      for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
+      L += (double)x2.betas_w * reg;
+    }
+    if (x2.expr_w > 0.f) {
+      const float *te = x2.texpr + (size_t)b * ne;
+      double reg = 0.0;
+      for (int l = 0; l < ne; ++l) reg += (double)te[l] * (double)te[l];
+      L += (double)x2.expr_w * reg;
+    }
+    lt_s = L;
+  }
+  for (int p = t; p < npk; p += blockDim.x) A[p] = 0.0;
+  __syncthreads();
+  // 2. accept or reject
+  const double lt = lt_s;
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
+  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
+  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
+  const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
+  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
+  const float *Est = ne ? (accept ? x2.texpr : x2.expr) + (size_t)b * ne : nullptr;
+  const float *Cst = (accept ? a.tlast : a.last) + (size_t)b * 3;
+  if (accept) {
+    lm_kp_take_trial(a, b, lnew);
+    for (int i = t; i < ne; i += blockDim.x) x2.expr[(size_t)b * ne + i] = x2.texpr[(size_t)b * ne + i];
+  }
+  double s, ds;
+  softplus_d((double)Cst[0], s, ds);
+  const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
+  PerspCam sc{};
+  if constexpr (PERSP) sc = persp_cam(x2.intr + (size_t)b * 3, Cst);
+  double *fz = nullptr;
+  if constexpr (PERSP) fz = lm_persp_factors();
+  // 3. normal equations: the keypoint rows 2k + c, kLmKpRows at a time, into the packed triangle
+  int r0e, c0e;                             // this thread's first packed entry
+  tri_rc(t, r0e, c0e);
+  double g = 0.0;
+  for (int r0 = 0; r0 < 2 * K; r0 += kLmKpRows) {
+    const int nr = min(kLmKpRows, 2 * K - r0);
+    __syncthreads();
+    for (int i = t; i < nr; i += blockDim.x) {
+      double wr, res;
+      lm_kp2d_row<PERSP>(M, tg, wt, s, cxy, robust, s2, (r0 + i) >> 1, (r0 + i) & 1, wr, res, &sc,
+                         PERSP ? fz + 2 * i : nullptr);
+      ws[i] = wr;
+      rs[i] = res;
+    }
+    __syncthreads();
+    for (int i = t; i < nr * P; i += blockDim.x) {
+      const int row = i / P, c = i % P;
+      const double wr = ws[row];
+      if (wr > 0.0) {                       // a dropped keypoint's rows are never read: they may be NaN
+        const double v = lm_kp2d_entry<false, PERSP>(J, M, P, oc, (r0 + row) >> 1, (r0 + row) & 1, c, s, ds, cxy,
+                                                     PERSP ? fz + 2 * row : nullptr);
+        Js[row * P + c] = v;
+        WJs[row * P + c] = wr * v;
+      }
+    }
+    __syncthreads();
+    int r = r0e, c = c0e;
+    for (int p = t; p < npk; p += blockDim.x) {
+      double acc = A[p];
+      for (int row = 0; row < nr; ++row)
+        if (ws[row] > 0.0) acc += WJs[row * P + r] * Js[row * P + c];
+      A[p] = acc;
+      c += blockDim.x;
+      while (c > r) {
+        c -= r + 1;
+        ++r;
+      }
+    }
+    if (t < P)
+      for (int row = 0; row < nr; ++row)
+        if (ws[row] > 0.0) g += WJs[row * P + t] * rs[row];
+  }
+  __syncthreads();
+  if (t < P) dg[t] = A[tri(t, t)];          // the diagonal of the keypoint rows: the first lambda
+  // the pose-prior rows of joint j (weight w_j / 2) reach only its diagonal block: its six lower entries.  Another
+  // thread than t adds the prior to diagonal entry t: every dg read has to come first
+  __syncthreads();
+  if (prior) {
+    for (int q = t; q < 6 * (a.n_rot - 1); q += blockDim.x) {
+      const int j = 1 + q / 6, u = q % 6, ar = u < 1 ? 0 : u < 3 ? 1 : 2, ac = u - ar * (ar + 1) / 2;
+      const float wj = x2.joint_w ? x2.joint_w[j] : x2.pose_w;
+      if (!(wj > 0.f)) continue;
+      const double hw = 0.5 * (double)wj;
+      const float *R = Rst + 9 * j;
+      const int p = tri(3 * j + ar, 3 * j + ac);
+      double acc = A[p];
+      for (int e = 0; e < 9; ++e) acc += (hw * rot_tangent(R, ar, e)) * rot_tangent(R, ac, e);
+      A[p] = acc;
+    }
+    if (t >= 3 && t < o) {
+      const float wj = x2.joint_w ? x2.joint_w[t / 3] : x2.pose_w;
+      if (wj > 0.f) {
+        const double hw = 0.5 * (double)wj;
+        const float *R = Rst + 9 * (t / 3), *R0 = anc + 9 * (t / 3);
+        for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
+      }
+    }
+  }
+  if (x2.betas_w > 0.f && t >= o && t < oe) g += (double)x2.betas_w * (double)Bst[t - o];
+  if (x2.expr_w > 0.f && t >= oe && t < oc) g += (double)x2.expr_w * (double)Est[t - oe];
+  if (t < P) y[t] = -g;
+  __syncthreads();
+  if (t == 0) {
+    double dmax = kDiagFloor;
+    if (a.first)
+      for (int j = 0; j < P; ++j) dmax = fmax(dmax, dg[j]);
+    const float lam = lm_lambda(a.first, accept, a.first ? 0.f : a.lambda[b], dmax, a.up, a.down);
+    a.lambda[b] = lam;
+    if (accept && !a.first) a.accepted[b] += 1;
+    lam_s = lam;
+    ok_s = isfinite(lnew);
+  }
+  __syncthreads();
+  if (t < P) {
+    const double lam = lam_s;
+    A[tri(t, t)] += t >= o && t < oe ? (double)x2.betas_w + lam : t >= oe && t < oc ? (double)x2.expr_w + lam : lam;
+  }
+  // 4. Cholesky A = L L^T on the packed triangle: column j scaled (its pivot into ld, a copy into col), then the
+  // trailing triangle updated, one warp per row
+  const int warp = t >> 5, lane = t & 31, nw = blockDim.x >> 5;
+  for (int j = 0; j < P; ++j) {
+    __syncthreads();
+    const double d = A[tri(j, j)];
+    const double ljj = sqrt(d);
+    if (t == 0) {
+      ok_s = ok_s && d > 0.0 && isfinite(d);
+      ld[j] = ljj;
+    }
+    for (int i = j + 1 + t; i < P; i += blockDim.x) {
+      const double v = A[tri(i, j)] / ljj;
+      A[tri(i, j)] = v;
+      col[i] = v;
+    }
+    __syncthreads();
+    for (int i = j + 1 + warp; i < P; i += nw) {
+      const double ci = col[i];
+      double *Ai = A + tri(i, 0);
+      for (int k = j + 1 + lane; k <= i; k += 32) Ai[k] -= ci * col[k];
+    }
+  }
+  // L z = -g (column order), then L^T delta = z (column order, from the last) into y
+  for (int j = 0; j < P; ++j) {
+    __syncthreads();
+    const double yj = y[j] / ld[j];
+    if (t == 0) z[j] = yj;
+    for (int i = j + 1 + t; i < P; i += blockDim.x) y[i] -= A[tri(i, j)] * yj;
+  }
+  for (int j = P - 1; j >= 0; --j) {
+    __syncthreads();
+    const double dj = z[j] / ld[j];
+    if (t == 0) y[j] = dj;
+    for (int i = t; i < j; i += blockDim.x) z[i] -= A[tri(j, i)] * dj;
+  }
+  __syncthreads();
+  // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
+  const bool ok = ok_s;
+  const float *sr = a.rot + (size_t)b * nr9;
+  float *trr = a.trot + (size_t)b * nr9;
+  for (int j = t; j < a.n_rot; j += blockDim.x) {
+    if (!ok) {
+      for (int e = 0; e < 9; ++e) trr[9 * j + e] = sr[9 * j + e];
+      continue;
+    }
+    lm_exp_gs(sr + 9 * j, y[3 * j], y[3 * j + 1], y[3 * j + 2], trr + 9 * j);
+  }
+  for (int l = t; l < nb; l += blockDim.x) {
+    const float v = a.betas[(size_t)b * nb + l];
+    a.tbetas[(size_t)b * nb + l] = ok ? (float)((double)v + y[o + l]) : v;
+  }
+  for (int l = t; l < ne; l += blockDim.x) {
+    const float v = x2.expr[(size_t)b * ne + l];
+    x2.texpr[(size_t)b * ne + l] = ok ? (float)((double)v + y[oe + l]) : v;
+  }
+  if (t < 3) {
+    const float v = a.last[(size_t)b * 3 + t];
+    a.tlast[(size_t)b * 3 + t] = ok ? (float)((double)v + y[oc + t]) : v;
+  }
+}
+
+// The wide entries' checks (check_lm_kp's with P counting the expression columns and kLmWideMaxP) and the launch
+int run_lm_kp2dw(const char *fn, int batch, LmKpArgs a, LmKp2dWideArgs x, bool persp, void *stream) {
+  const bool ptrs = (x.anchor || !(x.pose_w > 0.f || x.joint_w)) && (x.ne == 0 || (x.expr && x.texpr)) &&
+                    (!persp || x.intr);
+  SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
+                    a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && ptrs,
+                "%s: null argument", fn);
+  SHAPY_REQUIRE(batch >= 0 && a.K >= 1 && a.n_rot >= 1 && a.n_rot <= 64 && a.nb >= 1 && x.ne >= 0,
+                "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas, %d expression)", fn, batch, a.K, a.n_rot,
+                a.nb, x.ne);
+  SHAPY_REQUIRE(a.up >= 1.f && a.down >= 1.f && x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f &&
+                    x.expr_w >= 0.f,
+                "%s: robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
+                "lambda_down >= 1",
+                fn);
+  a.P = 3 * a.n_rot + a.nb + x.ne + 3;
+  if (a.P > kLmWideMaxP) {
+    set_error("%s: %d parameters, at most %d are supported", fn, a.P, kLmWideMaxP);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  if (batch == 0) return SHAPY_OK;
+  const size_t smem = lm_wide_smem_doubles(a.P) * sizeof(double);
+  auto kernel = persp ? lm_kp2dw_step_kernel<true> : lm_kp2dw_step_kernel<false>;
+  SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
+  kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -2104,4 +2402,44 @@ extern "C" int shapy_fit_lm_keypoints_2d_sequence_step(
                   smooth_rot_weight, smooth_transl_weight};
   return run_lm_kp2ds("shapy_fit_lm_keypoints_2d_sequence_step", batch, num_sequences, sequence_offsets, a, x,
                       trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_expressive_step(
+    int batch, int num_keypoints, int n_rot, int nb, int ne, const float *targets, const float *weights,
+    const float *pose_anchor, const float *joint_weights, float robust_sigma, float pose_prior_weight,
+    float betas_weight, float expression_weight, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *expression, float *camera, float *keypoints, float *jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_expression, float *trial_camera,
+    const float *trial_keypoints, const float *trial_jac, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
+  LmKp2dWideArgs x{};
+  static_cast<LmKp2dPerspArgs &>(x) =
+      LmKp2dPerspArgs{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, nullptr};
+  x.joint_w = joint_weights;
+  x.expr_w = expression_weight;
+  x.ne = ne;
+  x.expr = expression;
+  x.texpr = trial_expression;
+  return run_lm_kp2dw("shapy_fit_lm_keypoints_2d_expressive_step", batch, a, x, false, stream);
+}
+
+extern "C" int shapy_fit_lm_keypoints_2d_expressive_perspective_step(
+    int batch, int num_keypoints, int n_rot, int nb, int ne, const float *targets, const float *weights,
+    const float *intrinsics, const float *pose_anchor, const float *joint_weights, float robust_sigma,
+    float pose_prior_weight, float betas_weight, float expression_weight, float lambda_up, float lambda_down, int first,
+    float *rot, float *betas, float *expression, float *transl, float *keypoints, float *jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_expression,
+    float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream) {
+  LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
+             keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
+  LmKp2dWideArgs x{};
+  static_cast<LmKp2dPerspArgs &>(x) =
+      LmKp2dPerspArgs{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics};
+  x.joint_w = joint_weights;
+  x.expr_w = expression_weight;
+  x.ne = ne;
+  x.expr = expression;
+  x.texpr = trial_expression;
+  return run_lm_kp2dw("shapy_fit_lm_keypoints_2d_expressive_perspective_step", batch, a, x, true, stream);
 }

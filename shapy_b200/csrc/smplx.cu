@@ -920,12 +920,14 @@ __device__ __forceinline__ float kp_jdir(const SmplxDev &m, int j, int c, int l)
 }
 
 // v_posed of vertex v (template, the NB shape rows, the fp32 posedirs rows below Kp, in that order), M and the posed
-// vertex sum_s w_s (G_s.R (v_posed - J_s) + G_s.t), the skinning weights in ELL order
+// vertex sum_s w_s (G_s.R (v_posed - J_s) + G_s.t), the skinning weights in ELL order.  EXPR: the NE expression rows
+// follow the shape rows (all NC basis rows)
+template <bool EXPR = false>
 __device__ __forceinline__ void kp_vertex_state(const SmplxDev &m, int v, int Kp, const float *coef, const float *pf,
                                                 const float (*G)[12], const float (*Jr)[3], float *st) {
   const int V3 = m.V * 3;
   float p0 = m.v_template[3 * v], p1 = m.v_template[3 * v + 1], p2 = m.v_template[3 * v + 2];
-  for (int l = 0; l < m.NB; ++l) {
+  for (int l = 0; l < (EXPR ? m.NC : m.NB); ++l) {
     const float *S = m.basis + (size_t)l * m.V3p + 3 * v;
     p0 += S[0] * coef[l]; p1 += S[1] * coef[l]; p2 += S[2] * coef[l];
   }
@@ -1015,7 +1017,16 @@ __device__ __forceinline__ void kp_vertex_dbeta(const SmplxDev &m, int v, int l,
   }
 }
 
-__global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a) {
+// The expression-aware Jacobian's arguments: the expression (B, NE) rides after KpJacArgs, which keeps its layout
+struct KpJacExprArgs : KpJacArgs {
+  const float *expr;
+};
+
+// The body of both Jacobian kernels.  EXPR (smplx_kp_jac_expr_kernel): the chain and the vertex states at the
+// expression a.expr, and NE more columns after the betas: the expression rows are shape rows l in [NB, NC) of basis and
+// J_dirs, so their columns are the betas columns' formula over all NC coefficients (P = 3 n_rot + NC + 3)
+template <bool EXPR, typename Args>
+__device__ __forceinline__ void kp_jac_body(const Args &a) {
   const SmplxDev &m = a.m;
   const int b = blockIdx.x, t = threadIdx.x;
   __shared__ float R[kMaxJoints][9];
@@ -1027,8 +1038,10 @@ __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a
   __shared__ unsigned long long sub[kMaxJoints];    // bit i of sub[s]: i is s or one of its ancestors
   __shared__ int lut_row;
   extern __shared__ float cache[];                  // [n_entries][kKpState] when cached
-  const int NB = m.NB;
-  body_chain(m, a.betas, nullptr, a.rot, a.n_rot, b, R, Jr, G, coef);
+  const int NB = EXPR ? m.NC : m.NB;                // the shape-like columns: betas, then the expression with EXPR
+  const float *expr = nullptr;
+  if constexpr (EXPR) expr = a.expr;
+  body_chain(m, a.betas, expr, a.rot, a.n_rot, b, R, Jr, G, coef);
   if (t == 0) {
     for (int s = 0; s < m.J; ++s) sub[s] = (s ? sub[m.parents[s]] : 0ull) | (1ull << s);
     lut_row = m.D > 0 ? contour_lut_row(m, R) : 0;
@@ -1056,7 +1069,7 @@ __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a
       int v;
       float w;
       kp_entry(m, row, e, v, w);
-      kp_vertex_state(m, v, a.Kp, coef, pf, G, Jr, cache + (size_t)e * kKpState);
+      kp_vertex_state<EXPR>(m, v, a.Kp, coef, pf, G, Jr, cache + (size_t)e * kKpState);
     }
     __syncthreads();
   }
@@ -1074,7 +1087,7 @@ __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a
     auto state = [&](int e, int &v, float &w) -> const float * {
       kp_entry(m, row, e, v, w);
       if (a.cached) return cache + (size_t)e * kKpState;
-      kp_vertex_state(m, v, a.Kp, coef, pf, G, Jr, local);
+      kp_vertex_state<EXPR>(m, v, a.Kp, coef, pf, G, Jr, local);
       return local;
     };
     if (g < a.n_rot) {
@@ -1138,6 +1151,10 @@ __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a
     }
   }
 }
+
+__global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a) { kp_jac_body<false>(a); }
+
+__global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_expr_kernel(KpJacExprArgs a) { kp_jac_body<true>(a); }
 
 }  // namespace shapy
 
@@ -1662,6 +1679,30 @@ extern "C" int shapy_smplx_keypoint_jacobian(const shapy_smplx_t *m, const float
     SHAPY_CUDA_TRY(cudaFuncSetAttribute(smplx_kp_jac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   KpJacArgs a{d, betas, rot, transl, n_rot, (n_rot - 1) * 9, 3 * n_rot + d.NB + 3, n_entries, cached, keypoints, jac};
   smplx_kp_jac_kernel<<<B, kKpJacThreads, smem, (cudaStream_t)stream>>>(a);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" int shapy_smplx_keypoint_jacobian_expr(const shapy_smplx_t *m, const float *betas, const float *expr,
+                                                  const float *rot, int n_rot, const float *transl, int B,
+                                                  float *keypoints, float *jac, void *stream) {
+  SHAPY_REQUIRE(m && betas && expr && rot && keypoints && jac, "shapy_smplx_keypoint_jacobian_expr: null argument");
+  SHAPY_REQUIRE(B >= 0, "shapy_smplx_keypoint_jacobian_expr: batch %d", B);
+  SHAPY_REQUIRE(n_rot >= 1 && n_rot <= m->d.J, "shapy_smplx_keypoint_jacobian_expr: n_rot %d out of range", n_rot);
+  SHAPY_REQUIRE(m->d.NE >= 1, "shapy_smplx_keypoint_jacobian_expr: the model has no expression basis");
+  if (B == 0) return SHAPY_OK;
+  const SmplxDev &d = m->d;
+  const int n_entries = 3 * (d.L + d.D) + m->extra_nnz;
+  const int cached = n_entries <= kKpCacheEntries;
+  const size_t smem = cached ? (size_t)n_entries * kKpState * sizeof(float) : 0;
+  if (smem > 0)
+    SHAPY_CUDA_TRY(
+        cudaFuncSetAttribute(smplx_kp_jac_expr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  KpJacExprArgs a;
+  static_cast<KpJacArgs &>(a) =
+      KpJacArgs{d, betas, rot, transl, n_rot, (n_rot - 1) * 9, 3 * n_rot + d.NC + 3, n_entries, cached, keypoints, jac};
+  a.expr = expr;
+  smplx_kp_jac_expr_kernel<<<B, kKpJacThreads, smem, (cudaStream_t)stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

@@ -428,14 +428,18 @@ def _adam_result(params, grot, bpose, meas, **outputs):
     return res
 
 
-def _kp_lm_state(B, K, n_rot, nb, last, device, G=None):
+def _kp_lm_state(B, K, n_rot, nb, last, device, G=None, ne=None):
     """The state tensors of a keypoint LM step (ops.fit_lm_keypoints_step), `last` naming the last three parameters;
-    with G, the grouped steps' state: 'betas', 'loss', 'lambda' and 'accepted' per group."""
+    with G, the grouped steps' state: 'betas', 'loss', 'lambda' and 'accepted' per group; with ne, the wide 2D step's
+    state (ops.fit_lm_keypoints_2d_expressive_step): 'expression' (B, ne) and ne more Jacobian columns."""
     G = B if G is None else G
     mk = lambda *s: torch.empty(*s, dtype=torch.float32, device=device)  # noqa: E731
-    return {'rot': mk(B, n_rot, 3, 3), 'betas': mk(G, nb), last: mk(B, 3), 'keypoints': mk(B, K, 3),
-            'jac': mk(B, 3 * K, 3 * n_rot + nb + 3), 'loss': mk(G), 'lambda': mk(G),
-            'accepted': torch.zeros(G, dtype=torch.int32, device=device)}
+    state = {'rot': mk(B, n_rot, 3, 3), 'betas': mk(G, nb), last: mk(B, 3), 'keypoints': mk(B, K, 3),
+             'jac': mk(B, 3 * K, 3 * n_rot + nb + (ne or 0) + 3), 'loss': mk(G), 'lambda': mk(G),
+             'accepted': torch.zeros(G, dtype=torch.int32, device=device)}
+    if ne is not None:
+        state['expression'] = mk(B, ne)
+    return state
 
 
 def _kp_lm_result(state, last, **outputs):
@@ -556,12 +560,14 @@ def _start_rotations(params, pose_anchor, n):
     return rot0, torch.as_tensor(pose_anchor, dtype=torch.float32, device=rot0.device).reshape(n, 22, 3, 3).contiguous()
 
 
-def _forward_2d(body_model, grot, bpose, betas, last, intr):
+def _forward_2d(body_model, grot, bpose, betas, last, intr, parts=None, expression=None):
     """SMPLX.forward of a 2D fit with its proj_joints: `last` the weak-perspective camera (intr None) or the
-    translation seen by the perspective camera with intrinsics intr (B, 3)."""
+    translation seen by the perspective camera with intrinsics intr (B, 3); parts: the rotations of the pose parts
+    past the body by SMPLX.forward's names, expression (B, NE) or None."""
+    kw = dict(parts or {}, expression=expression)
     if intr is None:
-        return body_model(global_rot=grot, body_pose=bpose, betas=betas, camera=last, return_shaped=False)
-    out = body_model(global_rot=grot, body_pose=bpose, betas=betas, transl=last, return_shaped=False)
+        return body_model(global_rot=grot, body_pose=bpose, betas=betas, camera=last, return_shaped=False, **kw)
+    out = body_model(global_rot=grot, body_pose=bpose, betas=betas, transl=last, return_shaped=False, **kw)
     out['proj_joints'] = _project(out['joints'][:], intr)
     return out
 
@@ -682,7 +688,7 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                              robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
                              body_measurements=None, measurements=None, measurement_weights=None,
                              circumference_derivative='reference', groups=None, share_pose=False, focal_length=None,
-                             principal_point=None):
+                             principal_point=None, pose_width=22, fit_expression=False, expression_weight=0.0):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -731,7 +737,25 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     with a weighted keypoint at Y_z <= 0 is rejected by 'lm'; the returned loss is +inf for a body that has one.
     The measurement weights are the crop frame's; with targets in pixels a known height needs a larger weight to
     count (measurement_weights={'height': 1e6}: 1 mm of height costs what 1 px of one keypoint does).  groups and
-    share_pose are not supported with a focal length."""
+    share_pose are not supported with a focal length.
+    pose_width: 22 (the global rotation and the body), or 23, 24, 25, 40 or 55 to fit the jaw, the eyes and the hands
+    as well (SMPL-X's joint order: jaw, left eye, right eye, 15 left-hand and 15 right-hand joints); fit_expression
+    also fits the NE expression coefficients psi, with the regulariser expression_weight |psi|^2.  Either one takes
+    the wide path: init may carry raw 6D 'jaw_pose' (B, 6), 'leye_pose', 'reye_pose', 'left_hand_pose' (B, 90) and
+    'right_hand_pose' for the parts inside the width and 'expression' (B, NE); a part without one starts at the
+    identity and the expression at 0.  pose_prior_weight may then be a scalar or (pose_width,) per-joint weights with
+    joint 0 zero, so that the hands, jaw and eyes can be held differently from the body; pose_anchor is (B,
+    pose_width, 3, 3).  'lm' runs ops.smplx_keypoint_jacobian(expr=...) and ops.fit_lm_keypoints_2d_expressive_step per
+    iteration (two launches, no host synchronisation; at most 200 parameters); 'adam' fits the same loss through
+    SMPLX.forward.  The result also holds the raw 6D parts in the width, 'full_pose_mat' (B, pose_width, 3, 3) and,
+    when fitted, 'expression'.  A part is only as determined as its keypoints make it: one without a weighted keypoint
+    (the eyes: the OpenPose pupils are dropped on load) is held by its prior alone, and without a prior it stays where
+    it starts.  groups, share_pose and measurements are not supported on the wide path."""
+    if pose_width != 22 or fit_expression:
+        return _fit_keypoints_2d_expressive(body_model, keypoints2d, weights, init, method, iterations, robust_sigma,
+                                            pose_prior_weight, betas_weight, pose_anchor, lr, measurements, groups,
+                                            share_pose, focal_length, principal_point, pose_width, fit_expression,
+                                            expression_weight)
     iterations, sigma = _check_kp_fit('fit_body_to_keypoints_2d', body_model, method, iterations,
                                       circumference_derivative, body_measurements, measurements, robust_sigma,
                                       pose_prior_weight, betas_weight)
@@ -817,6 +841,157 @@ def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sig
         if intr is not None:
             per_body = _depth_rule(per_body, out['joints'][:], w)
     return _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+
+
+# the pose parts past the body in SMPL-X's joint order (SMPLX.forward's names) and their joint counts
+POSE_PARTS = (('jaw_pose', 1), ('leye_pose', 1), ('reye_pose', 1), ('left_hand_pose', 15), ('right_hand_pose', 15))
+POSE_WIDTHS = (22, 23, 24, 25, 40, 55)
+# the widest wide LM step: 55 rotations, 27 betas, 5 expression coefficients and the camera (or 16 and 16)
+LM_WIDE_MAX_PARAMS = 200
+
+
+def _parts_in(width):
+    """The pose parts inside a pose width: [(name, first joint, joint count)]."""
+    out, j = [], 22
+    for name, n in POSE_PARTS:
+        if j + n > width:
+            break
+        out.append((name, j, n))
+        j += n
+    return out
+
+
+def _fit_keypoints_2d_expressive(body_model, keypoints2d, weights, init, method, iterations, robust_sigma,
+                                 pose_prior_weight, betas_weight, pose_anchor, lr, measurements, groups, share_pose,
+                                 focal_length, principal_point, width, fit_expression, expression_weight):
+    """fit_body_to_keypoints_2d's wide path: the pose parts inside `width` and, with fit_expression, the expression."""
+    fn = 'fit_body_to_keypoints_2d'
+    if width not in POSE_WIDTHS:
+        raise ValueError(f'{fn}: pose_width must be one of {POSE_WIDTHS}, got {width}')
+    if groups is not None or share_pose or measurements is not None:
+        raise ValueError(f'{fn}: groups, share_pose and measurements are not supported with a pose_width past 22 or '
+                         f'fit_expression')
+    if focal_length is not None and principal_point is None:
+        raise ValueError(f'{fn}: focal_length needs principal_point')
+    if not expression_weight >= 0:
+        raise ValueError(f'{fn}: expression_weight must be >= 0')
+    jw = None
+    if np.ndim(pose_prior_weight) > 0:
+        jw = torch.as_tensor(pose_prior_weight, dtype=torch.float32).detach().cpu().reshape(-1)
+        if jw.shape != (width,) or float(jw[0]) != 0 or not bool((jw >= 0).all()):
+            raise ValueError(f'{fn}: per-joint pose_prior_weight must be ({width},), >= 0, with joint 0 zero')
+        pose_prior_weight = 0.0
+    ne = body_model.num_expression_coeffs if fit_expression else 0
+    nb = body_model.num_betas
+    if method == 'lm' and 3 * width + nb + ne + 3 > LM_WIDE_MAX_PARAMS:
+        raise ValueError(f"{fn}(method='lm'): {width} rotations, {nb} betas, {ne} expression coefficients and the "
+                         f'translation or camera are {3 * width + nb + ne + 3} parameters, at most '
+                         f'{LM_WIDE_MAX_PARAMS} are supported')
+    # _check_kp_fit's checks; its parameter bound is the 22-joint step's, so it sees the Adam method
+    iterations, sigma = _check_kp_fit(fn, body_model, 'adam' if method == 'lm' else method,
+                                      50 if method == 'lm' and iterations is None else iterations,
+                                      robust_sigma=robust_sigma, pose_prior_weight=pose_prior_weight,
+                                      betas_weight=betas_weight)
+    device = body_model.shapedirs.device
+    x, w = _keypoints_2d(fn, keypoints2d, weights, device)
+    B = x.shape[0]
+    intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
+    params = _init_2d(init, B, nb, device, method, x, w, intr)
+    init = _raw_init(init)
+    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device
+    ident[0::3].fill_(1.0)
+    parts = _parts_in(width)
+    for name, _, n in parts:
+        t = init.get(name)
+        t = ident.repeat(B, n) if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, 6 * n)
+        params[name] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    if fit_expression:
+        t = init.get('expression')
+        t = torch.zeros(B, ne, device=device) if t is None else \
+            torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, ne)
+        params['expression'] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    from . import ops
+    raw = torch.cat([params['global_rot'], params['body_pose']] + [params[name] for name, _, _ in parts], 1)
+    rot0 = ops.decode_rot6d(raw.detach()).contiguous()
+    anchor = rot0 if pose_anchor is None else \
+        torch.as_tensor(pose_anchor, dtype=torch.float32, device=device).reshape(B, width, 3, 3).contiguous()
+    pw, bw, ew = float(pose_prior_weight), float(betas_weight), float(expression_weight)
+    jw = None if jw is None else jw.to(device)
+    last = 'camera' if intr is None else 'transl'
+    if method == 'lm':
+        return _fit_keypoints_2d_expressive_lm(body_model, x, w, params, parts, rot0, anchor, int(iterations), sigma,
+                                               pw, jw, bw, ew, ne, intr)
+    from .autograd import Rot6dFunction
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        pr = {name: Rot6dFunction.apply(params[name]) for name, _, _ in parts}
+        expr = params.get('expression')
+        out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr, pr, expr)
+        rot = torch.cat([grot, bpose] + list(pr.values()), 1)
+        per_body = _kp2d_expressive_loss(out['proj_joints'], x, w, sigma, pw, jw, rot, anchor, bw, params['betas'],
+                                         ew, expr)
+        return per_body, out, rot
+
+    per_body, out, rot = _adam(list(params.values()), lr, iterations, loss_fn)
+    if intr is not None:
+        per_body = _depth_rule(per_body, out['joints'][:], w)
+    res = {k: v.detach() for k, v in params.items()}
+    res.update(global_rot_mat=rot[:, :1], body_pose_mat=rot[:, 1:22], full_pose_mat=rot, keypoints=out['joints'][:],
+               proj_joints=out['proj_joints'], loss=per_body)
+    return res
+
+
+def _kp2d_expressive_loss(proj, target, w, sigma, pw, jw, rot, anchor, bw, betas, ew, expr):
+    """_kp2d_loss over all n_rot rotations, the prior per joint with jw (n_rot,) (joint 0 unread), plus ew |psi|^2."""
+    per_body = _kp2d_loss(proj, target, w, sigma, pw if jw is None else 0.0, rot, anchor, bw, betas)
+    if jw is not None:
+        d = (rot[:, 1:] - anchor[:, 1:]).pow(2).sum((2, 3))                  # (B, n_rot - 1)
+        per_body = per_body + (0.5 * jw[1:] * d).sum(1)
+    if expr is not None and ew > 0:
+        per_body = per_body + ew * expr.pow(2).sum(1)
+    return per_body
+
+
+def _fit_keypoints_2d_expressive_lm(body_model, x, w, params, parts, rot0, anchor, iterations, sigma, pw, jw, bw, ew,
+                                    ne, intr):
+    from . import ops
+    device = x.device
+    packed = body_model.packed(device)
+    B, K = x.shape[0], x.shape[1]
+    nb, n_rot = params['betas'].shape[1], rot0.shape[1]
+    last = 'camera' if intr is None else 'transl'
+    expr0 = params['expression'] if ne else torch.zeros(B, 0, device=device)
+    trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'expression': expr0.clone().contiguous(),
+             last: params[last].contiguous()}
+    state = _kp_lm_state(B, K, n_rot, nb, last, device, ne=ne)
+    pose_anchor = anchor if (pw > 0 or jw is not None) else None
+    if B > 0:
+        for it in range(iterations + 1):
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'],
+                                                    expr=trial['expression'] if ne else None)
+            ops.fit_lm_keypoints_2d_expressive_step(state, trial, x, w, sigma, pw, bw, ew, LM_UP, LM_DOWN, it == 0,
+                                                    tkp, tjac, pose_anchor=pose_anchor, joint_weights=jw,
+                                                    intrinsics=intr)
+    rot = state['rot']
+    expr = state['expression'] if ne else None
+    pr = {name: rot[:, j:j + n] for name, j, n in parts}
+    with torch.no_grad():
+        out = _forward_2d(body_model, rot[:, :1], rot[:, 1:22], state['betas'], state[last], intr, pr, expr)
+        per_body = _kp2d_expressive_loss(out['proj_joints'], x, w, sigma, pw, jw, rot, anchor, bw, state['betas'], ew,
+                                         expr)
+        if intr is not None:
+            per_body = _depth_rule(per_body, out['joints'][:], w)
+    res = _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+    raw = rot[..., :2].reshape(B, 6 * n_rot)
+    res['body_pose'], res['body_pose_mat'] = raw[:, 6:132].contiguous(), rot[:, 1:22]
+    for name, j, n in parts:
+        res[name] = raw[:, 6 * j:6 * (j + n)].contiguous()
+    res['full_pose_mat'] = rot
+    if ne:
+        res['expression'] = state['expression']
+    return res
 
 
 class _SortedBatch:
@@ -1283,6 +1458,12 @@ def main(argv=None):
                         'perspective_start and the npz center / scale, or takes transl')
     p.add_argument('--robust-sigma', dest='robust_sigma', type=float, default=None)
     p.add_argument('--pose-prior-weight', dest='pose_prior_weight', type=float, default=0.0)
+    p.add_argument('--pose-width', dest='pose_width', type=int, default=22, choices=POSE_WIDTHS,
+                   help='with --keypoints-2d: rotations fitted, 22 (body), 25 (+ jaw and eyes) or 55 (+ hands)')
+    p.add_argument('--fit-expression', dest='fit_expression', action='store_true',
+                   help='with --keypoints-2d: also fit the facial expression')
+    p.add_argument('--expression-weight', dest='expression_weight', type=float, default=0.0,
+                   help='with --fit-expression: the regulariser weight on |expression|^2')
     p.add_argument('--share-pose', dest='share_pose', action='store_true',
                    help="with --keypoints-2d and a `groups` array: the images of a group are simultaneous views of "
                         "one posed body and share its body pose as well as its shape")
@@ -1299,6 +1480,10 @@ def main(argv=None):
     p.add_argument('--smooth-transl', dest='smooth_transl', type=float, default=0.0,
                    help='with --sequence: the weight of |transl_{t+1} - transl_t|^2 between consecutive frames')
     a = p.parse_args(argv)
+    if (a.pose_width != 22 or a.fit_expression or a.expression_weight) and \
+            (not a.keypoints_2d or a.calibrated or a.sequence):
+        raise SystemExit('--pose-width, --fit-expression and --expression-weight need --keypoints-2d and are not '
+                         'supported with --calibrated or --sequence')
 
     from . import synth
     from .body_measurements import BodyMeasurements
@@ -1360,7 +1545,7 @@ def _main_keypoints_2d(a, model, bm, targets):
     if a.calibrated and not (persp and 'cam_rot' in d.files and 'cam_transl' in d.files):
         raise SystemExit('--calibrated needs focal_length, cam_rot and cam_transl in --keypoints-2d')
     if a.init and not a.calibrated:
-        init = _load_init(a.init, x.shape[0], ('camera', 'transl'))
+        init = _load_init(a.init, x.shape[0], ('camera', 'transl', 'expression') + tuple(n for n, _ in POSE_PARTS))
         if persp and 'transl' not in init and 'camera' in init:
             if not ('center' in d.files and 'scale' in d.files):
                 raise SystemExit('--init with a camera and a focal_length needs center and scale in --keypoints-2d')
@@ -1374,7 +1559,9 @@ def _main_keypoints_2d(a, model, bm, targets):
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
                                    circumference_derivative=a.circumference_derivative, groups=groups,
-                                   share_pose=a.share_pose, focal_length=focal, principal_point=pp)
+                                   share_pose=a.share_pose, focal_length=focal, principal_point=pp,
+                                   pose_width=a.pose_width, fit_expression=a.fit_expression,
+                                   expression_weight=a.expression_weight)
     _save_result(a.output, res, {'bodies': int(x.shape[0])}, groups=groups)
 
 

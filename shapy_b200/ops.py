@@ -452,10 +452,14 @@ def fit_lm_step(state, targets, weights, betas_weight, lambda_up, lambda_down, f
                                       stream_ptr()), 'fit_lm_step')
 
 
-def smplx_keypoint_jacobian(model: SmplxModel, betas, rot, transl=None):
+def smplx_keypoint_jacobian(model: SmplxModel, betas, rot, transl=None, expr=None):
     """The keypoints (B, K, 3) of smplx_forward (its joints, expression zero) plus transl, and their Jacobian
     (B, 3K, P), P = 3 n_rot + NB + 3, with respect to [delta_j (right-multiplied tangents R_j Exp(delta_j)) | betas |
-    transl], in one launch (include/shapy_b200.h, shapy_smplx_keypoint_jacobian).  Returns (keypoints, jac)."""
+    transl], in one launch (include/shapy_b200.h, shapy_smplx_keypoint_jacobian).  Returns (keypoints, jac).
+    expr (B, NE): the keypoints at that expression and NE more columns after betas, P = 3 n_rot + NB + NE + 3
+    (shapy_smplx_keypoint_jacobian_expr); None is the launch above."""
+    if expr is not None:
+        return _smplx_keypoint_jacobian_expr(model, betas, rot, transl, expr)
     betas = _cuda_f32(betas, 'betas')
     rot = _cuda_f32(rot, 'rot')
     B, n_rot = rot.shape[0], rot.shape[1]
@@ -473,6 +477,27 @@ def smplx_keypoint_jacobian(model: SmplxModel, betas, rot, transl=None):
     with torch.cuda.device(dev):
         check(lib().shapy_smplx_keypoint_jacobian(model.handle, ptr(betas), ptr(rot), n_rot, ptr(transl), B, ptr(kp),
                                                   ptr(jac), stream_ptr()), 'smplx_keypoint_jacobian')
+    return kp, jac
+
+
+def _smplx_keypoint_jacobian_expr(model, betas, rot, transl, expr):
+    betas, rot, expr = _cuda_f32(betas, 'betas'), _cuda_f32(rot, 'rot'), _cuda_f32(expr, 'expression')
+    B, n_rot = rot.shape[0], rot.shape[1]
+    if rot.shape[2:] != (3, 3) or betas.shape != (B, model.NB) or expr.shape != (B, model.NE):
+        raise RuntimeError(f'rot must be (B, n_rot, 3, 3), betas ({B}, {model.NB}) and expr ({B}, {model.NE}), got '
+                           f'{tuple(rot.shape)}, {tuple(betas.shape)} and {tuple(expr.shape)}')
+    transl = None if transl is None else _cuda_f32(transl, 'transl')
+    if transl is not None and transl.shape != (B, 3):
+        raise RuntimeError(f'transl must be ({B}, 3), got {tuple(transl.shape)}')
+    dev = betas.device
+    kp = torch.empty(B, model.K, 3, dtype=torch.float32, device=dev)
+    jac = torch.empty(B, 3 * model.K, 3 * n_rot + model.NB + model.NE + 3, dtype=torch.float32, device=dev)
+    if B == 0:
+        return kp, jac
+    with torch.cuda.device(dev):
+        check(lib().shapy_smplx_keypoint_jacobian_expr(model.handle, ptr(betas), ptr(expr), ptr(rot), n_rot, ptr(transl),
+                                                       B, ptr(kp), ptr(jac), stream_ptr()),
+              'smplx_keypoint_jacobian')
     return kp, jac
 
 
@@ -627,6 +652,66 @@ def fit_lm_keypoints_2d_perspective_measurements_step(state, trial, targets, wei
     _fit_lm_kp2d('fit_lm_keypoints_2d_perspective_measurements_step', state, trial, targets, weights, robust_sigma,
                  pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
                  pose_anchor, (meas_targets, meas_weights, trial_meas, trial_meas_jac), intrinsics)
+
+
+def fit_lm_keypoints_2d_expressive_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight,
+                                        expression_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                                        pose_anchor=None, joint_weights=None, intrinsics=None):
+    """One Levenberg-Marquardt step per body of the 2D fit of the whole SMPL-X body (include/shapy_b200.h,
+    shapy_fit_lm_keypoints_2d_expressive_step, or _perspective_ with intrinsics), in place: any pose width and the
+    facial expression, P = 3 n_rot + NB + NE + 3 <= 200.  state: fit_lm_keypoints_2d_step's (or the perspective step's,
+    with 'transl') plus 'expression' (B, NE), NE >= 0; trial: {'rot', 'betas', 'expression', 'camera' or 'transl'};
+    trial_keypoints / trial_jac from smplx_keypoint_jacobian(..., expr=trial['expression']) without transl (without
+    expr when NE = 0).  joint_weights: None (pose_prior_weight on every joint j >= 1) or (n_rot,) float32 per-joint
+    pose-prior weights, joint 0 zero (a CPU tensor is checked, then copied; a CUDA tensor is used as it is, its joint 0
+    not read).  expression_weight: the regulariser expression_weight |psi|^2.  With NE = 0 and joint_weights None the
+    step is fit_lm_keypoints_2d_step's (or the perspective step's) bit for bit."""
+    what = 'fit_lm_keypoints_2d_expressive_step'
+    B, n_rot = trial['rot'].shape[:2]
+    nb, ne, K = trial['betas'].shape[1], trial['expression'].shape[1], targets.shape[1]
+    last = 'camera' if intrinsics is None else 'transl'
+    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
+                                pose_anchor)
+    if not expression_weight >= 0:
+        raise ValueError(f'{what}: expression_weight must be >= 0')
+    if joint_weights is not None:
+        jw = torch.as_tensor(joint_weights, dtype=torch.float32)
+        if jw.shape != (n_rot,):
+            raise RuntimeError(f'{what}: joint_weights must be ({n_rot},)')
+        if jw.device.type == 'cpu':
+            if not (float(jw[0]) == 0 and bool((jw >= 0).all())):
+                raise ValueError(f'{what}: joint_weights must be >= 0 with joint 0 zero')
+            jw = jw.to(trial['rot'].device)
+        if pose_anchor is None:
+            raise ValueError(f'{what}: joint_weights need pose_anchor')
+        joint_weights = jw.contiguous()
+    extra = [t for t in (pose_anchor, joint_weights, intrinsics) if t is not None]
+    ts = [state[k] for k in ('rot', 'betas', 'expression', last, 'keypoints', 'jac', 'loss', 'lambda')] + \
+        [trial[k] for k in ('rot', 'betas', 'expression', last)] + [targets, weights, trial_keypoints, trial_jac] + extra
+    _check_step_tensors(what, ts, 'the state, trial, targets, weights, anchor, joint weights and intrinsics',
+                        state['accepted'])
+    P = 3 * n_rot + nb + ne + 3
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2) or \
+            state['expression'].shape != (B, ne):
+        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}), targets ({B}, {K}, 2) and '
+                           f'expression ({B}, {ne})')
+    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
+        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
+    if intrinsics is not None and intrinsics.shape != (B, 3):
+        raise RuntimeError(f'{what}: intrinsics must be ({B}, 3)')
+    if B == 0:
+        return
+    e = (lambda t: ptr(t) if ne else None)  # noqa: E731
+    head = [B, K, n_rot, nb, ne, ptr(targets), ptr(weights)] + ([ptr(intrinsics)] if intrinsics is not None else []) + \
+        [ptr(pose_anchor), ptr(joint_weights), sigma, float(pose_prior_weight), float(betas_weight),
+         float(expression_weight), float(lambda_up), float(lambda_down), int(bool(first))]
+    persp = '' if intrinsics is None else '_perspective'
+    with torch.cuda.device(trial['rot'].device):
+        check(getattr(lib(), f'shapy_fit_lm_keypoints_2d_expressive{persp}_step')(
+            *head, ptr(state['rot']), ptr(state['betas']), e(state['expression']),
+            *[ptr(state[k]) for k in (last, 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
+            ptr(trial['rot']), ptr(trial['betas']), e(trial['expression']), ptr(trial[last]), ptr(trial_keypoints),
+            ptr(trial_jac), stream_ptr()), what)
 
 
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:
