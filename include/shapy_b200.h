@@ -381,8 +381,8 @@ int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
  * hands, jaw and eyes be held apart from the body.  The expression columns are damped by expression_weight + lambda,
  * the betas columns by betas_weight + lambda, the rest by lambda; g gains expression_weight psi.  expression /
  * trial_expression (B,ne) may be null when ne = 0.  With ne = 0 and joint_weights null every output equals
- * shapy_fit_lm_keypoints_2d_step's bit for bit (at n_rot, nb where that step runs).  One CTA per body, the packed
- * normal matrix in shared memory (one CTA per SM).  Other rules and errors as shapy_fit_lm_keypoints_2d_step. */
+ * shapy_fit_lm_keypoints_2d_step's bit for bit (at n_rot, nb where that step runs).  Other rules and errors as
+ * shapy_fit_lm_keypoints_2d_step. */
 int shapy_fit_lm_keypoints_2d_expressive_step(
     int batch, int num_keypoints, int n_rot, int nb, int ne, const float *targets, const float *weights,
     const float *pose_anchor, const float *joint_weights, float robust_sigma, float pose_prior_weight,

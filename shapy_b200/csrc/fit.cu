@@ -177,11 +177,12 @@ __global__ void __launch_bounds__(128) lm_step_kernel(LmArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The Levenberg-Marquardt steps of the keypoint fits, one CTA per body: pose and shape with a translation against 3D
-// keypoints (lm_kp_step_kernel), or with a weak-perspective camera against 2D keypoints (lm_kp2d_step_kernel).
+// The Levenberg-Marquardt steps of the keypoint fits: pose and shape with a translation against 3D keypoints
+// (lm_kp_step_kernel, one CTA per body), or with a camera against 2D keypoints (the grouped, calibrated and sequence
+// kernels below; the single-image 2D step keeps its normal matrix in shared memory instead, lm_kp2d_step_kernel).
 // Parameters [delta_j (3 n_rot) | beta (NB) | the last 3: t or c], P =3 n_rot + NB + 3, R_j(delta) = R_j Exp(delta_j);
 // the caller evaluates the trial with shapy_smplx_keypoint_jacobian.  The kernels differ in their loss and in the rows
-// they stage; the phases below, each by the whole CTA on the shared-memory state, are the same code in both:
+// they stage; the phases below, each by the whole CTA on the shared-memory state, are the same code in all:
 //   2. lm_kp_take_trial: an accepted trial becomes the state;
 //   3. lm_kp_pairs, lm_kp_add_rows, lm_kp_damp: the P x P normal matrix J^T W J and g = J^T W r from staged rows, the
 //      lower triangle spread over the threads' registers, then lambda by lm_step_kernel's policy on the diagonal;
@@ -545,40 +546,8 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp_step_kernel(LmKpArgs a, Lm
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The step of the fit of pose, shape and weak-perspective camera to 2D keypoints (shapy_fit_lm_keypoints_2d_step).
-// The camera c = (c0, c1, c2) takes the columns of transl (which a weak-perspective camera cannot see along z, and
-// which duplicates c1, c2 in x and y).  With s = softplus(c0) (threshold 20, as the forward) the projection is
-// p_k = s (kp_k,xy + (c1, c2)), and per body, in fp64, left to right:
-//   L = sum_{w_k > 0} w_k rho(|p_k - x_k|^2)  (k order)
-//     + 1/2 pose_w sum_{j >= 1} |R_j - R0_j|_F^2  (j order, row-major entries; when pose_w > 0)
-//     + betas_w |beta|^2  (l order; when betas_w > 0)
-// rho(e) = e at sigma = inf, else e q with q = sigma^2 / (sigma^2 + e) (Geman-McClure).  Rows of the normal equations,
-// accumulated into A and g in this order:
-//   keypoint rows 2k + c (c = 0 x, 1 y), weight w_k q_k^2 (the IRLS weight rho'(e_k), 1 at sigma = inf) at the state,
-//     residual p_kc - x_kc, Jacobian staged from the 3D keypoint Jacobian (transl columns skipped): s J_{3k+c} on the
-//     rotation and betas columns, ds/dc0 (kp_kc + c_{1+c}) on c0, s on c_{1+c};
-//   pose-prior rows (R_j - R0_j)_e, weight pose_w / 2, Jacobian R_j [e_a]x in column 3 j + a (d(R Exp d) = R [d]x),
-//     j = 1 .. n_rot - 1, e in row-major order: they only reach the 3 x 3 diagonal block of joint j;
-//   then g += betas_w beta on the betas columns.
-// The first lambda is 1e-3 max(diag A, 1e-6) of the keypoint rows alone; the diagonal then gets betas_w + lambda on the
-// betas columns and lambda elsewhere.
-//
-// MEAS (shapy_fit_lm_keypoints_2d_measurements_step) stacks the five virtual measurements under those rows, as the 3D
-// MEAS step does: L gains sum_{u_m > 0} u_m (t_m - meas_m)^2 (m order, summed on its own) between the pose prior and
-// the betas prior, and the measurement rows (plain least squares: rho applies to keypoints only) go into the betas
-// block of A and g after the pose-prior rows and before betas_w beta.  They do not count for the first lambda.  With
-// every measurement weight <= 0 the loss gains an exact 0 and no row is added, so the step equals the 2D step bit for
-// bit, for any sigma, pose prior and betas_w.
-//
-// The perspective 2D step (shapy_fit_lm_keypoints_2d_perspective_step, and _measurements_ with MEAS) is the same kernel
-// with the projection of a pinhole camera of known intrinsics (f, px, py) per body: camera frame x right, y down, z
-// forward, the last three parameters the translation t.  With Y_k = kp_k + t (fp64),
-//   p_k = f (Y_k,x / Y_k,z, Y_k,y / Y_k,z) + (px, py);
-// the loss is the 2D step's term for term with this p_k, and keypoint row 2k + c is (f / Y_z) (J_{3k+c} - (Y_c / Y_z)
-// J_{3k+2}) on every column, J_t = I on the t columns.  Depth rule: a trial with a weighted keypoint at Y_z <= 0 or
-// non-finite, or a body whose f is not finite and > 0, has loss +inf: it is rejected, and a start that breaks the rule
-// reports NaN and does not move.  The pose-prior and measurement rows, lambda, damping, solve and next trial (t +
-// delta_t) are the 2D step's.
+// The pieces of the 2D keypoint steps: the single-image step (lm_kp2d_step_kernel, which states the loss and the rows)
+// and the grouped, shared-pose, calibrated and sequence steps build on them.
 struct LmKp2dArgs {                     // what the 2D step takes beside LmKpArgs (targets (B, K, 2), last = camera)
   const float *anchor;                  // (B, n_rot, 3, 3), or null without a pose prior
   float sigma, pose_w, betas_w;
@@ -590,9 +559,6 @@ struct LmKp2dArgs {                     // what the 2D step takes beside LmKpArg
 struct LmKp2dPerspArgs : LmKp2dArgs {
   const float *intr;                    // (B, 3): f, px, py
 };
-
-template <bool PERSP>
-using Kp2dX = std::conditional_t<PERSP, LmKp2dPerspArgs, LmKp2dArgs>;
 
 // One body's pinhole camera at a point of the fit: focal length, principal point and translation t, in fp64
 struct PerspCam {
@@ -843,85 +809,10 @@ __device__ __forceinline__ void lm_kp2d_prior_rows(const LmKp2dArgs &x2, int o, 
   }
 }
 
-template <bool MEAS, bool PERSP = false>
-__global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2d_step_kernel(LmKpArgs a, Kp2dX<PERSP> x2) {
-  extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
-  __shared__ double Js[kLmKpRows][kLmKpMaxP], WJs[kLmKpRows][kLmKpMaxP];   // staged rows J_r and w J_r
-  __shared__ double rs[kLmKpRows], ws[kLmKpRows], y[kLmKpMaxP], dg[kLmKpMaxP];
-  __shared__ double lt_s;
-  __shared__ int ok_s;
-  const int b = blockIdx.x, t = threadIdx.x, P = a.P, K = a.K, R3 = 3 * a.K, nb = a.nb, nr9 = 9 * a.n_rot;
-  const int o = 3 * a.n_rot, oc = o + nb;     // first betas and first camera column
-  const float *tg = a.targets + (size_t)b * 2 * K, *wt = a.weights + (size_t)b * K;
-  const float *anc = x2.anchor ? x2.anchor + (size_t)b * nr9 : nullptr;
-  const bool robust = isfinite(x2.sigma);
-  const double s2 = (double)x2.sigma * (double)x2.sigma;
-  const float lcur = a.loss[b];
-  // 1. trial loss
-  if (t == 0) {
-    double L;
-    if constexpr (PERSP) {
-      const PerspCam tc = persp_cam(x2.intr + (size_t)b * 3, a.tlast + (size_t)b * 3);
-      L = lm_kp2d_trial_loss<true>(a, x2, b, tg, wt, anc, robust, s2, &tc);
-    } else {
-      L = lm_kp2d_trial_loss(a, x2, b, tg, wt, anc, robust, s2);
-    }
-    if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
-    if (x2.betas_w > 0.f) {
-      const float *tb = a.tbetas + (size_t)b * nb;
-      double reg = 0.0;
-      for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
-      L += (double)x2.betas_w * reg;
-    }
-    lt_s = L;
-  }
-  __syncthreads();
-  // 2. accept or reject
-  const double lt = lt_s;
-  const bool accept = lm_accept(a.first, lt, lcur);
-  const float lnew = lm_loss(accept, lt, lcur);
-  const float *J = (accept ? a.tjac : a.jac) + (size_t)b * R3 * P;
-  const float *M = (accept ? a.tkp : a.kp) + (size_t)b * R3;
-  const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
-  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
-  const float *Cst = (accept ? a.tlast : a.last) + (size_t)b * 3;
-  if (accept) {
-    lm_kp_take_trial(a, b, lnew);
-    if constexpr (MEAS) lm_meas_take_trial(x2.mb, b, nb);
-  }
-  double s, ds;
-  softplus_d((double)Cst[0], s, ds);
-  const double cxy[2] = {(double)Cst[1], (double)Cst[2]};
-  // 3. normal equations
-  int pr[kLmKpPairs], pc[kLmKpPairs];
-  double acc[kLmKpPairs], g = 0.0;
-  lm_kp_pairs(P, pr, pc, acc);
-  if constexpr (PERSP) {
-    const PerspCam sc = persp_cam(x2.intr + (size_t)b * 3, Cst);
-    lm_kp2d_keypoint_rows<false, true>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc,
-                                       g, &sc);
-  } else {
-    lm_kp2d_keypoint_rows<false>(K, P, J, M, tg, wt, s, ds, cxy, robust, s2, oc, Js, WJs, ws, rs, pr, pc, acc, g);
-  }
-#pragma unroll
-  for (int i = 0; i < kLmKpPairs; ++i)
-    if (pr[i] >= 0 && pr[i] == pc[i]) dg[pr[i]] = acc[i];     // the diagonal of the keypoint rows: the first lambda
-  lm_kp2d_prior_rows(x2, o, Rst, anc, pr, pc, acc, g);
-  if constexpr (MEAS)
-    lm_meas_add_rows(x2.mb, b, nb, o, (accept ? x2.mb.tmeas : x2.mb.meas) + (size_t)b * 5,
-                     (accept ? x2.mb.tjac : x2.mb.jac) + (size_t)b * 5 * nb, Js, WJs, ws, rs, pr, pc, acc, g);
-  if (x2.betas_w > 0.f && t >= o && t < oc) g += (double)x2.betas_w * (double)Bst[t - o];
-  lm_kp_damp(a, b, accept, lnew, A, y, pr, pc, acc, g, dg, 1, o, oc, x2.betas_w, ok_s);
-  // 4. Cholesky and the two triangular solves
-  lm_kp_solve(A, y, P, P, ok_s);
-  // 5. next trial (ok is uniform: every thread reads it after the last barrier); a failed step keeps the state
-  lm_kp_next_trial(a, b, y, ok_s);
-}
-
-// What the four keypoint entry points share, `fn` naming the one called: the checks of the arguments in `a` (its P is
-// set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors` its own scalars and the
-// sentence that states their and the lambda factors' ranges; then the launch, one CTA of kLmKpThreads per body with
-// P x P doubles of dynamic shared memory
+// What the 3D, grouped, calibrated and sequence keypoint entry points share, `fn` naming the one called: the checks of
+// the arguments in `a` (its P is set here), with `extra_ok` the entry point's own pointers and `factors_ok` / `factors`
+// its own scalars and the sentence that states their and the lambda factors' ranges; then the launch, one CTA of
+// kLmKpThreads per body with P x P doubles of dynamic shared memory
 inline int check_lm_kp(const char *fn, int batch, LmKpArgs &a, bool extra_ok, bool factors_ok, const char *factors) {
   SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
                     a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && extra_ok,
@@ -1841,43 +1732,68 @@ int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The wide 2D step (shapy_fit_lm_keypoints_2d_expressive_step, and _perspective_ with PERSP): the single-image 2D step
-// for the hands, jaw, eyes and facial expression of SMPL-X.  Parameters [delta_j (3 n_rot) | beta (nb) | psi (ne) | c
-// or t], P = 3 n_rot + nb + ne + 3 <= kLmWideMaxP, the columns of shapy_smplx_keypoint_jacobian_expr (of
-// shapy_smplx_keypoint_jacobian with ne = 0).  Per body, in fp64, left to right:
-//   L = the 2D step's keypoint term and pose prior (robust, the PERSP depth rule)
-//     + betas_w |beta|^2 (l order; when betas_w > 0) + expr_w |psi|^2 (l order; when expr_w > 0).
-// The pose prior is the 2D step's with the scalar pose_w; with per-joint weights w_j (joint_w, n_rot entries, joint 0
-// not read) it is sum_{j >= 1, w_j > 0} (1/2 w_j) |R_j - R0_j|_F^2 in j order, and joint j's rows have weight w_j / 2.
-// Rows, first lambda and policy are the 2D step's; the diagonal gets betas_w + lambda on the betas columns, expr_w +
-// lambda on the expression columns and lambda elsewhere, and g gains expr_w psi after betas_w beta.
+// The single-image 2D step: pose, shape and camera of each body against its 2D keypoints, one body per CTA
+// (shapy_fit_lm_keypoints_2d_step; _perspective_ with PERSP; _measurements_ with MEAS; the _expressive_ entries add the
+// pose parts past the body and the facial expression of SMPL-X).  Parameters [delta_j (3 n_rot) | beta (nb) | psi (ne)
+// | c or t], P = 3 n_rot + nb + ne + 3, the columns of shapy_smplx_keypoint_jacobian_expr (of
+// shapy_smplx_keypoint_jacobian with ne = 0); the 22-joint entries have ne = 0 and P <= kLmKpMaxP, the expressive ones
+// P <= kLmKp2dMaxP.  The weak-perspective camera c = (c0, c1, c2) takes the columns of transl (which a weak-perspective
+// camera cannot see along z, and which duplicates c1, c2 in x and y).  With s = softplus(c0) (threshold 20, as the
+// forward) the projection is p_k = s (kp_k,xy + (c1, c2)), and per body, in fp64, left to right:
+//   L = sum_{w_k > 0} w_k rho(|p_k - x_k|^2)  (k order)
+//     + 1/2 pose_w sum_{j >= 1} |R_j - R0_j|_F^2  (j order, row-major entries; when pose_w > 0)
+//     + sum_{u_m > 0} u_m (t_m - meas_m)^2  (MEAS; m order, summed on its own)
+//     + betas_w |beta|^2  (l order; when betas_w > 0) + expr_w |psi|^2  (l order; when expr_w > 0)
+// rho(e) = e at sigma = inf, else e q with q = sigma^2 / (sigma^2 + e) (Geman-McClure).  With per-joint weights w_j
+// (joint_w, n_rot entries, joint 0 not read) the pose prior is sum_{j >= 1, w_j > 0} (1/2 w_j) |R_j - R0_j|_F^2 in j
+// order.  Rows of the normal equations, accumulated into A and g in this order:
+//   keypoint rows 2k + c (c = 0 x, 1 y), weight w_k q_k^2 (the IRLS weight rho'(e_k), 1 at sigma = inf) at the state,
+//     residual p_kc - x_kc, Jacobian staged from the 3D keypoint Jacobian (transl columns skipped): s J_{3k+c} on the
+//     rotation, betas and expression columns, ds/dc0 (kp_kc + c_{1+c}) on c0, s on c_{1+c};
+//   pose-prior rows (R_j - R0_j)_e, weight pose_w / 2 (w_j / 2), Jacobian R_j [e_a]x in column 3 j + a
+//     (d(R Exp d) = R [d]x), j = 1 .. n_rot - 1, e in row-major order: they only reach the 3 x 3 diagonal block of
+//     joint j;
+//   MEAS: the five measurement rows (plain least squares: rho applies to keypoints only), residual meas_m - t_m, into
+//     the betas block of A and g;
+//   then g += betas_w beta on the betas columns and expr_w psi on the expression columns.
+// The first lambda is 1e-3 max(diag A, 1e-6) of the keypoint rows alone; the diagonal then gets betas_w + lambda on the
+// betas columns, expr_w + lambda on the expression columns and lambda elsewhere.  With every measurement weight <= 0
+// the loss gains an exact 0 and no row is added, so the MEAS step equals the step without, bit for bit, for any sigma,
+// pose prior and betas_w.
 //
-// One CTA of kLmKpThreads per body, one CTA per SM: the packed fp64 lower triangle of A (P (P + 1) / 2 entries, 160.8
-// KB at P = 200) and kLmKpRows staged rows of width P live in dynamic shared memory.  Each staged chunk is added into
-// the shared triangle (thread t owns the packed entries t + 256 i, each entry summing its rows in row order, as the
-// registers of the 2D step do), then the pose-prior rows into the joints' diagonal blocks.  The Cholesky is the 2D
-// step's right-looking one on the packed triangle, one warp per trailing row; the triangular solves keep its order.
-// With ne = 0, n_rot = 22 and scalar weights every operation is the 2D step's in the same order: the results are its
-// bits.
-constexpr int kLmWideMaxP = 200;
+// PERSP: the projection of a pinhole camera of known intrinsics (f, px, py) per body: camera frame x right, y down, z
+// forward, the last three parameters the translation t.  With Y_k = kp_k + t (fp64),
+//   p_k = f (Y_k,x / Y_k,z, Y_k,y / Y_k,z) + (px, py);
+// the loss is the weak-perspective one term for term with this p_k, and keypoint row 2k + c is (f / Y_z) (J_{3k+c} -
+// (Y_c / Y_z) J_{3k+2}) on every column, J_t = I on the t columns.  Depth rule: a trial with a weighted keypoint at
+// Y_z <= 0 or non-finite, or a body whose f is not finite and > 0, has loss +inf: it is rejected, and a start that
+// breaks the rule reports NaN and does not move.  The other rows, lambda, damping, solve and next trial (t + delta_t)
+// are the weak-perspective step's.
+//
+// One CTA of kLmKpThreads per body: the packed fp64 lower triangle of A (P (P + 1) / 2 entries, 160.8 KB at P = 200)
+// and kLmKpRows staged rows of width P live in dynamic shared memory.  Each staged chunk is added into the shared
+// triangle (thread t owns the packed entries t + 256 i, each entry summing its rows in row order), then the pose-prior
+// and measurement rows into their blocks.  The Cholesky is right-looking (column j scaled, then the trailing triangle
+// updated, one warp per trailing row), then L z = -g and L^T delta = z.
+constexpr int kLmKp2dMaxP = 200;
 
-struct LmKp2dWideArgs : LmKp2dPerspArgs {   // intr is null in the weak-perspective step
+struct LmKp2dStepArgs : LmKp2dPerspArgs {   // intr is null in the weak-perspective step
   const float *joint_w;                     // (n_rot) per-joint pose-prior weights, or null: pose_w for every joint
   float expr_w;
   int ne;
   float *expr, *texpr;                      // state and trial expression (B, ne); null when ne = 0
 };
 
-// dynamic shared memory of the wide step, in doubles: the packed triangle, Js and WJs (kLmKpRows x P each), y, z, dg,
+// dynamic shared memory of the 2D step, in doubles: the packed triangle, Js and WJs (kLmKpRows x P each), y, z, dg,
 // the scaled column and the Cholesky diagonal (P each), ws and rs (kLmKpRows each)
-__host__ __device__ inline size_t lm_wide_smem_doubles(int P) {
+__host__ __device__ inline size_t lm_kp2d_smem_doubles(int P) {
   return (size_t)P * (P + 1) / 2 + (size_t)2 * kLmKpRows * P + (size_t)5 * P + 2 * kLmKpRows;
 }
 
 // the packed position of the lower-triangle entry (i, k), k <= i
 __device__ __forceinline__ int tri(int i, int k) { return i * (i + 1) / 2 + k; }
 
-// the packed entry p of thread t's first entry: row r, column c (c <= r)
+// the row r and column c (c <= r) of the packed entry p
 __device__ __forceinline__ void tri_rc(int p, int &r, int &c) {
   r = (int)((sqrt(8.0 * p + 1.0) - 1.0) * 0.5);
   while ((r + 1) * (r + 2) / 2 <= p) ++r;
@@ -1885,8 +1801,8 @@ __device__ __forceinline__ void tri_rc(int p, int &r, int &c) {
   c = p - r * (r + 1) / 2;
 }
 
-template <bool PERSP>
-__global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs a, LmKp2dWideArgs x2) {
+template <bool MEAS, bool PERSP>
+__global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2d_step_kernel(LmKpArgs a, LmKp2dStepArgs x2) {
   extern __shared__ double smem[];
   __shared__ double lt_s, lam_s;
   __shared__ int ok_s;
@@ -1923,6 +1839,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs
         L += (0.5 * (double)x2.joint_w[j]) * q;
       }
     }
+    if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
     if (x2.betas_w > 0.f) {
       const float *tb = a.tbetas + (size_t)b * nb;
       double reg = 0.0;
@@ -1952,6 +1869,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs
   if (accept) {
     lm_kp_take_trial(a, b, lnew);
     for (int i = t; i < ne; i += blockDim.x) x2.expr[(size_t)b * ne + i] = x2.texpr[(size_t)b * ne + i];
+    if constexpr (MEAS) lm_meas_take_trial(x2.mb, b, nb);
   }
   double s, ds;
   softplus_d((double)Cst[0], s, ds);
@@ -2027,6 +1945,28 @@ __global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs
         for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
       }
     }
+  }
+  if constexpr (MEAS) {
+    // the five measurement rows at the state (values Mm, Jacobian Jm (5, nb)) into the betas block, in m order, each
+    // entry (o + r, o + c) by one thread; a dropped term's row is never read: it may be NaN
+    const float *Mm = (accept ? x2.mb.tmeas : x2.mb.meas) + (size_t)b * 5;
+    const float *Jm = (accept ? x2.mb.tjac : x2.mb.jac) + (size_t)b * 5 * nb;
+    const float *mt = x2.mb.targets + (size_t)b * 5, *mw = x2.mb.weights + (size_t)b * 5;
+    for (int q = t; q < nb * (nb + 1) / 2; q += blockDim.x) {
+      int r, c;
+      tri_rc(q, r, c);
+      double acc = A[tri(o + r, o + c)];
+      for (int m = 0; m < 5; ++m) {
+        const double w = mw[m];
+        if (w > 0.0) acc += (w * (double)Jm[m * nb + r]) * (double)Jm[m * nb + c];
+      }
+      A[tri(o + r, o + c)] = acc;
+    }
+    if (t >= o && t < oe)
+      for (int m = 0; m < 5; ++m) {
+        const double w = mw[m];
+        if (w > 0.0) g += (w * (double)Jm[m * nb + t - o]) * ((double)Mm[m] - (double)mt[m]);
+      }
   }
   if (x2.betas_w > 0.f && t >= o && t < oe) g += (double)x2.betas_w * (double)Bst[t - o];
   if (x2.expr_w > 0.f && t >= oe && t < oc) g += (double)x2.expr_w * (double)Est[t - oe];
@@ -2109,29 +2049,45 @@ __global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2dw_step_kernel(LmKpArgs
   }
 }
 
-// The wide entries' checks (check_lm_kp's with P counting the expression columns and kLmWideMaxP) and the launch
-int run_lm_kp2dw(const char *fn, int batch, LmKpArgs a, LmKp2dWideArgs x, bool persp, void *stream) {
+// The 2D step's arguments without per-joint weights and expression: what the 22-joint entries pass
+inline LmKp2dStepArgs kp2d_args(const float *anchor, float sigma, float pose_w, float betas_w, const LmMeasArgs &mb,
+                                const float *intr) {
+  LmKp2dStepArgs x{};
+  static_cast<LmKp2dPerspArgs &>(x) = LmKp2dPerspArgs{{anchor, sigma, pose_w, betas_w, mb}, intr};
+  return x;
+}
+
+// The single-image 2D entries' checks and the launch: `persp` and `meas` say which pointers the entry takes, and
+// max_p bounds P, kLmKpMaxP for the 22-joint entries (which take no expression and state none in their messages) and
+// kLmKp2dMaxP for the expressive ones
+int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool persp, bool meas, int max_p,
+                void *stream) {
+  const LmMeasArgs &mb = x.mb;
   const bool ptrs = (x.anchor || !(x.pose_w > 0.f || x.joint_w)) && (x.ne == 0 || (x.expr && x.texpr)) &&
-                    (!persp || x.intr);
+                    (!persp || x.intr) &&
+                    (!meas || (mb.targets && mb.weights && mb.meas && mb.jac && mb.tmeas && mb.tjac));
   SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
                     a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && ptrs,
                 "%s: null argument", fn);
-  SHAPY_REQUIRE(batch >= 0 && a.K >= 1 && a.n_rot >= 1 && a.n_rot <= 64 && a.nb >= 1 && x.ne >= 0,
-                "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas, %d expression)", fn, batch, a.K, a.n_rot,
-                a.nb, x.ne);
+  const bool sizes = batch >= 0 && a.K >= 1 && a.n_rot >= 1 && a.n_rot <= 64 && a.nb >= 1 && x.ne >= 0;
+  if (max_p == kLmKpMaxP)
+    SHAPY_REQUIRE(sizes, "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas)", fn, batch, a.K, a.n_rot, a.nb);
+  SHAPY_REQUIRE(sizes, "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas, %d expression)", fn, batch, a.K,
+                a.n_rot, a.nb, x.ne);
   SHAPY_REQUIRE(a.up >= 1.f && a.down >= 1.f && x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f &&
                     x.expr_w >= 0.f,
                 "%s: robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
                 "lambda_down >= 1",
                 fn);
   a.P = 3 * a.n_rot + a.nb + x.ne + 3;
-  if (a.P > kLmWideMaxP) {
-    set_error("%s: %d parameters, at most %d are supported", fn, a.P, kLmWideMaxP);
+  if (a.P > max_p) {
+    set_error("%s: %d parameters, at most %d are supported", fn, a.P, max_p);
     return SHAPY_ERR_UNSUPPORTED;
   }
   if (batch == 0) return SHAPY_OK;
-  const size_t smem = lm_wide_smem_doubles(a.P) * sizeof(double);
-  auto kernel = persp ? lm_kp2dw_step_kernel<true> : lm_kp2dw_step_kernel<false>;
+  const size_t smem = lm_kp2d_smem_doubles(a.P) * sizeof(double);
+  auto kernel = meas ? (persp ? lm_kp2d_step_kernel<true, true> : lm_kp2d_step_kernel<true, false>)
+                     : (persp ? lm_kp2d_step_kernel<false, true> : lm_kp2d_step_kernel<false, false>);
   SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
   kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
   SHAPY_LAUNCH_CHECK();
@@ -2199,13 +2155,9 @@ extern "C" int shapy_fit_lm_keypoints_2d_step(int batch, int num_keypoints, int 
                                               void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
-  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
-  return run_lm_kp("shapy_fit_lm_keypoints_2d_step", lm_kp2d_step_kernel<false>, batch, a, x,
-                   pose_anchor || !(pose_prior_weight > 0.f),
-                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
-                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                   "lambda_down >= 1",
-                   stream);
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_step", batch, a,
+                     kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}, nullptr), false,
+                     false, kLmKpMaxP, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_measurements_step(
@@ -2217,15 +2169,10 @@ extern "C" int shapy_fit_lm_keypoints_2d_measurements_step(
     const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
-  LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
-               LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
-  return run_lm_kp("shapy_fit_lm_keypoints_2d_measurements_step", lm_kp2d_step_kernel<true>, batch, a, x,
-                   (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas && meas_jac &&
-                       trial_meas && trial_meas_jac,
-                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
-                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                   "lambda_down >= 1",
-                   stream);
+  const LmMeasArgs m{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac};
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_measurements_step", batch, a,
+                     kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, m, nullptr), false, true,
+                     kLmKpMaxP, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_perspective_step(
@@ -2236,13 +2183,9 @@ extern "C" int shapy_fit_lm_keypoints_2d_perspective_step(
     float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
-  LmKp2dPerspArgs x{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics};
-  return run_lm_kp("shapy_fit_lm_keypoints_2d_perspective_step", lm_kp2d_step_kernel<false, true>, batch, a, x,
-                   intrinsics && (pose_anchor || !(pose_prior_weight > 0.f)),
-                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
-                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                   "lambda_down >= 1",
-                   stream);
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_perspective_step", batch, a,
+                     kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}, intrinsics),
+                     true, false, kLmKpMaxP, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
@@ -2254,17 +2197,10 @@ extern "C" int shapy_fit_lm_keypoints_2d_perspective_measurements_step(
     const float *trial_jac, const float *trial_meas, const float *trial_meas_jac, void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
-  LmKp2dPerspArgs x{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
-                     LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}},
-                    intrinsics};
-  return run_lm_kp("shapy_fit_lm_keypoints_2d_perspective_measurements_step", lm_kp2d_step_kernel<true, true>, batch,
-                   a, x,
-                   intrinsics && (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
-                       meas_jac && trial_meas && trial_meas_jac,
-                   robust_sigma > 0.f && pose_prior_weight >= 0.f && betas_weight >= 0.f,
-                   "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                   "lambda_down >= 1",
-                   stream);
+  const LmMeasArgs m{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac};
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_perspective_measurements_step", batch, a,
+                     kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, m, intrinsics), true, true,
+                     kLmKpMaxP, stream);
 }
 
 extern "C" size_t shapy_fit_lm_groups_workspace_bytes(int batch, int num_groups, int n_rot, int nb) {
@@ -2413,15 +2349,13 @@ extern "C" int shapy_fit_lm_keypoints_2d_expressive_step(
     const float *trial_keypoints, const float *trial_jac, void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, camera,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
-  LmKp2dWideArgs x{};
-  static_cast<LmKp2dPerspArgs &>(x) =
-      LmKp2dPerspArgs{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, nullptr};
+  LmKp2dStepArgs x = kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}, nullptr);
   x.joint_w = joint_weights;
   x.expr_w = expression_weight;
   x.ne = ne;
   x.expr = expression;
   x.texpr = trial_expression;
-  return run_lm_kp2dw("shapy_fit_lm_keypoints_2d_expressive_step", batch, a, x, false, stream);
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_expressive_step", batch, a, x, false, false, kLmKp2dMaxP, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_expressive_perspective_step(
@@ -2433,13 +2367,12 @@ extern "C" int shapy_fit_lm_keypoints_2d_expressive_perspective_step(
     float *trial_transl, const float *trial_keypoints, const float *trial_jac, void *stream) {
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
-  LmKp2dWideArgs x{};
-  static_cast<LmKp2dPerspArgs &>(x) =
-      LmKp2dPerspArgs{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics};
+  LmKp2dStepArgs x = kp2d_args(pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}, intrinsics);
   x.joint_w = joint_weights;
   x.expr_w = expression_weight;
   x.ne = ne;
   x.expr = expression;
   x.texpr = trial_expression;
-  return run_lm_kp2dw("shapy_fit_lm_keypoints_2d_expressive_perspective_step", batch, a, x, true, stream);
+  return run_lm_kp2d("shapy_fit_lm_keypoints_2d_expressive_perspective_step", batch, a, x, true, false, kLmKp2dMaxP,
+                     stream);
 }

@@ -512,9 +512,11 @@ def keypoint_jacobian_2d(body_model, rot, betas, camera):
     return {'proj_joints': s[:, None, None] * xy, 'jacobian': j2.view(B, 2 * K, P)}
 
 
-def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas):
+def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas, joint_w=None, expr_w=0.0, expr=None):
     """The 2D fit's per-body loss: sum_{w_k > 0} w_k rho(|proj_k - target_k|^2) + pose_w / 2 sum_{j >= 1}
-    |R_j - R0_j|_F^2 + betas_w |betas|^2, rho(e) = e (sigma None) or sigma^2 e / (sigma^2 + e)."""
+    |R_j - R0_j|_F^2 + betas_w |betas|^2, rho(e) = e (sigma None) or sigma^2 e / (sigma^2 + e), over all n_rot
+    rotations of rot.  joint_w (n_rot,) (joint 0 unread; with pose_w 0): the pose prior per joint,
+    sum_{j >= 1} joint_w_j / 2 |R_j - R0_j|_F^2; expr (B, NE): expr_w |psi|^2 as well."""
     keep = w > 0
     diff = torch.where(keep[..., None], proj - torch.where(keep[..., None], target, torch.zeros_like(target)),
                        torch.zeros_like(proj))
@@ -526,6 +528,11 @@ def _kp2d_loss(proj, target, w, sigma, pose_w, rot, anchor, betas_w, betas):
         per_body = per_body + 0.5 * pose_w * (rot[:, 1:] - anchor[:, 1:]).pow(2).sum((1, 2, 3))
     if betas_w > 0:
         per_body = per_body + betas_w * betas.pow(2).sum(1)
+    if joint_w is not None:
+        d = (rot[:, 1:] - anchor[:, 1:]).pow(2).sum((2, 3))                  # (B, n_rot - 1)
+        per_body = per_body + (0.5 * joint_w[1:] * d).sum(1)
+    if expr is not None and expr_w > 0:
+        per_body = per_body + expr_w * expr.pow(2).sum(1)
     return per_body
 
 
@@ -550,14 +557,17 @@ def _keypoints_2d(fn, keypoints2d, weights, device):
     return x, w.expand(B, K).contiguous()
 
 
-def _start_rotations(params, pose_anchor, n):
-    """The decoded starting rotations (n, 22, 3, 3) of a fit's raw 6D params, and the pose prior's anchor:
-    pose_anchor as (n, 22, 3, 3), by default the start."""
+def _start_rotations(params, pose_anchor, n, parts=()):
+    """The decoded starting rotations (n, n_rot, 3, 3) of a fit's raw 6D params, the global rotation, the body and the
+    pose parts `parts` of _parts_in (n_rot = 22 without), and the pose prior's anchor: pose_anchor as
+    (n, n_rot, 3, 3), by default the start."""
     from . import ops
-    rot0 = ops.decode_rot6d(torch.cat([params['global_rot'], params['body_pose']], 1).detach()).contiguous()
+    raw = torch.cat([params['global_rot'], params['body_pose']] + [params[name] for name, _, _ in parts], 1)
+    rot0 = ops.decode_rot6d(raw.detach()).contiguous()
     if pose_anchor is None:
         return rot0, rot0
-    return rot0, torch.as_tensor(pose_anchor, dtype=torch.float32, device=rot0.device).reshape(n, 22, 3, 3).contiguous()
+    return rot0, torch.as_tensor(pose_anchor, dtype=torch.float32, device=rot0.device).reshape(
+        n, rot0.shape[1], 3, 3).contiguous()
 
 
 def _forward_2d(body_model, grot, bpose, betas, last, intr, parts=None, expression=None):
@@ -751,96 +761,159 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     when fitted, 'expression'.  A part is only as determined as its keypoints make it: one without a weighted keypoint
     (the eyes: the OpenPose pupils are dropped on load) is held by its prior alone, and without a prior it stays where
     it starts.  groups, share_pose and measurements are not supported on the wide path."""
-    if pose_width != 22 or fit_expression:
-        return _fit_keypoints_2d_expressive(body_model, keypoints2d, weights, init, method, iterations, robust_sigma,
-                                            pose_prior_weight, betas_weight, pose_anchor, lr, measurements, groups,
-                                            share_pose, focal_length, principal_point, pose_width, fit_expression,
-                                            expression_weight)
-    iterations, sigma = _check_kp_fit('fit_body_to_keypoints_2d', body_model, method, iterations,
-                                      circumference_derivative, body_measurements, measurements, robust_sigma,
-                                      pose_prior_weight, betas_weight)
-    if share_pose and groups is None:
-        raise ValueError('fit_body_to_keypoints_2d: share_pose needs groups')
-    if focal_length is not None and (groups is not None or share_pose):
-        raise ValueError('fit_body_to_keypoints_2d: groups and share_pose are not supported with a focal_length')
-    if focal_length is not None and principal_point is None:
-        raise ValueError('fit_body_to_keypoints_2d: focal_length needs principal_point')
+    fn = 'fit_body_to_keypoints_2d'
+    wide = pose_width != 22 or fit_expression
+    ne, jw = 0, None
+    if wide:
+        if pose_width not in POSE_WIDTHS:
+            raise ValueError(f'{fn}: pose_width must be one of {POSE_WIDTHS}, got {pose_width}')
+        if groups is not None or share_pose or measurements is not None:
+            raise ValueError(f'{fn}: groups, share_pose and measurements are not supported with a pose_width past 22 '
+                             f'or fit_expression')
+        if focal_length is not None and principal_point is None:
+            raise ValueError(f'{fn}: focal_length needs principal_point')
+        if not expression_weight >= 0:
+            raise ValueError(f'{fn}: expression_weight must be >= 0')
+        if np.ndim(pose_prior_weight) > 0:
+            jw = torch.as_tensor(pose_prior_weight, dtype=torch.float32).detach().cpu().reshape(-1)
+            if jw.shape != (pose_width,) or float(jw[0]) != 0 or not bool((jw >= 0).all()):
+                raise ValueError(f'{fn}: per-joint pose_prior_weight must be ({pose_width},), >= 0, with joint 0 zero')
+            pose_prior_weight = 0.0
+        ne, nb = body_model.num_expression_coeffs if fit_expression else 0, body_model.num_betas
+        if method == 'lm' and 3 * pose_width + nb + ne + 3 > LM_WIDE_MAX_PARAMS:
+            raise ValueError(f"{fn}(method='lm'): {pose_width} rotations, {nb} betas, {ne} expression coefficients "
+                             f'and the translation or camera are {3 * pose_width + nb + ne + 3} parameters, at most '
+                             f'{LM_WIDE_MAX_PARAMS} are supported')
+        # _check_kp_fit's checks; its parameter bound is the 22-joint step's, so it sees the Adam method
+        iterations, sigma = _check_kp_fit(fn, body_model, 'adam' if method == 'lm' else method,
+                                          50 if method == 'lm' and iterations is None else iterations,
+                                          robust_sigma=robust_sigma, pose_prior_weight=pose_prior_weight,
+                                          betas_weight=betas_weight)
+    else:
+        iterations, sigma = _check_kp_fit(fn, body_model, method, iterations, circumference_derivative,
+                                          body_measurements, measurements, robust_sigma, pose_prior_weight,
+                                          betas_weight)
+        if share_pose and groups is None:
+            raise ValueError(f'{fn}: share_pose needs groups')
+        if focal_length is not None and (groups is not None or share_pose):
+            raise ValueError(f'{fn}: groups and share_pose are not supported with a focal_length')
+        if focal_length is not None and principal_point is None:
+            raise ValueError(f'{fn}: focal_length needs principal_point')
     from .autograd import Rot6dFunction
-    device = body_model.shapedirs.device
-    x, w = _keypoints_2d('fit_body_to_keypoints_2d', keypoints2d, weights, device)
+    device, nb = body_model.shapedirs.device, body_model.num_betas
+    x, w = _keypoints_2d(fn, keypoints2d, weights, device)
     B = x.shape[0]
     intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
-    params = _init_2d(init, B, body_model.num_betas, device, method, x, w, intr)
-    rot0, anchor = _start_rotations(params, None if share_pose else pose_anchor, B)
+    params = _init_2d(init, B, nb, device, method, x, w, intr)
+    parts = _parts_in(pose_width)
+    raw_init = _raw_init(init)
+    ident = torch.zeros(6, device=device) if parts else None     # IDENT6, filled on the device
+    if parts:
+        ident[0::3].fill_(1.0)
+    for name, _, n in parts:        # the pose parts past the body, by default at the identity
+        t = raw_init.get(name)
+        t = ident.repeat(B, n) if t is None else \
+            torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, 6 * n)
+        params[name] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    if fit_expression:
+        t = raw_init.get('expression')
+        t = torch.zeros(B, ne, device=device) if t is None else \
+            torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, ne)
+        params['expression'] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
+    rot0, anchor = _start_rotations(params, None if share_pose else pose_anchor, B, parts)
     if share_pose:          # per group: its shape is checked once the groups are known
         anchor = None if pose_anchor is None else torch.as_tensor(pose_anchor, dtype=torch.float32, device=device)
-    pw, bw = float(pose_prior_weight), float(betas_weight)
+    pw, bw, ew = float(pose_prior_weight), float(betas_weight), float(expression_weight)
     if groups is not None:
         return _fit_keypoints_2d_groups(body_model, x, w, params, rot0, anchor, method, int(iterations), sigma, pw, bw,
                                         lr, groups, body_measurements, measurements, measurement_weights,
                                         circumference_derivative, bool(share_pose))
+    jw = None if jw is None else jw.to(device)
     mt = _measurement_term(measurements, measurement_weights, B, device, body_measurements, circumference_derivative)
     last = 'camera' if intr is None else 'transl'
     if method == 'lm':
-        return _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, int(iterations), sigma, pw, bw, mt, intr)
+        return _fit_keypoints_2d_lm(body_model, x, w, params, parts, rot0, anchor, int(iterations), sigma, pw, jw, bw,
+                                    ew, ne, mt, intr, wide)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
         bpose = Rot6dFunction.apply(params['body_pose'])
-        out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr)
-        rot = torch.cat([grot, bpose], 1)
-        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'])
+        pr = {name: Rot6dFunction.apply(params[name]) for name, _, _ in parts}
+        expr = params.get('expression')
+        out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr, pr, expr)
+        rot = torch.cat([grot, bpose] + list(pr.values()), 1)
+        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'], jw, ew, expr)
         meas = None
         if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
             meas = mt.measure(body_model, params['betas'])
             per_body = per_body + mt.loss(meas, params['betas'], 0.0)
-        return per_body, out, grot, bpose, meas
+        return per_body, out, rot, meas
 
-    per_body, out, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
+    per_body, out, rot, meas = _adam(list(params.values()), lr, iterations, loss_fn)
     if intr is not None:
         per_body = _depth_rule(per_body, out['joints'][:], w)
-    return _adam_result(params, grot, bpose, meas, keypoints=out['joints'][:], proj_joints=out['proj_joints'],
-                        loss=per_body)
+    wide_out = {'full_pose_mat': rot} if wide else {}
+    return _adam_result(params, rot[:, :1], rot[:, 1:22], meas, **wide_out, keypoints=out['joints'][:],
+                        proj_joints=out['proj_joints'], loss=per_body)
 
 
-def _fit_keypoints_2d_lm(body_model, x, w, params, rot0, anchor, iterations, sigma, pw, bw, mt, intr):
+def _fit_keypoints_2d_lm(body_model, x, w, params, parts, rot0, anchor, iterations, sigma, pw, jw, bw, ew, ne, mt, intr,
+                         wide):
+    """The LM loop of fit_body_to_keypoints_2d: per iteration the keypoint Jacobian of the trial, with measurements
+    their trial values and Jacobian, and one single-image 2D step; `wide` runs the expressive step."""
     from . import ops
     device = x.device
     packed = body_model.packed(device)
     B, K = x.shape[0], x.shape[1]
-    nb = params['betas'].shape[1]
+    nb, n_rot = params['betas'].shape[1], rot0.shape[1]
     last = 'camera' if intr is None else 'transl'
     trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), last: params[last].contiguous()}
-    state = _kp_lm_state(B, K, 22, nb, last, device)
-    if intr is None:
-        step, mstep = ops.fit_lm_keypoints_2d_step, ops.fit_lm_keypoints_2d_measurements_step
-    else:       # the perspective steps, the intrinsics bound after the weights
-        step = lambda st, tr, x, w, *r, **kw: ops.fit_lm_keypoints_2d_perspective_step(st, tr, x, w, intr, *r, **kw)  # noqa: E731
-        mstep = lambda st, tr, x, w, *r, **kw: ops.fit_lm_keypoints_2d_perspective_measurements_step(  # noqa: E731
-            st, tr, x, w, intr, *r, **kw)
-    pose_anchor = anchor if pw > 0 else None
-    if mt is not None:
+    state = _kp_lm_state(B, K, n_rot, nb, last, device, ne=ne if wide else None)
+    kw = {'pose_anchor': anchor if pw > 0 or jw is not None else None}
+    if intr is not None:
+        kw['intrinsics'] = intr
+    if wide:
+        step = ops.fit_lm_keypoints_2d_expressive_step
+        trial['expression'] = (params['expression'] if ne else torch.zeros(B, 0, device=device)).clone().contiguous()
+        kw.update(expression_weight=ew, joint_weights=jw)
+    elif mt is None:
+        step = ops.fit_lm_keypoints_2d_step if intr is None else ops.fit_lm_keypoints_2d_perspective_step
+    else:
+        step = ops.fit_lm_keypoints_2d_measurements_step if intr is None else \
+            ops.fit_lm_keypoints_2d_perspective_measurements_step
         state.update(mt.state(nb, device))
     if B > 0:
         if mt is not None:
             mt.prime(body_model)
         for it in range(iterations + 1):
-            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'])
-            if mt is None:
-                step(state, trial, x, w, sigma, pw, bw, LM_UP, LM_DOWN, it == 0, tkp, tjac, pose_anchor=pose_anchor)
-            else:
+            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'],
+                                                    expr=trial['expression'] if ne else None)
+            if mt is not None:
                 tm, tmj = mt.trial(packed, body_model, trial['betas'])
-                mstep(state, trial, x, w, sigma, pw, bw, mt.tgt, mt.wt, LM_UP, LM_DOWN, it == 0, tkp, tjac, tm, tmj,
-                      pose_anchor=pose_anchor)
+                kw.update(meas_targets=mt.tgt, meas_weights=mt.wt, trial_meas=tm, trial_meas_jac=tmj)
+            step(state, trial, x, w, robust_sigma=sigma, pose_prior_weight=pw, betas_weight=bw, lambda_up=LM_UP,
+                 lambda_down=LM_DOWN, first=it == 0, trial_keypoints=tkp, trial_jac=tjac, **kw)
     rot = state['rot']
+    expr = state['expression'] if ne else None
+    pr = {name: rot[:, j:j + n] for name, j, n in parts}
     with torch.no_grad():
-        out = _forward_2d(body_model, rot[:, :1], rot[:, 1:], state['betas'], state[last], intr)
-        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'])
+        out = _forward_2d(body_model, rot[:, :1], rot[:, 1:22], state['betas'], state[last], intr, pr, expr)
+        per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, state['betas'], jw, ew, expr)
         if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
             per_body = per_body + mt.loss(state['meas'], state['betas'], 0.0)
         if intr is not None:
             per_body = _depth_rule(per_body, out['joints'][:], w)
-    return _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+    res = _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
+    if parts:
+        raw = rot[..., :2].reshape(B, 6 * n_rot)
+        res['body_pose'], res['body_pose_mat'] = raw[:, 6:132].contiguous(), rot[:, 1:22]
+        for name, j, n in parts:
+            res[name] = raw[:, 6 * j:6 * (j + n)].contiguous()
+    if wide:
+        res['full_pose_mat'] = rot
+    if ne:
+        res['expression'] = state['expression']
+    return res
 
 
 # the pose parts past the body in SMPL-X's joint order (SMPLX.forward's names) and their joint counts
@@ -859,139 +932,6 @@ def _parts_in(width):
         out.append((name, j, n))
         j += n
     return out
-
-
-def _fit_keypoints_2d_expressive(body_model, keypoints2d, weights, init, method, iterations, robust_sigma,
-                                 pose_prior_weight, betas_weight, pose_anchor, lr, measurements, groups, share_pose,
-                                 focal_length, principal_point, width, fit_expression, expression_weight):
-    """fit_body_to_keypoints_2d's wide path: the pose parts inside `width` and, with fit_expression, the expression."""
-    fn = 'fit_body_to_keypoints_2d'
-    if width not in POSE_WIDTHS:
-        raise ValueError(f'{fn}: pose_width must be one of {POSE_WIDTHS}, got {width}')
-    if groups is not None or share_pose or measurements is not None:
-        raise ValueError(f'{fn}: groups, share_pose and measurements are not supported with a pose_width past 22 or '
-                         f'fit_expression')
-    if focal_length is not None and principal_point is None:
-        raise ValueError(f'{fn}: focal_length needs principal_point')
-    if not expression_weight >= 0:
-        raise ValueError(f'{fn}: expression_weight must be >= 0')
-    jw = None
-    if np.ndim(pose_prior_weight) > 0:
-        jw = torch.as_tensor(pose_prior_weight, dtype=torch.float32).detach().cpu().reshape(-1)
-        if jw.shape != (width,) or float(jw[0]) != 0 or not bool((jw >= 0).all()):
-            raise ValueError(f'{fn}: per-joint pose_prior_weight must be ({width},), >= 0, with joint 0 zero')
-        pose_prior_weight = 0.0
-    ne = body_model.num_expression_coeffs if fit_expression else 0
-    nb = body_model.num_betas
-    if method == 'lm' and 3 * width + nb + ne + 3 > LM_WIDE_MAX_PARAMS:
-        raise ValueError(f"{fn}(method='lm'): {width} rotations, {nb} betas, {ne} expression coefficients and the "
-                         f'translation or camera are {3 * width + nb + ne + 3} parameters, at most '
-                         f'{LM_WIDE_MAX_PARAMS} are supported')
-    # _check_kp_fit's checks; its parameter bound is the 22-joint step's, so it sees the Adam method
-    iterations, sigma = _check_kp_fit(fn, body_model, 'adam' if method == 'lm' else method,
-                                      50 if method == 'lm' and iterations is None else iterations,
-                                      robust_sigma=robust_sigma, pose_prior_weight=pose_prior_weight,
-                                      betas_weight=betas_weight)
-    device = body_model.shapedirs.device
-    x, w = _keypoints_2d(fn, keypoints2d, weights, device)
-    B = x.shape[0]
-    intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
-    params = _init_2d(init, B, nb, device, method, x, w, intr)
-    init = _raw_init(init)
-    ident = torch.zeros(6, device=device)      # IDENT6, filled on the device
-    ident[0::3].fill_(1.0)
-    parts = _parts_in(width)
-    for name, _, n in parts:
-        t = init.get(name)
-        t = ident.repeat(B, n) if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, 6 * n)
-        params[name] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
-    if fit_expression:
-        t = init.get('expression')
-        t = torch.zeros(B, ne, device=device) if t is None else \
-            torch.as_tensor(t, dtype=torch.float32, device=device).reshape(B, ne)
-        params['expression'] = t.detach().clone().contiguous().requires_grad_(method == 'adam')
-    from . import ops
-    raw = torch.cat([params['global_rot'], params['body_pose']] + [params[name] for name, _, _ in parts], 1)
-    rot0 = ops.decode_rot6d(raw.detach()).contiguous()
-    anchor = rot0 if pose_anchor is None else \
-        torch.as_tensor(pose_anchor, dtype=torch.float32, device=device).reshape(B, width, 3, 3).contiguous()
-    pw, bw, ew = float(pose_prior_weight), float(betas_weight), float(expression_weight)
-    jw = None if jw is None else jw.to(device)
-    last = 'camera' if intr is None else 'transl'
-    if method == 'lm':
-        return _fit_keypoints_2d_expressive_lm(body_model, x, w, params, parts, rot0, anchor, int(iterations), sigma,
-                                               pw, jw, bw, ew, ne, intr)
-    from .autograd import Rot6dFunction
-
-    def loss_fn():
-        grot = Rot6dFunction.apply(params['global_rot'])
-        bpose = Rot6dFunction.apply(params['body_pose'])
-        pr = {name: Rot6dFunction.apply(params[name]) for name, _, _ in parts}
-        expr = params.get('expression')
-        out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr, pr, expr)
-        rot = torch.cat([grot, bpose] + list(pr.values()), 1)
-        per_body = _kp2d_expressive_loss(out['proj_joints'], x, w, sigma, pw, jw, rot, anchor, bw, params['betas'],
-                                         ew, expr)
-        return per_body, out, rot
-
-    per_body, out, rot = _adam(list(params.values()), lr, iterations, loss_fn)
-    if intr is not None:
-        per_body = _depth_rule(per_body, out['joints'][:], w)
-    res = {k: v.detach() for k, v in params.items()}
-    res.update(global_rot_mat=rot[:, :1], body_pose_mat=rot[:, 1:22], full_pose_mat=rot, keypoints=out['joints'][:],
-               proj_joints=out['proj_joints'], loss=per_body)
-    return res
-
-
-def _kp2d_expressive_loss(proj, target, w, sigma, pw, jw, rot, anchor, bw, betas, ew, expr):
-    """_kp2d_loss over all n_rot rotations, the prior per joint with jw (n_rot,) (joint 0 unread), plus ew |psi|^2."""
-    per_body = _kp2d_loss(proj, target, w, sigma, pw if jw is None else 0.0, rot, anchor, bw, betas)
-    if jw is not None:
-        d = (rot[:, 1:] - anchor[:, 1:]).pow(2).sum((2, 3))                  # (B, n_rot - 1)
-        per_body = per_body + (0.5 * jw[1:] * d).sum(1)
-    if expr is not None and ew > 0:
-        per_body = per_body + ew * expr.pow(2).sum(1)
-    return per_body
-
-
-def _fit_keypoints_2d_expressive_lm(body_model, x, w, params, parts, rot0, anchor, iterations, sigma, pw, jw, bw, ew,
-                                    ne, intr):
-    from . import ops
-    device = x.device
-    packed = body_model.packed(device)
-    B, K = x.shape[0], x.shape[1]
-    nb, n_rot = params['betas'].shape[1], rot0.shape[1]
-    last = 'camera' if intr is None else 'transl'
-    expr0 = params['expression'] if ne else torch.zeros(B, 0, device=device)
-    trial = {'rot': rot0.clone(), 'betas': params['betas'].contiguous(), 'expression': expr0.clone().contiguous(),
-             last: params[last].contiguous()}
-    state = _kp_lm_state(B, K, n_rot, nb, last, device, ne=ne)
-    pose_anchor = anchor if (pw > 0 or jw is not None) else None
-    if B > 0:
-        for it in range(iterations + 1):
-            tkp, tjac = ops.smplx_keypoint_jacobian(packed, trial['betas'], trial['rot'],
-                                                    expr=trial['expression'] if ne else None)
-            ops.fit_lm_keypoints_2d_expressive_step(state, trial, x, w, sigma, pw, bw, ew, LM_UP, LM_DOWN, it == 0,
-                                                    tkp, tjac, pose_anchor=pose_anchor, joint_weights=jw,
-                                                    intrinsics=intr)
-    rot = state['rot']
-    expr = state['expression'] if ne else None
-    pr = {name: rot[:, j:j + n] for name, j, n in parts}
-    with torch.no_grad():
-        out = _forward_2d(body_model, rot[:, :1], rot[:, 1:22], state['betas'], state[last], intr, pr, expr)
-        per_body = _kp2d_expressive_loss(out['proj_joints'], x, w, sigma, pw, jw, rot, anchor, bw, state['betas'], ew,
-                                         expr)
-        if intr is not None:
-            per_body = _depth_rule(per_body, out['joints'][:], w)
-    res = _kp_lm_result(state, last, keypoints=out['joints'][:], proj_joints=out['proj_joints'], loss=per_body)
-    raw = rot[..., :2].reshape(B, 6 * n_rot)
-    res['body_pose'], res['body_pose_mat'] = raw[:, 6:132].contiguous(), rot[:, 1:22]
-    for name, j, n in parts:
-        res[name] = raw[:, 6 * j:6 * (j + n)].contiguous()
-    res['full_pose_mat'] = rot
-    if ne:
-        res['expression'] = state['expression']
-    return res
 
 
 class _SortedBatch:

@@ -557,25 +557,48 @@ def fit_lm_keypoints_measurements_step(state, trial, targets, weights, meas_targ
 
 
 def _fit_lm_kp2d(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
-                 lambda_down, first, trial_keypoints, trial_jac, pose_anchor, meas=None, intrinsics=None):
-    """What the 2D keypoint steps share: the checks and the call, `meas` None or the measurement block
+                 lambda_down, first, trial_keypoints, trial_jac, pose_anchor, meas=None, intrinsics=None,
+                 expressive=None):
+    """What the single-image 2D keypoint steps share: the checks and the call, `meas` None or the measurement block
     (meas_targets, meas_weights, trial_meas, trial_meas_jac) of the stacked step, `intrinsics` None (the
-    weak-perspective camera 'camera') or (B, 3) (the perspective steps, translation 'transl')."""
+    weak-perspective camera 'camera') or (B, 3) (the perspective steps, translation 'transl'), `expressive` None (the
+    22-joint steps) or (expression_weight, joint_weights) of the expressive steps, whose state and trial hold
+    'expression'."""
     B, n_rot = trial['rot'].shape[:2]
     nb, K = trial['betas'].shape[1], targets.shape[1]
+    ex = expressive is not None
+    opt = lambda cond, *xs: list(xs) if cond else []  # noqa: E731
+    ne = trial['expression'].shape[1] if ex else 0
     last = 'camera' if intrinsics is None else 'transl'
     sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
                                 pose_anchor)
-    anchor = [] if pose_anchor is None else [pose_anchor]
-    intr = [] if intrinsics is None else [intrinsics]
-    mstate = [] if meas is None else [state['meas'], state['meas_jac']]
-    ts = [state[k] for k in ('rot', 'betas', last, 'keypoints', 'jac', 'loss', 'lambda')] + mstate + \
-        [trial[k] for k in ('rot', 'betas', last)] + [targets, weights, trial_keypoints, trial_jac] + anchor + intr + \
-        list(meas or ())
-    _check_step_tensors(what, ts, 'the state, trial, targets, weights, anchor and intrinsics', state['accepted'])
-    P = 3 * n_rot + nb + 3
-    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2):
-        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}) and targets ({B}, {K}, 2)')
+    expression_weight, joint_weights = expressive or (0.0, None)
+    if not expression_weight >= 0:
+        raise ValueError(f'{what}: expression_weight must be >= 0')
+    if joint_weights is not None:
+        jw = torch.as_tensor(joint_weights, dtype=torch.float32)
+        if jw.shape != (n_rot,):
+            raise RuntimeError(f'{what}: joint_weights must be ({n_rot},)')
+        if jw.device.type == 'cpu':
+            if not (float(jw[0]) == 0 and bool((jw >= 0).all())):
+                raise ValueError(f'{what}: joint_weights must be >= 0 with joint 0 zero')
+            jw = jw.to(trial['rot'].device)
+        if pose_anchor is None:
+            raise ValueError(f'{what}: joint_weights need pose_anchor')
+        joint_weights = jw.contiguous()
+    ekeys, mkeys = opt(ex, 'expression'), opt(meas is not None, 'meas', 'meas_jac')
+    params = ['rot', 'betas'] + ekeys + [last]
+    ts = [state[k] for k in params + ['keypoints', 'jac', 'loss', 'lambda'] + mkeys] + [trial[k] for k in params] + \
+        [targets, weights, trial_keypoints, trial_jac] + \
+        [t for t in (pose_anchor, joint_weights, intrinsics) if t is not None] + list(meas or ())
+    names = 'anchor, joint weights and intrinsics' if ex else 'anchor and intrinsics'
+    _check_step_tensors(what, ts, f'the state, trial, targets, weights, {names}', state['accepted'])
+    P = 3 * n_rot + nb + ne + 3
+    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2) or \
+            (ex and state['expression'].shape != (B, ne)):
+        shapes = f'jac must be ({B}, {3 * K}, {P}), weights ({B}, {K})'
+        shapes += f', targets ({B}, {K}, 2) and expression ({B}, {ne})' if ex else f' and targets ({B}, {K}, 2)'
+        raise RuntimeError(f'{what}: {shapes}')
     if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
     if intrinsics is not None and intrinsics.shape != (B, 3):
@@ -585,23 +608,20 @@ def _fit_lm_kp2d(what, state, trial, targets, weights, robust_sigma, pose_prior_
                            f'({B}, 5)')
     if B == 0:
         return
-    head = [B, K, n_rot, nb, ptr(targets), ptr(weights)] + [ptr(t) for t in intr] + \
-        [ptr(pose_anchor), sigma, float(pose_prior_weight), float(betas_weight)]
-    lam = [float(lambda_up), float(lambda_down), int(bool(first))]
-    tr = [ptr(trial['rot']), ptr(trial['betas']), ptr(trial[last]), ptr(trial_keypoints), ptr(trial_jac)]
-    persp = '' if intrinsics is None else '_perspective'
+    # the arguments in the order of the entry's C signature; a zero-width expression is passed as null
+    e = (lambda t: ptr(t) if ne else None)  # noqa: E731
+    head = [B, K, n_rot, nb, *opt(ex, ne), ptr(targets), ptr(weights), *opt(intrinsics is not None, ptr(intrinsics)),
+            ptr(pose_anchor), *opt(ex, ptr(joint_weights)), sigma, float(pose_prior_weight), float(betas_weight),
+            *opt(ex, float(expression_weight)), *map(ptr, (meas or ())[:2]), float(lambda_up), float(lambda_down),
+            int(bool(first))]
+    st = [ptr(state['rot']), ptr(state['betas'])] + [e(state[k]) for k in ekeys] + \
+        [ptr(state[k]) for k in (last, 'keypoints', 'jac', *mkeys, 'loss', 'lambda', 'accepted')]
+    tr = [ptr(trial['rot']), ptr(trial['betas'])] + [e(trial[k]) for k in ekeys] + \
+        [ptr(trial[last]), ptr(trial_keypoints), ptr(trial_jac), *map(ptr, (meas or ())[2:])]
+    entry = 'shapy_fit_lm_keypoints_2d' + '_expressive' * ex + '_perspective' * (intrinsics is not None) + \
+        '_measurements' * (meas is not None) + '_step'
     with torch.cuda.device(trial['rot'].device):
-        if meas is None:
-            check(getattr(lib(), f'shapy_fit_lm_keypoints_2d{persp}_step')(
-                *head, *lam,
-                *[ptr(state[k]) for k in ('rot', 'betas', last, 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
-                *tr, stream_ptr()), what)
-        else:
-            check(getattr(lib(), f'shapy_fit_lm_keypoints_2d{persp}_measurements_step')(
-                *head, ptr(meas[0]), ptr(meas[1]), *lam,
-                *[ptr(state[k]) for k in ('rot', 'betas', last, 'keypoints', 'jac', 'meas', 'meas_jac', 'loss',
-                                          'lambda', 'accepted')],
-                *tr, ptr(meas[2]), ptr(meas[3]), stream_ptr()), what)
+        check(getattr(lib(), entry)(*head, *st, *tr, stream_ptr()), what)
 
 
 def fit_lm_keypoints_2d_step(state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
@@ -666,52 +686,9 @@ def fit_lm_keypoints_2d_expressive_step(state, trial, targets, weights, robust_s
     pose-prior weights, joint 0 zero (a CPU tensor is checked, then copied; a CUDA tensor is used as it is, its joint 0
     not read).  expression_weight: the regulariser expression_weight |psi|^2.  With NE = 0 and joint_weights None the
     step is fit_lm_keypoints_2d_step's (or the perspective step's) bit for bit."""
-    what = 'fit_lm_keypoints_2d_expressive_step'
-    B, n_rot = trial['rot'].shape[:2]
-    nb, ne, K = trial['betas'].shape[1], trial['expression'].shape[1], targets.shape[1]
-    last = 'camera' if intrinsics is None else 'transl'
-    sigma = _check_kp2d_scalars(what, robust_sigma, pose_prior_weight, betas_weight, lambda_up, lambda_down,
-                                pose_anchor)
-    if not expression_weight >= 0:
-        raise ValueError(f'{what}: expression_weight must be >= 0')
-    if joint_weights is not None:
-        jw = torch.as_tensor(joint_weights, dtype=torch.float32)
-        if jw.shape != (n_rot,):
-            raise RuntimeError(f'{what}: joint_weights must be ({n_rot},)')
-        if jw.device.type == 'cpu':
-            if not (float(jw[0]) == 0 and bool((jw >= 0).all())):
-                raise ValueError(f'{what}: joint_weights must be >= 0 with joint 0 zero')
-            jw = jw.to(trial['rot'].device)
-        if pose_anchor is None:
-            raise ValueError(f'{what}: joint_weights need pose_anchor')
-        joint_weights = jw.contiguous()
-    extra = [t for t in (pose_anchor, joint_weights, intrinsics) if t is not None]
-    ts = [state[k] for k in ('rot', 'betas', 'expression', last, 'keypoints', 'jac', 'loss', 'lambda')] + \
-        [trial[k] for k in ('rot', 'betas', 'expression', last)] + [targets, weights, trial_keypoints, trial_jac] + extra
-    _check_step_tensors(what, ts, 'the state, trial, targets, weights, anchor, joint weights and intrinsics',
-                        state['accepted'])
-    P = 3 * n_rot + nb + ne + 3
-    if not _kp_step_shapes_ok(state, trial_jac, weights, B, K, P) or targets.shape != (B, K, 2) or \
-            state['expression'].shape != (B, ne):
-        raise RuntimeError(f'{what}: jac must be ({B}, {3 * K}, {P}), weights ({B}, {K}), targets ({B}, {K}, 2) and '
-                           f'expression ({B}, {ne})')
-    if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
-        raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
-    if intrinsics is not None and intrinsics.shape != (B, 3):
-        raise RuntimeError(f'{what}: intrinsics must be ({B}, 3)')
-    if B == 0:
-        return
-    e = (lambda t: ptr(t) if ne else None)  # noqa: E731
-    head = [B, K, n_rot, nb, ne, ptr(targets), ptr(weights)] + ([ptr(intrinsics)] if intrinsics is not None else []) + \
-        [ptr(pose_anchor), ptr(joint_weights), sigma, float(pose_prior_weight), float(betas_weight),
-         float(expression_weight), float(lambda_up), float(lambda_down), int(bool(first))]
-    persp = '' if intrinsics is None else '_perspective'
-    with torch.cuda.device(trial['rot'].device):
-        check(getattr(lib(), f'shapy_fit_lm_keypoints_2d_expressive{persp}_step')(
-            *head, ptr(state['rot']), ptr(state['betas']), e(state['expression']),
-            *[ptr(state[k]) for k in (last, 'keypoints', 'jac', 'loss', 'lambda', 'accepted')],
-            ptr(trial['rot']), ptr(trial['betas']), e(trial['expression']), ptr(trial[last]), ptr(trial_keypoints),
-            ptr(trial_jac), stream_ptr()), what)
+    _fit_lm_kp2d('fit_lm_keypoints_2d_expressive_step', state, trial, targets, weights, robust_sigma,
+                 pose_prior_weight, betas_weight, lambda_up, lambda_down, first, trial_keypoints, trial_jac,
+                 pose_anchor, intrinsics=intrinsics, expressive=(expression_weight, joint_weights))
 
 
 def smplx_backward_shape(model: SmplxModel, grad_v_shaped) -> torch.Tensor:

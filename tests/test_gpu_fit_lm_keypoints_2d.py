@@ -1,6 +1,6 @@
 """GPU: the 2D keypoint Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_step) against its NumPy restatement
-(tests/kp2d_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_cpu.py) at P = 7, 54, 55 (the 48 KB shared-memory opt-in)
-and 96, and fit_body_to_keypoints_2d end to end on the synthetic SMPL-X: loss definition, monotone losses, no host
+(tests/kp2d_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_cpu.py) at P = 7, 54, 55, 79, 80 (the 48 KB shared-memory
+opt-in) and 96, and fit_body_to_keypoints_2d end to end on the synthetic SMPL-X: loss definition, monotone losses, no host
 synchronisation, determinism, batch independence, time to quality against Adam, and robustness to outliers."""
 import math
 
@@ -31,8 +31,9 @@ def _rodrigues(aa):
 
 
 # ------------------------------------------------------------------------------------------------ step kernel
-# (n_rot, nb): P = 3 n_rot + nb + 3 = 7, 54, 55 (twice) and 96; K: 2K = 2, 16 (the staging boundary), 18 and 254 rows
-STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27)]
+# (n_rot, nb): P = 3 n_rot + nb + 3 = 7, 54, 55 (twice), 96, and 79 and 80 (the largest P under 48 KB of shared memory
+# without opting in, and the smallest that opts in); K: 2K = 2, 16 (the staging boundary), 18 and 254 rows
+STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10), (22, 11)]
 STEP_K = [1, 8, 9, 127]
 # (robust_sigma, pose_prior_weight, betas_weight)
 TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]

@@ -18,7 +18,9 @@ pytestmark = pytest.mark.gpu
 F, PP = 1000.0, (500.0, 500.0)
 
 # ------------------------------------------------------------------------------------------------ step kernel
-STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10)]
+# (n_rot, nb): P = 7, 54, 55 (twice), 96, and 78 and 79 (the largest P under 48 KB of shared memory without opting in,
+# and the smallest that opts in)
+STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10), (22, 9)]
 STEP_K = [1, 8, 9, 127]
 # (robust_sigma, pose_prior_weight, betas_weight), sigma in pixels
 TERMS = [(math.inf, 0.0, 0.0), (20.0, 500.0, 100.0)]
@@ -143,7 +145,7 @@ def test_step_kernel_vs_oracle(n_rot, nb, K, first, terms):
 
 @pytest.mark.parametrize('first', [False, True])
 def test_measurement_entry_with_dropped_measurements_is_the_plain_step(first):
-    for n_rot, nb, K in ((22, 10, 127), (8, 27, 9)):
+    for n_rot, nb, K in ((22, 10, 127), (8, 27, 9), (22, 9, 127)):
         c = _step_case(n_rot, nb, K, TERMS[1])
         B = c['rot'].shape[0]
         nan = lambda *s: torch.full(s, float('nan'), device='cuda')  # noqa: E731

@@ -431,7 +431,7 @@ LAYOUTS = {'1-2-3-5': (1, 2, 3, 5), '1-7-1-33-2': (1, 7, 1, 33, 2), '64': (64,)}
 @pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('K', STEP_K_2D)
-@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES + [(22, 10), (22, 11)])   # and P = 79 / 80, its 48 KB opt-in boundary
 def test_keypoint_2d_measurement_step_vs_oracle(n_rot, nb, K, first, terms):
     worst = kp2d._run_step(kp2d._step_case(n_rot, nb, K, terms, meas=True), first)
     print(f'[model-shapes] kp2dm step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first} terms={terms}: '

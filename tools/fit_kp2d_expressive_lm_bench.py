@@ -1,4 +1,4 @@
-"""Times the whole-body 2D keypoint Levenberg-Marquardt pieces against today's 22-joint ones on the seeded synthetic
+"""Times the whole-body 2D keypoint Levenberg-Marquardt pieces against the 22-joint ones on the seeded synthetic
 SMPL-X (weak-perspective camera, Geman-McClure loss, pose and betas priors on, later steps).
 
     python tools/fit_kp2d_expressive_lm_bench.py [--reps 5] [--out fit_kp2d_expressive_lm_bench.json]
@@ -7,9 +7,10 @@ Per batch size (64 and 4096 bodies), with CUDA events, arms alternating within e
 the mean time per call (microseconds):
   jac_79 / jac_188        shapy_smplx_keypoint_jacobian at n_rot = 22 (P = 79) / _expr at n_rot = 55, NE = 10 (P = 188)
   kp2d_step_79            shapy_fit_lm_keypoints_2d_step at P = 79
-  wide_step_79            shapy_fit_lm_keypoints_2d_expressive_step on the same P = 79 problem
+  wide_step_79            shapy_fit_lm_keypoints_2d_expressive_step on the same P = 79 problem: both entries run the
+                          one single-image 2D step kernel, so the two arms time the same kernel through two entries
   wide_step_188           shapy_fit_lm_keypoints_2d_expressive_step at P = 188
-  iter_79 / iter_188      one LM iteration (Jacobian + step) with today's step at P = 79 / the wide step at P = 188
+  iter_79 / iter_188      one LM iteration (Jacobian + step) at P = 79 / at P = 188
 The card's name, power limit and SM clocks are read in the same run; nothing is set.
 """
 import argparse
