@@ -47,6 +47,13 @@ __device__ __forceinline__ float lm_lambda(int first, bool accept, float lam, do
   return fminf(fmaxf(lam, kLambdaMin), kLambdaMax);
 }
 
+// |x|^2 of n fp32 values in fp64, in l order: the sum of every betas and expression regulariser
+__device__ __forceinline__ double lm_sq_norm(const float *x, int n) {
+  double s = 0.0;
+  for (int l = 0; l < n; ++l) s += (double)x[l] * (double)x[l];
+  return s;
+}
+
 struct LmArgs {
   int B, nb;
   const float *targets, *weights;
@@ -360,22 +367,20 @@ __device__ __forceinline__ void lm_exp_gs(const float *Rs, double d0, double d1,
   Rt[6] = (float)b12; Rt[7] = (float)b22; Rt[8] = (float)b32;
 }
 
-// Phase 5, the next trial from the state and delta = y: the rotations R_j Exp(delta_j) by Rodrigues in fp64,
-// re-orthonormalised by the 6D decoder's Gram-Schmidt of the first two columns, beta + delta_beta and the last three
-// parameters + their delta, all rounded to fp32; the state itself when the step failed (!ok)
+// The next trial rotation Rt: Rs Exp(d) (lm_exp_gs) when the step succeeded (ok), else a copy of the state's Rs
+__device__ __forceinline__ void lm_rot_next(const float *Rs, const double *d, bool ok, float *Rt) {
+  if (ok) lm_exp_gs(Rs, d[0], d[1], d[2], Rt);
+  else
+    for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
+}
+
+// Phase 5, the next trial from the state and delta = y: the rotations by lm_rot_next, beta + delta_beta and the last
+// three parameters + their delta, all rounded to fp32; the state itself when the step failed (!ok)
 __device__ __forceinline__ void lm_kp_next_trial(const LmKpArgs &a, int b, const double *y, bool ok) {
   const int t = threadIdx.x, nb = a.nb, o = 3 * a.n_rot;
   const float *sr = a.rot + (size_t)b * a.n_rot * 9;
   float *trr = a.trot + (size_t)b * a.n_rot * 9;
-  for (int j = t; j < a.n_rot; j += blockDim.x) {
-    const float *Rs = sr + 9 * j;
-    float *Rt = trr + 9 * j;
-    if (!ok) {
-      for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
-      continue;
-    }
-    lm_exp_gs(Rs, y[3 * j], y[3 * j + 1], y[3 * j + 2], Rt);
-  }
+  for (int j = t; j < a.n_rot; j += blockDim.x) lm_rot_next(sr + 9 * j, y + 3 * j, ok, trr + 9 * j);
   for (int l = t; l < nb; l += blockDim.x) {
     const float x = a.betas[(size_t)b * nb + l];
     a.tbetas[(size_t)b * nb + l] = ok ? (float)((double)x + y[o + l]) : x;
@@ -839,14 +844,18 @@ cudaError_t allow_dynamic_smem(void (*kernel)(Args...), size_t smem) {
   return e;
 }
 
-template <typename Extra>
-int launch_lm_kp(void (*kernel)(LmKpArgs, Extra), int batch, const LmKpArgs &a, const Extra &x, void *stream) {
-  const size_t smem = (size_t)a.P * a.P * sizeof(double);
-  SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
-  kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
+// One launch of `kernel` on `grid` CTAs of `block` threads with `smem` bytes of dynamic shared memory, opted in when
+// there are any, and its launch check
+template <typename... Params, typename... Args>
+int lm_launch(void (*kernel)(Params...), int grid, int block, size_t smem, void *stream, const Args &...args) {
+  if (smem > 0) SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
+  kernel<<<grid, block, smem, (cudaStream_t)stream>>>(args...);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
+
+// The dynamic shared memory of a CTA that holds one P x P fp64 normal matrix
+inline size_t lm_kp_smem(int P) { return (size_t)P * P * sizeof(double); }
 
 template <typename Extra>
 int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpArgs a, Extra x, bool extra_ok,
@@ -854,7 +863,23 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
   const int rc = check_lm_kp(fn, batch, a, extra_ok, factors_ok, factors);
   if (rc != SHAPY_OK) return rc;
   if (batch == 0) return SHAPY_OK;
-  return launch_lm_kp(kernel, batch, a, x, stream);
+  return lm_launch(kernel, batch, kLmKpThreads, lm_kp_smem(a.P), stream, a, x);
+}
+
+// The measurement block's six pointers of a _measurements_ entry
+inline bool lm_meas_ptrs(const LmMeasArgs &m) {
+  return m.targets && m.weights && m.meas && m.jac && m.tmeas && m.tjac;
+}
+
+// The scalars of the 2D steps, and the sentence that states their and the lambda factors' ranges
+inline bool lm_kp2d_factors_ok(const LmKp2dArgs &x) { return x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f; }
+constexpr const char *kLmKp2dFactors =
+    "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and lambda_down >= 1";
+
+// The pointers of a grouped, calibrated or sequence 2D entry beside check_lm_kp's: the anchor when there is a pose
+// prior, and the measurement block's with `meas`
+inline bool lm_kp2d_ptrs(const LmKp2dArgs &x, bool meas) {
+  return (x.anchor || !(x.pose_w > 0.f)) && (!meas || lm_meas_ptrs(x.mb));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -867,15 +892,16 @@ int run_lm_kp(const char *fn, void (*kernel)(LmKpArgs, Extra), int batch, LmKpAr
 // meets beta.  The exact LM step eliminates each image's block (a Schur complement), in three launches:
 //   1. lm_kp2dg_loss_kernel, per image: the bracket of the trial's loss into its scratch; on the first step also the
 //      diagonal of the trial's keypoint rows (the max of its n1 leading entries and its nb betas entries);
-//   2. lm_kp2dg_image_kernel, per image: the group's decision (lm_group_decide from the siblings' scratch), on accept
-//      the image's trial becomes its state; the 2D step's keypoint and pose-prior rows staged in the column order
-//      [delta | c | beta], the leading n1 x n1 block damped by lambda and factored alone (lm_kp_solve with n = n1), then
-//      X_i = A_i^-1 B_i by the solve's backward substitution on the rows of L21; into scratch S_i = C_i - B_i^T X_i
-//      (the factor's trailing block), s_i = g_beta,i - B_i^T A_i^-1 g_i, X_i, x_i = A_i^-1 g_i and the pivots' flag;
-//   3. lm_kp2dg_group_kernel, per group: the same decision, the group's state (loss, lambda, accepted; on accept beta
-//      and the measurements), S = sum_i S_i and s = sum_i s_i (image order), then the measurement rows (m order) and
-//      betas_w beta_g, (S + (betas_w + lambda) I) dbeta = -s by the same Cholesky, and per image delta_i = -x_i -
-//      X_i dbeta (l order) and the next trial R Exp(delta), c + delta_c, beta_g + dbeta (both trial betas arrays).
+//   2. lm_kp2dg_image_kernel, per image: the decision of its group (lm_group_of; lm_group_decide from the siblings'
+//      scratch), on accept the image's trial becomes its state; the 2D step's keypoint and pose-prior rows staged in the
+//      column order [delta | c | beta], the leading n1 x n1 block damped by lambda and factored alone (lm_kp_solve with
+//      n = n1), then X_i = A_i^-1 B_i (lm_kp_solve_rows); into scratch S_i = C_i - B_i^T X_i (the factor's trailing
+//      block), s_i = g_beta,i - B_i^T A_i^-1 g_i, X_i, x_i = A_i^-1 g_i and the pivots' flag;
+//   3. lm_kp2dg_group_kernel, per group: the same decision recorded in the group's state (lm_group_commit; on accept
+//      also beta and the measurements), S = sum_i S_i and s = sum_i s_i (image order), then the measurement rows (m
+//      order) and betas_w beta_g, (S + (betas_w + lambda) I) dbeta = -s by the same Cholesky, and per image delta_i =
+//      -x_i - X_i dbeta (l order) and the next trial R Exp(delta) (lm_rot_next), c + delta_c, beta_g + dbeta (both
+//      trial betas arrays).
 // The first lambda is 1e-3 max(1e-6, the largest diagonal entry of the group's keypoint rows): per image on its pose
 // and camera columns, summed over the images (image order) on the betas columns.  A group whose loss is not finite, or
 // one of whose factorisations fails, keeps its state.  Every CTA of a group decides from the same scratch in the same
@@ -948,12 +974,7 @@ __device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &
     if (x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x2, a.trot + (size_t)i0 * nr9, x2.anchor + (size_t)g * nr9, nr9);
   }
   if (x2.mb.weights) L += lm_meas_loss(x2.mb, g);
-  if (x2.betas_w > 0.f) {
-    const float *tb = a.tbetas + (size_t)g * nb;
-    double reg = 0.0;
-    for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
-    L += (double)x2.betas_w * reg;
-  }
+  if (x2.betas_w > 0.f) L += (double)x2.betas_w * lm_sq_norm(a.tbetas + (size_t)g * nb, nb);
   const float lcur = a.loss[g];
   LmGroupDecision d;
   d.accept = lm_accept(a.first, L, lcur);
@@ -969,6 +990,44 @@ __device__ LmGroupDecision lm_group_decide(const LmKpArgs &a, const LmKp2dArgs &
   }
   d.lam = lm_lambda(a.first, d.accept, a.first ? 0.f : a.lambda[g], dmax, a.up, a.down);
   return d;
+}
+
+// lm_group_decide by the group's own CTA, which also records it in the group state: the loss on accept, lambda and
+// the accept count
+template <bool SHARE>
+__device__ __forceinline__ LmGroupDecision lm_group_commit(const LmKpArgs &a, const LmKp2dArgs &x2,
+                                                           const LmGroupArgs &gr, int g) {
+  const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, g);
+  if (d.accept) a.loss[g] = d.lnew;
+  a.lambda[g] = d.lam;
+  if (d.accept && !a.first) a.accepted[g] += 1;
+  return d;
+}
+
+// The group g with off[g] <= b < off[g + 1] of image (view, frame) b, by one thread
+__device__ __forceinline__ int lm_group_of(const LmGroupArgs &gr, int b) {
+  int lo = 0, hi = gr.G - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (gr.off[mid] <= b) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// After lm_kp_solve(A, y, P, n, ..): X = A11^-1 B in place in the ns rows n.. of A, which held L21.  L11^T X = L21^T,
+// column by column from the last, as the solve's L^T delta = y
+__device__ __forceinline__ void lm_kp_solve_rows(double *A, int P, int n, int ns) {
+  const int t = threadIdx.x;
+  for (int j = n - 1; j >= 0; --j) {
+    for (int l = t; l < ns; l += blockDim.x) A[(n + l) * P + j] /= A[j * P + j];
+    __syncthreads();
+    for (int q = t; q < ns * j; q += blockDim.x) {
+      const int l = q / j, i = q % j;
+      A[(n + l) * P + i] -= A[j * P + i] * A[(n + l) * P + j];
+    }
+    __syncthreads();
+  }
 }
 
 template <bool SHARE>
@@ -1033,13 +1092,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArg
   const double s2 = (double)x2.sigma * (double)x2.sigma;
   // 2. the group's decision
   if (t == 0) {
-    int lo = 0, hi = gr.G - 1;            // the group g with off[g] <= b < off[g + 1]
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (gr.off[mid] <= b) lo = mid;
-      else hi = mid - 1;
-    }
-    const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, lo);
+    const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, lm_group_of(gr, b));
     accept_s = d.accept;
     lam_s = d.lam;
     ok_s = 1;
@@ -1065,16 +1118,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dg_image_kernel(LmKpArg
     for (int j = 0; j < n1; ++j) A[j * P + j] += (double)lam_s;
   // 4. the leading block factored alone: S_i in the trailing block, -s_i in y's tail, -x_i in y's head
   lm_kp_solve(A, y, P, n1, ok_s);
-  // X_i = A_i^-1 B_i: L11^T X = L21^T in place in the rows n1.. of A, as the solve's L^T delta = y, column by column
-  for (int j = n1 - 1; j >= 0; --j) {
-    for (int l = t; l < ns; l += blockDim.x) A[(n1 + l) * P + j] /= A[j * P + j];
-    __syncthreads();
-    for (int q = t; q < ns * j; q += blockDim.x) {
-      const int l = q / j, i = q % j;
-      A[(n1 + l) * P + i] -= A[j * P + i] * A[(n1 + l) * P + j];
-    }
-    __syncthreads();
-  }
+  lm_kp_solve_rows(A, P, n1, ns);       // X_i = A_i^-1 B_i
   double *scr = gr.scr + (size_t)b * gr.stride;
   double *S = scr + kScrDiag + ns, *sv = S + ns * ns, *X = sv + ns, *xv = X + n1 * ns;
   for (int q = t; q < ns * ns; q += blockDim.x) {
@@ -1100,12 +1144,9 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a
   const int i0 = gr.off[g], i1 = gr.off[g + 1];
   const LmMeasArgs &mb = x2.mb;
   if (t == 0) {
-    const LmGroupDecision d = lm_group_decide<SHARE>(a, x2, gr, g);
+    const LmGroupDecision d = lm_group_commit<SHARE>(a, x2, gr, g);
     accept_s = d.accept;
     lam_s = d.lam;
-    if (d.accept) a.loss[g] = d.lnew;
-    a.lambda[g] = d.lam;
-    if (d.accept && !a.first) a.accepted[g] += 1;
     bool ok = isfinite(d.lnew);         // a group without a finite loss does not move, nor one with a failed block
     for (int i = i0; i < i1; ++i) ok = ok && gr.scr[(size_t)i * gr.stride + kScrOk] != 0.0;
     ok_s = ok;
@@ -1155,18 +1196,11 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a
     }
     __syncthreads();
     for (int j = t; j < a.n_rot; j += blockDim.x) {
-      const float *Rs = a.rot + (size_t)i * nr9 + 9 * j;
       float *Rt = a.trot + (size_t)i * nr9 + 9 * j;
-      if (SHARE && j > 0) {               // a shared rotation: the group's, from its first image's rows
-        Rs = a.rot + (size_t)i0 * nr9 + 9 * j;
-        if (ok) lm_exp_gs(Rs, y[3 * j - 3], y[3 * j - 2], y[3 * j - 1], Rt);
-        else
-          for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
-        continue;
-      }
-      if (ok) lm_exp_gs(Rs, dv[3 * j], dv[3 * j + 1], dv[3 * j + 2], Rt);
+      if (SHARE && j > 0)                 // a shared rotation: the group's, from its first image's rows
+        lm_rot_next(a.rot + (size_t)i0 * nr9 + 9 * j, y + 3 * j - 3, ok, Rt);
       else
-        for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
+        lm_rot_next(a.rot + (size_t)i * nr9 + 9 * j, dv + 3 * j, ok, Rt);
     }
     if (t < 3) {
       const float x = a.last[(size_t)i * 3 + t];
@@ -1183,32 +1217,24 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2dg_group_kernel(LmKpArgs a
 }
 
 // The grouped entries' checks (check_lm_kp's, then the offsets, read on the host) and the three launches; the offsets
-// are copied into the workspace on the stream.  SHARE: the shared-pose entries, with the group anchor
+// are copied into the workspace on the stream.  SHARE: the shared-pose entries, with the group anchor; `meas`: the
+// _measurements_ entries
 template <bool SHARE>
 int run_lm_kp2dg(const char *fn, int batch, int G, const int32_t *offsets, LmKpArgs a, LmKp2dArgs x,
-                 float *tbetas_img, void *workspace, bool extra_ok, void *stream) {
-  const int rc = check_lm_kp(fn, batch, a, extra_ok && offsets && tbetas_img && workspace,
-                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f,
-                             "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                             "lambda_down >= 1");
+                 float *tbetas_img, void *workspace, bool meas, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, lm_kp2d_ptrs(x, meas) && offsets && tbetas_img && workspace,
+                             lm_kp2d_factors_ok(x), kLmKp2dFactors);
   if (rc != SHAPY_OK) return rc;
   const int orc = put_group_offsets(fn, "group_offsets", batch, G, offsets, workspace, stream);
   if (orc != SHAPY_OK || batch == 0) return orc;
   const int n1 = SHARE ? 6 : 3 * a.n_rot + 3, ns = a.P - n1;
   LmGroupArgs gr{G, (int *)workspace, (double *)((char *)workspace + lm_group_offsets_bytes(G)),
                  lm_group_stride(n1, ns), tbetas_img};
-  cudaStream_t st = (cudaStream_t)stream;
-  lm_kp2dg_loss_kernel<SHARE><<<batch, 128, 0, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
-  const size_t smem = (size_t)a.P * a.P * sizeof(double);
-  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2dg_image_kernel<SHARE>, smem));
-  lm_kp2dg_image_kernel<SHARE><<<batch, kLmKpThreads, smem, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
-  const size_t smem3 = (size_t)(ns * ns + n1) * sizeof(double);
-  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2dg_group_kernel<SHARE>, smem3));
-  lm_kp2dg_group_kernel<SHARE><<<G, kLmKpThreads, smem3, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
-  return SHAPY_OK;
+  const size_t smem = lm_kp_smem(a.P), smem3 = (size_t)(ns * ns + n1) * sizeof(double);
+  int e = lm_launch(lm_kp2dg_loss_kernel<SHARE>, batch, 128, 0, stream, a, x, gr);
+  if (e == SHAPY_OK) e = lm_launch(lm_kp2dg_image_kernel<SHARE>, batch, kLmKpThreads, smem, stream, a, x, gr);
+  if (e == SHAPY_OK) e = lm_launch(lm_kp2dg_group_kernel<SHARE>, G, kLmKpThreads, smem3, stream, a, x, gr);
+  return e;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1257,12 +1283,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dc_step_kernel(LmKpArgs
     }
     if (x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x2, a.trot + (size_t)b * nr9, anc, nr9);
     if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
-    if (x2.betas_w > 0.f) {
-      const float *tb = a.tbetas + (size_t)b * nb;
-      double reg = 0.0;
-      for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
-      L += (double)x2.betas_w * reg;
-    }
+    if (x2.betas_w > 0.f) L += (double)x2.betas_w * lm_sq_norm(a.tbetas + (size_t)b * nb, nb);
     lt_s = L;
   }
   __syncthreads();
@@ -1331,16 +1352,14 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2dc_step_kernel(LmKpArgs
 // launch; the offsets are copied into the workspace on the stream
 template <bool MEAS>
 int run_lm_kp2dc(const char *fn, int views, int G, const int32_t *offsets, LmKpArgs a, LmKp2dCalibArgs x,
-                 void *workspace, bool extra_ok, void *stream) {
-  const int rc = check_lm_kp(fn, G, a, extra_ok && offsets && x.intr && x.extr && workspace,
-                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f,
-                             "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                             "lambda_down >= 1");
+                 void *workspace, void *stream) {
+  const int rc = check_lm_kp(fn, G, a, lm_kp2d_ptrs(x, MEAS) && offsets && x.intr && x.extr && workspace,
+                             lm_kp2d_factors_ok(x), kLmKp2dFactors);
   if (rc != SHAPY_OK) return rc;
   const int orc = put_group_offsets(fn, "view_offsets", views, G, offsets, workspace, stream);
   if (orc != SHAPY_OK || G == 0) return orc;
   x.off = (const int *)workspace;
-  return launch_lm_kp(lm_kp2dc_step_kernel<MEAS>, G, a, x, stream);
+  return lm_launch(lm_kp2dc_step_kernel<MEAS>, G, kLmKpThreads, lm_kp_smem(a.P), stream, a, x);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1360,18 +1379,20 @@ int run_lm_kp2dc(const char *fn, int views, int G, const int32_t *offsets, LmKpA
 // D_{t+1},j^T D_t,j (D = the 9 x 3 tangent rows), and -stransl_w I on tau.  Three launches after the keypoint Jacobian:
 //   1. lm_kp2ds_loss_kernel, per frame: the bracket of the trial's loss into its scratch and, on the first step, the
 //      diagonal of its keypoint rows (lm_kp2dg_loss_kernel's slots), so that lm_group_decide<false> decides unchanged;
-//   2. lm_kp2ds_frame_kernel, per frame: the sequence's decision, on accept the frame's trial becomes its state; the
-//      perspective keypoint rows in the column order [delta | tau | beta], the pose-prior rows, then the diagonal blocks
-//      and gradient of the smoothness rows of the previous and the next frame (a neighbour read as accept ? trial :
-//      state, neither written during the launch); A_t (P x P lower) and -g_t into the frame's scratch;
-//   3. lm_kp2ds_sequence_kernel, per sequence: the decision, the sequence's state, then a block LDL^T sweep over its
-//      frames (block Thomas, the arrow carried along): with Dt_0 = D_0 + lambda I,
+//   2. lm_kp2ds_frame_kernel, per frame: the decision of its sequence (lm_group_of), on accept the frame's trial
+//      becomes its state; the perspective keypoint rows in the column order [delta | tau | beta], the pose-prior rows,
+//      then the diagonal blocks and gradient of the smoothness rows of the previous and the next frame (a neighbour read
+//      as accept ? trial : state, neither written during the launch); A_t (P x P lower) and -g_t into the frame's
+//      scratch;
+//   3. lm_kp2ds_sequence_kernel, per sequence: the decision recorded in the sequence's state (lm_group_commit), then a
+//      block LDL^T sweep over its frames (block Thomas, the arrow carried along): with Dt_0 = D_0 + lambda I,
 //        Dt_t = D_t + lambda I - C_{t-1} Dt_{t-1}^-1 C_{t-1}^T,  Bt_t = B_t - C_{t-1} Dt_{t-1}^-1 Bt_{t-1},
 //        rt_t = -g_t - C_{t-1} Dt_{t-1}^-1 rt_{t-1},  Et = E - sum_t Bt_t^T Dt_t^-1 Bt_t,  et = -g_beta - sum_t ...,
 //      each frame's [Dt_t | Bt_t] factored by lm_kp_solve with n = n1 in shared memory (the trailing block carries Et),
-//      then X_t = Dt_t^-1 Bt_t, Y_t = Dt_t^-1 C_t^T and y_t = Dt_t^-1 rt_t into the frame's scratch; Et (+ betas_w +
-//      lambda on its diagonal) dbeta = et - betas_w beta; from the last frame back, x_t = y_t - X_t dbeta - Y_t x_{t+1}
-//      and the next trial R Exp(delta), tau + dtau, beta + dbeta (trial betas per sequence and per frame).
+//      then X_t = Dt_t^-1 Bt_t (lm_kp_solve_rows), Y_t = Dt_t^-1 C_t^T and y_t = Dt_t^-1 rt_t into the frame's
+//      scratch; Et (+ betas_w + lambda on its diagonal) dbeta = et - betas_w beta; from the last frame back, x_t = y_t -
+//      X_t dbeta - Y_t x_{t+1} and the next trial R Exp(delta) (lm_rot_next), tau + dtau, beta + dbeta (trial betas
+//      per sequence and per frame).
 // The policy is the grouped step's per sequence: one decision, lambda, loss and accept count, the first lambda from the
 // diagonal of the keypoint rows (per frame on [delta | tau], summed over the frames on beta); a sequence whose loss is
 // not finite or one of whose pivots fails keeps its state.  Depth rule per frame, as the perspective step's: a trial
@@ -1388,17 +1409,6 @@ constexpr int kSeqA = kScrDiag;               // + nb
 __host__ __device__ inline int lm_seq_stride(int n1, int nb) {
   const int P = n1 + nb;
   return kSeqA + nb + P * P + P + n1 + nb * n1 + n1 * n1;
-}
-
-// The sequence of frame b (off[s] <= b < off[s + 1]), by one thread
-__device__ __forceinline__ int lm_seq_of(const LmGroupArgs &gr, int b) {
-  int lo = 0, hi = gr.G - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (gr.off[mid] <= b) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
 }
 
 // Phase 1: the smoothness term of the pair (b, b + 1) of the trial, rotations then translation
@@ -1467,7 +1477,7 @@ __global__ void __launch_bounds__(128) lm_kp2ds_loss_kernel(LmKpArgs a, LmKp2dSe
   const PerspCam tc = persp_cam(x2.intr + (size_t)b * 3, a.tlast + (size_t)b * 3);
   if (t == 0) {
     double L = lm_kp2d_trial_loss<true>(a, x2, b, tg, wt, anc, robust, s2, &tc);
-    if (b + 1 < gr.off[lm_seq_of(gr, b) + 1]) L += lm_seq_smooth_loss(a, x2, b);
+    if (b + 1 < gr.off[lm_group_of(gr, b) + 1]) L += lm_seq_smooth_loss(a, x2, b);
     scr[kScrLoss] = L;
   }
   if (!a.first) return;
@@ -1505,7 +1515,7 @@ __global__ void __launch_bounds__(kLmKpThreads, 2) lm_kp2ds_frame_kernel(LmKpArg
   const double s2 = (double)x2.sigma * (double)x2.sigma;
   // 2. the sequence's decision
   if (t == 0) {
-    const int s = lm_seq_of(gr, b);
+    const int s = lm_group_of(gr, b);
     accept_s = lm_group_decide<false>(a, x2, gr, s).accept;
     prev_s = b > gr.off[s];
     next_s = b + 1 < gr.off[s + 1];
@@ -1542,12 +1552,9 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2ds_sequence_kernel(LmKpArg
   const int i0 = gr.off[s], i1 = gr.off[s + 1];
   double *Ys = S + P * P;
   if (t == 0) {
-    const LmGroupDecision d = lm_group_decide<false>(a, x2, gr, s);
+    const LmGroupDecision d = lm_group_commit<false>(a, x2, gr, s);
     accept_s = d.accept;
     lam_s = d.lam;
-    if (d.accept) a.loss[s] = d.lnew;
-    a.lambda[s] = d.lam;
-    if (d.accept && !a.first) a.accepted[s] += 1;
     ok_s = isfinite(d.lnew);            // a sequence without a finite loss does not move, nor one with a failed pivot
   }
   __syncthreads();
@@ -1599,16 +1606,7 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2ds_sequence_kernel(LmKpArg
     // Dt_t factored: the trailing block becomes Et - Bt_t^T Dt_t^-1 Bt_t, y's tail et - Bt_t^T Dt_t^-1 rt_t, y's head
     // Dt_t^-1 rt_t (lm_kp_solve starts with a barrier)
     lm_kp_solve(S, y, P, n1, ok_s);
-    // X_t = Dt_t^-1 Bt_t in place in the rows n1.. of S, as the grouped image kernel does
-    for (int j = n1 - 1; j >= 0; --j) {
-      for (int l = t; l < nb; l += blockDim.x) S[(n1 + l) * P + j] /= S[j * P + j];
-      __syncthreads();
-      for (int q = t; q < nb * j; q += blockDim.x) {
-        const int l = q / j, k = q % j;
-        S[(n1 + l) * P + k] -= S[j * P + k] * S[(n1 + l) * P + j];
-      }
-      __syncthreads();
-    }
+    lm_kp_solve_rows(S, P, n1, nb);     // X_t = Dt_t^-1 Bt_t
     double *yo = scr + kSeqA + nb + P * P + P, *Xo = yo + n1, *Yo = Xo + nb * n1;
     for (int j = t; j < n1; j += blockDim.x) yo[j] = y[j];
     for (int q = t; q < nb * n1; q += blockDim.x) Xo[q] = S[(n1 + q / n1) * P + q % n1];
@@ -1683,13 +1681,8 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2ds_sequence_kernel(LmKpArg
       xc[j] = v;
     }
     __syncthreads();
-    for (int j = t; j < a.n_rot; j += blockDim.x) {
-      const float *Rs = a.rot + (size_t)i * nr9 + 9 * j;
-      float *Rt = a.trot + (size_t)i * nr9 + 9 * j;
-      if (ok) lm_exp_gs(Rs, xc[3 * j], xc[3 * j + 1], xc[3 * j + 2], Rt);
-      else
-        for (int e = 0; e < 9; ++e) Rt[e] = Rs[e];
-    }
+    for (int j = t; j < a.n_rot; j += blockDim.x)
+      lm_rot_next(a.rot + (size_t)i * nr9 + 9 * j, xc + 3 * j, ok, a.trot + (size_t)i * nr9 + 9 * j);
     if (t < 3) {
       const float x = a.last[(size_t)i * 3 + t];
       a.tlast[(size_t)i * 3 + t] = ok ? (float)((double)x + xc[o + t]) : x;
@@ -1706,10 +1699,10 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_kp2ds_sequence_kernel(LmKpArg
 // The sequence entry's checks (check_lm_kp's, the smoothness weights, then the offsets, read on the host) and the three
 // launches; the offsets are copied into the workspace on the stream
 int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpArgs a, LmKp2dSeqArgs x,
-                 float *tbetas_img, void *workspace, bool extra_ok, void *stream) {
-  const int rc = check_lm_kp(fn, batch, a, extra_ok && offsets && x.intr && tbetas_img && workspace,
-                             x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f && x.srot_w >= 0.f &&
-                                 isfinite(x.srot_w) && x.stransl_w >= 0.f && isfinite(x.stransl_w),
+                 float *tbetas_img, void *workspace, void *stream) {
+  const int rc = check_lm_kp(fn, batch, a, lm_kp2d_ptrs(x, false) && offsets && x.intr && tbetas_img && workspace,
+                             lm_kp2d_factors_ok(x) && x.srot_w >= 0.f && isfinite(x.srot_w) && x.stransl_w >= 0.f &&
+                                 isfinite(x.stransl_w),
                              "robust_sigma must be > 0 (inf: least squares), the prior weights >= 0, the smoothness "
                              "weights finite and >= 0 and lambda_up and lambda_down >= 1");
   if (rc != SHAPY_OK) return rc;
@@ -1718,17 +1711,12 @@ int run_lm_kp2ds(const char *fn, int batch, int G, const int32_t *offsets, LmKpA
   const int n1 = 3 * a.n_rot + 3;
   LmGroupArgs gr{G, (int *)workspace, (double *)((char *)workspace + lm_group_offsets_bytes(G)),
                  lm_seq_stride(n1, a.nb), tbetas_img};
-  cudaStream_t st = (cudaStream_t)stream;
-  lm_kp2ds_loss_kernel<<<batch, 128, 0, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
-  lm_kp2ds_frame_kernel<<<batch, kLmKpThreads, 0, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
   const int ny = n1 > a.nb ? n1 : a.nb;
   const size_t smem = (size_t)(a.P * a.P + ny * ny) * sizeof(double);
-  SHAPY_CUDA_TRY(allow_dynamic_smem(lm_kp2ds_sequence_kernel, smem));
-  lm_kp2ds_sequence_kernel<<<G, kLmKpThreads, smem, st>>>(a, x, gr);
-  SHAPY_LAUNCH_CHECK();
-  return SHAPY_OK;
+  int e = lm_launch(lm_kp2ds_loss_kernel, batch, 128, 0, stream, a, x, gr);
+  if (e == SHAPY_OK) e = lm_launch(lm_kp2ds_frame_kernel, batch, kLmKpThreads, 0, stream, a, x, gr);
+  if (e == SHAPY_OK) e = lm_launch(lm_kp2ds_sequence_kernel, G, kLmKpThreads, smem, stream, a, x, gr);
+  return e;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1840,18 +1828,8 @@ __global__ void __launch_bounds__(kLmKpThreads, 1) lm_kp2d_step_kernel(LmKpArgs 
       }
     }
     if constexpr (MEAS) L += lm_meas_loss(x2.mb, b);
-    if (x2.betas_w > 0.f) {
-      const float *tb = a.tbetas + (size_t)b * nb;
-      double reg = 0.0;
-      for (int l = 0; l < nb; ++l) reg += (double)tb[l] * (double)tb[l];
-      L += (double)x2.betas_w * reg;
-    }
-    if (x2.expr_w > 0.f) {
-      const float *te = x2.texpr + (size_t)b * ne;
-      double reg = 0.0;
-      for (int l = 0; l < ne; ++l) reg += (double)te[l] * (double)te[l];
-      L += (double)x2.expr_w * reg;
-    }
+    if (x2.betas_w > 0.f) L += (double)x2.betas_w * lm_sq_norm(a.tbetas + (size_t)b * nb, nb);
+    if (x2.expr_w > 0.f) L += (double)x2.expr_w * lm_sq_norm(x2.texpr + (size_t)b * ne, ne);
     lt_s = L;
   }
   for (int p = t; p < npk; p += blockDim.x) A[p] = 0.0;
@@ -2062,10 +2040,8 @@ inline LmKp2dStepArgs kp2d_args(const float *anchor, float sigma, float pose_w, 
 // kLmKp2dMaxP for the expressive ones
 int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool persp, bool meas, int max_p,
                 void *stream) {
-  const LmMeasArgs &mb = x.mb;
   const bool ptrs = (x.anchor || !(x.pose_w > 0.f || x.joint_w)) && (x.ne == 0 || (x.expr && x.texpr)) &&
-                    (!persp || x.intr) &&
-                    (!meas || (mb.targets && mb.weights && mb.meas && mb.jac && mb.tmeas && mb.tjac));
+                    (!persp || x.intr) && (!meas || lm_meas_ptrs(x.mb));
   SHAPY_REQUIRE(a.targets && a.weights && a.rot && a.betas && a.last && a.kp && a.jac && a.loss && a.lambda &&
                     a.accepted && a.trot && a.tbetas && a.tlast && a.tkp && a.tjac && ptrs,
                 "%s: null argument", fn);
@@ -2074,11 +2050,8 @@ int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool pe
     SHAPY_REQUIRE(sizes, "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas)", fn, batch, a.K, a.n_rot, a.nb);
   SHAPY_REQUIRE(sizes, "%s: bad size (batch %d, %d keypoints, n_rot %d, %d betas, %d expression)", fn, batch, a.K,
                 a.n_rot, a.nb, x.ne);
-  SHAPY_REQUIRE(a.up >= 1.f && a.down >= 1.f && x.sigma > 0.f && x.pose_w >= 0.f && x.betas_w >= 0.f &&
-                    x.expr_w >= 0.f,
-                "%s: robust_sigma must be > 0 (inf: least squares), the prior weights >= 0 and lambda_up and "
-                "lambda_down >= 1",
-                fn);
+  SHAPY_REQUIRE(a.up >= 1.f && a.down >= 1.f && lm_kp2d_factors_ok(x) && x.expr_w >= 0.f, "%s: %s", fn,
+                kLmKp2dFactors);
   a.P = 3 * a.n_rot + a.nb + x.ne + 3;
   if (a.P > max_p) {
     set_error("%s: %d parameters, at most %d are supported", fn, a.P, max_p);
@@ -2088,10 +2061,7 @@ int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool pe
   const size_t smem = lm_kp2d_smem_doubles(a.P) * sizeof(double);
   auto kernel = meas ? (persp ? lm_kp2d_step_kernel<true, true> : lm_kp2d_step_kernel<true, false>)
                      : (persp ? lm_kp2d_step_kernel<false, true> : lm_kp2d_step_kernel<false, false>);
-  SHAPY_CUDA_TRY(allow_dynamic_smem(kernel, smem));
-  kernel<<<batch, kLmKpThreads, smem, (cudaStream_t)stream>>>(a, x);
-  SHAPY_LAUNCH_CHECK();
-  return SHAPY_OK;
+  return lm_launch(kernel, batch, kLmKpThreads, smem, stream, a, x);
 }
 
 }  // namespace shapy
@@ -2140,8 +2110,7 @@ extern "C" int shapy_fit_lm_keypoints_measurements_step(
   LmKpArgs a{num_keypoints, n_rot, nb, 0, targets, weights, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl,
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, trial_keypoints, trial_jac};
   LmMeasArgs m{meas_targets, meas_weights, betas_weight, meas, meas_jac, trial_meas, trial_meas_jac};
-  return run_lm_kp("shapy_fit_lm_keypoints_measurements_step", lm_kp_step_kernel<true>, batch, a, m,
-                   meas_targets && meas_weights && meas && meas_jac && trial_meas && trial_meas_jac,
+  return run_lm_kp("shapy_fit_lm_keypoints_measurements_step", lm_kp_step_kernel<true>, batch, a, m, lm_meas_ptrs(m),
                    betas_weight >= 0.f, "lambda_up and lambda_down must be >= 1 and betas_weight >= 0", stream);
 }
 
@@ -2219,7 +2188,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_groups_step(
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
   return run_lm_kp2dg<false>("shapy_fit_lm_keypoints_2d_groups_step", batch, num_groups, group_offsets, a, x,
-                             trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+                             trial_betas_images, workspace, false, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_groups_measurements_step(
@@ -2235,10 +2204,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_groups_measurements_step(
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
                LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
   return run_lm_kp2dg<false>("shapy_fit_lm_keypoints_2d_groups_measurements_step", batch, num_groups, group_offsets,
-                             a, x, trial_betas_images, workspace,
-                      (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
-                          meas_jac && trial_meas && trial_meas_jac,
-                      stream);
+                             a, x, trial_betas_images, workspace, true, stream);
 }
 
 extern "C" size_t shapy_fit_lm_shared_pose_workspace_bytes(int batch, int num_groups, int n_rot, int nb) {
@@ -2257,7 +2223,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_step(
              keypoints, jac, loss, lambda, accepted, trial_rot, trial_betas, trial_camera, trial_keypoints, trial_jac};
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}};
   return run_lm_kp2dg<true>("shapy_fit_lm_keypoints_2d_shared_pose_step", batch, num_groups, group_offsets, a, x,
-                            trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+                            trial_betas_images, workspace, false, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
@@ -2273,10 +2239,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_shared_pose_measurements_step(
   LmKp2dArgs x{pose_anchor, robust_sigma, pose_prior_weight, betas_weight,
                LmMeasArgs{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac}};
   return run_lm_kp2dg<true>("shapy_fit_lm_keypoints_2d_shared_pose_measurements_step", batch, num_groups,
-                            group_offsets, a, x, trial_betas_images, workspace,
-                            (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
-                                meas_jac && trial_meas && trial_meas_jac,
-                            stream);
+                            group_offsets, a, x, trial_betas_images, workspace, true, stream);
 }
 
 extern "C" size_t shapy_fit_lm_calibrated_workspace_bytes(int num_views, int num_bodies) {
@@ -2296,7 +2259,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_calibrated_step(
   LmKp2dCalibArgs x{{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics},
                     extrinsics, nullptr};
   return run_lm_kp2dc<false>("shapy_fit_lm_keypoints_2d_calibrated_step", num_views, num_bodies, view_offsets, a, x,
-                             workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+                             workspace, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
@@ -2314,10 +2277,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_calibrated_measurements_step(
                      intrinsics},
                     extrinsics, nullptr};
   return run_lm_kp2dc<true>("shapy_fit_lm_keypoints_2d_calibrated_measurements_step", num_views, num_bodies,
-                            view_offsets, a, x, workspace,
-                            (pose_anchor || !(pose_prior_weight > 0.f)) && meas_targets && meas_weights && meas &&
-                                meas_jac && trial_meas && trial_meas_jac,
-                            stream);
+                            view_offsets, a, x, workspace, stream);
 }
 
 extern "C" size_t shapy_fit_lm_sequence_workspace_bytes(int batch, int num_sequences, int n_rot, int nb) {
@@ -2337,7 +2297,7 @@ extern "C" int shapy_fit_lm_keypoints_2d_sequence_step(
   LmKp2dSeqArgs x{{{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, LmMeasArgs{}}, intrinsics},
                   smooth_rot_weight, smooth_transl_weight};
   return run_lm_kp2ds("shapy_fit_lm_keypoints_2d_sequence_step", batch, num_sequences, sequence_offsets, a, x,
-                      trial_betas_images, workspace, pose_anchor || !(pose_prior_weight > 0.f), stream);
+                      trial_betas_images, workspace, stream);
 }
 
 extern "C" int shapy_fit_lm_keypoints_2d_expressive_step(

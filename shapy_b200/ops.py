@@ -905,6 +905,15 @@ def fit_lm_groups_workspace(B, G, n_rot, nb, device):
     return _workspace(lib().shapy_fit_lm_groups_workspace_bytes(int(B), int(G), int(n_rot), int(nb)), device)
 
 
+def _check_group_state(what, state, trial, G, B, nb):
+    """The per-group state of the grouped and sequence 2D steps: betas, trial betas, loss, lambda and accepted per
+    group (G rows), and image_betas per image (B rows)."""
+    if (state['betas'].shape != (G, nb) or trial['betas'].shape != (G, nb) or trial['image_betas'].shape != (B, nb) or
+            any(state[k].shape != (G,) for k in ('loss', 'lambda', 'accepted'))):
+        raise RuntimeError(f'{what}: betas and trial betas must be ({G}, {nb}), image_betas ({B}, {nb}) and loss, '
+                           f'lambda and accepted ({G},)')
+
+
 def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose_prior_weight, betas_weight, lambda_up,
                         lambda_down, first, trial_keypoints, trial_jac, group_offsets, workspace, pose_anchor,
                         meas=None, share_pose=False):
@@ -927,10 +936,7 @@ def _fit_lm_kp2d_groups(what, state, trial, targets, weights, robust_sigma, pose
     na = G if share_pose else B
     if pose_anchor is not None and pose_anchor.shape != (na, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({na}, {n_rot}, 3, 3)')
-    if (state['betas'].shape != (G, nb) or trial['betas'].shape != (G, nb) or trial['image_betas'].shape != (B, nb) or
-            any(state[k].shape != (G,) for k in ('loss', 'lambda', 'accepted'))):
-        raise RuntimeError(f'{what}: betas and trial betas must be ({G}, {nb}), image_betas ({B}, {nb}) and loss, '
-                           f'lambda and accepted ({G},)')
+    _check_group_state(what, state, trial, G, B, nb)
     if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], G, nb):
         raise RuntimeError(f'{what}: meas_jac must be ({G}, 5, {nb}) and the measurements, their targets and weights '
                            f'({G}, 5)')
@@ -1060,10 +1066,7 @@ def fit_lm_keypoints_2d_sequence_step(state, trial, targets, weights, intrinsics
         raise RuntimeError(f'{what}: intrinsics and transl must be ({B}, 3)')
     if pose_anchor is not None and pose_anchor.shape != (B, n_rot, 3, 3):
         raise RuntimeError(f'{what}: pose_anchor must be ({B}, {n_rot}, 3, 3)')
-    if (state['betas'].shape != (S, nb) or trial['betas'].shape != (S, nb) or trial['image_betas'].shape != (B, nb) or
-            any(state[k].shape != (S,) for k in ('loss', 'lambda', 'accepted'))):
-        raise RuntimeError(f'{what}: betas and trial betas must be ({S}, {nb}), image_betas ({B}, {nb}) and loss, '
-                           f'lambda and accepted ({S},)')
+    _check_group_state(what, state, trial, S, B, nb)
     L = lib()
     _check_workspace(what, workspace, L.shapy_fit_lm_sequence_workspace_bytes(B, S, n_rot, nb))
     if B == 0:

@@ -5,6 +5,7 @@ and camera, and the step is the Schur complement of the group's block-arrow norm
   image_scratch    launch 1 for one image: the bracket of its trial loss (keypoint term + pose prior) and, on the first
                    step, the max of its keypoint-row diagonal over [delta | c] and its betas entries
   decide           the group's decision from the images' scratch: (accept, loss after it, lambda), as lm_group_decide
+                   (and lm_group_commit, which also records it in the group state)
   image_block      launch 2 for one image: its normal equations with the columns reordered to [delta | c | beta], the
                    leading block damped by lambda and factored alone; (S_i, s_i, X_i, x_i, ok_i)
   lm_groups_step   shapy_fit_lm_keypoints_2d_groups_step (and _measurements_step, with `meas`) for one group: the
@@ -110,7 +111,7 @@ def image_block(targets, weights, kp, jac, camera, rot, lam, sigma=math.inf, anc
     for j in range(n1):
         A[j, j] += float(lam)
     A, y, ok = _solve_partial(A, g, n1)
-    W = A[n1:, :n1].copy()                       # the rows of L21, then X^T
+    W = A[n1:, :n1].copy()                       # the rows of L21, then X^T (lm_kp_solve_rows)
     with np.errstate(invalid='ignore', divide='ignore'):
         for j in range(n1 - 1, -1, -1):
             W[:, j] /= A[j, j]
