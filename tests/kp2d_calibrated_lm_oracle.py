@@ -1,17 +1,17 @@
 """NumPy float64 restatement of the calibrated 2D keypoint Levenberg-Marquardt step (test infrastructure), on top of
-tests/kp2d_persp_lm_oracle.py, tests/kp2d_lm_oracle.py and tests/kpm_lm_oracle.py.  One body seen by V views, each with
-intrinsics (f, px, py) and world-to-camera extrinsics ext (12,) = R row-major, then T.
+tests/kp2d_lm_oracle.py and oracle/lm_oracle.py.  One body seen by V views, each with intrinsics (f, px, py) and
+world-to-camera extrinsics ext (12,) = R row-major, then T.
 
   camera_points        Y_k = R (kp_k + t) + T in float64
   project              p_k = f (Y_k,x / Y_k,z, Y_k,y / Y_k,z) + (px, py)
   jacobian_calibrated  one view's projected (2K, P) Jacobian: row 2k + c = u . J3_k, u = (f / Y_z) (R[c, :] -
                        (Y_c / Y_z) R[2, :]), J3_k the (3 x P) block of keypoint k with J_t = I (u on the t columns)
-  loss                 the kernel's loss in fp64: the keypoint term of each view (kp2d_persp_lm_oracle.loss of its
+  loss                 the kernel's loss in fp64: the keypoint term of each view (kp2d_lm_oracle.keypoint_loss of its
                        camera-frame points, depth rule included) in view order, then the pose prior, the measurement sum
                        and the betas prior
-  normal_equations     A and g before damping: the keypoint rows of the views in order, then kp2d_persp_lm_oracle's
-                       pose-prior rows and betas_w beta, and kp2dm_lm_oracle's measurement rows; and the diagonal of the
-                       keypoint rows alone (the first lambda)
+  normal_equations     A and g before damping: the keypoint rows of the views in order, then the pose-prior rows
+                       (accumulated on their own, then added), the measurement rows and betas_w beta; and the diagonal
+                       of the keypoint rows alone (the first lambda)
   lm_keypoints_2d_calibrated_step
                        shapy_fit_lm_keypoints_2d_calibrated_step for one body: accept / reject, lambda and the loss
                        agree with float32 storage, the next trial to the last bits of the solve and of sin / cos
@@ -21,9 +21,8 @@ import math
 import numpy as np
 
 import kp2d_lm_oracle as o2
-import kp2d_persp_lm_oracle as op
-from kp_lm_oracle import DIAG_FLOOR, LAMBDA_INIT, LAMBDA_MAX, LAMBDA_MIN, exp_gram_schmidt
-from kpm_lm_oracle import meas_loss
+from oracle.lm_oracle import (cholesky_solve, lm_accept, lm_diag_max, lm_kp_next_trial, lm_lambda, lm_loss,
+                              lm_sq_norm, meas_loss, meas_rows)
 
 
 def _ext(ext):
@@ -38,7 +37,7 @@ def camera_points(kp, transl, ext):
 
 
 def project(kp, transl, intr, ext):
-    return op.project(camera_points(kp, transl, ext), np.zeros(3), intr)
+    return o2.project(camera_points(kp, transl, ext), np.zeros(3), intr)
 
 
 def jacobian_calibrated(kp, jac3, transl, intr, ext):
@@ -65,19 +64,13 @@ def loss(views, kp, transl, sigma=math.inf, rot=None, anchor=None, pose_w=0.0, b
     for v in range(len(wt)):
         with np.errstate(invalid='ignore', over='ignore', divide='ignore'):
             Y = camera_points(kp, transl, ext[v])
-        L += op.loss(tg[v], wt[v], Y, np.zeros(3), intr[v], sigma)
+        L += o2.keypoint_loss(tg[v], wt[v], Y, np.zeros(3), sigma, intr[v])
     if pose_w > 0.0:
-        q = 0.0
-        for d in (np.asarray(rot, np.float64)[1:] - np.asarray(anchor, np.float64)[1:]).reshape(-1):
-            q += d * d
-        L += 0.5 * float(np.float32(pose_w)) * q
+        L += o2.prior_loss(np.asarray(rot, np.float64)[1:], np.asarray(anchor, np.float64)[1:], pose_w)
     if meas is not None:
         L += meas_loss(*meas)
     if betas_w > 0.0:
-        reg = 0.0
-        for x in np.asarray(betas, np.float64):
-            reg += x * x
-        L += float(np.float32(betas_w)) * reg
+        L += float(np.float32(betas_w)) * lm_sq_norm(betas)
     return L
 
 
@@ -86,46 +79,21 @@ def normal_equations(views, kp, jac3, transl, sigma=math.inf, rot=None, anchor=N
     """(A, g, diag of the keypoint rows) before damping; meas None or (meas_targets, meas_weights, meas, meas_jac)."""
     tg, wt, intr, ext = views
     P = np.asarray(jac3).shape[1]
-    s2 = float(sigma) * float(sigma)
     A, g = np.zeros((P, P)), np.zeros(P)
     for v in range(len(wt)):
         with np.errstate(divide='ignore', invalid='ignore'):
             J2 = jacobian_calibrated(kp, jac3, transl, intr[v], ext[v])
             p = project(kp, transl, intr[v], ext[v])
-        for k in range(len(wt[v])):
-            w = float(wt[v][k])
-            if not w > 0.0:
-                continue
-            dx, dy = p[k, 0] - float(tg[v][k, 0]), p[k, 1] - float(tg[v][k, 1])
-            wr = w
-            if math.isfinite(sigma):
-                q = s2 / (s2 + (dx * dx + dy * dy))
-                wr = w * (q * q)
-            if not wr > 0.0:
-                continue
-            for c, r in ((0, dx), (1, dy)):
-                wj = wr * J2[2 * k + c]
-                A += np.outer(wj, J2[2 * k + c])
-                g += wj * r
+        o2.keypoint_rows(A, g, tg[v], wt[v], p, J2, sigma)
     dg = np.diag(A).copy()
-    # the pose-prior rows and betas_w beta: kp2d_persp_lm_oracle's with no keypoint row
-    K = len(wt[0])
-    Ap, gp, _ = op.normal_equations(np.zeros((K, 2)), np.zeros(K), kp, jac3, transl, intr[0], sigma, rot, anchor,
-                                    pose_w, betas, 0.0)
+    Ap, gp = np.zeros((P, P)), np.zeros(P)
+    o2.prior_rows(Ap, gp, rot, anchor, pose_w)
     A += Ap
     g += gp
     nb = len(betas)
     o = P - 3 - nb
     if meas is not None:
-        mt, mw, mv, mj = meas
-        Jm = np.asarray(mj, np.float64)
-        for m in range(5):
-            u = float(mw[m])
-            if not u > 0.0:
-                continue
-            uj = u * Jm[m]
-            A[o:o + nb, o:o + nb] += np.outer(uj, Jm[m])
-            g[o:o + nb] += uj * (float(mv[m]) - float(mt[m]))
+        meas_rows(A, g, o, *meas)
     if betas_w > 0.0:
         g[o:o + nb] += float(np.float32(betas_w)) * np.asarray(betas, np.float64)
     return A, g, dg
@@ -143,11 +111,10 @@ def lm_keypoints_2d_calibrated_step(state, views, lambda_up, lambda_down, first,
     lt = loss(views, trial_kp, trial['transl'], sigma, trial['rot'], anchor, pose_w, trial['betas'], betas_w,
               None if meas is None else (meas[0], meas[1], trial_meas[0]))
     lcur = state.get('loss', f(np.nan))
-    accept = bool(first) or (math.isfinite(lt) and lt < float(lcur))
+    accept = lm_accept(first, lt, lcur)
     new = {k: np.array(v, copy=True) if isinstance(v, np.ndarray) else v for k, v in state.items()}
-    lnew = lcur
+    lnew = lm_loss(accept, lt, lcur, f)
     if accept:
-        lnew = f(lt) if math.isfinite(lt) else f(np.nan)
         new.update({k: np.asarray(trial[k], f).copy() for k in ('rot', 'betas', 'transl')})
         new.update(keypoints=np.asarray(trial_kp, f).copy(), jac=np.asarray(trial_jac, f).copy(), loss=lnew)
         if meas is not None:
@@ -158,27 +125,12 @@ def lm_keypoints_2d_calibrated_step(state, views, lambda_up, lambda_down, first,
     P = len(g)
     n_rot, nb = new['rot'].shape[0], len(new['betas'])
     o = 3 * n_rot
-    if first:
-        dmax = DIAG_FLOOR
-        for j in range(P):
-            dmax = float(np.fmax(dmax, dg[j]))
-        lam = f(LAMBDA_INIT * dmax)
-    elif accept:
-        lam = f(f(state['lambda']) / f(lambda_down))
-    else:
-        lam = f(f(state['lambda']) * f(lambda_up))
-    lam = f(np.fmin(np.fmax(lam, f(LAMBDA_MIN)), f(LAMBDA_MAX)))
+    lam = lm_lambda(first, accept, state.get('lambda'), lm_diag_max(dg) if first else None, lambda_up, lambda_down, f)
     new['lambda'] = lam
     new['accepted'] = int(state.get('accepted', 0)) + (1 if accept and not first else 0)
     damp = float(np.float32(betas_w)) + float(lam)
     for j in range(P):
         A[j, j] += damp if o <= j < o + nb else float(lam)
-    y, ok = o2._solve(A, g)
+    y, ok = cholesky_solve(A, g)
     ok = ok and math.isfinite(float(lnew))
-    if not ok:
-        nxt = {k: np.asarray(new[k], f).copy() for k in ('rot', 'betas', 'transl')}
-    else:
-        nxt = {'rot': np.stack([exp_gram_schmidt(new['rot'][j], y[3 * j:3 * j + 3]) for j in range(n_rot)]).astype(f),
-               'betas': np.array([f(float(new['betas'][i]) + y[o + i]) for i in range(nb)], f),
-               'transl': np.array([f(float(new['transl'][i]) + y[o + nb + i]) for i in range(3)], f)}
-    return new, nxt, accept
+    return new, lm_kp_next_trial(new, y, ok, ('rot', 'betas', 'transl'), f), accept

@@ -1,5 +1,5 @@
 """NumPy float64 restatement of the sequence 2D keypoint Levenberg-Marquardt step (test infrastructure), on top of
-tests/kp2d_persp_lm_oracle.py and tests/kp2dg_lm_oracle.py: the frames of one sequence share their betas, each keeps
+tests/kp2d_lm_oracle.py (its perspective camera) and tests/kp2dg_lm_oracle.py: the frames of one sequence share their betas, each keeps
 its rotations and camera-frame translation, and consecutive frames are tied by smoothness rows, so the normal matrix
 of a sequence is block tridiagonal in its frames with an arrow of betas columns.
 
@@ -21,24 +21,17 @@ import math
 import numpy as np
 
 import kp2d_lm_oracle as o2
-import kp2d_persp_lm_oracle as op
 import kp2dg_lm_oracle as og
-from kp_lm_oracle import DIAG_FLOOR, exp_gram_schmidt
+from oracle.lm_oracle import exp_gram_schmidt, lm_diag_max, lm_sq_norm
 
 
 def smooth_loss(rot0, rot1, t0, t1, srw=0.0, stw=0.0):
     """srot_w / 2 sum_j |R1_j - R0_j|_F^2 (j order, row-major entries) + stransl_w |t1 - t0|^2, in fp64."""
     L = 0.0
     if srw > 0.0:
-        q = 0.0
-        for d in (np.asarray(rot1, np.float64) - np.asarray(rot0, np.float64)).reshape(-1):
-            q += d * d
-        L += 0.5 * float(np.float32(srw)) * q
+        L += o2.prior_loss(rot1, rot0, srw)
     if stw > 0.0:
-        q = 0.0
-        for d in np.asarray(t1, np.float64) - np.asarray(t0, np.float64):
-            q += d * d
-        L += float(np.float32(stw)) * q
+        L += float(np.float32(stw)) * lm_sq_norm(np.asarray(t1, np.float64) - np.asarray(t0, np.float64))
     return L
 
 
@@ -79,22 +72,19 @@ def frame_scratch(targets, weights, intr, trial_kp, trial_jac, trial, first, nxt
                   pose_w=0.0, srw=0.0, stw=0.0, dtype=np.float32):
     """(bracket, dmax over [delta | tau] from DIAG_FLOOR, the betas diagonal) of one frame's trial; nxt: the next
     frame's trial {'rot', 'transl'} when it is in the sequence."""
-    lt = op.loss(targets, weights, trial_kp, trial['transl'], intr, sigma, trial['rot'], anchor, pose_w)
+    lt = o2.loss(targets, weights, trial_kp, trial['transl'], sigma, trial['rot'], anchor, pose_w, intr=intr)
     if nxt is not None:
         lt += smooth_loss(trial['rot'], nxt['rot'], trial['transl'], nxt['transl'], srw, stw)
     if not first:
         return lt, None, None
     f = dtype
     with np.errstate(all='ignore'):
-        _, _, dg = op.normal_equations(targets, weights, np.asarray(trial_kp, f), np.asarray(trial_jac, f),
-                                       np.asarray(trial['transl'], f), intr, sigma)
+        _, _, dg = o2.normal_equations(targets, weights, np.asarray(trial_kp, f), np.asarray(trial_jac, f),
+                                       np.asarray(trial['transl'], f), sigma, intr=intr)
     nb = len(trial['betas'])
     n_rot = np.asarray(trial['rot']).shape[0]
     dg = dg[og.reorder(n_rot, nb)]
-    dmax = DIAG_FLOOR
-    for j in range(3 * n_rot + 3):
-        dmax = float(np.fmax(dmax, dg[j]))
-    return lt, dmax, dg[3 * n_rot + 3:].copy()
+    return lt, lm_diag_max(dg[:3 * n_rot + 3]), dg[3 * n_rot + 3:].copy()
 
 
 def frame_system(targets, weights, intr, kp, jac, rot, transl, neighbours=(), sigma=math.inf, anchor=None, pose_w=0.0,
@@ -103,7 +93,7 @@ def frame_system(targets, weights, intr, kp, jac, rot, transl, neighbours=(), si
     the (rot, transl) of the previous and the next frame, those in the sequence."""
     nb = np.asarray(jac).shape[1] - 3 * np.asarray(rot).shape[0] - 3
     with np.errstate(all='ignore'):
-        A, g, _ = op.normal_equations(targets, weights, kp, jac, transl, intr, sigma, rot, anchor, pose_w)
+        A, g, _ = o2.normal_equations(targets, weights, kp, jac, transl, sigma, rot, anchor, pose_w, intr=intr)
     perm = og.reorder(np.asarray(rot).shape[0], nb)
     A, g = A[perm][:, perm].copy(), g[perm].copy()
     rot, transl = np.asarray(rot, np.float64), np.asarray(transl, np.float64)

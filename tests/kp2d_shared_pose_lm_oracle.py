@@ -21,7 +21,7 @@ import numpy as np
 
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
-from kp_lm_oracle import DIAG_FLOOR, exp_gram_schmidt
+from oracle.lm_oracle import cholesky_solve, exp_gram_schmidt, lm_add_next, lm_diag_max, meas_rows
 
 N1 = 6                                                  # the image block [delta_0 | c]
 
@@ -29,14 +29,6 @@ N1 = 6                                                  # the image block [delta
 def order(n_rot, nb):
     o = 3 * n_rot
     return np.array([0, 1, 2, o + nb, o + nb + 1, o + nb + 2] + list(range(3, o)) + list(range(o, o + nb)))
-
-
-def prior_loss(rot, anchor, pose_w):
-    """1/2 pose_w sum_{j >= 1} |R_j - R0_j|_F^2, j order, row-major entries."""
-    q = 0.0
-    for d in (np.asarray(rot, np.float64)[1:] - np.asarray(anchor, np.float64)[1:]).reshape(-1):
-        q += d * d
-    return 0.5 * float(np.float32(pose_w)) * q
 
 
 def image_scratch(targets, weights, trial_kp, trial_jac, trial, first, sigma=math.inf, dtype=np.float32):
@@ -48,10 +40,7 @@ def image_scratch(targets, weights, trial_kp, trial_jac, trial, first, sigma=mat
     _, _, dg = o2.normal_equations(targets, weights, np.asarray(trial_kp, f), np.asarray(trial_jac, f),
                                    np.asarray(trial['camera'], f), sigma)
     dg = dg[order(np.asarray(trial['rot']).shape[0], len(trial['betas']))]
-    dmax = DIAG_FLOOR
-    for j in range(N1):
-        dmax = float(np.fmax(dmax, dg[j]))
-    return lt, dmax, dg[N1:].copy()
+    return lt, lm_diag_max(dg[:N1]), dg[N1:].copy()
 
 
 def decide(scratch, first, lcur, lam, lambda_up, lambda_down, trial_rot, anchor, pose_w, trial_betas, betas_w=0.0,
@@ -62,7 +51,8 @@ def decide(scratch, first, lcur, lam, lambda_up, lambda_down, trial_rot, anchor,
         L = sc[0][0]    # so their sum with the prior goes first and exact zeros follow (x + 0.0 is x)
         for s in sc[1:]:
             L += s[0]
-        sc = [[L + prior_loss(trial_rot, anchor, pose_w), *sc[0][1:]]] + [[0.0, *s[1:]] for s in sc[1:]]
+        sc = [[L + o2.prior_loss(np.asarray(trial_rot, np.float64)[1:], np.asarray(anchor, np.float64)[1:], pose_w),
+               *sc[0][1:]]] + [[0.0, *s[1:]] for s in sc[1:]]
     return og.decide(sc, first, lcur, lam, lambda_up, lambda_down, trial_betas, betas_w, meas_terms, dtype)
 
 
@@ -73,28 +63,13 @@ def image_block(targets, weights, kp, jac, camera, n_rot, lam, sigma=math.inf, n
     A, g = A[perm][:, perm].copy(), g[perm].copy()
     for j in range(N1):
         A[j, j] += float(lam)
-    A, y, ok = og._solve_partial(A, g, N1)
+    y, ok = cholesky_solve(A, g, N1)
     W = A[N1:, :N1].copy()                       # the rows of L21, then X^T
     with np.errstate(invalid='ignore', divide='ignore'):
         for j in range(N1 - 1, -1, -1):
             W[:, j] /= A[j, j]
             W[:, :j] -= np.outer(W[:, j], A[j, :j])
     return np.tril(A[N1:, N1:]), -y[N1:], W.T.copy(), -y[:N1], ok
-
-
-def add_prior_rows(S, s, rot, anchor, pose_w):
-    """The pose-prior rows of joints 1 .. added in place to the shared block's S and s, e order per joint."""
-    if not pose_w > 0.0:
-        return
-    hw = 0.5 * float(np.float32(pose_w))
-    rot, anchor = np.asarray(rot, np.float64), np.asarray(anchor, np.float64)
-    for j in range(1, rot.shape[0]):
-        D = np.stack([o2.rot_tangent(rot[j], a) for a in range(3)], 1)          # (9, 3)
-        res = (rot[j] - anchor[j]).reshape(9)
-        b = slice(3 * (j - 1), 3 * j)
-        for e in range(9):
-            S[b, b] += np.outer(hw * D[e], D[e])
-            s[b] += hw * D[e] * res[e]
 
 
 def shared_pose_step(state, images, lambda_up, lambda_down, first, trial, anchor, sigma=math.inf, pose_w=0.0,
@@ -135,23 +110,16 @@ def shared_pose_step(state, images, lambda_up, lambda_down, first, trial, anchor
     for b in blocks:
         S += b[0]
         s += b[1]
-    add_prior_rows(S, s, new['rot'][0], anchor, pose_w)
+    o2.prior_rows(S, s, new['rot'][0], anchor, pose_w, o=-3)     # joint j >= 1 at the shared columns 3 (j - 1) ..
     if meas is not None:
-        Jm = np.asarray(new['meas_jac'], np.float64)
-        for m in range(5):
-            u = float(meas['weights'][m])
-            if not u > 0.0:
-                continue
-            uj = u * Jm[m]
-            S[ob:, ob:] += np.outer(uj, Jm[m])
-            s[ob:] += uj * (float(new['meas'][m]) - float(meas['targets'][m]))
+        meas_rows(S, s, ob, meas['targets'], meas['weights'], new['meas'], new['meas_jac'])
     beta = np.asarray(new['betas'], np.float64)
     if betas_w > 0.0:
         s[ob:] += float(np.float32(betas_w)) * beta
     damp = float(np.float32(betas_w)) + float(lam)
     for j in range(ns):
         S[j, j] += damp if j >= ob else float(lam)
-    ds, ok = o2._solve(S, s)
+    ds, ok = cholesky_solve(S, s)
     ok = ok and math.isfinite(float(lnew)) and all(b[4] for b in blocks)
     nxt = {'rot': [], 'camera': []}
     body = [exp_gram_schmidt(new['rot'][0][j], ds[3 * (j - 1):3 * j]) for j in range(1, n_rot)]
@@ -165,12 +133,10 @@ def shared_pose_step(state, images, lambda_up, lambda_down, first, trial, anchor
             d[j] = v
         if ok:
             nxt['rot'].append(np.stack([exp_gram_schmidt(new['rot'][i][0], d[:3])] + body).astype(f))
-            nxt['camera'].append(np.array([f(float(new['camera'][i][t]) + d[3 + t]) for t in range(3)], f))
         else:
             nxt['rot'].append(np.asarray(new['rot'][i], f).copy())
-            nxt['camera'].append(np.asarray(new['camera'][i], f).copy())
-    nxt['betas'] = (np.array([f(float(new['betas'][l]) + ds[ob + l]) for l in range(nb)], f) if ok
-                    else np.asarray(new['betas'], f).copy())
+        nxt['camera'].append(lm_add_next(new['camera'][i], d[3:], ok, f))
+    nxt['betas'] = lm_add_next(new['betas'], ds[ob:], ok, f)
     return new, nxt, accept, blocks, ds
 
 

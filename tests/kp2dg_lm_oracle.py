@@ -1,5 +1,5 @@
 """NumPy float64 restatement of the grouped 2D keypoint Levenberg-Marquardt step (test infrastructure), on top of
-tests/kp2d_lm_oracle.py and tests/kpm_lm_oracle.py: the images of one group share their betas, each keeps its rotations
+tests/kp2d_lm_oracle.py and oracle/lm_oracle.py: the images of one group share their betas, each keeps its rotations
 and camera, and the step is the Schur complement of the group's block-arrow normal matrix.
 
   image_scratch    launch 1 for one image: the bracket of its trial loss (keypoint term + pose prior) and, on the first
@@ -17,8 +17,8 @@ import math
 import numpy as np
 
 import kp2d_lm_oracle as o2
-from kp_lm_oracle import DIAG_FLOOR, LAMBDA_INIT, LAMBDA_MAX, LAMBDA_MIN, exp_gram_schmidt
-from kpm_lm_oracle import meas_loss
+from oracle.lm_oracle import (cholesky_solve, lm_accept, lm_add_next, lm_diag_max, lm_lambda, lm_loss,
+                              lm_rot_next, lm_sq_norm, meas_loss, meas_rows)
 
 
 def reorder(n_rot, nb):
@@ -39,10 +39,7 @@ def image_scratch(targets, weights, trial_kp, trial_jac, trial, first, sigma=mat
                                    np.asarray(trial['camera'], f), sigma)
     nb = len(trial['betas'])
     dg = dg[reorder(np.asarray(trial['rot']).shape[0], nb)]
-    dmax = DIAG_FLOOR
-    for j in range(len(dg) - nb):
-        dmax = float(np.fmax(dmax, dg[j]))
-    return lt, dmax, dg[len(dg) - nb:].copy()
+    return lt, lm_diag_max(dg[:len(dg) - nb]), dg[len(dg) - nb:].copy()
 
 
 def decide(scratch, first, lcur, lam, lambda_up, lambda_down, trial_betas, betas_w=0.0, meas_terms=None,
@@ -56,49 +53,17 @@ def decide(scratch, first, lcur, lam, lambda_up, lambda_down, trial_betas, betas
     if meas_terms is not None:
         L += meas_loss(*meas_terms)
     if betas_w > 0.0:
-        reg = 0.0
-        for x in np.asarray(trial_betas, np.float64):
-            reg += x * x
-        L += float(np.float32(betas_w)) * reg
-    accept = bool(first) or (math.isfinite(L) and L < float(lcur))
-    lnew = (f(L) if math.isfinite(L) else f(np.nan)) if accept else lcur
-    if first:
-        dmax = DIAG_FLOOR
-        for s in scratch:
-            dmax = float(np.fmax(dmax, s[1]))
+        L += float(np.float32(betas_w)) * lm_sq_norm(trial_betas)
+    accept = lm_accept(first, L, lcur)
+    dmax = None
+    if first:       # the images' brackets, then the betas diagonal summed over the images in image order
+        dmax = lm_diag_max([s[1] for s in scratch])
         for l in range(len(scratch[0][2])):
             d = scratch[0][2][l]
             for s in scratch[1:]:
                 d += s[2][l]
-            dmax = float(np.fmax(dmax, d))
-        lam = f(LAMBDA_INIT * dmax)
-    elif accept:
-        lam = f(f(lam) / f(lambda_down))
-    else:
-        lam = f(f(lam) * f(lambda_up))
-    return accept, lnew, f(np.fmin(np.fmax(lam, f(LAMBDA_MIN)), f(LAMBDA_MAX)))
-
-
-def _solve_partial(A, g, n):
-    """lm_kp_solve with its leading n columns eliminated: (A with L11, L21 and the Schur block, y, ok)."""
-    P = len(g)
-    ok = True
-    with np.errstate(invalid='ignore', divide='ignore'):
-        for j in range(n):
-            d = A[j, j]
-            ok = ok and d > 0.0 and math.isfinite(d)
-            ljj = math.sqrt(d) if d >= 0 else float('nan')
-            A[j, j] = ljj
-            A[j + 1:, j] /= ljj
-            A[j + 1:, j + 1:] -= np.outer(A[j + 1:, j], A[j + 1:, j])
-        y = -g
-        for j in range(n):
-            y[j] = y[j] / A[j, j]
-            y[j + 1:] -= A[j + 1:, j] * y[j]
-        for j in range(n - 1, -1, -1):
-            y[j] = y[j] / A[j, j]
-            y[:j] -= A[j, :j] * y[j]
-    return A, y, ok
+            dmax = lm_diag_max([d], dmax)
+    return accept, lm_loss(accept, L, lcur, f), lm_lambda(first, accept, lam, dmax, lambda_up, lambda_down, f)
 
 
 def image_block(targets, weights, kp, jac, camera, rot, lam, sigma=math.inf, anchor=None, pose_w=0.0, nb=None):
@@ -110,7 +75,7 @@ def image_block(targets, weights, kp, jac, camera, rot, lam, sigma=math.inf, anc
     n1 = 3 * n_rot + 3
     for j in range(n1):
         A[j, j] += float(lam)
-    A, y, ok = _solve_partial(A, g, n1)
+    y, ok = cholesky_solve(A, g, n1)           # A now holds L11, L21 and the Schur block
     W = A[n1:, :n1].copy()                       # the rows of L21, then X^T (lm_kp_solve_rows)
     with np.errstate(invalid='ignore', divide='ignore'):
         for j in range(n1 - 1, -1, -1):
@@ -157,21 +122,14 @@ def lm_groups_step(state, images, lambda_up, lambda_down, first, trial, sigma=ma
         S += b[0]
         s += b[1]
     if meas is not None:
-        Jm = np.asarray(new['meas_jac'], np.float64)
-        for m in range(5):
-            u = float(meas['weights'][m])
-            if not u > 0.0:
-                continue
-            uj = u * Jm[m]
-            S += np.outer(uj, Jm[m])
-            s += uj * (float(new['meas'][m]) - float(meas['targets'][m]))
+        meas_rows(S, s, 0, meas['targets'], meas['weights'], new['meas'], new['meas_jac'])
     beta = np.asarray(new['betas'], np.float64)
     if betas_w > 0.0:
         s += float(np.float32(betas_w)) * beta
     damp = float(np.float32(betas_w)) + float(lam)
     for j in range(nb):
         S[j, j] += damp
-    db, ok = o2._solve(S, s)
+    db, ok = cholesky_solve(S, s)
     ok = ok and math.isfinite(float(lnew)) and all(b[4] for b in blocks)
     n_rot = np.asarray(new['rot'][0]).shape[0]
     o = 3 * n_rot
@@ -184,13 +142,7 @@ def lm_groups_step(state, images, lambda_up, lambda_down, first, trial, sigma=ma
             for l in range(nb):
                 v -= X[j, l] * db[l]
             d[j] = v
-        if ok:
-            nxt['rot'].append(np.stack([exp_gram_schmidt(new['rot'][i][j], d[3 * j:3 * j + 3])
-                                        for j in range(n_rot)]).astype(f))
-            nxt['camera'].append(np.array([f(float(new['camera'][i][t]) + d[o + t]) for t in range(3)], f))
-        else:
-            nxt['rot'].append(np.asarray(new['rot'][i], f).copy())
-            nxt['camera'].append(np.asarray(new['camera'][i], f).copy())
-    nxt['betas'] = (np.array([f(float(new['betas'][l]) + db[l]) for l in range(nb)], f) if ok
-                    else np.asarray(new['betas'], f).copy())
+        nxt['rot'].append(lm_rot_next(new['rot'][i], d, ok, f))
+        nxt['camera'].append(lm_add_next(new['camera'][i], d[o:], ok, f))
+    nxt['betas'] = lm_add_next(new['betas'], db, ok, f)
     return new, nxt, accept, blocks, db

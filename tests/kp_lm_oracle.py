@@ -2,10 +2,14 @@
 infrastructure).
 
   keypoint_jacobian    shapy_smplx_keypoint_jacobian for one body: the closed form of DESIGN.md §6b in float64,
-                       columns [delta_j (R_j Exp(delta_j) at delta = 0) | betas | transl]
-  lm_keypoints_step    shapy_fit_lm_keypoints_step for one body: the same fp64 operations in the same order (the
-                       kernel is compiled with -fmad=false), so accept / reject, lambda and the loss agree bit for bit
-                       with float32 storage, and the next trial to the last bits of the fp64 solve and of sin / cos
+                       columns [delta_j (R_j Exp(delta_j) at delta = 0) | betas | transl]; with expr,
+                       shapy_smplx_keypoint_jacobian_expr: the expression rows appended to the shape basis (they are
+                       shape rows NB .. NC-1), columns [delta_j | betas | expression | transl]
+  loss                 the kernel's loss in fp64: the keypoint term, then with measurements their sum and rho |betas|^2
+  lm_keypoints_step    shapy_fit_lm_keypoints_step (and with `meas` shapy_fit_lm_keypoints_measurements_step) for one
+                       body: the same fp64 operations in the same order (the kernel is compiled with -fmad=false), so
+                       accept / reject, lambda and the loss agree bit for bit with float32 storage, and the next trial
+                       to the last bits of the fp64 solve and of sin / cos
 """
 import math
 
@@ -13,9 +17,9 @@ import numpy as np
 import torch
 
 from oracle import smplx_oracle
-
-LAMBDA_MIN, LAMBDA_MAX = np.float32(1e-9), np.float32(1e9)
-LAMBDA_INIT, DIAG_FLOOR = 1e-3, 1e-6
+from oracle.lm_oracle import (DIAG_FLOOR, LAMBDA_INIT, LAMBDA_MAX, LAMBDA_MIN, cholesky_solve,  # noqa: F401
+                              exp_gram_schmidt, lm_accept, lm_diag_max, lm_kp_next_trial, lm_lambda, lm_loss,
+                              lm_sq_norm, meas_loss, meas_rows)
 
 
 def _np(t, dtype=np.float64):
@@ -31,8 +35,13 @@ def _cross(w, q):
     return np.cross(np.broadcast_to(w, q.shape), q)
 
 
-def keypoint_jacobian(model, betas, rot, transl=None, use_face_contour=True):
-    """One body: betas (NB,), rot (n_rot, 3, 3), transl (3,) or None -> (keypoints (K, 3), jac (3K, P)) float64."""
+def keypoint_jacobian(model, betas, rot, transl=None, use_face_contour=True, expr=None):
+    """One body: betas (NB,), rot (n_rot, 3, 3), transl (3,) or None, expr (NE,) or None -> (keypoints (K, 3), jac
+    (3K, P)) float64."""
+    if expr is not None:
+        model = dict(model)
+        model['shapedirs'] = torch.cat([torch.as_tensor(model['shapedirs']), torch.as_tensor(model['expr_dirs'])], 2)
+        betas = np.concatenate([np.asarray(betas, np.float64), np.asarray(expr, np.float64)])
     vt, S, Pd = _np(model['v_template']), _np(model['shapedirs']), _np(model['posedirs'])
     Jreg, W = _np(model['J_regressor']), _np(model['lbs_weights'])
     parents = _np(model['parents'], np.int64)
@@ -123,99 +132,73 @@ def keypoint_jacobian(model, betas, rot, transl=None, use_face_contour=True):
     return kp, np.concatenate(rows, 0)
 
 
-def loss(targets, weights, kp):
-    """The kernel's loss in fp64: w_k ((dx^2 + dy^2) + dz^2) summed in k order, weight <= 0 skipped."""
+def loss(targets, weights, kp, meas=None, betas=None, betas_weight=0.0):
+    """The kernel's loss in fp64: w_k ((dx^2 + dy^2) + dz^2) summed in k order, weight <= 0 skipped; with meas
+    (meas_targets, meas_weights, meas) the measurement sum and rho |betas|^2 follow, left to right, rho (float32) <= 0
+    adding nothing."""
     L = 0.0
     for k in range(len(weights)):
         w = float(weights[k])
         if w > 0.0:
             r = [float(kp[k, c]) - float(targets[k, c]) for c in range(3)]
             L += w * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2])
+    if meas is not None:
+        L += meas_loss(*meas)
+    rho = float(np.float32(betas_weight))
+    if rho > 0.0:
+        L += rho * lm_sq_norm(betas)
     return L
 
 
-def exp_gram_schmidt(Rs, d):
-    """R Exp(d) by Rodrigues in fp64, re-orthonormalised by the 6D decoder's Gram-Schmidt of the first two columns."""
-    d = [float(x) for x in d]
-    th2 = d[0] * d[0] + d[1] * d[1] + d[2] * d[2]
-    th = math.sqrt(th2)
-    if th < 1e-8:
-        s, c = 1.0 - th2 / 6.0, 0.5 - th2 / 24.0
-    else:
-        s, c = math.sin(th) / th, (1.0 - math.cos(th)) / th2
-    Kx = np.array([[0.0, -d[2], d[1]], [d[2], 0.0, -d[0]], [-d[1], d[0], 0.0]])
-    E = np.eye(3) + s * Kx + c * (np.outer(d, d) - th2 * np.eye(3))
-    M = np.asarray(Rs, np.float64) @ E
-    a, b = M[:, 0], M[:, 1]
-    b1 = a / max(math.sqrt(a @ a), 1e-12)
-    u = b - (b1 @ b) * b1
-    b2 = u / max(math.sqrt(u @ u), 1e-12)
-    return np.stack([b1, b2, np.cross(b1, b2)], 1)
-
-
-def lm_keypoints_step(state, targets, weights, lambda_up, lambda_down, first, trial, trial_kp, trial_jac,
-                      dtype=np.float32):
+def lm_keypoints_step(state, targets, weights, lambda_up, lambda_down, first, trial, trial_kp, trial_jac, meas=None,
+                      trial_meas=None, betas_weight=0.0, dtype=np.float32, return_delta=False):
     """One step for one body.  state: {'rot' (n_rot, 3, 3), 'betas', 'transl', 'keypoints' (K, 3), 'jac' (3K, P),
-    'loss', 'lambda', 'accepted'} (not modified); trial: {'rot', 'betas', 'transl'}.  Returns (new state, next trial,
-    accepted flag).  dtype: the storage precision (float32 as on the device; float64 gives a plain fp64 LM)."""
+    'loss', 'lambda', 'accepted'}, with meas also 'meas' (5,) and 'meas_jac' (5, NB) (not modified); trial: {'rot',
+    'betas', 'transl'}; meas None or (meas_targets, meas_weights), trial_meas (meas (5,), meas_jac (5, NB)) of the
+    trial.  The measurement rows and the betas regulariser are stacked under the keypoint rows, and the first lambda
+    reads the diagonal after them.  Returns (new state, next trial, accepted flag), and with return_delta the solved
+    step delta (P,) as a fourth item.  dtype: the storage precision (float32 as on the device; float64 gives a plain
+    fp64 LM)."""
     f = dtype
-    lt = loss(targets, weights, trial_kp)
+    rho = float(np.float32(betas_weight))
+    lt = loss(targets, weights, trial_kp, None if meas is None else (meas[0], meas[1], trial_meas[0]), trial['betas'],
+              rho)
     lcur = state.get('loss', f(np.nan))
-    accept = bool(first) or (math.isfinite(lt) and lt < float(lcur))
+    accept = lm_accept(first, lt, lcur)
     new = {k: np.array(v, copy=True) if isinstance(v, np.ndarray) else v for k, v in state.items()}
-    lnew = lcur
+    lnew = lm_loss(accept, lt, lcur, f)
     if accept:
-        lnew = f(lt) if math.isfinite(lt) else f(np.nan)
         new.update({k: np.asarray(trial[k], f).copy() for k in ('rot', 'betas', 'transl')})
         new.update(keypoints=np.asarray(trial_kp, f).copy(), jac=np.asarray(trial_jac, f).copy(), loss=lnew)
-    Jm = np.asarray(new['jac'], np.float64)
+        if meas is not None:
+            new.update(meas=np.asarray(trial_meas[0], f).copy(), meas_jac=np.asarray(trial_meas[1], f).copy())
+    Jk = np.asarray(new['jac'], np.float64)
     M = np.asarray(new['keypoints'], np.float64).reshape(-1)
     tg = np.asarray(targets, np.float64).reshape(-1)
-    P = Jm.shape[1]
+    P = Jk.shape[1]
+    nb = len(new['betas'])
+    o = 3 * new['rot'].shape[0]
     A, g = np.zeros((P, P)), np.zeros(P)
-    for r in range(Jm.shape[0]):
+    # keypoint rows in keypoint-major xyz order, then the measurement rows into the betas block in k order
+    for r in range(Jk.shape[0]):
         w = float(weights[r // 3])
         if not w > 0.0:
             continue
-        wj = w * Jm[r]
-        A += np.outer(wj, Jm[r])
+        wj = w * Jk[r]
+        A += np.outer(wj, Jk[r])
         g += wj * (M[r] - tg[r])
-    if first:
-        dmax = DIAG_FLOOR
-        for j in range(P):
-            dmax = float(np.fmax(dmax, A[j, j]))
-        lam = f(LAMBDA_INIT * dmax)
-    elif accept:
-        lam = f(f(state['lambda']) / f(lambda_down))
-    else:
-        lam = f(f(state['lambda']) * f(lambda_up))
-    lam = f(np.fmin(np.fmax(lam, f(LAMBDA_MIN)), f(LAMBDA_MAX)))
+    if meas is not None:
+        meas_rows(A, g, o, meas[0], meas[1], new['meas'], new['meas_jac'])
+    if rho > 0.0:
+        g[o:o + nb] += rho * np.asarray(new['betas'], np.float64)
+    lam = lm_lambda(first, accept, state.get('lambda'), lm_diag_max(np.diag(A)) if first else None, lambda_up,
+                    lambda_down, f)
     new['lambda'] = lam
     new['accepted'] = int(state.get('accepted', 0)) + (1 if accept and not first else 0)
+    damp = rho + float(lam)
     for j in range(P):
-        A[j, j] += float(lam)
-    ok = math.isfinite(float(lnew))
-    with np.errstate(invalid='ignore', divide='ignore'):
-        for j in range(P):
-            d = A[j, j]
-            ok = ok and d > 0.0 and math.isfinite(d)
-            ljj = math.sqrt(d) if d >= 0 else float('nan')
-            A[j, j] = ljj
-            A[j + 1:, j] /= ljj
-            A[j + 1:, j + 1:] -= np.outer(A[j + 1:, j], A[j + 1:, j])
-        y = -g
-        for j in range(P):
-            y[j] = y[j] / A[j, j]
-            y[j + 1:] -= A[j + 1:, j] * y[j]
-        for j in range(P - 1, -1, -1):
-            y[j] = y[j] / A[j, j]
-            y[:j] -= A[j, :j] * y[j]
-    n_rot = new['rot'].shape[0]
-    nb = len(new['betas'])
-    if not ok:
-        nxt = {k: np.asarray(new[k], f).copy() for k in ('rot', 'betas', 'transl')}
-    else:
-        nxt = {'rot': np.stack([exp_gram_schmidt(new['rot'][j], y[3 * j:3 * j + 3]) for j in range(n_rot)]).astype(f),
-               'betas': np.array([f(float(new['betas'][i]) + y[3 * n_rot + i]) for i in range(nb)], f),
-               'transl': np.array([f(float(new['transl'][i]) + y[3 * n_rot + nb + i]) for i in range(3)], f)}
-    return new, nxt, accept
+        A[j, j] += damp if o <= j < o + nb else float(lam)
+    y, ok = cholesky_solve(A, g)
+    ok = ok and math.isfinite(float(lnew))
+    nxt = lm_kp_next_trial(new, y, ok, ('rot', 'betas', 'transl'), f)
+    return (new, nxt, accept, y) if return_delta else (new, nxt, accept)

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import kp2d_calibrated_lm_oracle as oc
-import kp2d_persp_lm_oracle as op
+import kp2d_lm_oracle as o2
 from test_fit_lm_kp2d_cpu import _expm, _problem
 
 INTR = np.array([1000.0, 500.0, 480.0])
@@ -146,27 +146,26 @@ def test_depth_rule_per_view():
 def test_one_identity_view_is_the_perspective_step(first, sigma, pose_w, betas_w):
     evaluate, rng, rot, beta, kp, jac, _ = _case(24)
     t = np.array([0.1, -0.2, 5.0])
-    tg = op.project(kp, t, INTR) + rng.normal(size=(12, 2)) * 20.0
+    tg = o2.project(kp, t, INTR) + rng.normal(size=(12, 2)) * 20.0
     w = rng.uniform(0.5, 1.5, 12)
     w[3], tg[3] = 0.0, np.nan
     ident = np.concatenate([np.eye(3).reshape(9), np.zeros(3)])
     views = (tg[None], w[None], INTR[None], ident[None])
     anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
     A1, g1, d1 = oc.normal_equations(views, kp, jac, t, sigma, rot, anchor, pose_w, beta, betas_w)
-    A2, g2, d2 = op.normal_equations(tg, w, kp, jac, t, INTR, sigma, rot, anchor, pose_w, beta, betas_w)
+    A2, g2, d2 = o2.normal_equations(tg, w, kp, jac, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)
     for a, b in ((A1, A2), (g1, g2), (d1, d2)):
         assert np.abs(a - b).max() <= 1e-12 * np.abs(b).max()
     assert abs(oc.loss(views, kp, t, sigma, rot, anchor, pose_w, beta, betas_w) -
-               op.loss(tg, w, kp, t, INTR, sigma, rot, anchor, pose_w, beta, betas_w)) <= 1e-12 * abs(op.loss(
-                   tg, w, kp, t, INTR, sigma, rot, anchor, pose_w, beta, betas_w))
+               o2.loss(tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)) <= 1e-12 * abs(o2.loss(
+                   tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR))
     trial_kp, trial_jac = evaluate(np.stack([r @ _expm(rng.normal(size=3) * 0.05) for r in rot]), beta + 0.05)
     state = {'rot': rot, 'betas': beta, 'transl': t, 'keypoints': kp, 'jac': jac, 'lambda': np.float32(1e-2),
-             'loss': np.float32(op.loss(tg, w, kp, t, INTR, sigma, rot, anchor, pose_w, beta, betas_w))}
+             'loss': np.float32(o2.loss(tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR))}
     trial = {'rot': rot, 'betas': beta + 0.05, 'transl': t + 0.01}
     kw = dict(sigma=sigma, anchor=anchor, pose_w=pose_w, betas_w=betas_w, dtype=np.float64)
     n1, x1, a1 = oc.lm_keypoints_2d_calibrated_step(state, views, 10.0, 3.0, first, trial, trial_kp, trial_jac, **kw)
-    n2, x2, a2 = op.lm_keypoints_2d_perspective_step(state, tg, w, INTR, 10.0, 3.0, first, trial, trial_kp, trial_jac,
-                                                     **kw)
+    n2, x2, a2 = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, first, trial, trial_kp, trial_jac, intr=INTR, **kw)
     assert a1 == a2 and n1['accepted'] == n2['accepted']
     assert abs(n1['lambda'] - n2['lambda']) <= 1e-12 * n2['lambda']
     for k in ('rot', 'betas', 'transl'):

@@ -1,7 +1,7 @@
-"""CPU: the float64 restatement of the whole-body 2D keypoint LM step (tests/kp2d_expressive_lm_oracle.py).  Its
-expression and wide rotation columns against central differences of the float64 forward (tests/smplx_grad_ref.py);
-its packed solve against a dense solve at P = 7, 79, 188 and 200; at n_rot = 22 without expression it is today's
-weak-perspective and perspective oracles; a plain fp64 LM loop over the wide parameters never raises the loss.  The
+"""CPU: the float64 restatement of the whole-body 2D keypoint LM step (tests/kp2d_lm_oracle.py).  Its expression
+and wide rotation columns against central differences of the float64 forward (tests/smplx_grad_ref.py); its packed
+solve against a dense solve at P = 7, 79, 188 and 200; at n_rot = 22 a width-0 expression is the step without one, for
+the weak-perspective and perspective cameras; a plain fp64 LM loop over the wide parameters never raises the loss.  The
 command line refuses the wide flags outside the single-image 2D fit."""
 import math
 
@@ -9,9 +9,9 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_expressive_lm_oracle as ox
 import kp2d_lm_oracle as o2
-import kp2d_persp_lm_oracle as op
+from kp_lm_oracle import keypoint_jacobian
+from oracle.lm_oracle import cholesky_solve
 from shapy_b200 import synth
 from smplx_grad_ref import forward_differentiable
 from test_fit_lm_kp2d_cpu import _expm
@@ -31,7 +31,7 @@ def test_expression_and_wide_rotation_columns_vs_central_differences():
     n_rot, NB, NE = 55, 10, 10
     rot = _rotations(rng, n_rot, 0.3)
     beta, psi = rng.normal(size=NB) * 0.5, rng.normal(size=NE)
-    kp, jac = ox.keypoint_jacobian_expr(m, beta, psi, rot)
+    kp, jac = keypoint_jacobian(m, beta, rot, expr=psi)
     out = forward_differentiable(m, torch.tensor(beta)[None], torch.tensor(rot)[None], torch.tensor(psi)[None])
     assert np.abs(kp - out['joints'][0].numpy()).max() <= 1e-9
     h = 1e-6
@@ -60,14 +60,14 @@ def test_packed_solve_is_the_dense_solve(P):
     X = rng.normal(size=(P + 20, P))
     A = X.T @ X + 0.1 * np.eye(P)
     g = rng.normal(size=P)
-    y, ok = ox.packed_solve(A.copy(), g.copy())
-    yd, okd = o2._solve(A.copy(), g.copy())
+    y, ok = o2.packed_solve(A.copy(), g.copy())
+    yd, okd = cholesky_solve(A.copy(), g.copy())
     assert ok and okd
     assert np.array_equal(y, yd)                  # the same operations in the same order
     ref = np.linalg.solve(A, -g)
     assert np.abs(y - ref).max() <= 1e-9 * np.abs(ref).max()
     A[3, 3] = -1.0
-    assert not ox.packed_solve(A, g)[1]
+    assert not o2.packed_solve(A, g)[1]
 
 
 def _toy(seed, n_rot, nb, ne, K):
@@ -84,7 +84,7 @@ def test_no_expression_at_22_joints_is_todays_oracle(first, persp):
     lk = 'transl' if persp else 'camera'
     last = np.array([0.1, -0.2, 4.0]) if persp else np.array([1.0, 0.1, -0.1])
     intr = np.array([1000.0, 500.0, 480.0]) if persp else None
-    tg = (op.project(c['kp'], last, intr) if persp else o2.project(c['kp'], last)) + \
+    tg = o2.project(c['kp'], last, intr) + \
         rng.normal(size=(30, 2)) * (5.0 if persp else 0.02)
     w = rng.uniform(0.5, 1.5, 30)
     anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.1) for r in c['rot']])
@@ -96,13 +96,10 @@ def test_no_expression_at_22_joints_is_todays_oracle(first, persp):
     tkp, tjac = f32(c['kp'] + 0.01), f32(c['jac'] * 1.01)
     sigma = 20.0 if persp else 0.3
     kw = dict(sigma=sigma, anchor=anchor, pose_w=2.0, betas_w=0.1)
-    if persp:
-        want = op.lm_keypoints_2d_perspective_step(state, tg, w, intr, 10.0, 3.0, first, trial, tkp, tjac, **kw)
-    else:
-        want = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, first, trial, tkp, tjac, **kw)
+    want = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, first, trial, tkp, tjac, intr=intr, **kw)
     sx = dict(state, expression=np.zeros(0, np.float32))
     tx = dict(trial, expression=np.zeros(0, np.float32))
-    got = ox.lm_keypoints_2d_expressive_step(sx, tg, w, 10.0, 3.0, first, tx, tkp, tjac, intr=intr, **kw)
+    got = o2.lm_keypoints_2d_step(sx, tg, w, 10.0, 3.0, first, tx, tkp, tjac, intr=intr, **kw)
     assert got[2] == want[2]
     for k in ('rot', 'betas', lk, 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
         assert np.array_equal(got[0][k], want[0][k]), k
@@ -122,8 +119,8 @@ def test_fp64_lm_loop_never_raises_the_loss(persp):
     lk = 'transl' if persp else 'camera'
     last_t = np.array([0.1, -0.2, 4.0]) if persp else np.array([1.0, 0.05, -0.05])
     intr = np.array([1000.0, 500.0, 480.0]) if persp else None
-    kp_t, _ = ox.keypoint_jacobian_expr(m, beta_t, psi_t, rot_t)
-    tg = op.project(kp_t, last_t, intr) if persp else o2.project(kp_t, last_t)
+    kp_t, _ = keypoint_jacobian(m, beta_t, rot_t, expr=psi_t)
+    tg = o2.project(kp_t, last_t, intr)
     K = tg.shape[0]
     w = np.ones(K)
     jw = np.zeros(n_rot)
@@ -136,8 +133,8 @@ def test_fp64_lm_loop_never_raises_the_loss(persp):
               dtype=np.float64)
     losses = []
     for it in range(8):
-        kp, jac = ox.keypoint_jacobian_expr(m, trial['betas'], trial['expression'], trial['rot'])
-        state, trial, _ = ox.lm_keypoints_2d_expressive_step(state, tg, w, 10.0, 3.0, it == 0, trial, kp, jac, **kw)
+        kp, jac = keypoint_jacobian(m, trial['betas'], trial['rot'], expr=trial['expression'])
+        state, trial, _ = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, it == 0, trial, kp, jac, **kw)
         losses.append(float(state['loss']))
     assert all(b <= a for a, b in zip(losses, losses[1:])), losses
     assert losses[-1] < 0.5 * losses[0], losses

@@ -10,7 +10,7 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
-import kp2dm_lm_oracle as o2m
+from oracle.lm_oracle import meas_loss
 from test_fit_lm_kp2d_cpu import _expm, _problem
 
 K = 12
@@ -51,7 +51,7 @@ def _group_state(images, state, sigma, pose_w, betas_w, meas=None):
         L += o2.loss(im['targets'], im['weights'], state['keypoints'][i], state['camera'][i], sigma, state['rot'][i],
                      im['anchor'], pose_w)
     if meas is not None:
-        L += o2m.meas_loss(meas['targets'], meas['weights'], state['meas'])
+        L += meas_loss(meas['targets'], meas['weights'], state['meas'])
     if betas_w > 0:
         L += float(np.float32(betas_w)) * float(np.sum(np.asarray(state['betas']) ** 2))
     return np.float64(L)
@@ -143,13 +143,10 @@ def test_groups_of_one_equal_the_2d_oracles(first, with_meas, sigma, pose_w, bet
         if k in state:
             s[k] = state[k]
     im = images[0]
-    if meas is None:
-        want, wnxt, wacc = o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-                                                   im['trial_jac'], sigma, im['anchor'], pose_w, betas_w)
-    else:
-        want, wnxt, wacc = o2m.lm_keypoints_2d_measurements_step(
-            s, im['targets'], im['weights'], meas['targets'], meas['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-            im['trial_jac'], meas['trial_meas'], meas['trial_meas_jac'], sigma, im['anchor'], pose_w, betas_w)
+    mkw = {} if meas is None else dict(meas=(meas['targets'], meas['weights']),
+                                       trial_meas=(meas['trial_meas'], meas['trial_meas_jac']))
+    want, wnxt, wacc = o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
+                                               im['trial_jac'], sigma, im['anchor'], pose_w, betas_w, **mkw)
     assert acc == wacc
     for k in ('loss', 'lambda', 'accepted'):
         assert np.array_equal(new[k], want[k], equal_nan=True), (k, new[k], want[k])
@@ -159,14 +156,8 @@ def test_groups_of_one_equal_the_2d_oracles(first, with_meas, sigma, pose_w, bet
     # in float64 the two eliminations agree to rounding
     new64, nxt64, _, _, _ = og.lm_groups_step(state, images, 10.0, 3.0, first, trial, sigma, pose_w, betas_w, meas,
                                               dtype=np.float64)
-    if meas is None:
-        _, w64, _ = o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-                                            im['trial_jac'], sigma, im['anchor'], pose_w, betas_w, dtype=np.float64)
-    else:
-        _, w64, _ = o2m.lm_keypoints_2d_measurements_step(
-            s, im['targets'], im['weights'], meas['targets'], meas['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-            im['trial_jac'], meas['trial_meas'], meas['trial_meas_jac'], sigma, im['anchor'], pose_w, betas_w,
-            dtype=np.float64)
+    _, w64, _ = o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
+                                        im['trial_jac'], sigma, im['anchor'], pose_w, betas_w, dtype=np.float64, **mkw)
     for k in ('rot', 'camera'):
         assert np.abs(nxt64[k][0] - w64[k]).max() <= 1e-10 * max(1.0, np.abs(w64[k]).max()), k
     assert np.abs(nxt64['betas'] - w64['betas']).max() <= 1e-10 * max(1.0, np.abs(w64['betas']).max())

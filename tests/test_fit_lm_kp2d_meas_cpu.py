@@ -1,6 +1,6 @@
-"""CPU: the float64 restatement of the stacked 2D keypoint + measurement LM step (tests/kp2dm_lm_oracle.py) pinned to
+"""CPU: the float64 restatement of the stacked 2D keypoint + measurement LM step (tests/kp2d_lm_oracle.py) pinned to
 J^T W J and J^T W r of the explicitly stacked Jacobian (projected keypoint rows, pose-prior rows, measurement rows), to
-kp2d_lm_oracle when every measurement is dropped, on NaN in dropped and in weighted measurements, and run as a plain
+the step without measurements when every measurement is dropped, on NaN in dropped and in weighted measurements, and run as a plain
 fp64 LM on a small nonlinear problem."""
 import math
 
@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 import kp2d_lm_oracle as o2
-import kp2dm_lm_oracle as o2m
 from test_fit_lm_kp2d_cpu import _expm, _problem
 
 P = 10              # _problem: two rotations, one betas, the camera
@@ -49,8 +48,8 @@ def test_normal_equations_equal_the_stacked_jacobian(sigma, pose_w, betas_w):
     mw[2] = 0.0                                              # a dropped measurement, NaN value and row
     meas, mjac = c['meas'].copy(), c['mjac'].copy()
     meas[2], mjac[2] = np.nan, np.nan
-    A, g, dg = o2m.normal_equations(c['tg'], c['w'], c['kp'], c['jac'], c['cam'], c['mt'], mw, meas, mjac, sigma,
-                                    c['rot'], c['anchor'], pose_w, c['beta'], betas_w)
+    A, g, dg = o2.normal_equations(c['tg'], c['w'], c['kp'], c['jac'], c['cam'], sigma, c['rot'], c['anchor'], pose_w,
+                                   c['beta'], betas_w, meas=(c['mt'], mw, meas, mjac))
     J2 = o2.jacobian_2d(c['kp'], c['jac'], c['cam'])
     p = o2.project(c['kp'], c['cam'])
     rows, wts, res = [], [], []
@@ -115,7 +114,7 @@ def _same(a, b):
 @pytest.mark.parametrize('first', [False, True])
 def test_dropped_measurements_reproduce_the_2d_oracle_exactly(first):
     """Every measurement weight <= 0, NaN in the dropped values and rows: state, lambda, loss and next trial equal
-    kp2d_lm_oracle's exactly, with the robust loss and both priors on."""
+    the step without measurements (meas None) exactly, with the robust loss and both priors on."""
     c = _case(12)
     state, trial, tkp, tjac, tmeas, tmjac = _step_inputs(c)
     nan5, nan51 = np.full(5, np.nan), np.full((5, 1), np.nan)
@@ -124,8 +123,8 @@ def test_dropped_measurements_reproduce_the_2d_oracle_exactly(first):
     for s in (state, s2):
         s['loss'] = np.float64(1e9 if not first else np.nan)
     mw = np.array([0.0, -1.0, 0.0, 0.0, -0.0])
-    got = o2m.lm_keypoints_2d_measurements_step(state, c['tg'], c['w'], c['mt'], mw, 10.0, 3.0, first, trial, tkp,
-                                                tjac, nan5, nan51, **_kw(c))
+    got = o2.lm_keypoints_2d_step(state, c['tg'], c['w'], 10.0, 3.0, first, trial, tkp, tjac, meas=(c['mt'], mw),
+                                  trial_meas=(nan5, nan51), **_kw(c))
     want = o2.lm_keypoints_2d_step(s2, c['tg'], c['w'], 10.0, 3.0, first, trial, tkp, tjac, **_kw(c))
     assert got[2] == want[2] and got[2]
     _same({k: v for k, v in got[0].items() if k not in ('meas', 'meas_jac')}, want[0])
@@ -137,17 +136,18 @@ def test_nan_in_a_dropped_measurement_changes_nothing_and_a_weighted_nan_rejects
     state, trial, tkp, tjac, tmeas, tmjac = _step_inputs(c)
     mw = MW.copy()
     mw[3] = 0.0
-    state['loss'] = np.float64(o2m.loss(c['tg'], c['w'], c['kp'], c['cam'], c['mt'], mw, c['meas'], c['sigma'],
-                                        c['rot'], c['anchor'], c['pose_w'], c['beta'], c['betas_w']) * 10)
-    args = (c['tg'], c['w'], c['mt'], mw, 10.0, 3.0, False, trial, tkp, tjac)
-    base = o2m.lm_keypoints_2d_measurements_step(state, *args, tmeas, tmjac, **_kw(c))
+    state['loss'] = np.float64(o2.loss(c['tg'], c['w'], c['kp'], c['cam'], c['sigma'], c['rot'], c['anchor'],
+                                       c['pose_w'], c['beta'], c['betas_w'], meas=(c['mt'], mw, c['meas'])) * 10)
+    args = (c['tg'], c['w'], 10.0, 3.0, False, trial, tkp, tjac)
+    kw = dict(_kw(c), meas=(c['mt'], mw))
+    base = o2.lm_keypoints_2d_step(state, *args, trial_meas=(tmeas, tmjac), **kw)
     assert base[2]
     # NaN in the dropped measurement, state and trial
     sn = dict(state, meas=state['meas'].copy(), meas_jac=state['meas_jac'].copy())
     tmn, tjn = tmeas.copy(), tmjac.copy()
     for t in (sn['meas'], sn['meas_jac'], tmn, tjn):
         t[3] = np.nan
-    got = o2m.lm_keypoints_2d_measurements_step(sn, *args, tmn, tjn, **_kw(c))
+    got = o2.lm_keypoints_2d_step(sn, *args, trial_meas=(tmn, tjn), **kw)
     assert got[2]
     skip = lambda d: {k: np.delete(v, 3, 0) if k in ('meas', 'meas_jac') else v for k, v in d.items()}  # noqa: E731
     _same(skip(got[0]), skip(base[0]))
@@ -155,7 +155,7 @@ def test_nan_in_a_dropped_measurement_changes_nothing_and_a_weighted_nan_rejects
     # a weighted NaN trial measurement: rejected, the state kept, lambda up, the step from the state
     tmn = tmeas.copy()
     tmn[1] = np.nan
-    new, nxt, acc = o2m.lm_keypoints_2d_measurements_step(state, *args, tmn, tmjac, **_kw(c))
+    new, nxt, acc = o2.lm_keypoints_2d_step(state, *args, trial_meas=(tmn, tmjac), **kw)
     assert not acc and new['accepted'] == 0 and new['lambda'] == state['lambda'] * 10.0
     for k in ('rot', 'betas', 'camera', 'keypoints', 'meas', 'meas_jac', 'loss'):
         assert np.array_equal(new[k], state[k], equal_nan=True), k
@@ -181,8 +181,8 @@ def test_fp64_lm_loss_non_increasing_and_height_fixes_the_scale(sigma):
     for it in range(60):
         k, j = evaluate(trial['rot'], trial['betas'])
         m, mj = _measure(trial['betas'])
-        state, trial, _ = o2m.lm_keypoints_2d_measurements_step(state, tg, w, mt, mw, 10.0, 3.0, it == 0, trial, k, j,
-                                                                m, mj, sigma=sigma, dtype=np.float64)
+        state, trial, _ = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, it == 0, trial, k, j, sigma=sigma,
+                                                  meas=(mt, mw), trial_meas=(m, mj), dtype=np.float64)
         losses.append(float(state['loss']))
     assert all(b <= a for a, b in zip(losses, losses[1:])), losses
     assert losses[-1] < 1e-14, losses

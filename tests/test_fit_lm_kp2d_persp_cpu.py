@@ -1,4 +1,4 @@
-"""CPU: the float64 restatement of the perspective 2D keypoint LM step (tests/kp2d_persp_lm_oracle.py) pinned to
+"""CPU: the float64 restatement of the perspective 2D keypoint LM step (tests/kp2d_lm_oracle.py with intrinsics) pinned to
 central differences of its projection and loss (all columns, t included), the depth rule, a plain fp64 LM on a small
 nonlinear problem with rotations, a betas and the translation; fit.perspective_start against the crop projection; and
 PerspectiveCamera against the reference class's outputs."""
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_persp_lm_oracle as op
+import kp2d_lm_oracle as o2
 from test_fit_lm_kp2d_cpu import _expm, _problem
 
 INTR = np.array([1000.0, 500.0, 480.0])
@@ -21,7 +21,7 @@ def _case(seed, sigma_noise=20.0):
     rot = np.stack([_expm(rng.normal(size=3) * 0.5) for _ in range(2)])
     beta = np.array([0.3])
     kp, jac = evaluate(rot, beta)
-    tg = op.project(kp, T0, INTR) + rng.normal(size=(12, 2)) * sigma_noise
+    tg = o2.project(kp, T0, INTR) + rng.normal(size=(12, 2)) * sigma_noise
     w = rng.uniform(0.5, 1.5, 12)
     w[3], tg[3] = 0.0, np.nan
     return evaluate, rng, rot, beta, kp, jac, tg, w
@@ -38,14 +38,14 @@ def _at(evaluate, rot, beta, theta):
 def test_projected_jacobian_vs_central_differences_on_every_column():
     evaluate, _, rot, beta, kp, jac, _, _ = _case(11)
     jac[:, 7:] = 7.0                          # the 3D transl columns are not read: J_t = I
-    J2 = op.jacobian_persp(kp, jac, T0, INTR)
+    J2 = o2.jacobian_persp(kp, jac, T0, INTR)
     h = 1e-6
     fd = np.zeros((24, 10))
     for i in range(10):
         e = np.zeros(10)
         e[i] = h
         a, b = _at(evaluate, rot, beta, e), _at(evaluate, rot, beta, -e)
-        fd[:, i] = (op.project(a[3], a[2], INTR) - op.project(b[3], b[2], INTR)).reshape(-1) / (2 * h)
+        fd[:, i] = (o2.project(a[3], a[2], INTR) - o2.project(b[3], b[2], INTR)).reshape(-1) / (2 * h)
     assert np.abs(J2 - fd).max() <= 1e-6 * np.abs(fd).max()
 
 
@@ -57,11 +57,11 @@ def test_gradient_is_half_the_loss_gradient(sigma, pose_w, betas_w):
     evaluate, rng, rot, beta, kp, jac, tg, w = _case(12)
     anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
     jac[9:12] = np.nan
-    _, g, _ = op.normal_equations(tg, w, kp, jac, T0, INTR, sigma, rot, anchor, pose_w, beta, betas_w)
+    _, g, _ = o2.normal_equations(tg, w, kp, jac, T0, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)
 
     def L(theta):
         R, b, t, k = _at(evaluate, rot, beta, theta)
-        return op.loss(tg, w, k, t, INTR, sigma, R, anchor, pose_w, b, betas_w)
+        return o2.loss(tg, w, k, t, sigma, R, anchor, pose_w, b, betas_w, intr=INTR)
 
     h = 1e-6
     fd = np.zeros(10)
@@ -76,23 +76,23 @@ def test_depth_rule():
     """A weighted keypoint at Y_z <= 0 makes the loss +inf and the trial is rejected; a dropped one is ignored; a bad
     focal length is +inf; a start behind the camera reports NaN and does not move."""
     evaluate, _, rot, beta, kp, jac, tg, w = _case(13)
-    assert math.isfinite(op.loss(tg, w, kp, T0, INTR))
+    assert math.isfinite(o2.loss(tg, w, kp, T0, intr=INTR))
     behind = kp.copy()
     behind[5, 2] = -T0[2] - 0.1              # Y_z = -0.1
-    assert op.loss(tg, w, behind, T0, INTR) == math.inf
+    assert o2.loss(tg, w, behind, T0, intr=INTR) == math.inf
     behind[5, 2] = -T0[2]                    # Y_z = 0
-    assert op.loss(tg, w, behind, T0, INTR) == math.inf
+    assert o2.loss(tg, w, behind, T0, intr=INTR) == math.inf
     dropped = kp.copy()
     dropped[3, 2] = -T0[2] - 1.0             # keypoint 3 has weight 0
-    assert op.loss(tg, w, dropped, T0, INTR) == op.loss(tg, w, kp, T0, INTR)
+    assert o2.loss(tg, w, dropped, T0, intr=INTR) == o2.loss(tg, w, kp, T0, intr=INTR)
     for f in (0.0, -1000.0, math.nan, math.inf):
-        assert op.loss(tg, w, kp, T0, [f, 500.0, 480.0]) == math.inf
+        assert o2.loss(tg, w, kp, T0, intr=[f, 500.0, 480.0]) == math.inf
     state = {'rot': rot, 'betas': beta, 'transl': T0, 'keypoints': kp, 'jac': jac, 'lambda': np.float32(1e-3),
-             'loss': np.float32(op.loss(tg, w, kp, T0, INTR))}
+             'loss': np.float32(o2.loss(tg, w, kp, T0, intr=INTR))}
     trial = {'rot': rot, 'betas': beta, 'transl': T0}
-    new, nxt, acc = op.lm_keypoints_2d_perspective_step(state, tg, w, INTR, 10.0, 3.0, False, trial, behind, jac)
+    new, nxt, acc = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, False, trial, behind, jac, intr=INTR)
     assert not acc and new['loss'] == state['loss']
-    new, nxt, acc = op.lm_keypoints_2d_perspective_step({}, tg, w, INTR, 10.0, 3.0, True, trial, behind, jac)
+    new, nxt, acc = o2.lm_keypoints_2d_step({}, tg, w, 10.0, 3.0, True, trial, behind, jac, intr=INTR)
     assert acc and math.isnan(new['loss'])
     assert all(np.array_equal(nxt[k], np.asarray(trial[k], np.float32)) for k in ('rot', 'betas', 'transl'))
 
@@ -103,7 +103,7 @@ def test_fp64_lm_recovers_rotations_shape_and_translation(sigma):
     R1, R2 = _expm(rng.normal(size=3) * 0.6), _expm(rng.normal(size=3) * 0.6)
     bstar, tstar = np.array([0.6]), np.array([0.3, -0.1, 4.0])
     kp, _ = evaluate(np.stack([R1, R2]), bstar)
-    tg = op.project(kp, tstar, INTR)
+    tg = o2.project(kp, tstar, INTR)
     w = np.ones(12)
     w[2], tg[2] = 0.0, np.nan
     trial = {'rot': np.stack([R1 @ _expm(rng.normal(size=3) * 0.2), R2 @ _expm(rng.normal(size=3) * 0.2)]),
@@ -111,8 +111,8 @@ def test_fp64_lm_recovers_rotations_shape_and_translation(sigma):
     state, losses = {}, []
     for it in range(60):
         k, j = evaluate(trial['rot'], trial['betas'])
-        state, trial, _ = op.lm_keypoints_2d_perspective_step(state, tg, w, INTR, 10.0, 3.0, it == 0, trial, k, j,
-                                                              sigma=sigma, dtype=np.float64)
+        state, trial, _ = o2.lm_keypoints_2d_step(state, tg, w, 10.0, 3.0, it == 0, trial, k, j, sigma=sigma,
+                                                  intr=INTR, dtype=np.float64)
         losses.append(float(state['loss']))
     assert all(b <= a for a, b in zip(losses, losses[1:])), losses
     assert losses[-1] < 1e-12, losses

@@ -7,7 +7,7 @@ import math
 import numpy as np
 import pytest
 
-import kp2d_persp_lm_oracle as op
+import kp2d_lm_oracle as o2
 import kp2d_sequence_lm_oracle as osq
 import kp2dg_lm_oracle as og
 from test_fit_lm_kp2d_cpu import _expm, _problem
@@ -64,7 +64,7 @@ def _sequence(seed, T, sigma_noise=5.0):
         rot = np.stack([base[j] @ _expm(rng.normal(size=3) * 0.1 + 0.05 * t) for j in range(2)])
         tr = np.array([0.1 * t - 0.5, -0.2, 5.0 + 0.05 * t])
         kp, _ = evaluate(rot, beta)
-        tg = op.project(kp, tr, INTR) + rng.normal(size=(12, 2)) * sigma_noise
+        tg = o2.project(kp, tr, INTR) + rng.normal(size=(12, 2)) * sigma_noise
         w = rng.uniform(0.5, 1.5, 12)
         w[3], tg[3] = 0.0, np.nan
         anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
@@ -123,25 +123,24 @@ def test_one_frame_is_the_perspective_step(first, terms):
     rng = np.random.default_rng(32)
     st, trial = _step_args(evaluate, frames, rots, trs, beta, rng)
     fr = frames[0]
-    lcur = np.float32(op.loss(fr['targets'], fr['weights'], st['keypoints'][0], trs[0], INTR, sigma, rots[0],
-                              fr['anchor'], pw, beta, bw) * (0.5 if first else 1.01))
+    lcur = np.float32(o2.loss(fr['targets'], fr['weights'], st['keypoints'][0], trs[0], sigma, rots[0], fr['anchor'],
+                              pw, beta, bw, intr=INTR) * (0.5 if first else 1.01))
     s1 = dict(st, loss=lcur, **{'lambda': np.float32(0.02)}, accepted=0)
     new, nxt, acc = osq.lm_sequence_step(s1, frames, 10.0, 3.0, first, trial, sigma, pw, bw, 1e4, 1e4)
     s2 = {'rot': rots[0], 'betas': beta, 'transl': trs[0], 'keypoints': st['keypoints'][0], 'jac': st['jac'][0],
           'loss': lcur, 'lambda': np.float32(0.02), 'accepted': 0}
     tr2 = {'rot': trial['rot'][0], 'betas': trial['betas'], 'transl': trial['transl'][0]}
-    new2, nxt2, acc2 = op.lm_keypoints_2d_perspective_step(s2, fr['targets'], fr['weights'], INTR, 10.0, 3.0, first,
-                                                           tr2, fr['trial_kp'], fr['trial_jac'], sigma, fr['anchor'],
-                                                           pw, bw)
+    new2, nxt2, acc2 = o2.lm_keypoints_2d_step(s2, fr['targets'], fr['weights'], 10.0, 3.0, first, tr2, fr['trial_kp'],
+                                               fr['trial_jac'], sigma, fr['anchor'], pw, bw, intr=INTR)
     assert acc == acc2 and (acc or not first)
     assert new['loss'] == new2['loss'] and new['lambda'] == new2['lambda'] and new['accepted'] == new2['accepted']
     # the step to fp32 rounding of the same fp64 values (the sweep and the full solve agree to ~1e-12)
     for a, b in ((nxt['rot'][0], nxt2['rot']), (nxt['transl'][0], nxt2['transl']), (nxt['betas'], nxt2['betas'])):
         assert np.abs(np.asarray(a, np.float64) - b).max() <= 1e-6 * max(1.0, np.abs(b).max())
     new64, nxt64, _ = osq.lm_sequence_step(s1, frames, 10.0, 3.0, first, trial, sigma, pw, bw, dtype=np.float64)
-    new64b, nxt64b, _ = op.lm_keypoints_2d_perspective_step(s2, fr['targets'], fr['weights'], INTR, 10.0, 3.0, first,
-                                                            tr2, fr['trial_kp'], fr['trial_jac'], sigma, fr['anchor'],
-                                                            pw, bw, dtype=np.float64)
+    new64b, nxt64b, _ = o2.lm_keypoints_2d_step(s2, fr['targets'], fr['weights'], 10.0, 3.0, first, tr2,
+                                                fr['trial_kp'], fr['trial_jac'], sigma, fr['anchor'], pw, bw, intr=INTR,
+                                                dtype=np.float64)
     for a, b in ((nxt64['rot'][0], nxt64b['rot']), (nxt64['transl'][0], nxt64b['transl']),
                  (nxt64['betas'], nxt64b['betas'])):
         assert np.abs(a - b).max() <= 1e-12 * max(1.0, np.abs(b).max())
@@ -164,8 +163,8 @@ def test_zero_smoothness_is_the_dense_grouped_perspective_step():
     N = T * n1 + nb
     M, rhs = np.zeros((N, N)), np.zeros(N)
     for t, fr in enumerate(frames):
-        A, g, _ = op.normal_equations(fr['targets'], fr['weights'], new['keypoints'][t], new['jac'][t],
-                                      new['transl'][t], INTR, sigma, new['rot'][t], fr['anchor'], pw)
+        A, g, _ = o2.normal_equations(fr['targets'], fr['weights'], new['keypoints'][t], new['jac'][t],
+                                      new['transl'][t], sigma, new['rot'][t], fr['anchor'], pw, intr=INTR)
         perm = og.reorder(2, nb)
         A, g = A[perm][:, perm], g[perm]
         a = slice(t * n1, (t + 1) * n1)
@@ -181,8 +180,8 @@ def test_zero_smoothness_is_the_dense_grouped_perspective_step():
         assert np.abs(nxt['transl'][t] - (new['transl'][t] + d[t * n1 + 6:t * n1 + 9])).max() <= 1e-10
     assert np.abs(nxt['betas'] - (new['betas'] + d[T * n1:])).max() <= 1e-10
     # and the loss is the sum of the frames' perspective losses + the betas prior, with no smoothness term
-    L = sum(op.loss(fr['targets'], fr['weights'], fr['trial_kp'], trial['transl'][t], INTR, sigma, trial['rot'][t],
-                    fr['anchor'], pw) for t, fr in enumerate(frames))
+    L = sum(o2.loss(fr['targets'], fr['weights'], fr['trial_kp'], trial['transl'][t], sigma, trial['rot'][t],
+                    fr['anchor'], pw, intr=INTR) for t, fr in enumerate(frames))
     assert math.isclose(float(new['loss']), L + bw * float(np.sum(trial['betas'] ** 2)), rel_tol=1e-12)
 
 

@@ -12,7 +12,7 @@ import torch
 import kp2d_lm_oracle as o2
 import kp2d_shared_pose_lm_oracle as osp
 import kp2dg_lm_oracle as og
-import kp2dm_lm_oracle as o2m
+from oracle.lm_oracle import meas_loss
 from test_fit_lm_kp2d_cpu import _expm, _problem
 
 K = 12
@@ -53,9 +53,9 @@ def _group_state(images, state, anchor, sigma, pose_w, betas_w, meas=None):
     L = 0.0
     for i, im in enumerate(images):
         L += o2.loss(im['targets'], im['weights'], state['keypoints'][i], state['camera'][i], sigma)
-    L += osp.prior_loss(state['rot'][0], anchor, pose_w) if pose_w > 0 else 0.0
+    L += o2.prior_loss(state['rot'][0][1:], anchor[1:], pose_w) if pose_w > 0 else 0.0
     if meas is not None:
-        L += o2m.meas_loss(meas['targets'], meas['weights'], state['meas'])
+        L += meas_loss(meas['targets'], meas['weights'], state['meas'])
     if betas_w > 0:
         L += float(np.float32(betas_w)) * float(np.sum(np.asarray(state['betas']) ** 2))
     return np.float64(L)
@@ -165,12 +165,10 @@ def test_groups_of_one_equal_the_2d_oracles(first, with_meas, sigma, pose_w, bet
     t = {'rot': trial['rot'][0], 'camera': trial['camera'][0], 'betas': trial['betas']}
 
     def two_d(dtype):
-        if meas is None:
-            return o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-                                           im['trial_jac'], sigma, anchor, pose_w, betas_w, dtype=dtype)
-        return o2m.lm_keypoints_2d_measurements_step(
-            s, im['targets'], im['weights'], meas['targets'], meas['weights'], 10.0, 3.0, first, t, im['trial_kp'],
-            im['trial_jac'], meas['trial_meas'], meas['trial_meas_jac'], sigma, anchor, pose_w, betas_w, dtype=dtype)
+        mkw = {} if meas is None else dict(meas=(meas['targets'], meas['weights']),
+                                           trial_meas=(meas['trial_meas'], meas['trial_meas_jac']))
+        return o2.lm_keypoints_2d_step(s, im['targets'], im['weights'], 10.0, 3.0, first, t, im['trial_kp'],
+                                       im['trial_jac'], sigma, anchor, pose_w, betas_w, dtype=dtype, **mkw)
     new, nxt, acc, _, _ = osp.shared_pose_step(state, images, 10.0, 3.0, first, trial, anchor, sigma, pose_w, betas_w,
                                                meas)
     want, wnxt, wacc = two_d(np.float32)

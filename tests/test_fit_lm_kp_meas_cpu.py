@@ -1,5 +1,5 @@
-"""CPU: the float64 restatement of the stacked keypoint + measurement LM step (tests/kpm_lm_oracle.py): it reduces to
-the keypoint step without measurement rows, its step solves the damped normal equations of the stacked weighted
+"""CPU: the float64 restatement of the stacked keypoint + measurement LM step (tests/kp_lm_oracle.py with `meas`): it
+reduces to the keypoint step without measurement rows, its step solves the damped normal equations of the stacked weighted
 residual, its accept / reject / lambda sequence, and it fits a small nonlinear problem with a non-increasing loss."""
 import math
 
@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 
 import kp_lm_oracle
-import kpm_lm_oracle
 
 K, NB, N_ROT = 10, 2, 2
 P = 3 * N_ROT + NB + 3
@@ -74,8 +73,8 @@ def test_reduces_to_keypoint_step_without_measurement_rows():
         kp, jac, _, _ = [np.asarray(x, np.float32) for x in evaluate(trial_a['rot'], trial_a['betas'], trial_a['transl'])]
         nan5, nanj = np.full(5, np.nan, np.float32), np.full((5, NB), np.nan, np.float32)
         sa, trial_a, acc_a = kp_lm_oracle.lm_keypoints_step(sa, target, w, 10.0, 3.0, it == 0, trial_a, kp, jac)
-        sb, trial_b, acc_b = kpm_lm_oracle.lm_keypoints_measurements_step(sb, target, w, mt, mw, 0.0, 10.0, 3.0, it == 0,
-                                                                          trial_b, kp, jac, nan5, nanj)
+        sb, trial_b, acc_b = kp_lm_oracle.lm_keypoints_step(sb, target, w, 10.0, 3.0, it == 0, trial_b, kp, jac,
+                                                            meas=(mt, mw), trial_meas=(nan5, nanj), betas_weight=0.0)
         assert acc_a == acc_b
         for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'lambda', 'accepted'):
             assert np.array_equal(sa[k], sb[k]), (it, k)
@@ -98,8 +97,9 @@ def test_delta_solves_stacked_normal_equations(rho):
              'betas': rng.normal(size=NB) * 0.5, 'transl': rng.normal(size=3) * 0.1}
     kp, jac, meas, mjac = evaluate(trial['rot'], trial['betas'], trial['transl'])
     meas[1], mjac[1] = np.nan, np.nan                            # dropped: never read
-    new, _, acc, delta = kpm_lm_oracle.lm_keypoints_measurements_step(
-        {}, target, w, mt, mw, rho, 10.0, 3.0, True, trial, kp, jac, meas, mjac, dtype=np.float64, return_delta=True)
+    new, _, acc, delta = kp_lm_oracle.lm_keypoints_step(
+        {}, target, w, 10.0, 3.0, True, trial, kp, jac, meas=(mt, mw), trial_meas=(meas, mjac), betas_weight=rho,
+        dtype=np.float64, return_delta=True)
     assert acc
     o = 3 * N_ROT
     rows, res = [], []
@@ -149,8 +149,8 @@ def test_accept_reject_and_lambda_sequence():
         kp, jac, m, mj = ev(x)
         if edit:
             edit(m, mj)
-        return kpm_lm_oracle.lm_keypoints_measurements_step(state, tgt_kp, w, tgt_m, mw, rho, 10.0, 3.0, first, x, kp,
-                                                            jac, m, mj)
+        return kp_lm_oracle.lm_keypoints_step(state, tgt_kp, w, 10.0, 3.0, first, x, kp, jac, meas=(tgt_m, mw),
+                                              trial_meas=(m, mj), betas_weight=rho)
 
     s, _, acc = step({}, point(0.2), True)
     assert acc and s['accepted'] == 0
@@ -186,9 +186,8 @@ def test_fits_keypoints_and_measurements_with_non_increasing_loss():
     trial, state, losses = _start(), {}, []
     for it in range(40):
         kp, jac, m, mj = evaluate(trial['rot'], trial['betas'], trial['transl'])
-        state, trial, _ = kpm_lm_oracle.lm_keypoints_measurements_step(state, tgt_kp, w, tgt_m, mw, 0.0, 10.0, 3.0,
-                                                                       it == 0, trial, kp, jac, m, mj,
-                                                                       dtype=np.float64)
+        state, trial, _ = kp_lm_oracle.lm_keypoints_step(state, tgt_kp, w, 10.0, 3.0, it == 0, trial, kp, jac,
+                                                         meas=(tgt_m, mw), trial_meas=(m, mj), dtype=np.float64)
         losses.append(float(state['loss']))
     assert all(b <= a for a, b in zip(losses, losses[1:])), losses
     assert losses[-1] < 1e-12, losses

@@ -9,7 +9,6 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
-import kp2dm_lm_oracle as o2m
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -98,9 +97,9 @@ def _state_np(c, b):
          'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
     if 'meas' in c:
         s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
-        s['loss'] = np.float32(o2m.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], n(c['mt'][b]),
-                                        n(c['mw'][b]), s['meas'], c['sigma'], s['rot'], n(c['anchor'][b]), c['pw'],
-                                        s['betas'], c['bw']))
+        s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
+                                       n(c['anchor'][b]), c['pw'], s['betas'], c['bw'],
+                                       meas=(n(c['mt'][b]), n(c['mw'][b]), s['meas'])))
     else:
         s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
                                        n(c['anchor'][b]), c['pw'], s['betas'], c['bw']))
@@ -150,9 +149,10 @@ def _run_step(c, first):
     for b in range(B):
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'camera': n(c['tcam'][b])}
         if meas:
-            new, want, acc = o2m.lm_keypoints_2d_measurements_step(
-                s_np[b], n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), 10.0, 3.0, first, tr,
-                n(c['tkp'][b]), n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]), anchor=n(c['anchor'][b]), **kw)
+            new, want, acc = o2.lm_keypoints_2d_step(
+                s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
+                anchor=n(c['anchor'][b]), meas=(n(c['mt'][b]), n(c['mw'][b])),
+                trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), **kw)
         else:
             new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
                                                      n(c['tkp'][b]), n(c['tjac'][b]), anchor=n(c['anchor'][b]), **kw)

@@ -1,6 +1,6 @@
 """GPU: the whole-body 2D fit.  The expression-aware keypoint Jacobian (shapy_smplx_keypoint_jacobian_expr) against
 the 22-joint launch at psi = 0, the float64 restatement and the forward, on every model shape; the wide LM step
-(shapy_fit_lm_keypoints_2d_expressive_step and its perspective entry) against tests/kp2d_expressive_lm_oracle.py at
+(shapy_fit_lm_keypoints_2d_expressive_step and its perspective entry) against tests/kp2d_lm_oracle.py at
 P = 7 to 200, bit for bit against today's 2D steps at n_rot = 22 without expression over a 50-iteration loop, its
 argument errors; and fit_body_to_keypoints_2d(pose_width=55, fit_expression=True) end to end: launches, no host
 synchronisation, monotone losses, determinism, batch independence, Adam, the command line and quality."""
@@ -11,9 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_expressive_lm_oracle as ox
 import kp2d_lm_oracle as o2
-import kp2d_persp_lm_oracle as op
+import kp_lm_oracle
 from shapy_b200 import synth
 from test_gpu_fit_lm_keypoints_2d import _bits, _rodrigues
 from test_gpu_model_shapes import TOL, _inputs
@@ -61,7 +60,8 @@ def test_jacobian_expr(name, n_rot):
     kp, jac = kp.double().cpu().numpy(), jac.double().cpu().numpy()
     worst = 0.0
     for b in range(B):
-        k64, j64 = ox.keypoint_jacobian_expr(m, x['betas'][b], x['expression'][b], x['rot'][b], x['transl'][b])
+        k64, j64 = kp_lm_oracle.keypoint_jacobian(m, x['betas'][b], x['rot'][b], x['transl'][b],
+                                                  expr=x['expression'][b])
         assert np.abs(kp[b] - k64).max() <= 1e-5 * np.abs(k64).max(), b
         for block, cols in (('rot', slice(0, 3 * n_rot)), ('betas', slice(3 * n_rot, P0)),
                             ('expression', slice(P0, P0 + NE))):
@@ -120,7 +120,7 @@ def _case(n_rot, nb, ne, K, terms, persp):
 
     def proj(k, c, b):
         if persp:
-            return torch.from_numpy(op.project(k.numpy(), c.numpy(), intr[b].numpy())).float()
+            return torch.from_numpy(o2.project(k.numpy(), c.numpy(), intr[b].numpy())).float()
         return torch.from_numpy(o2.project(k.numpy(), c.numpy())).float()
     noise = 5.0 if persp else 0.02
     tg = torch.stack([proj(kp[b], last[b], b) for b in range(B)]) + noise * rn(B, K, 2)
@@ -164,9 +164,9 @@ def _state_np(c, b):
     s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'expression': n(c['expr'][b]), _lastkey(c): n(c['last'][b]),
          'keypoints': n(c['kp'][b]), 'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
     kw = _kw(c, b)
-    s['loss'] = np.float32(ox.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s[_lastkey(c)], kw['sigma'], s['rot'],
-                                   kw['anchor'], kw['pose_w'], kw['joint_w'], s['betas'], kw['betas_w'],
-                                   s['expression'], kw['expr_w'], kw['intr']))
+    s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s[_lastkey(c)], kw['sigma'], s['rot'],
+                                   kw['anchor'], kw['pose_w'], s['betas'], kw['betas_w'], kw['intr'], kw['joint_w'],
+                                   s['expression'], kw['expr_w']))
     return s
 
 
@@ -209,8 +209,8 @@ def test_step_kernel_vs_oracle(n_rot, nb, ne, K, first, terms, persp):
     flags, worst = [], 0.0
     for b in range(B):
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'expression': n(c['texpr'][b]), lk: n(c['tlast'][b])}
-        new, want, acc = ox.lm_keypoints_2d_expressive_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first,
-                                                            tr, n(c['tkp'][b]), n(c['tjac'][b]), **_kw(c, b))
+        new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
+                                                 n(c['tkp'][b]), n(c['tjac'][b]), **_kw(c, b))
         flags.append(acc)
         assert got['accepted'][b] == new['accepted'], b
         assert got['lambda'][b] == new['lambda'] or np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), \
@@ -493,9 +493,9 @@ def test_adam_loss_matches_the_oracle():
                                          torch.tensor([1.0, 0, 0, 1.0, 0, 0], device='cuda').repeat(B, 33)], 1))
     n = lambda t: t.detach().double().cpu().numpy()  # noqa: E731
     for b in range(B):
-        want = ox.loss(n(x[b]), np.ones(x.shape[1]), n(res['keypoints'][b]), n(res['camera'][b]), 0.2,
-                       n(res['full_pose_mat'][b]), n(anchor[b]), 0.0, jw, n(res['betas'][b]), 0.01,
-                       n(res['expression'][b]), 0.05)
+        want = o2.loss(n(x[b]), np.ones(x.shape[1]), n(res['keypoints'][b]), n(res['camera'][b]), 0.2,
+                       n(res['full_pose_mat'][b]), n(anchor[b]), 0.0, n(res['betas'][b]), 0.01, joint_w=jw,
+                       expr=n(res['expression'][b]), expr_w=0.05)
         assert abs(float(res['loss'][b]) - want) <= 1e-4 * abs(want), (b, float(res['loss'][b]), want)
 
 

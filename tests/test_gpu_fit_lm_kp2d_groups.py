@@ -11,7 +11,7 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
-from kpm_lm_oracle import meas_loss
+from oracle.lm_oracle import meas_loss
 from test_gpu_fit_lm_kp2d_meas import NAMES, N_ROT, _bits, _measure, _rodrigues, model  # noqa: F401
 from test_gpu_fit_lm_kp2d_meas import quality as quality_2d
 

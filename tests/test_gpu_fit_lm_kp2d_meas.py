@@ -1,5 +1,5 @@
 """GPU: the stacked 2D keypoint + measurement Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_measurements_step)
-against its NumPy restatement (tests/kp2dm_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_meas_cpu.py) and against
+against its NumPy restatement (tests/kp2d_lm_oracle.py with `meas`, pinned by tests/test_fit_lm_kp2d_meas_cpu.py) and against
 shapy_fit_lm_keypoints_2d_step when every measurement is dropped; and fit_body_to_keypoints_2d with known measurements
 end to end on the synthetic SMPL-X: unchanged without them, deterministic, batch independent, monotone, never
 synchronising, and the quality with known height and mass against the keypoints alone."""
@@ -10,7 +10,6 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
-import kp2dm_lm_oracle as o2m
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -107,9 +106,9 @@ def _state(c, with_meas=True):
     """The state and trial tensors on the device, the state's loss from the oracle (float32)."""
     B = c['rot'].shape[0]
     n = lambda t: t.numpy()  # noqa: E731
-    loss = torch.tensor([o2m.loss(n(c['tg'][b]), n(c['w'][b]), n(c['kp'][b]), n(c['cam'][b]), n(c['mt'][b]),
-                                  n(c['mw'][b]), n(c['meas'][b]), c['sigma'], n(c['rot'][b]), n(c['anchor'][b]),
-                                  c['pw'], n(c['betas'][b]), c['bw']) for b in range(B)]).float()
+    loss = torch.tensor([o2.loss(n(c['tg'][b]), n(c['w'][b]), n(c['kp'][b]), n(c['cam'][b]), c['sigma'],
+                                 n(c['rot'][b]), n(c['anchor'][b]), c['pw'], n(c['betas'][b]), c['bw'],
+                                 meas=(n(c['mt'][b]), n(c['mw'][b]), n(c['meas'][b]))) for b in range(B)]).float()
     cu = lambda t: t.cuda().contiguous()  # noqa: E731
     state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
              'jac': cu(c['jac']), 'loss': cu(loss), 'lambda': cu(c['lam']),
@@ -145,10 +144,10 @@ def test_step_kernel_vs_oracle(model, first, terms, derivative):
         s = {k: s0[k][b] for k in s0}
         s['accepted'] = 0
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'camera': n(c['tcam'][b])}
-        new, want, acc = o2m.lm_keypoints_2d_measurements_step(
-            s, n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]),
-            n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]), sigma=c['sigma'], anchor=n(c['anchor'][b]),
-            pose_w=c['pw'], betas_w=c['bw'])
+        new, want, acc = o2.lm_keypoints_2d_step(
+            s, n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]), sigma=c['sigma'],
+            anchor=n(c['anchor'][b]), pose_w=c['pw'], betas_w=c['bw'], meas=(n(c['mt'][b]), n(c['mw'][b])),
+            trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])))
         flags.append(acc)
         assert got['accepted'][b] == new['accepted'], b
         # softplus' exp / log1p may round differently on the device: loss and lambda to fp32 rounding

@@ -1,5 +1,5 @@
 """GPU: the perspective 2D keypoint Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_perspective_step) against its
-NumPy restatement (tests/kp2d_persp_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_persp_cpu.py) at P = 7 to 96, its
+NumPy restatement (tests/kp2d_lm_oracle.py with intrinsics, pinned by tests/test_fit_lm_kp2d_persp_cpu.py) at P = 7 to 96, its
 measurement entry against it, argument errors, and fit_body_to_keypoints_2d(focal_length=...) end to end on the
 synthetic SMPL-X: monotone losses, no host synchronisation, launches per iteration, determinism, batch independence,
 the returned loss, Adam, the command line, and quality against the weak-perspective fit."""
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_persp_lm_oracle as op
+import kp2d_lm_oracle as o2
 from shapy_b200 import synth
 from test_gpu_fit_lm_keypoints_2d import _bits, _get, _rodrigues
 
@@ -49,7 +49,7 @@ def _step_case(n_rot, nb, K, terms):
     tkp[1] = kp[1] + 0.1
     intr = torch.tensor([F, *PP]).repeat(B, 1)
     intr[5:, 0] = 800.0 + 400.0 * torch.rand(2, generator=gen)
-    proj = lambda k, t, b: torch.from_numpy(op.project(k.numpy(), t.numpy(), intr[b].numpy())).float()  # noqa: E731
+    proj = lambda k, t, b: torch.from_numpy(o2.project(k.numpy(), t.numpy(), intr[b].numpy())).float()  # noqa: E731
     tg = torch.stack([proj(kp[b], tr[b], b) for b in range(B)]) + 5.0 * rn(B, K, 2)
     tg[0], tg[1] = proj(tkp[0], ttr[0], 0), proj(kp[1], tr[1], 1)
     tkp[2, 0, 1] = float('nan')
@@ -72,8 +72,8 @@ def _state_np(c, b):
     n = lambda t: t.numpy()  # noqa: E731
     s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'transl': n(c['tr'][b]), 'keypoints': n(c['kp'][b]),
          'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-    s['loss'] = np.float32(op.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['transl'], n(c['intr'][b]),
-                                   c['sigma'], s['rot'], n(c['anchor'][b]), c['pw'], s['betas'], c['bw']))
+    s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['transl'], c['sigma'], s['rot'],
+                                   n(c['anchor'][b]), c['pw'], s['betas'], c['bw'], intr=n(c['intr'][b])))
     return s
 
 
@@ -116,10 +116,10 @@ def test_step_kernel_vs_oracle(n_rot, nb, K, first, terms):
     flags, worst = [], 0.0
     for b in range(B):
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttr'][b])}
-        new, want, acc = op.lm_keypoints_2d_perspective_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), n(c['intr'][b]),
-                                                             10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
-                                                             sigma=c['sigma'], anchor=n(c['anchor'][b]),
-                                                             pose_w=c['pw'], betas_w=c['bw'])
+        new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
+                                                 n(c['tkp'][b]), n(c['tjac'][b]), sigma=c['sigma'],
+                                                 anchor=n(c['anchor'][b]), pose_w=c['pw'], betas_w=c['bw'],
+                                                 intr=n(c['intr'][b]))
         flags.append(acc)
         assert got['accepted'][b] == new['accepted'], b
         assert np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), (b, got['lambda'][b], new['lambda'])

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_persp_lm_oracle as op
+import kp2d_lm_oracle as o2
 import kp2d_sequence_lm_oracle as osq
 from shapy_b200 import synth
 from test_gpu_fit_lm_keypoints_2d import _bits, _get, _rodrigues
@@ -47,7 +47,7 @@ def _step_case(n_rot, nb, K, terms, lens=LENS, seed=0):
     tkp, tjac = kp + 0.01 * rn(B, K, 3), jac + 0.03 * rn(B, 3 * K, P)
     intr = torch.tensor([F, *PP]).repeat(B, 1)
     intr[:, 0] *= 0.8 + 0.4 * torch.rand(B, generator=gen)
-    proj = lambda k, t, b: torch.from_numpy(op.project(k.numpy(), t.numpy(), intr[b].numpy())).float()  # noqa: E731
+    proj = lambda k, t, b: torch.from_numpy(o2.project(k.numpy(), t.numpy(), intr[b].numpy())).float()  # noqa: E731
     tg = torch.stack([proj(kp[b], tr[b], b) for b in range(B)]) + 5.0 * rn(B, K, 2)
     for b in range(off[0], off[1]):
         tg[b], anchor[b] = proj(tkp[b], ttr[b], b), trot[b]
@@ -82,8 +82,8 @@ def _state_loss(c, s):
     r = range(c['off'][s], c['off'][s + 1])
     L = 0.0
     for i in r:
-        L += op.loss(_n(c['tg'][i]), _n(c['w'][i]), _n(c['kp'][i]), _n(c['tr'][i]), _n(c['intr'][i]), sigma,
-                     _n(c['rot'][i]), _n(c['anchor'][i]), pw)
+        L += o2.loss(_n(c['tg'][i]), _n(c['w'][i]), _n(c['kp'][i]), _n(c['tr'][i]), sigma, _n(c['rot'][i]),
+                     _n(c['anchor'][i]), pw, intr=_n(c['intr'][i]))
         if i + 1 in r:
             L += osq.smooth_loss(_n(c['rot'][i]), _n(c['rot'][i + 1]), _n(c['tr'][i]), _n(c['tr'][i + 1]), srw, stw)
     if bw > 0:

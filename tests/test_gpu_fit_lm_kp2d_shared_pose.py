@@ -14,7 +14,7 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2d_shared_pose_lm_oracle as osp
-from kpm_lm_oracle import meas_loss
+from oracle.lm_oracle import meas_loss
 from test_gpu_fit_lm_kp2d_groups import quality as quality_groups
 from test_gpu_fit_lm_kp2d_meas import NAMES, N_ROT, _bits, _measure, _rodrigues, model  # noqa: F401
 from test_gpu_fit_lm_kp2d_meas import quality as quality_2d
@@ -45,7 +45,7 @@ def _state_loss(c, g, with_meas):
     for i in range(i0, c['off'][g + 1]):
         L += o2.loss(n(c['tg'][i]), n(c['w'][i]), n(c['kp'][i]), n(c['cam'][i]), c['sigma'])
     if c['pw'] > 0:
-        L += osp.prior_loss(n(c['rot'][i0]), n(c['ganchor'][g]), c['pw'])
+        L += o2.prior_loss(n(c['rot'][i0])[1:], n(c['ganchor'][g])[1:], c['pw'])
     if with_meas:
         L += meas_loss(n(c['mt'][g]), n(c['mw'][g]), n(c['meas'][g]))
     if c['bw'] > 0:

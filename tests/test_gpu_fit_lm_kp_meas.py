@@ -1,11 +1,11 @@
 """GPU: the stacked keypoint + measurement Levenberg-Marquardt step (shapy_fit_lm_keypoints_measurements_step) against
-its NumPy restatement (tests/kpm_lm_oracle.py) and against shapy_fit_lm_keypoints_step when the measurement block is
+its NumPy restatement (tests/kp_lm_oracle.py with `meas`) and against shapy_fit_lm_keypoints_step when the measurement block is
 empty; and fit_body_to_keypoints with measurements (LM and Adam) against the keypoint-only LM fit."""
 import numpy as np
 import pytest
 import torch
 
-import kpm_lm_oracle
+import kp_lm_oracle
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -86,8 +86,9 @@ def _step_case(model):
 
 def _state(c, rho):
     B = c['rot'].shape[0]
-    loss = torch.tensor([kpm_lm_oracle.loss(c['tg'][b].numpy(), c['w'][b].numpy(), c['kp'][b].numpy(), c['mt'][b].numpy(),
-                                            c['mw'][b].numpy(), c['meas'][b].numpy(), rho, c['betas'][b].numpy())
+    loss = torch.tensor([kp_lm_oracle.loss(c['tg'][b].numpy(), c['w'][b].numpy(), c['kp'][b].numpy(),
+                                           (c['mt'][b].numpy(), c['mw'][b].numpy(), c['meas'][b].numpy()),
+                                           c['betas'][b].numpy(), rho)
                          for b in range(B)]).float()
     loss[4] = float('nan')
     cu = lambda t: t.cuda().contiguous()  # noqa: E731
@@ -117,9 +118,9 @@ def test_step_kernel_vs_oracle(model, first, rho):
         s = {k: s0[k][b] for k in s0}
         s['accepted'] = 0
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
-        new, want, acc = kpm_lm_oracle.lm_keypoints_measurements_step(
-            s, n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), rho, 10.0, 3.0, first, tr, n(c['tkp'][b]),
-            n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]))
+        new, want, acc = kp_lm_oracle.lm_keypoints_step(
+            s, n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
+            meas=(n(c['mt'][b]), n(c['mw'][b])), trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), betas_weight=rho)
         flags.append(acc)
         assert got['accepted'][b] == new['accepted'], b
         assert got['lambda'][b] == new['lambda'], (b, got['lambda'][b], new['lambda'])

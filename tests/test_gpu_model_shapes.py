@@ -11,7 +11,7 @@ test_model_shapes_cpu.py pins at those shapes.
   * J^T c against the posed backward on the uncached NB = 27 model
   * both LM step kernels against their restatements at P = 7, 54, 55 (the 48 KB opt-in boundary) and 96, K = 1 to 127
   * every keypoint step entry launches at P = 96 and refuses P = 97 without a launch
-  * the 2D measurement step and both grouped 2D steps on random Jacobians against kp2dm_lm_oracle and kp2dg_lm_oracle at
+  * the 2D measurement step and both grouped 2D steps on random Jacobians against kp2d_lm_oracle and kp2dg_lm_oracle at
     the same shapes, groups of 1 to 64 images in regular and irregular layouts; groups of one against the 2D step and
     dropped measurements against the plain grouped step at every shape; no write outside any output or past the
     workspace
@@ -23,7 +23,6 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp_lm_oracle
-import kpm_lm_oracle
 import test_gpu_fit_lm_keypoints_2d as kp2d
 import test_gpu_fit_lm_kp2d_groups as grp
 from shapy_b200 import synth
@@ -302,8 +301,8 @@ def _run_step(c, first, rho=None):
              'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
         if meas:
             s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
-            s['loss'] = np.float32(kpm_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], n(c['mt'][b]),
-                                                      n(c['mw'][b]), s['meas'], rho, s['betas']))
+            s['loss'] = np.float32(kp_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'],
+                                                     (n(c['mt'][b]), n(c['mw'][b]), s['meas']), s['betas'], rho))
         else:
             s['loss'] = np.float32(kp_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints']))
         s_np.append(s)
@@ -325,9 +324,9 @@ def _run_step(c, first, rho=None):
     for b in range(B):
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
         if meas:
-            new, want, acc = kpm_lm_oracle.lm_keypoints_measurements_step(
-                s_np[b], n(c['tg'][b]), n(c['w'][b]), n(c['mt'][b]), n(c['mw'][b]), rho, 10.0, 3.0, first, tr,
-                n(c['tkp'][b]), n(c['tjac'][b]), n(c['tmeas'][b]), n(c['tmjac'][b]))
+            new, want, acc = kp_lm_oracle.lm_keypoints_step(
+                s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
+                meas=(n(c['mt'][b]), n(c['mw'][b])), trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), betas_weight=rho)
         else:
             new, want, acc = kp_lm_oracle.lm_keypoints_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
                                                             n(c['tkp'][b]), n(c['tjac'][b]))
@@ -421,7 +420,7 @@ def test_steps_refuse_97_parameters_without_a_launch():
 
 
 # ------------------------------------------------------------------------------------------------ 2D LM steps
-# the 2D steps on random Jacobians at STEP_SHAPES, against kp2dm_lm_oracle and kp2dg_lm_oracle (which
+# the 2D steps on random Jacobians at STEP_SHAPES, against kp2d_lm_oracle and kp2dg_lm_oracle (which
 # test_model_shapes_cpu.py pins at these shapes); K: 2K = 2, 16 (one full staging tile), 18 and 254 rows
 STEP_K_2D = [1, 8, 9, 127]
 GROUP_K = [1, 9, 127]

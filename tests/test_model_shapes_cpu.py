@@ -13,9 +13,10 @@ synth.make_smplx's sparse_rows):
   edge_2049        edge_2048 plus one non-zero in the last J14 row    2 049 entries: the first uncached count
 
   * kp_lm_oracle.keypoint_jacobian against central differences of the float64 forward on nb1_ne0 and nb27_ne5_dense
-  * kp_lm_oracle.lm_keypoints_step and kpm_lm_oracle against a dense solve of the damped normal equations at P = 7 and
-    P = 96
-  * kp2d_lm_oracle, kp2dm_lm_oracle and kp2dg_lm_oracle against explicitly stacked 2D rows and dense solves at
+  * kp_lm_oracle.lm_keypoints_step, with and without measurements, against a dense solve of the damped normal
+    equations at P = 7 and P = 96
+  * kp2d_lm_oracle (with and without measurements) and kp2dg_lm_oracle against explicitly stacked 2D rows and dense
+    solves at
     nb = 1 to 27 and P = 7 to 96 (the toy problems of the 2D CPU tests have nb = 1, where a Schur block, X_i and each
     measurement row's outer product have one entry)
   * fit_body_to_keypoints(method='lm') and fit_body_to_keypoints_2d(method='lm') refuse more than 96 parameters before
@@ -29,9 +30,7 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
-import kp2dm_lm_oracle as o2m
 import kp_lm_oracle
-import kpm_lm_oracle
 from shapy_b200 import synth
 from test_fit_lm_keypoints_cpu import _keypoints, _rodrigues
 
@@ -258,8 +257,9 @@ def test_oracle_keypoint_measurement_step_vs_dense_solve(P, rho):
     n_rot, nb = STEP_SHAPES[P]
     x, kp, jac, tg, w, meas, mjac, mt, mw = _random_step_problem(P + 1, n_rot, nb, 40)
     o = 3 * n_rot
-    new, _, acc, delta = kpm_lm_oracle.lm_keypoints_measurements_step(
-        {}, tg, w, mt, mw, rho, 10.0, 3.0, True, x, kp, jac, meas, mjac, dtype=np.float64, return_delta=True)
+    new, _, acc, delta = kp_lm_oracle.lm_keypoints_step(
+        {}, tg, w, 10.0, 3.0, True, x, kp, jac, meas=(mt, mw), trial_meas=(meas, mjac), betas_weight=rho,
+        dtype=np.float64, return_delta=True)
     assert acc
     A, g, r = _dense(jac, kp, tg, w, o, nb, mjac, meas, mt, mw)
     rho32 = float(np.float32(rho))
@@ -274,8 +274,9 @@ def test_oracle_keypoint_measurement_step_vs_dense_solve(P, rho):
     f = lambda t: np.asarray(t, np.float32)  # noqa: E731
     x32 = {k: f(v) for k, v in x.items()}
     a = kp_lm_oracle.lm_keypoints_step({}, f(tg), f(w), 10.0, 3.0, True, x32, f(kp), f(jac))
-    b = kpm_lm_oracle.lm_keypoints_measurements_step({}, f(tg), f(w), f(mt), np.zeros(5, np.float32), 0.0, 10.0, 3.0,
-                                                     True, x32, f(kp), f(jac), f(meas), f(mjac))
+    b = kp_lm_oracle.lm_keypoints_step({}, f(tg), f(w), 10.0, 3.0, True, x32, f(kp), f(jac),
+                                       meas=(f(mt), np.zeros(5, np.float32)), trial_meas=(f(meas), f(mjac)),
+                                       betas_weight=0.0)
     for k in ('rot', 'betas', 'transl', 'loss', 'lambda', 'accepted'):
         assert np.array_equal(a[0][k], b[0][k]), k
     for k in ('rot', 'betas', 'transl'):
@@ -303,7 +304,7 @@ def _check_step(nxt, x, want, o, nb, bar):
 @pytest.mark.parametrize('sigma,pose_w,betas_w', TERMS_2D)
 @pytest.mark.parametrize('n_rot,nb', SHAPES_2D)
 def test_oracle_2d_step_vs_dense_solve(n_rot, nb, sigma, pose_w, betas_w, with_meas):
-    """kp2d_lm_oracle (kp2dm_lm_oracle with measurements): A and g are J^T W J and J^T W r of the explicitly stacked
+    """kp2d_lm_oracle, with and without measurements: A and g are J^T W J and J^T W r of the explicitly stacked
     rows (projected keypoints with IRLS weights, pose prior, measurements) plus betas_w beta, the first lambda comes
     from the keypoint rows alone, and the fp64 step solves the damped system."""
     x, kp, jac, tg, w, anchor, meas, mjac, mt, mw = _random_2d_problem(100 * n_rot + nb, n_rot, nb, K_2D)
@@ -314,16 +315,11 @@ def test_oracle_2d_step_vs_dense_solve(n_rot, nb, sigma, pose_w, betas_w, with_m
                      pose_w=pose_w, **mrows)
     g[o:o + nb] += bw * x['betas']
     dkp = np.diag(_dense(jac, kp, tg, w, o, nb, camera=x['camera'], sigma=sigma)[0])
-    if with_meas:
-        A2, g2, dg = o2m.normal_equations(tg, w, kp, jac, x['camera'], mt, mw, meas, mjac, sigma, x['rot'], anchor,
-                                          pose_w, x['betas'], betas_w)
-        new, nxt, acc = o2m.lm_keypoints_2d_measurements_step({}, tg, w, mt, mw, 10.0, 3.0, True, x, kp, jac, meas,
-                                                              mjac, sigma, anchor, pose_w, betas_w, dtype=np.float64)
-    else:
-        A2, g2, dg = o2.normal_equations(tg, w, kp, jac, x['camera'], sigma, x['rot'], anchor, pose_w, x['betas'],
-                                         betas_w)
-        new, nxt, acc = o2.lm_keypoints_2d_step({}, tg, w, 10.0, 3.0, True, x, kp, jac, sigma, anchor, pose_w, betas_w,
-                                                dtype=np.float64)
+    A2, g2, dg = o2.normal_equations(tg, w, kp, jac, x['camera'], sigma, x['rot'], anchor, pose_w, x['betas'],
+                                     betas_w, meas=(mt, mw, meas, mjac) if with_meas else None)
+    mkw = dict(meas=(mt, mw), trial_meas=(meas, mjac)) if with_meas else {}
+    new, nxt, acc = o2.lm_keypoints_2d_step({}, tg, w, 10.0, 3.0, True, x, kp, jac, sigma, anchor, pose_w, betas_w,
+                                            dtype=np.float64, **mkw)
     assert acc
     assert np.abs(A2 - A).max() <= 1e-12 * np.abs(A).max()
     assert np.abs(g2 - g).max() <= 1e-12 * np.abs(g).max()
