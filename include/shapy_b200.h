@@ -17,6 +17,8 @@
  *   shapy_measure_*      BodyMeasurements.forward   mesh-mesh-intersection/body_measurements/body_measurements.py:217-246
  *   shapy_mmi_forward    mesh_to_mesh_forward       mesh-mesh-intersection/src/mesh_mesh_intersect.cpp:36-64
  *   shapy_mmi_forward_f64  (float / float64)        + src/mesh_mesh_intersect_cuda_op.cu:969-1079
+ *   shapy_closest_points, shapy_nearest_points, shapy_closest_points_backward   (no reference counterpart: the scan
+ *                        terms of shapy_b200.fit.fit_body_to_scan, on the LBVH of shapy_mmi_forward)
  *   shapy_head_*         IterativeRegression.forward regressor/human_shape/models/common/networks.py:536-592
  *   shapy_hrnet_*        HighResolutionNet.forward  regressor/human_shape/models/backbone/hrnet.py:426-498
  *   shapy_p2p_error      v2vhdError.__call__        regressor/human_shape/utils/metrics.py:368-456
@@ -566,6 +568,47 @@ size_t shapy_mmi_workspace_bytes_f64(int batch, int num_query, int num_target);
 int shapy_mmi_forward_f64(const double *query, const double *target, int batch, int num_query, int num_target,
                           int max_collisions, int64_t *collision_faces, double *collision_bcs, void *workspace,
                           size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------ scans */
+/* Exact closest point of every scan point on its own body's mesh: vertices (B,V,3), faces (F,3) int32 (indices < V,
+ * shared by the batch), points (B,N,3), weights (B,N) or NULL (all kept).  For each kept point: face_idx (B,N) the
+ * face of the closest point, bary (B,N,3) its barycentrics on that face, sq_dist (B,N) the squared distance, all
+ * fp32.  The closest point on a face is the Voronoi-region test over its vertices, edges and interior; a zero-area face
+ * is the nearest of its edges.  A point with weight <= 0 is never read (it may be NaN): face -1, zero barycentrics
+ * and distance.
+ * Deterministic and a function of the mesh and the points alone: the winner is the face with the smallest float
+ * squared distance, the smallest face index on a tie, whatever the tree's shape, so a body's result does not depend
+ * on the rest of the batch, and a tree refit from another pose gives the same bits as one built fresh.
+ * The LBVH of shapy_mmi_forward is built over the posed triangles in the workspace (>=
+ * shapy_closest_points_workspace_bytes(B, F)); refit != 0 keeps the tree a previous call built in the same workspace
+ * for the same B and faces and only recomputes its boxes from the new vertices.
+ * F > 32768 or N > 32768 returns SHAPY_ERR_UNSUPPORTED before any launch; B = 0 or N = 0 launches nothing. */
+size_t shapy_closest_points_workspace_bytes(int batch, int num_faces);
+int shapy_closest_points(const float *vertices, const int32_t *faces, int batch, int num_verts, int num_faces,
+                         const float *points, int num_points, const float *weights, int refit, int32_t *face_idx,
+                         float *bary, float *sq_dist, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Nearest kept scan point of every query (a model vertex): queries (B,Q,3), points (B,N,3), weights (B,N) or NULL;
+ * idx (B,Q) int32, sq_dist (B,Q).  Points with weight <= 0 are excluded (never read); the winner is the smallest
+ * float squared distance, the smallest point index on a tie; idx -1 and distance 0 when a body keeps no point.  The
+ * tree is the same LBVH over the points as degenerate triangles, workspace >= shapy_nearest_points_workspace_bytes.
+ * N must be >= 1; N > 32768 returns SHAPY_ERR_UNSUPPORTED; B = 0 or Q = 0 launches nothing. */
+size_t shapy_nearest_points_workspace_bytes(int batch, int num_points);
+int shapy_nearest_points(const float *queries, int batch, int num_queries, const float *points, int num_points,
+                         const float *weights, int32_t *idx, float *sq_dist, void *workspace, size_t workspace_bytes,
+                         void *stream);
+
+/* Backward of sq_dist of shapy_closest_points with respect to the vertices, face_idx and bary held at the forward's
+ * values: grad_vertices (B,V,3) = sum over the points of 2 g_i (q_i - p_i) bary_{i,c} at corner c of face_idx_i, q_i =
+ * sum_c bary_{i,c} x_c recomputed from `vertices`.  inc_ptr (V+1) / inc (3F) is the vertex -> (3 face + corner)
+ * incidence CSR of `faces` (shapy_b200.ops.face_incidence).  A point whose face is outside [0, F) adds nothing.  One
+ * CTA per body sorts its (face, point) pairs in shared memory; each vertex sums over its incident faces in CSR order
+ * and each face's points in index order: no atomics, bit-identical run to run and alone or in a batch.  No gradient
+ * with respect to the points.  F > 32768 or N > 32768 returns SHAPY_ERR_UNSUPPORTED; N = 0 zeroes grad_vertices. */
+int shapy_closest_points_backward(const float *vertices, const int32_t *faces, const int32_t *inc_ptr,
+                                  const int32_t *inc, int batch, int num_verts, int num_faces, const float *points,
+                                  int num_points, const int32_t *face_idx, const float *bary,
+                                  const float *grad_sq_dist, float *grad_vertices, void *stream);
 
 /* ------------------------------------------------------------ regression head */
 /* params_out (num_stages, B, P).  W0 (H0, F+P), W1 (H1, H0), W2 (P, H1) row-major as nn.Linear stores

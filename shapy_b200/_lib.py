@@ -157,6 +157,13 @@ _SIGS = {
     'shapy_mmi_workspace_bytes_f64': (c_size_t, [c_int, c_int, c_int]),
     'shapy_mmi_forward_f64': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_size_t, c_void_p]),
+    'shapy_closest_points_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'shapy_closest_points': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'shapy_nearest_points_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'shapy_nearest_points': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_size_t, c_void_p]),
+    'shapy_closest_points_backward': (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 5),
     'shapy_head_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     'shapy_head_forward': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,

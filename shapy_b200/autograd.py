@@ -7,6 +7,8 @@ only).
     SmplxFunction.apply(packed_model, betas, rot, expression, camera, want_v_shaped)
                                                 -> vertices, v_shaped, joints, proj_joints (None where not computed)
     Rot6dFunction.apply(raw)                    raw (B,6n) -> (B,n,3,3)
+    ClosestPointsFunction.apply(faces_i32, vertices, points, weights)
+                                                scan points (B,N,3) on posed meshes (B,V,3) -> sq_dist (B,N)
 
 The forward of each is the same launches as the no-grad path; the backward is the matching CUDA adjoint
 (measure_smem_kernel in gradient mode, the shape-blend adjoint, shapy_smplx_backward which recomputes the posed
@@ -97,6 +99,27 @@ class Rot6dFunction(torch.autograd.Function):
     def backward(ctx, grad_rot):
         raw, = ctx.saved_tensors
         return _ops.decode_rot6d_backward(raw, grad_rot.contiguous()).view_as(raw)
+
+
+class ClosestPointsFunction(torch.autograd.Function):
+    """ClosestPointsFunction.apply(faces_i32, vertices, points, weights, tree=None) -> sq_dist (B, N): the squared
+    distance of each scan point to its body's posed mesh (ops.closest_points), differentiable in the vertices only.
+    The backward is ops.closest_points_backward: the closest face and barycentrics held at the forward's values, which
+    at the exact closest point is the distance's derivative away from region switches.  tree: an ops.ScanTree the
+    forward refits (same bits as a fresh build)."""
+
+    @staticmethod
+    def forward(ctx, faces_i32, vertices, points, weights, tree=None):
+        face, bary, d2 = _ops.closest_points(vertices, faces_i32, points, weights, tree=tree)
+        ctx.save_for_backward(faces_i32, vertices, points, face, bary)
+        return d2
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_d2):
+        faces_i32, vertices, points, face, bary = ctx.saved_tensors
+        g = _ops.closest_points_backward(vertices, faces_i32, points, face, bary, grad_d2.contiguous())
+        return None, g, None, None, None
 
 
 def wants_grad(t) -> bool:

@@ -1,7 +1,8 @@
 // Batched LBVH mesh-mesh intersection: drop-in for mesh_mesh_intersect_cuda.mesh_to_mesh_forward
 // (reference mesh-mesh-intersection/src/mesh_mesh_intersect.cpp:36-64 and
 //  src/mesh_mesh_intersect_cuda_op.cu:969-1079), all bodies of the batch in the same launches, on the
-// caller's stream, no host synchronisation, no allocation.
+// caller's stream, no host synchronisation, no allocation.  The same tree serves the scan queries at the end of the
+// file (closest points on posed meshes, nearest scan points, and the scan distance's backward).
 //
 //   bvh_prepare_kernel   per body: triangle AABBs -> scene AABB -> 30-bit Morton code of each centroid
 //                        (op.cu:140-149, 613-668), then an in-shared-memory bitonic sort of the
@@ -390,4 +391,403 @@ extern "C" int shapy_mmi_forward_f64(const double *query, const double *target, 
                                      size_t workspace_bytes, void *stream) {
   return mmi_forward("shapy_mmi_forward_f64", query, target, B, Q, F, M, collision_faces, collision_bcs, workspace,
                      workspace_bytes, stream);
+}
+
+// ================================================================================================ scans
+// Closest points of scan points on a batch of posed meshes, the nearest scan point of each model vertex, and the
+// backward of the scan -> model squared distance.  Both queries run on the LBVH above (bvh_prepare_kernel,
+// bvh_topology_kernel, bvh_refit_kernel), built over a float triangle soup in the workspace: the posed triangles
+// gathered from (vertices, faces), or the scan points as degenerate triangles (p, p, p).
+//
+//   scan_mesh_soup_kernel / scan_point_soup_kernel   the primitives of each body, [B][P][9]
+//   scan_leaf_boxes_kernel    refit only: the leaf boxes of a tree built by an earlier call, from the new soup
+//   scan_query_kernel<kPts>   ONE THREAD PER QUERY, nearer child first, a 64-entry (node, box distance) stack
+//   scan_backward_kernel      ONE CTA PER BODY: bitonic sort of the (face, point) pairs in shared memory, then one
+//                             thread per vertex gathers over its incident faces (CSR order) and their points (index
+//                             order)
+//
+// The result is a function of the primitives and the queries only, not of the tree: a box is pruned only when its
+// squared distance exceeds the current best by more than a relative 1e-5 and an absolute 1e-12 m^2, which covers the
+// rounding of both distances, and a candidate wins on a strictly smaller squared distance or on an equal one with a
+// smaller primitive index.  So every primitive that could win is evaluated, and the winner is the lexicographic
+// minimum of (float squared distance, index) over all of them, whatever the tree's shape.
+namespace shapy {
+
+constexpr int kScanMaxPrims = 32768;  // the shared-memory sorts of bvh_prepare_kernel and scan_backward_kernel
+// A root-to-leaf path splits at strictly increasing prefix lengths of the (30-bit Morton code, 15-bit id) key, so
+// the tree is at most 45 internal nodes deep and the stack never holds more than 45 entries.
+constexpr int kScanStack = 64;
+
+struct ScanWs {
+  float *soup;  // [B][P][9]
+  BvhWs bvh;
+};
+
+static size_t scan_ws_layout(int B, int P, ScanWs *w, char *base) {
+  const size_t soup = align_up((size_t)B * P * 9 * 4, 256);
+  if (w) w->soup = (float *)base;
+  return soup + ws_layout(B, P, w ? &w->bvh : nullptr, base ? base + soup : nullptr);
+}
+
+__global__ void scan_mesh_soup_kernel(const float *__restrict__ vertices, const int *__restrict__ faces, int V, int F,
+                                      size_t n, float *__restrict__ soup) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // corner of [B][F][3]
+  if (i >= n) return;
+  const size_t bf = i / 3;
+  const int b = (int)(bf / F), f = (int)(bf % F), k = (int)(i % 3);
+  const float *s = vertices + ((size_t)b * V + faces[f * 3 + k]) * 3;
+  float *d = soup + i * 3;
+  d[0] = s[0]; d[1] = s[1]; d[2] = s[2];
+}
+
+// a point with weight <= 0 is never read: it goes in at the origin and the query skips it
+__global__ void scan_point_soup_kernel(const float *__restrict__ points, const float *__restrict__ weights, size_t n,
+                                       float *__restrict__ soup) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool keep = !weights || weights[i] > 0.f;
+  const float x = keep ? points[i * 3] : 0.f, y = keep ? points[i * 3 + 1] : 0.f, z = keep ? points[i * 3 + 2] : 0.f;
+  float *d = soup + i * 9;
+  for (int c = 0; c < 3; ++c) { d[3 * c] = x; d[3 * c + 1] = y; d[3 * c + 2] = z; }
+}
+
+__global__ void scan_leaf_boxes_kernel(const float *__restrict__ soup, int P, BvhWs w) {
+  const int b = blockIdx.y;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= P) return;
+  const int id = w.ids[(size_t)b * P + j];
+  const mmi::Box bx = mmi::box_f32(mmi::tri_box(ld_tri(soup + ((size_t)b * P + id) * 9)));
+  float *lb = w.leaf_box + ((size_t)b * P + j) * 6;
+  lb[0] = bx.lo.x; lb[1] = bx.lo.y; lb[2] = bx.lo.z; lb[3] = bx.hi.x; lb[4] = bx.hi.y; lb[5] = bx.hi.z;
+  if (j < P - 1) w.counters[(size_t)b * (P - 1) + j] = 0;
+}
+
+__device__ __forceinline__ float3 sub3(float3 a, float3 b) { return make_float3(a.x - b.x, a.y - b.y, a.z - b.z); }
+__device__ __forceinline__ float dot3(float3 a, float3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+
+// The Voronoi-region test of a non-degenerate triangle (a, b, c): the closest point of p is a + v ab + w ac.  Returns
+// false when the interior's denominator is not positive (a triangle too thin for the test), true otherwise.
+__device__ __forceinline__ bool tri_region(float3 ab, float3 ac, float3 ap, float3 bp, float3 cp, float &v, float &w) {
+  const float d1 = dot3(ab, ap), d2 = dot3(ac, ap);
+  if (d1 <= 0.f && d2 <= 0.f) { v = 0.f; w = 0.f; return true; }  // vertex a
+  const float d3 = dot3(ab, bp), d4 = dot3(ac, bp);
+  if (d3 >= 0.f && d4 <= d3) { v = 1.f; w = 0.f; return true; }  // vertex b
+  const float d5 = dot3(ab, cp), d6 = dot3(ac, cp);
+  if (d6 >= 0.f && d5 <= d6) { v = 0.f; w = 1.f; return true; }  // vertex c
+  const float vc = d1 * d4 - d3 * d2;
+  if (vc <= 0.f && d1 >= 0.f && d3 <= 0.f) { v = d1 - d3 > 0.f ? d1 / (d1 - d3) : 0.f; w = 0.f; return true; }  // ab
+  const float vb = d5 * d2 - d1 * d6;
+  if (vb <= 0.f && d2 >= 0.f && d6 <= 0.f) { v = 0.f; w = d2 - d6 > 0.f ? d2 / (d2 - d6) : 0.f; return true; }  // ac
+  const float va = d3 * d6 - d5 * d4;
+  const float e1 = d4 - d3, e2 = d5 - d6;
+  if (va <= 0.f && e1 >= 0.f && e2 >= 0.f) {  // bc
+    w = e1 + e2 > 0.f ? e1 / (e1 + e2) : 0.f;
+    v = 1.f - w;
+    return true;
+  }
+  const float den = va + vb + vc;  // interior
+  if (!(den > 0.f)) return false;
+  v = vb / den;
+  w = vc / den;
+  return true;
+}
+
+__device__ __forceinline__ float seg_t(float3 ap, float3 ab) {
+  const float l2 = dot3(ab, ab);
+  return l2 > 0.f ? fminf(fmaxf(dot3(ap, ab) / l2, 0.f), 1.f) : 0.f;
+}
+
+__device__ __forceinline__ float tri_d2(float3 ab, float3 ac, float3 ap, float v, float w) {
+  const float3 d = make_float3(ap.x - (ab.x * v + ac.x * w), ap.y - (ab.y * v + ac.y * w), ap.z - (ab.z * v + ac.z * w));
+  return dot3(d, d);
+}
+
+// Exact closest point of p on the triangle (a, b, c): squared distance, barycentrics (1 - v - w, v, w).  A zero-area
+// (or too thin) triangle is the nearest of its edges ab, ac, bc, the first of them on a tie.
+__device__ __forceinline__ float point_triangle(float3 p, float3 a, float3 b, float3 c, float &v, float &w) {
+  const float3 ab = sub3(b, a), ac = sub3(c, a), ap = sub3(p, a);
+  const float3 n = make_float3(ab.y * ac.z - ab.z * ac.y, ab.z * ac.x - ab.x * ac.z, ab.x * ac.y - ab.y * ac.x);
+  if (dot3(n, n) > 0.f && tri_region(ab, ac, ap, sub3(p, b), sub3(p, c), v, w)) return tri_d2(ab, ac, ap, v, w);
+  const float t0 = seg_t(ap, ab), t1 = seg_t(ap, ac), t2 = seg_t(sub3(p, b), sub3(c, b));
+  float bv = t0, bw = 0.f, best = tri_d2(ab, ac, ap, t0, 0.f);
+  const float e1 = tri_d2(ab, ac, ap, 0.f, t1);
+  if (e1 < best) { best = e1; bv = 0.f; bw = t1; }
+  const float e2 = tri_d2(ab, ac, ap, 1.f - t2, t2);
+  if (e2 < best) { best = e2; bv = 1.f - t2; bw = t2; }
+  v = bv;
+  w = bw;
+  return best;
+}
+
+__device__ __forceinline__ float box_d2(float3 p, const float *bx) {
+  const float dx = fmaxf(fmaxf(bx[0] - p.x, p.x - bx[3]), 0.f);
+  const float dy = fmaxf(fmaxf(bx[1] - p.y, p.y - bx[4]), 0.f);
+  const float dz = fmaxf(fmaxf(bx[2] - p.z, p.z - bx[5]), 0.f);
+  return dx * dx + dy * dy + dz * dz;
+}
+
+// the box of a child link of a finished tree (the refit's volatile reads are not needed once it has ended)
+__device__ __forceinline__ float scan_child_box_d2(const BvhNode *nodes, const float *leaf_box, int link, float3 p) {
+  const float *s = link < 0 ? leaf_box + (size_t)(~link) * 6 : nodes[link].lo;
+  float bx[6];
+  for (int c = 0; c < 6; ++c) bx[c] = __ldg(s + c);
+  return box_d2(p, bx);
+}
+
+// the largest box distance that can still hold a primitive as near as `best`
+__device__ __forceinline__ float prune_bound(float best) { return best + best * 1e-5f + 1e-12f; }
+
+// One thread per query point q of body blockIdx.y against the P primitives of that body's tree.  kPts: the
+// primitives are points (soup (p, p, p)), d2 = |q - p|^2 and a primitive with prim_w <= 0 is skipped; otherwise they
+// are triangles and a query with q_w <= 0 is not read (out -1, zero barycentrics and distance).
+template <bool kPts>
+__global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict__ queries, const float *__restrict__ q_w,
+                                                         int Q, const float *__restrict__ soup,
+                                                         const float *__restrict__ prim_w, int P, BvhWs w,
+                                                         int *__restrict__ idx_out, float *__restrict__ bary_out,
+                                                         float *__restrict__ d2_out) {
+  const int b = blockIdx.y;
+  const int qi = blockIdx.x * blockDim.x + threadIdx.x;
+  if (qi >= Q) return;
+  const size_t o = (size_t)b * Q + qi;
+  float best = INFINITY, bv = 0.f, bw = 0.f;
+  int best_id = -1;
+  if (kPts || !q_w || q_w[o] > 0.f) {
+    const float3 q = make_float3(queries[o * 3], queries[o * 3 + 1], queries[o * 3 + 2]);
+    const float *sb = soup + (size_t)b * P * 9;
+    const int *ids = w.ids + (size_t)b * P;
+    const BvhNode *nodes = w.nodes + (size_t)b * (P - 1);
+    const float *leaf_box = w.leaf_box + (size_t)b * P * 6;
+    auto leaf = [&](int j) {
+      const int id = __ldg(ids + j);
+      const float *t = sb + (size_t)id * 9;
+      float d2, v = 0.f, ww = 0.f;
+      if constexpr (kPts) {
+        if (prim_w && !(prim_w[(size_t)b * P + id] > 0.f)) return;
+        const float3 d = sub3(q, make_float3(t[0], t[1], t[2]));
+        d2 = dot3(d, d);
+      } else {
+        d2 = point_triangle(q, make_float3(t[0], t[1], t[2]), make_float3(t[3], t[4], t[5]),
+                            make_float3(t[6], t[7], t[8]), v, ww);
+      }
+      if (d2 < best || (d2 == best && id < best_id)) { best = d2; best_id = id; bv = v; bw = ww; }
+    };
+    if (P == 1) {
+      leaf(0);
+    } else {
+      int st_node[kScanStack];
+      float st_d[kScanStack];
+      int sp = 0, node = 0;
+      while (true) {
+        const int link[2] = {__ldg(&nodes[node].left), __ldg(&nodes[node].right)};
+        const float d[2] = {scan_child_box_d2(nodes, leaf_box, link[0], q), scan_child_box_d2(nodes, leaf_box, link[1], q)};
+        for (int c = 0; c < 2; ++c)
+          if (link[c] < 0 && d[c] <= prune_bound(best)) leaf(~link[c]);
+        const bool go0 = link[0] >= 0 && d[0] <= prune_bound(best), go1 = link[1] >= 0 && d[1] <= prune_bound(best);
+        if (go0 && go1) {
+          const int near = d[1] < d[0] ? 1 : 0;
+          st_node[sp] = link[1 - near];
+          st_d[sp] = d[1 - near];
+          ++sp;
+          node = link[near];
+        } else if (go0 || go1) {
+          node = link[go0 ? 0 : 1];
+        } else {
+          node = -1;
+          while (sp > 0) {
+            --sp;
+            if (st_d[sp] <= prune_bound(best)) { node = st_node[sp]; break; }
+          }
+          if (node < 0) break;
+        }
+      }
+    }
+  }
+  idx_out[o] = best_id;
+  d2_out[o] = best_id >= 0 ? best : 0.f;
+  if (!kPts) {
+    const bool hit = best_id >= 0;
+    bary_out[o * 3] = hit ? 1.f - bv - bw : 0.f;
+    bary_out[o * 3 + 1] = hit ? bv : 0.f;
+    bary_out[o * 3 + 2] = hit ? bw : 0.f;
+  }
+}
+
+// One CTA per body.  Dynamic smem: keys[npow2] (face, u32) + ids[npow2] (point, u16).  A point with a face outside
+// [0, F) (weight <= 0: -1) sorts last with key 0xFFFFFFFF and adds nothing.
+__global__ void __launch_bounds__(1024) scan_backward_kernel(
+    const float *__restrict__ vertices, const int *__restrict__ faces, const int *__restrict__ inc_ptr,
+    const int *__restrict__ inc, int V, int F, const float *__restrict__ points, int N, int npow2,
+    const int *__restrict__ face_idx, const float *__restrict__ bary, const float *__restrict__ grad,
+    float *__restrict__ grad_v) {
+  extern __shared__ __align__(16) unsigned char sm[];
+  unsigned *keys = reinterpret_cast<unsigned *>(sm);
+  unsigned short *ids = reinterpret_cast<unsigned short *>(sm + (size_t)npow2 * 4);
+  const int b = blockIdx.x, t = threadIdx.x;
+  for (int i = t; i < npow2; i += blockDim.x) {
+    const int f = i < N ? face_idx[(size_t)b * N + i] : -1;
+    keys[i] = f >= 0 && f < F ? (unsigned)f : 0xFFFFFFFFu;
+    ids[i] = (unsigned short)i;
+  }
+  __syncthreads();
+  for (int k = 2; k <= npow2; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = t; i < npow2; i += blockDim.x) {
+        const int ixj = i ^ j;
+        if (ixj > i) {
+          const unsigned ca = keys[i], cb = keys[ixj];
+          const unsigned short ia = ids[i], ib = ids[ixj];
+          const bool a_gt_b = ca > cb || (ca == cb && ia > ib);
+          if (a_gt_b == ((i & k) == 0)) { keys[i] = cb; keys[ixj] = ca; ids[i] = ib; ids[ixj] = ia; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  const float *vb = vertices + (size_t)b * V * 3;
+  const float *pb = points + (size_t)b * N * 3;
+  const float *cb = bary + (size_t)b * N * 3;
+  const float *gb = grad + (size_t)b * N;
+  for (int v = t; v < V; v += blockDim.x) {
+    float g[3] = {0.f, 0.f, 0.f};
+    for (int e = inc_ptr[v]; e < inc_ptr[v + 1]; ++e) {
+      const int f = inc[e] / 3, corner = inc[e] - 3 * f;
+      int lo = 0, hi = npow2;  // first key >= f
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (keys[mid] < (unsigned)f) lo = mid + 1; else hi = mid;
+      }
+      if (lo == npow2 || keys[lo] != (unsigned)f) continue;
+      const float *x0 = vb + (size_t)faces[f * 3] * 3, *x1 = vb + (size_t)faces[f * 3 + 1] * 3,
+                  *x2 = vb + (size_t)faces[f * 3 + 2] * 3;
+      for (int i = lo; i < npow2 && keys[i] == (unsigned)f; ++i) {
+        const int p = ids[i];
+        const float *l = cb + (size_t)p * 3;
+        const float s = 2.f * gb[p] * l[corner];
+        for (int c = 0; c < 3; ++c) g[c] += s * ((l[0] * x0[c] + l[1] * x1[c] + l[2] * x2[c]) - pb[(size_t)p * 3 + c]);
+      }
+    }
+    float *o = grad_v + ((size_t)b * V + v) * 3;
+    o[0] = g[0]; o[1] = g[1]; o[2] = g[2];
+  }
+}
+
+static int npow2_of(int n) {
+  int p = 1;
+  while (p < n) p <<= 1;
+  return p;
+}
+
+// Builds the tree over w.soup (P primitives per body), or with refit only recomputes its boxes.
+static int scan_tree(const ScanWs &w, int B, int P, bool refit, cudaStream_t st) {
+  if (refit) {
+    scan_leaf_boxes_kernel<<<dim3(ceil_div(P, 128), B), 128, 0, st>>>(w.soup, P, w.bvh);
+    SHAPY_LAUNCH_CHECK();
+  } else {
+    const int npow2 = npow2_of(P);
+    static std::atomic<unsigned long long> attr_done{0};
+    SHAPY_CUDA_TRY(set_max_dynamic_smem(bvh_prepare_kernel<float, unsigned short>, 200 * 1024, attr_done));
+    bvh_prepare_kernel<float, unsigned short><<<B, 1024, (size_t)npow2 * 6, st>>>(w.soup, P, npow2, w.bvh);
+    SHAPY_LAUNCH_CHECK();
+    if (P > 1) {
+      bvh_topology_kernel<<<dim3(ceil_div(P - 1, 128), B), 128, 0, st>>>(P, w.bvh);
+      SHAPY_LAUNCH_CHECK();
+    }
+  }
+  if (P > 1) {
+    bvh_refit_kernel<<<dim3(ceil_div(P, 128), B), 128, 0, st>>>(P, w.bvh);
+    SHAPY_LAUNCH_CHECK();
+  }
+  return SHAPY_OK;
+}
+
+static int scan_limit(const char *name, const char *what, int n) {
+  if (n <= kScanMaxPrims) return SHAPY_OK;
+  set_error("%s: %d %s per body exceed the %d supported (the tree and the backward sort them in shared memory)", name,
+            n, what, kScanMaxPrims);
+  return SHAPY_ERR_UNSUPPORTED;
+}
+
+static char *scan_base(void *workspace) { return (char *)(((uintptr_t)workspace + 255) & ~(uintptr_t)255); }
+
+}  // namespace shapy
+
+extern "C" size_t shapy_closest_points_workspace_bytes(int B, int F) {
+  if (B <= 0 || F <= 0) return 0;
+  return scan_ws_layout(B, F, nullptr, nullptr) + 256;
+}
+
+extern "C" int shapy_closest_points(const float *vertices, const int32_t *faces, int B, int V, int F,
+                                    const float *points, int N, const float *weights, int refit, int32_t *face_idx,
+                                    float *bary, float *sq_dist, void *workspace, size_t workspace_bytes,
+                                    void *stream) {
+  const char *name = "shapy_closest_points";
+  SHAPY_REQUIRE(B >= 0 && N >= 0 && V > 0 && F > 0, "%s: bad sizes", name);
+  if (int rc = scan_limit(name, "faces", F)) return rc;
+  if (int rc = scan_limit(name, "points", N)) return rc;
+  if (B == 0 || N == 0) return SHAPY_OK;
+  SHAPY_REQUIRE(vertices && faces && points && face_idx && bary && sq_dist, "%s: null argument", name);
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_closest_points_workspace_bytes(B, F), "%s: workspace too small",
+                name);
+  cudaStream_t st = (cudaStream_t)stream;
+  ScanWs w;
+  scan_ws_layout(B, F, &w, scan_base(workspace));
+  const size_t n = (size_t)B * F * 3;
+  scan_mesh_soup_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(vertices, faces, V, F, n, w.soup);
+  SHAPY_LAUNCH_CHECK();
+  if (int rc = scan_tree(w, B, F, refit != 0, st)) return rc;
+  scan_query_kernel<false><<<dim3(ceil_div(N, 128), B), 128, 0, st>>>(points, weights, N, w.soup, nullptr, F, w.bvh,
+                                                                       face_idx, bary, sq_dist);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" size_t shapy_nearest_points_workspace_bytes(int B, int N) { return shapy_closest_points_workspace_bytes(B, N); }
+
+extern "C" int shapy_nearest_points(const float *queries, int B, int Q, const float *points, int N,
+                                    const float *weights, int32_t *idx, float *sq_dist, void *workspace,
+                                    size_t workspace_bytes, void *stream) {
+  const char *name = "shapy_nearest_points";
+  SHAPY_REQUIRE(B >= 0 && Q >= 0 && N > 0, "%s: bad sizes", name);
+  if (int rc = scan_limit(name, "points", N)) return rc;
+  if (B == 0 || Q == 0) return SHAPY_OK;
+  SHAPY_REQUIRE(queries && points && idx && sq_dist, "%s: null argument", name);
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_nearest_points_workspace_bytes(B, N), "%s: workspace too small",
+                name);
+  cudaStream_t st = (cudaStream_t)stream;
+  ScanWs w;
+  scan_ws_layout(B, N, &w, scan_base(workspace));
+  const size_t n = (size_t)B * N;
+  scan_point_soup_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(points, weights, n, w.soup);
+  SHAPY_LAUNCH_CHECK();
+  if (int rc = scan_tree(w, B, N, false, st)) return rc;
+  scan_query_kernel<true><<<dim3(ceil_div(Q, 128), B), 128, 0, st>>>(queries, nullptr, Q, w.soup, weights, N, w.bvh,
+                                                                      idx, nullptr, sq_dist);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" int shapy_closest_points_backward(const float *vertices, const int32_t *faces, const int32_t *inc_ptr,
+                                             const int32_t *inc, int B, int V, int F, const float *points, int N,
+                                             const int32_t *face_idx, const float *bary, const float *grad_sq_dist,
+                                             float *grad_vertices, void *stream) {
+  const char *name = "shapy_closest_points_backward";
+  SHAPY_REQUIRE(B >= 0 && N >= 0 && V > 0 && F > 0, "%s: bad sizes", name);
+  if (int rc = scan_limit(name, "faces", F)) return rc;
+  if (int rc = scan_limit(name, "points", N)) return rc;
+  if (B == 0) return SHAPY_OK;
+  SHAPY_REQUIRE(vertices && faces && inc_ptr && inc && grad_vertices, "%s: null argument", name);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (N == 0) {
+    SHAPY_CUDA_TRY(cudaMemsetAsync(grad_vertices, 0, (size_t)B * V * 3 * sizeof(float), st));
+    return SHAPY_OK;
+  }
+  SHAPY_REQUIRE(points && face_idx && bary && grad_sq_dist, "%s: null argument", name);
+  const int npow2 = npow2_of(N);
+  static std::atomic<unsigned long long> attr_done{0};
+  SHAPY_CUDA_TRY(set_max_dynamic_smem(scan_backward_kernel, 200 * 1024, attr_done));
+  scan_backward_kernel<<<B, 1024, (size_t)npow2 * 6, st>>>(vertices, faces, inc_ptr, inc, V, F, points, N, npow2,
+                                                           face_idx, bary, grad_sq_dist, grad_vertices);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
 }

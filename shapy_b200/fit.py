@@ -107,6 +107,18 @@ translation do not jitter from frame to frame.  With method='lm' each iteration 
 and ops.fit_lm_keypoints_2d_sequence_step, whose three launches solve each sequence's block-tridiagonal normal matrix
 exactly by a block LDL^T sweep along its frames, no host synchronisation.
 
+fit_body_to_scan fits pose, shape and translation to 3D body scans or depth point clouds (B, N, 3), in metres in the
+model frame: per body the weighted mean of rho(d^2) over the scan points, d the distance to the exact closest point of
+the posed mesh, plus the mean of rho(e^2) over the model's vertices, e the distance to the nearest scan point, with
+the 2D fits' pose and betas priors and optionally known measurements.  Keypoints pin the bone lengths; a dense surface
+also sees depth and soft tissue.  The closest points, their gradient and the nearest points are CUDA launches on the
+batched LBVH of mesh_to_mesh_forward (ops.closest_points, ops.closest_points_backward, ops.nearest_points):
+deterministic, and a body's result does not depend on the rest of the batch.  The optimiser is the batched Adam of the
+other fits: an LM step would need the Jacobian of every vertex a correspondence touches, up to all of them.  Not
+covered: an LM scan fit, point-to-plane residuals, scan normals, a self-penetration term, rigid pre-alignment of scans
+in other frames or units, and reading PLY / OBJ files (load the points into an npz).
+
+    python -m shapy_b200.fit --synthetic --scan scan.npz --init pred.npz --robust-sigma 0.01 --output fit.npz
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
@@ -1354,6 +1366,117 @@ def fit_body_to_sequence(body_model, keypoints2d, focal_length, principal_point,
     return res
 
 
+def _scan_inputs(fn, body_model, points, weights, device):
+    """The scan points as a contiguous float32 (B, N, 3) tensor on `device` and their weights (None: all 1, (N,) or
+    (B, N)) as (B, N), checked before anything is launched."""
+    from .ops import MAX_SCAN_FACES, MAX_SCAN_POINTS
+    F = body_model.faces_tensor.shape[0]
+    if F > MAX_SCAN_FACES:
+        raise ValueError(f'{fn}: the model has {F} faces, the scan queries take at most {MAX_SCAN_FACES}')
+    pts = torch.as_tensor(points, dtype=torch.float32)
+    if pts.dim() != 3 or pts.shape[2] != 3 or pts.shape[1] == 0:
+        raise ValueError(f'{fn}: points must be (B, N, 3) with N >= 1, got {tuple(pts.shape)}')
+    B, N = pts.shape[:2]
+    if N > MAX_SCAN_POINTS:
+        raise ValueError(f'{fn}: {N} points per body exceed the {MAX_SCAN_POINTS} supported: subsample the scan')
+    if weights is None:
+        return pts.to(device).contiguous(), torch.ones(B, N, dtype=torch.float32, device=device)
+    w = torch.as_tensor(weights, dtype=torch.float32)
+    if tuple(w.shape) not in ((N,), (B, N)):
+        raise ValueError(f'{fn}: weights must be ({N},) or ({B}, {N}), got {tuple(w.shape)}')
+    if not bool(torch.isfinite(w).all()):
+        raise ValueError(f'{fn}: weights must be finite (a weight <= 0 drops its point)')
+    return pts.to(device).contiguous(), w.to(device).expand(B, N).contiguous()
+
+
+def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=None, lr=0.05, scan_to_model_weight=1.0,
+                     model_to_scan_weight=1.0, robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0,
+                     body_measurements=None, measurements=None, measurement_weights=None,
+                     circumference_derivative='reference'):
+    """Fits pose, shape and translation to 3D scans or point clouds: points (B, N, 3) in metres in the model frame,
+    N <= 32768 per body, weights None (all 1), (N,) or (B, N), a point with weight <= 0 dropped (it may be NaN).
+    Loss per body: scan_to_model_weight sum_i w_i rho(d_i^2) / sum_i w_i, d_i the distance of point i to the exact
+    closest point of the posed mesh (autograd.ClosestPointsFunction), + model_to_scan_weight sum_v rho(e_v^2) / V, e_v
+    the distance of vertex v to its nearest kept point (ops.nearest_points), + fit_body_to_keypoints_2d's chordal pose
+    prior pose_prior_weight / 2 sum_{j >= 1} |R_j - R0_j|_F^2 about the start and betas prior betas_weight |betas|^2,
+    + with measurements the measurement loss of fit_body_to_keypoints (same targets, weights and dropping rule).
+    rho is the Geman-McClure sigma^2 e / (sigma^2 + e) with robust_sigma in metres, the identity for None.  Each
+    distance term is a weighted mean, so its scale does not depend on how densely the scan is sampled.  For a partial
+    scan (one depth camera) set model_to_scan_weight=0: the unseen side of the body has no point to be near.
+    init: fit_body_to_keypoints' keys (raw 6D global_rot / body_pose, or the regressor's raw_ entries, betas, transl);
+    by default the identity pose, zero betas and the translation that puts the start body's vertex centroid on the
+    scan's weighted centroid (on the device, no synchronisation).  Adam as fit_body_to_keypoints' (the step size decays
+    from lr to lr / 100); iterations None means 600.  The posed mesh's tree is built at the first iteration and refit
+    after (the same bits as a rebuild).
+    Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat', 'body_pose_mat', 'vertices'
+    (B, V, 3) of the final parameters, 'loss' (B,)}, and with body_measurements 'measurements' (B, 5) of the fitted
+    betas (mass, height, chest, waist, hips), with or without measurement targets."""
+    fn = 'fit_body_to_scan'
+    iterations, sigma = _check_kp_fit(fn, body_model, 'adam', iterations, circumference_derivative, body_measurements,
+                                      measurements, robust_sigma, pose_prior_weight, betas_weight)
+    s2m, m2s = float(scan_to_model_weight), float(model_to_scan_weight)
+    if not (0 <= s2m < float('inf') and 0 <= m2s < float('inf') and s2m + m2s > 0):
+        raise ValueError(f'{fn}: the scan-to-model and model-to-scan weights must be finite, >= 0 and not both 0')
+    device = body_model.shapedirs.device
+    pts, w = _scan_inputs(fn, body_model, points, weights, device)
+    from . import ops
+    from .autograd import ClosestPointsFunction, Rot6dFunction
+    B, N = pts.shape[:2]
+    pw, bw = float(pose_prior_weight), float(betas_weight)
+    mt = _measurement_term(measurements, measurement_weights, B, device, body_measurements, circumference_derivative)
+    keep = w > 0
+    wk = torch.where(keep, w, torch.zeros_like(w))
+    wsum = wk.sum(1)
+    wden = torch.where(wsum > 0, wsum, torch.ones_like(wsum))
+    init = _raw_init(init)
+    params = _start_params(init, B, body_model.num_betas, device, 'adam', 'transl')
+    rot0, anchor = _start_rotations(params, None, B)
+    if init.get('transl') is None:
+        with torch.no_grad():
+            v0 = body_model(global_rot=rot0[:, :1], body_pose=rot0[:, 1:], betas=params['betas'],
+                            return_shaped=False)['vertices']
+            centroid = (torch.where(keep[..., None], pts, torch.zeros_like(pts)) * wk[..., None]).sum(1) / wden[:, None]
+            params['transl'].copy_(centroid - v0.mean(1))
+    faces = body_model.faces_i32
+    tree = ops.ScanTree()
+
+    def rho(e):
+        return e if sigma is None else sigma * sigma * e / (sigma * sigma + e)
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        v = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
+                       return_shaped=False)['vertices']
+        per_body = torch.zeros(B, dtype=torch.float32, device=device)
+        if s2m > 0:
+            d2 = ClosestPointsFunction.apply(faces, v, pts, w, tree)
+            per_body = per_body + s2m * (wk * rho(d2)).sum(1) / wden
+        if m2s > 0:
+            idx, _ = ops.nearest_points(v.detach(), pts, w)
+            found = (idx >= 0)[..., None]
+            nn = torch.gather(pts, 1, idx.clamp(min=0).long()[..., None].expand(-1, -1, 3))
+            e = torch.where(found, v - nn, torch.zeros_like(v)).pow(2).sum(-1)
+            per_body = per_body + m2s * rho(e).mean(1)
+        if pw > 0:
+            per_body = per_body + 0.5 * pw * (bpose - anchor[:, 1:]).pow(2).sum((1, 2, 3))
+        if bw > 0:
+            per_body = per_body + bw * params['betas'].pow(2).sum(1)
+        meas = None
+        if mt is not None:
+            meas = mt.measure(body_model, params['betas'])
+            per_body = per_body + mt.loss(meas, params['betas'], 0.0)
+        return per_body, v, grot, bpose, meas
+
+    per_body, v, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
+    if meas is None and body_measurements is not None:
+        with torch.no_grad():
+            vs = body_model.forward_shape(betas=params['betas'].detach())['v_shaped']
+            m = body_measurements.forward_vertices(vs, faces, circumference_derivative)['measurements']
+            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+    return _adam_result(params, grot, bpose, meas, vertices=v, loss=per_body)
+
+
 def main(argv=None):
     p = argparse.ArgumentParser(description='Fit SMPL-X betas to virtual measurements (batched, on the GPU)')
     src = p.add_mutually_exclusive_group(required=True)
@@ -1419,11 +1542,22 @@ def main(argv=None):
                    help='with --sequence: the weight of |R_{t+1} - R_t|_F^2 / 2 between consecutive frames')
     p.add_argument('--smooth-transl', dest='smooth_transl', type=float, default=0.0,
                    help='with --sequence: the weight of |transl_{t+1} - transl_t|^2 between consecutive frames')
+    p.add_argument('--scan', type=str, default=None,
+                   help='npz with points (B, N, 3) or (N, 3) in metres in the model frame and optional weights (B, N) '
+                        'or (N,): fit pose, shape and translation to the scans (fit_body_to_scan); the output holds '
+                        'the fitted vertices and the measurements of the fitted betas')
+    p.add_argument('--model-to-scan-weight', dest='model_to_scan_weight', type=float, default=1.0,
+                   help='with --scan: the weight of the model -> scan term (0 for a partial, single-view scan)')
     a = p.parse_args(argv)
     if (a.pose_width != 22 or a.fit_expression or a.expression_weight) and \
             (not a.keypoints_2d or a.calibrated or a.sequence):
         raise SystemExit('--pose-width, --fit-expression and --expression-weight need --keypoints-2d and are not '
                          'supported with --calibrated or --sequence')
+    scan = None
+    if a.scan:              # read and checked before the model goes to the device
+        if a.keypoints_2d:
+            raise SystemExit('--scan and --keypoints-2d are different fits: give one of them')
+        scan = _load_scan(a.scan)
 
     from . import synth
     from .body_measurements import BodyMeasurements
@@ -1443,6 +1577,16 @@ def main(argv=None):
         targets = {k: d[k].astype(np.float32) for k in NAMES if k in d.files}
     if a.keypoints_2d:      # known measurements only from --targets: --height has a default and is not used here
         return _main_keypoints_2d(a, model, BodyMeasurements(cfg).cuda() if targets else None, targets)
+    if scan is not None:    # the same: known measurements only from --targets
+        points, weights = scan
+        init = _load_init(a.init, points.shape[0], ('transl',)) if a.init else None
+        res = fit_body_to_scan(model, points, weights, init=init, iterations=a.iterations, lr=a.lr,
+                               model_to_scan_weight=a.model_to_scan_weight, robust_sigma=a.robust_sigma,
+                               pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight,
+                               body_measurements=BodyMeasurements(cfg).cuda(), measurements=targets,
+                               circumference_derivative=a.circumference_derivative)
+        return _save_result(a.output, res, {'bodies': int(points.shape[0]), 'points': int(points.shape[1])},
+                            names=np.array(NAMES))
     bm = BodyMeasurements(cfg).cuda()
     if targets is None:
         targets = {k: getattr(a, k) for k in NAMES}
@@ -1503,6 +1647,25 @@ def _main_keypoints_2d(a, model, bm, targets):
                                    pose_width=a.pose_width, fit_expression=a.fit_expression,
                                    expression_weight=a.expression_weight)
     _save_result(a.output, res, {'bodies': int(x.shape[0])}, groups=groups)
+
+
+def _load_scan(path):
+    """A --scan npz as (points (B, N, 3), weights (B, N) or None) float32 arrays; SystemExit on a malformed file."""
+    d = np.load(path)
+    if 'points' not in d.files:
+        raise SystemExit(f'--scan {path}: no `points` array')
+    points = d['points'].astype(np.float32)
+    points = points[None] if points.ndim == 2 else points
+    if points.ndim != 3 or points.shape[2] != 3 or points.shape[1] == 0:
+        raise SystemExit(f'--scan {path}: points must be (B, N, 3) or (N, 3) with N >= 1, got {d["points"].shape}')
+    weights = None
+    if 'weights' in d.files:
+        weights = d['weights'].astype(np.float32)
+        if weights.size != points.shape[0] * points.shape[1]:
+            raise SystemExit(f'--scan {path}: weights must be one per point, got {weights.shape} for points '
+                             f'{points.shape}')
+        weights = weights.reshape(points.shape[:2])
+    return points, weights
 
 
 def _load_init(path, n, last):

@@ -745,6 +745,123 @@ def mesh_to_mesh_forward(query_triangles, target_triangles, max_collisions=16, p
     return [faces, bcs]
 
 
+# -------------------------------------------------------------------------------------------- scans
+MAX_SCAN_FACES = 32768       # faces of a mesh the scan queries take (the tree's shared-memory sort)
+MAX_SCAN_POINTS = 32768      # scan points per body (the point tree's and the backward's shared-memory sorts)
+
+
+def _scan_points(points, weights, B=None):
+    """points (B, N, 3) and weights (B, N) or None as the scan entries take them; ValueError past the limits."""
+    p = _cuda_f32(points, 'points')
+    if p.dim() != 3 or p.shape[2] != 3 or (B is not None and p.shape[0] != B):
+        raise ValueError(f'points must be ({"B" if B is None else B}, N, 3), got {tuple(p.shape)}')
+    if p.shape[1] > MAX_SCAN_POINTS:
+        raise ValueError(f'{p.shape[1]} scan points per body exceed the {MAX_SCAN_POINTS} supported: subsample the scan')
+    if weights is not None:
+        weights = _cuda_f32(weights, 'weights')
+        if weights.shape != p.shape[:2]:
+            raise ValueError(f'weights must be {tuple(p.shape[:2])}, got {tuple(weights.shape)}')
+    return p, weights
+
+
+def _scan_mesh(vertices, faces_i32):
+    v = _cuda_f32(vertices, 'vertices')
+    faces_i32 = _faces_i32(faces_i32)
+    if v.dim() != 3 or v.shape[2] != 3 or faces_i32.dim() != 2 or faces_i32.shape[1] != 3 or faces_i32.shape[0] == 0:
+        raise ValueError(f'vertices must be (B, V, 3) and faces (F >= 1, 3), got {tuple(v.shape)} and '
+                         f'{tuple(faces_i32.shape)}')
+    if faces_i32.shape[0] > MAX_SCAN_FACES:
+        raise ValueError(f'{faces_i32.shape[0]} faces exceed the {MAX_SCAN_FACES} the scan queries support')
+    return v, faces_i32
+
+
+class ScanTree:
+    """The workspace of closest_points holding its LBVH, for a later call to refit instead of rebuilding."""
+
+    def __init__(self):
+        self.ws, self.key = None, None
+
+
+def closest_points(vertices, faces_i32, points, weights=None, tree=None):
+    """Exact closest point of each scan point on its body's mesh (include/shapy_b200.h, shapy_closest_points):
+    vertices (B, V, 3), faces_i32 (F, 3) int32, points (B, N, 3), weights (B, N) or None.  Returns (face_idx (B, N)
+    int32, bary (B, N, 3), sq_dist (B, N)); a point with weight <= 0 is never read and gets face -1, distance 0.
+    tree: a ScanTree; the first call with it builds the tree in it, the next ones with the same batch size and faces
+    refit it (the same bits as a fresh build)."""
+    v, faces_i32 = _scan_mesh(vertices, faces_i32)
+    B, V, F = v.shape[0], v.shape[1], faces_i32.shape[0]
+    p, w = _scan_points(points, weights, B)
+    N, dev = p.shape[1], v.device
+    face = torch.empty(B, N, dtype=torch.int32, device=dev)
+    bary = torch.empty(B, N, 3, dtype=torch.float32, device=dev)
+    d2 = torch.empty(B, N, dtype=torch.float32, device=dev)
+    if B == 0 or N == 0:
+        return face, bary, d2
+    _incidence_rows(faces_i32, V)          # checks that the faces index the vertices (cached for the backward)
+    with torch.cuda.device(dev):
+        nbytes = lib().shapy_closest_points_workspace_bytes(B, F)
+        key = (B, F, faces_i32.data_ptr(), faces_i32._version, dev.index)
+        if tree is None:
+            ws, refit = _WS.get('scan', nbytes, dev), 0
+        else:
+            refit = int(tree.key == key)
+            if not refit:
+                tree.ws, tree.key = _workspace(nbytes, dev), key
+            ws = tree.ws
+        check(lib().shapy_closest_points(ptr(v), ptr(faces_i32), B, V, F, ptr(p), N, ptr(w), refit, ptr(face),
+                                         ptr(bary), ptr(d2), ptr(ws), ws.numel(), stream_ptr()), 'closest_points')
+    return face, bary, d2
+
+
+def nearest_points(queries, points, weights=None):
+    """Nearest kept scan point of each query (include/shapy_b200.h, shapy_nearest_points): queries (B, Q, 3), points
+    (B, N, 3), weights (B, N) or None.  Returns (idx (B, Q) int32, sq_dist (B, Q)); idx -1 and distance 0 for a body
+    without a point of weight > 0."""
+    q = _cuda_f32(queries, 'queries')
+    if q.dim() != 3 or q.shape[2] != 3:
+        raise ValueError(f'queries must be (B, Q, 3), got {tuple(q.shape)}')
+    B, Q = q.shape[:2]
+    p, w = _scan_points(points, weights, B)
+    N, dev = p.shape[1], q.device
+    if N == 0:
+        return (torch.full((B, Q), -1, dtype=torch.int32, device=dev),
+                torch.zeros(B, Q, dtype=torch.float32, device=dev))
+    idx = torch.empty(B, Q, dtype=torch.int32, device=dev)
+    d2 = torch.empty(B, Q, dtype=torch.float32, device=dev)
+    if B == 0 or Q == 0:
+        return idx, d2
+    with torch.cuda.device(dev):
+        ws = _WS.get('scan_nn', lib().shapy_nearest_points_workspace_bytes(B, N), dev)
+        check(lib().shapy_nearest_points(ptr(q), B, Q, ptr(p), N, ptr(w), ptr(idx), ptr(d2), ptr(ws), ws.numel(),
+                                         stream_ptr()), 'nearest_points')
+    return idx, d2
+
+
+def closest_points_backward(vertices, faces_i32, points, face_idx, bary, grad_sq_dist):
+    """Gradient (B, V, 3) of closest_points' sq_dist with respect to the vertices, face and barycentrics held at the
+    forward's values (include/shapy_b200.h, shapy_closest_points_backward): deterministic, no atomics, one launch."""
+    v, faces_i32 = _scan_mesh(vertices, faces_i32)
+    B, V, F = v.shape[0], v.shape[1], faces_i32.shape[0]
+    p, _ = _scan_points(points, None, B)
+    N = p.shape[1]
+    g = _cuda_f32(grad_sq_dist, 'grad_sq_dist')
+    bary = _cuda_f32(bary, 'bary')
+    if not (torch.is_tensor(face_idx) and face_idx.is_cuda and face_idx.dtype == torch.int32):
+        raise RuntimeError('face_idx must be a CUDA int32 tensor')
+    face_idx = face_idx.contiguous()
+    if g.shape != (B, N) or face_idx.shape != (B, N) or bary.shape != (B, N, 3):
+        raise ValueError(f'grad_sq_dist and face_idx must be ({B}, {N}) and bary ({B}, {N}, 3)')
+    grad = torch.empty_like(v)
+    if B == 0:
+        return grad
+    with torch.cuda.device(v.device):
+        inc_ptr, inc = _incidence_rows(faces_i32, V)
+        check(lib().shapy_closest_points_backward(ptr(v), ptr(faces_i32), ptr(inc_ptr), ptr(inc), B, V, F, ptr(p), N,
+                                                  ptr(face_idx), ptr(bary), ptr(g), ptr(grad), stream_ptr()),
+              'closest_points_backward')
+    return grad
+
+
 # -------------------------------------------------------------------------------------------- head
 def head_forward(feats, W0, b0, W1, b1, W2, b2, mean, num_stages=3):
     feats = _cuda_f32(feats, 'features')
