@@ -28,7 +28,7 @@
 //     `stages` slots (full / empty mbarriers) runs ahead across tile boundaries; persistent, one CTA per SM.  Two
 //     consumer schedules:
 //       - cooperative: both consumers work on the same tile, each issuing wgmma m64nNk16 for 64 of its 128 rows, and
-//         both run the epilogue of their rows at the same time (the tensor cores idle meanwhile);
+//         both run the epilogue of their rows at the same time into one staging box (the tensor cores idle meanwhile);
 //       - ping-pong: each consumer owns whole tiles (two m64 accumulator sets, all 128 rows) and the two alternate
 //         through the CTA's tile sequence.  A pair of hand-off mbarriers orders the mainloops: a consumer starts its
 //         tile's k-blocks only after the other has issued all of the previous tile's, so one consumer's epilogue runs
@@ -36,9 +36,10 @@
 //     Both give every output row the same wgmma sequence and the same epilogue arithmetic.
 // Split-fp16 parity mode keeps activations and weights as fp16 hi + fp16 lo (x = hi + lo/2048) and issues
 // A_hi.[B_hi|B_lo] as ONE N = 2 NT wgmma into [D0|D1] plus A_lo.B_hi into D1' (out = D0 + (D1 + D1')/2048).
-// Epilogue: registers -> +bias (+residual) -> ReLU -> split to fp16 hi/lo -> global stores (cooperative), or -> the
-// consumer's shared-memory staging box, into which TMA loaded the residual during the mainloop, -> one TMA tensor store
-// per plane (ping-pong).
+// Epilogue, the same in both schedules: registers -> +bias (+residual) -> ReLU -> split to fp16 hi/lo -> stmatrix into
+// the tile's shared-memory staging box (ping-pong: the consumer's), into which TMA loaded the residual during the
+// mainloop (read back with ldmatrix) -> TMA tensor stores.  The box is stored in column boxes of 64 / 32 / 16 channels
+// with the TMA swizzle of their rows, so the 16-byte matrix rows and the TMA accesses are free of bank conflicts.
 // Replaces cuDNN conv + BatchNorm + ReLU + residual add (4 launches, 4 HBM round trips) of
 // regressor/human_shape/models/backbone/hrnet.py and torchvision BasicBlock / Bottleneck.
 #include <cmath>
@@ -59,7 +60,6 @@ constexpr int KCH = 64;   // channels per k-block: 128-byte rows, SWIZZLE_128B
 struct alignas(64) WgmmaParams {
   CUtensorMap a_hi[4], a_lo[4];  // [parity] (stride 2) or [0] (stride 1)
   CUtensorMap b_hi, b_lo;
-  int N, Ho, Wo;                 // output extent
   int TW, TH, TN;                // M-tile box (TW * TH * TN <= 128 rows)
   int tiles_w, tiles_h, tiles_n;
   int cin, cout, ksize, stride;
@@ -75,16 +75,14 @@ struct alignas(64) WgmmaParams {
   uint32_t h_slice;              // resident path: smem pitch of one 16-channel slice of a halo plane
   uint32_t w_bytes;              // resident path: TMA bytes (= smem bytes) of the whole weight set, all planes
   const float *bias;
-  __half *out_hi, *out_lo;
-  int out_ctot, out_coff;
-  const __half *res_hi, *res_lo;
-  int res_ctot, res_coff;
-  // ping-pong epilogue: output / residual maps over the [N][Ho][Wo] x cout view (box NT x o_bw x TH x TN, the padded
-  // grid's junk columns excluded), and the shared-memory staging box of each consumer
+  int res, res_lo;               // the epilogue adds a residual (hi plane; and lo plane, split mode)
+  int out_lo;                    // split mode: the epilogue stores the output's lo plane
+  // epilogue: output / residual maps over the [N][Ho][Wo] x cout view (boxes stage_cw(NT) x o_bw x TH x TN, the
+  // padded grid's junk columns excluded), and the shared-memory staging box of the tile (one per consumer in ping-pong)
   CUtensorMap o_hi, o_lo, r_hi, r_lo;
   int o_bw;                      // box width: Wo on the halo path, TW on the per-tap path
-  uint32_t o_plane;              // smem pitch of one staged plane (hi or lo)
-  uint32_t o_bytes;              // TMA bytes of one plane's box
+  uint32_t o_plane;              // smem pitch of one staged plane (hi or lo): 128 rows x NT
+  uint32_t o_bytes;              // TMA bytes of one plane's tile (all its column boxes)
 };
 
 constexpr int kThreads = 384;                // producer warpgroup + two consumer warpgroups
@@ -102,6 +100,11 @@ __device__ unsigned long long g_conv_stamps[6];
 template <bool SPLIT, int NT>
 constexpr int cons_accs() { return (SPLIT ? 2 * NT : NT) / 2 + (SPLIT ? NT / 2 : 0); }
 
+// The staging box of a plane is NT / CW column boxes of 128 rows x CW channels, each stored with the TMA swizzle of its
+// CW * 2-byte rows (128 / 64 / 32 B), CW the widest of 64, 32, 16 that divides NT: no padding, and the 8 rows of every
+// stmatrix / ldmatrix matrix (8 consecutive box rows, one 16-byte chunk) fall in 8 distinct 16-byte bank groups.
+constexpr int stage_cw(int nt) { return nt % 64 == 0 ? 64 : (nt % 32 == 0 ? 32 : 16); }
+
 template <bool SPLIT, int NT, bool HALO, bool PP, bool RES>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_constant__ WgmmaParams p) {
   static_assert(!RES || HALO, "the weight-resident path is a halo path");
@@ -112,22 +115,24 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   constexpr int MT = PP ? 2 : 1;                    // m64 accumulator sets per consumer: ping-pong owns all 128 rows
   constexpr int CONS = PP ? 1 : 2;                  // consumers that release each ring slot
   static_assert(!PP || MT * cons_accs<SPLIT, NT>() <= 192, "ping-pong accumulators must fit the consumer registers");
+  constexpr int CW = stage_cw(NT);                // channels per column box of the staged tile
+  constexpr uint32_t CB_BYTES = 128u * CW * 2;      // one column box (a multiple of its swizzle's 256 / 512 / 1024 B)
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t A_BLK = 128 * KCH * 2;
   // shared memory: [halo ring (halo path)] [ring of k-block stages: A (per-tap path) + B | resident weights]
-  //                [ping-pong: output staging box of consumer 0, of consumer 1] [mbarriers]
+  //                [output staging box (ping-pong: of consumer 0, of consumer 1), 1024-aligned] [mbarriers]
   const uint32_t h_stage = p.h_plane * PARTS;
   const uint32_t ring_base = smem_base + (HALO ? h_stage * p.hstages : 0u);
   const uint32_t kblk_bytes = (HALO ? 0u : A_BLK * PARTS) + p.b_stride;   // one stage = one k-block of one tap
-  const uint32_t o_base = ring_base + (RES ? p.w_bytes : kblk_bytes * p.stages);
-  const uint32_t bar_base = o_base + (PP ? 2u * p.o_plane * PARTS : 0u);
+  const uint32_t o_base = (ring_base + (RES ? p.w_bytes : kblk_bytes * p.stages) + 1023u) & ~1023u;
+  const uint32_t bar_base = o_base + (PP ? 2u : 1u) * p.o_plane * PARTS;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
   auto hfull_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
   auto hempty_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + p.hstages + s); };
   // ping-pong: consumer c arrives on handoff_bar(c) once it has issued every k-block of its tile
   auto handoff_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + c); };
-  // ping-pong: the residual box of consumer c's tile has landed in its staging box
+  // the residual of consumer c's tile (cooperative: of the tile, c = 0) has landed in its staging box
   auto res_bar = [&](int c) { return bar_base + 8u * (2 * p.stages + 2 * p.hstages + 2 + c); };
   // resident path: the weight set has landed
   const uint32_t w_bar = bar_base + 8u * (2 * p.stages + 2 * p.hstages + 4);
@@ -146,7 +151,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS); }
     for (int s = 0; s < (HALO ? p.hstages : 0); ++s) { mbar_init(hfull_bar(s), 1); mbar_init(hempty_bar(s), CONS); }
-    if (PP) for (int c = 0; c < 2; ++c) { mbar_init(handoff_bar(c), 1); mbar_init(res_bar(c), 1); }
+    for (int c = 0; c < 2; ++c) { mbar_init(handoff_bar(c), 1); mbar_init(res_bar(c), 1); }
     if (RES) mbar_init(w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -241,9 +246,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     int s = 0, hs = 0;
     uint32_t ph = 0, hph = 0, hoph = 0, rph = 0;
-    // ping-pong: this consumer's output staging box (hi plane, then lo), and the same bytes as a generic pointer
-    const uint32_t ob = o_base + (uint32_t)cw * p.o_plane * PARTS;
-    uint8_t *const ob_ptr = smem_raw + (ob - smem_u32(smem_raw));
+    // the output staging box this consumer writes (hi plane, then lo); one thread loads the residual into it and stores
+    // it, after a barrier over the threads that write it (ping-pong: this consumer; cooperative: both)
+    const uint32_t ob = o_base + (PP ? (uint32_t)cw : 0u) * p.o_plane * PARTS;
+    const bool issuer = t == 0 && (PP || cw == 0);
+    const int ebar = PP ? 1 + cw : 1, ethreads = PP ? 128 : 256;
+    const int rb = PP ? cw : 0;
     // ping-pong: step the ring positions over the k-blocks (and halo loads) of the other consumer's tile
     auto skip_tile = [&]() {
       const int q = s + iters, hq = hs + p.kpt;
@@ -263,11 +271,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
         mbar_wait(handoff_bar(cw ^ 1), hoph);
         hoph ^= 1;
       }
-      if (PP && p.res_hi && t == 0) {             // the residual box loads under the mainloop
+      if (p.res && issuer) {                      // the residual loads under the mainloop
         bulk_wait_read();                         // once the previous tile's output has left the staging box
-        mbar_expect_tx(res_bar(cw), p.o_bytes * ((SPLIT && p.res_lo) ? 2u : 1u));
-        tma_load_4d(ob, &p.r_hi, res_bar(cw), c_out0, w0, h0, n0);
-        if (SPLIT && p.res_lo) tma_load_4d(ob + p.o_plane, &p.r_lo, res_bar(cw), c_out0, w0, h0, n0);
+        mbar_expect_tx(res_bar(rb), p.o_bytes * ((SPLIT && p.res_lo) ? 2u : 1u));
+#pragma unroll
+        for (int k = 0; k < NT / CW; ++k) {
+          tma_load_4d(ob + k * CB_BYTES, &p.r_hi, res_bar(rb), c_out0 + k * CW, w0, h0, n0);
+          if (SPLIT && p.res_lo) tma_load_4d(ob + p.o_plane + k * CB_BYTES, &p.r_lo, res_bar(rb), c_out0 + k * CW, w0, h0, n0);
+        }
       }
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
@@ -428,74 +439,76 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       st2 = clock64();
 #endif
 
-      // ---- epilogue: this thread holds rows r0 and r0 + 8 of each m64 set, two adjacent columns of every 8-column group.
-      // Ping-pong stages the outputs in shared memory (over the residual, each element read and written by the same
-      // thread) and stores the box with one TMA store per plane; cooperative stores straight to global memory.
-      if (PP) {
-        if (p.res_hi) {
-          mbar_wait(res_bar(cw), rph);
-          rph ^= 1;
-        } else {
-          if (t == 0) bulk_wait_read();
-          named_bar_sync(1 + cw, 128);
-        }
+      // ---- epilogue: this thread holds rows r0 and r0 + 8 of each m64 set, two adjacent columns of every 8-column group
+      // (the mma C fragment).  The outputs are staged in shared memory over the residual, which TMA loaded there during
+      // the mainloop, 16 x 16 blocks at a time with ldmatrix / stmatrix (each element read and written by the same
+      // thread), and leave with one TMA store per column box and plane.
+      float2 bq[NT / 8];
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) bq[j] = __ldg(reinterpret_cast<const float2 *>(p.bias + c_out0 + 8 * j + 2 * (lane & 3)));
+      if (p.res) {
+        mbar_wait(res_bar(rb), rph);
+        rph ^= 1;
+      } else {
+        if (issuer) bulk_wait_read();
+        named_bar_sync(ebar, ethreads);
       }
-      const int q4 = lane & 3;
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
+        // this lane's row address serves matrix lane / 8 of each x4: rows + 8 for odd matrices, channels + 8 for 2, 3
+        const int row = (int)row0 + m * 64 + warp * 16 + (lane & 7) + (lane & 8);
+        const int dw = row % p.TW, dh = (row / p.TW) % p.TH, dn = row / (p.TW * p.TH);
+        // a tile row without a slot in the box (the padded grid's junk columns, rows past the box) goes to box row 127:
+        // the box then has fewer than 128 rows, so no slot is there.  Rows past Ho / N have slots; TMA drops them.
+        const uint32_t br = dn < p.TN && dw < p.o_bw ? (uint32_t)((dn * p.TH + dh) * p.o_bw + dw) : 127u;
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int row = (int)row0 + m * 64 + warp * 16 + (lane >> 2) + 8 * half;
-          const int dw = row % p.TW, dh = (row / p.TW) % p.TH, dn = row / (p.TW * p.TH);
-          const int ow = w0 + dw, oh = h0 + dh, on = n0 + dn;
-          if (!(dn < p.TN && ow < p.Wo && oh < p.Ho && on < p.N)) continue;
-          const size_t pix = ((size_t)on * p.Ho + oh) * p.Wo + ow;
-          const size_t oo = pix * p.out_ctot + p.out_coff + c_out0;
-          const size_t ro = pix * p.res_ctot + p.res_coff + c_out0;
-          const uint32_t so = (uint32_t)((dn * p.TH + dh) * p.o_bw + dw) * NT;   // element of the staging box
+        for (int jp = 0; jp < NT / 16; ++jp) {
+          const uint32_t o = br * (CW * 2) + (uint32_t)((16 * jp) % CW / 8 + (lane >> 4)) * 16;
+          const uint32_t a = ob + (16 * jp / CW) * CB_BYTES + (o ^ (((o >> 7) & (CW / 8 - 1)) << 4));   // the TMA swizzle
+          uint32_t rh[4], rl[4], sh[4], sl[4];
+          if (p.res) {
+            ldmatrix_x4(rh, a);
+            if (SPLIT && p.res_lo) ldmatrix_x4(rl, a + p.o_plane);
+          }
 #pragma unroll
-          for (int j = 0; j < NT / 8; ++j) {
-            const int c = 8 * j + 2 * q4;
-            const int i = 4 * j + 2 * half;
-            const float2 bq = __ldg(reinterpret_cast<const float2 *>(p.bias + c_out0 + c));
+          for (int k = 0; k < 4; ++k) {            // matrix k: rows + 8 (k & 1), 8-column group 2 jp + (k >> 1)
+            const int j = 2 * jp + (k >> 1);
+            const int i = 4 * j + 2 * (k & 1);
             float r0 = acc[m][i], r1 = acc[m][i + 1];
             if (SPLIT) {
               r0 += (acc[m][NT / 2 + i] + acl[m][SPLIT ? i : 0]) * kLoInv;
               r1 += (acc[m][NT / 2 + i + 1] + acl[m][SPLIT ? i + 1 : 0]) * kLoInv;
             }
-            r0 += bq.x; r1 += bq.y;
-            __half2 *const sh = reinterpret_cast<__half2 *>(ob_ptr + 2u * (so + c));
-            __half2 *const sl = reinterpret_cast<__half2 *>(ob_ptr + p.o_plane + 2u * (so + c));
-            if (p.res_hi) {
-              const __half2 rh = PP ? *sh : *reinterpret_cast<const __half2 *>(p.res_hi + ro + c);
-              r0 += __low2float(rh); r1 += __high2float(rh);
+            r0 += bq[j].x; r1 += bq[j].y;
+            if (p.res) {
+              const __half2 h = *reinterpret_cast<const __half2 *>(&rh[k]);
+              r0 += __low2float(h); r1 += __high2float(h);
               if (SPLIT && p.res_lo) {
-                const __half2 rl = PP ? *sl : *reinterpret_cast<const __half2 *>(p.res_lo + ro + c);
-                r0 += __low2float(rl) * kLoInv; r1 += __high2float(rl) * kLoInv;
+                const __half2 l = *reinterpret_cast<const __half2 *>(&rl[k]);
+                r0 += __low2float(l) * kLoInv; r1 += __high2float(l) * kLoInv;
               }
             }
             if (p.relu) { r0 = fmaxf(r0, 0.f); r1 = fmaxf(r1, 0.f); }
             __half h0_, h1_, l0_, l1_;
             split_store(r0, h0_, l0_);
             split_store(r1, h1_, l1_);
-            if (PP) {
-              *sh = __halves2half2(h0_, h1_);
-              if (SPLIT && p.out_lo) *sl = __halves2half2(l0_, l1_);
-            } else {
-              *reinterpret_cast<__half2 *>(p.out_hi + oo + c) = __halves2half2(h0_, h1_);
-              if (SPLIT && p.out_lo) *reinterpret_cast<__half2 *>(p.out_lo + oo + c) = __halves2half2(l0_, l1_);
-            }
+            const __half2 hv = __halves2half2(h0_, h1_), lv = __halves2half2(l0_, l1_);
+            sh[k] = *reinterpret_cast<const uint32_t *>(&hv);
+            sl[k] = *reinterpret_cast<const uint32_t *>(&lv);
           }
+          stmatrix_x4(a, sh);
+          if (SPLIT && p.out_lo) stmatrix_x4(a + p.o_plane, sl);
         }
       }
-      if (PP) {                                   // the staged box -> global memory; TMA drops rows past the map
-        fence_proxy_async_smem();
-        named_bar_sync(1 + cw, 128);
-        if (t == 0) {
-          tma_store_4d(&p.o_hi, ob, c_out0, w0, h0, n0);
-          if (SPLIT && p.out_lo) tma_store_4d(&p.o_lo, ob + p.o_plane, c_out0, w0, h0, n0);
-          bulk_commit();
+      fence_proxy_async_smem();                   // the staged tile -> global memory; TMA drops rows past the map
+      named_bar_sync(ebar, ethreads);
+      if (issuer) {
+#pragma unroll
+        for (int k = 0; k < NT / CW; ++k) {
+          tma_store_4d(&p.o_hi, ob + k * CB_BYTES, c_out0 + k * CW, w0, h0, n0);
+          if (SPLIT && p.out_lo) tma_store_4d(&p.o_lo, ob + p.o_plane + k * CB_BYTES, c_out0 + k * CW, w0, h0, n0);
         }
+        bulk_commit();
       }
 #ifdef SHAPY_CONV_STAMPS
       if (t == 0) {                               // warp 0's end of the epilogue
@@ -511,7 +524,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgmma_kernel(const __grid_co
       }
 #endif
     }
-    if (PP && t == 0) bulk_wait();                // the last stores have completed before shared memory is released
+    if (issuer) bulk_wait();                      // the last stores have completed before shared memory is released
   }
 }
 
@@ -610,7 +623,6 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   const int PARTS = split ? 2 : 1;
   pl->split = split;
   const int sms = sm_count();
-  p.N = out.N; p.Ho = out.H; p.Wo = out.W;
   p.TW = std::min(out.W, 128);
   p.TH = std::max(1, std::min(out.H, 128 / p.TW));
   p.TN = (p.TW == out.W && p.TH == out.H) ? std::max(1, std::min(out.N, 128 / (p.TW * p.TH))) : 1;
@@ -626,9 +638,12 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   const int Wp = out.W + 2;
   const uint32_t h_plane = (uint32_t)align_up((size_t)(128 + 2 * Wp + 2) * KCH * 2, 1024);
   {
-    // two halo slots and at least two weight slots of the widest cout tile must fit the shared-memory budget
-    const size_t b_max = align_up((size_t)std::min(w.cout, split ? 96 : 128) * KCH * 2 * PARTS, 1024);
-    const bool possible = w.ksize == 3 && w.stride == 1 && Wp <= 128 && 2 * (h_plane * PARTS + b_max) <= 216 * 1024;
+    // two halo slots, at least two weight slots and the staging box of the widest cout tile must fit the shared-memory
+    // budget
+    const int nt_max = std::min(w.cout, split ? 96 : 128);
+    const size_t b_max = align_up((size_t)nt_max * KCH * 2 * PARTS, 1024);
+    const bool possible = w.ksize == 3 && w.stride == 1 && Wp <= 128 &&
+                          2 * (h_plane * PARTS + b_max) + (size_t)nt_max * 128 * 2 * PARTS <= 222 * 1024;
     bool better = false;
     int th = 0;
     if (possible) {
@@ -701,13 +716,15 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   pl->resident = res_shape && pl->NT == w.cout && (data_path == WGMMA_RESIDENT || (data_path == WGMMA_AUTO && resident_enabled()));
   p.relu = relu;
   p.pdl_late = 1;
-  // ping-pong output staging: one box per consumer and plane (the output tile without the padded grid's junk columns)
+  // output staging: one box per plane (ping-pong: per consumer and plane) of 128 rows x NT; the output tile without the
+  // padded grid's junk columns fills its first o_bw x TH x TN rows
   p.o_bw = pl->halo ? out.W : p.TW;
   p.o_bytes = (uint32_t)pl->NT * p.o_bw * p.TH * p.TN * 2;
-  p.o_plane = (uint32_t)align_up((size_t)p.o_bytes, 1024);
+  p.o_plane = (uint32_t)pl->NT * 128 * 2;
+  auto staging = [&]() { return (pl->pingpong ? 2 : 1) * (size_t)p.o_plane * PARTS; };
   if (pl->resident) {
     // two halo slots of cin / 16 slices per plane, each slice the rows the furthest tap reads in 32-byte rows, the
-    // whole weight set, the staging boxes: up to the 227 KB a CTA may own
+    // whole weight set, the 1024-aligned staging boxes: up to the 227 KB a CTA may own
     const int S = w.cin / 16;
     p.h_slice = (uint32_t)align_up((size_t)(128 + 2 * Wp + 2) * 32, 256);
     p.h_plane = p.h_slice * S;
@@ -716,8 +733,8 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     p.b_tx = (uint32_t)pl->NT * 32;
     p.w_bytes = 9u * S * PARTS * p.b_tx;
     p.a_bytes = (uint32_t)p.TW * (p.TH + 2) * w.cin * 2;
-    const size_t staging = pl->pingpong ? 2 * (size_t)p.o_plane * PARTS : 0;
-    pl->smem = (size_t)p.h_plane * PARTS * p.hstages + p.w_bytes + staging + 8 * (2 * p.hstages + 5) + 1024;
+    pl->smem = align_up((size_t)p.h_plane * PARTS * p.hstages + p.w_bytes, 1024) + staging() + 8 * (2 * p.hstages + 5) +
+               1024;
     if (pl->smem > 227 * 1024) {
       if (data_path == WGMMA_RESIDENT) {
         set_error("wgmma_plan_create: the weight-resident path does not fit shared memory (cin %d cout %d, %zu B)",
@@ -741,22 +758,20 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     p.b_tx = (uint32_t)pl->NT * kbox * 2;
     p.b_stride = (uint32_t)align_up((size_t)p.b_bytes * PARTS, 1024);
   }
-  // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory; ping-pong takes its two staging boxes
-  // out of the weight ring and may use up to 222 KB
+  // one persistent CTA per SM owns (almost) all of its 227 KB of shared memory: the staging box(es) and the rings take
+  // up to 222 KB
   auto plan_smem = [&]() {
-    const size_t staging = pl->pingpong ? 2 * (size_t)p.o_plane * PARTS : 0;
-    const size_t budget = (pl->pingpong ? 222 : 216) * 1024 - staging;
+    const size_t budget = 222 * 1024 - staging();
     if (pl->halo) {
       p.h_plane = h_plane;
       p.hstages = 2;
       const size_t halo = (size_t)h_plane * PARTS * p.hstages;
       p.stages = halo + 2 * p.b_stride <= budget ? (int)std::min<size_t>(8, (budget - halo) / p.b_stride) : 0;
-      pl->smem = halo + staging + (size_t)p.b_stride * p.stages + 16 * (p.stages + p.hstages + 2) + 1024;
+      pl->smem = halo + staging() + (size_t)p.b_stride * p.stages + 16 * (p.stages + p.hstages + 2) + 1024;
     } else {
       const size_t stage = 128u * KCH * 2 * PARTS + p.b_stride;
       p.stages = (int)std::min<size_t>(8, budget / stage);
-      if (!pl->pingpong) p.stages = std::max(2, p.stages);
-      pl->smem = staging + stage * p.stages + 16 * (p.stages + 2) + 1024;
+      pl->smem = staging() + stage * p.stages + 16 * (p.stages + 2) + 1024;
     }
     // a planned ping-pong needs three weight slots: with two, the ring stalls the mainloop (split b64, NT 64: 111.8
     // against 103.9 us cooperative)
@@ -770,12 +785,16 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       return nullptr;
     }
     pl->pingpong = false;                         // the planner's choice is always at the cooperative cout tile
-    plan_smem();
+    if (!plan_smem()) {
+      set_error("wgmma_plan_create: no room for the ring and the staging box (cin %d cout %d %dx%d)", w.cin, w.cout,
+                out.H, out.W);
+      delete pl;
+      return nullptr;
+    }
   }
   p.bias = w.bias;
-  p.out_hi = out.hi; p.out_lo = out.lo; p.out_ctot = out.Ctot; p.out_coff = out.coff;
-  p.res_hi = res ? res->hi : nullptr; p.res_lo = res ? res->lo : nullptr;
-  p.res_ctot = res ? res->Ctot : 0; p.res_coff = res ? res->coff : 0;
+  p.out_lo = out.lo != nullptr;
+  p.res = res != nullptr; p.res_lo = res && res->lo;
   const int items = p.tiles_w * p.tiles_h * p.tiles_n * (w.cout / pl->NT);
   pl->grid = dim3(even_grid(items, sms), 1);
   {
@@ -789,11 +808,11 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
   if (getenv("SHAPY_CONV_DEBUG"))
     fprintf(stderr,
             "[wgmma] cin %d cout %d k %d s %d %dx%d N %d: %s %s NT %d tile %dx%dx%d grid %d stages %d+%d, staging "
-            "2x%ux%u B, smem %zu B, TMA %.1f MB, MMA %.2f GFLOP\n",
+            "%dx%ux%u B, smem %zu B, TMA %.1f MB, MMA %.2f GFLOP\n",
             w.cin, w.cout, w.ksize, w.stride, out.H, out.W, out.N,
             pl->resident ? "resident" : (pl->halo ? "halo" : "per-tap"),
             pl->pingpong ? "ping-pong" : "cooperative", pl->NT, p.TW, p.TH, p.TN, pl->grid.x, p.hstages, p.stages,
-            pl->pingpong ? (unsigned)PARTS : 0u, p.o_plane, pl->smem, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
+            pl->pingpong ? 2 : 1, (unsigned)PARTS, p.o_plane, pl->smem, pl->tma_bytes * 1e-6, pl->mma_flops * 1e-9);
   bool ok = true;
   const int swz = pl->resident ? 16 : KCH;   // row width of the shared-memory operands in channels: picks the swizzle
   // activation maps
@@ -825,15 +844,16 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     ok = ok && encode(&p.b_hi, w.w_hi, 3, dims, strides, box, swz);
     if (split) ok = ok && encode(&p.b_lo, w.w_lo, 3, dims, strides, box, swz);
   }
-  // ping-pong epilogue maps: the output view (out_coff / out_ctot as the activation maps carry coff / Ctot) and the
-  // residual view, in boxes of the staged tile; no swizzle (the epilogue addresses the box row-major)
+  // epilogue maps: the output view (out_coff / out_ctot as the activation maps carry coff / Ctot) and the residual
+  // view, in column boxes of the staged tile with the swizzle of their rows
   auto view_map = [&](CUtensorMap *m, const __half *base, const ActView &v) {
+    const int cw = stage_cw(pl->NT);
     cuuint64_t dims[4] = {(cuuint64_t)w.cout, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N};
     cuuint64_t strides[3] = {(cuuint64_t)v.Ctot * 2, (cuuint64_t)v.W * v.Ctot * 2, (cuuint64_t)v.H * v.W * v.Ctot * 2};
-    cuuint32_t box[4] = {(cuuint32_t)pl->NT, (cuuint32_t)p.o_bw, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
-    return encode(m, base + v.coff, 4, dims, strides, box, 0);
+    cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)p.o_bw, (cuuint32_t)p.TH, (cuuint32_t)p.TN};
+    return encode(m, base + v.coff, 4, dims, strides, box, cw);
   };
-  if (ok && pl->pingpong) {
+  if (ok) {
     ok = view_map(&p.o_hi, out.hi, out) && (!out.lo || view_map(&p.o_lo, out.lo, out));
     if (ok && res) ok = view_map(&p.r_hi, res->hi, *res) && (!split || !res->lo || view_map(&p.r_lo, res->lo, *res));
   }
