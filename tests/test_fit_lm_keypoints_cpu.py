@@ -5,35 +5,8 @@ import numpy as np
 import torch
 
 import kp_lm_oracle
+from lm_harness import keypoints_at, rodrigues
 from shapy_b200 import synth
-from smplx_grad_ref import forward_differentiable
-
-
-def _rodrigues(aa):
-    aa = torch.as_tensor(aa, dtype=torch.float64)
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
-
-
-def _skew(d):
-    z = torch.zeros_like(d[..., 0])
-    return torch.stack([z, -d[..., 2], d[..., 1], d[..., 2], z, -d[..., 0], -d[..., 1], d[..., 0], z],
-                       -1).view(*d.shape[:-1], 3, 3)
-
-
-def _keypoints(model, betas, rot, transl, params):
-    """Keypoints (N, K, 3) at the parameter offsets params (N, P) = [delta (3 n_rot) | betas | transl], float64."""
-    N, n_rot = params.shape[0], rot.shape[0]
-    nb = betas.shape[0]
-    d = params[:, :3 * n_rot].reshape(N, n_rot, 3)
-    R = rot.double()[None] @ torch.linalg.matrix_exp(_skew(d))
-    out = forward_differentiable(model, betas.double()[None] + params[:, 3 * n_rot:3 * n_rot + nb], R)
-    return out['joints'] + (transl.double()[None] + params[:, 3 * n_rot + nb:])[:, None]
 
 
 def test_oracle_jacobian_vs_central_differences():
@@ -41,14 +14,14 @@ def test_oracle_jacobian_vs_central_differences():
     gen = torch.Generator().manual_seed(4)
     n_rot = 22
     for b, neck in enumerate((1.2, -1.2)):                 # necks turned past both ends of the contour LUT
-        rot = _rodrigues(torch.randn(n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
-        rot[12] = _rodrigues(torch.tensor([0.0, neck, 0.0])).float()
+        rot = rodrigues(torch.randn(n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
+        rot[12] = rodrigues(torch.tensor([0.0, neck, 0.0])).float()
         betas = torch.randn(10, generator=gen)
         transl = torch.randn(3, generator=gen) * 0.1
         kp, jac = kp_lm_oracle.keypoint_jacobian(model, betas, rot, transl)
         P = 3 * n_rot + 10 + 3
         assert jac.shape == (3 * 123, P) and kp.shape == (123, 3)
-        base = _keypoints(model, betas, rot, transl, torch.zeros(1, P, dtype=torch.float64))[0].numpy()
+        base = keypoints_at(model, betas, rot, transl, torch.zeros(1, P, dtype=torch.float64))[0].numpy()
         assert np.abs(kp - base).max() <= 1e-9 * np.abs(base).max()
         h = 1e-5
         fd = []
@@ -56,7 +29,7 @@ def test_oracle_jacobian_vs_central_differences():
             e = torch.zeros(2 * len(half), P, dtype=torch.float64)
             for i, c in enumerate(half):
                 e[2 * i, c], e[2 * i + 1, c] = h, -h
-            y = _keypoints(model, betas, rot, transl, e).reshape(len(half), 2, -1).numpy()
+            y = keypoints_at(model, betas, rot, transl, e).reshape(len(half), 2, -1).numpy()
             fd.append(((y[:, 0] - y[:, 1]) / (2 * h)).T)
         fd = np.concatenate(fd, 1)
         for name, cols in (('rot', slice(0, 3 * n_rot)), ('betas', slice(3 * n_rot, 3 * n_rot + 10)),
@@ -72,7 +45,7 @@ def test_oracle_step_fits_rotations_with_non_increasing_loss():
     K = 12
     p = rng.normal(size=(K, 3))
     q = rng.normal(size=(K, 3)) * 0.2
-    R1, R2 = _rodrigues(rng.normal(size=3) * 0.8).numpy(), _rodrigues(rng.normal(size=3) * 0.8).numpy()
+    R1, R2 = rodrigues(rng.normal(size=3) * 0.8).numpy(), rodrigues(rng.normal(size=3) * 0.8).numpy()
     bstar, tstar = np.array([0.7]), rng.normal(size=3)
     half = K // 2
 

@@ -10,7 +10,7 @@ import torch
 
 import kp2d_calibrated_lm_oracle as oc
 import kp2d_lm_oracle as o2
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
 INTR = np.array([1000.0, 500.0, 480.0])
 T0 = np.array([0.1, -0.2, 0.3])                # the toy body's world translation
@@ -33,7 +33,7 @@ def _look_at(azimuth_deg, radius=6.0, height=0.0, target=np.zeros(3)):
 def _rand_ext(rng):
     """A random view 5-8 m from the origin, looking near it."""
     ext = _look_at(rng.uniform(0, 360), rng.uniform(5, 8), rng.uniform(-1, 1), rng.normal(size=3) * 0.2)
-    R = ext[:9].reshape(3, 3) @ _expm(rng.normal(size=3) * 0.05)
+    R = ext[:9].reshape(3, 3) @ expm(rng.normal(size=3) * 0.05)
     return np.concatenate([R.reshape(9), ext[9:]])
 
 
@@ -47,8 +47,8 @@ def _views(rng, kp, V=3, noise=20.0):
 
 
 def _case(seed, V=3):
-    evaluate, rng = _problem(seed)
-    rot = np.stack([_expm(rng.normal(size=3) * 0.5) for _ in range(2)])
+    evaluate, rng = toy_problem(seed)
+    rot = np.stack([expm(rng.normal(size=3) * 0.5) for _ in range(2)])
     beta = np.array([0.3])
     kp, jac = evaluate(rot, beta)
     return evaluate, rng, rot, beta, kp, jac, _views(rng, kp, V)
@@ -56,7 +56,7 @@ def _case(seed, V=3):
 
 def _at(evaluate, rot, beta, theta):
     """(rotations, betas, t, keypoints) at the offsets theta = [delta_0, delta_1 | beta | t]."""
-    R = np.stack([rot[j] @ _expm(theta[3 * j:3 * j + 3]) for j in range(2)])
+    R = np.stack([rot[j] @ expm(theta[3 * j:3 * j + 3]) for j in range(2)])
     b = beta + theta[6:7]
     kp, _ = evaluate(R, b)
     return R, b, T0 + theta[7:], kp
@@ -92,7 +92,7 @@ def test_gradient_is_half_the_loss_gradient(sigma, pose_w, betas_w, meas):
     """g = sum_views J^T W r + priors + measurement rows equals half the central-difference gradient of the loss; a
     dropped keypoint with NaN target and rows is never read."""
     evaluate, rng, rot, beta, kp, jac, views = _case(22)
-    anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
+    anchor = np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in rot])
     jac[9:12] = np.nan
     mf = _meas(rng, beta) if meas else None
     _, g, _ = oc.normal_equations(views, kp, jac, T0, sigma, rot, anchor, pose_w, beta, betas_w,
@@ -151,7 +151,7 @@ def test_one_identity_view_is_the_perspective_step(first, sigma, pose_w, betas_w
     w[3], tg[3] = 0.0, np.nan
     ident = np.concatenate([np.eye(3).reshape(9), np.zeros(3)])
     views = (tg[None], w[None], INTR[None], ident[None])
-    anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
+    anchor = np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in rot])
     A1, g1, d1 = oc.normal_equations(views, kp, jac, t, sigma, rot, anchor, pose_w, beta, betas_w)
     A2, g2, d2 = o2.normal_equations(tg, w, kp, jac, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)
     for a, b in ((A1, A2), (g1, g2), (d1, d2)):
@@ -159,7 +159,7 @@ def test_one_identity_view_is_the_perspective_step(first, sigma, pose_w, betas_w
     assert abs(oc.loss(views, kp, t, sigma, rot, anchor, pose_w, beta, betas_w) -
                o2.loss(tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)) <= 1e-12 * abs(o2.loss(
                    tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR))
-    trial_kp, trial_jac = evaluate(np.stack([r @ _expm(rng.normal(size=3) * 0.05) for r in rot]), beta + 0.05)
+    trial_kp, trial_jac = evaluate(np.stack([r @ expm(rng.normal(size=3) * 0.05) for r in rot]), beta + 0.05)
     state = {'rot': rot, 'betas': beta, 'transl': t, 'keypoints': kp, 'jac': jac, 'lambda': np.float32(1e-2),
              'loss': np.float32(o2.loss(tg, w, kp, t, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR))}
     trial = {'rot': rot, 'betas': beta + 0.05, 'transl': t + 0.01}
@@ -174,8 +174,8 @@ def test_one_identity_view_is_the_perspective_step(first, sigma, pose_w, betas_w
 
 @pytest.mark.parametrize('sigma', [math.inf, 50.0])
 def test_fp64_lm_on_a_noiseless_four_camera_rig_recovers_pose_shape_and_world_translation(sigma):
-    evaluate, rng = _problem(25)
-    R1, R2 = _expm(rng.normal(size=3) * 0.6), _expm(rng.normal(size=3) * 0.6)
+    evaluate, rng = toy_problem(25)
+    R1, R2 = expm(rng.normal(size=3) * 0.6), expm(rng.normal(size=3) * 0.6)
     bstar, tstar = np.array([0.6]), np.array([0.3, -0.1, 0.4])
     kp, _ = evaluate(np.stack([R1, R2]), bstar)
     ext = np.stack([_look_at(a) for a in (0.0, 90.0, 180.0, 270.0)])
@@ -184,7 +184,7 @@ def test_fp64_lm_on_a_noiseless_four_camera_rig_recovers_pose_shape_and_world_tr
     w = np.ones((4, 12))
     w[1, 2], tg[1, 2] = 0.0, np.nan
     views = (tg, w, intr, ext)
-    trial = {'rot': np.stack([R1 @ _expm(rng.normal(size=3) * 0.2), R2 @ _expm(rng.normal(size=3) * 0.2)]),
+    trial = {'rot': np.stack([R1 @ expm(rng.normal(size=3) * 0.2), R2 @ expm(rng.normal(size=3) * 0.2)]),
              'betas': np.zeros(1), 'transl': tstar + np.array([0.1, 0.1, -0.2])}
     state, losses = {}, []
     for it in range(60):

@@ -14,7 +14,7 @@ from kp_lm_oracle import keypoint_jacobian
 from oracle.lm_oracle import cholesky_solve
 from shapy_b200 import synth
 from smplx_grad_ref import forward_differentiable
-from test_fit_lm_kp2d_cpu import _expm
+from lm_harness import expm
 
 
 def _model():
@@ -22,7 +22,7 @@ def _model():
 
 
 def _rotations(rng, n, scale):
-    return np.stack([_expm(rng.normal(size=3) * scale) for _ in range(n)])
+    return np.stack([expm(rng.normal(size=3) * scale) for _ in range(n)])
 
 
 def test_expression_and_wide_rotation_columns_vs_central_differences():
@@ -49,7 +49,7 @@ def test_expression_and_wide_rotation_columns_vs_central_differences():
         d = np.zeros(3)
         d[a] = h
         rp, rm = rot.copy(), rot.copy()
-        rp[j], rm[j] = rot[j] @ _expm(d), rot[j] @ _expm(-d)
+        rp[j], rm[j] = rot[j] @ expm(d), rot[j] @ expm(-d)
         fd = (joints(rp, psi) - joints(rm, psi)) / (2 * h)
         assert np.abs(jac[:, 3 * j + a] - fd).max() <= 1e-6 * max(1.0, np.abs(fd).max()), (j, a)
 
@@ -87,11 +87,11 @@ def test_no_expression_at_22_joints_is_todays_oracle(first, persp):
     tg = o2.project(c['kp'], last, intr) + \
         rng.normal(size=(30, 2)) * (5.0 if persp else 0.02)
     w = rng.uniform(0.5, 1.5, 30)
-    anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.1) for r in c['rot']])
+    anchor = np.stack([r @ expm(rng.normal(size=3) * 0.1) for r in c['rot']])
     f32 = lambda x: np.asarray(x, np.float32)  # noqa: E731
     state = {'rot': f32(c['rot']), 'betas': f32(c['betas']), lk: f32(last), 'keypoints': f32(c['kp']),
              'jac': f32(c['jac']), 'loss': np.float32(50.0), 'lambda': np.float32(0.3), 'accepted': 0}
-    trial = {'rot': f32(np.stack([r @ _expm(rng.normal(size=3) * 0.05) for r in c['rot']])),
+    trial = {'rot': f32(np.stack([r @ expm(rng.normal(size=3) * 0.05) for r in c['rot']])),
              'betas': f32(c['betas'] + 0.05), lk: f32(last + 0.01)}
     tkp, tjac = f32(c['kp'] + 0.01), f32(c['jac'] * 1.01)
     sigma = 20.0 if persp else 0.3
@@ -125,7 +125,7 @@ def test_fp64_lm_loop_never_raises_the_loss(persp):
     w = np.ones(K)
     jw = np.zeros(n_rot)
     jw[1:22], jw[22:] = 0.5, 0.1
-    trial = {'rot': np.stack([r @ _expm(rng.normal(size=3) * 0.1) for r in rot_t]), 'betas': beta_t + 0.3,
+    trial = {'rot': np.stack([r @ expm(rng.normal(size=3) * 0.1) for r in rot_t]), 'betas': beta_t + 0.3,
              'expression': np.zeros(NE), lk: last_t + (np.array([0.02, 0.02, 0.3]) if persp else 0.05)}
     anchor = trial['rot'].copy()
     state = {'accepted': 0}

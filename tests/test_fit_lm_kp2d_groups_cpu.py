@@ -11,25 +11,25 @@ import torch
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
 from oracle.lm_oracle import meas_loss
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
 K = 12
 
 
 def _views(M, seed, sigma=math.inf, pose_w=0.0, noise=0.05):
-    """M views of one body of _problem (shared betas bstar, per-view rotations and camera), targets from bstar, a
+    """M views of one body of toy_problem (shared betas bstar, per-view rotations and camera), targets from bstar, a
     state and a trial near them."""
-    evaluate, rng = _problem(seed, K)
+    evaluate, rng = toy_problem(seed, K)
     bstar = np.array([0.5])
     images, state, trial = [], {'rot': [], 'camera': [], 'keypoints': [], 'jac': []}, {'rot': [], 'camera': []}
     beta_s, beta_t = bstar + 0.2, bstar + 0.1
     for _ in range(M):
-        R = np.stack([_expm(rng.normal(size=3) * 0.6) for _ in range(2)])
+        R = np.stack([expm(rng.normal(size=3) * 0.6) for _ in range(2)])
         cam = np.array([0.5 + 0.2 * rng.normal(), 0.1 * rng.normal(), 0.1 * rng.normal()])
         kp, _ = evaluate(R, bstar)
         tg = o2.project(kp, cam) + noise * rng.normal(size=(K, 2))
-        Rs = np.stack([r @ _expm(rng.normal(size=3) * 0.1) for r in R])
-        Rt = np.stack([r @ _expm(rng.normal(size=3) * 0.05) for r in R])
+        Rs = np.stack([r @ expm(rng.normal(size=3) * 0.1) for r in R])
+        Rt = np.stack([r @ expm(rng.normal(size=3) * 0.05) for r in R])
         cs, ct = cam + 0.05 * rng.normal(size=3), cam + 0.02 * rng.normal(size=3)
         ks, js = evaluate(Rs, beta_s)
         kt, jt = evaluate(Rt, beta_t)

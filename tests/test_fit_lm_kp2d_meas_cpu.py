@@ -8,9 +8,9 @@ import numpy as np
 import pytest
 
 import kp2d_lm_oracle as o2
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
-P = 10              # _problem: two rotations, one betas, the camera
+P = 10              # toy_problem: two rotations, one betas, the camera
 MW = np.array([1.0, 100.0, 2000.0, 1000.0, 1000.0])
 
 
@@ -24,10 +24,10 @@ def _measure(beta):
 
 
 def _case(seed, sigma=0.3, pose_w=0.5, betas_w=0.2):
-    evaluate, rng = _problem(seed)
-    rot = np.stack([_expm(rng.normal(size=3) * 0.5) for _ in range(2)])
+    evaluate, rng = toy_problem(seed)
+    rot = np.stack([expm(rng.normal(size=3) * 0.5) for _ in range(2)])
     beta, cam = np.array([0.3]), np.array([0.4, 0.05, -0.1])
-    anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
+    anchor = np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in rot])
     kp, jac = evaluate(rot, beta)
     tg = o2.project(kp, cam) + rng.normal(size=(12, 2)) * 0.2
     w = rng.uniform(0.5, 1.5, 12)
@@ -90,7 +90,7 @@ def test_normal_equations_equal_the_stacked_jacobian(sigma, pose_w, betas_w):
 
 def _step_inputs(c, seed=3):
     rng = np.random.default_rng(seed)
-    trot = np.stack([r @ _expm(rng.normal(size=3) * 0.02) for r in c['rot']])
+    trot = np.stack([r @ expm(rng.normal(size=3) * 0.02) for r in c['rot']])
     tbeta, tcam = c['beta'] + 0.02, c['cam'] + 0.01 * rng.normal(size=3)
     tkp, tjac = c['evaluate'](trot, tbeta)
     tjac[9:12] = np.nan
@@ -166,8 +166,8 @@ def test_nan_in_a_dropped_measurement_changes_nothing_and_a_weighted_nan_rejects
 def test_fp64_lm_loss_non_increasing_and_height_fixes_the_scale(sigma):
     """The targets are the projection of (R*, beta*, c*) and the measurements those of beta*: every iteration's loss is
     non-increasing and the fit ends at a zero of the total loss, the measurements matched."""
-    evaluate, rng = _problem(8)
-    R1, R2 = _expm(rng.normal(size=3) * 0.6), _expm(rng.normal(size=3) * 0.6)
+    evaluate, rng = toy_problem(8)
+    R1, R2 = expm(rng.normal(size=3) * 0.6), expm(rng.normal(size=3) * 0.6)
     bstar, cstar = np.array([0.6]), np.array([0.5, 0.1, -0.05])
     kp, _ = evaluate(np.stack([R1, R2]), bstar)
     tg = o2.project(kp, cstar)
@@ -175,7 +175,7 @@ def test_fp64_lm_loss_non_increasing_and_height_fixes_the_scale(sigma):
     w[2], tg[2] = 0.0, np.nan
     mt, _ = _measure(bstar)
     mw = np.array([1.0, 100.0, 0.0, 0.0, 0.0])              # mass and height
-    trial = {'rot': np.stack([R1 @ _expm(rng.normal(size=3) * 0.2), R2 @ _expm(rng.normal(size=3) * 0.2)]),
+    trial = {'rot': np.stack([R1 @ expm(rng.normal(size=3) * 0.2), R2 @ expm(rng.normal(size=3) * 0.2)]),
              'betas': np.zeros(1), 'camera': np.array([0.3, 0.0, 0.0])}
     state, losses = {}, []
     for it in range(60):

@@ -10,15 +10,15 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
 INTR = np.array([1000.0, 500.0, 480.0])
 T0 = np.array([0.1, -0.2, 5.0])              # the toy keypoints are ~N(0, 1): 5 m keeps them in front
 
 
 def _case(seed, sigma_noise=20.0):
-    evaluate, rng = _problem(seed)
-    rot = np.stack([_expm(rng.normal(size=3) * 0.5) for _ in range(2)])
+    evaluate, rng = toy_problem(seed)
+    rot = np.stack([expm(rng.normal(size=3) * 0.5) for _ in range(2)])
     beta = np.array([0.3])
     kp, jac = evaluate(rot, beta)
     tg = o2.project(kp, T0, INTR) + rng.normal(size=(12, 2)) * sigma_noise
@@ -29,7 +29,7 @@ def _case(seed, sigma_noise=20.0):
 
 def _at(evaluate, rot, beta, theta):
     """(rotations, betas, t, keypoints) at the offsets theta = [delta_0, delta_1 | beta | t]."""
-    R = np.stack([rot[j] @ _expm(theta[3 * j:3 * j + 3]) for j in range(2)])
+    R = np.stack([rot[j] @ expm(theta[3 * j:3 * j + 3]) for j in range(2)])
     b = beta + theta[6:7]
     kp, _ = evaluate(R, b)
     return R, b, T0 + theta[7:], kp
@@ -55,7 +55,7 @@ def test_gradient_is_half_the_loss_gradient(sigma, pose_w, betas_w):
     """g = J^T W r + priors equals half the central-difference gradient of the loss: the perspective rows, the IRLS
     weights, the pose-prior rows and betas_w beta; a dropped keypoint with NaN target and rows is never read."""
     evaluate, rng, rot, beta, kp, jac, tg, w = _case(12)
-    anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
+    anchor = np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in rot])
     jac[9:12] = np.nan
     _, g, _ = o2.normal_equations(tg, w, kp, jac, T0, sigma, rot, anchor, pose_w, beta, betas_w, intr=INTR)
 
@@ -99,14 +99,14 @@ def test_depth_rule():
 
 @pytest.mark.parametrize('sigma', [math.inf, 50.0])
 def test_fp64_lm_recovers_rotations_shape_and_translation(sigma):
-    evaluate, rng = _problem(14)
-    R1, R2 = _expm(rng.normal(size=3) * 0.6), _expm(rng.normal(size=3) * 0.6)
+    evaluate, rng = toy_problem(14)
+    R1, R2 = expm(rng.normal(size=3) * 0.6), expm(rng.normal(size=3) * 0.6)
     bstar, tstar = np.array([0.6]), np.array([0.3, -0.1, 4.0])
     kp, _ = evaluate(np.stack([R1, R2]), bstar)
     tg = o2.project(kp, tstar, INTR)
     w = np.ones(12)
     w[2], tg[2] = 0.0, np.nan
-    trial = {'rot': np.stack([R1 @ _expm(rng.normal(size=3) * 0.2), R2 @ _expm(rng.normal(size=3) * 0.2)]),
+    trial = {'rot': np.stack([R1 @ expm(rng.normal(size=3) * 0.2), R2 @ expm(rng.normal(size=3) * 0.2)]),
              'betas': np.zeros(1), 'transl': tstar + np.array([0.1, 0.1, 0.8])}
     state, losses = {}, []
     for it in range(60):

@@ -10,13 +10,13 @@ import pytest
 import kp2d_lm_oracle as o2
 import kp2d_sequence_lm_oracle as osq
 import kp2dg_lm_oracle as og
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
 INTR = np.array([1000.0, 500.0, 480.0])
 
 
 def _rots(rng, n=2, s=0.8):
-    return np.stack([_expm(rng.normal(size=3) * s) for _ in range(n)])
+    return np.stack([expm(rng.normal(size=3) * s) for _ in range(n)])
 
 
 def test_smoothness_rows_vs_central_differences():
@@ -30,8 +30,8 @@ def test_smoothness_rows_vs_central_differences():
     n1 = 9
 
     def L(th):
-        a = np.stack([r0[j] @ _expm(th[3 * j:3 * j + 3]) for j in range(2)])
-        b = np.stack([r1[j] @ _expm(th[n1 + 3 * j:n1 + 3 * j + 3]) for j in range(2)])
+        a = np.stack([r0[j] @ expm(th[3 * j:3 * j + 3]) for j in range(2)])
+        b = np.stack([r1[j] @ expm(th[n1 + 3 * j:n1 + 3 * j + 3]) for j in range(2)])
         return osq.smooth_loss(a, b, t0 + th[6:9], t1 + th[n1 + 6:], srw, stw)
 
     h = 1e-6
@@ -56,18 +56,18 @@ def test_smoothness_rows_vs_central_differences():
 def _sequence(seed, T, sigma_noise=5.0):
     """T frames of the toy body (two chained rotations, one betas) turning and walking in front of the camera, with
     noisy targets; returns (evaluate, frames, state-like per-frame (rot, transl), beta)."""
-    evaluate, rng = _problem(seed)
+    evaluate, rng = toy_problem(seed)
     beta = np.array([0.3])
     base = _rots(rng, s=0.5)
     frames, rots, trs = [], [], []
     for t in range(T):
-        rot = np.stack([base[j] @ _expm(rng.normal(size=3) * 0.1 + 0.05 * t) for j in range(2)])
+        rot = np.stack([base[j] @ expm(rng.normal(size=3) * 0.1 + 0.05 * t) for j in range(2)])
         tr = np.array([0.1 * t - 0.5, -0.2, 5.0 + 0.05 * t])
         kp, _ = evaluate(rot, beta)
         tg = o2.project(kp, tr, INTR) + rng.normal(size=(12, 2)) * sigma_noise
         w = rng.uniform(0.5, 1.5, 12)
         w[3], tg[3] = 0.0, np.nan
-        anchor = np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in rot])
+        anchor = np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in rot])
         frames.append({'targets': tg, 'weights': w, 'intr': INTR, 'anchor': anchor})
         rots.append(rot)
         trs.append(tr)
@@ -108,7 +108,7 @@ def test_block_sweep_equals_a_dense_solve(T):
 def _step_args(evaluate, frames, rots, trs, beta, rng):
     """A state at (rots, trs, beta) with its loss, and a trial nearby."""
     st = _state(evaluate, rots, trs, beta)
-    trial = {'rot': [np.stack([r @ _expm(rng.normal(size=3) * 0.05) for r in rot]) for rot in rots],
+    trial = {'rot': [np.stack([r @ expm(rng.normal(size=3) * 0.05) for r in rot]) for rot in rots],
              'transl': [t + rng.normal(size=3) * 0.02 for t in trs], 'betas': beta + 0.05}
     for t, fr in enumerate(frames):
         fr['trial_kp'], fr['trial_jac'] = evaluate(trial['rot'][t], trial['betas'])
@@ -190,7 +190,7 @@ def test_fp64_lm_loss_never_rises_on_a_short_sequence(smooth):
     T = 6
     evaluate, frames, rots, trs, beta = _sequence(50, T, sigma_noise=0.5)
     rng = np.random.default_rng(51)
-    trial = {'rot': [np.stack([r @ _expm(rng.normal(size=3) * 0.15) for r in rot]) for rot in rots],
+    trial = {'rot': [np.stack([r @ expm(rng.normal(size=3) * 0.15) for r in rot]) for rot in rots],
              'transl': [t + np.array([0.05, 0.05, 0.4]) * rng.normal(size=3) for t in trs], 'betas': np.zeros(1)}
     state, losses = {}, []
     for it in range(40):

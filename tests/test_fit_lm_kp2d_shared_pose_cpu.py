@@ -13,27 +13,27 @@ import kp2d_lm_oracle as o2
 import kp2d_shared_pose_lm_oracle as osp
 import kp2dg_lm_oracle as og
 from oracle.lm_oracle import meas_loss
-from test_fit_lm_kp2d_cpu import _expm, _problem
+from lm_harness import expm, toy_problem
 
 K = 12
 
 
 def _views(M, seed, noise=0.05):
-    """M views of one posed body of _problem: shared R_1* and betas*, per-view R_0 and camera; targets from them, and
+    """M views of one posed body of toy_problem: shared R_1* and betas*, per-view R_0 and camera; targets from them, and
     a state and a trial near them whose body rotation is one per group, as the device keeps it."""
-    evaluate, rng = _problem(seed, K)
+    evaluate, rng = toy_problem(seed, K)
     bstar = np.array([0.5])
-    R1 = _expm(rng.normal(size=3) * 0.6)
-    R1s, R1t = R1 @ _expm(rng.normal(size=3) * 0.1), R1 @ _expm(rng.normal(size=3) * 0.05)
+    R1 = expm(rng.normal(size=3) * 0.6)
+    R1s, R1t = R1 @ expm(rng.normal(size=3) * 0.1), R1 @ expm(rng.normal(size=3) * 0.05)
     images, state, trial = [], {'rot': [], 'camera': [], 'keypoints': [], 'jac': []}, {'rot': [], 'camera': []}
     beta_s, beta_t = bstar + 0.2, bstar + 0.1
     for _ in range(M):
-        R0 = _expm(rng.normal(size=3) * 0.6)
+        R0 = expm(rng.normal(size=3) * 0.6)
         cam = np.array([0.5 + 0.2 * rng.normal(), 0.1 * rng.normal(), 0.1 * rng.normal()])
         kp, _ = evaluate(np.stack([R0, R1]), bstar)
         tg = o2.project(kp, cam) + noise * rng.normal(size=(K, 2))
-        Rs = np.stack([R0 @ _expm(rng.normal(size=3) * 0.1), R1s])
-        Rt = np.stack([R0 @ _expm(rng.normal(size=3) * 0.05), R1t])
+        Rs = np.stack([R0 @ expm(rng.normal(size=3) * 0.1), R1s])
+        Rt = np.stack([R0 @ expm(rng.normal(size=3) * 0.05), R1t])
         cs, ct = cam + 0.05 * rng.normal(size=3), cam + 0.02 * rng.normal(size=3)
         ks, js = evaluate(Rs, beta_s)
         kt, jt = evaluate(Rt, beta_t)
@@ -44,7 +44,7 @@ def _views(M, seed, noise=0.05):
         trial['camera'].append(ct)
     state['betas'] = beta_s
     trial['betas'] = beta_t
-    anchor = np.stack([np.eye(3), R1 @ _expm(rng.normal(size=3) * 0.05)])
+    anchor = np.stack([np.eye(3), R1 @ expm(rng.normal(size=3) * 0.05)])
     return evaluate, images, state, trial, anchor, (R1, bstar)
 
 
@@ -212,10 +212,10 @@ def test_one_rotation_equals_the_grouped_oracle(first, with_meas):
     M = 3
     images, state, trial = [], {'rot': [], 'camera': [], 'keypoints': [], 'jac': []}, {'rot': [], 'camera': []}
     for _ in range(M):
-        R = _expm(rng.normal(size=3) * 0.6)[None]
+        R = expm(rng.normal(size=3) * 0.6)[None]
         cam = np.array([0.5, 0.0, 0.0]) + 0.1 * rng.normal(size=3)
         kp, _ = evaluate(R, np.array([0.5]))
-        Rs, Rt = R @ _expm(rng.normal(size=3) * 0.1), R @ _expm(rng.normal(size=3) * 0.05)
+        Rs, Rt = R @ expm(rng.normal(size=3) * 0.1), R @ expm(rng.normal(size=3) * 0.05)
         ks, js = evaluate(Rs, np.array([0.7]))
         kt, jt = evaluate(Rt, np.array([0.6]))
         images.append({'targets': o2.project(kp, cam) + 0.02 * rng.normal(size=(K, 2)),
@@ -308,9 +308,9 @@ def test_shared_start_is_the_chordal_mean_made_a_rotation_by_gram_schmidt():
     columns); decoded, the Gram-Schmidt of that mean.  Identical rotations give themselves back."""
     from shapy_b200.fit import _group_sum, _shared_body_raw, group_plan
     rng = np.random.default_rng(3)
-    base = np.stack([_expm(rng.normal(size=3)) for _ in range(21)])
-    views = [np.stack([r @ _expm(rng.normal(size=3) * 0.2) for r in base]) for _ in range(3)]
-    rot = torch.tensor(np.stack([np.concatenate([_expm(rng.normal(size=3))[None], v]) for v in views] +
+    base = np.stack([expm(rng.normal(size=3)) for _ in range(21)])
+    views = [np.stack([r @ expm(rng.normal(size=3) * 0.2) for r in base]) for _ in range(3)]
+    rot = torch.tensor(np.stack([np.concatenate([expm(rng.normal(size=3))[None], v]) for v in views] +
                                 [np.concatenate([np.eye(3)[None], base])]), dtype=torch.float32)  # (4, 22, 3, 3)
     order, off = group_plan(torch.tensor([0, 0, 0, 1]), 4)
     cnt = (off[1:] - off[:-1]).float()

@@ -5,6 +5,7 @@ LM loops never synchronise with the host, and Adam runs with the exact gradient.
 import pytest
 import torch
 
+import lm_harness as harness
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -130,13 +131,9 @@ def test_lm_loops_never_synchronise(model):
               init=_init(32))                                 # on the device before the check: no copy in the loop
     _kp_fit(module, kp, iterations=1, **kw)                 # packs the model, builds the incidence table
     fit_betas_to_measurements(module, bm, tg, method='lm', iterations=1, circumference_derivative='exact')
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = _kp_fit(module, kp, iterations=3, **kw)
-        res2 = fit_betas_to_measurements(module, bm, tg, method='lm', iterations=3, circumference_derivative='exact')
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, (res, res2) = harness.launches_without_sync(lambda: (
+        _kp_fit(module, kp, iterations=3, **kw),
+        fit_betas_to_measurements(module, bm, tg, method='lm', iterations=3, circumference_derivative='exact')))
     assert res['measurements'].shape == (32, 5) and res2['betas'].shape == (32, 10)
 
 

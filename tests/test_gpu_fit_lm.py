@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+import lm_harness as harness
+from lm_harness import bits
 from oracle import lm_oracle
 from shapy_b200 import synth
 
@@ -24,10 +26,6 @@ def _generic(nb):
     rng = torch.Generator().manual_seed(nb)
     d['shapedirs'] = torch.randn(d['shapedirs'].shape[0], 3, nb, generator=rng) * 0.01
     return d
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 def _setup(d, B, seed):
@@ -71,7 +69,7 @@ def test_jacobian_vs_composite_and_forward(nb, B):
     assert jac.shape == (B, 5, nb)
     # the measurements are the forward's, bit for bit, NaNs included
     want = ops.measure(lm, v_shaped=v, faces_i32=faces)
-    assert torch.equal(_bits(out), _bits(want))
+    assert torch.equal(bits(out), bits(want))
     assert int(status.item()) == int(want.status.item())
     # at 4096 bodies the composite runs on a sample of 512 of them
     rows = torch.arange(B) if B <= 64 else torch.randperm(B, generator=torch.Generator().manual_seed(1))[:512]
@@ -126,7 +124,7 @@ def test_nan_circumference_rows():
     _check_against_composite(jac, comp, scale)
     for i in (0, 2):
         o1, j1, _ = ops.measure_jacobian_betas(packed, lm, v[i:i + 1].clone(), faces)
-        assert torch.equal(_bits(j1[0]), _bits(jac[i])) and torch.equal(_bits(o1[0]), _bits(out[i]))
+        assert torch.equal(bits(j1[0]), bits(jac[i])) and torch.equal(bits(o1[0]), bits(out[i]))
 
 
 def _padded(d, V_total):
@@ -159,7 +157,7 @@ def test_global_vertex_source_equals_staged():
     assert torch.equal(vp[:, :d['v_template'].shape[0]], v)
     out, jac, _ = ops.measure_jacobian_betas(packed, lm, v, faces)
     outp, jacp, _ = ops.measure_jacobian_betas(big, lm, vp, faces)
-    assert torch.equal(_bits(outp), _bits(out))
+    assert torch.equal(bits(outp), bits(out))
     comp, scale = _composite(ops, packed, d['shapedirs'], lm, v, faces)
     _check_against_composite(jacp, comp, scale)
     _check_against_composite(jac, comp, scale)
@@ -271,12 +269,12 @@ def test_lm_deterministic_and_batch_independent(model):
     tg = _targets(model, 256)
     again = fit_betas_to_measurements(smplx, bm, tg, method='lm', iterations=50)
     for k in ('betas', 'measurements', 'loss'):
-        assert torch.equal(_bits(again[k]), _bits(FITS['lm'][k])), k
+        assert torch.equal(bits(again[k]), bits(FITS['lm'][k])), k
     rows = [3, 40, 77, 101, 150, 199, 230, 255]
     sub = {k: v[rows].contiguous() for k, v in tg.items()}
     res8 = fit_betas_to_measurements(smplx, bm, sub, method='lm', iterations=50)
     for k in ('betas', 'measurements', 'loss'):
-        assert torch.equal(_bits(res8[k]), _bits(FITS['lm'][k][rows])), k
+        assert torch.equal(bits(res8[k]), bits(FITS['lm'][k][rows])), k
 
 
 def test_lm_loop_never_synchronises(model):
@@ -284,12 +282,7 @@ def test_lm_loop_never_synchronises(model):
     smplx, bm = model
     tg = _targets(model, 32)
     fit_betas_to_measurements(smplx, bm, tg, method='lm', iterations=1)     # packs the model, caches the incidence
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_betas_to_measurements(smplx, bm, tg, method='lm', iterations=5)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_betas_to_measurements(smplx, bm, tg, method='lm', iterations=5))
     assert res['betas'].shape == (32, 10)
 
 

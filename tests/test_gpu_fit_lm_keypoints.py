@@ -9,6 +9,8 @@ import pytest
 import torch
 
 import kp_lm_oracle
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -19,23 +21,12 @@ TOL = 1e-4
 KP_TOL = 2e-6
 
 
-def _rodrigues(aa):
-    aa = aa.double()
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
-
-
 def _inputs(seed, B, n_rot):
     gen = torch.Generator().manual_seed(seed)
-    rot = _rodrigues(torch.randn(B, n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
+    rot = rodrigues(torch.randn(B, n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
     if n_rot > 15 and B > 1:                                 # necks turned past both ends of the contour LUT
-        rot[0, 12] = _rodrigues(torch.tensor([0.0, 1.2, 0.0])).float()
-        rot[1, 12] = _rodrigues(torch.tensor([0.0, -1.2, 0.0])).float()
+        rot[0, 12] = rodrigues(torch.tensor([0.0, 1.2, 0.0])).float()
+        rot[1, 12] = rodrigues(torch.tensor([0.0, -1.2, 0.0])).float()
     return rot, torch.randn(B, 10, generator=gen), torch.randn(B, 3, generator=gen) * 0.1
 
 
@@ -46,10 +37,6 @@ def _model(variant):
             m.pop(k)
         m['use_face_contour'] = False
     return m
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 def _blocks(n_rot):
@@ -122,11 +109,11 @@ def test_jacobian_deterministic_and_batch_independent():
     rot, betas, transl = rot.cuda(), betas.cuda(), transl.cuda()
     kp1, j1 = ops.smplx_keypoint_jacobian(packed, betas, rot, transl)
     kp2, j2 = ops.smplx_keypoint_jacobian(packed, betas, rot, transl)
-    assert torch.equal(_bits(kp1), _bits(kp2)) and torch.equal(_bits(j1), _bits(j2))
+    assert torch.equal(bits(kp1), bits(kp2)) and torch.equal(bits(j1), bits(j2))
     rows = [0, 1, 9, 20, 33, 41, 50, 63]
     kp8, j8 = ops.smplx_keypoint_jacobian(packed, betas[rows].contiguous(), rot[rows].contiguous(),
                                           transl[rows].contiguous())
-    assert torch.equal(_bits(kp8), _bits(kp1[rows])) and torch.equal(_bits(j8), _bits(j1[rows]))
+    assert torch.equal(bits(kp8), bits(kp1[rows])) and torch.equal(bits(j8), bits(j1[rows]))
 
 
 def _step_case():
@@ -138,7 +125,7 @@ def _step_case():
     B, K = 6, packed.K
     rot, betas, transl = _inputs(11, B, 22)
     gen = torch.Generator().manual_seed(12)
-    trot = (rot.double() @ _rodrigues(torch.randn(B, 22, 3, generator=gen, dtype=torch.float64) * 0.02)).float()
+    trot = (rot.double() @ rodrigues(torch.randn(B, 22, 3, generator=gen, dtype=torch.float64) * 0.02)).float()
     tbetas = betas + 0.05 * torch.randn(B, 10, generator=gen)
     ttransl = transl + 0.01 * torch.randn(B, 3, generator=gen)
     c = lambda t: t.cuda().contiguous()  # noqa: E731
@@ -161,34 +148,10 @@ def _step_case():
 
 @pytest.mark.parametrize('first', [False, True])
 def test_step_kernel_vs_oracle(first):
-    from shapy_b200 import ops
     c = _step_case()
-    B = c['rot'].shape[0]
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'transl': cu(c['transl']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(c['loss']), 'lambda': cu(c['lam']),
-             'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'transl': cu(c['ttransl'])}
-    ops.fit_lm_keypoints_step(state, trial, cu(c['tg']), cu(c['w']), 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']))
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    n = lambda t: t.numpy()  # noqa: E731
-    flags = []
-    for b in range(B):
-        s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'transl': n(c['transl'][b]), 'keypoints': n(c['kp'][b]),
-             'jac': n(c['jac'][b]), 'loss': n(c['loss'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
-        new, want, acc = kp_lm_oracle.lm_keypoints_step(s, n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                        n(c['tkp'][b]), n(c['tjac'][b]))
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        assert got['lambda'][b] == new['lambda'], (b, got['lambda'][b], new['lambda'])
-        assert np.array_equal(got['loss'][b], new['loss'], equal_nan=True), b
-        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac'):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'transl'):
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= 2e-6 * max(1.0, np.abs(want[k]).max()), (b, k, err)
+    state, trial = harness.kp_device(c)
+    harness.kp_step(c, state, trial, first)
+    flags, _ = harness.kp_check(c, state, trial, first)
     if first:
         assert all(flags)
     else:
@@ -225,8 +188,7 @@ def _fit(module, kp, **kw):
 
 @pytest.fixture(scope='module')
 def module():
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    return SMPLX(data_struct=synth.make_smplx(), use_face_contour=True).cuda()
+    return harness.smplx_module()
 
 
 def _rms(res, kp):
@@ -258,7 +220,7 @@ def test_lm_fit_8_bodies_alone_equal_their_batch_rows(module):
     rows = [3, 40, 77, 101, 150, 199, 230, 255]
     res8 = _fit(module, FITS['kp'][rows].contiguous(), method='lm')
     for k in ('global_rot', 'body_pose', 'betas', 'transl'):
-        assert torch.equal(_bits(res8[k]), _bits(FITS['lm'][k][rows])), k
+        assert torch.equal(bits(res8[k]), bits(FITS['lm'][k][rows])), k
 
 
 def test_lm_loop_never_synchronises(module):
@@ -267,12 +229,8 @@ def test_lm_loop_never_synchronises(module):
     mean = synth.mean_params().cuda()
     init = {'global_rot': mean[:6].expand(32, 6), 'body_pose': mean[6:132].expand(32, 126)}
     fit_body_to_keypoints(module, kp, init=init, method='lm', iterations=1)      # packs the model
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints(module, kp, init=init, method='lm', iterations=3)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints(module, kp, init=init, method='lm',
+                                                                         iterations=3))
     assert res['betas'].shape == (32, 10)
 
 

@@ -2,186 +2,34 @@
 (tests/kp2d_lm_oracle.py, pinned by tests/test_fit_lm_kp2d_cpu.py) at P = 7, 54, 55, 79, 80 (the 48 KB shared-memory
 opt-in) and 96, and fit_body_to_keypoints_2d end to end on the synthetic SMPL-X: loss definition, monotone losses, no host
 synchronisation, determinism, batch independence, time to quality against Adam, and robustness to outliers."""
-import math
-
 import numpy as np
 import pytest
 import torch
 
 import kp2d_lm_oracle as o2
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _rodrigues(aa):
-    aa = aa.double()
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
-
-
 # ------------------------------------------------------------------------------------------------ step kernel
+# The single-image 2D entries of lm_kp2d_step_kernel<MEAS, PERSP> are each tested on lm_harness.kp2d_case by
+# lm_harness.kp2d_run: the plain one here, the measurement one in test_gpu_model_shapes.py, the perspective ones in
+# test_gpu_fit_lm_kp2d_persp.py and the expressive ones in test_gpu_fit_lm_kp2d_expressive.py.
 # (n_rot, nb): P = 3 n_rot + nb + 3 = 7, 54, 55 (twice), 96, and 79 and 80 (the largest P under 48 KB of shared memory
 # without opting in, and the smallest that opts in); K: 2K = 2, 16 (the staging boundary), 18 and 254 rows
 STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10), (22, 11)]
 STEP_K = [1, 8, 9, 127]
-# (robust_sigma, pose_prior_weight, betas_weight)
-TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
 
 
-def _step_case(n_rot, nb, K, terms, meas=False):
-    """Six bodies with random Jacobians: body 0's trial hits its targets (accepted), body 1's state does and its trial
-    is far (rejected), body 2 has a weighted NaN trial keypoint (rejected), 3 to 5 random.  With K >= 8 keypoint 7 has
-    weight 0 and NaN targets, keypoints and rows in state and trial.  With `meas`, five random measurements and rows
-    stacked under them (drawn after everything else): body 0's trial and body 1's state hit their targets, body 3 has a
-    weighted NaN trial measurement (rejected), and the height has weight 0 and NaN values and rows in state and
-    trial."""
-    sigma, pw, bw = terms
-    B, P = 6, 3 * n_rot + nb + 3
-    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + (3 if pw else 0))
-    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
-    betas = rn(B, nb)
-    cam = rn(B, 3) * torch.tensor([0.5, 0.1, 0.1])
-    tbetas, tcam = betas + 0.05 * rn(B, nb), cam + 0.01 * rn(B, 3)
-    anchor[0], tbetas[0] = trot[0], 0.9 * betas[0]          # the priors favour body 0's trial and body 1's state too
-    anchor[1], tbetas[1] = rot[1], 1.1 * betas[1]
-    kp, jac = rn(B, K, 3), rn(B, 3 * K, P)
-    tkp, tjac = kp + 0.05 * rn(B, K, 3), jac + 0.1 * rn(B, 3 * K, P)
-    kp[0] = tkp[0] + 0.5
-    tkp[1] = kp[1] + 0.5
-    tg = torch.stack([torch.from_numpy(o2.project(kp[b].numpy(), cam[b].numpy())).float() for b in range(B)])
-    tg += 0.05 * rn(B, K, 2)
-    tg[0] = torch.from_numpy(o2.project(tkp[0].numpy(), tcam[0].numpy())).float()
-    tg[1] = torch.from_numpy(o2.project(kp[1].numpy(), cam[1].numpy())).float()
-    tkp[2, 0, 1] = float('nan')
-    w = torch.rand(B, K, generator=gen) + 0.5
-    if K >= 8:
-        w[:, 7] = 0.0
-        tg[:, 7] = float('nan')
-        for t in (kp, tkp):
-            t[:, 7] = float('nan')
-        for t in (jac, tjac):
-            t[:, 21:24] = float('nan')
-    c = dict(rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, trot=trot, tbetas=tbetas, tcam=tcam, tkp=tkp, tjac=tjac,
-             tg=tg, w=w, anchor=anchor, lam=torch.rand(B, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
-    if meas:
-        m, mj = torch.rand(B, 5, generator=gen) + 0.5, rn(B, 5, nb)
-        tm, tmj = m + 0.01 * rn(B, 5), mj + 0.1 * rn(B, 5, nb)
-        mt = m + 0.02 * rn(B, 5)
-        mt[0], mt[1] = tm[0], m[1]
-        mw = torch.rand(B, 5, generator=gen) * 2 + 0.5
-        mw[:, 1] = 0.0
-        for t in (m, tm, mj, tmj):
-            t[:, 1] = float('nan')
-        tm[3, 3] = float('nan')
-        c.update(meas=m, mjac=mj, tmeas=tm, tmjac=tmj, mt=mt, mw=mw)
-    return c
-
-
-def _state_np(c, b):
-    """Body b's state for the restatement, its loss the restatement's (float32)."""
-    n = lambda t: t.numpy()  # noqa: E731
-    s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'camera': n(c['cam'][b]), 'keypoints': n(c['kp'][b]),
-         'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-    if 'meas' in c:
-        s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
-        s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
-                                       n(c['anchor'][b]), c['pw'], s['betas'], c['bw'],
-                                       meas=(n(c['mt'][b]), n(c['mw'][b]), s['meas'])))
-    else:
-        s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['camera'], c['sigma'], s['rot'],
-                                       n(c['anchor'][b]), c['pw'], s['betas'], c['bw']))
-    return s
-
-
-def _device(c):
-    """The case's state and trial on the device, the state's loss from the restatement."""
-    B = c['rot'].shape[0]
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([_state_np(c, b)['loss'] for b in range(B)]))),
-             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    if 'meas' in c:
-        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'camera': cu(c['tcam'])}
-    return state, trial
-
-
-def _step(c, state, trial, first):
-    """One 2D step (with the case's measurement block, the stacked step) on the case's inputs."""
-    from shapy_b200 import ops
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    if 'meas' in c:
-        ops.fit_lm_keypoints_2d_measurements_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'],
-                                                  cu(c['mt']), cu(c['mw']), 10.0, 3.0, first, cu(c['tkp']),
-                                                  cu(c['tjac']), cu(c['tmeas']), cu(c['tmjac']),
-                                                  pose_anchor=cu(c['anchor']))
-    else:
-        ops.fit_lm_keypoints_2d_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
-                                     first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
-
-
-def _run_step(c, first):
-    """The kernel on the case (with its measurement block, the stacked step), then the restatement body by body;
-    returns the largest trial error over its bar."""
-    B = c['rot'].shape[0]
-    meas = 'meas' in c
-    n = lambda t: t.numpy()  # noqa: E731
-    kw = dict(sigma=c['sigma'], pose_w=c['pw'], betas_w=c['bw'])
-    s_np = [_state_np(c, b) for b in range(B)]
-    state, trial = _device(c)
-    _step(c, state, trial, first)
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
-    for b in range(B):
-        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'camera': n(c['tcam'][b])}
-        if meas:
-            new, want, acc = o2.lm_keypoints_2d_step(
-                s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
-                anchor=n(c['anchor'][b]), meas=(n(c['mt'][b]), n(c['mw'][b])),
-                trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), **kw)
-        else:
-            new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                     n(c['tkp'][b]), n(c['tjac'][b]), anchor=n(c['anchor'][b]), **kw)
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        # softplus' exp / log1p may round differently on the device: loss and lambda to fp32 rounding
-        assert np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), (b, got['lambda'][b], new['lambda'])
-        assert np.isclose(got['loss'][b], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (b, got['loss'][b],
-                                                                                          new['loss'])
-        for k in ('rot', 'betas', 'camera', 'keypoints', 'jac') + (('meas', 'meas_jac') if meas else ()):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'camera'):
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= bar, (b, k, err)
-            worst = max(worst, err / bar)
-    if first:
-        assert all(flags)
-    else:
-        assert flags[:3] == [True, False, False] and (not meas or not flags[3]), flags
-    return worst
-
-
-@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('terms', harness.KP2D_TERMS['weak'], ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('K', STEP_K)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_step_kernel_vs_oracle(n_rot, nb, K, first, terms):
-    worst = _run_step(_step_case(n_rot, nb, K, terms), first)
+    worst = harness.kp2d_run(first, n_rot=n_rot, nb=nb, K=K, terms=terms)
     print(f'[kp2d] step P={3 * n_rot + nb + 3} K={K} first={first} terms={terms}: trial error / bar {worst:.3f}')
 
 
@@ -238,25 +86,6 @@ class _FakeModel:
 
 
 # ------------------------------------------------------------------------------------------------ fit
-def _model(variant):
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    m = dict(synth.make_smplx())
-    if variant == 'no_contour_no_j14':
-        for k in ('extra_joint_regressor', 'source_idxs', 'target_idxs'):
-            m.pop(k)
-        return SMPLX(data_struct=m, use_face_contour=False).cuda()
-    return SMPLX(data_struct=m, use_face_contour=True).cuda()
-
-
-_MODELS = {}
-
-
-def _get(variant='full'):
-    if variant not in _MODELS:
-        _MODELS[variant] = _model(variant)
-    return _MODELS[variant]
-
-
 def _problem(module, B, seed=41):
     """Ground truth: betas ~ N(0, 1) clipped to 2, raw pose = mean + 0.3 N(0, 1), a random camera; targets its
     projected keypoints; the start a perturbed copy standing in for a regressor's prediction."""
@@ -311,7 +140,7 @@ def test_lm_loss_definition_and_monotone_losses(variant):
     and fit_body_to_keypoints_2d's returned loss is the kernel's."""
     from shapy_b200 import ops
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get(variant)
+    module = harness.smplx_module(variant)
     x, _, init = _problem(module, 64, seed=5)
     w = (torch.rand(64, x.shape[1], generator=torch.Generator().manual_seed(6)) + 0.5).cuda()
     w[:, 3] = 0.0
@@ -335,7 +164,7 @@ def test_lm_loss_definition_and_monotone_losses(variant):
     res = fit_body_to_keypoints_2d(module, x, w, init=init, method='lm', iterations=20, robust_sigma=0.05,
                                    pose_prior_weight=0.5, betas_weight=0.01)
     for k in ('betas', 'camera'):
-        assert torch.equal(_bits(res[k]), _bits(state[k])), k
+        assert torch.equal(bits(res[k]), bits(state[k])), k
     # the returned loss comes from SMPLX.forward's proj_joints, the kernel's from the Jacobian launch's keypoints
     assert float(((res['loss'] - state['loss']).abs() / state['loss']).max()) <= 1e-2
     assert res['proj_joints'].shape == x.shape and res['keypoints'].shape == (64, x.shape[1], 3)
@@ -343,23 +172,18 @@ def test_lm_loss_definition_and_monotone_losses(variant):
 
 def test_lm_loop_never_synchronises():
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init = _problem(module, 32, seed=7)
     fit_body_to_keypoints_2d(module, x, init=init, method='lm', iterations=1, robust_sigma=0.1,
                              pose_prior_weight=1.0)
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints_2d(module, x, init=init, method='lm', iterations=3, robust_sigma=0.1,
-                                       pose_prior_weight=1.0, betas_weight=0.01)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints_2d(
+        module, x, init=init, method='lm', iterations=3, robust_sigma=0.1, pose_prior_weight=1.0, betas_weight=0.01))
     assert res['betas'].shape == (32, 10)
 
 
 def test_lm_deterministic_and_batch_independent():
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init = _problem(module, 64, seed=8)
     kw = dict(method='lm', iterations=15, robust_sigma=0.1, pose_prior_weight=0.5)
     r1 = fit_body_to_keypoints_2d(module, x, init=init, **kw)
@@ -368,15 +192,15 @@ def test_lm_deterministic_and_batch_independent():
     r8 = fit_body_to_keypoints_2d(module, x[rows].contiguous(), init={k: v[rows].contiguous() for k, v in init.items()},
                                   **kw)
     for k in ('global_rot', 'body_pose', 'betas', 'camera', 'loss'):
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
-        assert torch.equal(_bits(r8[k]), _bits(r1[k][rows])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
+        assert torch.equal(bits(r8[k]), bits(r1[k][rows])), k
 
 
 def test_init_from_the_regressor_stage_output():
     """The regressor's stage dict (raw_global_rot, raw_body_pose, decoded matrices, betas, camera) works as-is."""
     from shapy_b200 import ops
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init = _problem(module, 8, seed=9)
     raw = torch.cat([init['global_rot'], init['body_pose']], 1)
     rot = ops.decode_rot6d(raw)
@@ -384,7 +208,7 @@ def test_init_from_the_regressor_stage_output():
              'body_pose': rot[:, 1:], 'betas': init['betas'], 'camera': init['camera']}
     a = fit_body_to_keypoints_2d(module, x, init=stage, method='lm', iterations=3)
     b = fit_body_to_keypoints_2d(module, x, init=init, method='lm', iterations=3)
-    assert torch.equal(_bits(a['betas']), _bits(b['betas'])) and torch.equal(_bits(a['camera']), _bits(b['camera']))
+    assert torch.equal(bits(a['betas']), bits(b['betas'])) and torch.equal(bits(a['camera']), bits(b['camera']))
 
 
 # Time to quality, 256 bodies, LM(50) against Adam(600); bars set just below / above the first run on an H100 80GB
@@ -398,7 +222,7 @@ LM_MPJPE_BAR = 0.20
 def test_time_to_quality_256_bodies_vs_adam():
     from shapy_b200.fit import fit_body_to_keypoints_2d
     from shapy_b200.metrics import PointError, build_alignment
-    module = _get()
+    module = harness.smplx_module()
     x, joints, init = _problem(module, 256)
     lm = fit_body_to_keypoints_2d(module, x, init=init, method='lm')
     adam = fit_body_to_keypoints_2d(module, x, init=init)
@@ -419,7 +243,7 @@ def test_robust_fit_beats_least_squares_on_outliers():
     """10 % of the keypoints moved by 0.3 in the crop frame: the Geman-McClure fit's inlier RMS beats the
     least-squares fit's."""
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init = _problem(module, 128, seed=43)
     gen = torch.Generator().manual_seed(44)
     out = (torch.rand(x.shape[:2], generator=gen) < 0.1).cuda()
@@ -438,10 +262,10 @@ def test_keypoint_jacobian_2d_vs_oracle_and_forward():
     proj_joints against SMPLX.forward's."""
     from shapy_b200 import ops
     from shapy_b200.fit import keypoint_jacobian, keypoint_jacobian_2d
-    module = _get()
+    module = harness.smplx_module()
     gen = torch.Generator().manual_seed(50)
     B = 8
-    rot = _rodrigues(torch.randn(B, 22, 3, generator=gen, dtype=torch.float64) * 0.4).float().cuda()
+    rot = rodrigues(torch.randn(B, 22, 3, generator=gen, dtype=torch.float64) * 0.4).float().cuda()
     betas = torch.randn(B, 10, generator=gen).cuda()
     cam = (torch.randn(B, 3, generator=gen) * torch.tensor([3.0, 0.2, 0.2])).cuda()
     cam[0, 0] = 25.0                                       # past softplus' threshold

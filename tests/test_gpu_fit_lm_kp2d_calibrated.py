@@ -12,8 +12,9 @@ import pytest
 import torch
 
 import kp2d_calibrated_lm_oracle as oc
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
-from test_gpu_fit_lm_keypoints_2d import _bits, _get, _rodrigues
 
 pytestmark = pytest.mark.gpu
 
@@ -49,9 +50,9 @@ def _step_case(n_rot, nb, K, terms, meas):
     B = sum(VIEWS)
     gen = torch.Generator().manual_seed(3000 * n_rot + 10 * nb + K + (3 if pw else 0) + (7 if meas else 0))
     rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(G, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(G, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(G, n_rot, 3).double() * 0.1)).float()
+    rot = rodrigues(rn(G, n_rot, 3).double() * 0.5).float()
+    trot = (rot.double() @ rodrigues(rn(G, n_rot, 3).double() * 0.05)).float()
+    anchor = (rot.double() @ rodrigues(rn(G, n_rot, 3).double() * 0.1)).float()
     betas = rn(G, nb)
     tr = 0.2 * rn(G, 3)
     tbetas, ttr = betas + 0.05 * rn(G, nb), tr + 0.02 * rn(G, 3)
@@ -165,27 +166,18 @@ def test_step_kernel_vs_oracle(n_rot, nb, K, first, terms, meas):
     state, trial = _device(c)
     m = c['meas']
     _step(c, state, trial, first, None if m is None else tuple(m[k].cuda() for k in ('mt', 'mw', 'tm', 'tmj')))
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
+    oracle = []
     for g in range(G):
         tr = {'rot': n(c['trot'][g]), 'betas': n(c['tbetas'][g]), 'transl': n(c['ttr'][g])}
         kw = {} if m is None else dict(meas=(n(m['mt'][g]), n(m['mw'][g])), trial_meas=(n(m['tm'][g]), n(m['tmj'][g])))
-        new, want, acc = oc.lm_keypoints_2d_calibrated_step(s_np[g], _views(c, g), 10.0, 3.0, first, tr, n(c['tkp'][g]),
-                                                            n(c['tjac'][g]), sigma=c['sigma'], anchor=n(c['anchor'][g]),
-                                                            pose_w=c['pw'], betas_w=c['bw'], **kw)
-        flags.append(acc)
-        assert got['accepted'][g] == new['accepted'], g
-        assert np.isclose(got['lambda'][g], new['lambda'], rtol=3e-7, atol=0), (g, got['lambda'][g], new['lambda'])
-        assert np.isclose(got['loss'][g], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (g, got['loss'][g],
-                                                                                          new['loss'])
-        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac') + (() if m is None else ('meas', 'meas_jac')):
-            assert np.array_equal(got[k][g], new[k], equal_nan=True), (g, k)
-        for k in ('rot', 'betas', 'transl'):
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][g] - want[k]).max()
-            assert err <= bar, (g, k, err)
-            worst = max(worst, err / bar)
+        oracle.append(oc.lm_keypoints_2d_calibrated_step(s_np[g], _views(c, g), 10.0, 3.0, first, tr, n(c['tkp'][g]),
+                                                         n(c['tjac'][g]), sigma=c['sigma'], anchor=n(c['anchor'][g]),
+                                                         pose_w=c['pw'], betas_w=c['bw'], **kw))
+    got, nxt = harness.numpy_of(state), harness.numpy_of(trial)
+    keys = ('rot', 'betas', 'transl')
+    flags, worst = harness.check_step(harness.rows_of(got, G), harness.rows_of(nxt, G), oracle,
+                                      keys + ('keypoints', 'jac') + (() if m is None else ('meas', 'meas_jac')), keys,
+                                      exact=False)
     if first:
         assert all(flags)
         assert math.isnan(got['loss'][3]) and np.array_equal(nxt['transl'][3], c['ttr'][3].numpy())   # does not move
@@ -210,7 +202,7 @@ def test_measurement_entry_with_dropped_measurements_is_the_plain_step(first):
         for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
             assert torch.equal(s1[k].view(torch.int32), s2[k].view(torch.int32)), k
         for k in t1:
-            assert torch.equal(_bits(t1[k]), _bits(t2[k])), k
+            assert torch.equal(bits(t1[k]), bits(t2[k])), k
 
 
 def test_argument_offset_and_workspace_errors_and_the_empty_batch():
@@ -326,12 +318,10 @@ def _fit(module, p, **kw):
 
 
 def test_lm_launches_no_synchronisation_and_monotone_losses():
-    from shapy_b200 import _lib
     from shapy_b200.body_measurements import BodyMeasurements
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 8, seed=72)
     bm = BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda()
-    L = _lib.lib()
     for meas, per_it in ((None, 2), ({'height': 1.7}, 4)):
         kw = dict(method='lm', robust_sigma=10.0, pose_prior_weight=100.0, body_measurements=bm if meas else None,
                   measurements=meas)
@@ -339,14 +329,8 @@ def test_lm_launches_no_synchronisation_and_monotone_losses():
         for init in (p['init'], {}):                          # and the default start
             counts = []
             for its in (3, 4):
-                torch.cuda.synchronize()
-                torch.cuda.set_sync_debug_mode('error')
-                try:
-                    n0 = L.shapy_launch_count()
-                    res = _fit(module, p, iterations=its, init=init, **kw)
-                    counts.append(L.shapy_launch_count() - n0)
-                finally:
-                    torch.cuda.set_sync_debug_mode(0)
+                n, res = harness.launches_without_sync(lambda: _fit(module, p, iterations=its, init=init, **kw))
+                counts.append(n)
             assert counts[1] - counts[0] == per_it, counts
         assert res['transl'].shape == (8, 3) and res['proj_joints'].shape == p['x'].shape
     # the kernel's loss never rises: the fit's state, iteration by iteration, through the returned loss of longer runs
@@ -360,25 +344,25 @@ def test_lm_launches_no_synchronisation_and_monotone_losses():
 
 
 def test_lm_deterministic_and_batch_independent():
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 16, seed=73)
     kw = dict(method='lm', iterations=12, robust_sigma=10.0, pose_prior_weight=100.0)
     r1, r2 = _fit(module, p, **kw), _fit(module, p, **kw)
     for k in r1:
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
     g, V = 5, p['V']
     rows = torch.arange(g * V, (g + 1) * V)
     q = dict(p, x=p['x'][rows], R=p['R'][rows], T=p['T'][rows], groups=None,
              init={k: v[g:g + 1] for k, v in p['init'].items()})
     one = _fit(module, q, **kw)
     for k in ('global_rot', 'body_pose', 'betas', 'transl'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][g:g + 1])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][g:g + 1])), k
     # the returned loss is recomputed by torch, whose reductions may round differently at another batch size
     assert torch.allclose(one['loss'], r1['loss'][g:g + 1], rtol=1e-6, atol=0)
 
 
 def test_start_behind_one_camera_reports_inf_and_does_not_move():
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 4, seed=74)
     init = {k: v.clone() for k, v in p['init'].items()}
     # body 1's root 4 m behind view 0 of its rig (its camera sits 3 m in front of the root): behind that camera only
@@ -386,10 +370,10 @@ def test_start_behind_one_camera_reports_inf_and_does_not_move():
     init['transl'][1] += 2.0 * (c - p['init']['transl'][1])
     res = _fit(module, p, init=init, method='lm', iterations=5)
     assert res['loss'][1] == float('inf') and torch.isfinite(res['loss'][[0, 2, 3]]).all()
-    assert torch.equal(_bits(res['transl'][1]), _bits(init['transl'][1]))
+    assert torch.equal(bits(res['transl'][1]), bits(init['transl'][1]))
     ref = _fit(module, p, method='lm', iterations=5)
     for k in ('transl', 'betas', 'loss'):
-        assert torch.equal(_bits(res[k][[0, 2, 3]]), _bits(ref[k][[0, 2, 3]])), k
+        assert torch.equal(bits(res[k][[0, 2, 3]]), bits(ref[k][[0, 2, 3]])), k
     # a view whose focal length is not finite and > 0 breaks the same rule: body 2 (views 8 .. 11) reports +inf from
     # the kernel's state (NaN) and from the host's recomputation alike, and does not move
     for bad in (0.0, -1000.0, float('nan'), float('inf')):
@@ -397,16 +381,16 @@ def test_start_behind_one_camera_reports_inf_and_does_not_move():
         f[9] = bad
         res = _fit(module, p, method='lm', iterations=5, focal_length=f)
         assert res['loss'][2] == float('inf'), bad
-        assert torch.equal(_bits(res['transl'][2]), _bits(p['init']['transl'][2])), bad
+        assert torch.equal(bits(res['transl'][2]), bits(p['init']['transl'][2])), bad
         for k in ('transl', 'betas', 'loss'):
-            assert torch.equal(_bits(res[k][[0, 1, 3]]), _bits(ref[k][[0, 1, 3]])), (bad, k)
+            assert torch.equal(bits(res[k][[0, 1, 3]]), bits(ref[k][[0, 1, 3]])), (bad, k)
 
 
 def test_equivariance_under_a_rigid_move_of_the_world():
     """Moving the world by X' = Q X + s, with every camera moved to match (R' = R Q^T, T' = T - R Q^T s) and the start
     mapped by calibrated_start from view 0's camera frame, moves the fit's result to match."""
     from shapy_b200.fit import calibrated_start
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 8, seed=75)
     # the 22 body joints: SMPL-X picks its dynamic face-contour landmarks by the head's global rotation, so they do not
     # move rigidly with the world
@@ -422,7 +406,7 @@ def test_equivariance_under_a_rigid_move_of_the_world():
     j0 = _root_joint(module, p['init']['betas'])
     Rc = R0 @ rot0[:, 0]
     tc = (R0 @ (j0 + p['init']['transl'])[..., None])[..., 0] + T0 - j0
-    Q = _rodrigues(torch.tensor([[0.3, -1.1, 0.5]], dtype=torch.float64))[0].float().cuda()
+    Q = rodrigues(torch.tensor([[0.3, -1.1, 0.5]], dtype=torch.float64))[0].float().cuda()
     s = torch.tensor([0.7, -0.2, 1.5], device='cuda')
     out = {}
     for name, (R, T) in {'world': (p['R'], p['T']), 'moved': (p['R'] @ Q.T, p['T'] - (p['R'] @ Q.T @ s))}.items():
@@ -442,7 +426,7 @@ def test_equivariance_under_a_rigid_move_of_the_world():
 
 
 def test_adam_lowers_the_loss():
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 8, seed=76)
     r0 = _fit(module, p, method='adam', iterations=0)
     r = _fit(module, p, method='adam', iterations=150, lr=0.01)
@@ -453,7 +437,7 @@ def test_adam_lowers_the_loss():
 
 def test_cli_on_a_written_npz(tmp_path):
     from shapy_b200 import fit
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 3, seed=77)
     n = lambda t: t.detach().cpu().numpy()  # noqa: E731
     from shapy_b200.human_shape.models.body_models.body_models import SMPLX
@@ -568,7 +552,7 @@ def _quality(module, p, which):
 
 @pytest.mark.parametrize('views', ['4_views', 'front_side'])
 def test_fit_quality_calibrated_vs_shared_pose_and_per_view(views):
-    module = _get()
+    module = harness.smplx_module()
     p = _rig(module, 64, views=(0.0, 90.0, 180.0, 270.0) if views == '4_views' else (0.0, 90.0))
     out = {which: _quality(module, p, which) for which in ('body', 'all')}
     print(f'fit_kp2d_calibrated_lm_64x{views}', out)

@@ -1,10 +1,9 @@
 """GPU: the whole-body 2D fit.  The expression-aware keypoint Jacobian (shapy_smplx_keypoint_jacobian_expr) against
 the 22-joint launch at psi = 0, the float64 restatement and the forward, on every model shape; the wide LM step
-(shapy_fit_lm_keypoints_2d_expressive_step and its perspective entry) against tests/kp2d_lm_oracle.py at
-P = 7 to 200, bit for bit against today's 2D steps at n_rot = 22 without expression over a 50-iteration loop, its
-argument errors; and fit_body_to_keypoints_2d(pose_width=55, fit_expression=True) end to end: launches, no host
-synchronisation, monotone losses, determinism, batch independence, Adam, the command line and quality."""
-import math
+(shapy_fit_lm_keypoints_2d_expressive_step and its perspective entry) against tests/kp2d_lm_oracle.py at P = 7 to 200,
+bit for bit against today's 2D steps at n_rot = 22 without expression over a 50-iteration loop, its argument errors;
+and fit_body_to_keypoints_2d(pose_width=55, fit_expression=True) end to end: launches, no host synchronisation,
+monotone losses, determinism, batch independence, Adam, the command line and quality."""
 import time
 
 import numpy as np
@@ -13,14 +12,13 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp_lm_oracle
+import lm_harness as harness
+from lm_harness import TOL, VARIANTS, bits, variant_model
 from shapy_b200 import synth
-from test_gpu_fit_lm_keypoints_2d import _bits, _rodrigues
-from test_gpu_model_shapes import TOL, _inputs
-from test_model_shapes_cpu import VARIANTS, variant_model
 
 pytestmark = pytest.mark.gpu
 
-F, PP = 1000.0, (500.0, 500.0)
+F, PP = harness.F, harness.PP
 
 
 # ------------------------------------------------------------------------------------------------ Jacobian
@@ -41,7 +39,7 @@ def test_jacobian_expr(name, n_rot):
     m, pk = variant_model(name), _packed(name)
     NB, NE, _ = VARIANTS[name]
     B = 3
-    x = _inputs(500 * NB + n_rot, B, n_rot, NB, NE)
+    x = harness.inputs(500 * NB + n_rot, B, n_rot, NB, NE)
     betas, rot, transl = x['betas'].cuda(), x['rot'].cuda(), x['transl'].cuda()
     expr = x['expression'].cuda()
     # psi = 0: the keypoints and every shared column are the 22-joint launch's bits
@@ -49,9 +47,9 @@ def test_jacobian_expr(name, n_rot):
     kpz, jacz = ops.smplx_keypoint_jacobian(pk, betas, rot, transl, expr=torch.zeros_like(expr))
     P0 = 3 * n_rot + NB
     assert jacz.shape == (B, 3 * pk.K, P0 + NE + 3)
-    assert torch.equal(_bits(kp0), _bits(kpz))
-    assert torch.equal(_bits(jac0[..., :P0]), _bits(jacz[..., :P0]))
-    assert torch.equal(_bits(jac0[..., P0:]), _bits(jacz[..., P0 + NE:]))
+    assert torch.equal(bits(kp0), bits(kpz))
+    assert torch.equal(bits(jac0[..., :P0]), bits(jacz[..., :P0]))
+    assert torch.equal(bits(jac0[..., P0:]), bits(jacz[..., P0 + NE:]))
     # psi != 0: every column against the float64 restatement, the keypoints against the forward
     kp, jac = ops.smplx_keypoint_jacobian(pk, betas, rot, transl, expr=expr)
     out = ops.smplx_forward(pk, betas, rot, expr=expr, want_vertices=True, want_v_shaped=False, want_joints=True)
@@ -86,151 +84,18 @@ def test_jacobian_expr_needs_an_expression_basis():
 STEP_SHAPES = [(1, 1, 0), (22, 10, 0), (22, 10, 10), (27, 6, 6), (27, 7, 6), (55, 10, 10), (55, 27, 5),
                (55, 16, 16)]
 STEP_K = [9, 127]
-# (robust_sigma, pose_prior_weight ('joint': per-joint weights), betas_weight, expression_weight)
-TERMS = [(math.inf, 0.0, 0.0, 0.0), (0.3, 'joint', 1.0, 0.5), (0.3, 2.0, 0.1, 0.0)]
-
-
-def _case(n_rot, nb, ne, K, terms, persp):
-    """Seven bodies with random Jacobians: body 0's trial hits its targets (accepted), body 1's state does and its
-    trial is far (rejected), body 2 has a weighted NaN trial keypoint (rejected), 3 to 6 random (perspective: body 3's
-    trial has a keypoint behind the camera).  Keypoint 7 has weight 0 and NaN targets, keypoints and rows."""
-    sigma, pw, bw, ew = terms
-    B, P = 7, 3 * n_rot + nb + ne + 3
-    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + ne + K + 7 * persp)
-    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
-    betas, expr = rn(B, nb), rn(B, ne)
-    if persp:
-        last = torch.cat([0.3 * rn(B, 2), 3.0 + torch.rand(B, 1, generator=gen)], 1)
-        tlast = last + 0.02 * rn(B, 3)
-        intr = torch.tensor([F, *PP]).repeat(B, 1)
-    else:
-        last = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
-        tlast = last + 0.02 * rn(B, 3)
-        intr = None
-    tbetas, texpr = betas + 0.05 * rn(B, nb), expr + 0.05 * rn(B, ne)
-    anchor[0], tbetas[0] = trot[0], 0.9 * betas[0]
-    anchor[1], tbetas[1] = rot[1], 1.1 * betas[1]
-    kp, jac = 0.4 * rn(B, K, 3), 0.3 * rn(B, 3 * K, P)
-    tkp, tjac = kp + 0.01 * rn(B, K, 3), jac + 0.03 * rn(B, 3 * K, P)
-    kp[0] = tkp[0] + 0.1
-    tkp[1] = kp[1] + 0.1
-
-    def proj(k, c, b):
-        if persp:
-            return torch.from_numpy(o2.project(k.numpy(), c.numpy(), intr[b].numpy())).float()
-        return torch.from_numpy(o2.project(k.numpy(), c.numpy())).float()
-    noise = 5.0 if persp else 0.02
-    tg = torch.stack([proj(kp[b], last[b], b) for b in range(B)]) + noise * rn(B, K, 2)
-    tg[0], tg[1] = proj(tkp[0], tlast[0], 0), proj(kp[1], last[1], 1)
-    tkp[2, 0, 1] = float('nan')
-    if persp:
-        tkp[3, 0, 2] = -tlast[3, 2] - 0.5
-    w = torch.rand(B, K, generator=gen) + 0.5
-    w[:, 7] = 0.0
-    tg[:, 7] = float('nan')
-    for t in (kp, tkp):
-        t[:, 7] = float('nan')
-    for t in (jac, tjac):
-        t[:, 21:24] = float('nan')
-    jw = None
-    if pw == 'joint':
-        jw = torch.rand(n_rot, generator=gen) * 3.0
-        jw[0] = 0.0
-        if n_rot > 3:
-            jw[2] = 0.0
-        pw = 0.0
-    if persp and math.isfinite(sigma):
-        sigma = sigma * 100.0
-    return dict(rot=rot, betas=betas, expr=expr, last=last, kp=kp, jac=jac, trot=trot, tbetas=tbetas, texpr=texpr,
-                tlast=tlast, tkp=tkp, tjac=tjac, tg=tg, w=w, intr=intr, anchor=anchor, jw=jw,
-                lam=torch.rand(B, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw, ew=ew)
-
-
-def _lastkey(c):
-    return 'camera' if c['intr'] is None else 'transl'
-
-
-def _kw(c, b):
-    n = lambda t: None if t is None else t.numpy()  # noqa: E731
-    return dict(sigma=c['sigma'], anchor=n(c['anchor'][b]), pose_w=c['pw'], joint_w=n(c['jw']), betas_w=c['bw'],
-                expr_w=c['ew'], intr=None if c['intr'] is None else n(c['intr'][b]))
-
-
-def _state_np(c, b):
-    n = lambda t: t.numpy()  # noqa: E731
-    s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'expression': n(c['expr'][b]), _lastkey(c): n(c['last'][b]),
-         'keypoints': n(c['kp'][b]), 'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-    kw = _kw(c, b)
-    s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s[_lastkey(c)], kw['sigma'], s['rot'],
-                                   kw['anchor'], kw['pose_w'], s['betas'], kw['betas_w'], kw['intr'], kw['joint_w'],
-                                   s['expression'], kw['expr_w']))
-    return s
-
-
-def _device(c):
-    B = c['rot'].shape[0]
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    lk = _lastkey(c)
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'expression': cu(c['expr']), lk: cu(c['last']),
-             'keypoints': cu(c['kp']), 'jac': cu(c['jac']),
-             'loss': cu(torch.tensor(np.array([_state_np(c, b)['loss'] for b in range(B)]))),
-             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'expression': cu(c['texpr']), lk: cu(c['tlast'])}
-    return state, trial
-
-
-def _step(c, state, trial, first):
-    from shapy_b200 import ops
-    cu = lambda t: None if t is None else t.cuda().contiguous()  # noqa: E731
-    ops.fit_lm_keypoints_2d_expressive_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'],
-                                            c['ew'], 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']),
-                                            pose_anchor=cu(c['anchor']), joint_weights=cu(c['jw']),
-                                            intrinsics=cu(c['intr']))
 
 
 @pytest.mark.parametrize('persp', [False, True], ids=['weak', 'persp'])
-@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_joint_priors', 'robust_scalar_prior'])
+@pytest.mark.parametrize('terms', range(3), ids=['lsq', 'robust_joint_priors', 'robust_scalar_prior'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('K', STEP_K)
 @pytest.mark.parametrize('n_rot,nb,ne', STEP_SHAPES)
 def test_step_kernel_vs_oracle(n_rot, nb, ne, K, first, terms, persp):
-    c = _case(n_rot, nb, ne, K, terms, persp)
-    B = c['rot'].shape[0]
-    lk = _lastkey(c)
-    n = lambda t: t.numpy()  # noqa: E731
-    s_np = [_state_np(c, b) for b in range(B)]
-    state, trial = _device(c)
-    _step(c, state, trial, first)
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
-    for b in range(B):
-        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'expression': n(c['texpr'][b]), lk: n(c['tlast'][b])}
-        new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                 n(c['tkp'][b]), n(c['tjac'][b]), **_kw(c, b))
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        assert got['lambda'][b] == new['lambda'] or np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), \
-            (b, got['lambda'][b], new['lambda'])
-        assert np.isclose(got['loss'][b], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (b, got['loss'][b],
-                                                                                          new['loss'])
-        for k in ('rot', 'betas', 'expression', lk, 'keypoints', 'jac'):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'expression', lk):
-            if want[k].size == 0:
-                continue
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= bar, (b, k, err)
-            worst = max(worst, err / bar)
-    if first:
-        assert all(flags)
-    else:
-        assert flags[:3] == [True, False, False], flags
-    print(f'[expressive] step P={3 * n_rot + nb + ne + 3} K={K} first={first} terms={terms} persp={persp}: trial '
+    """The wide step on lm_harness.kp2d_case with ne expression columns; terms indexes lm_harness.EXPR_TERMS."""
+    t = harness.EXPR_TERMS['persp' if persp else 'weak'][terms]
+    worst = harness.kp2d_run(first, n_rot=n_rot, nb=nb, K=K, terms=t, persp=persp, ne=ne)
+    print(f'[expressive] step P={3 * n_rot + nb + ne + 3} K={K} first={first} terms={t} persp={persp}: trial '
           f'error / bar {worst:.3f}')
 
 
@@ -289,16 +154,6 @@ def test_step_errors():
 
 
 # ------------------------------------------------------------------------------------------------ fits
-_MODULE = {}
-
-
-def _module():
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    if 'm' not in _MODULE:
-        _MODULE['m'] = SMPLX(data_struct=dict(synth.make_smplx()), use_face_contour=True).cuda()
-    return _MODULE['m']
-
-
 def _problem(module, B, seed=41, persp=False):
     """The 2D recipe's ground truth (betas, raw body pose, camera or translation) plus hands (raw 6D = identity + 0.3
     N), jaw (identity + 0.2 N) and psi ~ N(0, 1); targets the exact projections of every keypoint; the start the
@@ -373,7 +228,7 @@ def test_equals_todays_step_over_50_iterations(persp):
     over a 50-iteration loop: state, loss, lambda and accepted count."""
     from shapy_b200 import ops
     from shapy_b200.fit import LM_DOWN, LM_UP
-    module = _module()
+    module = harness.smplx_module()
     B = 48
     x, init, _ = _problem(module, B, seed=5, persp=persp)
     x = x.contiguous()
@@ -412,13 +267,13 @@ def test_equals_todays_step_over_50_iterations(persp):
     for k in ('rot', 'betas', lk, 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
         assert torch.equal(s0[k].view(torch.int32), s1[k].view(torch.int32)), k
     for k in ('rot', 'betas', lk):
-        assert torch.equal(_bits(t0[k]), _bits(t1[k])), k
+        assert torch.equal(bits(t0[k]), bits(t1[k])), k
     assert int(s1['accepted'].sum()) > B
 
 
 @pytest.mark.parametrize('persp', [False, True], ids=['weak', 'persp'])
 def test_wide_loop_monotone_deterministic_and_batch_independent(persp):
-    module = _module()
+    module = harness.smplx_module()
     B = 24
     x, init, _ = _problem(module, B, seed=9, persp=persp)
     w = torch.ones(B, x.shape[1], device='cuda')
@@ -427,33 +282,26 @@ def test_wide_loop_monotone_deterministic_and_batch_independent(persp):
     assert bool((d <= 0).all()), float(d.max())
     assert float(losses[-1].mean()) < float(losses[0].mean())
     again, st2 = _wide_loop(module, x, w, init, 12, persp)
-    assert torch.equal(_bits(losses), _bits(again))
+    assert torch.equal(bits(losses), bits(again))
     idx = torch.tensor([3, 17, 5], device='cuda')
     sub, st3 = _wide_loop(module, x[idx].contiguous(), w[idx].contiguous(), {k: v[idx] for k, v in init.items()}, 12,
                           persp)
-    assert torch.equal(_bits(losses[:, idx]), _bits(sub))
+    assert torch.equal(bits(losses[:, idx]), bits(sub))
     for k in ('rot', 'betas', 'expression'):
-        assert torch.equal(_bits(st[k]), _bits(st2[k]))
-        assert torch.equal(_bits(st[k][idx]), _bits(st3[k]))
+        assert torch.equal(bits(st[k]), bits(st2[k]))
+        assert torch.equal(bits(st[k][idx]), bits(st3[k]))
 
 
 def test_lm_fit_launches_and_never_synchronises():
-    from shapy_b200 import _lib
-    module = _module()
+    module = harness.smplx_module()
     B = 16
     x, init, _ = _problem(module, B, seed=3)
     kw = dict(pose_width=55, fit_expression=True, robust_sigma=0.1, pose_prior_weight=1.0, expression_weight=0.01)
     _fit(module, x, init, iterations=1, **kw)
-    torch.cuda.synchronize()
     counts = []
     for it in (3, 5):
-        n0 = _lib.lib().shapy_launch_count()
-        torch.cuda.set_sync_debug_mode('error')
-        try:
-            res = _fit(module, x, init, iterations=it, **kw)
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-        counts.append(_lib.lib().shapy_launch_count() - n0)
+        n, res = harness.launches_without_sync(lambda: _fit(module, x, init, iterations=it, **kw))
+        counts.append(n)
     assert counts[1] - counts[0] == 2 * 2, counts          # two launches per iteration
     assert res['full_pose_mat'].shape == (B, 55, 3, 3) and res['expression'].shape == (B, 10)
     assert res['left_hand_pose'].shape == (B, 90) and res['jaw_pose'].shape == (B, 6)
@@ -461,7 +309,7 @@ def test_lm_fit_launches_and_never_synchronises():
 
 
 def test_fit_arguments():
-    module = _module()
+    module = harness.smplx_module()
     x, init, _ = _problem(module, 2, seed=1)
     with pytest.raises(ValueError):
         _fit(module, x, init, pose_width=30)
@@ -480,7 +328,7 @@ def test_fit_arguments():
 def test_adam_loss_matches_the_oracle():
     """Adam's returned loss at its final parameters equals the step oracle's loss there (float64, per body)."""
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _module()
+    module = harness.smplx_module()
     B = 4
     x, init, _ = _problem(module, B, seed=13)
     jw = np.zeros(55)
@@ -534,7 +382,7 @@ def _quality(module, x, init, truth, persp, **kw):
 def test_quality_whole_body():
     """256 synthetic bodies with hands, jaw and expression, exact targets: today's 22-joint fit on all keypoints (a),
     on the body keypoints alone (b), the whole-body fit (c) and (c) under the perspective camera (d)."""
-    module = _module()
+    module = harness.smplx_module()
     B = 256
     x, init, truth = _problem(module, B, seed=77)
     xp, initp, truthp = _problem(module, B, seed=77, persp=True)

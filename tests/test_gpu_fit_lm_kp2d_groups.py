@@ -10,14 +10,18 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
-import kp2dg_lm_oracle as og
-from oracle.lm_oracle import meas_loss
-from test_gpu_fit_lm_kp2d_meas import NAMES, N_ROT, _bits, _measure, _rodrigues, model  # noqa: F401
-from test_gpu_fit_lm_kp2d_meas import quality as quality_2d
+import lm_harness as harness
+from lm_harness import (NAMES, N_ROT, bits, check_dropped_measurements, check_groups_of_one, groups_device, groups_step,
+                        rodrigues)
 
 pytestmark = pytest.mark.gpu
 TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
 SIZES = (1, 2, 3, 5)
+
+
+@pytest.fixture(scope='module')
+def model():
+    return harness.smplx_and_measurements()
 
 
 # ------------------------------------------------------------------------------------------------ step
@@ -40,11 +44,11 @@ def _group_case(model, terms, exact=False, sizes=SIZES, seed=43):
     gidx = torch.repeat_interleave(torch.arange(G), torch.tensor(sizes))
     gen = torch.Generator().manual_seed(seed)
     rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
+    rot = rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
     betas = rn(G, 10).clamp(-2, 2)
     cam = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
-    trot = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.02)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.05)).float()
+    trot = (rot.double() @ rodrigues(rn(B, N_ROT, 3).double() * 0.02)).float()
+    anchor = (rot.double() @ rodrigues(rn(B, N_ROT, 3).double() * 0.05)).float()
     tbetas, tcam = betas + 0.05 * rn(G, 10), cam + 0.01 * rn(B, 3)
     for g in (0, 2):
         tbetas[g] = 0.9 * betas[g]
@@ -84,110 +88,16 @@ def _group_case(model, terms, exact=False, sizes=SIZES, seed=43):
                 anchor=anchor, lam=torch.rand(G, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
 
 
-def _state_loss(c, g, with_meas):
-    n = lambda t: t.numpy()  # noqa: E731
-    L = 0.0
-    for i in range(c['off'][g], c['off'][g + 1]):
-        L += o2.loss(n(c['tg'][i]), n(c['w'][i]), n(c['kp'][i]), n(c['cam'][i]), c['sigma'], n(c['rot'][i]),
-                     n(c['anchor'][i]), c['pw'])
-    if with_meas:
-        L += meas_loss(n(c['mt'][g]), n(c['mw'][g]), n(c['meas'][g]))
-    if c['bw'] > 0:
-        L += float(np.float32(c['bw'])) * float(np.sum(n(c['betas'][g]).astype(np.float64) ** 2))
-    return L
-
-
-def _device(c, with_meas):
-    G = len(c['off']) - 1
-    B = c['rot'].shape[0]
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    loss = torch.tensor([_state_loss(c, g, with_meas) for g in range(G)]).float()
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'camera': cu(c['cam']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(loss), 'lambda': cu(c['lam']),
-             'accepted': torch.zeros(G, dtype=torch.int32, device='cuda')}
-    if with_meas:
-        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'image_betas': cu(c['tbetas'][c['gidx']]),
-             'camera': cu(c['tcam'])}
-    return state, trial, B, G
-
-
-def _groups_step(c, state, trial, first, with_meas, ws=None):
-    """One grouped step on the case at its n_rot and nb; ws: the workspace (by default a fresh one)."""
-    from shapy_b200 import ops
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    B, G = c['rot'].shape[0], len(c['off']) - 1
-    if ws is None:
-        ws = ops.fit_lm_groups_workspace(B, G, c['rot'].shape[1], c['betas'].shape[1], 'cuda')
-    off = torch.from_numpy(c['off'])
-    if with_meas:
-        ops.fit_lm_keypoints_2d_groups_measurements_step(
-            state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], cu(c['mt']), cu(c['mw']), 10.0, 3.0,
-            first, cu(c['tkp']), cu(c['tjac']), cu(c['tmeas']), cu(c['tmjac']), off, ws, pose_anchor=cu(c['anchor']))
-    else:
-        ops.fit_lm_keypoints_2d_groups_step(state, trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0,
-                                            3.0, first, cu(c['tkp']), cu(c['tjac']), off, ws,
-                                            pose_anchor=cu(c['anchor']))
-
-
-def _check_vs_oracle(c, s0, state, trial, first, with_meas):
-    """The stepped device state and next trial against kp2dg_lm_oracle group by group, from the state s0 (NumPy) before
-    the step: loss and lambda to fp32 rounding, the state bit for bit, the next trial within 2e-6 max(1, |x|) and each
-    image's trial betas its group's.  Returns (the groups' accepted flags, the largest trial error over its bar)."""
-    G = len(c['off']) - 1
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    n = lambda t: t.numpy()  # noqa: E731
-    flags, worst = [], 0.0
-    for g in range(G):
-        r = range(c['off'][g], c['off'][g + 1])
-        st = {k: [s0[k2][i] for i in r] for k, k2 in (('rot', 'rot'), ('camera', 'camera'), ('keypoints', 'keypoints'),
-                                                        ('jac', 'jac'))}
-        st.update(betas=s0['betas'][g], loss=s0['loss'][g], accepted=0, **{'lambda': s0['lambda'][g]})
-        if with_meas:
-            st.update(meas=s0['meas'][g], meas_jac=s0['meas_jac'][g])
-        images = [{'targets': n(c['tg'][i]), 'weights': n(c['w'][i]), 'anchor': n(c['anchor'][i]),
-                   'trial_kp': n(c['tkp'][i]), 'trial_jac': n(c['tjac'][i])} for i in r]
-        tr = {'rot': [n(c['trot'][i]) for i in r], 'camera': [n(c['tcam'][i]) for i in r],
-              'betas': n(c['tbetas'][g])}
-        mb = None if not with_meas else {'targets': n(c['mt'][g]), 'weights': n(c['mw'][g]),
-                                         'trial_meas': n(c['tmeas'][g]), 'trial_meas_jac': n(c['tmjac'][g])}
-        new, want, acc, _, _ = og.lm_groups_step(st, images, 10.0, 3.0, first, tr, c['sigma'], c['pw'], c['bw'], mb)
-        flags.append(acc)
-        assert got['accepted'][g] == new['accepted'], g
-        assert np.isclose(got['lambda'][g], new['lambda'], rtol=3e-7, atol=0), (g, got['lambda'][g], new['lambda'])
-        assert np.isclose(got['loss'][g], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (g, got['loss'][g],
-                                                                                          new['loss'])
-        assert np.array_equal(got['betas'][g], new['betas'], equal_nan=True), g
-        if with_meas:
-            for k in ('meas', 'meas_jac'):
-                assert np.array_equal(got[k][g], new[k], equal_nan=True), (g, k)
-        for j, i in enumerate(r):
-            for k in ('rot', 'camera', 'keypoints', 'jac'):
-                assert np.array_equal(got[k][i], new[k][j], equal_nan=True), (g, i, k)
-            for k in ('rot', 'camera'):
-                bar = 2e-6 * max(1.0, np.abs(want[k][j]).max())
-                err = np.abs(nxt[k][i] - want[k][j]).max()
-                assert err <= bar, (g, i, k, err)
-                worst = max(worst, err / bar)
-            assert np.array_equal(nxt['image_betas'][i], nxt['betas'][g])
-        bar = 2e-6 * max(1.0, np.abs(want['betas']).max())
-        err = np.abs(nxt['betas'][g] - want['betas']).max()
-        assert err <= bar, (g, 'betas', err)
-        worst = max(worst, err / bar)
-    return flags, worst
-
-
 @pytest.mark.parametrize('meas', [None, 'reference', 'exact'])
 @pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 def test_step_kernels_vs_oracle(model, first, terms, meas):
     c = _group_case(model, terms, exact=meas == 'exact')
     with_meas = meas is not None
-    state, trial, B, G = _device(c, with_meas)
-    s0 = {k: v.cpu().numpy() for k, v in state.items()}
-    _groups_step(c, state, trial, first, with_meas)
-    flags, worst = _check_vs_oracle(c, s0, state, trial, first, with_meas)
+    state, trial, B, G = groups_device(c, with_meas)
+    s0 = harness.numpy_of(state)
+    groups_step(c, state, trial, first, with_meas)
+    flags, worst = harness.check_groups_vs_oracle(c, s0, state, trial, first, with_meas)
     if first:
         assert all(flags)
     else:
@@ -201,47 +111,12 @@ def test_groups_of_one_equal_the_2d_step(model, first, terms):
     """Eight groups of one: loss, lambda, accepted and the state bit for bit as shapy_fit_lm_keypoints_2d_step; the
     next trial within 4e-6 max(1, |x|) (the CPU oracle test bounds the two eliminations' fp64 difference by 1e-10; what
     is left is the fp32 rounding of the result)."""
-    _check_groups_of_one(_group_case(model, terms, sizes=(1,) * 8), first)
-
-
-def _check_groups_of_one(c, first):
-    """The grouped step on a case of groups of one against shapy_fit_lm_keypoints_2d_step on the same images."""
-    from shapy_b200 import ops
-    state, trial, B, G = _device(c, False)
-    b_state = {k: v.clone() for k, v in state.items()}
-    b_trial = {k: v.clone() for k, v in trial.items() if k != 'image_betas'}
-    _groups_step(c, state, trial, first, False)
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    ops.fit_lm_keypoints_2d_step(b_state, b_trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
-                                 first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
-    for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(state[k]), _bits(b_state[k])), k
-    for k in ('rot', 'betas', 'camera'):
-        err = (trial[k] - b_trial[k]).abs().max()
-        assert float(err) <= 4e-6 * max(1.0, float(b_trial[k].abs().max())), (k, float(err))
+    check_groups_of_one(_group_case(model, terms, sizes=(1,) * 8), first)
 
 
 @pytest.mark.parametrize('first', [False, True])
 def test_dropped_measurements_equal_the_plain_groups_step_bit_for_bit(model, first):
-    _check_dropped_measurements(_group_case(model, TERMS[1]), first)
-
-
-def _check_dropped_measurements(c, first):
-    """Every measurement of the case dropped (weight 0 or -1, NaN values and rows): the measurements entry equals the
-    plain grouped entry bit for bit."""
-    for k in ('meas', 'tmeas', 'mjac', 'tmjac'):
-        c[k][:] = float('nan')
-    c['mw'][:] = 0.0
-    c['mw'][:, 1] = -1.0
-    a_state, a_trial, _, _ = _device(c, True)
-    b_state = {k: v.clone() for k, v in a_state.items() if k not in ('meas', 'meas_jac')}
-    b_trial = {k: v.clone() for k, v in a_trial.items()}
-    _groups_step(c, a_state, a_trial, first, True)
-    _groups_step(c, b_state, b_trial, first, False)
-    for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
-    for k in ('rot', 'betas', 'image_betas', 'camera'):
-        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+    check_dropped_measurements(_group_case(model, TERMS[1]), first)
 
 
 def test_argument_errors_and_empty_batch(model):
@@ -321,7 +196,7 @@ def _problem(module, bm, n_id, views=4, seed=41):
     with torch.no_grad():
         rot = ops.decode_rot6d(raw.cuda())
         out = module(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=bstar[groups].cuda(), camera=cam.cuda())
-        tgt = _measure(module, bm, bstar.cuda())
+        tgt = harness.measure(module, bm, bstar.cuda())
     init = {'global_rot': (raw[:, :6] + 0.1 * rn(B, 6)).cuda(), 'body_pose': (raw[:, 6:] + 0.1 * rn(B, 126)).cuda(),
             'betas': (bstar[groups] + 0.5 * rn(B, module.num_betas)).cuda(), 'camera': (cam + 0.05 * rn(B, 3)).cuda()}
     return dict(x=out['proj_joints'].clone(), joints=out['joints'][:].clone(), init=init, bstar=bstar.cuda(), tgt=tgt,
@@ -389,12 +264,12 @@ def test_lm_losses_monotone_launch_count_and_returned_by_the_fit(model, with_mea
                                    pose_prior_weight=0.5, betas_weight=0.01, groups=p['groups'], **kw)
     assert res['betas'].shape == (16, 10) and res['loss'].shape == (16,) and res['camera'].shape == (64, 3)
     for k in ('betas', 'loss'):
-        assert torch.equal(_bits(res[k]), _bits(state[k])), k
+        assert torch.equal(bits(res[k]), bits(state[k])), k
     inv = torch.argsort(o)
-    assert torch.equal(_bits(res['camera']), _bits(state['camera'][inv]))
-    assert torch.equal(_bits(res['global_rot_mat']), _bits(state['rot'][inv][:, :1]))
+    assert torch.equal(bits(res['camera']), bits(state['camera'][inv]))
+    assert torch.equal(bits(res['global_rot_mat']), bits(state['rot'][inv][:, :1]))
     if with_meas:
-        assert torch.equal(_bits(res['measurements']), _bits(state['meas']))
+        assert torch.equal(bits(res['measurements']), bits(state['meas']))
 
 
 def test_lm_deterministic_and_group_independent(model):
@@ -406,16 +281,16 @@ def test_lm_deterministic_and_group_independent(model):
     r1 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
     r2 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
     for k in r1:
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
     rows = (p['groups'] == 5).nonzero()[:, 0]                          # identity 5 alone, as label 0
     one = fit_body_to_keypoints_2d(module, p['x'][rows].contiguous(),
                                    init={k: v[rows].contiguous() for k, v in p['init'].items()},
                                    measurements={k: v[5:6].contiguous() for k, v in meas.items()},
                                    groups=torch.zeros(len(rows), dtype=torch.int64), **kw)
     for k in ('betas', 'measurements', 'loss'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][5:6])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][5:6])), k
     for k in ('camera', 'global_rot', 'body_pose'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][rows])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][rows])), k
 
 
 def test_lm_loop_never_synchronises(model):
@@ -425,12 +300,7 @@ def test_lm_loop_never_synchronises(model):
     kw = dict(init=p['init'], method='lm', robust_sigma=0.1, pose_prior_weight=1.0, betas_weight=0.01,
               body_measurements=bm, measurements=p['tg'], groups=p['groups'].cpu())   # labels on the host: no read
     fit_body_to_keypoints_2d(module, p['x'], iterations=1, **kw)       # packs the model, builds the incidence table
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw))
     assert res['measurements'].shape == (8, 5)
 
 
@@ -455,16 +325,6 @@ def test_adam_fits_one_betas_per_group(model):
 # 0.17 / 0.61 (0.97 / 1.0), 2D RMS < 2e-3 1.0 / 1.0, joint error 0.128 / 0.108 m (0.125 / 0.101 m).
 BETA_BARS = {'all': {'grouped': 0.86, 'grouped_height_mass': 0.82},
              'body': {'grouped': 0.35, 'grouped_height_mass': 0.28}}
-def quality(module, bm, p, res, grouped):
-    q = quality_2d(module, bm, dict(p, tgt=p['tgt'][p['groups']], bstar=p['bstar'][p['groups']]),
-                   dict(res, betas=res['betas'][p['groups']],
-                        **({'measurements': res['measurements'][p['groups']]} if 'measurements' in res else {})),
-                   p.get('w'))
-    if grouped:                       # per identity, not per image
-        meas = res['measurements'] if 'measurements' in res else _measure(module, bm, res['betas'])
-        q['median_beta_err'] = float((res['betas'] - p['bstar']).norm(dim=1).median())
-        q['height_1mm'] = float(((meas[:, 1] - p['tgt'][:, 1]).abs() < 1e-3).float().mean())
-    return q
 
 
 @pytest.mark.parametrize('which', ['all', 'body'])
@@ -479,6 +339,7 @@ def test_fit_quality_64_identities_4_views(model, which):
     kw = dict(init=p['init'], method='lm', weights=w)
     gm = {k: p['tg'][k] for k in ('height', 'mass')}
     hm = dict(body_measurements=bm, measurements={k: v[p['groups']] for k, v in gm.items()})
+    quality = harness.quality_groups
     q = {'per_image': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], **kw), False),
          'grouped': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], groups=p['groups'], **kw), True),
          'per_image_height_mass': quality(module, bm, p, fit_body_to_keypoints_2d(module, p['x'], **hm, **kw), False),

@@ -10,36 +10,19 @@ import pytest
 import torch
 
 import kp2d_lm_oracle as o2
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
-NAMES = ('mass', 'height', 'chest', 'waist', 'hips')
-N_ROT = 22
+NAMES, N_ROT = harness.NAMES, harness.N_ROT
 # (robust_sigma, pose_prior_weight, betas_weight)
 TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _rodrigues(aa):
-    aa = aa.double()
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
-
-
 @pytest.fixture(scope='module')
 def model():
-    from shapy_b200.body_measurements import BodyMeasurements
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    return (SMPLX(data_struct=synth.make_smplx(), use_face_contour=True).cuda(),
-            BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda())
+    return harness.smplx_and_measurements()
 
 
 # ------------------------------------------------------------------------------------------------ step
@@ -63,11 +46,11 @@ def _step_case(model, terms, exact=False):
     B = 8
     gen = torch.Generator().manual_seed(41)                   # the rotations and betas of test_gpu_fit_lm_kp_meas.py
     rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
+    rot = rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
     betas = rn(B, 10).clamp(-2, 2)
     cam = torch.stack([1.0 + 0.2 * rn(B), 0.1 * rn(B), 0.1 * rn(B)], 1)
-    trot = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.02)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, N_ROT, 3).double() * 0.05)).float()
+    trot = (rot.double() @ rodrigues(rn(B, N_ROT, 3).double() * 0.02)).float()
+    anchor = (rot.double() @ rodrigues(rn(B, N_ROT, 3).double() * 0.05)).float()
     tbetas, tcam = betas + 0.05 * rn(B, 10), cam + 0.01 * rn(B, 3)
     for b in (0, 2):                                          # the priors favour the accepted trials ...
         anchor[b], tbetas[b] = trot[b], 0.9 * betas[b]
@@ -136,31 +119,21 @@ def test_step_kernel_vs_oracle(model, first, terms, derivative):
     state, trial = _state(c)
     s0 = {k: v.cpu().numpy() for k, v in state.items()}
     _meas_step(c, state, trial, first)
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
     n = lambda t: t.numpy()  # noqa: E731
-    flags, worst = [], 0.0
+    oracle = []
     for b in range(B):
         s = {k: s0[k][b] for k in s0}
         s['accepted'] = 0
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'camera': n(c['tcam'][b])}
-        new, want, acc = o2.lm_keypoints_2d_step(
+        oracle.append(o2.lm_keypoints_2d_step(
             s, n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]), sigma=c['sigma'],
             anchor=n(c['anchor'][b]), pose_w=c['pw'], betas_w=c['bw'], meas=(n(c['mt'][b]), n(c['mw'][b])),
-            trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])))
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        # softplus' exp / log1p may round differently on the device: loss and lambda to fp32 rounding
-        assert np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), (b, got['lambda'][b], new['lambda'])
-        assert np.isclose(got['loss'][b], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (b, got['loss'][b],
-                                                                                          new['loss'])
-        for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'meas', 'meas_jac'):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'camera'):
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= bar, (b, k, err)
-            worst = max(worst, err / bar)
+            trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b]))))
+    got = harness.numpy_of(state)
+    keys = ('rot', 'betas', 'camera')
+    # softplus' exp / log1p may round differently on the device: loss and lambda to fp32 rounding
+    flags, worst = harness.check_step(harness.rows_of(got, B), harness.rows_of(harness.numpy_of(trial), B), oracle,
+                                 keys + ('keypoints', 'jac', 'meas', 'meas_jac'), keys, exact=False)
     if first:
         assert all(flags) and np.isnan(got['loss'][3])
     else:
@@ -187,9 +160,9 @@ def test_dropped_measurements_equal_the_2d_step_bit_for_bit(model, first, terms)
     ops.fit_lm_keypoints_2d_step(b_state, b_trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
                                  first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['anchor']))
     for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(a_state[k]), bits(b_state[k])), k
     for k in ('rot', 'betas', 'camera'):
-        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+        assert torch.equal(bits(a_trial[k]), bits(b_trial[k])), k
     assert bool(torch.isfinite(a_state['loss']).all())
 
 
@@ -206,17 +179,11 @@ def _problem(module, bm, B, seed=41):
     with torch.no_grad():
         rot = ops.decode_rot6d(raw.cuda())
         out = module(global_rot=rot[:, :1], body_pose=rot[:, 1:], betas=bstar.cuda(), camera=cam.cuda())
-        tgt = _measure(module, bm, bstar.cuda())
+        tgt = harness.measure(module, bm, bstar.cuda())
     init = {'global_rot': (raw[:, :6] + 0.1 * rn(B, 6)).cuda(), 'body_pose': (raw[:, 6:] + 0.1 * rn(B, 126)).cuda(),
             'betas': (bstar + 0.5 * rn(B, module.num_betas)).cuda(), 'camera': (cam + 0.05 * rn(B, 3)).cuda()}
     return dict(x=out['proj_joints'].clone(), joints=out['joints'][:].clone(), init=init, bstar=bstar.cuda(), tgt=tgt,
                 tg={k: tgt[:, i].contiguous() for i, k in enumerate(NAMES)})
-
-
-def _measure(module, bm, betas):
-    with torch.no_grad():
-        m = bm.forward_vertices(module.forward_shape(betas=betas)['v_shaped'], module.faces_i32)['measurements']
-    return torch.stack([m[k]['tensor'] for k in NAMES], 1)
 
 
 def _lm_loop(module, bm, p, w, iterations, sigma=None, pw=0.0, bw=0.0, measurements=None, exact=False):
@@ -268,9 +235,9 @@ def test_fit_without_measurements_is_unchanged(model):
                                    pose_prior_weight=0.5, betas_weight=0.01, body_measurements=bm)
     assert 'measurements' not in res
     for k in ('betas', 'camera'):
-        assert torch.equal(_bits(res[k]), _bits(state[k])), k
-    assert torch.equal(_bits(res['global_rot_mat']), _bits(state['rot'][:, :1]))
-    assert torch.equal(_bits(res['body_pose_mat']), _bits(state['rot'][:, 1:]))
+        assert torch.equal(bits(res[k]), bits(state[k])), k
+    assert torch.equal(bits(res['global_rot_mat']), bits(state['rot'][:, :1]))
+    assert torch.equal(bits(res['body_pose_mat']), bits(state['rot'][:, 1:]))
 
 
 @pytest.mark.parametrize('derivative', ['reference', 'exact'])
@@ -297,10 +264,10 @@ def test_lm_losses_monotone_and_returned_by_the_fit(model, derivative):
                                    pose_prior_weight=0.5, betas_weight=0.01, body_measurements=bm, measurements=meas,
                                    circumference_derivative=derivative)
     for k in ('betas', 'camera'):
-        assert torch.equal(_bits(res[k]), _bits(state[k])), k
-    assert torch.equal(_bits(res['measurements']), _bits(state['meas']))
-    torch.testing.assert_close(res['measurements'][fin], _measure(module, bm, res['betas'])[fin], rtol=1e-6, atol=1e-7,
-                               equal_nan=True)
+        assert torch.equal(bits(res[k]), bits(state[k])), k
+    assert torch.equal(bits(res['measurements']), bits(state['meas']))
+    torch.testing.assert_close(res['measurements'][fin], harness.measure(module, bm, res['betas'])[fin], rtol=1e-6,
+                               atol=1e-7, equal_nan=True)
     # the returned loss comes from SMPLX.forward's proj_joints, the kernel's from the Jacobian launch's keypoints
     assert float(((res['loss'] - state['loss']).abs() / state['loss'])[fin].max()) <= 1e-2
 
@@ -318,14 +285,14 @@ def test_lm_deterministic_and_batch_independent(model):
                                   init={k: v[rows].contiguous() for k, v in p['init'].items()},
                                   measurements={k: v[rows].contiguous() for k, v in meas.items()}, **kw)
     for k in ('global_rot', 'body_pose', 'betas', 'camera', 'measurements', 'loss'):
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
         if k != 'loss':                   # the returned loss is summed by torch, whose reduction order follows the batch
-            assert torch.equal(_bits(r8[k]), _bits(r1[k][rows])), k
+            assert torch.equal(bits(r8[k]), bits(r1[k][rows])), k
     one = fit_body_to_keypoints_2d(module, p['x'][17:18].contiguous(),
                                    init={k: v[17:18].contiguous() for k, v in p['init'].items()},
                                    measurements={k: v[17:18].contiguous() for k, v in meas.items()}, **kw)
     for k in ('betas', 'camera', 'measurements'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][17:18])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][17:18])), k
 
 
 def test_lm_loop_never_synchronises(model):
@@ -335,12 +302,7 @@ def test_lm_loop_never_synchronises(model):
     kw = dict(init=p['init'], method='lm', robust_sigma=0.1, pose_prior_weight=1.0, betas_weight=0.01,
               body_measurements=bm, measurements=p['tg'])
     fit_body_to_keypoints_2d(module, p['x'], iterations=1, **kw)      # packs the model, builds the incidence table
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw))
     assert res['measurements'].shape == (32, 5)
 
 
@@ -430,28 +392,8 @@ def test_argument_errors_and_empty_batch(model):
 #     in the image from this start, with or without measurements, and those decide the shares;
 #   body joints: height 0.961 / 0.180, mass 0.961 / 0.938, 2D RMS 1.0 / 1.0, |beta - beta*| 0.95 / 1.10, joint error
 #     0.125 / 0.127 m: the height is what the keypoints cannot see; the joint error is depth and pose, not size.
-RMS_THRESHOLD = 2e-3
 QUALITY_BARS = {'all': {'height_1mm': 0.38, 'mass_1pct': 0.92, 'frac_rms2d': 0.27},
                 'body': {'height_1mm': 0.94, 'mass_1pct': 0.94, 'frac_rms2d': 0.98}}
-
-
-def quality(module, bm, p, res, w=None):
-    """Shares of the bodies with height within 1 mm, mass within 1 % and 2D RMS (crop frame) within RMS_THRESHOLD; the
-    median |beta - beta*| and root-aligned 3D joint error [m]."""
-    from shapy_b200.metrics import PointError, build_alignment
-    meas = res['measurements'] if 'measurements' in res else _measure(module, bm, res['betas'])
-    tgt = p['tgt']
-    ok = torch.isfinite(tgt).all(1) & torch.isfinite(meas).all(1)
-    d = (res['proj_joints'] - p['x']).pow(2).sum(-1)
-    rms = d.mean(1).sqrt() if w is None else ((d * w).sum(1) / w.sum()).sqrt()
-    pe = PointError(build_alignment('root'))
-    pe(res['keypoints'].contiguous(), p['joints'])
-    return {'height_1mm': float((((meas[:, 1] - tgt[:, 1]).abs() < 1e-3) & ok).float().mean()),
-            'mass_1pct': float((((meas[:, 0] - tgt[:, 0]).abs() / tgt[:, 0].abs() < 1e-2) & ok).float().mean()),
-            'circ_0.5pct': float(((((meas - tgt).abs() / tgt.abs())[:, 2:] < 5e-3).all(1) & ok).float().mean()),
-            'frac_rms2d': float((rms < RMS_THRESHOLD).float().mean()), 'median_rms2d': float(rms.median()),
-            'median_beta_err': float((res['betas'] - p['bstar']).norm(dim=1).median()),
-            'median_root_mpjpe_m': float(pe.last_mean.median())}
 
 
 @pytest.mark.parametrize('which', ['all', 'body'])
@@ -467,7 +409,7 @@ def test_fit_quality_256_bodies(model, which):
     kpo = fit_body_to_keypoints_2d(module, p['x'], w, **kw)
     comb = fit_body_to_keypoints_2d(module, p['x'], w, **hm, **kw)
     start = fit_body_to_keypoints_2d(module, p['x'], w, iterations=0, **hm, **kw)['loss']
-    qk, qc = quality(module, bm, p, kpo, w), quality(module, bm, p, comb, w)
+    qk, qc = harness.quality_2d(module, bm, p, kpo, w), harness.quality_2d(module, bm, p, comb, w)
     print(f'fit_kp2d_meas_lm_256[{which}]', {'keypoints_only': qk, 'height_mass': qc,
                                              'median_loss': float(comb['loss'].median()),
                                              'median_start': float(start.median())})

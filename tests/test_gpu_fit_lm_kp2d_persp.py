@@ -1,103 +1,28 @@
-"""GPU: the perspective 2D keypoint Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_perspective_step) against its
-NumPy restatement (tests/kp2d_lm_oracle.py with intrinsics, pinned by tests/test_fit_lm_kp2d_persp_cpu.py) at P = 7 to 96, its
-measurement entry against it, argument errors, and fit_body_to_keypoints_2d(focal_length=...) end to end on the
-synthetic SMPL-X: monotone losses, no host synchronisation, launches per iteration, determinism, batch independence,
-the returned loss, Adam, the command line, and quality against the weak-perspective fit."""
-import math
-
+"""GPU: the perspective 2D keypoint Levenberg-Marquardt step (shapy_fit_lm_keypoints_2d_perspective_step) and its
+measurement entry against their NumPy restatement (tests/kp2d_lm_oracle.py with intrinsics, pinned by
+tests/test_fit_lm_kp2d_persp_cpu.py) at P = 7 to 96, the measurement entry with every measurement dropped against the
+plain one, argument errors, and fit_body_to_keypoints_2d(focal_length=...) end to end on the synthetic SMPL-X:
+monotone losses, no host synchronisation, launches per iteration, determinism, batch independence, the returned loss,
+Adam, the command line, and quality against the weak-perspective fit."""
 import numpy as np
 import pytest
 import torch
 
-import kp2d_lm_oracle as o2
+import lm_harness as harness
+from lm_harness import bits
 from shapy_b200 import synth
-from test_gpu_fit_lm_keypoints_2d import _bits, _get, _rodrigues
 
 pytestmark = pytest.mark.gpu
 
-F, PP = 1000.0, (500.0, 500.0)
+F, PP = harness.F, harness.PP
+
 
 # ------------------------------------------------------------------------------------------------ step kernel
 # (n_rot, nb): P = 7, 54, 55 (twice), 96, and 78 and 79 (the largest P under 48 KB of shared memory without opting in,
 # and the smallest that opts in)
 STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10), (22, 9)]
 STEP_K = [1, 8, 9, 127]
-# (robust_sigma, pose_prior_weight, betas_weight), sigma in pixels
-TERMS = [(math.inf, 0.0, 0.0), (20.0, 500.0, 100.0)]
-
-
-def _step_case(n_rot, nb, K, terms):
-    """Seven bodies with random Jacobians, keypoints about 4 m in front of a 1000 px camera: body 0's trial hits its
-    targets (accepted), body 1's state does and its trial is far (rejected), body 2 has a weighted NaN trial keypoint
-    (rejected), body 3's trial has a weighted keypoint behind the camera (rejected), body 4's trial a dropped one
-    behind it, 5 and 6 random.  With K >= 8 keypoint 7 has weight 0 and NaN targets, keypoints and rows."""
-    sigma, pw, bw = terms
-    B, P = 7, 3 * n_rot + nb + 3
-    gen = torch.Generator().manual_seed(2000 * n_rot + 10 * nb + K + (3 if pw else 0))
-    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
-    betas = rn(B, nb)
-    tr = torch.cat([0.3 * rn(B, 2), 3.0 + torch.rand(B, 1, generator=gen)], 1)
-    tbetas, ttr = betas + 0.05 * rn(B, nb), tr + 0.02 * rn(B, 3)
-    anchor[0], tbetas[0] = trot[0], 0.9 * betas[0]
-    anchor[1], tbetas[1] = rot[1], 1.1 * betas[1]
-    kp, jac = 0.4 * rn(B, K, 3), 0.3 * rn(B, 3 * K, P)
-    tkp, tjac = kp + 0.01 * rn(B, K, 3), jac + 0.03 * rn(B, 3 * K, P)
-    kp[0] = tkp[0] + 0.1
-    tkp[1] = kp[1] + 0.1
-    intr = torch.tensor([F, *PP]).repeat(B, 1)
-    intr[5:, 0] = 800.0 + 400.0 * torch.rand(2, generator=gen)
-    proj = lambda k, t, b: torch.from_numpy(o2.project(k.numpy(), t.numpy(), intr[b].numpy())).float()  # noqa: E731
-    tg = torch.stack([proj(kp[b], tr[b], b) for b in range(B)]) + 5.0 * rn(B, K, 2)
-    tg[0], tg[1] = proj(tkp[0], ttr[0], 0), proj(kp[1], tr[1], 1)
-    tkp[2, 0, 1] = float('nan')
-    tkp[3, 0, 2] = -ttr[3, 2] - 0.5                       # Y_z = -0.5
-    w = torch.rand(B, K, generator=gen) + 0.5
-    if K >= 8:
-        w[:, 7] = 0.0
-        tg[:, 7] = float('nan')
-        for t in (kp, tkp):
-            t[:, 7] = float('nan')
-        for t in (jac, tjac):
-            t[:, 21:24] = float('nan')
-        tkp[4, 7, 2] = -10.0                             # dropped and behind the camera: not read
-    return dict(rot=rot, betas=betas, tr=tr, kp=kp, jac=jac, trot=trot, tbetas=tbetas, ttr=ttr, tkp=tkp, tjac=tjac,
-                tg=tg, w=w, intr=intr, anchor=anchor, lam=torch.rand(B, generator=gen) + 0.01, sigma=sigma, pw=pw,
-                bw=bw)
-
-
-def _state_np(c, b):
-    n = lambda t: t.numpy()  # noqa: E731
-    s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'transl': n(c['tr'][b]), 'keypoints': n(c['kp'][b]),
-         'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-    s['loss'] = np.float32(o2.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'], s['transl'], c['sigma'], s['rot'],
-                                   n(c['anchor'][b]), c['pw'], s['betas'], c['bw'], intr=n(c['intr'][b])))
-    return s
-
-
-def _device(c):
-    B = c['rot'].shape[0]
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'transl': cu(c['tr']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([_state_np(c, b)['loss'] for b in range(B)]))),
-             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'transl': cu(c['ttr'])}
-    return state, trial
-
-
-def _step(c, state, trial, first, meas=None):
-    from shapy_b200 import ops
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    args = (state, trial, cu(c['tg']), cu(c['w']), cu(c['intr']), c['sigma'], c['pw'], c['bw'])
-    if meas is None:
-        ops.fit_lm_keypoints_2d_perspective_step(*args, 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']),
-                                                 pose_anchor=cu(c['anchor']))
-    else:
-        ops.fit_lm_keypoints_2d_perspective_measurements_step(*args, meas[0], meas[1], 10.0, 3.0, first,
-                                                              cu(c['tkp']), cu(c['tjac']), meas[2], meas[3],
-                                                              pose_anchor=cu(c['anchor']))
+TERMS = harness.KP2D_TERMS['persp']         # (robust_sigma, pose_prior_weight, betas_weight), sigma in pixels
 
 
 @pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
@@ -105,60 +30,37 @@ def _step(c, state, trial, first, meas=None):
 @pytest.mark.parametrize('K', STEP_K)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_step_kernel_vs_oracle(n_rot, nb, K, first, terms):
-    c = _step_case(n_rot, nb, K, terms)
-    B = c['rot'].shape[0]
-    n = lambda t: t.numpy()  # noqa: E731
-    s_np = [_state_np(c, b) for b in range(B)]
-    state, trial = _device(c)
-    _step(c, state, trial, first)
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
-    for b in range(B):
-        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttr'][b])}
-        new, want, acc = o2.lm_keypoints_2d_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                 n(c['tkp'][b]), n(c['tjac'][b]), sigma=c['sigma'],
-                                                 anchor=n(c['anchor'][b]), pose_w=c['pw'], betas_w=c['bw'],
-                                                 intr=n(c['intr'][b]))
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        assert np.isclose(got['lambda'][b], new['lambda'], rtol=3e-7, atol=0), (b, got['lambda'][b], new['lambda'])
-        assert np.isclose(got['loss'][b], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (b, got['loss'][b],
-                                                                                          new['loss'])
-        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac'):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'transl'):
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= bar, (b, k, err)
-            worst = max(worst, err / bar)
-    if first:
-        assert all(flags)
-        assert math.isnan(got['loss'][3]) and np.array_equal(nxt['transl'][3], c['ttr'][3].numpy())  # does not move
-    else:
-        assert flags[:4] == [True, False, False, False], flags
-    if K >= 8:
-        assert math.isfinite(got['loss'][4])
+    worst = harness.kp2d_run(first, n_rot=n_rot, nb=nb, K=K, terms=terms, persp=True)
     print(f'[kp2d persp] step P={3 * n_rot + nb + 3} K={K} first={first} terms={terms}: trial error / bar '
           f'{worst:.3f}')
+
+
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('first', [False, True])
+@pytest.mark.parametrize('K', STEP_K)
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
+def test_measurement_step_kernel_vs_oracle(n_rot, nb, K, first, terms):
+    worst = harness.kp2d_run(first, n_rot=n_rot, nb=nb, K=K, terms=terms, persp=True, meas=True)
+    print(f'[kp2d persp] measurement step P={3 * n_rot + nb + 3} K={K} first={first} terms={terms}: trial error / '
+          f'bar {worst:.3f}')
 
 
 @pytest.mark.parametrize('first', [False, True])
 def test_measurement_entry_with_dropped_measurements_is_the_plain_step(first):
     for n_rot, nb, K in ((22, 10, 127), (8, 27, 9), (22, 9, 127)):
-        c = _step_case(n_rot, nb, K, TERMS[1])
+        c = harness.kp2d_case(n_rot, nb, K, TERMS[1], persp=True)
         B = c['rot'].shape[0]
         nan = lambda *s: torch.full(s, float('nan'), device='cuda')  # noqa: E731
         meas = (nan(B, 5), torch.zeros(B, 5, device='cuda'), nan(B, 5), nan(B, 5, nb))
-        s1, t1 = _device(c)
-        _step(c, s1, t1, first)
-        s2, t2 = _device(c)
+        s1, t1 = harness.kp2d_device(c)
+        harness.kp2d_step(c, s1, t1, first)
+        s2, t2 = harness.kp2d_device(c)
         s2.update(meas=nan(B, 5), meas_jac=nan(B, 5, nb))
-        _step(c, s2, t2, first, meas)
+        harness.kp2d_step(c, s2, t2, first, meas)
         for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-            assert torch.equal(s1[k].view(torch.int32), s2[k].view(torch.int32)), k
+            assert torch.equal(bits(s1[k]), bits(s2[k])), k
         for k in t1:
-            assert torch.equal(_bits(t1[k]), _bits(t2[k])), k
+            assert torch.equal(bits(t1[k]), bits(t2[k])), k
 
 
 def test_argument_errors_raise_before_any_launch():
@@ -202,7 +104,7 @@ def test_argument_errors_raise_before_any_launch():
     for kw in (dict(focal_length=1000.0), dict(focal_length=1000.0, principal_point=(1.0, 2.0), groups=[0, 0]),
                dict(focal_length=[1.0, 2.0, 3.0], principal_point=(1.0, 2.0))):
         with pytest.raises(ValueError):
-            fit_body_to_keypoints_2d(_get(), x, method='lm', **kw)
+            fit_body_to_keypoints_2d(harness.smplx_module(), x, method='lm', **kw)
     st0 = {k: v[:0].contiguous() for k, v in st.items()}
     tr0 = {k: v[:0].contiguous() for k, v in tr.items()}
     ops.fit_lm_keypoints_2d_perspective_step(st0, tr0, z(0, K, 2), z(0, K), z(0, 3), None, 0.0, 0.0, 10.0, 3.0, True,
@@ -245,7 +147,7 @@ def test_lm_monotone_losses_and_the_returned_loss():
     PerspectiveCamera (SMPLX.forward with transl) within fp32 rounding of the kernel's."""
     from shapy_b200 import ops
     from shapy_b200.fit import LM_DOWN, LM_UP, _kp2d_loss, _project, fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init, _, _ = _problem(module, 64, seed=5)
     w = (torch.rand(64, x.shape[1], generator=torch.Generator().manual_seed(6)) + 0.5).cuda()
     w[:, 3] = 0.0
@@ -274,48 +176,41 @@ def test_lm_monotone_losses_and_the_returned_loss():
         res = fit_body_to_keypoints_2d(module, x, w, init=init, method='lm', iterations=20, robust_sigma=sigma,
                                        pose_prior_weight=pw, betas_weight=bw, **_kw())
         for k in ('betas', 'transl'):
-            assert torch.equal(_bits(res[k]), _bits(state[k])), k
+            assert torch.equal(bits(res[k]), bits(state[k])), k
         assert 'camera' not in res and res['proj_joints'].shape == x.shape
         with torch.no_grad():
             out = module(global_rot=state['rot'][:, :1], body_pose=state['rot'][:, 1:], betas=state['betas'],
                          transl=state['transl'], return_shaped=False)
             host = _kp2d_loss(_project(out['joints'][:], intr), x, w, sigma, pw, state['rot'], rot0, bw,
                               state['betas'])
-        assert torch.equal(_bits(res['loss']), _bits(host))
+        assert torch.equal(bits(res['loss']), bits(host))
         rel = float(((res['loss'] - state['loss']).abs() / state['loss'].abs().clamp_min(1.0)).max())   # px^2
         print(f'[kp2d persp] sigma={sigma}: returned loss vs kernel loss, max relative {rel:.2e}')
         assert rel <= 1e-2
 
 
 def test_lm_loop_never_synchronises_and_launches_per_iteration():
-    from shapy_b200 import _lib
     from shapy_b200.body_measurements import BodyMeasurements
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init, _, _ = _problem(module, 32, seed=7)
     bm = BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda()
-    L = _lib.lib()
     for meas, per_it in ((None, 2), ({'height': 1.7}, 4)):
         kw = _kw(method='lm', robust_sigma=10.0, pose_prior_weight=100.0, body_measurements=bm if meas else None,
                  measurements=meas)
         fit_body_to_keypoints_2d(module, x, init=init, iterations=1, **kw)
         counts = []
         for its in (3, 4):
-            torch.cuda.synchronize()
-            torch.cuda.set_sync_debug_mode('error')
-            try:
-                n0 = L.shapy_launch_count()
-                res = fit_body_to_keypoints_2d(module, x, init=init, iterations=its, **kw)
-                counts.append(L.shapy_launch_count() - n0)
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
+            n, res = harness.launches_without_sync(
+                lambda: fit_body_to_keypoints_2d(module, x, init=init, iterations=its, **kw))
+            counts.append(n)
         assert counts[1] - counts[0] == per_it, counts
         assert res['transl'].shape == (32, 3) and (meas is None or res['measurements'].shape == (32, 5))
 
 
 def test_lm_deterministic_and_batch_independent():
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init, _, _ = _problem(module, 64, seed=8)
     kw = _kw(method='lm', iterations=15, robust_sigma=10.0, pose_prior_weight=100.0)
     r1 = fit_body_to_keypoints_2d(module, x, init=init, **kw)
@@ -324,26 +219,26 @@ def test_lm_deterministic_and_batch_independent():
     r8 = fit_body_to_keypoints_2d(module, x[rows].contiguous(), init={k: v[rows].contiguous() for k, v in init.items()},
                                   **kw)
     for k in ('global_rot', 'body_pose', 'betas', 'transl', 'loss'):
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
     for k in ('global_rot', 'body_pose', 'betas', 'transl'):
-        assert torch.equal(_bits(r8[k]), _bits(r1[k][rows])), k
+        assert torch.equal(bits(r8[k]), bits(r1[k][rows])), k
     # the returned loss is recomputed by torch, whose reductions may round differently at another batch size
     assert torch.allclose(r8['loss'], r1['loss'][rows], rtol=1e-6, atol=0)
 
 
 def test_start_behind_the_camera_reports_inf_and_does_not_move():
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init, _, _ = _problem(module, 4, seed=9)
     init['transl'][1, 2] = -3.0
     res = fit_body_to_keypoints_2d(module, x, init=init, method='lm', iterations=5, **_kw())
     assert res['loss'][1] == float('inf') and torch.isfinite(res['loss'][[0, 2, 3]]).all()
-    assert torch.equal(_bits(res['transl'][1]), _bits(init['transl'][1]))
+    assert torch.equal(bits(res['transl'][1]), bits(init['transl'][1]))
 
 
 def test_adam_lowers_the_loss():
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    module = _get()
+    module = harness.smplx_module()
     x, _, init, _, _ = _problem(module, 16, seed=10)
     r0 = fit_body_to_keypoints_2d(module, x, init=init, iterations=0, **_kw())
     r = fit_body_to_keypoints_2d(module, x, init=init, iterations=200, lr=0.01, **_kw())
@@ -399,7 +294,7 @@ def test_quality_256_bodies_weak_vs_perspective():
     from shapy_b200.body_measurements import BodyMeasurements
     from shapy_b200.fit import fit_body_to_keypoints_2d, measurement_jacobian
     from shapy_b200.metrics import PointError, build_alignment
-    module = _get()
+    module = harness.smplx_module()
     B = 256
     x, joints, init, tstar, bstar = _problem(module, B)
     bm = BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda()

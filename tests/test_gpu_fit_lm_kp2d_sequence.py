@@ -13,8 +13,9 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2d_sequence_lm_oracle as osq
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
-from test_gpu_fit_lm_keypoints_2d import _bits, _get, _rodrigues
 
 pytestmark = pytest.mark.gpu
 
@@ -37,9 +38,9 @@ def _step_case(n_rot, nb, K, terms, lens=LENS, seed=0):
     gidx = torch.repeat_interleave(torch.arange(S), torch.tensor(lens))
     gen = torch.Generator().manual_seed(5000 * n_rot + 10 * nb + K + seed + (3 if terms[1] else 0))
     rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
+    rot = rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
+    trot = (rot.double() @ rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
+    anchor = (rot.double() @ rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
     betas = rn(S, nb)
     tr = torch.cat([0.3 * rn(B, 2), 3.0 + torch.rand(B, 1, generator=gen)], 1)
     tbetas, ttr = betas + 0.05 * rn(S, nb), tr + 0.02 * rn(B, 3)
@@ -116,13 +117,11 @@ def _step(c, state, trial, first):
 
 def _check_vs_oracle(c, s0, state, trial, first):
     """The stepped device state and next trial against kp2d_sequence_lm_oracle sequence by sequence: loss and lambda to
-    fp32 rounding, the state bit for bit, the next trial within 2e-6 max(1, |x|), each frame's trial betas its
-    sequence's.  Returns (the sequences' accepted flags, the largest trial error over its bar)."""
+    fp32 rounding, the state bit for bit, the next trial within 2e-6 max(1, |x|) (lm_harness.check_step), each frame's
+    trial betas its sequence's.  Returns (the sequences' accepted flags, the largest trial error over its bar)."""
     S = len(c['off']) - 1
     sigma, pw, bw, srw, stw = c['terms']
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
+    oracle = []
     for s in range(S):
         r = range(c['off'][s], c['off'][s + 1])
         st = {'rot': [s0['rot'][i] for i in r], 'transl': [s0['transl'][i] for i in r],
@@ -130,27 +129,14 @@ def _check_vs_oracle(c, s0, state, trial, first):
               'betas': s0['betas'][s], 'loss': s0['loss'][s], 'lambda': s0['lambda'][s], 'accepted': 0}
         tr = {'rot': [_n(c['trot'][i]) for i in r], 'transl': [_n(c['ttr'][i]) for i in r],
               'betas': _n(c['tbetas'][s])}
-        new, want, acc = osq.lm_sequence_step(st, _frames(c, s), 10.0, 3.0, first, tr, sigma, pw, bw, srw, stw)
-        flags.append(acc)
-        assert got['accepted'][s] == new['accepted'], s
-        assert np.isclose(got['lambda'][s], new['lambda'], rtol=3e-7, atol=0), (s, got['lambda'][s], new['lambda'])
-        assert np.isclose(got['loss'][s], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (s, got['loss'][s],
-                                                                                          new['loss'])
-        assert np.array_equal(got['betas'][s], new['betas'], equal_nan=True), s
-        for j, i in enumerate(r):
-            for k in ('rot', 'transl', 'keypoints', 'jac'):
-                assert np.array_equal(got[k][i], new[k][j], equal_nan=True), (s, i, k)
-            for k in ('rot', 'transl'):
-                bar = 2e-6 * max(1.0, np.abs(want[k][j]).max())
-                err = np.abs(nxt[k][i] - want[k][j]).max()
-                assert err <= bar, (s, i, k, err)
-                worst = max(worst, err / bar)
-            assert np.array_equal(nxt['image_betas'][i], nxt['betas'][s])
-        bar = 2e-6 * max(1.0, np.abs(want['betas']).max())
-        err = np.abs(nxt['betas'][s] - want['betas']).max()
-        assert err <= bar, (s, 'betas', err)
-        worst = max(worst, err / bar)
-    return flags, worst
+        oracle.append(osq.lm_sequence_step(st, _frames(c, s), 10.0, 3.0, first, tr, sigma, pw, bw, srw, stw))
+    got, nxt = harness.numpy_of(state), harness.numpy_of(trial)
+    for s in range(S):
+        for i in range(c['off'][s], c['off'][s + 1]):
+            assert np.array_equal(nxt['image_betas'][i], nxt['betas'][s]), (s, i)
+    image = ('rot', 'transl', 'keypoints', 'jac')
+    gs, xs = harness.group_rows(c, got, nxt, S, image, ())
+    return harness.check_step(gs, xs, oracle, image + ('betas',), ('rot', 'transl', 'betas'), exact=False)
 
 
 @pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors_smooth'])
@@ -199,7 +185,7 @@ def test_one_frame_sequences_are_the_perspective_step(first, terms):
                                              10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']),
                                              pose_anchor=cu(c['anchor']))
     for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(state[k]), bits(b_state[k])), k
     for k in ('rot', 'betas', 'transl'):
         err = (trial[k] - b_trial[k]).abs().max()
         assert float(err) <= 4e-6 * max(1.0, float(b_trial[k].abs().max())), (k, float(err))
@@ -334,23 +320,15 @@ SMOOTH = dict(smooth_rot_weight=3e3, smooth_transl_weight=1e4)
 
 
 def test_lm_launches_no_synchronisation_and_monotone_losses():
-    from shapy_b200 import _lib
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 4, 8, seed=82)
-    L = _lib.lib()
     kw = dict(method='lm', robust_sigma=10.0, pose_prior_weight=100.0, **SMOOTH)
     _fit(module, v, iterations=1, **kw)
     for init in (v['init'], {}):                                # and the default start
         counts = []
         for its in (3, 4):
-            torch.cuda.synchronize()
-            torch.cuda.set_sync_debug_mode('error')
-            try:
-                n0 = L.shapy_launch_count()
-                res = _fit(module, v, iterations=its, init=init, **kw)
-                counts.append(L.shapy_launch_count() - n0)
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
+            n, res = harness.launches_without_sync(lambda: _fit(module, v, iterations=its, init=init, **kw))
+            counts.append(n)
         assert counts[1] - counts[0] == 4, counts
     assert res['transl'].shape == (32, 3) and res['betas'].shape == (4, 10) and res['loss'].shape == (4,)
     assert res['proj_joints'].shape == v['x'].shape
@@ -367,27 +345,27 @@ def test_lm_launches_no_synchronisation_and_monotone_losses():
 def test_lm_deterministic_batch_independent_and_reversible():
     """Bitwise determinism; a sequence alone gives its bits in the batch; the labels need not be sorted; and every
     sequence's frames reversed give the reversed fit to tolerance (C_t against C_t^T)."""
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 6, 8, seed=83)
     kw = dict(method='lm', iterations=12, robust_sigma=10.0, pose_prior_weight=100.0, **SMOOTH)
     r1, r2 = _fit(module, v, **kw), _fit(module, v, **kw)
     for k in r1:
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
     s = 3
     rows = torch.arange(s * 8, (s + 1) * 8)
     one = _fit(module, dict(v, x=v['x'][rows], w=v['w'][rows]), sequences=None,
                init={k: t[rows] for k, t in v['init'].items()}, **kw)
     for k in ('global_rot', 'body_pose', 'transl'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][rows])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][rows])), k
     for k in ('betas', 'loss'):
-        assert torch.equal(_bits(one[k][0]), _bits(r1[k][s])), k
+        assert torch.equal(bits(one[k][0]), bits(r1[k][s])), k
     # interleaved labels: the same sequences in another batch order
     perm = torch.arange(48).reshape(6, 8).t().reshape(-1)
     mixed = _fit(module, dict(v, x=v['x'][perm], w=v['w'][perm], seq=v['seq'][perm]),
                  init={k: t[perm] for k, t in v['init'].items()}, **kw)
     for k in ('global_rot', 'transl'):
-        assert torch.equal(_bits(mixed[k]), _bits(r1[k][perm])), k
-    assert torch.equal(_bits(mixed['betas']), _bits(r1['betas']))
+        assert torch.equal(bits(mixed[k]), bits(r1[k][perm])), k
+    assert torch.equal(bits(mixed['betas']), bits(r1['betas']))
     rev = torch.arange(48).reshape(6, 8).flip(1).reshape(-1)
     back = _fit(module, dict(v, x=v['x'][rev], w=v['w'][rev]), init={k: t[rev] for k, t in v['init'].items()},
                 iterations=3, **{k: a for k, a in kw.items() if k != 'iterations'})
@@ -400,20 +378,20 @@ def test_lm_deterministic_batch_independent_and_reversible():
 
 
 def test_start_behind_the_camera_reports_inf_and_does_not_move():
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 3, 5, seed=84)
     init = {k: t.clone() for k, t in v['init'].items()}
     init['transl'][7, 2] = -3.0                                 # frame 2 of sequence 1
     res = _fit(module, v, init=init, method='lm', iterations=5, **SMOOTH)
     assert res['loss'][1] == float('inf') and torch.isfinite(res['loss'][[0, 2]]).all()
-    assert torch.equal(_bits(res['transl'][5:10]), _bits(init['transl'][5:10]))
+    assert torch.equal(bits(res['transl'][5:10]), bits(init['transl'][5:10]))
     ref = _fit(module, v, method='lm', iterations=5, **SMOOTH)
     for k in ('betas', 'loss'):
-        assert torch.equal(_bits(res[k][[0, 2]]), _bits(ref[k][[0, 2]])), k
+        assert torch.equal(bits(res[k][[0, 2]]), bits(ref[k][[0, 2]])), k
 
 
 def test_adam_lowers_the_loss():
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 4, 6, seed=85)
     r0 = _fit(module, v, method='adam', iterations=0, **SMOOTH)
     r = _fit(module, v, method='adam', iterations=150, lr=0.01, **SMOOTH)
@@ -425,7 +403,7 @@ def test_adam_lowers_the_loss():
 def test_cli_on_a_written_npz(tmp_path):
     from shapy_b200 import fit
     from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 2, 5, seed=86)
     K = SMPLX(data_struct=synth.make_smplx()).cuda().packed().K          # the command line's model: its keypoints lead
     n = lambda t: t.detach().cpu().numpy()  # noqa: E731
@@ -500,7 +478,7 @@ def quality_runs(module, v, iterations=50):
 
 
 def test_quality_32_videos():
-    module = _get()
+    module = harness.smplx_module()
     v = _video(module, 32, 32)
     rep = quality_runs(module, v)
     print('fit_kp2d_sequence_32x32', rep)

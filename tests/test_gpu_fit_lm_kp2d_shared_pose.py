@@ -14,23 +14,27 @@ import torch
 
 import kp2d_lm_oracle as o2
 import kp2d_shared_pose_lm_oracle as osp
+import lm_harness as harness
+from lm_harness import NAMES, N_ROT, bits, quality_2d, quality_groups
 from oracle.lm_oracle import meas_loss
-from test_gpu_fit_lm_kp2d_groups import quality as quality_groups
-from test_gpu_fit_lm_kp2d_meas import NAMES, N_ROT, _bits, _measure, _rodrigues, model  # noqa: F401
-from test_gpu_fit_lm_kp2d_meas import quality as quality_2d
-from test_gpu_model_shapes import STEP_SHAPES
-from test_gpu_model_shapes import _group_case as _random_case
 
 pytestmark = pytest.mark.gpu
-TERMS = [(math.inf, 0.0, 0.0), (0.3, 0.5, 0.1)]
+TERMS = harness.KP2D_TERMS['weak']
 SIZES = (1, 2, 3, 5)
+# (n_rot, nb): P = 7, 54, 55 (twice: the 48 KB opt-in boundary), 79 and 96
+STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27), (22, 10)]
+
+
+@pytest.fixture(scope='module')
+def model():
+    return harness.smplx_and_measurements()
 
 
 # ------------------------------------------------------------------------------------------------ step
 def _case(n_rot, nb, terms, sizes=SIZES, K=9):
-    """test_gpu_model_shapes' grouped case on random Jacobians, made a shared-pose one: every image of a group holds
-    its first image's rotations of joints 1 .. in state and trial, and the group's anchor is its first image's."""
-    c = _random_case(n_rot, nb, K, terms, sizes)
+    """lm_harness' random grouped case, made a shared-pose one: every image of a group holds its first image's
+    rotations of joints 1 .. in state and trial, and the group's anchor is its first image's."""
+    c = harness.random_group_case(n_rot, nb, K, terms, sizes)
     first = torch.from_numpy(c['off'][:-1]).long()
     for k in ('rot', 'trot'):
         c[k] = torch.cat([c[k][:, :1], c[k][first[c['gidx']], 1:]], 1).contiguous()
@@ -85,14 +89,13 @@ def _step(c, state, trial, first, with_meas, ws=None):
 
 
 def _check_vs_oracle(c, s0, state, trial, first, with_meas):
-    """The stepped device state and next trial against the oracle group by group: loss and lambda to fp32 rounding,
-    the state bit for bit, the next trial within 2e-6 max(1, |x|), each image's trial betas its group's and every
-    image's shared rotation rows the same bits.  Returns (the groups' accepted flags, the largest error over its bar)."""
+    """The stepped device state and next trial against the oracle group by group, by lm_harness.check_step; each
+    image's trial betas its group's and every image's shared rotation rows the same bits.  Returns (the groups'
+    accepted flags, the largest error over its bar)."""
     G = len(c['off']) - 1
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
     n = lambda t: t.numpy()  # noqa: E731
-    flags, worst = [], 0.0
+    got, nxt = harness.numpy_of(state), harness.numpy_of(trial)
+    oracle = []
     for g in range(G):
         r = range(c['off'][g], c['off'][g + 1])
         st = {k: [s0[k][i] for i in r] for k in ('rot', 'camera', 'keypoints', 'jac')}
@@ -104,38 +107,22 @@ def _check_vs_oracle(c, s0, state, trial, first, with_meas):
         tr = {'rot': [n(c['trot'][i]) for i in r], 'camera': [n(c['tcam'][i]) for i in r], 'betas': n(c['tbetas'][g])}
         mb = None if not with_meas else {'targets': n(c['mt'][g]), 'weights': n(c['mw'][g]),
                                          'trial_meas': n(c['tmeas'][g]), 'trial_meas_jac': n(c['tmjac'][g])}
-        new, want, acc, _, _ = osp.shared_pose_step(st, images, 10.0, 3.0, first, tr, n(c['ganchor'][g]), c['sigma'],
-                                                    c['pw'], c['bw'], mb)
-        flags.append(acc)
-        assert got['accepted'][g] == new['accepted'], g
-        assert np.isclose(got['lambda'][g], new['lambda'], rtol=3e-7, atol=0), (g, got['lambda'][g], new['lambda'])
-        assert np.isclose(got['loss'][g], new['loss'], rtol=3e-7, atol=0, equal_nan=True), (g, got['loss'][g],
-                                                                                          new['loss'])
-        assert np.array_equal(got['betas'][g], new['betas'], equal_nan=True), g
-        if with_meas:
-            for k in ('meas', 'meas_jac'):
-                assert np.array_equal(got[k][g], new[k], equal_nan=True), (g, k)
-        for j, i in enumerate(r):
-            for k in ('rot', 'camera', 'keypoints', 'jac'):
-                assert np.array_equal(got[k][i], new[k][j], equal_nan=True), (g, i, k)
-            for k in ('rot', 'camera'):
-                bar = 2e-6 * max(1.0, np.abs(want[k][j]).max())
-                err = np.abs(nxt[k][i] - want[k][j]).max()
-                assert err <= bar, (g, i, k, err)
-                worst = max(worst, err / bar)
+        oracle.append(osp.shared_pose_step(st, images, 10.0, 3.0, first, tr, n(c['ganchor'][g]), c['sigma'], c['pw'],
+                                           c['bw'], mb)[:3])
+        for i in r:
             assert np.array_equal(nxt['image_betas'][i], nxt['betas'][g])
-            assert np.array_equal(_bits(trial['rot'][i, 1:]).cpu(), _bits(trial['rot'][r[0], 1:]).cpu()), (g, i)
-        bar = 2e-6 * max(1.0, np.abs(want['betas']).max())
-        err = np.abs(nxt['betas'][g] - want['betas']).max()
-        assert err <= bar, (g, 'betas', err)
-        worst = max(worst, err / bar)
-    return flags, worst
+            assert np.array_equal(bits(trial['rot'][i, 1:]).cpu(), bits(trial['rot'][r[0], 1:]).cpu()), \
+                (g, i)
+    image = ('rot', 'camera', 'keypoints', 'jac')
+    gs, xs = harness.group_rows(c, got, nxt, G, image, ())
+    return harness.check_step(gs, xs, oracle, image + ('betas',) + (('meas', 'meas_jac') if with_meas else ()),
+                              ('rot', 'camera', 'betas'), exact=False)
 
 
 @pytest.mark.parametrize('with_meas', [False, True], ids=['kp2dsp', 'kp2dspm'])
 @pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
-@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES + [(22, 10)])
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_step_kernels_vs_oracle(n_rot, nb, first, terms, with_meas):
     """Both entries on groups of 1, 2, 3 and 5 images at P = 7 to 96, on the first and on a later step."""
     c = _case(n_rot, nb, terms)
@@ -153,7 +140,7 @@ def test_step_kernels_vs_oracle(n_rot, nb, first, terms, with_meas):
 
 @pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
-@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES + [(22, 10)])
+@pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_groups_of_one_equal_the_2d_step(n_rot, nb, first, terms):
     """Six groups of one: loss, lambda, accepted and the state bit for bit as shapy_fit_lm_keypoints_2d_step; the next
     trial within 4e-6 max(1, |x|) (the two eliminations differ by fp64 rounding, the CPU oracle test bounds it)."""
@@ -167,7 +154,7 @@ def test_groups_of_one_equal_the_2d_step(n_rot, nb, first, terms):
     ops.fit_lm_keypoints_2d_step(b_state, b_trial, cu(c['tg']), cu(c['w']), c['sigma'], c['pw'], c['bw'], 10.0, 3.0,
                                  first, cu(c['tkp']), cu(c['tjac']), pose_anchor=cu(c['ganchor']))
     for k in ('rot', 'betas', 'camera', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(state[k]), bits(b_state[k])), k
     for k in ('rot', 'betas', 'camera'):
         err = (trial[k] - b_trial[k]).abs().max()
         assert float(err) <= 4e-6 * max(1.0, float(b_trial[k].abs().max())), (k, float(err))
@@ -197,9 +184,9 @@ def test_one_rotation_equals_the_groups_step_bit_for_bit(nb, first, with_meas):
                                             10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']), off, ws,
                                             pose_anchor=anchor)
     for k in a_state:
-        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(a_state[k]), bits(b_state[k])), k
     for k in a_trial:
-        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+        assert torch.equal(bits(a_trial[k]), bits(b_trial[k])), k
 
 
 @pytest.mark.parametrize('first', [False, True])
@@ -216,9 +203,9 @@ def test_dropped_measurements_equal_the_plain_step_bit_for_bit(n_rot, nb, first)
     _step(c, a_state, a_trial, first, True)
     _step(c, b_state, b_trial, first, False)
     for k in b_state:
-        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(a_state[k]), bits(b_state[k])), k
     for k in b_trial:
-        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+        assert torch.equal(bits(a_trial[k]), bits(b_trial[k])), k
 
 
 def test_argument_errors_workspace_and_empty_batch(model):
@@ -319,7 +306,7 @@ def _problem(module, bm, n_id, views=(0.0, 90.0, 180.0, 270.0), seed=41):
         rot = torch.cat([grot[:, None], rot_id[groups, 1:]], 1)
         out = module(global_rot=rot[:, :1].cuda(), body_pose=rot[:, 1:].cuda(), betas=bstar[groups].cuda(),
                      camera=cam.cuda())
-        tgt = _measure(module, bm, bstar.cuda())
+        tgt = harness.measure(module, bm, bstar.cuda())
     raw_img = rot[..., :2].reshape(B, 132)                                            # as the decoder reads it
     init = {'global_rot': (raw_img[:, :6] + 0.1 * rn(B, 6)).cuda(),
             'body_pose': (raw_img[:, 6:] + 0.1 * rn(B, 126)).cuda(),
@@ -396,16 +383,16 @@ def test_lm_losses_monotone_launch_count_and_returned_by_the_fit(model, with_mea
     assert res['betas'].shape == (16, 10) and res['body_pose_mat'].shape == (16, 21, 3, 3)
     assert res['camera'].shape == (64, 3) and res['global_rot_mat'].shape == (64, 1, 3, 3)
     for k in ('betas', 'loss'):
-        assert torch.equal(_bits(res[k]), _bits(state[k])), k
+        assert torch.equal(bits(res[k]), bits(state[k])), k
     inv = torch.argsort(o)
-    assert torch.equal(_bits(res['camera']), _bits(state['camera'][inv]))
-    assert torch.equal(_bits(res['global_rot_mat']), _bits(state['rot'][inv][:, :1]))
-    assert torch.equal(_bits(res['body_pose_mat']), _bits(state['rot'][first, 1:]))
+    assert torch.equal(bits(res['camera']), bits(state['camera'][inv]))
+    assert torch.equal(bits(res['global_rot_mat']), bits(state['rot'][inv][:, :1]))
+    assert torch.equal(bits(res['body_pose_mat']), bits(state['rot'][first, 1:]))
     # every image's shared rows are its group's, bit for bit
     gidx = ps['groups']
-    assert torch.equal(_bits(state['rot'][:, 1:]), _bits(state['rot'][first[gidx], 1:]))
+    assert torch.equal(bits(state['rot'][:, 1:]), bits(state['rot'][first[gidx], 1:]))
     if with_meas:
-        assert torch.equal(_bits(res['measurements']), _bits(state['meas']))
+        assert torch.equal(bits(res['measurements']), bits(state['meas']))
 
 
 def test_lm_deterministic_and_group_independent(model):
@@ -418,16 +405,16 @@ def test_lm_deterministic_and_group_independent(model):
     r1 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
     r2 = fit_body_to_keypoints_2d(module, p['x'], init=p['init'], measurements=meas, groups=p['groups'], **kw)
     for k in r1:
-        assert torch.equal(_bits(r1[k]), _bits(r2[k])), k
+        assert torch.equal(bits(r1[k]), bits(r2[k])), k
     rows = (p['groups'] == 5).nonzero()[:, 0]                          # identity 5 alone, as label 0
     one = fit_body_to_keypoints_2d(module, p['x'][rows].contiguous(),
                                    init={k: v[rows].contiguous() for k, v in p['init'].items()},
                                    measurements={k: v[5:6].contiguous() for k, v in meas.items()},
                                    groups=torch.zeros(len(rows), dtype=torch.int64), **kw)
     for k in ('betas', 'measurements', 'loss', 'body_pose', 'body_pose_mat'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][5:6])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][5:6])), k
     for k in ('camera', 'global_rot'):
-        assert torch.equal(_bits(one[k]), _bits(r1[k][rows])), k
+        assert torch.equal(bits(one[k]), bits(r1[k][rows])), k
 
 
 def test_lm_loop_never_synchronises(model):
@@ -437,12 +424,7 @@ def test_lm_loop_never_synchronises(model):
     kw = dict(init=p['init'], method='lm', robust_sigma=0.1, pose_prior_weight=1.0, betas_weight=0.01,
               body_measurements=bm, measurements=p['tg'], groups=p['groups'].cpu(), share_pose=True)
     fit_body_to_keypoints_2d(module, p['x'], iterations=1, **kw)       # packs the model, builds the incidence table
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints_2d(module, p['x'], iterations=3, **kw))
     assert res['measurements'].shape == (8, 5) and res['body_pose'].shape == (8, 126)
 
 

@@ -6,34 +6,17 @@ import pytest
 import torch
 
 import kp_lm_oracle
+import lm_harness as harness
+from lm_harness import bits, rodrigues
 from shapy_b200 import synth
 
 pytestmark = pytest.mark.gpu
-NAMES = ('mass', 'height', 'chest', 'waist', 'hips')
-N_ROT = 22
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _rodrigues(aa):
-    aa = aa.double()
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
+NAMES, N_ROT = harness.NAMES, harness.N_ROT
 
 
 @pytest.fixture(scope='module')
 def model():
-    from shapy_b200.body_measurements import BodyMeasurements
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    return (SMPLX(data_struct=synth.make_smplx(), use_face_contour=True).cuda(),
-            BodyMeasurements({'landmarks': synth.load_landmarks()}).cuda())
+    return harness.smplx_and_measurements()
 
 
 def _evaluate(packed, lm, faces, rot, betas, transl):
@@ -55,10 +38,10 @@ def _step_case(model):
     packed, faces, lm = smplx.packed(), smplx.faces_i32, bm.landmarks()
     B = 8
     gen = torch.Generator().manual_seed(41)
-    rot = _rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
+    rot = rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.3).float()
     betas = torch.randn(B, 10, generator=gen).clamp(-2, 2)
     transl = torch.randn(B, 3, generator=gen) * 0.1
-    trot = (rot.double() @ _rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.02)).float()
+    trot = (rot.double() @ rodrigues(torch.randn(B, N_ROT, 3, generator=gen, dtype=torch.float64) * 0.02)).float()
     tbetas = betas + 0.05 * torch.randn(B, 10, generator=gen)
     ttransl = transl + 0.01 * torch.randn(B, 3, generator=gen)
     ttransl[1] += 0.05                                          # body 1's trial clearly worse, whatever rho
@@ -110,26 +93,19 @@ def test_step_kernel_vs_oracle(model, first, rho):
     cu = lambda t: t.cuda().contiguous()  # noqa: E731
     ops.fit_lm_keypoints_measurements_step(state, trial, cu(c['tg']), cu(c['w']), cu(c['mt']), cu(c['mw']), rho, 10.0,
                                            3.0, first, cu(c['tkp']), cu(c['tjac']), cu(c['tmeas']), cu(c['tmjac']))
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
     n = lambda t: t.numpy()  # noqa: E731
-    flags = []
+    oracle = []
     for b in range(B):
         s = {k: s0[k][b] for k in s0}
         s['accepted'] = 0
         tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
-        new, want, acc = kp_lm_oracle.lm_keypoints_step(
+        oracle.append(kp_lm_oracle.lm_keypoints_step(
             s, n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
-            meas=(n(c['mt'][b]), n(c['mw'][b])), trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), betas_weight=rho)
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        assert got['lambda'][b] == new['lambda'], (b, got['lambda'][b], new['lambda'])
-        assert np.array_equal(got['loss'][b], new['loss'], equal_nan=True), (b, got['loss'][b], new['loss'])
-        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'meas', 'meas_jac'):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'transl'):
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= 2e-6 * max(1.0, np.abs(want[k]).max()), (b, k, err)
+            meas=(n(c['mt'][b]), n(c['mw'][b])), trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), betas_weight=rho))
+    got, nxt = harness.numpy_of(state), harness.numpy_of(trial)
+    keys = ('rot', 'betas', 'transl')
+    flags, _ = harness.check_step(harness.rows_of(got, B), harness.rows_of(nxt, B), oracle,
+                             keys + ('keypoints', 'jac', 'meas', 'meas_jac'), keys, exact=True)
     if first:
         assert all(flags) and np.isnan(got['loss'][4])
     else:
@@ -157,9 +133,9 @@ def test_empty_measurement_block_equals_keypoint_step(model, first):
                                            cu(c['tmjac']))
     ops.fit_lm_keypoints_step(b_state, b_trial, cu(c['tg']), cu(c['w']), 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']))
     for k in ('rot', 'betas', 'transl', 'keypoints', 'jac', 'loss', 'lambda', 'accepted'):
-        assert torch.equal(_bits(a_state[k]), _bits(b_state[k])), k
+        assert torch.equal(bits(a_state[k]), bits(b_state[k])), k
     for k in ('rot', 'betas', 'transl'):
-        assert torch.equal(_bits(a_trial[k]), _bits(b_trial[k])), k
+        assert torch.equal(bits(a_trial[k]), bits(b_trial[k])), k
 
 
 # ------------------------------------------------------------------------------------------------ fit
@@ -201,12 +177,6 @@ def _fit(module, kp, **kw):
     return fit_body_to_keypoints(module, kp, init=init, **kw)
 
 
-def _measure(module, bm, betas):
-    with torch.no_grad():
-        m = bm.forward_vertices(module.forward_shape(betas=betas)['v_shaped'], module.faces_i32)['measurements']
-    return torch.stack([m[k]['tensor'] for k in NAMES], 1)
-
-
 def _shares(res, meas, kp, w, tgt, bstar):
     ok = torch.isfinite(tgt).all(1)
     rms = ((res['keypoints'] - kp).pow(2).sum(-1) * w).sum(1).div(w.sum()).sqrt()
@@ -233,7 +203,7 @@ def test_fit_quality_256_bodies(model, which):
     start = _fit(module, kp, weights=w, method='lm', iterations=0, **kw)['loss']
     FITS[which] = (kp, kw['measurements'], w, comb)
     sc = _shares(comb, comb['measurements'], kp, w, tgt, bstar)
-    sk = _shares(kpo, _measure(module, bm, kpo['betas']), kp, w, tgt, bstar)
+    sk = _shares(kpo, harness.measure(module, bm, kpo['betas']), kp, w, tgt, bstar)
     print(f'fit_kp_meas_lm_256[{which}]', {'combined': sc, 'keypoints_only': sk,
                                             'median_loss': float(comb['loss'].median()),
                                             'median_start': float(start.median())})
@@ -243,7 +213,7 @@ def test_fit_quality_256_bodies(model, which):
         assert sc[k] > sk[k], (k, sc[k], sk[k])
     assert all(sc[k] >= BARS[which][k] for k in BARS[which]), sc
     # the returned measurements are those of the returned betas
-    torch.testing.assert_close(comb['measurements'], _measure(module, bm, comb['betas']), rtol=1e-6, atol=1e-7,
+    torch.testing.assert_close(comb['measurements'], harness.measure(module, bm, comb['betas']), rtol=1e-6, atol=1e-7,
                                equal_nan=True)
 
 
@@ -273,7 +243,7 @@ def test_lm_fit_8_bodies_alone_equal_their_batch_rows(model):
     res8 = _fit(module, kp[rows].contiguous(), weights=w, method='lm', body_measurements=bm,
                 measurements={k: v[rows].contiguous() for k, v in tg.items()})
     for k in ('global_rot', 'body_pose', 'betas', 'transl', 'measurements'):
-        assert torch.equal(_bits(res8[k]), _bits(lm[k][rows])), k
+        assert torch.equal(bits(res8[k]), bits(lm[k][rows])), k
 
 
 def test_lm_loop_never_synchronises(model):
@@ -284,12 +254,7 @@ def test_lm_loop_never_synchronises(model):
     init = {'global_rot': mean[:6].expand(32, 6), 'body_pose': mean[6:132].expand(32, 126)}
     kw = dict(init=init, method='lm', body_measurements=bm, measurements=tg, betas_weight=0.01)
     fit_body_to_keypoints(module, kp, iterations=1, **kw)      # packs the model, builds the incidence table
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        res = fit_body_to_keypoints(module, kp, iterations=3, **kw)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+    _, res = harness.launches_without_sync(lambda: fit_body_to_keypoints(module, kp, iterations=3, **kw))
     assert res['measurements'].shape == (32, 5)
 
 

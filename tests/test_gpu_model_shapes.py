@@ -9,7 +9,8 @@ test_model_shapes_cpu.py pins at those shapes.
   * keypoint Jacobian against kp_lm_oracle: bar of test_gpu_fit_lm_keypoints, 1e-4 per body and column block
   * cached against uncached Jacobian entries (edge_2048 / edge_2049): the same bits
   * J^T c against the posed backward on the uncached NB = 27 model
-  * both LM step kernels against their restatements at P = 7, 54, 55 (the 48 KB opt-in boundary) and 96, K = 1 to 127
+  * both 3D LM step kernels against their restatements at P = 7, 54, 55 (the 48 KB opt-in boundary) and 96, K = 1 to
+    127
   * every keypoint step entry launches at P = 96 and refuses P = 97 without a launch
   * the 2D measurement step and both grouped 2D steps on random Jacobians against kp2d_lm_oracle and kp2dg_lm_oracle at
     the same shapes, groups of 1 to 64 images in regular and irregular layouts; groups of one against the 2D step and
@@ -21,47 +22,15 @@ import numpy as np
 import pytest
 import torch
 
-import kp2d_lm_oracle as o2
 import kp_lm_oracle
-import test_gpu_fit_lm_keypoints_2d as kp2d
-import test_gpu_fit_lm_kp2d_groups as grp
+import lm_harness as harness
+from lm_harness import KP_CACHE_ENTRIES, TOL, VARIANTS, bits, keypoint_entries, variant_model
 from shapy_b200 import synth
 from smplx_grad_ref import oracle_grads
-from test_model_shapes_cpu import KP_CACHE_ENTRIES, VARIANTS, keypoint_entries, variant_model
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
 NAMES = list(VARIANTS)
 CHANGED_KP = 15                   # the keypoint J14 row 13 overwrites (source_idxs[13]): edge_2049's added entry
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _rodrigues(aa):
-    aa = aa.double()
-    th = aa.norm(dim=-1, keepdim=True)
-    k = aa / th.clamp_min(1e-300)
-    kx, ky, kz = k.unbind(-1)
-    z = torch.zeros_like(kx)
-    K = torch.stack([z, -kz, ky, kz, z, -kx, -ky, kx, z], -1).view(*aa.shape[:-1], 3, 3)
-    s, c = th.sin()[..., None], th.cos()[..., None]
-    return torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * (K @ K)
-
-
-def _inputs(seed, B, n_rot, NB, NE=0):
-    """Rotations, betas (B, NB), expression (B, NE) or None, transl, camera; necks turned past both ends of the contour
-    LUT in bodies 0 and 1."""
-    gen = torch.Generator().manual_seed(seed)
-    rot = _rodrigues(torch.randn(B, n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
-    if n_rot > 15 and B > 1:
-        rot[0, 12] = _rodrigues(torch.tensor([0.0, 1.2, 0.0])).float()
-        rot[1, 12] = _rodrigues(torch.tensor([0.0, -1.2, 0.0])).float()
-    return dict(rot=rot, betas=torch.randn(B, NB, generator=gen),
-                expression=torch.randn(B, NE, generator=gen) if NE else None,
-                transl=torch.randn(B, 3, generator=gen) * 0.1,
-                camera=torch.randn(B, 3, generator=gen) * torch.tensor([3.0, 0.2, 0.2]) + torch.tensor([1.0, 0, 0]))
 
 
 def _check(name, got, ref, tol=TOL):
@@ -89,13 +58,6 @@ def packed():
     return get
 
 
-def _module(name):
-    from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    NB, NE, _ = VARIANTS[name]
-    return SMPLX(data_struct=variant_model(name), betas={'num': NB}, expression={'num': NE},
-                 use_face_contour=True).cuda()
-
-
 # ------------------------------------------------------------------------------------------------ posed backward
 @pytest.mark.parametrize('kind', ['mixed', 'j14'])
 @pytest.mark.parametrize('B', [1, 33])
@@ -107,7 +69,7 @@ def test_backward_vs_float64(packed, name, n_rot, B, kind):
     from shapy_b200 import ops
     m, pk = variant_model(name), packed(name)
     NB, NE, _ = VARIANTS[name]
-    x = _inputs(10000 * NB + 100 * n_rot + B, B, n_rot, NB, NE)
+    x = harness.inputs(10000 * NB + 100 * n_rot + B, B, n_rot, NB, NE)
     gen = torch.Generator().manual_seed(NB + n_rot + B)
     if kind == 'mixed':
         cot = dict(vertices=torch.randn(B, pk.V, 3, generator=gen), joints=torch.randn(B, pk.K, 3, generator=gen),
@@ -135,10 +97,10 @@ def test_backward_vs_float64(packed, name, n_rot, B, kind):
 def test_module_autograd_with_expression():
     """SMPLX.forward through autograd on nb16_ne16 (NC = 32): betas, expression, the rotations, transl."""
     name = 'nb16_ne16'
-    module = _module(name)
+    module = harness.smplx_module(name)
     NB, NE, _ = VARIANTS[name]
     B = 9
-    x = _inputs(16, B, 22, NB, NE)
+    x = harness.inputs(16, B, 22, NB, NE)
     leaf = {k: x[k].cuda().requires_grad_(True) for k in ('betas', 'expression', 'transl')}
     leaf['rot'] = x['rot'].cuda().requires_grad_(True)
     out = module(global_rot=leaf['rot'][:, :1], body_pose=leaf['rot'][:, 1:], betas=leaf['betas'],
@@ -168,7 +130,7 @@ def test_jacobian_vs_float64(packed, name, n_rot, with_transl):
     m, pk = variant_model(name), packed(name)
     NB = VARIANTS[name][0]
     B = 2
-    x = _inputs(1000 * NB + 10 * n_rot + with_transl, B, n_rot, NB)
+    x = harness.inputs(1000 * NB + 10 * n_rot + with_transl, B, n_rot, NB)
     transl = x['transl'] if with_transl else None
     kp, jac = ops.smplx_keypoint_jacobian(pk, x['betas'].cuda(), x['rot'].cuda(),
                                           None if transl is None else transl.cuda())
@@ -196,15 +158,15 @@ def test_cached_and_uncached_entries_give_the_same_bits(packed, n_rot):
     a, b = variant_model('edge_2048'), variant_model('edge_2049')
     assert keypoint_entries(a) == KP_CACHE_ENTRIES < keypoint_entries(b)
     B = 64
-    x = _inputs(2048 + n_rot, B, n_rot, 10)
+    x = harness.inputs(2048 + n_rot, B, n_rot, 10)
     args = (x['betas'].cuda(), x['rot'].cuda(), x['transl'].cuda())
     kp_a, jac_a = ops.smplx_keypoint_jacobian(packed('edge_2048'), *args)
     kp_b, jac_b = ops.smplx_keypoint_jacobian(packed('edge_2049'), *args)
     K = kp_a.shape[1]
     keep = torch.tensor([k for k in range(K) if k != CHANGED_KP], device='cuda')
     rows = (3 * keep[:, None] + torch.arange(3, device='cuda')).reshape(-1)
-    assert torch.equal(_bits(kp_a[:, keep]), _bits(kp_b[:, keep]))
-    assert torch.equal(_bits(jac_a[:, rows]), _bits(jac_b[:, rows]))
+    assert torch.equal(bits(kp_a[:, keep]), bits(kp_b[:, keep]))
+    assert torch.equal(bits(jac_a[:, rows]), bits(jac_b[:, rows]))
     # the added entry does reach keypoint 15 (the two models differ there)
     assert not torch.equal(kp_a[:, CHANGED_KP], kp_b[:, CHANGED_KP])
 
@@ -217,7 +179,7 @@ def test_jacobian_transpose_equals_backward(packed):
     name = 'nb27_ne5_dense'
     pk, NB = packed(name), VARIANTS[name][0]
     B, n_rot = 256, 22
-    x = _inputs(7, B, n_rot, NB)
+    x = harness.inputs(7, B, n_rot, NB)
     rot, betas, transl = x['rot'].cuda(), x['betas'].cuda(), x['transl'].cuda()
     c = torch.randn(B, pk.K, 3, generator=torch.Generator().manual_seed(8)).cuda()
     _, jac = ops.smplx_keypoint_jacobian(pk, betas, rot, transl)
@@ -246,105 +208,17 @@ STEP_SHAPES = [(1, 1), (8, 27), (12, 16), (17, 1), (22, 27)]
 STEP_K = [1, 5, 6, 127]           # 3K < 16 rows; K = 6 has a dropped keypoint 5 whose rows 15-17 straddle row 16
 
 
-def _step_case(n_rot, nb, K, meas):
-    """Six bodies with random well-conditioned Jacobians: body 0's trial hits its targets (accepted), body 1's state
-    does and its trial is far (rejected), body 2 has a weighted NaN trial keypoint (rejected), with measurements body
-    3 a weighted NaN trial measurement (rejected), 4 and 5 random.  With K >= 6 keypoint 5 has weight 0 and NaN
-    keypoints and rows in state and trial; with measurements the height has weight 0 and NaN values and rows."""
-    B, P = 6, 3 * n_rot + nb + 3
-    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + (7 if meas else 0))
-    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    betas, transl = rn(B, nb), rn(B, 3) * 0.1
-    tbetas, ttransl = betas + 0.05 * rn(B, nb), transl + 0.01 * rn(B, 3)
-    kp, jac = rn(B, K, 3), rn(B, 3 * K, P)
-    tkp, tjac = kp + 0.05 * rn(B, K, 3), jac + 0.1 * rn(B, 3 * K, P)
-    tg = kp + 0.05 * rn(B, K, 3)
-    w = torch.rand(B, K, generator=gen) + 0.5
-    kp[0] = tkp[0] + 0.5
-    tg[0] = tkp[0]
-    tg[1], tkp[1] = kp[1], kp[1] + 0.5
-    tkp[2, 0, 1] = float('nan')
-    if K >= 6:
-        w[:, 5] = 0.0
-        for t in (kp, tkp):
-            t[:, 5] = float('nan')
-        for t in (jac, tjac):
-            t[:, 15:18] = float('nan')
-    c = dict(rot=rot, betas=betas, transl=transl, kp=kp, jac=jac, trot=trot, tbetas=tbetas, ttransl=ttransl, tkp=tkp,
-             tjac=tjac, tg=tg, w=w, lam=torch.rand(B, generator=gen) + 0.01)
-    if meas:
-        m, mj = torch.rand(B, 5, generator=gen) + 0.5, rn(B, 5, nb)
-        tm, tmj = m + 0.01 * rn(B, 5), mj + 0.1 * rn(B, 5, nb)
-        mt = m + 0.02 * rn(B, 5)
-        mt[0], mt[1] = tm[0], m[1]
-        mw = torch.rand(B, 5, generator=gen) * 2 + 0.5
-        mw[:, 1] = 0.0
-        for t in (m, tm, mj, tmj):
-            t[:, 1] = float('nan')
-        tm[3, 3] = float('nan')
-        c.update(meas=m, mjac=mj, tmeas=tm, tmjac=tmj, mt=mt, mw=mw)
-    return c
-
-
-def _run_step(c, first, rho=None):
-    """The kernel on the case (rho None: the keypoint step), then the restatement body by body; returns the largest
-    trial error over its bar and the accepted flags."""
-    from shapy_b200 import ops
-    B = c['rot'].shape[0]
-    meas = rho is not None
-    n = lambda t: t.numpy()  # noqa: E731
-    s_np = []
-    for b in range(B):
-        s = {'rot': n(c['rot'][b]), 'betas': n(c['betas'][b]), 'transl': n(c['transl'][b]), 'keypoints': n(c['kp'][b]),
-             'jac': n(c['jac'][b]), 'lambda': n(c['lam'][b]), 'accepted': 0}
-        if meas:
-            s.update(meas=n(c['meas'][b]), meas_jac=n(c['mjac'][b]))
-            s['loss'] = np.float32(kp_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints'],
-                                                     (n(c['mt'][b]), n(c['mw'][b]), s['meas']), s['betas'], rho))
-        else:
-            s['loss'] = np.float32(kp_lm_oracle.loss(n(c['tg'][b]), n(c['w'][b]), s['keypoints']))
-        s_np.append(s)
-    cu = lambda t: t.cuda().contiguous()  # noqa: E731
-    state = {'rot': cu(c['rot']), 'betas': cu(c['betas']), 'transl': cu(c['transl']), 'keypoints': cu(c['kp']),
-             'jac': cu(c['jac']), 'loss': cu(torch.tensor(np.array([s['loss'] for s in s_np]))),
-             'lambda': cu(c['lam']), 'accepted': torch.zeros(B, dtype=torch.int32, device='cuda')}
-    trial = {'rot': cu(c['trot']), 'betas': cu(c['tbetas']), 'transl': cu(c['ttransl'])}
-    if meas:
-        state.update(meas=cu(c['meas']), meas_jac=cu(c['mjac']))
-        ops.fit_lm_keypoints_measurements_step(state, trial, cu(c['tg']), cu(c['w']), cu(c['mt']), cu(c['mw']), rho,
-                                               10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']), cu(c['tmeas']),
-                                               cu(c['tmjac']))
-    else:
-        ops.fit_lm_keypoints_step(state, trial, cu(c['tg']), cu(c['w']), 10.0, 3.0, first, cu(c['tkp']), cu(c['tjac']))
-    got = {k: v.cpu().numpy() for k, v in state.items()}
-    nxt = {k: v.cpu().numpy() for k, v in trial.items()}
-    flags, worst = [], 0.0
-    for b in range(B):
-        tr = {'rot': n(c['trot'][b]), 'betas': n(c['tbetas'][b]), 'transl': n(c['ttransl'][b])}
-        if meas:
-            new, want, acc = kp_lm_oracle.lm_keypoints_step(
-                s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr, n(c['tkp'][b]), n(c['tjac'][b]),
-                meas=(n(c['mt'][b]), n(c['mw'][b])), trial_meas=(n(c['tmeas'][b]), n(c['tmjac'][b])), betas_weight=rho)
-        else:
-            new, want, acc = kp_lm_oracle.lm_keypoints_step(s_np[b], n(c['tg'][b]), n(c['w'][b]), 10.0, 3.0, first, tr,
-                                                            n(c['tkp'][b]), n(c['tjac'][b]))
-        flags.append(acc)
-        assert got['accepted'][b] == new['accepted'], b
-        assert got['lambda'][b] == new['lambda'], (b, got['lambda'][b], new['lambda'])
-        assert np.array_equal(got['loss'][b], new['loss'], equal_nan=True), (b, got['loss'][b], new['loss'])
-        for k in ('rot', 'betas', 'transl', 'keypoints', 'jac') + (('meas', 'meas_jac') if meas else ()):
-            assert np.array_equal(got[k][b], new[k], equal_nan=True), (b, k)
-        for k in ('rot', 'betas', 'transl'):
-            bar = 2e-6 * max(1.0, np.abs(want[k]).max())
-            err = np.abs(nxt[k][b] - want[k]).max()
-            assert err <= bar, (b, k, err)
-            worst = max(worst, err / bar)
+def _kp_step_vs_oracle(n_rot, nb, K, first, rho=None):
+    """lm_harness.kp_random_case stepped once (rho None: the keypoint step) and checked against kp_lm_oracle; returns
+    the largest trial error over its bar."""
+    c = harness.kp_random_case(n_rot, nb, K, rho is not None, rho or 0.0)
+    state, trial = harness.kp_device(c, rho)
+    harness.kp_step(c, state, trial, first, rho)
+    flags, worst = harness.kp_check(c, state, trial, first, rho)
     if first:
         assert all(flags)
     else:
-        assert flags[:3] == [True, False, False] and (not meas or not flags[3]), flags
+        assert flags[:3] == [True, False, False] and (rho is None or not flags[3]), flags
     return worst
 
 
@@ -352,7 +226,7 @@ def _run_step(c, first, rho=None):
 @pytest.mark.parametrize('K', STEP_K)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_keypoint_step_vs_oracle(n_rot, nb, K, first):
-    worst = _run_step(_step_case(n_rot, nb, K, False), first)
+    worst = _kp_step_vs_oracle(n_rot, nb, K, first)
     print(f'[model-shapes] kp step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first}: trial error / bar {worst:.3f}')
 
 
@@ -361,7 +235,7 @@ def test_keypoint_step_vs_oracle(n_rot, nb, K, first):
 @pytest.mark.parametrize('K', STEP_K)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_keypoint_measurement_step_vs_oracle(n_rot, nb, K, first, rho):
-    worst = _run_step(_step_case(n_rot, nb, K, True), first, rho)
+    worst = _kp_step_vs_oracle(n_rot, nb, K, first, rho)
     print(f'[model-shapes] kpm step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first} rho={rho}: '
           f'trial error / bar {worst:.3f}')
 
@@ -425,83 +299,33 @@ def test_steps_refuse_97_parameters_without_a_launch():
 STEP_K_2D = [1, 8, 9, 127]
 GROUP_K = [1, 9, 127]
 LAYOUTS = {'1-2-3-5': (1, 2, 3, 5), '1-7-1-33-2': (1, 7, 1, 33, 2), '64': (64,)}
+TERMS = harness.KP2D_TERMS['weak']
 
 
-@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('K', STEP_K_2D)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES + [(22, 10), (22, 11)])   # and P = 79 / 80, its 48 KB opt-in boundary
 def test_keypoint_2d_measurement_step_vs_oracle(n_rot, nb, K, first, terms):
-    worst = kp2d._run_step(kp2d._step_case(n_rot, nb, K, terms, meas=True), first)
+    worst = harness.kp2d_run(first, n_rot=n_rot, nb=nb, K=K, terms=terms, meas=True)
     print(f'[model-shapes] kp2dm step P={3 * n_rot + nb + 3} nb={nb} K={K} first={first} terms={terms}: '
           f'trial error / bar {worst:.3f}')
 
 
-def _group_case(n_rot, nb, K, terms, sizes):
-    """test_gpu_fit_lm_kp2d_groups._group_case's cases on random Jacobians at (n_rot, nb): groups of `sizes` images,
-    group 0 targets the trial (accepted), 1 the state with the priors on its side and a trial 0.5 away (rejected), 2 the
-    trial (accepted), the rest noisy targets.  With K >= 8 keypoint 7 has weight 0 and NaN targets, keypoints and rows
-    in state and trial; measurement 2 of group 2 (of the last group when there are fewer) is dropped with NaN values
-    and rows."""
-    sigma, pw, bw = terms
-    G, B, P = len(sizes), sum(sizes), 3 * n_rot + nb + 3
-    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
-    gidx = torch.repeat_interleave(torch.arange(G), torch.tensor(sizes))
-    gen = torch.Generator().manual_seed(1000 * n_rot + 10 * nb + K + B + (3 if pw else 0))
-    rn = lambda *s: torch.randn(*s, generator=gen)  # noqa: E731
-    rot = _rodrigues(rn(B, n_rot, 3).double() * 0.5).float()
-    trot = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.05)).float()
-    anchor = (rot.double() @ _rodrigues(rn(B, n_rot, 3).double() * 0.1)).float()
-    betas, cam = rn(G, nb), rn(B, 3) * torch.tensor([0.5, 0.1, 0.1])
-    tbetas, tcam = betas + 0.05 * rn(G, nb), cam + 0.01 * rn(B, 3)
-    kp, jac = rn(B, K, 3), rn(B, 3 * K, P)
-    tkp, tjac = kp + 0.05 * rn(B, K, 3), jac + 0.1 * rn(B, 3 * K, P)
-    m, mj = torch.rand(G, 5, generator=gen) + 0.5, rn(G, 5, nb)
-    tm, tmj = m + 0.01 * rn(G, 5), mj + 0.1 * rn(G, 5, nb)
-    proj = lambda k, c: torch.stack([torch.from_numpy(o2.project(k[b].numpy(), c[b].numpy())).float()  # noqa: E731
-                                     for b in range(k.shape[0])])
-    tg = proj(kp, cam) + 0.05 * rn(B, K, 2)
-    mt = m + 0.02 * rn(G, 5)
-    for g, to_trial in zip(range(G), (True, False, True)):
-        r = slice(off[g], off[g + 1])
-        if to_trial:
-            kp[r] = tkp[r] + 0.5
-            tg[r], anchor[r], tbetas[g], mt[g] = proj(tkp[r], tcam[r]), trot[r], 0.9 * betas[g], tm[g]
-        else:
-            tkp[r] = kp[r] + 0.5
-            tg[r], anchor[r], tbetas[g], mt[g] = proj(kp[r], cam[r]), rot[r], 1.1 * betas[g], m[g]
-    w = torch.rand(B, K, generator=gen) + 0.5
-    if K >= 8:
-        w[:, 7] = 0.0
-        tg[:, 7] = float('nan')
-        for t in (kp, tkp):
-            t[:, 7] = float('nan')
-        for t in (jac, tjac):
-            t[:, 21:24] = float('nan')
-    mw = torch.rand(G, 5, generator=gen) * 2 + 0.5
-    gd = min(2, G - 1)
-    mw[gd, 2] = 0.0
-    for t in (m, tm, mj, tmj):
-        t[gd, 2] = float('nan')
-    return dict(off=off, gidx=gidx, rot=rot, betas=betas, cam=cam, kp=kp, jac=jac, meas=m, mjac=mj, trot=trot,
-                tbetas=tbetas, tcam=tcam, tkp=tkp, tjac=tjac, tmeas=tm, tmjac=tmj, tg=tg, w=w, mt=mt, mw=mw,
-                anchor=anchor, lam=torch.rand(G, generator=gen) + 0.01, sigma=sigma, pw=pw, bw=bw)
-
-
 @pytest.mark.parametrize('with_meas', [False, True], ids=['kp2dg', 'kp2dgm'])
 @pytest.mark.parametrize('layout', list(LAYOUTS))
-@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('K', GROUP_K)
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_groups_step_vs_oracle(n_rot, nb, K, first, terms, layout, with_meas):
     """Both grouped entries against kp2dg_lm_oracle: groups (1, 2, 3, 5), an irregular layout whose image kernel finds
     the groups of 1, 7, 1, 33 and 2 images by its binary search, and one group of 64 images."""
-    c = _group_case(n_rot, nb, K, terms, LAYOUTS[layout])
-    state, trial, _, G = grp._device(c, with_meas)
+    c = harness.random_group_case(n_rot, nb, K, terms, LAYOUTS[layout])
+    state, trial, _, G = harness.groups_device(c, with_meas)
     s0 = {k: v.cpu().numpy() for k, v in state.items()}
-    grp._groups_step(c, state, trial, first, with_meas)
-    flags, worst = grp._check_vs_oracle(c, s0, state, trial, first, with_meas)
+    harness.groups_step(c, state, trial, first, with_meas)
+    flags, worst = harness.check_groups_vs_oracle(c, s0, state, trial, first, with_meas)
     if first:
         assert all(flags)
     else:
@@ -510,18 +334,18 @@ def test_groups_step_vs_oracle(n_rot, nb, K, first, terms, layout, with_meas):
           f'layout={layout} first={first} terms={terms}: trial error / bar {worst:.3f}')
 
 
-@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_groups_of_one_equal_the_2d_step(n_rot, nb, first, terms):
-    grp._check_groups_of_one(_group_case(n_rot, nb, 9, terms, (1,) * 6), first)
+    harness.check_groups_of_one(harness.random_group_case(n_rot, nb, 9, terms, (1,) * 6), first)
 
 
-@pytest.mark.parametrize('terms', kp2d.TERMS, ids=['lsq', 'robust_priors'])
+@pytest.mark.parametrize('terms', TERMS, ids=['lsq', 'robust_priors'])
 @pytest.mark.parametrize('first', [False, True])
 @pytest.mark.parametrize('n_rot,nb', STEP_SHAPES)
 def test_dropped_measurements_equal_the_plain_groups_step(n_rot, nb, first, terms):
-    grp._check_dropped_measurements(_group_case(n_rot, nb, 9, terms, (1, 2, 3, 5)), first)
+    harness.check_dropped_measurements(harness.random_group_case(n_rot, nb, 9, terms, (1, 2, 3, 5)), first)
 
 
 GUARD = 64                        # sentinel elements on each side of a guarded output: 256 bytes, the alignment kept
@@ -545,14 +369,14 @@ def test_steps_write_nothing_outside_their_outputs(n_rot, nb, entry):
     shapy_fit_lm_groups_workspace_bytes and every input keep their bits, and the outputs equal those of unguarded
     tensors bit for bit."""
     from shapy_b200 import _lib
-    terms, K = kp2d.TERMS[1], 9
+    terms, K = TERMS[1], 9
     keys = ['tg', 'w', 'anchor', 'tkp', 'tjac'] + ([] if entry == 'kp2dg' else ['mt', 'mw', 'tmeas', 'tmjac'])
     if entry == 'kp2dm':
-        c = kp2d._step_case(n_rot, nb, K, terms, meas=True)
-        state, trial = kp2d._device(c)
+        c = harness.kp2d_case(n_rot, nb, K, terms, meas=True)
+        state, trial = harness.kp2d_device(c)
     else:
-        c = _group_case(n_rot, nb, K, terms, (1, 2, 3, 5))
-        state, trial, B, G = grp._device(c, entry == 'kp2dgm')
+        c = harness.random_group_case(n_rot, nb, K, terms, (1, 2, 3, 5))
+        state, trial, B, G = harness.groups_device(c, entry == 'kp2dgm')
         need = _lib.lib().shapy_fit_lm_groups_workspace_bytes(B, G, n_rot, nb)
         wbuf = torch.full((need // 4 + 1 + GUARD,), SENTINEL, dtype=torch.int32, device='cuda')
         ws = wbuf.view(torch.uint8)[:need]
@@ -564,19 +388,19 @@ def test_steps_write_nothing_outside_their_outputs(n_rot, nb, entry):
     for first in (True, False):
         a_st, a_tr = {k: v[0] for k, v in g_state.items()}, {k: v[0] for k, v in g_trial.items()}
         if entry == 'kp2dm':
-            kp2d._step(cd, a_st, a_tr, first)
-            kp2d._step(cd, state, trial, first)
+            harness.kp2d_step(cd, a_st, a_tr, first)
+            harness.kp2d_step(cd, state, trial, first)
         else:
-            grp._groups_step(cd, a_st, a_tr, first, entry == 'kp2dgm', ws)
-            grp._groups_step(cd, state, trial, first, entry == 'kp2dgm')
+            harness.groups_step(cd, a_st, a_tr, first, entry == 'kp2dgm', ws)
+            harness.groups_step(cd, state, trial, first, entry == 'kp2dgm')
     torch.cuda.synchronize()
     for what, gd, ref in (('state', g_state, state), ('trial', g_trial, trial)):
         for k, (v, buf) in gd.items():
             n = v.numel()
             assert bool((buf[:GUARD] == SENTINEL).all()) and bool((buf[GUARD + n:] == SENTINEL).all()), (what, k)
-            assert torch.equal(_bits(v), _bits(ref[k])), (what, k)
+            assert torch.equal(bits(v), bits(ref[k])), (what, k)
     for k in keys:
-        assert torch.equal(_bits(cd[k]), _bits(inputs[k])), k
+        assert torch.equal(bits(cd[k]), bits(inputs[k])), k
     if entry != 'kp2dm':
         assert torch.equal(wbuf.view(torch.uint8)[need:], tail)
 
@@ -611,7 +435,7 @@ def test_lm_fit(packed, name):
     from shapy_b200 import ops
     from shapy_b200.fit import fit_body_to_keypoints
     NB, NE, _ = VARIANTS[name]
-    module = _module(name)
+    module = harness.smplx_module(name)
     bm, kw = None, {}
     if FIT_CASES[name]:
         from shapy_b200.body_measurements import BodyMeasurements
@@ -642,26 +466,21 @@ def test_lm_fit(packed, name):
     res8 = fit(kp[rows].contiguous(), kw8)
     keys = ('global_rot', 'body_pose', 'betas', 'transl') + (('measurements',) if bm is not None else ())
     for k in keys:
-        assert torch.equal(_bits(res8[k]), _bits(res[k][rows])), k
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        fit(kp, kw, iterations=3)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+        assert torch.equal(bits(res8[k]), bits(res[k][rows])), k
+    harness.launches_without_sync(lambda: fit(kp, kw, iterations=3))
     # the Jacobian and the backward twice on the same inputs
     pk = packed(name)
-    x = _inputs(99, B, 22, NB, NE)
+    x = harness.inputs(99, B, 22, NB, NE)
     c = lambda t: None if t is None else t.cuda()  # noqa: E731
     j1, j2 = (ops.smplx_keypoint_jacobian(pk, c(x['betas']), c(x['rot']), c(x['transl'])) for _ in range(2))
-    assert all(torch.equal(_bits(a), _bits(b)) for a, b in zip(j1, j2))
+    assert all(torch.equal(bits(a), bits(b)) for a, b in zip(j1, j2))
     gen = torch.Generator().manual_seed(100)
     cot = dict(grad_vertices=torch.randn(B, pk.V, 3, generator=gen).cuda(),
                grad_joints=torch.randn(B, pk.K, 3, generator=gen).cuda(),
                grad_v_shaped=torch.randn(B, pk.V, 3, generator=gen).cuda())
     g1, g2 = (ops.smplx_backward(pk, c(x['betas']), c(x['rot']), expr=c(x['expression']), **cot) for _ in range(2))
     for k in ('betas', 'rot', 'expr'):
-        assert torch.equal(_bits(g1[k]), _bits(g2[k])), k
+        assert torch.equal(bits(g1[k]), bits(g2[k])), k
 
 
 def _fit_problem_2d(module, NB, G, views, bm=None, seed=33):
@@ -695,7 +514,7 @@ def test_lm_fit_2d(name, grouped):
     a sub-batch of whole groups gives the batch's rows bit for bit, and the loop never synchronises."""
     from shapy_b200.fit import fit_body_to_keypoints_2d
     NB = VARIANTS[name][0]
-    module = _module(name)
+    module = harness.smplx_module(name)
     bm = None
     if FIT_CASES[name]:
         from shapy_b200.body_measurements import BodyMeasurements
@@ -736,12 +555,7 @@ def test_lm_fit_2d(name, grouped):
     a = args(ids)
     sub, rows = fit(a), a[2]
     for k in ('global_rot', 'body_pose', 'camera'):
-        assert torch.equal(_bits(sub[k]), _bits(res[k][rows])), k
+        assert torch.equal(bits(sub[k]), bits(res[k][rows])), k
     for k in ('betas',) + (('measurements',) if bm is not None else ()) + (('loss',) if grouped else ()):
-        assert torch.equal(_bits(sub[k]), _bits(res[k][ids])), k
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
-        fit(every, iterations=3)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
+        assert torch.equal(bits(sub[k]), bits(res[k][ids])), k
+    harness.launches_without_sync(lambda: fit(every, iterations=3))

@@ -1,7 +1,7 @@
 """CPU: the model variants of the shape tests (tests/test_gpu_model_shapes.py) and the float64 restatements at their
 shapes, before the GPU kernels are compared with them.
 
-Variants of synth.make_smplx() (shape and expression rows randn * 5e-3 seeded as in
+Variants of synth.make_smplx(), defined in tests/lm_harness.py (shape and expression rows randn * 5e-3 seeded as in
 test_gpu_smplx_poses.test_shape_expression_counts, J14 rows seeded random supports with softmax weights as in
 synth.make_smplx's sparse_rows):
 
@@ -21,7 +21,6 @@ synth.make_smplx's sparse_rows):
     measurement row's outer product have one entry)
   * fit_body_to_keypoints(method='lm') and fit_body_to_keypoints_2d(method='lm') refuse more than 96 parameters before
     they touch the device"""
-import functools
 import math
 
 import numpy as np
@@ -31,65 +30,10 @@ import torch
 import kp2d_lm_oracle as o2
 import kp2dg_lm_oracle as og
 import kp_lm_oracle
+from lm_harness import KP_CACHE_ENTRIES, VARIANTS, keypoint_entries, keypoints_at, rodrigues, variant_model
 from shapy_b200 import synth
-from test_fit_lm_keypoints_cpu import _keypoints, _rodrigues
 
-KP_CACHE_ENTRIES = 2048           # kKpCacheEntries of smplx.cu: keypoint entries the Jacobian caches in shared memory
 LM_KP_MAX_P = 96                  # kLmKpMaxP of fit.cu
-# name -> (NB, NE, J14 non-zeros per row or None for synth.make_smplx's own 14 x 32)
-VARIANTS = {
-    'nb1_ne0': (1, 0, None),
-    'nb10_ne0': (10, 0, None),
-    'nb16_ne16': (16, 16, None),
-    'nb27_ne5_dense': (27, 5, [150] * 14),
-    'edge_2048': (10, 10, [132] * 13 + [128]),
-    'edge_2049': (10, 10, [132] * 13 + [128]),
-}
-EDGE_EXTRA = 0.02                 # the weight of edge_2049's added non-zero
-
-
-@functools.lru_cache(maxsize=None)
-def _base():
-    return synth.make_smplx()
-
-
-def _j14(seed, counts):
-    V = synth.NUM_VERTS
-    g = torch.Generator().manual_seed(seed)
-    R = torch.zeros(len(counts), V)
-    for r, n in enumerate(counts):
-        idx = torch.randperm(V, generator=g)[:n]
-        R[r, idx] = torch.softmax(torch.randn(n, generator=g), 0)
-    return R
-
-
-@functools.lru_cache(maxsize=None)
-def _variant(name):
-    NB, NE, counts = VARIANTS[name]
-    m = dict(_base())
-    V = m['v_template'].shape[0]
-    g = torch.Generator().manual_seed(NB * 100 + NE)
-    m['shapedirs'] = torch.randn(V, 3, NB, generator=g) * 5e-3
-    m['expr_dirs'] = torch.randn(V, 3, NE, generator=g) * 5e-3      # (V, 3, 0) when NE = 0: no expression basis
-    if counts is not None:
-        R = _j14(sum(counts), counts)
-        if name == 'edge_2049':
-            free = [int(v) for v in torch.randperm(V, generator=torch.Generator().manual_seed(5)) if R[-1, v] == 0]
-            R[-1, free[0]] = EDGE_EXTRA
-        m['extra_joint_regressor'] = R
-    return m
-
-
-def variant_model(name):
-    """A fresh dict of the variant's tensors (the tensors are shared: do not edit them in place)."""
-    return dict(_variant(name))
-
-
-def keypoint_entries(m, use_face_contour=True):
-    """3 (L + D) + nnz(J14): the entry count the keypoint Jacobian compares with KP_CACHE_ENTRIES."""
-    L = m['lmk_faces_idx'].shape[0]
-    D = m['dynamic_lmk_faces_idx'].shape[1] if use_face_contour else 0
-    return 3 * (L + D) + int((m['extra_joint_regressor'] != 0).sum())
 
 
 # ------------------------------------------------------------------------------------------------ variants
@@ -125,13 +69,13 @@ def test_oracle_jacobian_vs_central_differences(name):
     n_rot = 22
     P = 3 * n_rot + NB + 3
     for b, neck in enumerate((1.2, -1.2)):                 # necks turned past both ends of the contour LUT
-        rot = _rodrigues(torch.randn(n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
-        rot[12] = _rodrigues(torch.tensor([0.0, neck, 0.0])).float()
+        rot = rodrigues(torch.randn(n_rot, 3, generator=gen, dtype=torch.float64) * 0.4).float()
+        rot[12] = rodrigues(torch.tensor([0.0, neck, 0.0])).float()
         betas = torch.randn(NB, generator=gen)
         transl = torch.randn(3, generator=gen) * 0.1
         kp, jac = kp_lm_oracle.keypoint_jacobian(model, betas, rot, transl)
         assert jac.shape == (3 * 123, P) and kp.shape == (123, 3)
-        base = _keypoints(model, betas, rot, transl, torch.zeros(1, P, dtype=torch.float64))[0].numpy()
+        base = keypoints_at(model, betas, rot, transl, torch.zeros(1, P, dtype=torch.float64))[0].numpy()
         assert np.abs(kp - base).max() <= 1e-9 * np.abs(base).max()
         h = 1e-5
         fd = []
@@ -139,7 +83,7 @@ def test_oracle_jacobian_vs_central_differences(name):
             e = torch.zeros(2 * len(half), P, dtype=torch.float64)
             for i, c in enumerate(half):
                 e[2 * i, c], e[2 * i + 1, c] = h, -h
-            y = _keypoints(model, betas, rot, transl, e).reshape(len(half), 2, -1).numpy()
+            y = keypoints_at(model, betas, rot, transl, e).reshape(len(half), 2, -1).numpy()
             fd.append(((y[:, 0] - y[:, 1]) / (2 * h)).T)
         fd = np.concatenate(fd, 1)
         for block, cols in (('rot', slice(0, 3 * n_rot)), ('betas', slice(3 * n_rot, 3 * n_rot + NB)),
@@ -390,7 +334,7 @@ def test_oracle_groups_step_vs_dense_block_arrow_solve(n_rot, nb, sigma, pose_w,
 def _nb28_module():
     """An SMPLX module on the CPU with NB = 28, NE = 4 (NC = 32)."""
     from shapy_b200.human_shape.models.body_models.body_models import SMPLX
-    m = dict(_base())
+    m = dict(synth.make_smplx())
     g = torch.Generator().manual_seed(2800)
     m['shapedirs'] = torch.randn(m['v_template'].shape[0], 3, 28, generator=g) * 5e-3
     m['expr_dirs'] = m['expr_dirs'][:, :, :4]

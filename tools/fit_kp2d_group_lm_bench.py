@@ -81,7 +81,8 @@ def kernels(B, reps, module):
 
 def time_to_quality(module, bm):
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    from test_gpu_fit_lm_kp2d_groups import _problem, quality
+    from lm_harness import quality_groups as quality
+    from test_gpu_fit_lm_kp2d_groups import _problem
     p = _problem(module, bm, 64)
     gm = {k: p['tg'][k] for k in ('height', 'mass')}
     arms = (('per_image_lm_50', {}, False),

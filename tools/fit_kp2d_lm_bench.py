@@ -95,8 +95,9 @@ def kernels(B, reps):
 def time_to_quality():
     from shapy_b200.fit import fit_body_to_keypoints_2d
     from shapy_b200.metrics import PointError, build_alignment
-    from test_gpu_fit_lm_keypoints_2d import RMS_THRESHOLD, _get, _problem, _rms2d
-    module = _get()
+    from lm_harness import smplx_module
+    from test_gpu_fit_lm_keypoints_2d import RMS_THRESHOLD, _problem, _rms2d
+    module = smplx_module()
     x, joints, init = _problem(module, 256)
     for m in ('lm', 'adam'):                                     # warm-up
         fit_body_to_keypoints_2d(module, x, init=init, method=m, iterations=2)

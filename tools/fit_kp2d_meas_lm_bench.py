@@ -83,7 +83,8 @@ def kernels(B, reps, module, bm):
 
 def time_to_quality(module, bm):
     from shapy_b200.fit import fit_body_to_keypoints_2d
-    from test_gpu_fit_lm_kp2d_meas import N_ROT, _problem, quality
+    from lm_harness import N_ROT, quality_2d as quality
+    from test_gpu_fit_lm_kp2d_meas import _problem
     p = _problem(module, bm, 256)
     hm = {k: p['tg'][k] for k in ('height', 'mass')}
     arms = (('kp2d_lm_50', {}),
