@@ -65,12 +65,13 @@ struct WgmmaPlan;
 // by the planner's cost model (cooperative everywhere with SHAPY_CONV_PINGPONG=0) unless COOP or PINGPONG is or-ed in
 // (PINGPONG then limits the cout tile to what its accumulators fit).  AUTO takes the weight-resident halo path (weights
 // loaded once per CTA, 16-channel operand slices) where it fits, unless SHAPY_CONV_RESIDENT=0; RESIDENT forces it and
-// fails on a layer it cannot hold.
+// fails on a layer it cannot hold.  nt != 0 forces the cout tile (measurement of the planner's alternatives; fails
+// where no kernel runs that tile).
 enum WgmmaPath { WGMMA_AUTO = 0, WGMMA_PER_TAP = 1, WGMMA_HALO = 2, WGMMA_COOP = 4, WGMMA_PINGPONG = 8,
                  WGMMA_RESIDENT = 16 };
 bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out);
 WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
-                             int path = WGMMA_AUTO);
+                             int path = WGMMA_AUTO, int nt = 0);
 #ifdef SHAPY_CONV_STAMPS
 void wgmma_stamps_reset();
 void wgmma_stamps_print(const WgmmaPlan *p);

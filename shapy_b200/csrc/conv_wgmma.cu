@@ -42,10 +42,12 @@
 // with the TMA swizzle of their rows, so the 16-byte matrix rows and the TMA accesses are free of bank conflicts.
 // Replaces cuDNN conv + BatchNorm + ReLU + residual add (4 launches, 4 HBM round trips) of
 // regressor/human_shape/models/backbone/hrnet.py and torchvision BasicBlock / Bottleneck.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
 #include <type_traits>
 
 #include "conv.cuh"
@@ -609,17 +611,22 @@ bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out) {
 }
 
 WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &out, const ActView *res, bool relu,
-                             int path) {
+                             int path, int nt) {
   if (!wgmma_supported(w, in, out)) {
     set_error("wgmma_plan_create: unsupported convolution (cin %d cout %d k %d s %d)", w.cin, w.cout, w.ksize, w.stride);
     return nullptr;
   }
   const int data_path = path & (WGMMA_PER_TAP | WGMMA_HALO | WGMMA_RESIDENT);
   const int sched = path & (WGMMA_COOP | WGMMA_PINGPONG);
+  const bool split = in.lo != nullptr;
+  if (nt && (std::find(std::begin(kNts), std::end(kNts), nt) == std::end(kNts) || w.cout % nt || (split && nt > 96) ||
+             (sched == WGMMA_PINGPONG && !pingpong_fits(split, nt)) || (data_path == WGMMA_RESIDENT && nt != w.cout))) {
+    set_error("wgmma_plan_create: no kernel for cout tile %d (cin %d cout %d, split %d)", nt, w.cin, w.cout, (int)split);
+    return nullptr;
+  }
   auto *pl = new WgmmaPlan();
   memset(&pl->p, 0, sizeof(pl->p));
   WgmmaParams &p = pl->p;
-  const bool split = in.lo != nullptr;
   const int PARTS = split ? 2 : 1;
   pl->split = split;
   const int sms = sm_count();
@@ -666,39 +673,34 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
     }
   }
   {
-    // cout tile: balance SM utilisation (tiles per CTA round) against the per-wgmma operand cost.  A 128-row tile is two
-    // m64nNk16 per k-step; each reads 2 KB of A and N x 32 B of B from shared memory (128 B/cycle) and needs N / 2
-    // tensor cycles, plus a fixed per-tile epilogue / barrier cost.
+    // Cout tile and consumer schedule: the pair of least modelled time, the model fitted to the launch times of every
+    // candidate of every HRNet layer in both modes (tools/conv_plan_sweep.py, H100 SXM at 700 W, README).  One k16 step
+    // of a 128-row tile is two m64nNk16 (split: N = 2 NT and N = NT), each the larger of its shared-memory operand reads
+    // (2 KB of A and N x 32 B of B at 128 B/cycle) and N / 2 tensor cycles, plus 32 cycles of issue, over the k16 steps
+    // actually issued; a tile adds 1 000 cycles of operand wait, drain and staged epilogue.  Cooperative: each wave of
+    // tiles pays mainloop + epilogue.  Ping-pong: a consumer's epilogue runs under the other's mainloop, so a wave pays
+    // the larger of the two, plus one exposed epilogue.  One consumer issuing both m64 halves takes sqrt(64 / NT) x the
+    // cooperative mainloop in split mode, 0.3 x more on the halo path with several channel blocks (c96, c192: the
+    // consumers' tiles alternate over the 2-slot halo ring), and 0.9 x in fp16.  Waves count whole: a partial wave costs
+    // a full tile in the measured launches (384 -> 384 @7² fp16: NT 32 at 1.45 waves takes 1.8 x NT 48 at 0.97).
     const double m_tiles = (double)p.tiles_w * p.tiles_h * p.tiles_n;
-    auto mma_cyc = [](double n) { return 2.0 * std::max((2048.0 + 32.0 * n) / 128.0, n * 0.5); };
-    auto main_cyc = [&](int nt) {
-      return (split ? mma_cyc(2.0 * nt) + mma_cyc(nt) : mma_cyc(nt)) * w.ksize * w.ksize * p.kpt * (KCH / 16);
+    const int steps = w.ksize * w.ksize * ((p.kpt - 1) * (KCH / 16) + p.ks_last);
+    auto mma_cyc = [](double n) { return 2.0 * std::max((2048.0 + 32.0 * n) / 128.0, n * 0.5) + 32.0; };
+    auto main_cyc = [&](int c) { return (split ? mma_cyc(2.0 * c) + mma_cyc(c) : mma_cyc(c)) * steps; };
+    auto rounds = [&](int c) { return std::ceil(m_tiles * (w.cout / c) / sms); };
+    const double epi = 1000.0;
+    const double pp_halo = pl->halo && p.kpt > 1 ? 0.3 : 0.0;
+    auto coop_cost = [&](int c) { return rounds(c) * (main_cyc(c) + epi); };
+    auto pp_cost = [&](int c) {
+      const double slow = split ? std::sqrt(64.0 / c) + pp_halo : 0.9;
+      return rounds(c) * std::max(slow * main_cyc(c), epi) + epi;
     };
-    auto rounds = [&](int nt) { return std::ceil(m_tiles * (w.cout / nt) / sms); };
+    const bool pp_ok = sched == WGMMA_PINGPONG || (sched == 0 && pingpong_enabled());
     double best = 1e30;
-    int best_nt = 0;
-    for (int nt : kNts) {
-      if (w.cout % nt || (split && nt > 96)) continue;   // split: 3 NT / 2 accumulators per thread must fit 232 registers
-      const double cost = rounds(nt) * (main_cyc(nt) + 400.0 * nt / 16);
-      if (cost < best) { best = cost; best_nt = nt; }
-    }
-    // Schedule, from the cycle stamps of tools/conv_phase_stamps.py (H100 SXM, README): the per-tile cost outside the
-    // mainloop (epilogue, drain, refill) is ~100 cycles per cout in split mode and ~72 in fp16; one consumer issuing
-    // both m64 halves takes 1.25-1.6x (split) / 1.0-1.1x (fp16) the mainloop time of two consumers issuing one each.  The
-    // cooperative schedule pays mainloop + epilogue per tile, the ping-pong one the larger of the two (the epilogue
-    // runs under the other consumer's mainloop) and one exposed epilogue at the end.  The planner only weighs ping-pong
-    // at the cooperative cout tile: smaller tiles re-load the activations per cout tile and measured slower.
-    const double epi_c = split ? 100.0 : 72.0, pp_slow = split ? 1.3 : 1.1;
-    auto pp_cost = [&](int nt) { return rounds(nt) * std::max(pp_slow * main_cyc(nt), epi_c * nt) + epi_c * nt; };
-    if (sched == WGMMA_PINGPONG) {               // forced: the cheapest cout tile whose accumulators fit
-      double c = 1e30;
-      for (int nt : kNts)
-        if (w.cout % nt == 0 && pingpong_fits(split, nt) && pp_cost(nt) < c) { c = pp_cost(nt); pl->NT = nt; }
-      pl->pingpong = true;
-    } else {
-      pl->NT = best_nt;
-      pl->pingpong = sched == 0 && pingpong_enabled() && pingpong_fits(split, best_nt) &&
-                     pp_cost(best_nt) < rounds(best_nt) * (main_cyc(best_nt) + epi_c * best_nt);
+    for (int c : kNts) {
+      if (w.cout % c || (split && c > 96) || (nt && c != nt)) continue;   // split: 3 NT / 2 accumulators per thread must fit 232 registers
+      if (sched != WGMMA_PINGPONG && coop_cost(c) < best) { best = coop_cost(c); pl->NT = c; pl->pingpong = false; }
+      if (pp_ok && pingpong_fits(split, c) && pp_cost(c) < best) { best = pp_cost(c); pl->NT = c; pl->pingpong = true; }
     }
   }
   // Weight-resident path: a halo layer with one cout tile (kernels exist for cout 48 and 64) and cin <= 64, in 16-channel
@@ -784,7 +786,7 @@ WgmmaPlan *wgmma_plan_create(const ConvW &w, const ActView &in, const ActView &o
       delete pl;
       return nullptr;
     }
-    pl->pingpong = false;                         // the planner's choice is always at the cooperative cout tile
+    pl->pingpong = false;                         // the cooperative schedule at the same cout tile
     if (!plan_smem()) {
       set_error("wgmma_plan_create: no room for the ring and the staging box (cin %d cout %d %dx%d)", w.cin, w.cout,
                 out.H, out.W);

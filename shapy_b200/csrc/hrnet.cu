@@ -528,13 +528,13 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
   if (engine != 1) {
-    // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo, 4 = weight-resident halo; engine / 10:
-    // 0 = the planner's schedule, 1 = cooperative, 2 = ping-pong
-    const int e_path = engine % 10, e_sched = engine / 10;
+    // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo, 4 = weight-resident halo; engine / 10 %
+    // 10: 0 = the planner's schedule, 1 = cooperative, 2 = ping-pong; engine / 100: the cout tile (0 = the planner's)
+    const int e_path = engine % 10, e_sched = engine / 10 % 10, e_nt = engine / 100;
     const int path = (e_path == 2 ? WGMMA_PER_TAP
                                   : (e_path == 3 ? WGMMA_HALO : (e_path == 4 ? WGMMA_RESIDENT : WGMMA_AUTO))) |
                      (e_sched == 1 ? WGMMA_COOP : (e_sched == 2 ? WGMMA_PINGPONG : 0));
-    plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path);
+    plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path, e_nt);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }
     rc = wgmma_plan_launch(plan, st, true);
     if (const char *reps_s = getenv("SHAPY_CONV_TEST_REPS")) {

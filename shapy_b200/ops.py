@@ -989,7 +989,7 @@ def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=
     """Single convolution through either engine on fp32 NHWC tensors (unit tests).  engine: 0 = wgmma with the path
     the network would take, 1 = SIMT, 2 = wgmma per-tap path, 3 = wgmma halo-resident path, 4 = wgmma halo path with
     the weights resident in shared memory; + 10 forces the
-    cooperative consumer schedule of the wgmma engine, + 20 the ping-pong one."""
+    cooperative consumer schedule of the wgmma engine, + 20 the ping-pong one; + 100 * NT forces its cout tile NT."""
     x = _cuda_f32(x_nhwc, 'x')
     B, H, W, Cin = x.shape
     Cout, _, k, _ = weight.shape
