@@ -157,6 +157,18 @@ int shapy_smplx_keypoint_jacobian_expr(const shapy_smplx_t *m, const float *beta
                                        int n_rot, const float *transl, int batch, float *keypoints, float *jac,
                                        void *stream);
 
+/* Every posed vertex and its Jacobian, for the dense fits: betas (B,NB), rot (B,n_rot,3,3), transl (B,3) or NULL
+ * (zero); outputs vertices (B,V,3) and jac (B,V,3,P) fp32, row 3 v + c the c coordinate of vertex v, with the columns
+ * of shapy_smplx_keypoint_jacobian (P = 3 n_rot + NB + 3: delta_j, betas, transl) and its semantics (v_posed from the
+ * fp32 posedirs rows, the model buffers constants); a barycentric mix of three vertices' rows is the keypoint
+ * Jacobian's row of a landmark on that face up to fp32 rounding, and the vertices agree with shapy_smplx_forward to
+ * fp32 rounding.  The output is large: 4 V 3 P bytes per body, 9.9 MB at V = 10475 and P = 79 (635 MB at B = 64).
+ * One CTA per (tile of 32 vertices, body), each recomputing its body's kinematic chain.  No atomics: a body's result is
+ * bit-identical from run to run and independent of the rest of the batch.  1 <= n_rot <= J, B <= 65535 (SHAPY_ERR_ARG
+ * otherwise); batch 0: no launch. */
+int shapy_smplx_vertex_jacobian(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
+                                const float *transl, int batch, float *vertices, float *jac, void *stream);
+
 /* Adjoint of shapy_decode_rot6d: grad_raw (n, 6) from raw (n, 6) and grad_rot (n, 3, 3), elementwise.  The 1e-12
  * clamp of each norm passes gradient to the norm only where the norm is >= 1e-12 (torch's clamp_min). */
 int shapy_decode_rot6d_backward(const float *raw, int n, const float *grad_rot, float *grad_raw, void *stream);
@@ -597,6 +609,44 @@ size_t shapy_nearest_points_workspace_bytes(int batch, int num_points);
 int shapy_nearest_points(const float *queries, int batch, int num_queries, const float *points, int num_points,
                          const float *weights, int32_t *idx, float *sq_dist, void *workspace, size_t workspace_bytes,
                          void *stream);
+
+/* One Levenberg-Marquardt step per body of the fit of pose, shape and translation to 3D scans, with the policy,
+ * lambda constants, Cholesky and rotation update of shapy_fit_lm_keypoints_step.  Parameters [delta_j (3 n_rot) | beta
+ * (nb) | t], the columns of shapy_smplx_vertex_jacobian, P = 3 n_rot + nb + 3 <= 96 (SHAPY_ERR_UNSUPPORTED past that).
+ * Inputs: points (B,N,3) and weights (B,N) (a point with weight <= 0 is dropped and never read: it may be NaN), faces
+ * (F,3); the trial's vertices (B,V,3) and jac (B,V,3,P) of shapy_smplx_vertex_jacobian (with transl), its closest
+ * points trial_face_idx / trial_bary (B,N) / (B,N,3) of shapy_closest_points, and trial_nearest (B,V) of
+ * shapy_nearest_points (NULL when model_to_scan_weight is 0).  Loss per body, fp64, left to right:
+ *   s2m / W sum_{w_i > 0} w_i rho(d_i^2) + m2s / V sum_v rho(e_v^2) + pose_w / 2 sum_{j >= 1} |R_j - anchor_j|_F^2
+ *   + the measurement terms of shapy_fit_lm_keypoints_2d_measurements_step + betas_w |beta|^2,
+ * W = sum_{w_i > 0} w_i (1 when 0), d_i = |c_i - p_i|, c_i = sum_k bary_ik x_{f_i,k} the trial's closest point, e_v =
+ * |x_v - p_{nearest_v}| (a vertex without a nearest point adds nothing), rho the Geman-McClure e s^2 / (s^2 + e) at
+ * robust_sigma s, the identity at s = inf.  Rows at the held correspondences, each with the IRLS weight rho'(.) (times
+ * w_i s2m / W or m2s / V): a point whose barycentrics are all > 0 on a face of non-zero area gives one point-to-plane
+ * row n^T (c_i - p_i), n the face's unit normal held constant; any other kept point three point-to-point rows
+ * c_i - p_i; a vertex three rows x_v - p_{nearest_v}; then the chordal pose-prior rows, the measurement rows and
+ * betas_w.  Two launches: the rows in fp64 by chunks of 1024 points or vertices per CTA into workspace (>=
+ * shapy_fit_lm_scan_workspace_bytes(B, N, V, P)), then one CTA per body sums the chunks in chunk order.  The state:
+ * rot (B,n_rot,3,3), betas (B,nb), transl (B,3), normal_matrix (B,P,P) and gradient (B,P) fp64, the undamped data
+ * rows J^T W J and J^T W r at the state, loss, lambda, accepted; with measurements (meas_targets, meas_weights, meas,
+ * meas_jac, trial_meas, trial_meas_jac all non-NULL, as in shapy_fit_lm_keypoints_2d_measurements_step; all NULL
+ * without) meas (B,5) and meas_jac (B,5,nb).  On accept the trial's parameters, data rows and measurements become the
+ * state.  The first lambda reads the data rows' diagonal.  A body whose loss is not finite, or whose factorisation
+ * fails, gets its state as the trial.  With every measurement weight <= 0 the outputs equal the step without
+ * measurements bit for bit.  Deterministic, no atomics, a body's result independent of the rest of the batch.  A null
+ * pointer, a bad size, robust_sigma <= 0 or NaN, a negative or non-finite term weight, a negative prior weight, a
+ * lambda factor < 1 or a small workspace: SHAPY_ERR_ARG.  batch 0: no launch. */
+size_t shapy_fit_lm_scan_workspace_bytes(int batch, int num_points, int num_verts, int num_params);
+int shapy_fit_lm_scan_step(int batch, int num_points, int num_verts, int n_rot, int nb, const float *points,
+                           const float *weights, const int32_t *faces, const float *pose_anchor, float robust_sigma,
+                           float scan_to_model_weight, float model_to_scan_weight, float pose_prior_weight,
+                           float betas_weight, const float *meas_targets, const float *meas_weights, float lambda_up,
+                           float lambda_down, int first, float *rot, float *betas, float *transl,
+                           double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss,
+                           float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+                           const float *trial_vertices, const float *trial_jac, const int32_t *trial_face_idx,
+                           const float *trial_bary, const int32_t *trial_nearest, const float *trial_meas,
+                           const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream);
 
 /* Backward of sq_dist of shapy_closest_points with respect to the vertices, face_idx and bary held at the forward's
  * values: grad_vertices (B,V,3) = sum over the points of 2 g_i (q_i - p_i) bary_{i,c} at corner c of face_idx_i, q_i =

@@ -2064,6 +2064,334 @@ int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool pe
   return lm_launch(kernel, batch, kLmKpThreads, smem, stream, a, x);
 }
 
+
+// ---------------------------------------------------------------------------------------------------------------
+// The step of the fit to 3D scans (shapy_fit_lm_scan_step): parameters [delta_j (3 n_rot) | beta | t], the columns of
+// shapy_smplx_vertex_jacobian.  Loss, fp64, left to right: c_s Ls + c_m Lm + pose prior + measurements + betas_w
+// |beta|^2, c_s = s2m / sum_{w_i > 0} w_i (1 when that sum is 0), c_m = m2s / V, Ls = sum_i w_i rho(d_i^2) over the kept
+// points (d_i = |c_i - p_i|, c_i = sum_k b_ik x_{f_i,k}), Lm = sum_v rho(e_v^2) (e_v = |x_v - s_v|, s_v the vertex's
+// nearest kept point).  Two kernels:
+//   lm_scan_rows_kernel, one CTA per (chunk of kScanChunk points or vertices, body): the rows of the trial at its held
+//     correspondences, staged kScanItems items (3 row slots each) at a time in fp64, accumulated into the packed lower
+//     triangle of J^T U J (U the IRLS weights without c_s / c_m), J^T U r and the chunk's loss share; each thread owns
+//     one 4 x 4 block of the triangle in registers (SIMT fp64), and the partial sums go to the workspace.  A point with
+//     all barycentrics > 0 on a face of non-zero area gives one point-to-plane row n^T (c_i - p_i), n the face's unit
+//     normal held constant; any other kept point three point-to-point rows c_i - p_i; a vertex with a nearest point
+//     three rows x_v - s_v.  The chunking depends on N and V only; no atomics.
+//   lm_scan_step_kernel, one CTA per body: the chunks summed in chunk order into the trial's loss, A = c_s A_s +
+//     c_m A_m and g, the policy of the other steps, the state's A and g replaced by the trial's on accept (P^2 + P
+//     doubles instead of a Jacobian), then the pose-prior and measurement rows at the state, betas_w + lambda on the
+//     betas diagonal and lambda elsewhere, lm_kp_solve and the next trial.
+constexpr int kScanChunk = 1024;        // points or vertices per CTA of the row kernel
+constexpr int kScanItems = 16;          // items staged at a time: 3 row slots each
+constexpr int kScanRows = 3 * kScanItems;
+constexpr int kScanThreads = 320;       // >= the 4 x 4 blocks of the lower triangle at P = 96 (300)
+
+// doubles per (body, chunk) in the workspace: the packed lower triangle, g and the loss share
+__host__ __device__ inline size_t lm_scan_stride(int P) { return (size_t)P * (P + 1) / 2 + P + 1; }
+
+inline int lm_scan_chunks(int n) { return (n + kScanChunk - 1) / kScanChunk; }
+
+// rho(e) and its derivative: Geman-McClure e s2 / (s2 + e) and (s2 / (s2 + e))^2, or e and 1 for least squares
+__device__ __forceinline__ void scan_rho(bool robust, double s2, double e, double &rho, double &drho) {
+  if (robust) {
+    const double q = s2 / (s2 + e);
+    rho = e * q;
+    drho = q * q;
+  } else {
+    rho = e;
+    drho = 1.0;
+  }
+}
+
+struct LmScanRowArgs {
+  int N, V, P, ns, nm;                  // points, vertices, parameters, point chunks, vertex chunks
+  const float *points, *weights;        // (B, N, 3), (B, N)
+  const int32_t *faces;                 // (F, 3)
+  const float *verts, *jac;             // the trial's (B, V, 3), (B, V, 3, P)
+  const int32_t *face_idx, *nearest;    // (B, N), (B, V) or null (no model -> scan term)
+  const float *bary;                    // (B, N, 3)
+  float sigma, s2m, m2s;
+  double *ws;
+};
+
+__global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArgs a) {
+  __shared__ double Js[kScanRows][kLmKpMaxP];
+  __shared__ double us[kScanRows], rs[kScanRows], ls[kScanItems], cf[kScanItems][3], nrm[kScanItems][3];
+  __shared__ int vid[kScanItems][3], kind[kScanItems];   // kind: 1 point-to-plane, 2 point-to-point, 3 vertex
+  const int b = blockIdx.y, c = blockIdx.x, t = threadIdx.x, P = a.P, Pp = (P + 3) & ~3, nbw = Pp / 4;
+  const bool pts = c < a.ns;
+  const int i0 = (pts ? c : c - a.ns) * kScanChunk, n = min(kScanChunk, (pts ? a.N : a.V) - i0);
+  const bool active = pts ? a.s2m > 0.f : (a.m2s > 0.f && a.nearest);
+  const bool robust = isfinite(a.sigma);
+  const double s2 = (double)a.sigma * (double)a.sigma;
+  int bi = 0, bj = 0;
+  tri_rc(t, bi, bj);
+  const bool own = t < nbw * (nbw + 1) / 2;
+  double acc[4][4], g = 0.0, L = 0.0;
+  for (int x = 0; x < 4; ++x)
+    for (int y = 0; y < 4; ++y) acc[x][y] = 0.0;
+  const float *J = a.jac + (size_t)b * a.V * 3 * P;
+  for (int s0 = 0; active && s0 < n; s0 += kScanItems) {
+    const int ni = min(kScanItems, n - s0);
+    __syncthreads();
+    if (t < ni) {                       // item t: its rows' weights, residuals and what their entries need
+      for (int r = 0; r < 3; ++r) us[3 * t + r] = rs[3 * t + r] = 0.0;
+      ls[t] = 0.0;
+      kind[t] = 0;
+      const int i = i0 + s0 + t;
+      double d[3];
+      if (pts) {
+        const double w = a.weights[(size_t)b * a.N + i];
+        if (w > 0.0) {                  // a dropped point is never read
+          const int f = a.face_idx[(size_t)b * a.N + i];
+          const float *p = a.points + ((size_t)b * a.N + i) * 3, *bc = a.bary + ((size_t)b * a.N + i) * 3;
+          double X[3][3];
+          for (int k = 0; k < 3; ++k) {
+            const int v = a.faces[3 * f + k];
+            vid[t][k] = v;
+            cf[t][k] = bc[k];
+            for (int q = 0; q < 3; ++q) X[k][q] = a.verts[((size_t)b * a.V + v) * 3 + q];
+          }
+          for (int q = 0; q < 3; ++q) d[q] = cf[t][0] * X[0][q] + cf[t][1] * X[1][q] + cf[t][2] * X[2][q] - (double)p[q];
+          double rho, drho;
+          scan_rho(robust, s2, d[0] * d[0] + d[1] * d[1] + d[2] * d[2], rho, drho);
+          ls[t] = w * rho;
+          const double u = w * drho;
+          const double e1[3] = {X[1][0] - X[0][0], X[1][1] - X[0][1], X[1][2] - X[0][2]};
+          const double e2[3] = {X[2][0] - X[0][0], X[2][1] - X[0][1], X[2][2] - X[0][2]};
+          const double nv[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2],
+                                e1[0] * e2[1] - e1[1] * e2[0]};
+          const double nn = sqrt(nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2]);
+          if (cf[t][0] > 0.0 && cf[t][1] > 0.0 && cf[t][2] > 0.0 && nn > 0.0) {
+            for (int q = 0; q < 3; ++q) nrm[t][q] = nv[q] / nn;
+            kind[t] = 1;
+            us[3 * t] = u;
+            rs[3 * t] = nrm[t][0] * d[0] + nrm[t][1] * d[1] + nrm[t][2] * d[2];
+          } else {
+            kind[t] = 2;
+            for (int q = 0; q < 3; ++q) {
+              us[3 * t + q] = u;
+              rs[3 * t + q] = d[q];
+            }
+          }
+        }
+      } else {
+        const int q = a.nearest[(size_t)b * a.V + i];
+        if (q >= 0) {
+          const float *s = a.points + ((size_t)b * a.N + q) * 3;
+          for (int k = 0; k < 3; ++k) d[k] = (double)a.verts[((size_t)b * a.V + i) * 3 + k] - (double)s[k];
+          double rho, drho;
+          scan_rho(robust, s2, d[0] * d[0] + d[1] * d[1] + d[2] * d[2], rho, drho);
+          ls[t] = rho;
+          kind[t] = 3;
+          vid[t][0] = i;
+          for (int k = 0; k < 3; ++k) {
+            us[3 * t + k] = drho;
+            rs[3 * t + k] = d[k];
+          }
+        }
+      }
+    }
+    __syncthreads();
+    for (int e = t; e < 3 * ni * Pp; e += blockDim.x) {
+      const int row = e / Pp, col = e % Pp, it = row / 3, cc = row % 3;
+      if (!(us[row] > 0.0)) continue;
+      double x = 0.0;
+      if (col < P) {
+        const int k = kind[it];
+        auto mix = [&](int q) {       // sum_k b_k J_{v_k}, row q
+          const float *j0 = J + ((size_t)vid[it][0] * 3 + q) * P + col, *j1 = J + ((size_t)vid[it][1] * 3 + q) * P + col,
+                      *j2 = J + ((size_t)vid[it][2] * 3 + q) * P + col;
+          return cf[it][0] * (double)*j0 + cf[it][1] * (double)*j1 + cf[it][2] * (double)*j2;
+        };
+        if (k == 1) x = nrm[it][0] * mix(0) + nrm[it][1] * mix(1) + nrm[it][2] * mix(2);
+        else if (k == 2) x = mix(cc);
+        else x = (double)J[((size_t)vid[it][0] * 3 + cc) * P + col];
+      }
+      Js[row][col] = x;
+    }
+    __syncthreads();
+    if (t == 0)
+      for (int it = 0; it < ni; ++it) L += ls[it];
+    for (int row = 0; row < 3 * ni; ++row) {
+      const double u = us[row];
+      if (!(u > 0.0)) continue;
+      if (own) {
+        double ja[4], jb[4];
+        for (int x = 0; x < 4; ++x) {
+          ja[x] = u * Js[row][4 * bi + x];
+          jb[x] = Js[row][4 * bj + x];
+        }
+        for (int x = 0; x < 4; ++x)
+          for (int y = 0; y < 4; ++y) acc[x][y] += ja[x] * jb[y];
+      }
+      if (t < P) g += (u * Js[row][t]) * rs[row];
+    }
+  }
+  const int npk = P * (P + 1) / 2;
+  double *o = a.ws + ((size_t)b * (a.ns + a.nm) + c) * lm_scan_stride(P);
+  if (own)
+    for (int x = 0; x < 4; ++x)
+      for (int y = 0; y < 4; ++y) {
+        const int i = 4 * bi + x, j = 4 * bj + y;
+        if (i < P && j <= i) o[tri(i, j)] = acc[x][y];
+      }
+  if (t < P) o[npk + t] = g;
+  if (t == 0) o[npk + P] = L;
+}
+
+struct LmScanStepArgs {
+  int N, V, ns, nm;
+  const float *weights;                 // (B, N): sum_{w_i > 0} w_i normalises the scan -> model term
+  float s2m, m2s;
+  LmKp2dArgs x2;                        // anchor, pose_w and betas_w, and the measurement block with MEAS
+  double *A, *g;                        // the state's undamped data rows: (B, P, P) symmetric, (B, P)
+  const double *ws;
+};
+
+template <bool MEAS>
+__global__ void __launch_bounds__(kLmKpThreads) lm_scan_step_kernel(LmKpArgs a, LmScanStepArgs x) {
+  extern __shared__ double A[];         // [P][P]: the lower triangle of the normal matrix, then its Cholesky factor
+  __shared__ double y[kLmKpMaxP], dg[kLmKpMaxP], part[kLmKpThreads];
+  __shared__ double lt_s, cs_s, cm_s, lam_s;
+  __shared__ int ok_s;
+  const int b = blockIdx.x, t = threadIdx.x, P = a.P, nb = a.nb, nr9 = 9 * a.n_rot, o = 3 * a.n_rot;
+  const int npk = P * (P + 1) / 2, nc = x.ns + x.nm;
+  const size_t S = lm_scan_stride(P);
+  const double *wsb = x.ws + (size_t)b * nc * S;
+  const float *anc = x.x2.anchor ? x.x2.anchor + (size_t)b * nr9 : nullptr;
+  const float lcur = a.loss[b];
+  // 1. trial loss: sum_{w_i > 0} w_i strided over the threads, the threads' sums in thread order, then the chunks
+  double sw = 0.0;
+  for (int i = t; i < x.N; i += blockDim.x) {
+    const double w = x.weights[(size_t)b * x.N + i];
+    if (w > 0.0) sw += w;
+  }
+  part[t] = sw;
+  __syncthreads();
+  if (t == 0) {
+    double W = 0.0;
+    for (int q = 0; q < (int)blockDim.x; ++q) W += part[q];
+    const double cs = (double)x.s2m / (W > 0.0 ? W : 1.0), cm = (double)x.m2s / (double)x.V;
+    double Ls = 0.0, Lm = 0.0;
+    for (int c = 0; c < x.ns; ++c) Ls += wsb[c * S + npk + P];
+    for (int c = x.ns; c < nc; ++c) Lm += wsb[c * S + npk + P];
+    double L = cs * Ls + cm * Lm;
+    if (x.x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x.x2, a.trot + (size_t)b * nr9, anc, nr9);
+    if constexpr (MEAS) L += lm_meas_loss(x.x2.mb, b);
+    if (x.x2.betas_w > 0.f) L += (double)x.x2.betas_w * lm_sq_norm(a.tbetas + (size_t)b * nb, nb);
+    lt_s = L;
+    cs_s = cs;
+    cm_s = cm;
+  }
+  __syncthreads();
+  // 2. accept or reject; an accepted trial's data rows become the state's
+  const double lt = lt_s;
+  const bool accept = lm_accept(a.first, lt, lcur);
+  const float lnew = lm_loss(accept, lt, lcur);
+  const float *Rst = (accept ? a.trot : a.rot) + (size_t)b * nr9;
+  const float *Bst = (accept ? a.tbetas : a.betas) + (size_t)b * nb;
+  if (accept) {
+    lm_kp_take_trial(a, b, lnew);
+    if constexpr (MEAS) lm_meas_take_trial(x.x2.mb, b, nb);
+  }
+  double *Ab = x.A + (size_t)b * P * P, *gb = x.g + (size_t)b * P;
+  if (accept) {
+    const double cs = cs_s, cm = cm_s;
+    for (int p = t; p < npk + P; p += blockDim.x) {
+      double s1 = 0.0, s2 = 0.0;
+      for (int c = 0; c < x.ns; ++c) s1 += wsb[c * S + p];
+      for (int c = x.ns; c < nc; ++c) s2 += wsb[c * S + p];
+      const double v = cs * s1 + cm * s2;
+      if (p < npk) {
+        int r, k;
+        tri_rc(p, r, k);
+        A[r * P + k] = v;
+        Ab[r * P + k] = v;
+        Ab[k * P + r] = v;
+      } else {
+        y[p - npk] = v;
+        gb[p - npk] = v;
+      }
+    }
+  } else {
+    for (int p = t; p < npk; p += blockDim.x) {
+      int r, k;
+      tri_rc(p, r, k);
+      A[r * P + k] = Ab[r * P + k];
+    }
+    for (int i = t; i < P; i += blockDim.x) y[i] = gb[i];
+  }
+  __syncthreads();
+  if (t < P) dg[t] = A[t * P + t];      // the data rows' diagonal: the first lambda
+  __syncthreads();
+  // 3. the pose-prior rows of joint j (weight pose_w / 2) reach only its diagonal block, the measurement rows the betas
+  // block; each entry by one thread, and g_t by thread t
+  if (x.x2.pose_w > 0.f) {
+    const double hw = 0.5 * (double)x.x2.pose_w;
+    for (int q = t; q < 6 * (a.n_rot - 1); q += blockDim.x) {
+      const int j = 1 + q / 6, u = q % 6, ar = u < 1 ? 0 : u < 3 ? 1 : 2, ac = u - ar * (ar + 1) / 2;
+      const float *R = Rst + 9 * j;
+      double acc = A[(3 * j + ar) * P + 3 * j + ac];
+      for (int e = 0; e < 9; ++e) acc += (hw * rot_tangent(R, ar, e)) * rot_tangent(R, ac, e);
+      A[(3 * j + ar) * P + 3 * j + ac] = acc;
+    }
+  }
+  if constexpr (MEAS) {
+    const LmMeasArgs &mb = x.x2.mb;
+    const float *Jm = (accept ? mb.tjac : mb.jac) + (size_t)b * 5 * nb;
+    const float *mw = mb.weights + (size_t)b * 5;
+    for (int q = t; q < nb * (nb + 1) / 2; q += blockDim.x) {
+      int r, c;
+      tri_rc(q, r, c);
+      double acc = A[(o + r) * P + o + c];
+      for (int m = 0; m < 5; ++m) {
+        const double w = mw[m];
+        if (w > 0.0) acc += (w * (double)Jm[m * nb + r]) * (double)Jm[m * nb + c];
+      }
+      A[(o + r) * P + o + c] = acc;
+    }
+  }
+  if (t < P) {
+    double g = y[t];
+    if (x.x2.pose_w > 0.f && t >= 3 && t < o) {
+      const double hw = 0.5 * (double)x.x2.pose_w;
+      const float *R = Rst + 9 * (t / 3), *R0 = anc + 9 * (t / 3);
+      for (int e = 0; e < 9; ++e) g += (hw * rot_tangent(R, t % 3, e)) * ((double)R[e] - (double)R0[e]);
+    }
+    if constexpr (MEAS) {
+      const LmMeasArgs &mb = x.x2.mb;
+      const float *Mm = (accept ? mb.tmeas : mb.meas) + (size_t)b * 5;
+      const float *Jm = (accept ? mb.tjac : mb.jac) + (size_t)b * 5 * nb;
+      const float *mt = mb.targets + (size_t)b * 5, *mw = mb.weights + (size_t)b * 5;
+      if (t >= o && t < o + nb)
+        for (int m = 0; m < 5; ++m) {
+          const double w = mw[m];
+          if (w > 0.0) g += (w * (double)Jm[m * nb + t - o]) * ((double)Mm[m] - (double)mt[m]);
+        }
+    }
+    if (x.x2.betas_w > 0.f && t >= o && t < o + nb) g += (double)x.x2.betas_w * (double)Bst[t - o];
+    y[t] = -g;
+  }
+  __syncthreads();
+  if (t == 0) {
+    double dmax = kDiagFloor;
+    if (a.first)
+      for (int j = 0; j < P; ++j) dmax = fmax(dmax, dg[j]);
+    const float lam = lm_lambda(a.first, accept, a.first ? 0.f : a.lambda[b], dmax, a.up, a.down);
+    a.lambda[b] = lam;
+    if (accept && !a.first) a.accepted[b] += 1;
+    lam_s = lam;
+    ok_s = isfinite(lnew);
+  }
+  __syncthreads();
+  if (t < P) A[t * P + t] += t >= o && t < o + nb ? (double)x.x2.betas_w + lam_s : lam_s;
+  // 4. Cholesky and the two solves; 5. the next trial (a failed step keeps the state)
+  lm_kp_solve(A, y, P, P, ok_s);
+  lm_kp_next_trial(a, b, y, ok_s);
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -2335,4 +2663,59 @@ extern "C" int shapy_fit_lm_keypoints_2d_expressive_perspective_step(
   x.texpr = trial_expression;
   return run_lm_kp2d("shapy_fit_lm_keypoints_2d_expressive_perspective_step", batch, a, x, true, false, kLmKp2dMaxP,
                      stream);
+}
+
+extern "C" size_t shapy_fit_lm_scan_workspace_bytes(int batch, int num_points, int num_verts, int num_params) {
+  if (batch < 0 || num_points < 1 || num_verts < 1 || num_params < 1) return 0;
+  return (size_t)batch * (lm_scan_chunks(num_points) + lm_scan_chunks(num_verts)) * lm_scan_stride(num_params) *
+         sizeof(double);
+}
+
+extern "C" int shapy_fit_lm_scan_step(
+    int batch, int num_points, int num_verts, int n_rot, int nb, const float *points, const float *weights,
+    const int32_t *faces, const float *pose_anchor, float robust_sigma, float scan_to_model_weight,
+    float model_to_scan_weight, float pose_prior_weight, float betas_weight, const float *meas_targets,
+    const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl,
+    double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_vertices,
+    const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary, const int32_t *trial_nearest,
+    const float *trial_meas, const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream) {
+  const char *fn = "shapy_fit_lm_scan_step";
+  const LmMeasArgs mb{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac};
+  const bool with_meas = meas_targets || meas_weights || meas || meas_jac || trial_meas || trial_meas_jac;
+  const float s2m = scan_to_model_weight, m2s = model_to_scan_weight;
+  SHAPY_REQUIRE(points && weights && faces && rot && betas && transl && normal_matrix && gradient && loss && lambda &&
+                    accepted && trial_rot && trial_betas && trial_transl && trial_vertices && trial_jac &&
+                    trial_face_idx && trial_bary && workspace && (trial_nearest || !(m2s > 0.f)) &&
+                    (pose_anchor || !(pose_prior_weight > 0.f)) && (!with_meas || lm_meas_ptrs(mb)),
+                "%s: null argument", fn);
+  SHAPY_REQUIRE(batch >= 0 && batch <= 65535 && num_points >= 1 && num_verts >= 1 && n_rot >= 1 && n_rot <= 64 &&
+                    nb >= 1,
+                "%s: bad size (batch %d, %d points, %d vertices, n_rot %d, %d betas)", fn, batch, num_points, num_verts,
+                n_rot, nb);
+  SHAPY_REQUIRE(robust_sigma > 0.f && s2m >= 0.f && m2s >= 0.f && isfinite(s2m) && isfinite(m2s) &&
+                    pose_prior_weight >= 0.f && betas_weight >= 0.f && lambda_up >= 1.f && lambda_down >= 1.f,
+                "%s: robust_sigma must be > 0 (inf: least squares), the term and prior weights finite and >= 0 and "
+                "lambda_up and lambda_down >= 1",
+                fn);
+  const int P = 3 * n_rot + nb + 3;
+  if (P > kLmKpMaxP) {
+    set_error("%s: %d parameters, at most %d are supported", fn, P, kLmKpMaxP);
+    return SHAPY_ERR_UNSUPPORTED;
+  }
+  const size_t need = shapy_fit_lm_scan_workspace_bytes(batch, num_points, num_verts, P);
+  SHAPY_REQUIRE(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+  if (batch == 0) return SHAPY_OK;
+  const int ns = lm_scan_chunks(num_points), nm = lm_scan_chunks(num_verts);
+  LmScanRowArgs r{num_points, num_verts, P,  ns, nm, points, weights, faces, trial_vertices, trial_jac, trial_face_idx,
+                  trial_nearest, trial_bary, robust_sigma, s2m, m2s, (double *)workspace};
+  lm_scan_rows_kernel<<<dim3(ns + nm, batch), kScanThreads, 0, (cudaStream_t)stream>>>(r);
+  SHAPY_LAUNCH_CHECK();
+  LmKpArgs a{0, n_rot, nb, P, nullptr, nullptr, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl, nullptr,
+             nullptr, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, nullptr, nullptr};
+  LmScanStepArgs x{num_points, num_verts, ns, nm, weights, s2m, m2s,
+                   LmKp2dArgs{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, mb}, normal_matrix,
+                   gradient, (const double *)workspace};
+  return lm_launch(with_meas ? lm_scan_step_kernel<true> : lm_scan_step_kernel<false>, batch, kLmKpThreads,
+                   lm_kp_smem(P), stream, a, x);
 }

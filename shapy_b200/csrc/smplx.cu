@@ -1156,6 +1156,100 @@ __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_kernel(KpJacArgs a
 
 __global__ void __launch_bounds__(kKpJacThreads) smplx_kp_jac_expr_kernel(KpJacExprArgs a) { kp_jac_body<true>(a); }
 
+// ============================================================================================== vertex Jacobian
+// Every posed vertex (+ transl) and its Jacobian (3, P) with the columns of the keypoint Jacobian, for the dense fits
+// (the LM scan fit): one CTA per (tile of kVjTile vertices, body), grid (ceil(V / kVjTile), B).  Each CTA recomputes
+// its body's chain (jac_chain, a few microseconds of the CTA's time), then the tile's vertex states (kp_vertex_state),
+// then one work item per (vertex, column block) as in the keypoint Jacobian, into a shared-memory tile [vertex][xyz][P]
+// that is written out contiguously.  Same device functions, so a barycentric mix of these rows is the keypoint
+// Jacobian's landmark row up to fp32 rounding.  No atomics; a body's bits do not depend on the rest of the batch.
+constexpr int kVjTile = 32;
+
+// The per-body chain the vertex Jacobian starts from, in shared memory: kp_jac_body's prologue without the contour LUT
+// row (written apart so that the keypoint kernels keep their code): body_chain, the ancestor masks sub (bit i of
+// sub[s]: i is s or one of its ancestors), the pose feature pf (Kp entries) and dG_j.t / dbeta of the betas columns
+// level by level.  Ends on a barrier
+__device__ __forceinline__ void jac_chain(const SmplxDev &m, const float *betas, const float *rot, int n_rot,
+                                          int Kp, int NB, int b, float (*R)[9], float (*Jr)[3],
+                                          float (*G)[12], float *coef, float *pf, float (*dGt)[3][kMaxCoef],
+                                          unsigned long long *sub) {
+  const int t = threadIdx.x;
+  body_chain(m, betas, nullptr, rot, n_rot, b, R, Jr, G, coef);
+  if (t == 0)
+    for (int s = 0; s < m.J; ++s) sub[s] = (s ? sub[m.parents[s]] : 0ull) | (1ull << s);
+  for (int k = t; k < Kp; k += blockDim.x) {
+    const int j = 1 + k / 9, e = k % 9;
+    pf[k] = R[j][e] - ((e == 0 || e == 4 || e == 8) ? 1.f : 0.f);
+  }
+  // dG_j.t / dbeta level by level: dG_0.t = dJ_0, dG_j.t = G_p.R (dJ_j - dJ_p) + dG_p.t
+  for (int i = t; i < 3 * NB; i += blockDim.x) dGt[0][i / NB][i % NB] = kp_jdir(m, 0, i / NB, i % NB);
+  __syncthreads();
+  for (int lv = 1; lv < m.n_levels; ++lv) {
+    const int off = m.level_off[lv], cnt = m.level_off[lv + 1] - off;
+    for (int i = t; i < cnt * 3 * NB; i += blockDim.x) {
+      const int j = m.level_joints[off + i / (3 * NB)], c = (i / NB) % 3, l = i % NB, p = m.parents[j];
+      const float r0 = kp_jdir(m, j, 0, l) - kp_jdir(m, p, 0, l), r1 = kp_jdir(m, j, 1, l) - kp_jdir(m, p, 1, l),
+                  r2 = kp_jdir(m, j, 2, l) - kp_jdir(m, p, 2, l);
+      dGt[j][c][l] = G[p][c * 4] * r0 + G[p][c * 4 + 1] * r1 + G[p][c * 4 + 2] * r2 + dGt[p][c][l];
+    }
+    __syncthreads();
+  }
+}
+
+struct VertJacArgs {
+  SmplxDev m;
+  const float *betas, *rot, *transl;      // transl may be null (zero)
+  int n_rot, Kp, P;
+  float *verts, *jac;
+};
+
+__global__ void __launch_bounds__(kKpJacThreads) smplx_vertex_jac_kernel(VertJacArgs a) {
+  const SmplxDev &m = a.m;
+  const int b = blockIdx.y, v0 = blockIdx.x * kVjTile, t = threadIdx.x;
+  __shared__ float R[kMaxJoints][9];
+  __shared__ float Jr[kMaxJoints][3];
+  __shared__ float G[kMaxJoints][12];
+  __shared__ float coef[kMaxCoef];
+  __shared__ float pf[(kMaxJoints - 1) * 9];
+  __shared__ float dGt[kMaxJoints][3][kMaxCoef];
+  __shared__ unsigned long long sub[kMaxJoints];
+  __shared__ float st[kVjTile][kKpState];
+  extern __shared__ float tile[];                   // [nv][3][P]
+  jac_chain(m, a.betas, a.rot, a.n_rot, a.Kp, m.NB, b, R, Jr, G, coef, pf, dGt, sub);
+  const int nv = min(kVjTile, m.V - v0), P = a.P, NB = m.NB, NG = a.n_rot + 2;
+  for (int i = t; i < nv; i += blockDim.x) kp_vertex_state(m, v0 + i, a.Kp, coef, pf, G, Jr, st[i]);
+  __syncthreads();
+  // work items (vertex q, column block g): g < n_rot the 3 x 3 block of delta_g, g = n_rot the betas, then transl
+  for (int i = t; i < nv * NG; i += blockDim.x) {
+    const int q = i / NG, g = i % NG, v = v0 + q;
+    float *o = tile + (size_t)q * 3 * P;          // row c at o + c P
+    if (g < a.n_rot) {
+      float d[3][3];
+      kp_vertex_drot(m, v, g, st[q], G, Jr, R, sub, d);
+      for (int c = 0; c < 3; ++c)
+        for (int x = 0; x < 3; ++x) o[c * P + 3 * g + x] = d[x][c];
+    } else if (g == a.n_rot) {
+      for (int l = 0; l < NB; ++l) {
+        float d[3];
+        kp_vertex_dbeta(m, v, l, st[q], G, dGt, d);
+        for (int c = 0; c < 3; ++c) o[c * P + 3 * a.n_rot + l] = d[c];
+      }
+    } else {
+      for (int c = 0; c < 3; ++c)
+        for (int x = 0; x < 3; ++x) o[c * P + 3 * a.n_rot + NB + x] = c == x ? 1.f : 0.f;
+    }
+  }
+  __syncthreads();
+  const float *tr = a.transl ? a.transl + (size_t)b * 3 : nullptr;
+  const size_t base = (size_t)b * m.V + v0;
+  for (int i = t; i < nv * 3; i += blockDim.x) {
+    const float x = st[i / 3][12 + i % 3];
+    a.verts[base * 3 + i] = tr ? x + tr[i % 3] : x;
+  }
+  float *jb = a.jac + base * 3 * P;
+  for (int i = t; i < nv * 3 * P; i += blockDim.x) jb[i] = tile[i];
+}
+
 }  // namespace shapy
 
 using namespace shapy;
@@ -1703,6 +1797,22 @@ extern "C" int shapy_smplx_keypoint_jacobian_expr(const shapy_smplx_t *m, const 
       KpJacArgs{d, betas, rot, transl, n_rot, (n_rot - 1) * 9, 3 * n_rot + d.NC + 3, n_entries, cached, keypoints, jac};
   a.expr = expr;
   smplx_kp_jac_expr_kernel<<<B, kKpJacThreads, smem, (cudaStream_t)stream>>>(a);
+  SHAPY_LAUNCH_CHECK();
+  return SHAPY_OK;
+}
+
+extern "C" int shapy_smplx_vertex_jacobian(const shapy_smplx_t *m, const float *betas, const float *rot, int n_rot,
+                                           const float *transl, int B, float *vertices, float *jac, void *stream) {
+  SHAPY_REQUIRE(m && betas && rot && vertices && jac, "shapy_smplx_vertex_jacobian: null argument");
+  SHAPY_REQUIRE(B >= 0 && B <= 65535, "shapy_smplx_vertex_jacobian: batch %d", B);
+  SHAPY_REQUIRE(n_rot >= 1 && n_rot <= m->d.J, "shapy_smplx_vertex_jacobian: n_rot %d out of range", n_rot);
+  if (B == 0) return SHAPY_OK;
+  const SmplxDev &d = m->d;
+  const int P = 3 * n_rot + d.NB + 3;
+  const size_t smem = (size_t)kVjTile * 3 * P * sizeof(float);
+  SHAPY_CUDA_TRY(cudaFuncSetAttribute(smplx_vertex_jac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  VertJacArgs a{d, betas, rot, transl, n_rot, (n_rot - 1) * 9, P, vertices, jac};
+  smplx_vertex_jac_kernel<<<dim3(ceil_div(d.V, kVjTile), B), kKpJacThreads, smem, (cudaStream_t)stream>>>(a);
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }

@@ -114,11 +114,17 @@ the 2D fits' pose and betas priors and optionally known measurements.  Keypoints
 also sees depth and soft tissue.  The closest points, their gradient and the nearest points are CUDA launches on the
 batched LBVH of mesh_to_mesh_forward (ops.closest_points, ops.closest_points_backward, ops.nearest_points):
 deterministic, and a body's result does not depend on the rest of the batch.  The optimiser is the batched Adam of the
-other fits: an LM step would need the Jacobian of every vertex a correspondence touches, up to all of them.  Not
-covered: an LM scan fit, point-to-plane residuals, scan normals, a self-penetration term, rigid pre-alignment of scans
-in other frames or units, and reading PLY / OBJ files (load the points into an npz).
+other fits.  With method='lm' each iteration is the trial's vertices and their (V, 3, P) Jacobian in one launch
+(ops.smplx_vertex_jacobian, 4 V 3 P bytes per body: 9.9 MB at P = 79), the closest points (the tree refit) and the
+nearest points at those vertices, with measurements forward_shape and the measurement Jacobian, then
+ops.fit_lm_scan_step: the correspondences held as landmarks, one point-to-plane row per point interior to its face
+(three point-to-point rows otherwise, and for every vertex), IRLS weights under Geman-McClure, the normal equations
+summed in fp64 on the device.  No host synchronisation, and every body's loss is non-increasing; vertex_jacobian
+exposes the Jacobian.  Not covered: scan normals, a self-penetration term, rigid pre-alignment of scans in other
+frames or units, and reading PLY / OBJ files (load the points into an npz).
 
     python -m shapy_b200.fit --synthetic --scan scan.npz --init pred.npz --robust-sigma 0.01 --output fit.npz
+    python -m shapy_b200.fit --synthetic --scan scan.npz --method lm --output fit.npz
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --robust-sigma 0.05
     python -m shapy_b200.fit --synthetic --keypoints-2d kp.npz --init pred.npz --method lm --targets known.npz
 
@@ -372,6 +378,18 @@ def keypoint_jacobian(body_model, rot, betas, transl=None):
     f = lambda t: None if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).detach().contiguous()  # noqa: E731
     kp, jac = ops.smplx_keypoint_jacobian(body_model.packed(device), f(betas), f(rot), f(transl))
     return {'keypoints': kp, 'jacobian': jac}
+
+
+def vertex_jacobian(body_model, rot, betas, transl=None):
+    """Every posed vertex of the model (expression zero, plus transl) and its Jacobian without autograd, the
+    counterpart of keypoint_jacobian: rot (B, n_rot, 3, 3), betas (B, NB), transl (B, 3) or None.  Returns {'vertices'
+    (B, V, 3), 'jacobian' (B, V, 3, 3 n_rot + NB + 3)}, the columns of keypoint_jacobian.  The Jacobian takes 4 V 3 P
+    bytes per body (9.9 MB at V = 10475 and P = 79)."""
+    from . import ops
+    device = body_model.shapedirs.device
+    f = lambda t: None if t is None else torch.as_tensor(t, dtype=torch.float32, device=device).detach().contiguous()  # noqa: E731
+    v, jac = ops.smplx_vertex_jacobian(body_model.packed(device), f(betas), f(rot), f(transl))
+    return {'vertices': v, 'jacobian': jac}
 
 
 def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam',
@@ -1392,7 +1410,7 @@ def _scan_inputs(fn, body_model, points, weights, device):
 def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=None, lr=0.05, scan_to_model_weight=1.0,
                      model_to_scan_weight=1.0, robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0,
                      body_measurements=None, measurements=None, measurement_weights=None,
-                     circumference_derivative='reference'):
+                     circumference_derivative='reference', method='adam'):
     """Fits pose, shape and translation to 3D scans or point clouds: points (B, N, 3) in metres in the model frame,
     N <= 32768 per body, weights None (all 1), (N,) or (B, N), a point with weight <= 0 dropped (it may be NaN).
     Loss per body: scan_to_model_weight sum_i w_i rho(d_i^2) / sum_i w_i, d_i the distance of point i to the exact
@@ -1405,14 +1423,16 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
     scan (one depth camera) set model_to_scan_weight=0: the unseen side of the body has no point to be near.
     init: fit_body_to_keypoints' keys (raw 6D global_rot / body_pose, or the regressor's raw_ entries, betas, transl);
     by default the identity pose, zero betas and the translation that puts the start body's vertex centroid on the
-    scan's weighted centroid (on the device, no synchronisation).  Adam as fit_body_to_keypoints' (the step size decays
-    from lr to lr / 100); iterations None means 600.  The posed mesh's tree is built at the first iteration and refit
-    after (the same bits as a rebuild).
+    scan's weighted centroid (on the device, no synchronisation).  method: 'adam' (the default, as
+    fit_body_to_keypoints': the step size decays from lr to lr / 100) or 'lm' (batched Levenberg-Marquardt on the
+    vertex Jacobian, see the top; `lr` is ignored; the Jacobian takes 9.9 MB per body at 10 betas); iterations None
+    means 600 for Adam and 50 for LM.  The posed mesh's tree is built at the first iteration and refit after (the same
+    bits as a rebuild).
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat', 'body_pose_mat', 'vertices'
     (B, V, 3) of the final parameters, 'loss' (B,)}, and with body_measurements 'measurements' (B, 5) of the fitted
     betas (mass, height, chest, waist, hips), with or without measurement targets."""
     fn = 'fit_body_to_scan'
-    iterations, sigma = _check_kp_fit(fn, body_model, 'adam', iterations, circumference_derivative, body_measurements,
+    iterations, sigma = _check_kp_fit(fn, body_model, method, iterations, circumference_derivative, body_measurements,
                                       measurements, robust_sigma, pose_prior_weight, betas_weight)
     s2m, m2s = float(scan_to_model_weight), float(model_to_scan_weight)
     if not (0 <= s2m < float('inf') and 0 <= m2s < float('inf') and s2m + m2s > 0):
@@ -1429,7 +1449,7 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
     wsum = wk.sum(1)
     wden = torch.where(wsum > 0, wsum, torch.ones_like(wsum))
     init = _raw_init(init)
-    params = _start_params(init, B, body_model.num_betas, device, 'adam', 'transl')
+    params = _start_params(init, B, body_model.num_betas, device, method, 'transl')
     rot0, anchor = _start_rotations(params, None, B)
     if init.get('transl') is None:
         with torch.no_grad():
@@ -1443,11 +1463,8 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
     def rho(e):
         return e if sigma is None else sigma * sigma * e / (sigma * sigma + e)
 
-    def loss_fn():
-        grot = Rot6dFunction.apply(params['global_rot'])
-        bpose = Rot6dFunction.apply(params['body_pose'])
-        v = body_model(global_rot=grot, body_pose=bpose, betas=params['betas'], transl=params['transl'],
-                       return_shaped=False)['vertices']
+    def scan_loss(grot, bpose, betas, transl):
+        v = body_model(global_rot=grot, body_pose=bpose, betas=betas, transl=transl, return_shaped=False)['vertices']
         per_body = torch.zeros(B, dtype=torch.float32, device=device)
         if s2m > 0:
             d2 = ClosestPointsFunction.apply(faces, v, pts, w, tree)
@@ -1461,20 +1478,76 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
         if pw > 0:
             per_body = per_body + 0.5 * pw * (bpose - anchor[:, 1:]).pow(2).sum((1, 2, 3))
         if bw > 0:
-            per_body = per_body + bw * params['betas'].pow(2).sum(1)
+            per_body = per_body + bw * betas.pow(2).sum(1)
         meas = None
         if mt is not None:
-            meas = mt.measure(body_model, params['betas'])
-            per_body = per_body + mt.loss(meas, params['betas'], 0.0)
+            meas = mt.measure(body_model, betas)
+            per_body = per_body + mt.loss(meas, betas, 0.0)
+        return per_body, v, meas
+
+    def loss_fn():
+        grot = Rot6dFunction.apply(params['global_rot'])
+        bpose = Rot6dFunction.apply(params['body_pose'])
+        per_body, v, meas = scan_loss(grot, bpose, params['betas'], params['transl'])
         return per_body, v, grot, bpose, meas
 
-    per_body, v, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
-    if meas is None and body_measurements is not None:
+    def fitted_measurements(meas, betas):
+        if meas is None and body_measurements is not None:
+            with torch.no_grad():
+                vs = body_model.forward_shape(betas=betas.detach())['v_shaped']
+                m = body_measurements.forward_vertices(vs, faces, circumference_derivative)['measurements']
+                meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+        return meas
+
+    if method == 'lm':
+        state = _fit_scan_lm(body_model, pts, w, params, rot0, anchor, int(iterations), sigma, s2m, m2s, pw, bw, mt)
+        rot = state['rot']
         with torch.no_grad():
-            vs = body_model.forward_shape(betas=params['betas'].detach())['v_shaped']
-            m = body_measurements.forward_vertices(vs, faces, circumference_derivative)['measurements']
-            meas = torch.stack([m[k]['tensor'] for k in NAMES], 1)
+            per_body, v, meas = scan_loss(rot[:, :1], rot[:, 1:], state['betas'], state['transl'])
+        res = _kp_lm_result(state, 'transl', vertices=v, loss=per_body)
+        meas = fitted_measurements(res.get('measurements', meas), state['betas'])
+        if meas is not None:
+            res['measurements'] = meas
+        return res
+    per_body, v, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
+    meas = fitted_measurements(meas, params['betas'])
     return _adam_result(params, grot, bpose, meas, vertices=v, loss=per_body)
+
+
+def _fit_scan_lm(body_model, pts, w, params, rot0, anchor, iterations, sigma, s2m, m2s, pw, bw, mt):
+    """The LM loop of fit_body_to_scan: per iteration the trial's vertex Jacobian, closest and (m2s > 0) nearest
+    points, with measurements their trial values and Jacobian, then one ops.fit_lm_scan_step.  Returns the state."""
+    from . import ops
+    device = pts.device
+    packed = body_model.packed(device)
+    B, N = pts.shape[:2]
+    nb, V, faces = params['betas'].shape[1], packed.V, body_model.faces_i32
+    P = 3 * 22 + nb + 3
+    trial = {'rot': rot0.clone(), 'betas': params['betas'].detach().clone().contiguous(),
+             'transl': params['transl'].detach().clone().contiguous()}
+    mk = lambda *s, dtype=torch.float32: torch.empty(*s, dtype=dtype, device=device)  # noqa: E731
+    state = {'rot': mk(B, 22, 3, 3), 'betas': mk(B, nb), 'transl': mk(B, 3), 'A': mk(B, P, P, dtype=torch.float64),
+             'g': mk(B, P, dtype=torch.float64), 'loss': mk(B), 'lambda': mk(B),
+             'accepted': torch.zeros(B, dtype=torch.int32, device=device)}
+    if mt is not None:
+        state.update(mt.state(nb, device))
+    if B == 0:
+        return state
+    if mt is not None:
+        mt.prime(body_model)
+    ws = ops.fit_lm_scan_workspace(B, N, V, P, device)
+    tree = ops.ScanTree()
+    for it in range(iterations + 1):
+        v, jac = ops.smplx_vertex_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
+        face, bary, _ = ops.closest_points(v, faces, pts, w, tree)
+        nearest = ops.nearest_points(v, pts, w)[0] if m2s > 0 else None
+        meas = None
+        if mt is not None:
+            tm, tmj = mt.trial(packed, body_model, trial['betas'])
+            meas = (mt.tgt, mt.wt, tm, tmj)
+        ops.fit_lm_scan_step(state, trial, pts, w, faces, sigma, s2m, m2s, pw, bw, LM_UP, LM_DOWN, it == 0, v, jac, face,
+                             bary, nearest, ws, pose_anchor=anchor if pw > 0 else None, meas=meas)
+    return state
 
 
 def main(argv=None):
@@ -1498,7 +1571,8 @@ def main(argv=None):
     p.add_argument('--meas-vertices-path', dest='meas_vertices_path', type=str, default=None)
     p.add_argument('--betas-weight', dest='betas_weight', type=float, default=0.0)
     p.add_argument('--method', choices=('adam', 'lm'), default='adam',
-                   help='optimiser: Adam, or batched Levenberg-Marquardt on the measurement Jacobian')
+                   help='optimiser: Adam, or batched Levenberg-Marquardt on the measurement, keypoint or vertex '
+                        'Jacobian')
     p.add_argument('--circumference-derivative', dest='circumference_derivative', choices=CIRCUMFERENCE_DERIVATIVES,
                    default='reference', help="how the circumferences are differentiated: the reference's autograd "
                                              "semantics, or their exact derivative")
@@ -1584,7 +1658,7 @@ def main(argv=None):
                                model_to_scan_weight=a.model_to_scan_weight, robust_sigma=a.robust_sigma,
                                pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight,
                                body_measurements=BodyMeasurements(cfg).cuda(), measurements=targets,
-                               circumference_derivative=a.circumference_derivative)
+                               circumference_derivative=a.circumference_derivative, method=a.method)
         return _save_result(a.output, res, {'bodies': int(points.shape[0]), 'points': int(points.shape[1])},
                             names=np.array(NAMES))
     bm = BodyMeasurements(cfg).cuda()

@@ -480,6 +480,30 @@ def smplx_keypoint_jacobian(model: SmplxModel, betas, rot, transl=None, expr=Non
     return kp, jac
 
 
+def smplx_vertex_jacobian(model: SmplxModel, betas, rot, transl=None):
+    """Every posed vertex (B, V, 3) (+ transl) and its Jacobian (B, V, 3, P), P = 3 n_rot + NB + 3, with the columns of
+    smplx_keypoint_jacobian, in one launch (include/shapy_b200.h, shapy_smplx_vertex_jacobian).  The Jacobian takes
+    4 V 3 P bytes per body: 9.9 MB at V = 10475 and P = 79, 635 MB at B = 64.  Returns (vertices, jac)."""
+    betas = _cuda_f32(betas, 'betas')
+    rot = _cuda_f32(rot, 'rot')
+    B, n_rot = rot.shape[0], rot.shape[1]
+    if rot.dim() != 4 or rot.shape[2:] != (3, 3) or betas.shape != (B, model.NB):
+        raise RuntimeError(f'rot must be (B, n_rot, 3, 3) and betas ({B}, {model.NB}), got {tuple(rot.shape)} and '
+                           f'{tuple(betas.shape)}')
+    transl = None if transl is None else _cuda_f32(transl, 'transl')
+    if transl is not None and transl.shape != (B, 3):
+        raise RuntimeError(f'transl must be ({B}, 3), got {tuple(transl.shape)}')
+    dev = betas.device
+    verts = torch.empty(B, model.V, 3, dtype=torch.float32, device=dev)
+    jac = torch.empty(B, model.V, 3, 3 * n_rot + model.NB + 3, dtype=torch.float32, device=dev)
+    if B == 0:
+        return verts, jac
+    with torch.cuda.device(dev):
+        check(lib().shapy_smplx_vertex_jacobian(model.handle, ptr(betas), ptr(rot), n_rot, ptr(transl), B, ptr(verts),
+                                                ptr(jac), stream_ptr()), 'smplx_vertex_jacobian')
+    return verts, jac
+
+
 def _smplx_keypoint_jacobian_expr(model, betas, rot, transl, expr):
     betas, rot, expr = _cuda_f32(betas, 'betas'), _cuda_f32(rot, 'rot'), _cuda_f32(expr, 'expression')
     B, n_rot = rot.shape[0], rot.shape[1]
@@ -860,6 +884,76 @@ def closest_points_backward(vertices, faces_i32, points, face_idx, bary, grad_sq
                                                   ptr(face_idx), ptr(bary), ptr(g), ptr(grad), stream_ptr()),
               'closest_points_backward')
     return grad
+
+
+def fit_lm_scan_workspace(B, N, V, P, device):
+    """The scratch of fit_lm_scan_step (include/shapy_b200.h, shapy_fit_lm_scan_workspace_bytes): a uint8 CUDA tensor,
+    allocated once before an LM loop."""
+    return _workspace(lib().shapy_fit_lm_scan_workspace_bytes(int(B), int(N), int(V), int(P)), device)
+
+
+def fit_lm_scan_step(state, trial, points, weights, faces_i32, robust_sigma, scan_to_model_weight,
+                     model_to_scan_weight, pose_prior_weight, betas_weight, lambda_up, lambda_down, first,
+                     trial_vertices, trial_jac, trial_face_idx, trial_bary, trial_nearest, workspace, pose_anchor=None,
+                     meas=None):
+    """One Levenberg-Marquardt step per body of the scan fit (include/shapy_b200.h, shapy_fit_lm_scan_step), in place.
+    state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB), 'transl' (B, 3), 'A' (B, P, P) and 'g' (B, P) float64, 'loss',
+    'lambda' (B,), 'accepted' (B,) int32}, with meas also 'meas' (B, 5) and 'meas_jac' (B, 5, NB); trial: {'rot',
+    'betas', 'transl'}, the evaluated trial on entry and the next trial on return.  points (B, N, 3), weights (B, N),
+    faces_i32 (F, 3); the trial's vertices and Jacobian (smplx_vertex_jacobian, with transl), closest points
+    (closest_points) and nearest points (nearest_points; None when model_to_scan_weight is 0).  robust_sigma None or
+    inf: least squares.  meas: None or (meas_targets, meas_weights, trial_meas, trial_meas_jac).  workspace:
+    fit_lm_scan_workspace(B, N, V, P)."""
+    what = 'fit_lm_scan_step'
+    B, n_rot = trial['rot'].shape[:2]
+    nb, (N, V) = trial['betas'].shape[1], (points.shape[1], trial_vertices.shape[1])
+    P = 3 * n_rot + nb + 3
+    sigma = float('inf') if robust_sigma is None else float(robust_sigma)
+    if not (sigma > 0 and pose_prior_weight >= 0 and betas_weight >= 0 and 0 <= scan_to_model_weight < float('inf')
+            and 0 <= model_to_scan_weight < float('inf') and lambda_up >= 1 and lambda_down >= 1):
+        raise ValueError(f'{what}: robust_sigma must be > 0, the term weights finite and >= 0, the prior weights >= 0 '
+                         'and lambda_up and lambda_down >= 1')
+    if pose_prior_weight > 0 and pose_anchor is None:
+        raise ValueError(f'{what}: a pose prior needs pose_anchor')
+    if model_to_scan_weight > 0 and trial_nearest is None:
+        raise ValueError(f'{what}: the model -> scan term needs trial_nearest')
+    mkeys = ['meas', 'meas_jac'] if meas is not None else []
+    f32 = [state[k] for k in ['rot', 'betas', 'transl', 'loss', 'lambda'] + mkeys] + \
+        [trial[k] for k in ('rot', 'betas', 'transl')] + [points, weights, trial_vertices, trial_jac, trial_bary] + \
+        [t for t in (pose_anchor,) if t is not None] + list(meas or ())
+    _check_step_tensors(what, f32, 'the state, trial, points, weights, vertices, Jacobian, barycentrics and anchor',
+                        state['accepted'])
+    for t in [state['A'], state['g']]:
+        if not (t.is_cuda and t.is_contiguous() and t.dtype == torch.float64):
+            raise RuntimeError(f"{what}: state['A'] and state['g'] must be contiguous float64 CUDA tensors")
+    for t in [faces_i32, trial_face_idx] + ([] if trial_nearest is None else [trial_nearest]):
+        if not (torch.is_tensor(t) and t.is_cuda and t.is_contiguous() and t.dtype == torch.int32):
+            raise RuntimeError(f'{what}: faces, face_idx and nearest must be contiguous int32 CUDA tensors')
+    shapes_ok = (points.shape == (B, N, 3) and weights.shape == (B, N) and trial_vertices.shape == (B, V, 3) and
+                 trial_jac.shape == (B, V, 3, P) and trial_face_idx.shape == (B, N) and trial_bary.shape == (B, N, 3)
+                 and (trial_nearest is None or trial_nearest.shape == (B, V)) and state['A'].shape == (B, P, P) and
+                 state['g'].shape == (B, P) and (pose_anchor is None or pose_anchor.shape == (B, n_rot, 3, 3)))
+    if not shapes_ok:
+        raise RuntimeError(f'{what}: points must be ({B}, {N}, 3), weights, face_idx ({B}, {N}), bary ({B}, {N}, 3), '
+                           f'vertices ({B}, {V}, 3), jac ({B}, {V}, 3, {P}), nearest ({B}, {V}), A ({B}, {P}, {P}), '
+                           f'g ({B}, {P}) and pose_anchor ({B}, {n_rot}, 3, 3)')
+    if meas is not None and not _meas_step_shapes_ok(state, meas[2], meas[3], meas[0], meas[1], B, nb):
+        raise RuntimeError(f'{what}: meas_jac must be ({B}, 5, {nb}) and the measurements, their targets and weights '
+                           f'({B}, 5)')
+    if B == 0:
+        return
+    m = list(meas) if meas is not None else [None] * 4
+    with torch.cuda.device(points.device):
+        check(lib().shapy_fit_lm_scan_step(
+            B, N, V, n_rot, nb, ptr(points), ptr(weights), ptr(faces_i32), ptr(pose_anchor), sigma,
+            float(scan_to_model_weight), float(model_to_scan_weight), float(pose_prior_weight), float(betas_weight),
+            ptr(m[0]), ptr(m[1]), float(lambda_up), float(lambda_down), int(bool(first)),
+            *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'A', 'g')],
+            *[ptr(state.get(k)) for k in ('meas', 'meas_jac')],
+            *[ptr(state[k]) for k in ('loss', 'lambda', 'accepted')],
+            *[ptr(trial[k]) for k in ('rot', 'betas', 'transl')], ptr(trial_vertices), ptr(trial_jac),
+            ptr(trial_face_idx), ptr(trial_bary), ptr(trial_nearest), ptr(m[2]), ptr(m[3]), ptr(workspace),
+            workspace.numel(), stream_ptr()), what)
 
 
 # -------------------------------------------------------------------------------------------- head
