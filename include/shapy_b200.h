@@ -734,9 +734,15 @@ double shapy_hrnet_flops(const shapy_hrnet_t *p, int batch, int height, int widt
 
 /* Standalone conv for unit tests of the implicit-GEMM kernel: x (B,H,W,Cin) fp32 NHWC device,
  * y (B,Ho,Wo,Cout) fp32 NHWC device, res optional (same shape as y).  engine: 0 = wgmma with the path the network
- * would take, 1 = SIMT, 2 = wgmma per-tap path, 3 = wgmma halo-resident path (error where it does not apply). */
+ * would take, 1 = SIMT, 2 = wgmma per-tap path, 3 = wgmma halo-resident path (error where it does not apply).
+ * Views (0 = dense): in_ctot > 0 gives x in_ctot channels per pixel, of which the conv reads in_coff .. in_coff + cin;
+ * out_ctot > 0 writes the conv into channels out_coff .. out_coff + cout of (batch + 1, Ho, Wo, out_ctot) planes
+ * filled with NaN beforehand, and y returns all of them (batch + 1, Ho, Wo, out_ctot).  plan (optional, int[3]):
+ * the plan built, as the engine digits that force it: path (2, 3 or 4), schedule (1 cooperative, 2 ping-pong), cout
+ * tile; -1 each for the SIMT engine. */
 int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, const float *res, int batch, int height,
-                    int width, int relu, int mode, int engine, float *y, void *stream);
+                    int width, int relu, int mode, int engine, int in_ctot, int in_coff, int out_ctot, int out_coff,
+                    int *plan, float *y, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Input stage (SURVEY.md 8f rank 1): uint8 full images + crop windows -> normalised fp32 NCHW crops.

@@ -194,8 +194,8 @@ _SIGS = {
     'shapy_point_error_aligned': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, C.POINTER(c_int), c_int, c_void_p, c_void_p,
                                           c_void_p, c_size_t, c_void_p]),
     'shapy_regress_points': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
-    'shapy_conv_test': (c_int, [C.POINTER(ConvDesc), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                                c_void_p, c_void_p]),
+    'shapy_conv_test': (c_int, [C.POINTER(ConvDesc), c_void_p, c_void_p] + [c_int] * 10
+                        + [C.POINTER(c_int), c_void_p, c_void_p]),
 }
 
 EXPORTS = sorted(_SIGS)

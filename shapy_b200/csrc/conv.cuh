@@ -78,6 +78,8 @@ void wgmma_stamps_print(const WgmmaPlan *p);
 #endif
 void wgmma_plan_destroy(WgmmaPlan *p);
 void wgmma_plan_stats(const WgmmaPlan *p, double *tma_bytes, double *mma_flops);   // per launch, as planned
+// the plan as built: data path (WGMMA_PER_TAP, WGMMA_HALO or WGMMA_RESIDENT), ping-pong (1) or cooperative (0), cout tile
+void wgmma_plan_describe(const WgmmaPlan *p, int *path, int *pingpong, int *nt);
 int wgmma_plan_launch(const WgmmaPlan *p, cudaStream_t st, bool pdl);   // pdl: programmatic dependent launch
 
 }  // namespace shapy

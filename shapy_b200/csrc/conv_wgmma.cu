@@ -599,6 +599,12 @@ void wgmma_plan_stats(const WgmmaPlan *pl, double *tma_bytes, double *mma_flops)
   *mma_flops = pl->mma_flops;
 }
 
+void wgmma_plan_describe(const WgmmaPlan *pl, int *path, int *pingpong, int *nt) {
+  *path = pl->resident ? WGMMA_RESIDENT : (pl->halo ? WGMMA_HALO : WGMMA_PER_TAP);
+  *pingpong = pl->pingpong ? 1 : 0;
+  *nt = pl->NT;
+}
+
 static const int kNts[] = {128, 96, 64, 48, 32, 16};   // cout tiles with a kernel instantiation
 
 bool wgmma_supported(const ConvW &w, const ActView &in, const ActView &out) {

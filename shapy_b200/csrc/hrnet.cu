@@ -498,8 +498,13 @@ extern "C" double shapy_hrnet_flops(const shapy_hrnet_t *p, int B, int H, int W)
 
 // Standalone convolution on fp32 NHWC buffers (unit tests of both engines).
 extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, const float *res, int B, int H, int W,
-                               int relu, int mode, int engine, float *y, void *stream) {
+                               int relu, int mode, int engine, int in_ctot, int in_coff, int out_ctot, int out_coff,
+                               int *plan_out, float *y, void *stream) {
   SHAPY_REQUIRE(conv && x && y, "shapy_conv_test: null argument");
+  SHAPY_REQUIRE(in_ctot == 0 || (in_coff >= 0 && in_coff + conv->cin <= in_ctot),
+                "shapy_conv_test: input view of %d channels at %d in %d", conv->cin, in_coff, in_ctot);
+  SHAPY_REQUIRE(out_ctot == 0 || (out_coff >= 0 && out_coff + conv->cout <= out_ctot),
+                "shapy_conv_test: output view of %d channels at %d in %d", conv->cout, out_coff, out_ctot);
   cudaStream_t st = (cudaStream_t)stream;
   std::vector<void *> allocs;
   cudaError_t err = cudaSuccess;
@@ -522,11 +527,27 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
     if (mode && err == cudaSuccess) { err = cudaMalloc((void **)&v.lo, bytes); if (err == cudaSuccess) allocs.push_back(v.lo); }
     return v;
   };
-  ActView in = make(B, H, W, conv->cin), out = make(B, Ho, Wo, conv->cout), rv;
+  // in_ctot: x holds in_ctot channels per pixel, the convolution reads in_coff .. in_coff + cin.  out_ctot: the output
+  // is the slice out_coff .. out_coff + cout of B + 1 images of out_ctot channels, all filled with NaN first (0xFF
+  // bytes): y returns every channel of every image, so a write outside the slice, or to the image past B, shows.
+  ActView in = make(B, H, W, in_ctot ? in_ctot : conv->cin);
+  ActView out = make(out_ctot ? B + 1 : B, Ho, Wo, out_ctot ? out_ctot : conv->cout), rv;
   if (res) rv = make(B, Ho, Wo, conv->cout);
   if (err != cudaSuccess) { cleanup(); set_error("conv_test: %s", cudaGetErrorString(err)); return (int)err; }
   if ((rc = launch_nhwc_split(x, in, st))) { cleanup(); return rc; }
   if (res && (rc = launch_nhwc_split(res, rv, st))) { cleanup(); return rc; }
+  const ActView merged = out;
+  if (out_ctot) {
+    const size_t bytes = (size_t)out.N * Ho * Wo * out_ctot * sizeof(__half);
+    err = cudaMemsetAsync(out.hi, 0xFF, bytes, st);
+    if (err == cudaSuccess && out.lo) err = cudaMemsetAsync(out.lo, 0xFF, bytes, st);
+    if (err != cudaSuccess) { cleanup(); set_error("conv_test: %s", cudaGetErrorString(err)); return (int)err; }
+    out.N = B; out.C = conv->cout; out.coff = out_coff;
+  }
+  in.C = conv->cin; in.coff = in_ctot ? in_coff : 0;
+  // plan_out: path (2 per-tap, 3 halo, 4 weight-resident), schedule (1 cooperative, 2 ping-pong), cout tile: the digits
+  // of `engine` that force this plan; -1 for the SIMT engine
+  if (plan_out) plan_out[0] = plan_out[1] = plan_out[2] = -1;
   if (engine != 1) {
     // engine % 10: 0 = the path the network would take, 2 = per-tap, 3 = halo, 4 = weight-resident halo; engine / 10 %
     // 10: 0 = the planner's schedule, 1 = cooperative, 2 = ping-pong; engine / 100: the cout tile (0 = the planner's)
@@ -536,6 +557,13 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
                      (e_sched == 1 ? WGMMA_COOP : (e_sched == 2 ? WGMMA_PINGPONG : 0));
     plan = wgmma_plan_create(w, in, out, res ? &rv : nullptr, relu != 0, path, e_nt);
     if (!plan) { cleanup(); return SHAPY_ERR_UNSUPPORTED; }
+    if (plan_out) {
+      int p_path, p_pp, p_nt;
+      wgmma_plan_describe(plan, &p_path, &p_pp, &p_nt);
+      plan_out[0] = p_path == WGMMA_RESIDENT ? 4 : (p_path == WGMMA_HALO ? 3 : 2);
+      plan_out[1] = p_pp ? 2 : 1;
+      plan_out[2] = p_nt;
+    }
     rc = wgmma_plan_launch(plan, st, true);
     if (const char *reps_s = getenv("SHAPY_CONV_TEST_REPS")) {
 #ifdef SHAPY_CONV_STAMPS
@@ -568,7 +596,7 @@ extern "C" int shapy_conv_test(const shapy_conv_desc_t *conv, const float *x, co
   } else {
     rc = launch_conv_simt(w, in, out, res ? &rv : nullptr, relu != 0, st);
   }
-  if (!rc) rc = launch_nhwc_merge(out, y, false, st);
+  if (!rc) rc = launch_nhwc_merge(merged, y, false, st);
   cleanup();
   cudaError_t e2 = cudaGetLastError();
   if (!rc && e2 != cudaSuccess) { set_error("conv_test: %s", cudaGetErrorString(e2)); rc = (int)e2; }

@@ -4,6 +4,7 @@ PyTorch is used for device memory and streams only: every function takes CUDA fp
 the outputs with torch, and launches the hand-written sm_90a kernels on the current stream.  Nothing
 here computes with torch ops, and nothing falls back to the CPU: non-CUDA inputs raise.
 """
+import collections
 import ctypes as C
 import weakref
 
@@ -1079,14 +1080,30 @@ class HrnetPlan:
         return lib().shapy_hrnet_flops(self.handle, B, H, W)
 
 
-def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=False, mode=1, engine=0):
+class ConvPlan(collections.namedtuple('ConvPlan', 'path schedule nt')):
+    """A wgmma plan in conv_test's engine digits: path 2 per-tap, 3 halo, 4 weight-resident; schedule 1 cooperative,
+    2 ping-pong; nt the cout tile."""
+    @property
+    def engine(self):
+        """the conv_test engine number that forces this plan"""
+        return self.path + 10 * self.schedule + 100 * self.nt
+
+
+def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=False, mode=1, engine=0,
+              in_view=None, out_view=None, report=False):
     """Single convolution through either engine on fp32 NHWC tensors (unit tests).  engine: 0 = wgmma with the path
     the network would take, 1 = SIMT, 2 = wgmma per-tap path, 3 = wgmma halo-resident path, 4 = wgmma halo path with
     the weights resident in shared memory; + 10 forces the
-    cooperative consumer schedule of the wgmma engine, + 20 the ping-pong one; + 100 * NT forces its cout tile NT."""
+    cooperative consumer schedule of the wgmma engine, + 20 the ping-pong one; + 100 * NT forces its cout tile NT.
+    in_view=(ctot, coff): x has ctot channels and the convolution reads coff .. coff + cin of them.
+    out_view=(ctot, coff): the convolution writes channels coff .. coff + cout of (B + 1, Ho, Wo, ctot) planes filled
+    with NaN beforehand, and all of them are returned, the guard image B included.
+    report=True: returns (y, ConvPlan(path, schedule, nt)), the plan built in the engine digits above (-1 for SIMT)."""
     x = _cuda_f32(x_nhwc, 'x')
-    B, H, W, Cin = x.shape
-    Cout, _, k, _ = weight.shape
+    B, H, W, Cx = x.shape
+    Cout, Cin, k, _ = weight.shape
+    if Cx != (in_view[0] if in_view else Cin):
+        raise RuntimeError(f'x has {Cx} channels: expected {in_view[0] if in_view else Cin}')
     keep = []
 
     def hp(t):
@@ -1102,12 +1119,15 @@ def conv_test(x_nhwc, weight, bias=None, bn=None, stride=1, res_nhwc=None, relu=
         d.bn_weight, d.bn_bias, d.bn_mean, d.bn_var = hp(bn['weight']), hp(bn['bias']), hp(bn['mean']), hp(bn['var'])
         d.bn_eps = float(bn['eps'])
     Ho, Wo = (H // 2, W // 2) if stride == 2 else (H, W)
-    y = torch.empty(B, Ho, Wo, Cout, dtype=torch.float32, device=x.device)
+    y = torch.empty((B + 1, Ho, Wo, out_view[0]) if out_view else (B, Ho, Wo, Cout), dtype=torch.float32,
+                    device=x.device)
     res = None if res_nhwc is None else _cuda_f32(res_nhwc, 'res')
+    plan = (C.c_int * 3)()
     with torch.cuda.device(x.device):
-        check(lib().shapy_conv_test(C.byref(d), ptr(x), ptr(res), B, H, W, int(relu), mode, engine, ptr(y),
-                                    stream_ptr()), 'conv_test')
-    return y
+        check(lib().shapy_conv_test(C.byref(d), ptr(x), ptr(res), B, H, W, int(relu), mode, engine,
+                                    *(in_view or (0, 0)), *(out_view or (0, 0)), plan, ptr(y), stream_ptr()),
+              'conv_test')
+    return (y, ConvPlan(*plan)) if report else y
 
 
 def fit_lm_groups_workspace(B, G, n_rot, nb, device):

@@ -121,7 +121,8 @@ def test_hrnet_fp16_B32_vs_fp16_operand_reference(backbone):
     The two sides accumulate in different orders, so now and then an activation rounds to the neighbouring fp16 value;
     each such flip is as large as the rounding noise itself, so after ~110 layers the two fp16 realisations are as far
     from each other as either is from the fp32 network (measured: 1.1e-3 RMS, 2.5e-3 max on layer1).  The bars are
-    therefore fp16-noise sized; the per-layer check that cannot amplify (and does see a wrong tile at 1e-3) is
+    therefore fp16-noise sized; the per-layer checks that cannot amplify are tests/test_gpu_conv_layers.py (every
+    layer of this program, within a float64 per-element bound of half an fp16 ulp plus the accumulation error) and
     tests/test_gpu_conv.py::test_conv_fp16_benchmark_batch.  A wrong tile or a dropped tap here is O(1)."""
     bb = backbone.cuda().eval()
     bb.engine, bb.precision_mode = 0, 0

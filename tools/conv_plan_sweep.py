@@ -76,21 +76,21 @@ class StderrCapture:
         self.f.close()
 
 
-PLAN_RE = re.compile(r'\[wgmma\].*?: (\S+) (\S+) NT (\d+)')
+PATHS = {2: 'per-tap', 3: 'halo', 4: 'resident'}   # ops.ConvPlan digits
+SCHEDULES = {1: 'cooperative', 2: 'ping-pong'}
 TIME_RE = re.compile(r'\[conv_test\].*?: ([\d.]+) us/launch')
 STAMP_RE = re.compile(r'wait (\d+) mainloop (\d+) \(operand waits \d+\) drain (\d+) epilogue (\d+)')
 
 
 def run(ops, torch, x, w, r, s, mode, engine):
     with StderrCapture() as cap:
-        ops.conv_test(x, w, stride=s, res_nhwc=r, relu=True, mode=mode, engine=engine)
+        _, plan = ops.conv_test(x, w, stride=s, res_nhwc=r, relu=True, mode=mode, engine=engine, report=True)
         torch.cuda.synchronize()
-    plan, t = PLAN_RE.findall(cap.text), TIME_RE.findall(cap.text)
-    if not plan or not t:
-        raise RuntimeError(f'conv_test engine {engine}: no plan / timing line in\n{cap.text}')
+    t = TIME_RE.findall(cap.text)
+    if not t:
+        raise RuntimeError(f'conv_test engine {engine}: no timing line in\n{cap.text}')
     st = STAMP_RE.findall(cap.text)
-    path, sched, nt = plan[-1]
-    return (path, int(nt), sched), float(t[-1]), ('/'.join(st[-1]) if st else '')
+    return (PATHS[plan.path], plan.nt, SCHEDULES[plan.schedule]), float(t[-1]), ('/'.join(st[-1]) if st else '')
 
 
 def main():
@@ -120,7 +120,6 @@ def main():
                   ' | '.join(f'mode {m}: ' + ' '.join(f'{nt}{sc[0]}' for nt, sc in candidates(key[1], m)) for m in modes))
         return
     os.environ['SHAPY_CONV_TEST_REPS'] = str(a.reps)
-    os.environ['SHAPY_CONV_DEBUG'] = '1'
     import torch
     from shapy_b200 import ops
     q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
