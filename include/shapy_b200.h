@@ -19,6 +19,8 @@
  *   shapy_mmi_forward_f64  (float / float64)        + src/mesh_mesh_intersect_cuda_op.cu:969-1079
  *   shapy_closest_points, shapy_nearest_points, shapy_closest_points_backward   (no reference counterpart: the scan
  *                        terms of shapy_b200.fit.fit_body_to_scan, on the LBVH of shapy_mmi_forward)
+ *   shapy_self_collisions  (the self-collision pairs the reference's BVH gives SMPLify-X, on the scan LBVH)
+ *   shapy_penetration_*  DistanceFieldPenetrationLoss mesh-mesh-intersection/mesh_mesh_intersection/loss.py:201-317
  *   shapy_head_*         IterativeRegression.forward regressor/human_shape/models/common/networks.py:536-592
  *   shapy_hrnet_*        HighResolutionNet.forward  regressor/human_shape/models/backbone/hrnet.py:426-498
  *   shapy_p2p_error      v2vhdError.__call__        regressor/human_shape/utils/metrics.py:368-456
@@ -648,6 +650,29 @@ int shapy_fit_lm_scan_step(int batch, int num_points, int num_verts, int n_rot, 
                            const float *trial_bary, const int32_t *trial_nearest, const float *trial_meas,
                            const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream);
 
+/* shapy_fit_lm_scan_step with the self-penetration term of the fit: weight penetration_weight times the distance-field
+ * penetration loss of shapy_penetration_forward (penalize_outside, linear_max 1000) at penetration_sigma, at the pair
+ * rows pen_pairs (B,C,2) of shapy_self_collisions found on the trial's vertices (faces (F,3), num_faces F).  Each of a
+ * pair's six points with phi != 0 is one row: residual phi, weight penetration_weight, Jacobian the sum over the point
+ * and the cone triangle's three vertices of (d phi / d x)^T J_x, phi and its derivatives in fp64 from the float
+ * vertices.  Their chunks (1024 points each) follow the vertex chunks in the workspace (>=
+ * shapy_fit_lm_scan_penetration_workspace_bytes(B, N, V, P, C)); the step adds their loss after the model -> scan
+ * term and their sums to the data rows, so the trial loss that accept / reject compares includes the term.  A row
+ * whose first index is < 0, or with an index outside [0, F), adds nothing.  Everything else, including the error
+ * codes, is shapy_fit_lm_scan_step's; a negative or non-finite weight or sigma <= 0 is SHAPY_ERR_ARG. */
+size_t shapy_fit_lm_scan_penetration_workspace_bytes(int batch, int num_points, int num_verts, int num_params,
+                                                     int num_pairs);
+int shapy_fit_lm_scan_penetration_step(
+    int batch, int num_points, int num_verts, int n_rot, int nb, const float *points, const float *weights,
+    const int32_t *faces, int num_faces, const float *pose_anchor, float robust_sigma, float scan_to_model_weight,
+    float model_to_scan_weight, float pose_prior_weight, float betas_weight, const float *meas_targets,
+    const float *meas_weights, const int32_t *pen_pairs, int num_pairs, float penetration_weight,
+    float penetration_sigma, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl,
+    double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_vertices,
+    const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary, const int32_t *trial_nearest,
+    const float *trial_meas, const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Backward of sq_dist of shapy_closest_points with respect to the vertices, face_idx and bary held at the forward's
  * values: grad_vertices (B,V,3) = sum over the points of 2 g_i (q_i - p_i) bary_{i,c} at corner c of face_idx_i, q_i =
  * sum_c bary_{i,c} x_c recomputed from `vertices`.  inc_ptr (V+1) / inc (3F) is the vertex -> (3 face + corner)
@@ -659,6 +684,42 @@ int shapy_closest_points_backward(const float *vertices, const int32_t *faces, c
                                   const int32_t *inc, int batch, int num_verts, int num_faces, const float *points,
                                   int num_points, const int32_t *face_idx, const float *bary,
                                   const float *grad_sq_dist, float *grad_vertices, void *stream);
+
+/* ------------------------------------------------------------ self-penetration */
+/* Intersecting face pairs of each posed mesh: vertices (B,V,3), faces (F,3) int32 (indices < V).  T_f is the float
+ * triangle of face f.  A pair (f, g), f < g, is kept when the faces share no vertex index, box_overlap(tri_box(T_f),
+ * tri_box(T_g)) (inclusive) and sat11(T_f, T_g) hold (the predicates of shapy_mmi_forward), and, with part_labels (F)
+ * int32 in [0, 64) and ignored_part_pairs (64 uint64 on the device, bit j of word i set for an ignored label pair
+ * (i, j), symmetric) non-NULL, the pair of labels is not ignored.  Rows pairs (B,max_pairs,2) int32 in ascending
+ * (f, g) order, padded with -1; count (B) the number found, which may exceed max_pairs (the first max_pairs are
+ * written).  The result is a function of the body's triangles, the faces and the filter only: not of the tree, the
+ * traversal or the rest of the batch, and bit-identical run to run.  The tree is the LBVH of shapy_closest_points over
+ * the posed triangles, at the start of the workspace (>= shapy_self_collisions_workspace_bytes(B, F)), so the same
+ * workspace serves both calls; refit != 0 keeps a tree built there for the same B and faces and recomputes its boxes.
+ * Three launches after the tree: a count per face, a scan per body, and a write per face.  F > 32768 returns
+ * SHAPY_ERR_UNSUPPORTED; B = 0 launches nothing. */
+size_t shapy_self_collisions_workspace_bytes(int batch, int num_faces);
+int shapy_self_collisions(const float *vertices, const int32_t *faces, int batch, int num_verts, int num_faces,
+                          const int32_t *part_labels, const uint64_t *ignored_part_pairs, int refit, int max_pairs,
+                          int32_t *pairs, int32_t *count, void *workspace, size_t workspace_bytes, void *stream);
+
+/* The conical distance-field penetration loss of SMPLify-X (mesh-mesh-intersection/mesh_mesh_intersection/loss.py,
+ * DistanceFieldPenetrationLoss, vectorized=True) per body: loss (B) = the sum over the rows of pairs (B,C,2) int32
+ * (receiver, intruder) of the six points' phi^2, phi = ([a < 1] ((1 - a) psi)^2)^2 of each intruder vertex in the
+ * receiver's circumcircle cone and of each receiver vertex in the intruder's (see csrc/penetration.cu), at sigma,
+ * penalize_outside and linear_max.  A row whose first index is < 0 is skipped, as one with an index outside [0, F).
+ * The backward gives grad_vertices (B,V,3) of grad_loss (B) . loss; workspace >= shapy_penetration_workspace_bytes.
+ * One launch each, one CTA per body, no atomics: bit-identical run to run, a body independent of the batch.  C > 4096
+ * returns SHAPY_ERR_UNSUPPORTED; sigma <= 0 or a NaN linear_max SHAPY_ERR_ARG; C = 0 gives a zero loss and
+ * gradient. */
+int shapy_penetration_forward(const float *vertices, const int32_t *faces, int batch, int num_verts, int num_faces,
+                              const int32_t *pairs, int num_pairs, float sigma, int penalize_outside, float linear_max,
+                              float *loss, void *stream);
+size_t shapy_penetration_workspace_bytes(int batch, int num_pairs);
+int shapy_penetration_backward(const float *vertices, const int32_t *faces, int batch, int num_verts, int num_faces,
+                               const int32_t *pairs, int num_pairs, float sigma, int penalize_outside,
+                               float linear_max, const float *grad_loss, float *grad_vertices, void *workspace,
+                               size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------ regression head */
 /* params_out (num_stages, B, P).  W0 (H0, F+P), W1 (H1, H0), W2 (P, H1) row-major as nn.Linear stores

@@ -17,7 +17,7 @@ def install_as_reference():
     `mesh_mesh_intersection` and `body_measurements` in sys.modules so that the reference's
     regressor/demo.py and regressor/evaluate.py import the H100 path unchanged."""
     import importlib
-    from . import body_measurements, mesh_mesh_intersect_cuda, mesh_mesh_intersection
+    from . import body_measurements, mesh_mesh_intersect_cuda, mesh_mesh_intersection, mesh_mesh_intersection_loss
     models = importlib.import_module('shapy_b200.human_shape.models')
     sys.modules['human_shape.models'] = models
     for sub in ('build', 'backbone', 'backbone.hrnet', 'body_heads', 'body_heads.registry', 'body_models',
@@ -28,4 +28,6 @@ def install_as_reference():
         setattr(sys.modules['human_shape'], 'models', models)
     sys.modules['mesh_mesh_intersect_cuda'] = mesh_mesh_intersect_cuda
     sys.modules['mesh_mesh_intersection'] = mesh_mesh_intersection
+    sys.modules['mesh_mesh_intersection.loss'] = mesh_mesh_intersection_loss
+    mesh_mesh_intersection.loss = mesh_mesh_intersection_loss
     sys.modules['body_measurements'] = body_measurements

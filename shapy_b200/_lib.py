@@ -166,9 +166,22 @@ _SIGS = {
     'shapy_nearest_points': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_size_t, c_void_p]),
     'shapy_closest_points_backward': (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 5),
+    'shapy_self_collisions_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'shapy_self_collisions': (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_int]
+                              + [c_void_p] * 3 + [c_size_t, c_void_p]),
+    'shapy_penetration_forward': (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p, c_int, C.c_float, c_int,
+                                                                             C.c_float, c_void_p, c_void_p]),
+    'shapy_penetration_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'shapy_penetration_backward': (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p, c_int, C.c_float, c_int,
+                                                                              C.c_float] + [c_void_p] * 3
+                                   + [c_size_t, c_void_p]),
     'shapy_fit_lm_scan_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'shapy_fit_lm_scan_step': (c_int, [c_int] * 5 + [c_void_p] * 4 + [C.c_float] * 5 + [c_void_p] * 2
                                + [C.c_float, C.c_float, c_int] + [c_void_p] * 21 + [c_size_t, c_void_p]),
+    'shapy_fit_lm_scan_penetration_workspace_bytes': (c_size_t, [c_int] * 5),
+    'shapy_fit_lm_scan_penetration_step': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p] + [C.c_float] * 5
+                                           + [c_void_p] * 3 + [c_int, C.c_float, C.c_float, C.c_float, C.c_float, c_int]
+                                           + [c_void_p] * 21 + [c_size_t, c_void_p]),
     'shapy_head_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     'shapy_head_forward': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,

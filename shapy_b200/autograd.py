@@ -9,6 +9,8 @@ only).
     Rot6dFunction.apply(raw)                    raw (B,6n) -> (B,n,3,3)
     ClosestPointsFunction.apply(faces_i32, vertices, points, weights)
                                                 scan points (B,N,3) on posed meshes (B,V,3) -> sq_dist (B,N)
+    PenetrationFunction.apply(vertices, faces_i32, pairs, sigma, penalize_outside, linear_max)
+                                                self-penetration loss at fixed face pairs (B,C,2) -> (B,)
 
 The forward of each is the same launches as the no-grad path; the backward is the matching CUDA adjoint
 (measure_smem_kernel in gradient mode, the shape-blend adjoint, shapy_smplx_backward which recomputes the posed
@@ -120,6 +122,25 @@ class ClosestPointsFunction(torch.autograd.Function):
         faces_i32, vertices, points, face, bary = ctx.saved_tensors
         g = _ops.closest_points_backward(vertices, faces_i32, points, face, bary, grad_d2.contiguous())
         return None, g, None, None, None
+
+
+class PenetrationFunction(torch.autograd.Function):
+    """PenetrationFunction.apply(vertices, faces_i32, pairs, sigma, penalize_outside, linear_max) -> (B,): the
+    distance-field penetration loss of each body at the (receiver, intruder) face rows pairs (B, C, 2)
+    (ops.penetration_forward), differentiable in the vertices; the pairs are constants of the call."""
+
+    @staticmethod
+    def forward(ctx, vertices, faces_i32, pairs, sigma, penalize_outside, linear_max):
+        ctx.args = (float(sigma), bool(penalize_outside), float(linear_max))
+        ctx.save_for_backward(vertices, faces_i32, pairs)
+        return _ops.penetration_forward(vertices, faces_i32, pairs, *ctx.args)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_loss):
+        vertices, faces_i32, pairs = ctx.saved_tensors
+        g = _ops.penetration_backward(vertices, faces_i32, pairs, grad_loss.contiguous(), *ctx.args)
+        return g, None, None, None, None, None
 
 
 def wants_grad(t) -> bool:

@@ -791,3 +791,184 @@ extern "C" int shapy_closest_points_backward(const float *vertices, const int32_
   SHAPY_LAUNCH_CHECK();
   return SHAPY_OK;
 }
+
+// ======================================================================================================= self-collisions
+// Intersecting face pairs (f, g), f < g, of each posed mesh on the scan tree above (the soup of shapy_closest_points):
+//   self_face_kernel<false>  ONE THREAD PER FACE f: counts the faces g > f whose leaf box overlaps f's and that pass
+//                            self_pair
+//   self_scan_kernel    ONE CTA PER BODY: exclusive scan of the per-face counts -> each face's first output row
+//   self_face_kernel<true>   ONE THREAD PER FACE: the face's pairs in increasing g, each traversal keeping the kSelfSel
+//                       smallest g past the last one written, for as many rows as are left below max_pairs
+// A pair is a function of the two triangles, the faces and the part filter only, so the rows do not depend on the
+// tree's shape or on the rest of the batch, and every sum is over integers.
+namespace shapy {
+
+constexpr int kSelfSel = 8;
+
+// Visits every leaf whose box overlaps qb (inclusive test), depth first.
+template <typename Fn>
+__device__ __forceinline__ void box_traverse(const BvhNode *nodes, const float *leaf_box, int P, const mmi::Box &qb,
+                                             Fn &&leaf) {
+  if (P == 1) {
+    if (overlap6(qb, leaf_box)) leaf(0);
+    return;
+  }
+  int st[kScanStack];
+  int sp = 0, node = 0;
+  while (true) {
+    const int link[2] = {__ldg(&nodes[node].left), __ldg(&nodes[node].right)};
+    bool go[2];
+    for (int c = 0; c < 2; ++c) {
+      const float *s = link[c] < 0 ? leaf_box + (size_t)(~link[c]) * 6 : nodes[link[c]].lo;
+      float bx[6];
+      for (int k = 0; k < 6; ++k) bx[k] = __ldg(s + k);
+      const bool ov = overlap6(qb, bx);
+      if (ov && link[c] < 0) leaf(~link[c]);
+      go[c] = ov && link[c] >= 0;
+    }
+    if (go[0] && go[1]) {
+      st[sp++] = link[1];
+      node = link[0];
+    } else if (go[0] || go[1]) {
+      node = link[go[0] ? 0 : 1];
+    } else {
+      if (sp == 0) break;
+      node = st[--sp];
+    }
+  }
+}
+
+// f < g, boxes known to overlap: no shared vertex, labels not an ignored pair, and the reference's 11-axis SAT with
+// T_f first.  ignored: 64 masks, bit j of ignored[i] set when the label pair (i, j) is ignored (symmetric).
+__device__ __forceinline__ bool self_pair(const int *__restrict__ faces, const int *__restrict__ labels,
+                                          const unsigned long long *__restrict__ ignored, const float *sb, int f,
+                                          int g, const int fv[3], const mmi::TriT<float> &tf) {
+  const int g0 = __ldg(faces + 3 * g), g1 = __ldg(faces + 3 * g + 1), g2 = __ldg(faces + 3 * g + 2);
+  for (int k = 0; k < 3; ++k)
+    if (fv[k] == g0 || fv[k] == g1 || fv[k] == g2) return false;
+  if (labels && ((__ldg(ignored + __ldg(labels + f)) >> __ldg(labels + g)) & 1ull)) return false;
+  return mmi::sat11(tf, ld_tri(sb + (size_t)g * 9));
+}
+
+struct SelfWs {
+  ScanWs scan;
+  int *counts;   // [B][F]
+  int *offsets;  // [B][F]
+};
+
+static size_t self_ws_layout(int B, int F, SelfWs *w, char *base) {
+  size_t off = scan_ws_layout(B, F, w ? &w->scan : nullptr, base);
+  const size_t n = align_up((size_t)B * F * 4, 256);
+  if (w) { w->counts = (int *)(base + off); w->offsets = (int *)(base + off + n); }
+  return off + 2 * n;
+}
+
+template <bool kWrite>
+__global__ void __launch_bounds__(128) self_face_kernel(const int *__restrict__ faces, int F, SelfWs w,
+                                                        const int *__restrict__ labels,
+                                                        const unsigned long long *__restrict__ ignored, int max_pairs,
+                                                        int *__restrict__ pairs) {
+  const int b = blockIdx.y;
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const size_t o = (size_t)b * F + f;
+  const float *sb = w.scan.soup + (size_t)b * F * 9;
+  const int *ids = w.scan.bvh.ids + (size_t)b * F;
+  const BvhNode *nodes = w.scan.bvh.nodes + (size_t)b * (F - 1);
+  const float *leaf_box = w.scan.bvh.leaf_box + (size_t)b * F * 6;
+  const mmi::TriT<float> tf = ld_tri(sb + (size_t)f * 9);
+  const mmi::Box qb = mmi::tri_box(tf);
+  const int fv[3] = {__ldg(faces + 3 * f), __ldg(faces + 3 * f + 1), __ldg(faces + 3 * f + 2)};
+  if (!kWrite) {
+    int n = 0;
+    box_traverse(nodes, leaf_box, F, qb, [&](int j) {
+      const int g = __ldg(ids + j);
+      if (g > f && self_pair(faces, labels, ignored, sb, f, g, fv, tf)) ++n;
+    });
+    w.counts[o] = n;
+    return;
+  }
+  const int first = w.offsets[o];
+  const int room = min(w.counts[o], max_pairs - first);
+  int *out = pairs + ((size_t)b * max_pairs + first) * 2;
+  int last = f;
+  for (int k = 0; k < room;) {
+    int sel[kSelfSel];
+    int ns = 0;
+    box_traverse(nodes, leaf_box, F, qb, [&](int j) {
+      const int g = __ldg(ids + j);
+      if (g <= last || (ns == kSelfSel && g >= sel[kSelfSel - 1])) return;
+      if (!self_pair(faces, labels, ignored, sb, f, g, fv, tf)) return;
+      int i = ns < kSelfSel ? ns++ : kSelfSel - 1;  // insertion into the sorted kSelfSel smallest
+      for (; i > 0 && sel[i - 1] > g; --i) sel[i] = sel[i - 1];
+      sel[i] = g;
+    });
+    if (ns == 0) break;  // not reached: the count pass found `room` more
+    for (int i = 0; i < ns && k < room; ++i, ++k) {
+      out[2 * k] = f;
+      out[2 * k + 1] = sel[i];
+    }
+    last = sel[ns - 1];
+  }
+}
+
+__global__ void __launch_bounds__(1024) self_scan_kernel(int F, SelfWs w, int *__restrict__ count) {
+  __shared__ int part[1024];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const int per = (F + 1023) / 1024, lo = min(F, t * per), hi = min(F, lo + per);
+  const int *c = w.counts + (size_t)b * F;
+  int s = 0;
+  for (int i = lo; i < hi; ++i) s += c[i];
+  part[t] = s;
+  __syncthreads();
+  for (int d = 1; d < 1024; d <<= 1) {  // inclusive Hillis-Steele scan of the thread sums
+    const int v = t >= d ? part[t - d] : 0;
+    __syncthreads();
+    part[t] += v;
+    __syncthreads();
+  }
+  int run = part[t] - s;
+  int *off = w.offsets + (size_t)b * F;
+  for (int i = lo; i < hi; ++i) { off[i] = run; run += c[i]; }
+  if (t == 1023) count[b] = part[1023];
+}
+
+}  // namespace shapy
+
+extern "C" size_t shapy_self_collisions_workspace_bytes(int B, int F) {
+  if (B <= 0 || F <= 0) return 0;
+  return self_ws_layout(B, F, nullptr, nullptr) + 256;
+}
+
+extern "C" int shapy_self_collisions(const float *vertices, const int32_t *faces, int B, int V, int F,
+                                     const int32_t *part_labels, const uint64_t *ignored_part_pairs, int refit,
+                                     int max_pairs, int32_t *pairs, int32_t *count, void *workspace,
+                                     size_t workspace_bytes, void *stream) {
+  const char *name = "shapy_self_collisions";
+  SHAPY_REQUIRE(B >= 0 && V > 0 && F > 0 && max_pairs >= 0, "%s: bad sizes", name);
+  if (int rc = scan_limit(name, "faces", F)) return rc;
+  if (B == 0) return SHAPY_OK;
+  SHAPY_REQUIRE(vertices && faces && count && (pairs || max_pairs == 0), "%s: null argument", name);
+  SHAPY_REQUIRE(!part_labels == !ignored_part_pairs, "%s: part_labels and ignored_part_pairs go together", name);
+  SHAPY_REQUIRE(workspace && workspace_bytes >= shapy_self_collisions_workspace_bytes(B, F), "%s: workspace too small",
+                name);
+  cudaStream_t st = (cudaStream_t)stream;
+  SelfWs w;
+  self_ws_layout(B, F, &w, scan_base(workspace));
+  const size_t n = (size_t)B * F * 3;
+  scan_mesh_soup_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(vertices, faces, V, F, n, w.scan.soup);
+  SHAPY_LAUNCH_CHECK();
+  if (int rc = scan_tree(w.scan, B, F, refit != 0, st)) return rc;
+  const dim3 grid(ceil_div(F, 128), B);
+  const unsigned long long *ign = (const unsigned long long *)ignored_part_pairs;
+  self_face_kernel<false><<<grid, 128, 0, st>>>(faces, F, w, part_labels, ign, max_pairs, pairs);
+  SHAPY_LAUNCH_CHECK();
+  self_scan_kernel<<<B, 1024, 0, st>>>(F, w, count);
+  SHAPY_LAUNCH_CHECK();
+  if (max_pairs > 0) {
+    SHAPY_CUDA_TRY(cudaMemsetAsync(pairs, 0xFF, (size_t)B * max_pairs * 2 * sizeof(int32_t), st));
+    self_face_kernel<true><<<grid, 128, 0, st>>>(faces, F, w, part_labels, ign, max_pairs, pairs);
+    SHAPY_LAUNCH_CHECK();
+  }
+  return SHAPY_OK;
+}

@@ -14,6 +14,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "penetration.cuh"
 
 namespace shapy {
 
@@ -2077,9 +2078,13 @@ int run_lm_kp2d(const char *fn, int batch, LmKpArgs a, LmKp2dStepArgs x, bool pe
 //     one 4 x 4 block of the triangle in registers (SIMT fp64), and the partial sums go to the workspace.  A point with
 //     all barycentrics > 0 on a face of non-zero area gives one point-to-plane row n^T (c_i - p_i), n the face's unit
 //     normal held constant; any other kept point three point-to-point rows c_i - p_i; a vertex with a nearest point
-//     three rows x_v - s_v.  The chunking depends on N and V only; no atomics.
+//     three rows x_v - s_v.  With the penetration term, a second launch (<true>) covers the 6 C points of the pair
+//     rows (B, C, 2) in chunks after every body's scan chunks: point k < 3 is vertex k of the intruder in the receiver's cone, k >= 3 vertex k - 3 of the
+//     receiver in the intruder's cone; a point with phi != 0 gives one row phi, weight w_p, its Jacobian
+//     sum over the point and the cone's three vertices of (d phi / d x)^T J_x, phi and its derivatives in fp64
+//     (penetration.cuh).  The chunking depends on N, V and C only; no atomics.
 //   lm_scan_step_kernel, one CTA per body: the chunks summed in chunk order into the trial's loss, A = c_s A_s +
-//     c_m A_m and g, the policy of the other steps, the state's A and g replaced by the trial's on accept (P^2 + P
+//     c_m A_m (+ A_p, the penetration chunks, already weighted) and g, the policy of the other steps, the state's A and g replaced by the trial's on accept (P^2 + P
 //     doubles instead of a Jacobian), then the pose-prior and measurement rows at the state, betas_w + lambda on the
 //     betas diagonal and lambda elsewhere, lm_kp_solve and the next trial.
 constexpr int kScanChunk = 1024;        // points or vertices per CTA of the row kernel
@@ -2115,14 +2120,59 @@ struct LmScanRowArgs {
   double *ws;
 };
 
-__global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArgs a) {
+// The penetration rows: pairs (B, C, 2) of shapy_self_collisions on F faces, np chunks of the 6 C points per body,
+// weight w; their partial sums at ws, (B, np) chunks after the (B, ns + nm) of the scan terms.
+struct LmScanPenArgs {
+  const int32_t *pairs;
+  int C, np, F;
+  float w;
+  PenParams pen;
+  double *ws;
+};
+
+// Penetration point i of body b (pair i / 6, point i % 6): with phi != 0 its row (kind 4, weight w_p, residual phi,
+// loss share w_p phi^2) and d phi / d x of the point and the cone's three vertices.
+__device__ __forceinline__ void lm_scan_pen_item(const LmScanRowArgs &a, const LmScanPenArgs &pa, int b, int i,
+                                                 double (*pg)[3], int *vid, int &kind, double &u, double &r, double &l) {
+  int rf[3], qf[3];
+  if (!pen::pair_faces(pa.pairs + ((size_t)b * pa.C + i / 6) * 2, a.faces, pa.F, rf, qf)) return;
+  const int k = i % 6;
+  const int *cv = k < 3 ? rf : qf;       // the cone's face; the point is a vertex of the other face
+  const int pv = k < 3 ? qf[k] : rf[k - 3];
+  const float *vb = a.verts + (size_t)b * a.V * 3;
+  const pen::Cone<double> cone = pen::make_cone(pen::ld<double>(vb + 3 * cv[0]), pen::ld<double>(vb + 3 * cv[1]),
+                                                pen::ld<double>(vb + 3 * cv[2]));
+  const pen::V3<double> p = pen::ld<double>(vb + 3 * pv);
+  const pen::PointTerms<double> e = pen::point_terms(p, cone, pa.pen);
+  if (e.phi == 0.0) return;
+  pen::V3<double> gp{0.0, 0.0, 0.0}, gc = gp, gn = gp, gx[3] = {gp, gp, gp};
+  double gr = 0.0;
+  pen::point_backward(p, cone, e, pa.pen, 1.0, gp, gc, gn, gr);
+  pen::cone_backward(cone, gc, gn, gr, gx);
+  const pen::V3<double> gv[4] = {gp, gx[0], gx[1], gx[2]};
+  const int vv[4] = {pv, cv[0], cv[1], cv[2]};
+  for (int m = 0; m < 4; ++m) {
+    vid[m] = vv[m];
+    pg[m][0] = gv[m].x; pg[m][1] = gv[m].y; pg[m][2] = gv[m].z;
+  }
+  const double w = pa.w;
+  kind = 4;
+  u = w;
+  r = e.phi;
+  l = w * (e.phi * e.phi);
+}
+
+// PEN: the penetration chunks (blockIdx.x the chunk of pa), otherwise the point then vertex chunks of the scan terms.
+template <bool PEN>
+__global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArgs a, LmScanPenArgs pa) {
   __shared__ double Js[kScanRows][kLmKpMaxP];
   __shared__ double us[kScanRows], rs[kScanRows], ls[kScanItems], cf[kScanItems][3], nrm[kScanItems][3];
-  __shared__ int vid[kScanItems][3], kind[kScanItems];   // kind: 1 point-to-plane, 2 point-to-point, 3 vertex
+  __shared__ double pg[PEN ? kScanItems : 1][4][3];     // d phi / d x of a penetration point's four vertices
+  __shared__ int vid[kScanItems][PEN ? 4 : 3], kind[kScanItems];  // 1 point-to-plane, 2 point-to-point, 3 vertex, 4 pen
   const int b = blockIdx.y, c = blockIdx.x, t = threadIdx.x, P = a.P, Pp = (P + 3) & ~3, nbw = Pp / 4;
-  const bool pts = c < a.ns;
-  const int i0 = (pts ? c : c - a.ns) * kScanChunk, n = min(kScanChunk, (pts ? a.N : a.V) - i0);
-  const bool active = pts ? a.s2m > 0.f : (a.m2s > 0.f && a.nearest);
+  const bool pts = !PEN && c < a.ns;
+  const int i0 = (PEN ? c : pts ? c : c - a.ns) * kScanChunk, n = min(kScanChunk, (PEN ? 6 * pa.C : pts ? a.N : a.V) - i0);
+  const bool active = PEN ? pa.w > 0.f : pts ? a.s2m > 0.f : (a.m2s > 0.f && a.nearest);
   const bool robust = isfinite(a.sigma);
   const double s2 = (double)a.sigma * (double)a.sigma;
   int bi = 0, bj = 0;
@@ -2141,7 +2191,9 @@ __global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArg
       kind[t] = 0;
       const int i = i0 + s0 + t;
       double d[3];
-      if (pts) {
+      if constexpr (PEN) {
+        lm_scan_pen_item(a, pa, b, i, pg[t], vid[t], kind[t], us[3 * t], rs[3 * t], ls[t]);
+      } else if (pts) {
         const double w = a.weights[(size_t)b * a.N + i];
         if (w > 0.0) {                  // a dropped point is never read
           const int f = a.face_idx[(size_t)b * a.N + i];
@@ -2207,6 +2259,9 @@ __global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArg
         };
         if (k == 1) x = nrm[it][0] * mix(0) + nrm[it][1] * mix(1) + nrm[it][2] * mix(2);
         else if (k == 2) x = mix(cc);
+        else if (PEN)
+          for (int m = 0; m < 4; ++m)
+            for (int q = 0; q < 3; ++q) x += pg[it][m][q] * (double)J[((size_t)vid[it][m] * 3 + q) * P + col];
         else x = (double)J[((size_t)vid[it][0] * 3 + cc) * P + col];
       }
       Js[row][col] = x;
@@ -2230,7 +2285,8 @@ __global__ void __launch_bounds__(kScanThreads) lm_scan_rows_kernel(LmScanRowArg
     }
   }
   const int npk = P * (P + 1) / 2;
-  double *o = a.ws + ((size_t)b * (a.ns + a.nm) + c) * lm_scan_stride(P);
+  double *o = PEN ? pa.ws + ((size_t)b * pa.np + c) * lm_scan_stride(P)
+                  : a.ws + ((size_t)b * (a.ns + a.nm) + c) * lm_scan_stride(P);
   if (own)
     for (int x = 0; x < 4; ++x)
       for (int y = 0; y < 4; ++y) {
@@ -2248,6 +2304,8 @@ struct LmScanStepArgs {
   LmKp2dArgs x2;                        // anchor, pose_w and betas_w, and the measurement block with MEAS
   double *A, *g;                        // the state's undamped data rows: (B, P, P) symmetric, (B, P)
   const double *ws;
+  int np;                               // penetration chunks per body (0 without the term) and their partial sums
+  const double *wsp;
 };
 
 template <bool MEAS>
@@ -2259,7 +2317,7 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_scan_step_kernel(LmKpArgs a, 
   const int b = blockIdx.x, t = threadIdx.x, P = a.P, nb = a.nb, nr9 = 9 * a.n_rot, o = 3 * a.n_rot;
   const int npk = P * (P + 1) / 2, nc = x.ns + x.nm;
   const size_t S = lm_scan_stride(P);
-  const double *wsb = x.ws + (size_t)b * nc * S;
+  const double *wsb = x.ws + (size_t)b * nc * S, *wpb = x.wsp + (size_t)b * x.np * S;
   const float *anc = x.x2.anchor ? x.x2.anchor + (size_t)b * nr9 : nullptr;
   const float lcur = a.loss[b];
   // 1. trial loss: sum_{w_i > 0} w_i strided over the threads, the threads' sums in thread order, then the chunks
@@ -2278,6 +2336,11 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_scan_step_kernel(LmKpArgs a, 
     for (int c = 0; c < x.ns; ++c) Ls += wsb[c * S + npk + P];
     for (int c = x.ns; c < nc; ++c) Lm += wsb[c * S + npk + P];
     double L = cs * Ls + cm * Lm;
+    if (x.np) {
+      double Lp = 0.0;
+      for (int c = 0; c < x.np; ++c) Lp += wpb[c * S + npk + P];
+      L += Lp;
+    }
     if (x.x2.pose_w > 0.f) L += lm_kp2d_prior_loss(x.x2, a.trot + (size_t)b * nr9, anc, nr9);
     if constexpr (MEAS) L += lm_meas_loss(x.x2.mb, b);
     if (x.x2.betas_w > 0.f) L += (double)x.x2.betas_w * lm_sq_norm(a.tbetas + (size_t)b * nb, nb);
@@ -2313,6 +2376,21 @@ __global__ void __launch_bounds__(kLmKpThreads) lm_scan_step_kernel(LmKpArgs a, 
       } else {
         y[p - npk] = v;
         gb[p - npk] = v;
+      }
+    }
+    for (int p = t; x.np && p < npk + P; p += blockDim.x) {  // the penetration rows, by the thread that wrote p
+      double s3 = 0.0;
+      for (int c = 0; c < x.np; ++c) s3 += wpb[c * S + p];
+      if (p < npk) {
+        int r, k;
+        tri_rc(p, r, k);
+        const double v = A[r * P + k] + s3;
+        A[r * P + k] = v;
+        Ab[r * P + k] = v;
+        Ab[k * P + r] = v;
+      } else {
+        y[p - npk] += s3;
+        gb[p - npk] += s3;
       }
     }
   } else {
@@ -2671,23 +2749,39 @@ extern "C" size_t shapy_fit_lm_scan_workspace_bytes(int batch, int num_points, i
          sizeof(double);
 }
 
-extern "C" int shapy_fit_lm_scan_step(
-    int batch, int num_points, int num_verts, int n_rot, int nb, const float *points, const float *weights,
-    const int32_t *faces, const float *pose_anchor, float robust_sigma, float scan_to_model_weight,
-    float model_to_scan_weight, float pose_prior_weight, float betas_weight, const float *meas_targets,
-    const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl,
-    double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss, float *lambda,
-    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_vertices,
-    const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary, const int32_t *trial_nearest,
-    const float *trial_meas, const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream) {
-  const char *fn = "shapy_fit_lm_scan_step";
+extern "C" size_t shapy_fit_lm_scan_penetration_workspace_bytes(int batch, int num_points, int num_verts,
+                                                                int num_params, int num_pairs) {
+  if (batch < 0 || num_points < 1 || num_verts < 1 || num_params < 1 || num_pairs < 0) return 0;
+  return (size_t)batch * (lm_scan_chunks(num_points) + lm_scan_chunks(num_verts) + lm_scan_chunks(6 * num_pairs)) *
+         lm_scan_stride(num_params) * sizeof(double);
+}
+
+namespace shapy {
+// the penetration rows of shapy_fit_lm_scan_penetration_step; null: shapy_fit_lm_scan_step
+struct LmScanPen {
+  const int32_t *pairs;
+  int C, F;
+  float weight, sigma;
+};
+
+static int lm_scan_step_run(
+    const char *fn, int batch, int num_points, int num_verts, int n_rot, int nb, const float *points,
+    const float *weights, const int32_t *faces, const float *pose_anchor, float robust_sigma,
+    float scan_to_model_weight, float model_to_scan_weight, float pose_prior_weight, float betas_weight,
+    const float *meas_targets, const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot,
+    float *betas, float *transl, double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss,
+    float *lambda, int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl,
+    const float *trial_vertices, const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary,
+    const int32_t *trial_nearest, const float *trial_meas, const float *trial_meas_jac, const LmScanPen *pen,
+    void *workspace, size_t workspace_bytes, void *stream) {
   const LmMeasArgs mb{meas_targets, meas_weights, 0.f, meas, meas_jac, trial_meas, trial_meas_jac};
   const bool with_meas = meas_targets || meas_weights || meas || meas_jac || trial_meas || trial_meas_jac;
   const float s2m = scan_to_model_weight, m2s = model_to_scan_weight;
   SHAPY_REQUIRE(points && weights && faces && rot && betas && transl && normal_matrix && gradient && loss && lambda &&
                     accepted && trial_rot && trial_betas && trial_transl && trial_vertices && trial_jac &&
                     trial_face_idx && trial_bary && workspace && (trial_nearest || !(m2s > 0.f)) &&
-                    (pose_anchor || !(pose_prior_weight > 0.f)) && (!with_meas || lm_meas_ptrs(mb)),
+                    (pose_anchor || !(pose_prior_weight > 0.f)) && (!with_meas || lm_meas_ptrs(mb)) &&
+                    (!pen || pen->pairs || pen->C == 0),
                 "%s: null argument", fn);
   SHAPY_REQUIRE(batch >= 0 && batch <= 65535 && num_points >= 1 && num_verts >= 1 && n_rot >= 1 && n_rot <= 64 &&
                     nb >= 1,
@@ -2698,24 +2792,72 @@ extern "C" int shapy_fit_lm_scan_step(
                 "%s: robust_sigma must be > 0 (inf: least squares), the term and prior weights finite and >= 0 and "
                 "lambda_up and lambda_down >= 1",
                 fn);
+  SHAPY_REQUIRE(!pen || (pen->C >= 0 && pen->F >= 1 && pen->weight >= 0.f && isfinite(pen->weight) &&
+                         pen->sigma > 0.f && isfinite(pen->sigma)),
+                "%s: the penetration pairs, faces, weight (finite, >= 0) or sigma (finite, > 0) are bad", fn);
   const int P = 3 * n_rot + nb + 3;
   if (P > kLmKpMaxP) {
     set_error("%s: %d parameters, at most %d are supported", fn, P, kLmKpMaxP);
     return SHAPY_ERR_UNSUPPORTED;
   }
-  const size_t need = shapy_fit_lm_scan_workspace_bytes(batch, num_points, num_verts, P);
+  const size_t need = pen ? shapy_fit_lm_scan_penetration_workspace_bytes(batch, num_points, num_verts, P, pen->C)
+                          : shapy_fit_lm_scan_workspace_bytes(batch, num_points, num_verts, P);
   SHAPY_REQUIRE(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
   if (batch == 0) return SHAPY_OK;
-  const int ns = lm_scan_chunks(num_points), nm = lm_scan_chunks(num_verts);
+  const int ns = lm_scan_chunks(num_points), nm = lm_scan_chunks(num_verts), np = pen ? lm_scan_chunks(6 * pen->C) : 0;
   LmScanRowArgs r{num_points, num_verts, P,  ns, nm, points, weights, faces, trial_vertices, trial_jac, trial_face_idx,
                   trial_nearest, trial_bary, robust_sigma, s2m, m2s, (double *)workspace};
-  lm_scan_rows_kernel<<<dim3(ns + nm, batch), kScanThreads, 0, (cudaStream_t)stream>>>(r);
+  LmScanPenArgs pa{};
+  lm_scan_rows_kernel<false><<<dim3(ns + nm, batch), kScanThreads, 0, (cudaStream_t)stream>>>(r, pa);
   SHAPY_LAUNCH_CHECK();
+  if (np > 0) {
+    pa = LmScanPenArgs{pen->pairs, pen->C, np, pen->F, pen->weight, PenParams{pen->sigma, 1000.f, true},
+                       (double *)workspace + (size_t)batch * (ns + nm) * lm_scan_stride(P)};
+    lm_scan_rows_kernel<true><<<dim3(np, batch), kScanThreads, 0, (cudaStream_t)stream>>>(r, pa);
+    SHAPY_LAUNCH_CHECK();
+  }
   LmKpArgs a{0, n_rot, nb, P, nullptr, nullptr, lambda_up, lambda_down, first ? 1 : 0, rot, betas, transl, nullptr,
              nullptr, loss, lambda, accepted, trial_rot, trial_betas, trial_transl, nullptr, nullptr};
   LmScanStepArgs x{num_points, num_verts, ns, nm, weights, s2m, m2s,
                    LmKp2dArgs{pose_anchor, robust_sigma, pose_prior_weight, betas_weight, mb}, normal_matrix,
-                   gradient, (const double *)workspace};
+                   gradient, (const double *)workspace, np, pa.ws};
   return lm_launch(with_meas ? lm_scan_step_kernel<true> : lm_scan_step_kernel<false>, batch, kLmKpThreads,
                    lm_kp_smem(P), stream, a, x);
+}
+}  // namespace shapy
+
+extern "C" int shapy_fit_lm_scan_step(
+    int batch, int num_points, int num_verts, int n_rot, int nb, const float *points, const float *weights,
+    const int32_t *faces, const float *pose_anchor, float robust_sigma, float scan_to_model_weight,
+    float model_to_scan_weight, float pose_prior_weight, float betas_weight, const float *meas_targets,
+    const float *meas_weights, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl,
+    double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_vertices,
+    const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary, const int32_t *trial_nearest,
+    const float *trial_meas, const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream) {
+  return lm_scan_step_run("shapy_fit_lm_scan_step", batch, num_points, num_verts, n_rot, nb, points, weights, faces,
+                          pose_anchor, robust_sigma, scan_to_model_weight, model_to_scan_weight, pose_prior_weight,
+                          betas_weight, meas_targets, meas_weights, lambda_up, lambda_down, first, rot, betas, transl,
+                          normal_matrix, gradient, meas, meas_jac, loss, lambda, accepted, trial_rot, trial_betas,
+                          trial_transl, trial_vertices, trial_jac, trial_face_idx, trial_bary, trial_nearest,
+                          trial_meas, trial_meas_jac, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int shapy_fit_lm_scan_penetration_step(
+    int batch, int num_points, int num_verts, int n_rot, int nb, const float *points, const float *weights,
+    const int32_t *faces, int num_faces, const float *pose_anchor, float robust_sigma, float scan_to_model_weight,
+    float model_to_scan_weight, float pose_prior_weight, float betas_weight, const float *meas_targets,
+    const float *meas_weights, const int32_t *pen_pairs, int num_pairs, float penetration_weight,
+    float penetration_sigma, float lambda_up, float lambda_down, int first, float *rot, float *betas, float *transl,
+    double *normal_matrix, double *gradient, float *meas, float *meas_jac, float *loss, float *lambda,
+    int32_t *accepted, float *trial_rot, float *trial_betas, float *trial_transl, const float *trial_vertices,
+    const float *trial_jac, const int32_t *trial_face_idx, const float *trial_bary, const int32_t *trial_nearest,
+    const float *trial_meas, const float *trial_meas_jac, void *workspace, size_t workspace_bytes, void *stream) {
+  const LmScanPen pen{pen_pairs, num_pairs, num_faces, penetration_weight, penetration_sigma};
+  return lm_scan_step_run("shapy_fit_lm_scan_penetration_step", batch, num_points, num_verts, n_rot, nb, points,
+                          weights, faces, pose_anchor, robust_sigma, scan_to_model_weight, model_to_scan_weight,
+                          pose_prior_weight, betas_weight, meas_targets, meas_weights, lambda_up, lambda_down, first,
+                          rot, betas, transl, normal_matrix, gradient, meas, meas_jac, loss, lambda, accepted,
+                          trial_rot, trial_betas, trial_transl, trial_vertices, trial_jac, trial_face_idx, trial_bary,
+                          trial_nearest, trial_meas, trial_meas_jac, &pen, workspace, workspace_bytes, stream);
 }

@@ -120,7 +120,7 @@ nearest points at those vertices, with measurements forward_shape and the measur
 ops.fit_lm_scan_step: the correspondences held as landmarks, one point-to-plane row per point interior to its face
 (three point-to-point rows otherwise, and for every vertex), IRLS weights under Geman-McClure, the normal equations
 summed in fp64 on the device.  No host synchronisation, and every body's loss is non-increasing; vertex_jacobian
-exposes the Jacobian.  Not covered: scan normals, a self-penetration term, rigid pre-alignment of scans in other
+exposes the Jacobian.  Not covered: scan normals, rigid pre-alignment of scans in other
 frames or units, and reading PLY / OBJ files (load the points into an npz).
 
     python -m shapy_b200.fit --synthetic --scan scan.npz --init pred.npz --robust-sigma 0.01 --output fit.npz
@@ -246,6 +246,56 @@ def _adam(params, lr, iterations, loss_fn):
         sched.step()
     with torch.no_grad():
         return loss_fn()
+
+
+class _PenetrationTerm:
+    """The self-penetration term: weight x ops.penetration_forward (the reference's DistanceFieldPenetrationLoss at
+    penalize_outside=True, linear_max=1000) at the pairs ops.self_collisions finds on the detached posed vertices, through
+    autograd.PenetrationFunction into the vertices' cotangent.  `last` holds (loss, pair count) of the latest call."""
+
+    def __init__(self, weight, sigma, max_pairs, part_labels, ignored_part_pairs, faces):
+        from . import ops
+        self.weight, self.sigma, self.max_pairs, self.faces = float(weight), float(sigma), int(max_pairs), faces
+        # the filter goes to the device once, not at every iteration
+        self.filter = ops.make_part_filter(part_labels, ignored_part_pairs, faces.shape[0], faces.device)
+        self.last = None
+
+    def pairs(self, vertices, tree=None):
+        from . import ops
+        return ops.self_collisions(vertices.detach(), self.faces, self.max_pairs, tree, part_filter=self.filter)[0]
+
+    def __call__(self, vertices, tree=None):
+        from . import ops
+        from .autograd import PenetrationFunction
+        pairs, count = ops.self_collisions(vertices.detach(), self.faces, self.max_pairs, tree,
+                                           part_filter=self.filter)
+        pen = PenetrationFunction.apply(vertices, self.faces, pairs, self.sigma, True, 1000.0)
+        self.last = (pen.detach(), count)
+        return self.weight * pen
+
+    def outputs(self):
+        return {'penetration': self.last[0], 'penetration_pairs': self.last[1]}
+
+
+def _penetration_term(fn, body_model, method, weight, sigma, max_pairs, part_labels, ignored_part_pairs,
+                      lm_ok=False):
+    """None when weight is 0 (the fit runs exactly as without the term), else a _PenetrationTerm; ValueError before any
+    launch for a bad argument or, unless lm_ok, method='lm'."""
+    from .ops import MAX_PENETRATION_PAIRS, MAX_SCAN_FACES
+    if not (0 <= float(weight) < float('inf')):
+        raise ValueError(f'{fn}: penetration_weight must be finite and >= 0, got {weight}')
+    if float(weight) == 0:
+        return None
+    if method != 'adam' and not lm_ok:
+        raise ValueError(f"{fn}: the self-penetration term is not supported with method={method!r}")
+    if not float(sigma) > 0:
+        raise ValueError(f'{fn}: penetration_sigma must be > 0, got {sigma}')
+    if not 1 <= int(max_pairs) <= MAX_PENETRATION_PAIRS:
+        raise ValueError(f'{fn}: max_penetration_pairs must be in [1, {MAX_PENETRATION_PAIRS}], got {max_pairs}')
+    faces = body_model.faces_i32
+    if faces.shape[0] > MAX_SCAN_FACES:
+        raise ValueError(f'{fn}: the model has {faces.shape[0]} faces, self-collisions take at most {MAX_SCAN_FACES}')
+    return _PenetrationTerm(weight, sigma, max_pairs, part_labels, ignored_part_pairs, faces)
 
 
 def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
@@ -394,7 +444,8 @@ def vertex_jacobian(body_model, rot, betas, transl=None):
 
 def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, lr=0.05, init=None, method='adam',
                           body_measurements=None, measurements=None, measurement_weights=None, betas_weight=0.0,
-                          circumference_derivative='reference'):
+                          circumference_derivative='reference', penetration_weight=0.0, penetration_sigma=0.5,
+                          max_penetration_pairs=1024, part_labels=None, ignored_part_pairs=None):
     """Fits pose and shape so that the model's keypoints match `keypoints` (B, K, 3), K = body_model's keypoint count.
 
     weights: None (all 1), (K,) or (B, K) per-keypoint weights.  init: optional {'global_rot': (B, 6),
@@ -411,9 +462,16 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat' (B, 1, 3, 3),
     'body_pose_mat' (B, 21, 3, 3), 'keypoints' (B, K, 3) of the final parameters, 'loss' (B,) final per-body loss},
     with measurements also 'measurements' (B, 5) of the final betas (mass, height, chest, waist, hips), and 'loss'
-    the total: keypoints + measurements + betas_weight |betas|^2."""
+    the total: keypoints + measurements + betas_weight |betas|^2 (+ the self-penetration term).
+    penetration_weight > 0 (method='adam'; fit_body_to_scan also 'lm') adds penetration_weight times the distance-field self-penetration
+    loss of SMPLify-X (ops.penetration_forward at sigma=penetration_sigma) at the intersecting face pairs of the posed
+    mesh, found again at every iteration (ops.self_collisions, at most max_penetration_pairs per body, filtered by
+    part_labels / ignored_part_pairs, see ops.face_parts and ops.parent_child_part_pairs); the result then also has
+    'penetration' (B,) and 'penetration_pairs' (B,) (pairs found, before the cut) at the final parameters."""
     iterations, _ = _check_kp_fit('fit_body_to_keypoints', body_model, method, iterations, circumference_derivative,
                                   body_measurements, measurements)
+    pt = _penetration_term('fit_body_to_keypoints', body_model, method, penetration_weight, penetration_sigma,
+                           max_penetration_pairs, part_labels, ignored_part_pairs)
     if measurements is None and betas_weight != 0:
         raise ValueError('fit_body_to_keypoints: betas_weight needs measurements (the keypoint fit has no betas prior)')
     if not betas_weight >= 0:
@@ -438,6 +496,8 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
                          return_shaped=False)
         joints = out['joints'][:]                  # the KeypointTensor's tensor, still in the graph
         per_body = ((joints - kp).pow(2).sum(-1) * w).sum(1)
+        if pt is not None:
+            per_body = per_body + pt(out['vertices'])
         meas = None
         if mt is not None:
             meas = mt.measure(body_model, params['betas'])
@@ -445,7 +505,8 @@ def fit_body_to_keypoints(body_model, keypoints, weights=None, iterations=None, 
         return per_body, joints, grot, bpose, meas
 
     per_body, joints, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
-    return _adam_result(params, grot, bpose, meas, keypoints=joints, loss=per_body)
+    return _adam_result(params, grot, bpose, meas, keypoints=joints, loss=per_body,
+                        **({} if pt is None else pt.outputs()))
 
 
 def _adam_result(params, grot, bpose, meas, **outputs):
@@ -728,7 +789,9 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                              robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0, pose_anchor=None, lr=0.05,
                              body_measurements=None, measurements=None, measurement_weights=None,
                              circumference_derivative='reference', groups=None, share_pose=False, focal_length=None,
-                             principal_point=None, pose_width=22, fit_expression=False, expression_weight=0.0):
+                             principal_point=None, pose_width=22, fit_expression=False, expression_weight=0.0,
+                             penetration_weight=0.0, penetration_sigma=0.5, max_penetration_pairs=1024,
+                             part_labels=None, ignored_part_pairs=None):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -790,8 +853,14 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     SMPLX.forward.  The result also holds the raw 6D parts in the width, 'full_pose_mat' (B, pose_width, 3, 3) and,
     when fitted, 'expression'.  A part is only as determined as its keypoints make it: one without a weighted keypoint
     (the eyes: the OpenPose pupils are dropped on load) is held by its prior alone, and without a prior it stays where
-    it starts.  groups, share_pose and measurements are not supported on the wide path."""
+    it starts.  groups, share_pose and measurements are not supported on the wide path.
+    penetration_weight > 0, penetration_sigma, max_penetration_pairs, part_labels, ignored_part_pairs: the
+    self-penetration term of fit_body_to_keypoints, for a single-image fit (no groups) with method='adam'."""
     fn = 'fit_body_to_keypoints_2d'
+    pt = _penetration_term(fn, body_model, method, penetration_weight, penetration_sigma, max_penetration_pairs,
+                           part_labels, ignored_part_pairs)
+    if pt is not None and groups is not None:
+        raise ValueError(f'{fn}: the self-penetration term is not supported with groups')
     wide = pose_width != 22 or fit_expression
     ne, jw = 0, None
     if wide:
@@ -873,6 +942,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         out = _forward_2d(body_model, grot, bpose, params['betas'], params[last], intr, pr, expr)
         rot = torch.cat([grot, bpose] + list(pr.values()), 1)
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'], jw, ew, expr)
+        if pt is not None:
+            per_body = per_body + pt(out['vertices'])
         meas = None
         if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
             meas = mt.measure(body_model, params['betas'])
@@ -884,7 +955,7 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         per_body = _depth_rule(per_body, out['joints'][:], w)
     wide_out = {'full_pose_mat': rot} if wide else {}
     return _adam_result(params, rot[:, :1], rot[:, 1:22], meas, **wide_out, keypoints=out['joints'][:],
-                        proj_joints=out['proj_joints'], loss=per_body)
+                        proj_joints=out['proj_joints'], loss=per_body, **({} if pt is None else pt.outputs()))
 
 
 def _fit_keypoints_2d_lm(body_model, x, w, params, parts, rot0, anchor, iterations, sigma, pw, jw, bw, ew, ne, mt, intr,
@@ -1410,7 +1481,8 @@ def _scan_inputs(fn, body_model, points, weights, device):
 def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=None, lr=0.05, scan_to_model_weight=1.0,
                      model_to_scan_weight=1.0, robust_sigma=None, pose_prior_weight=0.0, betas_weight=0.0,
                      body_measurements=None, measurements=None, measurement_weights=None,
-                     circumference_derivative='reference', method='adam'):
+                     circumference_derivative='reference', method='adam', penetration_weight=0.0,
+                     penetration_sigma=0.5, max_penetration_pairs=1024, part_labels=None, ignored_part_pairs=None):
     """Fits pose, shape and translation to 3D scans or point clouds: points (B, N, 3) in metres in the model frame,
     N <= 32768 per body, weights None (all 1), (N,) or (B, N), a point with weight <= 0 dropped (it may be NaN).
     Loss per body: scan_to_model_weight sum_i w_i rho(d_i^2) / sum_i w_i, d_i the distance of point i to the exact
@@ -1430,10 +1502,17 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
     bits as a rebuild).
     Returns {'global_rot', 'body_pose' (raw 6D), 'betas', 'transl', 'global_rot_mat', 'body_pose_mat', 'vertices'
     (B, V, 3) of the final parameters, 'loss' (B,)}, and with body_measurements 'measurements' (B, 5) of the fitted
-    betas (mass, height, chest, waist, hips), with or without measurement targets."""
+    betas (mass, height, chest, waist, hips), with or without measurement targets.
+    penetration_weight > 0, penetration_sigma, max_penetration_pairs, part_labels, ignored_part_pairs: the
+    self-penetration term of fit_body_to_keypoints, its pairs found on the scan terms' tree; with method='lm' each
+    trial's pairs come from the tree closest_points has just refit on its vertices, each point with phi != 0 is one
+    row sqrt(w) phi, and the trial loss that accept / reject compares includes the term
+    (ops.fit_lm_scan_step(penetration=...))."""
     fn = 'fit_body_to_scan'
     iterations, sigma = _check_kp_fit(fn, body_model, method, iterations, circumference_derivative, body_measurements,
                                       measurements, robust_sigma, pose_prior_weight, betas_weight)
+    pt = _penetration_term(fn, body_model, method, penetration_weight, penetration_sigma, max_penetration_pairs,
+                           part_labels, ignored_part_pairs, lm_ok=True)
     s2m, m2s = float(scan_to_model_weight), float(model_to_scan_weight)
     if not (0 <= s2m < float('inf') and 0 <= m2s < float('inf') and s2m + m2s > 0):
         raise ValueError(f'{fn}: the scan-to-model and model-to-scan weights must be finite, >= 0 and not both 0')
@@ -1479,6 +1558,8 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
             per_body = per_body + 0.5 * pw * (bpose - anchor[:, 1:]).pow(2).sum((1, 2, 3))
         if bw > 0:
             per_body = per_body + bw * betas.pow(2).sum(1)
+        if pt is not None:
+            per_body = per_body + pt(v, tree)
         meas = None
         if mt is not None:
             meas = mt.measure(body_model, betas)
@@ -1500,23 +1581,25 @@ def fit_body_to_scan(body_model, points, weights=None, init=None, iterations=Non
         return meas
 
     if method == 'lm':
-        state = _fit_scan_lm(body_model, pts, w, params, rot0, anchor, int(iterations), sigma, s2m, m2s, pw, bw, mt)
+        state = _fit_scan_lm(body_model, pts, w, params, rot0, anchor, int(iterations), sigma, s2m, m2s, pw, bw, mt,
+                             pt)
         rot = state['rot']
         with torch.no_grad():
             per_body, v, meas = scan_loss(rot[:, :1], rot[:, 1:], state['betas'], state['transl'])
-        res = _kp_lm_result(state, 'transl', vertices=v, loss=per_body)
+        res = _kp_lm_result(state, 'transl', vertices=v, loss=per_body, **({} if pt is None else pt.outputs()))
         meas = fitted_measurements(res.get('measurements', meas), state['betas'])
         if meas is not None:
             res['measurements'] = meas
         return res
     per_body, v, grot, bpose, meas = _adam(list(params.values()), lr, iterations, loss_fn)
     meas = fitted_measurements(meas, params['betas'])
-    return _adam_result(params, grot, bpose, meas, vertices=v, loss=per_body)
+    return _adam_result(params, grot, bpose, meas, vertices=v, loss=per_body, **({} if pt is None else pt.outputs()))
 
 
-def _fit_scan_lm(body_model, pts, w, params, rot0, anchor, iterations, sigma, s2m, m2s, pw, bw, mt):
+def _fit_scan_lm(body_model, pts, w, params, rot0, anchor, iterations, sigma, s2m, m2s, pw, bw, mt, pt=None):
     """The LM loop of fit_body_to_scan: per iteration the trial's vertex Jacobian, closest and (m2s > 0) nearest
-    points, with measurements their trial values and Jacobian, then one ops.fit_lm_scan_step.  Returns the state."""
+    points, with the penetration term pt the self-collisions on the tree closest_points has just refit, with
+    measurements their trial values and Jacobian, then one ops.fit_lm_scan_step.  Returns the state."""
     from . import ops
     device = pts.device
     packed = body_model.packed(device)
@@ -1535,18 +1618,20 @@ def _fit_scan_lm(body_model, pts, w, params, rot0, anchor, iterations, sigma, s2
         return state
     if mt is not None:
         mt.prime(body_model)
-    ws = ops.fit_lm_scan_workspace(B, N, V, P, device)
+    ws = ops.fit_lm_scan_workspace(B, N, V, P, device) if pt is None else \
+        ops.fit_lm_scan_penetration_workspace(B, N, V, P, pt.max_pairs, device)
     tree = ops.ScanTree()
     for it in range(iterations + 1):
         v, jac = ops.smplx_vertex_jacobian(packed, trial['betas'], trial['rot'], trial['transl'])
         face, bary, _ = ops.closest_points(v, faces, pts, w, tree)
         nearest = ops.nearest_points(v, pts, w)[0] if m2s > 0 else None
+        pen = None if pt is None else (pt.pairs(v, tree), pt.weight, pt.sigma)
         meas = None
         if mt is not None:
             tm, tmj = mt.trial(packed, body_model, trial['betas'])
             meas = (mt.tgt, mt.wt, tm, tmj)
         ops.fit_lm_scan_step(state, trial, pts, w, faces, sigma, s2m, m2s, pw, bw, LM_UP, LM_DOWN, it == 0, v, jac, face,
-                             bary, nearest, ws, pose_anchor=anchor if pw > 0 else None, meas=meas)
+                             bary, nearest, ws, pose_anchor=anchor if pw > 0 else None, meas=meas, penetration=pen)
     return state
 
 
@@ -1622,7 +1707,16 @@ def main(argv=None):
                         'the fitted vertices and the measurements of the fitted betas')
     p.add_argument('--model-to-scan-weight', dest='model_to_scan_weight', type=float, default=1.0,
                    help='with --scan: the weight of the model -> scan term (0 for a partial, single-view scan)')
+    p.add_argument('--penetration-weight', dest='penetration_weight', type=float, default=0.0,
+                   help='with --scan or --keypoints-2d (adam, single image): the weight of the self-penetration term, '
+                        'its pairs filtered by the parts of ops.face_parts and the parent-child creases')
+    p.add_argument('--penetration-sigma', dest='penetration_sigma', type=float, default=0.5,
+                   help='the cone height sigma of the self-penetration term')
     a = p.parse_args(argv)
+    if a.penetration_weight and not ((a.scan and not a.keypoints_2d) or
+                                     (a.keypoints_2d and not (a.calibrated or a.sequence))):
+        raise SystemExit('--penetration-weight needs --scan or --keypoints-2d and is not supported with --calibrated '
+                         'or --sequence')
     if (a.pose_width != 22 or a.fit_expression or a.expression_weight) and \
             (not a.keypoints_2d or a.calibrated or a.sequence):
         raise SystemExit('--pose-width, --fit-expression and --expression-weight need --keypoints-2d and are not '
@@ -1658,7 +1752,8 @@ def main(argv=None):
                                model_to_scan_weight=a.model_to_scan_weight, robust_sigma=a.robust_sigma,
                                pose_prior_weight=a.pose_prior_weight, betas_weight=a.betas_weight,
                                body_measurements=BodyMeasurements(cfg).cuda(), measurements=targets,
-                               circumference_derivative=a.circumference_derivative, method=a.method)
+                               circumference_derivative=a.circumference_derivative, method=a.method,
+                               **_penetration_args(a, model))
         return _save_result(a.output, res, {'bodies': int(points.shape[0]), 'points': int(points.shape[1])},
                             names=np.array(NAMES))
     bm = BodyMeasurements(cfg).cuda()
@@ -1719,8 +1814,18 @@ def _main_keypoints_2d(a, model, bm, targets):
                                    circumference_derivative=a.circumference_derivative, groups=groups,
                                    share_pose=a.share_pose, focal_length=focal, principal_point=pp,
                                    pose_width=a.pose_width, fit_expression=a.fit_expression,
-                                   expression_weight=a.expression_weight)
+                                   expression_weight=a.expression_weight, **_penetration_args(a, model))
     _save_result(a.output, res, {'bodies': int(x.shape[0])}, groups=groups)
+
+
+def _penetration_args(a, model):
+    """The self-penetration keywords of a CLI fit: none at weight 0, else the weight, sigma and the part filter of the
+    model's skinning weights and kinematic tree."""
+    if not a.penetration_weight:
+        return {}
+    from . import ops
+    return dict(penetration_weight=a.penetration_weight, penetration_sigma=a.penetration_sigma,
+                part_labels=ops.face_parts(model), ignored_part_pairs=ops.parent_child_part_pairs(model.parents))
 
 
 def _load_scan(path):

@@ -887,16 +887,166 @@ def closest_points_backward(vertices, faces_i32, points, face_idx, bary, grad_sq
     return grad
 
 
+# ---------------------------------------------------------------------------------------------- self-penetration
+MAX_PART_LABELS = 64          # part labels of the self-collision filter (one 64-bit mask per label)
+MAX_PENETRATION_PAIRS = 4096  # rows per body the penetration loss takes (its backward's shared-memory sort)
+
+
+def make_part_filter(part_labels, ignored_part_pairs, F, device):
+    """The part filter of self_collisions on the device: (labels (F,) int32, masks (64,) uint64 as int64), or (None,
+    None) without labels.  Built on the host (one copy to the device): a loop builds it once and passes it as
+    self_collisions(part_filter=...)."""
+    if part_labels is None:
+        if ignored_part_pairs:
+            raise ValueError('ignored_part_pairs needs part_labels')
+        return None, None
+    lab = torch.as_tensor(part_labels).reshape(-1)
+    if lab.numel() != F:
+        raise ValueError(f'part_labels must have one label per face ({F}), got {lab.numel()}')
+    lab_h = lab.detach().cpu().numpy().astype(np.int64)
+    if lab_h.size and (lab_h.min() < 0 or lab_h.max() >= MAX_PART_LABELS):
+        raise ValueError(f'part labels must lie in [0, {MAX_PART_LABELS})')
+    masks = np.zeros(MAX_PART_LABELS, np.uint64)
+    for i, j in (ignored_part_pairs or ()):
+        i, j = int(i), int(j)
+        if not (0 <= i < MAX_PART_LABELS and 0 <= j < MAX_PART_LABELS):
+            raise ValueError(f'ignored part pair {(i, j)} outside [0, {MAX_PART_LABELS})')
+        masks[i] |= np.uint64(1) << np.uint64(j)
+        masks[j] |= np.uint64(1) << np.uint64(i)
+    return (torch.from_numpy(lab_h.astype(np.int32)).to(device),
+            torch.from_numpy(masks.view(np.int64)).to(device))
+
+
+def self_collisions(vertices, faces_i32, max_pairs, tree=None, part_labels=None, ignored_part_pairs=None,
+                    part_filter=None):
+    """Intersecting face pairs of each posed mesh (include/shapy_b200.h, shapy_self_collisions): vertices (B, V, 3),
+    faces_i32 (F, 3) int32, F <= MAX_SCAN_FACES.  A pair (f, g), f < g, is kept when the faces share no vertex, their
+    triangles' boxes overlap and the 11-axis SAT of mesh_to_mesh_forward finds them intersecting, and, with
+    part_labels (F,) in [0, 64), the unordered label pair is not in ignored_part_pairs (pairs of labels).  Returns
+    (pairs (B, max_pairs, 2) int32 in ascending (f, g) order padded with -1, count (B,) int32 the number found, which
+    exceeds max_pairs when rows were cut).  The pairs are the same bits whatever the tree, the batch or the run.
+    tree: the ops.ScanTree of closest_points; a call with the same batch size and faces refits it.  part_filter: the
+    device tensors of ops.make_part_filter in place of part_labels / ignored_part_pairs (no host work)."""
+    v, faces_i32 = _scan_mesh(vertices, faces_i32)
+    B, V, F = v.shape[0], v.shape[1], faces_i32.shape[0]
+    max_pairs, dev = int(max_pairs), v.device
+    if max_pairs < 0:
+        raise ValueError('max_pairs must be >= 0')
+    if part_filter is None:
+        labels, masks = make_part_filter(part_labels, ignored_part_pairs, F, dev)
+    else:
+        labels, masks = part_filter
+        if labels is not None and not (labels.is_cuda and labels.dtype == torch.int32 and labels.shape == (F,) and
+                                       masks.is_cuda and masks.shape == (MAX_PART_LABELS,)):
+            raise ValueError(f'part_filter must be ops.make_part_filter(..., {F}, device)')
+    pairs = torch.empty(B, max_pairs, 2, dtype=torch.int32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    if B == 0:
+        return pairs, count
+    _incidence_rows(faces_i32, V)          # checks that the faces index the vertices
+    with torch.cuda.device(dev):
+        nbytes = lib().shapy_self_collisions_workspace_bytes(B, F)
+        key = (B, F, faces_i32.data_ptr(), faces_i32._version, dev.index)
+        if tree is None:
+            ws, refit = _WS.get('self', nbytes, dev), 0
+        else:
+            refit = int(tree.key == key and tree.ws.numel() >= nbytes)
+            if not refit:
+                tree.ws, tree.key = _workspace(max(nbytes, lib().shapy_closest_points_workspace_bytes(B, F)), dev), key
+            ws = tree.ws
+        check(lib().shapy_self_collisions(ptr(v), ptr(faces_i32), B, V, F, ptr(labels), ptr(masks), refit, max_pairs,
+                                          ptr(pairs), ptr(count), ptr(ws), ws.numel(), stream_ptr()), 'self_collisions')
+    return pairs, count
+
+
+def face_parts(body_model):
+    """Each face's part: the joint with the largest lbs weight summed over the face's three vertices, the lower joint
+    index on a tie.  body_model: a mapping or object with `lbs_weights` (V, J) and `faces_tensor` (F, 3) (the
+    reference's buffer names).  Returns (F,) int64 on the CPU."""
+    get = body_model.get if isinstance(body_model, dict) else lambda k: getattr(body_model, k)
+    w = torch.as_tensor(get('lbs_weights')).detach().cpu().double()
+    faces = torch.as_tensor(get('faces_tensor')).detach().cpu().long()
+    return w[faces].sum(dim=1).argmax(dim=1)          # argmax returns the first maximum
+
+
+def parent_child_part_pairs(parents):
+    """The (joint, parent) label pairs of a kinematic tree (parents[0] < 0 is the root): the creases at every joint,
+    for self_collisions' ignored_part_pairs."""
+    p = torch.as_tensor(parents).reshape(-1).tolist()
+    return [(j, int(q)) for j, q in enumerate(p) if int(q) >= 0]
+
+
+def _penetration_args(vertices, faces_i32, pairs, sigma, linear_max):
+    v = _cuda_f32(vertices, 'vertices')
+    faces_i32 = _faces_i32(faces_i32)
+    if v.dim() != 3 or v.shape[2] != 3 or faces_i32.dim() != 2 or faces_i32.shape[1] != 3 or faces_i32.shape[0] == 0:
+        raise ValueError(f'vertices must be (B, V, 3) and faces (F >= 1, 3), got {tuple(v.shape)} and '
+                         f'{tuple(faces_i32.shape)}')
+    if not (torch.is_tensor(pairs) and pairs.is_cuda and pairs.dtype == torch.int32):
+        raise RuntimeError('pairs must be a CUDA int32 tensor')
+    pairs = pairs.contiguous()
+    if pairs.dim() != 3 or pairs.shape[0] != v.shape[0] or pairs.shape[2] != 2:
+        raise ValueError(f'pairs must be ({v.shape[0]}, C, 2), got {tuple(pairs.shape)}')
+    if pairs.shape[1] > MAX_PENETRATION_PAIRS:
+        raise ValueError(f'{pairs.shape[1]} pair rows per body exceed the {MAX_PENETRATION_PAIRS} supported')
+    if not (float(sigma) > 0) or float(linear_max) != float(linear_max):
+        raise ValueError('sigma must be > 0 and linear_max not NaN')
+    _incidence_rows(faces_i32, v.shape[1])          # the faces index the vertices
+    return v, faces_i32, pairs
+
+
+def penetration_forward(vertices, faces_i32, pairs, sigma=0.5, penalize_outside=True, linear_max=1000.0):
+    """The distance-field penetration loss (B,) of DistanceFieldPenetrationLoss at the (receiver, intruder) face rows
+    pairs (B, C, 2) int32 (include/shapy_b200.h, shapy_penetration_forward): a row whose first index is < 0 is
+    skipped.  One launch, deterministic."""
+    v, faces_i32, pairs = _penetration_args(vertices, faces_i32, pairs, sigma, linear_max)
+    B, V, F, Cn = v.shape[0], v.shape[1], faces_i32.shape[0], pairs.shape[1]
+    loss = torch.empty(B, dtype=torch.float32, device=v.device)
+    if B == 0:
+        return loss
+    with torch.cuda.device(v.device):
+        check(lib().shapy_penetration_forward(ptr(v), ptr(faces_i32), B, V, F, ptr(pairs), Cn, float(sigma),
+                                              int(bool(penalize_outside)), float(linear_max), ptr(loss), stream_ptr()),
+              'penetration_forward')
+    return loss
+
+
+def penetration_backward(vertices, faces_i32, pairs, grad_loss, sigma=0.5, penalize_outside=True, linear_max=1000.0):
+    """Gradient (B, V, 3) of grad_loss (B,) . penetration_forward with respect to the vertices, the pairs held
+    constant (include/shapy_b200.h, shapy_penetration_backward): one launch, no atomics, bit-identical run to run."""
+    v, faces_i32, pairs = _penetration_args(vertices, faces_i32, pairs, sigma, linear_max)
+    B, V, F, Cn = v.shape[0], v.shape[1], faces_i32.shape[0], pairs.shape[1]
+    g = _cuda_f32(grad_loss, 'grad_loss')
+    if g.shape != (B,):
+        raise ValueError(f'grad_loss must be ({B},), got {tuple(g.shape)}')
+    grad = torch.empty_like(v)
+    if B == 0:
+        return grad
+    with torch.cuda.device(v.device):
+        ws = _WS.get('penetration', lib().shapy_penetration_workspace_bytes(B, Cn), v.device)
+        check(lib().shapy_penetration_backward(ptr(v), ptr(faces_i32), B, V, F, ptr(pairs), Cn, float(sigma),
+                                               int(bool(penalize_outside)), float(linear_max), ptr(g), ptr(grad),
+                                               ptr(ws), ws.numel(), stream_ptr()), 'penetration_backward')
+    return grad
+
+
 def fit_lm_scan_workspace(B, N, V, P, device):
     """The scratch of fit_lm_scan_step (include/shapy_b200.h, shapy_fit_lm_scan_workspace_bytes): a uint8 CUDA tensor,
     allocated once before an LM loop."""
     return _workspace(lib().shapy_fit_lm_scan_workspace_bytes(int(B), int(N), int(V), int(P)), device)
 
 
+def fit_lm_scan_penetration_workspace(B, N, V, P, C, device):
+    """The scratch of fit_lm_scan_step with `penetration` rows of C pairs per body
+    (shapy_fit_lm_scan_penetration_workspace_bytes)."""
+    return _workspace(lib().shapy_fit_lm_scan_penetration_workspace_bytes(int(B), int(N), int(V), int(P), int(C)),
+                      device)
+
+
 def fit_lm_scan_step(state, trial, points, weights, faces_i32, robust_sigma, scan_to_model_weight,
                      model_to_scan_weight, pose_prior_weight, betas_weight, lambda_up, lambda_down, first,
                      trial_vertices, trial_jac, trial_face_idx, trial_bary, trial_nearest, workspace, pose_anchor=None,
-                     meas=None):
+                     meas=None, penetration=None):
     """One Levenberg-Marquardt step per body of the scan fit (include/shapy_b200.h, shapy_fit_lm_scan_step), in place.
     state: {'rot' (B, n_rot, 3, 3), 'betas' (B, NB), 'transl' (B, 3), 'A' (B, P, P) and 'g' (B, P) float64, 'loss',
     'lambda' (B,), 'accepted' (B,) int32}, with meas also 'meas' (B, 5) and 'meas_jac' (B, 5, NB); trial: {'rot',
@@ -904,7 +1054,9 @@ def fit_lm_scan_step(state, trial, points, weights, faces_i32, robust_sigma, sca
     faces_i32 (F, 3); the trial's vertices and Jacobian (smplx_vertex_jacobian, with transl), closest points
     (closest_points) and nearest points (nearest_points; None when model_to_scan_weight is 0).  robust_sigma None or
     inf: least squares.  meas: None or (meas_targets, meas_weights, trial_meas, trial_meas_jac).  workspace:
-    fit_lm_scan_workspace(B, N, V, P)."""
+    fit_lm_scan_workspace(B, N, V, P).  penetration: None, or (pairs (B, C, 2) int32 of self_collisions on the trial's
+    vertices, weight, sigma): the self-penetration rows (shapy_fit_lm_scan_penetration_step), with workspace
+    fit_lm_scan_penetration_workspace(B, N, V, P, C)."""
     what = 'fit_lm_scan_step'
     B, n_rot = trial['rot'].shape[:2]
     nb, (N, V) = trial['betas'].shape[1], (points.shape[1], trial_vertices.shape[1])
@@ -944,11 +1096,23 @@ def fit_lm_scan_step(state, trial, points, weights, faces_i32, robust_sigma, sca
     if B == 0:
         return
     m = list(meas) if meas is not None else [None] * 4
+    head = (B, N, V, n_rot, nb, ptr(points), ptr(weights), ptr(faces_i32))
+    terms = (sigma, float(scan_to_model_weight), float(model_to_scan_weight), float(pose_prior_weight),
+             float(betas_weight), ptr(m[0]), ptr(m[1]))
+    if penetration is None:
+        L, args = lib().shapy_fit_lm_scan_step, head + (ptr(pose_anchor),) + terms
+    else:
+        pairs, pw_, psig = penetration
+        if not (torch.is_tensor(pairs) and pairs.is_cuda and pairs.is_contiguous() and pairs.dtype == torch.int32
+                and pairs.dim() == 3 and pairs.shape[0] == B and pairs.shape[2] == 2):
+            raise RuntimeError(f'{what}: the penetration pairs must be a contiguous int32 CUDA ({B}, C, 2) tensor')
+        _incidence_rows(faces_i32, V)      # the faces index the vertices
+        L = lib().shapy_fit_lm_scan_penetration_step
+        args = head + (faces_i32.shape[0], ptr(pose_anchor)) + terms + (ptr(pairs), pairs.shape[1], float(pw_),
+                                                                          float(psig))
     with torch.cuda.device(points.device):
-        check(lib().shapy_fit_lm_scan_step(
-            B, N, V, n_rot, nb, ptr(points), ptr(weights), ptr(faces_i32), ptr(pose_anchor), sigma,
-            float(scan_to_model_weight), float(model_to_scan_weight), float(pose_prior_weight), float(betas_weight),
-            ptr(m[0]), ptr(m[1]), float(lambda_up), float(lambda_down), int(bool(first)),
+        check(L(
+            *args, float(lambda_up), float(lambda_down), int(bool(first)),
             *[ptr(state[k]) for k in ('rot', 'betas', 'transl', 'A', 'g')],
             *[ptr(state.get(k)) for k in ('meas', 'meas_jac')],
             *[ptr(state[k]) for k in ('loss', 'lambda', 'accepted')],

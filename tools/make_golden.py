@@ -43,6 +43,10 @@ Everything written here is a small fixture that travels to the GPU box, where
                         map_keypoints('openpose25_v1' -> 'smplx') and the OpenPose part index lists the thresholds use
   preprocess.npz        reference input stage (transf_utils.crop with cv2 + ToTensor + Normalize) on seeded uint8 images:
                         crop windows, crops with OpenCV's portable path (IPP off) and with this container's IPP build
+  ref_penetration.npz   the reference's DistanceFieldPenetrationLoss (mesh_mesh_intersection/loss.py, its own code) in
+                        float64 on seeded triangle soups with (receiver, intruder) rows padded with -1: the loss and its
+                        gradient with respect to the triangles for each (sigma, penalize_outside, linear_max,
+                        point2plane) setting, and a batch without a row
 """
 import hashlib
 import json
@@ -670,9 +674,46 @@ def openpose_fixture(crop_size=256):
     print('ref_openpose.npz', {k: v.shape for k, v in arrs.items()}, len(mapping['pairs']), 'mapped keypoints')
 
 
+PENETRATION_SETTINGS = [(0.5, True, 1000.0, False), (0.5, True, 1000.0, True), (0.5, False, 1000.0, False),
+                        (0.05, True, 1000.0, False), (0.3, True, 0.4, False), (1.5, False, 1000.0, True)]
+
+
+def penetration_fixture():
+    import importlib.util
+    spec = importlib.util.spec_from_file_location(
+        'ref_penetration_loss', os.path.join(REF, 'mesh-mesh-intersection', 'mesh_mesh_intersection', 'loss.py'))
+    m = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(m)
+    rng = np.random.default_rng(20261018)
+    B, F, C = 3, 24, 20
+    # clusters of small triangles around shared centres, so that many rows have points inside the cones
+    centres = rng.normal(size=(B, F, 1, 3)) * 0.05
+    tris = centres + rng.normal(size=(B, F, 3, 3)) * 0.08
+    idx = np.full((B, C, 2), -1, np.int64)
+    for b, n in enumerate([C, 11, 5]):
+        r = rng.integers(0, F, size=(n,))
+        i = (r + rng.integers(1, F, size=(n,))) % F
+        idx[b, :n, 0], idx[b, :n, 1] = r, i
+    perm = rng.permutation(C)              # padding rows between real ones
+    idx[1] = idx[1][perm]
+    out = dict(triangles=tris, collision_idxs=idx, settings=np.array(PENETRATION_SETTINGS, np.float64))
+    for k, (sigma, po, lmax, p2p) in enumerate(PENETRATION_SETTINGS):
+        t = torch.from_numpy(tris).requires_grad_(True)
+        loss = m.DistanceFieldPenetrationLoss(sigma=sigma, point2plane=p2p, penalize_outside=po, linear_max=lmax)(
+            t, torch.from_numpy(idx))
+        loss.sum().backward()
+        out[f'loss_{k}'] = loss.detach().numpy()
+        out[f'grad_{k}'] = t.grad.numpy()
+    t = torch.from_numpy(tris).requires_grad_(True)
+    out['loss_empty'] = m.DistanceFieldPenetrationLoss()(t, torch.full((B, 4, 2), -1, dtype=torch.long)).detach().numpy()
+    np.savez_compressed(os.path.join(G, 'ref_penetration.npz'), **out)
+    print('ref_penetration.npz', {k: v.tolist() for k, v in out.items() if k.startswith('loss')})
+
+
 if __name__ == '__main__':
     which = sys.argv[1:] or ['body', 'smplx', 'head', 'hrnet', 'preprocess', 'b2a', 'p2p', 'v2v', 'align', 'smplx_live',
-                             'smplx_full', 'camera', 'keypoint', 'measure_grad', 'smplx_grad', 'openpose']
+                             'smplx_full', 'camera', 'keypoint', 'measure_grad', 'smplx_grad', 'openpose',
+                             'penetration']
     torch.set_num_threads(8)
     if 'body' in which:
         body_fixture()
@@ -708,3 +749,5 @@ if __name__ == '__main__':
         measure_grad_fixture()
     if 'openpose' in which:
         openpose_fixture()
+    if 'penetration' in which:
+        penetration_fixture()
