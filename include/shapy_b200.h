@@ -21,6 +21,8 @@
  *                        terms of shapy_b200.fit.fit_body_to_scan, on the LBVH of shapy_mmi_forward)
  *   shapy_self_collisions  (the self-collision pairs the reference's BVH gives SMPLify-X, on the scan LBVH)
  *   shapy_penetration_*  DistanceFieldPenetrationLoss mesh-mesh-intersection/mesh_mesh_intersection/loss.py:201-317
+ *   shapy_silhouette_*, shapy_render_silhouette   (no reference counterpart: the silhouette term of the perspective
+ *                        2D fit, for the person masks SSP-3D ships, regressor/human_shape/data/datasets/ssp3d.py)
  *   shapy_head_*         IterativeRegression.forward regressor/human_shape/models/common/networks.py:536-592
  *   shapy_hrnet_*        HighResolutionNet.forward  regressor/human_shape/models/backbone/hrnet.py:426-498
  *   shapy_p2p_error      v2vhdError.__call__        regressor/human_shape/utils/metrics.py:368-456
@@ -720,6 +722,53 @@ int shapy_penetration_backward(const float *vertices, const int32_t *faces, int 
                                const int32_t *pairs, int num_pairs, float sigma, int penalize_outside,
                                float linear_max, const float *grad_loss, float *grad_vertices, void *workspace,
                                size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------ silhouettes */
+/* Conventions of the silhouette term of the perspective 2D fit.  A mask is (B,H,W) bytes, nonzero a person pixel, in
+ * the pixel frame of the fit's keypoints: pixel (r, c) has its centre at (x = c, y = r), as OpenPose and cv2 have it.
+ * The projection is the fit's, p = f (Y_x / Y_z, Y_y / Y_z) + (px, py) with intrinsics (B,3) = (f, px, py) and Y the
+ * posed vertex in the camera frame (transl included).  1 <= H, W <= 4096: larger masks return SHAPY_ERR_UNSUPPORTED
+ * before any launch.  No float atomics: every result is bit-identical run to run and alone or in a batch.
+ *
+ * shapy_silhouette_prepare, once per fit, five launches.  dist (B,H,W) fp32: the exact Euclidean distance from each
+ * pixel centre to the nearest person pixel, 0 inside the mask and 0 everywhere for an empty mask; the squared distance
+ * is computed in integers (a column pass, then per row the lower envelope of parabolas, Meijster's second phase) and
+ * dist = sqrtf((float)d^2).  The contour pixels are the person pixels with a 4-neighbour inside the image that is not
+ * a person pixel (the image border makes no pixel contour); contour_count (B) int32 is their number.  In raster order,
+ * every k-th of them, k = ceil(count / max_points) (1 when count <= max_points), is kept: contour (B,max_points,3)
+ * holds (c, r, 0) of the kept pixels first, then zeros, and contour_w (B,max_points) 1 for a kept pixel and 0 for
+ * padding: the points / weights inputs of shapy_closest_points.  workspace >= shapy_silhouette_workspace_bytes(B, H).
+ * max_points <= 0 is SHAPY_ERR_ARG, > 32768 SHAPY_ERR_UNSUPPORTED. */
+size_t shapy_silhouette_workspace_bytes(int batch, int height);
+int shapy_silhouette_prepare(const uint8_t *masks, int batch, int height, int width, int max_points, float *dist,
+                             float *contour, float *contour_w, int32_t *contour_count, void *workspace,
+                             size_t workspace_bytes, void *stream);
+
+/* The model -> mask half of the silhouette term.  vertices (B,V,3) in the camera frame, dist (B,H,W) of
+ * shapy_silhouette_prepare.  Each vertex is projected at the depth max(Y_z, 1e-3) (a vertex behind the camera gives no
+ * NaN or inf) to (u, v); projected (B,V,3) = (u, v, 0), the flat mesh whose closest points to the contour are the mask
+ * -> model half.  D(u, v) is dist sampled bilinearly at (u, v) clamped to the rectangle of pixel centres [0, W-1] x
+ * [0, H-1], in the cell [c0, c0 + 1] x [r0, r0 + 1], c0 = min(floor(x), W - 2) (0 when W = 1), likewise r0.
+ * model_to_mask (B) = (1/V) sum_v D(u_v, v_v)^2, one CTA per body, a fixed-order reduction.  One launch. */
+int shapy_silhouette_forward(const float *vertices, const float *intrinsics, const float *dist, int batch,
+                             int num_verts, int height, int width, float *projected, float *model_to_mask,
+                             void *stream);
+
+/* grad_vertices (B,V,3) of grad_model_to_mask (B) . model_to_mask + <grad_projected, projected>: per vertex, the
+ * bilinear gradient of D^2 recomputed (0 along an axis where (u, v) is clamped to the image) plus the (u, v) of
+ * grad_projected (B,V,3) (the mask -> model cotangent of shapy_closest_points_backward on the projected mesh, its z
+ * unread; NULL for none), through the projection; the depth gets no gradient where it is clamped.  One launch, one
+ * thread per vertex, no atomics. */
+int shapy_silhouette_backward(const float *vertices, const float *intrinsics, const float *dist, int batch,
+                              int num_verts, int height, int width, const float *grad_model_to_mask,
+                              const float *grad_projected, float *grad_vertices, void *stream);
+
+/* mask (B,H,W) bytes: 1 where the pixel centre lies inside a projected triangle of faces (F,3) whose three vertices
+ * have Y_z > 0 (the inclusive float32 edge test, either winding), else 0.  A triangle with an index outside [0, V) is
+ * skipped.  One warp per triangle over its clamped pixel box, so triangles of any size render; the result is a
+ * function of the triangles alone.  A memset and one launch (none when F = 0). */
+int shapy_render_silhouette(const float *vertices, const int32_t *faces, const float *intrinsics, int batch,
+                            int num_verts, int num_faces, int height, int width, uint8_t *mask, void *stream);
 
 /* ------------------------------------------------------------ regression head */
 /* params_out (num_stages, B, P).  W0 (H0, F+P), W1 (H1, H0), W2 (P, H1) row-major as nn.Linear stores

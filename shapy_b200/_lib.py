@@ -175,7 +175,12 @@ _SIGS = {
     'shapy_penetration_backward': (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p, c_int, C.c_float, c_int,
                                                                               C.c_float] + [c_void_p] * 3
                                    + [c_size_t, c_void_p]),
-    'shapy_fit_lm_scan_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'shapy_silhouette_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'shapy_silhouette_prepare': (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] * 5 + [c_size_t, c_void_p]),
+    'shapy_silhouette_forward': (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p] * 3),
+    'shapy_silhouette_backward': (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p] * 4),
+    'shapy_render_silhouette': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p] * 2),
+    'shapy_fit_lm_scan_workspace_bytes':(c_size_t, [c_int, c_int, c_int, c_int]),
     'shapy_fit_lm_scan_step': (c_int, [c_int] * 5 + [c_void_p] * 4 + [C.c_float] * 5 + [c_void_p] * 2
                                + [C.c_float, C.c_float, c_int] + [c_void_p] * 21 + [c_size_t, c_void_p]),
     'shapy_fit_lm_scan_penetration_workspace_bytes': (c_size_t, [c_int] * 5),

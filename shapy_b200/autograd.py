@@ -11,6 +11,8 @@ only).
                                                 scan points (B,N,3) on posed meshes (B,V,3) -> sq_dist (B,N)
     PenetrationFunction.apply(vertices, faces_i32, pairs, sigma, penalize_outside, linear_max)
                                                 self-penetration loss at fixed face pairs (B,C,2) -> (B,)
+    SilhouetteFunction.apply(vertices, intrinsics, faces_i32, dist, contour, contour_w, inv_count, tree)
+                                                the silhouette term of perspective posed meshes against masks -> (B,)
 
 The forward of each is the same launches as the no-grad path; the backward is the matching CUDA adjoint
 (measure_smem_kernel in gradient mode, the shape-blend adjoint, shapy_smplx_backward which recomputes the posed
@@ -141,6 +143,33 @@ class PenetrationFunction(torch.autograd.Function):
         vertices, faces_i32, pairs = ctx.saved_tensors
         g = _ops.penetration_backward(vertices, faces_i32, pairs, grad_loss.contiguous(), *ctx.args)
         return g, None, None, None, None, None
+
+
+class SilhouetteFunction(torch.autograd.Function):
+    """SilhouetteFunction.apply(vertices, intrinsics, faces_i32, dist, contour, contour_w, inv_count, tree=None) -> (B,):
+    the silhouette term of each body without its weight, (1/V) sum_v D(pi(v))^2 + inv_count sum_i d_i^2, from
+    ops.silhouette_prepare's dist, contour and contour_w; inv_count (B,) is 1 / (kept contour pixels), 0 for none.  D
+    is ops.silhouette_forward's; d_i the distance of contour pixel i to the projected mesh (u, v, 0), by
+    ops.closest_points on `tree` (an ops.ScanTree, refit after the first call).  Differentiable in the vertices: the
+    backward holds the closest face and barycentrics (ops.closest_points_backward on the projected mesh) and chains both
+    halves through the projection in ops.silhouette_backward."""
+
+    @staticmethod
+    def forward(ctx, vertices, intrinsics, faces_i32, dist, contour, contour_w, inv_count, tree=None):
+        proj, m2m = _ops.silhouette_forward(vertices, intrinsics, dist)
+        face, bary, d2 = _ops.closest_points(proj, faces_i32, contour, contour_w, tree=tree)
+        ctx.save_for_backward(vertices, intrinsics, faces_i32, dist, contour, inv_count, proj, face, bary)
+        return m2m + (d2 * inv_count[:, None]).sum(1)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        vertices, intrinsics, faces_i32, dist, contour, inv_count, proj, face, bary = ctx.saved_tensors
+        grad = grad.contiguous()
+        g_d2 = (grad * inv_count)[:, None].expand(face.shape).contiguous()
+        g_proj = _ops.closest_points_backward(proj, faces_i32, contour, face, bary, g_d2)
+        g = _ops.silhouette_backward(vertices, intrinsics, dist, grad, g_proj)
+        return g, None, None, None, None, None, None, None
 
 
 def wants_grad(t) -> bool:

@@ -23,8 +23,9 @@ ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC',
           '--expt-relaxed-constexpr']
 # per-file extra flags: the triangle predicates must round like the plain-C oracle, and the LM step like its NumPy
-# restatement (oracle/lm_oracle.py)
-EXTRA = {'measure.cu': ['-fmad=false'], 'bvh.cu': ['-fmad=false'], 'fit.cu': ['-fmad=false']}
+# restatement (oracle/lm_oracle.py), and the silhouette projection and edge test like tests/silhouette_oracle.py
+EXTRA = {'measure.cu': ['-fmad=false'], 'bvh.cu': ['-fmad=false'], 'fit.cu': ['-fmad=false'],
+         'silhouette.cu': ['-fmad=false']}
 
 
 def sources():

@@ -298,6 +298,75 @@ def _penetration_term(fn, body_model, method, weight, sigma, max_pairs, part_lab
     return _PenetrationTerm(weight, sigma, max_pairs, part_labels, ignored_part_pairs, faces)
 
 
+class _SilhouetteTerm:
+    """The silhouette term of the perspective 2D fit: weight x autograd.SilhouetteFunction, the model -> mask mean of
+    the squared mask distance at the projected vertices plus the mask -> model mean of the squared distance of the
+    kept contour pixels to the projected mesh, in px^2.  The masks are prepared once (ops.silhouette_prepare) and the
+    projected mesh's tree is built at the first call and refit after.  `last` holds the latest unweighted value."""
+
+    def __init__(self, weight, masks, max_points, faces, intr):
+        from . import ops
+        self.weight, self.masks, self.faces, self.intr = float(weight), masks, faces, intr
+        self.dist, self.contour, self.contour_w, _ = ops.silhouette_prepare(masks, max_points)
+        n = self.contour_w.sum(1)
+        self.inv_count = torch.where(n > 0, 1.0 / n.clamp(min=1.0), torch.zeros_like(n))
+        self.tree = ops.ScanTree()
+        self.last = None
+
+    def __call__(self, vertices):
+        from .autograd import SilhouetteFunction
+        s = SilhouetteFunction.apply(vertices, self.intr, self.faces, self.dist, self.contour, self.contour_w,
+                                     self.inv_count, self.tree)
+        self.last = s.detach()
+        return self.weight * s
+
+    def outputs(self, vertices):
+        """'silhouette' (B,) of the latest call, +inf for a body with a vertex at Y_z <= 0 or not finite, and
+        'silhouette_iou' (B,): the IoU of the rendered silhouette of `vertices` with the mask (1 when both are
+        empty)."""
+        from . import ops
+        z = vertices[..., 2]
+        bad = (~(z > 0) | ~torch.isfinite(z)).any(1)
+        sil = torch.where(bad, torch.full_like(self.last, float('inf')), self.last)
+        r = ops.render_silhouette(vertices.detach().contiguous(), self.faces, self.intr, self.masks.shape[1],
+                                  self.masks.shape[2])
+        m = self.masks != 0
+        inter, union = (r & m).sum((1, 2)), (r | m).sum((1, 2))
+        iou = torch.where(union > 0, inter.float() / union.clamp(min=1).float(), torch.ones_like(sil))
+        return {'silhouette': sil, 'silhouette_iou': iou}
+
+
+def _silhouette_masks(fn, body_model, method, silhouettes, weight, max_points, B, intr, device, groups, share_pose):
+    """None without silhouettes (the fit runs exactly as without the term), else the masks on the device for a
+    _SilhouetteTerm; ValueError, before any launch, for a bad argument or an unsupported fit."""
+    from .ops import MAX_SCAN_FACES, MAX_SCAN_POINTS, MAX_SILHOUETTE_SIDE
+    if silhouettes is None:
+        return None
+    if method != 'adam':
+        raise ValueError(f"{fn}: the silhouette term is not supported with method={method!r}")
+    if intr is None:
+        raise ValueError(f'{fn}: the silhouette term needs the perspective fit (focal_length and principal_point)')
+    if groups is not None or share_pose:
+        raise ValueError(f'{fn}: the silhouette term is not supported with groups or share_pose')
+    if not (0 <= float(weight) < float('inf')):
+        raise ValueError(f'{fn}: silhouette_weight must be finite and >= 0, got {weight}')
+    if not 1 <= int(max_points) <= MAX_SCAN_POINTS:
+        raise ValueError(f'{fn}: max_silhouette_points must be in [1, {MAX_SCAN_POINTS}], got {max_points}')
+    m = torch.as_tensor(silhouettes)
+    if m.dtype not in (torch.uint8, torch.bool):
+        raise ValueError(f'{fn}: silhouettes must be uint8 or bool, got {m.dtype}')
+    if m.dim() != 3 or m.shape[0] != B:
+        raise ValueError(f'{fn}: silhouettes must be ({B}, H, W), got {tuple(m.shape)}')
+    if not (1 <= m.shape[1] <= MAX_SILHOUETTE_SIDE and 1 <= m.shape[2] <= MAX_SILHOUETTE_SIDE):
+        raise ValueError(f'{fn}: silhouettes must be at most {MAX_SILHOUETTE_SIDE} x {MAX_SILHOUETTE_SIDE} and not '
+                         f'empty, got {tuple(m.shape[1:])}')
+    faces = body_model.faces_i32
+    if faces.shape[0] > MAX_SCAN_FACES:
+        raise ValueError(f'{fn}: the model has {faces.shape[0]} faces, the silhouette term takes at most '
+                         f'{MAX_SCAN_FACES}')
+    return m.to(device).contiguous()
+
+
 def fit_betas_to_measurements(body_model, body_measurements, targets, weights=None, betas_weight=0.0, iterations=None,
                               lr=0.05, betas_init=None, batch_size=None, method='adam',
                               circumference_derivative='reference'):
@@ -693,6 +762,9 @@ def _init_2d(init, B, nb, device, method, x=None, w=None, intr=None):
 
 # the distance [m] a perspective fit starts at without a translation: a person photographed whole with a phone
 START_DEPTH = 3.0
+# the default weight of the silhouette term against the keypoint term, both in px^2: the best median IoU of 1, 10 and
+# 100 in tests/test_gpu_fit_silhouette.py (README, "Silhouettes")
+SILHOUETTE_WEIGHT = 100.0
 
 
 def _intrinsics(focal_length, principal_point, B, device):
@@ -791,7 +863,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
                              circumference_derivative='reference', groups=None, share_pose=False, focal_length=None,
                              principal_point=None, pose_width=22, fit_expression=False, expression_weight=0.0,
                              penetration_weight=0.0, penetration_sigma=0.5, max_penetration_pairs=1024,
-                             part_labels=None, ignored_part_pairs=None):
+                             part_labels=None, ignored_part_pairs=None, silhouettes=None,
+                             silhouette_weight=SILHOUETTE_WEIGHT, max_silhouette_points=4096):
     """Fits pose, shape and the weak-perspective camera so that the projected keypoints proj_joints = softplus(c0)
     (joints_xy + c[1:3]) match `keypoints2d` (B, K, 2), K = body_model's keypoint count, in the normalised crop frame of
     the regressor's proj_joints (shapy_b200.keypoints2d.to_crop maps pixel detections there).
@@ -855,8 +928,18 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     (the eyes: the OpenPose pupils are dropped on load) is held by its prior alone, and without a prior it stays where
     it starts.  groups, share_pose and measurements are not supported on the wide path.
     penetration_weight > 0, penetration_sigma, max_penetration_pairs, part_labels, ignored_part_pairs: the
-    self-penetration term of fit_body_to_keypoints, for a single-image fit (no groups) with method='adam'."""
+    self-penetration term of fit_body_to_keypoints, for a single-image fit (no groups) with method='adam'.
+    silhouettes: None, or person masks (B, H, W) uint8 or bool (nonzero a person pixel, H, W <= 4096) in the pixel
+    frame of the keypoints (pixel (r, c) centred at (x = c, y = r)), for a perspective fit with method='adam' (the wide
+    path and the penetration term included; not with groups or share_pose).  The loss gains silhouette_weight times
+    (1/V) sum_v D(p_v)^2 + (1/N) sum_i d_i^2 in px^2: D the exact distance to the mask sampled bilinearly at each
+    projected vertex (clamped to the image), d_i the distance of each of the N kept contour pixels (at most
+    max_silhouette_points, every k-th in raster order past that) to the projected mesh.  The result gains 'silhouette'
+    (B,) (unweighted, +inf for a body with a vertex at Y_z <= 0) and 'silhouette_iou' (B,), the IoU of the rendered
+    silhouette of the final body with its mask.  See the README's silhouette section."""
     fn = 'fit_body_to_keypoints_2d'
+    if silhouettes is not None and (groups is not None or share_pose):
+        raise ValueError(f'{fn}: the silhouette term is not supported with groups or share_pose')
     pt = _penetration_term(fn, body_model, method, penetration_weight, penetration_sigma, max_penetration_pairs,
                            part_labels, ignored_part_pairs)
     if pt is not None and groups is not None:
@@ -903,6 +986,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     x, w = _keypoints_2d(fn, keypoints2d, weights, device)
     B = x.shape[0]
     intr = None if focal_length is None else _intrinsics(focal_length, principal_point, B, device)
+    masks = _silhouette_masks(fn, body_model, method, silhouettes, silhouette_weight, max_silhouette_points, B, intr,
+                              device, groups, share_pose)
     params = _init_2d(init, B, nb, device, method, x, w, intr)
     parts = _parts_in(pose_width)
     raw_init = _raw_init(init)
@@ -933,6 +1018,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     if method == 'lm':
         return _fit_keypoints_2d_lm(body_model, x, w, params, parts, rot0, anchor, int(iterations), sigma, pw, jw, bw,
                                     ew, ne, mt, intr, wide)
+    st = None if masks is None else _SilhouetteTerm(silhouette_weight, masks, max_silhouette_points,
+                                                    body_model.faces_i32, intr)
 
     def loss_fn():
         grot = Rot6dFunction.apply(params['global_rot'])
@@ -944,6 +1031,8 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
         per_body = _kp2d_loss(out['proj_joints'], x, w, sigma, pw, rot, anchor, bw, params['betas'], jw, ew, expr)
         if pt is not None:
             per_body = per_body + pt(out['vertices'])
+        if st is not None:
+            per_body = per_body + st(out['vertices'])
         meas = None
         if mt is not None:      # _kp2d_loss already counted betas_weight |betas|^2
             meas = mt.measure(body_model, params['betas'])
@@ -954,6 +1043,9 @@ def fit_body_to_keypoints_2d(body_model, keypoints2d, weights=None, init=None, m
     if intr is not None:
         per_body = _depth_rule(per_body, out['joints'][:], w)
     wide_out = {'full_pose_mat': rot} if wide else {}
+    if st is not None:
+        wide_out.update(st.outputs(out['vertices']))
+        per_body = torch.where(torch.isinf(wide_out['silhouette']), wide_out['silhouette'], per_body)
     return _adam_result(params, rot[:, :1], rot[:, 1:22], meas, **wide_out, keypoints=out['joints'][:],
                         proj_joints=out['proj_joints'], loss=per_body, **({} if pt is None else pt.outputs()))
 
@@ -1712,7 +1804,14 @@ def main(argv=None):
                         'its pairs filtered by the parts of ops.face_parts and the parent-child creases')
     p.add_argument('--penetration-sigma', dest='penetration_sigma', type=float, default=0.5,
                    help='the cone height sigma of the self-penetration term')
+    p.add_argument('--silhouettes', type=str, default=None,
+                   help='with a perspective --keypoints-2d (adam, single image): an npz with `masks` (B, H, W), nonzero '
+                        'a person pixel, in the keypoints\' pixel frame; the result gains silhouette and silhouette_iou')
+    p.add_argument('--silhouette-weight', dest='silhouette_weight', type=float, default=SILHOUETTE_WEIGHT,
+                   help='the weight of the silhouette term (px^2 against the keypoints\' px^2)')
     a = p.parse_args(argv)
+    if a.silhouettes and (not a.keypoints_2d or a.calibrated or a.sequence):
+        raise SystemExit('--silhouettes needs --keypoints-2d and is not supported with --calibrated or --sequence')
     if a.penetration_weight and not ((a.scan and not a.keypoints_2d) or
                                      (a.keypoints_2d and not (a.calibrated or a.sequence))):
         raise SystemExit('--penetration-weight needs --scan or --keypoints-2d and is not supported with --calibrated '
@@ -1808,13 +1907,18 @@ def _main_keypoints_2d(a, model, bm, targets):
         return _main_calibrated(a, model, bm, targets, d, x, w, focal, pp, groups)
     if a.sequence:
         return _main_sequence(a, model, d, x, w, focal, pp, init)
+    sil = {}
+    if a.silhouettes:
+        if not persp:
+            raise SystemExit('--silhouettes needs a perspective --keypoints-2d (a focal_length in the npz)')
+        sil = dict(silhouettes=np.load(a.silhouettes)['masks'], silhouette_weight=a.silhouette_weight)
     res = fit_body_to_keypoints_2d(model, x, w, init=init, method=a.method, iterations=a.iterations,
                                    robust_sigma=a.robust_sigma, pose_prior_weight=a.pose_prior_weight,
                                    betas_weight=a.betas_weight, lr=a.lr, body_measurements=bm, measurements=targets,
                                    circumference_derivative=a.circumference_derivative, groups=groups,
                                    share_pose=a.share_pose, focal_length=focal, principal_point=pp,
                                    pose_width=a.pose_width, fit_expression=a.fit_expression,
-                                   expression_weight=a.expression_weight, **_penetration_args(a, model))
+                                   expression_weight=a.expression_weight, **_penetration_args(a, model), **sil)
     _save_result(a.output, res, {'bodies': int(x.shape[0])}, groups=groups)
 
 

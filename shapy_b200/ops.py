@@ -1030,6 +1030,130 @@ def penetration_backward(vertices, faces_i32, pairs, grad_loss, sigma=0.5, penal
     return grad
 
 
+# ---------------------------------------------------------------------------------------------- silhouettes
+MAX_SILHOUETTE_SIDE = 4096    # mask height and width (the distance transform's row pass keeps a row in shared memory)
+
+
+def _silhouette_size(what, height, width):
+    if not (1 <= int(height) <= MAX_SILHOUETTE_SIDE and 1 <= int(width) <= MAX_SILHOUETTE_SIDE):
+        raise ValueError(f'{what}: masks must be at least 1 x 1 and at most {MAX_SILHOUETTE_SIDE} x '
+                         f'{MAX_SILHOUETTE_SIDE}, got {int(height)} x {int(width)}')
+    return int(height), int(width)
+
+
+def _silhouette_camera(what, vertices, intrinsics):
+    v = _cuda_f32(vertices, 'vertices')
+    if v.dim() != 3 or v.shape[2] != 3 or v.shape[1] == 0:
+        raise ValueError(f'{what}: vertices must be (B, V >= 1, 3), got {tuple(v.shape)}')
+    intr = _cuda_f32(intrinsics, 'intrinsics')
+    if intr.shape != (v.shape[0], 3):
+        raise ValueError(f'{what}: intrinsics must be ({v.shape[0]}, 3) (f, px, py), got {tuple(intr.shape)}')
+    return v, intr
+
+
+def _silhouette_dist(what, dist, B):
+    d = _cuda_f32(dist, 'dist')
+    if d.dim() != 3 or d.shape[0] != B:
+        raise ValueError(f'{what}: dist must be ({B}, H, W), got {tuple(d.shape)}')
+    _silhouette_size(what, d.shape[1], d.shape[2])
+    return d
+
+
+def silhouette_prepare(masks, max_points):
+    """The distance transform and contour of person masks (include/shapy_b200.h, shapy_silhouette_prepare): masks (B, H,
+    W) uint8 or bool on the device, nonzero a person pixel, H, W <= MAX_SILHOUETTE_SIDE; max_points in [1,
+    MAX_SCAN_POINTS].  Returns (dist (B, H, W), contour (B, max_points, 3), contour_w (B, max_points), count (B,) int32):
+    the exact Euclidean distance to the nearest person pixel (0 inside, 0 everywhere for an empty mask), the kept
+    contour pixels (c, r, 0) in raster order then zero padding, their weights (1 kept, 0 padding) and the number of
+    contour pixels found.  Five launches, deterministic."""
+    if not (torch.is_tensor(masks) and masks.is_cuda and masks.dtype in (torch.uint8, torch.bool)):
+        raise ValueError('silhouette_prepare: masks must be a CUDA uint8 or bool tensor')
+    if masks.dim() != 3:
+        raise ValueError(f'silhouette_prepare: masks must be (B, H, W), got {tuple(masks.shape)}')
+    B = masks.shape[0]
+    H, W = _silhouette_size('silhouette_prepare', masks.shape[1], masks.shape[2])
+    max_points = int(max_points)
+    if not 1 <= max_points <= MAX_SCAN_POINTS:
+        raise ValueError(f'silhouette_prepare: max_points must be in [1, {MAX_SCAN_POINTS}], got {max_points}')
+    m = masks.contiguous()
+    if m.dtype == torch.bool:
+        m = m.view(torch.uint8)
+    dev = m.device
+    dist = torch.empty(B, H, W, dtype=torch.float32, device=dev)
+    contour = torch.empty(B, max_points, 3, dtype=torch.float32, device=dev)
+    contour_w = torch.empty(B, max_points, dtype=torch.float32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    if B == 0:
+        return dist, contour, contour_w, count
+    with torch.cuda.device(dev):
+        ws = _WS.get('silhouette', lib().shapy_silhouette_workspace_bytes(B, H), dev)
+        check(lib().shapy_silhouette_prepare(ptr(m), B, H, W, max_points, ptr(dist), ptr(contour), ptr(contour_w),
+                                             ptr(count), ptr(ws), ws.numel(), stream_ptr()), 'silhouette_prepare')
+    return dist, contour, contour_w, count
+
+
+def silhouette_forward(vertices, intrinsics, dist):
+    """The model -> mask half of the silhouette term (include/shapy_b200.h, shapy_silhouette_forward): vertices (B, V,
+    3) in the camera frame, intrinsics (B, 3) (f, px, py), dist (B, H, W) of silhouette_prepare.  Returns (projected
+    (B, V, 3) = (u, v, 0) at the depth max(Y_z, 1e-3), model_to_mask (B,) = the mean over the vertices of the squared
+    bilinear distance at the projection clamped to the image).  One launch, deterministic."""
+    v, intr = _silhouette_camera('silhouette_forward', vertices, intrinsics)
+    B, V = v.shape[:2]
+    d = _silhouette_dist('silhouette_forward', dist, B)
+    proj = torch.empty_like(v)
+    m2m = torch.empty(B, dtype=torch.float32, device=v.device)
+    if B == 0:
+        return proj, m2m
+    with torch.cuda.device(v.device):
+        check(lib().shapy_silhouette_forward(ptr(v), ptr(intr), ptr(d), B, V, d.shape[1], d.shape[2], ptr(proj),
+                                             ptr(m2m), stream_ptr()), 'silhouette_forward')
+    return proj, m2m
+
+
+def silhouette_backward(vertices, intrinsics, dist, grad_model_to_mask, grad_projected=None):
+    """Gradient (B, V, 3) of grad_model_to_mask (B,) . model_to_mask + <grad_projected, projected> of
+    silhouette_forward with respect to the vertices (include/shapy_b200.h, shapy_silhouette_backward); grad_projected
+    (B, V, 3) or None, its z unread.  One launch, no atomics."""
+    v, intr = _silhouette_camera('silhouette_backward', vertices, intrinsics)
+    B, V = v.shape[:2]
+    d = _silhouette_dist('silhouette_backward', dist, B)
+    g = _cuda_f32(grad_model_to_mask, 'grad_model_to_mask')
+    if g.shape != (B,):
+        raise ValueError(f'silhouette_backward: grad_model_to_mask must be ({B},), got {tuple(g.shape)}')
+    if grad_projected is not None:
+        grad_projected = _cuda_f32(grad_projected, 'grad_projected')
+        if grad_projected.shape != v.shape:
+            raise ValueError(f'silhouette_backward: grad_projected must be {tuple(v.shape)}, got '
+                             f'{tuple(grad_projected.shape)}')
+    grad = torch.empty_like(v)
+    if B == 0:
+        return grad
+    with torch.cuda.device(v.device):
+        check(lib().shapy_silhouette_backward(ptr(v), ptr(intr), ptr(d), B, V, d.shape[1], d.shape[2], ptr(g),
+                                              ptr(grad_projected), ptr(grad), stream_ptr()), 'silhouette_backward')
+    return grad
+
+
+def render_silhouette(vertices, faces_i32, intrinsics, height, width):
+    """The silhouette (B, height, width) bool of each posed mesh (include/shapy_b200.h, shapy_render_silhouette): a
+    pixel is set when its centre lies inside a projected triangle whose three vertices have Y_z > 0.  vertices (B, V, 3)
+    in the camera frame, faces_i32 (F, 3), intrinsics (B, 3) (f, px, py).  Bit-identical run to run and alone or in a
+    batch."""
+    v, intr = _silhouette_camera('render_silhouette', vertices, intrinsics)
+    H, W = _silhouette_size('render_silhouette', height, width)
+    faces_i32 = _faces_i32(faces_i32)
+    if faces_i32.dim() != 2 or faces_i32.shape[1] != 3:
+        raise ValueError(f'render_silhouette: faces must be (F, 3), got {tuple(faces_i32.shape)}')
+    B, V = v.shape[:2]
+    mask = torch.empty(B, H, W, dtype=torch.bool, device=v.device)
+    if B == 0:
+        return mask
+    with torch.cuda.device(v.device):
+        check(lib().shapy_render_silhouette(ptr(v), ptr(faces_i32), ptr(intr), B, V, faces_i32.shape[0], H, W,
+                                            ptr(mask.view(torch.uint8)), stream_ptr()), 'render_silhouette')
+    return mask
+
+
 def fit_lm_scan_workspace(B, N, V, P, device):
     """The scratch of fit_lm_scan_step (include/shapy_b200.h, shapy_fit_lm_scan_workspace_bytes): a uint8 CUDA tensor,
     allocated once before an LM loop."""
