@@ -407,10 +407,11 @@ extern "C" int shapy_mmi_forward_f64(const double *query, const double *target, 
 //                             order)
 //
 // The result is a function of the primitives and the queries only, not of the tree: a box is pruned only when its
-// squared distance exceeds the current best by more than a relative 1e-5 and an absolute 1e-12 m^2, which covers the
-// rounding of both distances, and a candidate wins on a strictly smaller squared distance or on an equal one with a
-// smaller primitive index.  So every primitive that could win is evaluated, and the winner is the lexicographic
-// minimum of (float squared distance, index) over all of them, whatever the tree's shape.
+// computed squared distance exceeds prune_bound of the current best, which is proved below to exceed the box distance
+// of every primitive whose computed squared distance is <= best, and a candidate wins on a strictly smaller squared
+// distance or on an equal one with a smaller primitive index.  So every primitive that could win is evaluated, and the
+// winner is the lexicographic minimum of (float squared distance, index) over all of them, whatever the tree's shape
+// (tests/bvh_f32_oracle.py restates it).
 namespace shapy {
 
 constexpr int kScanMaxPrims = 32768;  // the shared-memory sorts of bvh_prepare_kernel and scan_backward_kernel
@@ -466,7 +467,8 @@ __device__ __forceinline__ float3 sub3(float3 a, float3 b) { return make_float3(
 __device__ __forceinline__ float dot3(float3 a, float3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 
 // The Voronoi-region test of a non-degenerate triangle (a, b, c): the closest point of p is a + v ab + w ac.  Returns
-// false when the interior's denominator is not positive (a triangle too thin for the test), true otherwise.
+// false when the interior's denominator is not positive (a triangle too thin for the test) or rounding put p's
+// projection outside the triangle, true otherwise; then v, w >= 0 and v + w <= 1 + 4u.
 __device__ __forceinline__ bool tri_region(float3 ab, float3 ac, float3 ap, float3 bp, float3 cp, float &v, float &w) {
   const float d1 = dot3(ab, ap), d2 = dot3(ac, ap);
   if (d1 <= 0.f && d2 <= 0.f) { v = 0.f; w = 0.f; return true; }  // vertex a
@@ -486,7 +488,9 @@ __device__ __forceinline__ bool tri_region(float3 ab, float3 ac, float3 ap, floa
     return true;
   }
   const float den = va + vb + vc;  // interior
-  if (!(den > 0.f)) return false;
+  // Rounding can reach here with p's projection outside the triangle (a negative va, vb or vc near a region's
+  // border); the edges then give the closest point, so (v, w) stays in the triangle (see prune_bound).
+  if (!(den > 0.f && va >= 0.f && vb >= 0.f && vc >= 0.f)) return false;
   v = vb / den;
   w = vc / den;
   return true;
@@ -534,8 +538,38 @@ __device__ __forceinline__ float scan_child_box_d2(const BvhNode *nodes, const f
   return box_d2(p, bx);
 }
 
-// the largest box distance that can still hold a primitive as near as `best`
-__device__ __forceinline__ float prune_bound(float best) { return best + best * 1e-5f + 1e-12f; }
+// The largest box distance that can still hold a primitive as near as `best`.
+//
+// Points: box_d2 of a point's leaf box is the same operations as its d2, so it rounds to the same value, and a node's
+// box contains its children's, so its box_d2 is no larger (every operation of box_d2 is monotone).  Any bound >= best
+// is exact; the relative one below keeps the points query's bits.
+__device__ __forceinline__ float relative_prune_bound(float best) { return best + best * 1e-5f + 1e-12f; }
+
+// Triangles: prune_bound(best, M) = (sqrt(best) + k u M)^2, u = 2^-24, k = 64, M the largest coordinate magnitude of
+// the query and the body's scene box (the root's box), so that every coordinate of p, a, b, c is <= M.  Claim: for
+// every leaf, with d2 = point_triangle(p, a, b, c) and b2 = box_d2(p, leaf box) as computed,
+// b2 <= prune_bound(d2, M).  Both sides are monotone in their argument (node boxes contain leaf boxes; sqrtf, + and *
+// round monotonically), so a leaf as near as `best`, and every node above it, is visited.  Proof, to first order in u
+// (the k chosen leaves the O(u^2) terms far below the margin), with |x| the Euclidean norm:
+//  1. tri_region and the edge fallback return v, w >= 0, v + w <= 1 + 4u.  So X = a + (b - a) v + (c - a) w lies
+//     within 4u |b - a, c - a| <= 4u 2 sqrt(3) M < 14u M of the triangle, whose points lie in the leaf box:
+//     D := the exact distance of p to the box <= |p - X| + 14u M.
+//  2. tri_d2's vector differs from p - X, per coordinate, by the rounding of ap (2u M), of ab and ac times v, w
+//     (2u M (v + w)), of the products and their sum (2 2u M (v + w)) and of the difference (u |d|): in norm by at
+//     most sqrt(3) 8u M + u |d| < 14u M + u |d|.  dot3 of a vector rounds its square down by at most (1 - u)^3.
+//     So s := sqrt(d2) >= (1 - 2.5u) |p - X| - 14u M.
+//  3. box_d2 rounds each of its 3 + 3 + 2 operations up by at most (1 + u): sqrt(b2) <= (1 + 2.5u) D.
+//  4. Then sqrt(b2) <= (1 + 5u) s + 28u M + 5u (14u M), and s <= |p - X| <= 2 sqrt(3) M (1 + 4u): 5u s <= 18u M,
+//     so sqrt(b2) <= s + 46u M.
+//  5. The bound as computed, fl(fl(fl(sqrt(d2)) + M ku)^2), is >= (s + 64u M)^2 (1 - u)^5: sqrtf and the add each
+//     round r down by at most (1 - u), squared, and the square rounds once more.  That is >= (s + 46u M)^2, as
+//     2.5u (s + 64u M) <= 18u M for s <= 7.2 M - 64u M, and s <= 3.5 M.  (M ku is exact: ku = 2^-18.)
+// The bound is a function of the query and its body only, so results stay independent of the batch.
+constexpr float kPruneSlack = 0x1p-18f;  // k u
+__device__ __forceinline__ float prune_bound(float best, float M) {
+  const float r = sqrtf(best) + M * kPruneSlack;
+  return r * r;
+}
 
 // One thread per query point q of body blockIdx.y against the P primitives of that body's tree.  kPts: the
 // primitives are points (soup (p, p, p)), d2 = |q - p|^2 and a primitive with prim_w <= 0 is skipped; otherwise they
@@ -550,7 +584,7 @@ __global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict
   const int qi = blockIdx.x * blockDim.x + threadIdx.x;
   if (qi >= Q) return;
   const size_t o = (size_t)b * Q + qi;
-  float best = INFINITY, bv = 0.f, bw = 0.f;
+  float best = INFINITY, lim = INFINITY, bv = 0.f, bw = 0.f;  // lim: the prune bound of best
   int best_id = -1;
   if (kPts || !q_w || q_w[o] > 0.f) {
     const float3 q = make_float3(queries[o * 3], queries[o * 3 + 1], queries[o * 3 + 2]);
@@ -558,6 +592,11 @@ __global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict
     const int *ids = w.ids + (size_t)b * P;
     const BvhNode *nodes = w.nodes + (size_t)b * (P - 1);
     const float *leaf_box = w.leaf_box + (size_t)b * P * 6;
+    float M = fmaxf(fmaxf(fabsf(q.x), fabsf(q.y)), fabsf(q.z));
+    if (!kPts) {
+      const float *root = P == 1 ? leaf_box : nodes[0].lo;
+      for (int c = 0; c < 6; ++c) M = fmaxf(M, fabsf(__ldg(root + c)));
+    }
     auto leaf = [&](int j) {
       const int id = __ldg(ids + j);
       const float *t = sb + (size_t)id * 9;
@@ -570,7 +609,10 @@ __global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict
         d2 = point_triangle(q, make_float3(t[0], t[1], t[2]), make_float3(t[3], t[4], t[5]),
                             make_float3(t[6], t[7], t[8]), v, ww);
       }
-      if (d2 < best || (d2 == best && id < best_id)) { best = d2; best_id = id; bv = v; bw = ww; }
+      if (d2 < best || (d2 == best && id < best_id)) {
+        best = d2; best_id = id; bv = v; bw = ww;
+        lim = kPts ? relative_prune_bound(best) : prune_bound(best, M);
+      }
     };
     if (P == 1) {
       leaf(0);
@@ -582,8 +624,8 @@ __global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict
         const int link[2] = {__ldg(&nodes[node].left), __ldg(&nodes[node].right)};
         const float d[2] = {scan_child_box_d2(nodes, leaf_box, link[0], q), scan_child_box_d2(nodes, leaf_box, link[1], q)};
         for (int c = 0; c < 2; ++c)
-          if (link[c] < 0 && d[c] <= prune_bound(best)) leaf(~link[c]);
-        const bool go0 = link[0] >= 0 && d[0] <= prune_bound(best), go1 = link[1] >= 0 && d[1] <= prune_bound(best);
+          if (link[c] < 0 && d[c] <= lim) leaf(~link[c]);
+        const bool go0 = link[0] >= 0 && d[0] <= lim, go1 = link[1] >= 0 && d[1] <= lim;
         if (go0 && go1) {
           const int near = d[1] < d[0] ? 1 : 0;
           st_node[sp] = link[1 - near];
@@ -596,7 +638,7 @@ __global__ void __launch_bounds__(128) scan_query_kernel(const float *__restrict
           node = -1;
           while (sp > 0) {
             --sp;
-            if (st_d[sp] <= prune_bound(best)) { node = st_node[sp]; break; }
+            if (st_d[sp] <= lim) { node = st_node[sp]; break; }
           }
           if (node < 0) break;
         }
